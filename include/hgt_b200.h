@@ -1,4 +1,4 @@
-/* hgt_b200.h — C ABI of libhgt_b200.so: the B200 (sm_100a) implementation of pyHGT's HGTConv
+/* hgt_b200.h — C ABI of libhgt_b200.so: the H100 (sm_90a) implementation of pyHGT's HGTConv
  * message-passing hot path.
  *
  * Boundary being replaced (reference = acbull/pyHGT, paths relative to the reference root):
@@ -167,8 +167,8 @@ int hgt_concat_linears(const float* const* w, const float* const* b, int32_t num
  * [240,d] is one hgt_typed_linear call, and its projection through every pair's K'/V' weights another. */
 
 /* out[cblock c of group g][m, n] = sum_k A[a_row0_g + m, k] * W[w_row0_g + c*cb_width + n, k] (+ bias).
- * fp32 in / fp32 out.  `impl`: 0 = auto, 1 = SIMT fp32 FMA kernel, 2 = tcgen05 split-bf16 tensor-core
- * kernel (three bf16 products of a hi/lo operand split accumulated in one fp32 TMEM accumulator: accurate
+ * fp32 in / fp32 out.  `impl`: 0 = auto, 1 = SIMT fp32 FMA kernel, 2 = wgmma split-bf16 tensor-core
+ * kernel (three bf16 products of a hi/lo operand split accumulated in one fp32 register accumulator: accurate
  * to ~1e-5 relative; needs cb_width % 16 == 0 and K >= 64, workspace for the split operands).
  * groups/cblocks are DEVICE arrays; h_groups is the same table on the host (used to size the grid; no
  * device read-back). */
@@ -239,7 +239,7 @@ int hgt_edge_backward(const float* q, const float* kv, const float* kvr, const f
  * elements).  dW / db are ACCUMULATED INTO (several groups may share W rows: the caller zero-initialises them once per
  * step); dA is written (rows BETWEEN / BEFORE the groups that no group covers are zeroed; rows past the last group are the
  * caller's) unless accumulate_dA != 0, in which case the product is added to its current content.  dA / dW / db may each be NULL to skip that product.
- * Tensor-core path (impl 0 = auto, 2 = force): tcgen05 split-bf16 x3 like the forward; takes the operands either as
+ * Tensor-core path (impl 0 = auto, 2 = force): wgmma split-bf16 x3 like the forward; takes the operands either as
  * fp32 (split here; the dout split pass also yields db) or already split by their producers (dout_hi/lo in dout's
  * layout; a_hi/a_lo [rows, K] as left by hgt_act_split in the forward) — with a pre-split dout, db is NOT computed.
  * impl 1 = fp32 SIMT kernels (any shape; also chosen automatically for cb_width % 8, K % 16, K < 64, overlapping groups

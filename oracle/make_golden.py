@@ -23,6 +23,40 @@ from pyhgt_b200 import synth                      # noqa: E402
 OUT_DIR = os.path.join(ROOT, "tests", "golden")
 
 
+PART_BYTES = 900 * 1024
+
+
+def save_fixture(fx, name):
+    """torch.save the fixture dict as tests/golden/<name>.pt plus, when it would exceed PART_BYTES, further files
+    <name>.part<i>.pt holding the remaining top-level keys (tests/conftest.py:load_golden merges them back), so that no
+    stored file passes 1 MB.  Returns the bytes written."""
+    import glob
+    import io
+    for old in glob.glob(os.path.join(OUT_DIR, name + ".part*.pt")):
+        os.remove(old)
+
+    def nbytes(obj):
+        buf = io.BytesIO()
+        torch.save(obj, buf)
+        return buf.tell()
+
+    parts, cur = [], {}
+    for k, v in fx.items():
+        if cur and nbytes({**cur, k: v}) > PART_BYTES:
+            parts.append(cur)
+            cur = {}
+        cur[k] = v
+    parts.append(cur)
+    total = 0
+    for i, part in enumerate(parts):
+        path = os.path.join(OUT_DIR, name + (".pt" if i == 0 else ".part%d.pt" % i))
+        torch.save(part, path)
+        size = os.path.getsize(path)
+        assert size < 1000 * 1000, "%s: one top-level entry alone exceeds the file limit (%d bytes)" % (path, size)
+        total += size
+    return total
+
+
 def _perturb(module, seed):
     """Move skip / relation_pri / LayerNorm affine / biases away from their constant inits so a
     missing term cannot hide behind a 1 or a 0."""
@@ -59,10 +93,9 @@ def conv_case(name, graph, d, heads, use_norm, use_RTE, seed, grads=False, feat_
         with torch.no_grad():
             fx["out"] = m(x, graph.node_type, graph.edge_index, graph.edge_type, graph.edge_time).clone()
     fx["att"] = m.att.detach().clone()
-    path = os.path.join(OUT_DIR, name + ".pt")
-    torch.save(fx, path)
+    size = save_fixture(fx, name)
     print("%-28s N=%d E=%d d=%d H=%d  %.0f KB" % (name, graph.num_nodes, graph.num_edges, d, heads,
-                                                 os.path.getsize(path) / 1024))
+                                                 size / 1024))
 
 
 def dense_case(name, graph, d, heads, use_norm, use_RTE, seed):
@@ -88,10 +121,9 @@ def dense_case(name, graph, d, heads, use_norm, use_RTE, seed):
     fx["grad_weight"] = w
     fx["grad_node_inp"] = xg.grad.detach().clone()
     fx["grad_params"] = {k: p.grad.detach().clone() for k, p in m.named_parameters() if p.grad is not None}
-    path = os.path.join(OUT_DIR, name + ".pt")
-    torch.save(fx, path)
+    size = save_fixture(fx, name)
     print("%-28s N=%d E=%d d=%d H=%d  %.0f KB" % (name, graph.num_nodes, graph.num_edges, d, heads,
-                                                 os.path.getsize(path) / 1024))
+                                                 size / 1024))
 
 
 def gnn_case(name, graph, in_dim, n_hid, heads, n_layers, seed):
@@ -117,9 +149,8 @@ def gnn_case(name, graph, in_dim, n_hid, heads, n_layers, seed):
     fx["grad_weight"] = w
     fx["grad_node_feature"] = xg.grad.detach().clone()
     fx["grad_params"] = {k: p.grad.detach().clone() for k, p in m.named_parameters() if p.grad is not None}
-    path = os.path.join(OUT_DIR, name + ".pt")
-    torch.save(fx, path)
-    print("%-28s N=%d E=%d  %.0f KB" % (name, graph.num_nodes, graph.num_edges, os.path.getsize(path) / 1024))
+    size = save_fixture(fx, name)
+    print("%-28s N=%d E=%d  %.0f KB" % (name, graph.num_nodes, graph.num_edges, size / 1024))
 
 
 def synthetic_sampled_subgraph(seed, n_per_type=(40, 25, 10), n_edges=300):
@@ -159,9 +190,8 @@ def to_torch_case(name, seed):
     fx = {"feature": feature, "time": times, "edge_list": plain_edges, "types": g.get_types(),
           "meta_graph": g.get_meta_graph(), "node_feature": ref[0], "node_type": ref[1], "edge_time": ref[2],
           "edge_index": ref[3], "edge_type": ref[4], "node_dict": ref[5], "edge_dict": ref[6]}
-    path = os.path.join(OUT_DIR, name + ".pt")
-    torch.save(fx, path)
-    print("%-28s N=%d E=%d  %.0f KB" % (name, ref[1].numel(), ref[4].numel(), os.path.getsize(path) / 1024))
+    size = save_fixture(fx, name)
+    print("%-28s N=%d E=%d  %.0f KB" % (name, ref[1].numel(), ref[4].numel(), size / 1024))
 
 
 def sampler_graph(data, seed, n_paper=300, n_author=200, n_venue=8, n_field=30, e_ap=1200, e_pp=900, e_pf=700):
@@ -208,17 +238,17 @@ def sampler_extractor(layer_data, graph):
     return feature, times, indxs, []
 
 
-def sampler_case(name, seed):
+def sampler_case(name, seed, n_inp=24, runs=((2, 8), (4, 16)), **graph_kw):
     """sample_subgraph (data.py:87-210) run by the UNMODIFIED reference with a seeded numpy RNG, then the reference's
     to_torch on the result.  The fixture stores the graph's edge_list as plain nested dicts (insertion orders kept)."""
     import numpy as np
     data = pyg_shim.load_reference_data()
-    g, years = sampler_graph(data, seed)
+    g, years = sampler_graph(data, seed, **graph_kw)
     time_range = {int(y): True for y in range(2000, 2016)}
-    pids = np.random.RandomState(100 + seed).choice(300, 24, replace=False)
+    pids = np.random.RandomState(100 + seed).choice(len(years), n_inp, replace=False)
     inp = {"paper": np.array([[int(p), int(years[p])] for p in pids])}
     cases = []
-    for depth, number in ((2, 8), (4, 16)):
+    for depth, number in runs:
         np.random.seed(7 + seed)
         feature, times, edge_list, indxs, _ = data.sample_subgraph(g, time_range, depth, number, inp, sampler_extractor)
         rng_after = np.random.get_state()[1].copy()
@@ -233,15 +263,40 @@ def sampler_case(name, seed):
                  for s_, d2 in d1.items()} for t, d1 in g.edge_list.items()}
     fx = {"edge_list": plain, "types": g.get_types(), "meta_graph": g.get_meta_graph(), "time_range": time_range,
           "inp": inp, "cases": cases}
-    path = os.path.join(OUT_DIR, name + ".pt")
-    torch.save(fx, path)
-    print("%-28s %d sampled cases  %.0f KB" % (name, len(cases), os.path.getsize(path) / 1024))
+    size = save_fixture(fx, name)
+    print("%-28s %d sampled cases  %.0f KB" % (name, len(cases), size / 1024))
+
+
+# Constructor arguments of the module-shape fixture: one small HGTConv and the ogbn-mag recipe model (4 layers, n_hid 512)
+MODULE_CONV_ARGS = (32, 32, 3, 4, 4, 0.2, True, True)
+MODULE_GNN_ARGS = dict(in_dim=129, n_hid=512, num_types=4, num_relations=9, n_heads=8, n_layers=4, prev_norm=True,
+                       last_norm=True, use_RTE=True)
+MODULE_CLASSIFIER_ARGS = (512, 349)
+
+
+def modules_case(name):
+    """Parameter names / shapes of the reference's HGTConv and GNN, and the size of its Classifier (model.py)."""
+    import json
+    conv, model = pyg_shim.load_reference()
+    shapes = lambda m: [[n, list(p.shape)] for n, p in m.named_parameters()]          # noqa: E731
+    fx = {"conv_args": list(MODULE_CONV_ARGS), "conv": shapes(conv.HGTConv(*MODULE_CONV_ARGS)),
+          "gnn_args": MODULE_GNN_ARGS, "gnn": shapes(model.GNN(**MODULE_GNN_ARGS)),
+          "classifier_args": list(MODULE_CLASSIFIER_ARGS),
+          "classifier_params": sum(p.numel() for p in model.Classifier(*MODULE_CLASSIFIER_ARGS).parameters())}
+    path = os.path.join(OUT_DIR, name + ".json")
+    with open(path, "w") as f:
+        json.dump(fx, f, indent=0)
+    print("%-28s %.0f KB" % (name, os.path.getsize(path) / 1024))
 
 
 def main():
     os.makedirs(OUT_DIR, exist_ok=True)
+    modules_case("reference_modules")
     to_torch_case("to_torch", seed=31)
     sampler_case("sampler", seed=3)
+    # a graph of ~4.7 k nodes / 24 k edges (with rev_ relations) sampled 5 deep, 64 wide from 64 papers
+    sampler_case("sampler_large", seed=11, n_inp=64, runs=((5, 64),), n_paper=2000, n_author=1500, n_venue=20,
+                 n_field=100, e_ap=5000, e_pp=4000, e_pf=3000)
     c1 = synth.make_c1()
     conv_case("c1_norte", c1, 64, 4, True, False, seed=10)              # BASELINE config 1
     conv_case("c1_rte", c1, 64, 4, True, True, seed=11, grads=True)

@@ -1,4 +1,4 @@
-"""pyhgt_b200 — B200 (sm_100a) implementation of pyHGT's HGTConv message-passing hot path.
+"""pyhgt_b200 — H100 (sm_90a) implementation of pyHGT's HGTConv message-passing hot path.
 
 Public surface mirrors the reference's pyHGT/conv.py for that path: HGTConv, RelTemporalEncoding,
 GeneralConv.  Everything runs through libhgt_b200.so (C ABI: include/hgt_b200.h); no CPU fallback.

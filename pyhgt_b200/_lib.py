@@ -1,6 +1,6 @@
 """ctypes binding of libhgt_b200.so (C ABI declared in include/hgt_b200.h).
 
-The library is built in-tree by ``pyhgt_b200/build.py`` (nvcc, sm_100a).  There is NO fallback: if the
+The library is built in-tree by ``pyhgt_b200/build.py`` (nvcc, sm_90a).  There is NO fallback: if the
 shared object is missing or a symbol is absent, loading raises.
 """
 import ctypes

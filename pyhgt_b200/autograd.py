@@ -4,7 +4,7 @@ OAG/train_paper_field.py:249 ``loss.backward()``).
 Every stage is a custom autograd.Function whose forward AND backward are hand-written kernels behind the C ABI:
 
     _FoldWeights     hgt_fold_weights / hgt_fold_backward        relation_att/msg/pri folded into the typed K/V weights
-    _TypedLinear     hgt_act_split + hgt_typed_linear_presplit   typed projections, a_linears, RTE tables (tcgen05
+    _TypedLinear     hgt_act_split + hgt_typed_linear_presplit   typed projections, a_linears, RTE tables (wgmma
                      / hgt_typed_linear_bwd                      split-bf16 forward, dX and dW; fp32 SIMT for odd shapes);
                                                                  the gelu in front of the a_linears (conv.py:119) lives in
                                                                  the operand split (forward) and the dX epilogue (backward)

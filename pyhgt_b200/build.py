@@ -1,4 +1,4 @@
-"""Build libhgt_b200.so (sm_100a) in-tree with nvcc.  No torch headers are involved: the library is
+"""Build libhgt_b200.so (sm_90a, H100) in-tree with nvcc.  No torch headers are involved: the library is
 plain CUDA C++ behind the C ABI in include/hgt_b200.h."""
 import os
 import subprocess
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB_PATH = os.path.join(HERE, "libhgt_b200.so")
 SOURCES = ["common.cu", "plan.cu", "linear.cu", "linear_tc.cu", "edge.cu", "edge_bwd.cu", "update.cu", "layer.cu", "linear_bwd.cu", "update_bwd.cu", "sampler.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 

@@ -2,7 +2,7 @@
 
 ``HGTConv`` keeps the reference's constructor (conv.py:12), five-argument ``forward`` (conv.py:56),
 public attributes (conv.py:15-25), ``.att`` side effect (conv.py:108), ``__repr__`` (conv.py:136-139) and
-parameter / state_dict names (conv.py:28-54), but computes through the hand-written sm_100a kernels
+parameter / state_dict names (conv.py:28-54), but computes through the hand-written sm_90a kernels
 behind the C ABI in include/hgt_b200.h:
 
     plan (once per graph)            hgt_plan_*          CSR by destination, pairs, gather rows, tiles
@@ -77,7 +77,7 @@ class HGTConv(nn.Module):
     # conv.py:308 stays valid).
     keep_att = True            # materialise self.att [E,H] like the reference (conv.py:108)
     edge_variant = 0           # 0 auto, 1 register gather, 2 bulk-copy ring (see csrc/edge.cu)
-    linear_impl = 0            # 0 auto, 1 fp32 SIMT, 2 tcgen05
+    linear_impl = 0            # 0 auto, 1 fp32 SIMT, 2 tensor cores (wgmma)
     event_sink = None          # bench.py: list receiving (stage, start_event, end_event) on the launch stream
     _has_skip = True           # DenseHGTConv (conv.py:143-280) has no skip gate
     emit_split = False         # also write the output as a bf16 hi/lo split for the next layer (model.GNN sets it)
@@ -444,7 +444,7 @@ class DenseHGTConv(HGTConv):
     softmax by destination, aggregation => the same CUDA kernels), but update() is
         y = LayerNorm_t(a_linear_t(agg) + x)                         (no gelu, no skip gate; conv.py:261-266)
         out = out_norm(out_linear(gelu(mid_linear(y))) + y)          (shared 2-layer FFN; conv.py:273-274)
-    Every stage runs through the C ABI (autograd.dense_hgt_forward): typed tcgen05 GEMMs with the FFN's gelu inside the
+    Every stage runs through the C ABI (autograd.dense_hgt_forward): typed tensor-core GEMMs with the FFN's gelu inside the
     operand split, the residual + LayerNorm in `hgt_update_epilogue`'s residual mode; training uses the same native backward
     kernels as HGTConv.  Parameter names match the reference (mid_linear, out_linear, out_norm; no `skip`)."""
     _has_skip = False

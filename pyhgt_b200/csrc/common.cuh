@@ -1,4 +1,4 @@
-// Shared helpers for libhgt_b200.so (sm_100a only).
+// Shared helpers for libhgt_b200.so (sm_90a, H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,7 +7,7 @@
 
 #include "hgt_b200.h"
 
-#define HGT_SM_COUNT_FALLBACK 148
+#define HGT_SM_COUNT_FALLBACK 132
 
 void hgt_set_error(const char* fmt, ...);
 int hgt_sm_count();

@@ -42,7 +42,7 @@ struct EdgeParams {
   int32_t d, H, DK, LPH, lph_shift;
   int32_t apply_gelu;
   float* agg_out;            // nullptr when only the split bf16 copy is wanted
-  __nv_bfloat16* g_hi;       // optional: result as bf16 hi/lo split (operand of the tcgen05 a_linear GEMM)
+  __nv_bfloat16* g_hi;       // optional: result as bf16 hi/lo split (operand of the tensor-core a_linear GEMM)
   __nv_bfloat16* g_lo;
   float* att_out;            // nullptr unless requested
   float* stats_out;          // nullptr unless requested

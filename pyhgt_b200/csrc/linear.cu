@@ -1,6 +1,6 @@
 // Typed (per-node-type) linear layers of HGTConv: weight folding (relation_att / relation_msg /
 // relation_pri into the K/V projections, SURVEY.md §8 a4) and the grouped GEMM front end.
-// This file holds the fp32 SIMT kernel (impl 1); the tcgen05 tensor-core kernel (impl 2) lives in
+// This file holds the fp32 SIMT kernel (impl 1); the wgmma tensor-core kernel (impl 2) lives in
 // linear_tc.cu and is dispatched from hgt_typed_linear below.
 #include "common.cuh"
 

@@ -7,15 +7,15 @@
 //   db[w_row0_g + c*width + n]    += sum_m dOut_c[m, n]
 // The reference gets these from autograd over per-edge nn.Linear calls (conv.py:96-104,125; OAG/train_paper_field.py:249).
 //
-// Tensor-core path (tcgen05, sm_100a): the same split-bf16 x3 scheme as the forward (x = hi + lo, three bf16 products
-// in one fp32 TMEM accumulator):
+// Tensor-core path (Hopper wgmma, tcp::split3_tile in tc_ptx.cuh): the same split-bf16 x3 scheme as the forward (x = hi + lo,
+// three bf16 products in one fp32 register accumulator):
 //   k_act_split / k_split_colsum   fp32 -> bf16 hi/lo (optionally gelu first); the dOut split pass also produces db
-//   k_lin_dx_tc   one 128 x BN tile of dA per CTA; K runs over (column block, 64-wide k-block); A operand = dOut tiles
-//                 (K-major), B operand = W^T (a transposed, zero-padded bf16 split of the small weight matrix);
-//                 epilogue: optional `+= dA`, optional `* gelu'(aux)` (the gelu in front of the a_linears, conv.py:119)
-//   k_lin_dw_tc   dW tile [128 of width] x [BN of K_in] per CTA, reduction over a chunk of the group's rows; both operands
-//                 are MN-major (the reduction index is the row index): TMA boxes {64 columns, 64 rows}, SWIZZLE_128B,
-//                 tcgen05 MN-major descriptors; partial tiles are added with red.global.add.v4.f32
+//   k_lin_dx_tc (DxJob)   one 128 x tile_n tile of dA per CTA; K runs over (column block, 64-wide k-block); A operand = dOut tiles
+//           (K-major), B operand = W^T (a transposed, zero-padded bf16 split of the small weight matrix);
+//           epilogue: optional `+= dA`, optional `* gelu'(aux)` (the gelu in front of the a_linears, conv.py:119)
+//   k_lin_dw_tc (DwJob)   dW tile [128 of width] x [tile_n of K_in] per CTA, reduction over a chunk of the group's rows; both operands
+//           are MN-major (the reduction index is the row index): TMA boxes {64 columns, 64 rows}, SWIZZLE_128B;
+//           partial tiles are added with red.global.add.v2.f32
 // Every (group, column block) gets its own tensor map (tight row extents => rows past the group are zero-filled by TMA, so the
 // reduction never sees a neighbour's rows); the maps live in the workspace (global memory).
 // SIMT fp32 path for shapes the tensor cores cannot take (width % 8, K % 16, overlapping groups such as the RTE tables).
@@ -35,10 +35,6 @@ namespace {
 using namespace tcp;
 
 constexpr int kMaxGroups = 64;
-constexpr int BK = 64;                  // 64 bf16 = one 128-byte swizzle row
-constexpr int UMMA_K = 16;
-constexpr int BW_THREADS = 192;         // warp 0: TMA, warp 1: MMA + TMEM, warps 2-5: epilogue
-constexpr uint32_t ATOM_BYTES = 64 * 128;   // one {64 x 64} bf16 TMA box
 
 // Tensor maps are read from global memory (written by a host copy earlier on the stream): acquire them for the TMA proxy.
 __device__ __forceinline__ void map_acquire(const CUtensorMap* m) {
@@ -166,274 +162,154 @@ k_split_colsum(const float* __restrict__ dout, const GcTask* __restrict__ tasks,
 }
 
 // ---- dX: dA tile = sum over (column block, k-block) of dOut tile x W^T tile --------------------------------------------
-struct DxSched {
+// A operand = dOut of the group's column blocks (K-major, two 64-row boxes), B operand = W^T (K-major, tile_n-row box).
+// Output columns past K_in (tile padding) and rows past the group are not stored.
+struct DxJob {
+  const CUtensorMap* maps;
+  int map_wt;
+  const GcTask* tasks;
+  const int32_t* group_task0;
+  const hgt_lin_group* groups;
+  int n_groups, K_in, width, n_tiles_n, tile_n;
+  float* dA;
+  int accumulate;
+  const float* gelu_aux;
   int32_t first_tile[kMaxGroups + 1];
-  int32_t n_tiles_n;
-  int32_t bn_box;            // rows of the W^T TMA box (n-tile width in shared memory)
+
+  struct Tile {
+    int m0, n0, task0, kb_per_c, n_cblocks;
+    int64_t rows, a_row0;
+  };
+
+  __device__ int decode(int tile, Tile& t) const {
+    int g = 0;
+    while (g + 1 < n_groups && tile >= first_tile[g + 1]) ++g;
+    const hgt_lin_group grp = groups[g];
+    const int local = tile - first_tile[g];
+    const int mt = local / n_tiles_n, nt = local - mt * n_tiles_n;
+    t.m0 = mt * BM;
+    t.n0 = nt * tile_n;
+    t.task0 = group_task0[g];
+    t.kb_per_c = (width + BK - 1) / BK;
+    t.rows = grp.m - t.m0;
+    t.a_row0 = grp.a_row0 + t.m0;
+    t.n_cblocks = grp.n_cblocks;
+    return grp.n_cblocks * t.kb_per_c;
+  }
+  __device__ void prefetch(const Tile& t) const {
+    map_acquire(maps + map_wt);
+    map_acquire(maps + map_wt + 1);
+    for (int c = 0; c < t.n_cblocks; ++c) {
+      map_acquire(maps + tasks[t.task0 + c].map_dout);
+      map_acquire(maps + tasks[t.task0 + c].map_dout + 1);
+    }
+  }
+  template <int BN>
+  __device__ void load(const Tile& t, int it, uint32_t sa, uint32_t bar) const {
+    const int c = it / t.kb_per_c, kb = it - c * t.kb_per_c;
+    const GcTask& tk = tasks[t.task0 + c];
+    const CUtensorMap* m_hi = maps + tk.map_dout;
+    const CUtensorMap* m_lo = m_hi + 1;
+    tma_load_2d(sa, m_hi, kb * BK, t.m0, bar);
+    tma_load_2d(sa + ATOM_BYTES, m_hi, kb * BK, t.m0 + 64, bar);
+    tma_load_2d(sa + A_BYTES, m_lo, kb * BK, t.m0, bar);
+    tma_load_2d(sa + A_BYTES + ATOM_BYTES, m_lo, kb * BK, t.m0 + 64, bar);
+    tma_load_2d(sa + 2 * A_BYTES, maps + map_wt, tk.wt_col0 + kb * BK, t.n0, bar);
+    tma_load_2d(sa + 2 * A_BYTES + BN * BK * 2, maps + map_wt + 1, tk.wt_col0 + kb * BK, t.n0, bar);
+  }
+  template <int BN>
+  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+    const int64_t rows = t.rows - 64 * c;
+    const int cols = K_in - t.n0;
+    const int64_t row0 = (t.a_row0 + 64 * c) * K_in + t.n0;
+    float* o = dA + row0;
+    const float* x = gelu_aux ? gelu_aux + row0 : nullptr;
+    const int ld = K_in;
+    const bool acc_in = accumulate != 0;
+    for_each_pair<BN>(acc, wq, lane, [&](int r, int col, float v0, float v1) {
+      if (r < rows && col < cols) {
+        const int64_t off = (int64_t)r * ld + col;
+        if (x) {
+          const float2 xv = *reinterpret_cast<const float2*>(x + off);
+          v0 *= gelu_grad(xv.x);
+          v1 *= gelu_grad(xv.y);
+        }
+        if (acc_in) {
+          const float2 ov = *reinterpret_cast<const float2*>(o + off);
+          v0 += ov.x;
+          v1 += ov.y;
+        }
+        *reinterpret_cast<float2*>(o + off) = make_float2(v0, v1);
+      }
+    });
+  }
 };
 
-__global__ void __launch_bounds__(BW_THREADS, 1)
-k_lin_dx_tc(const CUtensorMap* __restrict__ maps, int map_wt, const GcTask* __restrict__ tasks,
-            const int32_t* __restrict__ group_task0, const hgt_lin_group* __restrict__ groups, int n_groups, int K_in,
-            int width, float* __restrict__ dA, int accumulate, const float* __restrict__ gelu_aux, DxSched sc) {
-  extern __shared__ unsigned char smem_dyn[];
-  unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);
-  constexpr int STAGES = 2;
-  const uint32_t a_bytes = 128 * BK * 2;                       // 16 KB (two 64-row boxes)
-  const uint32_t b_bytes = (uint32_t)sc.bn_box * BK * 2;
-  const uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;      // A_hi, A_lo, B_hi, B_lo
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * stage_bytes);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+// ---- dW: [128 rows of the column block] x [tile_n columns of K_in] += dOut_c^T A over a chunk of rows -----------------
+// Both operands MN-major (the reduction index is the row index): TMA boxes {64 columns, 64 rows}; partial tiles are added
+// with red.global.add.v2.f32.
+struct DwJob {
+  const CUtensorMap* maps;
+  const GcTask* tasks;
+  int n_tasks, K_in, width, m_tiles, n_tiles, chunk_rows, tile_n;
+  float* dW;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int tile = blockIdx.x, g = 0;
-  while (g + 1 < n_groups && tile >= sc.first_tile[g + 1]) ++g;
-  const hgt_lin_group grp = groups[g];
-  const int local = tile - sc.first_tile[g];
-  const int mt = local / sc.n_tiles_n, nt = local - mt * sc.n_tiles_n;
-  const int64_t m0 = (int64_t)mt * 128;
-  const int n0 = nt * 256;
-  const int bn = min(256, K_in - n0);                           // multiple of 16
-  const int kb_per_c = (width + BK - 1) / BK;
-  const int total_iters = grp.n_cblocks * kb_per_c;
-  const int task0 = group_task0[g];
+  struct Tile {
+    int mt, n0, map_dout, map_x, w_row;
+    int64_t r0;
+  };
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(s_u32(&full_bar[s]), 1);
-      mbar_init(s_u32(&empty_bar[s]), 1);
-    }
-    mbar_init(s_u32(tmem_full_bar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  __device__ int decode(int unit, Tile& t) const {
+    int i = 0;
+    while (i + 1 < n_tasks && unit >= tasks[i + 1].first_unit) ++i;
+    const GcTask tk = tasks[i];
+    int local = unit - tk.first_unit;
+    const int chunk = local / (m_tiles * n_tiles);
+    local -= chunk * m_tiles * n_tiles;
+    t.mt = local / n_tiles;
+    t.n0 = (local - t.mt * n_tiles) * tile_n;
+    t.map_dout = tk.map_dout;
+    t.map_x = tk.map_x;
+    t.w_row = tk.w_row;
+    t.r0 = (int64_t)chunk * chunk_rows;
+    const int64_t r1 = min(tk.rows, t.r0 + chunk_rows);
+    return (int)((r1 - t.r0 + BK - 1) / BK);
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr_smem)),
-                 "r"(256u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  __device__ void prefetch(const Tile& t) const {
+    map_acquire(maps + t.map_dout);
+    map_acquire(maps + t.map_dout + 1);
+    map_acquire(maps + t.map_x);
+    map_acquire(maps + t.map_x + 1);
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const CUtensorMap* m_wt_hi = maps + map_wt;
-      const CUtensorMap* m_wt_lo = maps + map_wt + 1;
-      map_acquire(m_wt_hi);
-      map_acquire(m_wt_lo);
-      for (int c = 0; c < grp.n_cblocks; ++c) {
-        map_acquire(maps + tasks[task0 + c].map_dout);
-        map_acquire(maps + tasks[task0 + c].map_dout + 1);
-      }
-      for (int it = 0; it < total_iters; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-        mbar_wait(s_u32(&empty_bar[s]), ph ^ 1u);
-        const int c = it / kb_per_c, kb = it - c * kb_per_c;
-        const GcTask tk = tasks[task0 + c];
-        const CUtensorMap* m_hi = maps + tk.map_dout;
-        const CUtensorMap* m_lo = m_hi + 1;
-        const uint32_t bar = s_u32(&full_bar[s]);
-        const uint32_t sa = s_u32(smem + (size_t)s * stage_bytes);
-        mbar_expect_tx(bar, stage_bytes);
-        tma_load_2d(sa, m_hi, kb * BK, (int)m0, bar);
-        tma_load_2d(sa + ATOM_BYTES, m_hi, kb * BK, (int)m0 + 64, bar);
-        tma_load_2d(sa + a_bytes, m_lo, kb * BK, (int)m0, bar);
-        tma_load_2d(sa + a_bytes + ATOM_BYTES, m_lo, kb * BK, (int)m0 + 64, bar);
-        tma_load_2d(sa + 2 * a_bytes, m_wt_hi, tk.wt_col0 + kb * BK, n0, bar);
-        tma_load_2d(sa + 2 * a_bytes + b_bytes, m_wt_lo, tk.wt_col0 + kb * BK, n0, bar);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = idesc_bf16(128, bn, false, false);
-      for (int it = 0; it < total_iters; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-        mbar_wait(s_u32(&full_bar[s]), ph);
-        tc_fence_after();
-        const uint32_t sa = s_u32(smem + (size_t)s * stage_bytes);
-        const uint64_t a_hi = desc_k_sw128(sa), a_lo = desc_k_sw128(sa + a_bytes);
-        const uint64_t b_hi = desc_k_sw128(sa + 2 * a_bytes), b_lo = desc_k_sw128(sa + 2 * a_bytes + b_bytes);
+  template <int BN>
+  __device__ void load(const Tile& t, int it, uint32_t sa, uint32_t bar) const {
+    const int row = (int)(t.r0 + (int64_t)it * BK);
+    const CUtensorMap* d_hi = maps + t.map_dout;
+    const CUtensorMap* x_hi = maps + t.map_x;
 #pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k) {
-          const uint64_t o = (uint64_t)(2 * k);                 // +32 bytes inside the swizzle row
-          umma_bf16_ss(tmem_base, a_hi + o, b_hi + o, idesc, (it > 0 || k > 0) ? 1u : 0u);
-          umma_bf16_ss(tmem_base, a_hi + o, b_lo + o, idesc, 1u);
-          umma_bf16_ss(tmem_base, a_lo + o, b_hi + o, idesc, 1u);
-        }
-        umma_commit(s_u32(&empty_bar[s]));
-      }
-      umma_commit(s_u32(tmem_full_bar));
+    for (int j = 0; j < 2; ++j) {
+      tma_load_2d(sa + j * ATOM_BYTES, d_hi, t.mt * BM + j * 64, row, bar);
+      tma_load_2d(sa + A_BYTES + j * ATOM_BYTES, d_hi + 1, t.mt * BM + j * 64, row, bar);
     }
-  } else {
-    const int lg = warp & 3;                                     // TMEM lane quarter this warp may read
-    const int row = lg * 32 + lane;
-    mbar_wait(s_u32(tmem_full_bar), 0);
-    tc_fence_after();
-    const bool row_ok = total_iters > 0 && m0 + row < grp.m;
-    const int64_t grow = grp.a_row0 + m0 + row;
-    float* orow = dA + grow * K_in + n0;
-    const float* xrow = gelu_aux ? gelu_aux + grow * K_in + n0 : nullptr;
-    for (int c = 0; c < bn; c += 16) {
-      uint32_t r[16];
-      tmem_ld16(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)c, r);
-      tmem_ld_wait();
-      if (row_ok) {
 #pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                 __uint_as_float(r[j + 3]));
-          if (xrow) {
-            const float4 x = *reinterpret_cast<const float4*>(xrow + c + j);
-            v.x *= gelu_grad(x.x); v.y *= gelu_grad(x.y); v.z *= gelu_grad(x.z); v.w *= gelu_grad(x.w);
-          }
-          if (accumulate) {
-            const float4 o = *reinterpret_cast<const float4*>(orow + c + j);
-            v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-          }
-          *reinterpret_cast<float4*>(orow + c + j) = v;
-        }
-      }
+    for (int j = 0; j < BN / 64; ++j) {
+      tma_load_2d(sa + 2 * A_BYTES + j * ATOM_BYTES, x_hi, t.n0 + j * 64, row, bar);
+      tma_load_2d(sa + 2 * A_BYTES + BN * BK * 2 + j * ATOM_BYTES, x_hi + 1, t.n0 + j * 64, row, bar);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
+  template <int BN>
+  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+    const int rows = width - t.mt * BM - 64 * c;                   // rows of the dW tile = columns of the dOut block
+    const int cols = K_in - t.n0;
+    float* o = dW + ((int64_t)t.w_row + t.mt * BM + 64 * c) * K_in + t.n0;
+    const int ld = K_in;
+    for_each_pair<BN>(acc, wq, lane, [&](int r, int col, float v0, float v1) {
+      if (r < rows && col < cols)
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(o + (int64_t)r * ld + col), "f"(v0), "f"(v1)
+                     : "memory");
+    });
   }
-}
-
-// ---- dW: [128 rows of the column block] x [BN columns of K_in] += dOut_c^T A over a chunk of rows ---------------------
-__global__ void __launch_bounds__(BW_THREADS, 1)
-k_lin_dw_tc(const CUtensorMap* __restrict__ maps, const GcTask* __restrict__ tasks, int n_tasks, int K_in, int width,
-            int m_tiles, int n_tiles, int chunk_rows, float* __restrict__ dW) {
-  extern __shared__ unsigned char smem_dyn[];
-  unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);
-  constexpr int STAGES = 2;
-  const uint32_t a_bytes = 2 * ATOM_BYTES;                      // dOut: 128 columns = 2 atoms of {64 cols x 64 rows}
-  const int n_atoms = min(4, (K_in + 63) / 64);
-  const uint32_t b_bytes = (uint32_t)n_atoms * ATOM_BYTES;      // A: up to 256 columns
-  const uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * stage_bytes);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int unit = blockIdx.x, t = 0;
-  while (t + 1 < n_tasks && unit >= tasks[t + 1].first_unit) ++t;
-  const GcTask tk = tasks[t];
-  int local = unit - tk.first_unit;
-  const int chunk = local / (m_tiles * n_tiles);
-  local -= chunk * m_tiles * n_tiles;
-  const int mt = local / n_tiles, nt = local - mt * n_tiles;
-  const int n0 = nt * 256;
-  const int bn = min(256, K_in - n0);                            // multiple of 16
-  const int atoms_here = (bn + 63) / 64;
-  const int64_t r0 = (int64_t)chunk * chunk_rows;
-  const int64_t r1 = min(tk.rows, r0 + chunk_rows);
-  const int total_iters = (int)((r1 - r0 + BK - 1) / BK);
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(s_u32(&full_bar[s]), 1);
-      mbar_init(s_u32(&empty_bar[s]), 1);
-    }
-    mbar_init(s_u32(tmem_full_bar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr_smem)),
-                 "r"(256u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const CUtensorMap* d_hi = maps + tk.map_dout;
-      const CUtensorMap* d_lo = d_hi + 1;
-      const CUtensorMap* x_hi = maps + tk.map_x;
-      const CUtensorMap* x_lo = x_hi + 1;
-      map_acquire(d_hi); map_acquire(d_lo); map_acquire(x_hi); map_acquire(x_lo);
-      const uint32_t tx = 2 * a_bytes + 2 * (uint32_t)atoms_here * ATOM_BYTES;
-      for (int it = 0; it < total_iters; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-        mbar_wait(s_u32(&empty_bar[s]), ph ^ 1u);
-        const int row = (int)(r0 + (int64_t)it * BK);
-        const uint32_t bar = s_u32(&full_bar[s]);
-        const uint32_t sa = s_u32(smem + (size_t)s * stage_bytes);
-        mbar_expect_tx(bar, tx);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          tma_load_2d(sa + j * ATOM_BYTES, d_hi, mt * 128 + j * 64, row, bar);
-          tma_load_2d(sa + a_bytes + j * ATOM_BYTES, d_lo, mt * 128 + j * 64, row, bar);
-        }
-        for (int j = 0; j < atoms_here; ++j) {
-          tma_load_2d(sa + 2 * a_bytes + j * ATOM_BYTES, x_hi, n0 + j * 64, row, bar);
-          tma_load_2d(sa + 2 * a_bytes + b_bytes + j * ATOM_BYTES, x_lo, n0 + j * 64, row, bar);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = idesc_bf16(128, bn, true, true);
-      for (int it = 0; it < total_iters; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-        mbar_wait(s_u32(&full_bar[s]), ph);
-        tc_fence_after();
-        const uint32_t sa = s_u32(smem + (size_t)s * stage_bytes);
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k) {
-          const uint32_t ko = (uint32_t)k * UMMA_K * 128;          // 16 k-rows of 128 bytes
-          const uint64_t a_hi = desc_mn_sw128(sa + ko, ATOM_BYTES);
-          const uint64_t a_lo = desc_mn_sw128(sa + a_bytes + ko, ATOM_BYTES);
-          const uint64_t b_hi = desc_mn_sw128(sa + 2 * a_bytes + ko, ATOM_BYTES);
-          const uint64_t b_lo = desc_mn_sw128(sa + 2 * a_bytes + b_bytes + ko, ATOM_BYTES);
-          umma_bf16_ss(tmem_base, a_hi, b_hi, idesc, (it > 0 || k > 0) ? 1u : 0u);
-          umma_bf16_ss(tmem_base, a_hi, b_lo, idesc, 1u);
-          umma_bf16_ss(tmem_base, a_lo, b_hi, idesc, 1u);
-        }
-        umma_commit(s_u32(&empty_bar[s]));
-      }
-      umma_commit(s_u32(tmem_full_bar));
-    }
-  } else {
-    const int lg = warp & 3;
-    const int row = lg * 32 + lane;                                // row of the dW tile = column of the dOut block
-    mbar_wait(s_u32(tmem_full_bar), 0);
-    tc_fence_after();
-    const bool row_ok = total_iters > 0 && mt * 128 + row < width;
-    float* wrow = dW + ((int64_t)tk.w_row + mt * 128 + row) * K_in + n0;
-    for (int c = 0; c < bn; c += 16) {
-      uint32_t r[16];
-      tmem_ld16(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)c, r);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(wrow + c + j), "f"(__uint_as_float(r[j])),
-                       "f"(__uint_as_float(r[j + 1])), "f"(__uint_as_float(r[j + 2])), "f"(__uint_as_float(r[j + 3]))
-                       : "memory");
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
-  }
-}
+};
 
 // ---- SIMT fp32 fallbacks ------------------------------------------------------------------------------------------------
 // dA[a_row0 + m, k] (+)= sum_c sum_n dOut_c[m, n] * W[w_row + n, k].  One thread per (m, k); atomicAdd because groups may
@@ -613,6 +489,32 @@ BwdLayout bwd_layout(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_
   return L;
 }
 
+template <int BN>
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dx_tc(const __grid_constant__ DxJob job) {
+  split3_tile<BN, false>(job);
+}
+template <int BN>
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc(const __grid_constant__ DwJob job) {
+  split3_tile<BN, true>(job);
+}
+
+template <int BN>
+int launch_bwd(const DxJob& job, unsigned tiles, cudaStream_t st) {
+  const size_t smem = tile_smem_bytes<BN>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dx_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_lin_dx_tc<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+template <int BN>
+int launch_bwd(const DwJob& job, unsigned tiles, cudaStream_t st) {
+  const size_t smem = tile_smem_bytes<BN>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_lin_dw_tc<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int hgt_act_split(const float* in, int64_t ld, int64_t rows, int32_t K, int32_t act, float* out_f32,
@@ -788,7 +690,7 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
     if ((rc = make_map2(&maps[2 * nt + 2 * g + 1], a_lo + h_groups[g].a_row0 * K, h_groups[g].m, K, K, 64))) return rc;
   }
   const int map_wt = 2 * nt + 2 * n_groups;
-  const int bn_box = K >= 256 ? 256 : K;
+  const int bn_box = pick_tile_n(K);                 // rows of the W^T box = dX tile width
   if ((rc = make_map2(&maps[map_wt], wt_hi, K, L.wt_cols, L.wt_cols, bn_box))) return rc;
   if ((rc = make_map2(&maps[map_wt + 1], wt_lo, K, L.wt_cols, L.wt_cols, bn_box))) return rc;
   CUtensorMap* d_maps = reinterpret_cast<CUtensorMap*>(base + L.off_maps);
@@ -808,29 +710,42 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
         pos = std::max(pos, p.second);
       }
     }
-    DxSched sc;
-    sc.n_tiles_n = (K + 255) / 256;
-    sc.bn_box = bn_box;
+    DxJob job;
+    job.tile_n = pick_tile_n(K);
+    job.n_tiles_n = (K + job.tile_n - 1) / job.tile_n;
     int64_t total = 0;
     for (int g = 0; g < n_groups; ++g) {
-      sc.first_tile[g] = (int32_t)total;
-      total += (h_groups[g].m + 127) / 128 * sc.n_tiles_n;
+      job.first_tile[g] = (int32_t)total;
+      total += (h_groups[g].m + BM - 1) / BM * job.n_tiles_n;
       HGT_REQUIRE(total < 2147483647ll, "hgt_typed_linear_bwd: too many tiles");
     }
-    sc.first_tile[n_groups] = (int32_t)total;
+    job.first_tile[n_groups] = (int32_t)total;
     if (total > 0) {
-      const size_t smem = 1024 + 2 * (size_t)(2 * 128 * BK * 2 + 2 * bn_box * BK * 2) + 8 * 8 + 16;
-      HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dx_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       // the task table for dX only needs map indices / wt_col0 (already set); first_unit is unused here
       if (have_dsplit && (rc = upload_tasks())) return rc;
-      k_lin_dx_tc<<<(unsigned)total, BW_THREADS, smem, st>>>(d_maps, map_wt, d_tasks, d_gt0, groups, n_groups, K, cb_width,
-                                                             dA, accumulate_dA, gelu_aux, sc);
-      HGT_LAUNCH_CHECK();
+      job.maps = d_maps;
+      job.map_wt = map_wt;
+      job.tasks = d_tasks;
+      job.group_task0 = d_gt0;
+      job.groups = groups;
+      job.n_groups = n_groups;
+      job.K_in = K;
+      job.width = cb_width;
+      job.dA = dA;
+      job.accumulate = accumulate_dA;
+      job.gelu_aux = gelu_aux;
+      switch (job.tile_n) {
+        case 64: rc = launch_bwd<64>(job, (unsigned)total, st); break;
+        case 128: rc = launch_bwd<128>(job, (unsigned)total, st); break;
+        default: rc = launch_bwd<256>(job, (unsigned)total, st); break;
+      }
+      if (rc) return rc;
     }
   }
   // 6. dW
   if (dW) {
-    const int m_tiles = (cb_width + 127) / 128, n_tiles = (K + 255) / 256;
+    const int tile_n = pick_tile_n(K);
+    const int m_tiles = (cb_width + BM - 1) / BM, n_tiles = (K + tile_n - 1) / tile_n;
     // chunk the reduction so that the grid has a few waves of CTAs
     int64_t work = 0;
     for (int t = 0; t < nt; ++t) work += tasks[t].rows * m_tiles * n_tiles;
@@ -849,12 +764,23 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
     GcTask* d_tasks2 = d_tasks;
     HGT_CHECK_CUDA(cudaMemcpyAsync(d_tasks2, tasks.data(), (size_t)nt * sizeof(GcTask), cudaMemcpyHostToDevice, st));
     if (units > 0) {
-      const int n_atoms = std::min(4, (K + 63) / 64);
-      const size_t smem = 1024 + 2 * (size_t)(2 * 2 * ATOM_BYTES + 2 * n_atoms * ATOM_BYTES) + 8 * 8 + 16;
-      HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_lin_dw_tc<<<(unsigned)units, BW_THREADS, smem, st>>>(d_maps, d_tasks2, nt, K, cb_width, m_tiles, n_tiles, (int)chunk,
-                                                             dW);
-      HGT_LAUNCH_CHECK();
+      DwJob job;
+      job.maps = d_maps;
+      job.tasks = d_tasks2;
+      job.n_tasks = nt;
+      job.K_in = K;
+      job.width = cb_width;
+      job.m_tiles = m_tiles;
+      job.n_tiles = n_tiles;
+      job.chunk_rows = (int)chunk;
+      job.tile_n = tile_n;
+      job.dW = dW;
+      switch (tile_n) {
+        case 64: rc = launch_bwd<64>(job, (unsigned)units, st); break;
+        case 128: rc = launch_bwd<128>(job, (unsigned)units, st); break;
+        default: rc = launch_bwd<256>(job, (unsigned)units, st); break;
+      }
+      if (rc) return rc;
     }
   }
   return 0;

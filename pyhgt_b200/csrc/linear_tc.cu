@@ -1,99 +1,27 @@
-// Typed linear layers on the 5th-generation tensor cores (tcgen05) with fp32-grade accuracy.
+// Typed linear layers on the Hopper tensor cores (wgmma) with fp32-grade accuracy.
 //
 // fp32 operands are split into two bf16 terms, x = x_hi + x_lo (|x - x_hi - x_lo| <= 2^-17 |x|), and
 //     A*W^T  ~=  A_hi*W_hi^T + A_hi*W_lo^T + A_lo*W_hi^T            (dropped term ~2^-18)
-// is accumulated in ONE fp32 TMEM accumulator by running three bf16 passes over K inside the same
+// is accumulated in ONE fp32 register accumulator by running three bf16 products per k-step inside the same
 // tile: 3 tensor-core products at the bf16 rate instead of an fp32 FMA GEMM, error ~1e-5 relative —
 // far inside the 1e-3 parity bar, where a single bf16 or tf32 product would not be.
 //
-// Three kernels share the TMA / UMMA / TMEM plumbing below (all: SWIZZLE_128B K-major operands, fp32 accumulate in TMEM):
-//   k_typed_linear_tc3  (default when the column block is a multiple of 256): CTA PAIR, cta_group::2, W-stationary,
-//                       persistent; 256 x 256 pair tile, double-buffered TMEM accumulator, 8-warp transposing epilogue.
-//   k_typed_linear_tc2  same design on one CTA (n-tile = widest divisor of the column block whose resident W fits).
-//   k_typed_linear_tc   one 128 x BN tile per CTA, both operands streamed (fallback for very wide K).
-// Output tiles follow the same group / column-block tables as the SIMT kernel in linear.cu.
+// k_typed_linear_tc runs tcp::split3_tile (tc_ptx.cuh): one 128 x BN output tile per CTA, a TMA producer warpgroup and two wgmma
+// consumer warpgroups, both operands K-major with SWIZZLE_128B.  Output tiles follow the same group / column-block tables
+// as the SIMT kernel in linear.cu.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "tc_ptx.cuh"
 
 namespace {
 
+using namespace tcp;
+
 constexpr int kMaxGroups = 64;
-constexpr int TC_BM = 128;
-constexpr int TC_BK = 64;              // 64 bf16 = 128 bytes = one SWIZZLE_128B row
-constexpr int TC_THREADS = 192;
-constexpr int UMMA_K = 16;
-
-struct TcTilePrefix {
-  int32_t first_tile[kMaxGroups + 1];
-  int32_t n_tiles_n;
-};
-
-// ---- PTX wrappers ------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t s_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}"
-      : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  while (!mbar_try_wait(bar, parity)) {}
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 UMMA format): rows of 128 bytes,
-// 8-row swizzle atoms 1024 bytes apart (SBO), version 1, layout type 2.
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);          // start address, bits [0,14)
-  d |= (uint64_t)1 << 16;                               // leading byte offset (ignored for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;                     // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                               // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                               // SWIZZLE_128B
-  return d;
-}
 
 // ---- fp32 -> (bf16 hi, bf16 lo) split ------------------------------------------------------------
 __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_t rows, int K, int Kp,
@@ -122,813 +50,75 @@ __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_
   *reinterpret_cast<uint2*>(lo + r * Kp + c) = *reinterpret_cast<uint2*>(l);
 }
 
-// ---- the GEMM -------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(TC_THREADS, 2)
-k_typed_linear_tc(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                  const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-                  const float* __restrict__ bias, int Kp, int cb_width, int BN, int stages, int tmem_cols,
-                  const hgt_lin_group* __restrict__ groups, int n_groups,
-                  const hgt_lin_cblock* __restrict__ cblocks, float* __restrict__ out, TcTilePrefix tp) {
-  extern __shared__ unsigned char smem_dyn[];
-  // carve: [stages][A 16 KB | B BN*128 B] (1024-aligned), then barriers, tmem pointer, bias tile
-  unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);   // keeps the shared address space
-  const uint32_t a_bytes = TC_BM * TC_BK * 2;
-  const uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;
-  const uint32_t b_bytes_al = (b_bytes + 1023) & ~1023u;
-  const uint32_t stage_bytes = a_bytes + b_bytes_al;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)stages * stage_bytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + stages;
-  uint64_t* tmem_full_bar = bars + 2 * stages;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * stages + 1);
-  float* s_bias = reinterpret_cast<float*>(tmem_ptr_smem + 2);
+// ---- the GEMM: out_cb[m, n] = A[a_row0 + m, :] . W[w_row0 + cb * cb_width + n, :] (+ bias) ------------------------------
+// Rows of a tile past the group and columns past the column block are computed on neighbouring (or zero-filled) operand
+// rows and not stored.
+struct FwdJob {
+  CUtensorMap a_hi, a_lo, w_hi, w_lo;      // A box {64, 128 rows}, W box {64, tile_n rows}
+  const float* bias;
+  const hgt_lin_group* groups;
+  const hgt_lin_cblock* cblocks;
+  float* out;
+  int n_groups, cb_width, k_blocks, tile_n, n_tiles_n;
+  int32_t first_tile[kMaxGroups + 1];
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  struct Tile {
+    int a_row, w_row, cols;
+    int64_t rows, ld;
+    float* out;
+    const float* bias;
+  };
 
-  // ---- tile decode ----
-  int tile = blockIdx.x;
-  int g = 0;
-  while (g + 1 < n_groups && tile >= tp.first_tile[g + 1]) ++g;
-  const hgt_lin_group grp = groups[g];
-  int local = tile - tp.first_tile[g];
-  const int per_m = grp.n_cblocks * tp.n_tiles_n;
-  const int mt = local / per_m;
-  local -= mt * per_m;
-  const int cb = local / tp.n_tiles_n;
-  const int nt = local - cb * tp.n_tiles_n;
-  const hgt_lin_cblock cblk = cblocks[grp.cb_first + cb];
-  const int64_t m0 = (int64_t)mt * TC_BM;
-  const int n0 = nt * BN;
-  const int a_row = (int)(grp.a_row0 + m0);
-  const int w_row = grp.w_row0 + cb * cb_width + n0;
-  const int rows_here = (int)min((int64_t)TC_BM, grp.m - m0);
-  const int k_blocks = (Kp + TC_BK - 1) / TC_BK;
-  const int total_iters = 3 * k_blocks;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_lo) : "memory");
-    for (int s = 0; s < stages; ++s) {
-      mbar_init(s_u32(&full_bar[s]), 1);
-      mbar_init(s_u32(&empty_bar[s]), 1);
-    }
-    mbar_init(s_u32(tmem_full_bar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  __device__ int decode(int tile, Tile& t) const {
+    int g = 0;
+    while (g + 1 < n_groups && tile >= first_tile[g + 1]) ++g;
+    const hgt_lin_group grp = groups[g];
+    int local = tile - first_tile[g];
+    const int per_m = grp.n_cblocks * n_tiles_n;
+    const int mt = local / per_m;
+    local -= mt * per_m;
+    const int cb = local / n_tiles_n;
+    const int n0 = (local - cb * n_tiles_n) * tile_n;
+    const hgt_lin_cblock cblk = cblocks[grp.cb_first + cb];
+    const int64_t m0 = (int64_t)mt * BM;
+    t.a_row = (int)(grp.a_row0 + m0);
+    t.w_row = grp.w_row0 + cb * cb_width + n0;
+    t.cols = cb_width - n0;
+    t.rows = grp.m - m0;
+    t.ld = cblk.ld;
+    t.out = out + cblk.out_off + m0 * cblk.ld + n0;
+    t.bias = (grp.has_bias && bias) ? bias + t.w_row : nullptr;
+    return k_blocks;
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  __device__ void prefetch(const Tile&) const {
+    prefetch_map(&a_hi); prefetch_map(&a_lo); prefetch_map(&w_hi); prefetch_map(&w_lo);
   }
-  if (warp >= 2) {
-    for (int c = threadIdx.x - 64; c < BN; c += TC_THREADS - 64)
-      s_bias[c] = (grp.has_bias && bias) ? bias[w_row + c] : 0.f;
+  template <int BN>
+  __device__ void load(const Tile& t, int kb, uint32_t sa, uint32_t bar) const {
+    tma_load_2d(sa, &a_hi, kb * BK, t.a_row, bar);
+    tma_load_2d(sa + A_BYTES, &a_lo, kb * BK, t.a_row, bar);
+    tma_load_2d(sa + 2 * A_BYTES, &w_hi, kb * BK, t.w_row, bar);
+    tma_load_2d(sa + 2 * A_BYTES + BN * BK * 2, &w_lo, kb * BK, t.w_row, bar);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer =====
-      for (int it = 0; it < total_iters; ++it) {
-        const int s = it % stages;
-        const uint32_t ph = (uint32_t)(it / stages) & 1u;
-        mbar_wait(s_u32(&empty_bar[s]), ph ^ 1u);
-        const int pass = it / k_blocks;                    // 0: hi*hi, 1: hi*lo, 2: lo*hi
-        const int kb = it - pass * k_blocks;
-        const CUtensorMap* ma = (pass == 2) ? &map_a_lo : &map_a_hi;
-        const CUtensorMap* mw = (pass == 1) ? &map_w_lo : &map_w_hi;
-        const uint32_t bar = s_u32(&full_bar[s]);
-        const uint32_t sa = s_u32(smem + (size_t)s * stage_bytes);
-        mbar_expect_tx(bar, a_bytes + b_bytes);
-        tma_load_2d(sa, ma, kb * TC_BK, a_row, bar);
-        tma_load_2d(sa + a_bytes, mw, kb * TC_BK, w_row, bar);
+  template <int BN>
+  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+    float* o = t.out + (int64_t)(64 * c) * t.ld;
+    const int64_t rows = t.rows - 64 * c;
+    const float* b = t.bias;
+    const int cols = t.cols;
+    const int64_t ld = t.ld;
+    for_each_pair<BN>(acc, wq, lane, [&](int r, int col, float v0, float v1) {
+      if (r < rows && col < cols) {
+        if (b) v0 += __ldg(b + col), v1 += __ldg(b + col + 1);
+        *reinterpret_cast<float2*>(o + r * ld + col) = make_float2(v0, v1);
       }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      // instruction descriptor: D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1), K-major A and B,
-      // N>>3 at bits 17-22, M>>4 at bits 24-28
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)(TC_BM >> 4) << 24);
-      for (int it = 0; it < total_iters; ++it) {
-        const int s = it % stages;
-        const uint32_t ph = (uint32_t)(it / stages) & 1u;
-        mbar_wait(s_u32(&full_bar[s]), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sa = s_u32(smem + (size_t)s * stage_bytes);
-        const uint64_t da = make_sw128_desc(sa);
-        const uint64_t db = make_sw128_desc(sa + a_bytes);
-#pragma unroll
-        for (int k = 0; k < TC_BK / UMMA_K; ++k) {
-          // advance 16 bf16 = 32 bytes inside the 128-byte swizzle row: +2 in the (addr >> 4) field
-          umma_bf16_ss(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(s_u32(&empty_bar[s]));                  // frees the smem slot when these MMAs retire
-      }
-      umma_commit(s_u32(tmem_full_bar));                    // accumulator complete
-    }
-  } else {
-    // ===== epilogue warps: TMEM lane group = warp % 4 =====
-    const int lg = warp & 3;
-    const int row = lg * 32 + lane;
-    mbar_wait(s_u32(tmem_full_bar), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    float* orow = out + cblk.out_off + (m0 + row) * cblk.ld + n0;
-    const bool row_ok = row < rows_here;
-    for (int c = 0; c < BN; c += 16) {
-      uint32_t r[16];
-      tmem_ld16(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)c, r);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (row_ok) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          float4 v;
-          v.x = __uint_as_float(r[j + 0]) + s_bias[c + j + 0];
-          v.y = __uint_as_float(r[j + 1]) + s_bias[c + j + 1];
-          v.z = __uint_as_float(r[j + 2]) + s_bias[c + j + 2];
-          v.w = __uint_as_float(r[j + 3]) + s_bias[c + j + 3];
-          *reinterpret_cast<float4*>(orow + c + j) = v;
-        }
-      }
-    }
+    });
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols)
-                 : "memory");
-  }
-}
-
-
-// ---- W-stationary persistent GEMM (default) -------------------------------------------------------
-// A "unit" = one column task (group, column block, n-tile of BN columns) x a chunk of up to MCH m-tiles.
-// The CTA keeps the column task's W_hi / W_lo tiles (all K) resident in shared memory, streams the A_hi / A_lo
-// k-blocks of successive m-tiles through a ring, and issues per k-block the three products
-// A_hi*W_hi + A_hi*W_lo + A_lo*W_hi into a double-buffered TMEM accumulator, so the epilogue of m-tile i
-// overlaps the MMAs of m-tile i+1.  Units are ordered m-chunk-major so that CTAs running concurrently read the
-// same A rows from L2 with different W.  L2->SM traffic per output tile drops from 384 KB (tile-per-CTA kernel
-// below) to 128 KB (+ W amortised over the chunk).
-static int tc2_mch() { static int v = [] { const char* e = getenv("HGT_TC_MCH"); int x = e ? atoi(e) : 8; return x < 1 ? 1 : x; }(); return v; }
-static int tc2_stage_cap() { static int v = [] { const char* e = getenv("HGT_TC_STAGES"); int x = e ? atoi(e) : 8; return x < 2 ? 2 : x; }(); return v; }
-
-// Epilogue of one accumulator tile, shared by the persistent kernels.  8 epilogue warps: warp e (0..7) reads TMEM
-// lane quarter (warp id % 4) and the 16-column chunks c0 = 16*(e/4), +32, ...  TMEM hands each lane one ROW, so the
-// chunk is transposed through a per-warp staging buffer and written with 4 lanes per 64 contiguous bytes of a row
-// (full 32-byte sectors).  All shared-memory reads are issued before the dependent adds / predicated stores.
-constexpr int TC2_EPI_WARPS = 8;
-constexpr int TC2_THREADS = 64 + 32 * TC2_EPI_WARPS;
-constexpr int TC2_STG_LD = 20;                 // floats per staged row (16 + 4 pad)
-constexpr int TC2_STAGE_BYTES = TC2_EPI_WARPS * 32 * TC2_STG_LD * 4;
-
-__device__ __forceinline__ void tc_epilogue_tile(uint32_t t_row, int n_cols, int chunk0, float* stg, const float* s_bias,
-                                                 float* out_tile, int64_t ld, int64_t rows_left, int lane) {
-  // out_tile: address of (first row of this warp's 32-row slab, column 0 of the tile); rows_left: valid rows in the slab
-  const int sub = lane & 3, rsel = lane >> 2;
-  for (int c0 = 16 * chunk0; c0 < n_cols; c0 += 32) {
-    uint32_t r[16];
-    tmem_ld16(t_row + (uint32_t)c0, r);
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int j = 0; j < 16; j += 4)
-      *reinterpret_cast<uint4*>(stg + lane * TC2_STG_LD + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-    __syncwarp();
-    const float4 b = *reinterpret_cast<const float4*>(s_bias + c0 + sub * 4);
-    float4 v[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) v[k] = *reinterpret_cast<const float4*>(stg + (8 * k + rsel) * TC2_STG_LD + sub * 4);
-    __syncwarp();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int rr = 8 * k + rsel;
-      if (rr < rows_left) {
-        float4 w = v[k];
-        w.x += b.x; w.y += b.y; w.z += b.z; w.w += b.w;
-        *reinterpret_cast<float4*>(out_tile + (int64_t)rr * ld + c0 + sub * 4) = w;
-      }
-    }
-  }
-}
-
-// Same tile, software-pipelined: the TMEM load of chunk i+1 is in flight while chunk i goes through the staging buffer
-// and out to global memory (two named register buffers), and the staging buffer is swizzled so that neither side has
-// bank conflicts.  Measured at C2 together with the .cta-scope pair barriers below: projection 3.90 -> 3.81 ms
-// (profiles/r02_gemm_epilogue_ab.md); see DESIGN.md section 9 for what was ruled out as the limiter.
-__device__ __forceinline__ void tc_epi_chunk(const uint32_t (&r)[16], int c0, float* stg, const float* s_bias,
-                                             float* out_tile, int64_t ld, int64_t rows_left, int lane) {
-  // staging rows of 64 bytes, the 16-byte piece j of row r kept at position j ^ ((r >> 1) & 3): the row-per-lane writes
-  // and the 4-lanes-per-row reads both touch every bank once per quarter warp (no conflicts, 4 wavefronts per access)
-  const int sub = lane & 3, rsel = lane >> 2;
-  const int wsw = (lane >> 1) & 3;
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    *reinterpret_cast<uint4*>(stg + lane * 16 + ((j ^ wsw) << 2)) =
-        make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-  __syncwarp();
-  const float4 b = *reinterpret_cast<const float4*>(s_bias + c0 + sub * 4);
-  const int rsw = (sub ^ ((rsel >> 1) & 3)) << 2;                     // (8k + rsel) >> 1 & 3 == rsel >> 1 & 3
-  float4 v[4];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) v[k] = *reinterpret_cast<const float4*>(stg + (8 * k + rsel) * 16 + rsw);
-  __syncwarp();
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int rr = 8 * k + rsel;
-    if (rr < rows_left) {
-      float4 w = v[k];
-      w.x += b.x; w.y += b.y; w.z += b.z; w.w += b.w;
-      *reinterpret_cast<float4*>(out_tile + (int64_t)rr * ld + c0 + sub * 4) = w;
-    }
-  }
-}
-
-__device__ __forceinline__ void tc_epilogue_tile_pf(uint32_t t_row, int n_cols, int chunk0, float* stg,
-                                                    const float* s_bias, float* out_tile, int64_t ld,
-                                                    int64_t rows_left, int lane) {
-  uint32_t ra[16], rb[16];
-  int c0 = 16 * chunk0;
-  if (c0 >= n_cols) return;
-  tmem_ld16(t_row + (uint32_t)c0, ra);
-  for (; c0 < n_cols; c0 += 64) {
-    const bool has_b = c0 + 32 < n_cols;
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");       // ra has landed
-    if (has_b) tmem_ld16(t_row + (uint32_t)(c0 + 32), rb);
-    tc_epi_chunk(ra, c0, stg, s_bias, out_tile, ld, rows_left, lane);
-    if (!has_b) break;
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");       // rb has landed
-    if (c0 + 64 < n_cols) tmem_ld16(t_row + (uint32_t)(c0 + 64), ra);
-    tc_epi_chunk(rb, c0 + 32, stg, s_bias, out_tile, ld, rows_left, lane);
-  }
-}
-
-// Direct drain (HGT_TC_EPI bit 2, opt-in): tcgen05.ld.16x256b hands each quad of lanes 32 contiguous bytes of an
-// accumulator row (the m16n8 fragment layout: registers {0,1} = row lane/4, columns 2*(lane%4)+{0,1}; {2,3} = row
-// lane/4 + 8; the next four registers the next 8 columns), so the tile goes from registers to global memory as full
-// 32-byte sectors with no trip through shared memory.  A warp covers its 32 TMEM lanes with two 16-lane loads.
-// Parity-green on the whole GPU suite and the SAME speed as the staged drain at C2 (projection 3.778 vs 3.788 ms,
-// profiles/r02_gemm_epilogue_ab.md) — so the transpose's share of the shared-memory port is not what holds the kernel;
-// kept as an option because it needs no staging buffer.
-__device__ __forceinline__ void tmem_ld_16x256b_x2(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.16x256b.x2.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-
-__device__ __forceinline__ void tc_epi_direct_store(const uint32_t (&v)[8], int row0, int c0, const float* s_bias,
-                                                    float* out_tile, int64_t ld, int64_t rows_left, int lane) {
-  const int q = lane & 3, r0 = row0 + (lane >> 2);
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int col = c0 + 8 * i + 2 * q;
-    const float2 b = *reinterpret_cast<const float2*>(s_bias + col);
-    if (r0 < rows_left)
-      *reinterpret_cast<float2*>(out_tile + (int64_t)r0 * ld + col) =
-          make_float2(__uint_as_float(v[4 * i]) + b.x, __uint_as_float(v[4 * i + 1]) + b.y);
-    if (r0 + 8 < rows_left)
-      *reinterpret_cast<float2*>(out_tile + (int64_t)(r0 + 8) * ld + col) =
-          make_float2(__uint_as_float(v[4 * i + 2]) + b.x, __uint_as_float(v[4 * i + 3]) + b.y);
-  }
-}
-
-__device__ __forceinline__ void tc_epilogue_tile_direct(uint32_t t_row, int n_cols, int chunk0, const float* s_bias,
-                                                        float* out_tile, int64_t ld, int64_t rows_left, int lane) {
-  uint32_t a0[8], a1[8], b0[8], b1[8];                       // (rows 0-15, rows 16-31) of two chunks in flight
-  int c0 = 16 * chunk0;
-  if (c0 >= n_cols) return;
-  tmem_ld_16x256b_x2(t_row + (uint32_t)c0, a0);
-  tmem_ld_16x256b_x2(t_row + (16u << 16) + (uint32_t)c0, a1);
-  for (; c0 < n_cols; c0 += 64) {
-    const bool has_b = c0 + 32 < n_cols;
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    if (has_b) {
-      tmem_ld_16x256b_x2(t_row + (uint32_t)(c0 + 32), b0);
-      tmem_ld_16x256b_x2(t_row + (16u << 16) + (uint32_t)(c0 + 32), b1);
-    }
-    tc_epi_direct_store(a0, 0, c0, s_bias, out_tile, ld, rows_left, lane);
-    tc_epi_direct_store(a1, 16, c0, s_bias, out_tile, ld, rows_left, lane);
-    if (!has_b) break;
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    if (c0 + 64 < n_cols) {
-      tmem_ld_16x256b_x2(t_row + (uint32_t)(c0 + 64), a0);
-      tmem_ld_16x256b_x2(t_row + (16u << 16) + (uint32_t)(c0 + 64), a1);
-    }
-    tc_epi_direct_store(b0, 0, c0 + 32, s_bias, out_tile, ld, rows_left, lane);
-    tc_epi_direct_store(b1, 16, c0 + 32, s_bias, out_tile, ld, rows_left, lane);
-  }
-}
-
-struct Tc2Sched {
-  int32_t first_unit[kMaxGroups + 1];
-  int32_t n_tiles_n;
-  int32_t epi;                                   // bit 0: pipelined epilogue; bit 1: .cta-scope pair barriers; bit 2: direct drain (default 3)
 };
-static int tc2_epi() { static int v = [] { const char* e = getenv("HGT_TC_EPI"); return e ? atoi(e) : 3; }(); return v; }
 
-__global__ void __launch_bounds__(TC2_THREADS, 1)
-k_typed_linear_tc2(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                   const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-                   const float* __restrict__ bias, int Kp, int cb_width, int BN, int stages, int tmem_cols,
-                   const hgt_lin_group* __restrict__ groups, int n_groups,
-                   const hgt_lin_cblock* __restrict__ cblocks, float* __restrict__ out, Tc2Sched sc, int MCH) {
-  extern __shared__ unsigned char smem_dyn[];
-  unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);   // keeps the shared address space
-  const int k_blocks = (Kp + TC_BK - 1) / TC_BK;
-  const uint32_t a_bytes = TC_BM * TC_BK * 2;                       // one A tile (hi or lo)
-  const uint32_t b_bytes = (uint32_t)BN * TC_BK * 2;                // one W tile (hi or lo)
-  const uint32_t b_bytes_al = (b_bytes + 1023) & ~1023u;
-  const uint32_t w_region = (uint32_t)k_blocks * 2 * b_bytes_al;    // resident W
-  const uint32_t a_stage = a_bytes;                                 // one tile per stage: A_hi(kb), A_lo(kb), A_hi(kb+1), ...
-  unsigned char* w_smem = smem;
-  unsigned char* a_smem = smem + w_region;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + (size_t)stages * a_stage);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = bars + stages;
-  uint64_t* w_full = bars + 2 * stages;
-  uint64_t* w_empty = w_full + 1;
-  uint64_t* t_full = w_empty + 1;       // [2]
-  uint64_t* t_empty = t_full + 2;       // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(t_empty + 2);
-  float* s_bias = reinterpret_cast<float*>(tmem_ptr_smem + 4);        // 16-byte aligned: the barrier block is 16*(stages+3) B
-  float* s_stage = s_bias + ((BN + 3) & ~3);                          // [4 warps][32][TC2_STG_LD] epilogue transpose
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int total_units = sc.first_unit[n_groups];
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_lo) : "memory");
-    for (int s = 0; s < stages; ++s) {
-      mbar_init(s_u32(&a_full[s]), 1);
-      mbar_init(s_u32(&a_empty[s]), 1);
-    }
-    mbar_init(s_u32(w_full), 1);
-    mbar_init(s_u32(w_empty), 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(s_u32(&t_full[b]), 1);
-      mbar_init(s_u32(&t_empty[b]), TC2_EPI_WARPS);                  // one arrival per epilogue warp
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  // unit decode shared by all roles
-  struct Unit { int64_t m_first; int n_mt; int a_row0; int w_row; int64_t m_rows; int64_t out_off; int64_t ld; int n0;
-                int has_bias; };
-  auto decode = [&](int u, Unit& un) {
-    int g = 0;
-    while (g + 1 < n_groups && u >= sc.first_unit[g + 1]) ++g;
-    const hgt_lin_group grp = groups[g];
-    int local = u - sc.first_unit[g];
-    const int ncol = grp.n_cblocks * sc.n_tiles_n;
-    const int chunk = local / ncol;
-    const int col = local - chunk * ncol;
-    const int cb = col / sc.n_tiles_n;
-    const int nt = col - cb * sc.n_tiles_n;
-    const hgt_lin_cblock cblk = cblocks[grp.cb_first + cb];
-    const int64_t mt_total = (grp.m + TC_BM - 1) / TC_BM;
-    un.m_first = (int64_t)chunk * MCH;
-    un.n_mt = (int)min((int64_t)MCH, mt_total - un.m_first);
-    un.a_row0 = (int)grp.a_row0;
-    un.m_rows = grp.m;
-    un.n0 = nt * BN;
-    un.w_row = grp.w_row0 + cb * cb_width + un.n0;
-    un.out_off = cblk.out_off;
-    un.ld = cblk.ld;
-    un.has_bias = grp.has_bias;
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer =====
-      uint32_t a_it = 0, unit_it = 0;
-      for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++unit_it) {
-        Unit un;
-        decode(u, un);
-        mbar_wait(s_u32(w_empty), (unit_it & 1u) ^ 1u);               // previous unit's MMAs are done with W
-        mbar_expect_tx(s_u32(w_full), (uint32_t)k_blocks * 2 * b_bytes);
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          tma_load_2d(s_u32(w_smem + (size_t)(2 * kb) * b_bytes_al), &map_w_hi, kb * TC_BK, un.w_row, s_u32(w_full));
-          tma_load_2d(s_u32(w_smem + (size_t)(2 * kb + 1) * b_bytes_al), &map_w_lo, kb * TC_BK, un.w_row, s_u32(w_full));
-        }
-        for (int mt = 0; mt < un.n_mt; ++mt) {
-          const int a_row = un.a_row0 + (int)((un.m_first + mt) * TC_BM);
-          for (int j = 0; j < 2 * k_blocks; ++j, ++a_it) {
-            const int s = a_it % stages;
-            mbar_wait(s_u32(&a_empty[s]), ((a_it / stages) & 1u) ^ 1u);
-            const uint32_t bar = s_u32(&a_full[s]);
-            mbar_expect_tx(bar, a_bytes);
-            tma_load_2d(s_u32(a_smem + (size_t)s * a_stage), (j & 1) ? &map_a_lo : &map_a_hi, (j >> 1) * TC_BK, a_row, bar);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)(TC_BM >> 4) << 24);
-      uint32_t a_it = 0, unit_it = 0, acc_it = 0;
-      for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++unit_it) {
-        Unit un;
-        decode(u, un);
-        mbar_wait(s_u32(w_full), unit_it & 1u);
-        for (int mt = 0; mt < un.n_mt; ++mt, ++acc_it) {
-          const uint32_t buf = acc_it & 1u;
-          mbar_wait(s_u32(&t_empty[buf]), ((acc_it >> 1) & 1u) ^ 1u);  // epilogue drained this accumulator
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t tmem_d = tmem_base + buf * (uint32_t)BN;
-          for (int j = 0; j < 2 * k_blocks; ++j, ++a_it) {
-            const int s = a_it % stages;
-            const int kb = j >> 1;
-            mbar_wait(s_u32(&a_full[s]), (a_it / stages) & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t d_a = make_sw128_desc(s_u32(a_smem + (size_t)s * a_stage));
-            const uint64_t d_whi = make_sw128_desc(s_u32(w_smem + (size_t)(2 * kb) * b_bytes_al));
-            if (!(j & 1)) {
-              // A_hi(kb): A_hi*W_hi + A_hi*W_lo
-              const uint64_t d_wlo = make_sw128_desc(s_u32(w_smem + (size_t)(2 * kb + 1) * b_bytes_al));
-#pragma unroll
-              for (int k = 0; k < TC_BK / UMMA_K; ++k) {
-                const uint64_t o = (uint64_t)(2 * k);
-                umma_bf16_ss(tmem_d, d_a + o, d_whi + o, idesc, (j > 0 || k > 0) ? 1u : 0u);
-                umma_bf16_ss(tmem_d, d_a + o, d_wlo + o, idesc, 1u);
-              }
-            } else {
-              // A_lo(kb): A_lo*W_hi
-#pragma unroll
-              for (int k = 0; k < TC_BK / UMMA_K; ++k) {
-                const uint64_t o = (uint64_t)(2 * k);
-                umma_bf16_ss(tmem_d, d_a + o, d_whi + o, idesc, 1u);
-              }
-            }
-            umma_commit(s_u32(&a_empty[s]));
-          }
-          umma_commit(s_u32(&t_full[buf]));
-        }
-        umma_commit(s_u32(w_empty));
-      }
-    }
-  } else {
-    // ===== epilogue warps (8) =====
-    const int lg = warp & 3;
-    const int e = warp - 2;
-    const int et = threadIdx.x - 64;
-    float* stg = s_stage + (size_t)e * (32 * TC2_STG_LD);
-    uint32_t acc_it = 0;
-    for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
-      Unit un;
-      decode(u, un);
-      asm volatile("bar.sync 1, 256;" ::: "memory");               // previous unit's bias reads are finished
-      for (int c = et; c < BN; c += 32 * TC2_EPI_WARPS) s_bias[c] = (un.has_bias && bias) ? bias[un.w_row + c] : 0.f;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int mt = 0; mt < un.n_mt; ++mt, ++acc_it) {
-        const uint32_t buf = acc_it & 1u;
-        mbar_wait(s_u32(&t_full[buf]), (acc_it >> 1) & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int64_t m0 = (un.m_first + mt) * TC_BM + lg * 32;
-        if (sc.epi & 4)
-          tc_epilogue_tile_direct(tmem_base + ((uint32_t)(lg * 32) << 16) + buf * (uint32_t)BN, BN, e >> 2, s_bias,
-                                  out + un.out_off + m0 * un.ld + un.n0, un.ld, un.m_rows - m0, lane);
-        else if (sc.epi & 1)
-          tc_epilogue_tile_pf(tmem_base + ((uint32_t)(lg * 32) << 16) + buf * (uint32_t)BN, BN, e >> 2, stg, s_bias,
-                              out + un.out_off + m0 * un.ld + un.n0, un.ld, un.m_rows - m0, lane);
-        else
-          tc_epilogue_tile(tmem_base + ((uint32_t)(lg * 32) << 16) + buf * (uint32_t)BN, BN, e >> 2, stg, s_bias,
-                           out + un.out_off + m0 * un.ld + un.n0, un.ld, un.m_rows - m0, lane);
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(&t_empty[buf])) : "memory");
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols)
-                 : "memory");
-  }
-}
-
-
-// ---- 2-CTA (cta_group::2) W-stationary persistent GEMM -------------------------------------------
-// A CTA pair (cluster of 2, same TPC) computes a 256 x 256 tile per step: each CTA owns 128 rows of A / of the
-// accumulator and keeps HALF of the column task's W (128 of the 256 columns, all K, hi + lo) resident; the
-// tcgen05.mma.cta_group::2 instruction issued by the leader reads both halves of W from the two CTAs' shared
-// memory.  Each A byte streamed from L2 now feeds a 256-column product, so the A stream needs half the
-// bandwidth / in-flight bytes of the single-CTA kernel above (which it could not sustain: TMA-latency-bound at
-// ~45 % tensor-pipe utilisation).
-// Barrier protocol: a_full / w_full live in the LEADER (both CTAs' TMA loads complete_tx there through the
-// peer-bit-masked address, the leader's producer posts expect_tx for both); a_empty / w_empty / t_full are
-// per-CTA and signalled by multicast tcgen05.commit; t_empty lives in the leader and collects the 8 epilogue
-// warps of the pair.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_dst), "l"(map), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"((uint16_t)3)
-      : "memory");
-}
-// Barrier traffic between the two CTAs of a pair carries no generic-proxy data: operands arrive through TMA
-// (complete_tx), accumulators are handed over with tcgen05.commit / tcgen05.fence.  The arrive / wait therefore use the
-// default .cta-scope forms.  (The .release.cluster arrive compiles to MEMBAR.ALL.GPU + ERRBAR, which made every
-// epilogue warp wait for its global stores to be acknowledged before it could hand the accumulator back, and the
-// .acquire.cluster wait adds an L1 invalidate per wait: profiles/r02_gemm_tc3_c2_epi1_ncu_raw.csv, stall_membar = 20 %
-// of the warp samples.)
-// `strong` keeps the old forms for A/B runs (HGT_TC_EPI bit 1 clear).
-__device__ __forceinline__ void mbar_arrive_cta(uint32_t bar, uint32_t cta, bool strong) {
-  if (strong)
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-        "}"
-        ::"r"(bar), "r"(cta)
-        : "memory");
-  else
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-        "}"
-        ::"r"(bar), "r"(cta)
-        : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity, bool strong) {
-  uint32_t ok = 0;
-  if (strong) {
-    while (!ok) {
-      asm volatile(
-          "{\n\t"
-          ".reg .pred p;\n\t"
-          "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-          "selp.u32 %0, 1, 0, p;\n\t"
-          "}"
-          : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    }
-  } else {
-    while (!ok) {
-      asm volatile(
-          "{\n\t"
-          ".reg .pred p;\n\t"
-          "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-          "selp.u32 %0, 1, 0, p;\n\t"
-          "}"
-          : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    }
-  }
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC2_THREADS, 1)
-k_typed_linear_tc3(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                   const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-                   const float* __restrict__ bias, int Kp, int cb_width, int stages,
-                   const hgt_lin_group* __restrict__ groups, int n_groups,
-                   const hgt_lin_cblock* __restrict__ cblocks, float* __restrict__ out, Tc2Sched sc, int MCH) {
-  constexpr int BNH = 128;              // W columns resident per CTA
-  constexpr int BNP = 256;              // columns per pair step
-  constexpr int BMP = 256;              // rows per pair step
-  extern __shared__ unsigned char smem_dyn[];
-  unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);
-  const int k_blocks = (Kp + TC_BK - 1) / TC_BK;
-  const uint32_t a_bytes = TC_BM * TC_BK * 2;
-  const uint32_t b_bytes = (uint32_t)BNH * TC_BK * 2;               // 16 KB
-  const uint32_t w_region = (uint32_t)k_blocks * 2 * b_bytes;
-  unsigned char* w_smem = smem;
-  unsigned char* a_smem = smem + w_region;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + (size_t)stages * a_bytes);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = bars + stages;
-  uint64_t* w_full = bars + 2 * stages;
-  uint64_t* w_empty = w_full + 1;
-  uint64_t* t_full = w_empty + 1;       // [2]
-  uint64_t* t_empty = t_full + 2;       // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(t_empty + 2);
-  float* s_bias = reinterpret_cast<float*>(tmem_ptr_smem + 4);
-  float* s_stage = s_bias + BNP;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta = cluster_ctarank();
-  const bool leader = cta == 0;
-  const int pair_id = blockIdx.x >> 1;
-  const int n_pairs = gridDim.x >> 1;
-  const int total_units = sc.first_unit[n_groups];
-  const bool strong = !(sc.epi & 2);
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w_lo) : "memory");
-    for (int s = 0; s < stages; ++s) {
-      mbar_init(s_u32(&a_full[s]), 1);
-      mbar_init(s_u32(&a_empty[s]), 1);
-    }
-    mbar_init(s_u32(w_full), 1);
-    mbar_init(s_u32(w_empty), 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(s_u32(&t_full[b]), 1);
-      mbar_init(s_u32(&t_empty[b]), 2 * TC2_EPI_WARPS);              // epilogue warps of both CTAs (used in the leader)
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  cluster_sync_all();                                                // both CTAs' barriers exist before any remote arrive
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr_smem)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  struct Unit { int64_t pm_first; int n_pm; int a_row0; int w_row; int64_t m_rows; int64_t out_off; int64_t ld; int n0;
-                int has_bias; };
-  auto decode = [&](int u, Unit& un) {
-    int g = 0;
-    while (g + 1 < n_groups && u >= sc.first_unit[g + 1]) ++g;
-    const hgt_lin_group grp = groups[g];
-    int local = u - sc.first_unit[g];
-    const int ncol = grp.n_cblocks * sc.n_tiles_n;
-    const int chunk = local / ncol;
-    const int col = local - chunk * ncol;
-    const int cb = col / sc.n_tiles_n;
-    const int nt = col - cb * sc.n_tiles_n;
-    const hgt_lin_cblock cblk = cblocks[grp.cb_first + cb];
-    const int64_t pm_total = (grp.m + BMP - 1) / BMP;
-    un.pm_first = (int64_t)chunk * MCH;
-    un.n_pm = (int)min((int64_t)MCH, pm_total - un.pm_first);
-    un.a_row0 = (int)grp.a_row0;
-    un.m_rows = grp.m;
-    un.n0 = nt * BNP;
-    un.w_row = grp.w_row0 + cb * cb_width + un.n0;
-    un.out_off = cblk.out_off;
-    un.ld = cblk.ld;
-    un.has_bias = grp.has_bias;
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (both CTAs) =====
-      uint32_t a_it = 0, unit_it = 0;
-      for (int u = pair_id; u < total_units; u += n_pairs, ++unit_it) {
-        Unit un;
-        decode(u, un);
-        mbar_wait_cluster(s_u32(w_empty), (unit_it & 1u) ^ 1u, strong);
-        if (leader) mbar_expect_tx(s_u32(w_full), 2u * (uint32_t)k_blocks * 2 * b_bytes);
-        const int w_row = un.w_row + (int)cta * BNH;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          tma_load_2d_2sm(s_u32(w_smem + (size_t)(2 * kb) * b_bytes), &map_w_hi, kb * TC_BK, w_row, s_u32(w_full));
-          tma_load_2d_2sm(s_u32(w_smem + (size_t)(2 * kb + 1) * b_bytes), &map_w_lo, kb * TC_BK, w_row, s_u32(w_full));
-        }
-        for (int pm = 0; pm < un.n_pm; ++pm) {
-          const int a_row = un.a_row0 + (int)((un.pm_first + pm) * BMP) + (int)cta * TC_BM;
-          for (int j = 0; j < 2 * k_blocks; ++j, ++a_it) {
-            const int s = a_it % stages;
-            mbar_wait_cluster(s_u32(&a_empty[s]), ((a_it / stages) & 1u) ^ 1u, strong);
-            const uint32_t bar = s_u32(&a_full[s]);
-            if (leader) mbar_expect_tx(bar, 2u * a_bytes);
-            tma_load_2d_2sm(s_u32(a_smem + (size_t)s * a_bytes), (j & 1) ? &map_a_lo : &map_a_hi, (j >> 1) * TC_BK,
-                            a_row, bar);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ===== MMA issuer (leader CTA only) =====
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BNP >> 3) << 17) |
-                             ((uint32_t)(BMP >> 4) << 24);
-      uint32_t a_it = 0, unit_it = 0, acc_it = 0;
-      for (int u = pair_id; u < total_units; u += n_pairs, ++unit_it) {
-        Unit un;
-        decode(u, un);
-        mbar_wait_cluster(s_u32(w_full), unit_it & 1u, strong);
-        for (int pm = 0; pm < un.n_pm; ++pm, ++acc_it) {
-          const uint32_t buf = acc_it & 1u;
-          mbar_wait_cluster(s_u32(&t_empty[buf]), ((acc_it >> 1) & 1u) ^ 1u, strong);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t tmem_d = tmem_base + buf * (uint32_t)BNP;
-          for (int j = 0; j < 2 * k_blocks; ++j, ++a_it) {
-            const int s = a_it % stages;
-            const int kb = j >> 1;
-            mbar_wait_cluster(s_u32(&a_full[s]), (a_it / stages) & 1u, strong);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t d_a = make_sw128_desc(s_u32(a_smem + (size_t)s * a_bytes));
-            const uint64_t d_whi = make_sw128_desc(s_u32(w_smem + (size_t)(2 * kb) * b_bytes));
-            if (!(j & 1)) {
-              const uint64_t d_wlo = make_sw128_desc(s_u32(w_smem + (size_t)(2 * kb + 1) * b_bytes));
-#pragma unroll
-              for (int k = 0; k < TC_BK / UMMA_K; ++k) {
-                const uint64_t o = (uint64_t)(2 * k);
-                umma_bf16_ss_2sm(tmem_d, d_a + o, d_whi + o, idesc, (j > 0 || k > 0) ? 1u : 0u);
-                umma_bf16_ss_2sm(tmem_d, d_a + o, d_wlo + o, idesc, 1u);
-              }
-            } else {
-#pragma unroll
-              for (int k = 0; k < TC_BK / UMMA_K; ++k) {
-                const uint64_t o = (uint64_t)(2 * k);
-                umma_bf16_ss_2sm(tmem_d, d_a + o, d_whi + o, idesc, 1u);
-              }
-            }
-            umma_commit_2sm(s_u32(&a_empty[s]));
-          }
-          umma_commit_2sm(s_u32(&t_full[buf]));
-        }
-        umma_commit_2sm(s_u32(w_empty));
-      }
-    }
-  } else {
-    // ===== epilogue warps (8 per CTA): own 128 rows x 256 columns =====
-    const int lg = warp & 3;
-    const int e = warp - 2;
-    const int et = threadIdx.x - 64;
-    float* stg = s_stage + (size_t)e * (32 * TC2_STG_LD);
-    uint32_t acc_it = 0;
-    for (int u = pair_id; u < total_units; u += n_pairs) {
-      Unit un;
-      decode(u, un);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int c = et; c < BNP; c += 32 * TC2_EPI_WARPS) s_bias[c] = (un.has_bias && bias) ? bias[un.w_row + c] : 0.f;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int pm = 0; pm < un.n_pm; ++pm, ++acc_it) {
-        const uint32_t buf = acc_it & 1u;
-        mbar_wait_cluster(s_u32(&t_full[buf]), (acc_it >> 1) & 1u, strong);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int64_t m0 = (un.pm_first + pm) * BMP + (int64_t)cta * TC_BM + lg * 32;
-        if (sc.epi & 4)
-          tc_epilogue_tile_direct(tmem_base + ((uint32_t)(lg * 32) << 16) + buf * (uint32_t)BNP, BNP, e >> 2, s_bias,
-                                  out + un.out_off + m0 * un.ld + un.n0, un.ld, un.m_rows - m0, lane);
-        else if (sc.epi & 1)
-          tc_epilogue_tile_pf(tmem_base + ((uint32_t)(lg * 32) << 16) + buf * (uint32_t)BNP, BNP, e >> 2, stg, s_bias,
-                              out + un.out_off + m0 * un.ld + un.n0, un.ld, un.m_rows - m0, lane);
-        else
-          tc_epilogue_tile(tmem_base + ((uint32_t)(lg * 32) << 16) + buf * (uint32_t)BNP, BNP, e >> 2, stg, s_bias,
-                           out + un.out_off + m0 * un.ld + un.n0, un.ld, un.m_rows - m0, lane);
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cta(s_u32(&t_empty[buf]), 0, strong);      // the leader's barrier collects both CTAs
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  cluster_sync_all();                                                // peer may still be reading our W through the MMA
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
+template <int BN>
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob job) {
+  split3_tile<BN, false>(job);
 }
 
 // ---- host side ------------------------------------------------------------------------------------
@@ -953,19 +143,13 @@ int make_map(CUtensorMap* m, const void* base, int64_t rows, int Kp, int box_row
   HGT_REQUIRE(fn != nullptr, "hgt_typed_linear: cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)Kp * 2};
-  cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   HGT_REQUIRE(r == CUDA_SUCCESS, "hgt_typed_linear: cuTensorMapEncodeTiled failed (%d) rows=%lld Kp=%d box=%d",
               (int)r, (long long)rows, Kp, box_rows);
-  return 0;
-}
-
-int pick_bn(int cb_width) {
-  for (int bn = 128; bn >= 16; bn -= 16)
-    if (cb_width % bn == 0) return bn;
   return 0;
 }
 
@@ -980,14 +164,20 @@ void extents(const hgt_lin_group* h_groups, int n_groups, int cb_width, int64_t*
   }
 }
 
-}  // namespace
+template <int BN>
+int launch_fwd(const FwdJob& job, unsigned tiles, cudaStream_t st) {
+  const size_t smem = tile_smem_bytes<BN>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_typed_linear_tc<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
 
-static const bool g_tc_no_pair = [] { const char* e = getenv("HGT_TC_NO_PAIR"); return e && e[0] == '1'; }();
-static const bool g_tc_tile_per_cta = [] { const char* e = getenv("HGT_TC_TILE_PER_CTA"); return e && e[0] == '1'; }();
+}  // namespace
 
 bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width) {
   (void)lda;
-  return cb_width % 16 == 0 && pick_bn(cb_width) > 0 && K >= TC_BK;
+  return cb_width % 16 == 0 && cb_width > 0 && K >= BK;
 }
 
 size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width) {
@@ -1044,8 +234,8 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
                   const float* W, const float* bias, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
                   const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, float* out,
                   void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  const int BN = pick_bn(cb_width);
-  HGT_REQUIRE(BN > 0, "hgt_typed_linear(tc): cb_width=%d has no multiple-of-16 tile", cb_width);
+  HGT_REQUIRE(hgt_typed_linear_tc_supported(lda, K, cb_width), "hgt_typed_linear(tc): unsupported K=%d cb_width=%d", K,
+              cb_width);
   const int Kp = (K + 7) / 8 * 8;
   int64_t a_rows, w_rows;
   extents(h_groups, n_groups, cb_width, &a_rows, &w_rows);
@@ -1070,121 +260,32 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
     if (n > 0) k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, K, w_rows, K, Kp, w_hi, w_lo);
     HGT_LAUNCH_CHECK();
   }
-  CUtensorMap m_a_hi, m_a_lo, m_w_hi, m_w_lo;
-  int rc;
-  if ((rc = make_map(&m_a_hi, a_hi, a_rows, Kp, TC_BM))) return rc;
-  if ((rc = make_map(&m_a_lo, a_lo, a_rows, Kp, TC_BM))) return rc;
-  if ((rc = make_map(&m_w_hi, w_hi, w_rows, Kp, BN))) return rc;
-  if ((rc = make_map(&m_w_lo, w_lo, w_rows, Kp, BN))) return rc;
-
-  const int k_blocks = (Kp + TC_BK - 1) / TC_BK;
-  if (!g_tc_tile_per_cta && !g_tc_no_pair && cb_width % 256 == 0) {
-    // ---- 2-CTA kernel: 128 W columns resident per CTA, pair tile 256 x 256 ----
-    const size_t w_region = (size_t)k_blocks * 2 * 128 * TC_BK * 2;
-    const size_t a_stage = (size_t)TC_BM * TC_BK * 2;
-    const size_t misc = 1024 + 256 + 256 * 4 + 64 + TC2_STAGE_BYTES + 1024;
-    if (w_region + misc + 4 * a_stage <= 227 * 1024) {
-      int stages = (int)((227 * 1024 - w_region - misc) / a_stage);
-      if (stages > tc2_stage_cap()) stages = tc2_stage_cap();
-      Tc2Sched sc;
-      const int mch = tc2_mch();
-      sc.n_tiles_n = cb_width / 256;
-      sc.epi = tc2_epi();
-      int64_t units = 0;
-      for (int g = 0; g < n_groups; ++g) {
-        sc.first_unit[g] = (int32_t)units;
-        int64_t pm = (h_groups[g].m + 255) / 256;
-        units += (pm + mch - 1) / mch * h_groups[g].n_cblocks * sc.n_tiles_n;
-        HGT_REQUIRE(units < 2147483647ll, "hgt_typed_linear(tc): too many units");
-      }
-      sc.first_unit[n_groups] = (int32_t)units;
-      if (units == 0) return 0;
-      if ((rc = make_map(&m_w_hi, w_hi, w_rows, Kp, 128))) return rc;
-      if ((rc = make_map(&m_w_lo, w_lo, w_rows, Kp, 128))) return rc;
-      size_t smem = 1024 + w_region + (size_t)stages * a_stage + (2 * stages + 6) * 8 + 16 + 256 * 4 + 64 +
-                    TC2_STAGE_BYTES;
-      int pairs = hgt_sm_count() / 2;
-      if (pairs > units) pairs = (int)units;
-      HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_typed_linear_tc3<<<2 * pairs, TC2_THREADS, smem, st>>>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, bias, Kp, cb_width,
-                                                               stages, groups, n_groups, cblocks, out, sc, mch);
-      HGT_LAUNCH_CHECK();
-      return 0;
-    }
-  }
-  if (!g_tc_tile_per_cta) {
-    // ---- W-stationary persistent kernel ----
-    // widest n-tile whose resident W (all K, hi + lo) still leaves room for >= 4 A stages of 16 KB
-    const size_t a_stage = (size_t)TC_BM * TC_BK * 2;
-    int bn = 0, stages = 0;
-    size_t w_region = 0;
-    for (int c = 128; c >= 16; c -= 16) {
-      if (cb_width % c) continue;
-      const size_t wr = (size_t)k_blocks * 2 * (((size_t)c * TC_BK * 2 + 1023) & ~(size_t)1023);
-      const size_t misc = 1024 + 256 + (size_t)c * 4 + 64 + TC2_STAGE_BYTES + 1024;
-      if (wr + misc + 4 * a_stage > 227 * 1024) continue;
-      bn = c;
-      w_region = wr;
-      stages = (int)((227 * 1024 - wr - misc) / a_stage);
-      break;
-    }
-    if (bn > 0) {
-      if (stages > tc2_stage_cap()) stages = tc2_stage_cap();
-      if (stages >= 2) {
-        Tc2Sched sc;
-        const int mch = tc2_mch();
-        sc.n_tiles_n = cb_width / bn;
-        sc.epi = tc2_epi();
-        int64_t units = 0;
-        for (int g = 0; g < n_groups; ++g) {
-          sc.first_unit[g] = (int32_t)units;
-          int64_t mt = (h_groups[g].m + TC_BM - 1) / TC_BM;
-          units += (mt + mch - 1) / mch * h_groups[g].n_cblocks * sc.n_tiles_n;
-          HGT_REQUIRE(units < 2147483647ll, "hgt_typed_linear(tc): too many units");
-        }
-        sc.first_unit[n_groups] = (int32_t)units;
-        if (units == 0) return 0;
-        if ((rc = make_map(&m_w_hi, w_hi, w_rows, Kp, bn))) return rc;
-        if ((rc = make_map(&m_w_lo, w_lo, w_rows, Kp, bn))) return rc;
-        int tmem_cols = 32;
-        while (tmem_cols < 2 * bn) tmem_cols <<= 1;
-        size_t smem = 1024 + w_region + (size_t)stages * a_stage + (2 * stages + 6) * 8 + 16 + (size_t)bn * 4 + 64 +
-                      TC2_STAGE_BYTES;
-        HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int grid = hgt_sm_count();
-        if (grid > units) grid = (int)units;
-        k_typed_linear_tc2<<<grid, TC2_THREADS, smem, st>>>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, bias, Kp, cb_width, bn,
-                                                            stages, tmem_cols, groups, n_groups, cblocks, out, sc, mch);
-        HGT_LAUNCH_CHECK();
-        return 0;
-      }
-    }
-  }
-  // ---- one tile per CTA (fallback for very wide K; HGT_TC_TILE_PER_CTA=1 forces it) ----
-  TcTilePrefix tp;
-  tp.n_tiles_n = cb_width / BN;
+  FwdJob job;
+  job.tile_n = pick_tile_n(cb_width);
+  job.n_tiles_n = (cb_width + job.tile_n - 1) / job.tile_n;
   int64_t total = 0;
   for (int g = 0; g < n_groups; ++g) {
-    tp.first_tile[g] = (int32_t)total;
-    total += (h_groups[g].m + TC_BM - 1) / TC_BM * h_groups[g].n_cblocks * tp.n_tiles_n;
+    job.first_tile[g] = (int32_t)total;
+    total += (h_groups[g].m + BM - 1) / BM * h_groups[g].n_cblocks * job.n_tiles_n;
     HGT_REQUIRE(total < 2147483647ll, "hgt_typed_linear(tc): too many tiles");
   }
-  tp.first_tile[n_groups] = (int32_t)total;
+  job.first_tile[n_groups] = (int32_t)total;
   if (total == 0) return 0;
-
-  const uint32_t a_bytes = TC_BM * TC_BK * 2;
-  const uint32_t b_bytes_al = ((uint32_t)BN * TC_BK * 2 + 1023) & ~1023u;
-  const uint32_t stage_bytes = a_bytes + b_bytes_al;
-  int stages = (int)((100 * 1024) / stage_bytes);
-  if (stages > 6) stages = 6;
-  if (stages < 2) stages = 2;
-  int tmem_cols = 32;
-  while (tmem_cols < BN) tmem_cols <<= 1;
-  size_t smem = 1024 + (size_t)stages * stage_bytes + (2 * stages + 1) * 8 + 16 + (size_t)BN * 4 + 64;
-  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_typed_linear_tc<<<(unsigned)total, TC_THREADS, smem, st>>>(m_a_hi, m_a_lo, m_w_hi, m_w_lo, bias, Kp, cb_width,
-                                                               BN, stages, tmem_cols, groups, n_groups, cblocks, out,
-                                                               tp);
-  HGT_LAUNCH_CHECK();
-  return 0;
+  int rc;
+  if ((rc = make_map(&job.a_hi, a_hi, a_rows, Kp, BM))) return rc;
+  if ((rc = make_map(&job.a_lo, a_lo, a_rows, Kp, BM))) return rc;
+  if ((rc = make_map(&job.w_hi, w_hi, w_rows, Kp, job.tile_n))) return rc;
+  if ((rc = make_map(&job.w_lo, w_lo, w_rows, Kp, job.tile_n))) return rc;
+  job.bias = bias;
+  job.groups = groups;
+  job.cblocks = cblocks;
+  job.out = out;
+  job.n_groups = n_groups;
+  job.cb_width = cb_width;
+  job.k_blocks = (Kp + BK - 1) / BK;
+  switch (job.tile_n) {
+    case 64: return launch_fwd<64>(job, (unsigned)total, st);
+    case 128: return launch_fwd<128>(job, (unsigned)total, st);
+    default: return launch_fwd<256>(job, (unsigned)total, st);
+  }
 }

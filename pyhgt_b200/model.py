@@ -3,7 +3,7 @@ stack of ``GeneralConv('hgt')`` layers — SURVEY.md §8(f) rank 1.  Parameter n
 (``adapt_ws.{t}.{weight,bias}``, ``gcs.{l}.base_conv.*``) so reference checkpoints load.
 
 The adapter is the same "per-type linear dispatch" as inside HGTConv and runs through the same C-ABI grouped GEMM
-(``hgt_typed_linear``: tcgen05 when in_dim >= 64 and n_hid % 16 == 0, fp32 SIMT otherwise); every layer shares
+(``hgt_typed_linear``: tensor cores when in_dim >= 64 and n_hid % 16 == 0, fp32 SIMT otherwise); every layer shares
 the one cached graph plan.  Under autograd the adapter uses the same GEMM with its native backward
 (``autograd._TypedLinear``).
 """

@@ -1,12 +1,9 @@
 """pyhgt_b200.data.to_torch (SURVEY.md §8f rank 2) against the reference's own to_torch (pyHGT/data.py:212-256):
 the golden fixture was produced by the unmodified reference on a synthetic sampled sub-graph (oracle/make_golden.py);
 outputs must be IDENTICAL (node order, edge order, dtypes, dict contents)."""
-import time
 
-import pytest
 import torch
 
-from oracle import pyg_shim
 from pyhgt_b200 import data as hdata
 from tests.conftest import load_golden
 
@@ -42,18 +39,3 @@ def test_to_torch_empty_edge_list():
     out = hdata.to_torch(fx["feature"], fx["time"], {}, g)
     assert out[3].shape == (2, 0) and out[4].numel() == 0 and out[2].numel() == 0
     assert torch.equal(out[0], fx["node_feature"])
-
-
-@pytest.mark.skipif(not pyg_shim.reference_available(), reason="reference tree only exists in the dev container")
-def test_to_torch_matches_live_reference_and_is_faster():
-    from oracle import make_golden as mg
-    data, g, feature, times, edge_list = mg.synthetic_sampled_subgraph(seed=5, n_per_type=(3000, 2000, 300), n_edges=60000)
-    import warnings
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        t0 = time.perf_counter(); ref = data.to_torch(feature, times, edge_list, g); t_ref = time.perf_counter() - t0
-    t0 = time.perf_counter(); out = hdata.to_torch(feature, times, edge_list, g); t_new = time.perf_counter() - t0
-    for a, b in zip(out[:5], ref[:5]):
-        assert torch.equal(a, b)
-    assert out[5] == ref[5] and out[6] == ref[6]
-    assert t_new < t_ref, "vectorised ingest (%.3f s) should beat the reference's per-edge loop (%.3f s)" % (t_new, t_ref)

@@ -1,4 +1,4 @@
-"""GPU tests of the native backward kernels (run on the B200 box: ``pytest -m gpu``): hgt_typed_linear_bwd (tcgen05 dX /
+"""GPU tests of the native backward kernels (run on an H100: ``pytest -m gpu``): hgt_typed_linear_bwd (wgmma dX /
 dW with MN-major operands, and the fp32 SIMT path), hgt_update_backward, hgt_fold_backward — each against float64 torch
 autograd of the same expression — and the absence of library GEMMs on the training path."""
 import ctypes

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: ``pytest -m gpu``).  The CUDA path (through the C ABI) is compared
+"""GPU parity tests (run on an H100: ``pytest -m gpu``).  The CUDA path (through the C ABI) is compared
 with (a) golden outputs of the reference itself (tests/golden, made by oracle/make_golden.py) and (b) the CPU
 oracle on seeded graphs.  Tolerance from BASELINE.json north_star: 1e-3 (allclose rtol=atol=1e-3 and relative
 Frobenius error <= 1e-3); index handling is bit-exact."""
@@ -251,9 +251,10 @@ def test_hub_split_matches_unsplit(monkeypatch):
     P.clear_plan_cache()
 
 
-@pytest.mark.parametrize("K,width,m_rows", [(256, 256, 1000), (64, 64, 130), (400, 400, 300), (128, 48, 257), (104, 32, 64)])
+@pytest.mark.parametrize("K,width,m_rows", [(256, 256, 1000), (64, 64, 130), (400, 400, 300), (128, 48, 257), (104, 32, 64),
+                                            (128, 128, 300)])
 def test_typed_linear_tensor_core_matches_fp64(K, width, m_rows):
-    """tcgen05 split-bf16 GEMM (impl 2) against float64: error must be ~1e-5 relative, far inside 1e-3."""
+    """wgmma split-bf16 GEMM (impl 2) against float64: error must be ~1e-5 relative, far inside 1e-3."""
     import ctypes
     from pyhgt_b200 import _lib, plan as P
     dev = _dev()
