@@ -195,7 +195,8 @@ int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W
 /*  q       [N, d]        rank order, Q[i] = W_q^{type(i)} x_i + b
  *  kv      [rows+1, 2d]  row = [K' | V'] of <source node, relation>; last row all zero
  *  kvr     [P*240+1, 2d] RTE contribution per <pair, dt> (NULL when !use_RTE); last row all zero
- *  tiles / hubs from hgt_plan_tiles;  partial workspace: n_split * (2*H + d) floats
+ *  tiles / hubs from hgt_plan_tiles;  partial workspace: n_split slots of round4(2*H) + round4(d) floats
+ *          (round4: rounded up to a multiple of 4, which keeps every slot's accumulator 16-byte aligned)
  *  agg_out [N, d]  gelu(sum_e att[e] * V'[e]) if apply_gelu else the raw sum   (conv.py:119)
  *  att_out [E, H]  softmax weights in ORIGINAL edge order (conv.py:108 `self.att`) or NULL
  *  stats_out [N, 2H] per-destination (max, sum) per head, or NULL (kept for the backward pass)

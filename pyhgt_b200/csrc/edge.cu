@@ -46,10 +46,16 @@ struct EdgeParams {
   __nv_bfloat16* g_lo;
   float* att_out;            // nullptr unless requested
   float* stats_out;          // nullptr unless requested
-  float* partial;            // [n_split][2*H + d]
+  float* partial;            // [n_split][partial_stride(H, d)]
   int32_t* tile_counter;
   int32_t stages;            // TMA variant
 };
+
+// One partial slot (the un-normalised result of a hub piece, merged by k_merge_partials): per-head m at [0, H), l at
+// [H, 2H), the accumulator row from partial_acc_off(H).  The accumulator offset and the slot stride are rounded up to 4
+// floats: the lanes store their chunks with float4 / float2 stores, which need 16 / 8-byte alignment for any H.
+__host__ __device__ __forceinline__ int partial_acc_off(int H) { return (2 * H + 3) & ~3; }
+__host__ __device__ __forceinline__ int partial_stride(int H, int d) { return partial_acc_off(H) + ((d + 3) & ~3); }
 
 // sharded runs: destination `dst` lies past the active (owned) prefix of its node type
 __device__ __forceinline__ bool dst_inactive(const EdgeParams& p, int dst) {
@@ -159,12 +165,12 @@ __device__ __forceinline__ void finalize_destination(const EdgeParams& p, const 
                                                       bool split_piece, int pslot) {
   if (split_piece) {
     // un-normalised partial result of a hub piece; merged by k_merge_partials
-    float* w = p.partial + (int64_t)pslot * (2 * p.H + p.d);
+    float* w = p.partial + (int64_t)pslot * partial_stride(p.H, p.d);
     if (lm.head_ok && lm.sub == 0) { w[lm.h] = st.m; w[p.H + lm.h] = st.l; }
 #pragma unroll
     for (int t = 0; t < NCH; ++t) {
       int o = lm.off<VEC>(t);
-      if (o >= 0) store_vec<VEC>(w + 2 * p.H + o, st.acc[t]);
+      if (o >= 0) store_vec<VEC>(w + partial_acc_off(p.H) + o, st.acc[t]);
     }
     return;
   }
@@ -506,7 +512,7 @@ k_merge_partials(EdgeParams p, const int32_t* __restrict__ hubs, int n_hubs_host
   __shared__ float s_M[32], s_L[32], s_inv[32];
   __shared__ float s_red[32][33];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int stride = 2 * p.H + p.d;
+  const int stride = partial_stride(p.H, p.d), acc_off = partial_acc_off(p.H);
   for (int hb = blockIdx.x; hb < n_hubs; hb += gridDim.x) {
     const int dst = hubs[4 * hb], slot0 = hubs[4 * hb + 1], pieces = hubs[4 * hb + 2];
     const float* part = p.partial + (int64_t)slot0 * stride;
@@ -533,7 +539,7 @@ k_merge_partials(EdgeParams p, const int32_t* __restrict__ hubs, int n_hubs_host
         const float M = s_M[h];
         for (int k = warp; k < pieces; k += 32) {
           const float* w = part + (int64_t)k * stride;
-          a = fmaf(w[2 * p.H + c], __expf(w[h] - M), a);
+          a = fmaf(w[acc_off + c], __expf(w[h] - M), a);
         }
       }
       s_red[warp][lane] = a;
@@ -603,7 +609,7 @@ int dispatch_nch(const EdgeParams& p, int nch, int variant, int grid, size_t sme
 
 extern "C" int hgt_edge_workspace_bytes(int32_t n_split_tiles, int32_t d, int32_t n_heads, size_t* out_bytes) {
   HGT_REQUIRE(out_bytes, "hgt_edge_workspace_bytes: out_bytes is NULL");
-  *out_bytes = 256 + sizeof(float) * (size_t)(n_split_tiles > 0 ? n_split_tiles : 0) * (2 * (size_t)n_heads + d);
+  *out_bytes = 256 + sizeof(float) * (size_t)(n_split_tiles > 0 ? n_split_tiles : 0) * partial_stride(n_heads, d);
   return 0;
 }
 

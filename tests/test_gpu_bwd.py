@@ -96,6 +96,11 @@ def _bwd_case(K, width, groups_spec, act, impl, seed=0):
     (400, 400, [(900, 3), (333, 1)], 0),                     # OAG width: 400 = 256 + 144 columns, 3.125 row tiles of 128
     (128, 256, [(777, 1), (600, 1)], 0),                     # adapter-like: in_dim 128 -> n_hid 256
     (64, 64, [(640, 3)], 1),
+    (512, 256, [(700, 3), (300, 1)], 0),                     # K_in 512: dX and dW at BN 256 with 2 column tiles
+    (384, 128, [(600, 3), (257, 1)], 1),                     # K_in 384: BN 128 with 3 column tiles
+    (256, 16, [(300, 3), (200, 1)], 0),                      # widths the backward takes on the tensor cores (width % 8
+    (256, 24, [(300, 3), (100, 1)], 1),                      # == 0) although the forward does not
+    (256, 256, [(37, 3), (0, 1), (600, 1), (1, 1)], 0),      # groups under 64 rows and an empty group
 ])
 def test_typed_linear_bwd_tensor_core_matches_fp64(K, width, spec, act):
     (ra, ea), (rw, ew), (rb, eb) = _bwd_case(K, width, spec, act, impl=2)

@@ -230,6 +230,37 @@ def test_mag_shaped_medium_graph_vs_oracle(variant):
     _close(m.att, ref_att, "mag x0.005 att", atol=1e-4)
 
 
+@pytest.mark.parametrize("d,H", [(96, 3), (256, 1), (80, 5)])
+def test_split_destination_with_odd_head_count_vs_oracle(d, H):
+    """A destination above TILE_SPLIT_EDGES with an odd head count, so the per-head (m, l) block of a piece's partial row
+    is not a multiple of 4 floats: the accumulator behind it must stay 16-byte aligned for the lanes' float4 stores (all
+    three shapes take VEC 4).  Fused inference call and the per-stage path, against the CPU oracle."""
+    import pyhgt_b200
+    from pyhgt_b200 import plan as P
+    dev = _dev()
+    g = synth.make_random(600, 3000, 2, 2, seed=17)
+    gen = torch.Generator().manual_seed(18)
+    n_hub = P.TILE_SPLIT_EDGES + 700
+    g.edge_index = torch.cat([g.edge_index, torch.stack([torch.randint(0, 600, (n_hub,), generator=gen),
+                                                         torch.full((n_hub,), 7, dtype=torch.int64)])], 1)
+    g.edge_type = torch.cat([g.edge_type, torch.randint(0, 2, (n_hub,), generator=gen)])
+    g.edge_time = torch.cat([g.edge_time, torch.randint(0, 240, (n_hub,), generator=gen)])
+    torch.manual_seed(19)
+    m = pyhgt_b200.HGTConv(d, d, 2, 2, H, 0.2, True, True).eval()
+    x = torch.randn(600, d, generator=gen)
+    params = {k: v.detach().clone() for k, v in m.state_dict().items()}
+    ref, ref_att = hgt_oracle.hgt_forward_ref_port(params, x, g.node_type, g.edge_index, g.edge_type, g.edge_time,
+                                                   num_types=2, num_relations=2, n_heads=H)
+    m = m.to(dev)
+    for fused in (True, False):
+        m.fused_call = fused
+        with torch.no_grad():
+            out = m(x.to(dev), g.node_type.to(dev), g.edge_index.to(dev), g.edge_type.to(dev), g.edge_time.to(dev))
+        torch.cuda.synchronize()
+        _close(out, ref, "d=%d H=%d split hub out (fused %s)" % (d, H, fused))
+        _close(m.att, ref_att, "d=%d H=%d split hub att (fused %s)" % (d, H, fused), atol=1e-4)
+
+
 def test_hub_split_matches_unsplit(monkeypatch):
     """Force hub splitting at a tiny threshold: result must not change."""
     from pyhgt_b200 import plan as P
@@ -252,7 +283,11 @@ def test_hub_split_matches_unsplit(monkeypatch):
 
 
 @pytest.mark.parametrize("K,width,m_rows", [(256, 256, 1000), (64, 64, 130), (400, 400, 300), (128, 48, 257), (104, 32, 64),
-                                            (128, 128, 300)])
+                                            (128, 128, 300),
+                                            (512, 128, 300),     # BN 128, 8 k-blocks: the 3-stage ring wraps twice
+                                            (256, 384, 300),     # BN 128, 3 column tiles
+                                            (256, 512, 300),     # BN 256, 2 column tiles
+                                            (100, 64, 300)])     # K % 8 != 0: the split pads K to 104
 def test_typed_linear_tensor_core_matches_fp64(K, width, m_rows):
     """wgmma split-bf16 GEMM (impl 2) against float64: error must be ~1e-5 relative, far inside 1e-3."""
     import ctypes
@@ -281,6 +316,90 @@ def test_typed_linear_tensor_core_matches_fp64(K, width, m_rows):
         assert torch.isfinite(got).all()
         err = (got - ref).abs().max().item()
         assert err < 5e-5 * max(1.0, ref.abs().max().item()), "max abs err %.3g" % err
+
+
+def _tc_groups_case(K, width, spec, act, seed=0):
+    """Tensor-core forward over a hand-made group table.  spec: list of (m rows, n_cblocks); column block 0 of a group
+    goes to a [m, width] region, the others pairwise interleaved in [m, 2*width] regions, as in the projection buffer.
+    act None: hgt_typed_linear (impl 2) splits the fp32 A itself; act 0 / 1: hgt_act_split (identity / gelu) makes the
+    bf16 split and hgt_typed_linear_presplit consumes it.  Returns the worst error over the column blocks (max abs error
+    relative to max(1, max|ref|)) and checks that nothing outside the column blocks is written."""
+    import ctypes
+    from pyhgt_b200 import _lib, plan as P
+    dev = _dev()
+    gen = torch.Generator().manual_seed(seed)
+    rows_total = sum(m for m, _ in spec)
+    A = torch.randn(rows_total, K, generator=gen)
+    n_wrows = sum(nc for _, nc in spec) * width
+    W = torch.randn(n_wrows, K, generator=gen) / K ** 0.5
+    b = torch.randn(n_wrows, generator=gen)
+    groups, cblocks, regions = [], [], []
+    off, a_row0, w_row0 = 0, 0, 0
+    for gi, (m, nc) in enumerate(spec):
+        first = len(cblocks)
+        cblocks.append((off, width)); regions.append((off, width, m, w_row0, a_row0, gi % 2 == 0)); off += m * width
+        c = 1
+        while c < nc:
+            pair = min(2, nc - c)
+            for j in range(pair):
+                cblocks.append((off + j * width, 2 * width))
+                regions.append((off + j * width, 2 * width, m, w_row0 + (c + j) * width, a_row0, gi % 2 == 0))
+            off += m * 2 * width
+            c += pair
+        off = (off + 31) // 32 * 32
+        groups.append((a_row0, m, w_row0, nc, first, int(gi % 2 == 0)))
+        a_row0 += m
+        w_row0 += nc * width
+    out_elems = off + 64
+    tab = P._pack_groups(groups, cblocks, dev)
+    Ad, Wd, bd = A.to(dev), W.to(dev), b.to(dev)
+    out = torch.full((out_elems,), float("nan"), device=dev)
+    st = torch.cuda.current_stream().cuda_stream
+    wsb = ctypes.c_size_t()
+    if act is None:
+        _lib.call("hgt_typed_linear_workspace_bytes", tab[1].ctypes.data, len(groups), K, width, 2, ctypes.byref(wsb))
+        ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+        _lib.call("hgt_typed_linear", Ad.data_ptr(), K, Wd.data_ptr(), bd.data_ptr(), K, width, tab[0].data_ptr(),
+                  tab[1].ctypes.data, len(groups), tab[3].data_ptr(), out.data_ptr(), 2, ws.data_ptr(), ws.numel(), st)
+    else:
+        hi = torch.empty((rows_total, K), dtype=torch.bfloat16, device=dev)
+        lo = torch.empty((rows_total, K), dtype=torch.bfloat16, device=dev)
+        _lib.call("hgt_act_split", Ad.data_ptr(), K, rows_total, K, act, None, hi.data_ptr(), lo.data_ptr(), st)
+        _lib.call("hgt_typed_linear_presplit_workspace_bytes", tab[1].ctypes.data, len(groups), K, width,
+                  ctypes.byref(wsb))
+        ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+        _lib.call("hgt_typed_linear_presplit", hi.data_ptr(), lo.data_ptr(), Wd.data_ptr(), bd.data_ptr(), K, width,
+                  tab[0].data_ptr(), tab[1].ctypes.data, len(groups), tab[3].data_ptr(), out.data_ptr(), ws.data_ptr(),
+                  ws.numel(), st)
+    torch.cuda.synchronize()
+    got_all = out.cpu().double()
+    A64 = torch.nn.functional.gelu(A.double()) if act == 1 else A.double()
+    written = torch.zeros(out_elems, dtype=torch.bool)
+    worst = 0.0
+    for (o0, ld, m, wr, ar, has_b) in regions:
+        if m == 0:
+            continue
+        ref = A64[ar:ar + m] @ W[wr:wr + width].double().t() + (b[wr:wr + width].double() if has_b else 0)
+        got = torch.as_strided(got_all, (m, width), (ld, 1), o0)
+        torch.as_strided(written, (m, width), (ld, 1), o0).fill_(True)
+        assert torch.isfinite(got).all()
+        worst = max(worst, (got - ref).abs().max().item() / max(1.0, ref.abs().max().item()))
+    assert torch.isnan(got_all[~written]).all(), "the GEMM wrote outside its column blocks"
+    return worst
+
+
+@pytest.mark.parametrize("K,width,spec,act", [
+    (256, 128, [(1, 1), (127, 3), (0, 1), (129, 2)], None),   # 1 / 127 / 129-row groups and an empty one among them
+    (256, 256, [(129, 3), (0, 3), (1, 1), (300, 1)], None),
+    (256, 256, [(1000, 3), (130, 1)], 1),                      # gelu split -> presplit GEMM, as the a_linears run
+    (400, 400, [(127, 3), (1, 1), (300, 1)], 1),               # BN 64, 16-column last tile
+    (128, 256, [(333, 3), (0, 1), (64, 1)], 0),
+])
+def test_typed_linear_tensor_core_group_edges_and_presplit_match_fp64(K, width, spec, act):
+    """Group sizes at the 128-row tile edges and empty groups, through hgt_typed_linear (act None) and through
+    hgt_act_split + hgt_typed_linear_presplit called directly (act 0 / 1), against float64."""
+    err = _tc_groups_case(K, width, spec, act)
+    assert err < 5e-5, "max abs err %.3g (relative to max(1, max|ref|))" % err
 
 
 @pytest.mark.parametrize("world", [2, 3])
