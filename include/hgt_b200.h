@@ -95,6 +95,18 @@ int hgt_plan_tiles(const int32_t* row_ptr, int64_t n_nodes, int64_t n_edges,
                    int32_t* d_n_tiles, int32_t* h_n_tiles,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* Source-major index for the deterministic edge backward: the CSR positions [0, n_edges) stably sorted by key[c]
+ * (kv_row: rows of the [K'|V'] table, or rte_row: rows of the RTE table), so every owned row lists its edges in CSR order.
+ *   src_ptr [n_rows+1]: entries of row r are [src_ptr[r], src_ptr[r+1]); entries whose key is n_rows (the trailing
+ *            all-zero row that collects edges matching no triple) lie past src_ptr[n_rows] and get no work;
+ *   src_dst [n_edges]: destination (rank order) of every entry;  src_oth [n_edges]: other[c] of every entry, or NULL
+ *            together with other.
+ * No host read-back; work tiles over it come from hgt_plan_tiles(src_ptr, n_rows, ...) in its sync-free mode.
+ * workspace: hgt_plan_workspace_bytes(n_rows, n_edges). */
+int hgt_plan_source_index(const int32_t* key, const int32_t* other, const int32_t* row_ptr, int64_t n_nodes,
+                          int64_t n_edges, int32_t n_rows, int32_t* src_ptr, int32_t* src_dst, int32_t* src_oth,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
 /* out[k,:] = in[perm[k],:]  (rows of `width` floats); used only when node_type is not pre-sorted. */
 int hgt_gather_rows(const float* in, const int32_t* perm, int64_t n_rows, int32_t width,
                     float* out, void* stream);
@@ -231,6 +243,33 @@ int hgt_edge_backward(const float* q, const float* kv, const float* kvr, const f
                       float* dq, float* dkv, float* dkvr, void* workspace, size_t workspace_bytes,
                       const int32_t* d_tile_counts, void* stream);
 
+/* Deterministic backward of hgt_edge_forward: the same gradients without float atomics, bitwise repeatable.
+ * hgt_edge_backward_dst: destination pass.  Writes dq [N,d] (zero-initialised here; hub pieces go to partial rows in the
+ *   workspace and are summed in piece order through `hubs`) and D [N,H] = <dagg_i, agg_i> per head (rows of
+ *   destinations without in-edges are not written).  Does not touch the K'/V' gradients.
+ * hgt_edge_backward_rows: row pass over a source-major index (hgt_plan_source_index + hgt_plan_tiles).  One warp owns a
+ *   row of `own` ([own_rows_total, 2d]: the [K'|V'] table keyed by kv_row, or the RTE table keyed by rte_row) and walks its
+ *   entries in order: it gathers Q_i, dagg_i, (m, l)_i, D_i and the row src_oth[j] of `oth` (the other table, added to
+ *   the key / value row as in the forward; NULL without RTE), and writes grad[row] = [sum ds Q_i | sum p dagg_i] with
+ *   one store.  Rows [n_rows, own_rows_total) (the trailing all-zero row) are zeroed.  Split rows: partial rows summed
+ *   in piece order.
+ * tiles / n_tiles / n_split / hubs / n_hubs / d_tile_counts as for hgt_edge_forward (for the row pass: from
+ *   hgt_plan_tiles over src_ptr).  Every d / n_heads that hgt_edge_backward takes is supported.
+ * workspace: hgt_edge_backward_det_workspace_bytes(n_split of the destination tiles, n_split of the row tiles, d); the
+ *   passes run one after the other on the stream, so one workspace serves all of them. */
+int hgt_edge_backward_det_workspace_bytes(int32_t n_split_dst, int32_t n_split_rows, int32_t d, size_t* out_bytes);
+int hgt_edge_backward_dst(const float* q, const float* kv, const float* kvr, const float* agg, const float* dagg,
+                          const float* stats, const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                          const int32_t* tiles, int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
+                          int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D,
+                          void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_rows(const float* q, const float* dagg, const float* stats, const float* D, const float* own,
+                           const float* oth, const int32_t* src_ptr, const int32_t* src_dst, const int32_t* src_oth,
+                           int32_t n_rows, int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles,
+                           int32_t n_split, const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads,
+                           float* grad, void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                           void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Backward of the typed linears (training path).  For the group / column-block tables of the forward call:
  *   dA[a_row0_g + m, k]             = sum_c sum_n dOut_c[m, n] * W[w_row0_g + c*cb_width + n, k]   (* gelu'(gelu_aux) if given)
@@ -255,6 +294,22 @@ int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, const void* dou
                          float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
                          int32_t impl, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Deterministic twin of hgt_typed_linear_bwd (same arguments and results, no float atomics).  dW: every (column block,
+ * row chunk) stores its partial tile into the workspace, and the partials are added to dW in (column block, chunk) order;
+ * db: per-CTA partial column sums, added in the same order; SIMT dA: one thread per element, over the covering groups in
+ * group order.  The workspace grows by the partial slots: tensor cores ~ (4 * SMs / tiles per block + blocks) slots of
+ * cb_width x K floats, SIMT at most ~256 + blocks such slots, plus rows / 256 bias rows of cb_width floats. */
+int hgt_typed_linear_bwd_det_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups,
+                                             const hgt_lin_cblock* h_cblocks, int32_t K, int32_t cb_width, int64_t lda,
+                                             int64_t dout_elems, int32_t have_dout_split, int32_t have_a_split,
+                                             int32_t impl, size_t* out_bytes);
+int hgt_typed_linear_bwd_det(const float* dout, const void* dout_hi, const void* dout_lo, int64_t dout_elems,
+                             const float* A, int64_t lda, const void* a_hi, const void* a_lo,
+                             const float* W, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                             const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
+                             float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
+                             int32_t impl, void* workspace, size_t workspace_bytes, void* stream);
+
 /* act(in) as fp32 (out_f32 [rows, K], or NULL) and/or as the bf16 hi/lo operand split (hi/lo [rows, K], or NULL; needs
  * K % 8 == 0).  act: 0 = identity, 1 = exact-erf gelu (conv.py:119).  The training forward keeps the split for the
  * backward pass (it is the A operand of the dW product). */
@@ -270,6 +325,14 @@ int hgt_update_backward(const float* dout, const float* o, const float* x, const
                         const float* skip, const float* norm_w, const int32_t* perm, const int32_t* type_active,
                         int64_t n_nodes, int32_t d,
                         float* d_o, float* d_x, float* d_skip, float* d_norm_w, float* d_norm_b, void* stream);
+/* Deterministic twin: blocks never cross a type boundary, each stores its d norm / d skip sums in its own workspace slot,
+ * and each type's slots are added in block order (no atomics).  Outputs are written, not accumulated. */
+int hgt_update_backward_det_workspace_bytes(int64_t n_nodes, int32_t num_types, int32_t d, size_t* out_bytes);
+int hgt_update_backward_det(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                            int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                            const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
+                            float* d_skip, float* d_norm_w, float* d_norm_b, void* workspace, size_t workspace_bytes,
+                            void* stream);
 
 /* Backward of hgt_fold_weights for the K'/V' blocks: from d W_cat / d b_cat to the gradients of k_linears / v_linears
  * (stacked [T, d_out, d_in] / [T, d_out]) and relation_att / relation_msg [R,H,dk,dk], relation_pri [R,H]; all outputs
@@ -280,6 +343,14 @@ int hgt_fold_backward(const float* d_w_cat, const float* d_b_cat, const float* c
                       int32_t n_heads, int32_t d_in, int32_t d_out, int32_t n_pairs, const int32_t* pair_type,
                       const int32_t* pair_rel, const int32_t* cat_row0, float* d_wk, float* d_bk, float* d_wv,
                       float* d_bv, float* d_att, float* d_msg, float* d_pri, void* stream);
+/* Deterministic twin: every output element is computed by one thread (warp for the relation matrices), which loops over
+ * the <type, relation> pairs in pair order.  Same arguments and results. */
+int hgt_fold_backward_det(const float* d_w_cat, const float* d_b_cat, const float* const* wk, const float* const* bk,
+                          const float* const* wv, const float* const* bv, const float* relation_att,
+                          const float* relation_msg, const float* relation_pri, int32_t num_types, int32_t num_relations,
+                          int32_t n_heads, int32_t d_in, int32_t d_out, int32_t n_pairs, const int32_t* pair_type,
+                          const int32_t* pair_rel, const int32_t* cat_row0, float* d_wk, float* d_bk, float* d_wv,
+                          float* d_bv, float* d_att, float* d_msg, float* d_pri, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Update epilogue (conv.py:129-133): y = o*sigmoid(skip[t]) + x*(1-sigmoid(skip[t])); LayerNorm_t(y)

@@ -51,6 +51,21 @@ SIGNATURES = {
     "hgt_conv_workspace_bytes": [_p, _c.POINTER(_sz)],
     "hgt_conv_forward": [_p, _p, _sz, _p],
     "hgt_update_epilogue": [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p],
+    # deterministic training backward (torch.use_deterministic_algorithms)
+    "hgt_plan_source_index": [_p, _p, _p, _i64, _i64, _i32, _p, _p, _p, _p, _sz, _p],
+    "hgt_edge_backward_det_workspace_bytes": [_i32, _i32, _i32, _c.POINTER(_sz)],
+    "hgt_edge_backward_dst": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32, _i32, _p, _p, _p,
+                              _sz, _p, _p],
+    "hgt_edge_backward_rows": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _p, _i32, _i32, _p, _i32, _i32, _i32, _p,
+                               _p, _sz, _p, _p],
+    "hgt_typed_linear_bwd_det_workspace_bytes": [_p, _i32, _p, _i32, _i32, _i64, _i64, _i32, _i32, _i32,
+                                                 _c.POINTER(_sz)],
+    "hgt_typed_linear_bwd_det": [_p, _p, _p, _i64, _p, _i64, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i32, _p, _p,
+                                 _p, _i32, _p, _sz, _p],
+    "hgt_update_backward_det_workspace_bytes": [_i64, _i32, _i32, _c.POINTER(_sz)],
+    "hgt_update_backward_det": [_p, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_fold_backward_det": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p,
+                              _p, _p, _p, _p, _p, _p],
 }
 
 class ConvArgs(ctypes.Structure):

@@ -15,6 +15,12 @@ No per-edge intermediates are kept: the edge backward recomputes the softmax wei
 (max, sum); the typed linears keep the bf16 hi/lo split of their input (the A operand of the dW product).  No cuBLAS,
 no torch matmul on this path.  Gradients reach ``node_inp`` and every parameter of conv.py:28-54 including ``emb.*``.
 The inference path (``torch.no_grad``) does not come through here: it uses the fused kernels in conv.py.
+
+Under ``torch.use_deterministic_algorithms(True)`` (``warn_only=True`` included) every stage records the flag in its
+forward and its backward calls the deterministic twins instead: hgt_edge_backward_dst + hgt_edge_backward_rows (a
+source-major second pass that owns every K'/V' and RTE gradient row, plan.source_index), hgt_typed_linear_bwd_det,
+hgt_update_backward_det and hgt_fold_backward_det.  They use no float atomics, so two identical steps give bitwise equal
+gradients.  With the flag off nothing changes.
 """
 import ctypes
 
@@ -73,6 +79,7 @@ class _TypedLinear(torch.autograd.Function):
                       ws.numel(), st)
         ctx.table, ctx.width, ctx.has_bias, ctx.act, ctx.use_tc = table, width, b_cat is not None, act, use_tc
         ctx.out_elems = out_elems
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         # gelu'(a) needs the un-activated input; the dW product needs act(a): as the bf16 split (tensor cores) or fp32
         ctx.save_for_backward(a if (act or not use_tc) else None, a_act if (act and not use_tc) else None, hi, lo, w_cat)
         return out
@@ -90,12 +97,13 @@ class _TypedLinear(torch.autograd.Function):
         dw = torch.zeros_like(w_cat)                                   # small: [sum of out rows, K]
         db = torch.zeros(w_cat.shape[0], dtype=torch.float32, device=dev) if ctx.has_bias else None
         impl = 2 if ctx.use_tc else 1
+        fn = "hgt_typed_linear_bwd_det" if ctx.det else "hgt_typed_linear_bwd"
         a_f32 = a_act if a_act is not None else a                      # SIMT dW operand (act already applied)
         # tables whose groups overlap in rows (sharded per-pair compaction) come with disjoint sub-tables: the first call
         # writes dA, the others accumulate into it; dW / db accumulate anyway
         tables = getattr(ctx.table, "bwd_tables", None) or [ctx.table]
         if not ctx.use_tc:
-            tables = [ctx.table]                                       # the SIMT dX uses atomics: overlap is fine
+            tables = [ctx.table]                                       # the SIMT dX adds overlapping groups itself
         if need_da:
             # hgt_typed_linear_bwd zeroes the gaps between the first table's groups; rows past its last group (other
             # sub-tables' rows, nodes of unknown type) are zeroed here
@@ -107,10 +115,10 @@ class _TypedLinear(torch.autograd.Function):
             g_dev, g_host, n_g, _ = tab
             c_host = tab.c_host
             wsb = ctypes.c_size_t()
-            _lib.call("hgt_typed_linear_bwd_workspace_bytes", g_host.ctypes.data, n_g, c_host.ctypes.data, K, width, K,
+            _lib.call(fn + "_workspace_bytes", g_host.ctypes.data, n_g, c_host.ctypes.data, K, width, K,
                       ctx.out_elems, 0, int(hi is not None), impl, ctypes.byref(wsb))
             ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-            _lib.call("hgt_typed_linear_bwd", dout.data_ptr(), None, None, ctx.out_elems, _lib.ptr(a_f32), K, _lib.ptr(hi),
+            _lib.call(fn, dout.data_ptr(), None, None, ctx.out_elems, _lib.ptr(a_f32), K, _lib.ptr(hi),
                       _lib.ptr(lo), w_cat.data_ptr(), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g,
                       c_host.ctypes.data, _lib.ptr(da), int(ti > 0), a.data_ptr() if ctx.act else None, dw.data_ptr(),
                       _lib.ptr(db), impl, ws.data_ptr(), ws.numel(), _stream())
@@ -143,6 +151,7 @@ class _EdgeAttention(torch.autograd.Function):
                   variant, _lib.ptr(plan.tile_counts_dev), plan.type_row0_dev.data_ptr(), plan.num_types,
                   _lib.ptr(lt.type_active_dev), _stream())
         ctx.plan, ctx.lt, ctx.d, ctx.n_heads, ctx.has_kvr = plan, lt, d, n_heads, kvr is not None
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         ctx.save_for_backward(proj, kvr, agg, stats)
         if att is not None:
             ctx.mark_non_differentiable(att)
@@ -161,8 +170,11 @@ class _EdgeAttention(torch.autograd.Function):
         dq = dproj[lt.q_off:lt.q_off + N * d]
         dkv = dproj[lt.kv_off:]
         dkvr = torch.empty_like(kvr) if kvr is not None else None
-        ws = torch.empty(256, dtype=torch.uint8, device=proj.device)
         dagg = dagg.contiguous()
+        if ctx.det:
+            _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr)
+            return dproj, dkvr, None, None, None, None, None, None
+        ws = torch.empty(256, dtype=torch.uint8, device=proj.device)
         _lib.call("hgt_edge_backward", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
                   stats.data_ptr(), plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
                   None if kvr is None else plan.rte_row.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, N, d, H,
@@ -170,6 +182,33 @@ class _EdgeAttention(torch.autograd.Function):
                   dq.data_ptr(), dkv.data_ptr(), _lib.ptr(dkvr), ws.data_ptr(), ws.numel(),
                   _lib.ptr(plan.tile_counts_dev), _stream())
         return dproj, dkvr, None, None, None, None, None, None
+
+
+def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr):
+    """Deterministic edge backward: destination pass (dq, D), then one row pass over the [K'|V'] rows and, with RTE, one
+    over the RTE rows; each gradient row is written once by its owner."""
+    N = plan.n_nodes
+    st = _stream()
+    kvi = _plan.source_index(plan, "kv")
+    rti = _plan.source_index(plan, "rte") if kvr is not None else None
+    D = torch.empty((N, H), dtype=torch.float32, device=q.device)
+    wsb = ctypes.c_size_t()
+    _lib.call("hgt_edge_backward_det_workspace_bytes", plan.n_split, max(kvi.n_split, rti.n_split if rti else 0), d,
+              ctypes.byref(wsb))
+    ws = torch.empty(wsb.value, dtype=torch.uint8, device=q.device)
+    _lib.call("hgt_edge_backward_dst", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
+              stats.data_ptr(), plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
+              None if kvr is None else plan.rte_row.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, plan.n_split,
+              plan.hubs.data_ptr(), plan.n_hubs, N, d, H, dq.data_ptr(), D.data_ptr(), ws.data_ptr(), ws.numel(),
+              _lib.ptr(plan.tile_counts_dev), st)
+    passes = [(kv, kvr, kvi, plan.kv_rows + 1, dkv)]
+    if kvr is not None:
+        passes.append((kvr, kv, rti, kvr.numel() // (2 * d), dkvr))
+    for own, oth, idx, own_rows, grad in passes:
+        _lib.call("hgt_edge_backward_rows", q.data_ptr(), dagg.data_ptr(), stats.data_ptr(), D.data_ptr(), own.data_ptr(),
+                  _lib.ptr(oth), idx.ptr.data_ptr(), idx.dst.data_ptr(), None if oth is None else idx.oth.data_ptr(),
+                  idx.n_rows, own_rows, idx.tiles.data_ptr(), idx.n_tiles, idx.n_split, idx.hubs.data_ptr(), idx.n_hubs,
+                  d, H, grad.data_ptr(), ws.data_ptr(), ws.numel(), idx.counts_dev.data_ptr(), st)
 
 
 class _FoldWeights(torch.autograd.Function):
@@ -191,6 +230,7 @@ class _FoldWeights(torch.autograd.Function):
                   plan.pair_rel_dev.data_ptr(), lt.cat_row0_dev.data_ptr(), lt.q_row0_dev.data_ptr(), w_cat.data_ptr(),
                   b_cat.data_ptr(), st)
         ctx.module, ctx.plan, ctx.lt, ctx.tabs = m, plan, lt, tabs
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return w_cat, b_cat
 
     @staticmethod
@@ -204,7 +244,7 @@ class _FoldWeights(torch.autograd.Function):
         d_bk, d_bv = torch.empty((T, d), **f32), torch.empty((T, d), **f32)
         d_att, d_msg = torch.empty((R, H, dk, dk), **f32), torch.empty((R, H, dk, dk), **f32)
         d_pri = torch.empty((R, H), **f32)
-        _lib.call("hgt_fold_backward", dw_cat.data_ptr(), db_cat.data_ptr(), tabs[2].data_ptr(), tabs[3].data_ptr(),
+        _lib.call("hgt_fold_backward_det" if ctx.det else "hgt_fold_backward", dw_cat.data_ptr(), db_cat.data_ptr(), tabs[2].data_ptr(), tabs[3].data_ptr(),
                   tabs[4].data_ptr(), tabs[5].data_ptr(), m.relation_att.data_ptr(), m.relation_msg.data_ptr(),
                   m.relation_pri.data_ptr(), T, R, H, d_in, d, plan.n_pairs, plan.pair_type_dev.data_ptr(),
                   plan.pair_rel_dev.data_ptr(), lt.cat_row0_dev.data_ptr(), d_wk.data_ptr(), d_bk.data_ptr(),
@@ -232,6 +272,7 @@ class _UpdateEpilogue(torch.autograd.Function):
                   _lib.ptr(norm_w), _lib.ptr(norm_b), _lib.ptr(perm), _lib.ptr(type_active), N, d, out.data_ptr(), None,
                   None, _stream())
         ctx.T, ctx.has_norm, ctx.has_skip = T, norm_w is not None, skip is not None
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         ctx.save_for_backward(o, x, skip, norm_w, type_row0, perm, type_active)
         return out
 
@@ -246,9 +287,16 @@ class _UpdateEpilogue(torch.autograd.Function):
         d_skip = torch.empty(T, dtype=torch.float32, device=dev) if ctx.has_skip else None
         d_nw = torch.empty((T, d), dtype=torch.float32, device=dev) if ctx.has_norm else None
         d_nb = torch.empty((T, d), dtype=torch.float32, device=dev) if ctx.has_norm else None
-        _lib.call("hgt_update_backward", dout.data_ptr(), o.data_ptr(), x.data_ptr(), type_row0.data_ptr(), T,
-                  _lib.ptr(skip), _lib.ptr(norm_w), _lib.ptr(perm), _lib.ptr(type_active), N, d, d_o.data_ptr(),
-                  d_x.data_ptr(), _lib.ptr(d_skip), _lib.ptr(d_nw), _lib.ptr(d_nb), _stream())
+        args = (dout.data_ptr(), o.data_ptr(), x.data_ptr(), type_row0.data_ptr(), T, _lib.ptr(skip), _lib.ptr(norm_w),
+                _lib.ptr(perm), _lib.ptr(type_active), N, d, d_o.data_ptr(), d_x.data_ptr(), _lib.ptr(d_skip),
+                _lib.ptr(d_nw), _lib.ptr(d_nb))
+        if ctx.det:
+            wsb = ctypes.c_size_t()
+            _lib.call("hgt_update_backward_det_workspace_bytes", N, T, d, ctypes.byref(wsb))
+            ws = torch.empty(wsb.value, dtype=torch.uint8, device=dev)
+            _lib.call("hgt_update_backward_det", *args, ws.data_ptr(), ws.numel(), _stream())
+        else:
+            _lib.call("hgt_update_backward", *args, _stream())
         return d_o, d_x, d_skip, d_nw, d_nb, None, None, None, None
 
 

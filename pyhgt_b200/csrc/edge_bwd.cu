@@ -9,7 +9,18 @@
 // [K'|V'] gradient table (and the RTE gradient table) with vector fp32 reductions (red.global.add.v4.f32):
 // many edges share a <source, relation> row.  The trailing all-zero row collects the gradient of edges that
 // matched no triple and is discarded by the caller.
+//
+// Deterministic variant (hgt_edge_backward_dst + hgt_edge_backward_rows, chosen by the caller under
+// torch.use_deterministic_algorithms): every gradient row has one owner and no float atomics are used.
+//   destination pass  the same walk without the dk / dv scatter; writes dq (hub pieces: partial rows merged in piece
+//                     order) and D_i = <dagg_i, agg_i> per head;
+//   row pass          one warp owns a [K'|V'] row (or an RTE row) and walks its edges in a source-major index
+//                     (hgt_plan_source_index): per edge it gathers Q_i, dagg_i, (m, l)_i, D_i and the other table's row,
+//                     recomputes p / ds and accumulates dK = sum ds Q_i, dV = sum p dagg_i in registers; rows with more
+//                     than the split threshold of edges are cut into pieces whose partial rows are merged in piece order.
 #include "common.cuh"
+
+#include <type_traits>
 
 namespace {
 
@@ -33,6 +44,8 @@ struct BwdParams {
   float* dkv;                // [rows+1, 2d] zero-initialised
   float* dkvr;               // [P*240+1, 2d] zero-initialised or nullptr
   int32_t* tile_counter;
+  float* D;                  // deterministic destination pass: [N, H] D_i per head
+  float* partial;            // deterministic destination pass: [n_split, d] partial dq of hub pieces
 };
 
 template <int VEC>
@@ -63,9 +76,21 @@ __device__ __forceinline__ float head_sum(float v, int lph) {
   return v;
 }
 
-template <int VEC, int NCH>
-__global__ void __launch_bounds__(kWarps * 32)
-k_edge_bwd(BwdParams p) {
+template <int VEC>
+__device__ __forceinline__ void st_vec(float* p, const float (&v)[VEC]) {
+  if constexpr (VEC == 4) {
+    *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  } else if constexpr (VEC == 2) {
+    *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]);
+  } else {
+    *p = v[0];
+  }
+}
+
+// DET = false: hgt_edge_backward (dk / dv scattered with reductions).  DET = true: destination pass of the
+// deterministic backward (no scatter; D_i saved; hub pieces write partial dq rows).
+template <int VEC, int NCH, bool DET>
+__device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
   const int lane = threadIdx.x & 31;
   const int lph = p.LPH;
   const int h = lane >> p.lph_shift;
@@ -112,6 +137,9 @@ k_edge_bwd(BwdParams p) {
           for (int v = 0; v < VEC; ++v) dq[t][v] = 0.f;
         }
         const float D = head_sum(dpart, lph);
+        if constexpr (DET) {
+          if (head_ok && sub == 0 && seg_begin == p.row_ptr[dst]) p.D[(int64_t)dst * p.H + h] = D;
+        }
         float m = 0.f, inv_l = 0.f;
         if (head_ok) {
           m = p.stats[(int64_t)dst * 2 * p.H + h];
@@ -146,34 +174,50 @@ k_edge_bwd(BwdParams p) {
           const float dp = head_sum(dppart, lph);
           const float pe = __expf(s - m) * inv_l;
           const float ds = pe * (dp - D);
-          float* gk = p.dkv + row * row_stride;
+          if constexpr (DET) {
 #pragma unroll
-          for (int t = 0; t < NCH; ++t) {
-            if (offs[t] >= 0) {
-              float gkv[VEC], gvv[VEC];
+            for (int t = 0; t < NCH; ++t)
+              if (offs[t] >= 0) {
 #pragma unroll
-              for (int v = 0; v < VEC; ++v) {
-                dq[t][v] = fmaf(ds, kk[t][v], dq[t][v]);
-                gkv[v] = ds * q[t][v];
-                gvv[v] = pe * da[t][v];
+                for (int v = 0; v < VEC; ++v) dq[t][v] = fmaf(ds, kk[t][v], dq[t][v]);
               }
-              red_add_vec<VEC>(gk + offs[t], gkv);
-              red_add_vec<VEC>(gk + p.d + offs[t], gvv);
-              if (rte) {
-                red_add_vec<VEC>(p.dkvr + rrow * row_stride + offs[t], gkv);
-                red_add_vec<VEC>(p.dkvr + rrow * row_stride + p.d + offs[t], gvv);
+          } else {
+            float* gk = p.dkv + row * row_stride;
+#pragma unroll
+            for (int t = 0; t < NCH; ++t) {
+              if (offs[t] >= 0) {
+                float gkv[VEC], gvv[VEC];
+#pragma unroll
+                for (int v = 0; v < VEC; ++v) {
+                  dq[t][v] = fmaf(ds, kk[t][v], dq[t][v]);
+                  gkv[v] = ds * q[t][v];
+                  gvv[v] = pe * da[t][v];
+                }
+                red_add_vec<VEC>(gk + offs[t], gkv);
+                red_add_vec<VEC>(gk + p.d + offs[t], gvv);
+                if (rte) {
+                  red_add_vec<VEC>(p.dkvr + rrow * row_stride + offs[t], gkv);
+                  red_add_vec<VEC>(p.dkvr + rrow * row_stride + p.d + offs[t], gvv);
+                }
               }
             }
           }
         }
         float* gq = p.dq + (int64_t)dst * p.d;
+        if constexpr (DET) {
+          if (split) gq = p.partial + (int64_t)(-tl.y - 1) * p.d;
 #pragma unroll
-        for (int t = 0; t < NCH; ++t) {
-          if (offs[t] >= 0) {
-            if (split) red_add_vec<VEC>(gq + offs[t], dq[t]);
-            else {
+          for (int t = 0; t < NCH; ++t)
+            if (offs[t] >= 0) st_vec<VEC>(gq + offs[t], dq[t]);
+        } else {
 #pragma unroll
-              for (int v = 0; v < VEC; ++v) gq[offs[t] + v] = dq[t][v];
+          for (int t = 0; t < NCH; ++t) {
+            if (offs[t] >= 0) {
+              if (split) red_add_vec<VEC>(gq + offs[t], dq[t]);
+              else {
+#pragma unroll
+                for (int v = 0; v < VEC; ++v) gq[offs[t] + v] = dq[t][v];
+              }
             }
           }
         }
@@ -183,15 +227,227 @@ k_edge_bwd(BwdParams p) {
   }
 }
 
-template <int VEC>
-int dispatch(const BwdParams& p, int nch, int grid, cudaStream_t st) {
-  switch (nch) {
-    case 1: k_edge_bwd<VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
-    case 2: k_edge_bwd<VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
-    case 4: k_edge_bwd<VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
-    case 8: k_edge_bwd<VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
-    default: hgt_set_error("hgt_edge_backward: unsupported chunk count %d", nch); return 1;
+template <int VEC, int NCH>
+__global__ void __launch_bounds__(kWarps * 32)
+k_edge_bwd(BwdParams p) {
+  edge_bwd_dst<VEC, NCH, false>(p);
+}
+
+template <int VEC, int NCH>
+__global__ void __launch_bounds__(kWarps * 32)
+k_edge_bwd_dst(BwdParams p) {
+  edge_bwd_dst<VEC, NCH, true>(p);
+}
+
+// ---- deterministic row pass --------------------------------------------------------------------------------------------
+struct RowParams {
+  const float* q;
+  const float* dagg;
+  const float* stats;        // [N, 2H] (m, l)
+  const float* D;            // [N, H] from the destination pass
+  const float* own;          // table of the owned rows [rows, 2d] ([K'|V'] or the RTE table)
+  const float* oth;          // the other table added to every edge's key / value row, or nullptr
+  const int32_t* ptr;        // [n_rows + 1] source-major index over the owned rows
+  const int32_t* e_dst;      // per index entry: destination (rank order)
+  const int32_t* e_oth;      // per index entry: row of the other table (unused without oth)
+  const int32_t* tiles;
+  int32_t n_tiles;
+  const int32_t* d_counts;
+  int32_t d, H, DK, LPH, lph_shift;
+  float* grad;               // [rows, 2d] gradient of the owned table
+  float* partial;            // [n_split, 2d] partial rows of split row pieces
+  int32_t* tile_counter;
+};
+
+template <int VEC, int NCH>
+__global__ void __launch_bounds__(kWarps * 32)
+k_edge_bwd_rows(RowParams p) {
+  const int lane = threadIdx.x & 31;
+  const int lph = p.LPH;
+  const int h = lane >> p.lph_shift;
+  const int sub = lane & (lph - 1);
+  const bool head_ok = h < p.H;
+  int offs[NCH];
+#pragma unroll
+  for (int t = 0; t < NCH; ++t) {
+    int o = (sub + t * lph) * VEC;
+    offs[t] = (head_ok && o < p.DK) ? h * p.DK + o : -1;
   }
+  const int64_t row_stride = 2 * (int64_t)p.d;
+  const bool two = p.oth != nullptr;
+
+  const int n_tiles = p.d_counts ? p.d_counts[0] : p.n_tiles;
+  for (;;) {
+    int tile = 0;
+    if (lane == 0) tile = atomicAdd(p.tile_counter, 1);
+    tile = __shfl_sync(0xffffffffu, tile, 0);
+    if (tile >= n_tiles) break;
+    const int4 tl = reinterpret_cast<const int4*>(p.tiles)[tile];
+    const bool split = tl.y < 0;
+    const int r_begin = tl.x, r_end = split ? tl.x + 1 : tl.y;
+    int seg_begin = tl.z;
+    for (int row = r_begin; row < r_end; ++row) {
+      const int seg_end = split ? tl.w : p.ptr[row + 1];
+      float ko[NCH][VEC], vo[NCH][VEC], gk[NCH][VEC], gv[NCH][VEC];
+#pragma unroll
+      for (int t = 0; t < NCH; ++t)
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) { ko[t][v] = vo[t][v] = gk[t][v] = gv[t][v] = 0.f; }
+      if (seg_end > seg_begin) {
+        const float* orow = p.own + (int64_t)row * row_stride;
+#pragma unroll
+        for (int t = 0; t < NCH; ++t)
+          if (offs[t] >= 0) {
+            ld_vec<VEC>(ko[t], orow + offs[t]);
+            ld_vec<VEC>(vo[t], orow + p.d + offs[t]);
+          }
+      }
+      for (int j = seg_begin; j < seg_end; ++j) {
+        const int64_t i = p.e_dst[j];
+        const float* xrow = two ? p.oth + (int64_t)p.e_oth[j] * row_stride : nullptr;
+        float q[NCH][VEC], da[NCH][VEC];
+        float spart = 0.f, dppart = 0.f;
+#pragma unroll
+        for (int t = 0; t < NCH; ++t) {
+          if (offs[t] >= 0) {
+            float kk[VEC], vv[VEC];
+            ld_vec<VEC>(q[t], p.q + i * p.d + offs[t]);
+            ld_vec<VEC>(da[t], p.dagg + i * p.d + offs[t]);
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) { kk[v] = ko[t][v]; vv[v] = vo[t][v]; }
+            if (two) {
+              float a[VEC], b[VEC];
+              ld_vec<VEC>(a, xrow + offs[t]);
+              ld_vec<VEC>(b, xrow + p.d + offs[t]);
+#pragma unroll
+              for (int v = 0; v < VEC; ++v) { kk[v] += a[v]; vv[v] += b[v]; }
+            }
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) {
+              spart = fmaf(q[t][v], kk[v], spart);
+              dppart = fmaf(da[t][v], vv[v], dppart);
+            }
+          } else {
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) { q[t][v] = 0.f; da[t][v] = 0.f; }
+          }
+        }
+        const float s = head_sum(spart, lph);
+        const float dp = head_sum(dppart, lph);
+        float m = 0.f, inv_l = 0.f, D = 0.f;
+        if (head_ok) {
+          m = p.stats[i * 2 * p.H + h];
+          inv_l = 1.0f / (p.stats[i * 2 * p.H + p.H + h] + 1e-16f);
+          D = p.D[i * p.H + h];
+        }
+        const float pe = __expf(s - m) * inv_l;
+        const float ds = pe * (dp - D);
+#pragma unroll
+        for (int t = 0; t < NCH; ++t)
+#pragma unroll
+          for (int v = 0; v < VEC; ++v) {
+            gk[t][v] = fmaf(ds, q[t][v], gk[t][v]);
+            gv[t][v] = fmaf(pe, da[t][v], gv[t][v]);
+          }
+      }
+      float* out = split ? p.partial + (int64_t)(-tl.y - 1) * row_stride : p.grad + (int64_t)row * row_stride;
+#pragma unroll
+      for (int t = 0; t < NCH; ++t)
+        if (offs[t] >= 0) {
+          st_vec<VEC>(out + offs[t], gk[t]);
+          st_vec<VEC>(out + p.d + offs[t], gv[t]);
+        }
+      seg_begin = seg_end;
+    }
+  }
+}
+
+// Hub pieces of either pass: out[row] = sum of the pieces' partial rows, added in piece order.  One CTA per hub.
+__global__ void __launch_bounds__(256)
+k_merge_piece_rows(const int32_t* __restrict__ hubs, const int32_t* __restrict__ d_counts, int n_hubs_host,
+                   const float* __restrict__ partial, int width, float* __restrict__ out) {
+  const int n_hubs = d_counts ? d_counts[2] : n_hubs_host;
+  for (int hb = blockIdx.x; hb < n_hubs; hb += gridDim.x) {
+    const int row = hubs[4 * hb], slot0 = hubs[4 * hb + 1], pieces = hubs[4 * hb + 2];
+    for (int c = threadIdx.x; c < width; c += blockDim.x) {
+      float s = 0.f;
+      for (int i = 0; i < pieces; ++i) s += partial[(int64_t)(slot0 + i) * width + c];
+      out[(int64_t)row * width + c] = s;
+    }
+  }
+}
+
+template <typename Params, int VEC>
+int dispatch(const Params& p, int nch, int grid, cudaStream_t st, bool det) {
+  if constexpr (std::is_same<Params, RowParams>::value) {
+    switch (nch) {
+      case 1: k_edge_bwd_rows<VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd_rows<VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd_rows<VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd_rows<VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      default: hgt_set_error("hgt_edge_backward_rows: unsupported chunk count %d", nch); return 1;
+    }
+  } else if (det) {
+    switch (nch) {
+      case 1: k_edge_bwd_dst<VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd_dst<VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd_dst<VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd_dst<VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      default: hgt_set_error("hgt_edge_backward_dst: unsupported chunk count %d", nch); return 1;
+    }
+  } else {
+    switch (nch) {
+      case 1: k_edge_bwd<VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd<VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd<VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd<VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      default: hgt_set_error("hgt_edge_backward: unsupported chunk count %d", nch); return 1;
+    }
+  }
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+// Lane mapping shared by every pass: LPH lanes per head, VEC floats per load, NCH chunks per lane.
+struct LaneMap {
+  int DK, LPH, lph_shift, vec, nch;
+};
+
+int lane_map(int d, int n_heads, LaneMap& m, const char* who) {
+  HGT_REQUIRE(n_heads >= 1 && n_heads <= 32 && d % n_heads == 0, "%s: bad d=%d / n_heads=%d", who, d, n_heads);
+  m.DK = d / n_heads;
+  int hp = 1;
+  while (hp < n_heads) hp <<= 1;
+  m.LPH = 32 / hp;
+  int shift = 0;
+  while ((1 << shift) < m.LPH) ++shift;
+  m.lph_shift = shift;
+  m.vec = 1;
+  for (int v : {4, 2})
+    if (m.DK % v == 0 && m.DK / v >= m.LPH) { m.vec = v; break; }
+  int chunks = (m.DK + m.vec * m.LPH - 1) / (m.vec * m.LPH);
+  m.nch = 1;
+  while (m.nch < chunks) m.nch <<= 1;
+  HGT_REQUIRE(m.nch <= 8, "%s: head width d_k=%d needs %d chunks per lane (max 8)", who, m.DK, chunks);
+  return 0;
+}
+
+template <typename Params>
+int launch_pass(const Params& p, const LaneMap& lm, int n_tiles, cudaStream_t st, bool det) {
+  HGT_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), st));
+  int grid = hgt_sm_count() * 4;
+  int max_ctas = (n_tiles + kWarps - 1) / kWarps;
+  if (grid > max_ctas) grid = max_ctas;
+  if (lm.vec == 4) return dispatch<Params, 4>(p, lm.nch, grid, st, det);
+  if (lm.vec == 2) return dispatch<Params, 2>(p, lm.nch, grid, st, det);
+  return dispatch<Params, 1>(p, lm.nch, grid, st, det);
+}
+
+int merge_pieces(const int32_t* hubs, int32_t n_hubs, const int32_t* d_counts, const float* partial, int width,
+                 float* out, cudaStream_t st) {
+  if (n_hubs <= 0) return 0;
+  const int grid = n_hubs < 4 * hgt_sm_count() ? n_hubs : 4 * hgt_sm_count();
+  k_merge_piece_rows<<<grid, 256, 0, st>>>(hubs, d_counts, n_hubs, partial, width, out);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -218,26 +474,89 @@ extern "C" int hgt_edge_backward(const float* q, const float* kv, const float* k
   BwdParams p;
   p.q = q; p.kv = kv; p.kvr = kvr; p.agg = agg; p.dagg = dagg; p.stats = stats; p.row_ptr = row_ptr;
   p.kv_row = kv_row; p.rte_row = rte_row; p.tiles = tiles; p.n_tiles = n_tiles; p.d_counts = d_tile_counts; p.d = d; p.H = n_heads;
-  p.DK = d / n_heads;
-  int hp = 1;
-  while (hp < n_heads) hp <<= 1;
-  p.LPH = 32 / hp;
-  int shift = 0;
-  while ((1 << shift) < p.LPH) ++shift;
-  p.lph_shift = shift;
+  LaneMap lm;
+  int rc = lane_map(d, n_heads, lm, "hgt_edge_backward");
+  if (rc) return rc;
+  p.DK = lm.DK; p.LPH = lm.LPH; p.lph_shift = lm.lph_shift;
   p.dq = dq; p.dkv = dkv; p.dkvr = dkvr;
   p.tile_counter = reinterpret_cast<int32_t*>(workspace);
-  int vec = 1;
-  for (int v : {4, 2})
-    if (p.DK % v == 0 && p.DK / v >= p.LPH) { vec = v; break; }
-  int chunks = (p.DK + vec * p.LPH - 1) / (vec * p.LPH), nch = 1;
-  while (nch < chunks) nch <<= 1;
-  HGT_REQUIRE(nch <= 8, "hgt_edge_backward: head width d_k=%d needs %d chunks per lane (max 8)", p.DK, chunks);
-  HGT_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), st));
-  int grid = hgt_sm_count() * 4;
-  int max_ctas = (n_tiles + kWarps - 1) / kWarps;
-  if (grid > max_ctas) grid = max_ctas;
-  if (vec == 4) return dispatch<4>(p, nch, grid, st);
-  if (vec == 2) return dispatch<2>(p, nch, grid, st);
-  return dispatch<1>(p, nch, grid, st);
+  p.D = nullptr; p.partial = nullptr;
+  return launch_pass(p, lm, n_tiles, st, false);
+}
+
+extern "C" int hgt_edge_backward_det_workspace_bytes(int32_t n_split_dst, int32_t n_split_rows, int32_t d,
+                                                     size_t* out_bytes) {
+  HGT_REQUIRE(out_bytes && d > 0 && n_split_dst >= 0 && n_split_rows >= 0,
+              "hgt_edge_backward_det_workspace_bytes: bad argument");
+  const size_t a = (size_t)n_split_dst * d, b = (size_t)n_split_rows * 2 * d;
+  *out_bytes = 256 + sizeof(float) * (a > b ? a : b);
+  return 0;
+}
+
+extern "C" int hgt_edge_backward_dst(const float* q, const float* kv, const float* kvr, const float* agg,
+                                     const float* dagg, const float* stats, const int32_t* row_ptr,
+                                     const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles,
+                                     int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
+                                     int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D,
+                                     void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                                     void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  HGT_REQUIRE((kvr != nullptr) == (rte_row != nullptr), "hgt_edge_backward_dst: kvr and rte_row must go together");
+  HGT_REQUIRE(dq && D, "hgt_edge_backward_dst: NULL output");
+  size_t need = 0;
+  hgt_edge_backward_det_workspace_bytes(n_split > 0 ? n_split : 0, 0, d, &need);
+  HGT_REQUIRE(workspace && workspace_bytes >= need, "hgt_edge_backward_dst: workspace too small (%zu < %zu)",
+              workspace_bytes, need);
+  HGT_REQUIRE(n_split <= 0 || (hubs && n_hubs > 0), "hgt_edge_backward_dst: split tiles present but no hub list given");
+  // destinations without in-edges keep a zero dq
+  if (n_nodes > 0) HGT_CHECK_CUDA(cudaMemsetAsync(dq, 0, (size_t)n_nodes * d * sizeof(float), st));
+  if (n_nodes == 0 || n_tiles == 0) return 0;
+  LaneMap lm;
+  int rc = lane_map(d, n_heads, lm, "hgt_edge_backward_dst");
+  if (rc) return rc;
+  BwdParams p;
+  p.q = q; p.kv = kv; p.kvr = kvr; p.agg = agg; p.dagg = dagg; p.stats = stats; p.row_ptr = row_ptr;
+  p.kv_row = kv_row; p.rte_row = rte_row; p.tiles = tiles; p.n_tiles = n_tiles; p.d_counts = d_tile_counts;
+  p.d = d; p.H = n_heads; p.DK = lm.DK; p.LPH = lm.LPH; p.lph_shift = lm.lph_shift;
+  p.dq = dq; p.dkv = nullptr; p.dkvr = nullptr;
+  p.tile_counter = reinterpret_cast<int32_t*>(workspace);
+  p.D = D;
+  p.partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  if ((rc = launch_pass(p, lm, n_tiles, st, true))) return rc;
+  return n_split > 0 ? merge_pieces(hubs, n_hubs, d_tile_counts, p.partial, d, dq, st) : 0;
+}
+
+extern "C" int hgt_edge_backward_rows(const float* q, const float* dagg, const float* stats, const float* D,
+                                      const float* own, const float* oth, const int32_t* src_ptr,
+                                      const int32_t* src_dst, const int32_t* src_oth, int32_t n_rows,
+                                      int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
+                                      const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads, float* grad,
+                                      void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                                      void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  HGT_REQUIRE(own && grad && (oth == nullptr || src_oth), "hgt_edge_backward_rows: NULL argument");
+  HGT_REQUIRE(n_rows >= 0 && own_rows_total >= n_rows, "hgt_edge_backward_rows: n_rows=%d own_rows_total=%lld", n_rows,
+              (long long)own_rows_total);
+  size_t need = 0;
+  hgt_edge_backward_det_workspace_bytes(0, n_split > 0 ? n_split : 0, d, &need);
+  HGT_REQUIRE(workspace && workspace_bytes >= need, "hgt_edge_backward_rows: workspace too small (%zu < %zu)",
+              workspace_bytes, need);
+  HGT_REQUIRE(n_split <= 0 || (hubs && n_hubs > 0), "hgt_edge_backward_rows: split tiles present but no hub list given");
+  // rows past n_rows (the trailing all-zero row that collects unmatched edges) get no work: their gradient is zero
+  if (own_rows_total > n_rows)
+    HGT_CHECK_CUDA(cudaMemsetAsync(grad + (int64_t)n_rows * 2 * d, 0, (size_t)(own_rows_total - n_rows) * 2 * d * sizeof(float),
+                                   st));
+  if (n_rows == 0 || n_tiles == 0) return 0;
+  LaneMap lm;
+  int rc = lane_map(d, n_heads, lm, "hgt_edge_backward_rows");
+  if (rc) return rc;
+  RowParams p;
+  p.q = q; p.dagg = dagg; p.stats = stats; p.D = D; p.own = own; p.oth = oth; p.ptr = src_ptr; p.e_dst = src_dst;
+  p.e_oth = src_oth; p.tiles = tiles; p.n_tiles = n_tiles; p.d_counts = d_tile_counts;
+  p.d = d; p.H = n_heads; p.DK = lm.DK; p.LPH = lm.LPH; p.lph_shift = lm.lph_shift;
+  p.grad = grad;
+  p.tile_counter = reinterpret_cast<int32_t*>(workspace);
+  p.partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  if ((rc = launch_pass(p, lm, n_tiles, st, true))) return rc;
+  return n_split > 0 ? merge_pieces(hubs, n_hubs, d_tile_counts, p.partial, 2 * d, grad, st) : 0;
 }

@@ -118,9 +118,11 @@ struct GcTask {            // one (group, column block)
 // One CTA = one task x SPLIT_ROWS rows.  Thread (cx, ry): float4 column cx*4, rows ry, ry+RY, ...; column sums are reduced
 // across ry in shared memory and added to db with one atomic per column and CTA.
 constexpr int SPLIT_ROWS = 256;
-__global__ void __launch_bounds__(256)
-k_split_colsum(const float* __restrict__ dout, const GcTask* __restrict__ tasks, int n_tasks, int width,
-               __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, float* __restrict__ db) {
+// DET: the column sums of a CTA go to its own row of db_part [unit][width] (reduced in unit order by k_reduce_rows).
+template <bool DET>
+__device__ __forceinline__ void split_colsum(const float* __restrict__ dout, const GcTask* __restrict__ tasks, int n_tasks,
+                                             int width, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo,
+                                             float* __restrict__ db) {
   __shared__ float red[256 * 4];
   int unit = blockIdx.x, t = 0;
   while (t + 1 < n_tasks && unit >= tasks[t + 1].first_unit) ++t;
@@ -153,12 +155,24 @@ k_split_colsum(const float* __restrict__ dout, const GcTask* __restrict__ tasks,
         for (int j = 0; j < 4; ++j) {
           float a = 0.f;
           for (int y = 0; y < ryn; ++y) a += red[(y * cxn + cx) * 4 + j];
-          atomicAdd(db + tk.w_row + c0 * 4 + j, a);
+          if constexpr (DET) db[(int64_t)unit * width + c0 * 4 + j] = a;
+          else atomicAdd(db + tk.w_row + c0 * 4 + j, a);
         }
       }
       __syncthreads();
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+k_split_colsum(const float* __restrict__ dout, const GcTask* __restrict__ tasks, int n_tasks, int width,
+               __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, float* __restrict__ db) {
+  split_colsum<false>(dout, tasks, n_tasks, width, hi, lo, db);
+}
+__global__ void __launch_bounds__(256)
+k_split_colsum_det(const float* __restrict__ dout, const GcTask* __restrict__ tasks, int n_tasks, int width,
+                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, float* __restrict__ db_part) {
+  split_colsum<true>(dout, tasks, n_tasks, width, hi, lo, db_part);
 }
 
 // ---- dX: dA tile = sum over (column block, k-block) of dOut tile x W^T tile --------------------------------------------
@@ -311,6 +325,53 @@ struct DwJob {
   }
 };
 
+// Deterministic dW: every unit (task, chunk, tile) stores its partial tile into its own [width, K_in] slot
+// (slot = unit / (m_tiles * n_tiles) = the task's first chunk slot + chunk); k_reduce_rows adds the slots in chunk order.
+struct DwJobDet : DwJob {
+  float* part;
+
+  struct Tile : DwJob::Tile {
+    int64_t slot;
+  };
+
+  __device__ int decode(int unit, Tile& t) const {
+    t.slot = unit / (m_tiles * n_tiles);
+    return DwJob::decode(unit, t);
+  }
+  template <int BN>
+  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+    const int rows = width - t.mt * BM - 64 * c;
+    const int cols = K_in - t.n0;
+    float* o = part + (t.slot * width + t.mt * BM + 64 * c) * K_in + t.n0;
+    const int ld = K_in;
+    for_each_pair<BN>(acc, wq, lane, [&](int r, int col, float v0, float v1) {
+      if (r < rows && col < cols) *reinterpret_cast<float2*>(o + (int64_t)r * ld + col) = make_float2(v0, v1);
+    });
+  }
+};
+
+// out[wr, k] += sum over the tasks covering W row wr (task order), over their slots (chunk order) of
+// part[slot, wr - w_row, k].  slot = first_unit / units_per_slot + chunk, n_chunks slots per task.  One thread per
+// element: each W row has one owner however many tasks share it.  k_cols = 1 reduces the bias partials.
+__global__ void k_reduce_rows(const float* __restrict__ part, const GcTask* __restrict__ tasks, int n_tasks, int width,
+                              int k_cols, int64_t w_rows, int units_per_slot, int bias_only, float* __restrict__ out) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= w_rows * k_cols) return;
+  const int64_t wr = i / k_cols;
+  const int k = (int)(i - wr * k_cols);
+  float s = 0.f;
+  bool any = false;
+  for (int t = 0; t < n_tasks; ++t) {
+    const GcTask& tk = tasks[t];
+    if (wr < tk.w_row || wr >= tk.w_row + width || (bias_only && !tk.has_bias)) continue;
+    any = true;
+    const int64_t slot0 = tk.first_unit / units_per_slot;
+    const int64_t n = wr - tk.w_row;
+    for (int c = 0; c < tk.n_chunks; ++c) s += part[((slot0 + c) * width + n) * k_cols + k];
+  }
+  if (any) out[i] += s;
+}
+
 // ---- SIMT fp32 fallbacks ------------------------------------------------------------------------------------------------
 // dA[a_row0 + m, k] (+)= sum_c sum_n dOut_c[m, n] * W[w_row + n, k].  One thread per (m, k); atomicAdd because groups may
 // share A rows (the RTE tables: every <type, relation> pair projects the same 240-row table).
@@ -338,12 +399,43 @@ __global__ void k_lin_dx_simt(const float* __restrict__ dout, const float* __res
   atomicAdd(dA + o, acc);
 }
 
+// Deterministic dA: one thread per element of rows [0, a_rows); the groups that cover the row are added in group order.
+__global__ void k_lin_dx_simt_det(const float* __restrict__ dout, const float* __restrict__ W,
+                                  const GcTask* __restrict__ tasks, const int32_t* __restrict__ group_task0,
+                                  const hgt_lin_group* __restrict__ groups, int n_groups, int64_t a_rows, int K_in,
+                                  int width, const float* __restrict__ gelu_aux, int accumulate, float* __restrict__ dA) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= a_rows * K_in) return;
+  const int64_t row = i / K_in;
+  const int k = (int)(i - row * K_in);
+  float acc = 0.f;
+  bool any = false;
+  for (int g = 0; g < n_groups; ++g) {
+    const hgt_lin_group grp = groups[g];
+    if (row < grp.a_row0 || row >= grp.a_row0 + grp.m) continue;
+    any = true;
+    const int64_t m = row - grp.a_row0;
+    for (int c = 0; c < grp.n_cblocks; ++c) {
+      const GcTask tk = tasks[group_task0[g] + c];
+      const float* drow = dout + tk.out_off + m * tk.ld;
+      const float* wcol = W + (int64_t)tk.w_row * K_in + k;
+      for (int n = 0; n < width; ++n) acc = fmaf(drow[n], wcol[(int64_t)n * K_in], acc);
+    }
+  }
+  if (any && gelu_aux) acc *= gelu_grad(gelu_aux[i]);
+  dA[i] = accumulate ? dA[i] + acc : acc;
+}
+
 // dW[w_row + n, k] += sum_m dOut_c[m, n] * A[a_row0 + m, k];  db[w_row + n] += sum_m dOut_c[m, n].
 // One CTA = one task x (32 n) x (32 k) x a chunk of rows; 256 threads, 4 outputs each.
 constexpr int DW_SIMT_ROWS = 2048;
-__global__ void __launch_bounds__(256)
-k_lin_dw_simt(const float* __restrict__ dout, const float* __restrict__ A, int64_t lda, const GcTask* __restrict__ tasks,
-              int n_tasks, int K_in, int width, int n_tiles, int k_tiles, float* __restrict__ dW, float* __restrict__ db) {
+// DET: partial tiles / bias sums go to the unit's slot (unit / (n_tiles * k_tiles)) of dW = part [slot][width][K_in] and
+// db = db_part [slot][width]; chunks of chunk_rows rows.
+template <bool DET>
+__device__ __forceinline__ void lin_dw_simt(const float* __restrict__ dout, const float* __restrict__ A, int64_t lda,
+                                            const GcTask* __restrict__ tasks, int n_tasks, int K_in, int width,
+                                            int n_tiles, int k_tiles, int64_t chunk_rows, float* __restrict__ dW,
+                                            float* __restrict__ db) {
   __shared__ float sd[32][33], sa[32][33];
   int unit = blockIdx.x, t = 0;
   while (t + 1 < n_tasks && unit >= tasks[t + 1].first_unit) ++t;
@@ -353,7 +445,7 @@ k_lin_dw_simt(const float* __restrict__ dout, const float* __restrict__ A, int64
   local -= chunk * n_tiles * k_tiles;
   const int ntile = local / k_tiles, ktile = local - ntile * k_tiles;
   const int n0 = ntile * 32, k0 = ktile * 32;
-  const int64_t r0 = (int64_t)chunk * DW_SIMT_ROWS, r1 = min(tk.rows, r0 + DW_SIMT_ROWS);
+  const int64_t r0 = (int64_t)chunk * chunk_rows, r1 = min(tk.rows, r0 + chunk_rows);
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;       // ty: 0..7
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
   float bsum = 0.f;
@@ -385,9 +477,26 @@ k_lin_dw_simt(const float* __restrict__ dout, const float* __restrict__ A, int64
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int n = n0 + ty + 8 * j;
-    if (n < width && k0 + tx < K_in) atomicAdd(dW + ((int64_t)tk.w_row + n) * K_in + k0 + tx, acc[j]);
+    if (n < width && k0 + tx < K_in) {
+      if constexpr (DET) dW[((int64_t)(unit / (n_tiles * k_tiles)) * width + n) * K_in + k0 + tx] = acc[j];
+      else atomicAdd(dW + ((int64_t)tk.w_row + n) * K_in + k0 + tx, acc[j]);
+    }
   }
-  if (db && tk.has_bias && ktile == 0 && ty == 0 && n0 + tx < width) atomicAdd(db + tk.w_row + n0 + tx, bsum);
+  if (db && tk.has_bias && ktile == 0 && ty == 0 && n0 + tx < width) {
+    if constexpr (DET) db[(int64_t)(unit / (n_tiles * k_tiles)) * width + n0 + tx] = bsum;
+    else atomicAdd(db + tk.w_row + n0 + tx, bsum);
+  }
+}
+__global__ void __launch_bounds__(256)
+k_lin_dw_simt(const float* __restrict__ dout, const float* __restrict__ A, int64_t lda, const GcTask* __restrict__ tasks,
+              int n_tasks, int K_in, int width, int n_tiles, int k_tiles, float* __restrict__ dW, float* __restrict__ db) {
+  lin_dw_simt<false>(dout, A, lda, tasks, n_tasks, K_in, width, n_tiles, k_tiles, DW_SIMT_ROWS, dW, db);
+}
+__global__ void __launch_bounds__(256)
+k_lin_dw_simt_det(const float* __restrict__ dout, const float* __restrict__ A, int64_t lda,
+                  const GcTask* __restrict__ tasks, int n_tasks, int K_in, int width, int n_tiles, int k_tiles,
+                  int64_t chunk_rows, float* __restrict__ dw_part, float* __restrict__ db_part) {
+  lin_dw_simt<true>(dout, A, lda, tasks, n_tasks, K_in, width, n_tiles, k_tiles, chunk_rows, dw_part, db_part);
 }
 
 // ---- host helpers ---------------------------------------------------------------------------------------------------------
@@ -428,8 +537,27 @@ struct BwdLayout {
   int Kp, wpad;
   int64_t a_rows, w_rows, wt_cols;
   int n_tasks;
+  int64_t dw_chunk;          // rows per dW reduction chunk (deterministic mode)
   size_t off_maps, off_tasks, off_gt0, off_gfirst, off_dhi, off_dlo, off_ahi, off_alo, off_wthi, off_wtlo, total;
+  size_t off_part, off_dbp;  // deterministic mode: dW partial slots [slot][width][K], bias partials [unit][width]
 };
+
+// Rows per chunk of the tensor-core dW reduction: a few waves of CTAs over all (task, tile) pairs.
+int64_t tc_dw_chunk(int64_t task_rows, int width, int K) {
+  const int64_t m_tiles = (width + BM - 1) / BM, n_tiles = (K + pick_tile_n(K) - 1) / pick_tile_n(K);
+  int64_t chunk = task_rows * m_tiles * n_tiles / (4 * (int64_t)hgt_sm_count());
+  chunk = (chunk + BK - 1) / BK * BK;
+  if (chunk < 1024) chunk = 1024;
+  if (chunk > 32768) chunk = 32768;
+  return chunk;
+}
+
+// The SIMT dW keeps at most ~256 partial slots in deterministic mode (plus one per task for rounding).
+int64_t simt_det_chunk(int64_t task_rows) {
+  int64_t chunk = (task_rows + 255) / 256;
+  chunk = (chunk + 31) / 32 * 32;
+  return chunk < DW_SIMT_ROWS ? DW_SIMT_ROWS : chunk;
+}
 
 bool groups_overlap(const hgt_lin_group* h, int n) {
   for (int i = 0; i < n; ++i)
@@ -457,7 +585,7 @@ bool bwd_tc_ok(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_cblock
 }
 
 BwdLayout bwd_layout(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_cblock* h_cb, int K, int width,
-                     int64_t lda, int64_t dout_elems, bool have_dsplit, bool have_asplit, int impl) {
+                     int64_t lda, int64_t dout_elems, bool have_dsplit, bool have_asplit, int impl, bool det) {
   BwdLayout L{};
   L.tc = impl == 2 || (impl == 0 && bwd_tc_ok(h_groups, n_groups, h_cb, K, width, lda));
   L.Kp = K;
@@ -484,6 +612,20 @@ BwdLayout bwd_layout(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_
     L.off_alo = take(have_asplit ? 0 : (size_t)L.a_rows * L.Kp * 2);
     L.off_wthi = take((size_t)K * L.wt_cols * 2);
     L.off_wtlo = take((size_t)K * L.wt_cols * 2);
+  }
+  L.dw_chunk = 0;
+  L.off_part = L.off_dbp = 0;
+  if (det) {
+    int64_t task_rows = 0;
+    for (int g = 0; g < n_groups; ++g) task_rows += h_groups[g].m * h_groups[g].n_cblocks;
+    L.dw_chunk = L.tc ? tc_dw_chunk(task_rows, width, K) : simt_det_chunk(task_rows);
+    int64_t slots = 0, units = 0;
+    for (int g = 0; g < n_groups; ++g) {
+      slots += (h_groups[g].m + L.dw_chunk - 1) / L.dw_chunk * h_groups[g].n_cblocks;
+      units += (h_groups[g].m + SPLIT_ROWS - 1) / SPLIT_ROWS * h_groups[g].n_cblocks;
+    }
+    L.off_part = take((size_t)slots * width * K * sizeof(float));
+    L.off_dbp = take((size_t)std::max(slots, L.tc ? units : 0) * width * sizeof(float));
   }
   L.total = p + 256;
   return L;
@@ -515,6 +657,19 @@ int launch_bwd(const DwJob& job, unsigned tiles, cudaStream_t st) {
   return 0;
 }
 
+template <int BN>
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc_det(const __grid_constant__ DwJobDet job) {
+  split3_tile<BN, true>(job);
+}
+template <int BN>
+int launch_bwd(const DwJobDet& job, unsigned tiles, cudaStream_t st) {
+  const size_t smem = tile_smem_bytes<BN>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc_det<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_lin_dw_tc_det<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int hgt_act_split(const float* in, int64_t ld, int64_t rows, int32_t K, int32_t act, float* out_f32,
@@ -531,23 +686,26 @@ extern "C" int hgt_act_split(const float* in, int64_t ld, int64_t rows, int32_t 
   return 0;
 }
 
-extern "C" int hgt_typed_linear_bwd_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups,
-                                                    const hgt_lin_cblock* h_cblocks, int32_t K, int32_t cb_width,
-                                                    int64_t lda, int64_t dout_elems, int32_t have_dout_split,
-                                                    int32_t have_a_split, int32_t impl, size_t* out_bytes) {
+namespace {
+
+GcTask* d_tasks_ptr(char* base, const BwdLayout& L) { return reinterpret_cast<GcTask*>(base + L.off_tasks); }
+
+int bwd_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks, int32_t K,
+                        int32_t cb_width, int64_t lda, int64_t dout_elems, int32_t have_dout_split, int32_t have_a_split,
+                        int32_t impl, size_t* out_bytes, bool det) {
   HGT_REQUIRE(out_bytes && (n_groups == 0 || (h_groups && h_cblocks)), "hgt_typed_linear_bwd_workspace_bytes: NULL argument");
   HGT_REQUIRE(n_groups >= 0 && n_groups <= kMaxGroups, "hgt_typed_linear_bwd: n_groups=%d exceeds %d", n_groups, kMaxGroups);
   *out_bytes = bwd_layout(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dout_split != 0,
-                          have_a_split != 0, impl).total;
+                          have_a_split != 0, impl, det).total;
   return 0;
 }
 
-extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo, int64_t dout_elems,
-                                    const float* A, int64_t lda, const void* a_hi_in, const void* a_lo_in,
-                                    const float* W, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
-                                    const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
-                                    float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
-                                    int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
+int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo, int64_t dout_elems,
+                     const float* A, int64_t lda, const void* a_hi_in, const void* a_lo_in,
+                     const float* W, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                     const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
+                     float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
+                     int32_t impl, void* workspace, size_t workspace_bytes, void* stream_, bool det) {
   cudaStream_t st = (cudaStream_t)stream_;
   HGT_REQUIRE(n_groups >= 0 && n_groups <= kMaxGroups, "hgt_typed_linear_bwd: n_groups=%d exceeds %d", n_groups, kMaxGroups);
   HGT_REQUIRE(K > 0 && cb_width > 0 && W, "hgt_typed_linear_bwd: K=%d cb_width=%d", K, cb_width);
@@ -555,7 +713,8 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
   HGT_REQUIRE(groups && h_groups && h_cblocks, "hgt_typed_linear_bwd: NULL group tables");
   const bool have_dsplit = dout_hi && dout_lo, have_asplit = a_hi_in && a_lo_in;
   HGT_REQUIRE(dout || have_dsplit, "hgt_typed_linear_bwd: neither dout nor its bf16 split given");
-  const BwdLayout L = bwd_layout(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dsplit, have_asplit, impl);
+  const BwdLayout L = bwd_layout(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dsplit, have_asplit, impl,
+                                 det);
   HGT_REQUIRE(workspace && workspace_bytes >= L.total, "hgt_typed_linear_bwd: workspace too small (%zu < %zu)",
               workspace_bytes, L.total);
   if (L.tc)
@@ -565,6 +724,8 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
   else
     HGT_REQUIRE(dout && (A || !dW), "hgt_typed_linear_bwd: the SIMT path needs fp32 dout and A");
   char* base = reinterpret_cast<char*>(hgt_align_up(reinterpret_cast<size_t>(workspace), 256));
+  float* part = det ? reinterpret_cast<float*>(base + L.off_part) : nullptr;
+  float* db_part = det ? reinterpret_cast<float*>(base + L.off_dbp) : nullptr;
 
   // ---- task table (one entry per group x column block) ----
   std::vector<GcTask> tasks(std::max(L.n_tasks, 1));
@@ -600,6 +761,15 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
   }
   gt0[n_groups] = nt;
   gfirst[n_groups] = elems;
+  // deterministic mode: sum of partial slots per W row (tasks in order, then slots in order); each row has one owner
+  auto reduce_rows = [&](const float* src, int k_cols, int units_per_slot, int bias_only, float* out) -> int {
+    const int64_t n = L.w_rows * k_cols;
+    if (n == 0) return 0;
+    k_reduce_rows<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src, d_tasks_ptr(base, L), nt, cb_width, k_cols,
+                                                                L.w_rows, units_per_slot, bias_only, out);
+    HGT_LAUNCH_CHECK();
+    return 0;
+  };
   GcTask* d_tasks = reinterpret_cast<GcTask*>(base + L.off_tasks);
   int32_t* d_gt0 = reinterpret_cast<int32_t*>(base + L.off_gt0);
   int64_t* d_gfirst = reinterpret_cast<int64_t*>(base + L.off_gfirst);
@@ -613,7 +783,15 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
 
   if (!L.tc) {
     // ---------------- SIMT fp32 path ----------------
-    if (dA) {
+    if (dA && det) {
+      if ((rc = upload_tasks())) return rc;
+      const int64_t n = L.a_rows * K;
+      if (n > 0) {
+        k_lin_dx_simt_det<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dout, W, d_tasks, d_gt0, groups, n_groups, L.a_rows,
+                                                                       K, cb_width, gelu_aux, accumulate_dA, dA);
+        HGT_LAUNCH_CHECK();
+      }
+    } else if (dA) {
       if (!accumulate_dA) HGT_CHECK_CUDA(cudaMemsetAsync(dA, 0, (size_t)L.a_rows * K * sizeof(float), st));
       if ((rc = upload_tasks())) return rc;
       if (elems > 0) {
@@ -624,15 +802,22 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
     }
     if (dW) {
       const int n_tiles = (cb_width + 31) / 32, k_tiles = (K + 31) / 32;
+      const int64_t chunk_rows = det ? L.dw_chunk : DW_SIMT_ROWS;
       int64_t units = 0;
       for (int t = 0; t < nt; ++t) {
         tasks[t].first_unit = (int32_t)units;
-        tasks[t].n_chunks = (int32_t)((tasks[t].rows + DW_SIMT_ROWS - 1) / DW_SIMT_ROWS);
+        tasks[t].n_chunks = (int32_t)((tasks[t].rows + chunk_rows - 1) / chunk_rows);
         units += (int64_t)tasks[t].n_chunks * n_tiles * k_tiles;
         HGT_REQUIRE(units < 2147483647ll, "hgt_typed_linear_bwd: too many units");
       }
       if ((rc = upload_tasks())) return rc;
-      if (units > 0) {
+      if (units > 0 && det) {
+        k_lin_dw_simt_det<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles,
+                                                           chunk_rows, part, db ? db_part : nullptr);
+        HGT_LAUNCH_CHECK();
+        if ((rc = reduce_rows(part, K, n_tiles * k_tiles, 0, dW))) return rc;
+        if (db && (rc = reduce_rows(db_part, 1, n_tiles * k_tiles, 1, db))) return rc;
+      } else if (units > 0) {
         k_lin_dw_simt<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles, dW, db);
         HGT_LAUNCH_CHECK();
       }
@@ -657,11 +842,16 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
     int64_t units = 0;
     for (int t = 0; t < nt; ++t) {
       tasks[t].first_unit = (int32_t)units;
-      units += (tasks[t].rows + SPLIT_ROWS - 1) / SPLIT_ROWS;
+      tasks[t].n_chunks = (int32_t)((tasks[t].rows + SPLIT_ROWS - 1) / SPLIT_ROWS);
+      units += tasks[t].n_chunks;
       HGT_REQUIRE(units < 2147483647ll, "hgt_typed_linear_bwd: too many units");
     }
     if ((rc = upload_tasks())) return rc;
-    if (units > 0) {
+    if (units > 0 && det) {
+      k_split_colsum_det<<<(unsigned)units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo, db ? db_part : nullptr);
+      HGT_LAUNCH_CHECK();
+      if (db && (rc = reduce_rows(db_part, 1, 1, 1, db))) return rc;
+    } else if (units > 0) {
       k_split_colsum<<<(unsigned)units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo, db);
       HGT_LAUNCH_CHECK();
     }
@@ -747,12 +937,9 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
     const int tile_n = pick_tile_n(K);
     const int m_tiles = (cb_width + BM - 1) / BM, n_tiles = (K + tile_n - 1) / tile_n;
     // chunk the reduction so that the grid has a few waves of CTAs
-    int64_t work = 0;
-    for (int t = 0; t < nt; ++t) work += tasks[t].rows * m_tiles * n_tiles;
-    int64_t chunk = work / (4 * (int64_t)hgt_sm_count());
-    chunk = (chunk + BK - 1) / BK * BK;
-    if (chunk < 1024) chunk = 1024;
-    if (chunk > 32768) chunk = 32768;
+    int64_t task_rows = 0;
+    for (int t = 0; t < nt; ++t) task_rows += tasks[t].rows;
+    const int64_t chunk = tc_dw_chunk(task_rows, cb_width, K);
     int64_t units = 0;
     for (int t = 0; t < nt; ++t) {
       tasks[t].first_unit = (int32_t)units;
@@ -775,13 +962,66 @@ extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, cons
       job.chunk_rows = (int)chunk;
       job.tile_n = tile_n;
       job.dW = dW;
-      switch (tile_n) {
-        case 64: rc = launch_bwd<64>(job, (unsigned)units, st); break;
-        case 128: rc = launch_bwd<128>(job, (unsigned)units, st); break;
-        default: rc = launch_bwd<256>(job, (unsigned)units, st); break;
+      if (det) {
+        DwJobDet dj;
+        static_cast<DwJob&>(dj) = job;
+        dj.part = part;
+        switch (tile_n) {
+          case 64: rc = launch_bwd<64>(dj, (unsigned)units, st); break;
+          case 128: rc = launch_bwd<128>(dj, (unsigned)units, st); break;
+          default: rc = launch_bwd<256>(dj, (unsigned)units, st); break;
+        }
+        if (rc) return rc;
+        if ((rc = reduce_rows(part, K, m_tiles * n_tiles, 0, dW))) return rc;
+      } else {
+        switch (tile_n) {
+          case 64: rc = launch_bwd<64>(job, (unsigned)units, st); break;
+          case 128: rc = launch_bwd<128>(job, (unsigned)units, st); break;
+          default: rc = launch_bwd<256>(job, (unsigned)units, st); break;
+        }
+        if (rc) return rc;
       }
-      if (rc) return rc;
     }
   }
   return 0;
+}
+
+}  // namespace
+
+extern "C" int hgt_typed_linear_bwd_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups,
+                                                    const hgt_lin_cblock* h_cblocks, int32_t K, int32_t cb_width,
+                                                    int64_t lda, int64_t dout_elems, int32_t have_dout_split,
+                                                    int32_t have_a_split, int32_t impl, size_t* out_bytes) {
+  return bwd_workspace_bytes(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dout_split, have_a_split,
+                             impl, out_bytes, false);
+}
+
+extern "C" int hgt_typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo, int64_t dout_elems,
+                                    const float* A, int64_t lda, const void* a_hi_in, const void* a_lo_in,
+                                    const float* W, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                                    const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
+                                    float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
+                                    int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
+  return typed_linear_bwd(dout, dout_hi, dout_lo, dout_elems, A, lda, a_hi_in, a_lo_in, W, K, cb_width, groups, h_groups,
+                          n_groups, h_cblocks, dA, accumulate_dA, gelu_aux, dW, db, impl, workspace, workspace_bytes,
+                          stream_, false);
+}
+
+extern "C" int hgt_typed_linear_bwd_det_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups,
+                                                        const hgt_lin_cblock* h_cblocks, int32_t K, int32_t cb_width,
+                                                        int64_t lda, int64_t dout_elems, int32_t have_dout_split,
+                                                        int32_t have_a_split, int32_t impl, size_t* out_bytes) {
+  return bwd_workspace_bytes(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dout_split, have_a_split,
+                             impl, out_bytes, true);
+}
+
+extern "C" int hgt_typed_linear_bwd_det(const float* dout, const void* dout_hi, const void* dout_lo, int64_t dout_elems,
+                                        const float* A, int64_t lda, const void* a_hi_in, const void* a_lo_in,
+                                        const float* W, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                                        const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
+                                        float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
+                                        int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
+  return typed_linear_bwd(dout, dout_hi, dout_lo, dout_elems, A, lda, a_hi_in, a_lo_in, W, K, cb_width, groups, h_groups,
+                          n_groups, h_cblocks, dA, accumulate_dA, gelu_aux, dW, db, impl, workspace, workspace_bytes,
+                          stream_, true);
 }

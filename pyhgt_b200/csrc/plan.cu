@@ -369,6 +369,40 @@ k_halo_push_split(const float4* __restrict__ x_own, const int32_t* __restrict__ 
 
 inline unsigned blocks_for(int64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
+// ---- source-major index (deterministic edge backward) ------------------------------------------
+__global__ void k_iota(int64_t n, int32_t* __restrict__ out) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = (int32_t)i;
+}
+
+// entry j of the index: CSR position pos[j] (stably sorted by key) -> its destination (rank order) and its row in the
+// other table; pos and dst share a buffer (each thread reads and writes its own entry)
+__global__ void k_source_fill(const int32_t* __restrict__ row_ptr, int64_t N, int64_t E, const int32_t* __restrict__ other,
+                              int32_t* __restrict__ pos_dst, int32_t* __restrict__ oth_out) {
+  int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (j >= E) return;
+  const int32_t c = pos_dst[j];
+  int64_t lo = 0, hi = N;                                  // last k with row_ptr[k] <= c
+  while (hi - lo > 1) {
+    int64_t mid = (lo + hi) >> 1;
+    if (row_ptr[mid] <= c) lo = mid; else hi = mid;
+  }
+  pos_dst[j] = (int32_t)lo;
+  if (oth_out) oth_out[j] = other[c];
+}
+
+// ptr[r] = first index entry whose key is >= r (keys sorted); ptr[n_rows] therefore excludes the trailing zero row
+__global__ void k_source_ptr(const int32_t* __restrict__ keys, int64_t E, int32_t n_rows, int32_t* __restrict__ ptr) {
+  int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (r > n_rows) return;
+  int64_t lo = 0, hi = E;
+  while (lo < hi) {
+    int64_t mid = (lo + hi) >> 1;
+    if (keys[mid] < r) lo = mid + 1; else hi = mid;
+  }
+  ptr[r] = (int32_t)lo;
+}
+
 }  // namespace
 
 extern "C" int hgt_plan_workspace_bytes(int64_t n_nodes, int64_t n_edges, size_t* out_bytes) {
@@ -576,6 +610,33 @@ extern "C" int hgt_halo_push_split(const float* x_own, const int32_t* push_peer,
   else if (vpr <= 64) k_halo_push_split<2><<<g, 256, 0, st>>>(xo, push_peer, push_src, push_dst, n_items, vpr, self_rank, row_base, hp, lp, xl);
   else if (vpr <= 128) k_halo_push_split<4><<<g, 256, 0, st>>>(xo, push_peer, push_src, push_dst, n_items, vpr, self_rank, row_base, hp, lp, xl);
   else k_halo_push_split<8><<<g, 256, 0, st>>>(xo, push_peer, push_src, push_dst, n_items, vpr, self_rank, row_base, hp, lp, xl);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int hgt_plan_source_index(const int32_t* key, const int32_t* other, const int32_t* row_ptr, int64_t n_nodes,
+                                     int64_t n_edges, int32_t n_rows, int32_t* src_ptr, int32_t* src_dst,
+                                     int32_t* src_oth, void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  HGT_REQUIRE(src_ptr && (n_edges == 0 || (key && row_ptr && src_dst)) && ((other != nullptr) == (src_oth != nullptr)),
+              "hgt_plan_source_index: NULL argument");
+  HGT_REQUIRE(n_rows >= 0, "hgt_plan_source_index: n_rows=%d", n_rows);
+  PlanScratch s;
+  size_t need = carve(s, workspace, n_rows, n_edges);
+  HGT_REQUIRE(workspace_bytes >= need, "hgt_plan_source_index: workspace too small (%zu < %zu)", workspace_bytes, need);
+  if (n_edges == 0) {
+    HGT_CHECK_CUDA(cudaMemsetAsync(src_ptr, 0, sizeof(int32_t) * ((size_t)n_rows + 1), st));
+    return 0;
+  }
+  k_iota<<<blocks_for(n_edges), kThreads, 0, st>>>(n_edges, s.vals_in);
+  HGT_LAUNCH_CHECK();
+  size_t tmp = s.cub_bytes;
+  // LSD radix sort: stable, so every row's entries keep CSR (destination) order
+  HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, key, s.keys_out, (const int32_t*)s.vals_in, src_dst,
+                                                 (int)n_edges, 0, bits_for((int64_t)n_rows + 1), st));
+  k_source_fill<<<blocks_for(n_edges), kThreads, 0, st>>>(row_ptr, n_nodes, n_edges, other, src_dst, src_oth);
+  HGT_LAUNCH_CHECK();
+  k_source_ptr<<<blocks_for((int64_t)n_rows + 1), kThreads, 0, st>>>(s.keys_out, n_edges, n_rows, src_ptr);
   HGT_LAUNCH_CHECK();
   return 0;
 }

@@ -61,6 +61,7 @@ class GraphPlan:
     tile_counts_dev: torch.Tensor = None   # sync-free plans: device {n_tiles, n_split, n_hubs}; the host fields are bounds
     flags_dev: torch.Tensor = None         # sync-free plans: range-check flags left on the device (see check())
     _layer_tables: dict = field(default_factory=dict)
+    _source_index: dict = field(default_factory=dict)   # "kv" / "rte" -> SourceIndex (deterministic backward)
 
     def check(self):
         """Sync-free plans defer the index range checks: this reads the flags back (one host sync) and raises like
@@ -293,6 +294,64 @@ def build_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relat
                      n_tiles=n_tiles, n_split=n_split, hubs=hubs[:max(n_hubs, 1)], n_hubs=n_hubs,
                      pair_type_dev=pair_type_d, pair_rel_dev=pair_rel_d,
                      tile_counts_dev=n_tiles_d if sync_free else None, flags_dev=flags_d if sync_free else None)
+
+
+# ---- source-major index of the deterministic edge backward -------------------------------------------
+
+@dataclass
+class SourceIndex:
+    """CSR positions stably sorted by the row they read in one table (kv_row: the [K'|V'] table; rte_row: the RTE table):
+    ptr [n_rows+1] over the owned rows, per entry its destination (rank order) and its row in the other table, and work
+    tiles over ptr (rows above TILE_SPLIT_EDGES entries are split).  The counts stay on the device (counts_dev); n_tiles /
+    n_split / n_hubs are the bounds the arrays were sized with."""
+    n_rows: int
+    ptr: torch.Tensor
+    dst: torch.Tensor
+    oth: torch.Tensor
+    tiles: torch.Tensor
+    n_tiles: int
+    n_split: int
+    hubs: torch.Tensor
+    n_hubs: int
+    counts_dev: torch.Tensor
+
+
+def source_index(plan, which):
+    """The source-major index of `plan` keyed by kv_row (which="kv") or rte_row (which="rte"), built on first use with
+    no host synchronisation and cached on the plan.  The trailing all-zero row (edges that match no triple) gets no
+    entry in ptr: its gradient is discarded."""
+    hit = plan._source_index.get(which)
+    if hit is not None:
+        return hit
+    if which == "kv":
+        key, other, n_rows = plan.kv_row, plan.rte_row, plan.kv_rows
+    else:
+        key, other, n_rows = plan.rte_row, plan.kv_row, plan.n_pairs * RTE_MAX_LEN
+    dev = plan.row_ptr.device
+    E = plan.n_edges
+    i32 = dict(dtype=torch.int32, device=dev)
+    st = _stream()
+    ws_bytes = ctypes.c_size_t()
+    _lib.call("hgt_plan_workspace_bytes", n_rows, E, ctypes.byref(ws_bytes))
+    ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
+    ptr = torch.empty(n_rows + 1, **i32)
+    dst = torch.empty(max(E, 1), **i32)
+    oth = torch.empty(max(E, 1), **i32) if other is not None else None
+    _lib.call("hgt_plan_source_index", key.data_ptr(), _lib.ptr(other), plan.row_ptr.data_ptr(), plan.n_nodes, E, n_rows,
+              ptr.data_ptr(), dst.data_ptr(), _lib.ptr(oth), ws.data_ptr(), ws.numel(), st)
+    max_tiles = (2 * E + n_rows) // (2 * TILE_TARGET_EDGES) + 3 * (E // TILE_SPLIT_EDGES) + 16
+    tiles = torch.empty((max_tiles, 4), **i32)
+    max_hubs = E // TILE_SPLIT_EDGES + 1
+    hubs = torch.empty((max_hubs, 4), **i32)
+    counts = torch.zeros(4, **i32)
+    _lib.call("hgt_plan_tiles", ptr.data_ptr(), n_rows, E, TILE_TARGET_EDGES, TILE_SPLIT_EDGES, tiles.data_ptr(),
+              max_tiles, hubs.data_ptr(), max_hubs, counts.data_ptr(), None, ws.data_ptr(), ws.numel(), st)
+    has_hub = E > TILE_SPLIT_EDGES
+    idx = SourceIndex(n_rows=n_rows, ptr=ptr, dst=dst, oth=oth, tiles=tiles, n_tiles=max_tiles if n_rows > 0 else 0,
+                      n_split=2 * (E // TILE_SPLIT_EDGES) + 1 if has_hub else 0, hubs=hubs,
+                      n_hubs=max_hubs if has_hub else 0, counts_dev=counts)
+    plan._source_index[which] = idx
+    return idx
 
 
 # ---- typed-linear descriptor tables (depend on the plan and on the layer's d_in / d_out) -------------
