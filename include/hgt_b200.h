@@ -457,6 +457,89 @@ int64_t hgt_sampler_add_budget(const int64_t* h_target_ids, const int64_t* h_tar
                                int32_t n_states, int64_t sampled_number, const int64_t* h_draw_off,
                                const int64_t* h_draw_pos, int64_t no_time, int64_t max_time, int64_t* h_counters);
 
+/* ------------------------------------------------------------------------------------------------
+ * HGSampling on the GPU (pyHGT/data.py:87-256; pyhgt_b200/sampler.py: sample_subgraph_cuda).  Same distribution over
+ * sampled node sets, times and order as the host sampler, drawn with Philox (seed, step) streams instead of numpy's;
+ * bitwise repeatable for a given seed.  A batch runs: rows of the seeds written by the caller, add_budget for the seeds
+ * of every seed type, then per sampling layer and type select + add_budget, then rebuild_count -> (read back) ->
+ * rebuild_write.  Node types are numbered 0..T-1 ("slots"); the node with id `i` of type t is state slot type_off[t]+i.
+ * ---------------------------------------------------------------------------------------------- */
+
+/* One <target type, source type, relation> adjacency in CSR form, rows in the reference dict's insertion order.  The
+ * struct itself lives in DEVICE memory (an array of them per call), as do the arrays it points to. */
+typedef struct {
+  const int64_t* row_of; int64_t n_row_of;   /* target id -> CSR row, -1 = no adjacency */
+  const int64_t* ptr;                         /* [rows+1] positions into nbr / time */
+  const int64_t* nbr; const int64_t* time;    /* neighbour ids and edge times in dict order (no_time = None) */
+  int32_t tgt_type, src_type;                 /* type slots */
+  int32_t skip;                               /* 1 for the 'self' relation: never sampled from (data.py:116) */
+  int32_t rel;                                /* edge_type value in the to_torch layout (data.py:237-238) */
+} hgt_gsample_block;
+
+/* Sampler state of one batch: the struct is passed by HOST pointer, its fields are DEVICE arrays.
+ * Initial values: ser -1, n_layer 0, score 0, bstamp -1, last_seq -1, first_seq / type_min INT64_MAX, type_seq -1
+ * (except the seed types' layer numbers), counters {number of seed types, 0}. */
+typedef struct {
+  int32_t num_types; int32_t pad;
+  const int64_t* type_off;   /* [T+1] first state slot of each type (id range of type t: type_off[t+1]-type_off[t]) */
+  const int64_t* lid_off;    /* [T+1] first entry of each type in lid (capacity of type t: lid_off[t+1]-lid_off[t]) */
+  int32_t* ser;              /* [slots] position of the node in layer_data[type] (data.py:133-141,166), -1 = not sampled */
+  int64_t* ltime;            /* [slots] its time in layer_data */
+  int64_t* lid;              /* sampled ids of every type in ser order */
+  int64_t* n_layer;          /* [T] nodes sampled per type */
+  unsigned long long* score; /* [slots] budget score, fixed point with 40 fraction bits */
+  int64_t* btime;            /* [slots] budget time (last writer, data.py:130) */
+  int64_t* bstamp;           /* [slots] budget insertion stamp, -1 = not in the budget */
+  int64_t* last_seq;         /* [slots] scratch */
+  int64_t* first_seq;        /* [slots] scratch */
+  int64_t* type_min;         /* [2T] scratch */
+  int64_t* type_seq;         /* [2T] first-touch number of layer_data[t] (2t) and budget[t] (2t+1), -1 = untouched */
+  int64_t* counters;         /* [2] next first-touch numbers */
+} hgt_gsample_state;
+
+/* add_budget (data.py:108-130) for the targets tgt_id / tgt_time [max_targets] of one type, whose blocks (non-'self'
+ * ones are sampled) are blocks[0..n_blocks) in dict order.  n_targets: device count (<= max_targets), or NULL =
+ * max_targets.  time_filter = 0 disables the max_time test (ogbn-mag variant: time_range=None).  `step`: a number unique
+ * to this call within the batch (< 2^22), selects the random stream and orders the insertion stamps.
+ * flags[0] is set when a neighbour id lies outside its type's id range. */
+int hgt_gsample_add_budget_workspace_bytes(int64_t max_targets, int32_t n_blocks, int64_t sampled_number,
+                                           size_t* out_bytes);
+int hgt_gsample_add_budget(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks,
+                           const int64_t* tgt_id, const int64_t* tgt_time, int64_t max_targets, const int64_t* n_targets,
+                           int64_t sampled_number, int32_t time_filter, int64_t max_time, int64_t no_time, uint64_t seed,
+                           int64_t step, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Selection of one (layer, type) (data.py:150-170): every budget entry in insertion order when the budget holds fewer
+ * than sampled_number entries, else sampled_number entries without replacement with p ~ score^2 (ordered); they join
+ * the layer, leave the budget, and are written to tgt_id / tgt_time [sampled_number] with their count in *n_targets
+ * (device), ready for hgt_gsample_add_budget.  n_ids: the type's id range.  flags[0]: layer capacity exceeded. */
+int hgt_gsample_select_workspace_bytes(int64_t n_ids, size_t* out_bytes);
+int hgt_gsample_select(const hgt_gsample_state* h_state, int32_t type, int64_t n_ids, int64_t sampled_number,
+                       uint64_t seed, int64_t step, int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets,
+                       int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Rebuild of the sampled adjacency (data.py:190-209), pass 1: for every block b (all relations, 'self' included) and
+ * every sampled target r of its type, the number of neighbours in the sample, at cnt_off[b] + r (cnt_off [n_blocks+1]:
+ * room for lid capacity of the target type; n_count = cnt_off[n_blocks]).  ex [n_count+1]: exclusive prefix of those
+ * counts; totals [n_blocks]: edges per block.  max_rows >= every type's lid capacity.  flags[1]: an edge_time outside
+ * [0, 240) (data.py:250, RelTemporalEncoding size); flags[2]: a sampled id >= feat_rows[type] (feat_rows [T] or NULL). */
+int hgt_gsample_rebuild_workspace_bytes(int64_t n_count, size_t* out_bytes);
+int hgt_gsample_rebuild_count(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks,
+                              const int64_t* cnt_off, int64_t n_count, int64_t max_rows, const int64_t* feat_rows,
+                              int64_t* ex, int64_t* totals, int32_t* flags, void* workspace, size_t workspace_bytes,
+                              void* stream);
+/* Pass 2: the to_torch layout (data.py:226-256).  node_off [T]: first output row of each type (-1 = not laid out),
+ * type_out [T]: its node_type value; self_off [T]: first edge of its self loops (-1 = none), blk_out [n_blocks]: first
+ * edge of each block's edges (-1 = none).  edge_index [2, n_edges] (row 0 = source), edge_type / edge_time [n_edges],
+ * node_type / node_time [rows]; node_feature [rows, feat_dim] gathered from feat[t] (a DEVICE array of T device
+ * pointers to [ids, feat_dim] float tables) or NULL. */
+int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks,
+                              const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
+                              const int64_t* type_out, const int64_t* self_off, int64_t self_rel, int64_t max_rows,
+                              int64_t n_edges, const float* const* feat, int32_t feat_dim, int64_t* node_type,
+                              int64_t* node_time, float* node_feature, int64_t* edge_index, int64_t* edge_type,
+                              int64_t* edge_time, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -66,6 +66,16 @@ SIGNATURES = {
     "hgt_update_backward_det": [_p, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_fold_backward_det": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p,
                               _p, _p, _p, _p, _p, _p],
+    # HGSampling on the GPU (sampler.sample_subgraph_cuda)
+    "hgt_gsample_add_budget_workspace_bytes": [_i64, _i32, _i64, _c.POINTER(_sz)],
+    "hgt_gsample_add_budget": [_p, _p, _i32, _p, _p, _i64, _p, _i64, _i32, _i64, _i64, _c.c_uint64, _i64, _p, _p, _sz,
+                               _p],
+    "hgt_gsample_select_workspace_bytes": [_i64, _c.POINTER(_sz)],
+    "hgt_gsample_select": [_p, _i32, _i64, _i64, _c.c_uint64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_rebuild_workspace_bytes": [_i64, _c.POINTER(_sz)],
+    "hgt_gsample_rebuild_count": [_p, _p, _i32, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _p, _i32, _p, _p, _p, _p, _p,
+                                  _p, _p],
 }
 
 class ConvArgs(ctypes.Structure):

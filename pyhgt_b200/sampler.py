@@ -453,6 +453,312 @@ def _sample_slices(fg, time_range, sampled_depth, sampled_number, inp, feature_e
     return _finish(fg, states, layer_order, feature_extractor)
 
 
+class _GBlock(_c.Structure):                 # hgt_gsample_block (include/hgt_b200.h)
+    _fields_ = [("row_of", _c.c_void_p), ("n_row_of", _c.c_int64), ("ptr", _c.c_void_p), ("nbr", _c.c_void_p),
+                ("time", _c.c_void_p), ("tgt_type", _c.c_int32), ("src_type", _c.c_int32), ("skip", _c.c_int32),
+                ("rel", _c.c_int32)]
+
+
+class _GState(_c.Structure):                 # hgt_gsample_state
+    _PTRS = ("type_off", "lid_off", "ser", "ltime", "lid", "n_layer", "score", "btime", "bstamp", "last_seq",
+             "first_seq", "type_min", "type_seq", "counters")
+    _fields_ = [("num_types", _c.c_int32), ("pad", _c.c_int32)] + [(n, _c.c_void_p) for n in _PTRS]
+
+
+_I64_MAX = np.iinfo(np.int64).max
+
+
+class DeviceGraph:
+    """A ``FrozenGraph`` uploaded once to a CUDA device for ``sample_subgraph_cuda``: the CSR blocks (neighbour ids and
+    edge times in dict order, id -> row maps) and, optionally, per-type feature tables ``{type: Tensor[n_ids, F]}``
+    (row = node id) that the sampled batch's ``node_feature`` is gathered from.
+
+    Node types are laid out in ``graph.get_types()`` order (as ``to_torch`` does), so every type of the graph's
+    ``edge_list`` must be one of them; relation names come from ``graph.get_meta_graph()`` plus ``'self'``."""
+
+    def __init__(self, frozen_graph, device, features=None):
+        import torch
+        fg = frozen_graph if isinstance(frozen_graph, FrozenGraph) else FrozenGraph(frozen_graph)
+        self.fg, self.device = fg, torch.device(device)
+        if self.device.type != "cuda":
+            raise ValueError("DeviceGraph needs a CUDA device, got %s" % self.device)
+        graph = fg.graph
+        self.types = list(graph.get_types())
+        self.slot = {t: i for i, t in enumerate(self.types)}
+        missing = [t for t in fg.types if t not in self.slot]
+        if missing:
+            raise KeyError("node types %r occur in edge_list but not in graph.get_types()" % (missing,))
+        self.edge_dict = {e[2]: i for i, e in enumerate(graph.get_meta_graph())}     # data.py:237-238
+        self.edge_dict['self'] = len(self.edge_dict)
+        self.n_ids = [fg.n_ids.get(t, 0) for t in self.types]
+        dev = self.device
+
+        def up(a):
+            return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(dev)
+
+        self._keep = []
+        self.blocks = []                                  # (target slot, source slot, relation, skip) in dict order
+        cblocks = []
+        for t_t, tes in fg.blocks.items():
+            for s_t, rels in tes.items():
+                for r, blk in rels.items():
+                    if r not in self.edge_dict:
+                        raise KeyError("relation %r of edge_list is not in graph.get_meta_graph()" % (r,))
+                    arrs = [up(blk.row_of), up(blk.ptr), up(blk.nbr), up(blk.time)]
+                    self._keep += arrs
+                    cb = _GBlock(arrs[0].data_ptr(), blk.row_of.shape[0], arrs[1].data_ptr(), arrs[2].data_ptr(),
+                                 arrs[3].data_ptr(), self.slot[t_t], self.slot[s_t], 1 if r == 'self' else 0,
+                                 self.edge_dict[r])
+                    self.blocks.append((self.slot[t_t], self.slot[s_t], r))
+                    cblocks.append(cb)
+        self.n_blocks = len(cblocks)
+        self.blocks_dev = self._struct_array(cblocks)
+        # per target type: its blocks, in dict order (the add_budget of that type walks them)
+        self.type_blocks = {}
+        for ti in range(len(self.types)):
+            own = [cb for cb, (tt, _, _) in zip(cblocks, self.blocks) if tt == ti]
+            if own:
+                self.type_blocks[ti] = (self._struct_array(own), len(own))
+        self.features, self.feat_dim = None, 0
+        if features is not None:
+            dims = {int(v.shape[1]) for v in features.values()}
+            if len(dims) != 1:
+                raise ValueError("feature tables must all have the same width, got %s" % sorted(dims))
+            self.feat_dim = dims.pop()
+            tabs, ptrs, rows = {}, [], []
+            for t in self.types:
+                v = features.get(t)
+                if v is not None:
+                    v = v.to(device=dev, dtype=torch.float32).contiguous()
+                    tabs[t] = v
+                ptrs.append(0 if v is None else v.data_ptr())
+                rows.append(0 if v is None else v.shape[0])
+            self.features = tabs
+            self.feat_ptrs = torch.tensor(np.asarray(ptrs, dtype=np.uint64).view(np.int64), device=dev)
+            self.feat_rows = up(rows)
+
+    def _struct_array(self, structs):
+        import torch
+        raw = b"".join(bytes(s) for s in structs) or b"\0"
+        return torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.device)
+
+
+def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None):
+    """HGSampling (pyHGT/data.py:87-210) and ``to_torch`` (data.py:212-256) on the GPU.
+
+    Same distribution over sampled node sets, their times and their order as ``sample_subgraph`` (the host sampler,
+    which replays numpy's stream), drawn from a Philox stream seeded by one draw of ``generator`` (a ``torch.Generator``;
+    None = torch's default CPU generator): the same generator state gives bitwise-identical outputs.
+    ``time_range=None`` turns the time filter off (ogbn-mag variant).  Seed ids of a type must be distinct.
+
+    Returns ``(node_feature, node_type, edge_time, edge_index, edge_type, node_dict, edge_dict, indxs, node_time)``: the
+    first seven as ``to_torch(..., device=dgraph.device, prebuild_plan=True)`` would return them (node_feature gathered
+    from the DeviceGraph's feature tables, None without them), and per sampled type (in ``layer_data`` key order) the
+    sampled ids (``indxs``) and times in ``ser`` order, as device tensors.  The sync-free plan of the graph is built.
+    Host synchronisation: one small read-back per sampling layer (the type order) and one at the end."""
+    import torch
+    from . import _lib
+    from . import plan as _plan
+    dg = dgraph
+    dev = dg.device
+    W = int(sampled_number)
+    depth = int(sampled_depth)
+    if W <= 0 or depth < 0:
+        raise ValueError("sampled_number must be positive and sampled_depth non-negative")
+    T = len(dg.types)
+
+    seeds = []                                            # (slot, ids, times) in inp order
+    for _type in inp:
+        if _type not in dg.slot:
+            raise KeyError("seed type %r is not in graph.get_types()" % (_type,))
+        arr = np.asarray(inp[_type], dtype=np.int64).reshape(-1, 2)
+        if arr.shape[0] == 0:
+            continue
+        ids = np.ascontiguousarray(arr[:, 0])
+        if ids.min() < 0:
+            raise ValueError("seed ids of type %r must be non-negative" % (_type,))
+        if np.unique(ids).shape[0] != ids.shape[0]:
+            raise ValueError("duplicate seed ids of type %r" % (_type,))
+        seeds.append((dg.slot[_type], ids, np.ascontiguousarray(arr[:, 1])))
+    n_ids = list(dg.n_ids)
+    n_seed = [0] * T
+    for s, ids, _ in seeds:
+        n_ids[s] = max(n_ids[s], int(ids.max()) + 1)      # seeds beyond the graph become isolated nodes
+        n_seed[s] = ids.shape[0]
+    cap = [min(n_ids[t], n_seed[t] + depth * W) for t in range(T)]
+    type_off = np.concatenate([[0], np.cumsum(n_ids)]).astype(np.int64)
+    lid_off = np.concatenate([[0], np.cumsum(cap)]).astype(np.int64)
+    n_slots, n_lid = int(type_off[-1]), int(lid_off[-1])
+
+    i64 = dict(dtype=torch.int64, device=dev)
+    small = np.concatenate([type_off, lid_off])
+    small_d = _plan._to_dev_async(small, dev)
+    ser = torch.full((max(n_slots, 1),), -1, dtype=torch.int32, device=dev)
+    ltime = torch.zeros(max(n_slots, 1), **i64)
+    lid = torch.zeros(max(n_lid, 1), **i64)
+    score = torch.zeros(max(n_slots, 1), **i64)
+    btime = torch.zeros(max(n_slots, 1), **i64)
+    bstamp = torch.full((max(n_slots, 1),), -1, **i64)
+    last_seq = torch.full((max(n_slots, 1),), -1, **i64)
+    first_seq = torch.full((max(n_slots, 1),), _I64_MAX, **i64)
+    # one small buffer the host reads: [n_layer T | type_seq 2T | block totals | flags]
+    NB = dg.n_blocks
+    meta = torch.zeros(T + 2 * T + NB + 2, **i64)
+    n_layer, type_seq, totals = meta[:T], meta[T:3 * T], meta[3 * T:3 * T + NB]
+    flags = meta[3 * T + NB:].view(torch.int32)           # 4 int32 flags
+    type_min = torch.full((max(2 * T, 1),), _I64_MAX, **i64)
+    counters = torch.zeros(2, **i64)
+
+    # seeds enter layer_data first, in inp order (data.py:135-137)
+    seq0 = np.full(2 * T, -1, dtype=np.int64)
+    for k, (s, _, _) in enumerate(seeds):
+        seq0[2 * s] = k
+    if seeds:
+        slots = np.concatenate([type_off[s] + ids for s, ids, _ in seeds])
+        sers = np.concatenate([np.arange(ids.shape[0]) for _, ids, _ in seeds])
+        tms = np.concatenate([tm for _, _, tm in seeds])
+        lpos = np.concatenate([lid_off[s] + np.arange(ids.shape[0]) for s, ids, _ in seeds])
+        lids = np.concatenate([ids for _, ids, _ in seeds])
+        nl = np.zeros(T, dtype=np.int64)
+        for s, ids, _ in seeds:
+            nl[s] = ids.shape[0]
+        up = _plan._to_dev_async(np.concatenate([slots, sers, tms, lpos, lids, nl, seq0, [len(seeds), 0]]), dev)
+        n = slots.shape[0]
+        sl_d, ser_d, tm_d, lp_d, li_d = (up[i * n:(i + 1) * n] for i in range(5))
+        ser.index_put_((sl_d,), ser_d.to(torch.int32))
+        ltime.index_put_((sl_d,), tm_d)
+        lid.index_put_((lp_d,), li_d)
+        n_layer.copy_(up[5 * n:5 * n + T])
+        type_seq.copy_(up[5 * n + T:5 * n + 3 * T])
+        counters.copy_(up[5 * n + 3 * T:])
+    else:
+        type_seq.fill_(-1)
+
+    cst = _GState(T, 0, small_d.data_ptr(), small_d.data_ptr() + 8 * (T + 1), ser.data_ptr(), ltime.data_ptr(),
+                  lid.data_ptr(), n_layer.data_ptr(), score.data_ptr(), btime.data_ptr(), bstamp.data_ptr(),
+                  last_seq.data_ptr(), first_seq.data_ptr(), type_min.data_ptr(), type_seq.data_ptr(),
+                  counters.data_ptr())
+    st = torch.cuda.current_stream(dev).cuda_stream
+    if generator is None:
+        seed = int(torch.randint(0, 2 ** 63 - 1, (1,)))
+    else:
+        seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=generator, device=generator.device))
+    time_filter = time_range is not None
+    max_time = int(np.max(list(time_range.keys()))) if time_filter else 0
+
+    max_nb = max((nb for _, nb in dg.type_blocks.values()), default=0)
+    max_tg = max([W] + n_seed)
+    bud_ws, sel_ws = _c.c_size_t(), _c.c_size_t()
+    _lib.call("hgt_gsample_add_budget_workspace_bytes", max_tg, max_nb, W, _c.byref(bud_ws))
+    _lib.call("hgt_gsample_select_workspace_bytes", max(n_ids, default=0), _c.byref(sel_ws))
+    ws = torch.empty(max(bud_ws.value, sel_ws.value, 1), dtype=torch.uint8, device=dev)
+    tgt = torch.zeros(2 * W + 1, **i64)                   # [ids W | times W | count]
+    tgt_id, tgt_time, n_tgt = tgt[:W], tgt[W:2 * W], tgt[2 * W:]
+    step = [0]
+
+    def add_budget(s, ids_d, tms_d, max_targets, count_d):
+        ent = dg.type_blocks.get(s)
+        if ent is not None and max_targets > 0:
+            _lib.call("hgt_gsample_add_budget", _c.byref(cst), ent[0].data_ptr(), ent[1], ids_d.data_ptr(),
+                      tms_d.data_ptr(), max_targets, _lib.ptr(count_d), W, int(time_filter), max_time, _NO_TIME, seed,
+                      step[0], flags.data_ptr(), ws.data_ptr(), ws.numel(), st)
+        step[0] += 1
+
+    if seeds:                                             # then their budgets (data.py:139-141)
+        n = slots.shape[0]
+        o = 0
+        for s, ids, _ in seeds:
+            m = ids.shape[0]
+            add_budget(s, li_d[o:o + m], tm_d[o:o + m], m, None)
+            o += m
+    for _layer in range(depth):                           # data.py:146-170
+        ts = type_seq.cpu().numpy()                       # the per-layer read-back: list(budget.keys())
+        order = sorted((t for t in range(T) if ts[2 * t + 1] >= 0), key=lambda t: ts[2 * t + 1])
+        for s in order:
+            _lib.call("hgt_gsample_select", _c.byref(cst), s, n_ids[s], W, seed, step[0], tgt_id.data_ptr(),
+                      tgt_time.data_ptr(), n_tgt.data_ptr(), flags.data_ptr(), ws.data_ptr(), ws.numel(), st)
+            add_budget(s, tgt_id, tgt_time, W, n_tgt)
+
+    # rebuild (data.py:181-209): count pass, then the one read-back of the batch
+    cnt_off = np.concatenate([[0], np.cumsum([cap[tt] for tt, _, _ in dg.blocks])]).astype(np.int64)
+    n_count = int(cnt_off[-1])
+    max_rows = max(cap, default=0)
+    rb_ws = _c.c_size_t()
+    _lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
+    rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
+    ex = torch.empty(n_count + 1, **i64)
+    cnt_off_d = _plan._to_dev_async(cnt_off, dev)
+    _lib.call("hgt_gsample_rebuild_count", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(), n_count,
+              max_rows, _lib.ptr(dg.feat_rows) if dg.features is not None else None, ex.data_ptr(),
+              totals.data_ptr(), flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
+    h = meta.cpu().numpy()
+    nl = h[:T]
+    ts = h[T:3 * T]
+    tot = h[3 * T:3 * T + NB]
+    fl = h[3 * T + NB:].view(np.int32)
+    if fl[0]:
+        raise IndexError("a neighbour id lies outside its node type's id range in the device graph")
+    if fl[1]:
+        raise IndexError("edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
+    if dg.features is not None:
+        lacking = [dg.types[t] for t in range(T) if nl[t] and dg.types[t] not in dg.features]
+        if lacking:
+            raise KeyError("no feature table for sampled node types %r" % (lacking,))
+    if fl[2]:
+        raise IndexError("a sampled node id lies outside its type's feature table")
+
+    # the to_torch layout (data.py:226-256): nodes type by type; edges in the order of _finish's edge_list
+    node_off = np.concatenate([[0], np.cumsum(nl)]).astype(np.int64)
+    N = int(node_off[-1])
+    layer_order = sorted((t for t in range(T) if ts[2 * t] >= 0), key=lambda t: ts[2 * t])
+    self_rel = dg.edge_dict['self']
+    self_off = np.full(T, -1, dtype=np.int64)
+    blk_out = np.full(max(NB, 1), -1, dtype=np.int64)
+    pairs = set()
+    E = 0
+    for tt in layer_order:
+        if nl[tt] == 0:
+            continue
+        self_off[tt] = E                                  # 'self' loops first (data.py:181-184)
+        E += int(nl[tt])
+        pairs.add((tt, self_rel))
+        own = [b for b, (t_, _, _) in enumerate(dg.blocks) if t_ == tt]
+        # edge_list[tt] already holds source tt with relation 'self' first: the (tt, tt) blocks follow it, 'self' first
+        same = [b for b in own if dg.blocks[b][1] == tt]
+        grouped = [b for b in same if dg.blocks[b][2] == 'self'] + [b for b in same if dg.blocks[b][2] != 'self']
+        grouped += [b for b in own if dg.blocks[b][1] != tt]
+        for b in grouped:
+            if tot[b]:
+                blk_out[b] = E
+                E += int(tot[b])
+                pairs.add((dg.blocks[b][1], dg.edge_dict[dg.blocks[b][2]]))
+    tabs = _plan._to_dev_async(np.concatenate([blk_out, node_off[:T], np.arange(T, dtype=np.int64), self_off]), dev)
+    nb1 = blk_out.shape[0]
+    blk_out_d, node_off_d = tabs[:nb1], tabs[nb1:nb1 + T]
+    type_out_d, self_off_d = tabs[nb1 + T:nb1 + 2 * T], tabs[nb1 + 2 * T:]
+    node_type = torch.empty(N, **i64)
+    node_time = torch.empty(N, **i64)
+    node_feature = torch.empty((N, dg.feat_dim), dtype=torch.float32, device=dev) if dg.features is not None else None
+    edge_index = torch.empty((2, E), **i64)
+    edge_type = torch.empty(E, **i64)
+    edge_time = torch.empty(E, **i64)
+    _lib.call("hgt_gsample_rebuild_write", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(),
+              ex.data_ptr(), blk_out_d.data_ptr(), node_off_d.data_ptr(), type_out_d.data_ptr(), self_off_d.data_ptr(),
+              self_rel, max_rows, E, _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim,
+              node_type.data_ptr(), node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(),
+              edge_type.data_ptr(), edge_time.data_ptr(), st)
+    meta_plan = {"type_count": [int(v) for v in nl] + [0], "sorted": True, "pairs": sorted(pairs)}
+    _plan.get_plan(node_type, edge_index, edge_type, edge_time, T, len(dg.edge_dict), host_meta=meta_plan)
+
+    node_dict = {t: [int(node_off[i]), i] for i, t in enumerate(dg.types)}
+    indxs, times = {}, {}
+    for t in layer_order:
+        if nl[t]:
+            indxs[dg.types[t]] = lid[int(lid_off[t]):int(lid_off[t] + nl[t])]
+            times[dg.types[t]] = node_time[int(node_off[t]):int(node_off[t + 1])]
+    return (node_feature, node_type, edge_time, edge_index, edge_type, node_dict, dict(dg.edge_dict), indxs, times)
+
+
 def _finish(fg, states, layer_order, feature_extractor):
     """layer_data -> features (data.py:174) and the sampled adjacency (data.py:181-209)."""
     ref_graph = fg.graph

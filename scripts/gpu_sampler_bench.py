@@ -1,0 +1,181 @@
+"""Host HGSampling vs device HGSampling per batch, next to the training step they feed.
+
+Workload: a seeded synthetic heterograph with the MAG schema (paper / author / field / venue, every relation with its
+rev_* twin, 'self' loops on every type; about 1 M edges), frozen once (sampler.FrozenGraph) and uploaded once
+(sampler.DeviceGraph).  Each setting samples from 128 paper seeds; the recipe setting is depth 6, width 520
+(pyHGT ogbn-mag/train_ogbn_mag.py:44-47), the small one depth 3, width 64.
+
+Prints one JSON line per setting:
+  host_ms        sample_subgraph (batched native path, one process) + to_torch onto the device with the sync-free plan,
+                 wall clock, median over --host-batches;
+  device_ms      sample_subgraph_cuda (same outputs, features gathered on the device), CUDA events after warm-up,
+                 median over --batches (>= 20);
+  train_ms       fwd + bwd of a 4-layer n_hid=512 GNN (HGT) on one device batch, CUDA events, median;
+  plus the batch sizes, the card name and its power limit.
+
+    python scripts/gpu_sampler_bench.py [--scale 1.0] [--batches 20] [--host-batches 3]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+from collections import defaultdict
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+F_IN = 128
+
+
+class _Graph:
+    def __init__(self, edge_list, types, meta):
+        self.edge_list, self._t, self._m = edge_list, types, meta
+
+    def get_types(self):
+        return self._t
+
+    def get_meta_graph(self):
+        return self._m
+
+
+def make_graph(scale, seed=0):
+    """MAG-schema graph: papers cite papers, are written by authors, have fields and a venue (years 1990-2020)."""
+    rng = np.random.RandomState(seed)
+    n = {"paper": int(100000 * scale), "author": int(60000 * scale), "field": int(8000 * scale), "venue": 500}
+    year = rng.randint(1990, 2021, n["paper"])
+    el = defaultdict(lambda: defaultdict(lambda: defaultdict(dict)))
+    meta = []
+
+    def add(tt, st, rel, tgt, src, tm):
+        fwd, rev = el[tt][st][rel], el[st][tt]["rev_" + rel]
+        for a, b, t in zip(tgt.tolist(), src.tolist(), tm.tolist()):
+            fwd.setdefault(a, {})[b] = t
+            rev.setdefault(b, {})[a] = t
+        meta.extend([(tt, st, rel), (st, tt, "rev_" + rel)])
+
+    P = n["paper"]
+    # heavy-tailed citation / authorship degrees so that hubs (degree >> width) occur
+    cited = (rng.pareto(1.2, 4 * P) * 50).astype(np.int64) % P
+    citing = rng.randint(0, P, 4 * P)
+    add("paper", "paper", "PP_cite", citing, cited, year[citing])
+    pa = rng.randint(0, P, 3 * P)
+    au = (rng.pareto(1.5, 3 * P) * 30).astype(np.int64) % n["author"]
+    add("paper", "author", "AP_write", pa, au, year[pa])
+    pf = rng.randint(0, P, 3 * P)
+    fi = (rng.pareto(1.0, 3 * P) * 20).astype(np.int64) % n["field"]
+    add("paper", "field", "PF_in_L2", pf, fi, year[pf])
+    add("paper", "venue", "PV_Journal", np.arange(P), rng.randint(0, n["venue"], P), year)
+    for t in n:                                            # 'self' relation of every type (not sampled from)
+        ids = np.arange(n[t])
+        rel = el[t][t]["self"]
+        for i in ids.tolist():
+            rel[i] = {i: None}
+        meta.append((t, t, "self"))
+    seen, meta_u = set(), []
+    for m in meta:
+        if m[2] != "self" and m not in seen:
+            seen.add(m)
+            meta_u.append(m)
+    n_edges = sum(len(v) for a in el.values() for b in a.values() for c in b.values() for v in c.values())
+    return _Graph(el, list(n), meta_u), n, year, n_edges
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, timeout=30).stdout.strip().splitlines()[0]
+        return [s.strip() for s in q.split(",")]
+    except Exception:                                      # noqa: BLE001
+        return [torch.cuda.get_device_name(0), "not measured"]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--scale", type=float, default=1.0)
+    ap.add_argument("--batches", type=int, default=20)
+    ap.add_argument("--host-batches", type=int, default=3)
+    ap.add_argument("--settings", default="6x520,3x64")
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    from pyhgt_b200 import data as hdata, sampler
+    from pyhgt_b200.model import GNN
+    import pyhgt_b200
+    dev = torch.device("cuda:0")
+    t0 = time.time()
+    g, n, year, n_edges = make_graph(args.scale)
+    fg = sampler.FrozenGraph(g)
+    rng = np.random.RandomState(1)
+    tables = {t: torch.from_numpy(rng.randn(max(fg.n_ids.get(t, 1), 1), F_IN).astype(np.float32)) for t in n}
+    dg = sampler.DeviceGraph(fg, dev, tables)
+    build_s = time.time() - t0
+    time_range = {y: True for y in range(1990, 2016)}
+    tables_np = {t: v.numpy() for t, v in tables.items()}
+
+    def extractor(layer_data, graph):
+        feature, times, indxs = {}, {}, {}
+        for t in graph.get_types():
+            ids = np.fromiter(layer_data[t].keys(), dtype=np.int64) if t in layer_data else np.zeros(0, np.int64)
+            feature[t] = tables_np[t][ids]
+            times[t] = np.array([layer_data[t][i][1] for i in ids.tolist()], dtype=np.int64)
+            indxs[t] = ids
+        return feature, times, indxs, []
+
+    def seeds(i):
+        r = np.random.RandomState(100 + i)
+        p = r.choice(np.nonzero(year <= 2015)[0], 128, replace=False)
+        return {"paper": np.stack([p, year[p]], 1)}
+
+    edge_dict = {e[2]: i for i, e in enumerate(g.get_meta_graph())}
+    edge_dict["self"] = len(edge_dict)
+    torch.manual_seed(0)
+    gnn = GNN(F_IN, 512, len(n), len(edge_dict), 8, 4, 0.2, "hgt", True, False, True).to(dev).train()
+    pyhgt_b200.HGTConv.keep_att = False
+    name, power = card()
+    for setting in args.settings.split(","):
+        depth, width = (int(v) for v in setting.split("x"))
+        host = []
+        for i in range(args.host_batches):
+            np.random.seed(i)
+            torch.cuda.synchronize()
+            a = time.perf_counter()
+            feature, times, edge_list, _, _ = sampler.sample_subgraph(fg, time_range, depth, width, seeds(i), extractor)
+            hdata.to_torch(feature, times, edge_list, g, device=dev, prebuild_plan=True)
+            torch.cuda.synchronize()
+            host.append((time.perf_counter() - a) * 1e3)
+        gen = torch.Generator().manual_seed(0)
+        for i in range(3):
+            out = sampler.sample_subgraph_cuda(dg, time_range, depth, width, seeds(i), gen)
+        devt = []
+        for i in range(args.batches):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            out = sampler.sample_subgraph_cuda(dg, time_range, depth, width, seeds(i), gen)
+            e1.record()
+            torch.cuda.synchronize()
+            devt.append(e0.elapsed_time(e1))
+        nf, nt, etime, ei, et = out[:5]
+        train = []
+        for i in range(8):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            y = gnn(nf, nt, etime, ei, et)
+            y.square().mean().backward()
+            e1.record()
+            torch.cuda.synchronize()
+            if i >= 3:
+                train.append(e0.elapsed_time(e1))
+        print(json.dumps({"setting": {"depth": depth, "width": width, "seeds": 128},
+                          "graph": {"nodes": n, "edges": n_edges, "build_s": round(build_s, 1)},
+                          "batch": {"nodes": int(nt.numel()), "edges": int(ei.shape[1])},
+                          "host_ms": round(float(np.median(host)), 2), "host_batches": len(host),
+                          "device_ms": round(float(np.median(devt)), 3), "device_batches": len(devt),
+                          "train_fwd_bwd_ms": round(float(np.median(train)), 3),
+                          "gpu": name, "power_limit": power}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
