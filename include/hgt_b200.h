@@ -540,6 +540,92 @@ int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const hgt_gsampl
                               int64_t* node_time, float* node_feature, int64_t* edge_index, int64_t* edge_type,
                               int64_t* edge_time, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * B subgraphs ("members") in one pass (pyhgt_b200/sampler.py: sample_subgraphs_cuda).  The members share the graph,
+ * the time filter, the depth and the width; each has its own seeds, Philox seed, step numbers and rows of the state, and
+ * member b's result is bitwise the single-subgraph run with its seed and steps (the entry points above are B = 1).
+ * Memory: about 52 bytes per state slot, i.e. B x 52 B x (sum of the id ranges) for the dense arrays.
+ * ---------------------------------------------------------------------------------------------- */
+
+/* Like hgt_gsample_state with a member dimension: type_off / lid_off hold [B*(T+1)] ABSOLUTE positions (member b's type
+ * t: slots type_off[b*(T+1)+t] .. [b*(T+1)+t+1], lid entries likewise); the dense arrays hold every member's slots;
+ * n_layer [B*T], type_min / type_seq [B*2T], counters [B*2]; seed [B] is each member's Philox seed.  Initial values as
+ * for hgt_gsample_state, per member. */
+typedef struct {
+  int32_t num_types; int32_t n_members;
+  const int64_t* type_off;
+  const int64_t* lid_off;
+  int32_t* ser;
+  int64_t* ltime;
+  int64_t* lid;
+  int64_t* n_layer;
+  unsigned long long* score;
+  int64_t* btime;
+  int64_t* bstamp;
+  int64_t* last_seq;
+  int64_t* first_seq;
+  int64_t* type_min;
+  int64_t* type_seq;
+  int64_t* counters;
+  const uint64_t* seed;
+} hgt_gsample_batch_state;
+
+/* add_budget for every member at once: member b's targets are tgt_id / tgt_time [b*max_targets ...] (n_targets[b] of
+ * them, device) of node type type[b] (device [B]; -1 = the member sits this step out), whose blocks are
+ * blocks[type_blocks[2t] .. type_blocks[2t+1]) (device [2T]; max_blocks >= every such count); step [B] (device) is the
+ * member's step number.  Otherwise as hgt_gsample_add_budget. */
+int hgt_gsample_batch_add_budget_workspace_bytes(int32_t n_members, int64_t max_targets, int32_t max_blocks,
+                                                 int64_t sampled_number, size_t* out_bytes);
+int hgt_gsample_batch_add_budget(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
+                                 const int32_t* type_blocks, int32_t max_blocks, const int32_t* type, const int64_t* step,
+                                 const int64_t* tgt_id, const int64_t* tgt_time, int64_t max_targets,
+                                 const int64_t* n_targets, int64_t sampled_number, int32_t time_filter, int64_t max_time,
+                                 int64_t no_time, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Selection for every member at once: member b selects from type[b] (-1 = none: n_targets[b] = 0) with step[b]; its ids
+ * are sorted at positions sel_off[b] .. sel_off[b+1] (device [B+1], = the type's id range; n_total = sel_off[B],
+ * max_ids >= every range).  Member b's targets go to tgt_id / tgt_time [b*sampled_number ...], their count to
+ * n_targets[b].  Otherwise as hgt_gsample_select. */
+int hgt_gsample_batch_select_workspace_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes);
+int hgt_gsample_batch_select(const hgt_gsample_batch_state* h_state, const int32_t* type, const int64_t* step,
+                             const int64_t* sel_off, int64_t n_total, int64_t max_ids, int64_t sampled_number,
+                             int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets, int32_t* flags, void* workspace,
+                             size_t workspace_bytes, void* stream);
+
+/* Rebuild of every member at once (workspace: hgt_gsample_rebuild_workspace_bytes(n_count)).  cnt_off [B*n_blocks+1]:
+ * member b, block k counts at cnt_off[b*n_blocks+k]; totals [B*n_blocks]. */
+int hgt_gsample_batch_rebuild_count(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
+                                    int32_t n_blocks, const int64_t* cnt_off, int64_t n_count, int64_t max_rows,
+                                    const int64_t* feat_rows, int64_t* ex, int64_t* totals, int32_t* flags,
+                                    void* workspace, size_t workspace_bytes, void* stream);
+/* blk_out [B*n_blocks], node_off / self_off [B*T]: member-local as in hgt_gsample_rebuild_write; mem_out [B*3] (device):
+ * member b's {first node row, first edge, edge count} in the shared outputs.  Member b's edge_index is the [2, E_b]
+ * block at edge_index + 2 * first edge, with member-local node ids: each member is exactly a to_torch layout. */
+int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
+                                    int32_t n_blocks, const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out,
+                                    const int64_t* node_off, const int64_t* type_out, const int64_t* self_off,
+                                    int64_t self_rel, const int64_t* mem_out, int64_t max_rows, const float* const* feat,
+                                    int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature,
+                                    int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream);
+
+/* Disjoint union of B batches in the to_torch layout (sampler.py: merge_batches).  The member structs live in DEVICE
+ * memory.  loc_off [B*(T+1)]: member b's first local row of each type (loc_off[b*(T+1)+T] = its node count); uoff [B*T]:
+ * the union row of member b's first type-t row (type-major: node_type of the union is sorted).  member_rows [sum N_b]:
+ * the union row of every member row, member b's at node_base.  Edges go to edge_base + e, endpoints remapped (ids
+ * outside the member become -1).  node_feature may be NULL (then the members' are not read). */
+typedef struct {
+  const float* node_feature;
+  const int64_t* edge_index;
+  const int64_t* edge_type;
+  const int64_t* edge_time;
+  int64_t n_nodes, n_edges;
+  int64_t node_base, edge_base;
+} hgt_merge_member;
+int hgt_merge_batches(const hgt_merge_member* members, int32_t n_members, int32_t num_types, const int64_t* loc_off,
+                      const int64_t* uoff, int64_t max_rows, int64_t max_edges, int64_t n_edges, int32_t feat_dim,
+                      int64_t* node_type, float* node_feature, int64_t* member_rows, int64_t* edge_index,
+                      int64_t* edge_type, int64_t* edge_time, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -76,6 +76,16 @@ SIGNATURES = {
     "hgt_gsample_rebuild_count": [_p, _p, _i32, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_gsample_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _p, _i32, _p, _p, _p, _p, _p,
                                   _p, _p],
+    # B subgraphs per pass (sampler.sample_subgraphs_cuda) and their disjoint union (sampler.merge_batches)
+    "hgt_gsample_batch_add_budget_workspace_bytes": [_i32, _i64, _i32, _i64, _c.POINTER(_sz)],
+    "hgt_gsample_batch_add_budget": [_p, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _i64, _i32, _i64, _i64, _p, _p, _sz,
+                                     _p],
+    "hgt_gsample_batch_select_workspace_bytes": [_i32, _i64, _c.POINTER(_sz)],
+    "hgt_gsample_batch_select": [_p, _p, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_batch_rebuild_count": [_p, _p, _i32, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_batch_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p, _p,
+                                        _p, _p, _p],
+    "hgt_merge_batches": [_p, _i32, _i32, _p, _p, _i64, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p],
 }
 
 class ConvArgs(ctypes.Structure):

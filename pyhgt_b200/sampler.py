@@ -465,6 +465,17 @@ class _GState(_c.Structure):                 # hgt_gsample_state
     _fields_ = [("num_types", _c.c_int32), ("pad", _c.c_int32)] + [(n, _c.c_void_p) for n in _PTRS]
 
 
+class _GBatchState(_c.Structure):            # hgt_gsample_batch_state
+    _fields_ = ([("num_types", _c.c_int32), ("n_members", _c.c_int32)] +
+                [(n, _c.c_void_p) for n in _GState._PTRS + ("seed",)])
+
+
+# hgt_merge_member (include/hgt_b200.h)
+MERGE_MEMBER_DTYPE = np.dtype([("node_feature", "<u8"), ("edge_index", "<u8"), ("edge_type", "<u8"),
+                               ("edge_time", "<u8"), ("n_nodes", "<i8"), ("n_edges", "<i8"), ("node_base", "<i8"),
+                               ("edge_base", "<i8")])
+
+
 _I64_MAX = np.iinfo(np.int64).max
 
 
@@ -513,12 +524,15 @@ class DeviceGraph:
                     cblocks.append(cb)
         self.n_blocks = len(cblocks)
         self.blocks_dev = self._struct_array(cblocks)
-        # per target type: its blocks, in dict order (the add_budget of that type walks them)
-        self.type_blocks = {}
+        # the blocks of a target type are contiguous (edge_list is walked target type first), in dict order: the
+        # add_budget of that type walks blocks_dev[begin:end)
+        rng = np.zeros(2 * max(len(self.types), 1), dtype=np.int32)
         for ti in range(len(self.types)):
-            own = [cb for cb, (tt, _, _) in zip(cblocks, self.blocks) if tt == ti]
+            own = [b for b, (tt, _, _) in enumerate(self.blocks) if tt == ti]
             if own:
-                self.type_blocks[ti] = (self._struct_array(own), len(own))
+                rng[2 * ti], rng[2 * ti + 1] = own[0], own[-1] + 1
+        self.max_type_blocks = int(np.max(rng[1::2] - rng[0::2]))
+        self.type_block_range = torch.from_numpy(rng).to(dev)
         self.features, self.feat_dim = None, 0
         if features is not None:
             dims = {int(v.shape[1]) for v in features.values()}
@@ -543,31 +557,9 @@ class DeviceGraph:
         return torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.device)
 
 
-def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None):
-    """HGSampling (pyHGT/data.py:87-210) and ``to_torch`` (data.py:212-256) on the GPU.
-
-    Same distribution over sampled node sets, their times and their order as ``sample_subgraph`` (the host sampler,
-    which replays numpy's stream), drawn from a Philox stream seeded by one draw of ``generator`` (a ``torch.Generator``;
-    None = torch's default CPU generator): the same generator state gives bitwise-identical outputs.
-    ``time_range=None`` turns the time filter off (ogbn-mag variant).  Seed ids of a type must be distinct.
-
-    Returns ``(node_feature, node_type, edge_time, edge_index, edge_type, node_dict, edge_dict, indxs, node_time)``: the
-    first seven as ``to_torch(..., device=dgraph.device, prebuild_plan=True)`` would return them (node_feature gathered
-    from the DeviceGraph's feature tables, None without them), and per sampled type (in ``layer_data`` key order) the
-    sampled ids (``indxs``) and times in ``ser`` order, as device tensors.  The sync-free plan of the graph is built.
-    Host synchronisation: one small read-back per sampling layer (the type order) and one at the end."""
-    import torch
-    from . import _lib
-    from . import plan as _plan
-    dg = dgraph
-    dev = dg.device
-    W = int(sampled_number)
-    depth = int(sampled_depth)
-    if W <= 0 or depth < 0:
-        raise ValueError("sampled_number must be positive and sampled_depth non-negative")
-    T = len(dg.types)
-
-    seeds = []                                            # (slot, ids, times) in inp order
+def _device_seeds(dg, inp):
+    """[(type slot, ids, times)] of one seed dict, in inp order (empty types dropped), validated."""
+    seeds = []
     for _type in inp:
         if _type not in dg.slot:
             raise KeyError("seed type %r is not in graph.get_types()" % (_type,))
@@ -580,19 +572,100 @@ def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp,
         if np.unique(ids).shape[0] != ids.shape[0]:
             raise ValueError("duplicate seed ids of type %r" % (_type,))
         seeds.append((dg.slot[_type], ids, np.ascontiguousarray(arr[:, 1])))
-    n_ids = list(dg.n_ids)
-    n_seed = [0] * T
-    for s, ids, _ in seeds:
-        n_ids[s] = max(n_ids[s], int(ids.max()) + 1)      # seeds beyond the graph become isolated nodes
-        n_seed[s] = ids.shape[0]
-    cap = [min(n_ids[t], n_seed[t] + depth * W) for t in range(T)]
-    type_off = np.concatenate([[0], np.cumsum(n_ids)]).astype(np.int64)
-    lid_off = np.concatenate([[0], np.cumsum(cap)]).astype(np.int64)
-    n_slots, n_lid = int(type_off[-1]), int(lid_off[-1])
+    return seeds
+
+
+class _Upload:
+    """Small host tables -> ONE pinned, non-blocking copy; device views by name afterwards."""
+
+    def __init__(self):
+        self.parts, self.where, self.n = [], {}, 0
+
+    def add(self, name, arr, dtype=np.int64):
+        a = np.ascontiguousarray(np.asarray(arr).reshape(-1), dtype=dtype)
+        raw = a.view(np.uint8)
+        raw = np.concatenate([raw, np.zeros((-raw.shape[0]) % 8, np.uint8)])
+        self.where[name] = (self.n, a.shape[0], dtype)
+        self.parts.append(raw.view(np.int64))
+        self.n += raw.shape[0] // 8
+
+    def to(self, dev):
+        from . import plan as _plan
+        self.d = _plan._to_dev_async(np.concatenate(self.parts + [np.zeros(1, np.int64)]), dev)
+        self.base = self.d.data_ptr()
+        return self
+
+    def ptr(self, name):
+        """Device address of a table (no tensor op: the per-layer loop is host-bound)."""
+        return self.base + 8 * self.where[name][0]
+
+    def view(self, name):
+        import torch
+        o, n, dtype = self.where[name]
+        return (self.d[o:].view(torch.int32) if dtype == np.int32 else self.d[o:])[:n]
+
+
+def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None):
+    """HGSampling (pyHGT/data.py:87-210) and ``to_torch`` (data.py:212-256) on the GPU.
+
+    Same distribution over sampled node sets, their times and their order as ``sample_subgraph`` (the host sampler,
+    which replays numpy's stream), drawn from a Philox stream seeded by one draw of ``generator`` (a ``torch.Generator``;
+    None = torch's default CPU generator): the same generator state gives bitwise-identical outputs.
+    ``time_range=None`` turns the time filter off (ogbn-mag variant).  Seed ids of a type must be distinct.
+
+    Returns ``(node_feature, node_type, edge_time, edge_index, edge_type, node_dict, edge_dict, indxs, node_time)``: the
+    first seven as ``to_torch(..., device=dgraph.device, prebuild_plan=True)`` would return them (node_feature gathered
+    from the DeviceGraph's feature tables, None without them), and per sampled type (in ``layer_data`` key order) the
+    sampled ids (``indxs``) and times in ``ser`` order, as device tensors.  The sync-free plan of the graph is built.
+    Host synchronisation: one small read-back per sampling layer (the type order) and one at the end.  This is
+    ``sample_subgraphs_cuda`` with one seed dict."""
+    return sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, [inp], generator)[0]
+
+
+def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inps, generator=None):
+    """B = len(inps) subgraphs in one device pass: the device equivalent of the reference's pool of ``sample_subgraph``
+    calls (ogbn-mag/train_ogbn_mag.py:82-102, the variance-reduced evaluation's ``vr_num`` samples around the same seeds).
+
+    Returns a list of B tuples, each with the shape and meaning of ``sample_subgraph_cuda``'s; the tensors are views into
+    buffers shared by the batch, and each member's sync-free plan is built.  Member b's Philox seed is the b-th of B
+    successive draws of ``generator`` (each the one draw ``sample_subgraph_cuda`` makes), and member b is bitwise what
+    ``sample_subgraph_cuda`` returns from a generator advanced by b draws.  Every kernel launch and read-back is shared by
+    the members: one read-back per sampling layer (every member's type order) and one at the end, whatever B is.
+
+    Device memory: about B x 52 bytes x (sum of the graph's id ranges) of sampler state (~100 MB per member at ogbn-mag
+    scale), plus add_budget scratch of B x 24 bytes x width x (max targets x blocks per type)."""
+    import torch
+    from . import _lib
+    from . import plan as _plan
+    dg = dgraph
+    dev = dg.device
+    W = int(sampled_number)
+    depth = int(sampled_depth)
+    if W <= 0 or depth < 0:
+        raise ValueError("sampled_number must be positive and sampled_depth non-negative")
+    members = [_device_seeds(dg, inp) for inp in inps]
+    B = len(members)
+    if B == 0:
+        return []
+    T, NB = len(dg.types), dg.n_blocks
+
+    # per member: id ranges (seeds beyond the graph become isolated nodes) and layer capacities, laid out member-major
+    n_ids = np.tile(np.asarray(dg.n_ids, dtype=np.int64).reshape(1, T), (B, 1))
+    n_seed = np.zeros((B, T), dtype=np.int64)
+    for b, seeds in enumerate(members):
+        for s, ids, _ in seeds:
+            n_ids[b, s] = max(n_ids[b, s], int(ids.max()) + 1)
+            n_seed[b, s] = ids.shape[0]
+    cap = np.minimum(n_ids, n_seed + depth * W)
+
+    def offsets(per):                                      # [B, T] sizes -> [B, T+1] absolute starts
+        flat = np.concatenate([[0], np.cumsum(per.reshape(-1))]).astype(np.int64)
+        return np.stack([flat[b * T:b * T + T + 1] for b in range(B)]), int(flat[-1])
+
+    type_off, n_slots = offsets(n_ids)
+    lid_off, n_lid = offsets(cap)
 
     i64 = dict(dtype=torch.int64, device=dev)
-    small = np.concatenate([type_off, lid_off])
-    small_d = _plan._to_dev_async(small, dev)
     ser = torch.full((max(n_slots, 1),), -1, dtype=torch.int32, device=dev)
     ltime = torch.zeros(max(n_slots, 1), **i64)
     lid = torch.zeros(max(n_lid, 1), **i64)
@@ -601,119 +674,213 @@ def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp,
     bstamp = torch.full((max(n_slots, 1),), -1, **i64)
     last_seq = torch.full((max(n_slots, 1),), -1, **i64)
     first_seq = torch.full((max(n_slots, 1),), _I64_MAX, **i64)
-    # one small buffer the host reads: [n_layer T | type_seq 2T | block totals | flags]
-    NB = dg.n_blocks
-    meta = torch.zeros(T + 2 * T + NB + 2, **i64)
-    n_layer, type_seq, totals = meta[:T], meta[T:3 * T], meta[3 * T:3 * T + NB]
-    flags = meta[3 * T + NB:].view(torch.int32)           # 4 int32 flags
-    type_min = torch.full((max(2 * T, 1),), _I64_MAX, **i64)
-    counters = torch.zeros(2, **i64)
+    # one small buffer the host reads: [n_layer B*T | type_seq B*2T | block totals B*NB | flags]
+    meta = torch.zeros(3 * B * T + B * NB + 2, **i64)
+    n_layer, type_seq = meta[:B * T], meta[B * T:3 * B * T]
+    totals = meta[3 * B * T:3 * B * T + B * NB]
+    flags = meta[3 * B * T + B * NB:].view(torch.int32)   # 4 int32 flags
+    type_min = torch.full((max(2 * B * T, 1),), _I64_MAX, **i64)
+    counters = torch.zeros(2 * B, **i64)
 
-    # seeds enter layer_data first, in inp order (data.py:135-137)
-    seq0 = np.full(2 * T, -1, dtype=np.int64)
-    for k, (s, _, _) in enumerate(seeds):
-        seq0[2 * s] = k
-    if seeds:
-        slots = np.concatenate([type_off[s] + ids for s, ids, _ in seeds])
-        sers = np.concatenate([np.arange(ids.shape[0]) for _, ids, _ in seeds])
-        tms = np.concatenate([tm for _, _, tm in seeds])
-        lpos = np.concatenate([lid_off[s] + np.arange(ids.shape[0]) for s, ids, _ in seeds])
-        lids = np.concatenate([ids for _, ids, _ in seeds])
-        nl = np.zeros(T, dtype=np.int64)
-        for s, ids, _ in seeds:
-            nl[s] = ids.shape[0]
-        up = _plan._to_dev_async(np.concatenate([slots, sers, tms, lpos, lids, nl, seq0, [len(seeds), 0]]), dev)
-        n = slots.shape[0]
-        sl_d, ser_d, tm_d, lp_d, li_d = (up[i * n:(i + 1) * n] for i in range(5))
-        ser.index_put_((sl_d,), ser_d.to(torch.int32))
-        ltime.index_put_((sl_d,), tm_d)
-        lid.index_put_((lp_d,), li_d)
-        n_layer.copy_(up[5 * n:5 * n + T])
-        type_seq.copy_(up[5 * n + T:5 * n + 3 * T])
-        counters.copy_(up[5 * n + 3 * T:])
-    else:
-        type_seq.fill_(-1)
-
-    cst = _GState(T, 0, small_d.data_ptr(), small_d.data_ptr() + 8 * (T + 1), ser.data_ptr(), ltime.data_ptr(),
-                  lid.data_ptr(), n_layer.data_ptr(), score.data_ptr(), btime.data_ptr(), bstamp.data_ptr(),
-                  last_seq.data_ptr(), first_seq.data_ptr(), type_min.data_ptr(), type_seq.data_ptr(),
-                  counters.data_ptr())
-    st = torch.cuda.current_stream(dev).cuda_stream
     if generator is None:
-        seed = int(torch.randint(0, 2 ** 63 - 1, (1,)))
+        draws = [int(torch.randint(0, 2 ** 63 - 1, (1,))) for _ in range(B)]
     else:
-        seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=generator, device=generator.device))
+        draws = [int(torch.randint(0, 2 ** 63 - 1, (1,), generator=generator, device=generator.device))
+                 for _ in range(B)]
+
+    # seeds enter layer_data first, in inp order (data.py:135-137); their add_budget runs seed type after seed type,
+    # step j being every member's j-th seed type
+    up = _Upload()
+    up.add("type_off", type_off)
+    up.add("lid_off", lid_off)
+    up.add("seed", np.asarray(draws, dtype=np.uint64).view(np.int64))
+    seq0 = np.full((B, 2 * T), -1, dtype=np.int64)
+    nl0 = np.zeros((B, T), dtype=np.int64)
+    cnt0 = np.zeros((B, 2), dtype=np.int64)
+    slots, sers, tms, lpos, lids = [], [], [], [], []
+    for b, seeds in enumerate(members):
+        cnt0[b, 0] = len(seeds)
+        for k, (s, ids, tm) in enumerate(seeds):
+            seq0[b, 2 * s] = k
+            nl0[b, s] = ids.shape[0]
+            slots.append(type_off[b, s] + ids)
+            sers.append(np.arange(ids.shape[0]))
+            tms.append(tm)
+            lpos.append(lid_off[b, s] + np.arange(ids.shape[0]))
+            lids.append(ids)
+    n_in = sum(a.shape[0] for a in slots)
+    for name, parts in (("slots", slots), ("sers", sers), ("tms", tms), ("lpos", lpos), ("lids", lids)):
+        up.add(name, np.concatenate(parts) if parts else np.zeros(0, np.int64))
+    up.add("nl0", nl0)
+    up.add("seq0", seq0)
+    up.add("cnt0", cnt0)
+    J = max(len(s) for s in members)
+    seed_steps = []                                       # (max targets, names) of seed step j
+    for j in range(J):
+        M = max((s[j][1].shape[0] for s in members if j < len(s)), default=0)
+        ids_j, tms_j = np.zeros((B, M), np.int64), np.zeros((B, M), np.int64)
+        n_j, type_j = np.zeros(B, np.int64), np.full(B, -1, np.int32)
+        for b, seeds in enumerate(members):
+            if j < len(seeds):
+                s, ids, tm = seeds[j]
+                ids_j[b, :ids.shape[0]], tms_j[b, :ids.shape[0]] = ids, tm
+                n_j[b], type_j[b] = ids.shape[0], s
+        for name, arr, dt in (("ids", ids_j, np.int64), ("tms", tms_j, np.int64), ("n", n_j, np.int64),
+                              ("type", type_j, np.int32), ("step", np.full(B, j), np.int64)):
+            up.add("seed%d_%s" % (j, name), arr, dt)
+        seed_steps.append(M)
+    d = up.to(dev)
+    if n_in:
+        sl_d = d.view("slots")
+        ser.index_put_((sl_d,), d.view("sers").to(torch.int32))
+        ltime.index_put_((sl_d,), d.view("tms"))
+        lid.index_put_((d.view("lpos"),), d.view("lids"))
+    n_layer.copy_(d.view("nl0"))
+    type_seq.copy_(d.view("seq0"))
+    counters.copy_(d.view("cnt0"))
+
+    cst = _GBatchState(T, B, d.ptr("type_off"), d.ptr("lid_off"), ser.data_ptr(), ltime.data_ptr(), lid.data_ptr(),
+                       n_layer.data_ptr(), score.data_ptr(), btime.data_ptr(), bstamp.data_ptr(), last_seq.data_ptr(),
+                       first_seq.data_ptr(), type_min.data_ptr(), type_seq.data_ptr(), counters.data_ptr(),
+                       d.ptr("seed"))
+    st = torch.cuda.current_stream(dev).cuda_stream
     time_filter = time_range is not None
     max_time = int(np.max(list(time_range.keys()))) if time_filter else 0
 
-    max_nb = max((nb for _, nb in dg.type_blocks.values()), default=0)
-    max_tg = max([W] + n_seed)
+    max_nb = dg.max_type_blocks
+    max_tg = max([W] + seed_steps)
     bud_ws, sel_ws = _c.c_size_t(), _c.c_size_t()
-    _lib.call("hgt_gsample_add_budget_workspace_bytes", max_tg, max_nb, W, _c.byref(bud_ws))
-    _lib.call("hgt_gsample_select_workspace_bytes", max(n_ids, default=0), _c.byref(sel_ws))
+    _lib.call("hgt_gsample_batch_add_budget_workspace_bytes", B, max_tg, max_nb, W, _c.byref(bud_ws))
+    _lib.call("hgt_gsample_batch_select_workspace_bytes", B, int(n_ids.max(axis=1).sum()), _c.byref(sel_ws))
     ws = torch.empty(max(bud_ws.value, sel_ws.value, 1), dtype=torch.uint8, device=dev)
-    tgt = torch.zeros(2 * W + 1, **i64)                   # [ids W | times W | count]
-    tgt_id, tgt_time, n_tgt = tgt[:W], tgt[W:2 * W], tgt[2 * W:]
-    step = [0]
+    tgt = torch.zeros(2 * B * W + B, **i64)               # [ids B*W | times B*W | counts B]
+    tgt_id, tgt_time, n_tgt = tgt[:B * W], tgt[B * W:2 * B * W], tgt[2 * B * W:]
 
-    def add_budget(s, ids_d, tms_d, max_targets, count_d):
-        ent = dg.type_blocks.get(s)
-        if ent is not None and max_targets > 0:
-            _lib.call("hgt_gsample_add_budget", _c.byref(cst), ent[0].data_ptr(), ent[1], ids_d.data_ptr(),
-                      tms_d.data_ptr(), max_targets, _lib.ptr(count_d), W, int(time_filter), max_time, _NO_TIME, seed,
-                      step[0], flags.data_ptr(), ws.data_ptr(), ws.numel(), st)
-        step[0] += 1
+    blocks_p, range_p, flags_p, ws_p, ws_n = (dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr(),
+                                              flags.data_ptr(), ws.data_ptr(), ws.numel())
+    tgt_id_p, tgt_time_p, n_tgt_p = tgt_id.data_ptr(), tgt_time.data_ptr(), n_tgt.data_ptr()
 
-    if seeds:                                             # then their budgets (data.py:139-141)
-        n = slots.shape[0]
-        o = 0
-        for s, ids, _ in seeds:
-            m = ids.shape[0]
-            add_budget(s, li_d[o:o + m], tm_d[o:o + m], m, None)
-            o += m
+    def add_budget(type_p, step_p, ids_p, tms_p, max_targets, count_p):
+        _lib.call("hgt_gsample_batch_add_budget", _c.byref(cst), blocks_p, range_p, max_nb, type_p, step_p, ids_p,
+                  tms_p, max_targets, count_p, W, int(time_filter), max_time, _NO_TIME, flags_p, ws_p, ws_n, st)
+
+    for j, M in enumerate(seed_steps):                    # the seeds' budgets (data.py:139-141)
+        add_budget(d.ptr("seed%d_type" % j), d.ptr("seed%d_step" % j), d.ptr("seed%d_ids" % j),
+                   d.ptr("seed%d_tms" % j), M, d.ptr("seed%d_n" % j))
+    step = np.asarray([len(s) for s in members], dtype=np.int64)   # a member's next step number
     for _layer in range(depth):                           # data.py:146-170
-        ts = type_seq.cpu().numpy()                       # the per-layer read-back: list(budget.keys())
-        order = sorted((t for t in range(T) if ts[2 * t + 1] >= 0), key=lambda t: ts[2 * t + 1])
-        for s in order:
-            _lib.call("hgt_gsample_select", _c.byref(cst), s, n_ids[s], W, seed, step[0], tgt_id.data_ptr(),
-                      tgt_time.data_ptr(), n_tgt.data_ptr(), flags.data_ptr(), ws.data_ptr(), ws.numel(), st)
-            add_budget(s, tgt_id, tgt_time, W, n_tgt)
+        ts = type_seq.cpu().numpy().reshape(B, 2 * T)     # the per-layer read-back: every member's list(budget.keys())
+        orders = [sorted((t for t in range(T) if ts[b, 2 * t + 1] >= 0), key=lambda t: ts[b, 2 * t + 1])
+                  for b in range(B)]
+        K = max(len(o) for o in orders)
+        if K == 0:
+            continue
+        # step k of the layer: member b selects its k-th budget type (or sits out), then adds its budget
+        typ = np.full((K, B), -1, dtype=np.int32)
+        for b, o in enumerate(orders):
+            typ[:len(o), b] = o
+        rng = np.where(typ >= 0, n_ids[np.arange(B)[None, :], np.maximum(typ, 0)], 0)      # ids each member sorts
+        off = np.zeros((K, B + 1), dtype=np.int64)
+        np.cumsum(rng, axis=1, out=off[:, 1:])
+        up = _Upload()
+        up.add("type", typ, np.int32)
+        up.add("step", step[None, :] + np.arange(K)[:, None])
+        up.add("off", off)
+        d = up.to(dev)
+        type0, step0, off0 = d.ptr("type"), d.ptr("step"), d.ptr("off")
+        for k in range(K):
+            type_p, step_p = type0 + 4 * k * B, step0 + 8 * k * B
+            _lib.call("hgt_gsample_batch_select", _c.byref(cst), type_p, step_p, off0 + 8 * k * (B + 1),
+                      int(off[k, B]), int(rng[k].max()), W, tgt_id_p, tgt_time_p, n_tgt_p, flags_p, ws_p, ws_n, st)
+            add_budget(type_p, step_p, tgt_id_p, tgt_time_p, W, n_tgt_p)
+        step += np.asarray([len(o) for o in orders], dtype=np.int64)
 
     # rebuild (data.py:181-209): count pass, then the one read-back of the batch
-    cnt_off = np.concatenate([[0], np.cumsum([cap[tt] for tt, _, _ in dg.blocks])]).astype(np.int64)
+    cnt_off = np.concatenate([[0], np.cumsum([cap[b, tt] for b in range(B) for tt, _, _ in dg.blocks])]).astype(np.int64)
     n_count = int(cnt_off[-1])
-    max_rows = max(cap, default=0)
+    max_rows = int(cap.max()) if cap.size else 0
     rb_ws = _c.c_size_t()
     _lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
     rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
     ex = torch.empty(n_count + 1, **i64)
     cnt_off_d = _plan._to_dev_async(cnt_off, dev)
-    _lib.call("hgt_gsample_rebuild_count", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(), n_count,
-              max_rows, _lib.ptr(dg.feat_rows) if dg.features is not None else None, ex.data_ptr(),
+    _lib.call("hgt_gsample_batch_rebuild_count", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(),
+              n_count, max_rows, _lib.ptr(dg.feat_rows) if dg.features is not None else None, ex.data_ptr(),
               totals.data_ptr(), flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
     h = meta.cpu().numpy()
-    nl = h[:T]
-    ts = h[T:3 * T]
-    tot = h[3 * T:3 * T + NB]
-    fl = h[3 * T + NB:].view(np.int32)
+    nl = h[:B * T].reshape(B, T)
+    ts = h[B * T:3 * B * T].reshape(B, 2 * T)
+    tot = h[3 * B * T:3 * B * T + B * NB].reshape(B, NB)
+    fl = h[3 * B * T + B * NB:].view(np.int32)
     if fl[0]:
         raise IndexError("a neighbour id lies outside its node type's id range in the device graph")
     if fl[1]:
         raise IndexError("edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
     if dg.features is not None:
-        lacking = [dg.types[t] for t in range(T) if nl[t] and dg.types[t] not in dg.features]
+        lacking = sorted({dg.types[t] for b in range(B) for t in range(T) if nl[b, t] and dg.types[t] not in dg.features})
         if lacking:
             raise KeyError("no feature table for sampled node types %r" % (lacking,))
     if fl[2]:
         raise IndexError("a sampled node id lies outside its type's feature table")
 
-    # the to_torch layout (data.py:226-256): nodes type by type; edges in the order of _finish's edge_list
+    # the to_torch layout of every member (data.py:226-256), member after member in the shared outputs
+    lay = [_member_layout(dg, nl[b], ts[b], tot[b]) for b in range(B)]
+    N_b = np.asarray([int(nl[b].sum()) for b in range(B)], dtype=np.int64)
+    E_b = np.asarray([l[3] for l in lay], dtype=np.int64)
+    node_base = np.concatenate([[0], np.cumsum(N_b)]).astype(np.int64)
+    edge_base = np.concatenate([[0], np.cumsum(E_b)]).astype(np.int64)
+    up = _Upload()
+    up.add("blk_out", np.concatenate([l[1] for l in lay] + [np.full(1, -1, np.int64)]))
+    up.add("node_off", np.concatenate([l[0][:T] for l in lay]))
+    up.add("type_out", np.arange(T))
+    up.add("self_off", np.concatenate([l[2] for l in lay]))
+    up.add("mem_out", np.stack([node_base[:B], edge_base[:B], E_b], 1))
+    d = up.to(dev)
+    N, E = int(node_base[-1]), int(edge_base[-1])
+    self_rel = dg.edge_dict['self']
+    node_type = torch.empty(N, **i64)
+    node_time = torch.empty(N, **i64)
+    node_feature = torch.empty((N, dg.feat_dim), dtype=torch.float32, device=dev) if dg.features is not None else None
+    edge_index = torch.empty(2 * E, **i64)                # member b's [2, E_b] block at 2 * edge_base[b]
+    edge_type = torch.empty(E, **i64)
+    edge_time = torch.empty(E, **i64)
+    _lib.call("hgt_gsample_batch_rebuild_write", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(),
+              ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel,
+              d.ptr("mem_out"), max_rows,
+              _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
+              node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
+              edge_time.data_ptr(), st)
+
+    out = []
+    for b in range(B):
+        node_off, _, _, _, pairs, layer_order = lay[b]
+        n0, n1, e0, e1 = int(node_base[b]), int(node_base[b + 1]), int(edge_base[b]), int(edge_base[b + 1])
+        nt, ntime = node_type[n0:n1], node_time[n0:n1]
+        ei = edge_index[2 * e0:2 * e1].view(2, e1 - e0)
+        et, etime = edge_type[e0:e1], edge_time[e0:e1]
+        meta_plan = {"type_count": [int(v) for v in nl[b]] + [0], "sorted": True, "pairs": sorted(pairs)}
+        _plan.get_plan(nt, ei, et, etime, T, len(dg.edge_dict), host_meta=meta_plan)
+        node_dict = {t: [int(node_off[i]), i] for i, t in enumerate(dg.types)}
+        indxs, times = {}, {}
+        for t in layer_order:
+            if nl[b, t]:
+                indxs[dg.types[t]] = lid[int(lid_off[b, t]):int(lid_off[b, t] + nl[b, t])]
+                times[dg.types[t]] = ntime[int(node_off[t]):int(node_off[t + 1])]
+        out.append((node_feature[n0:n1] if node_feature is not None else None, nt, etime, ei, et, node_dict,
+                    dict(dg.edge_dict), indxs, times))
+    return out
+
+
+def _member_layout(dg, nl, ts, tot):
+    """One member's to_torch layout (data.py:226-256) from its sampled counts nl [T], first-touch numbers ts [2T] and
+    per-block edge totals tot [NB]: nodes type by type, edges in the order of _finish's edge_list.  Returns
+    (node_off [T+1], blk_out [NB], self_off [T], n_edges, <source type, relation> pairs, layer_data key order)."""
+    T, NB = len(dg.types), dg.n_blocks
     node_off = np.concatenate([[0], np.cumsum(nl)]).astype(np.int64)
-    N = int(node_off[-1])
     layer_order = sorted((t for t in range(T) if ts[2 * t] >= 0), key=lambda t: ts[2 * t])
     self_rel = dg.edge_dict['self']
     self_off = np.full(T, -1, dtype=np.int64)
-    blk_out = np.full(max(NB, 1), -1, dtype=np.int64)
+    blk_out = np.full(NB, -1, dtype=np.int64)
     pairs = set()
     E = 0
     for tt in layer_order:
@@ -732,31 +899,92 @@ def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp,
                 blk_out[b] = E
                 E += int(tot[b])
                 pairs.add((dg.blocks[b][1], dg.edge_dict[dg.blocks[b][2]]))
-    tabs = _plan._to_dev_async(np.concatenate([blk_out, node_off[:T], np.arange(T, dtype=np.int64), self_off]), dev)
-    nb1 = blk_out.shape[0]
-    blk_out_d, node_off_d = tabs[:nb1], tabs[nb1:nb1 + T]
-    type_out_d, self_off_d = tabs[nb1 + T:nb1 + 2 * T], tabs[nb1 + 2 * T:]
+    return node_off, blk_out, self_off, E, pairs, layer_order
+
+
+def union_layout(type_counts, edge_counts):
+    """Host side of ``merge_batches``: member b has type_counts[b][t] nodes of type t (type-sorted) and edge_counts[b]
+    edges.  The union is type-major (type 0 of every member, then type 1, ...).  Returns (loc_off [B, T+1]: member b's
+    first local row of each type, uoff [B, T]: the union row of that first row, node_base [B+1] / edge_base [B+1]: prefix
+    sums of the members' node / edge counts, union_count [T]: nodes per type of the union)."""
+    tc = np.asarray(type_counts, dtype=np.int64)
+    B = len(edge_counts)
+    tc = tc.reshape(B, -1)
+    T = tc.shape[1]
+    loc_off = np.zeros((B, T + 1), dtype=np.int64)
+    loc_off[:, 1:] = np.cumsum(tc, axis=1)
+    union_count = tc.sum(axis=0)
+    type_row0 = np.concatenate([[0], np.cumsum(union_count)])[:T]
+    uoff = type_row0[None, :] + np.cumsum(tc, axis=0) - tc
+    node_base = np.concatenate([[0], np.cumsum(loc_off[:, T])]).astype(np.int64)
+    edge_base = np.concatenate([[0], np.cumsum(np.asarray(edge_counts, dtype=np.int64))]).astype(np.int64)
+    return loc_off, uoff.astype(np.int64), node_base, edge_base, union_count
+
+
+def merge_batches(batches, num_types, num_relations):
+    """Disjoint union of B device batches in the ``to_torch`` layout (each ``(node_feature, node_type, edge_time,
+    edge_index, edge_type, ...)``, from ``sample_subgraphs_cuda``, ``sample_subgraph_cuda`` or ``to_torch``) as ONE
+    graph, for a single forward over all of them (variance-reduced evaluation: ogbn-mag/eval_ogbn_mag.py:128-152).
+
+    The union is type-major, so its ``node_type`` is sorted and the layers take their sorted, sync-free paths; edges
+    keep their order, member after member.  Returns ``(node_feature, node_type, edge_time, edge_index, edge_type,
+    member_rows)`` with ``member_rows[b]`` the union rows of member b's nodes in member order (``out[member_rows[b]]`` is
+    member b's output).  node_feature is None when the members have none.
+
+    Per-type counts and <source type, relation> pairs come from each member's cached plan (the samplers and
+    ``to_torch(prebuild_plan=True)`` build one), so there is no device read-back; a member whose plan has left the plan
+    cache gets it rebuilt, which reads back once.  The union's plan is built sync-free from the same host numbers."""
+    import torch
+    from . import _lib
+    from . import plan as _plan
+    T, R = int(num_types), int(num_relations)
+    if not batches:
+        raise ValueError("merge_batches needs at least one batch")
+    dev = batches[0][1].device
+    feats = [bt[0] for bt in batches]
+    if any(f is None for f in feats) and not all(f is None for f in feats):
+        raise ValueError("either every batch has node features or none has")
+    with_feat = feats[0] is not None
+    F = int(feats[0].shape[1]) if with_feat else 0
+    plans, keep = [], []
+    for bt in batches:
+        nf, nt, etime, ei, et = bt[:5]
+        p = _plan.get_plan(nt, ei, et, etime, T, R)
+        if not p.sorted_types or p.type_count[T] != 0:
+            raise ValueError("merge_batches needs batches whose node_type is sorted (the to_torch layout)")
+        if with_feat and (nf.dtype != torch.float32 or nf.dim() != 2 or nf.shape[1] != F or nf.shape[0] != p.n_nodes):
+            raise ValueError("node features must be float32 [N, %d] in every batch" % F)
+        plans.append(p)
+        keep.append((nf.contiguous() if with_feat else None, ei.contiguous(), et.contiguous(), etime.contiguous()))
+    loc_off, uoff, node_base, edge_base, union_count = union_layout([p.type_count[:T] for p in plans],
+                                                                    [p.n_edges for p in plans])
+    B = len(batches)
+    mem = np.zeros(B, dtype=MERGE_MEMBER_DTYPE)
+    for b, (nf, ei, et, etime) in enumerate(keep):
+        mem[b] = (nf.data_ptr() if nf is not None else 0, ei.data_ptr(), et.data_ptr(), etime.data_ptr(),
+                  plans[b].n_nodes, plans[b].n_edges, node_base[b], edge_base[b])
+    up = _Upload()
+    up.add("mem", mem.view(np.int64))
+    up.add("loc_off", loc_off)
+    up.add("uoff", uoff)
+    d = up.to(dev)
+    N, E = int(node_base[-1]), int(edge_base[-1])
+    i64 = dict(dtype=torch.int64, device=dev)
     node_type = torch.empty(N, **i64)
-    node_time = torch.empty(N, **i64)
-    node_feature = torch.empty((N, dg.feat_dim), dtype=torch.float32, device=dev) if dg.features is not None else None
+    node_feature = torch.empty((N, F), dtype=torch.float32, device=dev) if with_feat else None
+    rows = torch.empty(N, **i64)
     edge_index = torch.empty((2, E), **i64)
     edge_type = torch.empty(E, **i64)
     edge_time = torch.empty(E, **i64)
-    _lib.call("hgt_gsample_rebuild_write", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(),
-              ex.data_ptr(), blk_out_d.data_ptr(), node_off_d.data_ptr(), type_out_d.data_ptr(), self_off_d.data_ptr(),
-              self_rel, max_rows, E, _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim,
-              node_type.data_ptr(), node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(),
-              edge_type.data_ptr(), edge_time.data_ptr(), st)
-    meta_plan = {"type_count": [int(v) for v in nl] + [0], "sorted": True, "pairs": sorted(pairs)}
-    _plan.get_plan(node_type, edge_index, edge_type, edge_time, T, len(dg.edge_dict), host_meta=meta_plan)
-
-    node_dict = {t: [int(node_off[i]), i] for i, t in enumerate(dg.types)}
-    indxs, times = {}, {}
-    for t in layer_order:
-        if nl[t]:
-            indxs[dg.types[t]] = lid[int(lid_off[t]):int(lid_off[t] + nl[t])]
-            times[dg.types[t]] = node_time[int(node_off[t]):int(node_off[t + 1])]
-    return (node_feature, node_type, edge_time, edge_index, edge_type, node_dict, dict(dg.edge_dict), indxs, times)
+    _lib.call("hgt_merge_batches", d.ptr("mem"), B, T, d.ptr("loc_off"), d.ptr("uoff"),
+              int(loc_off[:, T].max()), int(max(p.n_edges for p in plans)), E, F, node_type.data_ptr(),
+              _lib.ptr(node_feature), rows.data_ptr(), edge_index.data_ptr(), edge_type.data_ptr(),
+              edge_time.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    pairs = sorted({pr for p in plans for pr in p.pairs})
+    _plan.get_plan(node_type, edge_index, edge_type, edge_time, T, R,
+                   host_meta={"type_count": [int(v) for v in union_count] + [0], "sorted": True, "pairs": pairs})
+    member_rows = [rows[int(node_base[b]):int(node_base[b + 1])] for b in range(B)]
+    return node_feature, node_type, edge_time, edge_index, edge_type, member_rows
 
 
 def _finish(fg, states, layer_order, feature_extractor):

@@ -10,8 +10,13 @@ Prints one JSON line per setting:
                  wall clock, median over --host-batches;
   device_ms      sample_subgraph_cuda (same outputs, features gathered on the device), CUDA events after warm-up,
                  median over --batches (>= 20);
+  device_ms_per_subgraph
+                 sample_subgraphs_cuda with B = 1, 8, 32 seed dicts per call, CUDA events / B, median;
   train_ms       fwd + bwd of a 4-layer n_hid=512 GNN (HGT) on one device batch, CUDA events, median;
   plus the batch sizes, the card name and its power limit.
+Then one `vr_eval` line: 8 subgraphs of the first setting around the same 128 seeds, the GNN plus a linear head under
+eval() / no_grad, timed as 8 single samples + 8 forwards and as one batched sample + merge_batches + one forward, with
+the max abs difference of the averaged logits between the two.
 
     python scripts/gpu_sampler_bench.py [--scale 1.0] [--batches 20] [--host-batches 3]
 """
@@ -157,6 +162,20 @@ def main():
             e1.record()
             torch.cuda.synchronize()
             devt.append(e0.elapsed_time(e1))
+        per_sub = {}
+        for B in (1, 8, 32):
+            inps = [seeds(i) for i in range(B)]
+            for _ in range(2):
+                sampler.sample_subgraphs_cuda(dg, time_range, depth, width, inps, gen)
+            tb = []
+            for i in range(max(5, args.batches // B)):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                sampler.sample_subgraphs_cuda(dg, time_range, depth, width, inps, gen)
+                e1.record()
+                torch.cuda.synchronize()
+                tb.append(e0.elapsed_time(e1) / B)
+            per_sub[str(B)] = round(float(np.median(tb)), 3)
         nf, nt, etime, ei, et = out[:5]
         train = []
         for i in range(8):
@@ -173,8 +192,62 @@ def main():
                           "batch": {"nodes": int(nt.numel()), "edges": int(ei.shape[1])},
                           "host_ms": round(float(np.median(host)), 2), "host_batches": len(host),
                           "device_ms": round(float(np.median(devt)), 3), "device_batches": len(devt),
+                          "device_ms_per_subgraph": per_sub,
                           "train_fwd_bwd_ms": round(float(np.median(train)), 3),
                           "gpu": name, "power_limit": power}), flush=True)
+    vr_eval(args, dg, g, gnn, edge_dict, seeds(0), time_range, name, power)
+
+
+def vr_eval(args, dg, g, gnn, edge_dict, inp, time_range, name, power, n_vr=8, n_cls=349):
+    """Variance-reduced evaluation (pyHGT ogbn-mag/eval_ogbn_mag.py:128-152): n_vr subgraphs around the same 128 seeds,
+    logits of the seeds averaged.  Timed two ways from the same generator state (so the same subgraphs): n_vr single
+    samples and n_vr forwards, and one batched sample + merge_batches + one forward over the union."""
+    from pyhgt_b200 import sampler
+    depth, width = (int(v) for v in args.settings.split(",")[0].split("x"))
+    dev = dg.device
+    T, R = len(dg.types), len(edge_dict)
+    torch.manual_seed(1)
+    head = torch.nn.Linear(512, n_cls).to(dev)
+    gnn.eval()
+    n_seed = inp["paper"].shape[0]
+
+    def singles(gen):
+        acc = 0
+        for _ in range(n_vr):
+            b = sampler.sample_subgraph_cuda(dg, time_range, depth, width, inp, gen)
+            p0 = b[5]["paper"][0]
+            acc = acc + head(gnn(*b[:5])[p0:p0 + n_seed])
+        return acc / n_vr
+
+    def batched(gen):
+        bs = sampler.sample_subgraphs_cuda(dg, time_range, depth, width, [inp] * n_vr, gen)
+        nf, nt, etime, ei, et, rows = sampler.merge_batches(bs, T, R)
+        y = gnn(nf, nt, etime, ei, et)
+        sel = torch.cat([rows[v][b[5]["paper"][0]:b[5]["paper"][0] + n_seed] for v, b in enumerate(bs)])
+        return head(y[sel]).view(n_vr, n_seed, n_cls).mean(0)
+
+    times = {}
+    with torch.no_grad():
+        for label, fn in (("singles", singles), ("batched", batched)):
+            for _ in range(2):
+                fn(torch.Generator().manual_seed(0))
+            tl = []
+            for i in range(max(5, args.batches // 4)):
+                gen = torch.Generator().manual_seed(i)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                fn(gen)
+                e1.record()
+                torch.cuda.synchronize()
+                tl.append(e0.elapsed_time(e1))
+            times[label] = (round(float(np.median(tl)), 2), len(tl))
+        diff = (singles(torch.Generator().manual_seed(7)) - batched(torch.Generator().manual_seed(7))).abs().max().item()
+    gnn.train()
+    print(json.dumps({"vr_eval": {"subgraphs": n_vr, "seeds": n_seed, "depth": depth, "width": width,
+                                  "model": "GNN 4 layers n_hid 512 + linear head, eval, no_grad"},
+                      "singles_ms": times["singles"][0], "batched_merged_ms": times["batched"][0],
+                      "repeats": times["singles"][1], "max_abs_diff": diff,
+                      "gpu": name, "power_limit": power}), flush=True)
 
 
 if __name__ == "__main__":
