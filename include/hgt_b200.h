@@ -608,6 +608,26 @@ int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_state, cons
                                     int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature,
                                     int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream);
 
+/* The two rebuild passes with an edge mask (sampler.py: sample_subgraphs_cuda(..., edge_mask=...)).  min_ser
+ * [2*n_blocks] (device, not NULL), shared by every member: an edge of block k is kept iff its target ser >=
+ * min_ser[2k] and its source ser >= min_ser[2k+1]; {0, 0} keeps the whole block.  Pass the same table to both passes:
+ * totals and the edge layout then count kept edges only, in block order, and the edge_time check (flags[1]) looks at
+ * kept edges only.  The neighbour id check (flags[0]) still covers every edge.  Otherwise as the unmasked entry points,
+ * which are these with no mask. */
+int hgt_gsample_batch_rebuild_count_masked(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
+                                           int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                           int64_t n_count, int64_t max_rows, const int64_t* feat_rows, int64_t* ex,
+                                           int64_t* totals, int32_t* flags, void* workspace, size_t workspace_bytes,
+                                           void* stream);
+int hgt_gsample_batch_rebuild_write_masked(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
+                                           int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                           const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
+                                           const int64_t* type_out, const int64_t* self_off, int64_t self_rel,
+                                           const int64_t* mem_out, int64_t max_rows, const float* const* feat,
+                                           int32_t feat_dim, int64_t* node_type, int64_t* node_time,
+                                           float* node_feature, int64_t* edge_index, int64_t* edge_type,
+                                           int64_t* edge_time, void* stream);
+
 /* Disjoint union of B batches in the to_torch layout (sampler.py: merge_batches).  The member structs live in DEVICE
  * memory.  loc_off [B*(T+1)]: member b's first local row of each type (loc_off[b*(T+1)+T] = its node count); uoff [B*T]:
  * the union row of member b's first type-t row (type-major: node_type of the union is sorted).  member_rows [sum N_b]:

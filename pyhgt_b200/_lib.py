@@ -85,6 +85,10 @@ SIGNATURES = {
     "hgt_gsample_batch_rebuild_count": [_p, _p, _i32, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_gsample_batch_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p, _p,
                                         _p, _p, _p],
+    # the same rebuild with a per-block edge mask (sample_subgraphs_cuda(..., edge_mask=...))
+    "hgt_gsample_batch_rebuild_count_masked": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_batch_rebuild_write_masked": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p,
+                                               _p, _p, _p, _p, _p, _p],
     "hgt_merge_batches": [_p, _i32, _i32, _p, _p, _i64, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p],
 }
 

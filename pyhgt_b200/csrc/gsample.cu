@@ -7,7 +7,8 @@
 //     reference's processing order for the last-writer time and the first-entry stamp), so it is bitwise repeatable;
 //   * selection (data.py:150-165): Efraimidis-Spirakis keys log(u)/score^2 sorted with CUB (same ordered distribution as
 //     np.random.choice(p, replace=False)), or the insertion stamp when the budget is smaller than the width;
-//   * rebuild (data.py:181-209) + to_torch layout (data.py:226-256): count / scan / write per adjacency block.
+//   * rebuild (data.py:181-209) + to_torch layout (data.py:226-256): count / scan / write per adjacency block, optionally
+//     dropping edges by per-block minimum target / source sers (the OAG scripts' label-leak mask).
 // Every stage runs B independent subgraphs ("members") at once: each member has its own rows of the state, its own seed
 // and its own step numbers, and everything a member computes depends on its own rows alone, so member b of a batch is
 // bitwise the single-subgraph run with b's seed.  The single-subgraph entry points are the B = 1 case.
@@ -330,10 +331,19 @@ __global__ void k_sel_finish(hgt_gsample_batch_state st, PerMember<int32_t> type
   n_targets[m] = c;
 }
 
+// The caller's edge mask (sampler.py: edge_mask; the OAG scripts drop the edges that would leak a seed's label between
+// sample_subgraph and to_torch): an edge of block b with target ser r and source ser sser is dropped unless
+// r >= min_ser[2b] and sser >= min_ser[2b+1].  min_ser == NULL keeps every edge.  Both rebuild passes use this one
+// predicate, so the count pass's prefix sum and the edges the write pass lays out agree.
+__device__ __forceinline__ bool masked_out(const int64_t* min_ser, int b, int64_t r, int64_t sser) {
+  return min_ser && (r < min_ser[2 * b] || sser < min_ser[2 * b + 1]);
+}
+
 // One warp per <member (grid.z), block (grid.y), target ser r>: neighbours of the target that are in the member's sample
-// (data.py:190-209), counted, with the edge_time range check of to_torch (data.py:250; RelTemporalEncoding has 240 rows).
+// (data.py:190-209) and not masked out, counted, with the edge_time range check of to_torch on those kept edges
+// (data.py:250; RelTemporalEncoding has 240 rows).
 __global__ void k_rb_count(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
-                           const int64_t* cnt_off, int64_t* cnt, int32_t* flags) {
+                           const int64_t* min_ser, const int64_t* cnt_off, int64_t* cnt, int32_t* flags) {
   const int lane = threadIdx.x & 31;
   const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int b = blockIdx.y;
@@ -353,7 +363,8 @@ __global__ void k_rb_count(hgt_gsample_batch_state st, const hgt_gsample_block* 
       for (int64_t p = a + lane; p < e; p += 32) {
         const int64_t sid = blk.nbr[p];
         if (sid < 0 || sid >= sn) { flags[0] = 1; continue; }
-        if (st.ser[sb + sid] < 0) continue;
+        const int32_t sser = st.ser[sb + sid];
+        if (sser < 0 || masked_out(min_ser, b, r, sser)) continue;
         ++c;
         const int64_t dt = tt - st.ltime[sb + sid] + 120;
         if (dt < 0 || dt >= HGT_RTE_MAX_LEN) flags[1] = 1;
@@ -377,10 +388,11 @@ __global__ void k_rb_check_features(hgt_gsample_batch_state st, const int64_t* f
 }
 
 // blk_out / node_off / self_off are member-local (member m's rows [m * n_blocks ...] / [m * T ...]); edge_index holds
-// each member's [2, E_m] block at 2 * edge_base, node ids member-local.
+// each member's [2, E_m] block at 2 * edge_base, node ids member-local.  The ballot keeps the kept edges in block order.
 __global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
-                           const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
-                           MemOut mo, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time) {
+                           const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out,
+                           const int64_t* node_off, MemOut mo, int64_t* edge_index, int64_t* edge_type,
+                           int64_t* edge_time) {
   const int lane = threadIdx.x & 31;
   const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int b = blockIdx.y;
@@ -409,8 +421,9 @@ __global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* 
       sid = blk.nbr[p];
       if (sid >= 0 && sid < sn) sser = st.ser[sb + sid];
     }
-    const unsigned keep = __ballot_sync(kFull, sser >= 0);
-    if (sser >= 0) {
+    const bool kept = sser >= 0 && !masked_out(min_ser, b, r, sser);
+    const unsigned keep = __ballot_sync(kFull, kept);
+    if (kept) {
       const int64_t o = e + __popc(keep & ((1u << lane) - 1u));
       ei[o] = noff[S] + sser;                                           // row 0 = source (data.py:245,254)
       ei[n_edges + o] = dst;
@@ -625,9 +638,9 @@ int select(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMembe
 }
 
 int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
-                  const int64_t* cnt_off, int64_t n_count, int64_t max_rows, const int64_t* feat_rows, int64_t* ex,
-                  int64_t* totals, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream,
-                  const char* what) {
+                  const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count, int64_t max_rows,
+                  const int64_t* feat_rows, int64_t* ex, int64_t* totals, int32_t* flags, void* workspace,
+                  size_t workspace_bytes, void* stream, const char* what) {
   HGT_REQUIRE(n_blocks >= 0 && n_blocks < 65536 && hs.num_types < 65536 && hs.n_members >= 1 &&
                   hs.n_members < 65536 && max_rows >= 0,
               "%s: bad arguments", what);
@@ -641,7 +654,7 @@ int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* bl
   HGT_CHECK_CUDA(cudaMemsetAsync(cnt + n_count, 0, sizeof(int64_t), st));
   if (n_blocks > 0 && max_rows > 0) {
     k_rb_count<<<dim3((unsigned)blocks_for(max_rows, kWarps), n_blocks, hs.n_members), kThreads, 0, st>>>(
-        hs, blocks, n_blocks, cnt_off, cnt, flags);
+        hs, blocks, n_blocks, min_ser, cnt_off, cnt, flags);
     HGT_LAUNCH_CHECK();
   }
   HGT_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(cub_tmp, tmp, cnt, ex, (int)(n_count + 1), st));
@@ -659,7 +672,8 @@ int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* bl
 }
 
 int rebuild_write(const hgt_gsample_batch_state& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
-                  const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
+                  const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out,
+                  const int64_t* node_off,
                   const int64_t* type_out, const int64_t* self_off, int64_t self_rel, MemOut mo, int64_t max_rows,
                   const float* const* feat, int32_t feat_dim, int64_t* node_type, int64_t* node_time,
                   float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream,
@@ -671,7 +685,7 @@ int rebuild_write(const hgt_gsample_batch_state& hs, const hgt_gsample_block* bl
   if (max_rows == 0) return 0;
   if (n_blocks > 0) {
     k_rb_write<<<dim3((unsigned)blocks_for(max_rows, kWarps), n_blocks, hs.n_members), kThreads, 0, st>>>(
-        hs, blocks, n_blocks, cnt_off, ex, blk_out, node_off, mo, edge_index, edge_type, edge_time);
+        hs, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, mo, edge_index, edge_type, edge_time);
     HGT_LAUNCH_CHECK();
   }
   if (hs.num_types > 0) {
@@ -733,8 +747,8 @@ extern "C" int hgt_gsample_rebuild_count(const hgt_gsample_state* h_state, const
                                          const int64_t* feat_rows, int64_t* ex, int64_t* totals, int32_t* flags,
                                          void* workspace, size_t workspace_bytes, void* stream) {
   HGT_REQUIRE(h_state, "hgt_gsample_rebuild_count: bad arguments");
-  return rebuild_count(as_batch(*h_state), blocks, n_blocks, cnt_off, n_count, max_rows, feat_rows, ex, totals, flags,
-                       workspace, workspace_bytes, stream, "hgt_gsample_rebuild_count");
+  return rebuild_count(as_batch(*h_state), blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, ex, totals,
+                       flags, workspace, workspace_bytes, stream, "hgt_gsample_rebuild_count");
 }
 
 extern "C" int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks,
@@ -745,8 +759,8 @@ extern "C" int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const
                                          int64_t* node_time, float* node_feature, int64_t* edge_index,
                                          int64_t* edge_type, int64_t* edge_time, void* stream) {
   HGT_REQUIRE(h_state && n_edges >= 0, "hgt_gsample_rebuild_write: bad arguments");
-  return rebuild_write(as_batch(*h_state), blocks, n_blocks, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {nullptr, n_edges}, max_rows, feat, feat_dim, node_type, node_time, node_feature,
+  return rebuild_write(as_batch(*h_state), blocks, n_blocks, nullptr, cnt_off, ex, blk_out, node_off, type_out,
+                       self_off, self_rel, {nullptr, n_edges}, max_rows, feat, feat_dim, node_type, node_time, node_feature,
                        edge_index, edge_type, edge_time, stream, "hgt_gsample_rebuild_write");
 }
 
@@ -792,8 +806,19 @@ extern "C" int hgt_gsample_batch_rebuild_count(const hgt_gsample_batch_state* h_
                                                int64_t max_rows, const int64_t* feat_rows, int64_t* ex, int64_t* totals,
                                                int32_t* flags, void* workspace, size_t workspace_bytes, void* stream) {
   HGT_REQUIRE(h_state, "hgt_gsample_batch_rebuild_count: bad arguments");
-  return rebuild_count(*h_state, blocks, n_blocks, cnt_off, n_count, max_rows, feat_rows, ex, totals, flags, workspace,
-                       workspace_bytes, stream, "hgt_gsample_batch_rebuild_count");
+  return rebuild_count(*h_state, blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, ex, totals, flags,
+                       workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count");
+}
+
+extern "C" int hgt_gsample_batch_rebuild_count_masked(const hgt_gsample_batch_state* h_state,
+                                                      const hgt_gsample_block* blocks, int32_t n_blocks,
+                                                      const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count,
+                                                      int64_t max_rows, const int64_t* feat_rows, int64_t* ex,
+                                                      int64_t* totals, int32_t* flags, void* workspace,
+                                                      size_t workspace_bytes, void* stream) {
+  HGT_REQUIRE(h_state && min_ser, "hgt_gsample_batch_rebuild_count_masked: bad arguments");
+  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, ex, totals, flags,
+                       workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count_masked");
 }
 
 extern "C" int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
@@ -805,7 +830,19 @@ extern "C" int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_
                                                int64_t* edge_index, int64_t* edge_type, int64_t* edge_time,
                                                void* stream) {
   HGT_REQUIRE(h_state && mem_out, "hgt_gsample_batch_rebuild_write: bad arguments");
-  return rebuild_write(*h_state, blocks, n_blocks, cnt_off, ex, blk_out, node_off, type_out, self_off, self_rel,
-                       {mem_out, 0}, max_rows, feat, feat_dim, node_type, node_time, node_feature, edge_index,
-                       edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write");
+  return rebuild_write(*h_state, blocks, n_blocks, nullptr, cnt_off, ex, blk_out, node_off, type_out, self_off,
+                       self_rel, {mem_out, 0}, max_rows, feat, feat_dim, node_type, node_time, node_feature,
+                       edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write");
+}
+
+extern "C" int hgt_gsample_batch_rebuild_write_masked(
+    const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks, const int64_t* min_ser,
+    const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
+    const int64_t* self_off, int64_t self_rel, const int64_t* mem_out, int64_t max_rows, const float* const* feat,
+    int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature, int64_t* edge_index,
+    int64_t* edge_type, int64_t* edge_time, void* stream) {
+  HGT_REQUIRE(h_state && min_ser && mem_out, "hgt_gsample_batch_rebuild_write_masked: bad arguments");
+  return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
+                       self_rel, {mem_out, 0}, max_rows, feat, feat_dim, node_type, node_time, node_feature,
+                       edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write_masked");
 }

@@ -575,6 +575,27 @@ def _device_seeds(dg, inp):
     return seeds
 
 
+def _edge_mask_table(dg, edge_mask):
+    """edge_mask ``{(target_type, source_type, relation): (min_target_ser, min_source_ser)}`` -> the rebuild's min_ser
+    table [2 * n_blocks] (0, 0 = keep the block whole), or None for no mask (None or {})."""
+    if not edge_mask:
+        return None
+    index = {(dg.types[t], dg.types[s], r): b for b, (t, s, r) in enumerate(dg.blocks)}
+    table = np.zeros(2 * dg.n_blocks, dtype=np.int64)
+    for key, rule in edge_mask.items():
+        if not isinstance(key, tuple) or len(key) != 3:
+            raise KeyError("edge_mask keys are (target_type, source_type, relation), got %r" % (key,))
+        if key[2] == 'self':
+            raise ValueError("edge_mask: the 'self' relation cannot be masked, got %r" % (key,))
+        if key not in index:
+            raise KeyError("edge_mask: %r is not a <target type, source type, relation> block of the graph" % (key,))
+        min_t, min_s = (int(v) for v in rule)
+        if min_t < 0 or min_s < 0:
+            raise ValueError("edge_mask: thresholds must be non-negative, got %r for %r" % (tuple(rule), key))
+        table[2 * index[key]:2 * index[key] + 2] = min_t, min_s
+    return table
+
+
 class _Upload:
     """Small host tables -> ONE pinned, non-blocking copy; device views by name afterwards."""
 
@@ -605,7 +626,7 @@ class _Upload:
         return (self.d[o:].view(torch.int32) if dtype == np.int32 else self.d[o:])[:n]
 
 
-def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None):
+def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None, edge_mask=None):
     """HGSampling (pyHGT/data.py:87-210) and ``to_torch`` (data.py:212-256) on the GPU.
 
     Same distribution over sampled node sets, their times and their order as ``sample_subgraph`` (the host sampler,
@@ -613,18 +634,28 @@ def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp,
     None = torch's default CPU generator): the same generator state gives bitwise-identical outputs.
     ``time_range=None`` turns the time filter off (ogbn-mag variant).  Seed ids of a type must be distinct.
 
+    ``edge_mask`` ``{(target_type, source_type, relation): (min_target_ser, min_source_ser)}`` drops, from the sampled
+    adjacency, every edge of that block whose target ser or source ser (position in ``layer_data[type]``; seeds are
+    0..n-1 in ``inp`` order) is below its minimum: the masking the OAG scripts apply to ``edge_list`` between
+    ``sample_subgraph`` and ``to_torch`` so that a seed's label does not leak through its edge to the label node
+    (OAG/train_paper_field.py:109-122).  Sampling is untouched: nodes, features, times and ``indxs`` are bitwise those
+    of the same call without the mask, and the edges are its edges minus the masked ones, in the same order.  Keys must
+    be blocks of the graph (KeyError) other than ``'self'`` (ValueError); thresholds are non-negative.
+
     Returns ``(node_feature, node_type, edge_time, edge_index, edge_type, node_dict, edge_dict, indxs, node_time)``: the
     first seven as ``to_torch(..., device=dgraph.device, prebuild_plan=True)`` would return them (node_feature gathered
     from the DeviceGraph's feature tables, None without them), and per sampled type (in ``layer_data`` key order) the
     sampled ids (``indxs``) and times in ``ser`` order, as device tensors.  The sync-free plan of the graph is built.
     Host synchronisation: one small read-back per sampling layer (the type order) and one at the end.  This is
     ``sample_subgraphs_cuda`` with one seed dict."""
-    return sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, [inp], generator)[0]
+    return sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, [inp], generator, edge_mask)[0]
 
 
-def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inps, generator=None):
+def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inps, generator=None, edge_mask=None):
     """B = len(inps) subgraphs in one device pass: the device equivalent of the reference's pool of ``sample_subgraph``
     calls (ogbn-mag/train_ogbn_mag.py:82-102, the variance-reduced evaluation's ``vr_num`` samples around the same seeds).
+    ``edge_mask`` (see ``sample_subgraph_cuda``) applies to every member; it acts in the rebuild's count and write passes
+    and adds no launch and no read-back.
 
     Returns a list of B tuples, each with the shape and meaning of ``sample_subgraph_cuda``'s; the tensors are views into
     buffers shared by the batch, and each member's sync-free plan is built.  Member b's Philox seed is the b-th of B
@@ -643,6 +674,7 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     depth = int(sampled_depth)
     if W <= 0 or depth < 0:
         raise ValueError("sampled_number must be positive and sampled_depth non-negative")
+    min_ser = _edge_mask_table(dg, edge_mask)
     members = [_device_seeds(dg, inp) for inp in inps]
     B = len(members)
     if B == 0:
@@ -803,10 +835,13 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     _lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
     rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
     ex = torch.empty(n_count + 1, **i64)
-    cnt_off_d = _plan._to_dev_async(cnt_off, dev)
-    _lib.call("hgt_gsample_batch_rebuild_count", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(),
-              n_count, max_rows, _lib.ptr(dg.feat_rows) if dg.features is not None else None, ex.data_ptr(),
-              totals.data_ptr(), flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
+    # the mask table rides behind cnt_off in the same copy; the masked entry points take it right after n_blocks
+    cnt_off_d = _plan._to_dev_async(cnt_off if min_ser is None else np.concatenate([cnt_off, min_ser]), dev)
+    masked = () if min_ser is None else (cnt_off_d.data_ptr() + 8 * cnt_off.shape[0],)
+    suffix = "" if min_ser is None else "_masked"
+    _lib.call("hgt_gsample_batch_rebuild_count" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
+              cnt_off_d.data_ptr(), n_count, max_rows, _lib.ptr(dg.feat_rows) if dg.features is not None else None,
+              ex.data_ptr(), totals.data_ptr(), flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
     h = meta.cpu().numpy()
     nl = h[:B * T].reshape(B, T)
     ts = h[B * T:3 * B * T].reshape(B, 2 * T)
@@ -844,9 +879,9 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     edge_index = torch.empty(2 * E, **i64)                # member b's [2, E_b] block at 2 * edge_base[b]
     edge_type = torch.empty(E, **i64)
     edge_time = torch.empty(E, **i64)
-    _lib.call("hgt_gsample_batch_rebuild_write", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, cnt_off_d.data_ptr(),
-              ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel,
-              d.ptr("mem_out"), max_rows,
+    _lib.call("hgt_gsample_batch_rebuild_write" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
+              cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
+              d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
               _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
               node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
               edge_time.data_ptr(), st)
@@ -873,7 +908,8 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
 
 def _member_layout(dg, nl, ts, tot):
     """One member's to_torch layout (data.py:226-256) from its sampled counts nl [T], first-touch numbers ts [2T] and
-    per-block edge totals tot [NB]: nodes type by type, edges in the order of _finish's edge_list.  Returns
+    per-block edge totals tot [NB] (kept edges only under an edge mask: an emptied block is laid out like one the sample
+    never reached): nodes type by type, edges in the order of _finish's edge_list.  Returns
     (node_off [T+1], blk_out [NB], self_off [T], n_edges, <source type, relation> pairs, layer_data key order)."""
     T, NB = len(dg.types), dg.n_blocks
     node_off = np.concatenate([[0], np.cumsum(nl)]).astype(np.int64)

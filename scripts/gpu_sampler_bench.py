@@ -14,6 +14,8 @@ Prints one JSON line per setting:
                  sample_subgraphs_cuda with B = 1, 8, 32 seed dicts per call, CUDA events / B, median;
   train_ms       fwd + bwd of a 4-layer n_hid=512 GNN (HGT) on one device batch, CUDA events, median;
   plus the batch sizes, the card name and its power limit.
+Then one `edge_mask` line: `device_ms_per_subgraph` with the OAG paper-field label mask and without it, alternating
+call by call, at every setting and B = 1, 8, 32.
 Then one `vr_eval` line: 8 subgraphs of the first setting around the same 128 seeds, the GNN plus a linear head under
 eval() / no_grad, timed as 8 single samples + 8 forwards and as one batched sample + merge_batches + one forward, with
 the max abs difference of the averaged logits between the two.
@@ -195,7 +197,42 @@ def main():
                           "device_ms_per_subgraph": per_sub,
                           "train_fwd_bwd_ms": round(float(np.median(train)), 3),
                           "gpu": name, "power_limit": power}), flush=True)
+    mask_timing(args, dg, seeds, time_range, name, power)
     vr_eval(args, dg, g, gnn, edge_dict, seeds(0), time_range, name, power)
+
+
+def mask_timing(args, dg, seeds, time_range, name, power, n_seed=128):
+    """The paper-field label-leak mask (OAG/train_paper_field.py:109-122) against no mask, at every setting and B = 1, 8,
+    32: `edge_mask` acts inside the rebuild's count and write passes, so it should cost nothing measurable.  In this
+    graph PF_in_L2 has paper as its target (OAG names the paper -> field direction rev_PF_in_L2), hence the keys.
+    The two variants alternate call by call from the same generator state; CUDA events / B, median."""
+    from pyhgt_b200 import sampler
+    mask = {("paper", "field", "PF_in_L2"): (n_seed, 0), ("field", "paper", "rev_PF_in_L2"): (0, n_seed)}
+    variants = (("none", None), ("mask", mask))
+    res, edges = {}, {}
+    for setting in args.settings.split(","):
+        depth, width = (int(v) for v in setting.split("x"))
+        per = {}
+        for B in (1, 8, 32):
+            inps = [seeds(i) for i in range(B)]
+            tl = {label: [] for label, _ in variants}
+            for i in range(2 + max(5, args.batches // B)):
+                for label, m in (variants if i % 2 == 0 else variants[::-1]):
+                    gen = torch.Generator().manual_seed(i)
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    out = sampler.sample_subgraphs_cuda(dg, time_range, depth, width, inps, gen, edge_mask=m)
+                    e1.record()
+                    torch.cuda.synchronize()
+                    if i >= 2:                                 # the first two rounds warm both variants up
+                        tl[label].append(e0.elapsed_time(e1) / B)
+                    if B == 1 and i == 0:
+                        edges.setdefault(setting, {})[label] = int(out[0][3].shape[1])
+            per[str(B)] = {label: round(float(np.median(v)), 3) for label, v in tl.items()}
+        res[setting] = per
+    print(json.dumps({"edge_mask": "paper-field label mask, %d paper seeds" % n_seed,
+                      "device_ms_per_subgraph": res, "edges_of_one_subgraph": edges,
+                      "gpu": name, "power_limit": power}), flush=True)
 
 
 def vr_eval(args, dg, g, gnn, edge_dict, inp, time_range, name, power, n_vr=8, n_cls=349):
