@@ -10,10 +10,10 @@
 // Tensor-core path (Hopper wgmma, tcp::split3_tile in tc_ptx.cuh): the same split-bf16 x3 scheme as the forward (x = hi + lo,
 // three bf16 products in one fp32 register accumulator):
 //   k_act_split / k_split_colsum   fp32 -> bf16 hi/lo (optionally gelu first); the dOut split pass also produces db
-//   k_lin_dx_tc (DxJob)   one 128 x tile_n tile of dA per CTA; K runs over (column block, 64-wide k-block); A operand = dOut tiles
+//   k_lin_dx_tc (DxJob)   128 x tile_n tiles of dA (persistent CTAs); K runs over (column block, 64-wide k-block); A operand = dOut tiles
 //           (K-major), B operand = W^T (a transposed, zero-padded bf16 split of the small weight matrix);
 //           epilogue: optional `+= dA`, optional `* gelu'(aux)` (the gelu in front of the a_linears, conv.py:119)
-//   k_lin_dw_tc (DwJob)   dW tile [128 of width] x [tile_n of K_in] per CTA, reduction over a chunk of the group's rows; both operands
+//   k_lin_dw_tc (DwJob)   dW tiles [128 of width] x [tile_n of K_in] (persistent CTAs), each a reduction over a chunk of the group's rows; both operands
 //           are MN-major (the reduction index is the row index): TMA boxes {64 columns, 64 rows}, SWIZZLE_128B;
 //           partial tiles are added with red.global.add.v2.f32
 // Every (group, column block) gets its own tensor map (tight row extents => rows past the group are zero-filled by TMA, so the
@@ -232,7 +232,7 @@ struct DxJob {
     tma_load_2d(sa + 2 * A_BYTES + BN * BK * 2, maps + map_wt + 1, tk.wt_col0 + kb * BK, t.n0, bar);
   }
   template <int BN>
-  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+  __device__ void store(const Tile& t, const float* acc, float*, int c, int wq, int lane) const {
     const int64_t rows = t.rows - 64 * c;
     const int cols = K_in - t.n0;
     const int64_t row0 = (t.a_row0 + 64 * c) * K_in + t.n0;
@@ -312,7 +312,7 @@ struct DwJob {
     }
   }
   template <int BN>
-  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+  __device__ void store(const Tile& t, const float* acc, float*, int c, int wq, int lane) const {
     const int rows = width - t.mt * BM - 64 * c;                   // rows of the dW tile = columns of the dOut block
     const int cols = K_in - t.n0;
     float* o = dW + ((int64_t)t.w_row + t.mt * BM + 64 * c) * K_in + t.n0;
@@ -339,7 +339,7 @@ struct DwJobDet : DwJob {
     return DwJob::decode(unit, t);
   }
   template <int BN>
-  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+  __device__ void store(const Tile& t, const float* acc, float*, int c, int wq, int lane) const {
     const int rows = width - t.mt * BM - 64 * c;
     const int cols = K_in - t.n0;
     float* o = part + (t.slot * width + t.mt * BM + 64 * c) * K_in + t.n0;
@@ -632,40 +632,40 @@ BwdLayout bwd_layout(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_
 }
 
 template <int BN>
-__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dx_tc(const __grid_constant__ DxJob job) {
-  split3_tile<BN, false>(job);
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dx_tc(const __grid_constant__ DxJob job, int n_tiles) {
+  split3_tile<BN, false, BK>(job, n_tiles);
 }
 template <int BN>
-__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc(const __grid_constant__ DwJob job) {
-  split3_tile<BN, true>(job);
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc(const __grid_constant__ DwJob job, int n_tiles) {
+  split3_tile<BN, true, BK>(job, n_tiles);
 }
 
 template <int BN>
-int launch_bwd(const DxJob& job, unsigned tiles, cudaStream_t st) {
+int launch_bwd(const DxJob& job, int tiles, cudaStream_t st) {
   const size_t smem = tile_smem_bytes<BN>();
   HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dx_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_lin_dx_tc<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  k_lin_dx_tc<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
 template <int BN>
-int launch_bwd(const DwJob& job, unsigned tiles, cudaStream_t st) {
+int launch_bwd(const DwJob& job, int tiles, cudaStream_t st) {
   const size_t smem = tile_smem_bytes<BN>();
   HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_lin_dw_tc<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  k_lin_dw_tc<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
 
 template <int BN>
-__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc_det(const __grid_constant__ DwJobDet job) {
-  split3_tile<BN, true>(job);
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc_det(const __grid_constant__ DwJobDet job, int n_tiles) {
+  split3_tile<BN, true, BK>(job, n_tiles);
 }
 template <int BN>
-int launch_bwd(const DwJobDet& job, unsigned tiles, cudaStream_t st) {
+int launch_bwd(const DwJobDet& job, int tiles, cudaStream_t st) {
   const size_t smem = tile_smem_bytes<BN>();
   HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc_det<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_lin_dw_tc_det<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  k_lin_dw_tc_det<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -925,9 +925,9 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
       job.accumulate = accumulate_dA;
       job.gelu_aux = gelu_aux;
       switch (job.tile_n) {
-        case 64: rc = launch_bwd<64>(job, (unsigned)total, st); break;
-        case 128: rc = launch_bwd<128>(job, (unsigned)total, st); break;
-        default: rc = launch_bwd<256>(job, (unsigned)total, st); break;
+        case 64: rc = launch_bwd<64>(job, (int)total, st); break;
+        case 128: rc = launch_bwd<128>(job, (int)total, st); break;
+        default: rc = launch_bwd<256>(job, (int)total, st); break;
       }
       if (rc) return rc;
     }
@@ -967,17 +967,17 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
         static_cast<DwJob&>(dj) = job;
         dj.part = part;
         switch (tile_n) {
-          case 64: rc = launch_bwd<64>(dj, (unsigned)units, st); break;
-          case 128: rc = launch_bwd<128>(dj, (unsigned)units, st); break;
-          default: rc = launch_bwd<256>(dj, (unsigned)units, st); break;
+          case 64: rc = launch_bwd<64>(dj, (int)units, st); break;
+          case 128: rc = launch_bwd<128>(dj, (int)units, st); break;
+          default: rc = launch_bwd<256>(dj, (int)units, st); break;
         }
         if (rc) return rc;
         if ((rc = reduce_rows(part, K, m_tiles * n_tiles, 0, dW))) return rc;
       } else {
         switch (tile_n) {
-          case 64: rc = launch_bwd<64>(job, (unsigned)units, st); break;
-          case 128: rc = launch_bwd<128>(job, (unsigned)units, st); break;
-          default: rc = launch_bwd<256>(job, (unsigned)units, st); break;
+          case 64: rc = launch_bwd<64>(job, (int)units, st); break;
+          case 128: rc = launch_bwd<128>(job, (int)units, st); break;
+          default: rc = launch_bwd<256>(job, (int)units, st); break;
         }
         if (rc) return rc;
       }

@@ -6,8 +6,11 @@
 // tile: 3 tensor-core products at the bf16 rate instead of an fp32 FMA GEMM, error ~1e-5 relative —
 // far inside the 1e-3 parity bar, where a single bf16 or tf32 product would not be.
 //
-// k_typed_linear_tc runs tcp::split3_tile (tc_ptx.cuh): one 128 x BN output tile per CTA, a TMA producer warpgroup and two wgmma
-// consumer warpgroups, both operands K-major with SWIZZLE_128B.  Output tiles follow the same group / column-block tables
+// k_typed_linear_tc runs tcp::split3_tile (tc_ptx.cuh): a persistent grid of one CTA per SM walking the 128 x BN output tiles,
+// a TMA producer warpgroup and two wgmma consumer warpgroups, both operands K-major.  At BN = 128 / 256 the k-blocks are 32
+// wide (SWIZZLE_64B): at BN = 256 that makes a 4-deep ring of 48 KB stages instead of 2 x 96 KB.  BN = 64 keeps 64-wide
+// k-blocks (SWIZZLE_128B, 4 stages): its k-blocks are short enough that halving them costs more in barrier waits than the
+// deeper ring gains (measured on the d = 400 OAG shape).  Output tiles follow the same group / column-block tables
 // as the SIMT kernel in linear.cu.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -22,6 +25,7 @@ namespace {
 using namespace tcp;
 
 constexpr int kMaxGroups = 64;
+template <int BN> constexpr int fwd_bk() { return BN == 64 ? 64 : 32; }    // k-block of the forward GEMM
 
 // ---- fp32 -> (bf16 hi, bf16 lo) split ------------------------------------------------------------
 __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_t rows, int K, int Kp,
@@ -54,7 +58,7 @@ __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_
 // Rows of a tile past the group and columns past the column block are computed on neighbouring (or zero-filled) operand
 // rows and not stored.
 struct FwdJob {
-  CUtensorMap a_hi, a_lo, w_hi, w_lo;      // A box {64, 128 rows}, W box {64, tile_n rows}
+  CUtensorMap a_hi, a_lo, w_hi, w_lo;      // A box {fwd_bk, 128 rows}, W box {fwd_bk, tile_n rows}
   const float* bias;
   const hgt_lin_group* groups;
   const hgt_lin_cblock* cblocks;
@@ -95,30 +99,47 @@ struct FwdJob {
   }
   template <int BN>
   __device__ void load(const Tile& t, int kb, uint32_t sa, uint32_t bar) const {
-    tma_load_2d(sa, &a_hi, kb * BK, t.a_row, bar);
-    tma_load_2d(sa + A_BYTES, &a_lo, kb * BK, t.a_row, bar);
-    tma_load_2d(sa + 2 * A_BYTES, &w_hi, kb * BK, t.w_row, bar);
-    tma_load_2d(sa + 2 * A_BYTES + BN * BK * 2, &w_lo, kb * BK, t.w_row, bar);
+    constexpr int KB = fwd_bk<BN>();
+    constexpr uint32_t A = a_bytes<KB>();
+    const int k = kb * KB;
+    tma_load_2d(sa, &a_hi, k, t.a_row, bar);
+    tma_load_2d(sa + A, &a_lo, k, t.a_row, bar);
+    tma_load_2d(sa + 2 * A, &w_hi, k, t.w_row, bar);
+    tma_load_2d(sa + 2 * A + BN * KB * 2, &w_lo, k, t.w_row, bar);
   }
+  // Through shared memory, whole row segments per warp (tcp::store_staged).  cols is a multiple of 16, so a 4-column
+  // group is either inside the column block or past it.
   template <int BN>
-  __device__ void store(const Tile& t, const float* acc, int c, int wq, int lane) const {
+  __device__ void store(const Tile& t, const float* acc, float* stage, int c, int wq, int lane) const {
     float* o = t.out + (int64_t)(64 * c) * t.ld;
     const int64_t rows = t.rows - 64 * c;
     const float* b = t.bias;
     const int cols = t.cols;
     const int64_t ld = t.ld;
-    for_each_pair<BN>(acc, wq, lane, [&](int r, int col, float v0, float v1) {
-      if (r < rows && col < cols) {
-        if (b) v0 += __ldg(b + col), v1 += __ldg(b + col + 1);
-        *reinterpret_cast<float2*>(o + r * ld + col) = make_float2(v0, v1);
-      }
-    });
+    const bool vec4 = ((reinterpret_cast<uintptr_t>(o) | (uintptr_t)(ld * 4)) & 15) == 0;
+    store_staged<BN>(
+        acc, stage, c, wq, lane,
+        [&](int, int col, float v0, float v1) {
+          if (b && col < cols) v0 += __ldg(b + col), v1 += __ldg(b + col + 1);
+          return make_float2(v0, v1);
+        },
+        [&](int r, int col, float4 v) {
+          if (r < rows && col < cols) {
+            float* p = o + r * ld + col;
+            if (vec4) {
+              *reinterpret_cast<float4*>(p) = v;
+            } else {
+              *reinterpret_cast<float2*>(p) = make_float2(v.x, v.y);
+              *reinterpret_cast<float2*>(p + 2) = make_float2(v.z, v.w);
+            }
+          }
+        });
   }
 };
 
 template <int BN>
-__global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob job) {
-  split3_tile<BN, false>(job);
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob job, int n_tiles) {
+  split3_tile<BN, false, fwd_bk<BN>()>(job, n_tiles);
 }
 
 // ---- host side ------------------------------------------------------------------------------------
@@ -138,15 +159,16 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int make_map(CUtensorMap* m, const void* base, int64_t rows, int Kp, int box_rows) {
+int make_map(CUtensorMap* m, const void* base, int64_t rows, int Kp, int box_rows, int kb) {
   EncodeTiledFn fn = get_encode_fn();
   HGT_REQUIRE(fn != nullptr, "hgt_typed_linear: cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)Kp * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)kb, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, kb == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   HGT_REQUIRE(r == CUDA_SUCCESS, "hgt_typed_linear: cuTensorMapEncodeTiled failed (%d) rows=%lld Kp=%d box=%d",
               (int)r, (long long)rows, Kp, box_rows);
@@ -164,11 +186,20 @@ void extents(const hgt_lin_group* h_groups, int n_groups, int cb_width, int64_t*
   }
 }
 
+// The tensor maps and the k-block count follow the kernel's k-block, fwd_bk<BN>().
 template <int BN>
-int launch_fwd(const FwdJob& job, unsigned tiles, cudaStream_t st) {
-  const size_t smem = tile_smem_bytes<BN>();
+int launch_fwd(FwdJob& job, const __nv_bfloat16* const ops[4], int64_t a_rows, int64_t w_rows, int Kp, int tiles,
+               cudaStream_t st) {
+  constexpr int KB = fwd_bk<BN>();
+  int rc;
+  if ((rc = make_map(&job.a_hi, ops[0], a_rows, Kp, BM, KB))) return rc;
+  if ((rc = make_map(&job.a_lo, ops[1], a_rows, Kp, BM, KB))) return rc;
+  if ((rc = make_map(&job.w_hi, ops[2], w_rows, Kp, BN, KB))) return rc;
+  if ((rc = make_map(&job.w_lo, ops[3], w_rows, Kp, BN, KB))) return rc;
+  job.k_blocks = (Kp + KB - 1) / KB;
+  const size_t smem = tile_smem_bytes<BN, KB>();
   HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_typed_linear_tc<BN><<<tiles, TILE_THREADS, smem, st>>>(job);
+  k_typed_linear_tc<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -271,21 +302,16 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
   }
   job.first_tile[n_groups] = (int32_t)total;
   if (total == 0) return 0;
-  int rc;
-  if ((rc = make_map(&job.a_hi, a_hi, a_rows, Kp, BM))) return rc;
-  if ((rc = make_map(&job.a_lo, a_lo, a_rows, Kp, BM))) return rc;
-  if ((rc = make_map(&job.w_hi, w_hi, w_rows, Kp, job.tile_n))) return rc;
-  if ((rc = make_map(&job.w_lo, w_lo, w_rows, Kp, job.tile_n))) return rc;
   job.bias = bias;
   job.groups = groups;
   job.cblocks = cblocks;
   job.out = out;
   job.n_groups = n_groups;
   job.cb_width = cb_width;
-  job.k_blocks = (Kp + BK - 1) / BK;
+  const __nv_bfloat16* const ops[4] = {a_hi, a_lo, w_hi, w_lo};
   switch (job.tile_n) {
-    case 64: return launch_fwd<64>(job, (unsigned)total, st);
-    case 128: return launch_fwd<128>(job, (unsigned)total, st);
-    default: return launch_fwd<256>(job, (unsigned)total, st);
+    case 64: return launch_fwd<64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
+    case 128: return launch_fwd<128>(job, ops, a_rows, w_rows, Kp, (int)total, st);
+    default: return launch_fwd<256>(job, ops, a_rows, w_rows, Kp, (int)total, st);
   }
 }
