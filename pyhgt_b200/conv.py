@@ -67,6 +67,11 @@ class _PointerTable:
     def get(self, tensors, device):
         key = tuple(t.data_ptr() for t in tensors) + (str(device),)
         if key != self.key:
+            if torch.device(device).type == "cuda" and torch.cuda.is_current_stream_capturing():
+                # the rebuild is a pageable host copy: it cannot be captured, and a captured launch would keep reading
+                # the old table at every replay
+                raise _lib.HgtError("a parameter moved while a CUDA graph was being captured: run the step once eagerly "
+                                    "(warm-up) so the pointer tables match the parameters the graph will use")
             self.dev = torch.tensor([t.data_ptr() for t in tensors], dtype=torch.int64).to(device)
             self.key = key
         return self.dev

@@ -23,6 +23,7 @@
 #include <cuda_bf16.h>
 
 #include <stdlib.h>
+#include <string.h>
 #include <algorithm>
 #include <utility>
 #include <vector>
@@ -36,9 +37,37 @@ using namespace tcp;
 
 constexpr int kMaxGroups = 64;
 
-// Tensor maps are read from global memory (written by a host copy earlier on the stream): acquire them for the TMA proxy.
+// Tensor maps are read from global memory (written by k_upload earlier on the stream): acquire them for the TMA proxy.
 __device__ __forceinline__ void map_acquire(const CUtensorMap* m) {
   asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(m) : "memory");
+}
+
+// Host tables (task table, group offsets, tensor maps) reach the workspace by value in k_upload's parameter block, not
+// through a host-memory copy: a CUDA graph records kernel parameters when the launch is captured, so the backward can be
+// captured and replayed with no host buffer that has to outlive the call.  The block stays within the classic 4 KB
+// parameter limit.
+constexpr uint32_t kUploadBytes = 4096 - 16;
+struct UploadChunk {
+  unsigned char* dst;
+  uint32_t n;
+  alignas(16) unsigned char bytes[kUploadBytes];
+};
+static_assert(sizeof(UploadChunk) == 4096, "k_upload's parameter block must stay at 4 KB");
+
+__global__ void __launch_bounds__(256) k_upload(const __grid_constant__ UploadChunk c) {
+  for (uint32_t i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.bytes[i];
+}
+
+int upload_bytes(void* dst, const void* src, size_t bytes, cudaStream_t st) {
+  UploadChunk c{};
+  for (size_t o = 0; o < bytes; o += kUploadBytes) {
+    c.dst = static_cast<unsigned char*>(dst) + o;
+    c.n = (uint32_t)std::min(bytes - o, (size_t)kUploadBytes);
+    memcpy(c.bytes, static_cast<const unsigned char*>(src) + o, c.n);
+    k_upload<<<1, 256, 0, st>>>(c);
+    HGT_LAUNCH_CHECK();
+  }
+  return 0;
 }
 
 __device__ __forceinline__ float gelu_grad(float x) {
@@ -773,18 +802,25 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
   GcTask* d_tasks = reinterpret_cast<GcTask*>(base + L.off_tasks);
   int32_t* d_gt0 = reinterpret_cast<int32_t*>(base + L.off_gt0);
   int64_t* d_gfirst = reinterpret_cast<int64_t*>(base + L.off_gfirst);
-  auto upload_tasks = [&]() -> int {
-    HGT_CHECK_CUDA(cudaMemcpyAsync(d_tasks, tasks.data(), (size_t)nt * sizeof(GcTask), cudaMemcpyHostToDevice, st));
-    return 0;
+  auto upload_tasks = [&]() -> int { return upload_bytes(d_tasks, tasks.data(), (size_t)nt * sizeof(GcTask), st); };
+  // One upload of the contiguous workspace head [tensor maps (tensor cores only) | tasks | gt0 | gfirst]: the regions
+  // are laid out in that order by bwd_layout; the alignment gaps between them are written as zeros.
+  auto upload_head = [&](const std::vector<CUtensorMap>* maps) -> int {
+    const size_t begin = maps ? L.off_maps : L.off_tasks;
+    std::vector<unsigned char> img(L.off_gfirst + gfirst.size() * sizeof(int64_t) - begin, 0);
+    if (maps) memcpy(img.data(), maps->data(), maps->size() * sizeof(CUtensorMap));
+    memcpy(img.data() + (L.off_tasks - begin), tasks.data(), (size_t)nt * sizeof(GcTask));
+    memcpy(img.data() + (L.off_gt0 - begin), gt0.data(), gt0.size() * sizeof(int32_t));
+    memcpy(img.data() + (L.off_gfirst - begin), gfirst.data(), gfirst.size() * sizeof(int64_t));
+    return upload_bytes(base + begin, img.data(), img.size(), st);
   };
-  HGT_CHECK_CUDA(cudaMemcpyAsync(d_gt0, gt0.data(), gt0.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  HGT_CHECK_CUDA(cudaMemcpyAsync(d_gfirst, gfirst.data(), gfirst.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   int rc;
 
   if (!L.tc) {
     // ---------------- SIMT fp32 path ----------------
+    // the head carries the dX task table (first_unit unused there); dW uploads its own below
+    if ((rc = upload_head(nullptr))) return rc;
     if (dA && det) {
-      if ((rc = upload_tasks())) return rc;
       const int64_t n = L.a_rows * K;
       if (n > 0) {
         k_lin_dx_simt_det<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dout, W, d_tasks, d_gt0, groups, n_groups, L.a_rows,
@@ -793,7 +829,6 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
       }
     } else if (dA) {
       if (!accumulate_dA) HGT_CHECK_CUDA(cudaMemsetAsync(dA, 0, (size_t)L.a_rows * K * sizeof(float), st));
-      if ((rc = upload_tasks())) return rc;
       if (elems > 0) {
         k_lin_dx_simt<<<(unsigned)((elems + 255) / 256), 256, 0, st>>>(dout, W, d_tasks, d_gt0, groups, n_groups, d_gfirst, K,
                                                                        cb_width, gelu_aux, dA);
@@ -837,39 +872,8 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
   __nv_bfloat16* wt_hi = reinterpret_cast<__nv_bfloat16*>(base + L.off_wthi);
   __nv_bfloat16* wt_lo = reinterpret_cast<__nv_bfloat16*>(base + L.off_wtlo);
 
-  // 1. dOut split (+ db) unless the producer already split it
-  if (!have_dsplit) {
-    int64_t units = 0;
-    for (int t = 0; t < nt; ++t) {
-      tasks[t].first_unit = (int32_t)units;
-      tasks[t].n_chunks = (int32_t)((tasks[t].rows + SPLIT_ROWS - 1) / SPLIT_ROWS);
-      units += tasks[t].n_chunks;
-      HGT_REQUIRE(units < 2147483647ll, "hgt_typed_linear_bwd: too many units");
-    }
-    if ((rc = upload_tasks())) return rc;
-    if (units > 0 && det) {
-      k_split_colsum_det<<<(unsigned)units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo, db ? db_part : nullptr);
-      HGT_LAUNCH_CHECK();
-      if (db && (rc = reduce_rows(db_part, 1, 1, 1, db))) return rc;
-    } else if (units > 0) {
-      k_split_colsum<<<(unsigned)units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo, db);
-      HGT_LAUNCH_CHECK();
-    }
-  }
-  // 2. A split (dW needs it) unless saved by the forward
-  if (dW && !have_asplit && L.a_rows > 0) {
-    HGT_REQUIRE(A, "hgt_typed_linear_bwd: dW needs A or its bf16 split");
-    const int64_t n = L.a_rows * (K / 4);
-    k_act_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, L.a_rows, K, K, 0, nullptr, a_hi, a_lo);
-    HGT_LAUNCH_CHECK();
-  }
-  // 3. W^T split (dX)
-  if (dA) {
-    const int64_t n = (int64_t)K * L.wt_cols;
-    k_wt_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, L.w_rows, K, cb_width, L.wpad, L.wt_cols, wt_hi, wt_lo);
-    HGT_LAUNCH_CHECK();
-  }
-  // 4. tensor maps: per task dOut hi/lo {cols = width, rows = m}; per group A hi/lo {cols = K, rows = m}; W^T hi/lo
+  // 1. tensor maps: per task dOut hi/lo {cols = width, rows = m}; per group A hi/lo {cols = K, rows = m}; W^T hi/lo.
+  //    They encode addresses only, so they go up with the task table before any kernel runs.
   std::vector<CUtensorMap> maps(2 * nt + 2 * n_groups + 2);
   for (int t = 0; t < nt; ++t) {
     if ((rc = make_map2(&maps[2 * t], d_hi + tasks[t].out_off, tasks[t].rows, cb_width, tasks[t].ld, 64))) return rc;
@@ -884,7 +888,41 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
   if ((rc = make_map2(&maps[map_wt], wt_hi, K, L.wt_cols, L.wt_cols, bn_box))) return rc;
   if ((rc = make_map2(&maps[map_wt + 1], wt_lo, K, L.wt_cols, L.wt_cols, bn_box))) return rc;
   CUtensorMap* d_maps = reinterpret_cast<CUtensorMap*>(base + L.off_maps);
-  HGT_CHECK_CUDA(cudaMemcpyAsync(d_maps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice, st));
+  // the task table of the dOut split pass (the dX kernel reads only map indices / wt_col0 from it)
+  int64_t split_units = 0;
+  if (!have_dsplit) {
+    for (int t = 0; t < nt; ++t) {
+      tasks[t].first_unit = (int32_t)split_units;
+      tasks[t].n_chunks = (int32_t)((tasks[t].rows + SPLIT_ROWS - 1) / SPLIT_ROWS);
+      split_units += tasks[t].n_chunks;
+      HGT_REQUIRE(split_units < 2147483647ll, "hgt_typed_linear_bwd: too many units");
+    }
+  }
+  if ((rc = upload_head(&maps))) return rc;
+
+  // 2. dOut split (+ db) unless the producer already split it
+  if (split_units > 0 && det) {
+    k_split_colsum_det<<<(unsigned)split_units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo,
+                                                              db ? db_part : nullptr);
+    HGT_LAUNCH_CHECK();
+    if (db && (rc = reduce_rows(db_part, 1, 1, 1, db))) return rc;
+  } else if (split_units > 0) {
+    k_split_colsum<<<(unsigned)split_units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo, db);
+    HGT_LAUNCH_CHECK();
+  }
+  // 3. A split (dW needs it) unless saved by the forward
+  if (dW && !have_asplit && L.a_rows > 0) {
+    HGT_REQUIRE(A, "hgt_typed_linear_bwd: dW needs A or its bf16 split");
+    const int64_t n = L.a_rows * (K / 4);
+    k_act_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, L.a_rows, K, K, 0, nullptr, a_hi, a_lo);
+    HGT_LAUNCH_CHECK();
+  }
+  // 4. W^T split (dX)
+  if (dA) {
+    const int64_t n = (int64_t)K * L.wt_cols;
+    k_wt_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, L.w_rows, K, cb_width, L.wpad, L.wt_cols, wt_hi, wt_lo);
+    HGT_LAUNCH_CHECK();
+  }
 
   // 5. dX
   if (dA) {
@@ -911,8 +949,6 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
     }
     job.first_tile[n_groups] = (int32_t)total;
     if (total > 0) {
-      // the task table for dX only needs map indices / wt_col0 (already set); first_unit is unused here
-      if (have_dsplit && (rc = upload_tasks())) return rc;
       job.maps = d_maps;
       job.map_wt = map_wt;
       job.tasks = d_tasks;
@@ -949,7 +985,7 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
     }
     // the split / dX kernels enqueued above read the previous version of the table: stream order keeps them apart
     GcTask* d_tasks2 = d_tasks;
-    HGT_CHECK_CUDA(cudaMemcpyAsync(d_tasks2, tasks.data(), (size_t)nt * sizeof(GcTask), cudaMemcpyHostToDevice, st));
+    if ((rc = upload_tasks())) return rc;
     if (units > 0) {
       DwJob job;
       job.maps = d_maps;

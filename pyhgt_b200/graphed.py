@@ -8,11 +8,18 @@ is captured ONCE into a CUDA graph for a static *signature* — padded node coun
 because the plan build is sync-free when the host knows the signature (plan.get_plan(host_meta=...)): no read-back, tile
 counts stay on the device, grids are sized by upper bounds.
 
-Batches are padded to the signature on the host (vectorised numpy):
+Host batches are padded to the signature on the host (vectorised numpy, `pad_batch`); device batches (from
+`sample_subgraph(s)_cuda`, `to_torch(device=cuda)` or `merge_batches`) are scattered into the static buffers on the device
+by `hgt_merge_batches` with one member, their sizes read from the batch's cached plan, so they never visit the host.
+Either way:
   * nodes stay type-contiguous (the layout `to_torch` produces, data.py:232-235); type t gets `type_counts[t]` slots, real
     nodes first, the rest isolated zero-feature nodes whose output rows are dropped;
   * one extra node of out-of-range type closes the array; padding edges are self loops on it (they match no
     <source type, target type, relation> triple and their destination row is discarded), so they cannot touch a real row.
+
+GraphedForward replays an inference forward; GraphedTrainStep replays a whole training step (plan rebuild, forward, loss,
+backward, gradient clipping, optimizer step).  The backward's typed GEMMs carry their host-built tables in kernel
+parameters (csrc/linear_bwd.cu: k_upload), which is what lets a graph record them.
 """
 import numpy as np
 import torch
@@ -95,80 +102,323 @@ def pad_batch(sig, node_feature, node_type, edge_time, edge_index, edge_type, ou
     return x, sig.node_type, etm, ei, ety, new_id
 
 
-class GraphedForward:
+def _misfit(sig, counts, n_edges):
+    return ValueError("batch (type counts %s, %d edges) does not fit the signature (%s, %d edges) or has new "
+                      "<type, relation> pairs" % (list(counts), n_edges, sig.type_counts, sig.n_edges))
+
+
+def device_batch_sizes(sig, node_feature, node_type, edge_time, edge_index, edge_type):
+    """Per-type node counts and the edge count of a device batch (type-contiguous, the to_torch layout), read from its
+    cached plan like `merge_batches` does, so no device read-back.  Raises ValueError if the batch does not fit."""
+    T = sig.num_types
+    plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time, T, sig.num_relations)
+    if not plan.sorted_types or plan.type_count[T] != 0:
+        raise ValueError("graphed batches need type-contiguous nodes with types in [0, %d) (what to_torch emits)" % T)
+    counts = plan.type_count[:T]
+    if not sig.fits(counts, plan.n_edges, plan.pairs):
+        raise _misfit(sig, counts, plan.n_edges)
+    if (node_feature is None or node_feature.dtype != torch.float32 or node_feature.dim() != 2 or node_feature.shape[0] != plan.n_nodes
+            or node_feature.shape[1] != sig.feat_dim):
+        raise ValueError("node_feature must be float32 [%d, %d], got %s %s" % (plan.n_nodes, sig.feat_dim,
+                                                                            getattr(node_feature, "dtype", None),
+                                                                            tuple(getattr(node_feature, "shape", ()))))
+    return counts, plan.n_edges
+
+
+def _check_targets(spec, targets, counts, device):
+    """`targets` {type: tensor} against the declared {type: (trailing shape, dtype, fill)}: every declared type is given,
+    with at most as many rows as the batch has nodes of that type."""
+    targets = {} if targets is None else {int(t): v for t, v in targets.items()}
+    if set(targets) != set(spec):
+        raise ValueError("targets given for node types %s, declared for %s" % (sorted(targets), sorted(spec)))
+    for t, (shape, dtype, _) in spec.items():
+        y = targets[t]
+        if not isinstance(y, torch.Tensor) or y.dtype != dtype or tuple(y.shape[1:]) != shape:
+            raise ValueError("targets[%d] must be a %s tensor of shape [rows, %s]" % (t, dtype, ", ".join(map(str, shape))))
+        if y.shape[0] > counts[t]:
+            raise ValueError("targets[%d] has %d rows but the batch has %d nodes of type %d" % (t, y.shape[0], counts[t], t))
+        if y.is_cuda and y.device != device:
+            raise ValueError("targets[%d] is on %s, the graph runs on %s" % (t, y.device, device))
+    return targets
+
+
+class _Graphed:
+    """Static padded input buffers of one signature and the per-batch copy-in (host or device batches)."""
+
+    def __init__(self, sig, device):
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise _lib.HgtError("%s needs a CUDA device" % type(self).__name__)
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())    # "cuda" -> "cuda:<n>": compared with tensors' devices
+        self.sig, self.dev = sig, dev
+        i64 = dict(dtype=torch.int64, device=dev)
+        self.x = torch.zeros((sig.n_nodes, sig.feat_dim), dtype=torch.float32, device=dev)
+        self.nt = torch.from_numpy(sig.node_type).to(dev)                 # static
+        self.ei = torch.zeros((2, sig.n_edges), **i64)
+        self.et = torch.zeros(sig.n_edges, **i64)
+        self.tm = torch.zeros(sig.n_edges, **i64)
+        self.h = None                                                      # pinned staging, made by the first host batch
+        self.graph = None
+        self.plan = None
+        self._staged = None
+        self._pins = []
+        self.stream = torch.cuda.Stream(device=dev)
+
+    def _rebuild_plan(self):
+        s = self.sig
+        self.plan = _plan.rebuild_plan(self.nt, self.ei, self.et, self.tm if s.use_time else None, s.num_types,
+                                       s.num_relations, s.host_meta())
+
+    @staticmethod
+    def _is_device(batch):
+        return batch[1].is_cuda
+
+    def _sizes(self, batch):
+        """(per-type counts, n_edges) of a batch; device batches are checked against the signature here."""
+        if self._is_device(batch):
+            return device_batch_sizes(self.sig, *batch)
+        nt = batch[1].numpy()
+        T = self.sig.num_types
+        counts = np.bincount(nt[(nt >= 0) & (nt < T)], minlength=T)[:T] if nt.size else np.zeros(T, dtype=np.int64)
+        return counts.tolist(), int(batch[4].numel())
+
+    def _stage(self, batch):
+        """Host batch: pad it straight into the pinned staging buffers and enqueue the copies (node_type is static).
+        Returns the new index of every real node as a device tensor."""
+        if self._staged is not None:
+            self._staged.synchronize()                       # the previous batch's copies have left the staging buffers
+        if self.h is None:
+            self.h = [torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in (self.x, self.tm, self.ei, self.et)]
+        hx, htm, hei, het = self.h
+        new_id = pad_batch(self.sig, *batch, out=(hx.numpy(), htm.numpy(), hei.numpy(), het.numpy()))[5]
+        for h, dst in ((hx, self.x), (htm, self.tm), (hei, self.ei), (het, self.et)):
+            dst.copy_(h, non_blocking=True)
+        self._staged = torch.cuda.Event()
+        self._staged.record(self.stream)
+        return torch.from_numpy(new_id).pin_memory().to(self.dev, non_blocking=True)
+
+    def _scatter(self, batch, counts, n_edges):
+        """Device batch: hgt_merge_batches with this one member at union offsets sig.row0 writes the feature rows and the
+        remapped edges into the static buffers; the padding is stream-ordered fills.  Returns the new row of every real
+        node (a device tensor).  No host synchronisation."""
+        from . import sampler as _sampler
+        sig, T = self.sig, self.sig.num_types
+        nf, _, etime, ei, et = batch
+        n, E = int(sum(counts)), int(n_edges)
+        nf, ei, et = nf.contiguous(), ei.contiguous(), et.contiguous()
+        etime = torch.full((E,), 120, dtype=torch.int64, device=self.dev) if etime is None else etime.contiguous()
+        for t in (nf, ei, et, etime):
+            t.record_stream(self.stream)
+        mem = np.zeros(1, dtype=_sampler.MERGE_MEMBER_DTYPE)
+        mem[0] = (nf.data_ptr(), ei.data_ptr(), et.data_ptr(), etime.data_ptr(), n, E, 0, 0)
+        up = _sampler._Upload()
+        up.add("mem", mem.view(np.int64))
+        up.add("loc_off", np.concatenate([[0], np.cumsum(counts)]).astype(np.int64))
+        up.add("uoff", sig.row0[:T])
+        d = up.to(self.dev)
+        rows = torch.empty(n, dtype=torch.int64, device=self.dev)
+        self.x.zero_()
+        _lib.call("hgt_merge_batches", d.ptr("mem"), 1, T, d.ptr("loc_off"), d.ptr("uoff"), n, E, sig.n_edges,
+                  sig.feat_dim, self.nt.data_ptr(), self.x.data_ptr(), rows.data_ptr(), self.ei.data_ptr(),
+                  self.et.data_ptr(), self.tm.data_ptr(), self.stream.cuda_stream)
+        self.ei[:, E:].fill_(sig.n_nodes - 1)
+        self.et[E:].zero_()
+        self.tm[E:].fill_(120)
+        return rows
+
+    def _feed(self, batch, sizes):
+        return self._scatter(batch, *sizes) if self._is_device(batch) else self._stage(batch)
+
+    def _capture(self, fn):
+        """Capture fn() on self.stream; the table uploads captured in it re-read their pinned sources at every replay, so
+        those are kept (self._pins)."""
+        self.stream.synchronize()
+        _plan._PIN_KEEP = self._pins
+        try:
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, stream=self.stream):
+                out = fn()
+        finally:
+            _plan._PIN_KEEP = None
+        self.graph = graph
+        return out
+
+
+class GraphedForward(_Graphed):
     """Capture `fn(node_feature, node_type, edge_time, edge_index, edge_type) -> [N, d]` (an HGTConv / GNN forward under
     no_grad; note GNN's argument order, model.py:69) for one signature and replay it per batch.
 
         sig = GraphSignature(type_counts=[...], n_edges=..., pairs=[...], num_relations=R, feat_dim=F)
         g = GraphedForward(lambda x, nt, tm, ei, et: gnn(x, nt, tm, ei, et), sig, device)
-        out = g(node_feature, node_type, edge_time, edge_index, edge_type)     # host tensors of one batch
+        out = g(node_feature, node_type, edge_time, edge_index, edge_type)     # one batch, host or device tensors
     """
 
     def __init__(self, fn, sig, device):
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise _lib.HgtError("GraphedForward needs a CUDA device")
-        self.fn, self.sig, self.dev = fn, sig, dev
-        i64 = dict(dtype=torch.int64, device=dev)
-        self.x = torch.zeros((sig.n_nodes, sig.feat_dim), dtype=torch.float32, device=dev)
-        self.nt = torch.zeros(sig.n_nodes, **i64)
-        self.ei = torch.zeros((2, sig.n_edges), **i64)
-        self.et = torch.zeros(sig.n_edges, **i64)
-        self.tm = torch.zeros(sig.n_edges, **i64)
-        # pinned staging for the per-batch copies
-        self.h = [torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in (self.x, self.nt, self.tm, self.ei, self.et)]
-        self.graph = None
+        super().__init__(sig, device)
+        self.fn = fn
         self.out = None
-        self.plan = None
-        self._staged = None
-        self._nt_done = False
-        self._pins = []
-        self.stream = torch.cuda.Stream(device=dev)
 
     def _run(self):
-        s = self.sig
-        self.plan = _plan.rebuild_plan(self.nt, self.ei, self.et, self.tm if s.use_time else None, s.num_types,
-                                       s.num_relations, s.host_meta())
+        self._rebuild_plan()
         with torch.no_grad():
             return self.fn(self.x, self.nt, self.tm, self.ei, self.et)
 
-    def _stage(self, batch):
-        """Pad the batch straight into the pinned staging buffers and enqueue the copies (node_type is static)."""
-        if self._staged is not None:
-            self._staged.synchronize()                       # the previous batch's copies have left the staging buffers
-        hx, hnt, htm, hei, het = self.h
-        out = (hx.numpy(), htm.numpy(), hei.numpy(), het.numpy())
-        new_id = pad_batch(self.sig, *batch, out=out)[5]
-        if not self._nt_done:
-            hnt.copy_(torch.from_numpy(self.sig.node_type))
-            self.nt.copy_(hnt, non_blocking=True)
-            self._nt_done = True
-        for h, dst in ((hx, self.x), (htm, self.tm), (hei, self.ei), (het, self.et)):
-            dst.copy_(h, non_blocking=True)
-        self._staged = torch.cuda.Event()
-        self._staged.record(self.stream)
-        return new_id
-
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type):
+        batch = (node_feature, node_type, edge_time, edge_index, edge_type)
         cur = torch.cuda.current_stream(self.dev)
         self.stream.wait_stream(cur)
         with torch.cuda.stream(self.stream):
-            new_id = self._stage((node_feature, node_type, edge_time, edge_index, edge_type))
+            idx = self._feed(batch, self._sizes(batch))
             if self.graph is None:
                 for _ in range(2):                          # eager warm-up: pointer tables, pinned-block cache
                     self._run()
-                self.stream.synchronize()
-                # the table uploads captured below re-read their pinned sources at every replay: keep them (self._pins)
-                _plan._PIN_KEEP = self._pins
-                try:
-                    self.graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(self.graph, stream=self.stream):
-                        self.out = self._run()
-                finally:
-                    _plan._PIN_KEEP = None
+                self.out = self._capture(self._run)
             self.graph.replay()
-            idx = torch.from_numpy(new_id).pin_memory().to(self.dev, non_blocking=True)
             res = self.out.index_select(0, idx)
         cur.wait_stream(self.stream)
         res.record_stream(cur)
         return res
+
+
+class GraphedTrainStep(_Graphed):
+    """One training step captured in a CUDA graph for one signature and replayed per batch:
+
+        step = GraphedTrainStep(loss_fn, sig, device, optimizer=opt, clip_norm=1.0,
+                                targets={paper_t: ((), torch.int64, -100)})
+        loss, *aux = step(node_feature, node_type, edge_time, edge_index, edge_type, targets={paper_t: y})
+
+    `loss_fn(x, node_type, edge_time, edge_index, edge_type, targets)` runs on the static padded tensors (real rows of
+    type t at sig.row0[t] + i; `targets[t]` is the static [sig.type_counts[t], *shape] buffer: the call's rows first, the
+    rest `fill`) and returns the loss or (loss, *aux).  The graph holds the plan rebuild, the forward, the loss, its
+    backward, then clip_grad_norm_(params, clip_norm, foreach=True) if clip_norm is given and optimizer.step() if an
+    optimizer is given.  Batches are host or device tensors, as for GraphedForward.
+
+    Every call makes exactly one update on its batch.  The first call warms up (two forward/backward passes: parameters
+    and optimizer state stay untouched, but the RNG advances and module buffers such as BatchNorm running statistics see
+    the batch), runs its real step eagerly on the static buffers (which creates the optimizer state) and then captures;
+    later calls replay.  If that capture fails, the call raises after its update and the object refuses further calls.  The returned tensors are static (the next call overwrites them) and
+    the call does not synchronise with the host.  Without an optimizer the gradients land in `.grad` of `params`: static
+    tensors written afresh by every call (no accumulation across calls).
+
+    The optimizer must be built with capturable=True in every group; a learning-rate scheduler works when `lr` is a
+    tensor (the schedulers fill_ it in place).  Every other hyperparameter is baked into the graph at capture: a later
+    call raises RuntimeError if one of them changed (OneCycleLR's default cycle_momentum=True rewrites `betas` every
+    step; use cycle_momentum=False).  Dropout draws new masks at every replay.  The deterministic-algorithms
+    flag is frozen at the first call: a later call with the flag changed raises RuntimeError.  A batch that does not fit
+    the signature raises ValueError before anything is copied."""
+
+    def __init__(self, loss_fn, sig, device, optimizer=None, clip_norm=None, targets=None, params=None):
+        if optimizer is not None:
+            for g in optimizer.param_groups:
+                if not g.get("capturable", False):
+                    raise ValueError("GraphedTrainStep needs an optimizer built with capturable=True in every param group")
+        if params is None:
+            if optimizer is None:
+                raise ValueError("GraphedTrainStep needs `params` (the tensors to differentiate) or an optimizer")
+            params = [p for g in optimizer.param_groups for p in g["params"]]
+        if clip_norm is not None and not clip_norm > 0:
+            raise ValueError("clip_norm must be positive, got %r" % (clip_norm,))
+        spec = {}
+        for t, (shape, dtype, fill) in (targets or {}).items():
+            t = int(t)
+            if not 0 <= t < sig.num_types:
+                raise ValueError("targets: node type %d outside [0, %d)" % (t, sig.num_types))
+            if not isinstance(dtype, torch.dtype):
+                raise ValueError("targets[%d]: dtype must be a torch.dtype, got %r" % (t, dtype))
+            spec[t] = (tuple(int(v) for v in shape), dtype, fill)
+        super().__init__(sig, device)
+        self.loss_fn, self.optimizer, self.clip_norm = loss_fn, optimizer, clip_norm
+        self.params = [p for p in params if p.requires_grad]
+        self.spec = spec
+        self.y = {t: torch.full((sig.type_counts[t],) + shape, fill, dtype=dtype, device=self.dev)
+                  for t, (shape, dtype, fill) in spec.items()}
+        self.det = None
+        self.hyper = None
+        self.out = None
+        self.capture_failed = False
+
+    def _hyperparameters(self):
+        """The optimizer's per-group hyperparameters that a captured step holds by value (tensors are read at replay)."""
+        if self.optimizer is None:
+            return []
+        return [{k: v for k, v in g.items() if k != "params" and not isinstance(v, torch.Tensor)
+                 and not (isinstance(v, (tuple, list)) and any(isinstance(e, torch.Tensor) for e in v))}
+                for g in self.optimizer.param_groups]
+
+    def _copy_targets(self, targets):
+        for t, y in targets.items():
+            buf = self.y[t]
+            r = y.shape[0]
+            buf[r:].fill_(self.spec[t][2])
+            if r:
+                buf[:r].copy_(y if y.is_cuda else y.pin_memory(), non_blocking=True)
+
+    def _forward_backward(self):
+        self._rebuild_plan()
+        res = self.loss_fn(self.x, self.nt, self.tm, self.ei, self.et, self.y)
+        res = tuple(res) if isinstance(res, (tuple, list)) else (res,)
+        res[0].backward()
+        return tuple(r.detach() for r in res)
+
+    def _step(self):
+        res = self._forward_backward()
+        if self.clip_norm is not None:
+            torch.nn.utils.clip_grad_norm_(self.params, self.clip_norm, foreach=True)
+        if self.optimizer is not None:
+            self.optimizer.step()
+        return res
+
+    def _first_call(self):
+        for p in self.params:
+            p.grad = None
+        for _ in range(2):                                  # warm-up: pointer tables, pinned-block cache; no update
+            self._forward_backward()
+            for p in self.params:
+                p.grad = None
+        eager = self._step()                                # this call's update, eagerly (creates the optimizer state)
+        grads = [p.grad for p in self.params]
+        for p in self.params:
+            p.grad = None                                   # the graph allocates its own static .grad tensors
+        try:
+            self.out = self._capture(self._step)
+        except Exception:
+            self.capture_failed = True          # the update is done: a retry must not make a second one
+            raise
+        for o, e in zip(self.out, eager):
+            o.copy_(e)
+        for p, g in zip(self.params, grads):
+            if p.grad is not None and g is not None:
+                p.grad.copy_(g)
+
+    def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type, targets=None):
+        if self.capture_failed:
+            raise RuntimeError("the first call of this GraphedTrainStep made its update but failed to capture the step; "
+                               "build a new one")
+        det = torch.are_deterministic_algorithms_enabled()
+        if self.graph is not None and det != self.det:
+            raise RuntimeError("GraphedTrainStep was captured with torch deterministic algorithms %s: the flag cannot "
+                               "change afterwards" % ("on" if self.det else "off"))
+        if self.graph is not None:
+            hyper = self._hyperparameters()
+            if hyper != self.hyper:
+                changed = sorted({k for a, b in zip(hyper, self.hyper) for k in set(a) | set(b) if a.get(k) != b.get(k)})
+                raise RuntimeError("optimizer hyperparameters %s changed after the step was captured: the graph holds "
+                                   "their captured values (keep them fixed, or make them tensors updated in place)"
+                                   % changed)
+        batch = (node_feature, node_type, edge_time, edge_index, edge_type)
+        cur = torch.cuda.current_stream(self.dev)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            sizes = self._sizes(batch)
+            targets = _check_targets(self.spec, targets, sizes[0], self.dev)
+            self._feed(batch, sizes)
+            self._copy_targets(targets)
+            if self.graph is None:
+                self.det = det
+                self._first_call()
+                self.hyper = self._hyperparameters()
+            else:
+                self.graph.replay()
+        cur.wait_stream(self.stream)
+        return self.out
