@@ -198,6 +198,17 @@ int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W
                               int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                               int32_t n_groups, const hgt_lin_cblock* cblocks, float* out,
                               void* workspace, size_t workspace_bytes, void* stream);
+/* The same two products with a bf16 output: `out` is bf16 and the column blocks' out_off / ld count bf16 elements.  Same
+ * tiles, k order and bias add as the fp32 call; each fp32 result is rounded to nearest-even once when it is stored, so
+ * the output equals the fp32 call's output converted to bf16, bitwise.  Workspaces: the fp32 calls' queries. */
+int hgt_typed_linear_bf16(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                          int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                          int32_t n_groups, const hgt_lin_cblock* cblocks, void* out, int32_t impl,
+                          void* workspace, size_t workspace_bytes, void* stream);
+int hgt_typed_linear_presplit_bf16(const void* a_hi, const void* a_lo, const float* W, const float* bias, int32_t K,
+                                   int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                   int32_t n_groups, const hgt_lin_cblock* cblocks, void* out,
+                                   void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused edge kernel: gather -> relation-specific score -> softmax by destination -> weighted sum
@@ -269,6 +280,37 @@ int hgt_edge_backward_rows(const float* q, const float* dagg, const float* stats
                            int32_t n_split, const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads,
                            float* grad, void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
                            void* stream);
+
+/* The edge forward and the three backward passes on bf16 gather tables: kv [rows+1, 2d] and kvr [P*240+1, 2d] (own /
+ * oth for the row pass) hold bf16 elements and are widened to fp32 in registers; q, agg, dagg, stats, att and every
+ * output and gradient (dq, dkv, dkvr, grad, D) stay fp32 in the layouts of the fp32 calls.  Arguments, workspaces,
+ * supported shapes and the TMA / LDG choice (row bytes, now 4d, % 16) as for the fp32 calls. */
+int hgt_edge_forward_bf16(const float* q, const void* kv, const void* kvr,
+                          const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                          const int32_t* csr_eid, const int32_t* tiles, int32_t n_tiles, int32_t n_split_tiles,
+                          const int32_t* hubs, int32_t n_hubs,
+                          int64_t n_nodes, int64_t n_edges, int32_t d, int32_t n_heads, int32_t apply_gelu,
+                          float* agg_out, float* att_out, float* stats_out, void* g_hi, void* g_lo,
+                          void* workspace, size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
+                          const int32_t* type_row0, int32_t num_types, const int32_t* type_active, void* stream);
+int hgt_edge_backward_bf16(const float* q, const void* kv, const void* kvr, const float* agg, const float* dagg,
+                           const float* stats, const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                           const int32_t* tiles, int32_t n_tiles, int64_t n_nodes, int32_t d, int32_t n_heads,
+                           int64_t kv_rows_total, int64_t kvr_rows_total,
+                           float* dq, float* dkv, float* dkvr, void* workspace, size_t workspace_bytes,
+                           const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_dst_bf16(const float* q, const void* kv, const void* kvr, const float* agg, const float* dagg,
+                               const float* stats, const int32_t* row_ptr, const int32_t* kv_row,
+                               const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
+                               const int32_t* hubs, int32_t n_hubs, int64_t n_nodes, int32_t d, int32_t n_heads,
+                               float* dq, float* D, void* workspace, size_t workspace_bytes,
+                               const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_rows_bf16(const float* q, const float* dagg, const float* stats, const float* D, const void* own,
+                                const void* oth, const int32_t* src_ptr, const int32_t* src_dst,
+                                const int32_t* src_oth, int32_t n_rows, int64_t own_rows_total, const int32_t* tiles,
+                                int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs, int32_t d,
+                                int32_t n_heads, float* grad, void* workspace, size_t workspace_bytes,
+                                const int32_t* d_tile_counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Backward of the typed linears (training path).  For the group / column-block tables of the forward call:

@@ -66,6 +66,17 @@ SIGNATURES = {
     "hgt_update_backward_det": [_p, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_fold_backward_det": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p,
                               _p, _p, _p, _p, _p, _p],
+    # bf16 gather tables (HGT layers under torch.autocast(dtype=torch.bfloat16)): same arguments as the fp32 twins
+    "hgt_typed_linear_bf16": [_p, _i64, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i32, _p, _sz, _p],
+    "hgt_typed_linear_presplit_bf16": [_p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _p, _sz, _p],
+    "hgt_edge_forward_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i64, _i32, _i32, _i32, _p, _p,
+                              _p, _p, _p, _p, _sz, _i32, _p, _p, _i32, _p, _p],
+    "hgt_edge_backward_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, _i64, _i64, _p, _p, _p, _p,
+                               _sz, _p, _p],
+    "hgt_edge_backward_dst_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32, _i32, _p, _p,
+                                   _p, _sz, _p, _p],
+    "hgt_edge_backward_rows_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _p, _i32, _i32, _p, _i32, _i32, _i32,
+                                    _p, _p, _sz, _p, _p],
     # HGSampling on the GPU (sampler.sample_subgraph_cuda)
     "hgt_gsample_add_budget_workspace_bytes": [_i64, _i32, _i64, _c.POINTER(_sz)],
     "hgt_gsample_add_budget": [_p, _p, _i32, _p, _p, _i64, _p, _i64, _i32, _i64, _i64, _c.c_uint64, _i64, _p, _p, _sz,

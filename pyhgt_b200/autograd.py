@@ -21,6 +21,12 @@ forward and its backward calls the deterministic twins instead: hgt_edge_backwar
 source-major second pass that owns every K'/V' and RTE gradient row, plan.source_index), hgt_typed_linear_bwd_det,
 hgt_update_backward_det and hgt_fold_backward_det.  They use no float atomics, so two identical steps give bitwise equal
 gradients.  With the flag off nothing changes.
+
+Under ``torch.autocast("cuda", dtype=torch.bfloat16)`` (bf16_tables()) the two gathered tables, [K'|V'] and the RTE table
+KVR, are stored in bf16: the projection writes Q by its own fp32 call and the K'/V' blocks straight into the bf16 table
+(hgt_typed_linear[_presplit]_bf16, rounded once from the fp32 accumulator), and the edge kernels read them through their
+_bf16 entry points.  The layer output, att, the softmax statistics, Q and every gradient stay fp32; the stages record the
+switch on ctx, so the backward follows the forward.  fp16 autocast keeps fp32 tables.
 """
 import ctypes
 
@@ -35,57 +41,91 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def bf16_tables():
+    """The switch for bf16 gather tables, read once per layer forward: bf16 autocast on CUDA."""
+    return torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
+
+
 def _tc_shape_ok(K, width):
     """Shapes both the tensor-core forward (hgt_typed_linear_presplit) and backward (hgt_typed_linear_bwd) take."""
     return K % 16 == 0 and K >= 64 and width % 16 == 0
 
 
 class _TypedLinear(torch.autograd.Function):
-    """out_flat[cblock c of group g][m, :] = act(A)[rows_g] @ W_cat[rows of (g, c)]^T + b_cat   (act: 0 none, 1 gelu)."""
+    """out_flat[cblock c of group g][m, :] = act(A)[rows_g] @ W_cat[rows of (g, c)]^T + b_cat   (act: 0 none, 1 gelu).
+
+    tables16 (bf16 gather tables) = (q_table or None, q_elems, kv_table, kv_off, kv_zero_ranges): the same product split
+    into an fp32 Q buffer [q_elems] (q_table) and a bf16 table [out_elems - kv_off] (kv_table, offsets relative to kv_off,
+    zero ranges relative to it too).  The forward then returns (stand-in, q, table): the stand-in is a zero-stride fp32
+    tensor of out_elems that only carries the gradient, which arrives in the flat layout of the fp32 output, so the
+    backward is the same."""
 
     @staticmethod
-    def forward(ctx, a, w_cat, b_cat, table, width, out_elems, impl, act, zero_ranges):
-        g_dev, g_host, n_g, c_dev = table
+    def forward(ctx, a, w_cat, b_cat, table, width, out_elems, impl, act, zero_ranges, tables16=None):
         a = a.contiguous()
         w_cat = w_cat.contiguous()
         rows, K = a.shape
         dev = a.device
         st = _stream()
-        out = torch.empty(out_elems, dtype=torch.float32, device=dev)
-        for (z0, z1) in zero_ranges:                                   # padding / all-zero table rows only
-            if z1 > z0:
-                out[z0:z1].zero_()
+        if tables16 is None:
+            out = torch.empty(out_elems, dtype=torch.float32, device=dev)
+            for (z0, z1) in zero_ranges:                               # padding / all-zero table rows only
+                if z1 > z0:
+                    out[z0:z1].zero_()
+        else:
+            q_table, q_elems, kv_table, kv_off, kv_zero = tables16
+            q = torch.empty(q_elems, dtype=torch.float32, device=dev) if q_table is not None else None
+            kv = torch.empty(out_elems - kv_off, dtype=torch.bfloat16, device=dev)
+            for (z0, z1) in kv_zero:
+                if z1 > z0:
+                    kv[z0:z1].zero_()
         use_tc = impl in (0, 2) and _tc_shape_ok(K, width)
         hi = lo = a_act = None
-        wsb = ctypes.c_size_t()
         if use_tc:
             hi = torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
             lo = torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
             _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, None, hi.data_ptr(), lo.data_ptr(), st)
-            _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, K, width, ctypes.byref(wsb))
-            ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-            _lib.call("hgt_typed_linear_presplit", hi.data_ptr(), lo.data_ptr(), w_cat.data_ptr(), _lib.ptr(b_cat), K, width,
-                      g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), out.data_ptr(), ws.data_ptr(),
-                      ws.numel(), st)
         else:
             a_act = a
             if act:
                 a_act = torch.empty_like(a)
                 _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, a_act.data_ptr(), None, None, st)
-            _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, K, width, 1, ctypes.byref(wsb))
-            ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-            _lib.call("hgt_typed_linear", a_act.data_ptr(), K, w_cat.data_ptr(), _lib.ptr(b_cat), K, width,
-                      g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), out.data_ptr(), 1, ws.data_ptr(),
-                      ws.numel(), st)
+
+        def gemm(tab, dst):
+            g_dev, g_host, n_g, c_dev = tab
+            sfx = "_bf16" if dst.dtype == torch.bfloat16 else ""
+            wsb = ctypes.c_size_t()
+            if use_tc:
+                _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, K, width, ctypes.byref(wsb))
+                ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+                _lib.call("hgt_typed_linear_presplit" + sfx, hi.data_ptr(), lo.data_ptr(), w_cat.data_ptr(),
+                          _lib.ptr(b_cat), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(),
+                          dst.data_ptr(), ws.data_ptr(), ws.numel(), st)
+            else:
+                _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, K, width, 1, ctypes.byref(wsb))
+                ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+                _lib.call("hgt_typed_linear" + sfx, a_act.data_ptr(), K, w_cat.data_ptr(), _lib.ptr(b_cat), K, width,
+                          g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), dst.data_ptr(), 1, ws.data_ptr(),
+                          ws.numel(), st)
+
+        if tables16 is None:
+            gemm(table, out)
+        else:
+            if q is not None:
+                gemm(q_table, q)
+            gemm(kv_table, kv)
         ctx.table, ctx.width, ctx.has_bias, ctx.act, ctx.use_tc = table, width, b_cat is not None, act, use_tc
         ctx.out_elems = out_elems
         ctx.det = torch.are_deterministic_algorithms_enabled()
         # gelu'(a) needs the un-activated input; the dW product needs act(a): as the bf16 split (tensor cores) or fp32
         ctx.save_for_backward(a if (act or not use_tc) else None, a_act if (act and not use_tc) else None, hi, lo, w_cat)
-        return out
+        if tables16 is None:
+            return out
+        ctx.mark_non_differentiable(*[t for t in (q, kv) if t is not None])
+        return torch.zeros(1, dtype=torch.float32, device=dev).expand(out_elems), q, kv
 
     @staticmethod
-    def backward(ctx, dout):
+    def backward(ctx, dout, *_unused):
         a, a_act, hi, lo, w_cat = ctx.saved_tensors
         width = ctx.width
         K = w_cat.shape[1]
@@ -122,29 +162,34 @@ class _TypedLinear(torch.autograd.Function):
                       _lib.ptr(lo), w_cat.data_ptr(), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g,
                       c_host.ctypes.data, _lib.ptr(da), int(ti > 0), a.data_ptr() if ctx.act else None, dw.data_ptr(),
                       _lib.ptr(db), impl, ws.data_ptr(), ws.numel(), _stream())
-        return da, dw, db, None, None, None, None, None, None
+        return da, dw, db, None, None, None, None, None, None, None
 
 
 class _EdgeAttention(torch.autograd.Function):
     """agg[i] = sum_{e -> i} softmax_i(<Q[i], K'[e]>) * V'[e]   (conv.py:99,108-111 + scatter-add).  Takes and returns
     the FLAT projection buffer (Q at q_off, the [K'|V'] table at kv_off): its gradient is produced as one buffer, so
-    autograd never assembles it from slices."""
+    autograd never assembles it from slices.  tables16 (bf16 gather tables): (Q, bf16 [K'|V'] table, bf16 RTE table or
+    None) from _TypedLinear; proj / kvr are then its stand-ins and receive the fp32 gradients in the same layouts."""
 
     @staticmethod
-    def forward(ctx, proj, kvr, plan, lt, d, n_heads, want_att, variant):
+    def forward(ctx, proj, kvr, plan, lt, d, n_heads, want_att, variant, tables16=None):
         N = plan.n_nodes
         dev = proj.device
-        proj = proj.contiguous()
-        q = proj[lt.q_off:lt.q_off + N * d]
-        kv = proj[lt.kv_off:]
+        ctx.bf16 = tables16 is not None
+        if ctx.bf16:
+            q, kv, kvr = tables16
+        else:
+            proj = proj.contiguous()
+            q = proj[lt.q_off:lt.q_off + N * d]
+            kv = proj[lt.kv_off:]
+            kvr = None if kvr is None else kvr.contiguous()
         ws_bytes = ctypes.c_size_t()
         _lib.call("hgt_edge_workspace_bytes", plan.n_split, d, n_heads, ctypes.byref(ws_bytes))
         ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
         agg = torch.empty((N, d), dtype=torch.float32, device=dev)
         stats = torch.empty((N, 2 * n_heads), dtype=torch.float32, device=dev)
         att = torch.empty((plan.n_edges, n_heads), dtype=torch.float32, device=dev) if want_att else None
-        kvr = None if kvr is None else kvr.contiguous()
-        _lib.call("hgt_edge_forward", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
+        _lib.call("hgt_edge_forward_bf16" if ctx.bf16 else "hgt_edge_forward", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
                   plan.kv_row.data_ptr(), None if kvr is None else plan.rte_row.data_ptr(), plan.csr_eid.data_ptr(),
                   plan.tiles.data_ptr(), plan.n_tiles, plan.n_split, plan.hubs.data_ptr(), plan.n_hubs, N, plan.n_edges, d,
                   n_heads, 0, agg.data_ptr(), _lib.ptr(att), stats.data_ptr(), None, None, ws.data_ptr(), ws.numel(),
@@ -152,41 +197,42 @@ class _EdgeAttention(torch.autograd.Function):
                   _lib.ptr(lt.type_active_dev), _stream())
         ctx.plan, ctx.lt, ctx.d, ctx.n_heads, ctx.has_kvr = plan, lt, d, n_heads, kvr is not None
         ctx.det = torch.are_deterministic_algorithms_enabled()
-        ctx.save_for_backward(proj, kvr, agg, stats)
+        ctx.proj_elems = proj.numel()
+        ctx.save_for_backward(q, kv, kvr, agg, stats)
         if att is not None:
             ctx.mark_non_differentiable(att)
         return agg, att
 
     @staticmethod
     def backward(ctx, dagg, _datt=None):
-        proj, kvr, agg, stats = ctx.saved_tensors
+        q, kv, kvr, agg, stats = ctx.saved_tensors
         plan, lt, d, H = ctx.plan, ctx.lt, ctx.d, ctx.n_heads
         N = plan.n_nodes
-        q = proj[lt.q_off:lt.q_off + N * d]
-        kv = proj[lt.kv_off:]
-        dproj = torch.empty_like(proj)                                 # hgt_edge_backward zero-initialises dq / dkv
+        f32 = dict(dtype=torch.float32, device=q.device)
+        dproj = torch.empty(ctx.proj_elems, **f32)                     # hgt_edge_backward zero-initialises dq / dkv
         if lt.kv_off > N * d:
             dproj[N * d:lt.kv_off].zero_()                             # alignment gap
         dq = dproj[lt.q_off:lt.q_off + N * d]
         dkv = dproj[lt.kv_off:]
-        dkvr = torch.empty_like(kvr) if kvr is not None else None
+        dkvr = torch.empty(kvr.numel(), **f32) if kvr is not None else None
         dagg = dagg.contiguous()
+        sfx = "_bf16" if ctx.bf16 else ""
         if ctx.det:
-            _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr)
-            return dproj, dkvr, None, None, None, None, None, None
-        ws = torch.empty(256, dtype=torch.uint8, device=proj.device)
-        _lib.call("hgt_edge_backward", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
+            _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx)
+            return dproj, dkvr, None, None, None, None, None, None, None
+        ws = torch.empty(256, dtype=torch.uint8, device=q.device)
+        _lib.call("hgt_edge_backward" + sfx, q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
                   stats.data_ptr(), plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
                   None if kvr is None else plan.rte_row.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, N, d, H,
                   plan.kv_rows + 1, 0 if kvr is None else kvr.numel() // (2 * d),
                   dq.data_ptr(), dkv.data_ptr(), _lib.ptr(dkvr), ws.data_ptr(), ws.numel(),
                   _lib.ptr(plan.tile_counts_dev), _stream())
-        return dproj, dkvr, None, None, None, None, None, None
+        return dproj, dkvr, None, None, None, None, None, None, None
 
 
-def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr):
+def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx=""):
     """Deterministic edge backward: destination pass (dq, D), then one row pass over the [K'|V'] rows and, with RTE, one
-    over the RTE rows; each gradient row is written once by its owner."""
+    over the RTE rows; each gradient row is written once by its owner.  sfx "_bf16": bf16 kv / kvr tables."""
     N = plan.n_nodes
     st = _stream()
     kvi = _plan.source_index(plan, "kv")
@@ -196,7 +242,7 @@ def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr):
     _lib.call("hgt_edge_backward_det_workspace_bytes", plan.n_split, max(kvi.n_split, rti.n_split if rti else 0), d,
               ctypes.byref(wsb))
     ws = torch.empty(wsb.value, dtype=torch.uint8, device=q.device)
-    _lib.call("hgt_edge_backward_dst", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
+    _lib.call("hgt_edge_backward_dst" + sfx, q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
               stats.data_ptr(), plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
               None if kvr is None else plan.rte_row.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, plan.n_split,
               plan.hubs.data_ptr(), plan.n_hubs, N, d, H, dq.data_ptr(), D.data_ptr(), ws.data_ptr(), ws.numel(),
@@ -205,7 +251,7 @@ def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr):
     if kvr is not None:
         passes.append((kvr, kv, rti, kvr.numel() // (2 * d), dkvr))
     for own, oth, idx, own_rows, grad in passes:
-        _lib.call("hgt_edge_backward_rows", q.data_ptr(), dagg.data_ptr(), stats.data_ptr(), D.data_ptr(), own.data_ptr(),
+        _lib.call("hgt_edge_backward_rows" + sfx, q.data_ptr(), dagg.data_ptr(), stats.data_ptr(), D.data_ptr(), own.data_ptr(),
                   _lib.ptr(oth), idx.ptr.data_ptr(), idx.dst.data_ptr(), None if oth is None else idx.oth.data_ptr(),
                   idx.n_rows, own_rows, idx.tiles.data_ptr(), idx.n_tiles, idx.n_split, idx.hubs.data_ptr(), idx.n_hubs,
                   d, H, grad.data_ptr(), ws.data_ptr(), ws.numel(), idx.counts_dev.data_ptr(), st)
@@ -300,8 +346,36 @@ class _UpdateEpilogue(torch.autograd.Function):
         return d_o, d_x, d_skip, d_nw, d_nb, None, None, None, None
 
 
-def typed_linear(a, w_cat, b_cat, table, width, out_elems, impl=0, act=0, zero_ranges=()):
-    return _TypedLinear.apply(a, w_cat, b_cat, table, width, out_elems, impl, act, tuple(zero_ranges))
+def typed_linear(a, w_cat, b_cat, table, width, out_elems, impl=0, act=0, zero_ranges=(), tables16=None):
+    return _TypedLinear.apply(a, w_cat, b_cat, table, width, out_elems, impl, act, tuple(zero_ranges), tables16)
+
+
+def _project(m, x, w_cat, b_cat, plan, lt, bf16):
+    """Typed projections of a layer: the flat [Q | pad | K'V' table | zero row] buffer and, with RTE, the RTE table
+    [P*240+1, 2d] (+ all-zero row).  bf16: those two are gradient stand-ins and the third result holds what the edge kernel
+    reads, (Q, bf16 [K'|V'] table, bf16 RTE table or None); otherwise it is None."""
+    N, P, d, d_in = plan.n_nodes, plan.n_pairs, m.out_dim, m.in_dim
+    kv_end = lt.kv_off + plan.kv_rows * 2 * d
+    if bf16:
+        proj, q, kv = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, m.linear_impl, 0, (),
+                                   (lt.q_groups, N * d, lt.kv_groups, lt.kv_off,
+                                    ((kv_end - lt.kv_off, lt.proj_elems - lt.kv_off),)))
+    else:
+        proj = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, m.linear_impl, 0,
+                            ((N * d, lt.kv_off), (kv_end, lt.proj_elems)))
+    kvr = kvr16 = None
+    if m.use_RTE:
+        # RT = lin(emb.weight) [240, d_in] (conv.py:299), then projected with every pair's K'/V' weights (no bias)
+        rt = typed_linear(m.emb.emb.weight, m.emb.lin.weight, m.emb.lin.bias, lt.rt_group, d_in,
+                          _plan.RTE_MAX_LEN * d_in, 1).view(_plan.RTE_MAX_LEN, d_in)
+        n_kvr = (P * _plan.RTE_MAX_LEN + 1) * 2 * d
+        zero = ((P * _plan.RTE_MAX_LEN * 2 * d, n_kvr),)
+        if bf16:
+            kvr, _, kvr16 = typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, (),
+                                         (None, 0, lt.rte_groups, 0, zero))
+        else:
+            kvr = typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, zero)
+    return proj, kvr, ((q, kv, kvr16) if bf16 else None)
 
 
 def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, active=None, kv_runs=None):
@@ -324,19 +398,10 @@ def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, 
               [l.weight for l in m.v_linears] + [l.bias for l in m.v_linears] +
               [m.relation_att, m.relation_msg, m.relation_pri])
     w_cat, b_cat = _FoldWeights.apply(m, plan, lt, *params)
-    kv_end = lt.kv_off + plan.kv_rows * 2 * d
-    proj = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, m.linear_impl, 0,
-                        ((N * d, lt.kv_off), (kv_end, lt.proj_elems)))
-    kvr = None
-    if m.use_RTE:
-        # RT = lin(emb.weight) [240, d_in] (conv.py:299), then projected with every pair's K'/V' weights (no bias)
-        rt = typed_linear(m.emb.emb.weight, m.emb.lin.weight, m.emb.lin.bias, lt.rt_group, d_in,
-                          _plan.RTE_MAX_LEN * d_in, 1).view(_plan.RTE_MAX_LEN, d_in)
-        n_kvr = (P * _plan.RTE_MAX_LEN + 1) * 2 * d
-        kvr = typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, ((P * _plan.RTE_MAX_LEN * 2 * d, n_kvr),))
+    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables())
 
     # 2. fused edge kernel
-    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant)
+    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant, tables16)
     m.att = att
 
     # 3. a_linears on gelu(agg) (conv.py:119,125): the gelu is applied inside the operand split / the dX epilogue
@@ -373,16 +438,8 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
               [l.weight for l in m.v_linears] + [l.bias for l in m.v_linears] +
               [m.relation_att, m.relation_msg, m.relation_pri])
     w_cat, b_cat = _FoldWeights.apply(m, plan, lt, *params)
-    kv_end = lt.kv_off + plan.kv_rows * 2 * d
-    proj = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, m.linear_impl, 0,
-                        ((N * d, lt.kv_off), (kv_end, lt.proj_elems)))
-    kvr = None
-    if m.use_RTE:
-        rt = typed_linear(m.emb.emb.weight, m.emb.lin.weight, m.emb.lin.bias, lt.rt_group, d_in,
-                          _plan.RTE_MAX_LEN * d_in, 1).view(_plan.RTE_MAX_LEN, d_in)
-        n_kvr = (P * _plan.RTE_MAX_LEN + 1) * 2 * d
-        kvr = typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, ((P * _plan.RTE_MAX_LEN * 2 * d, n_kvr),))
-    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant)
+    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables())
+    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant, tables16)
     m.att = att
 
     drop = m.training and m.drop.p > 0

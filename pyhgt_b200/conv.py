@@ -12,6 +12,9 @@ behind the C ABI in include/hgt_b200.h:
     typed output linear              hgt_typed_linear    a_linears
     gated skip + LayerNorm           hgt_update_epilogue
 
+Under ``torch.autocast("cuda", dtype=torch.bfloat16)`` the [K'|V'] and RTE gather tables are stored in bf16 (see
+autograd.py); inference then takes the per-stage path below instead of the one-call fused entry point.
+
 There is no CPU path: CPU tensors raise.  ``GeneralConv`` mirrors conv.py:303-323 so that pyHGT's
 model.py (``from .conv import *``) runs unchanged on top of this module.
 """
@@ -163,12 +166,13 @@ class HGTConv(nn.Module):
         return _T()
 
     def _typed_linear(self, a, lda, w, bias, k, width, table, out, impl, st):
-        """hgt_typed_linear with its (impl-dependent) workspace; table = (groups_dev, groups_host, n, cblocks_dev)."""
+        """hgt_typed_linear with its (impl-dependent) workspace; table = (groups_dev, groups_host, n, cblocks_dev).
+        A bf16 `out` takes hgt_typed_linear_bf16."""
         g_dev, g_host, n_g, c_dev = table
         ws_bytes = ctypes.c_size_t()
         _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, k, width, impl, ctypes.byref(ws_bytes))
         ws = torch.empty(max(ws_bytes.value, 1), dtype=torch.uint8, device=out.device)
-        _lib.call("hgt_typed_linear", a.data_ptr(), lda, w.data_ptr(), _lib.ptr(bias), k, width, g_dev.data_ptr(),
+        _lib.call("hgt_typed_linear_bf16" if out.dtype == torch.bfloat16 else "hgt_typed_linear", a.data_ptr(), lda, w.data_ptr(), _lib.ptr(bias), k, width, g_dev.data_ptr(),
                   g_host.ctypes.data, n_g, c_dev.data_ptr(), out.data_ptr(), impl, ws.data_ptr(), ws.numel(), st)
 
     def _check_inputs(self, node_inp, edge_time):
@@ -292,13 +296,16 @@ class HGTConv(nn.Module):
     def _forward_impl(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att, save,
                       active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None):
         """out_map / out_rows (sharded runs): int32 [N] map from rank-order row to output row and the number of output
-        rows; rows that are not active (halo sources) are never written, so the output holds exactly the owned rows."""
+        rows; rows that are not active (halo sources) are never written, so the output holds exactly the owned rows.
+        Under bf16 autocast the layer runs the per-stage path with bf16 gather tables."""
+        from .autograd import bf16_tables
+        bf16 = bf16_tables()
         if (self.fused_call and not save and HGTConv.event_sink is None and type(self)._has_skip
-                and not (self.training and self.drop.p > 0)):
+                and not (self.training and self.drop.p > 0) and not bf16):
             return self._forward_fused(node_inp, node_type, edge_index, edge_type, edge_time, want_att,
                                        active_per_type, out_map, out_rows, x_split, kv_runs)
         c = self._core(node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs)
+                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs, bf16=bf16)
         plan, lt, o, x_sorted, N, d, T, st = c["plan"], c["lt"], c["o"], c["x_sorted"], c["N"], c["d"], c["T"], c["st"]
         f32 = dict(dtype=torch.float32, device=o.device)
         norm_w = norm_b = None
@@ -326,9 +333,10 @@ class HGTConv(nn.Module):
         return out, c["att"], (c if save else None)
 
     def _core(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-              gelu_before_a, x_split=None, kv_runs=None):
+              gelu_before_a, x_split=None, kv_runs=None, bf16=False):
         """Everything up to and including the typed a_linear: plan, weight fold, typed projections, fused edge kernel
-        (gelu fused iff gelu_before_a and not save), a_linears.  Returns a dict of the intermediates."""
+        (gelu fused iff gelu_before_a and not save), a_linears.  Returns a dict of the intermediates.  bf16: bf16 [K'|V'] and
+        RTE tables (Q and everything else fp32)."""
         dev = node_inp.device
         d_in, d = self.in_dim, self.out_dim
         H, T, R = self.n_heads, self.num_types, self.num_relations
@@ -368,12 +376,39 @@ class HGTConv(nn.Module):
                   w_cat.data_ptr(), b_cat.data_ptr(), st)
 
         # 2. typed projections: Q [N,d] and the folded [K'|V'] table (+ trailing all-zero row)
-        proj = torch.empty(lt.proj_elems, **f32)
-        q_tab = proj[lt.q_off:lt.q_off + N * d]
-        kv_tab = proj[lt.kv_off:]
+        tab_dtype = torch.bfloat16 if bf16 else torch.float32
+        if bf16:
+            proj = None
+            q_tab = torch.empty(N * d, **f32)
+            kv_tab = torch.empty((plan.kv_rows + 1) * 2 * d, dtype=tab_dtype, device=dev)
+        else:
+            proj = torch.empty(lt.proj_elems, **f32)
+            q_tab = proj[lt.q_off:lt.q_off + N * d]
+            kv_tab = proj[lt.kv_off:]
         kv_tab[plan.kv_rows * 2 * d:].zero_()
         with self._stage("proj_linear"):
-            if x_split is not None and plan.sorted_types:
+            if bf16:
+                # Q by its own fp32 call, the K'/V' blocks straight into the bf16 table; the tensor-core path splits A once
+                xs = x_split if plan.sorted_types else None
+                if xs is None and self.linear_impl in (0, 2) and d_in % 16 == 0 and d_in >= 64 and d % 16 == 0:
+                    xs = (torch.empty((N, d_in), dtype=torch.bfloat16, device=dev),
+                          torch.empty((N, d_in), dtype=torch.bfloat16, device=dev))
+                    _lib.call("hgt_act_split", x_sorted.data_ptr(), d_in, N, d_in, 0, None, xs[0].data_ptr(),
+                              xs[1].data_ptr(), st)
+                for tab, dst in ((lt.q_groups, q_tab), (lt.kv_groups, kv_tab)):
+                    if xs is None:
+                        self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, dst, self.linear_impl, st)
+                        continue
+                    g_dev, g_host, n_g, c_dev = tab
+                    wsb = ctypes.c_size_t()
+                    _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, d_in, d,
+                              ctypes.byref(wsb))
+                    ws1 = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+                    _lib.call("hgt_typed_linear_presplit_bf16" if dst.dtype == torch.bfloat16 else "hgt_typed_linear_presplit",
+                              xs[0].data_ptr(), xs[1].data_ptr(), w_cat.data_ptr(), b_cat.data_ptr(), d_in, d,
+                              g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), dst.data_ptr(), ws1.data_ptr(),
+                              ws1.numel(), st)
+            elif x_split is not None and plan.sorted_types:
                 # A operand already split by its producer (the fused halo pull): tensor-core GEMM without the split pass
                 g_dev, g_host, n_g, c_dev = lt.proj_groups
                 wsb = ctypes.c_size_t()
@@ -390,7 +425,7 @@ class HGTConv(nn.Module):
             rt = torch.empty((_plan.RTE_MAX_LEN, d_in), **f32)
             self._typed_linear(self.emb.emb.weight, d_in, self.emb.lin.weight, self.emb.lin.bias, d_in, d_in,
                                lt.rt_group, rt, 1, st)
-            kvr = torch.empty((P * _plan.RTE_MAX_LEN + 1) * 2 * d, **f32)
+            kvr = torch.empty((P * _plan.RTE_MAX_LEN + 1) * 2 * d, dtype=tab_dtype, device=dev)
             kvr[P * _plan.RTE_MAX_LEN * 2 * d:].zero_()
             self._typed_linear(rt, d_in, w_cat, None, d_in, d, lt.rte_groups, kvr, 1, st)
 
@@ -408,7 +443,7 @@ class HGTConv(nn.Module):
         att = torch.empty((E, H), **f32) if want_att else None
         stats = torch.empty((N, 2 * H), **f32) if save else None
         with self._stage("edge"):
-            _lib.call("hgt_edge_forward", q_tab.data_ptr(), kv_tab.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
+            _lib.call("hgt_edge_forward_bf16" if bf16 else "hgt_edge_forward", q_tab.data_ptr(), kv_tab.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
                       plan.kv_row.data_ptr(), _lib.ptr(plan.rte_row) if self.use_RTE else None,
                       plan.csr_eid.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, plan.n_split,
                       plan.hubs.data_ptr(), plan.n_hubs, N, E, d, H, 1 if (gelu_before_a and not save) else 0,
@@ -440,7 +475,7 @@ class HGTConv(nn.Module):
                 self._typed_linear(g_act, d, wa_cat, ba_cat, d, d, lt.upd_groups, o, self.linear_impl, st)
         if self.training and self.drop.p > 0:
             o = self.drop(o)                                       # conv.py:125 (train mode only)
-        return dict(plan=plan, lt=lt, x_sorted=x_sorted, w_cat=w_cat, proj=proj, kvr=kvr, agg=agg, o=o, stats=stats,
+        return dict(plan=plan, lt=lt, x_sorted=x_sorted, w_cat=w_cat, proj=proj, q=q_tab, kv=kv_tab, kvr=kvr, agg=agg, o=o, stats=stats,
                     att=att, N=N, d=d, T=T, st=st)
 
 

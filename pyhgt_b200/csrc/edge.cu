@@ -14,8 +14,10 @@
 //   variant 1 (LDG)  : vector loads straight into registers, EDGE_UNROLL rows in flight per warp.
 //   variant 2 (TMA)  : cp.async.bulk (1-D bulk tensor copy, SASS UBLKCP) into a per-warp shared-memory
 //                      ring with mbarrier transaction counting; the warp issues STAGES rows ahead.
-// Roofline: HBM-bound; algorithmic bytes per edge = 2*d*4 (row) + 4 (kv_row) [+4 rte_row, +2*d*4 from L2]
-// and per destination d*4 (Q) + d*4 (agg) + 4 (row_ptr).
+// Roofline: HBM-bound; algorithmic bytes per edge = 2*d*s_kv (row) + 4 (kv_row) [+4 rte_row, +2*d*s_kv from L2]
+// and per destination d*4 (Q) + d*4 (agg) + 4 (row_ptr), with s_kv = 4 (fp32 tables) or 2 (bf16 tables,
+// hgt_edge_forward_bf16: every kernel is templated on the table element type KV and widens rows to fp32 in registers;
+// the lane map, the softmax and every output are the same).
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -27,8 +29,8 @@ constexpr int kCtaThreads = kWarpsPerCta * 32;
 
 struct EdgeParams {
   const float* q;
-  const float* kv;
-  const float* kvr;          // nullptr when !use_RTE
+  const void* kv;            // KV elements (float or bf16)
+  const void* kvr;           // nullptr when !use_RTE
   const int32_t* row_ptr;
   const int32_t* kv_row;
   const int32_t* rte_row;
@@ -89,6 +91,39 @@ __device__ __forceinline__ void load_vec_nc(float (&dst)[VEC], const float* p) {
     asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(dst[0]) : "l"(p));
   }
 }
+// bf16 table rows: VEC elements (8 / 4 / 2 bytes) widened to fp32, which is exact
+__device__ __forceinline__ float bf16_lo(uint32_t u) { return __uint_as_float(u << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u & 0xffff0000u); }
+
+template <int VEC>
+__device__ __forceinline__ void load_vec(float (&dst)[VEC], const __nv_bfloat16* p) {
+  if constexpr (VEC == 4) {
+    const uint2 u = *reinterpret_cast<const uint2*>(p);
+    dst[0] = bf16_lo(u.x); dst[1] = bf16_hi(u.x); dst[2] = bf16_lo(u.y); dst[3] = bf16_hi(u.y);
+  } else if constexpr (VEC == 2) {
+    const uint32_t u = *reinterpret_cast<const uint32_t*>(p);
+    dst[0] = bf16_lo(u); dst[1] = bf16_hi(u);
+  } else {
+    dst[0] = __bfloat162float(*p);
+  }
+}
+template <int VEC>
+__device__ __forceinline__ void load_vec_nc(float (&dst)[VEC], const __nv_bfloat16* p) {
+  if constexpr (VEC == 4) {
+    uint32_t a, b;
+    asm volatile("ld.global.nc.L1::no_allocate.v2.b32 {%0,%1}, [%2];" : "=r"(a), "=r"(b) : "l"(p));
+    dst[0] = bf16_lo(a); dst[1] = bf16_hi(a); dst[2] = bf16_lo(b); dst[3] = bf16_hi(b);
+  } else if constexpr (VEC == 2) {
+    uint32_t a;
+    asm volatile("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(a) : "l"(p));
+    dst[0] = bf16_lo(a); dst[1] = bf16_hi(a);
+  } else {
+    unsigned short a;
+    asm volatile("ld.global.nc.L1::no_allocate.b16 %0, [%1];" : "=h"(a) : "l"(p));
+    dst[0] = __uint_as_float((uint32_t)a << 16);
+  }
+}
+
 template <int VEC>
 __device__ __forceinline__ void store_vec(float* p, const float (&src)[VEC]) {
   using V = typename VecT<VEC>::type;
@@ -206,14 +241,16 @@ __device__ __forceinline__ void finalize_destination(const EdgeParams& p, const 
 // ------------------------------------------------------------------------------------------------
 // variant 1: direct register gather
 // ------------------------------------------------------------------------------------------------
-template <int VEC, int NCH>
+template <class KV, int VEC, int NCH>
 __global__ void __launch_bounds__(kCtaThreads, 1)
 k_edge_fwd_ldg(EdgeParams p) {
   // rows in flight per warp: bounded by the register budget (2 * U * NCH * VEC floats of staging)
   constexpr int EDGE_UNROLL = (NCH * VEC >= 32) ? 1 : (NCH * VEC >= 16 ? 2 : 4);
   const int lane = threadIdx.x & 31;
   const LaneMap lm(p, lane);
-  const bool rte = p.kvr != nullptr;
+  const KV* const kvt = static_cast<const KV*>(p.kv);
+  const KV* const kvrt = static_cast<const KV*>(p.kvr);
+  const bool rte = kvrt != nullptr;
   const int64_t row_stride = 2 * (int64_t)p.d;
   int offs[NCH];
 #pragma unroll
@@ -251,7 +288,7 @@ k_edge_fwd_ldg(EdgeParams p) {
 #pragma unroll
           for (int u = 0; u < EDGE_UNROLL; ++u) {
             if (u < nb) {
-              const float* row = p.kv + (int64_t)p.kv_row[c0 + u] * row_stride;
+              const KV* row = kvt + (int64_t)p.kv_row[c0 + u] * row_stride;
 #pragma unroll
               for (int t = 0; t < NCH; ++t) {
                 if (offs[t] >= 0) {
@@ -268,7 +305,7 @@ k_edge_fwd_ldg(EdgeParams p) {
 #pragma unroll
             for (int u = 0; u < EDGE_UNROLL; ++u) {
               if (u < nb) {
-                const float* row = p.kvr + (int64_t)p.rte_row[c0 + u] * row_stride;
+                const KV* row = kvrt + (int64_t)p.rte_row[c0 + u] * row_stride;
 #pragma unroll
                 for (int t = 0; t < NCH; ++t) {
                   if (offs[t] >= 0) {
@@ -362,16 +399,18 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src_gmem
                : "memory");
 }
 
-template <int VEC, int NCH>
+template <class KV, int VEC, int NCH>
 __global__ void __launch_bounds__(kCtaThreads, (VEC * NCH <= 4) ? 2 : 1)   // narrow rows (d_k <= 16): two CTAs per SM
 k_edge_fwd_tma(EdgeParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const LaneMap lm(p, lane);
-  const bool rte = p.kvr != nullptr;
+  const KV* const kvt = static_cast<const KV*>(p.kv);
+  const KV* const kvrt = static_cast<const KV*>(p.kvr);
+  const bool rte = kvrt != nullptr;
   const int S = p.stages;
-  const uint32_t row_bytes = 2u * (uint32_t)p.d * 4u;
+  const uint32_t row_bytes = 2u * (uint32_t)p.d * (uint32_t)sizeof(KV);
   const uint32_t slot_bytes = rte ? 2u * row_bytes : row_bytes;
   const int64_t row_stride = 2 * (int64_t)p.d;
   // layout: [warps][S][slot_bytes] rows, then [warps][S] mbarriers
@@ -427,8 +466,8 @@ k_edge_fwd_tma(EdgeParams p) {
         const uint32_t bar = smem_u32(&bars[slot]);
         const uint32_t dst = smem_u32(ring + (size_t)slot * slot_bytes);
         mbar_expect_tx(bar, slot_bytes);
-        bulk_g2s(dst, p.kv + (int64_t)row * row_stride, row_bytes, bar);
-        if (rte) bulk_g2s(dst + row_bytes, p.kvr + (int64_t)rrow * row_stride, row_bytes, bar);
+        bulk_g2s(dst, kvt + (int64_t)row * row_stride, row_bytes, bar);
+        if (rte) bulk_g2s(dst + row_bytes, kvrt + (int64_t)rrow * row_stride, row_bytes, bar);
       }
       ++issue_it;
     };
@@ -455,7 +494,7 @@ k_edge_fwd_tma(EdgeParams p) {
         for (int c = seg_begin; c < seg_end; ++c) {
           const uint32_t slot = it % S;
           mbar_wait(smem_u32(&bars[slot]), (it / S) & 1u);
-          const float* srow = reinterpret_cast<const float*>(ring + (size_t)slot * slot_bytes);
+          const KV* srow = reinterpret_cast<const KV*>(ring + (size_t)slot * slot_bytes);
           float kk[NCH][VEC], vv[NCH][VEC];
           float part = 0.f;
 #pragma unroll
@@ -576,34 +615,42 @@ k_merge_partials(EdgeParams p, const int32_t* __restrict__ hubs, int n_hubs_host
   }
 }
 
-template <int VEC, int NCH>
+template <class KV, int VEC, int NCH>
 int launch_variant(const EdgeParams& p, int variant, int grid, size_t smem, cudaStream_t st) {
   if (variant == 1) {
-    k_edge_fwd_ldg<VEC, NCH><<<grid, kCtaThreads, 0, st>>>(p);
+    k_edge_fwd_ldg<KV, VEC, NCH><<<grid, kCtaThreads, 0, st>>>(p);
   } else {
     static size_t configured = 0;            // per instantiation: raise the dynamic shared-memory limit once, not per launch
     if (smem > configured) {
-      HGT_CHECK_CUDA(cudaFuncSetAttribute(k_edge_fwd_tma<VEC, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      HGT_CHECK_CUDA(cudaFuncSetAttribute(k_edge_fwd_tma<KV, VEC, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)smem));
       configured = smem;
     }
-    k_edge_fwd_tma<VEC, NCH><<<grid, kCtaThreads, smem, st>>>(p);
+    k_edge_fwd_tma<KV, VEC, NCH><<<grid, kCtaThreads, smem, st>>>(p);
   }
   HGT_LAUNCH_CHECK();
   return 0;
 }
 
-template <int VEC>
+template <class KV, int VEC>
 int dispatch_nch(const EdgeParams& p, int nch, int variant, int grid, size_t smem, cudaStream_t st) {
   switch (nch) {
-    case 1: return launch_variant<VEC, 1>(p, variant, grid, smem, st);
-    case 2: return launch_variant<VEC, 2>(p, variant, grid, smem, st);
-    case 4: return launch_variant<VEC, 4>(p, variant, grid, smem, st);
-    case 8: return launch_variant<VEC, 8>(p, variant, grid, smem, st);
+    case 1: return launch_variant<KV, VEC, 1>(p, variant, grid, smem, st);
+    case 2: return launch_variant<KV, VEC, 2>(p, variant, grid, smem, st);
+    case 4: return launch_variant<KV, VEC, 4>(p, variant, grid, smem, st);
+    case 8: return launch_variant<KV, VEC, 8>(p, variant, grid, smem, st);
   }
   hgt_set_error("hgt_edge_forward: internal: unsupported chunk count %d", nch);
   return 1;
 }
+
+template <class KV>
+int edge_forward(const float* q, const KV* kv, const KV* kvr, const int32_t* row_ptr, const int32_t* kv_row,
+                 const int32_t* rte_row, const int32_t* csr_eid, const int32_t* tiles, int32_t n_tiles,
+                 int32_t n_split_tiles, const int32_t* hubs, int32_t n_hubs, int64_t n_nodes, int32_t d,
+                 int32_t n_heads, int32_t apply_gelu, float* agg_out, float* att_out, float* stats_out, void* g_hi,
+                 void* g_lo, void* workspace, size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
+                 const int32_t* type_row0, int32_t num_types, const int32_t* type_active, cudaStream_t st);
 
 }  // namespace
 
@@ -622,8 +669,38 @@ extern "C" int hgt_edge_forward(const float* q, const float* kv, const float* kv
                                 size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
                                 const int32_t* type_row0, int32_t num_types, const int32_t* type_active,
                                 void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
   (void)n_edges;
+  return edge_forward<float>(q, kv, kvr, row_ptr, kv_row, rte_row, csr_eid, tiles, n_tiles, n_split_tiles, hubs, n_hubs,
+                             n_nodes, d, n_heads, apply_gelu, agg_out, att_out, stats_out, g_hi, g_lo, workspace,
+                             workspace_bytes, variant, d_tile_counts, type_row0, num_types, type_active,
+                             (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_forward_bf16(const float* q, const void* kv, const void* kvr, const int32_t* row_ptr,
+                                     const int32_t* kv_row, const int32_t* rte_row, const int32_t* csr_eid,
+                                     const int32_t* tiles, int32_t n_tiles, int32_t n_split_tiles, const int32_t* hubs,
+                                     int32_t n_hubs, int64_t n_nodes, int64_t n_edges, int32_t d, int32_t n_heads,
+                                     int32_t apply_gelu, float* agg_out, float* att_out, float* stats_out, void* g_hi,
+                                     void* g_lo, void* workspace, size_t workspace_bytes, int32_t variant,
+                                     const int32_t* d_tile_counts, const int32_t* type_row0, int32_t num_types,
+                                     const int32_t* type_active, void* stream_) {
+  (void)n_edges;
+  return edge_forward<__nv_bfloat16>(q, static_cast<const __nv_bfloat16*>(kv), static_cast<const __nv_bfloat16*>(kvr),
+                                     row_ptr, kv_row, rte_row, csr_eid, tiles, n_tiles, n_split_tiles, hubs, n_hubs,
+                                     n_nodes, d, n_heads, apply_gelu, agg_out, att_out, stats_out, g_hi, g_lo,
+                                     workspace, workspace_bytes, variant, d_tile_counts, type_row0, num_types,
+                                     type_active, (cudaStream_t)stream_);
+}
+
+namespace {
+
+template <class KV>
+int edge_forward(const float* q, const KV* kv, const KV* kvr, const int32_t* row_ptr, const int32_t* kv_row,
+                 const int32_t* rte_row, const int32_t* csr_eid, const int32_t* tiles, int32_t n_tiles,
+                 int32_t n_split_tiles, const int32_t* hubs, int32_t n_hubs, int64_t n_nodes, int32_t d,
+                 int32_t n_heads, int32_t apply_gelu, float* agg_out, float* att_out, float* stats_out, void* g_hi,
+                 void* g_lo, void* workspace, size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
+                 const int32_t* type_row0, int32_t num_types, const int32_t* type_active, cudaStream_t st) {
   HGT_REQUIRE(n_heads >= 1 && n_heads <= 32, "hgt_edge_forward: n_heads=%d unsupported (1..32)", n_heads);
   HGT_REQUIRE(d % n_heads == 0, "hgt_edge_forward: d=%d not divisible by n_heads=%d", d, n_heads);
   HGT_REQUIRE((kvr != nullptr) == (rte_row != nullptr), "hgt_edge_forward: kvr and rte_row must go together");
@@ -664,7 +741,7 @@ extern "C" int hgt_edge_forward(const float* q, const float* kv, const float* kv
   const int sms = hgt_sm_count();
   int grid = sms;
   size_t smem = 0;
-  const size_t row_bytes = 2 * (size_t)d * 4;
+  const size_t row_bytes = 2 * (size_t)d * sizeof(KV);
   const size_t slot_bytes = kvr ? 2 * row_bytes : row_bytes;
   if (variant == 0) variant = 2;
   // narrow rows (one float4 per lane): the kernel is bound by per-destination latency, not by bytes in flight, so two
@@ -687,9 +764,9 @@ extern "C" int hgt_edge_forward(const float* q, const float* kv, const float* kv
   if (grid > max_ctas) grid = max_ctas;
   HGT_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), st));
   int rc;
-  if (vec == 4) rc = dispatch_nch<4>(p, nch, variant, grid, smem, st);
-  else if (vec == 2) rc = dispatch_nch<2>(p, nch, variant, grid, smem, st);
-  else rc = dispatch_nch<1>(p, nch, variant, grid, smem, st);
+  if (vec == 4) rc = dispatch_nch<KV, 4>(p, nch, variant, grid, smem, st);
+  else if (vec == 2) rc = dispatch_nch<KV, 2>(p, nch, variant, grid, smem, st);
+  else rc = dispatch_nch<KV, 1>(p, nch, variant, grid, smem, st);
   if (rc) return rc;
   if (n_split_tiles > 0) {
     HGT_REQUIRE(hubs != nullptr && n_hubs > 0, "hgt_edge_forward: split tiles present but no hub list given");
@@ -698,3 +775,5 @@ extern "C" int hgt_edge_forward(const float* q, const float* kv, const float* kv
   }
   return 0;
 }
+
+}  // namespace

@@ -18,6 +18,11 @@
 //                     (hgt_plan_source_index): per edge it gathers Q_i, dagg_i, (m, l)_i, D_i and the other table's row,
 //                     recomputes p / ds and accumulates dK = sum ds Q_i, dV = sum p dagg_i in registers; rows with more
 //                     than the split threshold of edges are cut into pieces whose partial rows are merged in piece order.
+//
+// hgt_edge_backward*_bf16: the same passes on bf16 [K'|V'] / RTE tables (KV = __nv_bfloat16), widened to fp32 in registers;
+// every gradient stays fp32 in the layouts above.
+#include <cuda_bf16.h>
+
 #include "common.cuh"
 
 #include <type_traits>
@@ -28,8 +33,8 @@ constexpr int kWarps = 8;
 
 struct BwdParams {
   const float* q;
-  const float* kv;
-  const float* kvr;
+  const void* kv;             // KV elements (float or bf16)
+  const void* kvr;
   const float* agg;
   const float* dagg;
   const float* stats;        // [N, 2H] (m, l)
@@ -61,6 +66,20 @@ __device__ __forceinline__ void ld_vec(float (&dst)[VEC], const float* p) {
   }
 }
 template <int VEC>
+__device__ __forceinline__ void ld_vec(float (&dst)[VEC], const __nv_bfloat16* p) {
+  // bf16 -> fp32 is exact: the element is the high half of the fp32 word
+  if constexpr (VEC == 4) {
+    const uint2 u = *reinterpret_cast<const uint2*>(p);
+    dst[0] = __uint_as_float(u.x << 16); dst[1] = __uint_as_float(u.x & 0xffff0000u);
+    dst[2] = __uint_as_float(u.y << 16); dst[3] = __uint_as_float(u.y & 0xffff0000u);
+  } else if constexpr (VEC == 2) {
+    const uint32_t u = *reinterpret_cast<const uint32_t*>(p);
+    dst[0] = __uint_as_float(u << 16); dst[1] = __uint_as_float(u & 0xffff0000u);
+  } else {
+    dst[0] = __bfloat162float(*p);
+  }
+}
+template <int VEC>
 __device__ __forceinline__ void red_add_vec(float* p, const float (&v)[VEC]) {
   if constexpr (VEC == 4) {
     asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3])
@@ -89,8 +108,10 @@ __device__ __forceinline__ void st_vec(float* p, const float (&v)[VEC]) {
 
 // DET = false: hgt_edge_backward (dk / dv scattered with reductions).  DET = true: destination pass of the
 // deterministic backward (no scatter; D_i saved; hub pieces write partial dq rows).
-template <int VEC, int NCH, bool DET>
+template <class KV, int VEC, int NCH, bool DET>
 __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
+  const KV* const kvt = static_cast<const KV*>(p.kv);
+  const KV* const kvrt = static_cast<const KV*>(p.kvr);
   const int lane = threadIdx.x & 31;
   const int lph = p.LPH;
   const int h = lane >> p.lph_shift;
@@ -103,7 +124,7 @@ __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
     offs[t] = (head_ok && o < p.DK) ? h * p.DK + o : -1;
   }
   const int64_t row_stride = 2 * (int64_t)p.d;
-  const bool rte = p.kvr != nullptr;
+  const bool rte = kvrt != nullptr;
 
   const int n_tiles = p.d_counts ? p.d_counts[0] : p.n_tiles;
   for (;;) {
@@ -148,7 +169,7 @@ __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
         for (int c = seg_begin; c < seg_end; ++c) {
           const int64_t row = p.kv_row[c];
           const int64_t rrow = rte ? p.rte_row[c] : 0;
-          const float* kvp = p.kv + row * row_stride;
+          const KV* kvp = kvt + row * row_stride;
           float kk[NCH][VEC], vv[NCH][VEC];
           float spart = 0.f, dppart = 0.f;
 #pragma unroll
@@ -158,8 +179,8 @@ __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
               ld_vec<VEC>(vv[t], kvp + p.d + offs[t]);
               if (rte) {
                 float a[VEC], b[VEC];
-                ld_vec<VEC>(a, p.kvr + rrow * row_stride + offs[t]);
-                ld_vec<VEC>(b, p.kvr + rrow * row_stride + p.d + offs[t]);
+                ld_vec<VEC>(a, kvrt + rrow * row_stride + offs[t]);
+                ld_vec<VEC>(b, kvrt + rrow * row_stride + p.d + offs[t]);
 #pragma unroll
                 for (int v = 0; v < VEC; ++v) { kk[t][v] += a[v]; vv[t][v] += b[v]; }
               }
@@ -227,16 +248,16 @@ __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
   }
 }
 
-template <int VEC, int NCH>
+template <class KV, int VEC, int NCH>
 __global__ void __launch_bounds__(kWarps * 32)
 k_edge_bwd(BwdParams p) {
-  edge_bwd_dst<VEC, NCH, false>(p);
+  edge_bwd_dst<KV, VEC, NCH, false>(p);
 }
 
-template <int VEC, int NCH>
+template <class KV, int VEC, int NCH>
 __global__ void __launch_bounds__(kWarps * 32)
 k_edge_bwd_dst(BwdParams p) {
-  edge_bwd_dst<VEC, NCH, true>(p);
+  edge_bwd_dst<KV, VEC, NCH, true>(p);
 }
 
 // ---- deterministic row pass --------------------------------------------------------------------------------------------
@@ -245,8 +266,8 @@ struct RowParams {
   const float* dagg;
   const float* stats;        // [N, 2H] (m, l)
   const float* D;            // [N, H] from the destination pass
-  const float* own;          // table of the owned rows [rows, 2d] ([K'|V'] or the RTE table)
-  const float* oth;          // the other table added to every edge's key / value row, or nullptr
+  const void* own;           // table of the owned rows [rows, 2d] ([K'|V'] or the RTE table), KV elements
+  const void* oth;           // the other table added to every edge's key / value row, or nullptr
   const int32_t* ptr;        // [n_rows + 1] source-major index over the owned rows
   const int32_t* e_dst;      // per index entry: destination (rank order)
   const int32_t* e_oth;      // per index entry: row of the other table (unused without oth)
@@ -259,9 +280,11 @@ struct RowParams {
   int32_t* tile_counter;
 };
 
-template <int VEC, int NCH>
+template <class KV, int VEC, int NCH>
 __global__ void __launch_bounds__(kWarps * 32)
 k_edge_bwd_rows(RowParams p) {
+  const KV* const own = static_cast<const KV*>(p.own);
+  const KV* const oth = static_cast<const KV*>(p.oth);
   const int lane = threadIdx.x & 31;
   const int lph = p.LPH;
   const int h = lane >> p.lph_shift;
@@ -274,7 +297,7 @@ k_edge_bwd_rows(RowParams p) {
     offs[t] = (head_ok && o < p.DK) ? h * p.DK + o : -1;
   }
   const int64_t row_stride = 2 * (int64_t)p.d;
-  const bool two = p.oth != nullptr;
+  const bool two = oth != nullptr;
 
   const int n_tiles = p.d_counts ? p.d_counts[0] : p.n_tiles;
   for (;;) {
@@ -294,7 +317,7 @@ k_edge_bwd_rows(RowParams p) {
 #pragma unroll
         for (int v = 0; v < VEC; ++v) { ko[t][v] = vo[t][v] = gk[t][v] = gv[t][v] = 0.f; }
       if (seg_end > seg_begin) {
-        const float* orow = p.own + (int64_t)row * row_stride;
+        const KV* orow = own + (int64_t)row * row_stride;
 #pragma unroll
         for (int t = 0; t < NCH; ++t)
           if (offs[t] >= 0) {
@@ -304,7 +327,7 @@ k_edge_bwd_rows(RowParams p) {
       }
       for (int j = seg_begin; j < seg_end; ++j) {
         const int64_t i = p.e_dst[j];
-        const float* xrow = two ? p.oth + (int64_t)p.e_oth[j] * row_stride : nullptr;
+        const KV* xrow = two ? oth + (int64_t)p.e_oth[j] * row_stride : nullptr;
         float q[NCH][VEC], da[NCH][VEC];
         float spart = 0.f, dppart = 0.f;
 #pragma unroll
@@ -377,30 +400,30 @@ k_merge_piece_rows(const int32_t* __restrict__ hubs, const int32_t* __restrict__
   }
 }
 
-template <typename Params, int VEC>
+template <class KV, typename Params, int VEC>
 int dispatch(const Params& p, int nch, int grid, cudaStream_t st, bool det) {
   if constexpr (std::is_same<Params, RowParams>::value) {
     switch (nch) {
-      case 1: k_edge_bwd_rows<VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 2: k_edge_bwd_rows<VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 4: k_edge_bwd_rows<VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 8: k_edge_bwd_rows<VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 1: k_edge_bwd_rows<KV, VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd_rows<KV, VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd_rows<KV, VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd_rows<KV, VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
       default: hgt_set_error("hgt_edge_backward_rows: unsupported chunk count %d", nch); return 1;
     }
   } else if (det) {
     switch (nch) {
-      case 1: k_edge_bwd_dst<VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 2: k_edge_bwd_dst<VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 4: k_edge_bwd_dst<VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 8: k_edge_bwd_dst<VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 1: k_edge_bwd_dst<KV, VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd_dst<KV, VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd_dst<KV, VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd_dst<KV, VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
       default: hgt_set_error("hgt_edge_backward_dst: unsupported chunk count %d", nch); return 1;
     }
   } else {
     switch (nch) {
-      case 1: k_edge_bwd<VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 2: k_edge_bwd<VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 4: k_edge_bwd<VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 8: k_edge_bwd<VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 1: k_edge_bwd<KV, VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd<KV, VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd<KV, VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd<KV, VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
       default: hgt_set_error("hgt_edge_backward: unsupported chunk count %d", nch); return 1;
     }
   }
@@ -432,15 +455,15 @@ int lane_map(int d, int n_heads, LaneMap& m, const char* who) {
   return 0;
 }
 
-template <typename Params>
+template <class KV, typename Params>
 int launch_pass(const Params& p, const LaneMap& lm, int n_tiles, cudaStream_t st, bool det) {
   HGT_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), st));
   int grid = hgt_sm_count() * 4;
   int max_ctas = (n_tiles + kWarps - 1) / kWarps;
   if (grid > max_ctas) grid = max_ctas;
-  if (lm.vec == 4) return dispatch<Params, 4>(p, lm.nch, grid, st, det);
-  if (lm.vec == 2) return dispatch<Params, 2>(p, lm.nch, grid, st, det);
-  return dispatch<Params, 1>(p, lm.nch, grid, st, det);
+  if (lm.vec == 4) return dispatch<KV, Params, 4>(p, lm.nch, grid, st, det);
+  if (lm.vec == 2) return dispatch<KV, Params, 2>(p, lm.nch, grid, st, det);
+  return dispatch<KV, Params, 1>(p, lm.nch, grid, st, det);
 }
 
 int merge_pieces(const int32_t* hubs, int32_t n_hubs, const int32_t* d_counts, const float* partial, int width,
@@ -452,15 +475,12 @@ int merge_pieces(const int32_t* hubs, int32_t n_hubs, const int32_t* d_counts, c
   return 0;
 }
 
-}  // namespace
-
-extern "C" int hgt_edge_backward(const float* q, const float* kv, const float* kvr, const float* agg,
-                                 const float* dagg, const float* stats, const int32_t* row_ptr,
-                                 const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
-                                 int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total,
-                                 int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr,
-                                 void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts, void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+template <class KV>
+int edge_backward(const float* q, const KV* kv, const KV* kvr, const float* agg, const float* dagg, const float* stats,
+                  const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles,
+                  int32_t n_tiles, int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total,
+                  int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr, void* workspace, size_t workspace_bytes,
+                  const int32_t* d_tile_counts, cudaStream_t st) {
   HGT_REQUIRE(n_heads >= 1 && n_heads <= 32 && d % n_heads == 0, "hgt_edge_backward: bad d=%d / n_heads=%d", d, n_heads);
   HGT_REQUIRE((kvr != nullptr) == (rte_row != nullptr) && (kvr != nullptr) == (dkvr != nullptr),
               "hgt_edge_backward: kvr, rte_row and dkvr must go together");
@@ -481,7 +501,33 @@ extern "C" int hgt_edge_backward(const float* q, const float* kv, const float* k
   p.dq = dq; p.dkv = dkv; p.dkvr = dkvr;
   p.tile_counter = reinterpret_cast<int32_t*>(workspace);
   p.D = nullptr; p.partial = nullptr;
-  return launch_pass(p, lm, n_tiles, st, false);
+  return launch_pass<KV>(p, lm, n_tiles, st, false);
+}
+
+}  // namespace
+
+extern "C" int hgt_edge_backward(const float* q, const float* kv, const float* kvr, const float* agg,
+                                 const float* dagg, const float* stats, const int32_t* row_ptr,
+                                 const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                                 int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total,
+                                 int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr,
+                                 void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts, void* stream_) {
+  return edge_backward<float>(q, kv, kvr, agg, dagg, stats, row_ptr, kv_row, rte_row, tiles, n_tiles, n_nodes, d, n_heads,
+                              kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace, workspace_bytes, d_tile_counts,
+                              (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_bf16(const float* q, const void* kv, const void* kvr, const float* agg,
+                                      const float* dagg, const float* stats, const int32_t* row_ptr,
+                                      const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles,
+                                      int32_t n_tiles, int64_t n_nodes, int32_t d, int32_t n_heads,
+                                      int64_t kv_rows_total, int64_t kvr_rows_total, float* dq, float* dkv,
+                                      float* dkvr, void* workspace, size_t workspace_bytes,
+                                      const int32_t* d_tile_counts, void* stream_) {
+  return edge_backward<__nv_bfloat16>(q, static_cast<const __nv_bfloat16*>(kv), static_cast<const __nv_bfloat16*>(kvr),
+                                      agg, dagg, stats, row_ptr, kv_row, rte_row, tiles, n_tiles, n_nodes, d, n_heads,
+                                      kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace, workspace_bytes,
+                                      d_tile_counts, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_edge_backward_det_workspace_bytes(int32_t n_split_dst, int32_t n_split_rows, int32_t d,
@@ -493,14 +539,14 @@ extern "C" int hgt_edge_backward_det_workspace_bytes(int32_t n_split_dst, int32_
   return 0;
 }
 
-extern "C" int hgt_edge_backward_dst(const float* q, const float* kv, const float* kvr, const float* agg,
-                                     const float* dagg, const float* stats, const int32_t* row_ptr,
-                                     const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles,
-                                     int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
-                                     int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D,
-                                     void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
-                                     void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+namespace {
+
+template <class KV>
+int edge_backward_dst(const float* q, const KV* kv, const KV* kvr, const float* agg, const float* dagg,
+                      const float* stats, const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                      const int32_t* tiles, int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
+                      int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D, void* workspace,
+                      size_t workspace_bytes, const int32_t* d_tile_counts, cudaStream_t st) {
   HGT_REQUIRE((kvr != nullptr) == (rte_row != nullptr), "hgt_edge_backward_dst: kvr and rte_row must go together");
   HGT_REQUIRE(dq && D, "hgt_edge_backward_dst: NULL output");
   size_t need = 0;
@@ -522,18 +568,16 @@ extern "C" int hgt_edge_backward_dst(const float* q, const float* kv, const floa
   p.tile_counter = reinterpret_cast<int32_t*>(workspace);
   p.D = D;
   p.partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  if ((rc = launch_pass(p, lm, n_tiles, st, true))) return rc;
+  if ((rc = launch_pass<KV>(p, lm, n_tiles, st, true))) return rc;
   return n_split > 0 ? merge_pieces(hubs, n_hubs, d_tile_counts, p.partial, d, dq, st) : 0;
 }
 
-extern "C" int hgt_edge_backward_rows(const float* q, const float* dagg, const float* stats, const float* D,
-                                      const float* own, const float* oth, const int32_t* src_ptr,
-                                      const int32_t* src_dst, const int32_t* src_oth, int32_t n_rows,
-                                      int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
-                                      const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads, float* grad,
-                                      void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
-                                      void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+template <class KV>
+int edge_backward_rows(const float* q, const float* dagg, const float* stats, const float* D, const KV* own,
+                       const KV* oth, const int32_t* src_ptr, const int32_t* src_dst, const int32_t* src_oth,
+                       int32_t n_rows, int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
+                       const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads, float* grad, void* workspace,
+                       size_t workspace_bytes, const int32_t* d_tile_counts, cudaStream_t st) {
   HGT_REQUIRE(own && grad && (oth == nullptr || src_oth), "hgt_edge_backward_rows: NULL argument");
   HGT_REQUIRE(n_rows >= 0 && own_rows_total >= n_rows, "hgt_edge_backward_rows: n_rows=%d own_rows_total=%lld", n_rows,
               (long long)own_rows_total);
@@ -557,6 +601,58 @@ extern "C" int hgt_edge_backward_rows(const float* q, const float* dagg, const f
   p.grad = grad;
   p.tile_counter = reinterpret_cast<int32_t*>(workspace);
   p.partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  if ((rc = launch_pass(p, lm, n_tiles, st, true))) return rc;
+  if ((rc = launch_pass<KV>(p, lm, n_tiles, st, true))) return rc;
   return n_split > 0 ? merge_pieces(hubs, n_hubs, d_tile_counts, p.partial, 2 * d, grad, st) : 0;
+}
+
+}  // namespace
+
+extern "C" int hgt_edge_backward_dst(const float* q, const float* kv, const float* kvr, const float* agg,
+                                     const float* dagg, const float* stats, const int32_t* row_ptr,
+                                     const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles,
+                                     int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
+                                     int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D,
+                                     void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                                     void* stream_) {
+  return edge_backward_dst<float>(q, kv, kvr, agg, dagg, stats, row_ptr, kv_row, rte_row, tiles, n_tiles, n_split, hubs,
+                                  n_hubs, n_nodes, d, n_heads, dq, D, workspace, workspace_bytes, d_tile_counts,
+                                  (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_dst_bf16(const float* q, const void* kv, const void* kvr, const float* agg,
+                                          const float* dagg, const float* stats, const int32_t* row_ptr,
+                                          const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles,
+                                          int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
+                                          int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D,
+                                          void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                                          void* stream_) {
+  return edge_backward_dst<__nv_bfloat16>(q, static_cast<const __nv_bfloat16*>(kv),
+                                          static_cast<const __nv_bfloat16*>(kvr), agg, dagg, stats, row_ptr, kv_row,
+                                          rte_row, tiles, n_tiles, n_split, hubs, n_hubs, n_nodes, d, n_heads, dq, D,
+                                          workspace, workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_rows(const float* q, const float* dagg, const float* stats, const float* D,
+                                      const float* own, const float* oth, const int32_t* src_ptr,
+                                      const int32_t* src_dst, const int32_t* src_oth, int32_t n_rows,
+                                      int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
+                                      const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads, float* grad,
+                                      void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                                      void* stream_) {
+  return edge_backward_rows<float>(q, dagg, stats, D, own, oth, src_ptr, src_dst, src_oth, n_rows, own_rows_total, tiles,
+                                   n_tiles, n_split, hubs, n_hubs, d, n_heads, grad, workspace, workspace_bytes,
+                                   d_tile_counts, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_rows_bf16(const float* q, const float* dagg, const float* stats, const float* D,
+                                           const void* own, const void* oth, const int32_t* src_ptr,
+                                           const int32_t* src_dst, const int32_t* src_oth, int32_t n_rows,
+                                           int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles,
+                                           int32_t n_split, const int32_t* hubs, int32_t n_hubs, int32_t d,
+                                           int32_t n_heads, float* grad, void* workspace, size_t workspace_bytes,
+                                           const int32_t* d_tile_counts, void* stream_) {
+  return edge_backward_rows<__nv_bfloat16>(q, dagg, stats, D, static_cast<const __nv_bfloat16*>(own),
+                                           static_cast<const __nv_bfloat16*>(oth), src_ptr, src_dst, src_oth, n_rows,
+                                           own_rows_total, tiles, n_tiles, n_split, hubs, n_hubs, d, n_heads, grad,
+                                           workspace, workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
 }

@@ -1,12 +1,19 @@
 // Typed (per-node-type) linear layers of HGTConv: weight folding (relation_att / relation_msg /
 // relation_pri into the K/V projections, SURVEY.md §8 a4) and the grouped GEMM front end.
 // This file holds the fp32 SIMT kernel (impl 1); the wgmma tensor-core kernel (impl 2) lives in
-// linear_tc.cu and is dispatched from hgt_typed_linear below.
+// linear_tc.cu and is dispatched from hgt_typed_linear below.  hgt_typed_linear_bf16 runs the same kernels with a bf16
+// output, each fp32 result rounded to nearest-even once when it is stored.
+#include <cuda_bf16.h>
+
 #include "common.cuh"
 
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
                         int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                         int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, void* workspace,
+                        size_t workspace_bytes, cudaStream_t st);
+int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                        int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                        int32_t n_groups, const hgt_lin_cblock* cblocks, __nv_bfloat16* out, void* workspace,
                         size_t workspace_bytes, cudaStream_t st);
 bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width);
 size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width);
@@ -75,11 +82,15 @@ struct TilePrefix {
   int32_t n_tiles_n;   // n-tiles per column block
 };
 
+__device__ __forceinline__ void store_out(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store_out(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+template <class OutT>
 __global__ void __launch_bounds__(GEMM_THREADS)
 k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __restrict__ W,
                     const float* __restrict__ bias, int K, int cb_width,
                     const hgt_lin_group* __restrict__ groups, int n_groups,
-                    const hgt_lin_cblock* __restrict__ cblocks, float* __restrict__ out, TilePrefix tp) {
+                    const hgt_lin_cblock* __restrict__ cblocks, OutT* __restrict__ out, TilePrefix tp) {
   __shared__ __align__(16) float As[BK][LDA_S];
   __shared__ __align__(16) float Ws[BK][LDW_S];
   int tile = blockIdx.x;
@@ -150,7 +161,7 @@ k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __res
     for (int j = 0; j < 4; ++j)
       if (tn * 4 + j < cols_here) bj[j] = bias[w_row0 + tn * 4 + j];
   }
-  float* Og = out + cblk.out_off + m0 * cblk.ld + n0;
+  OutT* Og = out + cblk.out_off + m0 * cblk.ld + n0;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     int r = tm * 8 + i;
@@ -158,7 +169,7 @@ k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __res
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       int c = tn * 4 + j;
-      if (c < cols_here) Og[(int64_t)r * cblk.ld + c] = acc[i][j] + bj[j];
+      if (c < cols_here) store_out(Og + (int64_t)r * cblk.ld + c, acc[i][j] + bj[j]);
     }
   }
 }
@@ -211,11 +222,13 @@ extern "C" int hgt_typed_linear_workspace_bytes(const hgt_lin_group* h_groups, i
   return 0;
 }
 
-extern "C" int hgt_typed_linear(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
-                                int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
-                                int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int32_t impl,
-                                void* workspace, size_t workspace_bytes, void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+namespace {
+
+template <class OutT>
+int typed_linear(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
+                 const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
+                 const hgt_lin_cblock* cblocks, OutT* out, int32_t impl, void* workspace, size_t workspace_bytes,
+                 cudaStream_t st) {
   HGT_REQUIRE(n_groups >= 0, "hgt_typed_linear: n_groups=%d", n_groups);
   HGT_REQUIRE(K > 0 && cb_width > 0, "hgt_typed_linear: K=%d cb_width=%d", K, cb_width);
   if (n_groups == 0) return 0;
@@ -224,8 +237,8 @@ extern "C" int hgt_typed_linear(const float* A, int64_t lda, const float* W, con
     // chunks (same stream, same workspace: launches are ordered)
     for (int g0 = 0; g0 < n_groups; g0 += kMaxGroups) {
       const int n = n_groups - g0 < kMaxGroups ? n_groups - g0 : kMaxGroups;
-      int rc = hgt_typed_linear(A, lda, W, bias, K, cb_width, groups + g0, h_groups + g0, n, cblocks, out, impl,
-                                workspace, workspace_bytes, stream_);
+      int rc = typed_linear(A, lda, W, bias, K, cb_width, groups + g0, h_groups + g0, n, cblocks, out, impl, workspace,
+                            workspace_bytes, st);
       if (rc) return rc;
     }
     return 0;
@@ -250,8 +263,26 @@ extern "C" int hgt_typed_linear(const float* A, int64_t lda, const float* W, con
   }
   tp.first_tile[n_groups] = (int32_t)total;
   if (total == 0) return 0;
-  k_typed_linear_simt<<<(unsigned)total, GEMM_THREADS, 0, st>>>(A, lda, W, bias, K, cb_width, groups, n_groups,
-                                                                cblocks, out, tp);
+  k_typed_linear_simt<OutT><<<(unsigned)total, GEMM_THREADS, 0, st>>>(A, lda, W, bias, K, cb_width, groups, n_groups,
+                                                                      cblocks, out, tp);
   HGT_LAUNCH_CHECK();
   return 0;
+}
+
+}  // namespace
+
+extern "C" int hgt_typed_linear(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                                int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int32_t impl,
+                                void* workspace, size_t workspace_bytes, void* stream_) {
+  return typed_linear(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, impl, workspace,
+                      workspace_bytes, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_typed_linear_bf16(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                                     int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                     int32_t n_groups, const hgt_lin_cblock* cblocks, void* out, int32_t impl,
+                                     void* workspace, size_t workspace_bytes, void* stream_) {
+  return typed_linear(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks,
+                      static_cast<__nv_bfloat16*>(out), impl, workspace, workspace_bytes, (cudaStream_t)stream_);
 }

@@ -11,7 +11,8 @@
 // wide (SWIZZLE_64B): at BN = 256 that makes a 4-deep ring of 48 KB stages instead of 2 x 96 KB.  BN = 64 keeps 64-wide
 // k-blocks (SWIZZLE_128B, 4 stages): its k-blocks are short enough that halving them costs more in barrier waits than the
 // deeper ring gains (measured on the d = 400 OAG shape).  Output tiles follow the same group / column-block tables
-// as the SIMT kernel in linear.cu.
+// as the SIMT kernel in linear.cu.  The output is fp32, or bf16 (hgt_typed_linear[_presplit]_bf16): the same tile, rounded
+// to nearest-even once as the epilogue stores it.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -54,22 +55,41 @@ __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_
   *reinterpret_cast<uint2*>(lo + r * Kp + c) = *reinterpret_cast<uint2*>(l);
 }
 
+// Columns col .. col + 3 of an output row: fp32, or bf16 rounded to nearest-even.  aligned: p is 4-element aligned.
+__device__ __forceinline__ void store4(float* p, float4 v, bool aligned) {
+  if (aligned) {
+    *reinterpret_cast<float4*>(p) = v;
+  } else {
+    *reinterpret_cast<float2*>(p) = make_float2(v.x, v.y);
+    *reinterpret_cast<float2*>(p + 2) = make_float2(v.z, v.w);
+  }
+}
+__device__ __forceinline__ void store4(__nv_bfloat16* p, float4 v, bool aligned) {
+  const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+  if (aligned) {
+    *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+  } else {
+    p[0] = a.x; p[1] = a.y; p[2] = b.x; p[3] = b.y;
+  }
+}
+
 // ---- the GEMM: out_cb[m, n] = A[a_row0 + m, :] . W[w_row0 + cb * cb_width + n, :] (+ bias) ------------------------------
 // Rows of a tile past the group and columns past the column block are computed on neighbouring (or zero-filled) operand
 // rows and not stored.
+template <class OutT>
 struct FwdJob {
   CUtensorMap a_hi, a_lo, w_hi, w_lo;      // A box {fwd_bk, 128 rows}, W box {fwd_bk, tile_n rows}
   const float* bias;
   const hgt_lin_group* groups;
   const hgt_lin_cblock* cblocks;
-  float* out;
+  OutT* out;
   int n_groups, cb_width, k_blocks, tile_n, n_tiles_n;
   int32_t first_tile[kMaxGroups + 1];
 
   struct Tile {
     int a_row, w_row, cols;
     int64_t rows, ld;
-    float* out;
+    OutT* out;
     const float* bias;
   };
 
@@ -111,12 +131,12 @@ struct FwdJob {
   // group is either inside the column block or past it.
   template <int BN>
   __device__ void store(const Tile& t, const float* acc, float* stage, int c, int wq, int lane) const {
-    float* o = t.out + (int64_t)(64 * c) * t.ld;
+    OutT* o = t.out + (int64_t)(64 * c) * t.ld;
     const int64_t rows = t.rows - 64 * c;
     const float* b = t.bias;
     const int cols = t.cols;
     const int64_t ld = t.ld;
-    const bool vec4 = ((reinterpret_cast<uintptr_t>(o) | (uintptr_t)(ld * 4)) & 15) == 0;
+    const bool vec4 = ((reinterpret_cast<uintptr_t>(o) | (uintptr_t)(ld * sizeof(OutT))) & (4 * sizeof(OutT) - 1)) == 0;
     store_staged<BN>(
         acc, stage, c, wq, lane,
         [&](int, int col, float v0, float v1) {
@@ -124,21 +144,13 @@ struct FwdJob {
           return make_float2(v0, v1);
         },
         [&](int r, int col, float4 v) {
-          if (r < rows && col < cols) {
-            float* p = o + r * ld + col;
-            if (vec4) {
-              *reinterpret_cast<float4*>(p) = v;
-            } else {
-              *reinterpret_cast<float2*>(p) = make_float2(v.x, v.y);
-              *reinterpret_cast<float2*>(p + 2) = make_float2(v.z, v.w);
-            }
-          }
+          if (r < rows && col < cols) store4(o + r * ld + col, v, vec4);
         });
   }
 };
 
-template <int BN>
-__global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob job, int n_tiles) {
+template <int BN, class OutT>
+__global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob<OutT> job, int n_tiles) {
   split3_tile<BN, false, fwd_bk<BN>()>(job, n_tiles);
 }
 
@@ -187,8 +199,8 @@ void extents(const hgt_lin_group* h_groups, int n_groups, int cb_width, int64_t*
 }
 
 // The tensor maps and the k-block count follow the kernel's k-block, fwd_bk<BN>().
-template <int BN>
-int launch_fwd(FwdJob& job, const __nv_bfloat16* const ops[4], int64_t a_rows, int64_t w_rows, int Kp, int tiles,
+template <int BN, class OutT>
+int launch_fwd(FwdJob<OutT>& job, const __nv_bfloat16* const ops[4], int64_t a_rows, int64_t w_rows, int Kp, int tiles,
                cudaStream_t st) {
   constexpr int KB = fwd_bk<BN>();
   int rc;
@@ -198,8 +210,8 @@ int launch_fwd(FwdJob& job, const __nv_bfloat16* const ops[4], int64_t a_rows, i
   if ((rc = make_map(&job.w_lo, ops[3], w_rows, Kp, BN, KB))) return rc;
   job.k_blocks = (Kp + KB - 1) / KB;
   const size_t smem = tile_smem_bytes<BN, KB>();
-  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_typed_linear_tc<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_typed_linear_tc<BN, OutT><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -218,14 +230,23 @@ size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_gr
   return 4 * 256 + 2 * hgt_align_up((size_t)a_rows * Kp * 2, 256) + 2 * hgt_align_up((size_t)w_rows * Kp * 2, 256);
 }
 
+template <class OutT>
 static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, const __nv_bfloat16* a_lo_in,
                   const float* W, const float* bias, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
-                  const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, float* out,
+                  const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
                   void* workspace, size_t workspace_bytes, cudaStream_t st);
 
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
                         const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
                         const hgt_lin_cblock* cblocks, float* out, void* workspace, size_t workspace_bytes,
+                        cudaStream_t st) {
+  return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace,
+                workspace_bytes, st);
+}
+
+int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
+                        const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
+                        const hgt_lin_cblock* cblocks, __nv_bfloat16* out, void* workspace, size_t workspace_bytes,
                         cudaStream_t st) {
   return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace,
                 workspace_bytes, st);
@@ -238,11 +259,11 @@ extern "C" int hgt_typed_linear_presplit_workspace_bytes(const hgt_lin_group* h_
   return 0;
 }
 
-extern "C" int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W, const float* bias,
-                                         int32_t K, int32_t cb_width, const hgt_lin_group* groups,
-                                         const hgt_lin_group* h_groups, int32_t n_groups,
-                                         const hgt_lin_cblock* cblocks, float* out, void* workspace,
-                                         size_t workspace_bytes, void* stream_) {
+template <class OutT>
+static int typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W, const float* bias, int32_t K,
+                                 int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                 int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out, void* workspace,
+                                 size_t workspace_bytes, cudaStream_t st) {
   HGT_REQUIRE(a_hi && a_lo, "hgt_typed_linear_presplit: NULL operand");
   HGT_REQUIRE(K % 8 == 0 && hgt_typed_linear_tc_supported(K, K, cb_width),
               "hgt_typed_linear_presplit: unsupported shape K=%d cb_width=%d", K, cb_width);
@@ -250,20 +271,38 @@ extern "C" int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, con
   if (n_groups > kMaxGroups) {                               // see hgt_typed_linear: chunked launches
     for (int g0 = 0; g0 < n_groups; g0 += kMaxGroups) {
       const int n = n_groups - g0 < kMaxGroups ? n_groups - g0 : kMaxGroups;
-      int rc = hgt_typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups + g0, h_groups + g0, n, cblocks, out,
-                                         workspace, workspace_bytes, stream_);
+      int rc = typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups + g0, h_groups + g0, n, cblocks, out,
+                                     workspace, workspace_bytes, st);
       if (rc) return rc;
     }
     return 0;
   }
   return tc_run(nullptr, 0, reinterpret_cast<const __nv_bfloat16*>(a_hi), reinterpret_cast<const __nv_bfloat16*>(a_lo),
-                W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace, workspace_bytes,
-                (cudaStream_t)stream_);
+                W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace, workspace_bytes, st);
 }
 
+extern "C" int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W, const float* bias,
+                                         int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                                         const hgt_lin_group* h_groups, int32_t n_groups,
+                                         const hgt_lin_cblock* cblocks, float* out, void* workspace,
+                                         size_t workspace_bytes, void* stream_) {
+  return typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace,
+                               workspace_bytes, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_typed_linear_presplit_bf16(const void* a_hi, const void* a_lo, const float* W, const float* bias,
+                                              int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                                              const hgt_lin_group* h_groups, int32_t n_groups,
+                                              const hgt_lin_cblock* cblocks, void* out, void* workspace,
+                                              size_t workspace_bytes, void* stream_) {
+  return typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks,
+                               static_cast<__nv_bfloat16*>(out), workspace, workspace_bytes, (cudaStream_t)stream_);
+}
+
+template <class OutT>
 static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, const __nv_bfloat16* a_lo_in,
                   const float* W, const float* bias, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
-                  const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, float* out,
+                  const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
                   void* workspace, size_t workspace_bytes, cudaStream_t st) {
   HGT_REQUIRE(hgt_typed_linear_tc_supported(lda, K, cb_width), "hgt_typed_linear(tc): unsupported K=%d cb_width=%d", K,
               cb_width);
@@ -291,7 +330,7 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
     if (n > 0) k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, K, w_rows, K, Kp, w_hi, w_lo);
     HGT_LAUNCH_CHECK();
   }
-  FwdJob job;
+  FwdJob<OutT> job;
   job.tile_n = pick_tile_n(cb_width);
   job.n_tiles_n = (cb_width + job.tile_n - 1) / job.tile_n;
   int64_t total = 0;

@@ -371,6 +371,8 @@ class LayerTables:
     kv_off: int
     proj_elems: int
     type_active_dev: torch.Tensor = None
+    q_groups: tuple = None        # proj_groups split for bf16 gather tables: the Q blocks alone (offsets into [N, d_out])
+    kv_groups: tuple = None       # ... and the K'/V' blocks alone (offsets relative to kv_off)
 
 
 class GroupTable(tuple):
@@ -457,6 +459,19 @@ def layer_tables(plan, d_in, d_out, active=None, kv_runs=None):
         if len(g2) <= 64 and all((s_, r_) in runs for (s_, r_) in plan.pairs):
             groups, cblocks = g2, c2
     proj = _pack_groups(groups, cblocks, dev)
+    # bf16 gather tables (autocast): the same groups, rows and weights, with the leading Q block of a group (written to the
+    # fp32 Q buffer) and its K'/V' blocks (written straight to the bf16 table) in separate tables
+    qg, qc, kg, kc = [], [], [], []
+    for (a0, m_, w0, ncb, cb0, has_bias) in groups:
+        cbs = cblocks[cb0:cb0 + ncb]
+        if cbs[0][0] < kv_off:
+            qg.append((a0, m_, w0, 1, len(qc), has_bias))
+            qc.append(cbs[0])
+            cbs, w0 = cbs[1:], w0 + d_out
+        if cbs:
+            kg.append((a0, m_, w0, len(cbs), len(kc), has_bias))
+            kc.extend((off - kv_off, ld) for off, ld in cbs)
+    q_groups, kv_groups = _pack_groups(qg, qc, dev), _pack_groups(kg, kc, dev)
     # The backward's dX writes rows non-atomically, so it takes groups with DISJOINT row ranges: split the table into
     # such subsets (greedy interval colouring; the first subset writes dA, the others accumulate into it).
     subsets = []
@@ -490,6 +505,6 @@ def layer_tables(plan, d_in, d_out, active=None, kv_runs=None):
     lt = LayerTables(cat_rows=rows, q_row0=q_row0, cat_row0=cat_row0, q_row0_dev=small[:T],
                      cat_row0_dev=small[T:T + max(P, 1)],
                      type_active_dev=None if active is None else small[T + max(P, 1):], proj_groups=proj, rte_groups=rte, upd_groups=upd, rt_group=rt_group, q_off=q_off,
-                     kv_off=kv_off, proj_elems=proj_elems)
+                     kv_off=kv_off, proj_elems=proj_elems, q_groups=q_groups, kv_groups=kv_groups)
     plan._layer_tables[key] = lt
     return lt
