@@ -107,6 +107,44 @@ int hgt_plan_source_index(const int32_t* key, const int32_t* other, const int32_
                           int64_t n_edges, int32_t n_rows, int32_t* src_ptr, int32_t* src_dst, int32_t* src_oth,
                           void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Trimmed forward (GNN.forward(..., out_nodes=)): layer l of L only needs the nodes within L-l hops of an output node.
+ * ---------------------------------------------------------------------------------------------- */
+
+/* Hop layout of a batch.  dist[v] [N] int32 = min(L+1, length of the shortest directed path (source -> destination)
+ * from v to any out_nodes entry), by L edge-parallel passes from the out_nodes.  hop_perm [N] int32: the nodes stably
+ * sorted by (type, dist) — types 0..T-1 in order, nodes of a type outside [0,T) last in their original order;
+ * hop_rank [N] int32 its inverse; hop_node_type [N] int64 = node_type[hop_perm]; hop_edge_index [2,E] int64 = hop_rank of
+ * every endpoint (edge order kept); out_rows [n_out] int64 = hop_rank[out_nodes].
+ * meta (int32, zeroed here) = [counts T*(L+2) | presence T*R | flags 4]:
+ *   counts[t*(L+2)+b]: nodes of type t with dist == b (b = L+1: farther or unreachable);
+ *   presence[s*R+r] = 1 where a valid edge has <source type s, relation r> (as hgt_plan_edges_sort);
+ *   flags[0]: an edge endpoint outside [0,N); flags[1]: an edge_time of such an edge outside [0,240) (edge_time may be
+ *   NULL); flags[2]: an out_nodes entry outside [0,N) (the outputs derived from it are then meaningless).
+ * Nothing is read back or synchronised.  workspace: hgt_plan_workspace_bytes(n_nodes, n_edges). */
+int hgt_trim_layout(const int64_t* edge_index, const int64_t* edge_type, const int64_t* edge_time,
+                    const int64_t* node_type, int64_t n_nodes, int64_t n_edges, int32_t num_types,
+                    int32_t num_relations, const int64_t* out_nodes, int64_t n_out, int32_t n_layers,
+                    int32_t* dist, int32_t* hop_perm, int32_t* hop_rank, int64_t* hop_node_type,
+                    int64_t* hop_edge_index, int64_t* out_rows, int32_t* meta, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
+/* hgt_plan_tiles (sync-free mode, same tile / hub / count formats) over the destinations of n_ranges ascending, disjoint
+ * row ranges ranges[2j] .. ranges[2j+1] (device int32 [n_ranges,2]) of row_ptr; n_range_rows = total rows in the ranges
+ * (host).  No tile crosses a range end, so an edge kernel launched with these tiles reads and writes only the rows of
+ * the ranges.  Bounds: max_tiles >= (2E+N)/(2*target_edges) + 3*(E/split_edges) + 16 + n_ranges, max_hubs and split
+ * pieces as for hgt_plan_tiles.  workspace: hgt_plan_workspace_bytes(n_nodes, n_edges). */
+int hgt_plan_range_tiles(const int32_t* row_ptr, int64_t n_nodes, int64_t n_edges, const int32_t* ranges,
+                         int32_t n_ranges, int64_t n_range_rows, int32_t target_edges, int32_t split_edges,
+                         int32_t* tiles, int64_t max_tiles, int32_t* hubs, int64_t max_hubs, int32_t* d_n_tiles,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
+/* out_key[c] = key[c] for CSR positions c whose destination lies in one of the row ranges (as hgt_plan_range_tiles),
+ * no_work_row otherwise: with no_work_row = n_rows, hgt_plan_source_index(out_key, ...) then indexes only the edges of
+ * those destinations. */
+int hgt_plan_mask_rows(const int32_t* key, const int32_t* row_ptr, const int32_t* ranges, int32_t n_ranges,
+                       int64_t n_edges, int32_t no_work_row, int32_t* out_key, void* stream);
+
 /* out[k,:] = in[perm[k],:]  (rows of `width` floats); used only when node_type is not pre-sorted. */
 int hgt_gather_rows(const float* in, const int32_t* perm, int64_t n_rows, int32_t width,
                     float* out, void* stream);

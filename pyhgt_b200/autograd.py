@@ -311,9 +311,10 @@ class _UpdateEpilogue(torch.autograd.Function):
     def forward(ctx, o, x, skip, norm_w, norm_b, type_row0, T, perm, type_active=None):
         N, d = o.shape
         o, x = o.contiguous(), x.contiguous()
-        # with type_active (sharded training) the rows past the active prefix of a type have no output row: they stay
-        # unwritten (the caller selects the owned rows) and receive no gradient (hgt_update_backward skips them)
-        out = torch.empty((N, d), dtype=torch.float32, device=o.device)
+        # with type_active (sharded training, trimmed layers) the rows past the active prefix of a type have no output
+        # row: they are zero (never an uninitialised row a later stage could read) and receive no gradient
+        # (hgt_update_backward skips them)
+        out = (torch.zeros if type_active is not None else torch.empty)((N, d), dtype=torch.float32, device=o.device)
         _lib.call("hgt_update_epilogue", o.data_ptr(), x.data_ptr(), type_row0.data_ptr(), T, _lib.ptr(skip),
                   _lib.ptr(norm_w), _lib.ptr(norm_b), _lib.ptr(perm), _lib.ptr(type_active), N, d, out.data_ptr(), None,
                   None, _stream())
@@ -378,12 +379,18 @@ def _project(m, x, w_cat, b_cat, plan, lt, bf16):
     return proj, kvr, ((q, kv, kvr16) if bf16 else None)
 
 
-def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, active=None, kv_runs=None):
-    """`active` (sharded training): active[t] = number of leading nodes of type t (rank order) that are destinations on
-    this rank; Q / a_linear / update run for them only, the remaining rows (halo sources) only get K'/V' rows and their
-    output rows stay zero.  `kv_runs`: per-pair row ranges that need K'/V' (plan.layer_tables)."""
+def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, active=None, kv_runs=None, plan=None,
+                      want_att=None):
+    """`active` (sharded training, trimmed layers): active[t] = number of leading nodes of type t (rank order) that are
+    destinations here; Q / a_linear / update run for them only, the remaining rows (halo sources) only get K'/V' rows and
+    their output rows stay zero.  `kv_runs`: per-pair row ranges that need K'/V' (plan.layer_tables).  `plan`: an explicit
+    plan (a trimmed layer's view, trim.py) instead of the cached plan of the tensors.  `want_att`: materialise m.att
+    (default m.keep_att)."""
     d_in, d, H, T, R = m.in_dim, m.out_dim, m.n_heads, m.num_types, m.num_relations
-    plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if m.use_RTE else None, T, R)
+    if plan is None:
+        plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if m.use_RTE else None, T, R)
+    if want_att is None:
+        want_att = bool(m.keep_att)
     N, P = plan.n_nodes, plan.n_pairs
     if node_inp.shape[0] != N:
         raise ValueError("node_inp has %d rows but node_type has %d" % (node_inp.shape[0], N))
@@ -401,7 +408,7 @@ def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, 
     proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables())
 
     # 2. fused edge kernel
-    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant, tables16)
+    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, want_att, m.edge_variant, tables16)
     m.att = att
 
     # 3. a_linears on gelu(agg) (conv.py:119,125): the gelu is applied inside the operand split / the dX epilogue

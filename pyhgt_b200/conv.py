@@ -60,6 +60,14 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def _output_rows(rows, d, dev, lt, out_map):
+    """The layer's output buffer.  With an active prefix and no out_map the update epilogue leaves the rows past the
+    prefix unwritten: they are zeroed, so a later layer never reads an uninitialised row."""
+    if lt.type_active_dev is not None and out_map is None:
+        return torch.zeros((rows, d), dtype=torch.float32, device=dev)
+    return torch.empty((rows, d), dtype=torch.float32, device=dev)
+
+
 class _PointerTable:
     """Device array of per-type parameter pointers, rebuilt only when a parameter moves."""
 
@@ -201,14 +209,29 @@ class HGTConv(nn.Module):
         self.att = att
         return out
 
+    def _forward_view(self, node_inp, view, edge_time):
+        """One layer of a trimmed GNN forward (trim.py) on the hop layout's rows: Q, a_linear and update for the view's
+        active prefix of every type, K'/V' for its `kv_runs`, the edge kernels over its destination tiles.  The other
+        output rows are zero; `.att` is None (the softmax of the skipped destinations is never computed)."""
+        self._check_inputs(node_inp, edge_time)
+        self.att = None
+        if torch.is_grad_enabled() and (node_inp.requires_grad or any(p.requires_grad for p in self.parameters())):
+            from .autograd import hgt_conv_autograd
+            return hgt_conv_autograd(self, node_inp, None, None, None, None, active=view.active,
+                                     kv_runs=view.kv_runs, plan=view.plan, want_att=False)
+        out, _, _ = self._forward_impl(node_inp, None, None, None, None, want_att=False, save=False,
+                                       active_per_type=view.active, kv_runs=view.kv_runs, plan=view.plan)
+        return out
+
     # ------------------------------------------------------------------------------------------
     def _forward_fused(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att,
-                       active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None):
+                       active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None, plan=None):
         """Inference through the single entry point hgt_conv_forward (csrc/layer.cu).  The argument block is cached per
         (plan tables, parameter locations); per call only the data pointers change."""
         dev = node_inp.device
         d_in, d, H, T, R = self.in_dim, self.out_dim, self.n_heads, self.num_types, self.num_relations
-        plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if self.use_RTE else None, T, R)
+        if plan is None:
+            plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if self.use_RTE else None, T, R)
         N, E = plan.n_nodes, plan.n_edges
         if node_inp.shape[0] != N:
             raise ValueError("node_inp has %d rows but node_type has %d" % (node_inp.shape[0], N))
@@ -276,7 +299,7 @@ class HGTConv(nn.Module):
         if out_map is not None and not plan.sorted_types:
             raise ValueError("out_map needs a type-sorted node order")
         a.out_map = _lib.ptr(out_map)
-        out = torch.empty((N if out_rows is None else out_rows, d), dtype=torch.float32, device=dev)
+        out = _output_rows(N if out_rows is None else out_rows, d, dev, lt, out_map)
         att = torch.empty((E, H), dtype=torch.float32, device=dev) if want_att else None
         a.out, a.att = out.data_ptr(), _lib.ptr(att)
         o_hi = o_lo = None
@@ -294,25 +317,26 @@ class HGTConv(nn.Module):
         return out, att, None
 
     def _forward_impl(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att, save,
-                      active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None):
+                      active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None, plan=None):
         """out_map / out_rows (sharded runs): int32 [N] map from rank-order row to output row and the number of output
         rows; rows that are not active (halo sources) are never written, so the output holds exactly the owned rows.
-        Under bf16 autocast the layer runs the per-stage path with bf16 gather tables."""
+        Without out_map, rows past the active prefix are zero.  plan: an explicit plan (a trimmed layer's view, trim.py)
+        instead of the cached plan of the tensors.  Under bf16 autocast the layer runs the per-stage path with bf16
+        gather tables."""
         from .autograd import bf16_tables
         bf16 = bf16_tables()
         if (self.fused_call and not save and HGTConv.event_sink is None and type(self)._has_skip
                 and not (self.training and self.drop.p > 0) and not bf16):
             return self._forward_fused(node_inp, node_type, edge_index, edge_type, edge_time, want_att,
-                                       active_per_type, out_map, out_rows, x_split, kv_runs)
+                                       active_per_type, out_map, out_rows, x_split, kv_runs, plan)
         c = self._core(node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs, bf16=bf16)
+                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs, bf16=bf16, plan=plan)
         plan, lt, o, x_sorted, N, d, T, st = c["plan"], c["lt"], c["o"], c["x_sorted"], c["N"], c["d"], c["T"], c["st"]
-        f32 = dict(dtype=torch.float32, device=o.device)
         norm_w = norm_b = None
         if self.use_norm:
             norm_w = torch.stack([n.weight for n in self.norms]).contiguous()
             norm_b = torch.stack([n.bias for n in self.norms]).contiguous()
-        out = torch.empty((N if out_rows is None else out_rows, d), **f32)
+        out = _output_rows(N if out_rows is None else out_rows, d, o.device, lt, out_map)
         if out_map is not None:
             if not plan.sorted_types:
                 raise ValueError("out_map needs a type-sorted node order")
@@ -333,7 +357,7 @@ class HGTConv(nn.Module):
         return out, c["att"], (c if save else None)
 
     def _core(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-              gelu_before_a, x_split=None, kv_runs=None, bf16=False):
+              gelu_before_a, x_split=None, kv_runs=None, bf16=False, plan=None):
         """Everything up to and including the typed a_linear: plan, weight fold, typed projections, fused edge kernel
         (gelu fused iff gelu_before_a and not save), a_linears.  Returns a dict of the intermediates.  bf16: bf16 [K'|V'] and
         RTE tables (Q and everything else fp32)."""
@@ -341,7 +365,8 @@ class HGTConv(nn.Module):
         d_in, d = self.in_dim, self.out_dim
         H, T, R = self.n_heads, self.num_types, self.num_relations
         st = _stream()
-        plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if self.use_RTE else None, T, R)
+        if plan is None:
+            plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if self.use_RTE else None, T, R)
         N, E, P = plan.n_nodes, plan.n_edges, plan.n_pairs
         if node_inp.shape[0] != N:
             raise ValueError("node_inp has %d rows but node_type has %d" % (node_inp.shape[0], N))

@@ -151,42 +151,72 @@ __global__ void k_edge_fill(const int64_t* __restrict__ edge_index, const int64_
 }
 
 // ---- work tiles --------------------------------------------------------------------------------
+// The destinations a tile plan covers: every row [0, N) (r == nullptr), or the rows of n ascending, disjoint ranges
+// [r[2j], r[2j+1]) (a trimmed layer's destinations).  Tile planning walks positions k of the concatenated ranges.
+struct RowRanges {
+  const int32_t* r;
+  int n;
+  int64_t N;
+  // row at position k, and whether it opens its range (a tile never spans two ranges)
+  __device__ __forceinline__ int64_t row(int64_t k, bool* first) const {
+    if (r == nullptr) { *first = k == 0; return k; }
+    for (int j = 0; j < n; ++j) {
+      const int64_t len = r[2 * j + 1] - r[2 * j];
+      if (k < len) { *first = k == 0; return r[2 * j] + k; }
+      k -= len;
+    }
+    *first = false;
+    return N;
+  }
+  // end of the range holding `row`
+  __device__ __forceinline__ int64_t end_of(int64_t row) const {
+    if (r == nullptr) return N;
+    for (int j = 0; j < n; ++j)
+      if (row >= r[2 * j] && row < r[2 * j + 1]) return r[2 * j + 1];
+    return N;
+  }
+};
+
 // cost(k) = 2*deg(k) + 1 (an edge reads a 2d-float KV row, every destination writes a d-float row).
 // A destination starts a tile when its cost prefix enters a new bucket of `tc` units; a hub
 // (deg > split) gets ceil(deg/split) tiles of its own.
-__device__ __forceinline__ bool tile_starts_at(const int32_t* row_ptr, int64_t k, int tc, int split) {
-  if (k == 0) return true;
+__device__ __forceinline__ bool tile_starts_at(const int32_t* row_ptr, int64_t k, bool first, int tc, int split) {
+  if (first) return true;
   int32_t deg_prev = row_ptr[k] - row_ptr[k - 1];
   if (deg_prev > split) return true;                       // first destination after a hub
   int64_t c1 = 2 * (int64_t)row_ptr[k] + k, c0 = 2 * (int64_t)row_ptr[k - 1] + (k - 1);
   return (c1 / tc) != (c0 / tc);
 }
 
-__global__ void k_tile_emit_counts(const int32_t* __restrict__ row_ptr, int64_t N, int tc, int split,
+__global__ void k_tile_emit_counts(const int32_t* __restrict__ row_ptr, int64_t M, RowRanges rr, int tc, int split,
                                    int64_t* __restrict__ packed) {
-  int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (k > N) return;
-  if (k == N) { packed[k] = 0; return; }
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i > M) return;
+  if (i == M) { packed[i] = 0; return; }
+  bool first;
+  const int64_t k = rr.row(i, &first);
   int32_t deg = row_ptr[k + 1] - row_ptr[k];
   int64_t emit, emit_split;
   if (deg > split) {
     emit = (deg + split - 1) / split;
     emit_split = emit;
   } else {
-    emit = tile_starts_at(row_ptr, k, tc, split) ? 1 : 0;
+    emit = tile_starts_at(row_ptr, k, first, tc, split) ? 1 : 0;
     emit_split = 0;
   }
-  packed[k] = (emit << 32) | emit_split;
+  packed[i] = (emit << 32) | emit_split;
 }
 
-__global__ void k_tile_write(const int32_t* __restrict__ row_ptr, int64_t N, int tc, int split,
+__global__ void k_tile_write(const int32_t* __restrict__ row_ptr, int64_t M, RowRanges rr, int tc, int split,
                              const int64_t* __restrict__ packed_scan, int32_t* __restrict__ tiles,
                              int64_t max_tiles, int32_t* __restrict__ n_tiles, int32_t* __restrict__ hubs,
                              int64_t max_hubs) {
-  int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (k > N) return;
-  int64_t slot = packed_scan[k] >> 32, pslot = packed_scan[k] & 0xffffffffll;
-  if (k == N) { n_tiles[0] = (int32_t)slot; n_tiles[1] = (int32_t)pslot; return; }
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i > M) return;
+  int64_t slot = packed_scan[i] >> 32, pslot = packed_scan[i] & 0xffffffffll;
+  if (i == M) { n_tiles[0] = (int32_t)slot; n_tiles[1] = (int32_t)pslot; return; }
+  bool first;
+  const int64_t k = rr.row(i, &first);
   int32_t b = row_ptr[k], deg = row_ptr[k + 1] - b;
   if (deg > split) {
     int pieces = (deg + split - 1) / split;
@@ -202,23 +232,126 @@ __global__ void k_tile_write(const int32_t* __restrict__ row_ptr, int64_t N, int
       int32_t eb = b + i * per, ee = min(b + deg, eb + per);
       t[0] = (int32_t)k; t[1] = -(int32_t)(pslot + i) - 1; t[2] = eb; t[3] = ee;
     }
-  } else if (tile_starts_at(row_ptr, k, tc, split)) {
+  } else if (tile_starts_at(row_ptr, k, first, tc, split)) {
     if (slot >= max_tiles) return;
     int32_t* t = tiles + 4 * slot;
     t[0] = (int32_t)k; t[1] = 0; t[2] = b; t[3] = 0;     // end fields patched by k_tile_close
   }
 }
 
-__global__ void k_tile_close(const int32_t* __restrict__ row_ptr, int64_t N, int32_t* __restrict__ tiles,
+__global__ void k_tile_close(const int32_t* __restrict__ row_ptr, RowRanges rr, int32_t* __restrict__ tiles,
                              const int32_t* __restrict__ n_tiles) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   int nt = n_tiles[0];
   if (i >= nt) return;
   int32_t* t = tiles + 4 * i;
   if (t[1] < 0) return;                                   // hub piece: complete
-  int32_t dend = (i + 1 < nt) ? tiles[4 * (i + 1)] : (int32_t)N;
-  t[1] = dend;
+  int64_t dend = (i + 1 < nt) ? tiles[4 * (i + 1)] : rr.N;
+  const int64_t rend = rr.end_of(t[0]);                    // the next tile may open the next range
+  if (rend < dend) dend = rend;
+  t[1] = (int32_t)dend;
   t[3] = row_ptr[dend];
+}
+
+// ---- hop layout (GNN.forward(out_nodes=)) ---------------------------------------------------------
+__global__ void k_hop_init(const int64_t* __restrict__ out_nodes, int64_t n_out, int64_t N, int32_t far,
+                           int32_t* __restrict__ dist, int32_t* __restrict__ flags) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < N) dist[i] = far;
+  if (i < n_out) {
+    const int64_t v = out_nodes[i];
+    if (v < 0 || v >= N) flags[2] = 1;
+  }
+}
+
+__global__ void k_hop_seeds(const int64_t* __restrict__ out_nodes, int64_t n_out, int64_t N, int32_t* __restrict__ dist) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n_out) return;
+  const int64_t v = out_nodes[i];
+  if (v >= 0 && v < N) dist[v] = 0;
+}
+
+// the range checks and <source type, relation> presence of hgt_plan_edges_sort / hgt_plan_edges_fill, for the hop plan
+__global__ void k_hop_edge_scan(const int64_t* __restrict__ edge_index, const int64_t* __restrict__ edge_type,
+                                const int64_t* __restrict__ edge_time, const int64_t* __restrict__ node_type, int64_t N,
+                                int64_t E, int T, int R, int32_t* __restrict__ presence, int32_t* __restrict__ flags) {
+  int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const int64_t src = edge_index[e], dst = edge_index[E + e];
+  if (src < 0 || src >= N || dst < 0 || dst >= N) { flags[0] = 1; return; }
+  const int64_t s = node_type[src], t = node_type[dst], r = edge_type[e];
+  if (s >= 0 && s < T && t >= 0 && t < T && r >= 0 && r < R) {
+    presence[s * R + r] = 1;
+    if (edge_time) {
+      const int64_t dt = edge_time[e];
+      if (dt < 0 || dt >= HGT_RTE_MAX_LEN) flags[1] = 1;
+    }
+  }
+}
+
+// BFS pass h: a source one edge away from a node at distance h-1 is at distance h (if not nearer).  Every write of a
+// pass stores the same value h, and a pass reads only the values h-1 the previous pass finished.
+__global__ void k_hop_pass(const int64_t* __restrict__ edge_index, int64_t N, int64_t E, int32_t h,
+                           int32_t* __restrict__ dist) {
+  int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const int64_t src = edge_index[e], dst = edge_index[E + e];
+  if (src < 0 || src >= N || dst < 0 || dst >= N) return;
+  if (dist[dst] == h - 1 && dist[src] > h) dist[src] = h;
+}
+
+// sort key of node v: type * (L+2) + min(dist, L+1); unknown types (bucket T) share one key and stay last
+__global__ void k_hop_keys(const int64_t* __restrict__ node_type, const int32_t* __restrict__ dist, int64_t N, int T,
+                           int L, int32_t* __restrict__ keys, int32_t* __restrict__ vals, int32_t* __restrict__ counts) {
+  int64_t v = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  int32_t key = -1;
+  if (v < N) {
+    const int64_t t = node_type[v];
+    const int32_t b = min(dist[v], L + 1);
+    const bool known = t >= 0 && t < T;
+    keys[v] = known ? (int32_t)t * (L + 2) + b : T * (L + 2);
+    vals[v] = (int32_t)v;
+    if (known) key = keys[v];
+  }
+  const unsigned same = __match_any_sync(0xffffffffu, key);
+  if (key >= 0 && (int)(threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&counts[key], __popc(same));
+}
+
+__global__ void k_hop_nodes(const int32_t* __restrict__ hop_perm, const int64_t* __restrict__ node_type, int64_t N,
+                            int32_t* __restrict__ hop_rank, int64_t* __restrict__ hop_node_type) {
+  int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const int32_t v = hop_perm[j];
+  hop_rank[v] = (int32_t)j;
+  hop_node_type[j] = node_type[v];
+}
+
+// edges keep their order; endpoints become hop rows (invalid endpoints are flagged and raise before any use)
+__global__ void k_hop_edges(const int64_t* __restrict__ edge_index, int64_t N, int64_t E,
+                            const int32_t* __restrict__ hop_rank, int64_t* __restrict__ hop_edge_index) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= 2 * E) return;
+  const int64_t v = edge_index[i];
+  hop_edge_index[i] = (v >= 0 && v < N) ? hop_rank[v] : 0;
+}
+
+__global__ void k_hop_out_rows(const int64_t* __restrict__ out_nodes, int64_t n_out, int64_t N,
+                               const int32_t* __restrict__ hop_rank, int64_t* __restrict__ out_rows) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n_out) return;
+  const int64_t v = out_nodes[i];
+  out_rows[i] = (v >= 0 && v < N) ? hop_rank[v] : 0;
+}
+
+// key[c] of CSR positions whose destination lies in none of the ranges -> no_work_row
+__global__ void k_mask_rows(const int32_t* __restrict__ key, const int32_t* __restrict__ row_ptr,
+                            const int32_t* __restrict__ ranges, int n_ranges, int64_t E, int32_t no_work_row,
+                            int32_t* __restrict__ out) {
+  int64_t c = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (c >= E) return;
+  bool in = false;
+  for (int j = 0; j < n_ranges && !in; ++j) in = c >= row_ptr[ranges[2 * j]] && c < row_ptr[ranges[2 * j + 1]];
+  out[c] = in ? key[c] : no_work_row;
 }
 
 __global__ void k_gather_rows(const float4* __restrict__ in, const int32_t* __restrict__ perm, int64_t n_rows,
@@ -500,21 +633,22 @@ extern "C" int hgt_plan_tiles(const int32_t* row_ptr, int64_t n_nodes, int64_t n
   PlanScratch s;
   size_t need = carve(s, workspace, n_nodes, n_edges);
   HGT_REQUIRE(workspace_bytes >= need, "hgt_plan_tiles: workspace too small (%zu < %zu)", workspace_bytes, need);
+  const RowRanges all{nullptr, 0, n_nodes};
   int64_t* packed = s.packed;
   void* tmp = s.cub_tmp;
   size_t tmp_bytes = s.cub_bytes;
-  k_tile_emit_counts<<<blocks_for(n_nodes + 1), kThreads, 0, st>>>(row_ptr, n_nodes, tc, split_edges, packed);
+  k_tile_emit_counts<<<blocks_for(n_nodes + 1), kThreads, 0, st>>>(row_ptr, n_nodes, all, tc, split_edges, packed);
   HGT_LAUNCH_CHECK();
   HGT_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, (const int64_t*)packed, packed,
                                                (int)(n_nodes + 1), st));
-  k_tile_write<<<blocks_for(n_nodes + 1), kThreads, 0, st>>>(row_ptr, n_nodes, tc, split_edges, packed, tiles,
+  k_tile_write<<<blocks_for(n_nodes + 1), kThreads, 0, st>>>(row_ptr, n_nodes, all, tc, split_edges, packed, tiles,
                                                              max_tiles, d_n_tiles, hubs, max_hubs);
   HGT_LAUNCH_CHECK();
   if (h_n_tiles == nullptr) {
     // sync-free mode: the counts stay on the device (the edge kernels read them through d_tile_counts); tile slots past
     // max_tiles are never written (k_tile_write clamps), so callers size max_tiles / max_hubs with the documented bounds
     if (max_tiles > 0) {
-      k_tile_close<<<blocks_for(max_tiles), kThreads, 0, st>>>(row_ptr, n_nodes, tiles, d_n_tiles);
+      k_tile_close<<<blocks_for(max_tiles), kThreads, 0, st>>>(row_ptr, all, tiles, d_n_tiles);
       HGT_LAUNCH_CHECK();
     }
     return 0;
@@ -526,7 +660,111 @@ extern "C" int hgt_plan_tiles(const int32_t* row_ptr, int64_t n_nodes, int64_t n
   HGT_REQUIRE(h_n_tiles[2] <= max_hubs, "hgt_plan_tiles: %d hubs exceed max_hubs=%lld", h_n_tiles[2],
               (long long)max_hubs);
   if (h_n_tiles[0] > 0) {
-    k_tile_close<<<blocks_for(h_n_tiles[0]), kThreads, 0, st>>>(row_ptr, n_nodes, tiles, d_n_tiles);
+    k_tile_close<<<blocks_for(h_n_tiles[0]), kThreads, 0, st>>>(row_ptr, all, tiles, d_n_tiles);
+    HGT_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+extern "C" int hgt_plan_range_tiles(const int32_t* row_ptr, int64_t n_nodes, int64_t n_edges, const int32_t* ranges,
+                                    int32_t n_ranges, int64_t n_range_rows, int32_t target_edges, int32_t split_edges,
+                                    int32_t* tiles, int64_t max_tiles, int32_t* hubs, int64_t max_hubs,
+                                    int32_t* d_n_tiles, void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  HGT_REQUIRE(target_edges >= 1 && split_edges >= 1, "hgt_plan_range_tiles: bad tile parameters");
+  HGT_REQUIRE(n_ranges >= 0 && (n_ranges == 0 || ranges) && n_range_rows >= 0 && n_range_rows <= n_nodes,
+              "hgt_plan_range_tiles: bad ranges (n_ranges=%d, n_range_rows=%lld, n_nodes=%lld)", n_ranges,
+              (long long)n_range_rows, (long long)n_nodes);
+  HGT_CHECK_CUDA(cudaMemsetAsync(d_n_tiles, 0, 3 * sizeof(int32_t), st));
+  if (n_range_rows == 0) return 0;
+  PlanScratch s;
+  size_t need = carve(s, workspace, n_nodes, n_edges);
+  HGT_REQUIRE(workspace_bytes >= need, "hgt_plan_range_tiles: workspace too small (%zu < %zu)", workspace_bytes, need);
+  const RowRanges rr{ranges, n_ranges, n_nodes};
+  const int tc = 2 * target_edges;
+  size_t tmp_bytes = s.cub_bytes;
+  k_tile_emit_counts<<<blocks_for(n_range_rows + 1), kThreads, 0, st>>>(row_ptr, n_range_rows, rr, tc, split_edges,
+                                                                        s.packed);
+  HGT_LAUNCH_CHECK();
+  HGT_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(s.cub_tmp, tmp_bytes, (const int64_t*)s.packed, s.packed,
+                                               (int)(n_range_rows + 1), st));
+  k_tile_write<<<blocks_for(n_range_rows + 1), kThreads, 0, st>>>(row_ptr, n_range_rows, rr, tc, split_edges, s.packed,
+                                                                  tiles, max_tiles, d_n_tiles, hubs, max_hubs);
+  HGT_LAUNCH_CHECK();
+  if (max_tiles > 0) {
+    k_tile_close<<<blocks_for(max_tiles), kThreads, 0, st>>>(row_ptr, rr, tiles, d_n_tiles);
+    HGT_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+extern "C" int hgt_plan_mask_rows(const int32_t* key, const int32_t* row_ptr, const int32_t* ranges, int32_t n_ranges,
+                                  int64_t n_edges, int32_t no_work_row, int32_t* out_key, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  HGT_REQUIRE(n_edges == 0 || (key && row_ptr && out_key && (n_ranges == 0 || ranges)),
+              "hgt_plan_mask_rows: NULL argument");
+  if (n_edges == 0) return 0;
+  k_mask_rows<<<blocks_for(n_edges), kThreads, 0, st>>>(key, row_ptr, ranges, n_ranges, n_edges, no_work_row, out_key);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int hgt_trim_layout(const int64_t* edge_index, const int64_t* edge_type, const int64_t* edge_time,
+                               const int64_t* node_type, int64_t n_nodes, int64_t n_edges, int32_t num_types,
+                               int32_t num_relations, const int64_t* out_nodes, int64_t n_out, int32_t n_layers,
+                               int32_t* dist, int32_t* hop_perm, int32_t* hop_rank, int64_t* hop_node_type,
+                               int64_t* hop_edge_index, int64_t* out_rows, int32_t* meta, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  const int T = num_types, R = num_relations, L = n_layers;
+  HGT_REQUIRE(T >= 1 && T <= 4096 && R >= 1 && L >= 1 && L <= 64, "hgt_trim_layout: T=%d R=%d L=%d unsupported", T, R, L);
+  HGT_REQUIRE((int64_t)T * (L + 2) < (1ll << 30), "hgt_trim_layout: T*(L+2) too large");
+  HGT_REQUIRE(meta && (n_nodes == 0 || (node_type && dist && hop_perm && hop_rank && hop_node_type)) &&
+                  (n_edges == 0 || (edge_index && edge_type && hop_edge_index)) && (n_out == 0 || (out_nodes && out_rows)),
+              "hgt_trim_layout: NULL argument");
+  PlanScratch s;
+  size_t need = carve(s, workspace, n_nodes, n_edges);
+  HGT_REQUIRE(workspace_bytes >= need, "hgt_trim_layout: workspace too small (%zu < %zu)", workspace_bytes, need);
+  const int n_counts = T * (L + 2);
+  int32_t* counts = meta;
+  int32_t* presence = meta + n_counts;
+  int32_t* flags = presence + T * R;
+  HGT_CHECK_CUDA(cudaMemsetAsync(meta, 0, sizeof(int32_t) * (n_counts + T * R + 4), st));
+  const int64_t n_init = n_nodes > n_out ? n_nodes : n_out;
+  if (n_init > 0) {
+    k_hop_init<<<blocks_for(n_init), kThreads, 0, st>>>(out_nodes, n_out, n_nodes, L + 1, dist, flags);
+    HGT_LAUNCH_CHECK();
+  }
+  if (n_out > 0) {
+    k_hop_seeds<<<blocks_for(n_out), kThreads, 0, st>>>(out_nodes, n_out, n_nodes, dist);
+    HGT_LAUNCH_CHECK();
+  }
+  if (n_edges > 0) {
+    k_hop_edge_scan<<<blocks_for(n_edges), kThreads, 0, st>>>(edge_index, edge_type, edge_time, node_type, n_nodes,
+                                                              n_edges, T, R, presence, flags);
+    HGT_LAUNCH_CHECK();
+    for (int h = 1; h <= L; ++h) {
+      k_hop_pass<<<blocks_for(n_edges), kThreads, 0, st>>>(edge_index, n_nodes, n_edges, h, dist);
+      HGT_LAUNCH_CHECK();
+    }
+  }
+  if (n_nodes > 0) {
+    k_hop_keys<<<blocks_for(n_nodes), kThreads, 0, st>>>(node_type, dist, n_nodes, T, L, s.keys_in, s.vals_in, counts);
+    HGT_LAUNCH_CHECK();
+    size_t tmp = s.cub_bytes;
+    // LSD radix sort: stable, so within a (type, hop) bucket nodes keep their original order
+    HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, (const int32_t*)s.keys_in, s.keys_out,
+                                                   (const int32_t*)s.vals_in, hop_perm, (int)n_nodes, 0,
+                                                   bits_for((int64_t)n_counts + 1), st));
+    k_hop_nodes<<<blocks_for(n_nodes), kThreads, 0, st>>>(hop_perm, node_type, n_nodes, hop_rank, hop_node_type);
+    HGT_LAUNCH_CHECK();
+  }
+  if (n_edges > 0) {
+    k_hop_edges<<<blocks_for(2 * n_edges), kThreads, 0, st>>>(edge_index, n_nodes, n_edges, hop_rank, hop_edge_index);
+    HGT_LAUNCH_CHECK();
+  }
+  if (n_out > 0) {
+    k_hop_out_rows<<<blocks_for(n_out), kThreads, 0, st>>>(out_nodes, n_out, n_nodes, hop_rank, out_rows);
     HGT_LAUNCH_CHECK();
   }
   return 0;

@@ -37,23 +37,23 @@ class GNN(nn.Module):
             if isinstance(gc.base_conv, HGTConv) and type(gc.base_conv) is HGTConv:
                 gc.base_conv.emit_split = True
 
-    def _adapter_table(self, plan, dev):
-        key = ("adapter", self.in_dim, self.n_hid)
+    def _adapter_table(self, plan, dev, rows=None):
+        """Grouped-GEMM table of the input adapter over the first rows[t] nodes of every type (default: all of them)."""
+        rows = tuple(plan.type_count[:self.num_types] if rows is None else rows)
+        key = ("adapter", self.in_dim, self.n_hid, rows)
         table = plan._layer_tables.get(key)
         if table is None:
             groups, cblocks = [], []
             for t in range(self.num_types):
-                if plan.type_count[t]:
-                    groups.append((plan.type_row0[t], plan.type_count[t], t * self.n_hid, 1, len(cblocks), 1))
+                if rows[t]:
+                    groups.append((plan.type_row0[t], rows[t], t * self.n_hid, 1, len(cblocks), 1))
                     cblocks.append((plan.type_row0[t] * self.n_hid, self.n_hid))
             table = plan._layer_tables[key] = _plan._pack_groups(groups, cblocks, dev)
         return table
 
-    def _adapter_cuda(self, node_feature, node_type, edge_index, edge_type, edge_time):
+    def _adapter_cuda(self, node_feature, plan, rows=None):
         conv0 = self.gcs[0].base_conv
         T = self.num_types
-        plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if conv0.use_RTE else None, T,
-                              conv0.num_relations)
         dev, N = node_feature.device, plan.n_nodes
         st = torch.cuda.current_stream().cuda_stream
         x = node_feature.contiguous()
@@ -61,14 +61,15 @@ class GNN(nn.Module):
             xs = torch.empty_like(x)
             _lib.call("hgt_gather_rows", x.data_ptr(), plan.perm.data_ptr(), N, self.in_dim, xs.data_ptr(), st)
             x = xs
-        table = self._adapter_table(plan, dev)
+        table = self._adapter_table(plan, dev, rows)
         w_cat = torch.empty((T * self.n_hid, self.in_dim), dtype=torch.float32, device=dev)
         b_cat = torch.empty(T * self.n_hid, dtype=torch.float32, device=dev)
         wp = conv0._ptrs("adapt_w", [l.weight for l in self.adapt_ws], dev)
         bp = conv0._ptrs("adapt_b", [l.bias for l in self.adapt_ws], dev)
         _lib.call("hgt_concat_linears", wp.data_ptr(), bp.data_ptr(), T, self.n_hid, self.in_dim, w_cat.data_ptr(),
                   b_cat.data_ptr(), st)
-        res = torch.zeros((N, self.n_hid), dtype=torch.float32, device=dev)     # unknown-type rows stay 0 (model.py:70)
+        # unknown-type rows stay 0 (model.py:70), and so do the rows past `rows`
+        res = torch.zeros((N, self.n_hid), dtype=torch.float32, device=dev)
         conv0._typed_linear(x, self.in_dim, w_cat, b_cat, self.in_dim, self.n_hid, table, res, conv0.linear_impl, st)
         n_known = plan.type_row0[T]
         res[:n_known].tanh_()                                                    # model.py:75
@@ -76,37 +77,69 @@ class GNN(nn.Module):
             res = res.index_select(0, plan.rank.long())
         return res
 
-    def _adapter_autograd(self, node_feature, node_type, edge_index, edge_type, edge_time):
+    def _adapter_autograd(self, node_feature, plan, rows=None):
         """Training path of the adapter: the same grouped GEMM with its native backward (autograd._TypedLinear)."""
         from .autograd import typed_linear
         conv0 = self.gcs[0].base_conv
-        T = self.num_types
-        plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if conv0.use_RTE else None, T,
-                              conv0.num_relations)
+        T, h = self.num_types, self.n_hid
         N = plan.n_nodes
         x = node_feature if plan.sorted_types else node_feature.index_select(0, plan.perm.long())
-        table = self._adapter_table(plan, node_feature.device)
+        table = self._adapter_table(plan, node_feature.device, rows)
         w_cat = torch.cat([l.weight for l in self.adapt_ws], 0)
         b_cat = torch.cat([l.bias for l in self.adapt_ws], 0)
         n_known = plan.type_row0[T]
-        res = typed_linear(x, w_cat, b_cat, table, self.n_hid, N * self.n_hid, conv0.linear_impl, 0,
-                           ((n_known * self.n_hid, N * self.n_hid),)).view(N, self.n_hid)
+        zero = [((plan.type_row0[t] + rows[t]) * h, plan.type_row0[t + 1] * h) for t in range(T)] if rows else []
+        res = typed_linear(x, w_cat, b_cat, table, h, N * h, conv0.linear_impl, 0,
+                           zero + [(n_known * h, N * h)]).view(N, h)
         res = torch.cat([torch.tanh(res[:n_known]), res[n_known:]], 0) if n_known < N else torch.tanh(res)   # model.py:75
         if not plan.sorted_types:
             res = res.index_select(0, plan.rank.long())
         return res
 
-    def forward(self, node_feature, node_type, edge_time, edge_index, edge_type):
+    def forward(self, node_feature, node_type, edge_time, edge_index, edge_type, *, out_nodes=None):
+        """pyHGT/model.py:64-80.  `out_nodes` (optional): 1-D int64 CUDA tensor of node ids (original order, duplicates
+        allowed).  The call then returns only those rows, ``[len(out_nodes), n_hid]``, equal to ``forward(...)[out_nodes]``,
+        and computes every layer only over the nodes the requested rows depend on (trim.py: layer l of L over the nodes
+        within L - l hops of an out_nodes entry).  Inference and training both take this path; each layer's ``.att`` is
+        then None.  In train mode dropout still applies, but its masks are drawn over the trimmed shapes, so they differ
+        from those of the untrimmed call.  Only 'hgt' layers support it ('dense_hgt' raises ValueError)."""
         grad = torch.is_grad_enabled() and (node_feature.requires_grad or any(p.requires_grad for p in self.parameters()))
         if not node_feature.is_cuda:
             raise _lib.HgtError("pyhgt_b200.GNN runs on CUDA tensors only (got %s): there is no CPU fallback"
                                 % node_feature.device)
-        if grad:
-            res = self._adapter_autograd(node_feature, node_type, edge_index, edge_type, edge_time)
-        else:
-            res = self._adapter_cuda(node_feature, node_type, edge_index, edge_type, edge_time)
+        if out_nodes is not None:
+            return self._forward_trimmed(node_feature, node_type, edge_time, edge_index, edge_type, out_nodes, grad)
+        conv0 = self.gcs[0].base_conv
+        plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if conv0.use_RTE else None, self.num_types,
+                              conv0.num_relations)
+        res = self._adapter_autograd(node_feature, plan) if grad else self._adapter_cuda(node_feature, plan)
         meta_xs = self.drop(res)
         del res
         for gc in self.gcs:
             meta_xs = gc(meta_xs, node_type, edge_index, edge_type, edge_time)
         return meta_xs
+
+    def _forward_trimmed(self, node_feature, node_type, edge_time, edge_index, edge_type, out_nodes, grad):
+        from . import trim
+        if any(type(gc.base_conv) is not HGTConv for gc in self.gcs):
+            raise ValueError("GNN.forward(out_nodes=) supports conv_name='hgt' only")
+        if not out_nodes.is_cuda:
+            raise _lib.HgtError("out_nodes must be a CUDA tensor (got %s): there is no CPU fallback" % out_nodes.device)
+        if node_feature.dim() != 2 or node_feature.shape[0] != node_type.numel():
+            raise ValueError("node_feature must be [N, in_dim] with N = len(node_type), got %s"
+                             % (tuple(node_feature.shape),))
+        if out_nodes.numel() == 0:
+            return node_feature.new_zeros((0, self.n_hid))
+        conv0 = self.gcs[0].base_conv
+        lay = trim.get_layout(node_type, edge_index, edge_type, edge_time if conv0.use_RTE else None, out_nodes,
+                              self.num_types, conv0.num_relations, len(self.gcs))
+        x = node_feature.index_select(0, lay.perm)                               # hop order
+        if grad:
+            res = self._adapter_autograd(x, lay.plan, lay.adapter_rows)
+        else:
+            res = self._adapter_cuda(x, lay.plan, lay.adapter_rows)
+        meta_xs = self.drop(res)
+        del res
+        for gc, view in zip(self.gcs, lay.layers):
+            meta_xs = gc.base_conv._forward_view(meta_xs, view, edge_time)
+        return meta_xs.index_select(0, lay.out_rows)

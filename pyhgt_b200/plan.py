@@ -60,6 +60,8 @@ class GraphPlan:
     pair_rel_dev: torch.Tensor = None
     tile_counts_dev: torch.Tensor = None   # sync-free plans: device {n_tiles, n_split, n_hubs}; the host fields are bounds
     flags_dev: torch.Tensor = None         # sync-free plans: range-check flags left on the device (see check())
+    dst_ranges: torch.Tensor = None        # a trimmed layer's view (trim.py): [n, 2] int32 row ranges of the destinations
+    n_dst_ranges: int = 0                  # its tiles cover; the source index then holds only their edges
     _layer_tables: dict = field(default_factory=dict)
     _source_index: dict = field(default_factory=dict)   # "kv" / "rte" -> SourceIndex (deterministic backward)
 
@@ -82,8 +84,8 @@ _CACHE = []          # [(weakrefs, versions, key_extra, plan)], most recent last
 _CACHE_SIZE = 8
 
 
-def _cache_lookup(tensors, extra):
-    for entry in reversed(_CACHE):
+def _cache_lookup(tensors, extra, cache=_CACHE):
+    for entry in reversed(cache):
         refs, versions, ex, plan = entry
         if ex != extra:
             continue
@@ -102,12 +104,12 @@ def _cache_lookup(tensors, extra):
     return None
 
 
-def _cache_store(tensors, extra, plan):
+def _cache_store(tensors, extra, plan, cache=_CACHE, size=None):
     refs = [None if t is None else weakref.ref(t) for t in tensors]
     versions = [None if t is None else t._version for t in tensors]
-    _CACHE.append((refs, versions, extra, plan))
-    if len(_CACHE) > _CACHE_SIZE:
-        _CACHE.pop(0)
+    cache.append((refs, versions, extra, plan))
+    if len(cache) > (_CACHE_SIZE if size is None else size):
+        cache.pop(0)
 
 
 def clear_plan_cache():
@@ -331,6 +333,13 @@ def source_index(plan, which):
     E = plan.n_edges
     i32 = dict(dtype=torch.int32, device=dev)
     st = _stream()
+    if plan.dst_ranges is not None:
+        # a trimmed layer computes some destinations only: the other edges go to the no-work row, so the row pass never
+        # reads the softmax statistics or D of a destination the layer did not compute
+        masked = torch.empty(max(E, 1), **i32)
+        _lib.call("hgt_plan_mask_rows", key.data_ptr(), plan.row_ptr.data_ptr(), plan.dst_ranges.data_ptr(),
+                  plan.n_dst_ranges, E, n_rows, masked.data_ptr(), st)
+        key = masked
     ws_bytes = ctypes.c_size_t()
     _lib.call("hgt_plan_workspace_bytes", n_rows, E, ctypes.byref(ws_bytes))
     ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
