@@ -129,6 +129,28 @@ int hgt_trim_layout(const int64_t* edge_index, const int64_t* edge_type, const i
                     int64_t* hop_edge_index, int64_t* out_rows, int32_t* meta, void* workspace,
                     size_t workspace_bytes, void* stream);
 
+/* hgt_trim_layout with host-given slot sizes, so that every size derived from the layout is known on the host before
+ * the call and nothing needs reading back (a CUDA graph can capture it).  hop_bounds: host int32 [T, L+2].  The n_rows
+ * hop rows are, per type in type order, one region of hop_bounds[t][b] rows for every hop class b = 0..L+1, then a tail
+ * [sum of the bounds, n_rows) for the nodes of types outside [0,T).  The nodes of a class fill its region in
+ * hgt_trim_layout's order; unused rows are padding: hop_perm = n_nodes (gather from a zero row appended to
+ * node_feature), hop_node_type = the region's type (T in the tail), no edges.  A node that does not fit its region is
+ * dropped (hop_rank = -1): its edge endpoints and out_rows entries become the pad row n_rows-1, and no region is
+ * written past its end.  Dropping is harmless for hop class L+1 and the tail (no layer computes those rows or reads
+ * them as typed sources) when a tail row exists to serve as the pad; any other drop sets flags[3] (overflow).
+ * hop_perm, hop_node_type: [n_rows]; dist, hop_rank: [n_nodes]; hop_edge_index, out_rows as hgt_trim_layout.
+ * meta (int32) = [counts T*(L+2) | presence T*R | flags 4 | offsets T*(L+2)+2]: counts, presence and flags[0..2] as
+ * hgt_trim_layout (counts are the actual class sizes, whatever the bounds); offsets[k] the first row of region k,
+ * offsets[T*(L+2)] the tail's, offsets[T*(L+2)+1] = n_rows.  The bounds reach the device in kernel parameters, not by a
+ * host-memory copy.  With bounds equal to the counts and n_rows = n_nodes the outputs are hgt_trim_layout's, bitwise.
+ * n_rows >= the sum of the bounds, and >= 1 if n_nodes > 0.  workspace: hgt_plan_workspace_bytes(n_nodes, n_edges). */
+int hgt_trim_layout_bounded(const int64_t* edge_index, const int64_t* edge_type, const int64_t* edge_time,
+                            const int64_t* node_type, int64_t n_nodes, int64_t n_edges, int32_t num_types,
+                            int32_t num_relations, const int64_t* out_nodes, int64_t n_out, int32_t n_layers,
+                            const int32_t* hop_bounds, int64_t n_rows, int32_t* dist, int32_t* hop_perm,
+                            int32_t* hop_rank, int64_t* hop_node_type, int64_t* hop_edge_index, int64_t* out_rows,
+                            int32_t* meta, void* workspace, size_t workspace_bytes, void* stream);
+
 /* hgt_plan_tiles (sync-free mode, same tile / hub / count formats) over the destinations of n_ranges ascending, disjoint
  * row ranges ranges[2j] .. ranges[2j+1] (device int32 [n_ranges,2]) of row_ptr; n_range_rows = total rows in the ranges
  * (host).  No tile crosses a range end, so an edge kernel launched with these tiles reads and writes only the rows of

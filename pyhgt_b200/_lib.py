@@ -103,6 +103,8 @@ SIGNATURES = {
     "hgt_merge_batches": [_p, _i32, _i32, _p, _p, _i64, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p],
     # trimmed forward (GNN.forward(out_nodes=), trim.py)
     "hgt_trim_layout": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_trim_layout_bounded": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _i64, _p, _p, _p, _p, _p,
+                                _p, _p, _p, _sz, _p],
     "hgt_plan_range_tiles": [_p, _i64, _i64, _p, _i32, _i64, _i32, _i32, _p, _i64, _p, _i64, _p, _p, _sz, _p],
     "hgt_plan_mask_rows": [_p, _p, _p, _i32, _i64, _i32, _p, _p],
 }

@@ -317,30 +317,81 @@ __global__ void k_hop_keys(const int64_t* __restrict__ node_type, const int32_t*
   if (key >= 0 && (int)(threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&counts[key], __popc(same));
 }
 
-__global__ void k_hop_nodes(const int32_t* __restrict__ hop_perm, const int64_t* __restrict__ node_type, int64_t N,
-                            int32_t* __restrict__ hop_rank, int64_t* __restrict__ hop_node_type) {
-  int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (j >= N) return;
-  const int32_t v = hop_perm[j];
-  hop_rank[v] = (int32_t)j;
-  hop_node_type[j] = node_type[v];
+// Host slot offsets reach the device by value in the kernel's parameter block (as linear_bwd.cu's k_upload), so a CUDA
+// graph that captures the layout records them: no host-memory copy.
+constexpr int kOffChunk = 1000;
+struct OffChunk {
+  int32_t first, n;
+  int32_t v[kOffChunk];
+};
+static_assert(sizeof(OffChunk) <= 4096 - 16, "k_put_offsets' parameter block must stay under 4 KB");
+
+__global__ void k_put_offsets(const __grid_constant__ OffChunk c, int32_t* __restrict__ off) {
+  for (int i = threadIdx.x; i < c.n; i += blockDim.x) off[c.first + i] = c.v[i];
 }
 
-// edges keep their order; endpoints become hop rows (invalid endpoints are flagged and raise before any use)
+// Empty slots of a bounded layout: hop_perm = N (the zero row the caller appends to node_feature), the type of their
+// region (T in the tail).  Runs before k_hop_place, which overwrites the filled slots.
+__global__ void k_hop_slots(const int32_t* __restrict__ off, int n_keys, int L2, int T, int64_t N, int64_t n_rows,
+                            int32_t* __restrict__ hop_perm, int64_t* __restrict__ hop_node_type) {
+  int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (r >= n_rows) return;
+  int lo = 0, hi = n_keys;                                   // the last region k with off[k] <= r (k = n_keys: tail)
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (off[mid] <= r) lo = mid; else hi = mid - 1;
+  }
+  hop_perm[r] = (int32_t)N;
+  hop_node_type[r] = lo < n_keys ? lo / L2 : T;
+}
+
+// Slot of the node at sorted position j (key k, i.e. its (type, hop) class; k = n_keys: a type outside [0,T)): the
+// row off[k] + its index within the class, if that lies below off[k+1].  off == NULL (exact layout): every class starts
+// where it starts in the sorted order, so the row is j.  A node that does not fit is dropped (hop_rank -1): the caller
+// re-points its edges at the pad row n_rows-1.  That is harmless for the hop class L+1 and unknown types, whose rows no
+// layer computes or reads as typed sources, as long as a tail row exists to be the pad; anything else sets flags[3].
+__global__ void k_hop_place(const int32_t* __restrict__ keys, const int32_t* __restrict__ nodes, int64_t N,
+                            const int32_t* __restrict__ off, int n_keys, int L2, const int64_t* __restrict__ node_type,
+                            int32_t* __restrict__ hop_perm, int32_t* __restrict__ hop_rank,
+                            int64_t* __restrict__ hop_node_type, int32_t* __restrict__ flags) {
+  int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const int32_t k = keys[j], v = nodes[j];
+  int64_t lo = 0, hi = j;                                    // first sorted position of key k
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (keys[mid] < k) lo = mid + 1; else hi = mid;
+  }
+  const int64_t row = off ? off[k] + (j - lo) : j;
+  if (off == nullptr || row < off[k + 1]) {
+    hop_perm[row] = v;
+    hop_rank[v] = (int32_t)row;
+    hop_node_type[row] = node_type[v];
+    return;
+  }
+  hop_rank[v] = -1;
+  const bool unread = k == n_keys || k % L2 == L2 - 1;
+  if (!unread || off[n_keys + 1] <= off[n_keys]) flags[3] = 1;
+}
+
+// edges keep their order; endpoints become hop rows, dropped nodes the pad row (invalid endpoints are flagged and raise
+// before any use)
 __global__ void k_hop_edges(const int64_t* __restrict__ edge_index, int64_t N, int64_t E,
-                            const int32_t* __restrict__ hop_rank, int64_t* __restrict__ hop_edge_index) {
+                            const int32_t* __restrict__ hop_rank, int32_t pad_row, int64_t* __restrict__ hop_edge_index) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= 2 * E) return;
   const int64_t v = edge_index[i];
-  hop_edge_index[i] = (v >= 0 && v < N) ? hop_rank[v] : 0;
+  const int32_t r = (v >= 0 && v < N) ? hop_rank[v] : 0;
+  hop_edge_index[i] = r >= 0 ? r : pad_row;
 }
 
 __global__ void k_hop_out_rows(const int64_t* __restrict__ out_nodes, int64_t n_out, int64_t N,
-                               const int32_t* __restrict__ hop_rank, int64_t* __restrict__ out_rows) {
+                               const int32_t* __restrict__ hop_rank, int32_t pad_row, int64_t* __restrict__ out_rows) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n_out) return;
   const int64_t v = out_nodes[i];
-  out_rows[i] = (v >= 0 && v < N) ? hop_rank[v] : 0;
+  const int32_t r = (v >= 0 && v < N) ? hop_rank[v] : 0;
+  out_rows[i] = r >= 0 ? r : pad_row;
 }
 
 // key[c] of CSR positions whose destination lies in none of the ranges -> no_work_row
@@ -709,26 +760,63 @@ extern "C" int hgt_plan_mask_rows(const int32_t* key, const int32_t* row_ptr, co
   return 0;
 }
 
-extern "C" int hgt_trim_layout(const int64_t* edge_index, const int64_t* edge_type, const int64_t* edge_time,
-                               const int64_t* node_type, int64_t n_nodes, int64_t n_edges, int32_t num_types,
-                               int32_t num_relations, const int64_t* out_nodes, int64_t n_out, int32_t n_layers,
-                               int32_t* dist, int32_t* hop_perm, int32_t* hop_rank, int64_t* hop_node_type,
-                               int64_t* hop_edge_index, int64_t* out_rows, int32_t* meta, void* workspace,
-                               size_t workspace_bytes, void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+namespace {
+
+// The hop layout of hgt_trim_layout (bounds == NULL: every (type, hop) class gets exactly its own nodes, n_rows = N)
+// and hgt_trim_layout_bounded (host slot bounds, n_rows rows).  One BFS, one stable sort, one placement.
+int trim_layout(const char* fn, const int64_t* edge_index, const int64_t* edge_type, const int64_t* edge_time,
+                const int64_t* node_type, int64_t n_nodes, int64_t n_edges, int32_t num_types, int32_t num_relations,
+                const int64_t* out_nodes, int64_t n_out, int32_t n_layers, const int32_t* bounds, int64_t n_rows,
+                int32_t* dist, int32_t* hop_perm, int32_t* hop_rank, int64_t* hop_node_type, int64_t* hop_edge_index,
+                int64_t* out_rows, int32_t* meta, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   const int T = num_types, R = num_relations, L = n_layers;
-  HGT_REQUIRE(T >= 1 && T <= 4096 && R >= 1 && L >= 1 && L <= 64, "hgt_trim_layout: T=%d R=%d L=%d unsupported", T, R, L);
-  HGT_REQUIRE((int64_t)T * (L + 2) < (1ll << 30), "hgt_trim_layout: T*(L+2) too large");
-  HGT_REQUIRE(meta && (n_nodes == 0 || (node_type && dist && hop_perm && hop_rank && hop_node_type)) &&
+  HGT_REQUIRE(T >= 1 && T <= 4096 && R >= 1 && L >= 1 && L <= 64, "%s: T=%d R=%d L=%d unsupported", fn, T, R, L);
+  HGT_REQUIRE((int64_t)T * (L + 2) < (1ll << 30), "%s: T*(L+2) too large", fn);
+  HGT_REQUIRE(n_nodes >= 0 && n_edges >= 0 && n_out >= 0 && n_rows >= 0 && n_rows < 2147483000ll,
+              "%s: n_nodes=%lld n_edges=%lld n_out=%lld n_rows=%lld out of range", fn, (long long)n_nodes,
+              (long long)n_edges, (long long)n_out, (long long)n_rows);
+  HGT_REQUIRE(meta && (n_nodes == 0 || (node_type && dist && hop_rank)) &&
+                  (n_rows == 0 || (hop_perm && hop_node_type)) &&
                   (n_edges == 0 || (edge_index && edge_type && hop_edge_index)) && (n_out == 0 || (out_nodes && out_rows)),
-              "hgt_trim_layout: NULL argument");
+              "%s: NULL argument", fn);
   PlanScratch s;
   size_t need = carve(s, workspace, n_nodes, n_edges);
-  HGT_REQUIRE(workspace_bytes >= need, "hgt_trim_layout: workspace too small (%zu < %zu)", workspace_bytes, need);
+  HGT_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", fn, workspace_bytes, need);
   const int n_counts = T * (L + 2);
   int32_t* counts = meta;
   int32_t* presence = meta + n_counts;
   int32_t* flags = presence + T * R;
+  int32_t* off = nullptr;
+  if (bounds) {
+    // slot offsets: region (t, b) = [off[t*(L+2)+b], off[t*(L+2)+b+1]), the tail [off[n_counts], n_rows)
+    HGT_REQUIRE(n_nodes == 0 || n_rows >= 1, "%s: n_rows must be at least 1 (the pad row)", fn);
+    off = flags + 4;
+    int64_t row = 0;
+    OffChunk c;
+    c.first = 0;
+    c.n = 0;
+    for (int k = 0; k <= n_counts + 1; ++k) {
+      const int64_t v = k <= n_counts ? row : n_rows;
+      if (k < n_counts) {
+        HGT_REQUIRE(bounds[k] >= 0, "%s: hop bound %d of type %d is negative (%d)", fn, k % (L + 2), k / (L + 2),
+                    bounds[k]);
+        row += bounds[k];
+        HGT_REQUIRE(row < 2147483000ll, "%s: hop bounds sum past the int32 row range", fn);
+      }
+      if (k == n_counts + 1)
+        HGT_REQUIRE(n_rows >= row, "%s: n_rows=%lld is below the sum of the hop bounds (%lld)", fn, (long long)n_rows,
+                    (long long)row);
+      c.v[c.n++] = (int32_t)v;
+      if (c.n == kOffChunk || k == n_counts + 1) {
+        k_put_offsets<<<1, 256, 0, st>>>(c, off);
+        HGT_LAUNCH_CHECK();
+        c.first += c.n;
+        c.n = 0;
+      }
+    }
+  } else {
+    HGT_REQUIRE(n_rows == n_nodes, "%s: n_rows must equal n_nodes", fn);
+  }
   HGT_CHECK_CUDA(cudaMemsetAsync(meta, 0, sizeof(int32_t) * (n_counts + T * R + 4), st));
   const int64_t n_init = n_nodes > n_out ? n_nodes : n_out;
   if (n_init > 0) {
@@ -748,26 +836,61 @@ extern "C" int hgt_trim_layout(const int64_t* edge_index, const int64_t* edge_ty
       HGT_LAUNCH_CHECK();
     }
   }
+  if (off && n_rows > 0) {
+    k_hop_slots<<<blocks_for(n_rows), kThreads, 0, st>>>(off, n_counts, L + 2, T, n_nodes, n_rows, hop_perm,
+                                                         hop_node_type);
+    HGT_LAUNCH_CHECK();
+  }
   if (n_nodes > 0) {
     k_hop_keys<<<blocks_for(n_nodes), kThreads, 0, st>>>(node_type, dist, n_nodes, T, L, s.keys_in, s.vals_in, counts);
     HGT_LAUNCH_CHECK();
     size_t tmp = s.cub_bytes;
     // LSD radix sort: stable, so within a (type, hop) bucket nodes keep their original order
+    int32_t* sorted_nodes = s.counts;                        // [N+2] int32, otherwise unused here
     HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, (const int32_t*)s.keys_in, s.keys_out,
-                                                   (const int32_t*)s.vals_in, hop_perm, (int)n_nodes, 0,
+                                                   (const int32_t*)s.vals_in, sorted_nodes, (int)n_nodes, 0,
                                                    bits_for((int64_t)n_counts + 1), st));
-    k_hop_nodes<<<blocks_for(n_nodes), kThreads, 0, st>>>(hop_perm, node_type, n_nodes, hop_rank, hop_node_type);
+    k_hop_place<<<blocks_for(n_nodes), kThreads, 0, st>>>(s.keys_out, sorted_nodes, n_nodes, off, n_counts, L + 2,
+                                                          node_type, hop_perm, hop_rank, hop_node_type, flags);
     HGT_LAUNCH_CHECK();
   }
+  const int32_t pad_row = n_rows > 0 ? (int32_t)(n_rows - 1) : 0;
   if (n_edges > 0) {
-    k_hop_edges<<<blocks_for(2 * n_edges), kThreads, 0, st>>>(edge_index, n_nodes, n_edges, hop_rank, hop_edge_index);
+    k_hop_edges<<<blocks_for(2 * n_edges), kThreads, 0, st>>>(edge_index, n_nodes, n_edges, hop_rank, pad_row,
+                                                              hop_edge_index);
     HGT_LAUNCH_CHECK();
   }
   if (n_out > 0) {
-    k_hop_out_rows<<<blocks_for(n_out), kThreads, 0, st>>>(out_nodes, n_out, n_nodes, hop_rank, out_rows);
+    k_hop_out_rows<<<blocks_for(n_out), kThreads, 0, st>>>(out_nodes, n_out, n_nodes, hop_rank, pad_row, out_rows);
     HGT_LAUNCH_CHECK();
   }
   return 0;
+}
+
+}  // namespace
+
+extern "C" int hgt_trim_layout(const int64_t* edge_index, const int64_t* edge_type, const int64_t* edge_time,
+                               const int64_t* node_type, int64_t n_nodes, int64_t n_edges, int32_t num_types,
+                               int32_t num_relations, const int64_t* out_nodes, int64_t n_out, int32_t n_layers,
+                               int32_t* dist, int32_t* hop_perm, int32_t* hop_rank, int64_t* hop_node_type,
+                               int64_t* hop_edge_index, int64_t* out_rows, int32_t* meta, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  return trim_layout("hgt_trim_layout", edge_index, edge_type, edge_time, node_type, n_nodes, n_edges, num_types,
+                     num_relations, out_nodes, n_out, n_layers, nullptr, n_nodes, dist, hop_perm, hop_rank,
+                     hop_node_type, hop_edge_index, out_rows, meta, workspace, workspace_bytes, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_trim_layout_bounded(const int64_t* edge_index, const int64_t* edge_type, const int64_t* edge_time,
+                                       const int64_t* node_type, int64_t n_nodes, int64_t n_edges, int32_t num_types,
+                                       int32_t num_relations, const int64_t* out_nodes, int64_t n_out, int32_t n_layers,
+                                       const int32_t* hop_bounds, int64_t n_rows, int32_t* dist, int32_t* hop_perm,
+                                       int32_t* hop_rank, int64_t* hop_node_type, int64_t* hop_edge_index,
+                                       int64_t* out_rows, int32_t* meta, void* workspace, size_t workspace_bytes,
+                                       void* stream_) {
+  HGT_REQUIRE(hop_bounds, "hgt_trim_layout_bounded: NULL hop_bounds");
+  return trim_layout("hgt_trim_layout_bounded", edge_index, edge_type, edge_time, node_type, n_nodes, n_edges,
+                     num_types, num_relations, out_nodes, n_out, n_layers, hop_bounds, n_rows, dist, hop_perm, hop_rank,
+                     hop_node_type, hop_edge_index, out_rows, meta, workspace, workspace_bytes, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_gather_rows(const float* in, const int32_t* perm, int64_t n_rows, int32_t width, float* out,

@@ -252,11 +252,28 @@ class GraphedForward(_Graphed):
         sig = GraphSignature(type_counts=[...], n_edges=..., pairs=[...], num_relations=R, feat_dim=F)
         g = GraphedForward(lambda x, nt, tm, ei, et: gnn(x, nt, tm, ei, et), sig, device)
         out = g(node_feature, node_type, edge_time, edge_index, edge_type)     # one batch, host or device tensors
+
+    With per_node=False, `fn` returns rows of its own choosing and the call returns (a copy of) them as they are, e.g. a
+    trimmed forward of the first C papers:
+
+        rows = torch.arange(C, device=device) + int(sig.row0[paper])
+        seeds = [torch.arange(C, device=device) + p0 for p0 in first_paper_row_of_each_batch]
+        tsig = trim.TrimSignature.for_batches(batches, seeds, n_layers, 0.1, num_types=T, num_relations=R)
+        g = GraphedForward(lambda x, nt, tm, ei, et: gnn(x, nt, tm, ei, et, out_nodes=rows, trim_signature=tsig),
+                           sig, device, per_node=False)
+
+    The trimmed layout is then laid out inside the graph, for every replayed batch.  Size the signature with the rows the
+    graph requests, C per batch: when a batch has fewer than C papers, the rows past them are padding nodes, but they are
+    still out_nodes, so they sit in hop class 0 and take slots of hop_bounds[paper][0] (their own output rows are
+    padding).  Sized on fewer seeds, such a batch overflows and the call returns NaN rows.  The layout built inside the
+    graph is not reachable from the host, so to find out why a replay returned NaN, rebuild it eagerly on the static
+    buffers and check it: trim.get_layout(g.nt, g.ei, g.et, g.tm, rows, T, R, n_layers, tsig, g.plan.pairs).check().
     """
 
-    def __init__(self, fn, sig, device):
+    def __init__(self, fn, sig, device, per_node=True):
         super().__init__(sig, device)
         self.fn = fn
+        self.per_node = bool(per_node)
         self.out = None
 
     def _run(self):
@@ -275,7 +292,7 @@ class GraphedForward(_Graphed):
                     self._run()
                 self.out = self._capture(self._run)
             self.graph.replay()
-            res = self.out.index_select(0, idx)
+            res = self.out.index_select(0, idx) if self.per_node else self.out.clone()
         cur.wait_stream(self.stream)
         res.record_stream(cur)
         return res

@@ -96,19 +96,28 @@ class GNN(nn.Module):
             res = res.index_select(0, plan.rank.long())
         return res
 
-    def forward(self, node_feature, node_type, edge_time, edge_index, edge_type, *, out_nodes=None):
+    def forward(self, node_feature, node_type, edge_time, edge_index, edge_type, *, out_nodes=None, trim_signature=None):
         """pyHGT/model.py:64-80.  `out_nodes` (optional): 1-D int64 CUDA tensor of node ids (original order, duplicates
         allowed).  The call then returns only those rows, ``[len(out_nodes), n_hid]``, equal to ``forward(...)[out_nodes]``,
         and computes every layer only over the nodes the requested rows depend on (trim.py: layer l of L over the nodes
         within L - l hops of an out_nodes entry).  Inference and training both take this path; each layer's ``.att`` is
         then None.  In train mode dropout still applies, but its masks are drawn over the trimmed shapes, so they differ
-        from those of the untrimmed call.  Only 'hgt' layers support it ('dense_hgt' raises ValueError)."""
+        from those of the untrimmed call.  Only 'hgt' layers support it ('dense_hgt' raises ValueError).
+
+        `trim_signature` (optional, with out_nodes): a trim.TrimSignature.  The layout of a new batch is then built
+        without reading anything back (its pairs come from the batch's cached plan, which sample_subgraph(s)_cuda,
+        merge_batches and the graphed classes leave), so the call can be captured in a CUDA graph.  Rows are padded to
+        the bounds; padding changes no real row.  If a (type, hop) class of the batch exceeds its bound or an out_nodes id
+        is out of range, every returned row is NaN and the layout's check() raises (trim.get_layout(...).check())."""
         grad = torch.is_grad_enabled() and (node_feature.requires_grad or any(p.requires_grad for p in self.parameters()))
         if not node_feature.is_cuda:
             raise _lib.HgtError("pyhgt_b200.GNN runs on CUDA tensors only (got %s): there is no CPU fallback"
                                 % node_feature.device)
         if out_nodes is not None:
-            return self._forward_trimmed(node_feature, node_type, edge_time, edge_index, edge_type, out_nodes, grad)
+            return self._forward_trimmed(node_feature, node_type, edge_time, edge_index, edge_type, out_nodes, grad,
+                                         trim_signature)
+        if trim_signature is not None:
+            raise ValueError("trim_signature needs out_nodes")
         conv0 = self.gcs[0].base_conv
         plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if conv0.use_RTE else None, self.num_types,
                               conv0.num_relations)
@@ -119,7 +128,7 @@ class GNN(nn.Module):
             meta_xs = gc(meta_xs, node_type, edge_index, edge_type, edge_time)
         return meta_xs
 
-    def _forward_trimmed(self, node_feature, node_type, edge_time, edge_index, edge_type, out_nodes, grad):
+    def _forward_trimmed(self, node_feature, node_type, edge_time, edge_index, edge_type, out_nodes, grad, tsig=None):
         from . import trim
         if any(type(gc.base_conv) is not HGTConv for gc in self.gcs):
             raise ValueError("GNN.forward(out_nodes=) supports conv_name='hgt' only")
@@ -131,9 +140,17 @@ class GNN(nn.Module):
         if out_nodes.numel() == 0:
             return node_feature.new_zeros((0, self.n_hid))
         conv0 = self.gcs[0].base_conv
-        lay = trim.get_layout(node_type, edge_index, edge_type, edge_time if conv0.use_RTE else None, out_nodes,
-                              self.num_types, conv0.num_relations, len(self.gcs))
-        x = node_feature.index_select(0, lay.perm)                               # hop order
+        tm = edge_time if conv0.use_RTE else None
+        pairs = None
+        if tsig is not None:
+            # the pairs of the batch's cached plan (a batch without one costs one read-back here)
+            pairs = _plan.get_plan(node_type, edge_index, edge_type, tm, self.num_types, conv0.num_relations).pairs
+        lay = trim.get_layout(node_type, edge_index, edge_type, tm, out_nodes, self.num_types, conv0.num_relations,
+                              len(self.gcs), tsig, pairs)
+        if lay.padded:                                                           # hop order; padding rows are zero
+            x = node_feature.index_select(0, lay.gather).masked_fill_(lay.pad_rows, 0.0)
+        else:
+            x = node_feature.index_select(0, lay.perm)                           # hop order
         if grad:
             res = self._adapter_autograd(x, lay.plan, lay.adapter_rows)
         else:
@@ -142,4 +159,7 @@ class GNN(nn.Module):
         del res
         for gc, view in zip(self.gcs, lay.layers):
             meta_xs = gc.base_conv._forward_view(meta_xs, view, edge_time)
-        return meta_xs.index_select(0, lay.out_rows)
+        out = meta_xs.index_select(0, lay.out_rows)
+        if lay.padded:                                          # overflow / bad ids: NaN rows instead of a host sync
+            out = torch.where(lay.bad, torch.full_like(out, float("nan")), out)
+        return out
