@@ -1,10 +1,10 @@
 """bf16 gather tables under torch.autocast(dtype=torch.bfloat16): the bf16-output typed GEMM, the edge forward / backward on
 bf16 [K'|V'] and RTE tables, the layers that use them, and the switch that selects them.
 
-What each deliberate fault is caught by:
+What each deliberate fault is caught by (the edge tests are in tests/test_gpu_edge_instances.py):
   truncation instead of round-to-nearest-even in the GEMM epilogue   test_gemm_bf16_output_equals_rounded_fp32
-  fp32 row stride in the bf16 gather                                 test_edge_forward_bf16_matches_fp64
-  the RTE table read as fp32 in the backward                         test_edge_backward_bf16_matches_fp64 (rte=True)
+  fp32 row stride in the bf16 gather                                 test_edge_forward_matches_fp64 (dtype bf16)
+  the RTE table read as fp32 in the backward                         test_edge_backward_matches_fp64 (bf16, rte=True)
 """
 import ctypes
 import contextlib
@@ -16,7 +16,7 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 from pyhgt_b200 import _lib, plan as P, synth          # noqa: E402
-from pyhgt_b200.autograd import _edge_backward_det     # noqa: E402
+from tests.test_gpu_edge_instances import _edge_ref    # noqa: E402
 
 BF16 = torch.bfloat16
 # Deviation of a layer's output from the fp32 path with bf16 tables (8-bit mantissa of K' / V'): max-abs over LayerNorm'd
@@ -109,154 +109,8 @@ def test_gemm_bf16_output_equals_rounded_fp32(path, K, width, ms, shared):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# 2. / 3. edge forward and backward on bf16 tables against float64 on the same tables, widened
-
-def _graph(T, R, n_nodes=900, n_edges=6000, hub_edges=2500, seed=0):
-    """Random typed graph with one hub destination above the split threshold."""
-    g = synth.make_random(n_nodes, n_edges, T, R, seed=seed, self_loops=20)
-    gen = torch.Generator().manual_seed(seed + 1)
-    hub = 3
-    src = torch.cat([g.edge_index[0], torch.randint(0, n_nodes, (hub_edges,), generator=gen)])
-    dst = torch.cat([g.edge_index[1], torch.full((hub_edges,), hub, dtype=torch.int64)])
-    g.edge_index = torch.stack([src, dst])
-    g.edge_type = torch.cat([g.edge_type, torch.randint(0, R, (hub_edges,), generator=gen)])
-    g.edge_time = torch.cat([g.edge_time, torch.randint(0, 240, (hub_edges,), generator=gen)])
-    assert hub_edges > P.TILE_SPLIT_EDGES
-    return g
-
-
-def _tables(plan, d, rte, seed):
-    """Q fp32 [N, d] and bf16 [K'|V'] / RTE tables with their trailing all-zero row."""
-    dev = _dev()
-    gen = torch.Generator().manual_seed(seed)
-    q = torch.randn(plan.n_nodes, d, generator=gen).to(dev)
-    kv = torch.randn(plan.kv_rows + 1, 2 * d, generator=gen).to(BF16).to(dev)
-    kv[-1].zero_()
-    kvr = None
-    if rte:
-        kvr = (0.5 * torch.randn(plan.n_pairs * P.RTE_MAX_LEN + 1, 2 * d, generator=gen)).to(BF16).to(dev)
-        kvr[-1].zero_()
-    return q, kv, kvr
-
-
-def _edge_ref(plan, q, kv, kvr, H):
-    """float64 edge attention on the given (widened) tables: agg [N, d], att per CSR position [E, H], (m, l) [N, H]."""
-    N, d = q.shape
-    dk = d // H
-    rp = plan.row_ptr.cpu().long()
-    E = int(rp[-1])
-    dst = torch.repeat_interleave(torch.arange(N), rp[1:] - rp[:-1])
-    kr = plan.kv_row[:E].cpu().long()
-    kk, vv = kv[kr, :d], kv[kr, d:]
-    if kvr is not None:
-        rr = plan.rte_row[:E].cpu().long()
-        kk, vv = kk + kvr[rr, :d], vv + kvr[rr, d:]
-    s = (q[dst].view(E, H, dk) * kk.view(E, H, dk)).sum(-1)
-    m = torch.full((N, H), -float("inf"), dtype=s.dtype).index_reduce_(0, dst, s.detach(), "amax")
-    p = torch.exp(s - m[dst])
-    l = torch.zeros(N, H, dtype=s.dtype).index_add(0, dst, p)
-    att = p / (l[dst] + 1e-16)
-    agg = torch.zeros(N, H, dk, dtype=s.dtype).index_add(0, dst, att[:, :, None] * vv.view(E, H, dk)).view(N, d)
-    return agg, att, m, l
-
-
-EDGE_SHAPES = [(16, 4), (64, 4), (100, 4), (96, 3), (250, 5)]     # d_k = 4, 16, 25, 32, 50; odd head counts
-
-
-@pytest.mark.parametrize("variant", [1, 2])
-@pytest.mark.parametrize("d,H", EDGE_SHAPES)
-@pytest.mark.parametrize("rte", [False, True])
-def test_edge_forward_bf16_matches_fp64(variant, d, H, rte):
-    dev = _dev()
-    T, R = 3, 2
-    g = _graph(T, R, seed=d + H)
-    plan = P.build_plan(g.node_type.to(dev), g.edge_index.to(dev), g.edge_type.to(dev),
-                        g.edge_time.to(dev) if rte else None, T, R)
-    assert plan.n_split > 0
-    q, kv, kvr = _tables(plan, d, rte, seed=d)
-    N, E = plan.n_nodes, plan.n_edges
-    agg = torch.full((N, d), float("nan"), device=dev)
-    att = torch.empty(E, H, device=dev)
-    stats = torch.empty(N, 2 * H, device=dev)
-    wsb = ctypes.c_size_t()
-    _lib.call("hgt_edge_workspace_bytes", plan.n_split, d, H, ctypes.byref(wsb))
-    ws = torch.empty(wsb.value, dtype=torch.uint8, device=dev)
-    _lib.call("hgt_edge_forward_bf16", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
-              plan.kv_row.data_ptr(), plan.rte_row.data_ptr() if rte else None, plan.csr_eid.data_ptr(),
-              plan.tiles.data_ptr(), plan.n_tiles, plan.n_split, plan.hubs.data_ptr(), plan.n_hubs, N, E, d, H, 0,
-              agg.data_ptr(), att.data_ptr(), stats.data_ptr(), None, None, ws.data_ptr(), ws.numel(), variant,
-              _lib.ptr(plan.tile_counts_dev), plan.type_row0_dev.data_ptr(), T, None, _st())
-    torch.cuda.synchronize()
-    ref, att_ref, m_ref, l_ref = _edge_ref(plan, q.cpu().double(), kv.cpu().double(),
-                                           None if kvr is None else kvr.cpu().double(), H)
-    has_in = (plan.row_ptr[1:] - plan.row_ptr[:-1]).cpu() > 0
-    torch.testing.assert_close(agg.cpu().double(), ref, rtol=1e-4, atol=1e-5)
-    eid = plan.csr_eid[:E].cpu().long()
-    torch.testing.assert_close(att.cpu().double()[eid], att_ref, rtol=1e-4, atol=1e-6)
-    torch.testing.assert_close(stats[:, :H].cpu().double()[has_in], m_ref[has_in], rtol=1e-5, atol=1e-5)
-    torch.testing.assert_close(stats[:, H:].cpu().double()[has_in], l_ref[has_in], rtol=1e-4, atol=1e-5)
-
-
-def _max_err(got, ref):
-    return float((got.double() - ref).abs().max() / ref.abs().max().clamp_min(1.0))
-
-
-@pytest.mark.parametrize("det", [False, True])
-@pytest.mark.parametrize("d,H", EDGE_SHAPES)
-@pytest.mark.parametrize("rte", [False, True])
-def test_edge_backward_bf16_matches_fp64(det, d, H, rte):
-    dev = _dev()
-    T, R = 3, 2
-    g = _graph(T, R, seed=2 * d + H)
-    plan = P.build_plan(g.node_type.to(dev), g.edge_index.to(dev), g.edge_type.to(dev),
-                        g.edge_time.to(dev) if rte else None, T, R)
-    q, kv, kvr = _tables(plan, d, rte, seed=d + 1)
-    N, E = plan.n_nodes, plan.n_edges
-    agg = torch.empty(N, d, device=dev)
-    stats = torch.empty(N, 2 * H, device=dev)
-    wsb = ctypes.c_size_t()
-    _lib.call("hgt_edge_workspace_bytes", plan.n_split, d, H, ctypes.byref(wsb))
-    ws = torch.empty(wsb.value, dtype=torch.uint8, device=dev)
-    _lib.call("hgt_edge_forward_bf16", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
-              plan.kv_row.data_ptr(), plan.rte_row.data_ptr() if rte else None, plan.csr_eid.data_ptr(),
-              plan.tiles.data_ptr(), plan.n_tiles, plan.n_split, plan.hubs.data_ptr(), plan.n_hubs, N, E, d, H, 0,
-              agg.data_ptr(), None, stats.data_ptr(), None, None, ws.data_ptr(), ws.numel(), 0,
-              _lib.ptr(plan.tile_counts_dev), plan.type_row0_dev.data_ptr(), T, None, _st())
-    dagg = torch.randn(N, d, generator=torch.Generator().manual_seed(5)).to(dev)
-
-    def run():
-        dq = torch.empty(N, d, device=dev)
-        dkv = torch.empty(plan.kv_rows + 1, 2 * d, device=dev)
-        dkvr = torch.empty_like(kvr, dtype=torch.float32) if rte else None
-        if det:
-            _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, "_bf16")
-        else:
-            w2 = torch.empty(256, dtype=torch.uint8, device=dev)
-            _lib.call("hgt_edge_backward_bf16", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(),
-                      dagg.data_ptr(), stats.data_ptr(), plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
-                      plan.rte_row.data_ptr() if rte else None, plan.tiles.data_ptr(), plan.n_tiles, N, d, H,
-                      plan.kv_rows + 1, kvr.shape[0] if rte else 0, dq.data_ptr(), dkv.data_ptr(), _lib.ptr(dkvr),
-                      w2.data_ptr(), w2.numel(), _lib.ptr(plan.tile_counts_dev), _st())
-        torch.cuda.synchronize()
-        return dq, dkv, dkvr
-
-    got = run()
-    q64 = q.cpu().double().requires_grad_(True)
-    kv64 = kv.cpu().double().requires_grad_(True)
-    kvr64 = kvr.cpu().double().requires_grad_(True) if rte else None
-    ref_agg, _, _, _ = _edge_ref(plan, q64, kv64, kvr64, H)
-    (ref_agg * dagg.cpu().double()).sum().backward()
-    rows = plan.kv_rows
-    assert _max_err(got[0].cpu(), q64.grad) <= 5e-5
-    assert _max_err(got[1][:rows].cpu(), kv64.grad[:rows]) <= 5e-5
-    if rte:
-        assert _max_err(got[2][:-1].cpu(), kvr64.grad[:-1]) <= 5e-5
-    if det:
-        again = run()
-        for a, b in zip(got, again):
-            if a is not None:
-                assert torch.equal(a, b)
-
+# 2. / 3. the edge forward and backward on bf16 tables against float64: tests/test_gpu_edge_instances.py, with the fp32
+# tables, at every <VEC, NCH> instance
 
 # ---------------------------------------------------------------------------------------------------------------------
 # 4. layers under bf16 autocast

@@ -11,6 +11,9 @@ The graphs have isolated destinations, self loops, duplicate edges and per-type 
 128, with one type of 37 nodes and one type with no nodes.  Two destinations lie above plan.TILE_SPLIT_EDGES, so the
 split-destination path (k_merge_partials in the forward, atomic dq in the backward) runs at every head width.
 """
+import contextlib
+import copy
+
 import pytest
 import torch
 
@@ -33,6 +36,11 @@ CASES = {
     "h6_d384": (384, 6, 3, 3, False, False),          # d_k 64: <4,4>; BN 128 with 3 column tiles
     "h1_d256": (256, 1, 3, 2, False, False),          # d_k 256: LPH 32, <4,2>
     "h32_d256_rte": (256, 32, 3, 2, True, True),      # d_k 8: LPH 1, <4,2>
+    "mag_d512_h8_rte": (512, 8, 4, 4, True, False),   # d_k 64: <4,4> with RTE on the fp32 register path (fewer than 2
+                                                      # TMA ring stages fit); update NV 4 / NPL 16; BN 256, 2 column tiles
+    "d1024_h8": (1024, 8, 3, 3, False, True),         # d_k 128: <4,8> (EDGE_UNROLL 1); update launch_vec<8>, NPL 32
+    "h3_d78_rte": (78, 3, 3, 4, True, False),         # d_k 26: <2,2>; the scalar update epilogue (d % 4 != 0) and SIMT
+                                                      # GEMMs in both runs (RTE's sinusoid table needs an even width)
 }
 
 # Relative-Frobenius bounds per tensor: (out and d node_inp, each parameter gradient), about 10x the worst error observed
@@ -51,6 +59,9 @@ FRO_BOUND = {
     "h6_d384": (3e-5, 1e-4),             # 2.6e-6, 1.2e-5
     "h1_d256": (3e-5, 1.5e-4),           # 2.1e-6, 1.3e-5 (skip)
     "h32_d256_rte": (3e-5, 1.5e-4),      # 2.4e-6, 1.3e-5 (skip)
+    "mag_d512_h8_rte": (4e-5, 1.5e-4),   # 3.7e-6, 1.2e-5
+    "d1024_h8": (5e-5, 2e-4),            # 5.0e-6, 1.8e-5 (relation_pri)
+    "h3_d78_rte": (2e-6, 2.5e-5),        # 1.4e-7, 2.3e-6 (skip; both runs SIMT)
 }
 
 
@@ -238,44 +249,111 @@ def test_unmatched_edges_backward_matches_float64(impl, monkeypatch):
     _compare_all("unmatched edges impl %d" % impl, native, ref, bounds)
 
 
+# The GNN recipes: name -> (in_dim, n_hid, n_heads, n_layers, use_RTE), with prev_norm and last_norm on.  Their graphs
+# are at _recipe_graph.  The bounds (out and d node_feature, parameters) are about 10x the worst relative Frobenius error
+# observed over both linear_impl runs and both settings of the deterministic flag on an H100 SXM (80 GB HBM3, 400 W
+# power limit), which the comment gives as (out / d node_feature, parameters).
+RECIPES = {
+    # 128 -> 256 into one HGTConv(256, 256, H=8) (edge backward <4,2>): the adapter's forward runs with BN 256, its dX
+    # and dW with BN 128 over K = 128
+    "adapter_128_256": ((128, 256, 8, 1, False), (5e-5, 1.5e-4)),      # 5.2e-6, 1.6e-5 (relation_pri)
+    # ogbn-mag (reference ogbn-mag/train_ogbn_mag.py): K = 129, so the adapter's forward runs the padded-K tensor-core GEMM
+    # (Kp = 136) and its backward the SIMT GEMMs (K % 16 != 0); edge <4,4> with RTE, on the fp32 register path
+    # because fewer than 2 TMA ring stages fit
+    "ogbn_mag": ((129, 512, 8, 4, True), (4e-5, 1.5e-4)),               # 3.8e-6, 1.5e-5 (relation_pri)
+    # OAG (reference OAG/train_paper_venue.py and train_paper_field.py; train_author_disambiguation.py runs 3 layers):
+    # in_dim 768 + 401 = 1169 (Kp = 1176), n_hid 400, edge <2,8>
+    "oag": ((1169, 400, 8, 4, True), (8e-5, 2e-4)),                     # 8.1e-6, 1.8e-5 (skip)
+    "oag_author_disambiguation": ((1169, 400, 8, 3, True), (8e-5, 2e-4)),  # 8.3e-6, 1.8e-5 (skip)
+}
+
+
+def _recipe_graph(name):
+    if name == "ogbn_mag":
+        # 1164 nodes of 4 types (institution 5), 12666 edges; Zipf destinations put two papers above TILE_SPLIT_EDGES
+        return synth.make_mag_shaped(scale=6e-4, seed=2, dst_zipf=1.2)
+    if name.startswith("oag"):
+        return synth.make_oag_shaped(seed=3, n_nodes=1200, n_edges=7000)     # 6 types, 10 relations incl. 'self'
+    return _graph(3, 4, 71, False)
+
+
+def _oracle_gnn(params, x, g, m):
+    """The GNN in float64: tanh(Linear_t(x)) (model.py:70-75), then hgt_forward_ref_port layer by layer."""
+    h = torch.zeros(g.num_nodes, m.n_hid, dtype=torch.float64)
+    for t in range(m.num_types):
+        sel = g.node_type == t
+        h[sel] = torch.tanh(x[sel] @ params["adapt_ws.%d.weight" % t].t() + params["adapt_ws.%d.bias" % t])
+    for i, gc in enumerate(m.gcs):
+        pre = "gcs.%d.base_conv." % i
+        h = _oracle_layer({k[len(pre):]: v for k, v in params.items() if k.startswith(pre)}, h, g, gc.base_conv)
+    return h
+
+
+def _recipe(name):
+    """Graph, GNN state, input, loss weight and the float64 result of one recipe (computed once for every run)."""
+    key = ("recipe", name)
+    if key not in _CACHE:
+        from pyhgt_b200.model import GNN
+        (F_in, d, H, L, rte), _ = RECIPES[name]
+        seed = sum(map(ord, name)) % 1000
+        g = _recipe_graph(name)
+        torch.manual_seed(seed)
+        m = _perturb(GNN(F_in, d, g.num_types, g.num_relations, H, L, 0.0, "hgt", True, True, rte), seed + 1)
+        x = torch.randn(g.num_nodes, F_in, generator=torch.Generator().manual_seed(seed + 2))
+        w = torch.randn(g.num_nodes, d, generator=torch.Generator().manual_seed(seed + 3))
+        params = _f64_params(m)
+        xr = x.double().requires_grad_(True)
+        out = _oracle_gnn(params, xr, g, m)
+        (out * w.double()).sum().backward()
+        ref = (out.detach(), xr.grad, {k: v.grad for k, v in params.items()})
+        _CACHE[key] = (g, m, x, w, ref)
+    return _CACHE[key]
+
+
+@contextlib.contextmanager
+def _deterministic(on):
+    prev = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(on)
+    try:
+        yield
+    finally:
+        torch.use_deterministic_algorithms(prev)
+
+
+@pytest.mark.parametrize("det", [False, True])
 @pytest.mark.parametrize("impl", [0, 1])
-def test_gnn_adapter_projection_k_neq_width_matches_float64(impl, monkeypatch):
-    """A projection with K != width on the training path: HGTConv itself needs in_dim == out_dim (the skip connection,
-    conv.py:131), so this is the GNN's typed input adapter, tanh(Linear_t(x)) with 128 -> 256, feeding one
-    HGTConv(256, 256, H=8) layer (edge backward <4,2>).  The adapter's forward runs with BN 256, its dX and dW with
-    BN 128 over K=128.  Worst relative Frobenius error observed on an H100: 5.1e-6 (out, d node_inp), 1.4e-5
-    (parameters: relation_pri, see FRO_BOUND for why it needs more than 1e-4)."""
+@pytest.mark.parametrize("recipe", list(RECIPES))
+def test_gnn_adapter_projection_k_neq_width_matches_float64(recipe, impl, det, monkeypatch):
+    """A GNN training step (typed input adapter tanh(Linear_t(x)) with K != width, then the HGTConv stack; dropout 0 in
+    train mode) against float64 autograd: out, d node_feature and every parameter gradient, at the reference's own
+    training recipes.  HGTConv itself needs in_dim == out_dim (the skip connection, conv.py:131), so the adapter is
+    the training path's only projection with K != width.  Under torch.use_deterministic_algorithms two steps are
+    bitwise equal."""
     import pyhgt_b200
-    from pyhgt_b200.model import GNN
     dev = _dev()
     monkeypatch.setattr(pyhgt_b200.HGTConv, "keep_att", False)
-    T, R, F_in, d, H = 3, 4, 128, 256, 8
-    g = _graph(T, R, 71, False)
-    torch.manual_seed(72)
-    m = GNN(F_in, d, T, R, H, 1, 0.0, "hgt", True, True, False)
-    _perturb(m, 73)
-    x = torch.randn(g.num_nodes, F_in, generator=torch.Generator().manual_seed(74))
-    w = torch.randn(g.num_nodes, d, generator=torch.Generator().manual_seed(75))
-    params = _f64_params(m)
-    xr = x.double().requires_grad_(True)
-    h = torch.zeros(g.num_nodes, d, dtype=torch.float64)
-    for t in range(T):                                               # model.py:70-75
-        sel = g.node_type == t
-        h[sel] = torch.tanh(xr[sel] @ params["adapt_ws.%d.weight" % t].t() + params["adapt_ws.%d.bias" % t])
-    conv = m.gcs[0].base_conv
-    pre = "gcs.0.base_conv."
-    out = _oracle_layer({k[len(pre):]: v for k, v in params.items() if k.startswith(pre)}, h, g, conv)
-    (out * w.double()).sum().backward()
-    ref = (out.detach(), xr.grad, {k: v.grad for k, v in params.items()})
-    m = m.to(dev).train()
+    g, m0, x, w, ref = _recipe(recipe)
+    m = copy.deepcopy(m0).to(dev).train()
     for c in m.gcs:
         c.base_conv.linear_impl = impl
-    xg = x.to(dev).requires_grad_(True)
-    o = m(xg, g.node_type.to(dev), g.edge_time.to(dev), g.edge_index.to(dev), g.edge_type.to(dev))
-    (o * w.to(dev)).sum().backward()
-    torch.cuda.synchronize()
-    native = (o.detach(), xg.grad, {k: p.grad for k, p in m.named_parameters()})
-    _compare_all("GNN adapter 128->256 impl %d" % impl, native, ref, (5e-5, 1.5e-4))
+    args = (g.node_type.to(dev), g.edge_time.to(dev), g.edge_index.to(dev), g.edge_type.to(dev))
+
+    def step():
+        m.zero_grad(set_to_none=True)
+        xg = x.to(dev).requires_grad_(True)
+        o = m(xg, *args)
+        (o * w.to(dev)).sum().backward()
+        torch.cuda.synchronize()
+        return o.detach(), xg.grad, {k: p.grad for k, p in m.named_parameters()}
+
+    with _deterministic(det):
+        native = step()
+        again = step() if det else None
+    _compare_all("GNN %s impl %d det %d" % (recipe, impl, det), native, ref, RECIPES[recipe][1])
+    if det:
+        assert torch.equal(native[0], again[0]) and torch.equal(native[1], again[1])
+        for k, v in native[2].items():
+            assert (v is None and again[2][k] is None) or torch.equal(v, again[2][k]), k
 
 
 def test_c4_three_layer_stack_matches_float64(monkeypatch):
