@@ -8,9 +8,10 @@
 //
 // k_typed_linear_tc runs tcp::split3_tile (tc_ptx.cuh): a persistent grid of one CTA per SM walking the 128 x BN output tiles,
 // a TMA producer warpgroup and two wgmma consumer warpgroups, both operands K-major.  At BN = 128 / 256 the k-blocks are 32
-// wide (SWIZZLE_64B): at BN = 256 that makes a 4-deep ring of 48 KB stages instead of 2 x 96 KB.  BN = 64 keeps 64-wide
-// k-blocks (SWIZZLE_128B, 4 stages): its k-blocks are short enough that halving them costs more in barrier waits than the
-// deeper ring gains (measured on the d = 400 OAG shape).  Output tiles follow the same group / column-block tables
+// wide (SWIZZLE_64B); their epilogue drains through asynchronous TMA tensor stores (tcp::store_tma), whose 64 KB of staging
+// leaves a ring of 3 x 48 KB stages at BN = 256 and 5 x 32 KB at BN = 128.  BN = 64 keeps 64-wide k-blocks (SWIZZLE_128B,
+// 4 stages) and the staged st.global epilogue: its k-blocks are short enough that halving them costs more in barrier
+// waits than the deeper ring gains (measured on the d = 400 OAG shape).  Output tiles follow the same group / column-block tables
 // as the SIMT kernel in linear.cu.  The output is fp32, or bf16 (hgt_typed_linear[_presplit]_bf16): the same tile, rounded
 // to nearest-even once as the epilogue stores it.
 #include <cuda.h>
@@ -27,6 +28,8 @@ using namespace tcp;
 
 constexpr int kMaxGroups = 64;
 template <int BN> constexpr int fwd_bk() { return BN == 64 ? 64 : 32; }    // k-block of the forward GEMM
+template <int BN> constexpr bool fwd_tma_store() { return BN != 64; }      // tensor-store epilogue (FwdJob::store)
+template <int BN> constexpr uint32_t fwd_out_stage() { return fwd_tma_store<BN>() ? TMA_STAGE_BYTES : OUT_STAGE_BYTES; }
 
 // ---- fp32 -> (bf16 hi, bf16 lo) split ------------------------------------------------------------
 __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_t rows, int K, int Kp,
@@ -59,9 +62,11 @@ __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_
 __device__ __forceinline__ void store4(float* p, float4 v, bool aligned) {
   if (aligned) {
     *reinterpret_cast<float4*>(p) = v;
-  } else {
+  } else if ((reinterpret_cast<uintptr_t>(p) & 7) == 0) {
     *reinterpret_cast<float2*>(p) = make_float2(v.x, v.y);
     *reinterpret_cast<float2*>(p + 2) = make_float2(v.z, v.w);
+  } else {
+    p[0] = v.x; p[1] = v.y; p[2] = v.z; p[3] = v.w;
   }
 }
 __device__ __forceinline__ void store4(__nv_bfloat16* p, float4 v, bool aligned) {
@@ -83,14 +88,17 @@ struct FwdJob {
   const hgt_lin_group* groups;
   const hgt_lin_cblock* cblocks;
   OutT* out;
+  const CUtensorMap* out_maps;             // BN = 128 / 256: output map of (group g, column block cb) at map_first[g] + cb
   int n_groups, cb_width, k_blocks, tile_n, n_tiles_n;
   int32_t first_tile[kMaxGroups + 1];
+  int32_t map_first[kMaxGroups];
 
   struct Tile {
-    int a_row, w_row, cols;
+    int a_row, w_row, cols, m0, n0;
     int64_t rows, ld;
     OutT* out;
     const float* bias;
+    const CUtensorMap* map;
   };
 
   __device__ int decode(int tile, Tile& t) const {
@@ -112,6 +120,9 @@ struct FwdJob {
     t.ld = cblk.ld;
     t.out = out + cblk.out_off + m0 * cblk.ld + n0;
     t.bias = (grp.has_bias && bias) ? bias + t.w_row : nullptr;
+    t.m0 = (int)m0;
+    t.n0 = n0;
+    t.map = out_maps + map_first[g] + cb;
     return k_blocks;
   }
   __device__ void prefetch(const Tile&) const {
@@ -127,8 +138,10 @@ struct FwdJob {
     tma_load_2d(sa + 2 * A, &w_hi, k, t.w_row, bar);
     tma_load_2d(sa + 2 * A + BN * KB * 2, &w_lo, k, t.w_row, bar);
   }
-  // Through shared memory, whole row segments per warp (tcp::store_staged).  cols is a multiple of 16, so a 4-column
-  // group is either inside the column block or past it.
+  // BN = 128 / 256: asynchronous TMA tensor stores (tcp::store_tma) where the destination rows are 16-byte aligned, so
+  // the stores overlap the next tile's products.  Otherwise, and at BN = 64, through shared memory with whole row segments
+  // per warp (tcp::store_staged).  cols is a multiple of 16, so a 4-column group is either inside the column block or
+  // past it.  Both paths add the bias in fp32 and round once, so they write the same bits.
   template <int BN>
   __device__ void store(const Tile& t, const float* acc, float* stage, int c, int wq, int lane) const {
     OutT* o = t.out + (int64_t)(64 * c) * t.ld;
@@ -136,22 +149,59 @@ struct FwdJob {
     const float* b = t.bias;
     const int cols = t.cols;
     const int64_t ld = t.ld;
-    const bool vec4 = ((reinterpret_cast<uintptr_t>(o) | (uintptr_t)(ld * sizeof(OutT))) & (4 * sizeof(OutT) - 1)) == 0;
-    store_staged<BN>(
-        acc, stage, c, wq, lane,
-        [&](int, int col, float v0, float v1) {
-          if (b && col < cols) v0 += __ldg(b + col), v1 += __ldg(b + col + 1);
-          return make_float2(v0, v1);
-        },
-        [&](int r, int col, float4 v) {
-          if (r < rows && col < cols) store4(o + r * ld + col, v, vec4);
-        });
+    auto pair = [&](int, int col, float v0, float v1) {
+      if (b && col < cols) v0 += __ldg(b + col), v1 += __ldg(b + col + 1);
+      return make_float2(v0, v1);
+    };
+    const uintptr_t align = reinterpret_cast<uintptr_t>(o) | (uintptr_t)(ld * sizeof(OutT));
+    if constexpr (fwd_tma_store<BN>()) {
+      if ((align & 15) == 0) {
+        store_tma<BN, OutT>(acc, reinterpret_cast<unsigned char*>(stage), c, wq, lane, pair, t.map, t.n0, t.m0 + 64 * c,
+                            cols);
+        return;
+      }
+      if (wq == 0 && lane == 0) bulk_wait_read<0>();          // store_staged reuses the tensor stores' buffers
+    }
+    const bool vec4 = (align & (4 * sizeof(OutT) - 1)) == 0;
+    store_staged<BN>(acc, stage, c, wq, lane, pair, [&](int r, int col, float4 v) {
+      if (r < rows && col < cols) store4(o + r * ld + col, v, vec4);
+    });
   }
 };
 
 template <int BN, class OutT>
 __global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob<OutT> job, int n_tiles) {
-  split3_tile<BN, false, fwd_bk<BN>()>(job, n_tiles);
+  split3_tile<BN, false, fwd_bk<BN>(), fwd_out_stage<BN>()>(job, n_tiles);
+}
+
+// ---- output tensor maps of the tensor-store epilogue ----------------------------------------------------------------
+// One map per (group, column block) of a launch: base out + out_off, rows = the group's m, columns = cb_width, row stride
+// ld.  The column-block table lives on the device, so the maps are built there: a copy of a host-encoded template (element
+// type, box, swizzle, columns) with the address, the row count and the row stride replaced.  Maps of blocks whose rows
+// are not 16-byte aligned are left unwritten; their tiles take the staged epilogue.
+struct MapFirst {
+  int32_t v[kMaxGroups];
+};
+
+template <class OutT>
+__global__ void k_out_maps(const __grid_constant__ CUtensorMap tmpl, const hgt_lin_group* __restrict__ groups,
+                           const hgt_lin_cblock* __restrict__ cblocks, OutT* out, const MapFirst first, CUtensorMap* maps) {
+  const hgt_lin_group grp = groups[blockIdx.x];
+  for (int cb = threadIdx.x; cb < grp.n_cblocks; cb += blockDim.x) {
+    const hgt_lin_cblock cblk = cblocks[grp.cb_first + cb];
+    OutT* base = out + cblk.out_off;
+    const uint64_t stride = (uint64_t)cblk.ld * sizeof(OutT);
+    if (grp.m <= 0 || ((reinterpret_cast<uintptr_t>(base) | stride) & 15) != 0) continue;
+    CUtensorMap* m = maps + first.v[blockIdx.x] + cb;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) reinterpret_cast<uint4*>(m)[i] = reinterpret_cast<const uint4*>(&tmpl)[i];
+    const uint64_t gm = (uint64_t)__cvta_generic_to_global(m);
+    asm volatile("tensormap.replace.tile.global_address.global.b1024.b64 [%0], %1;" ::"l"(gm), "l"(base) : "memory");
+    asm volatile("tensormap.replace.tile.global_dim.global.b1024.b32 [%0], 1, %1;" ::"l"(gm), "r"((uint32_t)grp.m)
+                 : "memory");
+    asm volatile("tensormap.replace.tile.global_stride.global.b1024.b64 [%0], 0, %1;" ::"l"(gm), "l"(stride) : "memory");
+  }
+  asm volatile("fence.proxy.tensormap::generic.release.gpu;" ::: "memory");
 }
 
 // ---- host side ------------------------------------------------------------------------------------
@@ -187,6 +237,30 @@ int make_map(CUtensorMap* m, const void* base, int64_t rows, int Kp, int box_row
   return 0;
 }
 
+// Template of the output maps: `cb_width` columns of OutT, boxes of 128 bytes x 64 rows with SWIZZLE_128B (the layout
+// tcp::store_tma stages).  `dummy` (16-byte aligned) and the row count / stride are placeholders that k_out_maps replaces.
+template <class OutT>
+int make_out_template(CUtensorMap* m, void* dummy, int cb_width) {
+  EncodeTiledFn fn = get_encode_fn();
+  HGT_REQUIRE(fn != nullptr, "hgt_typed_linear: cuTensorMapEncodeTiled not available from the driver");
+  cuuint64_t dims[2] = {(cuuint64_t)cb_width, 64};
+  cuuint64_t strides[1] = {(cuuint64_t)hgt_align_up((size_t)cb_width * sizeof(OutT), 16)};
+  cuuint32_t box[2] = {128 / (cuuint32_t)sizeof(OutT), 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(m, sizeof(OutT) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dummy, dims,
+                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  HGT_REQUIRE(r == CUDA_SUCCESS, "hgt_typed_linear: cuTensorMapEncodeTiled (output) failed (%d) cb_width=%d", (int)r,
+              cb_width);
+  return 0;
+}
+
+int64_t n_out_maps(const hgt_lin_group* h_groups, int n_groups) {
+  int64_t n = 0;
+  for (int g = 0; g < n_groups; ++g) n += h_groups[g].n_cblocks;
+  return n;
+}
+
 void extents(const hgt_lin_group* h_groups, int n_groups, int cb_width, int64_t* a_rows, int64_t* w_rows) {
   *a_rows = 0;
   *w_rows = 0;
@@ -209,7 +283,16 @@ int launch_fwd(FwdJob<OutT>& job, const __nv_bfloat16* const ops[4], int64_t a_r
   if ((rc = make_map(&job.w_hi, ops[2], w_rows, Kp, BN, KB))) return rc;
   if ((rc = make_map(&job.w_lo, ops[3], w_rows, Kp, BN, KB))) return rc;
   job.k_blocks = (Kp + KB - 1) / KB;
-  const size_t smem = tile_smem_bytes<BN, KB>();
+  if constexpr (fwd_tma_store<BN>()) {
+    CUtensorMap tmpl;
+    MapFirst first;
+    if ((rc = make_out_template<OutT>(&tmpl, const_cast<CUtensorMap*>(job.out_maps), job.cb_width))) return rc;
+    for (int g = 0; g < job.n_groups; ++g) first.v[g] = job.map_first[g];
+    k_out_maps<OutT><<<job.n_groups, 64, 0, st>>>(tmpl, job.groups, job.cblocks, job.out, first,
+                                                  const_cast<CUtensorMap*>(job.out_maps));
+    HGT_LAUNCH_CHECK();
+  }
+  const size_t smem = tile_smem_bytes<BN, KB, fwd_out_stage<BN>()>();
   HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_typed_linear_tc<BN, OutT><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
@@ -227,7 +310,8 @@ size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_gr
   int64_t a_rows, w_rows;
   extents(h_groups, n_groups, cb_width, &a_rows, &w_rows);
   const int Kp = (K + 7) / 8 * 8;
-  return 4 * 256 + 2 * hgt_align_up((size_t)a_rows * Kp * 2, 256) + 2 * hgt_align_up((size_t)w_rows * Kp * 2, 256);
+  return 5 * 256 + 2 * hgt_align_up((size_t)a_rows * Kp * 2, 256) + 2 * hgt_align_up((size_t)w_rows * Kp * 2, 256) +
+         hgt_align_up((size_t)n_out_maps(h_groups, n_groups) * sizeof(CUtensorMap), 256);
 }
 
 template <class OutT>
@@ -316,7 +400,8 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
   __nv_bfloat16* a_hi = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)a_rows * Kp * 2, 256);
   __nv_bfloat16* a_lo = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)a_rows * Kp * 2, 256);
   __nv_bfloat16* w_hi = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)w_rows * Kp * 2, 256);
-  __nv_bfloat16* w_lo = reinterpret_cast<__nv_bfloat16*>(p);
+  __nv_bfloat16* w_lo = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)w_rows * Kp * 2, 256);
+  CUtensorMap* out_maps = reinterpret_cast<CUtensorMap*>(p);
   {
     int64_t n = a_rows * (Kp / 4);
     if (a_hi_in) {
@@ -333,8 +418,10 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
   FwdJob<OutT> job;
   job.tile_n = pick_tile_n(cb_width);
   job.n_tiles_n = (cb_width + job.tile_n - 1) / job.tile_n;
-  int64_t total = 0;
+  int64_t total = 0, maps = 0;
   for (int g = 0; g < n_groups; ++g) {
+    job.map_first[g] = (int32_t)maps;
+    maps += h_groups[g].n_cblocks;
     job.first_tile[g] = (int32_t)total;
     total += (h_groups[g].m + BM - 1) / BM * h_groups[g].n_cblocks * job.n_tiles_n;
     HGT_REQUIRE(total < 2147483647ll, "hgt_typed_linear(tc): too many tiles");
@@ -345,6 +432,7 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
   job.groups = groups;
   job.cblocks = cblocks;
   job.out = out;
+  job.out_maps = out_maps;
   job.n_groups = n_groups;
   job.cb_width = cb_width;
   const __nv_bfloat16* const ops[4] = {a_hi, a_lo, w_hi, w_lo};

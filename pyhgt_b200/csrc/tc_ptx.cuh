@@ -13,9 +13,11 @@
 // Operand tiles are TMA boxes with SWIZZLE_128B, 64 bf16 (128 bytes) along the inner dimension (KB = 64), or with
 // SWIZZLE_64B, 32 bf16 (KB = 32: half the stage, twice the ring depth).  MN = false: both operands K-major (inner dimension =
 // reduction); MN = true: both MN-major (inner dimension = output row / column, the reduction runs over the box rows; KB = 64
-// only).  The Job supplies the tile decode, the loads of one stage and the epilogue.
+// only).  The Job supplies the tile decode, the loads of one stage and the epilogue (store_staged: st.global from a shared
+// staging block; store_tma: TMA tensor stores that drain while the consumer runs the next tile).
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 
 #include "common.cuh"
@@ -123,20 +125,29 @@ constexpr int BK = 64;                            // 64 bf16 = 128 bytes = one S
 constexpr int TILE_THREADS = 384;
 constexpr uint32_t A_BYTES = BM * BK * 2;         // one A operand (hi or lo) of a stage: 16 KB
 constexpr uint32_t ATOM_BYTES = 64 * BK * 2;      // one {64 x 64} bf16 box: 8 KB
-constexpr uint32_t SMEM_BUDGET = 192 * 1024;      // pipeline stages; H100 allows 227 KB of shared memory per block
+constexpr uint32_t SMEM_LIMIT = 227 * 1024;       // shared memory a block may use on H100
+constexpr uint32_t SMEM_BUDGET = 192 * 1024;      // most the pipeline stages take
 constexpr uint32_t OUT_STAGE_BYTES = 2 * 64 * 64 * 4;  // epilogue staging after the ring: one 64 x 64 fp32 block per consumer
+// Staging of the tensor-store epilogue (store_tma): per consumer two 64 x 64 buffers (at most fp32), so one buffer fills
+// while the other drains.
+constexpr uint32_t TMA_BUF_BYTES = 64 * 64 * 4;
+constexpr uint32_t TMA_STAGE_BYTES = 2 * 2 * TMA_BUF_BYTES;
 
-// Stage layout for a k-block of KB bf16: {A_hi, A_lo, B_hi, B_lo}; a consumer's 64-row A slab is one atom.
+// Stage layout for a k-block of KB bf16: {A_hi, A_lo, B_hi, B_lo}; a consumer's 64-row A slab is one atom.  The ring
+// takes what the epilogue staging (OUT bytes) and the barriers leave, up to SMEM_BUDGET.
 template <int KB> constexpr uint32_t a_bytes() { return BM * KB * 2; }
 template <int KB> constexpr uint32_t atom_bytes() { return 64 * KB * 2; }
 template <int BN, int KB = BK> constexpr uint32_t stage_bytes() { return 2 * a_bytes<KB>() + 2 * (uint32_t)BN * KB * 2; }
-template <int BN, int KB = BK> constexpr int n_stages() { return (int)(SMEM_BUDGET / stage_bytes<BN, KB>()); }
-template <int BN, int KB = BK> constexpr size_t tile_smem_bytes() {
-  return 1024 + (size_t)n_stages<BN, KB>() * stage_bytes<BN, KB>() + OUT_STAGE_BYTES +
-         2 * n_stages<BN, KB>() * sizeof(uint64_t);
+template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES> constexpr int n_stages() {
+  constexpr uint32_t left = SMEM_LIMIT - 1024 - OUT - 256;
+  return (int)((left < SMEM_BUDGET ? left : SMEM_BUDGET) / stage_bytes<BN, KB>());
 }
-static_assert(tile_smem_bytes<256, 32>() <= 227 * 1024 && tile_smem_bytes<256>() <= 227 * 1024 &&
-                  tile_smem_bytes<128, 32>() <= 227 * 1024 && tile_smem_bytes<64>() <= 227 * 1024,
+template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES> constexpr size_t tile_smem_bytes() {
+  return 1024 + (size_t)n_stages<BN, KB, OUT>() * stage_bytes<BN, KB>() + OUT +
+         2 * n_stages<BN, KB, OUT>() * sizeof(uint64_t);
+}
+static_assert(tile_smem_bytes<256, 32, TMA_STAGE_BYTES>() <= SMEM_LIMIT && tile_smem_bytes<256>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<128, 32, TMA_STAGE_BYTES>() <= SMEM_LIMIT && tile_smem_bytes<64>() <= SMEM_LIMIT,
               "ring + epilogue staging must fit the 227 KB a block may use");
 
 // Output tile width: 64, 128 or 256 columns, the one that pads `width` least (ties go to the wider tile).  Columns past
@@ -236,19 +247,84 @@ __device__ __forceinline__ void store_staged(const float* acc, float* stage, int
   }
 }
 
-// Called by a __global__ kernel with __launch_bounds__(TILE_THREADS, 1) and tile_smem_bytes<BN, KB>() of dynamic shared
+// TMA tensor stores shared -> global (the async proxy).  Each thread tracks its own bulk groups.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+// A tensor map written to global memory by an earlier kernel (generic proxy): acquire it for the TMA proxy.
+__device__ __forceinline__ void tensormap_acquire(const CUtensorMap* m) {
+  asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(m) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+__device__ __forceinline__ void put2(float* p, float2 v) { *reinterpret_cast<float2*>(p) = v; }
+__device__ __forceinline__ void put2(__nv_bfloat16* p, float2 v) {
+  *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(v.x, v.y);
+}
+
+// Asynchronous epilogue of one consumer warpgroup (c): its 64 x BN accumulator goes out in 64-column blocks.  Each block
+// is written to shared memory as OutT in the SWIZZLE_128B layout of `map`'s boxes (128-byte rows, 64 rows; 16-byte chunk q
+// of row r at q ^ (r & 7); fp32: two boxes of 32 columns, bf16: one box of 64) and sent to global memory by TMA tensor
+// stores that one thread (the warpgroup's first) issues.  The map's extents clip the rows past the group and the columns
+// past the column block.  The stores drain while the consumer goes on to the next block or the next tile's products.
+// Block b uses buffer b & 1 of `stage` (two TMA_BUF_BYTES buffers, 1024-byte aligned); BN / 64 is even, so the buffers
+// alternate across tiles too.  Before a buffer is rewritten the issuing thread waits until the bulk group that read it two
+// blocks earlier is done (it commits one group per block).
+// pair(row, col, v0, v1) -> float2 as in store_staged; the block's row 0, column 0 is element (col0 + 64 b, row0) of
+// the map; `cols`: columns of the tile inside the column block.
+template <int BN, class OutT, class Pair>
+__device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage, int c, int wq, int lane, Pair pair,
+                                          const CUtensorMap* map, int col0, int row0, int cols) {
+  static_assert(BN % 128 == 0, "the two buffers alternate across tiles only for an even number of 64-column blocks");
+  constexpr int BOX_COLS = 128 / (int)sizeof(OutT);
+  const bool issuer = wq == 0 && lane == 0;
+  const int r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
+  if (issuer) tensormap_acquire(map);
+#pragma unroll
+  for (int blk = 0; blk < BN / 64; ++blk) {
+    unsigned char* buf = stage + (blk & 1) * TMA_BUF_BYTES;
+    if (issuer) bulk_wait_read<1>();
+    bar_sync_named(1 + c, 128);                                 // the buffer has been read out
+#pragma unroll
+    for (int j = 8 * blk; j < 8 * blk + 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h, lc = 8 * j + c0 - 64 * blk;
+        const uint32_t x = (uint32_t)(lc % BOX_COLS) * sizeof(OutT);       // byte in the box row
+        put2(reinterpret_cast<OutT*>(buf + (lc / BOX_COLS) * 8192 + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))),
+             pair(r, 8 * j + c0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+      }
+    }
+    fence_proxy_async_smem();                                   // the writes are visible to the tensor stores
+    bar_sync_named(1 + c, 128);
+    if (issuer) {
+#pragma unroll
+      for (int bx = 0; bx < 64 / BOX_COLS; ++bx)
+        if (64 * blk + BOX_COLS * bx < cols) tma_store_2d(map, s_u32(buf + bx * 8192), col0 + 64 * blk + BOX_COLS * bx, row0);
+      bulk_commit();
+    }
+  }
+}
+
+// Called by a __global__ kernel with __launch_bounds__(TILE_THREADS, 1) and tile_smem_bytes<BN, KB, OUT>() of dynamic shared
 // memory; `job` is the kernel's __grid_constant__ parameter (it holds the tensor maps), `n_tiles` the number of tiles
 // job.decode() accepts.  Every tile's k-blocks run in ascending order into a freshly zeroed accumulator, so a tile's
-// result does not depend on the grid size or on which CTA computes it.
-template <int BN, bool MN, int KB, class Job>
+// result does not depend on the grid size or on which CTA computes it.  job.store gets consumer c's half of the OUT bytes
+// of epilogue staging.
+template <int BN, bool MN, int KB, uint32_t OUT = OUT_STAGE_BYTES, class Job>
 __device__ __forceinline__ void split3_tile(const Job& job, int n_tiles) {
-  constexpr int S = n_stages<BN, KB>();
+  constexpr int S = n_stages<BN, KB, OUT>();
   constexpr uint32_t STAGE = stage_bytes<BN, KB>();
   constexpr uint32_t A = a_bytes<KB>(), ATOM = atom_bytes<KB>();
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);
-  float* out_stage = reinterpret_cast<float*>(smem + (size_t)S * STAGE);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)S * STAGE + OUT_STAGE_BYTES);
+  unsigned char* out_stage = smem + (size_t)S * STAGE;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)S * STAGE + OUT);
   uint64_t* empty_bar = full_bar + S;
   const uint32_t base = s_u32(smem);
   const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -309,9 +385,10 @@ __device__ __forceinline__ void split3_tile(const Job& job, int n_tiles) {
       if (iters > 0) {
         __syncwarp();
         if (lane == 0) mbar_arrive(s_u32(&empty_bar[prev]));     // the producer may refill it during the store
-        job.template store<BN>(t, acc, out_stage + c * 64 * 64, c, warp & 3, lane);
+        job.template store<BN>(t, acc, reinterpret_cast<float*>(out_stage + c * (OUT / 2)), c, warp & 3, lane);
       }
     }
+    bulk_wait_all();                                              // bulk stores of the epilogue, if it issued any
   }
 }
 
