@@ -241,7 +241,10 @@ int hgt_concat_linears(const float* const* w, const float* const* b, int32_t num
 /* out[cblock c of group g][m, n] = sum_k A[a_row0_g + m, k] * W[w_row0_g + c*cb_width + n, k] (+ bias).
  * fp32 in / fp32 out.  `impl`: 0 = auto, 1 = SIMT fp32 FMA kernel, 2 = wgmma split-bf16 tensor-core
  * kernel (three bf16 products of a hi/lo operand split accumulated in one fp32 register accumulator: accurate
- * to ~1e-5 relative; needs cb_width % 16 == 0 and K >= 64, workspace for the split operands).
+ * to ~1e-5 relative; needs cb_width % 16 == 0 and K >= 64, workspace for the split operands), 3 = auto with ONE bf16
+ * product on the tensor cores (both operands rounded to bf16 to nearest-even, products accumulated in fp32: torch's
+ * "medium" float32 matmul precision; only the hi halves are made, so the workspace is at most impl 2's) and the fp32
+ * SIMT kernel where auto would pick it.  Any other impl is rejected, by the workspace query too.
  * groups/cblocks are DEVICE arrays; h_groups is the same table on the host (used to size the grid; no
  * device read-back). */
 int hgt_typed_linear_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K,
@@ -251,7 +254,8 @@ int hgt_typed_linear(const float* A, int64_t lda, const float* W, const float* b
                      int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int32_t impl,
                      void* workspace, size_t workspace_bytes, void* stream);
 /* Same product on the tensor-core kernel with the A operand already split by its producer: a_hi / a_lo are bf16
- * [rows, K] (K % 8 == 0, row stride K).  Saves the split pass over A (workspace: W split only). */
+ * [rows, K] (K % 8 == 0, row stride K).  Saves the split pass over A (workspace: W split only).  a_lo == NULL selects
+ * one bf16 product (a_hi * bf16(W), as impl 3); the workspace query's answer covers both. */
 int hgt_typed_linear_presplit_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K,
                                               int32_t cb_width, size_t* out_bytes);
 int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W, const float* bias, int32_t K,
@@ -284,7 +288,8 @@ int hgt_typed_linear_presplit_bf16(const void* a_hi, const void* a_lo, const flo
  *  att_out [E, H]  softmax weights in ORIGINAL edge order (conv.py:108 `self.att`) or NULL
  *  stats_out [N, 2H] per-destination (max, sum) per head, or NULL (kept for the backward pass)
  *  g_hi / g_lo [N, d] bf16 or NULL: the same result as a bf16 hi/lo split (x = hi + lo to ~2^-17), i.e. the
- *           pre-split A operand of hgt_typed_linear_presplit; agg_out may then be NULL.  Needs d % 8 == 0.
+ *           pre-split A operand of hgt_typed_linear_presplit; agg_out may then be NULL.  Needs d % 8 == 0.  g_hi without
+ *           g_lo writes the hi half only (the operand of a one-product GEMM, a_lo == NULL).
  *  variant: 0 = auto, 1 = direct register gather (LDG), 2 = bulk-async-copy shared-memory ring (TMA)
  *  d_tile_counts: NULL, or the device counts {n_tiles, n_split, n_hubs} hgt_plan_tiles wrote in its sync-free mode; then
  *           n_tiles / n_split_tiles / n_hubs are the UPPER BOUNDS the arrays were sized with and the kernels read the
@@ -381,7 +386,10 @@ int hgt_edge_backward_rows_bf16(const float* q, const float* dagg, const float* 
  * elements).  dW / db are ACCUMULATED INTO (several groups may share W rows: the caller zero-initialises them once per
  * step); dA is written (rows BETWEEN / BEFORE the groups that no group covers are zeroed; rows past the last group are the
  * caller's) unless accumulate_dA != 0, in which case the product is added to its current content.  dA / dW / db may each be NULL to skip that product.
- * Tensor-core path (impl 0 = auto, 2 = force): wgmma split-bf16 x3 like the forward; takes the operands either as
+ * Tensor-core path (impl 0 = auto, 2 = force): wgmma split-bf16 x3 like the forward; impl 3 = auto with one bf16 product
+ * (dout, A and W rounded to bf16; only their hi halves are made, so dout_lo / a_lo may be NULL with a pre-split
+ * dout_hi / a_hi, and the workspace is at most impl 2's; db is still summed from the fp32 dout; where auto picks SIMT the
+ * result stays fp32 SIMT, except that a pre-split A selects the tensor cores as impl 2 does); any other impl is rejected; takes the operands either as
  * fp32 (split here; the dout split pass also yields db) or already split by their producers (dout_hi/lo in dout's
  * layout; a_hi/a_lo [rows, K] as left by hgt_act_split in the forward) — with a pre-split dout, db is NOT computed.
  * impl 1 = fp32 SIMT kernels (any shape; also chosen automatically for cb_width % 8, K % 16, K < 64, overlapping groups
@@ -414,7 +422,7 @@ int hgt_typed_linear_bwd_det(const float* dout, const void* dout_hi, const void*
                              int32_t impl, void* workspace, size_t workspace_bytes, void* stream);
 
 /* act(in) as fp32 (out_f32 [rows, K], or NULL) and/or as the bf16 hi/lo operand split (hi/lo [rows, K], or NULL; needs
- * K % 8 == 0).  act: 0 = identity, 1 = exact-erf gelu (conv.py:119).  The training forward keeps the split for the
+ * K % 8 == 0; hi without lo writes only the hi half, bitwise the same, the operand of a one-product GEMM).  act: 0 = identity, 1 = exact-erf gelu (conv.py:119).  The training forward keeps the split for the
  * backward pass (it is the A operand of the dW product). */
 int hgt_act_split(const float* in, int64_t ld, int64_t rows, int32_t K, int32_t act, float* out_f32,
                   void* hi, void* lo, void* stream);
@@ -465,7 +473,8 @@ int hgt_fold_backward_det(const float* d_w_cat, const float* d_b_cat, const floa
  *   (sharded runs: the remaining rows are halo sources that need no output);
  *   out [N,d] in ORIGINAL node order;
  *   out_hi / out_lo [N,d] bf16 or NULL: `out` again as the bf16 hi/lo split that the NEXT layer's projection GEMM
- *   consumes (hgt_typed_linear_presplit) — only with perm == NULL, type_active == NULL, d % 8 == 0.
+ *   consumes (hgt_typed_linear_presplit) — only with perm == NULL, type_active == NULL, d % 8 == 0; out_hi without
+ *   out_lo writes the hi half only (for a one-product GEMM).
  * ---------------------------------------------------------------------------------------------- */
 int hgt_update_epilogue(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
                         const float* skip, const float* norm_w, const float* norm_b,
@@ -485,7 +494,9 @@ typedef struct {
   /* sizes and switches */
   int64_t n_nodes, n_edges, kv_rows, cat_rows, q_off, kv_off, proj_elems;
   int32_t num_types, num_relations, n_heads, d_in, d_out, n_pairs;
-  int32_t use_rte, use_norm, edge_variant, linear_impl;
+  int32_t use_rte, use_norm, edge_variant;
+  int32_t linear_impl;        /* hgt_typed_linear's impl for the projection and a_linear GEMMs; 3: one bf16 product, then
+                                 the edge kernel's operand split is hi only and x_lo is not read */
   int32_t n_tiles, n_split, n_hubs;
   int32_t n_proj_groups, n_rte_groups, n_upd_groups;
   /* plan (hgt_plan_*) */

@@ -27,6 +27,12 @@ KVR, are stored in bf16: the projection writes Q by its own fp32 call and the K'
 (hgt_typed_linear[_presplit]_bf16, rounded once from the fp32 accumulator), and the edge kernels read them through their
 _bf16 entry points.  The layer output, att, the softmax statistics, Q and every gradient stay fp32; the stages record the
 switch on ctx, so the backward follows the forward.  fp16 autocast keeps fp32 tables.
+
+Under ``torch.set_float32_matmul_precision("medium")`` (bf16_matmuls()) the typed GEMMs that would run on the tensor cores
+(linear_impl 0 or 2) run with one bf16 product instead of the split-bf16 x3 (C impl 3): the operands are rounded to bf16
+and only that hi half is produced, saved for dW and read.  This is torch's documented meaning of "medium" ("bfloat16
+datatype for internal computations"); note that torch's own CUDA matmuls run TF32 at "medium", so these GEMMs are less
+precise than torch's there.  "high" and "highest" keep the x3 scheme.  The stages record the setting on ctx.
 """
 import ctypes
 
@@ -46,6 +52,18 @@ def bf16_tables():
     return torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
 
 
+def bf16_matmuls():
+    """The switch for one bf16 product in the tensor-core GEMMs, read once per layer forward:
+    torch.get_float32_matmul_precision() == "medium"."""
+    return torch.get_float32_matmul_precision() == "medium"
+
+
+def gemm_impl(linear_impl, one_product):
+    """The C `impl` of a layer's typed GEMMs: 3 (auto, one bf16 product on the tensor cores) where the layer would take
+    the tensor cores (linear_impl 0 or 2) and one_product is set; linear_impl otherwise (1 keeps fp32 SIMT)."""
+    return 3 if one_product and linear_impl in (0, 2) else linear_impl
+
+
 def _tc_shape_ok(K, width):
     """Shapes both the tensor-core forward (hgt_typed_linear_presplit) and backward (hgt_typed_linear_bwd) take."""
     return K % 16 == 0 and K >= 64 and width % 16 == 0
@@ -58,7 +76,7 @@ class _TypedLinear(torch.autograd.Function):
     into an fp32 Q buffer [q_elems] (q_table) and a bf16 table [out_elems - kv_off] (kv_table, offsets relative to kv_off,
     zero ranges relative to it too).  The forward then returns (stand-in, q, table): the stand-in is a zero-stride fp32
     tensor of out_elems that only carries the gradient, which arrives in the flat layout of the fp32 output, so the
-    backward is the same."""
+    backward is the same.  impl 3: one bf16 product on the tensor cores, only the hi half of act(A) is made and saved."""
 
     @staticmethod
     def forward(ctx, a, w_cat, b_cat, table, width, out_elems, impl, act, zero_ranges, tables16=None):
@@ -79,12 +97,13 @@ class _TypedLinear(torch.autograd.Function):
             for (z0, z1) in kv_zero:
                 if z1 > z0:
                     kv[z0:z1].zero_()
-        use_tc = impl in (0, 2) and _tc_shape_ok(K, width)
+        use_tc = impl in (0, 2, 3) and _tc_shape_ok(K, width)
+        one = use_tc and impl == 3
         hi = lo = a_act = None
         if use_tc:
             hi = torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
-            lo = torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
-            _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, None, hi.data_ptr(), lo.data_ptr(), st)
+            lo = None if one else torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
+            _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, None, hi.data_ptr(), _lib.ptr(lo), st)
         else:
             a_act = a
             if act:
@@ -98,7 +117,7 @@ class _TypedLinear(torch.autograd.Function):
             if use_tc:
                 _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, K, width, ctypes.byref(wsb))
                 ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                _lib.call("hgt_typed_linear_presplit" + sfx, hi.data_ptr(), lo.data_ptr(), w_cat.data_ptr(),
+                _lib.call("hgt_typed_linear_presplit" + sfx, hi.data_ptr(), _lib.ptr(lo), w_cat.data_ptr(),
                           _lib.ptr(b_cat), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(),
                           dst.data_ptr(), ws.data_ptr(), ws.numel(), st)
             else:
@@ -115,6 +134,7 @@ class _TypedLinear(torch.autograd.Function):
                 gemm(q_table, q)
             gemm(kv_table, kv)
         ctx.table, ctx.width, ctx.has_bias, ctx.act, ctx.use_tc = table, width, b_cat is not None, act, use_tc
+        ctx.one = one
         ctx.out_elems = out_elems
         ctx.det = torch.are_deterministic_algorithms_enabled()
         # gelu'(a) needs the un-activated input; the dW product needs act(a): as the bf16 split (tensor cores) or fp32
@@ -136,7 +156,7 @@ class _TypedLinear(torch.autograd.Function):
         da = torch.empty((rows, K), dtype=torch.float32, device=dev) if need_da else None
         dw = torch.zeros_like(w_cat)                                   # small: [sum of out rows, K]
         db = torch.zeros(w_cat.shape[0], dtype=torch.float32, device=dev) if ctx.has_bias else None
-        impl = 2 if ctx.use_tc else 1
+        impl = (3 if ctx.one else 2) if ctx.use_tc else 1
         fn = "hgt_typed_linear_bwd_det" if ctx.det else "hgt_typed_linear_bwd"
         a_f32 = a_act if a_act is not None else a                      # SIMT dW operand (act already applied)
         # tables whose groups overlap in rows (sharded per-pair compaction) come with disjoint sub-tables: the first call
@@ -351,18 +371,19 @@ def typed_linear(a, w_cat, b_cat, table, width, out_elems, impl=0, act=0, zero_r
     return _TypedLinear.apply(a, w_cat, b_cat, table, width, out_elems, impl, act, tuple(zero_ranges), tables16)
 
 
-def _project(m, x, w_cat, b_cat, plan, lt, bf16):
+def _project(m, x, w_cat, b_cat, plan, lt, bf16, impl):
     """Typed projections of a layer: the flat [Q | pad | K'V' table | zero row] buffer and, with RTE, the RTE table
     [P*240+1, 2d] (+ all-zero row).  bf16: those two are gradient stand-ins and the third result holds what the edge kernel
-    reads, (Q, bf16 [K'|V'] table, bf16 RTE table or None); otherwise it is None."""
+    reads, (Q, bf16 [K'|V'] table, bf16 RTE table or None); otherwise it is None.  impl: the projection GEMM's (gemm_impl;
+    the RTE tables stay fp32 SIMT)."""
     N, P, d, d_in = plan.n_nodes, plan.n_pairs, m.out_dim, m.in_dim
     kv_end = lt.kv_off + plan.kv_rows * 2 * d
     if bf16:
-        proj, q, kv = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, m.linear_impl, 0, (),
+        proj, q, kv = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, impl, 0, (),
                                    (lt.q_groups, N * d, lt.kv_groups, lt.kv_off,
                                     ((kv_end - lt.kv_off, lt.proj_elems - lt.kv_off),)))
     else:
-        proj = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, m.linear_impl, 0,
+        proj = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, impl, 0,
                             ((N * d, lt.kv_off), (kv_end, lt.proj_elems)))
     kvr = kvr16 = None
     if m.use_RTE:
@@ -405,7 +426,8 @@ def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, 
               [l.weight for l in m.v_linears] + [l.bias for l in m.v_linears] +
               [m.relation_att, m.relation_msg, m.relation_pri])
     w_cat, b_cat = _FoldWeights.apply(m, plan, lt, *params)
-    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables())
+    impl = gemm_impl(m.linear_impl, bf16_matmuls())
+    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables(), impl)
 
     # 2. fused edge kernel
     agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, want_att, m.edge_variant, tables16)
@@ -414,7 +436,7 @@ def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, 
     # 3. a_linears on gelu(agg) (conv.py:119,125): the gelu is applied inside the operand split / the dX epilogue
     wa_cat = torch.cat([l.weight for l in m.a_linears], 0)
     ba_cat = torch.cat([l.bias for l in m.a_linears], 0)
-    o = typed_linear(agg, wa_cat, ba_cat, lt.upd_groups, d, N * d, m.linear_impl, 1).view(N, d)
+    o = typed_linear(agg, wa_cat, ba_cat, lt.upd_groups, d, N * d, impl, 1).view(N, d)
     if m.training and m.drop.p > 0:
         o = m.drop(o)                                                            # conv.py:125
 
@@ -445,14 +467,15 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
               [l.weight for l in m.v_linears] + [l.bias for l in m.v_linears] +
               [m.relation_att, m.relation_msg, m.relation_pri])
     w_cat, b_cat = _FoldWeights.apply(m, plan, lt, *params)
-    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables())
+    impl = gemm_impl(m.linear_impl, bf16_matmuls())
+    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables(), impl)
     agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant, tables16)
     m.att = att
 
     drop = m.training and m.drop.p > 0
     wa_cat = torch.cat([l.weight for l in m.a_linears], 0)
     ba_cat = torch.cat([l.bias for l in m.a_linears], 0)
-    o = typed_linear(agg, wa_cat, ba_cat, lt.upd_groups, d, N * d, m.linear_impl, 0).view(N, d)     # conv.py:261
+    o = typed_linear(agg, wa_cat, ba_cat, lt.upd_groups, d, N * d, impl, 0).view(N, d)              # conv.py:261
     if drop:
         o = m.drop(o)
     norm_w = torch.stack([n.weight for n in m.norms]) if m.use_norm else None
@@ -466,9 +489,9 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
         one = lambda w_: _plan._pack_groups([(0, n_known, 0, 1, 0, 1)], [(0, w_)], dev)            # noqa: E731
         tabs = plan._layer_tables[key] = (one(2 * d), one(d),
                                           _plan._to_dev_async(np.asarray([0, n_known, N], dtype=np.int32), dev))
-    hmid = typed_linear(y, m.mid_linear.weight, m.mid_linear.bias, tabs[0], 2 * d, N * 2 * d, m.linear_impl, 0,
+    hmid = typed_linear(y, m.mid_linear.weight, m.mid_linear.bias, tabs[0], 2 * d, N * 2 * d, impl, 0,
                         ((n_known * 2 * d, N * 2 * d),)).view(N, 2 * d)
-    z = typed_linear(hmid, m.out_linear.weight, m.out_linear.bias, tabs[1], d, N * d, m.linear_impl, 1,
+    z = typed_linear(hmid, m.out_linear.weight, m.out_linear.bias, tabs[1], d, N * d, impl, 1,
                      ((n_known * d, N * d),)).view(N, d)                                             # gelu inside
     if drop:
         z = m.drop(z)

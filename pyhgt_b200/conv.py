@@ -68,6 +68,16 @@ def _output_rows(rows, d, dev, lt, out_map):
     return torch.empty((rows, d), dtype=torch.float32, device=dev)
 
 
+def _split_hint(node_inp, x, N, d_in, impl):
+    """The bf16 operand split a previous layer's update epilogue left on node_inp (`_hgt_split` = (hi, lo or None,
+    version)), or None.  A hint without its lo half only serves a one-product GEMM (impl 3); impl 3 reads hi alone."""
+    hint = getattr(node_inp, "_hgt_split", None)
+    if (hint is None or hint[2] != node_inp._version or x is not node_inp or tuple(hint[0].shape) != (N, d_in)
+            or d_in % 16 or d_in < 64 or (hint[1] is None and impl != 3)):
+        return None
+    return (hint[0], None if impl == 3 else hint[1])
+
+
 class _PointerTable:
     """Device array of per-type parameter pointers, rebuilt only when a parameter moves."""
 
@@ -93,7 +103,8 @@ class HGTConv(nn.Module):
     # conv.py:308 stays valid).
     keep_att = True            # materialise self.att [E,H] like the reference (conv.py:108)
     edge_variant = 0           # 0 auto, 1 register gather, 2 bulk-copy ring (see csrc/edge.cu)
-    linear_impl = 0            # 0 auto, 1 fp32 SIMT, 2 tensor cores (wgmma)
+    linear_impl = 0            # 0 auto, 1 fp32 SIMT, 2 tensor cores (wgmma); 0 / 2 take one bf16 product under
+                               # torch.set_float32_matmul_precision("medium") (autograd.bf16_matmuls)
     event_sink = None          # bench.py: list receiving (stage, start_event, end_event) on the launch stream
     _has_skip = True           # DenseHGTConv (conv.py:143-280) has no skip gate
     emit_split = False         # also write the output as a bf16 hi/lo split for the next layer (model.GNN sets it)
@@ -225,9 +236,12 @@ class HGTConv(nn.Module):
 
     # ------------------------------------------------------------------------------------------
     def _forward_fused(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att,
-                       active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None, plan=None):
+                       active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None, plan=None, impl=None):
         """Inference through the single entry point hgt_conv_forward (csrc/layer.cu).  The argument block is cached per
-        (plan tables, parameter locations); per call only the data pointers change."""
+        (plan tables, parameter locations); per call only the data pointers change.  impl: the GEMMs' C impl
+        (autograd.gemm_impl), linear_impl by default."""
+        if impl is None:
+            impl = self.linear_impl
         dev = node_inp.device
         d_in, d, H, T, R = self.in_dim, self.out_dim, self.n_heads, self.num_types, self.num_relations
         if plan is None:
@@ -288,14 +302,11 @@ class HGTConv(nn.Module):
             ent = cache[key] = (a, lt, plan, tabs)                 # keep the tables the pointers refer to alive
         a = ent[0]
         x = node_inp.contiguous()
-        if x_split is None and plan.sorted_types and self.linear_impl in (0, 2):
-            hint = getattr(node_inp, "_hgt_split", None)
-            if (hint is not None and hint[2] == node_inp._version and x is node_inp
-                    and tuple(hint[0].shape) == (N, d_in) and d_in % 16 == 0 and d_in >= 64):
-                x_split = (hint[0], hint[1])
-        a.edge_variant, a.linear_impl = self.edge_variant, self.linear_impl
+        if x_split is None and plan.sorted_types and impl != 1:
+            x_split = _split_hint(node_inp, x, N, d_in, impl)
+        a.edge_variant, a.linear_impl = self.edge_variant, impl
         a.x = x.data_ptr()
-        a.x_hi, a.x_lo = (x_split[0].data_ptr(), x_split[1].data_ptr()) if x_split is not None else (None, None)
+        a.x_hi, a.x_lo = (x_split[0].data_ptr(), _lib.ptr(x_split[1])) if x_split is not None else (None, None)
         if out_map is not None and not plan.sorted_types:
             raise ValueError("out_map needs a type-sorted node order")
         a.out_map = _lib.ptr(out_map)
@@ -306,7 +317,7 @@ class HGTConv(nn.Module):
         if (self.emit_split and plan.sorted_types and out_map is None and lt.type_active_dev is None and d % 16 == 0
                 and d >= 64):
             o_hi = torch.empty((N, d), dtype=torch.bfloat16, device=dev)
-            o_lo = torch.empty((N, d), dtype=torch.bfloat16, device=dev)
+            o_lo = None if impl == 3 else torch.empty((N, d), dtype=torch.bfloat16, device=dev)
         a.out_hi, a.out_lo = _lib.ptr(o_hi), _lib.ptr(o_lo)
         wsb = ctypes.c_size_t()
         _lib.call("hgt_conv_workspace_bytes", ctypes.byref(a), ctypes.byref(wsb))
@@ -323,14 +334,15 @@ class HGTConv(nn.Module):
         Without out_map, rows past the active prefix are zero.  plan: an explicit plan (a trimmed layer's view, trim.py)
         instead of the cached plan of the tensors.  Under bf16 autocast the layer runs the per-stage path with bf16
         gather tables."""
-        from .autograd import bf16_tables
+        from .autograd import bf16_matmuls, bf16_tables, gemm_impl
         bf16 = bf16_tables()
+        impl = gemm_impl(self.linear_impl, bf16_matmuls())
         if (self.fused_call and not save and HGTConv.event_sink is None and type(self)._has_skip
                 and not (self.training and self.drop.p > 0) and not bf16):
             return self._forward_fused(node_inp, node_type, edge_index, edge_type, edge_time, want_att,
-                                       active_per_type, out_map, out_rows, x_split, kv_runs, plan)
+                                       active_per_type, out_map, out_rows, x_split, kv_runs, plan, impl)
         c = self._core(node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs, bf16=bf16, plan=plan)
+                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs, bf16=bf16, plan=plan, impl=impl)
         plan, lt, o, x_sorted, N, d, T, st = c["plan"], c["lt"], c["o"], c["x_sorted"], c["N"], c["d"], c["T"], c["st"]
         norm_w = norm_b = None
         if self.use_norm:
@@ -347,7 +359,7 @@ class HGTConv(nn.Module):
         if (self.emit_split and perm_ptr is None and lt.type_active_dev is None and d % 16 == 0 and d >= 64
                 and not self.training):
             o_hi = torch.empty((N, d), dtype=torch.bfloat16, device=o.device)
-            o_lo = torch.empty((N, d), dtype=torch.bfloat16, device=o.device)
+            o_lo = None if impl == 3 else torch.empty((N, d), dtype=torch.bfloat16, device=o.device)
         with self._stage("update_epilogue"):
             _lib.call("hgt_update_epilogue", o.data_ptr(), x_sorted.data_ptr(), plan.type_row0_dev.data_ptr(), T,
                       self.skip.data_ptr(), _lib.ptr(norm_w), _lib.ptr(norm_b), perm_ptr,
@@ -357,10 +369,14 @@ class HGTConv(nn.Module):
         return out, c["att"], (c if save else None)
 
     def _core(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-              gelu_before_a, x_split=None, kv_runs=None, bf16=False, plan=None):
+              gelu_before_a, x_split=None, kv_runs=None, bf16=False, plan=None, impl=None):
         """Everything up to and including the typed a_linear: plan, weight fold, typed projections, fused edge kernel
         (gelu fused iff gelu_before_a and not save), a_linears.  Returns a dict of the intermediates.  bf16: bf16 [K'|V'] and
-        RTE tables (Q and everything else fp32)."""
+        RTE tables (Q and everything else fp32).  impl: the GEMMs' C impl (autograd.gemm_impl; 3 = one bf16 product, no lo
+        halves are made or read), linear_impl by default."""
+        if impl is None:
+            impl = self.linear_impl
+        one = impl == 3
         dev = node_inp.device
         d_in, d = self.in_dim, self.out_dim
         H, T, R = self.n_heads, self.num_types, self.num_relations
@@ -373,11 +389,8 @@ class HGTConv(nn.Module):
         lt = _plan.layer_tables(plan, d_in, d, active_per_type, kv_runs)
         f32 = dict(dtype=torch.float32, device=dev)
         x = node_inp.contiguous()
-        if x_split is None and plan.sorted_types and self.linear_impl in (0, 2):
-            hint = getattr(node_inp, "_hgt_split", None)            # left by the previous layer's update epilogue
-            if (hint is not None and hint[2] == node_inp._version and x is node_inp
-                    and tuple(hint[0].shape) == (N, d_in) and d_in % 16 == 0 and d_in >= 64):
-                x_split = (hint[0], hint[1])
+        if x_split is None and plan.sorted_types and impl != 1:
+            x_split = _split_hint(node_inp, x, N, d_in, impl)       # left by the previous layer's update epilogue
         if plan.sorted_types:
             x_sorted = x
         else:
@@ -415,14 +428,14 @@ class HGTConv(nn.Module):
             if bf16:
                 # Q by its own fp32 call, the K'/V' blocks straight into the bf16 table; the tensor-core path splits A once
                 xs = x_split if plan.sorted_types else None
-                if xs is None and self.linear_impl in (0, 2) and d_in % 16 == 0 and d_in >= 64 and d % 16 == 0:
+                if xs is None and impl != 1 and d_in % 16 == 0 and d_in >= 64 and d % 16 == 0:
                     xs = (torch.empty((N, d_in), dtype=torch.bfloat16, device=dev),
-                          torch.empty((N, d_in), dtype=torch.bfloat16, device=dev))
+                          None if one else torch.empty((N, d_in), dtype=torch.bfloat16, device=dev))
                     _lib.call("hgt_act_split", x_sorted.data_ptr(), d_in, N, d_in, 0, None, xs[0].data_ptr(),
-                              xs[1].data_ptr(), st)
+                              _lib.ptr(xs[1]), st)
                 for tab, dst in ((lt.q_groups, q_tab), (lt.kv_groups, kv_tab)):
                     if xs is None:
-                        self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, dst, self.linear_impl, st)
+                        self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, dst, impl, st)
                         continue
                     g_dev, g_host, n_g, c_dev = tab
                     wsb = ctypes.c_size_t()
@@ -430,7 +443,7 @@ class HGTConv(nn.Module):
                               ctypes.byref(wsb))
                     ws1 = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
                     _lib.call("hgt_typed_linear_presplit_bf16" if dst.dtype == torch.bfloat16 else "hgt_typed_linear_presplit",
-                              xs[0].data_ptr(), xs[1].data_ptr(), w_cat.data_ptr(), b_cat.data_ptr(), d_in, d,
+                              xs[0].data_ptr(), None if one else _lib.ptr(xs[1]), w_cat.data_ptr(), b_cat.data_ptr(), d_in, d,
                               g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), dst.data_ptr(), ws1.data_ptr(),
                               ws1.numel(), st)
             elif x_split is not None and plan.sorted_types:
@@ -439,11 +452,12 @@ class HGTConv(nn.Module):
                 wsb = ctypes.c_size_t()
                 _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, d_in, d, ctypes.byref(wsb))
                 ws1 = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                _lib.call("hgt_typed_linear_presplit", x_split[0].data_ptr(), x_split[1].data_ptr(), w_cat.data_ptr(),
+                _lib.call("hgt_typed_linear_presplit", x_split[0].data_ptr(), None if one else _lib.ptr(x_split[1]),
+                          w_cat.data_ptr(),
                           b_cat.data_ptr(), d_in, d, g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(),
                           proj.data_ptr(), ws1.data_ptr(), ws1.numel(), st)
             else:
-                self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, lt.proj_groups, proj, self.linear_impl, st)
+                self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, lt.proj_groups, proj, impl, st)
         kvr = None
         if self.use_RTE:
             # RT = lin(emb.weight) [240,d] (conv.py:299), then projected with every pair's K'/V' weights (no bias)
@@ -460,11 +474,11 @@ class HGTConv(nn.Module):
         ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
         # When the a_linear GEMM will run on the tensor cores, the edge kernel writes gelu(agg) directly as the bf16
         # hi/lo operand split (no fp32 round trip, no separate split pass).
-        fuse_split = (gelu_before_a and not save and self.linear_impl in (0, 2) and d % 16 == 0 and d >= 64
+        fuse_split = (gelu_before_a and not save and impl != 1 and d % 16 == 0 and d >= 64
                       and not (self.training and self.drop.p > 0))
         g_act = None if fuse_split else torch.empty((N, d), **f32)
         g_hi = torch.empty((N, d), dtype=torch.bfloat16, device=dev) if fuse_split else None
-        g_lo = torch.empty((N, d), dtype=torch.bfloat16, device=dev) if fuse_split else None
+        g_lo = torch.empty((N, d), dtype=torch.bfloat16, device=dev) if fuse_split and not one else None
         att = torch.empty((E, H), **f32) if want_att else None
         stats = torch.empty((N, 2 * H), **f32) if save else None
         with self._stage("edge"):
@@ -493,11 +507,11 @@ class HGTConv(nn.Module):
                 wsb = ctypes.c_size_t()
                 _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, d, d, ctypes.byref(wsb))
                 ws2 = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                _lib.call("hgt_typed_linear_presplit", g_hi.data_ptr(), g_lo.data_ptr(), wa_cat.data_ptr(),
+                _lib.call("hgt_typed_linear_presplit", g_hi.data_ptr(), _lib.ptr(g_lo), wa_cat.data_ptr(),
                           ba_cat.data_ptr(), d, d, g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(),
                           o.data_ptr(), ws2.data_ptr(), ws2.numel(), st)
             else:
-                self._typed_linear(g_act, d, wa_cat, ba_cat, d, d, lt.upd_groups, o, self.linear_impl, st)
+                self._typed_linear(g_act, d, wa_cat, ba_cat, d, d, lt.upd_groups, o, impl, st)
         if self.training and self.drop.p > 0:
             o = self.drop(o)                                       # conv.py:125 (train mode only)
         return dict(plan=plan, lt=lt, x_sorted=x_sorted, w_cat=w_cat, proj=proj, q=q_tab, kv=kv_tab, kvr=kvr, agg=agg, o=o, stats=stats,

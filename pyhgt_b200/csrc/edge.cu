@@ -134,6 +134,7 @@ __device__ __forceinline__ void store_vec(float* p, const float (&src)[VEC]) {
   *reinterpret_cast<V*>(p) = v;
 }
 
+// lo == NULL: hi only (the operand of a one-product GEMM)
 template <int VEC>
 __device__ __forceinline__ void store_split_bf16(__nv_bfloat16* hi, __nv_bfloat16* lo, const float (&src)[VEC]) {
   __nv_bfloat16 h[VEC], l[VEC];
@@ -144,13 +145,13 @@ __device__ __forceinline__ void store_split_bf16(__nv_bfloat16* hi, __nv_bfloat1
   }
   if constexpr (VEC == 4) {
     *reinterpret_cast<uint2*>(hi) = *reinterpret_cast<uint2*>(h);
-    *reinterpret_cast<uint2*>(lo) = *reinterpret_cast<uint2*>(l);
+    if (lo) *reinterpret_cast<uint2*>(lo) = *reinterpret_cast<uint2*>(l);
   } else if constexpr (VEC == 2) {
     *reinterpret_cast<uint32_t*>(hi) = *reinterpret_cast<uint32_t*>(h);
-    *reinterpret_cast<uint32_t*>(lo) = *reinterpret_cast<uint32_t*>(l);
+    if (lo) *reinterpret_cast<uint32_t*>(lo) = *reinterpret_cast<uint32_t*>(l);
   } else {
     hi[0] = h[0];
-    lo[0] = l[0];
+    if (lo) lo[0] = l[0];
   }
 }
 
@@ -222,7 +223,7 @@ __device__ __forceinline__ void finalize_destination(const EdgeParams& p, const 
         r[v] = p.apply_gelu ? hgt_gelu_erf(x) : x;
       }
       if (p.agg_out) store_vec<VEC>(orow + o, r);
-      if (p.g_hi) store_split_bf16<VEC>(p.g_hi + (int64_t)dst * p.d + o, p.g_lo + (int64_t)dst * p.d + o, r);
+      if (p.g_hi) store_split_bf16<VEC>(p.g_hi + (int64_t)dst * p.d + o, p.g_lo ? p.g_lo + (int64_t)dst * p.d + o : nullptr, r);
     }
   }
   if (p.stats_out && lm.head_ok && lm.sub == 0) {
@@ -593,7 +594,7 @@ k_merge_partials(EdgeParams p, const int32_t* __restrict__ hubs, int n_hubs_host
         if (p.g_hi) {
           const __nv_bfloat16 h = __float2bfloat16_rn(t);
           p.g_hi[(int64_t)dst * p.d + c] = h;
-          p.g_lo[(int64_t)dst * p.d + c] = __float2bfloat16_rn(t - __bfloat162float(h));
+          if (p.g_lo) p.g_lo[(int64_t)dst * p.d + c] = __float2bfloat16_rn(t - __bfloat162float(h));
         }
       }
       __syncthreads();
@@ -704,8 +705,8 @@ int edge_forward(const float* q, const KV* kv, const KV* kvr, const int32_t* row
   HGT_REQUIRE(n_heads >= 1 && n_heads <= 32, "hgt_edge_forward: n_heads=%d unsupported (1..32)", n_heads);
   HGT_REQUIRE(d % n_heads == 0, "hgt_edge_forward: d=%d not divisible by n_heads=%d", d, n_heads);
   HGT_REQUIRE((kvr != nullptr) == (rte_row != nullptr), "hgt_edge_forward: kvr and rte_row must go together");
-  HGT_REQUIRE((g_hi != nullptr) == (g_lo != nullptr) && (agg_out != nullptr || g_hi != nullptr),
-              "hgt_edge_forward: need agg_out and/or the (g_hi, g_lo) pair");
+  HGT_REQUIRE((g_hi != nullptr || g_lo == nullptr) && (agg_out != nullptr || g_hi != nullptr),
+              "hgt_edge_forward: need agg_out and/or g_hi (g_lo only with g_hi)");
   HGT_REQUIRE(g_hi == nullptr || d % 8 == 0, "hgt_edge_forward: split output needs d %% 8 == 0 (d=%d)", d);
   size_t need = 0;
   hgt_edge_workspace_bytes(n_split_tiles, d, n_heads, &need);

@@ -4,6 +4,8 @@
 // the given stream without any host synchronisation.  This is what a non-Python host binds for the layer
 // (reference boundary: HGTConv.forward, pyHGT/conv.py:56-134); the Python class uses it too, so that a layer costs
 // one ctypes call instead of a dozen (the reference's sampled-subgraph batches are launch/host-bound).
+// linear_impl 3 runs the tensor-core GEMMs with one bf16 product: the edge kernel then writes gelu(agg) as bf16 hi only,
+// and a pre-split x needs no lo half.
 #include "common.cuh"
 
 int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
@@ -38,9 +40,11 @@ int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
   Carver c(base);
   const int64_t N = a->n_nodes;
   const int d = a->d_out, din = a->d_in;
+  HGT_REQUIRE(a->linear_impl >= 0 && a->linear_impl <= 3, "hgt_conv_forward: unknown linear_impl %d", a->linear_impl);
+  const bool one = a->linear_impl == 3;                    // one bf16 product: no lo halves
   const bool tc_upd = a->linear_impl != 1 && hgt_typed_linear_tc_supported(d, d, d);
   L->fuse_split = tc_upd;                                  // edge kernel writes gelu(agg) as the bf16 hi/lo split
-  L->presplit_x = a->x_hi != nullptr && a->x_lo != nullptr && a->perm == nullptr && a->linear_impl != 1 &&
+  L->presplit_x = a->x_hi != nullptr && (a->x_lo != nullptr || one) && a->perm == nullptr && a->linear_impl != 1 &&
                   hgt_typed_linear_tc_supported(din, din, d);
   L->x_sorted = a->perm ? c.take<float>((size_t)N * din) : nullptr;
   L->w_cat = c.take<float>((size_t)(a->cat_rows > 0 ? a->cat_rows : 1) * din);
@@ -64,7 +68,7 @@ int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
   L->g_hi = L->g_lo = nullptr;
   if (L->fuse_split) {
     L->g_hi = c.take_bytes((size_t)N * d * 2);
-    L->g_lo = c.take_bytes((size_t)N * d * 2);
+    L->g_lo = one ? nullptr : c.take_bytes((size_t)N * d * 2);
   } else {
     L->g_act = c.take<float>((size_t)N * d);
   }
@@ -120,7 +124,7 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
   // trailing all-zero [K'|V'] row (edges that match no <s,t,r> triple)
   HGT_CHECK_CUDA(cudaMemsetAsync(L.proj + a->kv_off + a->kv_rows * 2 * (int64_t)d, 0, sizeof(float) * 2 * d, st));
   if (L.presplit_x)
-    rc = hgt_typed_linear_presplit(a->x_hi, a->x_lo, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
+    rc = hgt_typed_linear_presplit(a->x_hi, a->linear_impl == 3 ? nullptr : a->x_lo, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
                                    a->n_proj_groups, a->proj_cblocks, L.proj, L.ws_proj, L.ws_proj_bytes + 256, stream);
   else
     rc = hgt_typed_linear(x_sorted, din, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups, a->n_proj_groups,

@@ -1,7 +1,7 @@
 // Typed (per-node-type) linear layers of HGTConv: weight folding (relation_att / relation_msg /
 // relation_pri into the K/V projections, SURVEY.md §8 a4) and the grouped GEMM front end.
-// This file holds the fp32 SIMT kernel (impl 1); the wgmma tensor-core kernel (impl 2) lives in
-// linear_tc.cu and is dispatched from hgt_typed_linear below.  hgt_typed_linear_bf16 runs the same kernels with a bf16
+// This file holds the fp32 SIMT kernel (impl 1); the wgmma tensor-core kernel (impl 2, split-bf16 x3; impl 3, auto with
+// one bf16 product on the tensor cores) lives in linear_tc.cu and is dispatched from hgt_typed_linear below.  hgt_typed_linear_bf16 runs the same kernels with a bf16
 // output, each fp32 result rounded to nearest-even once when it is stored.
 #include <cuda_bf16.h>
 
@@ -9,14 +9,15 @@
 
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
                         int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
-                        int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, void* workspace,
-                        size_t workspace_bytes, cudaStream_t st);
+                        int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int32_t products,
+                        void* workspace, size_t workspace_bytes, cudaStream_t st);
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
                         int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
-                        int32_t n_groups, const hgt_lin_cblock* cblocks, __nv_bfloat16* out, void* workspace,
-                        size_t workspace_bytes, cudaStream_t st);
+                        int32_t n_groups, const hgt_lin_cblock* cblocks, __nv_bfloat16* out, int32_t products,
+                        void* workspace, size_t workspace_bytes, cudaStream_t st);
 bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width);
-size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width);
+size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width,
+                                     int32_t products);
 
 namespace {
 
@@ -217,8 +218,13 @@ extern "C" int hgt_concat_linears(const float* const* w, const float* const* b, 
 extern "C" int hgt_typed_linear_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K,
                                                 int32_t cb_width, int32_t impl, size_t* out_bytes) {
   HGT_REQUIRE(out_bytes && (h_groups || n_groups == 0), "hgt_typed_linear_workspace_bytes: NULL argument");
-  if (impl == 0) impl = hgt_typed_linear_tc_supported(K, K, cb_width) ? 2 : 1;
-  *out_bytes = (impl == 2 && n_groups > 0) ? hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width) : 0;
+  HGT_REQUIRE(impl >= 0 && impl <= 3, "hgt_typed_linear_workspace_bytes: unknown impl %d", impl);
+  const bool tc = hgt_typed_linear_tc_supported(K, K, cb_width);
+  if (impl == 0) impl = tc ? 2 : 1;
+  if (impl == 3 && !tc) impl = 1;
+  *out_bytes = (impl >= 2 && n_groups > 0)
+                   ? hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width, impl == 3 ? 1 : 3)
+                   : 0;
   return 0;
 }
 
@@ -243,13 +249,14 @@ int typed_linear(const float* A, int64_t lda, const float* W, const float* bias,
     }
     return 0;
   }
-  if (impl == 0) impl = hgt_typed_linear_tc_supported(lda, K, cb_width) ? 2 : 1;
-  if (impl == 2) {
-    HGT_REQUIRE(hgt_typed_linear_tc_supported(lda, K, cb_width),
-                "hgt_typed_linear: tensor-core kernel does not support lda=%lld K=%d cb_width=%d",
+  const bool tc = hgt_typed_linear_tc_supported(lda, K, cb_width);
+  if (impl == 0) impl = tc ? 2 : 1;
+  if (impl == 3 && !tc) impl = 1;                         // one bf16 product where auto takes the tensor cores
+  if (impl == 2 || impl == 3) {
+    HGT_REQUIRE(tc, "hgt_typed_linear: tensor-core kernel does not support lda=%lld K=%d cb_width=%d",
                 (long long)lda, K, cb_width);
-    return hgt_typed_linear_tc(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace,
-                               workspace_bytes, st);
+    return hgt_typed_linear_tc(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out,
+                               impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
   }
   HGT_REQUIRE(impl == 1, "hgt_typed_linear: unknown impl %d", impl);
   TilePrefix tp;

@@ -19,6 +19,8 @@
 // Every (group, column block) gets its own tensor map (tight row extents => rows past the group are zero-filled by TMA, so the
 // reduction never sees a neighbour's rows); the maps live in the workspace (global memory).
 // SIMT fp32 path for shapes the tensor cores cannot take (width % 8, K % 16, overlapping groups such as the RTE tables).
+// impl 3: the tensor-core kernels with one bf16 product (tcp P = 1, torch's "medium" float32 matmul precision): only the
+// hi halves of dOut, A and W^T are written and read; db is still summed from the fp32 dOut.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -75,6 +77,7 @@ __device__ __forceinline__ float gelu_grad(float x) {
   return 0.5f * (1.0f + erff(x * 0.70710678118654752440f)) + x * 0.39894228040143267794f * __expf(-0.5f * x * x);
 }
 
+// lo == NULL: hi only
 __device__ __forceinline__ void split4(const float (&v)[4], uint2* hi, uint2* lo) {
   __nv_bfloat16 h[4], l[4];
 #pragma unroll
@@ -83,10 +86,10 @@ __device__ __forceinline__ void split4(const float (&v)[4], uint2* hi, uint2* lo
     l[j] = __float2bfloat16_rn(v[j] - __bfloat162float(h[j]));
   }
   *hi = *reinterpret_cast<uint2*>(h);
-  *lo = *reinterpret_cast<uint2*>(l);
+  if (lo) *lo = *reinterpret_cast<uint2*>(l);
 }
 
-// ---- fp32 [rows, K] (row stride ld) -> act(x) as fp32 and/or the bf16 hi/lo split [rows, Kp] -------------------------
+// ---- fp32 [rows, K] (row stride ld) -> act(x) as fp32 and/or the bf16 hi/lo split [rows, Kp] (lo NULL: hi only) ------
 __global__ void k_act_split(const float* __restrict__ in, int64_t ld, int64_t rows, int K, int Kp, int act,
                             float* __restrict__ out_f32, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
   const int vec_per_row = Kp / 4;
@@ -112,10 +115,11 @@ __global__ void k_act_split(const float* __restrict__ in, int64_t ld, int64_t ro
     for (int j = 0; j < 4; ++j)
       if (c + j < K) out_f32[r * K + c + j] = v[j];
   }
-  if (hi) split4(v, reinterpret_cast<uint2*>(hi + r * Kp + c), reinterpret_cast<uint2*>(lo + r * Kp + c));
+  if (hi) split4(v, reinterpret_cast<uint2*>(hi + r * Kp + c), lo ? reinterpret_cast<uint2*>(lo + r * Kp + c) : nullptr);
 }
 
-// ---- W [w_rows, K] -> W^T split, block-padded:  WT[k, blk*wpad + n] = W[blk*width + n, k], zero for n >= width ----------
+// ---- W [w_rows, K] -> W^T split, block-padded:  WT[k, blk*wpad + n] = W[blk*width + n, k], zero for n >= width (lo NULL:
+// hi only) ------------------------------------------------------------------------------------------------------------
 __global__ void k_wt_split(const float* __restrict__ W, int64_t w_rows, int K, int width, int wpad, int64_t wt_cols,
                            __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -129,7 +133,7 @@ __global__ void k_wt_split(const float* __restrict__ W, int64_t w_rows, int K, i
   if (n < width && wr < w_rows) v = W[wr * K + k];
   const __nv_bfloat16 h = __float2bfloat16_rn(v);
   hi[i] = h;
-  lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
 }
 
 // ---- dOut split pass + bias gradient ---------------------------------------------------------------------------------
@@ -170,7 +174,7 @@ __device__ __forceinline__ void split_colsum(const float* __restrict__ dout, con
         const int64_t off = tk.out_off + r * tk.ld + c0 * 4;
         const float4 v4 = *reinterpret_cast<const float4*>(dout + off);
         const float v[4] = {v4.x, v4.y, v4.z, v4.w};
-        split4(v, reinterpret_cast<uint2*>(hi + off), reinterpret_cast<uint2*>(lo + off));
+        split4(v, reinterpret_cast<uint2*>(hi + off), lo ? reinterpret_cast<uint2*>(lo + off) : nullptr);
 #pragma unroll
         for (int j = 0; j < 4; ++j) s[j] += v[j];
       }
@@ -247,18 +251,22 @@ struct DxJob {
       map_acquire(maps + tasks[t.task0 + c].map_dout + 1);
     }
   }
-  template <int BN>
+  template <int BN, int KB, int P>
   __device__ void load(const Tile& t, int it, uint32_t sa, uint32_t bar) const {
+    static_assert(KB == BK, "64-wide k-blocks");
+    constexpr uint32_t B = b_offset<BK, P>();
     const int c = it / t.kb_per_c, kb = it - c * t.kb_per_c;
     const GcTask& tk = tasks[t.task0 + c];
     const CUtensorMap* m_hi = maps + tk.map_dout;
     const CUtensorMap* m_lo = m_hi + 1;
     tma_load_2d(sa, m_hi, kb * BK, t.m0, bar);
     tma_load_2d(sa + ATOM_BYTES, m_hi, kb * BK, t.m0 + 64, bar);
-    tma_load_2d(sa + A_BYTES, m_lo, kb * BK, t.m0, bar);
-    tma_load_2d(sa + A_BYTES + ATOM_BYTES, m_lo, kb * BK, t.m0 + 64, bar);
-    tma_load_2d(sa + 2 * A_BYTES, maps + map_wt, tk.wt_col0 + kb * BK, t.n0, bar);
-    tma_load_2d(sa + 2 * A_BYTES + BN * BK * 2, maps + map_wt + 1, tk.wt_col0 + kb * BK, t.n0, bar);
+    tma_load_2d(sa + B, maps + map_wt, tk.wt_col0 + kb * BK, t.n0, bar);
+    if constexpr (P == 3) {
+      tma_load_2d(sa + A_BYTES, m_lo, kb * BK, t.m0, bar);
+      tma_load_2d(sa + A_BYTES + ATOM_BYTES, m_lo, kb * BK, t.m0 + 64, bar);
+      tma_load_2d(sa + B + BN * BK * 2, maps + map_wt + 1, tk.wt_col0 + kb * BK, t.n0, bar);
+    }
   }
   template <int BN>
   __device__ void store(const Tile& t, const float* acc, float*, int c, int wq, int lane) const {
@@ -324,20 +332,22 @@ struct DwJob {
     map_acquire(maps + t.map_x);
     map_acquire(maps + t.map_x + 1);
   }
-  template <int BN>
+  template <int BN, int KB, int P>
   __device__ void load(const Tile& t, int it, uint32_t sa, uint32_t bar) const {
+    static_assert(KB == BK, "64-row k-blocks");
+    constexpr uint32_t B = b_offset<BK, P>();
     const int row = (int)(t.r0 + (int64_t)it * BK);
     const CUtensorMap* d_hi = maps + t.map_dout;
     const CUtensorMap* x_hi = maps + t.map_x;
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       tma_load_2d(sa + j * ATOM_BYTES, d_hi, t.mt * BM + j * 64, row, bar);
-      tma_load_2d(sa + A_BYTES + j * ATOM_BYTES, d_hi + 1, t.mt * BM + j * 64, row, bar);
+      if constexpr (P == 3) tma_load_2d(sa + A_BYTES + j * ATOM_BYTES, d_hi + 1, t.mt * BM + j * 64, row, bar);
     }
 #pragma unroll
     for (int j = 0; j < BN / 64; ++j) {
-      tma_load_2d(sa + 2 * A_BYTES + j * ATOM_BYTES, x_hi, t.n0 + j * 64, row, bar);
-      tma_load_2d(sa + 2 * A_BYTES + BN * BK * 2 + j * ATOM_BYTES, x_hi + 1, t.n0 + j * 64, row, bar);
+      tma_load_2d(sa + B + j * ATOM_BYTES, x_hi, t.n0 + j * 64, row, bar);
+      if constexpr (P == 3) tma_load_2d(sa + B + BN * BK * 2 + j * ATOM_BYTES, x_hi + 1, t.n0 + j * 64, row, bar);
     }
   }
   template <int BN>
@@ -562,7 +572,7 @@ int make_map2(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int6
 }
 
 struct BwdLayout {
-  bool tc;
+  bool tc, one;              // tensor cores; one bf16 product (impl 3): no lo halves
   int Kp, wpad;
   int64_t a_rows, w_rows, wt_cols;
   int n_tasks;
@@ -616,7 +626,10 @@ bool bwd_tc_ok(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_cblock
 BwdLayout bwd_layout(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_cblock* h_cb, int K, int width,
                      int64_t lda, int64_t dout_elems, bool have_dsplit, bool have_asplit, int impl, bool det) {
   BwdLayout L{};
-  L.tc = impl == 2 || (impl == 0 && bwd_tc_ok(h_groups, n_groups, h_cb, K, width, lda));
+  // impl 3 with a pre-split A (the forward kept only its bf16 hi half) needs the tensor cores, as impl 2 does
+  L.tc = impl == 2 || (impl == 3 && have_asplit) ||
+         ((impl == 0 || impl == 3) && bwd_tc_ok(h_groups, n_groups, h_cb, K, width, lda));
+  L.one = L.tc && impl == 3;
   L.Kp = K;
   L.wpad = (width + BK - 1) / BK * BK;
   L.a_rows = 0;
@@ -636,11 +649,11 @@ BwdLayout bwd_layout(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_
   L.off_gfirst = take((size_t)(n_groups + 1) * sizeof(int64_t));
   if (L.tc) {
     L.off_dhi = take(have_dsplit ? 0 : (size_t)dout_elems * 2);
-    L.off_dlo = take(have_dsplit ? 0 : (size_t)dout_elems * 2);
+    L.off_dlo = take(have_dsplit || L.one ? 0 : (size_t)dout_elems * 2);
     L.off_ahi = take(have_asplit ? 0 : (size_t)L.a_rows * L.Kp * 2);
-    L.off_alo = take(have_asplit ? 0 : (size_t)L.a_rows * L.Kp * 2);
+    L.off_alo = take(have_asplit || L.one ? 0 : (size_t)L.a_rows * L.Kp * 2);
     L.off_wthi = take((size_t)K * L.wt_cols * 2);
-    L.off_wtlo = take((size_t)K * L.wt_cols * 2);
+    L.off_wtlo = take(L.one ? 0 : (size_t)K * L.wt_cols * 2);
   }
   L.dw_chunk = 0;
   L.off_part = L.off_dbp = 0;
@@ -660,50 +673,61 @@ BwdLayout bwd_layout(const hgt_lin_group* h_groups, int n_groups, const hgt_lin_
   return L;
 }
 
-template <int BN>
+// P: bf16 products per k-step (3: split, 1: hi only)
+template <int BN, int P>
 __global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dx_tc(const __grid_constant__ DxJob job, int n_tiles) {
-  split3_tile<BN, false, BK>(job, n_tiles);
+  split3_tile<BN, false, BK, OUT_STAGE_BYTES, P>(job, n_tiles);
 }
-template <int BN>
+template <int BN, int P>
 __global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc(const __grid_constant__ DwJob job, int n_tiles) {
-  split3_tile<BN, true, BK>(job, n_tiles);
+  split3_tile<BN, true, BK, OUT_STAGE_BYTES, P>(job, n_tiles);
 }
 
-template <int BN>
+template <int BN, int P>
 int launch_bwd(const DxJob& job, int tiles, cudaStream_t st) {
-  const size_t smem = tile_smem_bytes<BN>();
-  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dx_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_lin_dx_tc<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
+  const size_t smem = tile_smem_bytes<BN, BK, OUT_STAGE_BYTES, P>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dx_tc<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_lin_dx_tc<BN, P><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
-template <int BN>
+template <int BN, int P>
 int launch_bwd(const DwJob& job, int tiles, cudaStream_t st) {
-  const size_t smem = tile_smem_bytes<BN>();
-  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_lin_dw_tc<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
+  const size_t smem = tile_smem_bytes<BN, BK, OUT_STAGE_BYTES, P>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_lin_dw_tc<BN, P><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
 
-template <int BN>
+template <int BN, int P>
 __global__ void __launch_bounds__(TILE_THREADS, 1) k_lin_dw_tc_det(const __grid_constant__ DwJobDet job, int n_tiles) {
-  split3_tile<BN, true, BK>(job, n_tiles);
+  split3_tile<BN, true, BK, OUT_STAGE_BYTES, P>(job, n_tiles);
 }
-template <int BN>
+template <int BN, int P>
 int launch_bwd(const DwJobDet& job, int tiles, cudaStream_t st) {
-  const size_t smem = tile_smem_bytes<BN>();
-  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc_det<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_lin_dw_tc_det<BN><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
+  const size_t smem = tile_smem_bytes<BN, BK, OUT_STAGE_BYTES, P>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_lin_dw_tc_det<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_lin_dw_tc_det<BN, P><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
+}
+
+// Tile width (64 / 128 / 256) x products (3 / 1) of one of the three tensor-core jobs.
+template <class Job>
+int launch_bwd_any(const Job& job, int tile_n, bool one, int tiles, cudaStream_t st) {
+  switch (tile_n) {
+    case 64: return one ? launch_bwd<64, 1>(job, tiles, st) : launch_bwd<64, 3>(job, tiles, st);
+    case 128: return one ? launch_bwd<128, 1>(job, tiles, st) : launch_bwd<128, 3>(job, tiles, st);
+    default: return one ? launch_bwd<256, 1>(job, tiles, st) : launch_bwd<256, 3>(job, tiles, st);
+  }
 }
 
 }  // namespace
 
 extern "C" int hgt_act_split(const float* in, int64_t ld, int64_t rows, int32_t K, int32_t act, float* out_f32,
                              void* hi, void* lo, void* stream_) {
-  HGT_REQUIRE(in && (out_f32 || (hi && lo)), "hgt_act_split: NULL argument");
+  HGT_REQUIRE(in && (out_f32 || hi) && (hi || !lo), "hgt_act_split: NULL argument");
   HGT_REQUIRE(act == 0 || act == 1, "hgt_act_split: act=%d (0 = identity, 1 = gelu)", act);
   HGT_REQUIRE(!hi || K % 8 == 0, "hgt_act_split: the bf16 split needs K %% 8 == 0 (K=%d)", K);
   if (rows == 0) return 0;
@@ -724,6 +748,7 @@ int bwd_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, const h
                         int32_t impl, size_t* out_bytes, bool det) {
   HGT_REQUIRE(out_bytes && (n_groups == 0 || (h_groups && h_cblocks)), "hgt_typed_linear_bwd_workspace_bytes: NULL argument");
   HGT_REQUIRE(n_groups >= 0 && n_groups <= kMaxGroups, "hgt_typed_linear_bwd: n_groups=%d exceeds %d", n_groups, kMaxGroups);
+  HGT_REQUIRE(impl >= 0 && impl <= 3, "hgt_typed_linear_bwd_workspace_bytes: unknown impl %d", impl);
   *out_bytes = bwd_layout(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dout_split != 0,
                           have_a_split != 0, impl, det).total;
   return 0;
@@ -740,7 +765,9 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
   HGT_REQUIRE(K > 0 && cb_width > 0 && W, "hgt_typed_linear_bwd: K=%d cb_width=%d", K, cb_width);
   if (n_groups == 0) return 0;
   HGT_REQUIRE(groups && h_groups && h_cblocks, "hgt_typed_linear_bwd: NULL group tables");
-  const bool have_dsplit = dout_hi && dout_lo, have_asplit = a_hi_in && a_lo_in;
+  HGT_REQUIRE(impl >= 0 && impl <= 3, "hgt_typed_linear_bwd: unknown impl %d", impl);
+  // impl 3 reads only the hi halves, so a producer's split may come without its lo half
+  const bool have_dsplit = dout_hi && (dout_lo || impl == 3), have_asplit = a_hi_in && (a_lo_in || impl == 3);
   HGT_REQUIRE(dout || have_dsplit, "hgt_typed_linear_bwd: neither dout nor its bf16 split given");
   const BwdLayout L = bwd_layout(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dsplit, have_asplit, impl,
                                  det);
@@ -871,6 +898,11 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
                                     : reinterpret_cast<__nv_bfloat16*>(base + L.off_alo);
   __nv_bfloat16* wt_hi = reinterpret_cast<__nv_bfloat16*>(base + L.off_wthi);
   __nv_bfloat16* wt_lo = reinterpret_cast<__nv_bfloat16*>(base + L.off_wtlo);
+  // One product: the producers write no lo halves; the lo maps repeat the hi ones (never loaded, valid to prefetch).
+  __nv_bfloat16* const d_lo_w = L.one ? nullptr : d_lo;
+  __nv_bfloat16* const a_lo_w = L.one ? nullptr : a_lo;
+  __nv_bfloat16* const wt_lo_w = L.one ? nullptr : wt_lo;
+  if (L.one) d_lo = d_hi, a_lo = a_hi, wt_lo = wt_hi;
 
   // 1. tensor maps: per task dOut hi/lo {cols = width, rows = m}; per group A hi/lo {cols = K, rows = m}; W^T hi/lo.
   //    They encode addresses only, so they go up with the task table before any kernel runs.
@@ -902,25 +934,25 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
 
   // 2. dOut split (+ db) unless the producer already split it
   if (split_units > 0 && det) {
-    k_split_colsum_det<<<(unsigned)split_units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo,
+    k_split_colsum_det<<<(unsigned)split_units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo_w,
                                                               db ? db_part : nullptr);
     HGT_LAUNCH_CHECK();
     if (db && (rc = reduce_rows(db_part, 1, 1, 1, db))) return rc;
   } else if (split_units > 0) {
-    k_split_colsum<<<(unsigned)split_units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo, db);
+    k_split_colsum<<<(unsigned)split_units, 256, 0, st>>>(dout, d_tasks, nt, cb_width, d_hi, d_lo_w, db);
     HGT_LAUNCH_CHECK();
   }
   // 3. A split (dW needs it) unless saved by the forward
   if (dW && !have_asplit && L.a_rows > 0) {
     HGT_REQUIRE(A, "hgt_typed_linear_bwd: dW needs A or its bf16 split");
     const int64_t n = L.a_rows * (K / 4);
-    k_act_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, L.a_rows, K, K, 0, nullptr, a_hi, a_lo);
+    k_act_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, L.a_rows, K, K, 0, nullptr, a_hi, a_lo_w);
     HGT_LAUNCH_CHECK();
   }
   // 4. W^T split (dX)
   if (dA) {
     const int64_t n = (int64_t)K * L.wt_cols;
-    k_wt_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, L.w_rows, K, cb_width, L.wpad, L.wt_cols, wt_hi, wt_lo);
+    k_wt_split<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, L.w_rows, K, cb_width, L.wpad, L.wt_cols, wt_hi, wt_lo_w);
     HGT_LAUNCH_CHECK();
   }
 
@@ -960,12 +992,7 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
       job.dA = dA;
       job.accumulate = accumulate_dA;
       job.gelu_aux = gelu_aux;
-      switch (job.tile_n) {
-        case 64: rc = launch_bwd<64>(job, (int)total, st); break;
-        case 128: rc = launch_bwd<128>(job, (int)total, st); break;
-        default: rc = launch_bwd<256>(job, (int)total, st); break;
-      }
-      if (rc) return rc;
+      if ((rc = launch_bwd_any(job, job.tile_n, L.one, (int)total, st))) return rc;
     }
   }
   // 6. dW
@@ -1002,20 +1029,10 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
         DwJobDet dj;
         static_cast<DwJob&>(dj) = job;
         dj.part = part;
-        switch (tile_n) {
-          case 64: rc = launch_bwd<64>(dj, (int)units, st); break;
-          case 128: rc = launch_bwd<128>(dj, (int)units, st); break;
-          default: rc = launch_bwd<256>(dj, (int)units, st); break;
-        }
-        if (rc) return rc;
+        if ((rc = launch_bwd_any(dj, tile_n, L.one, (int)units, st))) return rc;
         if ((rc = reduce_rows(part, K, m_tiles * n_tiles, 0, dW))) return rc;
       } else {
-        switch (tile_n) {
-          case 64: rc = launch_bwd<64>(job, (int)units, st); break;
-          case 128: rc = launch_bwd<128>(job, (int)units, st); break;
-          default: rc = launch_bwd<256>(job, (int)units, st); break;
-        }
-        if (rc) return rc;
+        if ((rc = launch_bwd_any(job, tile_n, L.one, (int)units, st))) return rc;
       }
     }
   }

@@ -14,6 +14,10 @@
 // waits than the deeper ring gains (measured on the d = 400 OAG shape).  Output tiles follow the same group / column-block tables
 // as the SIMT kernel in linear.cu.  The output is fp32, or bf16 (hgt_typed_linear[_presplit]_bf16): the same tile, rounded
 // to nearest-even once as the epilogue stores it.
+//
+// One-product mode (P = 1: impl 3, or a presplit call with a_lo == NULL): the operands are rounded to bf16 (the hi half
+// of the split, bitwise) and one bf16 product per k-step is accumulated, torch's "medium" float32 matmul precision.  Its
+// stages hold {A_hi, W_hi} only; tiles, epilogues, barriers and tile order are those of P = 3.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -27,11 +31,11 @@ namespace {
 using namespace tcp;
 
 constexpr int kMaxGroups = 64;
-template <int BN> constexpr int fwd_bk() { return BN == 64 ? 64 : 32; }    // k-block of the forward GEMM
+template <int BN> constexpr int fwd_bk() { return BN == 64 ? 64 : 32; }    // k-block of the forward GEMM (P = 3)
 template <int BN> constexpr bool fwd_tma_store() { return BN != 64; }      // tensor-store epilogue (FwdJob::store)
 template <int BN> constexpr uint32_t fwd_out_stage() { return fwd_tma_store<BN>() ? TMA_STAGE_BYTES : OUT_STAGE_BYTES; }
 
-// ---- fp32 -> (bf16 hi, bf16 lo) split ------------------------------------------------------------
+// ---- fp32 -> (bf16 hi, bf16 lo) split; lo == NULL: hi only -------------------------------------------
 __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_t rows, int K, int Kp,
                              __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
   const int vec_per_row = Kp / 4;
@@ -55,7 +59,7 @@ __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_
     l[j] = __float2bfloat16_rn(v[j] - __bfloat162float(h[j]));
   }
   *reinterpret_cast<uint2*>(hi + r * Kp + c) = *reinterpret_cast<uint2*>(h);
-  *reinterpret_cast<uint2*>(lo + r * Kp + c) = *reinterpret_cast<uint2*>(l);
+  if (lo) *reinterpret_cast<uint2*>(lo + r * Kp + c) = *reinterpret_cast<uint2*>(l);
 }
 
 // Columns col .. col + 3 of an output row: fp32, or bf16 rounded to nearest-even.  aligned: p is 4-element aligned.
@@ -128,15 +132,16 @@ struct FwdJob {
   __device__ void prefetch(const Tile&) const {
     prefetch_map(&a_hi); prefetch_map(&a_lo); prefetch_map(&w_hi); prefetch_map(&w_lo);
   }
-  template <int BN>
+  template <int BN, int KB, int P>
   __device__ void load(const Tile& t, int kb, uint32_t sa, uint32_t bar) const {
-    constexpr int KB = fwd_bk<BN>();
-    constexpr uint32_t A = a_bytes<KB>();
+    constexpr uint32_t A = a_bytes<KB>(), B = b_offset<KB, P>();
     const int k = kb * KB;
     tma_load_2d(sa, &a_hi, k, t.a_row, bar);
-    tma_load_2d(sa + A, &a_lo, k, t.a_row, bar);
-    tma_load_2d(sa + 2 * A, &w_hi, k, t.w_row, bar);
-    tma_load_2d(sa + 2 * A + BN * KB * 2, &w_lo, k, t.w_row, bar);
+    tma_load_2d(sa + B, &w_hi, k, t.w_row, bar);
+    if constexpr (P == 3) {
+      tma_load_2d(sa + A, &a_lo, k, t.a_row, bar);
+      tma_load_2d(sa + B + BN * KB * 2, &w_lo, k, t.w_row, bar);
+    }
   }
   // BN = 128 / 256: asynchronous TMA tensor stores (tcp::store_tma) where the destination rows are 16-byte aligned, so
   // the stores overlap the next tile's products.  Otherwise, and at BN = 64, through shared memory with whole row segments
@@ -169,9 +174,9 @@ struct FwdJob {
   }
 };
 
-template <int BN, class OutT>
+template <int BN, class OutT, int P = 3, int KB = fwd_bk<BN>()>
 __global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob<OutT> job, int n_tiles) {
-  split3_tile<BN, false, fwd_bk<BN>(), fwd_out_stage<BN>()>(job, n_tiles);
+  split3_tile<BN, false, KB, fwd_out_stage<BN>(), P>(job, n_tiles);
 }
 
 // ---- output tensor maps of the tensor-store epilogue ----------------------------------------------------------------
@@ -272,16 +277,16 @@ void extents(const hgt_lin_group* h_groups, int n_groups, int cb_width, int64_t*
   }
 }
 
-// The tensor maps and the k-block count follow the kernel's k-block, fwd_bk<BN>().
-template <int BN, class OutT>
+// The tensor maps and the k-block count follow the kernel's k-block KB.  At P = 1 the lo maps repeat the hi ones (the
+// kernel does not load them; they stay valid for its prefetches).
+template <int BN, class OutT, int P = 3, int KB = fwd_bk<BN>()>
 int launch_fwd(FwdJob<OutT>& job, const __nv_bfloat16* const ops[4], int64_t a_rows, int64_t w_rows, int Kp, int tiles,
                cudaStream_t st) {
-  constexpr int KB = fwd_bk<BN>();
   int rc;
   if ((rc = make_map(&job.a_hi, ops[0], a_rows, Kp, BM, KB))) return rc;
-  if ((rc = make_map(&job.a_lo, ops[1], a_rows, Kp, BM, KB))) return rc;
+  if ((rc = make_map(&job.a_lo, ops[P == 3 ? 1 : 0], a_rows, Kp, BM, KB))) return rc;
   if ((rc = make_map(&job.w_hi, ops[2], w_rows, Kp, BN, KB))) return rc;
-  if ((rc = make_map(&job.w_lo, ops[3], w_rows, Kp, BN, KB))) return rc;
+  if ((rc = make_map(&job.w_lo, ops[P == 3 ? 3 : 2], w_rows, Kp, BN, KB))) return rc;
   job.k_blocks = (Kp + KB - 1) / KB;
   if constexpr (fwd_tma_store<BN>()) {
     CUtensorMap tmpl;
@@ -292,9 +297,10 @@ int launch_fwd(FwdJob<OutT>& job, const __nv_bfloat16* const ops[4], int64_t a_r
                                                   const_cast<CUtensorMap*>(job.out_maps));
     HGT_LAUNCH_CHECK();
   }
-  const size_t smem = tile_smem_bytes<BN, KB, fwd_out_stage<BN>()>();
-  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN, OutT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_typed_linear_tc<BN, OutT><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
+  const size_t smem = tile_smem_bytes<BN, KB, fwd_out_stage<BN>(), P>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN, OutT, P, KB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+  k_typed_linear_tc<BN, OutT, P, KB><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -306,11 +312,14 @@ bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width) {
   return cb_width % 16 == 0 && cb_width > 0 && K >= BK;
 }
 
-size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width) {
+// P = 1 needs no lo halves.
+size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width,
+                                     int32_t products) {
   int64_t a_rows, w_rows;
   extents(h_groups, n_groups, cb_width, &a_rows, &w_rows);
   const int Kp = (K + 7) / 8 * 8;
-  return 5 * 256 + 2 * hgt_align_up((size_t)a_rows * Kp * 2, 256) + 2 * hgt_align_up((size_t)w_rows * Kp * 2, 256) +
+  const size_t halves = products == 1 ? 1 : 2;
+  return 5 * 256 + halves * hgt_align_up((size_t)a_rows * Kp * 2, 256) + halves * hgt_align_up((size_t)w_rows * Kp * 2, 256) +
          hgt_align_up((size_t)n_out_maps(h_groups, n_groups) * sizeof(CUtensorMap), 256);
 }
 
@@ -318,28 +327,28 @@ template <class OutT>
 static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, const __nv_bfloat16* a_lo_in,
                   const float* W, const float* bias, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
                   const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
-                  void* workspace, size_t workspace_bytes, cudaStream_t st);
+                  int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st);
 
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
                         const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
-                        const hgt_lin_cblock* cblocks, float* out, void* workspace, size_t workspace_bytes,
-                        cudaStream_t st) {
-  return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace,
-                workspace_bytes, st);
+                        const hgt_lin_cblock* cblocks, float* out, int32_t products, void* workspace,
+                        size_t workspace_bytes, cudaStream_t st) {
+  return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, products,
+                workspace, workspace_bytes, st);
 }
 
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
                         const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
-                        const hgt_lin_cblock* cblocks, __nv_bfloat16* out, void* workspace, size_t workspace_bytes,
-                        cudaStream_t st) {
-  return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace,
-                workspace_bytes, st);
+                        const hgt_lin_cblock* cblocks, __nv_bfloat16* out, int32_t products, void* workspace,
+                        size_t workspace_bytes, cudaStream_t st) {
+  return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, products,
+                workspace, workspace_bytes, st);
 }
 
 extern "C" int hgt_typed_linear_presplit_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K,
                                                          int32_t cb_width, size_t* out_bytes) {
   HGT_REQUIRE(out_bytes && (h_groups || n_groups == 0), "hgt_typed_linear_presplit_workspace_bytes: NULL argument");
-  *out_bytes = n_groups > 0 ? hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width) : 0;
+  *out_bytes = n_groups > 0 ? hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width, 3) : 0;   // fits P = 1 too
   return 0;
 }
 
@@ -348,7 +357,7 @@ static int typed_linear_presplit(const void* a_hi, const void* a_lo, const float
                                  int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                                  int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out, void* workspace,
                                  size_t workspace_bytes, cudaStream_t st) {
-  HGT_REQUIRE(a_hi && a_lo, "hgt_typed_linear_presplit: NULL operand");
+  HGT_REQUIRE(a_hi, "hgt_typed_linear_presplit: NULL operand");          // a_lo == NULL: one bf16 product
   HGT_REQUIRE(K % 8 == 0 && hgt_typed_linear_tc_supported(K, K, cb_width),
               "hgt_typed_linear_presplit: unsupported shape K=%d cb_width=%d", K, cb_width);
   if (n_groups == 0) return 0;
@@ -362,7 +371,8 @@ static int typed_linear_presplit(const void* a_hi, const void* a_lo, const float
     return 0;
   }
   return tc_run(nullptr, 0, reinterpret_cast<const __nv_bfloat16*>(a_hi), reinterpret_cast<const __nv_bfloat16*>(a_lo),
-                W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, workspace, workspace_bytes, st);
+                W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, a_lo ? 3 : 1, workspace, workspace_bytes,
+                st);
 }
 
 extern "C" int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W, const float* bias,
@@ -387,26 +397,29 @@ template <class OutT>
 static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, const __nv_bfloat16* a_lo_in,
                   const float* W, const float* bias, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
                   const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
-                  void* workspace, size_t workspace_bytes, cudaStream_t st) {
+                  int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   HGT_REQUIRE(hgt_typed_linear_tc_supported(lda, K, cb_width), "hgt_typed_linear(tc): unsupported K=%d cb_width=%d", K,
               cb_width);
+  HGT_REQUIRE(products == 3 || products == 1, "hgt_typed_linear(tc): products=%d", products);
+  const bool one = products == 1;
   const int Kp = (K + 7) / 8 * 8;
   int64_t a_rows, w_rows;
   extents(h_groups, n_groups, cb_width, &a_rows, &w_rows);
-  size_t need = hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width);
+  size_t need = hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width, products);
   HGT_REQUIRE(workspace && workspace_bytes >= need, "hgt_typed_linear(tc): workspace too small (%zu < %zu)",
               workspace_bytes, need);
+  const size_t a_half = hgt_align_up((size_t)a_rows * Kp * 2, 256), w_half = hgt_align_up((size_t)w_rows * Kp * 2, 256);
   char* p = reinterpret_cast<char*>(hgt_align_up(reinterpret_cast<size_t>(workspace), 256));
-  __nv_bfloat16* a_hi = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)a_rows * Kp * 2, 256);
-  __nv_bfloat16* a_lo = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)a_rows * Kp * 2, 256);
-  __nv_bfloat16* w_hi = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)w_rows * Kp * 2, 256);
-  __nv_bfloat16* w_lo = reinterpret_cast<__nv_bfloat16*>(p); p += hgt_align_up((size_t)w_rows * Kp * 2, 256);
+  __nv_bfloat16* a_hi = reinterpret_cast<__nv_bfloat16*>(p); p += a_half;
+  __nv_bfloat16* a_lo = one ? nullptr : reinterpret_cast<__nv_bfloat16*>(p); p += one ? 0 : a_half;
+  __nv_bfloat16* w_hi = reinterpret_cast<__nv_bfloat16*>(p); p += w_half;
+  __nv_bfloat16* w_lo = one ? nullptr : reinterpret_cast<__nv_bfloat16*>(p); p += one ? 0 : w_half;
   CUtensorMap* out_maps = reinterpret_cast<CUtensorMap*>(p);
   {
     int64_t n = a_rows * (Kp / 4);
     if (a_hi_in) {
       a_hi = const_cast<__nv_bfloat16*>(a_hi_in);            // split by the producer (e.g. the edge kernel)
-      a_lo = const_cast<__nv_bfloat16*>(a_lo_in);
+      a_lo = one ? nullptr : const_cast<__nv_bfloat16*>(a_lo_in);
     } else if (n > 0) {
       k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, a_rows, K, Kp, a_hi, a_lo);
       HGT_LAUNCH_CHECK();
@@ -436,6 +449,20 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
   job.n_groups = n_groups;
   job.cb_width = cb_width;
   const __nv_bfloat16* const ops[4] = {a_hi, a_lo, w_hi, w_lo};
+  if (one) {
+    // k-block of the one-product kernel at BN = 128 / 256 (DESIGN.md §5.2): HGT_TC_P1_KB=32 selects the SWIZZLE_64B
+    // variant of the P = 3 kernel, for A/B measurements
+    static const bool kb32 = [] { const char* e = getenv("HGT_TC_P1_KB"); return e && e[0] == '3' && e[1] == '2'; }();
+    switch (job.tile_n) {
+      case 64: return launch_fwd<64, OutT, 1, 64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
+      case 128:
+        return kb32 ? launch_fwd<128, OutT, 1, 32>(job, ops, a_rows, w_rows, Kp, (int)total, st)
+                    : launch_fwd<128, OutT, 1, 64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
+      default:
+        return kb32 ? launch_fwd<256, OutT, 1, 32>(job, ops, a_rows, w_rows, Kp, (int)total, st)
+                    : launch_fwd<256, OutT, 1, 64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
+    }
+  }
   switch (job.tile_n) {
     case 64: return launch_fwd<64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
     case 128: return launch_fwd<128>(job, ops, a_rows, w_rows, Kp, (int)total, st);

@@ -1,13 +1,17 @@
 // Hopper (sm_90a) tensor-core plumbing shared by the typed-linear GEMMs (linear_tc.cu forward, linear_bwd.cu dX / dW):
 // mbarrier, TMA tile loads, wgmma shared-memory descriptors and instructions, and one warp-specialised kernel template.
 //
-// Every GEMM here is the split-bf16 x3 product: fp32 operands are split into x = x_hi + x_lo (two bf16 terms) and
+// By default every GEMM here is the split-bf16 x3 product (P = 3): fp32 operands are split into x = x_hi + x_lo (two bf16
+// terms) and
 //     A*B  ~=  A_hi*B_hi + A_hi*B_lo + A_lo*B_hi            (dropped term ~2^-18 relative)
-// is accumulated in one fp32 register accumulator, three bf16 wgmma products per k-step.
+// is accumulated in one fp32 register accumulator, three bf16 wgmma products per k-step.  P = 1 is the single bf16
+// product A_hi*B_hi (torch.set_float32_matmul_precision("medium")): a stage holds {A_hi, B_hi} only, so it is half the
+// size and the ring twice as deep.
 //
-// split3_tile<BN, MN, KB, Job>: the body of a persistent kernel (384 threads, at most one CTA per SM) whose CTAs walk the
+// split3_tile<BN, MN, KB, OUT, P, Job>: the body of a persistent kernel (384 threads, at most one CTA per SM) whose CTAs walk the
 // 128 x BN output tiles blockIdx.x, blockIdx.x + gridDim.x, ...
-//   warpgroup 0   TMA producer (one thread): per k-block one pipeline stage {A_hi, A_lo, B_hi, B_lo}; the ring runs on
+//   warpgroup 0   TMA producer (one thread): per k-block one pipeline stage {A_hi, A_lo, B_hi, B_lo} (P = 3) or
+//                 {A_hi, B_hi} (P = 1); the ring runs on
 //                 across tiles, so the next tile's first stages load while the consumers finish and store this one
 //   warpgroups 1-2  consumers: rows [64 c, 64 c + 64) of the tile, wgmma m64nBNk16 from shared memory
 // Operand tiles are TMA boxes with SWIZZLE_128B, 64 bf16 (128 bytes) along the inner dimension (KB = 64), or with
@@ -133,21 +137,33 @@ constexpr uint32_t OUT_STAGE_BYTES = 2 * 64 * 64 * 4;  // epilogue staging after
 constexpr uint32_t TMA_BUF_BYTES = 64 * 64 * 4;
 constexpr uint32_t TMA_STAGE_BYTES = 2 * 2 * TMA_BUF_BYTES;
 
-// Stage layout for a k-block of KB bf16: {A_hi, A_lo, B_hi, B_lo}; a consumer's 64-row A slab is one atom.  The ring
-// takes what the epilogue staging (OUT bytes) and the barriers leave, up to SMEM_BUDGET.
+// Stage layout for a k-block of KB bf16: {A_hi, A_lo, B_hi, B_lo} at P = 3, {A_hi, B_hi} at P = 1; a consumer's 64-row A
+// slab is one atom, B_lo follows B_hi.  The ring takes what the epilogue staging (OUT bytes) and the barriers leave, up
+// to SMEM_BUDGET.
 template <int KB> constexpr uint32_t a_bytes() { return BM * KB * 2; }
 template <int KB> constexpr uint32_t atom_bytes() { return 64 * KB * 2; }
-template <int BN, int KB = BK> constexpr uint32_t stage_bytes() { return 2 * a_bytes<KB>() + 2 * (uint32_t)BN * KB * 2; }
-template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES> constexpr int n_stages() {
-  constexpr uint32_t left = SMEM_LIMIT - 1024 - OUT - 256;
-  return (int)((left < SMEM_BUDGET ? left : SMEM_BUDGET) / stage_bytes<BN, KB>());
+template <int KB, int P> constexpr uint32_t b_offset() { return (P == 3 ? 2u : 1u) * a_bytes<KB>(); }   // B_hi in a stage
+template <int BN, int KB = BK, int P = 3> constexpr uint32_t stage_bytes() {
+  static_assert(P == 3 || P == 1, "three bf16 products (split) or one");
+  return (P == 3 ? 2u : 1u) * (a_bytes<KB>() + (uint32_t)BN * KB * 2);
 }
-template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES> constexpr size_t tile_smem_bytes() {
-  return 1024 + (size_t)n_stages<BN, KB, OUT>() * stage_bytes<BN, KB>() + OUT +
-         2 * n_stages<BN, KB, OUT>() * sizeof(uint64_t);
+template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES, int P = 3> constexpr int n_stages() {
+  constexpr uint32_t left = SMEM_LIMIT - 1024 - OUT - 256;
+  return (int)((left < SMEM_BUDGET ? left : SMEM_BUDGET) / stage_bytes<BN, KB, P>());
+}
+template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES, int P = 3> constexpr size_t tile_smem_bytes() {
+  return 1024 + (size_t)n_stages<BN, KB, OUT, P>() * stage_bytes<BN, KB, P>() + OUT +
+         2 * n_stages<BN, KB, OUT, P>() * sizeof(uint64_t);
 }
 static_assert(tile_smem_bytes<256, 32, TMA_STAGE_BYTES>() <= SMEM_LIMIT && tile_smem_bytes<256>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<128, 32, TMA_STAGE_BYTES>() <= SMEM_LIMIT && tile_smem_bytes<64>() <= SMEM_LIMIT,
+                  tile_smem_bytes<128, 32, TMA_STAGE_BYTES>() <= SMEM_LIMIT && tile_smem_bytes<64>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<256, 32, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<256, 64, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<128, 32, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<128, 64, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<256, 64, OUT_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<128, 64, OUT_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
+                  tile_smem_bytes<64, 64, OUT_STAGE_BYTES, 1>() <= SMEM_LIMIT,
               "ring + epilogue staging must fit the 227 KB a block may use");
 
 // Output tile width: 64, 128 or 256 columns, the one that pads `width` least (ties go to the wider tile).  Columns past
@@ -168,8 +184,9 @@ inline unsigned persistent_grid(int tiles) {
   return (unsigned)(tiles < sms ? tiles : sms);
 }
 
-// The 3 products of one k-block.  a_hi / a_lo: this warpgroup's 64-row A slab; b_hi / b_lo: the BN-column B tile.
-template <int BN, bool MN, int KB>
+// The P products of one k-block.  a_hi / a_lo: this warpgroup's 64-row A slab; b_hi / b_lo: the BN-column B tile (the lo
+// halves are not read at P = 1).
+template <int BN, bool MN, int KB, int P = 3>
 __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
   static_assert(!MN || KB == 64, "MN-major operands use 64-row k-blocks");
   constexpr uint32_t kstep = MN ? 16 * 128 : 32;       // 16 k: 16 rows of 128 bytes, or 32 bytes inside the swizzle row
@@ -183,17 +200,23 @@ __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_hi, uint32_t a
     const uint64_t bh = make_desc<KB>(b_hi + o, lbo), bl = make_desc<KB>(b_lo + o, lbo);
     if constexpr (BN == 64) {
       wgmma_n64<T, T>(acc, ah, bh);
-      wgmma_n64<T, T>(acc, ah, bl);
-      wgmma_n64<T, T>(acc, al, bh);
+      if constexpr (P == 3) {
+        wgmma_n64<T, T>(acc, ah, bl);
+        wgmma_n64<T, T>(acc, al, bh);
+      }
     } else {
       wgmma_n128<T, T>(acc, ah, bh);
-      wgmma_n128<T, T>(acc, ah, bl);
-      wgmma_n128<T, T>(acc, al, bh);
+      if constexpr (P == 3) {
+        wgmma_n128<T, T>(acc, ah, bl);
+        wgmma_n128<T, T>(acc, al, bh);
+      }
       if constexpr (BN == 256) {
         const uint64_t bh2 = make_desc<KB>(b_hi + o + b_half, lbo), bl2 = make_desc<KB>(b_lo + o + b_half, lbo);
         wgmma_n128<T, T>(acc + 64, ah, bh2);
-        wgmma_n128<T, T>(acc + 64, ah, bl2);
-        wgmma_n128<T, T>(acc + 64, al, bh2);
+        if constexpr (P == 3) {
+          wgmma_n128<T, T>(acc + 64, ah, bl2);
+          wgmma_n128<T, T>(acc + 64, al, bh2);
+        }
       }
     }
   }
@@ -311,16 +334,16 @@ __device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage
   }
 }
 
-// Called by a __global__ kernel with __launch_bounds__(TILE_THREADS, 1) and tile_smem_bytes<BN, KB, OUT>() of dynamic shared
+// Called by a __global__ kernel with __launch_bounds__(TILE_THREADS, 1) and tile_smem_bytes<BN, KB, OUT, P>() of dynamic shared
 // memory; `job` is the kernel's __grid_constant__ parameter (it holds the tensor maps), `n_tiles` the number of tiles
 // job.decode() accepts.  Every tile's k-blocks run in ascending order into a freshly zeroed accumulator, so a tile's
 // result does not depend on the grid size or on which CTA computes it.  job.store gets consumer c's half of the OUT bytes
-// of epilogue staging.
-template <int BN, bool MN, int KB, uint32_t OUT = OUT_STAGE_BYTES, class Job>
+// of epilogue staging.  job.load<BN, KB, P>() fills one stage in the layout of stage_bytes<BN, KB, P>().
+template <int BN, bool MN, int KB, uint32_t OUT = OUT_STAGE_BYTES, int P = 3, class Job>
 __device__ __forceinline__ void split3_tile(const Job& job, int n_tiles) {
-  constexpr int S = n_stages<BN, KB, OUT>();
-  constexpr uint32_t STAGE = stage_bytes<BN, KB>();
-  constexpr uint32_t A = a_bytes<KB>(), ATOM = atom_bytes<KB>();
+  constexpr int S = n_stages<BN, KB, OUT, P>();
+  constexpr uint32_t STAGE = stage_bytes<BN, KB, P>();
+  constexpr uint32_t A = a_bytes<KB>(), ATOM = atom_bytes<KB>(), B = b_offset<KB, P>();
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);
   unsigned char* out_stage = smem + (size_t)S * STAGE;
@@ -352,7 +375,7 @@ __device__ __forceinline__ void split3_tile(const Job& job, int n_tiles) {
           mbar_wait(s_u32(&empty_bar[s]), phase ^ 1u);
           const uint32_t bar = s_u32(&full_bar[s]);
           mbar_expect_tx(bar, STAGE);
-          job.template load<BN>(t, it, base + (uint32_t)s * STAGE, bar);
+          job.template load<BN, KB, P>(t, it, base + (uint32_t)s * STAGE, bar);
           if (++s == S) s = 0, phase ^= 1u;
         }
       }
@@ -371,7 +394,7 @@ __device__ __forceinline__ void split3_tile(const Job& job, int n_tiles) {
         mbar_wait(s_u32(&full_bar[s]), phase);
         const uint32_t sa = base + (uint32_t)s * STAGE;
         wgmma_fence();
-        mma_kblock<BN, MN, KB>(acc, sa + c * ATOM, sa + A + c * ATOM, sa + 2 * A, sa + 2 * A + (uint32_t)BN * KB * 2);
+        mma_kblock<BN, MN, KB, P>(acc, sa + c * ATOM, sa + A + c * ATOM, sa + B, sa + B + (uint32_t)BN * KB * 2);
         wgmma_commit();
         if (it > 0) {                                             // the previous k-block's products have retired
           wgmma_wait<1>();

@@ -85,7 +85,7 @@ __device__ __forceinline__ void split_store(uint2* hi, uint2* lo, int64_t idx, c
     l[j] = __float2bfloat16_rn(f[j] - __bfloat162float(h[j]));
   }
   hi[idx] = *reinterpret_cast<uint2*>(h);
-  lo[idx] = *reinterpret_cast<uint2*>(l);
+  if (lo) lo[idx] = *reinterpret_cast<uint2*>(l);            // NULL: hi only
 }
 
 // Vectorised variant: d % 4 == 0, each lane owns NV float4 chunks (chunk c = lane + 32*i), 128-bit loads/stores.
@@ -215,7 +215,7 @@ int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type
   const bool aligned = (d % 4 == 0) && ((reinterpret_cast<uintptr_t>(o) | reinterpret_cast<uintptr_t>(x) |
                                         reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(norm_w) |
                                         reinterpret_cast<uintptr_t>(norm_b)) % 16 == 0);
-  HGT_REQUIRE((out_hi != nullptr) == (out_lo != nullptr), "hgt_update_epilogue: out_hi/out_lo must go together");
+  HGT_REQUIRE(out_hi != nullptr || out_lo == nullptr, "hgt_update_epilogue: out_lo needs out_hi");
   HGT_REQUIRE(out_hi == nullptr || (aligned && d % 8 == 0 && perm == nullptr && type_active == nullptr),
               "hgt_update_epilogue: the split output needs d %% 8 == 0, 16-byte aligned buffers and identity row order");
   uint2* hi2 = reinterpret_cast<uint2*>(out_hi);

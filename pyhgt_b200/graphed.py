@@ -20,6 +20,10 @@ Either way:
 GraphedForward replays an inference forward; GraphedTrainStep replays a whole training step (plan rebuild, forward, loss,
 backward, gradient clipping, optimizer step).  The backward's typed GEMMs carry their host-built tables in kernel
 parameters (csrc/linear_bwd.cu: k_upload), which is what lets a graph record them.
+
+Both classes also record at capture whether the typed GEMMs ran with one bf16 product
+(torch.set_float32_matmul_precision("medium"), autograd.bf16_matmuls): the graph holds those kernels, so a later call
+under a setting that picks the other ones raises ValueError.
 """
 import numpy as np
 import torch
@@ -160,6 +164,7 @@ class _Graphed:
         self.tm = torch.zeros(sig.n_edges, **i64)
         self.h = None                                                      # pinned staging, made by the first host batch
         self.graph = None
+        self.one_product = None                                            # bf16_matmuls() at capture
         self.plan = None
         self._staged = None
         self._pins = []
@@ -230,6 +235,18 @@ class _Graphed:
     def _feed(self, batch, sizes):
         return self._scatter(batch, *sizes) if self._is_device(batch) else self._stage(batch)
 
+    def _check_precision(self):
+        """Record bf16_matmuls() before the first capture; raise ValueError if a later call's setting differs."""
+        from .autograd import bf16_matmuls
+        one = bf16_matmuls()
+        if self.graph is None:
+            self.one_product = one
+        elif one != self.one_product:
+            raise ValueError("%s was captured with %s typed GEMMs, but torch.get_float32_matmul_precision() is now %r: "
+                             "build a new one for this setting" % (type(self).__name__,
+                                                                    "one-product bf16" if self.one_product else "split-bf16 x3",
+                                                                    torch.get_float32_matmul_precision()))
+
     def _capture(self, fn):
         """Capture fn() on self.stream; the table uploads captured in it re-read their pinned sources at every replay, so
         those are kept (self._pins)."""
@@ -282,6 +299,7 @@ class GraphedForward(_Graphed):
             return self.fn(self.x, self.nt, self.tm, self.ei, self.et)
 
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type):
+        self._check_precision()
         batch = (node_feature, node_type, edge_time, edge_index, edge_type)
         cur = torch.cuda.current_stream(self.dev)
         self.stream.wait_stream(cur)
@@ -423,6 +441,7 @@ class GraphedTrainStep(_Graphed):
                 raise RuntimeError("optimizer hyperparameters %s changed after the step was captured: the graph holds "
                                    "their captured values (keep them fixed, or make them tensors updated in place)"
                                    % changed)
+        self._check_precision()
         batch = (node_feature, node_type, edge_time, edge_index, edge_type)
         cur = torch.cuda.current_stream(self.dev)
         self.stream.wait_stream(cur)

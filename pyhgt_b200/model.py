@@ -12,6 +12,7 @@ import torch.nn as nn
 
 from . import _lib
 from . import plan as _plan
+from .autograd import bf16_matmuls, gemm_impl
 from .conv import GeneralConv, HGTConv
 
 
@@ -70,7 +71,8 @@ class GNN(nn.Module):
                   b_cat.data_ptr(), st)
         # unknown-type rows stay 0 (model.py:70), and so do the rows past `rows`
         res = torch.zeros((N, self.n_hid), dtype=torch.float32, device=dev)
-        conv0._typed_linear(x, self.in_dim, w_cat, b_cat, self.in_dim, self.n_hid, table, res, conv0.linear_impl, st)
+        impl = gemm_impl(conv0.linear_impl, bf16_matmuls())
+        conv0._typed_linear(x, self.in_dim, w_cat, b_cat, self.in_dim, self.n_hid, table, res, impl, st)
         n_known = plan.type_row0[T]
         res[:n_known].tanh_()                                                    # model.py:75
         if not plan.sorted_types:
@@ -89,7 +91,7 @@ class GNN(nn.Module):
         b_cat = torch.cat([l.bias for l in self.adapt_ws], 0)
         n_known = plan.type_row0[T]
         zero = [((plan.type_row0[t] + rows[t]) * h, plan.type_row0[t + 1] * h) for t in range(T)] if rows else []
-        res = typed_linear(x, w_cat, b_cat, table, h, N * h, conv0.linear_impl, 0,
+        res = typed_linear(x, w_cat, b_cat, table, h, N * h, gemm_impl(conv0.linear_impl, bf16_matmuls()), 0,
                            zero + [(n_known * h, N * h)]).view(N, h)
         res = torch.cat([torch.tanh(res[:n_known]), res[n_known:]], 0) if n_known < N else torch.tanh(res)   # model.py:75
         if not plan.sorted_types:
