@@ -65,6 +65,14 @@ int hgt_plan_edges_sort(const int64_t* edge_index, const int64_t* edge_type, con
                         int32_t* row_ptr, int32_t* csr_eid, int32_t* presence, int32_t* flags,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/* Destination extent of every node type, from the CSR of hgt_plan_edges_sort: dst_end [T] int32 (zeroed here) =
+ * 1 + the rank of the last row of type t that has an in-edge, or 0 if none has.  Every edge counts, also one that
+ * matches no <source type, relation> pair.  perm [N]: from hgt_plan_nodes.  Rows of type t at ranks >= dst_end[t] have
+ * no in-edges: their aggregate is 0 and the layer output is exact without computing their Q, edge or a_linear rows
+ * (hgt_conv_args.type_dst, hgt_update_epilogue_dst).  Nothing is read back or synchronised. */
+int hgt_plan_dst_end(const int32_t* row_ptr, const int32_t* perm, const int64_t* node_type, int64_t n_nodes,
+                     int32_t num_types, int32_t* dst_end, void* stream);
+
 /* Per-CSR-edge gather indices.
  *   pair_of [T*R] int32: pair id of <source_type, relation> or -1;  pair_row0 [P] int32: first KV-table
  *   row of each pair;  type_row0 [T+1] int32: first rank of each type;  zero_row: index of the all-zero
@@ -295,7 +303,8 @@ int hgt_typed_linear_presplit_bf16(const void* a_hi, const void* a_lo, const flo
  *           n_tiles / n_split_tiles / n_hubs are the UPPER BOUNDS the arrays were sized with and the kernels read the
  *           true counts from the device (no host read-back between plan build and layer).
  *  type_row0 [T+2] / type_active [T]: NULL, or (sharded runs) the same tables hgt_update_epilogue takes: destinations
- *           past the active prefix of their type are halo sources — they have no in-edges and no output row is written. */
+ *           past the active prefix of their type are halo sources — they have no in-edges and no output row is written.
+ *           The type extents of hgt_plan_dst_end serve as type_active too: the rows past them have no in-edges. */
 int hgt_edge_workspace_bytes(int32_t n_split_tiles, int32_t d, int32_t n_heads, size_t* out_bytes);
 int hgt_edge_forward(const float* q, const float* kv, const float* kvr,
                      const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
@@ -480,6 +489,14 @@ int hgt_update_epilogue(const float* o, const float* x, const int32_t* type_row0
                         const float* skip, const float* norm_w, const float* norm_b,
                         const int32_t* perm, const int32_t* type_active, int64_t n_nodes, int32_t d,
                         float* out, void* out_hi, void* out_lo, void* stream);
+/* hgt_update_epilogue without type_active, for a layer whose a_linear covered only the first type_dst[t] rows of every
+ * type t (type_dst [T] int32, the extents of hgt_plan_dst_end): the other rows have no in-edges, so their a_linear
+ * output is exactly the bias, and they read o = bias[t] ([T, d], the a_linears' biases) instead of their `o` row, which
+ * is never read.  Every row is written, as by hgt_update_epilogue. */
+int hgt_update_epilogue_dst(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
+                            const float* skip, const float* norm_w, const float* norm_b, const int32_t* perm,
+                            const int32_t* type_dst, const float* bias, int64_t n_nodes, int32_t d, float* out,
+                            void* out_hi, void* out_lo, void* stream);
 
 
 /* ------------------------------------------------------------------------------------------------
@@ -534,6 +551,9 @@ typedef struct {
   float* out;                 /* [N or out rows, d_out] */
   float* att;                 /* [E, H] or NULL */
   void* out_hi; void* out_lo; /* optional: out again as the bf16 hi/lo split for the next layer */
+  const int32_t* type_dst;    /* [T] or NULL: extents of hgt_plan_dst_end (not with type_active).  The proj and upd tables
+                                 then hold Q and a_linear rows for the first type_dst[t] rows of each type only; the other
+                                 rows have no in-edges and take the a_linear bias (hgt_update_epilogue_dst) */
 } hgt_conv_args;
 
 uint64_t hgt_conv_args_size(void);   /* sizeof(hgt_conv_args): lets a foreign-language binding check its struct layout */

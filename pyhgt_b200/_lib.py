@@ -51,6 +51,9 @@ SIGNATURES = {
     "hgt_conv_workspace_bytes": [_p, _c.POINTER(_sz)],
     "hgt_conv_forward": [_p, _p, _sz, _p],
     "hgt_update_epilogue": [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p],
+    # inference over each type's destination extent (plan.GraphPlan.dst_extent)
+    "hgt_plan_dst_end": [_p, _p, _p, _i64, _i32, _p, _p],
+    "hgt_update_epilogue_dst": [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p],
     # deterministic training backward (torch.use_deterministic_algorithms)
     "hgt_plan_source_index": [_p, _p, _p, _i64, _i64, _i32, _p, _p, _p, _p, _sz, _p],
     "hgt_edge_backward_det_workspace_bytes": [_i32, _i32, _i32, _c.POINTER(_sz)],
@@ -121,7 +124,7 @@ class ConvArgs(ctypes.Structure):
             "rt_groups", "h_rt_groups", "rt_cblocks", "upd_groups", "h_upd_groups", "upd_cblocks",
             "wq", "bq", "wk", "bk", "wv", "bv", "wa", "ba", "norm_w", "norm_b",
             "relation_att", "relation_msg", "relation_pri", "skip", "emb_weight", "emb_lin_w", "emb_lin_b",
-            "x", "x_hi", "x_lo", "out", "att", "out_hi", "out_lo"]
+            "x", "x_hi", "x_lo", "out", "att", "out_hi", "out_lo", "type_dst"]
     _fields_ = ([(n, ctypes.c_int64) for n in _I64] + [(n, ctypes.c_int32) for n in _I32] +
                 [(n, ctypes.c_void_p) for n in _PTR])
 

@@ -236,10 +236,12 @@ class HGTConv(nn.Module):
 
     # ------------------------------------------------------------------------------------------
     def _forward_fused(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att,
-                       active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None, plan=None, impl=None):
+                       active_per_type=None, out_map=None, out_rows=None, x_split=None, kv_runs=None, plan=None, impl=None,
+                       dst=False):
         """Inference through the single entry point hgt_conv_forward (csrc/layer.cu).  The argument block is cached per
         (plan tables, parameter locations); per call only the data pointers change.  impl: the GEMMs' C impl
-        (autograd.gemm_impl), linear_impl by default."""
+        (autograd.gemm_impl), linear_impl by default.  dst: tables over each type's destination extent
+        (plan.layer_tables)."""
         if impl is None:
             impl = self.linear_impl
         dev = node_inp.device
@@ -249,7 +251,7 @@ class HGTConv(nn.Module):
         N, E = plan.n_nodes, plan.n_edges
         if node_inp.shape[0] != N:
             raise ValueError("node_inp has %d rows but node_type has %d" % (node_inp.shape[0], N))
-        lt = _plan.layer_tables(plan, d_in, d, active_per_type, kv_runs)
+        lt = _plan.layer_tables(plan, d_in, d, active_per_type, kv_runs, dst)
         tabs = [self._ptrs("wq", [l.weight for l in self.q_linears], dev),
                 self._ptrs("bq", [l.bias for l in self.q_linears], dev),
                 self._ptrs("wk", [l.weight for l in self.k_linears], dev),
@@ -276,6 +278,7 @@ class HGTConv(nn.Module):
             a.perm = None if plan.sorted_types else plan.perm.data_ptr()
             a.type_row0 = plan.type_row0_dev.data_ptr()
             a.type_active = _lib.ptr(lt.type_active_dev)
+            a.type_dst = _lib.ptr(lt.type_dst_dev)
             a.row_ptr, a.kv_row = plan.row_ptr.data_ptr(), plan.kv_row.data_ptr()
             a.rte_row = plan.rte_row.data_ptr() if self.use_RTE else None
             a.csr_eid, a.tiles, a.hubs = plan.csr_eid.data_ptr(), plan.tiles.data_ptr(), plan.hubs.data_ptr()
@@ -333,16 +336,21 @@ class HGTConv(nn.Module):
         rows; rows that are not active (halo sources) are never written, so the output holds exactly the owned rows.
         Without out_map, rows past the active prefix are zero.  plan: an explicit plan (a trimmed layer's view, trim.py)
         instead of the cached plan of the tensors.  Under bf16 autocast the layer runs the per-stage path with bf16
-        gather tables."""
+        gather tables.
+        A whole-graph inference forward computes Q, the edge pass and the a_linear only over each type's destination
+        extent (plan.GraphPlan.dst_extent): the rows past it have no in-edges, so their a_linear output is exactly the
+        bias, which the update epilogue reads instead.  Not with dropout on `o`, which would have to touch those rows."""
         from .autograd import bf16_matmuls, bf16_tables, gemm_impl
         bf16 = bf16_tables()
         impl = gemm_impl(self.linear_impl, bf16_matmuls())
+        dst = (not save and active_per_type is None and kv_runs is None and out_map is None and plan is None
+               and type(self)._has_skip and not (self.training and self.drop.p > 0))
         if (self.fused_call and not save and HGTConv.event_sink is None and type(self)._has_skip
                 and not (self.training and self.drop.p > 0) and not bf16):
             return self._forward_fused(node_inp, node_type, edge_index, edge_type, edge_time, want_att,
-                                       active_per_type, out_map, out_rows, x_split, kv_runs, plan, impl)
+                                       active_per_type, out_map, out_rows, x_split, kv_runs, plan, impl, dst)
         c = self._core(node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs, bf16=bf16, plan=plan, impl=impl)
+                       gelu_before_a=True, x_split=x_split, kv_runs=kv_runs, bf16=bf16, plan=plan, impl=impl, dst=dst)
         plan, lt, o, x_sorted, N, d, T, st = c["plan"], c["lt"], c["o"], c["x_sorted"], c["N"], c["d"], c["T"], c["st"]
         norm_w = norm_b = None
         if self.use_norm:
@@ -361,19 +369,25 @@ class HGTConv(nn.Module):
             o_hi = torch.empty((N, d), dtype=torch.bfloat16, device=o.device)
             o_lo = None if impl == 3 else torch.empty((N, d), dtype=torch.bfloat16, device=o.device)
         with self._stage("update_epilogue"):
-            _lib.call("hgt_update_epilogue", o.data_ptr(), x_sorted.data_ptr(), plan.type_row0_dev.data_ptr(), T,
-                      self.skip.data_ptr(), _lib.ptr(norm_w), _lib.ptr(norm_b), perm_ptr,
-                      _lib.ptr(lt.type_active_dev), N, d, out.data_ptr(), _lib.ptr(o_hi), _lib.ptr(o_lo), st)
+            if lt.type_dst_dev is not None:
+                _lib.call("hgt_update_epilogue_dst", o.data_ptr(), x_sorted.data_ptr(), plan.type_row0_dev.data_ptr(), T,
+                          self.skip.data_ptr(), _lib.ptr(norm_w), _lib.ptr(norm_b), perm_ptr, lt.type_dst_dev.data_ptr(),
+                          c["ba_cat"].data_ptr(), N, d, out.data_ptr(), _lib.ptr(o_hi), _lib.ptr(o_lo), st)
+            else:
+                _lib.call("hgt_update_epilogue", o.data_ptr(), x_sorted.data_ptr(), plan.type_row0_dev.data_ptr(), T,
+                          self.skip.data_ptr(), _lib.ptr(norm_w), _lib.ptr(norm_b), perm_ptr,
+                          _lib.ptr(lt.type_active_dev), N, d, out.data_ptr(), _lib.ptr(o_hi), _lib.ptr(o_lo), st)
         if o_hi is not None:
             out._hgt_split = (o_hi, o_lo, out._version)          # consumed by the next layer's projection (see _core)
         return out, c["att"], (c if save else None)
 
     def _core(self, node_inp, node_type, edge_index, edge_type, edge_time, want_att, save, active_per_type,
-              gelu_before_a, x_split=None, kv_runs=None, bf16=False, plan=None, impl=None):
+              gelu_before_a, x_split=None, kv_runs=None, bf16=False, plan=None, impl=None, dst=False):
         """Everything up to and including the typed a_linear: plan, weight fold, typed projections, fused edge kernel
         (gelu fused iff gelu_before_a and not save), a_linears.  Returns a dict of the intermediates.  bf16: bf16 [K'|V'] and
         RTE tables (Q and everything else fp32).  impl: the GEMMs' C impl (autograd.gemm_impl; 3 = one bf16 product, no lo
-        halves are made or read), linear_impl by default."""
+        halves are made or read), linear_impl by default.  dst: tables over each type's destination extent
+        (plan.layer_tables); `o` then holds only the rows inside the extents."""
         if impl is None:
             impl = self.linear_impl
         one = impl == 3
@@ -386,7 +400,7 @@ class HGTConv(nn.Module):
         N, E, P = plan.n_nodes, plan.n_edges, plan.n_pairs
         if node_inp.shape[0] != N:
             raise ValueError("node_inp has %d rows but node_type has %d" % (node_inp.shape[0], N))
-        lt = _plan.layer_tables(plan, d_in, d, active_per_type, kv_runs)
+        lt = _plan.layer_tables(plan, d_in, d, active_per_type, kv_runs, dst)
         f32 = dict(dtype=torch.float32, device=dev)
         x = node_inp.contiguous()
         if x_split is None and plan.sorted_types and impl != 1:
@@ -488,7 +502,7 @@ class HGTConv(nn.Module):
                       plan.hubs.data_ptr(), plan.n_hubs, N, E, d, H, 1 if (gelu_before_a and not save) else 0,
                       _lib.ptr(g_act), _lib.ptr(att), _lib.ptr(stats), _lib.ptr(g_hi), _lib.ptr(g_lo), ws.data_ptr(),
                       ws.numel(), self.edge_variant, _lib.ptr(plan.tile_counts_dev), plan.type_row0_dev.data_ptr(), T,
-                      _lib.ptr(lt.type_active_dev), st)
+                      _lib.ptr(lt.type_active_dev if lt.type_dst_dev is None else lt.type_dst_dev), st)
 
         # 4. typed output linear (conv.py:125 / conv.py:261)
         agg = None
@@ -515,7 +529,7 @@ class HGTConv(nn.Module):
         if self.training and self.drop.p > 0:
             o = self.drop(o)                                       # conv.py:125 (train mode only)
         return dict(plan=plan, lt=lt, x_sorted=x_sorted, w_cat=w_cat, proj=proj, q=q_tab, kv=kv_tab, kvr=kvr, agg=agg, o=o, stats=stats,
-                    att=att, N=N, d=d, T=T, st=st)
+                    att=att, N=N, d=d, T=T, st=st, ba_cat=ba_cat)
 
 
 class DenseHGTConv(HGTConv):

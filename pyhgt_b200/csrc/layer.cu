@@ -11,7 +11,8 @@
 int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
                              const float* skip, const float* norm_w, const float* norm_b, const float* const* norm_wp,
                              const float* const* norm_bp, const int32_t* perm, const int32_t* type_active,
-                             int64_t n_nodes, int32_t d, float* out, void* out_hi, void* out_lo, cudaStream_t st);
+                             const int32_t* type_dst, const float* bias, int64_t n_nodes, int32_t d, float* out,
+                             void* out_hi, void* out_lo, cudaStream_t st);
 bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width);
 
 namespace {
@@ -102,6 +103,7 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
   HGT_REQUIRE(a && workspace, "hgt_conv_forward: NULL argument");
   HGT_REQUIRE(a->d_in == a->d_out, "hgt_conv_forward: in_dim must equal out_dim (conv.py:131)");
   HGT_REQUIRE(!a->use_rte || a->rte_row, "hgt_conv_forward: use_rte needs rte_row");
+  HGT_REQUIRE(!(a->type_active && a->type_dst), "hgt_conv_forward: type_active and type_dst exclude each other");
   cudaStream_t st = (cudaStream_t)stream;
   Layout L;
   void* base = reinterpret_cast<void*>(hgt_align_up(reinterpret_cast<size_t>(workspace), 256));
@@ -139,11 +141,13 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
                                a->rte_cblocks, L.kvr, 1, nullptr, 0, stream)))
       return rc;
   }
+  // rows past type_dst[t] have no in-edges: as type_active, the edge kernel skips them (their Q rows were not computed)
+  const int32_t* dst_rows = a->type_active ? a->type_active : a->type_dst;
   if ((rc = hgt_edge_forward(L.proj + a->q_off, L.proj + a->kv_off, L.kvr, a->row_ptr, a->kv_row,
                              a->use_rte ? a->rte_row : nullptr, a->csr_eid, a->tiles, a->n_tiles, a->n_split, a->hubs,
                              a->n_hubs, N, a->n_edges, d, a->n_heads, 1, L.g_act, a->att, nullptr, L.g_hi, L.g_lo,
                              L.ws_edge, L.ws_edge_bytes, a->edge_variant, a->d_tile_counts, a->type_row0, T,
-                             a->type_active, stream)))
+                             dst_rows, stream)))
     return rc;
   if ((rc = hgt_concat_linears(a->wa, a->ba, T, d, d, L.wa_cat, L.ba_cat, stream))) return rc;
   if (L.fuse_split)
@@ -156,5 +160,6 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
   const int32_t* perm_out = a->out_map ? a->out_map : a->perm;
   return hgt_update_epilogue_impl(L.o, x_sorted, a->type_row0, T, a->skip, nullptr, nullptr,
                                   a->use_norm ? a->norm_w : nullptr, a->use_norm ? a->norm_b : nullptr, perm_out,
-                                  a->type_active, N, d, a->out, a->out_hi, a->out_lo, st);
+                                  a->type_active, a->type_dst, a->type_dst ? L.ba_cat : nullptr, N, d, a->out, a->out_hi,
+                                  a->out_lo, st);
 }

@@ -117,6 +117,21 @@ __global__ void k_edge_keys(const int64_t* __restrict__ edge_index, const int64_
   if (key >= 0 && (int)(threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&counts[key], __popc(same));
 }
 
+// dst_end[t] = max over rows r (rank order) of type t with an in-edge of r + 1.  Rows are type-contiguous, so the lanes of
+// a warp mostly share a type: one atomicMax per type and warp.
+__global__ void k_dst_end(const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ perm,
+                          const int64_t* __restrict__ node_type, int64_t N, int T, int32_t* __restrict__ dst_end) {
+  const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  int32_t t = -1;
+  if (r < N && row_ptr[r + 1] > row_ptr[r]) {
+    const int64_t nt = node_type[perm[r]];
+    if (nt >= 0 && nt < T) t = (int32_t)nt;
+  }
+  const unsigned same = __match_any_sync(0xffffffffu, t);
+  const int32_t end = __reduce_max_sync(same, t >= 0 ? (int32_t)(r + 1) : 0);
+  if (t >= 0 && (int)(threadIdx.x & 31) == __ffs(same) - 1) atomicMax(&dst_end[t], end);
+}
+
 __global__ void k_edge_fill(const int64_t* __restrict__ edge_index, const int64_t* __restrict__ edge_type,
                             const int64_t* __restrict__ edge_time, const int64_t* __restrict__ node_type,
                             const int32_t* __restrict__ rank, const int32_t* __restrict__ csr_eid,
@@ -650,6 +665,18 @@ extern "C" int hgt_plan_edges_sort(const int64_t* edge_index, const int64_t* edg
                                                    (const int32_t*)s.vals_in, csr_eid, (int)n_edges, 0,
                                                    bits_for(n_nodes > 1 ? n_nodes : 2), st));
   }
+  return 0;
+}
+
+extern "C" int hgt_plan_dst_end(const int32_t* row_ptr, const int32_t* perm, const int64_t* node_type, int64_t n_nodes,
+                                int32_t num_types, int32_t* dst_end, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  HGT_REQUIRE(num_types >= 1 && dst_end && (n_nodes == 0 || (row_ptr && perm && node_type)),
+              "hgt_plan_dst_end: bad argument");
+  HGT_CHECK_CUDA(cudaMemsetAsync(dst_end, 0, sizeof(int32_t) * num_types, st));
+  if (n_nodes == 0) return 0;
+  k_dst_end<<<blocks_for(n_nodes), kThreads, 0, st>>>(row_ptr, perm, node_type, n_nodes, num_types, dst_end);
+  HGT_LAUNCH_CHECK();
   return 0;
 }
 

@@ -14,7 +14,8 @@ k_update_epilogue(const float* __restrict__ o, const float* __restrict__ x, cons
                   int T, const float* __restrict__ skip, const float* __restrict__ norm_w,
                   const float* __restrict__ norm_b, const float* const* __restrict__ norm_wp,
                   const float* const* __restrict__ norm_bp, const int32_t* __restrict__ perm,
-                  const int32_t* __restrict__ type_active, int64_t n_nodes, int d, float* __restrict__ out) {
+                  const int32_t* __restrict__ type_active, const int32_t* __restrict__ type_dst,
+                  const float* __restrict__ bias, int64_t n_nodes, int d, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   if (row >= n_nodes) return;
@@ -31,7 +32,8 @@ k_update_epilogue(const float* __restrict__ o, const float* __restrict__ x, cons
   // skip == NULL: plain residual y = o + x (DenseHGTConv, conv.py:261,273)
   const float alpha = skip ? 1.0f / (1.0f + __expf(-skip[t])) : 1.0f;    // torch.sigmoid(self.skip[t]), conv.py:129
   const float beta = skip ? 1.0f - alpha : 1.0f;
-  const float* op = o + row * d;
+  // rows past type_dst[t] have no in-edges: their a_linear output is exactly the bias, and their `o` row was not written
+  const float* op = (type_dst && row - type_row0[t] >= type_dst[t]) ? bias + (int64_t)t * d : o + row * d;
   const float* xp = x + row * d;
   float y[kMaxPerLane];
   float sum = 0.f;
@@ -95,7 +97,8 @@ k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, 
                       int T, const float* __restrict__ skip, const float* __restrict__ norm_w,
                       const float* __restrict__ norm_b, const float* const* __restrict__ norm_wp,
                       const float* const* __restrict__ norm_bp, const int32_t* __restrict__ perm,
-                      const int32_t* __restrict__ type_active, int64_t n_nodes, int d, float* __restrict__ out,
+                      const int32_t* __restrict__ type_active, const int32_t* __restrict__ type_dst,
+                      const float* __restrict__ bias, int64_t n_nodes, int d, float* __restrict__ out,
                       uint2* __restrict__ out_hi, uint2* __restrict__ out_lo) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
@@ -108,14 +111,24 @@ k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, 
     if (t0 < T && row - type_row0[t0] >= type_active[t0]) return;
     if (perm && perm[row] < 0) return;
   }
+  const float4* op = reinterpret_cast<const float4*>(o + row * d);
+  bool tail = false;
+  if (type_dst) {
+    // rows past type_dst[t] have no in-edges: their a_linear output is exactly the bias, and their `o` row was not written
+    int t0 = 0;
+    while (t0 < T && row >= type_row0[t0 + 1]) ++t0;
+    if (t0 < T && row - type_row0[t0] >= type_dst[t0]) {
+      tail = true;
+      op = reinterpret_cast<const float4*>(bias + (int64_t)t0 * d);
+    }
+  }
   // issue the row loads first; the (short, warp-uniform) type search overlaps with them
   float4 ov[NV], xv[NV];
-  const float4* op = reinterpret_cast<const float4*>(o + row * d);
   const float4* xp = reinterpret_cast<const float4*>(x + row * d);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int c = lane + 32 * i;
-    if (c < nvec) { ov[i] = __ldcs(op + c); xv[i] = __ldcs(xp + c); }
+    if (c < nvec) { ov[i] = tail ? __ldg(op + c) : __ldcs(op + c); xv[i] = __ldcs(xp + c); }
     else { ov[i] = make_float4(0.f, 0.f, 0.f, 0.f); xv[i] = ov[i]; }
   }
   int t = 0;
@@ -191,13 +204,13 @@ k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, 
 template <int NV>
 void launch_vec(const float* o, const float* x, const int32_t* type_row0, int T, const float* skip,
                 const float* norm_w, const float* norm_b, const float* const* norm_wp, const float* const* norm_bp,
-                const int32_t* perm, const int32_t* type_active, int64_t n_nodes, int d, float* out, uint2* out_hi,
-                uint2* out_lo, cudaStream_t st) {
+                const int32_t* perm, const int32_t* type_active, const int32_t* type_dst, const float* bias,
+                int64_t n_nodes, int d, float* out, uint2* out_hi, uint2* out_lo, cudaStream_t st) {
   const int warps_per_block = 8;
   unsigned grid = (unsigned)((n_nodes + warps_per_block - 1) / warps_per_block);
   k_update_epilogue_vec<NV><<<grid, warps_per_block * 32, 0, st>>>(o, x, type_row0, T, skip, norm_w, norm_b, norm_wp,
-                                                                  norm_bp, perm, type_active, n_nodes, d, out, out_hi,
-                                                                  out_lo);
+                                                                  norm_bp, perm, type_active, type_dst, bias, n_nodes,
+                                                                  d, out, out_hi, out_lo);
 }
 
 }  // namespace
@@ -205,7 +218,10 @@ void launch_vec(const float* o, const float* x, const int32_t* type_row0, int T,
 int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
                              const float* skip, const float* norm_w, const float* norm_b, const float* const* norm_wp,
                              const float* const* norm_bp, const int32_t* perm, const int32_t* type_active,
-                             int64_t n_nodes, int32_t d, float* out, void* out_hi, void* out_lo, cudaStream_t st) {
+                             const int32_t* type_dst, const float* bias, int64_t n_nodes, int32_t d, float* out,
+                             void* out_hi, void* out_lo, cudaStream_t st) {
+  HGT_REQUIRE(type_dst == nullptr || (bias != nullptr && type_active == nullptr),
+              "hgt_update_epilogue: type_dst needs the a_linear bias and excludes type_active");
   HGT_REQUIRE(d >= 1 && d <= 32 * kMaxPerLane, "hgt_update_epilogue: d=%d unsupported (max %d)", d,
               32 * kMaxPerLane);
   HGT_REQUIRE((norm_w == nullptr) == (norm_b == nullptr) && (norm_wp == nullptr) == (norm_bp == nullptr),
@@ -214,7 +230,8 @@ int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type
   // with pointer tables the per-type vectors are separate nn.LayerNorm parameters: torch allocations, 16-byte aligned
   const bool aligned = (d % 4 == 0) && ((reinterpret_cast<uintptr_t>(o) | reinterpret_cast<uintptr_t>(x) |
                                         reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(norm_w) |
-                                        reinterpret_cast<uintptr_t>(norm_b)) % 16 == 0);
+                                        reinterpret_cast<uintptr_t>(norm_b) |
+                                        reinterpret_cast<uintptr_t>(bias)) % 16 == 0);
   HGT_REQUIRE(out_hi != nullptr || out_lo == nullptr, "hgt_update_epilogue: out_lo needs out_hi");
   HGT_REQUIRE(out_hi == nullptr || (aligned && d % 8 == 0 && perm == nullptr && type_active == nullptr),
               "hgt_update_epilogue: the split output needs d %% 8 == 0, 16-byte aligned buffers and identity row order");
@@ -222,17 +239,17 @@ int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type
   uint2* lo2 = reinterpret_cast<uint2*>(out_lo);
   if (aligned && d <= 1024) {
     const int nv = (d / 4 + 31) / 32;
-    if (nv <= 1) launch_vec<1>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, n_nodes, d, out, hi2, lo2, st);
-    else if (nv <= 2) launch_vec<2>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, n_nodes, d, out, hi2, lo2, st);
-    else if (nv <= 4) launch_vec<4>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, n_nodes, d, out, hi2, lo2, st);
-    else launch_vec<8>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, n_nodes, d, out, hi2, lo2, st);
+    if (nv <= 1) launch_vec<1>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
+    else if (nv <= 2) launch_vec<2>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
+    else if (nv <= 4) launch_vec<4>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
+    else launch_vec<8>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
     HGT_LAUNCH_CHECK();
     return 0;
   }
   const int warps_per_block = 8;
   unsigned grid = (unsigned)((n_nodes + warps_per_block - 1) / warps_per_block);
   k_update_epilogue<<<grid, warps_per_block * 32, 0, st>>>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp,
-                                                           norm_bp, perm, type_active, n_nodes, d, out);
+                                                           norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -242,5 +259,14 @@ extern "C" int hgt_update_epilogue(const float* o, const float* x, const int32_t
                                    const int32_t* perm, const int32_t* type_active, int64_t n_nodes, int32_t d,
                                    float* out, void* out_hi, void* out_lo, void* stream_) {
   return hgt_update_epilogue_impl(o, x, type_row0, num_types, skip, norm_w, norm_b, nullptr, nullptr, perm,
-                                  type_active, n_nodes, d, out, out_hi, out_lo, (cudaStream_t)stream_);
+                                  type_active, nullptr, nullptr, n_nodes, d, out, out_hi, out_lo, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_update_epilogue_dst(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
+                                       const float* skip, const float* norm_w, const float* norm_b, const int32_t* perm,
+                                       const int32_t* type_dst, const float* bias, int64_t n_nodes, int32_t d,
+                                       float* out, void* out_hi, void* out_lo, void* stream_) {
+  HGT_REQUIRE(type_dst && bias, "hgt_update_epilogue_dst: NULL type_dst / bias");
+  return hgt_update_epilogue_impl(o, x, type_row0, num_types, skip, norm_w, norm_b, nullptr, nullptr, perm, nullptr,
+                                  type_dst, bias, n_nodes, d, out, out_hi, out_lo, (cudaStream_t)stream_);
 }

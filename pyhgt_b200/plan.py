@@ -62,6 +62,9 @@ class GraphPlan:
     flags_dev: torch.Tensor = None         # sync-free plans: range-check flags left on the device (see check())
     dst_ranges: torch.Tensor = None        # a trimmed layer's view (trim.py): [n, 2] int32 row ranges of the destinations
     n_dst_ranges: int = 0                  # its tiles cover; the source index then holds only their edges
+    dst_extent: list = None                # [T] host ints: rows [dst_extent[t], type_count[t]) of type t (rank order,
+                                           # counted from the type's first row) have no in-edges; sync-free plans: the
+                                           # type counts
     _layer_tables: dict = field(default_factory=dict)
     _source_index: dict = field(default_factory=dict)   # "kv" / "rte" -> SourceIndex (deterministic backward)
 
@@ -196,12 +199,14 @@ def build_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relat
     _lib.call("hgt_plan_workspace_bytes", N, E, ctypes.byref(ws_bytes))
     ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
 
-    # one small buffer for everything the host may read back: [type_count T+1 | sorted 1 | presence T*R | flags 4]
-    meta = torch.zeros(T + 1 + 1 + T * R + 4, **i32)
+    # one small buffer for everything the host may read back:
+    # [type_count T+1 | sorted 1 | presence T*R | flags 4 | dst_end T]
+    meta = torch.zeros(T + 1 + 1 + T * R + 4 + T, **i32)
     type_count_d = meta[:T + 1]
     sorted_d = meta[T + 1:T + 2]
     presence_d = meta[T + 2:T + 2 + T * R]
-    flags_d = meta[T + 2 + T * R:]
+    flags_d = meta[T + 2 + T * R:T + 6 + T * R]
+    dst_end_d = meta[T + 6 + T * R:]
     sync_free = host_meta is not None
     if sync_free and host_meta.get("sorted", False):
         rank = torch.arange(max(N, 1), **i32)                  # type-contiguous layout (to_torch): identity order
@@ -228,6 +233,7 @@ def build_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relat
             if 0 <= s_ < T and 0 <= r_ < R:
                 presence[s_, r_] = 1
     else:
+        _lib.call("hgt_plan_dst_end", row_ptr.data_ptr(), perm.data_ptr(), nt.data_ptr(), N, T, dst_end_d.data_ptr(), st)
         meta_h = meta.cpu().numpy()                       # the one host sync of the node/edge pass
         type_count = [int(v) for v in meta_h[:T + 1]]
         sorted_types = bool(meta_h[T + 1])
@@ -238,6 +244,10 @@ def build_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relat
     type_row0 = [0]
     for c in type_count:
         type_row0.append(type_row0[-1] + c)
+    if sync_free:
+        dst_extent = type_count[:T]
+    else:
+        dst_extent = [max(0, int(e) - type_row0[t]) for t, e in enumerate(meta_h[T + 6 + T * R:])]
     pairs, pair_row0, pair_of = [], [], -np.ones(T * R, dtype=np.int32)
     rows = 0
     for s in range(T):
@@ -295,7 +305,8 @@ def build_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relat
                      pairs=pairs, pair_row0=pair_row0, kv_rows=rows, tiles=tiles[:max(n_tiles, 1)],
                      n_tiles=n_tiles, n_split=n_split, hubs=hubs[:max(n_hubs, 1)], n_hubs=n_hubs,
                      pair_type_dev=pair_type_d, pair_rel_dev=pair_rel_d,
-                     tile_counts_dev=n_tiles_d if sync_free else None, flags_dev=flags_d if sync_free else None)
+                     tile_counts_dev=n_tiles_d if sync_free else None, flags_dev=flags_d if sync_free else None,
+                     dst_extent=dst_extent)
 
 
 # ---- source-major index of the deterministic edge backward -------------------------------------------
@@ -380,6 +391,7 @@ class LayerTables:
     kv_off: int
     proj_elems: int
     type_active_dev: torch.Tensor = None
+    type_dst_dev: torch.Tensor = None   # [T] int32: the plan's dst_extent when the tables cover it (layer_tables(dst=True))
     q_groups: tuple = None        # proj_groups split for bf16 gather tables: the Q blocks alone (offsets into [N, d_out])
     kv_groups: tuple = None       # ... and the K'/V' blocks alone (offsets relative to kv_off)
 
@@ -402,13 +414,21 @@ def _pack_groups(groups, cblocks, dev):
     return tab
 
 
-def layer_tables(plan, d_in, d_out, active=None, kv_runs=None):
+def layer_tables(plan, d_in, d_out, active=None, kv_runs=None, dst=False):
     """`active[t]` (sharded runs): only the first active[t] nodes of type t (in rank order) are destinations
     that need Q / a_linear / update; the rest of the type (halo sources) only get K'/V' rows.
     `kv_runs` (sharded runs): (((type, relation), ((row0, row1), ...)), ...) — type-relative row ranges whose K'/V' rows
     some local edge reads; the projection then covers those ranges only (the other rows of the table are never
-    gathered and stay unwritten)."""
-    key = (d_in, d_out, None if active is None else tuple(active), kv_runs)
+    gathered and stay unwritten).
+    `dst` (inference without active / kv_runs): Q and a_linear rows only for the first plan.dst_extent[t] rows of each
+    type, like `active`, but every row keeps its output: the rows past the extent have no in-edges, and the update
+    epilogue gives them the a_linear bias (type_dst_dev).  A plan whose extents cover every row gets the plain tables."""
+    ext = None
+    if (dst and active is None and kv_runs is None and plan.dst_extent is not None
+            and any(e < c for e, c in zip(plan.dst_extent, plan.type_count))):
+        ext = [int(e) for e in plan.dst_extent]
+        active = ext
+    key = (d_in, d_out, None if active is None else tuple(active), kv_runs, ext is not None)
     hit = plan._layer_tables.get(key)
     if hit is not None:
         return hit
@@ -513,7 +533,8 @@ def layer_tables(plan, d_in, d_out, active=None, kv_runs=None):
     small = _to_dev_async(np.asarray(q_row0 + (cat_row0 if P else [0]) + act, dtype=np.int32), dev)
     lt = LayerTables(cat_rows=rows, q_row0=q_row0, cat_row0=cat_row0, q_row0_dev=small[:T],
                      cat_row0_dev=small[T:T + max(P, 1)],
-                     type_active_dev=None if active is None else small[T + max(P, 1):], proj_groups=proj, rte_groups=rte, upd_groups=upd, rt_group=rt_group, q_off=q_off,
+                     type_active_dev=None if active is None or ext is not None else small[T + max(P, 1):],
+                     type_dst_dev=None if ext is None else small[T + max(P, 1):], proj_groups=proj, rte_groups=rte, upd_groups=upd, rt_group=rt_group, q_off=q_off,
                      kv_off=kv_off, proj_elems=proj_elems, q_groups=q_groups, kv_groups=kv_groups)
     plan._layer_tables[key] = lt
     return lt
