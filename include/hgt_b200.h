@@ -184,7 +184,8 @@ int hgt_gather_rows(const float* in, const int32_t* perm, int64_t n_rows, int32_
  * feature buffer (NVLink peer mappings, e.g. torch symmetric memory `buffer_ptrs_dev`); `row_base` is added to every
  * src_row (double-buffered publish areas inside one symmetric allocation).  The caller orders the ranks: publish ->
  * barrier -> pull; with two publish areas used alternately that ONE barrier per exchange also guarantees that nobody
- * still reads the area about to be overwritten.  width % 4 == 0. */
+ * still reads the area about to be overwritten.  Any width: rows of a multiple of 4 floats into a 16-byte aligned `out`
+ * move as float4 (the peer buffers are then assumed 16-byte aligned, as allocations are), other rows float by float. */
 int hgt_halo_pull(uint64_t peer_ptrs_dev, const int32_t* src_rank, const int32_t* src_row, int64_t n_rows,
                   int32_t width, int64_t row_base, float* out, void* stream);
 /* Same pull fused with the operand conversion of the projection GEMM: every row is written as the bf16 hi/lo split

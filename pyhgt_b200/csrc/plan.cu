@@ -457,6 +457,23 @@ __global__ void k_halo_pull(const float* const* __restrict__ peers, const int32_
     }
   }
 }
+// Same pull one float per lane, for rows that are not 16-byte aligned (width % 4 != 0 or an unaligned output).
+__global__ void k_halo_pull_scalar(const float* const* __restrict__ peers, const int32_t* __restrict__ src_rank,
+                                   const int32_t* __restrict__ src_row, int64_t n_rows, int width, int64_t row_base,
+                                   float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t r = warp; r < n_rows; r += n_warps) {
+    const float* src = peers[src_rank[r]] + (row_base + src_row[r]) * width;
+    float* dst = out + r * width;
+    for (int c = lane; c < width; c += 32) {
+      float v;
+      asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(src + c));
+      dst[c] = v;
+    }
+  }
+}
 
 // Pull + convert: the halo rows are only ever consumed as the bf16 hi/lo operand split of the projection GEMM, so the
 // conversion is done while the row crosses NVLink; fp32 is kept only for the rows this rank owns (skip connection).
@@ -937,15 +954,19 @@ extern "C" int hgt_gather_rows(const float* in, const int32_t* perm, int64_t n_r
 extern "C" int hgt_halo_pull(uint64_t peer_ptrs_dev, const int32_t* src_rank, const int32_t* src_row, int64_t n_rows,
                              int32_t width, int64_t row_base, float* out, void* stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
-  HGT_REQUIRE(width % 4 == 0, "hgt_halo_pull: row width %d must be a multiple of 4 floats", width);
   if (n_rows == 0) return 0;
   const int warps_per_block = 8;
   int64_t blocks = (n_rows + warps_per_block - 1) / warps_per_block;
   int64_t cap = (int64_t)hgt_sm_count() * 16;
   if (blocks > cap) blocks = cap;
-  k_halo_pull<<<(unsigned)blocks, warps_per_block * 32, 0, st>>>(reinterpret_cast<const float* const*>(peer_ptrs_dev),
-                                                                 src_rank, src_row, n_rows, width / 4, row_base,
-                                                                 reinterpret_cast<float4*>(out));
+  auto pf = reinterpret_cast<const float* const*>(peer_ptrs_dev);
+  // the peer buffers' own alignment cannot be read here: they are allocations (symmetric memory), 16-byte aligned
+  if (width % 4 == 0 && (uintptr_t)out % 16 == 0)
+    k_halo_pull<<<(unsigned)blocks, warps_per_block * 32, 0, st>>>(pf, src_rank, src_row, n_rows, width / 4, row_base,
+                                                                   reinterpret_cast<float4*>(out));
+  else
+    k_halo_pull_scalar<<<(unsigned)blocks, warps_per_block * 32, 0, st>>>(pf, src_rank, src_row, n_rows, width,
+                                                                          row_base, out);
   HGT_LAUNCH_CHECK();
   return 0;
 }

@@ -419,8 +419,9 @@ class ShardedGraph:
         `graph` = (node_type, edge_index, edge_type, edge_time) device tensors holding this rank's LOCAL graph, for
         callers that stream the shard from the host every step (the plan is rebuilt when they change)."""
         from .conv import HGTConv
+        split = x_own.is_cuda and conv.linear_impl in (0, 2)
         with HGTConv._stage("halo_exchange"):
-            x_local, x_split = self.exchange(x_own, split=x_own.is_cuda and conv.linear_impl in (0, 2))
+            x_local, x_split = self.exchange(x_own, split=True) if split else (self.exchange(x_own), None)
         l_nt, l_ei, l_et, l_tm = (self.node_type, self.edge_index, self.edge_type, self.edge_time) if graph is None else graph
         if x_local.is_cuda:
             # the update epilogue writes each owned row straight to its position in owned_global order

@@ -405,7 +405,9 @@ def test_typed_linear_tensor_core_group_edges_and_presplit_match_fp64(K, width, 
 @pytest.mark.parametrize("world", [2, 3])
 def test_sharded_local_forward_matches_full_graph(world):
     """The kernels on one rank's shard (owned + halo rows, Q/update restricted to owned rows) reproduce the
-    full-graph result on the owned rows.  The halo exchange itself is covered by tests/test_sharded_cpu.py."""
+    full-graph result on the owned rows.  x_local is built directly, so no halo exchange runs here: the NCCL / gloo
+    exchange is covered by tests/test_sharded_cpu.py, the peer-memory kernels and ShardedGraph.forward's p2p and push
+    paths by tests/test_gpu_halo.py."""
     import pyhgt_b200
     from pyhgt_b200 import sharded
     dev = _dev()

@@ -1,6 +1,7 @@
 """Host-side logic of the multi-GPU path (pyhgt_b200/sharded.py) on CPU with the gloo backend, world_size 2:
 partition + halo all-to-all must hand every rank exactly the rows it needs, so that the ORACLE run on the local
-shard reproduces the full-graph oracle on the owned rows.  (The CUDA kernels are exercised by the -m gpu tests.)"""
+shard reproduces the full-graph oracle on the owned rows.  (The CUDA halo kernels and the p2p / push exchange of
+ShardedGraph, emulated on one GPU, are tested in tests/test_gpu_halo.py.)"""
 import os
 import socket
 
