@@ -543,7 +543,8 @@ typedef struct {
   const float* const* wk; const float* const* bk;
   const float* const* wv; const float* const* bv;
   const float* const* wa; const float* const* ba;
-  const float* const* norm_w; const float* const* norm_b;   /* NULL when !use_norm */
+  const float* const* norm_w; const float* const* norm_b;   /* NULL when !use_norm; the vectors may sit at any float
+                                                               alignment (e.g. views into one flat parameter buffer) */
   const float* relation_att; const float* relation_msg; const float* relation_pri; const float* skip;
   const float* emb_weight; const float* emb_lin_w; const float* emb_lin_b;   /* NULL when !use_rte */
   /* data */

@@ -183,13 +183,25 @@ k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, 
   }
   for (int s = 16; s > 0; s >>= 1) var += __shfl_xor_sync(0xffffffffu, var, s);
   const float rstd = rsqrtf(var / d + 1e-5f);
-  const float4* w = reinterpret_cast<const float4*>(norm_wp ? norm_wp[t] : norm_w + (int64_t)t * d);
-  const float4* b = reinterpret_cast<const float4*>(norm_bp ? norm_bp[t] : norm_b + (int64_t)t * d);
+  const float* wf = norm_wp ? norm_wp[t] : norm_w + (int64_t)t * d;
+  const float* bf = norm_bp ? norm_bp[t] : norm_b + (int64_t)t * d;
+  // pointer-table entries are separate parameters, possibly views at any float offset into one flat buffer
+  // (vector_to_parameters, FSDP): they take scalar loads unless both are 16-byte aligned (warp-uniform)
+  const bool wb_vec = ((reinterpret_cast<uintptr_t>(wf) | reinterpret_cast<uintptr_t>(bf)) & 15) == 0;
+  const float4* w = reinterpret_cast<const float4*>(wf);
+  const float4* b = reinterpret_cast<const float4*>(bf);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int c = lane + 32 * i;
     if (c < nvec) {
-      const float4 wv = __ldg(w + c), bv = __ldg(b + c);
+      float4 wv, bv;
+      if (wb_vec) {
+        wv = __ldg(w + c);
+        bv = __ldg(b + c);
+      } else {
+        wv = make_float4(__ldg(wf + 4 * c), __ldg(wf + 4 * c + 1), __ldg(wf + 4 * c + 2), __ldg(wf + 4 * c + 3));
+        bv = make_float4(__ldg(bf + 4 * c), __ldg(bf + 4 * c + 1), __ldg(bf + 4 * c + 2), __ldg(bf + 4 * c + 3));
+      }
       float4 r;
       r.x = (y[i].x - mean) * rstd * wv.x + bv.x;
       r.y = (y[i].y - mean) * rstd * wv.y + bv.y;
@@ -227,7 +239,8 @@ int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type
   HGT_REQUIRE((norm_w == nullptr) == (norm_b == nullptr) && (norm_wp == nullptr) == (norm_bp == nullptr),
               "hgt_update_epilogue: LayerNorm weight and bias must go together");
   if (n_nodes == 0) return 0;
-  // with pointer tables the per-type vectors are separate nn.LayerNorm parameters: torch allocations, 16-byte aligned
+  // pointer-table LayerNorm vectors (norm_wp / norm_bp) may sit at any float offset: the vector kernel tests them
+  // row by row and loads misaligned ones as scalars, so only the [T,d] arrays norm_w / norm_b are checked here
   const bool aligned = (d % 4 == 0) && ((reinterpret_cast<uintptr_t>(o) | reinterpret_cast<uintptr_t>(x) |
                                         reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(norm_w) |
                                         reinterpret_cast<uintptr_t>(norm_b) |

@@ -1,6 +1,7 @@
 """GPU tests of the native backward kernels (run on an H100: ``pytest -m gpu``): hgt_typed_linear_bwd (wgmma dX /
-dW with MN-major operands, and the fp32 SIMT path), hgt_update_backward, hgt_fold_backward — each against float64 torch
-autograd of the same expression — and the absence of library GEMMs on the training path."""
+dW with MN-major operands, and the fp32 SIMT path) and hgt_update_backward, each against float64 torch autograd of the
+same expression, and the absence of library GEMMs on the training path.  hgt_fold_backward and every instance of the
+update backward are tested in test_gpu_small_stage_instances.py."""
 import ctypes
 
 import pytest
