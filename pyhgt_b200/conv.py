@@ -440,13 +440,9 @@ class HGTConv(nn.Module):
         kv_tab[plan.kv_rows * 2 * d:].zero_()
         with self._stage("proj_linear"):
             if bf16:
-                # Q by its own fp32 call, the K'/V' blocks straight into the bf16 table; the tensor-core path splits A once
+                # Q by its own fp32 call, the K'/V' blocks straight into the bf16 table; the tensor-core GEMM splits
+                # fp32 x as it loads it, unless the previous layer left x split
                 xs = x_split if plan.sorted_types else None
-                if xs is None and impl != 1 and d_in % 16 == 0 and d_in >= 64 and d % 16 == 0:
-                    xs = (torch.empty((N, d_in), dtype=torch.bfloat16, device=dev),
-                          None if one else torch.empty((N, d_in), dtype=torch.bfloat16, device=dev))
-                    _lib.call("hgt_act_split", x_sorted.data_ptr(), d_in, N, d_in, 0, None, xs[0].data_ptr(),
-                              _lib.ptr(xs[1]), st)
                 for tab, dst in ((lt.q_groups, q_tab), (lt.kv_groups, kv_tab)):
                     if xs is None:
                         self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, dst, impl, st)

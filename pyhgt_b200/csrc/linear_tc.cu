@@ -18,6 +18,14 @@
 // One-product mode (P = 1: impl 3, or a presplit call with a_lo == NULL): the operands are rounded to bf16 (the hi half
 // of the split, bitwise) and one bf16 product per k-step is accumulated, torch's "medium" float32 matmul precision.  Its
 // stages hold {A_hi, W_hi} only; tiles, epilogues, barriers and tile order are those of P = 3.
+//
+// A operand: at BN = 128 / 256, hgt_typed_linear[_bf16] loads fp32 A with TMA (boxes of 32 floats x 128 rows,
+// SWIZZLE_128B) and each consumer warpgroup splits its rows in shared memory, in place, into the bf16 halves its wgmma
+// reads (tcp::split_a_slab): the same bits k_split_bf16 would write, so the result equals the presplit entry points' on
+// hgt_act_split's halves, bitwise.  A k-block's fp32 A takes as many bytes as {A_hi, A_lo} did (twice A_hi's at P = 1),
+// and there is no separate pass over A and no A halves in the workspace.  k_split_bf16 still splits A first for 64-column
+// tiles (splits_a_first) and for an A that TMA cannot load as fp32 (base not 16-byte aligned, or lda % 4 != 0).  W is
+// split once per call by k_split_bf16.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -85,7 +93,8 @@ __device__ __forceinline__ void store4(__nv_bfloat16* p, float4 v, bool aligned)
 // ---- the GEMM: out_cb[m, n] = A[a_row0 + m, :] . W[w_row0 + cb * cb_width + n, :] (+ bias) ------------------------------
 // Rows of a tile past the group and columns past the column block are computed on neighbouring (or zero-filled) operand
 // rows and not stored.
-template <class OutT>
+// AF: a_hi is the fp32 A map (box {32, 128 rows}, one or two per k-block) and a_lo repeats it.
+template <class OutT, bool AF = false>
 struct FwdJob {
   CUtensorMap a_hi, a_lo, w_hi, w_lo;      // A box {fwd_bk, 128 rows}, W box {fwd_bk, tile_n rows}
   const float* bias;
@@ -134,14 +143,17 @@ struct FwdJob {
   }
   template <int BN, int KB, int P>
   __device__ void load(const Tile& t, int kb, uint32_t sa, uint32_t bar) const {
-    constexpr uint32_t A = a_bytes<KB>(), B = b_offset<KB, P>();
+    constexpr uint32_t A = a_bytes<KB>(), B = b_offset<KB, P, AF>();
     const int k = kb * KB;
-    tma_load_2d(sa, &a_hi, k, t.a_row, bar);
-    tma_load_2d(sa + B, &w_hi, k, t.w_row, bar);
-    if constexpr (P == 3) {
-      tma_load_2d(sa + A, &a_lo, k, t.a_row, bar);
-      tma_load_2d(sa + B + BN * KB * 2, &w_lo, k, t.w_row, bar);
+    if constexpr (AF) {
+#pragma unroll
+      for (int j = 0; j < KB / 32; ++j) tma_load_2d(sa + j * A32_BOX, &a_hi, k + 32 * j, t.a_row, bar);
+    } else {
+      tma_load_2d(sa, &a_hi, k, t.a_row, bar);
+      if constexpr (P == 3) tma_load_2d(sa + A, &a_lo, k, t.a_row, bar);
     }
+    tma_load_2d(sa + B, &w_hi, k, t.w_row, bar);
+    if constexpr (P == 3) tma_load_2d(sa + B + BN * KB * 2, &w_lo, k, t.w_row, bar);
   }
   // BN = 128 / 256: asynchronous TMA tensor stores (tcp::store_tma) where the destination rows are 16-byte aligned, so
   // the stores overlap the next tile's products.  Otherwise, and at BN = 64, through shared memory with whole row segments
@@ -174,9 +186,10 @@ struct FwdJob {
   }
 };
 
-template <int BN, class OutT, int P = 3, int KB = fwd_bk<BN>()>
-__global__ void __launch_bounds__(TILE_THREADS, 1) k_typed_linear_tc(const __grid_constant__ FwdJob<OutT> job, int n_tiles) {
-  split3_tile<BN, false, KB, fwd_out_stage<BN>(), P>(job, n_tiles);
+template <int BN, class OutT, int P = 3, int KB = fwd_bk<BN>(), bool AF = false>
+__global__ void __launch_bounds__(TILE_THREADS, 1)
+    k_typed_linear_tc(const __grid_constant__ FwdJob<OutT, AF> job, int n_tiles) {
+  split3_tile<BN, false, KB, fwd_out_stage<BN>(), P, AF>(job, n_tiles);
 }
 
 // ---- output tensor maps of the tensor-store epilogue ----------------------------------------------------------------
@@ -242,6 +255,28 @@ int make_map(CUtensorMap* m, const void* base, int64_t rows, int Kp, int box_row
   return 0;
 }
 
+// fp32 A as the GEMM loads it (AF): K columns at row stride lda, boxes of 32 floats (128 bytes, SWIZZLE_128B) x 128 rows.
+// TMA zero-fills columns k >= K and rows past `rows`, as the split's padding to Kp did.  Needs A 16-byte aligned and
+// lda % 4 == 0 (a_fp32_loadable).
+int make_map_f32(CUtensorMap* m, const float* base, int64_t rows, int K, int64_t lda) {
+  EncodeTiledFn fn = get_encode_fn();
+  HGT_REQUIRE(fn != nullptr, "hgt_typed_linear: cuTensorMapEncodeTiled not available from the driver");
+  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)lda * 4};
+  cuuint32_t box[2] = {32, (cuuint32_t)BM};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  HGT_REQUIRE(r == CUDA_SUCCESS, "hgt_typed_linear: cuTensorMapEncodeTiled (fp32 A) failed (%d) rows=%lld K=%d lda=%lld",
+              (int)r, (long long)rows, K, (long long)lda);
+  return 0;
+}
+
+bool a_fp32_loadable(const float* A, int64_t lda) {
+  return A && (reinterpret_cast<uintptr_t>(A) & 15) == 0 && lda % 4 == 0;
+}
+
 // Template of the output maps: `cb_width` columns of OutT, boxes of 128 bytes x 64 rows with SWIZZLE_128B (the layout
 // tcp::store_tma stages).  `dummy` (16-byte aligned) and the row count / stride are placeholders that k_out_maps replaces.
 template <class OutT>
@@ -277,17 +312,31 @@ void extents(const hgt_lin_group* h_groups, int n_groups, int cb_width, int64_t*
   }
 }
 
-// The tensor maps and the k-block count follow the kernel's k-block KB.  At P = 1 the lo maps repeat the hi ones (the
-// kernel does not load them; they stay valid for its prefetches).
-template <int BN, class OutT, int P = 3, int KB = fwd_bk<BN>()>
-int launch_fwd(FwdJob<OutT>& job, const __nv_bfloat16* const ops[4], int64_t a_rows, int64_t w_rows, int Kp, int tiles,
-               cudaStream_t st) {
+// Operands of one launch: A as fp32 (a32, lda; AF) or as bf16 halves (a_hi, a_lo), W as bf16 halves.  Halves are K-major
+// at row stride Kp; a lo pointer is NULL at P = 1.
+struct FwdOps {
+  const float* a32;
+  int64_t lda;
+  const __nv_bfloat16 *a_hi, *a_lo, *w_hi, *w_lo;
+  int64_t a_rows, w_rows;
+  int K, Kp;
+};
+
+// The tensor maps and the k-block count follow the kernel's k-block KB.  At P = 1 (and for A under AF) the lo maps repeat
+// the hi ones (the kernel does not load them; they stay valid for its prefetches).
+template <int BN, class OutT, int P = 3, int KB = fwd_bk<BN>(), bool AF = false>
+int launch_fwd(FwdJob<OutT, AF>& job, const FwdOps& ops, int tiles, cudaStream_t st) {
   int rc;
-  if ((rc = make_map(&job.a_hi, ops[0], a_rows, Kp, BM, KB))) return rc;
-  if ((rc = make_map(&job.a_lo, ops[P == 3 ? 1 : 0], a_rows, Kp, BM, KB))) return rc;
-  if ((rc = make_map(&job.w_hi, ops[2], w_rows, Kp, BN, KB))) return rc;
-  if ((rc = make_map(&job.w_lo, ops[P == 3 ? 3 : 2], w_rows, Kp, BN, KB))) return rc;
-  job.k_blocks = (Kp + KB - 1) / KB;
+  if constexpr (AF) {
+    if ((rc = make_map_f32(&job.a_hi, ops.a32, ops.a_rows, ops.K, ops.lda))) return rc;
+    job.a_lo = job.a_hi;
+  } else {
+    if ((rc = make_map(&job.a_hi, ops.a_hi, ops.a_rows, ops.Kp, BM, KB))) return rc;
+    if ((rc = make_map(&job.a_lo, P == 3 ? ops.a_lo : ops.a_hi, ops.a_rows, ops.Kp, BM, KB))) return rc;
+  }
+  if ((rc = make_map(&job.w_hi, ops.w_hi, ops.w_rows, ops.Kp, BN, KB))) return rc;
+  if ((rc = make_map(&job.w_lo, P == 3 ? ops.w_lo : ops.w_hi, ops.w_rows, ops.Kp, BN, KB))) return rc;
+  job.k_blocks = (ops.Kp + KB - 1) / KB;
   if constexpr (fwd_tma_store<BN>()) {
     CUtensorMap tmpl;
     MapFirst first;
@@ -297,12 +346,70 @@ int launch_fwd(FwdJob<OutT>& job, const __nv_bfloat16* const ops[4], int64_t a_r
                                                   const_cast<CUtensorMap*>(job.out_maps));
     HGT_LAUNCH_CHECK();
   }
-  const size_t smem = tile_smem_bytes<BN, KB, fwd_out_stage<BN>(), P>();
-  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN, OutT, P, KB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem));
-  k_typed_linear_tc<BN, OutT, P, KB><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
+  const size_t smem = tile_smem_bytes<BN, KB, fwd_out_stage<BN>(), P, AF>();
+  HGT_CHECK_CUDA(cudaFuncSetAttribute(k_typed_linear_tc<BN, OutT, P, KB, AF>,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_typed_linear_tc<BN, OutT, P, KB, AF><<<persistent_grid(tiles), TILE_THREADS, smem, st>>>(job, tiles);
   HGT_LAUNCH_CHECK();
   return 0;
+}
+
+// Fills the job's tile tables and launches the instance for its tile width, product count and A operand.
+template <class OutT, bool AF>
+int run_fwd(const FwdOps& ops, const float* bias, int32_t cb_width, const hgt_lin_group* groups,
+            const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
+            CUtensorMap* out_maps, bool one, cudaStream_t st) {
+  FwdJob<OutT, AF> job;
+  job.tile_n = pick_tile_n(cb_width);
+  job.n_tiles_n = (cb_width + job.tile_n - 1) / job.tile_n;
+  int64_t total = 0, maps = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    job.map_first[g] = (int32_t)maps;
+    maps += h_groups[g].n_cblocks;
+    job.first_tile[g] = (int32_t)total;
+    total += (h_groups[g].m + BM - 1) / BM * h_groups[g].n_cblocks * job.n_tiles_n;
+    HGT_REQUIRE(total < 2147483647ll, "hgt_typed_linear(tc): too many tiles");
+  }
+  job.first_tile[n_groups] = (int32_t)total;
+  if (total == 0) return 0;
+  job.bias = bias;
+  job.groups = groups;
+  job.cblocks = cblocks;
+  job.out = out;
+  job.out_maps = out_maps;
+  job.n_groups = n_groups;
+  job.cb_width = cb_width;
+  const int tiles = (int)total;
+  // 64-column tiles read A split by k_split_bf16 (tc_run): only the presplit instances exist for them
+  if constexpr (AF) HGT_REQUIRE(job.tile_n != 64, "hgt_typed_linear(tc): no fp32-A kernel for 64-column tiles");
+  if (one) {
+    // k-block of the one-product kernel at BN = 128 / 256 (DESIGN.md §5.2): 32 (SWIZZLE_64B, as at P = 3) for fp32 A,
+    // whose 64-wide stages would leave a ring of two at BN = 256; 64 (SWIZZLE_128B) for presplit A.  HGT_TC_P1_KB=32 or
+    // 64 selects one for both, for A/B measurements.
+    static const int kb_env = [] {
+      const char* e = getenv("HGT_TC_P1_KB");
+      return !e ? 0 : (e[0] == '3' && e[1] == '2') ? 32 : (e[0] == '6' && e[1] == '4') ? 64 : 0;
+    }();
+    const bool kb32 = kb_env ? kb_env == 32 : AF;
+    switch (job.tile_n) {
+      case 64:
+        if constexpr (!AF) return launch_fwd<64, OutT, 1, 64>(job, ops, tiles, st);
+        return 1;
+      case 128:
+        return kb32 ? launch_fwd<128, OutT, 1, 32, AF>(job, ops, tiles, st)
+                    : launch_fwd<128, OutT, 1, 64, AF>(job, ops, tiles, st);
+      default:
+        return kb32 ? launch_fwd<256, OutT, 1, 32, AF>(job, ops, tiles, st)
+                    : launch_fwd<256, OutT, 1, 64, AF>(job, ops, tiles, st);
+    }
+  }
+  switch (job.tile_n) {
+    case 64:
+      if constexpr (!AF) return launch_fwd<64, OutT, 3, fwd_bk<64>()>(job, ops, tiles, st);
+      return 1;
+    case 128: return launch_fwd<128, OutT, 3, fwd_bk<128>(), AF>(job, ops, tiles, st);
+    default: return launch_fwd<256, OutT, 3, fwd_bk<256>(), AF>(job, ops, tiles, st);
+  }
 }
 
 }  // namespace
@@ -312,14 +419,21 @@ bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width) {
   return cb_width % 16 == 0 && cb_width > 0 && K >= BK;
 }
 
-// P = 1 needs no lo halves.
+// 64-column tiles read A split by k_split_bf16: each 128-row block of A is read by every column tile of its group (seven
+// at d = 400), and splitting it once up front is cheaper than splitting it in every tile (DESIGN.md §4).
+static bool splits_a_first(int32_t cb_width) { return pick_tile_n(cb_width) == 64; }
+
+// W's halves (P = 1 needs no lo), A's halves for 64-column tiles, and the output maps.  At 128 / 256 columns A needs
+// none: the GEMM splits fp32 A itself.  An fp32 A that TMA cannot load splits into stream-ordered memory of its own
+// (tc_run).  The presplit entry points take the P = 3 size.
 size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width,
                                      int32_t products) {
   int64_t a_rows, w_rows;
   extents(h_groups, n_groups, cb_width, &a_rows, &w_rows);
   const int Kp = (K + 7) / 8 * 8;
   const size_t halves = products == 1 ? 1 : 2;
-  return 5 * 256 + halves * hgt_align_up((size_t)a_rows * Kp * 2, 256) + halves * hgt_align_up((size_t)w_rows * Kp * 2, 256) +
+  const size_t a = splits_a_first(cb_width) ? halves * hgt_align_up((size_t)a_rows * Kp * 2, 256) : 0;
+  return 4 * 256 + a + halves * hgt_align_up((size_t)w_rows * Kp * 2, 256) +
          hgt_align_up((size_t)n_out_maps(h_groups, n_groups) * sizeof(CUtensorMap), 256);
 }
 
@@ -402,70 +516,60 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
               cb_width);
   HGT_REQUIRE(products == 3 || products == 1, "hgt_typed_linear(tc): products=%d", products);
   const bool one = products == 1;
-  const int Kp = (K + 7) / 8 * 8;
-  int64_t a_rows, w_rows;
-  extents(h_groups, n_groups, cb_width, &a_rows, &w_rows);
+  FwdOps ops;
+  ops.K = K;
+  ops.Kp = (K + 7) / 8 * 8;
+  extents(h_groups, n_groups, cb_width, &ops.a_rows, &ops.w_rows);
   size_t need = hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width, products);
   HGT_REQUIRE(workspace && workspace_bytes >= need, "hgt_typed_linear(tc): workspace too small (%zu < %zu)",
               workspace_bytes, need);
-  const size_t a_half = hgt_align_up((size_t)a_rows * Kp * 2, 256), w_half = hgt_align_up((size_t)w_rows * Kp * 2, 256);
+  const size_t w_half = hgt_align_up((size_t)ops.w_rows * ops.Kp * 2, 256);
+  const size_t a_half = hgt_align_up((size_t)ops.a_rows * ops.Kp * 2, 256);
   char* p = reinterpret_cast<char*>(hgt_align_up(reinterpret_cast<size_t>(workspace), 256));
-  __nv_bfloat16* a_hi = reinterpret_cast<__nv_bfloat16*>(p); p += a_half;
-  __nv_bfloat16* a_lo = one ? nullptr : reinterpret_cast<__nv_bfloat16*>(p); p += one ? 0 : a_half;
+  __nv_bfloat16* a_ws = nullptr;                              // A's halves in the workspace (64-column tiles)
+  if (splits_a_first(cb_width)) a_ws = reinterpret_cast<__nv_bfloat16*>(p), p += (one ? 1 : 2) * a_half;
   __nv_bfloat16* w_hi = reinterpret_cast<__nv_bfloat16*>(p); p += w_half;
   __nv_bfloat16* w_lo = one ? nullptr : reinterpret_cast<__nv_bfloat16*>(p); p += one ? 0 : w_half;
   CUtensorMap* out_maps = reinterpret_cast<CUtensorMap*>(p);
-  {
-    int64_t n = a_rows * (Kp / 4);
-    if (a_hi_in) {
-      a_hi = const_cast<__nv_bfloat16*>(a_hi_in);            // split by the producer (e.g. the edge kernel)
-      a_lo = one ? nullptr : const_cast<__nv_bfloat16*>(a_lo_in);
-    } else if (n > 0) {
-      k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, a_rows, K, Kp, a_hi, a_lo);
-      HGT_LAUNCH_CHECK();
-    }
-    n = w_rows * (Kp / 4);
-    if (n > 0) k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, K, w_rows, K, Kp, w_hi, w_lo);
+  ops.w_hi = w_hi;
+  ops.w_lo = w_lo;
+  int64_t n = ops.w_rows * (ops.Kp / 4);
+  if (n > 0) k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, K, ops.w_rows, K, ops.Kp, w_hi, w_lo);
+  HGT_LAUNCH_CHECK();
+  ops.a32 = A;
+  ops.lda = lda;
+  ops.a_hi = a_hi_in;                                         // split by the producer (e.g. the edge kernel)
+  ops.a_lo = one ? nullptr : a_lo_in;
+  if (a_hi_in)
+    return run_fwd<OutT, false>(ops, bias, cb_width, groups, h_groups, n_groups, cblocks, out, out_maps, one, st);
+  n = ops.a_rows * (ops.Kp / 4);
+  if (a_ws) {
+    if (n == 0) return 0;
+    ops.a_hi = a_ws;
+    ops.a_lo = one ? nullptr : a_ws + a_half / 2;
+    k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, ops.a_rows, K, ops.Kp, a_ws,
+                                                              const_cast<__nv_bfloat16*>(ops.a_lo));
     HGT_LAUNCH_CHECK();
+    return run_fwd<OutT, false>(ops, bias, cb_width, groups, h_groups, n_groups, cblocks, out, out_maps, one, st);
   }
-  FwdJob<OutT> job;
-  job.tile_n = pick_tile_n(cb_width);
-  job.n_tiles_n = (cb_width + job.tile_n - 1) / job.tile_n;
-  int64_t total = 0, maps = 0;
-  for (int g = 0; g < n_groups; ++g) {
-    job.map_first[g] = (int32_t)maps;
-    maps += h_groups[g].n_cblocks;
-    job.first_tile[g] = (int32_t)total;
-    total += (h_groups[g].m + BM - 1) / BM * h_groups[g].n_cblocks * job.n_tiles_n;
-    HGT_REQUIRE(total < 2147483647ll, "hgt_typed_linear(tc): too many tiles");
-  }
-  job.first_tile[n_groups] = (int32_t)total;
-  if (total == 0) return 0;
-  job.bias = bias;
-  job.groups = groups;
-  job.cblocks = cblocks;
-  job.out = out;
-  job.out_maps = out_maps;
-  job.n_groups = n_groups;
-  job.cb_width = cb_width;
-  const __nv_bfloat16* const ops[4] = {a_hi, a_lo, w_hi, w_lo};
-  if (one) {
-    // k-block of the one-product kernel at BN = 128 / 256 (DESIGN.md §5.2): HGT_TC_P1_KB=32 selects the SWIZZLE_64B
-    // variant of the P = 3 kernel, for A/B measurements
-    static const bool kb32 = [] { const char* e = getenv("HGT_TC_P1_KB"); return e && e[0] == '3' && e[1] == '2'; }();
-    switch (job.tile_n) {
-      case 64: return launch_fwd<64, OutT, 1, 64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
-      case 128:
-        return kb32 ? launch_fwd<128, OutT, 1, 32>(job, ops, a_rows, w_rows, Kp, (int)total, st)
-                    : launch_fwd<128, OutT, 1, 64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
-      default:
-        return kb32 ? launch_fwd<256, OutT, 1, 32>(job, ops, a_rows, w_rows, Kp, (int)total, st)
-                    : launch_fwd<256, OutT, 1, 64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
-    }
-  }
-  switch (job.tile_n) {
-    case 64: return launch_fwd<64>(job, ops, a_rows, w_rows, Kp, (int)total, st);
-    case 128: return launch_fwd<128>(job, ops, a_rows, w_rows, Kp, (int)total, st);
-    default: return launch_fwd<256>(job, ops, a_rows, w_rows, Kp, (int)total, st);
-  }
+  if (a_fp32_loadable(A, lda))                                // the GEMM splits A as it loads it
+    return run_fwd<OutT, true>(ops, bias, cb_width, groups, h_groups, n_groups, cblocks, out, out_maps, one, st);
+  // An fp32 A that TMA cannot load (base not 16-byte aligned, or lda % 4 != 0) is split first, into stream-ordered
+  // memory of its own, so that the workspace need not hold halves of A for every caller.
+  if (n == 0) return 0;
+  void* halves = nullptr;
+  HGT_CHECK_CUDA(cudaMallocAsync(&halves, (one ? 1 : 2) * a_half, st));
+  const int rc = [&]() -> int {
+    __nv_bfloat16* a_hi = static_cast<__nv_bfloat16*>(halves);
+    __nv_bfloat16* a_lo = one ? nullptr : a_hi + a_half / 2;
+    k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, ops.a_rows, K, ops.Kp, a_hi, a_lo);
+    HGT_LAUNCH_CHECK();
+    ops.a_hi = a_hi;
+    ops.a_lo = a_lo;
+    return run_fwd<OutT, false>(ops, bias, cb_width, groups, h_groups, n_groups, cblocks, out, out_maps, one, st);
+  }();
+  const cudaError_t freed = cudaFreeAsync(halves, st);
+  if (rc) return rc;
+  HGT_CHECK_CUDA(freed);
+  return 0;
 }

@@ -14,6 +14,8 @@
 //                 {A_hi, B_hi} (P = 1); the ring runs on
 //                 across tiles, so the next tile's first stages load while the consumers finish and store this one
 //   warpgroups 1-2  consumers: rows [64 c, 64 c + 64) of the tile, wgmma m64nBNk16 from shared memory
+// AF = true (the forward's fp32 A): a stage holds A as fp32 in place of its halves, and each consumer splits its rows
+// into hi / lo in shared memory (split_a_slab) before the k-block's products.
 // Operand tiles are TMA boxes with SWIZZLE_128B, 64 bf16 (128 bytes) along the inner dimension (KB = 64), or with
 // SWIZZLE_64B, 32 bf16 (KB = 32: half the stage, twice the ring depth).  MN = false: both operands K-major (inner dimension =
 // reduction); MN = true: both MN-major (inner dimension = output row / column, the reduction runs over the box rows; KB = 64
@@ -65,15 +67,15 @@ __device__ __forceinline__ void prefetch_map(const CUtensorMap* map) {
 
 // sm_90 shared-memory matrix descriptor, SWIZZLE_128B (KB = 64, layout type 1 at bits 62-63) or SWIZZLE_64B (KB = 32,
 // layout type 2).  Tiles start 1024-byte aligned (base offset 0).  K-major: rows of 2 * KB bytes, 8-row swizzle atoms
-// SBO = 16 * KB bytes apart, LBO unused.  MN-major (KB = 64): 64 MN-elements per 128-byte row, one row per k; groups of 8
-// k-rows SBO = 1024 bytes apart, 64-element MN atoms LBO apart.
+// SBO bytes apart (16 * KB when packed), LBO unused.  MN-major (KB = 64): 64 MN-elements per 128-byte row, one row per k;
+// groups of 8 k-rows SBO = 1024 bytes apart, 64-element MN atoms LBO apart.
 template <int KB>
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes = 16 * KB) {
   static_assert(KB == 64 || KB == 32, "k-block of 64 (SWIZZLE_128B) or 32 (SWIZZLE_64B) bf16");
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((16 * KB) >> 4) << 32;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
   d |= (uint64_t)(KB == 64 ? 1 : 2) << 62;
   return d;
 }
@@ -138,32 +140,44 @@ constexpr uint32_t TMA_BUF_BYTES = 64 * 64 * 4;
 constexpr uint32_t TMA_STAGE_BYTES = 2 * 2 * TMA_BUF_BYTES;
 
 // Stage layout for a k-block of KB bf16: {A_hi, A_lo, B_hi, B_lo} at P = 3, {A_hi, B_hi} at P = 1; a consumer's 64-row A
-// slab is one atom, B_lo follows B_hi.  The ring takes what the epilogue staging (OUT bytes) and the barriers leave, up
-// to SMEM_BUDGET.
+// slab is one atom, B_lo follows B_hi.  AF (fp32 A): the A part is the k-block of A as fp32, KB / 32 boxes of 128 rows x
+// 32 floats (A32_BOX bytes each), which the consumers split in place (split_a_slab); at P = 3 that is the size of
+// {A_hi, A_lo}, at P = 1 twice that of A_hi.  The ring takes what the epilogue staging (OUT bytes) and the barriers leave,
+// up to SMEM_BUDGET.
+constexpr uint32_t A32_BOX = BM * 32 * 4;         // one fp32 A box: 128 rows x 128 bytes, 16 KB
 template <int KB> constexpr uint32_t a_bytes() { return BM * KB * 2; }
 template <int KB> constexpr uint32_t atom_bytes() { return 64 * KB * 2; }
-template <int KB, int P> constexpr uint32_t b_offset() { return (P == 3 ? 2u : 1u) * a_bytes<KB>(); }   // B_hi in a stage
-template <int BN, int KB = BK, int P = 3> constexpr uint32_t stage_bytes() {
+template <int KB, int P, bool AF = false> constexpr uint32_t b_offset() {                 // B_hi in a stage
+  return AF ? 2u * a_bytes<KB>() : (P == 3 ? 2u : 1u) * a_bytes<KB>();
+}
+template <int BN, int KB = BK, int P = 3, bool AF = false> constexpr uint32_t stage_bytes() {
   static_assert(P == 3 || P == 1, "three bf16 products (split) or one");
-  return (P == 3 ? 2u : 1u) * (a_bytes<KB>() + (uint32_t)BN * KB * 2);
+  return b_offset<KB, P, AF>() + (P == 3 ? 2u : 1u) * (uint32_t)BN * KB * 2;
 }
-template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES, int P = 3> constexpr int n_stages() {
+template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES, int P = 3, bool AF = false> constexpr int n_stages() {
   constexpr uint32_t left = SMEM_LIMIT - 1024 - OUT - 256;
-  return (int)((left < SMEM_BUDGET ? left : SMEM_BUDGET) / stage_bytes<BN, KB, P>());
+  return (int)((left < SMEM_BUDGET ? left : SMEM_BUDGET) / stage_bytes<BN, KB, P, AF>());
 }
-template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES, int P = 3> constexpr size_t tile_smem_bytes() {
-  return 1024 + (size_t)n_stages<BN, KB, OUT, P>() * stage_bytes<BN, KB, P>() + OUT +
-         2 * n_stages<BN, KB, OUT, P>() * sizeof(uint64_t);
+template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES, int P = 3, bool AF = false>
+constexpr size_t tile_smem_bytes() {
+  return 1024 + (size_t)n_stages<BN, KB, OUT, P, AF>() * stage_bytes<BN, KB, P, AF>() + OUT +
+         2 * n_stages<BN, KB, OUT, P, AF>() * sizeof(uint64_t);
 }
-static_assert(tile_smem_bytes<256, 32, TMA_STAGE_BYTES>() <= SMEM_LIMIT && tile_smem_bytes<256>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<128, 32, TMA_STAGE_BYTES>() <= SMEM_LIMIT && tile_smem_bytes<64>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<256, 32, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<256, 64, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<128, 32, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<128, 64, TMA_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
+// Every forward (AF and presplit) and backward instance.
+template <bool AF> constexpr bool fwd_fits() {
+  return tile_smem_bytes<256, 32, TMA_STAGE_BYTES, 3, AF>() <= SMEM_LIMIT &&
+         tile_smem_bytes<128, 32, TMA_STAGE_BYTES, 3, AF>() <= SMEM_LIMIT &&
+         tile_smem_bytes<64, 64, OUT_STAGE_BYTES, 3, AF>() <= SMEM_LIMIT &&
+         tile_smem_bytes<256, 32, TMA_STAGE_BYTES, 1, AF>() <= SMEM_LIMIT &&
+         tile_smem_bytes<256, 64, TMA_STAGE_BYTES, 1, AF>() <= SMEM_LIMIT &&
+         tile_smem_bytes<128, 32, TMA_STAGE_BYTES, 1, AF>() <= SMEM_LIMIT &&
+         tile_smem_bytes<128, 64, TMA_STAGE_BYTES, 1, AF>() <= SMEM_LIMIT &&
+         tile_smem_bytes<64, 64, OUT_STAGE_BYTES, 1, AF>() <= SMEM_LIMIT &&
+         n_stages<256, 64, TMA_STAGE_BYTES, 1, AF>() >= 2 && n_stages<64, 64, OUT_STAGE_BYTES, 3, AF>() >= 2;
+}
+static_assert(fwd_fits<false>() && fwd_fits<true>() && tile_smem_bytes<256>() <= SMEM_LIMIT &&
                   tile_smem_bytes<256, 64, OUT_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<128, 64, OUT_STAGE_BYTES, 1>() <= SMEM_LIMIT &&
-                  tile_smem_bytes<64, 64, OUT_STAGE_BYTES, 1>() <= SMEM_LIMIT,
+                  tile_smem_bytes<128, 64, OUT_STAGE_BYTES, 1>() <= SMEM_LIMIT,
               "ring + epilogue staging must fit the 227 KB a block may use");
 
 // Output tile width: 64, 128 or 256 columns, the one that pads `width` least (ties go to the wider tile).  Columns past
@@ -184,9 +198,9 @@ inline unsigned persistent_grid(int tiles) {
   return (unsigned)(tiles < sms ? tiles : sms);
 }
 
-// The P products of one k-block.  a_hi / a_lo: this warpgroup's 64-row A slab; b_hi / b_lo: the BN-column B tile (the lo
-// halves are not read at P = 1).
-template <int BN, bool MN, int KB, int P = 3>
+// The P products of one k-block.  a_hi / a_lo: this warpgroup's 64-row A slab, 8-row groups A_SBO bytes apart; b_hi /
+// b_lo: the BN-column B tile (the lo halves are not read at P = 1).
+template <int BN, bool MN, int KB, int P = 3, uint32_t A_SBO = 16 * KB>
 __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
   static_assert(!MN || KB == 64, "MN-major operands use 64-row k-blocks");
   constexpr uint32_t kstep = MN ? 16 * 128 : 32;       // 16 k: 16 rows of 128 bytes, or 32 bytes inside the swizzle row
@@ -196,7 +210,7 @@ __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_hi, uint32_t a
 #pragma unroll
   for (int k = 0; k < KB / 16; ++k) {
     const uint32_t o = (uint32_t)k * kstep;
-    const uint64_t ah = make_desc<KB>(a_hi + o, lbo), al = make_desc<KB>(a_lo + o, lbo);
+    const uint64_t ah = make_desc<KB>(a_hi + o, lbo, A_SBO), al = make_desc<KB>(a_lo + o, lbo, A_SBO);
     const uint64_t bh = make_desc<KB>(b_hi + o, lbo), bl = make_desc<KB>(b_lo + o, lbo);
     if constexpr (BN == 64) {
       wgmma_n64<T, T>(acc, ah, bh);
@@ -220,6 +234,62 @@ __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_hi, uint32_t a
       }
     }
   }
+}
+
+__device__ __forceinline__ float4 lds128(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts64(uint32_t a, __nv_bfloat162 x, __nv_bfloat162 y) {
+  asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(a), "r"(*reinterpret_cast<uint32_t*>(&x)),
+               "r"(*reinterpret_cast<uint32_t*>(&y)) : "memory");
+}
+
+// AF: one consumer warpgroup splits its 64-row slab of a stage's fp32 A in place into the bf16 halves mma_kblock reads,
+// x = hi + lo with hi = rn(x), lo = rn(x - hi), bitwise what k_split_bf16 writes.  `slab` is the slab in box 0 (box j,
+// k 32 j .. 32 j + 31, lies A32_BOX * j further; 128-byte rows, 16-byte chunk q of row r at q ^ (r & 7), as TMA's
+// SWIZZLE_128B writes it).  The halves are K-major:
+//   KB = 32 (SWIZZLE_64B)  A_hi's 8-row groups 1024 bytes apart at the slab, A_lo 512 bytes after each group of A_hi;
+//   KB = 64 (SWIZZLE_128B) A_hi packed at the slab, A_lo packed at the slab of box 1.
+// Either way rows 16 w .. 16 w + 15 go where warp w read them from, so a warp only waits for itself between its loads and
+// its stores.  A load takes four rows whose 64-bit stores are free of bank conflicts in each half-warp: rows {0, 1, 2, 3}
+// + 4 i at KB = 32, {0, 4, 1, 5} (+ 2, + 8) at KB = 64.  The caller fences the stores to the async proxy and syncs the
+// warpgroup before the products.
+template <int KB>
+__device__ __forceinline__ int split_row(int i, int lr) {
+  return KB == 32 ? 4 * i + lr : 8 * (i >> 1) + 2 * (i & 1) + 4 * (lr & 1) + (lr >> 1);
+}
+template <int KB, int P>
+__device__ __forceinline__ void split_a_slab(uint32_t slab, int wq, int lane) {
+  constexpr int NB = KB / 32;
+  const int lr = lane >> 3, q = lane & 7;
+  float4 v[NB][4];
+#pragma unroll
+  for (int j = 0; j < NB; ++j)
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      v[j][i] = lds128(slab + j * A32_BOX + (16 * wq + split_row<KB>(i, lr)) * 128 + 16 * q);
+  __syncwarp();
+#pragma unroll
+  for (int j = 0; j < NB; ++j)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = 16 * wq + split_row<KB>(i, lr), x = r & 7;
+      const int L = q ^ x;                                      // columns 32 j + 4 L .. + 3 of the k-block
+      // two elements per conversion (cvt.rn.bf16x2.f32): the same round-to-nearest-even as __float2bfloat16_rn
+      const float4 f = v[j][i];
+      const __nv_bfloat162 h01 = __floats2bfloat162_rn(f.x, f.y), h23 = __floats2bfloat162_rn(f.z, f.w);
+      const uint32_t half = (uint32_t)(L & 1) << 3;
+      const uint32_t off = KB == 32 ? (r >> 3) * 1024 + x * 64 + ((((L >> 1) ^ (x >> 1)) << 4) | half)
+                                    : (r >> 3) * 1024 + x * 128 + ((((4 * j + (L >> 1)) ^ x) << 4) | half);
+      sts64(slab + off, h01, h23);
+      if constexpr (P == 3) {
+        const __nv_bfloat162 l01 = __floats2bfloat162_rn(f.x - __low2float(h01), f.y - __high2float(h01));
+        const __nv_bfloat162 l23 = __floats2bfloat162_rn(f.z - __low2float(h23), f.w - __high2float(h23));
+        sts64(slab + off + (KB == 32 ? 512 : A32_BOX), l01, l23);
+      }
+    }
 }
 
 // Accumulator fragment of wgmma m64nN (f32): acc[4 j + 2 h + e] is row 16 * warp + lane / 4 + 8 h of the warpgroup's 64
@@ -338,12 +408,18 @@ __device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage
 // memory; `job` is the kernel's __grid_constant__ parameter (it holds the tensor maps), `n_tiles` the number of tiles
 // job.decode() accepts.  Every tile's k-blocks run in ascending order into a freshly zeroed accumulator, so a tile's
 // result does not depend on the grid size or on which CTA computes it.  job.store gets consumer c's half of the OUT bytes
-// of epilogue staging.  job.load<BN, KB, P>() fills one stage in the layout of stage_bytes<BN, KB, P>().
-template <int BN, bool MN, int KB, uint32_t OUT = OUT_STAGE_BYTES, int P = 3, class Job>
+// of epilogue staging.  job.load<BN, KB, P>() fills one stage in the layout of stage_bytes<BN, KB, P, AF>().  AF: the stage
+// holds A as fp32 (K-major only), and each consumer splits its slab of it (split_a_slab) before the k-block's products.
+template <int BN, bool MN, int KB, uint32_t OUT = OUT_STAGE_BYTES, int P = 3, bool AF = false, class Job>
 __device__ __forceinline__ void split3_tile(const Job& job, int n_tiles) {
-  constexpr int S = n_stages<BN, KB, OUT, P>();
-  constexpr uint32_t STAGE = stage_bytes<BN, KB, P>();
-  constexpr uint32_t A = a_bytes<KB>(), ATOM = atom_bytes<KB>(), B = b_offset<KB, P>();
+  static_assert(!AF || !MN, "fp32 A is loaded K-major");
+  constexpr int S = n_stages<BN, KB, OUT, P, AF>();
+  constexpr uint32_t STAGE = stage_bytes<BN, KB, P, AF>();
+  constexpr uint32_t ATOM = atom_bytes<KB>(), B = b_offset<KB, P, AF>();
+  // A_lo of consumer 0 relative to its A_hi, and the stride of A's 8-row groups (split_a_slab's layout under AF)
+  constexpr uint32_t A = AF ? (KB == 32 ? 512u : A32_BOX) : a_bytes<KB>();
+  constexpr uint32_t A_SBO = AF ? 1024u : 16u * KB;
+  constexpr uint32_t SLAB = AF ? 64u * 128u : ATOM;               // consumer c's A slab starts c * SLAB into the stage
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (s_u32(smem_dyn) & 1023u)) & 1023u);
   unsigned char* out_stage = smem + (size_t)S * STAGE;
@@ -393,8 +469,13 @@ __device__ __forceinline__ void split3_tile(const Job& job, int n_tiles) {
       for (int it = 0; it < iters; ++it) {
         mbar_wait(s_u32(&full_bar[s]), phase);
         const uint32_t sa = base + (uint32_t)s * STAGE;
+        if constexpr (AF) {
+          split_a_slab<KB, P>(sa + c * SLAB, warp & 3, lane);
+          fence_proxy_async_smem();                               // the halves are visible to wgmma
+          bar_sync_named(1 + c, 128);
+        }
         wgmma_fence();
-        mma_kblock<BN, MN, KB, P>(acc, sa + c * ATOM, sa + A + c * ATOM, sa + B, sa + B + (uint32_t)BN * KB * 2);
+        mma_kblock<BN, MN, KB, P, A_SBO>(acc, sa + c * SLAB, sa + A + c * SLAB, sa + B, sa + B + (uint32_t)BN * KB * 2);
         wgmma_commit();
         if (it > 0) {                                             // the previous k-block's products have retired
           wgmma_wait<1>();

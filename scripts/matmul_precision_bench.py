@@ -6,8 +6,8 @@ bf16 product), alternating in one process.  Prints one JSON line per round, work
   c4 training step (3 layers, forward + backward): median ms per step and max_memory_allocated;
   gemm: the typed GEMM alone at the C2 projection shape (K = 256; groups of 736,389 / 1,134,649 / 8,740 / 59,965 rows;
       five 256-wide column blocks), fp32 and bf16 output: P = 3 (impl 2) and P = 1 (impl 3).  The one-product kernel's
-      k-block at 128 / 256 columns is 64 unless HGT_TC_P1_KB=32; the script measures that variant in a child process
-      (--gemm-only), since the switch is read once per process.
+      k-block at 128 / 256 columns is 32 for fp32 A unless HGT_TC_P1_KB=64; the script measures that variant in a child
+      process (--gemm-only), since the switch is read once per process.
 The card name, power limit and SM clock are read in the same run.  Writes nothing.
 
     python scripts/matmul_precision_bench.py [--steps 10] [--warmup 3] [--rounds 2] [--scale 1.0]
@@ -165,7 +165,7 @@ def gemm_lines(steps, warmup, rnd, dev, card, variant):
     flops = 2.0 * a0 * ncb * width * K
     for dtype in (torch.float32, torch.bfloat16):
         out = torch.empty(out0, dtype=dtype, device=dev)
-        for impl in ((3,) if variant == "kb32" else (2, 3)):
+        for impl in ((3,) if variant == "kb64" else (2, 3)):
             wsb = ctypes.c_size_t()
             _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, K, width, impl, ctypes.byref(wsb))
             ws = torch.empty(wsb.value, dtype=torch.uint8, device=dev)
@@ -175,7 +175,7 @@ def gemm_lines(steps, warmup, rnd, dev, card, variant):
                                                   out.data_ptr(), impl, ws.data_ptr(), ws.numel(), st), steps, warmup)
             print(json.dumps(dict(card, round=rnd, config="gemm_c2_projection", out_dtype=str(dtype).split(".")[1],
                                   products=1 if impl == 3 else 3,
-                                  p1_kblock=(32 if variant == "kb32" else 64) if impl == 3 else None,
+                                  p1_kblock=(64 if variant == "kb64" else 32) if impl == 3 else None,
                                   workspace_gb=round(wsb.value / 1e9, 2), ms=med, min_ms=lo, max_ms=hi,
                                   tflops_per_product=round(flops / (med / 1e3) / 1e12, 1),
                                   out_gb=round(out.numel() * out.element_size() / 1e9, 2))), flush=True)
@@ -190,19 +190,19 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--scale", type=float, default=1.0)
     ap.add_argument("--configs", default="gemm,c2,c3,c5,c4")
-    ap.add_argument("--gemm-only", action="store_true", help="only the GEMM lines (used for the HGT_TC_P1_KB=32 child)")
+    ap.add_argument("--gemm-only", action="store_true", help="only the GEMM lines (used for the HGT_TC_P1_KB=64 child)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("matmul_precision_bench.py measures on a CUDA device; none is available")
     dev = torch.device("cuda:0")
     card = _card(dev)
-    variant = "kb32" if os.environ.get("HGT_TC_P1_KB") == "32" else "kb64"
+    variant = "kb64" if os.environ.get("HGT_TC_P1_KB") == "64" else "kb32"
     for rnd in range(args.rounds):
         for config in (["gemm"] if args.gemm_only else args.configs.split(",")):
             if config == "gemm":
                 gemm_lines(args.steps, args.warmup, rnd, dev, card, variant)
                 if not args.gemm_only:
-                    env = dict(os.environ, HGT_TC_P1_KB="32")
+                    env = dict(os.environ, HGT_TC_P1_KB="64")
                     subprocess.run([sys.executable, os.path.abspath(__file__), "--gemm-only", "--rounds", "1",
                                     "--steps", str(args.steps), "--warmup", str(args.warmup)], env=env, check=True)
             elif config == "c4":
