@@ -114,6 +114,11 @@ int hgt_plan_tiles(const int32_t* row_ptr, int64_t n_nodes, int64_t n_edges,
 int hgt_plan_source_index(const int32_t* key, const int32_t* other, const int32_t* row_ptr, int64_t n_nodes,
                           int64_t n_edges, int32_t n_rows, int32_t* src_ptr, int32_t* src_dst, int32_t* src_oth,
                           void* workspace, size_t workspace_bytes, void* stream);
+/* The same index, and src_pos [E]: the CSR position of every entry, in index order, from the same sort (the row pass of
+ * the att gradient, hgt_edge_backward_rows_att, reads datt there). */
+int hgt_plan_source_index_pos(const int32_t* key, const int32_t* other, const int32_t* row_ptr, int64_t n_nodes,
+                              int64_t n_edges, int32_t n_rows, int32_t* src_ptr, int32_t* src_dst, int32_t* src_oth,
+                              int32_t* src_pos, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Trimmed forward (GNN.forward(..., out_nodes=)): layer l of L only needs the nodes within L-l hops of an output node.
@@ -386,6 +391,61 @@ int hgt_edge_backward_rows_bf16(const float* q, const float* dagg, const float* 
                                 int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs, int32_t d,
                                 int32_t n_heads, float* grad, void* workspace, size_t workspace_bytes,
                                 const int32_t* d_tile_counts, void* stream);
+
+/* Backward with a gradient of att as well (a loss term reads the softmax weights att_out of hgt_edge_forward).  With
+ * datt [E,H] in ORIGINAL edge order and p = att:  C_i = sum_{e->i} p_e datt_e,  ds_e = p_e ((dp_e + datt_e) - (D_i + C_i));
+ * dq, d[K'|V'] and dkvr follow from ds as in the calls above.  datt = 0 gives bitwise their results.
+ * hgt_edge_att_grad_prep: writes c_att [N,H] (rows of destinations the tiles cover) and datt_csr [E,H] = datt permuted to
+ *   CSR order (datt_csr[c] = datt[csr_eid[c]]).  att is the forward's att_out.  tiles / n_split / hubs / n_hubs /
+ *   d_tile_counts: the edge tiles, as for hgt_edge_forward.  No float atomics (hub pieces summed in piece order), so one
+ *   call serves the atomic and the deterministic backward.  workspace: hgt_edge_att_grad_workspace_bytes(n_split, H).
+ * hgt_edge_backward_att / _dst_att / _rows_att (+ _bf16): the calls above with datt_csr and c_att (rows pass: datt_csr
+ *   and src_pos [E], the CSR position of every entry of the source-major index, in index order, from
+ *   hgt_plan_source_index_pos).  The destination pass stores D_i + C_i
+ *   into D, which the row pass reads unchanged.  Workspaces as above. */
+int hgt_edge_att_grad_workspace_bytes(int32_t n_split, int32_t n_heads, size_t* out_bytes);
+int hgt_edge_att_grad_prep(const float* att, const float* datt, const int32_t* csr_eid, const int32_t* row_ptr,
+                           const int32_t* tiles, int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
+                           int64_t n_nodes, int32_t n_heads, float* c_att, float* datt_csr, void* workspace,
+                           size_t workspace_bytes, const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_att(const float* q, const float* kv, const float* kvr, const float* agg, const float* dagg,
+                          const float* stats, const float* datt_csr, const float* c_att, const int32_t* row_ptr,
+                          const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                          int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total, int64_t kvr_rows_total,
+                          float* dq, float* dkv, float* dkvr, void* workspace, size_t workspace_bytes,
+                          const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_dst_att(const float* q, const float* kv, const float* kvr, const float* agg, const float* dagg,
+                              const float* stats, const float* datt_csr, const float* c_att, const int32_t* row_ptr,
+                              const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                              int32_t n_split, const int32_t* hubs, int32_t n_hubs, int64_t n_nodes, int32_t d,
+                              int32_t n_heads, float* dq, float* D, void* workspace, size_t workspace_bytes,
+                              const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_rows_att(const float* q, const float* dagg, const float* stats, const float* D,
+                               const float* datt_csr, const float* own, const float* oth, const int32_t* src_ptr,
+                               const int32_t* src_dst, const int32_t* src_oth, const int32_t* src_pos, int32_t n_rows,
+                               int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
+                               const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads, float* grad,
+                               void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_att_bf16(const float* q, const void* kv, const void* kvr, const float* agg, const float* dagg,
+                               const float* stats, const float* datt_csr, const float* c_att, const int32_t* row_ptr,
+                               const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                               int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total,
+                               int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr, void* workspace,
+                               size_t workspace_bytes, const int32_t* d_tile_counts, void* stream);
+int hgt_edge_backward_dst_att_bf16(const float* q, const void* kv, const void* kvr, const float* agg, const float* dagg,
+                                   const float* stats, const float* datt_csr, const float* c_att,
+                                   const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                                   const int32_t* tiles, int32_t n_tiles, int32_t n_split, const int32_t* hubs,
+                                   int32_t n_hubs, int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D,
+                                   void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                                   void* stream);
+int hgt_edge_backward_rows_att_bf16(const float* q, const float* dagg, const float* stats, const float* D,
+                                    const float* datt_csr, const void* own, const void* oth, const int32_t* src_ptr,
+                                    const int32_t* src_dst, const int32_t* src_oth, const int32_t* src_pos,
+                                    int32_t n_rows, int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles,
+                                    int32_t n_split, const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads,
+                                    float* grad, void* workspace, size_t workspace_bytes,
+                                    const int32_t* d_tile_counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Backward of the typed linears (training path).  For the group / column-block tables of the forward call:

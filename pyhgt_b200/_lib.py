@@ -56,6 +56,7 @@ SIGNATURES = {
     "hgt_update_epilogue_dst": [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p],
     # deterministic training backward (torch.use_deterministic_algorithms)
     "hgt_plan_source_index": [_p, _p, _p, _i64, _i64, _i32, _p, _p, _p, _p, _sz, _p],
+    "hgt_plan_source_index_pos": [_p, _p, _p, _i64, _i64, _i32, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_edge_backward_det_workspace_bytes": [_i32, _i32, _i32, _c.POINTER(_sz)],
     "hgt_edge_backward_dst": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32, _i32, _p, _p, _p,
                               _sz, _p, _p],
@@ -80,6 +81,21 @@ SIGNATURES = {
                                    _p, _sz, _p, _p],
     "hgt_edge_backward_rows_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _p, _i32, _i32, _p, _i32, _i32, _i32,
                                     _p, _p, _sz, _p, _p],
+    # gradient of att (a loss term reads HGTConv.att): C / CSR-order datt, then the edge backward passes with datt
+    "hgt_edge_att_grad_workspace_bytes": [_i32, _i32, _c.POINTER(_sz)],
+    "hgt_edge_att_grad_prep": [_p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32, _p, _p, _p, _sz, _p, _p],
+    "hgt_edge_backward_att": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, _i64, _i64, _p, _p,
+                              _p, _p, _sz, _p, _p],
+    "hgt_edge_backward_dst_att": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32, _i32,
+                                  _p, _p, _p, _sz, _p, _p],
+    "hgt_edge_backward_rows_att": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _p, _i32, _i32, _p, _i32, _i32,
+                                   _i32, _p, _p, _sz, _p, _p],
+    "hgt_edge_backward_att_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, _i64, _i64, _p,
+                                   _p, _p, _p, _sz, _p, _p],
+    "hgt_edge_backward_dst_att_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32,
+                                       _i32, _p, _p, _p, _sz, _p, _p],
+    "hgt_edge_backward_rows_att_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _p, _i32, _i32, _p, _i32,
+                                        _i32, _i32, _p, _p, _sz, _p, _p],
     # HGSampling on the GPU (sampler.sample_subgraph_cuda)
     "hgt_gsample_add_budget_workspace_bytes": [_i64, _i32, _i64, _c.POINTER(_sz)],
     "hgt_gsample_add_budget": [_p, _p, _i32, _p, _p, _i64, _p, _i64, _i32, _i64, _i64, _c.c_uint64, _i64, _p, _p, _sz,

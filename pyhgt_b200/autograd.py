@@ -8,7 +8,9 @@ Every stage is a custom autograd.Function whose forward AND backward are hand-wr
                      / hgt_typed_linear_bwd                      split-bf16 forward, dX and dW; fp32 SIMT for odd shapes);
                                                                  the gelu in front of the a_linears (conv.py:119) lives in
                                                                  the operand split (forward) and the dX epilogue (backward)
-    _EdgeAttention   hgt_edge_forward / hgt_edge_backward        score -> softmax by destination -> weighted aggregation
+    _EdgeAttention   hgt_edge_forward / hgt_edge_backward        score -> softmax by destination -> weighted aggregation;
+                                                                 att is differentiable: a loss term on it takes the
+                                                                 hgt_edge_att_grad_prep + hgt_edge_backward*_att calls
     _UpdateEpilogue  hgt_update_epilogue / hgt_update_backward   sigmoid(skip) gate + LayerNorm (conv.py:129-133)
 
 No per-edge intermediates are kept: the edge backward recomputes the softmax weights from the saved per-destination
@@ -35,6 +37,7 @@ datatype for internal computations"); note that torch's own CUDA matmuls run TF3
 precise than torch's there.  "high" and "highest" keep the x3 scheme.  The stages record the setting on ctx.
 """
 import ctypes
+import weakref
 
 import numpy as np
 import torch
@@ -45,6 +48,29 @@ from . import plan as _plan
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
+
+
+# layers whose .att is still a node of the last training step's autograd graph (it keeps that graph alive)
+_ATT_GRAPH_LAYERS = weakref.WeakSet()
+
+
+def _set_att(m, att):
+    m.att = att
+    if att is not None and att.requires_grad:
+        _ATT_GRAPH_LAYERS.add(m)
+
+
+def release_att_graphs(params):
+    """Detach `.att` of the layers that own one of `params` and whose att still holds an autograd graph.  That graph
+    keeps the parameters' AccumulateGrad nodes alive, and the next step would reuse them on the stream they were made
+    on; graphed.py calls this for the parameters of the step it captures, before and after the capture.  Layers of
+    other models keep their att (and a loss term on it that has not run backward yet)."""
+    owned = {id(p) for p in params}
+    for m in list(_ATT_GRAPH_LAYERS):
+        if any(id(p) in owned for p in m.parameters()):
+            if m.att is not None:
+                m.att = m.att.detach()
+            _ATT_GRAPH_LAYERS.discard(m)
 
 
 def bf16_tables():
@@ -218,17 +244,20 @@ class _EdgeAttention(torch.autograd.Function):
         ctx.plan, ctx.lt, ctx.d, ctx.n_heads, ctx.has_kvr = plan, lt, d, n_heads, kvr is not None
         ctx.det = torch.are_deterministic_algorithms_enabled()
         ctx.proj_elems = proj.numel()
-        ctx.save_for_backward(q, kv, kvr, agg, stats)
-        if att is not None:
-            ctx.mark_non_differentiable(att)
+        # att is differentiable (conv.py:108 makes it a node of the graph): a loss term on it arrives as datt.  Without
+        # materialised grads an unused att gives datt None, and the backward runs exactly the calls without it.
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(q, kv, kvr, agg, stats, att)
         return agg, att
 
     @staticmethod
-    def backward(ctx, dagg, _datt=None):
-        q, kv, kvr, agg, stats = ctx.saved_tensors
+    def backward(ctx, dagg, datt=None):
+        q, kv, kvr, agg, stats, att = ctx.saved_tensors
         plan, lt, d, H = ctx.plan, ctx.lt, ctx.d, ctx.n_heads
         N = plan.n_nodes
         f32 = dict(dtype=torch.float32, device=q.device)
+        if dagg is None:                                               # the loss reads att only
+            dagg = torch.zeros((N, d), **f32)
         dproj = torch.empty(ctx.proj_elems, **f32)                     # hgt_edge_backward zero-initialises dq / dkv
         if lt.kv_off > N * d:
             dproj[N * d:lt.kv_off].zero_()                             # alignment gap
@@ -237,12 +266,16 @@ class _EdgeAttention(torch.autograd.Function):
         dkvr = torch.empty(kvr.numel(), **f32) if kvr is not None else None
         dagg = dagg.contiguous()
         sfx = "_bf16" if ctx.bf16 else ""
+        att_grad = _att_grad_prep(att, datt, plan, H) if datt is not None else None
         if ctx.det:
-            _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx)
+            _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx, att_grad)
             return dproj, dkvr, None, None, None, None, None, None, None
         ws = torch.empty(256, dtype=torch.uint8, device=q.device)
-        _lib.call("hgt_edge_backward" + sfx, q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
-                  stats.data_ptr(), plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
+        fn, extra = "hgt_edge_backward", ()
+        if att_grad is not None:
+            fn, extra = "hgt_edge_backward_att", (att_grad[0].data_ptr(), att_grad[1].data_ptr())
+        _lib.call(fn + sfx, q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
+                  stats.data_ptr(), *extra, plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
                   None if kvr is None else plan.rte_row.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, N, d, H,
                   plan.kv_rows + 1, 0 if kvr is None else kvr.numel() // (2 * d),
                   dq.data_ptr(), dkv.data_ptr(), _lib.ptr(dkvr), ws.data_ptr(), ws.numel(),
@@ -250,20 +283,41 @@ class _EdgeAttention(torch.autograd.Function):
         return dproj, dkvr, None, None, None, None, None, None, None
 
 
-def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx=""):
+def _att_grad_prep(att, datt, plan, H):
+    """(datt in CSR order [E, H], C [N, H]) for the *_att backward calls: hgt_edge_att_grad_prep."""
+    dev = att.device
+    datt = datt.contiguous()
+    datt_csr = torch.empty((max(plan.n_edges, 1), H), dtype=torch.float32, device=dev)
+    c_att = torch.empty((plan.n_nodes, H), dtype=torch.float32, device=dev)
+    wsb = ctypes.c_size_t()
+    _lib.call("hgt_edge_att_grad_workspace_bytes", plan.n_split, H, ctypes.byref(wsb))
+    ws = torch.empty(wsb.value, dtype=torch.uint8, device=dev)
+    _lib.call("hgt_edge_att_grad_prep", att.data_ptr(), datt.data_ptr(), plan.csr_eid.data_ptr(), plan.row_ptr.data_ptr(),
+              plan.tiles.data_ptr(), plan.n_tiles, plan.n_split, plan.hubs.data_ptr(), plan.n_hubs, plan.n_nodes, H,
+              c_att.data_ptr(), datt_csr.data_ptr(), ws.data_ptr(), ws.numel(), _lib.ptr(plan.tile_counts_dev), _stream())
+    return datt_csr, c_att
+
+
+def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx="", att_grad=None):
     """Deterministic edge backward: destination pass (dq, D), then one row pass over the [K'|V'] rows and, with RTE, one
-    over the RTE rows; each gradient row is written once by its owner.  sfx "_bf16": bf16 kv / kvr tables."""
+    over the RTE rows; each gradient row is written once by its owner.  sfx "_bf16": bf16 kv / kvr tables.  att_grad:
+    None, or (datt_csr, C) from _att_grad_prep: the *_att passes, the row passes reading datt at the CSR positions the
+    source-major indices carry (plan.source_index(..., with_pos=True))."""
     N = plan.n_nodes
     st = _stream()
-    kvi = _plan.source_index(plan, "kv")
-    rti = _plan.source_index(plan, "rte") if kvr is not None else None
+    with_pos = att_grad is not None
+    kvi = _plan.source_index(plan, "kv", with_pos)
+    rti = _plan.source_index(plan, "rte", with_pos) if kvr is not None else None
     D = torch.empty((N, H), dtype=torch.float32, device=q.device)
     wsb = ctypes.c_size_t()
     _lib.call("hgt_edge_backward_det_workspace_bytes", plan.n_split, max(kvi.n_split, rti.n_split if rti else 0), d,
               ctypes.byref(wsb))
     ws = torch.empty(wsb.value, dtype=torch.uint8, device=q.device)
-    _lib.call("hgt_edge_backward_dst" + sfx, q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(), dagg.data_ptr(),
-              stats.data_ptr(), plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
+    att_sfx, dst_extra = "", ()
+    if att_grad is not None:
+        att_sfx, dst_extra = "_att", (att_grad[0].data_ptr(), att_grad[1].data_ptr())
+    _lib.call("hgt_edge_backward_dst" + att_sfx + sfx, q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), agg.data_ptr(),
+              dagg.data_ptr(), stats.data_ptr(), *dst_extra, plan.row_ptr.data_ptr(), plan.kv_row.data_ptr(),
               None if kvr is None else plan.rte_row.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, plan.n_split,
               plan.hubs.data_ptr(), plan.n_hubs, N, d, H, dq.data_ptr(), D.data_ptr(), ws.data_ptr(), ws.numel(),
               _lib.ptr(plan.tile_counts_dev), st)
@@ -271,10 +325,18 @@ def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, 
     if kvr is not None:
         passes.append((kvr, kv, rti, kvr.numel() // (2 * d), dkvr))
     for own, oth, idx, own_rows, grad in passes:
-        _lib.call("hgt_edge_backward_rows" + sfx, q.data_ptr(), dagg.data_ptr(), stats.data_ptr(), D.data_ptr(), own.data_ptr(),
-                  _lib.ptr(oth), idx.ptr.data_ptr(), idx.dst.data_ptr(), None if oth is None else idx.oth.data_ptr(),
-                  idx.n_rows, own_rows, idx.tiles.data_ptr(), idx.n_tiles, idx.n_split, idx.hubs.data_ptr(), idx.n_hubs,
-                  d, H, grad.data_ptr(), ws.data_ptr(), ws.numel(), idx.counts_dev.data_ptr(), st)
+        src_oth = None if oth is None else idx.oth.data_ptr()
+        if att_grad is None:
+            _lib.call("hgt_edge_backward_rows" + sfx, q.data_ptr(), dagg.data_ptr(), stats.data_ptr(), D.data_ptr(),
+                      own.data_ptr(), _lib.ptr(oth), idx.ptr.data_ptr(), idx.dst.data_ptr(), src_oth,
+                      idx.n_rows, own_rows, idx.tiles.data_ptr(), idx.n_tiles, idx.n_split, idx.hubs.data_ptr(),
+                      idx.n_hubs, d, H, grad.data_ptr(), ws.data_ptr(), ws.numel(), idx.counts_dev.data_ptr(), st)
+        else:
+            _lib.call("hgt_edge_backward_rows_att" + sfx, q.data_ptr(), dagg.data_ptr(), stats.data_ptr(), D.data_ptr(),
+                      att_grad[0].data_ptr(), own.data_ptr(), _lib.ptr(oth), idx.ptr.data_ptr(), idx.dst.data_ptr(),
+                      src_oth, idx.pos.data_ptr(), idx.n_rows, own_rows, idx.tiles.data_ptr(), idx.n_tiles, idx.n_split,
+                      idx.hubs.data_ptr(), idx.n_hubs, d, H, grad.data_ptr(), ws.data_ptr(), ws.numel(),
+                      idx.counts_dev.data_ptr(), st)
 
 
 class _FoldWeights(torch.autograd.Function):
@@ -431,7 +493,7 @@ def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, 
 
     # 2. fused edge kernel
     agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, want_att, m.edge_variant, tables16)
-    m.att = att
+    _set_att(m, att)
 
     # 3. a_linears on gelu(agg) (conv.py:119,125): the gelu is applied inside the operand split / the dX epilogue
     wa_cat = torch.cat([l.weight for l in m.a_linears], 0)
@@ -470,7 +532,7 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
     impl = gemm_impl(m.linear_impl, bf16_matmuls())
     proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables(), impl)
     agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant, tables16)
-    m.att = att
+    _set_att(m, att)
 
     drop = m.training and m.drop.p > 0
     wa_cat = torch.cat([l.weight for l in m.a_linears], 0)

@@ -156,10 +156,13 @@ class HGTConv(nn.Module):
     def __getstate__(self):
         """Launch caches (ctypes argument blocks, device pointer tables, pinned plans) are per-process state: they are
         dropped from the pickled / deep-copied module so `torch.save(model)` (OAG/train_paper_field.py:279) works after
-        a forward; they are rebuilt lazily."""
+        a forward; they are rebuilt lazily.  After a training forward `att` is a non-leaf tensor of the autograd graph,
+        which deepcopy refuses: the copy keeps its values, detached."""
         state = self.__dict__.copy()
         state.pop("_args_cache", None)
         state["_ptr_tables"] = {}
+        if state.get("att") is not None:
+            state["att"] = state["att"].detach()
         return state
 
     # ------------------------------------------------------------------------------------------

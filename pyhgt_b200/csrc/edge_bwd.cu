@@ -21,6 +21,13 @@
 //
 // hgt_edge_backward*_bf16: the same passes on bf16 [K'|V'] / RTE tables (KV = __nv_bfloat16), widened to fp32 in registers;
 // every gradient stays fp32 in the layouts above.
+//
+// Gradient of att as well (ATT = true, the *_att entry points): with an incoming datt_e (the loss reads att itself)
+//                 C_i = sum_e p_e datt_e       ds_e = p_e * ((dp_e + datt_e) - (D_i + C_i))
+// and dq / dk / dv as above.  hgt_edge_att_grad_prep computes C [N, H] and datt permuted to CSR order (one warp per
+// destination tile, hub pieces merged in piece order: no float atomics, so it serves both backward modes); the passes
+// read datt at the edge's CSR position (the row pass through a per-entry position beside its source-major index) and
+// add C_i to D_i once per destination.  With datt = 0 the grouping gives bitwise the ds of the ATT = false passes.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -49,8 +56,10 @@ struct BwdParams {
   float* dkv;                // [rows+1, 2d] zero-initialised
   float* dkvr;               // [P*240+1, 2d] zero-initialised or nullptr
   int32_t* tile_counter;
-  float* D;                  // deterministic destination pass: [N, H] D_i per head
+  float* D;                  // deterministic destination pass: [N, H] D_i per head (+ C_i with ATT)
   float* partial;            // deterministic destination pass: [n_split, d] partial dq of hub pieces
+  const float* datt_csr;     // ATT: [E, H] gradient of att in CSR order
+  const float* c_att;        // ATT: [N, H] C_i = sum_e p_e datt_e
 };
 
 template <int VEC>
@@ -107,8 +116,8 @@ __device__ __forceinline__ void st_vec(float* p, const float (&v)[VEC]) {
 }
 
 // DET = false: hgt_edge_backward (dk / dv scattered with reductions).  DET = true: destination pass of the
-// deterministic backward (no scatter; D_i saved; hub pieces write partial dq rows).
-template <class KV, int VEC, int NCH, bool DET>
+// deterministic backward (no scatter; D_i saved; hub pieces write partial dq rows).  ATT: datt_e and C_i enter ds.
+template <class KV, int VEC, int NCH, bool DET, bool ATT>
 __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
   const KV* const kvt = static_cast<const KV*>(p.kv);
   const KV* const kvrt = static_cast<const KV*>(p.kvr);
@@ -157,7 +166,8 @@ __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
 #pragma unroll
           for (int v = 0; v < VEC; ++v) dq[t][v] = 0.f;
         }
-        const float D = head_sum(dpart, lph);
+        const float D = ATT ? head_sum(dpart, lph) + (head_ok ? p.c_att[(int64_t)dst * p.H + h] : 0.f)
+                            : head_sum(dpart, lph);
         if constexpr (DET) {
           if (head_ok && sub == 0 && seg_begin == p.row_ptr[dst]) p.D[(int64_t)dst * p.H + h] = D;
         }
@@ -194,7 +204,13 @@ __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
           const float s = head_sum(spart, lph);
           const float dp = head_sum(dppart, lph);
           const float pe = __expf(s - m) * inv_l;
-          const float ds = pe * (dp - D);
+          float ds;
+          if constexpr (ATT) {
+            const float dat = head_ok ? p.datt_csr[(int64_t)c * p.H + h] : 0.f;
+            ds = pe * ((dp + dat) - D);
+          } else {
+            ds = pe * (dp - D);
+          }
           if constexpr (DET) {
 #pragma unroll
             for (int t = 0; t < NCH; ++t)
@@ -248,16 +264,16 @@ __device__ __forceinline__ void edge_bwd_dst(const BwdParams& p) {
   }
 }
 
-template <class KV, int VEC, int NCH>
+template <class KV, int VEC, int NCH, bool ATT>
 __global__ void __launch_bounds__(kWarps * 32)
 k_edge_bwd(BwdParams p) {
-  edge_bwd_dst<KV, VEC, NCH, false>(p);
+  edge_bwd_dst<KV, VEC, NCH, false, ATT>(p);
 }
 
-template <class KV, int VEC, int NCH>
+template <class KV, int VEC, int NCH, bool ATT>
 __global__ void __launch_bounds__(kWarps * 32)
 k_edge_bwd_dst(BwdParams p) {
-  edge_bwd_dst<KV, VEC, NCH, true>(p);
+  edge_bwd_dst<KV, VEC, NCH, true, ATT>(p);
 }
 
 // ---- deterministic row pass --------------------------------------------------------------------------------------------
@@ -278,9 +294,12 @@ struct RowParams {
   float* grad;               // [rows, 2d] gradient of the owned table
   float* partial;            // [n_split, 2d] partial rows of split row pieces
   int32_t* tile_counter;
+  const float* datt_csr;     // ATT: [E, H] gradient of att in CSR order
+  const int32_t* e_pos;      // ATT: per index entry: its CSR position
 };
 
-template <class KV, int VEC, int NCH>
+// ATT: D holds D_i + C_i (destination pass) and datt_e is read at the entry's CSR position.
+template <class KV, int VEC, int NCH, bool ATT>
 __global__ void __launch_bounds__(kWarps * 32)
 k_edge_bwd_rows(RowParams p) {
   const KV* const own = static_cast<const KV*>(p.own);
@@ -364,7 +383,13 @@ k_edge_bwd_rows(RowParams p) {
           D = p.D[i * p.H + h];
         }
         const float pe = __expf(s - m) * inv_l;
-        const float ds = pe * (dp - D);
+        float ds;
+        if constexpr (ATT) {
+          const float dat = head_ok ? p.datt_csr[(int64_t)p.e_pos[j] * p.H + h] : 0.f;
+          ds = pe * ((dp + dat) - D);
+        } else {
+          ds = pe * (dp - D);
+        }
 #pragma unroll
         for (int t = 0; t < NCH; ++t)
 #pragma unroll
@@ -400,30 +425,69 @@ k_merge_piece_rows(const int32_t* __restrict__ hubs, const int32_t* __restrict__
   }
 }
 
-template <class KV, typename Params, int VEC>
+// C_i and datt in CSR order for the ATT passes.  One warp per destination tile (the edge tiles of the plan), static
+// tile order; HP = next_pow2(H) lanes cover the heads of one edge and 32 / HP edges are walked side by side, so each
+// edge's H weights are read and written as one contiguous run.  The lanes of a head are summed with a fixed butterfly;
+// hub pieces write partial C rows that k_merge_piece_rows adds in piece order.  No float atomics: deterministic.
+__global__ void __launch_bounds__(kWarps * 32)
+k_att_grad_prep(const float* __restrict__ att, const float* __restrict__ datt, const int32_t* __restrict__ csr_eid,
+                const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ tiles, int n_tiles_host,
+                const int32_t* __restrict__ d_counts, int H, int hp_shift, float* __restrict__ c_att,
+                float* __restrict__ datt_csr, float* __restrict__ partial) {
+  const int lane = threadIdx.x & 31;
+  const int HP = 1 << hp_shift;
+  const int h = lane & (HP - 1);
+  const int first = lane >> hp_shift;
+  const int step = 32 >> hp_shift;
+  const bool head_ok = h < H;
+  const int n_tiles = d_counts ? d_counts[0] : n_tiles_host;
+  for (int tile = blockIdx.x * kWarps + (threadIdx.x >> 5); tile < n_tiles; tile += gridDim.x * kWarps) {
+    const int4 tl = reinterpret_cast<const int4*>(tiles)[tile];
+    const bool split = tl.y < 0;
+    const int d_begin = tl.x, d_end = split ? tl.x + 1 : tl.y;
+    int seg_begin = tl.z;
+    for (int dst = d_begin; dst < d_end; ++dst) {
+      const int seg_end = split ? tl.w : row_ptr[dst + 1];
+      float acc = 0.f;
+      if (head_ok) {
+        for (int c = seg_begin + first; c < seg_end; c += step) {
+          const int64_t e = csr_eid[c];
+          const float g = datt[e * H + h];
+          datt_csr[(int64_t)c * H + h] = g;
+          acc = fmaf(att[e * H + h], g, acc);
+        }
+      }
+      for (int o = 16; o >= HP; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+      if (head_ok && first == 0) (split ? partial + (int64_t)(-tl.y - 1) * H : c_att + (int64_t)dst * H)[h] = acc;
+      seg_begin = seg_end;
+    }
+  }
+}
+
+template <class KV, typename Params, int VEC, bool ATT>
 int dispatch(const Params& p, int nch, int grid, cudaStream_t st, bool det) {
   if constexpr (std::is_same<Params, RowParams>::value) {
     switch (nch) {
-      case 1: k_edge_bwd_rows<KV, VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 2: k_edge_bwd_rows<KV, VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 4: k_edge_bwd_rows<KV, VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 8: k_edge_bwd_rows<KV, VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 1: k_edge_bwd_rows<KV, VEC, 1, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd_rows<KV, VEC, 2, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd_rows<KV, VEC, 4, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd_rows<KV, VEC, 8, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
       default: hgt_set_error("hgt_edge_backward_rows: unsupported chunk count %d", nch); return 1;
     }
   } else if (det) {
     switch (nch) {
-      case 1: k_edge_bwd_dst<KV, VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 2: k_edge_bwd_dst<KV, VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 4: k_edge_bwd_dst<KV, VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 8: k_edge_bwd_dst<KV, VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 1: k_edge_bwd_dst<KV, VEC, 1, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd_dst<KV, VEC, 2, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd_dst<KV, VEC, 4, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd_dst<KV, VEC, 8, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
       default: hgt_set_error("hgt_edge_backward_dst: unsupported chunk count %d", nch); return 1;
     }
   } else {
     switch (nch) {
-      case 1: k_edge_bwd<KV, VEC, 1><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 2: k_edge_bwd<KV, VEC, 2><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 4: k_edge_bwd<KV, VEC, 4><<<grid, kWarps * 32, 0, st>>>(p); break;
-      case 8: k_edge_bwd<KV, VEC, 8><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 1: k_edge_bwd<KV, VEC, 1, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 2: k_edge_bwd<KV, VEC, 2, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 4: k_edge_bwd<KV, VEC, 4, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
+      case 8: k_edge_bwd<KV, VEC, 8, ATT><<<grid, kWarps * 32, 0, st>>>(p); break;
       default: hgt_set_error("hgt_edge_backward: unsupported chunk count %d", nch); return 1;
     }
   }
@@ -455,15 +519,21 @@ int lane_map(int d, int n_heads, LaneMap& m, const char* who) {
   return 0;
 }
 
-template <class KV, typename Params>
+template <class KV, bool ATT, typename Params>
 int launch_pass(const Params& p, const LaneMap& lm, int n_tiles, cudaStream_t st, bool det) {
   HGT_CHECK_CUDA(cudaMemsetAsync(p.tile_counter, 0, sizeof(int32_t), st));
   int grid = hgt_sm_count() * 4;
   int max_ctas = (n_tiles + kWarps - 1) / kWarps;
   if (grid > max_ctas) grid = max_ctas;
-  if (lm.vec == 4) return dispatch<KV, Params, 4>(p, lm.nch, grid, st, det);
-  if (lm.vec == 2) return dispatch<KV, Params, 2>(p, lm.nch, grid, st, det);
-  return dispatch<KV, Params, 1>(p, lm.nch, grid, st, det);
+  if (lm.vec == 4) return dispatch<KV, Params, 4, ATT>(p, lm.nch, grid, st, det);
+  if (lm.vec == 2) return dispatch<KV, Params, 2, ATT>(p, lm.nch, grid, st, det);
+  return dispatch<KV, Params, 1, ATT>(p, lm.nch, grid, st, det);
+}
+
+// The passes' ATT = false instances when datt_csr is NULL (the calls without an att gradient), ATT = true otherwise.
+template <class KV, typename Params>
+int launch_pass_att(const Params& p, const LaneMap& lm, int n_tiles, cudaStream_t st, bool det) {
+  return p.datt_csr ? launch_pass<KV, true>(p, lm, n_tiles, st, det) : launch_pass<KV, false>(p, lm, n_tiles, st, det);
 }
 
 int merge_pieces(const int32_t* hubs, int32_t n_hubs, const int32_t* d_counts, const float* partial, int width,
@@ -477,14 +547,15 @@ int merge_pieces(const int32_t* hubs, int32_t n_hubs, const int32_t* d_counts, c
 
 template <class KV>
 int edge_backward(const float* q, const KV* kv, const KV* kvr, const float* agg, const float* dagg, const float* stats,
-                  const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles,
-                  int32_t n_tiles, int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total,
-                  int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr, void* workspace, size_t workspace_bytes,
-                  const int32_t* d_tile_counts, cudaStream_t st) {
+                  const float* datt_csr, const float* c_att, const int32_t* row_ptr, const int32_t* kv_row,
+                  const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles, int64_t n_nodes, int32_t d,
+                  int32_t n_heads, int64_t kv_rows_total, int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr,
+                  void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts, cudaStream_t st) {
   HGT_REQUIRE(n_heads >= 1 && n_heads <= 32 && d % n_heads == 0, "hgt_edge_backward: bad d=%d / n_heads=%d", d, n_heads);
   HGT_REQUIRE((kvr != nullptr) == (rte_row != nullptr) && (kvr != nullptr) == (dkvr != nullptr),
               "hgt_edge_backward: kvr, rte_row and dkvr must go together");
   HGT_REQUIRE(workspace && workspace_bytes >= 256, "hgt_edge_backward: workspace too small");
+  HGT_REQUIRE((datt_csr != nullptr) == (c_att != nullptr), "hgt_edge_backward_att: datt_csr and c_att must go together");
   // the kernel accumulates (dk / dv of a <source, relation> row come from many edges): this call owns the initialisation
   if (n_nodes > 0) HGT_CHECK_CUDA(cudaMemsetAsync(dq, 0, (size_t)n_nodes * d * sizeof(float), st));
   if (kv_rows_total > 0) HGT_CHECK_CUDA(cudaMemsetAsync(dkv, 0, (size_t)kv_rows_total * 2 * d * sizeof(float), st));
@@ -501,7 +572,8 @@ int edge_backward(const float* q, const KV* kv, const KV* kvr, const float* agg,
   p.dq = dq; p.dkv = dkv; p.dkvr = dkvr;
   p.tile_counter = reinterpret_cast<int32_t*>(workspace);
   p.D = nullptr; p.partial = nullptr;
-  return launch_pass<KV>(p, lm, n_tiles, st, false);
+  p.datt_csr = datt_csr; p.c_att = c_att;
+  return launch_pass_att<KV>(p, lm, n_tiles, st, false);
 }
 
 }  // namespace
@@ -512,9 +584,9 @@ extern "C" int hgt_edge_backward(const float* q, const float* kv, const float* k
                                  int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total,
                                  int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr,
                                  void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts, void* stream_) {
-  return edge_backward<float>(q, kv, kvr, agg, dagg, stats, row_ptr, kv_row, rte_row, tiles, n_tiles, n_nodes, d, n_heads,
-                              kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace, workspace_bytes, d_tile_counts,
-                              (cudaStream_t)stream_);
+  return edge_backward<float>(q, kv, kvr, agg, dagg, stats, nullptr, nullptr, row_ptr, kv_row, rte_row, tiles, n_tiles,
+                              n_nodes, d, n_heads, kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace,
+                              workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_edge_backward_bf16(const float* q, const void* kv, const void* kvr, const float* agg,
@@ -525,9 +597,9 @@ extern "C" int hgt_edge_backward_bf16(const float* q, const void* kv, const void
                                       float* dkvr, void* workspace, size_t workspace_bytes,
                                       const int32_t* d_tile_counts, void* stream_) {
   return edge_backward<__nv_bfloat16>(q, static_cast<const __nv_bfloat16*>(kv), static_cast<const __nv_bfloat16*>(kvr),
-                                      agg, dagg, stats, row_ptr, kv_row, rte_row, tiles, n_tiles, n_nodes, d, n_heads,
-                                      kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace, workspace_bytes,
-                                      d_tile_counts, (cudaStream_t)stream_);
+                                      agg, dagg, stats, nullptr, nullptr, row_ptr, kv_row, rte_row, tiles, n_tiles,
+                                      n_nodes, d, n_heads, kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace,
+                                      workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_edge_backward_det_workspace_bytes(int32_t n_split_dst, int32_t n_split_rows, int32_t d,
@@ -543,12 +615,15 @@ namespace {
 
 template <class KV>
 int edge_backward_dst(const float* q, const KV* kv, const KV* kvr, const float* agg, const float* dagg,
-                      const float* stats, const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
-                      const int32_t* tiles, int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
-                      int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D, void* workspace,
-                      size_t workspace_bytes, const int32_t* d_tile_counts, cudaStream_t st) {
+                      const float* stats, const float* datt_csr, const float* c_att, const int32_t* row_ptr,
+                      const int32_t* kv_row, const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                      int32_t n_split, const int32_t* hubs, int32_t n_hubs, int64_t n_nodes, int32_t d, int32_t n_heads,
+                      float* dq, float* D, void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                      cudaStream_t st) {
   HGT_REQUIRE((kvr != nullptr) == (rte_row != nullptr), "hgt_edge_backward_dst: kvr and rte_row must go together");
   HGT_REQUIRE(dq && D, "hgt_edge_backward_dst: NULL output");
+  HGT_REQUIRE((datt_csr != nullptr) == (c_att != nullptr),
+              "hgt_edge_backward_dst_att: datt_csr and c_att must go together");
   size_t need = 0;
   hgt_edge_backward_det_workspace_bytes(n_split > 0 ? n_split : 0, 0, d, &need);
   HGT_REQUIRE(workspace && workspace_bytes >= need, "hgt_edge_backward_dst: workspace too small (%zu < %zu)",
@@ -568,17 +643,21 @@ int edge_backward_dst(const float* q, const KV* kv, const KV* kvr, const float* 
   p.tile_counter = reinterpret_cast<int32_t*>(workspace);
   p.D = D;
   p.partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  if ((rc = launch_pass<KV>(p, lm, n_tiles, st, true))) return rc;
+  p.datt_csr = datt_csr; p.c_att = c_att;
+  if ((rc = launch_pass_att<KV>(p, lm, n_tiles, st, true))) return rc;
   return n_split > 0 ? merge_pieces(hubs, n_hubs, d_tile_counts, p.partial, d, dq, st) : 0;
 }
 
 template <class KV>
-int edge_backward_rows(const float* q, const float* dagg, const float* stats, const float* D, const KV* own,
-                       const KV* oth, const int32_t* src_ptr, const int32_t* src_dst, const int32_t* src_oth,
-                       int32_t n_rows, int64_t own_rows_total, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
-                       const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads, float* grad, void* workspace,
-                       size_t workspace_bytes, const int32_t* d_tile_counts, cudaStream_t st) {
+int edge_backward_rows(const float* q, const float* dagg, const float* stats, const float* D, const float* datt_csr,
+                       const KV* own, const KV* oth, const int32_t* src_ptr, const int32_t* src_dst,
+                       const int32_t* src_oth, const int32_t* src_pos, int32_t n_rows, int64_t own_rows_total,
+                       const int32_t* tiles, int32_t n_tiles, int32_t n_split, const int32_t* hubs, int32_t n_hubs,
+                       int32_t d, int32_t n_heads, float* grad, void* workspace, size_t workspace_bytes,
+                       const int32_t* d_tile_counts, cudaStream_t st) {
   HGT_REQUIRE(own && grad && (oth == nullptr || src_oth), "hgt_edge_backward_rows: NULL argument");
+  HGT_REQUIRE((datt_csr != nullptr) == (src_pos != nullptr),
+              "hgt_edge_backward_rows_att: datt_csr and src_pos must go together");
   HGT_REQUIRE(n_rows >= 0 && own_rows_total >= n_rows, "hgt_edge_backward_rows: n_rows=%d own_rows_total=%lld", n_rows,
               (long long)own_rows_total);
   size_t need = 0;
@@ -601,7 +680,8 @@ int edge_backward_rows(const float* q, const float* dagg, const float* stats, co
   p.grad = grad;
   p.tile_counter = reinterpret_cast<int32_t*>(workspace);
   p.partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  if ((rc = launch_pass<KV>(p, lm, n_tiles, st, true))) return rc;
+  p.datt_csr = datt_csr; p.e_pos = src_pos;
+  if ((rc = launch_pass_att<KV>(p, lm, n_tiles, st, true))) return rc;
   return n_split > 0 ? merge_pieces(hubs, n_hubs, d_tile_counts, p.partial, 2 * d, grad, st) : 0;
 }
 
@@ -614,9 +694,9 @@ extern "C" int hgt_edge_backward_dst(const float* q, const float* kv, const floa
                                      int64_t n_nodes, int32_t d, int32_t n_heads, float* dq, float* D,
                                      void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
                                      void* stream_) {
-  return edge_backward_dst<float>(q, kv, kvr, agg, dagg, stats, row_ptr, kv_row, rte_row, tiles, n_tiles, n_split, hubs,
-                                  n_hubs, n_nodes, d, n_heads, dq, D, workspace, workspace_bytes, d_tile_counts,
-                                  (cudaStream_t)stream_);
+  return edge_backward_dst<float>(q, kv, kvr, agg, dagg, stats, nullptr, nullptr, row_ptr, kv_row, rte_row, tiles,
+                                  n_tiles, n_split, hubs, n_hubs, n_nodes, d, n_heads, dq, D, workspace,
+                                  workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_edge_backward_dst_bf16(const float* q, const void* kv, const void* kvr, const float* agg,
@@ -627,7 +707,8 @@ extern "C" int hgt_edge_backward_dst_bf16(const float* q, const void* kv, const 
                                           void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
                                           void* stream_) {
   return edge_backward_dst<__nv_bfloat16>(q, static_cast<const __nv_bfloat16*>(kv),
-                                          static_cast<const __nv_bfloat16*>(kvr), agg, dagg, stats, row_ptr, kv_row,
+                                          static_cast<const __nv_bfloat16*>(kvr), agg, dagg, stats, nullptr, nullptr,
+                                          row_ptr, kv_row,
                                           rte_row, tiles, n_tiles, n_split, hubs, n_hubs, n_nodes, d, n_heads, dq, D,
                                           workspace, workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
 }
@@ -639,9 +720,9 @@ extern "C" int hgt_edge_backward_rows(const float* q, const float* dagg, const f
                                       const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads, float* grad,
                                       void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
                                       void* stream_) {
-  return edge_backward_rows<float>(q, dagg, stats, D, own, oth, src_ptr, src_dst, src_oth, n_rows, own_rows_total, tiles,
-                                   n_tiles, n_split, hubs, n_hubs, d, n_heads, grad, workspace, workspace_bytes,
-                                   d_tile_counts, (cudaStream_t)stream_);
+  return edge_backward_rows<float>(q, dagg, stats, D, nullptr, own, oth, src_ptr, src_dst, src_oth, nullptr, n_rows,
+                                   own_rows_total, tiles, n_tiles, n_split, hubs, n_hubs, d, n_heads, grad, workspace,
+                                   workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_edge_backward_rows_bf16(const float* q, const float* dagg, const float* stats, const float* D,
@@ -651,8 +732,127 @@ extern "C" int hgt_edge_backward_rows_bf16(const float* q, const float* dagg, co
                                            int32_t n_split, const int32_t* hubs, int32_t n_hubs, int32_t d,
                                            int32_t n_heads, float* grad, void* workspace, size_t workspace_bytes,
                                            const int32_t* d_tile_counts, void* stream_) {
-  return edge_backward_rows<__nv_bfloat16>(q, dagg, stats, D, static_cast<const __nv_bfloat16*>(own),
-                                           static_cast<const __nv_bfloat16*>(oth), src_ptr, src_dst, src_oth, n_rows,
-                                           own_rows_total, tiles, n_tiles, n_split, hubs, n_hubs, d, n_heads, grad,
-                                           workspace, workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
+  return edge_backward_rows<__nv_bfloat16>(q, dagg, stats, D, nullptr, static_cast<const __nv_bfloat16*>(own),
+                                           static_cast<const __nv_bfloat16*>(oth), src_ptr, src_dst, src_oth, nullptr,
+                                           n_rows, own_rows_total, tiles, n_tiles, n_split, hubs, n_hubs, d, n_heads,
+                                           grad, workspace, workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
+}
+
+// ---- gradient of att -------------------------------------------------------------------------------------------------
+
+extern "C" int hgt_edge_att_grad_workspace_bytes(int32_t n_split, int32_t n_heads, size_t* out_bytes) {
+  HGT_REQUIRE(out_bytes && n_split >= 0 && n_heads >= 1 && n_heads <= 32,
+              "hgt_edge_att_grad_workspace_bytes: bad argument");
+  *out_bytes = 256 + sizeof(float) * (size_t)n_split * n_heads;
+  return 0;
+}
+
+extern "C" int hgt_edge_att_grad_prep(const float* att, const float* datt, const int32_t* csr_eid,
+                                      const int32_t* row_ptr, const int32_t* tiles, int32_t n_tiles, int32_t n_split,
+                                      const int32_t* hubs, int32_t n_hubs, int64_t n_nodes, int32_t n_heads,
+                                      float* c_att, float* datt_csr, void* workspace, size_t workspace_bytes,
+                                      const int32_t* d_tile_counts, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  HGT_REQUIRE(n_heads >= 1 && n_heads <= 32, "hgt_edge_att_grad_prep: bad n_heads=%d", n_heads);
+  HGT_REQUIRE(c_att && datt_csr && (n_tiles == 0 || (att && datt && csr_eid && row_ptr && tiles)),
+              "hgt_edge_att_grad_prep: NULL argument");
+  size_t need = 0;
+  hgt_edge_att_grad_workspace_bytes(n_split > 0 ? n_split : 0, n_heads, &need);
+  HGT_REQUIRE(workspace && workspace_bytes >= need, "hgt_edge_att_grad_prep: workspace too small (%zu < %zu)",
+              workspace_bytes, need);
+  HGT_REQUIRE(n_split <= 0 || (hubs && n_hubs > 0), "hgt_edge_att_grad_prep: split tiles present but no hub list given");
+  if (n_nodes == 0 || n_tiles == 0) return 0;
+  int hp_shift = 0;
+  while ((1 << hp_shift) < n_heads) ++hp_shift;
+  int grid = hgt_sm_count() * 4;
+  const int max_ctas = (n_tiles + kWarps - 1) / kWarps;
+  if (grid > max_ctas) grid = max_ctas;
+  float* partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  k_att_grad_prep<<<grid, kWarps * 32, 0, st>>>(att, datt, csr_eid, row_ptr, tiles, n_tiles, d_tile_counts, n_heads,
+                                                hp_shift, c_att, datt_csr, partial);
+  HGT_LAUNCH_CHECK();
+  return n_split > 0 ? merge_pieces(hubs, n_hubs, d_tile_counts, partial, n_heads, c_att, st) : 0;
+}
+
+extern "C" int hgt_edge_backward_att(const float* q, const float* kv, const float* kvr, const float* agg,
+                                     const float* dagg, const float* stats, const float* datt_csr, const float* c_att,
+                                     const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                                     const int32_t* tiles, int32_t n_tiles, int64_t n_nodes, int32_t d, int32_t n_heads,
+                                     int64_t kv_rows_total, int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr,
+                                     void* workspace, size_t workspace_bytes, const int32_t* d_tile_counts,
+                                     void* stream_) {
+  HGT_REQUIRE(datt_csr && c_att, "hgt_edge_backward_att: NULL datt_csr / c_att");
+  return edge_backward<float>(q, kv, kvr, agg, dagg, stats, datt_csr, c_att, row_ptr, kv_row, rte_row, tiles, n_tiles,
+                              n_nodes, d, n_heads, kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace,
+                              workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_att_bf16(const float* q, const void* kv, const void* kvr, const float* agg,
+                                          const float* dagg, const float* stats, const float* datt_csr,
+                                          const float* c_att, const int32_t* row_ptr, const int32_t* kv_row,
+                                          const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                                          int64_t n_nodes, int32_t d, int32_t n_heads, int64_t kv_rows_total,
+                                          int64_t kvr_rows_total, float* dq, float* dkv, float* dkvr, void* workspace,
+                                          size_t workspace_bytes, const int32_t* d_tile_counts, void* stream_) {
+  HGT_REQUIRE(datt_csr && c_att, "hgt_edge_backward_att_bf16: NULL datt_csr / c_att");
+  return edge_backward<__nv_bfloat16>(q, static_cast<const __nv_bfloat16*>(kv), static_cast<const __nv_bfloat16*>(kvr),
+                                      agg, dagg, stats, datt_csr, c_att, row_ptr, kv_row, rte_row, tiles, n_tiles,
+                                      n_nodes, d, n_heads, kv_rows_total, kvr_rows_total, dq, dkv, dkvr, workspace,
+                                      workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_dst_att(const float* q, const float* kv, const float* kvr, const float* agg,
+                                         const float* dagg, const float* stats, const float* datt_csr,
+                                         const float* c_att, const int32_t* row_ptr, const int32_t* kv_row,
+                                         const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                                         int32_t n_split, const int32_t* hubs, int32_t n_hubs, int64_t n_nodes,
+                                         int32_t d, int32_t n_heads, float* dq, float* D, void* workspace,
+                                         size_t workspace_bytes, const int32_t* d_tile_counts, void* stream_) {
+  HGT_REQUIRE(datt_csr && c_att, "hgt_edge_backward_dst_att: NULL datt_csr / c_att");
+  return edge_backward_dst<float>(q, kv, kvr, agg, dagg, stats, datt_csr, c_att, row_ptr, kv_row, rte_row, tiles,
+                                  n_tiles, n_split, hubs, n_hubs, n_nodes, d, n_heads, dq, D, workspace,
+                                  workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_dst_att_bf16(const float* q, const void* kv, const void* kvr, const float* agg,
+                                              const float* dagg, const float* stats, const float* datt_csr,
+                                              const float* c_att, const int32_t* row_ptr, const int32_t* kv_row,
+                                              const int32_t* rte_row, const int32_t* tiles, int32_t n_tiles,
+                                              int32_t n_split, const int32_t* hubs, int32_t n_hubs, int64_t n_nodes,
+                                              int32_t d, int32_t n_heads, float* dq, float* D, void* workspace,
+                                              size_t workspace_bytes, const int32_t* d_tile_counts, void* stream_) {
+  HGT_REQUIRE(datt_csr && c_att, "hgt_edge_backward_dst_att_bf16: NULL datt_csr / c_att");
+  return edge_backward_dst<__nv_bfloat16>(q, static_cast<const __nv_bfloat16*>(kv),
+                                          static_cast<const __nv_bfloat16*>(kvr), agg, dagg, stats, datt_csr, c_att,
+                                          row_ptr, kv_row, rte_row, tiles, n_tiles, n_split, hubs, n_hubs, n_nodes, d,
+                                          n_heads, dq, D, workspace, workspace_bytes, d_tile_counts,
+                                          (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_rows_att(const float* q, const float* dagg, const float* stats, const float* D,
+                                          const float* datt_csr, const float* own, const float* oth,
+                                          const int32_t* src_ptr, const int32_t* src_dst, const int32_t* src_oth,
+                                          const int32_t* src_pos, int32_t n_rows, int64_t own_rows_total,
+                                          const int32_t* tiles, int32_t n_tiles, int32_t n_split, const int32_t* hubs,
+                                          int32_t n_hubs, int32_t d, int32_t n_heads, float* grad, void* workspace,
+                                          size_t workspace_bytes, const int32_t* d_tile_counts, void* stream_) {
+  HGT_REQUIRE(datt_csr && src_pos, "hgt_edge_backward_rows_att: NULL datt_csr / src_pos");
+  return edge_backward_rows<float>(q, dagg, stats, D, datt_csr, own, oth, src_ptr, src_dst, src_oth, src_pos, n_rows,
+                                   own_rows_total, tiles, n_tiles, n_split, hubs, n_hubs, d, n_heads, grad, workspace,
+                                   workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_edge_backward_rows_att_bf16(const float* q, const float* dagg, const float* stats, const float* D,
+                                               const float* datt_csr, const void* own, const void* oth,
+                                               const int32_t* src_ptr, const int32_t* src_dst, const int32_t* src_oth,
+                                               const int32_t* src_pos, int32_t n_rows, int64_t own_rows_total,
+                                               const int32_t* tiles, int32_t n_tiles, int32_t n_split,
+                                               const int32_t* hubs, int32_t n_hubs, int32_t d, int32_t n_heads,
+                                               float* grad, void* workspace, size_t workspace_bytes,
+                                               const int32_t* d_tile_counts, void* stream_) {
+  HGT_REQUIRE(datt_csr && src_pos, "hgt_edge_backward_rows_att_bf16: NULL datt_csr / src_pos");
+  return edge_backward_rows<__nv_bfloat16>(q, dagg, stats, D, datt_csr, static_cast<const __nv_bfloat16*>(own),
+                                           static_cast<const __nv_bfloat16*>(oth), src_ptr, src_dst, src_oth, src_pos,
+                                           n_rows, own_rows_total, tiles, n_tiles, n_split, hubs, n_hubs, d, n_heads,
+                                           grad, workspace, workspace_bytes, d_tile_counts, (cudaStream_t)stream_);
 }

@@ -1023,16 +1023,19 @@ extern "C" int hgt_halo_push_split(const float* x_own, const int32_t* push_peer,
   return 0;
 }
 
-extern "C" int hgt_plan_source_index(const int32_t* key, const int32_t* other, const int32_t* row_ptr, int64_t n_nodes,
-                                     int64_t n_edges, int32_t n_rows, int32_t* src_ptr, int32_t* src_dst,
-                                     int32_t* src_oth, void* workspace, size_t workspace_bytes, void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+namespace {
+
+// src_pos (or NULL): the CSR position of every entry, which the sort leaves in src_dst before k_source_fill turns it
+// into the destination
+int source_index(const int32_t* key, const int32_t* other, const int32_t* row_ptr, int64_t n_nodes, int64_t n_edges,
+                 int32_t n_rows, int32_t* src_ptr, int32_t* src_dst, int32_t* src_oth, int32_t* src_pos,
+                 void* workspace, size_t workspace_bytes, cudaStream_t st, const char* who) {
   HGT_REQUIRE(src_ptr && (n_edges == 0 || (key && row_ptr && src_dst)) && ((other != nullptr) == (src_oth != nullptr)),
-              "hgt_plan_source_index: NULL argument");
-  HGT_REQUIRE(n_rows >= 0, "hgt_plan_source_index: n_rows=%d", n_rows);
+              "%s: NULL argument", who);
+  HGT_REQUIRE(n_rows >= 0, "%s: n_rows=%d", who, n_rows);
   PlanScratch s;
   size_t need = carve(s, workspace, n_rows, n_edges);
-  HGT_REQUIRE(workspace_bytes >= need, "hgt_plan_source_index: workspace too small (%zu < %zu)", workspace_bytes, need);
+  HGT_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", who, workspace_bytes, need);
   if (n_edges == 0) {
     HGT_CHECK_CUDA(cudaMemsetAsync(src_ptr, 0, sizeof(int32_t) * ((size_t)n_rows + 1), st));
     return 0;
@@ -1043,9 +1046,29 @@ extern "C" int hgt_plan_source_index(const int32_t* key, const int32_t* other, c
   // LSD radix sort: stable, so every row's entries keep CSR (destination) order
   HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, key, s.keys_out, (const int32_t*)s.vals_in, src_dst,
                                                  (int)n_edges, 0, bits_for((int64_t)n_rows + 1), st));
+  if (src_pos)
+    HGT_CHECK_CUDA(cudaMemcpyAsync(src_pos, src_dst, sizeof(int32_t) * (size_t)n_edges, cudaMemcpyDeviceToDevice, st));
   k_source_fill<<<blocks_for(n_edges), kThreads, 0, st>>>(row_ptr, n_nodes, n_edges, other, src_dst, src_oth);
   HGT_LAUNCH_CHECK();
   k_source_ptr<<<blocks_for((int64_t)n_rows + 1), kThreads, 0, st>>>(s.keys_out, n_edges, n_rows, src_ptr);
   HGT_LAUNCH_CHECK();
   return 0;
+}
+
+}  // namespace
+
+extern "C" int hgt_plan_source_index(const int32_t* key, const int32_t* other, const int32_t* row_ptr, int64_t n_nodes,
+                                     int64_t n_edges, int32_t n_rows, int32_t* src_ptr, int32_t* src_dst,
+                                     int32_t* src_oth, void* workspace, size_t workspace_bytes, void* stream_) {
+  return source_index(key, other, row_ptr, n_nodes, n_edges, n_rows, src_ptr, src_dst, src_oth, nullptr, workspace,
+                      workspace_bytes, (cudaStream_t)stream_, "hgt_plan_source_index");
+}
+
+extern "C" int hgt_plan_source_index_pos(const int32_t* key, const int32_t* other, const int32_t* row_ptr,
+                                         int64_t n_nodes, int64_t n_edges, int32_t n_rows, int32_t* src_ptr,
+                                         int32_t* src_dst, int32_t* src_oth, int32_t* src_pos, void* workspace,
+                                         size_t workspace_bytes, void* stream_) {
+  HGT_REQUIRE(n_edges == 0 || src_pos, "hgt_plan_source_index_pos: NULL src_pos");
+  return source_index(key, other, row_ptr, n_nodes, n_edges, n_rows, src_ptr, src_dst, src_oth, src_pos, workspace,
+                      workspace_bytes, (cudaStream_t)stream_, "hgt_plan_source_index_pos");
 }

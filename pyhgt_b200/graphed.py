@@ -415,11 +415,18 @@ class GraphedTrainStep(_Graphed):
         grads = [p.grad for p in self.params]
         for p in self.params:
             p.grad = None                                   # the graph allocates its own static .grad tensors
+        # the trained layers' .att of the eager steps hold their graphs, whose AccumulateGrad nodes were made on this
+        # stream: released, the captured backward makes its own on the capture stream.  Released again after the
+        # capture, so that a later eager step does not reuse the capture stream's nodes (.att then stays a detached
+        # view of the static att every replay rewrites)
+        from .autograd import release_att_graphs
+        release_att_graphs(self.params)
         try:
             self.out = self._capture(self._step)
         except Exception:
             self.capture_failed = True          # the update is done: a retry must not make a second one
             raise
+        release_att_graphs(self.params)
         for o, e in zip(self.out, eager):
             o.copy_(e)
         for p, g in zip(self.params, grads):

@@ -316,7 +316,8 @@ class SourceIndex:
     """CSR positions stably sorted by the row they read in one table (kv_row: the [K'|V'] table; rte_row: the RTE table):
     ptr [n_rows+1] over the owned rows, per entry its destination (rank order) and its row in the other table, and work
     tiles over ptr (rows above TILE_SPLIT_EDGES entries are split).  The counts stay on the device (counts_dev); n_tiles /
-    n_split / n_hubs are the bounds the arrays were sized with."""
+    n_split / n_hubs are the bounds the arrays were sized with.  pos: per entry its CSR position, or None (only the row
+    pass of the att gradient reads it)."""
     n_rows: int
     ptr: torch.Tensor
     dst: torch.Tensor
@@ -327,14 +328,16 @@ class SourceIndex:
     hubs: torch.Tensor
     n_hubs: int
     counts_dev: torch.Tensor
+    pos: torch.Tensor = None
 
 
-def source_index(plan, which):
+def source_index(plan, which, with_pos=False):
     """The source-major index of `plan` keyed by kv_row (which="kv") or rte_row (which="rte"), built on first use with
     no host synchronisation and cached on the plan.  The trailing all-zero row (edges that match no triple) gets no
-    entry in ptr: its gradient is discarded."""
+    entry in ptr: its gradient is discarded.  with_pos: the index also carries every entry's CSR position, from the same
+    sort (hgt_plan_source_index_pos); a cached index without them is built again with them."""
     hit = plan._source_index.get(which)
-    if hit is not None:
+    if hit is not None and (hit.pos is not None or not with_pos):
         return hit
     if which == "kv":
         key, other, n_rows = plan.kv_row, plan.rte_row, plan.kv_rows
@@ -357,8 +360,15 @@ def source_index(plan, which):
     ptr = torch.empty(n_rows + 1, **i32)
     dst = torch.empty(max(E, 1), **i32)
     oth = torch.empty(max(E, 1), **i32) if other is not None else None
-    _lib.call("hgt_plan_source_index", key.data_ptr(), _lib.ptr(other), plan.row_ptr.data_ptr(), plan.n_nodes, E, n_rows,
-              ptr.data_ptr(), dst.data_ptr(), _lib.ptr(oth), ws.data_ptr(), ws.numel(), st)
+    if with_pos:
+        pos = torch.empty(max(E, 1), **i32)
+        _lib.call("hgt_plan_source_index_pos", key.data_ptr(), _lib.ptr(other), plan.row_ptr.data_ptr(), plan.n_nodes,
+                  E, n_rows, ptr.data_ptr(), dst.data_ptr(), _lib.ptr(oth), pos.data_ptr(), ws.data_ptr(), ws.numel(),
+                  st)
+    else:
+        pos = None
+        _lib.call("hgt_plan_source_index", key.data_ptr(), _lib.ptr(other), plan.row_ptr.data_ptr(), plan.n_nodes, E,
+                  n_rows, ptr.data_ptr(), dst.data_ptr(), _lib.ptr(oth), ws.data_ptr(), ws.numel(), st)
     max_tiles = (2 * E + n_rows) // (2 * TILE_TARGET_EDGES) + 3 * (E // TILE_SPLIT_EDGES) + 16
     tiles = torch.empty((max_tiles, 4), **i32)
     max_hubs = E // TILE_SPLIT_EDGES + 1
@@ -369,7 +379,7 @@ def source_index(plan, which):
     has_hub = E > TILE_SPLIT_EDGES
     idx = SourceIndex(n_rows=n_rows, ptr=ptr, dst=dst, oth=oth, tiles=tiles, n_tiles=max_tiles if n_rows > 0 else 0,
                       n_split=2 * (E // TILE_SPLIT_EDGES) + 1 if has_hub else 0, hubs=hubs,
-                      n_hubs=max_hubs if has_hub else 0, counts_dev=counts)
+                      n_hubs=max_hubs if has_hub else 0, counts_dev=counts, pos=pos)
     plan._source_index[which] = idx
     return idx
 
