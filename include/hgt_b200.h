@@ -344,6 +344,13 @@ int hgt_edge_backward(const float* q, const float* kv, const float* kvr, const f
  *   the key / value row as in the forward; NULL without RTE), and writes grad[row] = [sum ds Q_i | sum p dagg_i] with
  *   one store.  Rows [n_rows, own_rows_total) (the trailing all-zero row) are zeroed.  Split rows: partial rows summed
  *   in piece order.
+ *   In place: grad may be `own` itself (fp32 tables, hgt_edge_backward_rows[_att]; the bf16 entry points have an fp32
+ *   grad and a bf16 own, which never alias).  The result is then bitwise that of a separate grad.  This holds because
+ *   every read of own[r] precedes every write of grad[r]: the owning warp loads its row before walking the row's
+ *   entries and stores it once at the end; the pieces of a split row (every piece of it is split) read the row and write
+ *   workspace partials, which a later launch sums into grad[r]; a row without entries loads nothing and stores zeros;
+ *   rows past n_rows are zeroed before the pass and never read as `own`; own is read with coherent loads.  `oth` must
+ *   not alias grad: the RTE row pass reads the [K'|V'] rows as oth, so it runs before an in-place [K'|V'] pass.
  * tiles / n_tiles / n_split / hubs / n_hubs / d_tile_counts as for hgt_edge_forward (for the row pass: from
  *   hgt_plan_tiles over src_ptr).  Every d / n_heads that hgt_edge_backward takes is supported.
  * workspace: hgt_edge_backward_det_workspace_bytes(n_split of the destination tiles, n_split of the row tiles, d); the

@@ -108,57 +108,12 @@ class _TypedLinear(torch.autograd.Function):
     def forward(ctx, a, w_cat, b_cat, table, width, out_elems, impl, act, zero_ranges, tables16=None):
         a = a.contiguous()
         w_cat = w_cat.contiguous()
-        rows, K = a.shape
-        dev = a.device
-        st = _stream()
-        if tables16 is None:
-            out = torch.empty(out_elems, dtype=torch.float32, device=dev)
-            for (z0, z1) in zero_ranges:                               # padding / all-zero table rows only
-                if z1 > z0:
-                    out[z0:z1].zero_()
-        else:
-            q_table, q_elems, kv_table, kv_off, kv_zero = tables16
-            q = torch.empty(q_elems, dtype=torch.float32, device=dev) if q_table is not None else None
-            kv = torch.empty(out_elems - kv_off, dtype=torch.bfloat16, device=dev)
-            for (z0, z1) in kv_zero:
-                if z1 > z0:
-                    kv[z0:z1].zero_()
+        K = a.shape[1]
         use_tc = impl in (0, 2, 3) and _tc_shape_ok(K, width)
         one = use_tc and impl == 3
-        hi = lo = a_act = None
-        if use_tc:
-            hi = torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
-            lo = None if one else torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
-            _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, None, hi.data_ptr(), _lib.ptr(lo), st)
-        else:
-            a_act = a
-            if act:
-                a_act = torch.empty_like(a)
-                _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, a_act.data_ptr(), None, None, st)
-
-        def gemm(tab, dst):
-            g_dev, g_host, n_g, c_dev = tab
-            sfx = "_bf16" if dst.dtype == torch.bfloat16 else ""
-            wsb = ctypes.c_size_t()
-            if use_tc:
-                _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, K, width, ctypes.byref(wsb))
-                ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                _lib.call("hgt_typed_linear_presplit" + sfx, hi.data_ptr(), _lib.ptr(lo), w_cat.data_ptr(),
-                          _lib.ptr(b_cat), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(),
-                          dst.data_ptr(), ws.data_ptr(), ws.numel(), st)
-            else:
-                _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, K, width, 1, ctypes.byref(wsb))
-                ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                _lib.call("hgt_typed_linear" + sfx, a_act.data_ptr(), K, w_cat.data_ptr(), _lib.ptr(b_cat), K, width,
-                          g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), dst.data_ptr(), 1, ws.data_ptr(),
-                          ws.numel(), st)
-
-        if tables16 is None:
-            gemm(table, out)
-        else:
-            if q is not None:
-                gemm(q_table, q)
-            gemm(kv_table, kv)
+        out, q, kv = _linear_outputs(out_elems, zero_ranges, tables16, a.device)
+        hi, lo, a_act = _split_operand(a, act, use_tc, one)
+        _linear_gemms(hi, lo, a_act, w_cat, b_cat, table, width, use_tc, tables16, out, q, kv)
         ctx.table, ctx.width, ctx.has_bias, ctx.act, ctx.use_tc = table, width, b_cat is not None, act, use_tc
         ctx.one = one
         ctx.out_elems = out_elems
@@ -168,47 +123,122 @@ class _TypedLinear(torch.autograd.Function):
         if tables16 is None:
             return out
         ctx.mark_non_differentiable(*[t for t in (q, kv) if t is not None])
-        return torch.zeros(1, dtype=torch.float32, device=dev).expand(out_elems), q, kv
+        return torch.zeros(1, dtype=torch.float32, device=a.device).expand(out_elems), q, kv
 
     @staticmethod
     def backward(ctx, dout, *_unused):
         a, a_act, hi, lo, w_cat = ctx.saved_tensors
-        width = ctx.width
-        K = w_cat.shape[1]
-        dev = w_cat.device
-        rows = hi.shape[0] if hi is not None else a.shape[0]
-        need_da = ctx.needs_input_grad[0]
-        dout = dout.contiguous()
-        da = torch.empty((rows, K), dtype=torch.float32, device=dev) if need_da else None
-        dw = torch.zeros_like(w_cat)                                   # small: [sum of out rows, K]
-        db = torch.zeros(w_cat.shape[0], dtype=torch.float32, device=dev) if ctx.has_bias else None
-        impl = (3 if ctx.one else 2) if ctx.use_tc else 1
-        fn = "hgt_typed_linear_bwd_det" if ctx.det else "hgt_typed_linear_bwd"
-        a_f32 = a_act if a_act is not None else a                      # SIMT dW operand (act already applied)
-        # tables whose groups overlap in rows (sharded per-pair compaction) come with disjoint sub-tables: the first call
-        # writes dA, the others accumulate into it; dW / db accumulate anyway
-        tables = getattr(ctx.table, "bwd_tables", None) or [ctx.table]
-        if not ctx.use_tc:
-            tables = [ctx.table]                                       # the SIMT dX adds overlapping groups itself
-        if need_da:
-            # hgt_typed_linear_bwd zeroes the gaps between the first table's groups; rows past its last group (other
-            # sub-tables' rows, nodes of unknown type) are zeroed here
-            g0, n0 = tables[0][1], tables[0][2]
-            end0 = int((g0["a_row0"][:n0] + g0["m"][:n0]).max()) if n0 else 0
-            if end0 < rows:
-                da[end0:].zero_()
-        for ti, tab in enumerate(tables):
-            g_dev, g_host, n_g, _ = tab
-            c_host = tab.c_host
-            wsb = ctypes.c_size_t()
-            _lib.call(fn + "_workspace_bytes", g_host.ctypes.data, n_g, c_host.ctypes.data, K, width, K,
-                      ctx.out_elems, 0, int(hi is not None), impl, ctypes.byref(wsb))
-            ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-            _lib.call(fn, dout.data_ptr(), None, None, ctx.out_elems, _lib.ptr(a_f32), K, _lib.ptr(hi),
-                      _lib.ptr(lo), w_cat.data_ptr(), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g,
-                      c_host.ctypes.data, _lib.ptr(da), int(ti > 0), a.data_ptr() if ctx.act else None, dw.data_ptr(),
-                      _lib.ptr(db), impl, ws.data_ptr(), ws.numel(), _stream())
+        da, dw, db = _linear_backward(ctx, dout, a, a_act, hi, lo, w_cat, ctx.needs_input_grad[0])
         return da, dw, db, None, None, None, None, None, None, None
+
+
+def _split_operand(a, act, use_tc, one):
+    """act(a) as the typed GEMM reads it: (hi, lo, a_act), the bf16 hi/lo split on the tensor cores (hi only for one
+    bf16 product) or a_act, fp32 act(a), on the SIMT path."""
+    rows, K = a.shape
+    dev = a.device
+    st = _stream()
+    hi = lo = a_act = None
+    if use_tc:
+        hi = torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
+        lo = None if one else torch.empty((rows, K), dtype=torch.bfloat16, device=dev)
+        _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, None, hi.data_ptr(), _lib.ptr(lo), st)
+    else:
+        a_act = a
+        if act:
+            a_act = torch.empty_like(a)
+            _lib.call("hgt_act_split", a.data_ptr(), K, rows, K, act, a_act.data_ptr(), None, None, st)
+    return hi, lo, a_act
+
+
+def _linear_outputs(out_elems, zero_ranges, tables16, dev):
+    """The output buffers of _TypedLinear: (out, None, None), or (None, q or None, kv) with tables16."""
+    out = q = kv = None
+    if tables16 is None:
+        out = torch.empty(out_elems, dtype=torch.float32, device=dev)
+        for (z0, z1) in zero_ranges:                                   # padding / all-zero table rows only
+            if z1 > z0:
+                out[z0:z1].zero_()
+    else:
+        q_table, q_elems, kv_table, kv_off, kv_zero = tables16
+        q = torch.empty(q_elems, dtype=torch.float32, device=dev) if q_table is not None else None
+        kv = torch.empty(out_elems - kv_off, dtype=torch.bfloat16, device=dev)
+        for (z0, z1) in kv_zero:
+            if z1 > z0:
+                kv[z0:z1].zero_()
+    return out, q, kv
+
+
+def _linear_gemms(hi, lo, a_act, w_cat, b_cat, table, width, use_tc, tables16, out, q, kv):
+    """The forward product of _TypedLinear on its split operand into the buffers of _linear_outputs.  The GEMMs are
+    deterministic: the same call on the same operands writes the same outputs bit for bit."""
+    K = w_cat.shape[1]
+    dev = w_cat.device
+    st = _stream()
+
+    def gemm(tab, dst):
+        g_dev, g_host, n_g, c_dev = tab
+        sfx = "_bf16" if dst.dtype == torch.bfloat16 else ""
+        wsb = ctypes.c_size_t()
+        if use_tc:
+            _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, K, width, ctypes.byref(wsb))
+            ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+            _lib.call("hgt_typed_linear_presplit" + sfx, hi.data_ptr(), _lib.ptr(lo), w_cat.data_ptr(),
+                      _lib.ptr(b_cat), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(),
+                      dst.data_ptr(), ws.data_ptr(), ws.numel(), st)
+        else:
+            _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, K, width, 1, ctypes.byref(wsb))
+            ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+            _lib.call("hgt_typed_linear" + sfx, a_act.data_ptr(), K, w_cat.data_ptr(), _lib.ptr(b_cat), K, width,
+                      g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), dst.data_ptr(), 1, ws.data_ptr(),
+                      ws.numel(), st)
+
+    if tables16 is None:
+        gemm(table, out)
+    else:
+        if q is not None:
+            gemm(tables16[0], q)
+        gemm(tables16[2], kv)
+
+
+def _linear_backward(ctx, dout, a, a_act, hi, lo, w_cat, need_da):
+    """dA, dW, db of _TypedLinear from the gradient of its flat output; ctx carries the forward's table, width,
+    has_bias, act, use_tc, one, out_elems and det."""
+    width = ctx.width
+    K = w_cat.shape[1]
+    dev = w_cat.device
+    rows = hi.shape[0] if hi is not None else a.shape[0]
+    dout = dout.contiguous()
+    da = torch.empty((rows, K), dtype=torch.float32, device=dev) if need_da else None
+    dw = torch.zeros_like(w_cat)                                       # small: [sum of out rows, K]
+    db = torch.zeros(w_cat.shape[0], dtype=torch.float32, device=dev) if ctx.has_bias else None
+    impl = (3 if ctx.one else 2) if ctx.use_tc else 1
+    fn = "hgt_typed_linear_bwd_det" if ctx.det else "hgt_typed_linear_bwd"
+    a_f32 = a_act if a_act is not None else a                          # SIMT dW operand (act already applied)
+    # tables whose groups overlap in rows (sharded per-pair compaction) come with disjoint sub-tables: the first call
+    # writes dA, the others accumulate into it; dW / db accumulate anyway
+    tables = getattr(ctx.table, "bwd_tables", None) or [ctx.table]
+    if not ctx.use_tc:
+        tables = [ctx.table]                                           # the SIMT dX adds overlapping groups itself
+    if need_da:
+        # hgt_typed_linear_bwd zeroes the gaps between the first table's groups; rows past its last group (other
+        # sub-tables' rows, nodes of unknown type) are zeroed here
+        g0, n0 = tables[0][1], tables[0][2]
+        end0 = int((g0["a_row0"][:n0] + g0["m"][:n0]).max()) if n0 else 0
+        if end0 < rows:
+            da[end0:].zero_()
+    for ti, tab in enumerate(tables):
+        g_dev, g_host, n_g, _ = tab
+        c_host = tab.c_host
+        wsb = ctypes.c_size_t()
+        _lib.call(fn + "_workspace_bytes", g_host.ctypes.data, n_g, c_host.ctypes.data, K, width, K,
+                  ctx.out_elems, 0, int(hi is not None), impl, ctypes.byref(wsb))
+        ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
+        _lib.call(fn, dout.data_ptr(), None, None, ctx.out_elems, _lib.ptr(a_f32), K, _lib.ptr(hi),
+                  _lib.ptr(lo), w_cat.data_ptr(), K, width, g_dev.data_ptr(), g_host.ctypes.data, n_g,
+                  c_host.ctypes.data, _lib.ptr(da), int(ti > 0), a.data_ptr() if ctx.act else None, dw.data_ptr(),
+                  _lib.ptr(db), impl, ws.data_ptr(), ws.numel(), _stream())
+    return da, dw, db
 
 
 class _EdgeAttention(torch.autograd.Function):
@@ -220,7 +250,6 @@ class _EdgeAttention(torch.autograd.Function):
     @staticmethod
     def forward(ctx, proj, kvr, plan, lt, d, n_heads, want_att, variant, tables16=None):
         N = plan.n_nodes
-        dev = proj.device
         ctx.bf16 = tables16 is not None
         if ctx.bf16:
             q, kv, kvr = tables16
@@ -229,18 +258,7 @@ class _EdgeAttention(torch.autograd.Function):
             q = proj[lt.q_off:lt.q_off + N * d]
             kv = proj[lt.kv_off:]
             kvr = None if kvr is None else kvr.contiguous()
-        ws_bytes = ctypes.c_size_t()
-        _lib.call("hgt_edge_workspace_bytes", plan.n_split, d, n_heads, ctypes.byref(ws_bytes))
-        ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
-        agg = torch.empty((N, d), dtype=torch.float32, device=dev)
-        stats = torch.empty((N, 2 * n_heads), dtype=torch.float32, device=dev)
-        att = torch.empty((plan.n_edges, n_heads), dtype=torch.float32, device=dev) if want_att else None
-        _lib.call("hgt_edge_forward_bf16" if ctx.bf16 else "hgt_edge_forward", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
-                  plan.kv_row.data_ptr(), None if kvr is None else plan.rte_row.data_ptr(), plan.csr_eid.data_ptr(),
-                  plan.tiles.data_ptr(), plan.n_tiles, plan.n_split, plan.hubs.data_ptr(), plan.n_hubs, N, plan.n_edges, d,
-                  n_heads, 0, agg.data_ptr(), _lib.ptr(att), stats.data_ptr(), None, None, ws.data_ptr(), ws.numel(),
-                  variant, _lib.ptr(plan.tile_counts_dev), plan.type_row0_dev.data_ptr(), plan.num_types,
-                  _lib.ptr(lt.type_active_dev), _stream())
+        agg, att, stats = _edge_forward(q, kv, kvr, plan, lt, d, n_heads, want_att, variant, ctx.bf16)
         ctx.plan, ctx.lt, ctx.d, ctx.n_heads, ctx.has_kvr = plan, lt, d, n_heads, kvr is not None
         ctx.det = torch.are_deterministic_algorithms_enabled()
         ctx.proj_elems = proj.numel()
@@ -283,6 +301,25 @@ class _EdgeAttention(torch.autograd.Function):
         return dproj, dkvr, None, None, None, None, None, None, None
 
 
+def _edge_forward(q, kv, kvr, plan, lt, d, n_heads, want_att, variant, bf16):
+    """hgt_edge_forward[_bf16]: (agg [N, d], att [E, H] or None, softmax statistics [N, 2H])."""
+    N = plan.n_nodes
+    dev = q.device
+    ws_bytes = ctypes.c_size_t()
+    _lib.call("hgt_edge_workspace_bytes", plan.n_split, d, n_heads, ctypes.byref(ws_bytes))
+    ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
+    agg = torch.empty((N, d), dtype=torch.float32, device=dev)
+    stats = torch.empty((N, 2 * n_heads), dtype=torch.float32, device=dev)
+    att = torch.empty((plan.n_edges, n_heads), dtype=torch.float32, device=dev) if want_att else None
+    _lib.call("hgt_edge_forward_bf16" if bf16 else "hgt_edge_forward", q.data_ptr(), kv.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
+              plan.kv_row.data_ptr(), None if kvr is None else plan.rte_row.data_ptr(), plan.csr_eid.data_ptr(),
+              plan.tiles.data_ptr(), plan.n_tiles, plan.n_split, plan.hubs.data_ptr(), plan.n_hubs, N, plan.n_edges, d,
+              n_heads, 0, agg.data_ptr(), _lib.ptr(att), stats.data_ptr(), None, None, ws.data_ptr(), ws.numel(),
+              variant, _lib.ptr(plan.tile_counts_dev), plan.type_row0_dev.data_ptr(), plan.num_types,
+              _lib.ptr(lt.type_active_dev), _stream())
+    return agg, att, stats
+
+
 def _att_grad_prep(att, datt, plan, H):
     """(datt in CSR order [E, H], C [N, H]) for the *_att backward calls: hgt_edge_att_grad_prep."""
     dev = att.device
@@ -298,11 +335,12 @@ def _att_grad_prep(att, datt, plan, H):
     return datt_csr, c_att
 
 
-def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx="", att_grad=None):
+def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, sfx="", att_grad=None, rte_first=False):
     """Deterministic edge backward: destination pass (dq, D), then one row pass over the [K'|V'] rows and, with RTE, one
     over the RTE rows; each gradient row is written once by its owner.  sfx "_bf16": bf16 kv / kvr tables.  att_grad:
     None, or (datt_csr, C) from _att_grad_prep: the *_att passes, the row passes reading datt at the CSR positions the
-    source-major indices carry (plan.source_index(..., with_pos=True))."""
+    source-major indices carry (plan.source_index(..., with_pos=True)).  rte_first: the RTE row pass, which reads the
+    K'/V' rows, runs before the K'/V' pass, so that dkv may be kv itself (fp32 tables; _ProjectEdgeLean)."""
     N = plan.n_nodes
     st = _stream()
     with_pos = att_grad is not None
@@ -324,6 +362,8 @@ def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, 
     passes = [(kv, kvr, kvi, plan.kv_rows + 1, dkv)]
     if kvr is not None:
         passes.append((kvr, kv, rti, kvr.numel() // (2 * d), dkvr))
+    if rte_first:
+        passes.reverse()
     for own, oth, idx, own_rows, grad in passes:
         src_oth = None if oth is None else idx.oth.data_ptr()
         if att_grad is None:
@@ -337,6 +377,80 @@ def _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, 
                       src_oth, idx.pos.data_ptr(), idx.n_rows, own_rows, idx.tiles.data_ptr(), idx.n_tiles, idx.n_split,
                       idx.hubs.data_ptr(), idx.n_hubs, d, H, grad.data_ptr(), ws.data_ptr(), ws.numel(),
                       idx.counts_dev.data_ptr(), st)
+
+
+class _ProjectEdgeLean(torch.autograd.Function):
+    """The typed projection and the edge attention of a layer as one stage that keeps neither Q nor the [K'|V'] table
+    for the backward (HGTConv.recompute_tables).  The forward saves what the projection's own backward needs anyway (the
+    bf16 split of x, or fp32 x on the SIMT path, and W_cat), b_cat, the RTE table and the edge kernel's outputs.  The
+    backward
+      1. recomputes the projection with the forward's GEMM calls on those operands: the same tables bit for bit;
+      2. runs the destination pass: dq into its own [N, d] buffer, and D;
+      3. with RTE, runs the RTE row pass into dkvr (it reads the K'/V' rows, so it goes before 4);
+      4. runs the K'/V' row pass.  fp32 tables: each row's gradient is written over the row itself (hgt_edge_backward_rows
+         accepts grad == own), then dq is copied over Q, which turns the recomputed buffer into its own gradient.  bf16
+         tables: the fp32 gradient goes to its own buffer, as in _EdgeAttention;
+      5. runs the projection backward (dX, dW, db) as _TypedLinear does.
+    The edge passes are the source-major ones whatever the deterministic flag (only they can write in place); with the
+    flag on the gradients are those of _TypedLinear + _EdgeAttention bit for bit.  kvr: the RTE table (fp32) or its
+    gradient stand-in (bf16, kvr16 is then the table the kernels read)."""
+
+    @staticmethod
+    def forward(ctx, x, w_cat, b_cat, kvr, plan, lt, d, n_heads, want_att, variant, impl, bf16, kvr16):
+        x = x.contiguous()
+        w_cat = w_cat.contiguous()
+        N, K = plan.n_nodes, x.shape[1]
+        use_tc = impl in (0, 2, 3) and _tc_shape_ok(K, d)
+        one = use_tc and impl == 3
+        zero_ranges, tables16 = _proj_layout(plan, lt, d, bf16)
+        out, q, kv = _linear_outputs(lt.proj_elems, zero_ranges, tables16, x.device)
+        hi, lo, a_act = _split_operand(x, 0, use_tc, one)
+        _linear_gemms(hi, lo, a_act, w_cat, b_cat, lt.proj_groups, d, use_tc, tables16, out, q, kv)
+        if bf16:
+            table = kvr16
+        else:
+            q, kv = out[lt.q_off:lt.q_off + N * d], out[lt.kv_off:]
+            table = None if kvr is None else kvr.contiguous()
+        agg, att, stats = _edge_forward(q, kv, table, plan, lt, d, n_heads, want_att, variant, bf16)
+        # the attributes _linear_backward reads, as _TypedLinear records them
+        ctx.table, ctx.width, ctx.has_bias, ctx.act, ctx.use_tc = lt.proj_groups, d, b_cat is not None, 0, use_tc
+        ctx.one = one
+        ctx.out_elems = lt.proj_elems
+        ctx.det = torch.are_deterministic_algorithms_enabled()
+        ctx.plan, ctx.lt, ctx.d, ctx.n_heads, ctx.bf16 = plan, lt, d, n_heads, bf16
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(None if use_tc else x, hi, lo, w_cat, b_cat, table, agg, stats, att)
+        return agg, att
+
+    @staticmethod
+    def backward(ctx, dagg, datt=None):
+        x, hi, lo, w_cat, b_cat, kvr, agg, stats, att = ctx.saved_tensors
+        plan, lt, d, H = ctx.plan, ctx.lt, ctx.d, ctx.n_heads
+        N = plan.n_nodes
+        f32 = dict(dtype=torch.float32, device=agg.device)
+        zero_ranges, tables16 = _proj_layout(plan, lt, d, ctx.bf16)
+        out, q, kv = _linear_outputs(lt.proj_elems, zero_ranges, tables16, agg.device)
+        _linear_gemms(hi, lo, x, w_cat, b_cat, lt.proj_groups, d, ctx.use_tc, tables16, out, q, kv)
+        if dagg is None:                                               # the loss reads att only
+            dagg = torch.zeros((N, d), **f32)
+        dagg = dagg.contiguous()
+        att_grad = _att_grad_prep(att, datt, plan, H) if datt is not None else None
+        if ctx.bf16:
+            dproj = torch.empty(lt.proj_elems, **f32)
+            if lt.kv_off > N * d:
+                dproj[N * d:lt.kv_off].zero_()                         # alignment gap
+            dq, dkv = dproj[lt.q_off:lt.q_off + N * d], dproj[lt.kv_off:]
+        else:
+            q, kv = out[lt.q_off:lt.q_off + N * d], out[lt.kv_off:]
+            dproj, dq, dkv = out, torch.empty(N * d, **f32), kv        # the gap and the zero row stay zero
+        dkvr = torch.empty(kvr.numel(), **f32) if kvr is not None else None
+        _edge_backward_det(q, kv, kvr, agg, dagg, stats, plan, d, H, dq, dkv, dkvr, "_bf16" if ctx.bf16 else "",
+                           att_grad, rte_first=True)
+        if not ctx.bf16:
+            q.copy_(dq)
+        q = kv = dq = dkv = None                                       # bf16: the tables go before dX / dW
+        dx, dw, db = _linear_backward(ctx, dproj, x, None, hi, lo, w_cat, ctx.needs_input_grad[0])
+        return dx, dw, db, dkvr, None, None, None, None, None, None, None, None, None
 
 
 class _FoldWeights(torch.autograd.Function):
@@ -433,33 +547,70 @@ def typed_linear(a, w_cat, b_cat, table, width, out_elems, impl=0, act=0, zero_r
     return _TypedLinear.apply(a, w_cat, b_cat, table, width, out_elems, impl, act, tuple(zero_ranges), tables16)
 
 
+def _proj_layout(plan, lt, d, bf16):
+    """(zero_ranges, tables16) of the projection's typed GEMM: the flat [Q | pad | K'V' table | zero row] buffer with its
+    padding and zero row cleared, or, with bf16 tables, the fp32 Q buffer and the bf16 [K'|V'] table (zero row cleared)."""
+    kv_end = lt.kv_off + plan.kv_rows * 2 * d
+    if bf16:
+        return (), (lt.q_groups, plan.n_nodes * d, lt.kv_groups, lt.kv_off,
+                    ((kv_end - lt.kv_off, lt.proj_elems - lt.kv_off),))
+    return ((plan.n_nodes * d, lt.kv_off), (kv_end, lt.proj_elems)), None
+
+
+def _rte_tables(m, w_cat, plan, lt, bf16):
+    """(kvr, kvr16) of a layer: with RTE the table [P*240+1, 2d] (+ all-zero row) and, with bf16 tables, kvr is its
+    gradient stand-in and kvr16 the bf16 table; (None, None) without RTE."""
+    if not m.use_RTE:
+        return None, None
+    P, d, d_in = plan.n_pairs, m.out_dim, m.in_dim
+    # RT = lin(emb.weight) [240, d_in] (conv.py:299), then projected with every pair's K'/V' weights (no bias)
+    rt = typed_linear(m.emb.emb.weight, m.emb.lin.weight, m.emb.lin.bias, lt.rt_group, d_in,
+                      _plan.RTE_MAX_LEN * d_in, 1).view(_plan.RTE_MAX_LEN, d_in)
+    n_kvr = (P * _plan.RTE_MAX_LEN + 1) * 2 * d
+    zero = ((P * _plan.RTE_MAX_LEN * 2 * d, n_kvr),)
+    if bf16:
+        kvr, _, kvr16 = typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, (),
+                                     (None, 0, lt.rte_groups, 0, zero))
+        return kvr, kvr16
+    return typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, zero), None
+
+
 def _project(m, x, w_cat, b_cat, plan, lt, bf16, impl):
     """Typed projections of a layer: the flat [Q | pad | K'V' table | zero row] buffer and, with RTE, the RTE table
     [P*240+1, 2d] (+ all-zero row).  bf16: those two are gradient stand-ins and the third result holds what the edge kernel
     reads, (Q, bf16 [K'|V'] table, bf16 RTE table or None); otherwise it is None.  impl: the projection GEMM's (gemm_impl;
     the RTE tables stay fp32 SIMT)."""
-    N, P, d, d_in = plan.n_nodes, plan.n_pairs, m.out_dim, m.in_dim
-    kv_end = lt.kv_off + plan.kv_rows * 2 * d
-    if bf16:
-        proj, q, kv = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, impl, 0, (),
-                                   (lt.q_groups, N * d, lt.kv_groups, lt.kv_off,
-                                    ((kv_end - lt.kv_off, lt.proj_elems - lt.kv_off),)))
-    else:
-        proj = typed_linear(x, w_cat, b_cat, lt.proj_groups, d, lt.proj_elems, impl, 0,
-                            ((N * d, lt.kv_off), (kv_end, lt.proj_elems)))
-    kvr = kvr16 = None
-    if m.use_RTE:
-        # RT = lin(emb.weight) [240, d_in] (conv.py:299), then projected with every pair's K'/V' weights (no bias)
-        rt = typed_linear(m.emb.emb.weight, m.emb.lin.weight, m.emb.lin.bias, lt.rt_group, d_in,
-                          _plan.RTE_MAX_LEN * d_in, 1).view(_plan.RTE_MAX_LEN, d_in)
-        n_kvr = (P * _plan.RTE_MAX_LEN + 1) * 2 * d
-        zero = ((P * _plan.RTE_MAX_LEN * 2 * d, n_kvr),)
-        if bf16:
-            kvr, _, kvr16 = typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, (),
-                                         (None, 0, lt.rte_groups, 0, zero))
-        else:
-            kvr = typed_linear(rt, w_cat, None, lt.rte_groups, d, n_kvr, 1, 0, zero)
+    zero_ranges, tables16 = _proj_layout(plan, lt, m.out_dim, bf16)
+    res = typed_linear(x, w_cat, b_cat, lt.proj_groups, m.out_dim, lt.proj_elems, impl, 0, zero_ranges, tables16)
+    proj, q, kv = res if bf16 else (res, None, None)
+    kvr, kvr16 = _rte_tables(m, w_cat, plan, lt, bf16)
     return proj, kvr, ((q, kv, kvr16) if bf16 else None)
+
+
+# layers that ran a training forward: GraphedTrainStep freezes their recompute_tables switch at capture
+_TRAINED_LAYERS = weakref.WeakSet()
+
+
+def recompute_switches(params):
+    """{layer: bool(recompute_tables)} of the layers that ran a training forward and own one of `params`."""
+    owned = {id(p) for p in params}
+    return {m: bool(m.recompute_tables) for m in list(_TRAINED_LAYERS) if any(id(p) in owned for p in m.parameters())}
+
+
+def _project_edge(m, x, w_cat, b_cat, plan, lt, impl, want_att):
+    """Typed projections and edge attention of a layer: (agg, att).  m.recompute_tables, read here once per training
+    forward, selects _ProjectEdgeLean (the backward rebuilds the projection tables); otherwise the projection buffer is
+    kept for the backward (_project + _EdgeAttention)."""
+    d, H = m.out_dim, m.n_heads
+    bf16 = bf16_tables()
+    if torch.is_grad_enabled():
+        _TRAINED_LAYERS.add(m)
+        if m.recompute_tables:
+            kvr, kvr16 = _rte_tables(m, w_cat, plan, lt, bf16)
+            return _ProjectEdgeLean.apply(x, w_cat, b_cat, kvr, plan, lt, d, H, want_att, m.edge_variant, impl, bf16,
+                                          kvr16)
+    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16, impl)
+    return _EdgeAttention.apply(proj, kvr, plan, lt, d, H, want_att, m.edge_variant, tables16)
 
 
 def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, active=None, kv_runs=None, plan=None,
@@ -489,10 +640,9 @@ def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, 
               [m.relation_att, m.relation_msg, m.relation_pri])
     w_cat, b_cat = _FoldWeights.apply(m, plan, lt, *params)
     impl = gemm_impl(m.linear_impl, bf16_matmuls())
-    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables(), impl)
 
-    # 2. fused edge kernel
-    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, want_att, m.edge_variant, tables16)
+    # 2. fused edge kernel (with m.recompute_tables one stage with the projection, whose backward rebuilds the tables)
+    agg, att = _project_edge(m, x, w_cat, b_cat, plan, lt, impl, want_att)
     _set_att(m, att)
 
     # 3. a_linears on gelu(agg) (conv.py:119,125): the gelu is applied inside the operand split / the dX epilogue
@@ -530,8 +680,7 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
               [m.relation_att, m.relation_msg, m.relation_pri])
     w_cat, b_cat = _FoldWeights.apply(m, plan, lt, *params)
     impl = gemm_impl(m.linear_impl, bf16_matmuls())
-    proj, kvr, tables16 = _project(m, x, w_cat, b_cat, plan, lt, bf16_tables(), impl)
-    agg, att = _EdgeAttention.apply(proj, kvr, plan, lt, d, H, bool(m.keep_att), m.edge_variant, tables16)
+    agg, att = _project_edge(m, x, w_cat, b_cat, plan, lt, impl, bool(m.keep_att))
     _set_att(m, att)
 
     drop = m.training and m.drop.p > 0

@@ -102,6 +102,8 @@ class HGTConv(nn.Module):
     # Class-level switches (kept out of the constructor so the reference's positional call at
     # conv.py:308 stays valid).
     keep_att = True            # materialise self.att [E,H] like the reference (conv.py:108)
+    recompute_tables = False   # training: keep neither Q nor the [K'|V'] table for the backward, which recomputes them
+                               # with the forward's projection GEMM (time for memory; autograd._ProjectEdgeLean)
     edge_variant = 0           # 0 auto, 1 register gather, 2 bulk-copy ring (see csrc/edge.cu)
     linear_impl = 0            # 0 auto, 1 fp32 SIMT, 2 tensor cores (wgmma); 0 / 2 take one bf16 product under
                                # torch.set_float32_matmul_precision("medium") (autograd.bf16_matmuls)

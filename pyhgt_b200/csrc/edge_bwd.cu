@@ -298,6 +298,10 @@ struct RowParams {
   const int32_t* e_pos;      // ATT: per index entry: its CSR position
 };
 
+// grad may be own itself (fp32 tables; the in-place contract of hgt_edge_backward_rows in hgt_b200.h): a row is read
+// only by its owning warp, before that warp's one store of it, or by the pieces of a split row, which store to
+// `partial`.  Neither pointer is __restrict__, so own stays on coherent loads (no ld.global.nc).
+
 // ATT: D holds D_i + C_i (destination pass) and datt_e is read at the entry's CSR position.
 template <class KV, int VEC, int NCH, bool ATT>
 __global__ void __launch_bounds__(kWarps * 32)

@@ -340,7 +340,8 @@ class GraphedTrainStep(_Graphed):
     tensor (the schedulers fill_ it in place).  Every other hyperparameter is baked into the graph at capture: a later
     call raises RuntimeError if one of them changed (OneCycleLR's default cycle_momentum=True rewrites `betas` every
     step; use cycle_momentum=False).  Dropout draws new masks at every replay.  The deterministic-algorithms
-    flag is frozen at the first call: a later call with the flag changed raises RuntimeError.  A batch that does not fit
+    flag and the `recompute_tables` switch of the layers that own `params` are frozen at the first call: a later call
+    with one of them changed raises RuntimeError.  A batch that does not fit
     the signature raises ValueError before anything is copied."""
 
     def __init__(self, loss_fn, sig, device, optimizer=None, clip_norm=None, targets=None, params=None):
@@ -369,6 +370,7 @@ class GraphedTrainStep(_Graphed):
         self.y = {t: torch.full((sig.type_counts[t],) + shape, fill, dtype=dtype, device=self.dev)
                   for t, (shape, dtype, fill) in spec.items()}
         self.det = None
+        self.recompute = None
         self.hyper = None
         self.out = None
         self.capture_failed = False
@@ -441,6 +443,9 @@ class GraphedTrainStep(_Graphed):
         if self.graph is not None and det != self.det:
             raise RuntimeError("GraphedTrainStep was captured with torch deterministic algorithms %s: the flag cannot "
                                "change afterwards" % ("on" if self.det else "off"))
+        if self.graph is not None and any(bool(m.recompute_tables) != v for m, v in self.recompute.items()):
+            raise RuntimeError("a layer's recompute_tables changed after the GraphedTrainStep was captured: the graph "
+                               "holds the backward of the switch as it was at the first call")
         if self.graph is not None:
             hyper = self._hyperparameters()
             if hyper != self.hyper:
@@ -460,6 +465,8 @@ class GraphedTrainStep(_Graphed):
             if self.graph is None:
                 self.det = det
                 self._first_call()
+                from .autograd import recompute_switches
+                self.recompute = recompute_switches(self.params)
                 self.hyper = self._hyperparameters()
             else:
                 self.graph.replay()
