@@ -568,6 +568,50 @@ int hgt_update_epilogue_dst(const float* o, const float* x, const int32_t* type_
 
 
 /* ------------------------------------------------------------------------------------------------
+ * Fused dropout: training dropout drawn inside the kernels, nothing stored.
+ *
+ * Mask contract.  Element (row, col) of an [N, d] tensor is kept iff word (col % 4) of
+ *     Philox4x32-10(counter = (q_lo32, q_hi32, 0, 0), key = (seed_lo32, seed_hi32)),   q = row * ceil(d / 4) + col / 4
+ * is >= thr, thr = (uint32)((double)p * 2^32) with p the fp32 value passed.  `row` is the kernel's rank-order row (never
+ * perm[row]); `seed` is ONE 64-bit value read from DEVICE memory by the kernel (no host read-back, so a captured CUDA
+ * graph draws new masks whenever the seed buffer is rewritten).  Philox4x32-10 is the raw ten-round block function
+ * (curand_Philox4x32_10): no generator state, no curand_init.  Kept values are multiplied by s = 1 / (1 - p) in fp32;
+ * p >= 1 drops every element (s = 0); p <= 0 is refused.  The mask therefore depends on (seed, row, col, d, p) alone: not
+ * on the launch geometry, the vector or scalar kernel instance, perm / type_active, or the deterministic twin.  A
+ * backward kernel given the same (seed, p) regenerates the forward's mask bit for bit.
+ *
+ * hgt_update_epilogue_drop: hgt_update_epilogue with o <- o * mask * s applied as the row is loaded.  Rows that are not
+ *   written (type_active, perm < 0) or are written as zeros (unknown type) draw nothing.  There is no type_dst form (that
+ *   table belongs to inference).  out_hi / out_lo as in hgt_update_epilogue.
+ * hgt_update_backward_drop[_det]: hgt_update_backward[_det] for that forward.  `o` is the PRE-dropout tensor the forward
+ *   read; the kernels use o * mask * s wherever the plain ones use o (LayerNorm recompute, d skip) and store
+ *   d o * mask * s.  The _det form takes the workspace of hgt_update_backward_det_workspace_bytes.
+ * hgt_tanh_dropout: out = tanh(x) * mask * s over the first n_rows of [n_total, d]; rows past n_rows (nodes of unknown
+ *   type) are copied unchanged.  out may alias x.
+ * hgt_tanh_dropout_bwd: d_x = dout * mask * s * (1 - tanh(x)^2) from `out` alone (where the mask is 1, tanh(x) = out / s;
+ *   elsewhere the gradient is 0); rows past n_rows: d_x = dout.  d_x may alias dout.
+ * ---------------------------------------------------------------------------------------------- */
+int hgt_update_epilogue_drop(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
+                             const float* skip, const float* norm_w, const float* norm_b, const int32_t* perm,
+                             const int32_t* type_active, int64_t n_nodes, int32_t d, float* out, void* out_hi,
+                             void* out_lo, const uint64_t* seed, float p, void* stream);
+int hgt_update_backward_drop(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                             int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                             const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
+                             float* d_skip, float* d_norm_w, float* d_norm_b, const uint64_t* seed, float p,
+                             void* stream);
+int hgt_update_backward_drop_det(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                                 int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                                 const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
+                                 float* d_skip, float* d_norm_w, float* d_norm_b, void* workspace,
+                                 size_t workspace_bytes, const uint64_t* seed, float p, void* stream);
+int hgt_tanh_dropout(const float* x, int64_t n_rows, int64_t n_total, int32_t d, const uint64_t* seed, float p,
+                     float* out, void* stream);
+int hgt_tanh_dropout_bwd(const float* dout, const float* out, int64_t n_rows, int64_t n_total, int32_t d,
+                         const uint64_t* seed, float p, float* d_x, void* stream);
+
+
+/* ------------------------------------------------------------------------------------------------
  * Whole layer in one call (inference): HGTConv.forward, pyHGT/conv.py:56-134.
  * Every pointer below is a DEVICE pointer except the h_* tables (host copies of the typed-linear group tables, used
  * only to size grids).  Parameter pointer tables (wq ... norm_b) are device arrays of num_types device pointers, one

@@ -16,6 +16,7 @@ _p = _c.c_void_p
 _i32 = _c.c_int32
 _i64 = _c.c_int64
 _sz = _c.c_size_t
+_f32 = _c.c_float
 
 # name -> argtypes; every function returns int except where noted.  Mirrors include/hgt_b200.h.
 SIGNATURES = {
@@ -126,6 +127,13 @@ SIGNATURES = {
                                 _p, _p, _p, _sz, _p],
     "hgt_plan_range_tiles": [_p, _i64, _i64, _p, _i32, _i64, _i32, _i32, _p, _i64, _p, _i64, _p, _p, _sz, _p],
     "hgt_plan_mask_rows": [_p, _p, _p, _i32, _i64, _i32, _p, _p],
+    # fused dropout (HGTConv.fused_dropout / GNN.fused_dropout): the plain twins' arguments + (seed, p) before the stream
+    "hgt_update_epilogue_drop": [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p, _f32, _p],
+    "hgt_update_backward_drop": [_p, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _f32, _p],
+    "hgt_update_backward_drop_det": [_p, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _sz, _p,
+                                     _f32, _p],
+    "hgt_tanh_dropout": [_p, _i64, _i64, _i32, _p, _f32, _p, _p],
+    "hgt_tanh_dropout_bwd": [_p, _p, _i64, _i64, _i32, _p, _f32, _p, _p],
 }
 
 class ConvArgs(ctypes.Structure):

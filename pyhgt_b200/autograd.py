@@ -24,6 +24,12 @@ source-major second pass that owns every K'/V' and RTE gradient row, plan.source
 hgt_update_backward_det and hgt_fold_backward_det.  They use no float atomics, so two identical steps give bitwise equal
 gradients.  With the flag off nothing changes.
 
+With ``HGTConv.fused_dropout`` (and ``GNN.fused_dropout`` for the input adapter) training dropout is drawn inside the
+update kernels instead of by ``nn.Dropout``: _UpdateEpilogue takes (seed, p), hgt_update_epilogue_drop scales ``o`` by a
+counter-based mask as it loads the row, and hgt_update_backward_drop[_det] regenerates the mask from the saved one-element
+seed tensor.  The saved ``o`` is the pre-dropout tensor; no mask and no dropped copy exist.  The masks are a different
+random stream from ``nn.Dropout``'s, which is why the switch is off by default (mask contract: include/hgt_b200.h).
+
 Under ``torch.autocast("cuda", dtype=torch.bfloat16)`` (bf16_tables()) the two gathered tables, [K'|V'] and the RTE table
 KVR, are stored in bf16: the projection writes Q by its own fp32 call and the K'/V' blocks straight into the bf16 table
 (hgt_typed_linear[_presplit]_bf16, rounded once from the fp32 accumulator), and the edge kernels read them through their
@@ -48,6 +54,17 @@ from . import plan as _plan
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
+
+
+def fused_drop_p(m):
+    """Drop probability of module `m` (a layer or the GNN) when its dropout is drawn inside the kernels, else 0."""
+    return float(m.drop.p) if (m.training and m.drop.p > 0 and m.fused_dropout) else 0.0
+
+
+def drop_seed(dev):
+    """One 64-bit Philox key for one dropout site of one forward, drawn on the device from torch's CUDA generator: it
+    follows torch.manual_seed, needs no host read-back, and inside a CUDA graph every replay draws a new one."""
+    return torch.randint(0, 2 ** 62, (1,), dtype=torch.int64, device=dev)
 
 
 # layers whose .att is still a node of the last training step's autograd graph (it keeps that graph alive)
@@ -501,27 +518,31 @@ class _FoldWeights(torch.autograd.Function):
 class _UpdateEpilogue(torch.autograd.Function):
     """out[perm[k]] = LayerNorm_t(o[k] * sigmoid(skip[t]) + x[k] * (1 - sigmoid(skip[t])))   (conv.py:129-133);
     skip=None: the plain residual o + x of DenseHGTConv (conv.py:261,273).  type_row0: [T+2] int32 row prefix (rows past
-    type_row0[T] are written as zeros), perm: rank-order row -> output row, or None."""
+    type_row0[T] are written as zeros), perm: rank-order row -> output row, or None.  seed (one int64 on the device) with
+    p > 0: `o` is the pre-dropout tensor and the kernels apply the mask of (seed, p) (fused dropout)."""
 
     @staticmethod
-    def forward(ctx, o, x, skip, norm_w, norm_b, type_row0, T, perm, type_active=None):
+    def forward(ctx, o, x, skip, norm_w, norm_b, type_row0, T, perm, type_active=None, seed=None, p=0.0):
         N, d = o.shape
         o, x = o.contiguous(), x.contiguous()
         # with type_active (sharded training, trimmed layers) the rows past the active prefix of a type have no output
         # row: they are zero (never an uninitialised row a later stage could read) and receive no gradient
         # (hgt_update_backward skips them)
         out = (torch.zeros if type_active is not None else torch.empty)((N, d), dtype=torch.float32, device=o.device)
-        _lib.call("hgt_update_epilogue", o.data_ptr(), x.data_ptr(), type_row0.data_ptr(), T, _lib.ptr(skip),
-                  _lib.ptr(norm_w), _lib.ptr(norm_b), _lib.ptr(perm), _lib.ptr(type_active), N, d, out.data_ptr(), None,
-                  None, _stream())
-        ctx.T, ctx.has_norm, ctx.has_skip = T, norm_w is not None, skip is not None
+        args = (o.data_ptr(), x.data_ptr(), type_row0.data_ptr(), T, _lib.ptr(skip), _lib.ptr(norm_w), _lib.ptr(norm_b),
+                _lib.ptr(perm), _lib.ptr(type_active), N, d, out.data_ptr(), None, None)
+        if seed is not None:
+            _lib.call("hgt_update_epilogue_drop", *args, seed.data_ptr(), p, _stream())
+        else:
+            _lib.call("hgt_update_epilogue", *args, _stream())
+        ctx.T, ctx.has_norm, ctx.has_skip, ctx.p = T, norm_w is not None, skip is not None, p
         ctx.det = torch.are_deterministic_algorithms_enabled()
-        ctx.save_for_backward(o, x, skip, norm_w, type_row0, perm, type_active)
+        ctx.save_for_backward(o, x, skip, norm_w, type_row0, perm, type_active, seed)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        o, x, skip, norm_w, type_row0, perm, type_active = ctx.saved_tensors
+        o, x, skip, norm_w, type_row0, perm, type_active, seed = ctx.saved_tensors
         T = ctx.T
         N, d = o.shape
         dev = o.device
@@ -533,14 +554,41 @@ class _UpdateEpilogue(torch.autograd.Function):
         args = (dout.data_ptr(), o.data_ptr(), x.data_ptr(), type_row0.data_ptr(), T, _lib.ptr(skip), _lib.ptr(norm_w),
                 _lib.ptr(perm), _lib.ptr(type_active), N, d, d_o.data_ptr(), d_x.data_ptr(), _lib.ptr(d_skip),
                 _lib.ptr(d_nw), _lib.ptr(d_nb))
+        drop = () if seed is None else (seed.data_ptr(), ctx.p)
+        sfx = "" if seed is None else "_drop"
         if ctx.det:
             wsb = ctypes.c_size_t()
             _lib.call("hgt_update_backward_det_workspace_bytes", N, T, d, ctypes.byref(wsb))
             ws = torch.empty(wsb.value, dtype=torch.uint8, device=dev)
-            _lib.call("hgt_update_backward_det", *args, ws.data_ptr(), ws.numel(), _stream())
+            _lib.call("hgt_update_backward%s_det" % sfx, *args, ws.data_ptr(), ws.numel(), *drop, _stream())
         else:
-            _lib.call("hgt_update_backward", *args, _stream())
-        return d_o, d_x, d_skip, d_nw, d_nb, None, None, None, None
+            _lib.call("hgt_update_backward" + sfx, *args, *drop, _stream())
+        return d_o, d_x, d_skip, d_nw, d_nb, None, None, None, None, None, None
+
+
+class _TanhDropout(torch.autograd.Function):
+    """out = tanh(x) * mask * s over the first n_rows of x [N, d], the remaining rows unchanged (hgt_tanh_dropout): the GNN
+    adapter's tanh and dropout as one pass that keeps `out` alone for the backward."""
+
+    @staticmethod
+    def forward(ctx, x, n_rows, seed, p):
+        x = x.contiguous()
+        N, d = x.shape
+        out = torch.empty_like(x)
+        _lib.call("hgt_tanh_dropout", x.data_ptr(), n_rows, N, d, seed.data_ptr(), p, out.data_ptr(), _stream())
+        ctx.n_rows, ctx.p = n_rows, p
+        ctx.save_for_backward(out, seed)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        out, seed = ctx.saved_tensors
+        N, d = out.shape
+        dout = dout.contiguous()
+        d_x = torch.empty_like(out)
+        _lib.call("hgt_tanh_dropout_bwd", dout.data_ptr(), out.data_ptr(), ctx.n_rows, N, d, seed.data_ptr(), ctx.p,
+                  d_x.data_ptr(), _stream())
+        return d_x, None, None, None
 
 
 def typed_linear(a, w_cat, b_cat, table, width, out_elems, impl=0, act=0, zero_ranges=(), tables16=None):
@@ -597,6 +645,16 @@ def recompute_switches(params):
     return {m: bool(m.recompute_tables) for m in list(_TRAINED_LAYERS) if any(id(p) in owned for p in m.parameters())}
 
 
+# modules with a dropout site (layers, GNN) that ran a training forward: GraphedTrainStep freezes their fused_dropout
+_DROPOUT_MODULES = weakref.WeakSet()
+
+
+def fused_dropout_switches(params):
+    """{module: bool(fused_dropout)} of the layers / GNNs that ran a training forward and own one of `params`."""
+    owned = {id(p) for p in params}
+    return {m: bool(m.fused_dropout) for m in list(_DROPOUT_MODULES) if any(id(p) in owned for p in m.parameters())}
+
+
 def _project_edge(m, x, w_cat, b_cat, plan, lt, impl, want_att):
     """Typed projections and edge attention of a layer: (agg, att).  m.recompute_tables, read here once per training
     forward, selects _ProjectEdgeLean (the backward rebuilds the projection tables); otherwise the projection buffer is
@@ -605,6 +663,7 @@ def _project_edge(m, x, w_cat, b_cat, plan, lt, impl, want_att):
     bf16 = bf16_tables()
     if torch.is_grad_enabled():
         _TRAINED_LAYERS.add(m)
+        _DROPOUT_MODULES.add(m)
         if m.recompute_tables:
             kvr, kvr16 = _rte_tables(m, w_cat, plan, lt, bf16)
             return _ProjectEdgeLean.apply(x, w_cat, b_cat, kvr, plan, lt, d, H, want_att, m.edge_variant, impl, bf16,
@@ -649,14 +708,16 @@ def hgt_conv_autograd(m, node_inp, node_type, edge_index, edge_type, edge_time, 
     wa_cat = torch.cat([l.weight for l in m.a_linears], 0)
     ba_cat = torch.cat([l.bias for l in m.a_linears], 0)
     o = typed_linear(agg, wa_cat, ba_cat, lt.upd_groups, d, N * d, impl, 1).view(N, d)
-    if m.training and m.drop.p > 0:
+    p_fused = fused_drop_p(m)                                                    # conv.py:125, inside the update kernels
+    if m.training and m.drop.p > 0 and not p_fused:
         o = m.drop(o)                                                            # conv.py:125
 
     # 4. gated skip + LayerNorm, written in original node order; rows of unknown type stay zero (conv.py:120)
     norm_w = torch.stack([n.weight for n in m.norms]) if m.use_norm else None
     norm_b = torch.stack([n.bias for n in m.norms]) if m.use_norm else None
     return _UpdateEpilogue.apply(o, x, m.skip, norm_w, norm_b, plan.type_row0_dev, T,
-                                 None if plan.sorted_types else plan.perm, lt.type_active_dev)
+                                 None if plan.sorted_types else plan.perm, lt.type_active_dev,
+                                 drop_seed(o.device) if p_fused else None, p_fused)
 
 
 def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
@@ -683,7 +744,8 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
     agg, att = _project_edge(m, x, w_cat, b_cat, plan, lt, impl, bool(m.keep_att))
     _set_att(m, att)
 
-    drop = m.training and m.drop.p > 0
+    p_fused = fused_drop_p(m)
+    drop = m.training and m.drop.p > 0 and not p_fused
     wa_cat = torch.cat([l.weight for l in m.a_linears], 0)
     ba_cat = torch.cat([l.bias for l in m.a_linears], 0)
     o = typed_linear(agg, wa_cat, ba_cat, lt.upd_groups, d, N * d, impl, 0).view(N, d)              # conv.py:261
@@ -691,7 +753,8 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
         o = m.drop(o)
     norm_w = torch.stack([n.weight for n in m.norms]) if m.use_norm else None
     norm_b = torch.stack([n.bias for n in m.norms]) if m.use_norm else None
-    y = _UpdateEpilogue.apply(o, x, None, norm_w, norm_b, plan.type_row0_dev, T, None)              # rank order
+    y = _UpdateEpilogue.apply(o, x, None, norm_w, norm_b, plan.type_row0_dev, T, None, None,
+                              drop_seed(dev) if p_fused else None, p_fused)                        # rank order
 
     n_known = plan.type_row0[T]
     key = ("dense_ffn", d)
@@ -708,4 +771,5 @@ def dense_hgt_forward(m, node_inp, node_type, edge_index, edge_type, edge_time):
         z = m.drop(z)
     # shared out_norm over every known row, residual with y, written in original node order; unknown types -> zeros
     return _UpdateEpilogue.apply(z, y, None, m.out_norm.weight.view(1, d), m.out_norm.bias.view(1, d), tabs[2], 1,
-                                 None if plan.sorted_types else plan.perm)
+                                 None if plan.sorted_types else plan.perm, None,
+                                 drop_seed(dev) if p_fused else None, p_fused)

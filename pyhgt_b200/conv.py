@@ -104,6 +104,9 @@ class HGTConv(nn.Module):
     keep_att = True            # materialise self.att [E,H] like the reference (conv.py:108)
     recompute_tables = False   # training: keep neither Q nor the [K'|V'] table for the backward, which recomputes them
                                # with the forward's projection GEMM (time for memory; autograd._ProjectEdgeLean)
+    fused_dropout = False      # training: draw dropout inside the update kernels (counter-based masks regenerated in the
+                               # backward, nothing stored) instead of nn.Dropout.  Off by default because the masks are
+                               # another random stream: a run seeded with torch.manual_seed keeps its nn.Dropout masks
     edge_variant = 0           # 0 auto, 1 register gather, 2 bulk-copy ring (see csrc/edge.cu)
     linear_impl = 0            # 0 auto, 1 fp32 SIMT, 2 tensor cores (wgmma); 0 / 2 take one bf16 product under
                                # torch.set_float32_matmul_precision("medium") (autograd.bf16_matmuls)
@@ -345,7 +348,7 @@ class HGTConv(nn.Module):
         A whole-graph inference forward computes Q, the edge pass and the a_linear only over each type's destination
         extent (plan.GraphPlan.dst_extent): the rows past it have no in-edges, so their a_linear output is exactly the
         bias, which the update epilogue reads instead.  Not with dropout on `o`, which would have to touch those rows."""
-        from .autograd import bf16_matmuls, bf16_tables, gemm_impl
+        from .autograd import bf16_matmuls, bf16_tables, drop_seed, fused_drop_p, gemm_impl
         bf16 = bf16_tables()
         impl = gemm_impl(self.linear_impl, bf16_matmuls())
         dst = (not save and active_per_type is None and kv_runs is None and out_map is None and plan is None
@@ -373,8 +376,14 @@ class HGTConv(nn.Module):
                 and not self.training):
             o_hi = torch.empty((N, d), dtype=torch.bfloat16, device=o.device)
             o_lo = None if impl == 3 else torch.empty((N, d), dtype=torch.bfloat16, device=o.device)
+        p_fused = fused_drop_p(self)
         with self._stage("update_epilogue"):
-            if lt.type_dst_dev is not None:
+            if p_fused:                                           # train mode under no_grad: `o` is still undropped
+                _lib.call("hgt_update_epilogue_drop", o.data_ptr(), x_sorted.data_ptr(), plan.type_row0_dev.data_ptr(),
+                          T, self.skip.data_ptr(), _lib.ptr(norm_w), _lib.ptr(norm_b), perm_ptr,
+                          _lib.ptr(lt.type_active_dev), N, d, out.data_ptr(), _lib.ptr(o_hi), _lib.ptr(o_lo),
+                          drop_seed(o.device).data_ptr(), p_fused, st)
+            elif lt.type_dst_dev is not None:
                 _lib.call("hgt_update_epilogue_dst", o.data_ptr(), x_sorted.data_ptr(), plan.type_row0_dev.data_ptr(), T,
                           self.skip.data_ptr(), _lib.ptr(norm_w), _lib.ptr(norm_b), perm_ptr, lt.type_dst_dev.data_ptr(),
                           c["ba_cat"].data_ptr(), N, d, out.data_ptr(), _lib.ptr(o_hi), _lib.ptr(o_lo), st)
@@ -527,8 +536,8 @@ class HGTConv(nn.Module):
                           o.data_ptr(), ws2.data_ptr(), ws2.numel(), st)
             else:
                 self._typed_linear(g_act, d, wa_cat, ba_cat, d, d, lt.upd_groups, o, impl, st)
-        if self.training and self.drop.p > 0:
-            o = self.drop(o)                                       # conv.py:125 (train mode only)
+        if self.training and self.drop.p > 0 and not self.fused_dropout:
+            o = self.drop(o)                       # conv.py:125 (train mode only; fused_dropout: in the update epilogue)
         return dict(plan=plan, lt=lt, x_sorted=x_sorted, w_cat=w_cat, proj=proj, q=q_tab, kv=kv_tab, kvr=kvr, agg=agg, o=o, stats=stats,
                     att=att, N=N, d=d, T=T, st=st, ba_cat=ba_cat)
 

@@ -12,7 +12,7 @@ int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type
                              const float* skip, const float* norm_w, const float* norm_b, const float* const* norm_wp,
                              const float* const* norm_bp, const int32_t* perm, const int32_t* type_active,
                              const int32_t* type_dst, const float* bias, int64_t n_nodes, int32_t d, float* out,
-                             void* out_hi, void* out_lo, cudaStream_t st);
+                             void* out_hi, void* out_lo, const uint64_t* seed, float p, cudaStream_t st);
 bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width);
 
 namespace {
@@ -161,5 +161,5 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
   return hgt_update_epilogue_impl(L.o, x_sorted, a->type_row0, T, a->skip, nullptr, nullptr,
                                   a->use_norm ? a->norm_w : nullptr, a->use_norm ? a->norm_b : nullptr, perm_out,
                                   a->type_active, a->type_dst, a->type_dst ? L.ba_cat : nullptr, N, d, a->out, a->out_hi,
-                                  a->out_lo, st);
+                                  a->out_lo, nullptr, 0.f, st);
 }

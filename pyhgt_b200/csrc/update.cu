@@ -1,6 +1,9 @@
 // HGTConv.update epilogue (conv.py:129-133): sigmoid(skip)-gated residual + per-type LayerNorm.
 // One warp per node row; the row (d <= 1024 floats) stays in registers between the two LayerNorm passes.
 // HBM-bound: reads o and x (2*d*4 B), writes out (d*4 B) per node.
+// DROP instances (hgt_update_epilogue_drop) scale `o` by a counter-based dropout mask as the row is loaded; the mask is a
+// function of (seed, row, column) alone (hgt_b200.h, "Fused dropout"), so nothing is stored for the backward.
+// hgt_tanh_dropout[_bwd] is the same mask behind the GNN adapter's tanh.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -9,13 +12,15 @@ namespace {
 
 constexpr int kMaxPerLane = 32;   // d <= 1024
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 k_update_epilogue(const float* __restrict__ o, const float* __restrict__ x, const int32_t* __restrict__ type_row0,
                   int T, const float* __restrict__ skip, const float* __restrict__ norm_w,
                   const float* __restrict__ norm_b, const float* const* __restrict__ norm_wp,
                   const float* const* __restrict__ norm_bp, const int32_t* __restrict__ perm,
                   const int32_t* __restrict__ type_active, const int32_t* __restrict__ type_dst,
-                  const float* __restrict__ bias, int64_t n_nodes, int d, float* __restrict__ out) {
+                  const float* __restrict__ bias, int64_t n_nodes, int d, float* __restrict__ out,
+                  const uint64_t* __restrict__ seed, uint32_t thr, float scale) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   if (row >= n_nodes) return;
@@ -35,13 +40,17 @@ k_update_epilogue(const float* __restrict__ o, const float* __restrict__ x, cons
   // rows past type_dst[t] have no in-edges: their a_linear output is exactly the bias, and their `o` row was not written
   const float* op = (type_dst && row - type_row0[t] >= type_dst[t]) ? bias + (int64_t)t * d : o + row * d;
   const float* xp = x + row * d;
+  uint32_t kept = 0;
+  if constexpr (DROP) kept = hgt_drop_row_bits<kMaxPerLane>(hgt_drop_key(seed), row, d, thr, lane);
   float y[kMaxPerLane];
   float sum = 0.f;
 #pragma unroll
   for (int i = 0; i < kMaxPerLane; ++i) {
     int c = lane + i * 32;
     if (c < d) {
-      y[i] = op[c] * alpha + xp[c] * beta;                 // conv.py:131,133
+      float ov = op[c];
+      if constexpr (DROP) ov = hgt_drop_apply(ov, (kept >> i) & 1u, scale);
+      y[i] = ov * alpha + xp[c] * beta;                    // conv.py:131,133
       sum += y[i];
     } else {
       y[i] = 0.f;
@@ -91,7 +100,7 @@ __device__ __forceinline__ void split_store(uint2* hi, uint2* lo, int64_t idx, c
 }
 
 // Vectorised variant: d % 4 == 0, each lane owns NV float4 chunks (chunk c = lane + 32*i), 128-bit loads/stores.
-template <int NV>
+template <int NV, bool DROP>
 __global__ void __launch_bounds__(256)
 k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, const int32_t* __restrict__ type_row0,
                       int T, const float* __restrict__ skip, const float* __restrict__ norm_w,
@@ -99,7 +108,8 @@ k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, 
                       const float* const* __restrict__ norm_bp, const int32_t* __restrict__ perm,
                       const int32_t* __restrict__ type_active, const int32_t* __restrict__ type_dst,
                       const float* __restrict__ bias, int64_t n_nodes, int d, float* __restrict__ out,
-                      uint2* __restrict__ out_hi, uint2* __restrict__ out_lo) {
+                      uint2* __restrict__ out_hi, uint2* __restrict__ out_lo, const uint64_t* __restrict__ seed,
+                      uint32_t thr, float scale) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   if (row >= n_nodes) return;
@@ -149,6 +159,20 @@ k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, 
   }
   const float alpha = skip ? 1.0f / (1.0f + __expf(-skip[t])) : 1.0f;
   const float beta = skip ? 1.0f - alpha : 1.0f;
+  if constexpr (DROP) {                          // rows that left above drew nothing
+    const uint2 key = hgt_drop_key(seed);
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const int c = lane + 32 * i;
+      if (c < nvec) {
+        const uint32_t kept = hgt_drop_keep4(key, (uint64_t)row * nvec + c, thr);
+        ov[i].x = hgt_drop_apply(ov[i].x, kept & 1u, scale);
+        ov[i].y = hgt_drop_apply(ov[i].y, kept & 2u, scale);
+        ov[i].z = hgt_drop_apply(ov[i].z, kept & 4u, scale);
+        ov[i].w = hgt_drop_apply(ov[i].w, kept & 8u, scale);
+      }
+    }
+  }
   float4 y[NV];
   float sum = 0.f;
 #pragma unroll
@@ -213,16 +237,17 @@ k_update_epilogue_vec(const float* __restrict__ o, const float* __restrict__ x, 
   }
 }
 
-template <int NV>
+template <int NV, bool DROP>
 void launch_vec(const float* o, const float* x, const int32_t* type_row0, int T, const float* skip,
                 const float* norm_w, const float* norm_b, const float* const* norm_wp, const float* const* norm_bp,
                 const int32_t* perm, const int32_t* type_active, const int32_t* type_dst, const float* bias,
-                int64_t n_nodes, int d, float* out, uint2* out_hi, uint2* out_lo, cudaStream_t st) {
+                int64_t n_nodes, int d, float* out, uint2* out_hi, uint2* out_lo, const uint64_t* seed, HgtDrop dp,
+                cudaStream_t st) {
   const int warps_per_block = 8;
   unsigned grid = (unsigned)((n_nodes + warps_per_block - 1) / warps_per_block);
-  k_update_epilogue_vec<NV><<<grid, warps_per_block * 32, 0, st>>>(o, x, type_row0, T, skip, norm_w, norm_b, norm_wp,
-                                                                  norm_bp, perm, type_active, type_dst, bias, n_nodes,
-                                                                  d, out, out_hi, out_lo);
+  k_update_epilogue_vec<NV, DROP><<<grid, warps_per_block * 32, 0, st>>>(
+      o, x, type_row0, T, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out,
+      out_hi, out_lo, seed, dp.thr, dp.scale);
 }
 
 }  // namespace
@@ -231,7 +256,9 @@ int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type
                              const float* skip, const float* norm_w, const float* norm_b, const float* const* norm_wp,
                              const float* const* norm_bp, const int32_t* perm, const int32_t* type_active,
                              const int32_t* type_dst, const float* bias, int64_t n_nodes, int32_t d, float* out,
-                             void* out_hi, void* out_lo, cudaStream_t st) {
+                             void* out_hi, void* out_lo, const uint64_t* seed, float p, cudaStream_t st) {
+  HGT_REQUIRE(seed == nullptr || (type_dst == nullptr && p > 0.f),
+              "hgt_update_epilogue_drop: dropout needs p > 0 and excludes type_dst (an inference-only table)");
   HGT_REQUIRE(type_dst == nullptr || (bias != nullptr && type_active == nullptr),
               "hgt_update_epilogue: type_dst needs the a_linear bias and excludes type_active");
   HGT_REQUIRE(d >= 1 && d <= 32 * kMaxPerLane, "hgt_update_epilogue: d=%d unsupported (max %d)", d,
@@ -250,19 +277,34 @@ int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type
               "hgt_update_epilogue: the split output needs d %% 8 == 0, 16-byte aligned buffers and identity row order");
   uint2* hi2 = reinterpret_cast<uint2*>(out_hi);
   uint2* lo2 = reinterpret_cast<uint2*>(out_lo);
+  const HgtDrop dp = seed ? hgt_drop_params(p) : HgtDrop{0u, 1.f, 1.f};
   if (aligned && d <= 1024) {
     const int nv = (d / 4 + 31) / 32;
-    if (nv <= 1) launch_vec<1>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
-    else if (nv <= 2) launch_vec<2>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
-    else if (nv <= 4) launch_vec<4>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
-    else launch_vec<8>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out, hi2, lo2, st);
+#define HGT_UE(NV)                                                                                                      \
+  do {                                                                                                                  \
+    if (seed) launch_vec<NV, true>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active, \
+                                   type_dst, bias, n_nodes, d, out, hi2, lo2, seed, dp, st);                             \
+    else launch_vec<NV, false>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp, norm_bp, perm, type_active,    \
+                               type_dst, bias, n_nodes, d, out, hi2, lo2, seed, dp, st);                                 \
+  } while (0)
+    if (nv <= 1) HGT_UE(1);
+    else if (nv <= 2) HGT_UE(2);
+    else if (nv <= 4) HGT_UE(4);
+    else HGT_UE(8);
+#undef HGT_UE
     HGT_LAUNCH_CHECK();
     return 0;
   }
   const int warps_per_block = 8;
   unsigned grid = (unsigned)((n_nodes + warps_per_block - 1) / warps_per_block);
-  k_update_epilogue<<<grid, warps_per_block * 32, 0, st>>>(o, x, type_row0, num_types, skip, norm_w, norm_b, norm_wp,
-                                                           norm_bp, perm, type_active, type_dst, bias, n_nodes, d, out);
+  if (seed)
+    k_update_epilogue<true><<<grid, warps_per_block * 32, 0, st>>>(o, x, type_row0, num_types, skip, norm_w, norm_b,
+                                                                   norm_wp, norm_bp, perm, type_active, type_dst, bias,
+                                                                   n_nodes, d, out, seed, dp.thr, dp.scale);
+  else
+    k_update_epilogue<false><<<grid, warps_per_block * 32, 0, st>>>(o, x, type_row0, num_types, skip, norm_w, norm_b,
+                                                                    norm_wp, norm_bp, perm, type_active, type_dst, bias,
+                                                                    n_nodes, d, out, seed, dp.thr, dp.scale);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -272,7 +314,8 @@ extern "C" int hgt_update_epilogue(const float* o, const float* x, const int32_t
                                    const int32_t* perm, const int32_t* type_active, int64_t n_nodes, int32_t d,
                                    float* out, void* out_hi, void* out_lo, void* stream_) {
   return hgt_update_epilogue_impl(o, x, type_row0, num_types, skip, norm_w, norm_b, nullptr, nullptr, perm,
-                                  type_active, nullptr, nullptr, n_nodes, d, out, out_hi, out_lo, (cudaStream_t)stream_);
+                                  type_active, nullptr, nullptr, n_nodes, d, out, out_hi, out_lo, nullptr, 0.f,
+                                  (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_update_epilogue_dst(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
@@ -281,5 +324,91 @@ extern "C" int hgt_update_epilogue_dst(const float* o, const float* x, const int
                                        float* out, void* out_hi, void* out_lo, void* stream_) {
   HGT_REQUIRE(type_dst && bias, "hgt_update_epilogue_dst: NULL type_dst / bias");
   return hgt_update_epilogue_impl(o, x, type_row0, num_types, skip, norm_w, norm_b, nullptr, nullptr, perm, nullptr,
-                                  type_dst, bias, n_nodes, d, out, out_hi, out_lo, (cudaStream_t)stream_);
+                                  type_dst, bias, n_nodes, d, out, out_hi, out_lo, nullptr, 0.f, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_update_epilogue_drop(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
+                                        const float* skip, const float* norm_w, const float* norm_b,
+                                        const int32_t* perm, const int32_t* type_active, int64_t n_nodes, int32_t d,
+                                        float* out, void* out_hi, void* out_lo, const uint64_t* seed, float p,
+                                        void* stream_) {
+  HGT_REQUIRE(seed, "hgt_update_epilogue_drop: NULL seed");
+  return hgt_update_epilogue_impl(o, x, type_row0, num_types, skip, norm_w, norm_b, nullptr, nullptr, perm,
+                                  type_active, nullptr, nullptr, n_nodes, d, out, out_hi, out_lo, seed, p,
+                                  (cudaStream_t)stream_);
+}
+
+// ---- tanh + dropout of the GNN input adapter (model.py:75-76) -------------------------------------------------------------
+namespace {
+
+// One thread per 4-column chunk.  VEC: d % 4 == 0 and 16-byte aligned buffers (128-bit accesses); otherwise the chunk's
+// columns go one by one (the last chunk of a row may be short).  BWD: x = dout, y = the forward's output, out = d x.
+template <bool VEC, bool BWD>
+__global__ void __launch_bounds__(256)
+k_tanh_dropout(const float* x, const float* y, int64_t n_rows, int64_t n_total, int d, const uint64_t* __restrict__ seed,
+               uint32_t thr, float scale, float keep, float* out) {
+  const int nchunk = (d + 3) >> 2;
+  const int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (q >= n_total * nchunk) return;
+  const int64_t row = q / nchunk;
+  const int c = (int)(q - row * nchunk);
+  const bool through = row >= n_rows;              // rows of unknown type pass unchanged
+  const uint32_t kept = through ? 0u : hgt_drop_keep4(hgt_drop_key(seed), (uint64_t)q, thr);
+  auto f = [&](float xv, float yv, uint32_t k) {
+    if (through) return xv;
+    if (!BWD) return hgt_drop_apply(tanhf(xv), k, scale);
+    const float th = yv * keep;                    // kept: tanh(x) = out / scale
+    return hgt_drop_apply(xv * (1.0f - th * th), k, scale);
+  };
+  if (VEC) {
+    const float4 xv = __ldcs(reinterpret_cast<const float4*>(x) + q);
+    float4 yv = xv;
+    if (BWD) yv = __ldcs(reinterpret_cast<const float4*>(y) + q);
+    float4 r;
+    r.x = f(xv.x, yv.x, kept & 1u);
+    r.y = f(xv.y, yv.y, kept & 2u);
+    r.z = f(xv.z, yv.z, kept & 4u);
+    r.w = f(xv.w, yv.w, kept & 8u);
+    __stcs(reinterpret_cast<float4*>(out) + q, r);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int col = 4 * c + j;
+      if (col < d) {
+        const int64_t e = row * d + col;
+        out[e] = f(x[e], BWD ? y[e] : 0.f, (kept >> j) & 1u);
+      }
+    }
+  }
+}
+
+template <bool BWD>
+int tanh_dropout_launch(const char* who, const float* x, const float* y, int64_t n_rows, int64_t n_total, int32_t d,
+                        const uint64_t* seed, float p, float* out, cudaStream_t st) {
+  HGT_REQUIRE(x && out && seed && (y || !BWD), "%s: NULL argument", who);
+  HGT_REQUIRE(d >= 1 && n_rows >= 0 && n_rows <= n_total && p > 0.f, "%s: needs d >= 1, 0 <= n_rows <= n_total, p > 0", who);
+  if (n_total == 0) return 0;
+  const HgtDrop dp = hgt_drop_params(p);
+  const int64_t n = n_total * ((d + 3) / 4);
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  const bool vec = d % 4 == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) |
+                                   reinterpret_cast<uintptr_t>(out)) % 16 == 0);
+  if (vec) k_tanh_dropout<true, BWD><<<grid, 256, 0, st>>>(x, y, n_rows, n_total, d, seed, dp.thr, dp.scale, dp.keep, out);
+  else k_tanh_dropout<false, BWD><<<grid, 256, 0, st>>>(x, y, n_rows, n_total, d, seed, dp.thr, dp.scale, dp.keep, out);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int hgt_tanh_dropout(const float* x, int64_t n_rows, int64_t n_total, int32_t d, const uint64_t* seed,
+                                float p, float* out, void* stream_) {
+  return tanh_dropout_launch<false>("hgt_tanh_dropout", x, nullptr, n_rows, n_total, d, seed, p, out,
+                                    (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_tanh_dropout_bwd(const float* dout, const float* out, int64_t n_rows, int64_t n_total, int32_t d,
+                                    const uint64_t* seed, float p, float* d_x, void* stream_) {
+  return tanh_dropout_launch<true>("hgt_tanh_dropout_bwd", dout, out, n_rows, n_total, d, seed, p, d_x,
+                                   (cudaStream_t)stream_);
 }

@@ -5,6 +5,8 @@
 //                         -> d k_linears / v_linears (weight, bias), d relation_att / relation_msg / relation_pri
 // The *_det entry points compute the same gradients without float atomics (torch.use_deterministic_algorithms): every
 // output element has one owner, and partial sums are added in a fixed order.
+// The DROP instances (hgt_update_backward_drop[_det]) take the PRE-dropout `o` and the forward's seed: they regenerate the
+// mask (hgt_b200.h, "Fused dropout"), use o * mask * s wherever the others use o, and store d o * mask * s.
 #include "common.cuh"
 
 namespace {
@@ -16,14 +18,14 @@ namespace {
 constexpr int UB_WARPS = 8;
 constexpr int UB_ROWS_PER_WARP = 16;
 
-template <int NPL>
+template <int NPL, bool DROP>
 __global__ void __launch_bounds__(UB_WARPS * 32)
 k_update_bwd(const float* __restrict__ dout, const float* __restrict__ o, const float* __restrict__ x,
              const int32_t* __restrict__ type_row0, int T, const float* __restrict__ skip,
              const float* __restrict__ norm_w, const int32_t* __restrict__ perm,
              const int32_t* __restrict__ type_active, int64_t n_nodes, int d,
              float* __restrict__ d_o, float* __restrict__ d_x, float* __restrict__ d_skip, float* __restrict__ d_nw,
-             float* __restrict__ d_nb) {
+             float* __restrict__ d_nb, const uint64_t* __restrict__ seed, uint32_t thr, float scale) {
   extern __shared__ float s_red[];                  // [2*d + 1] block-level partial sums (uniform-type blocks)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t block_row0 = (int64_t)blockIdx.x * UB_WARPS * UB_ROWS_PER_WARP;
@@ -77,6 +79,8 @@ k_update_bwd(const float* __restrict__ dout, const float* __restrict__ o, const 
   };
 
   const int64_t w_row0 = block_row0 + (int64_t)warp * UB_ROWS_PER_WARP;
+  uint2 key = make_uint2(0u, 0u);
+  if constexpr (DROP) key = hgt_drop_key(seed);
   for (int rr = 0; rr < UB_ROWS_PER_WARP; ++rr) {
     const int64_t row = w_row0 + rr;
     if (row >= n_nodes) break;
@@ -99,13 +103,17 @@ k_update_bwd(const float* __restrict__ dout, const float* __restrict__ o, const 
     const float* gr = dout + (perm ? (int64_t)perm[row] : row) * d;
     const float* orow = o + row * d;
     const float* xrow = x + row * d;
+    uint32_t kept = 0;
+    if constexpr (DROP) kept = hgt_drop_row_bits<NPL>(key, row, d, thr, lane);
     float y[NPL], g[NPL], df[NPL];
     float sum = 0.f;
 #pragma unroll
     for (int i = 0; i < NPL; ++i) {
       const int c = lane + 32 * i;
       if (c < d) {
-        const float ov = orow[c], xv = xrow[c];
+        float ov = orow[c];
+        const float xv = xrow[c];
+        if constexpr (DROP) ov = hgt_drop_apply(ov, (kept >> i) & 1u, scale);
         g[i] = gr[c];
         df[i] = ov - xv;
         y[i] = ov * a + xv * b1;
@@ -154,7 +162,7 @@ k_update_bwd(const float* __restrict__ dout, const float* __restrict__ o, const 
     for (int i = 0; i < NPL; ++i) {
       const int c = lane + 32 * i;
       if (c < d) {
-        dorow[c] = a * g[i];
+        dorow[c] = DROP ? hgt_drop_apply(a * g[i], (kept >> i) & 1u, scale) : a * g[i];
         dxrow[c] = b1 * g[i];
         acc_a = fmaf(g[i], df[i], acc_a);
       }
@@ -266,13 +274,13 @@ __device__ __forceinline__ int64_t ud_blocks_before(const int32_t* type_row0, in
   return b;
 }
 
-template <int NPL>
+template <int NPL, bool DROP>
 __global__ void __launch_bounds__(UB_WARPS * 32)
 k_update_bwd_det(const float* __restrict__ dout, const float* __restrict__ o, const float* __restrict__ x,
                  const int32_t* __restrict__ type_row0, int T, const float* __restrict__ skip,
                  const float* __restrict__ norm_w, const int32_t* __restrict__ perm,
                  const int32_t* __restrict__ type_active, int d, float* __restrict__ d_o, float* __restrict__ d_x,
-                 float* __restrict__ part) {
+                 float* __restrict__ part, const uint64_t* __restrict__ seed, uint32_t thr, float scale) {
   extern __shared__ float s_red[];                  // [2*d + 1]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int t = 0;
@@ -296,6 +304,8 @@ k_update_bwd_det(const float* __restrict__ dout, const float* __restrict__ o, co
   const float a = (known && skip) ? 1.0f / (1.0f + __expf(-skip[t])) : 1.0f;
   const float b1 = (known && skip) ? 1.0f - a : 1.0f;
   const int64_t w_row0 = block_row0 + (int64_t)warp * UD_ROWS_PER_WARP;
+  uint2 key = make_uint2(0u, 0u);
+  if constexpr (DROP) key = hgt_drop_key(seed);
   for (int rr = 0; rr < UD_ROWS_PER_WARP; ++rr) {
     const int64_t row = w_row0 + rr;
     if (row >= type_end) break;
@@ -312,13 +322,17 @@ k_update_bwd_det(const float* __restrict__ dout, const float* __restrict__ o, co
     const float* gr = dout + (perm ? (int64_t)perm[row] : row) * d;
     const float* orow = o + row * d;
     const float* xrow = x + row * d;
+    uint32_t kept = 0;
+    if constexpr (DROP) kept = hgt_drop_row_bits<NPL>(key, row, d, thr, lane);
     float y[NPL], g[NPL], df[NPL];
     float sum = 0.f;
 #pragma unroll
     for (int i = 0; i < NPL; ++i) {
       const int c = lane + 32 * i;
       if (c < d) {
-        const float ov = orow[c], xv = xrow[c];
+        float ov = orow[c];
+        const float xv = xrow[c];
+        if constexpr (DROP) ov = hgt_drop_apply(ov, (kept >> i) & 1u, scale);
         g[i] = gr[c];
         df[i] = ov - xv;
         y[i] = ov * a + xv * b1;
@@ -367,7 +381,7 @@ k_update_bwd_det(const float* __restrict__ dout, const float* __restrict__ o, co
     for (int i = 0; i < NPL; ++i) {
       const int c = lane + 32 * i;
       if (c < d) {
-        dorow[c] = a * g[i];
+        dorow[c] = DROP ? hgt_drop_apply(a * g[i], (kept >> i) & 1u, scale) : a * g[i];
         dxrow[c] = b1 * g[i];
         acc_a = fmaf(g[i], df[i], acc_a);
       }
@@ -505,24 +519,25 @@ __global__ void k_fold_bwd_pri_det(const float* __restrict__ rel_att, const floa
   if (lane == 0) d_pri[wid] = s * inv;
 }
 
-template <int NPL>
+template <int NPL, bool DROP>
 void launch_update_bwd(const float* dout, const float* o, const float* x, const int32_t* type_row0, int T,
                        const float* skip, const float* norm_w, const int32_t* perm, const int32_t* type_active,
                        int64_t n, int d, float* d_o,
-                       float* d_x, float* d_skip, float* d_nw, float* d_nb, cudaStream_t st) {
+                       float* d_x, float* d_skip, float* d_nw, float* d_nb, const uint64_t* seed, HgtDrop dp,
+                       cudaStream_t st) {
   const int rows_per_block = UB_WARPS * UB_ROWS_PER_WARP;
   const unsigned grid = (unsigned)((n + rows_per_block - 1) / rows_per_block);
-  k_update_bwd<NPL><<<grid, UB_WARPS * 32, (2 * d + 1) * sizeof(float), st>>>(dout, o, x, type_row0, T, skip, norm_w, perm,
-                                                                             type_active, n, d, d_o, d_x, d_skip, d_nw,
-                                                                             d_nb);
+  k_update_bwd<NPL, DROP><<<grid, UB_WARPS * 32, (2 * d + 1) * sizeof(float), st>>>(
+      dout, o, x, type_row0, T, skip, norm_w, perm, type_active, n, d, d_o, d_x, d_skip, d_nw, d_nb, seed, dp.thr, dp.scale);
 }
 
-template <int NPL>
+template <int NPL, bool DROP>
 void launch_update_bwd_det(const float* dout, const float* o, const float* x, const int32_t* type_row0, int T,
                            const float* skip, const float* norm_w, const int32_t* perm, const int32_t* type_active,
-                           unsigned grid, int d, float* d_o, float* d_x, float* part, cudaStream_t st) {
-  k_update_bwd_det<NPL><<<grid, UB_WARPS * 32, (2 * d + 1) * sizeof(float), st>>>(dout, o, x, type_row0, T, skip, norm_w,
-                                                                                 perm, type_active, d, d_o, d_x, part);
+                           unsigned grid, int d, float* d_o, float* d_x, float* part, const uint64_t* seed, HgtDrop dp,
+                           cudaStream_t st) {
+  k_update_bwd_det<NPL, DROP><<<grid, UB_WARPS * 32, (2 * d + 1) * sizeof(float), st>>>(
+      dout, o, x, type_row0, T, skip, norm_w, perm, type_active, d, d_o, d_x, part, seed, dp.thr, dp.scale);
 }
 
 size_t update_det_slots(int64_t n_nodes, int32_t num_types) {
@@ -531,11 +546,13 @@ size_t update_det_slots(int64_t n_nodes, int32_t num_types) {
 
 }  // namespace
 
-extern "C" int hgt_update_backward(const float* dout, const float* o, const float* x, const int32_t* type_row0,
-                                   int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
-                                   const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x, float* d_skip, float* d_norm_w,
-                                   float* d_norm_b, void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+static int update_backward_impl(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                                int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                                const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
+                                float* d_skip, float* d_norm_w, float* d_norm_b, const uint64_t* seed, float p,
+                                cudaStream_t st) {
+  HGT_REQUIRE(!seed || p > 0.f, "hgt_update_backward_drop: dropout needs p > 0");
+  const HgtDrop dp = seed ? hgt_drop_params(p) : HgtDrop{0u, 1.f, 1.f};
   HGT_REQUIRE(dout && o && x && type_row0 && d_o && d_x && (d_skip || !skip), "hgt_update_backward: NULL argument");
   HGT_REQUIRE(d >= 1 && d <= 1024, "hgt_update_backward: d=%d unsupported (max 1024)", d);
   HGT_REQUIRE(!norm_w || (d_norm_w && d_norm_b), "hgt_update_backward: LayerNorm gradients need output buffers");
@@ -546,8 +563,13 @@ extern "C" int hgt_update_backward(const float* dout, const float* o, const floa
   }
   if (n_nodes == 0) return 0;
   const int npl = (d + 31) / 32;
-#define HGT_UB(N) launch_update_bwd<N>(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, n_nodes, d, d_o, d_x, d_skip, \
-                                       d_norm_w, d_norm_b, st)
+#define HGT_UB(N)                                                                                                        \
+  do {                                                                                                                   \
+    if (seed) launch_update_bwd<N, true>(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, n_nodes, d,   \
+                                         d_o, d_x, d_skip, d_norm_w, d_norm_b, seed, dp, st);                            \
+    else launch_update_bwd<N, false>(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, n_nodes, d, d_o,  \
+                                     d_x, d_skip, d_norm_w, d_norm_b, seed, dp, st);                                     \
+  } while (0)
   if (npl <= 2) HGT_UB(2);
   else if (npl <= 4) HGT_UB(4);
   else if (npl <= 8) HGT_UB(8);
@@ -556,6 +578,24 @@ extern "C" int hgt_update_backward(const float* dout, const float* o, const floa
 #undef HGT_UB
   HGT_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int hgt_update_backward(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                                   int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                                   const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x, float* d_skip, float* d_norm_w,
+                                   float* d_norm_b, void* stream_) {
+  return update_backward_impl(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, n_nodes, d, d_o, d_x,
+                              d_skip, d_norm_w, d_norm_b, nullptr, 0.f, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_update_backward_drop(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                                        int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                                        const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
+                                        float* d_skip, float* d_norm_w, float* d_norm_b, const uint64_t* seed, float p,
+                                        void* stream_) {
+  HGT_REQUIRE(seed, "hgt_update_backward_drop: NULL seed");
+  return update_backward_impl(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, n_nodes, d, d_o, d_x,
+                              d_skip, d_norm_w, d_norm_b, seed, p, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_fold_backward(const float* d_w_cat, const float* d_b_cat, const float* const* wk,
@@ -603,12 +643,13 @@ extern "C" int hgt_update_backward_det_workspace_bytes(int64_t n_nodes, int32_t 
   return 0;
 }
 
-extern "C" int hgt_update_backward_det(const float* dout, const float* o, const float* x, const int32_t* type_row0,
-                                       int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
-                                       const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
-                                       float* d_skip, float* d_norm_w, float* d_norm_b, void* workspace,
-                                       size_t workspace_bytes, void* stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+static int update_backward_det_impl(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                                    int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                                    const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
+                                    float* d_skip, float* d_norm_w, float* d_norm_b, void* workspace,
+                                    size_t workspace_bytes, const uint64_t* seed, float p, cudaStream_t st) {
+  HGT_REQUIRE(!seed || p > 0.f, "hgt_update_backward_drop_det: dropout needs p > 0");
+  const HgtDrop dp = seed ? hgt_drop_params(p) : HgtDrop{0u, 1.f, 1.f};
   HGT_REQUIRE(dout && o && x && type_row0 && d_o && d_x && (d_skip || !skip), "hgt_update_backward_det: NULL argument");
   HGT_REQUIRE(d >= 1 && d <= 1024, "hgt_update_backward_det: d=%d unsupported (max 1024)", d);
   HGT_REQUIRE(!norm_w || (d_norm_w && d_norm_b), "hgt_update_backward_det: LayerNorm gradients need output buffers");
@@ -620,8 +661,13 @@ extern "C" int hgt_update_backward_det(const float* dout, const float* o, const 
   if (n_nodes > 0) {
     const unsigned grid = (unsigned)update_det_slots(n_nodes, num_types);
     const int npl = (d + 31) / 32;
-#define HGT_UBD(N) launch_update_bwd_det<N>(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, grid, d, d_o, \
-                                            d_x, part, st)
+#define HGT_UBD(N)                                                                                                       \
+  do {                                                                                                                   \
+    if (seed) launch_update_bwd_det<N, true>(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, grid, d,  \
+                                             d_o, d_x, part, seed, dp, st);                                              \
+    else launch_update_bwd_det<N, false>(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, grid, d, d_o, \
+                                         d_x, part, seed, dp, st);                                                       \
+  } while (0)
     if (npl <= 2) HGT_UBD(2);
     else if (npl <= 4) HGT_UBD(4);
     else if (npl <= 8) HGT_UBD(8);
@@ -638,6 +684,27 @@ extern "C" int hgt_update_backward_det(const float* dout, const float* o, const 
     HGT_LAUNCH_CHECK();
   }
   return 0;
+}
+
+extern "C" int hgt_update_backward_det(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                                       int32_t num_types, const float* skip, const float* norm_w, const int32_t* perm,
+                                       const int32_t* type_active, int64_t n_nodes, int32_t d, float* d_o, float* d_x,
+                                       float* d_skip, float* d_norm_w, float* d_norm_b, void* workspace,
+                                       size_t workspace_bytes, void* stream_) {
+  return update_backward_det_impl(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, n_nodes, d, d_o, d_x,
+                                  d_skip, d_norm_w, d_norm_b, workspace, workspace_bytes, nullptr, 0.f,
+                                  (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_update_backward_drop_det(const float* dout, const float* o, const float* x, const int32_t* type_row0,
+                                            int32_t num_types, const float* skip, const float* norm_w,
+                                            const int32_t* perm, const int32_t* type_active, int64_t n_nodes, int32_t d,
+                                            float* d_o, float* d_x, float* d_skip, float* d_norm_w, float* d_norm_b,
+                                            void* workspace, size_t workspace_bytes, const uint64_t* seed, float p,
+                                            void* stream_) {
+  HGT_REQUIRE(seed, "hgt_update_backward_drop_det: NULL seed");
+  return update_backward_det_impl(dout, o, x, type_row0, num_types, skip, norm_w, perm, type_active, n_nodes, d, d_o, d_x,
+                                  d_skip, d_norm_w, d_norm_b, workspace, workspace_bytes, seed, p, (cudaStream_t)stream_);
 }
 
 extern "C" int hgt_fold_backward_det(const float* d_w_cat, const float* d_b_cat, const float* const* wk,

@@ -339,9 +339,10 @@ class GraphedTrainStep(_Graphed):
     The optimizer must be built with capturable=True in every group; a learning-rate scheduler works when `lr` is a
     tensor (the schedulers fill_ it in place).  Every other hyperparameter is baked into the graph at capture: a later
     call raises RuntimeError if one of them changed (OneCycleLR's default cycle_momentum=True rewrites `betas` every
-    step; use cycle_momentum=False).  Dropout draws new masks at every replay.  The deterministic-algorithms
-    flag and the `recompute_tables` switch of the layers that own `params` are frozen at the first call: a later call
-    with one of them changed raises RuntimeError.  A batch that does not fit
+    step; use cycle_momentum=False).  Dropout draws new masks at every replay, nn.Dropout's and the in-kernel masks
+    of `fused_dropout` alike (their seed is drawn on the device inside the graph).  The deterministic-algorithms
+    flag and the `recompute_tables` and `fused_dropout` switches of the modules that own `params` are frozen at the
+    first call: a later call with one of them changed raises RuntimeError.  A batch that does not fit
     the signature raises ValueError before anything is copied."""
 
     def __init__(self, loss_fn, sig, device, optimizer=None, clip_norm=None, targets=None, params=None):
@@ -371,6 +372,7 @@ class GraphedTrainStep(_Graphed):
                   for t, (shape, dtype, fill) in spec.items()}
         self.det = None
         self.recompute = None
+        self.fused_drop = None
         self.hyper = None
         self.out = None
         self.capture_failed = False
@@ -446,6 +448,9 @@ class GraphedTrainStep(_Graphed):
         if self.graph is not None and any(bool(m.recompute_tables) != v for m, v in self.recompute.items()):
             raise RuntimeError("a layer's recompute_tables changed after the GraphedTrainStep was captured: the graph "
                                "holds the backward of the switch as it was at the first call")
+        if self.graph is not None and any(bool(m.fused_dropout) != v for m, v in self.fused_drop.items()):
+            raise RuntimeError("a module's fused_dropout changed after the GraphedTrainStep was captured: the graph "
+                               "holds the dropout kernels of the switch as it was at the first call")
         if self.graph is not None:
             hyper = self._hyperparameters()
             if hyper != self.hyper:
@@ -465,8 +470,9 @@ class GraphedTrainStep(_Graphed):
             if self.graph is None:
                 self.det = det
                 self._first_call()
-                from .autograd import recompute_switches
+                from .autograd import fused_dropout_switches, recompute_switches
                 self.recompute = recompute_switches(self.params)
+                self.fused_drop = fused_dropout_switches(self.params)
                 self.hyper = self._hyperparameters()
             else:
                 self.graph.replay()

@@ -12,11 +12,14 @@ import torch.nn as nn
 
 from . import _lib
 from . import plan as _plan
-from .autograd import bf16_matmuls, gemm_impl
+from .autograd import _DROPOUT_MODULES, _TanhDropout, bf16_matmuls, drop_seed, fused_drop_p, gemm_impl
 from .conv import GeneralConv, HGTConv
 
 
 class GNN(nn.Module):
+    fused_dropout = False      # training: the adapter's tanh and dropout as one pass (hgt_tanh_dropout) that keeps a single
+                               # [N, n_hid] tensor for the backward; the layers have their own HGTConv.fused_dropout
+
     def __init__(self, in_dim, n_hid, num_types, num_relations, n_heads, n_layers, dropout=0.2, conv_name='hgt',
                  prev_norm=False, last_norm=False, use_RTE=True):
         super().__init__()
@@ -74,7 +77,12 @@ class GNN(nn.Module):
         impl = gemm_impl(conv0.linear_impl, bf16_matmuls())
         conv0._typed_linear(x, self.in_dim, w_cat, b_cat, self.in_dim, self.n_hid, table, res, impl, st)
         n_known = plan.type_row0[T]
-        res[:n_known].tanh_()                                                    # model.py:75
+        p_fused = fused_drop_p(self)
+        if p_fused:                                                              # model.py:75-76 in one pass, in place
+            _lib.call("hgt_tanh_dropout", res.data_ptr(), n_known, N, self.n_hid, drop_seed(dev).data_ptr(), p_fused,
+                      res.data_ptr(), st)
+        else:
+            res[:n_known].tanh_()                                                # model.py:75
         if not plan.sorted_types:
             res = res.index_select(0, plan.rank.long())
         return res
@@ -93,7 +101,12 @@ class GNN(nn.Module):
         zero = [((plan.type_row0[t] + rows[t]) * h, plan.type_row0[t + 1] * h) for t in range(T)] if rows else []
         res = typed_linear(x, w_cat, b_cat, table, h, N * h, gemm_impl(conv0.linear_impl, bf16_matmuls()), 0,
                            zero + [(n_known * h, N * h)]).view(N, h)
-        res = torch.cat([torch.tanh(res[:n_known]), res[n_known:]], 0) if n_known < N else torch.tanh(res)   # model.py:75
+        _DROPOUT_MODULES.add(self)
+        p_fused = fused_drop_p(self)
+        if p_fused:                                                              # model.py:75-76 in one pass
+            res = _TanhDropout.apply(res, n_known, drop_seed(res.device), p_fused)
+        else:
+            res = torch.cat([torch.tanh(res[:n_known]), res[n_known:]], 0) if n_known < N else torch.tanh(res)   # model.py:75
         if not plan.sorted_types:
             res = res.index_select(0, plan.rank.long())
         return res
@@ -124,7 +137,7 @@ class GNN(nn.Module):
         plan = _plan.get_plan(node_type, edge_index, edge_type, edge_time if conv0.use_RTE else None, self.num_types,
                               conv0.num_relations)
         res = self._adapter_autograd(node_feature, plan) if grad else self._adapter_cuda(node_feature, plan)
-        meta_xs = self.drop(res)
+        meta_xs = res if fused_drop_p(self) else self.drop(res)                  # fused: the adapter already dropped
         del res
         for gc in self.gcs:
             meta_xs = gc(meta_xs, node_type, edge_index, edge_type, edge_time)
@@ -157,7 +170,7 @@ class GNN(nn.Module):
             res = self._adapter_autograd(x, lay.plan, lay.adapter_rows)
         else:
             res = self._adapter_cuda(x, lay.plan, lay.adapter_rows)
-        meta_xs = self.drop(res)
+        meta_xs = res if fused_drop_p(self) else self.drop(res)
         del res
         for gc, view in zip(self.gcs, lay.layers):
             meta_xs = gc.base_conv._forward_view(meta_xs, view, edge_time)
