@@ -46,16 +46,23 @@ def drop_scale(p):
 def drop_mask(seed, n_rows, d, p):
     """bool [n_rows, d]: element (row, col) is kept iff word col % 4 of Philox(counter = (q, 0, 0), key = seed) >= thr,
     q = row * ceil(d / 4) + col // 4.  p >= 1 keeps nothing."""
+    return drop_mask_rows(seed, np.arange(n_rows), d, p)
+
+
+def drop_mask_rows(seed, rows, d, p):
+    """The rows `rows` (rank rows, any order) of drop_mask: bool [len(rows), d].  For masks too large to draw whole,
+    such as the sampled rows of a full-graph layer."""
+    rows = np.asarray(rows, dtype=np.uint64).reshape(-1)
     if np.float32(p) >= 1:
-        return np.zeros((n_rows, d), dtype=bool)
+        return np.zeros((rows.size, d), dtype=bool)
     nchunk = (d + 3) // 4
-    q = np.arange(n_rows * nchunk, dtype=np.uint64)
+    q = (rows[:, None] * np.uint64(nchunk) + np.arange(nchunk, dtype=np.uint64)[None, :]).reshape(-1)
     seed = int(seed) & (2 ** 64 - 1)
     zero = np.zeros_like(q)
     words = philox4x32_10((q & U32, q >> np.uint64(32), zero, zero),
                           (np.full_like(q, seed & 0xFFFFFFFF), np.full_like(q, seed >> 32)))
-    keep = np.stack(words, 1) >= np.uint32(drop_threshold(p))                   # [n_rows * nchunk, 4]
-    return keep.reshape(n_rows, nchunk * 4)[:, :d]
+    keep = np.stack(words, 1) >= np.uint32(drop_threshold(p))                   # [rows * nchunk, 4]
+    return keep.reshape(rows.size, nchunk * 4)[:, :d]
 
 
 def test_philox_known_answers():
@@ -74,6 +81,7 @@ def test_mask_contract():
     m = drop_mask(1234567890123, 64, 78, 0.2)
     assert m.shape == (64, 78)
     assert np.array_equal(m[:10], drop_mask(1234567890123, 10, 78, 0.2))
+    assert np.array_equal(m[[63, 5, 0, 5]], drop_mask_rows(1234567890123, [63, 5, 0, 5], 78, 0.2))
     assert np.array_equal(m[:, :77], drop_mask(1234567890123, 64, 77, 0.2))     # ceil(78 / 4) == ceil(77 / 4)
     assert not np.array_equal(m[:, :64], drop_mask(1234567890123, 64, 64, 0.2))
     assert not np.array_equal(m, drop_mask(1234567890124, 64, 78, 0.2))
