@@ -288,6 +288,31 @@ int hgt_typed_linear_presplit_bf16(const void* a_hi, const void* a_lo, const flo
                                    int32_t n_groups, const hgt_lin_cblock* cblocks, void* out,
                                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* 24-bit gather tables (inference [K'|V'] and RTE tables).
+ * Element: the fp32 bit pattern b rounded to nearest-even at bit 8 (b + 0x7F + ((b >> 8) & 1), low 8 bits cleared):
+ * sign, 8-bit exponent and 15 stored mantissa bits, relative error <= 2^-16.  A NaN stays a quiet NaN with its sign,
+ * Inf stays Inf, finite values that round past FLT_MAX become Inf; +-0 and subnormals follow the same rule.
+ * Storage: the rounded word's bits 31..16 are the element's 16-bit "hi", bits 15..8 its 8-bit "lo"; it decodes to the
+ * fp32 word (hi << 16) | (lo << 8).
+ * Rows (planar): a table row of n logical elements is [hi x n (u16) | lo x n (u8)], 3n bytes; element c of the row has
+ * its hi at byte 2c and its lo at byte 2n + c.  A [K'|V'] row (n = 2d) takes 6d bytes.
+ * hgt_typed_linear_t24 / hgt_typed_linear_presplit_t24: the fp32 calls' product (same tiles, k order and bias add).
+ * Column blocks with out_off < t24_off are fp32 at out + out_off, as in the fp32 calls (out may be NULL when there are
+ * none); the others are 24-bit at out24, each result rounded once into this format as it is stored, so the output equals
+ * the fp32 call's output encoded, bitwise.  One call thus writes the Q blocks (fp32) and the K'/V' blocks (24-bit) of
+ * the projection table, whose K'/V' blocks start at kv_off.  The 24-bit blocks' out_off - t24_off and ld count logical
+ * elements: a block's rows have ld elements each (row stride 3 ld bytes), and out_off - t24_off = row * ld + col places
+ * element (row, col) of the table at hi byte row * 3 ld + 2 col and lo byte row * 3 ld + 2 ld + col of out24.
+ * Workspaces: the fp32 calls' queries. */
+int hgt_typed_linear_t24(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                         int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                         int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off, void* out24,
+                         int32_t impl, void* workspace, size_t workspace_bytes, void* stream);
+int hgt_typed_linear_presplit_t24(const void* a_hi, const void* a_lo, const float* W, const float* bias, int32_t K,
+                                  int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                  int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off,
+                                  void* out24, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Fused edge kernel: gather -> relation-specific score -> softmax by destination -> weighted sum
  * (conv.py:99,108-111 + PyG scatter-add), one pass over the destination-sorted CSR.
@@ -380,6 +405,17 @@ int hgt_edge_forward_bf16(const float* q, const void* kv, const void* kvr,
                           float* agg_out, float* att_out, float* stats_out, void* g_hi, void* g_lo,
                           void* workspace, size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
                           const int32_t* type_row0, int32_t num_types, const int32_t* type_active, void* stream);
+/* The edge forward on 24-bit gather tables (see hgt_typed_linear_t24): kv [rows+1] and kvr [P*240+1] rows of 6d bytes,
+ * decoded to fp32 in registers; everything else as hgt_edge_forward_bf16.  Needs d % 8 == 0.  There is no backward:
+ * training keeps fp32 (or bf16) tables. */
+int hgt_edge_forward_t24(const float* q, const void* kv, const void* kvr,
+                         const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                         const int32_t* csr_eid, const int32_t* tiles, int32_t n_tiles, int32_t n_split_tiles,
+                         const int32_t* hubs, int32_t n_hubs,
+                         int64_t n_nodes, int64_t n_edges, int32_t d, int32_t n_heads, int32_t apply_gelu,
+                         float* agg_out, float* att_out, float* stats_out, void* g_hi, void* g_lo,
+                         void* workspace, size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
+                         const int32_t* type_row0, int32_t num_types, const int32_t* type_active, void* stream);
 int hgt_edge_backward_bf16(const float* q, const void* kv, const void* kvr, const float* agg, const float* dagg,
                            const float* stats, const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
                            const int32_t* tiles, int32_t n_tiles, int64_t n_nodes, int32_t d, int32_t n_heads,
@@ -618,6 +654,7 @@ int hgt_tanh_dropout_bwd(const float* dout, const float* out, int64_t n_rows, in
  * per nn.Linear / nn.LayerNorm of the module (conv.py:34-40).  The plan arrays come from hgt_plan_*; the typed-linear
  * tables are the ones hgt_typed_linear takes (projection: Q + [K'|V'] blocks; rte: K'R/V'R tables; rt: the single
  * 240 x d group of RelTemporalEncoding.lin; upd: a_linears).  Nothing is allocated or synchronised.
+ * With d_out % 8 == 0 the [K'|V'] and RTE tables are 24-bit (hgt_typed_linear_t24, hgt_edge_forward_t24).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
   /* sizes and switches */

@@ -74,8 +74,14 @@ SIGNATURES = {
     # bf16 gather tables (HGT layers under torch.autocast(dtype=torch.bfloat16)): same arguments as the fp32 twins
     "hgt_typed_linear_bf16": [_p, _i64, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i32, _p, _sz, _p],
     "hgt_typed_linear_presplit_bf16": [_p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _p, _sz, _p],
+    # 24-bit gather tables: the fp32 twins' arguments with (out, t24_off, out24) for out
+    "hgt_typed_linear_t24": [_p, _i64, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i64, _p, _i32, _p, _sz, _p],
+    "hgt_typed_linear_presplit_t24": [_p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _sz, _p],
     "hgt_edge_forward_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i64, _i32, _i32, _i32, _p, _p,
                               _p, _p, _p, _p, _sz, _i32, _p, _p, _i32, _p, _p],
+    # 24-bit gather tables (inference forwards that keep nothing for a backward): same arguments as the bf16 twins
+    "hgt_edge_forward_t24": [_p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i64, _i32, _i32, _i32, _p, _p,
+                             _p, _p, _p, _p, _sz, _i32, _p, _p, _i32, _p, _p],
     "hgt_edge_backward_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, _i64, _i64, _p, _p, _p, _p,
                                _sz, _p, _p],
     "hgt_edge_backward_dst_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32, _i32, _p, _p,

@@ -60,6 +60,10 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+# entry-point suffix of a gather table's storage dtype: fp32, bf16 (autocast) or 24-bit (uint8 bytes, planar)
+_TABLE_SUFFIX = {torch.float32: "", torch.bfloat16: "_bf16", torch.uint8: "_t24"}
+
+
 def _output_rows(rows, d, dev, lt, out_map):
     """The layer's output buffer.  With an active prefix and no out_map the update epilogue leaves the rows past the
     prefix unwritten: they are zeroed, so a later layer never reads an uninitialised row."""
@@ -192,15 +196,17 @@ class HGTConv(nn.Module):
                     HGTConv.event_sink.append((name, self_.a, self_.b))
         return _T()
 
-    def _typed_linear(self, a, lda, w, bias, k, width, table, out, impl, st):
+    def _typed_linear(self, a, lda, w, bias, k, width, table, out, impl, st, out32=None, t24_off=0):
         """hgt_typed_linear with its (impl-dependent) workspace; table = (groups_dev, groups_host, n, cblocks_dev).
-        A bf16 `out` takes hgt_typed_linear_bf16."""
+        A bf16 `out` takes hgt_typed_linear_bf16, a uint8 one (a 24-bit table) hgt_typed_linear_t24, which writes the
+        column blocks before t24_off as fp32 to out32."""
         g_dev, g_host, n_g, c_dev = table
         ws_bytes = ctypes.c_size_t()
         _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, k, width, impl, ctypes.byref(ws_bytes))
         ws = torch.empty(max(ws_bytes.value, 1), dtype=torch.uint8, device=out.device)
-        _lib.call("hgt_typed_linear_bf16" if out.dtype == torch.bfloat16 else "hgt_typed_linear", a.data_ptr(), lda, w.data_ptr(), _lib.ptr(bias), k, width, g_dev.data_ptr(),
-                  g_host.ctypes.data, n_g, c_dev.data_ptr(), out.data_ptr(), impl, ws.data_ptr(), ws.numel(), st)
+        outs = (_lib.ptr(out32), t24_off, out.data_ptr()) if out.dtype == torch.uint8 else (out.data_ptr(),)
+        _lib.call("hgt_typed_linear" + _TABLE_SUFFIX[out.dtype], a.data_ptr(), lda, w.data_ptr(), _lib.ptr(bias), k, width, g_dev.data_ptr(),
+                  g_host.ctypes.data, n_g, c_dev.data_ptr(), *outs, impl, ws.data_ptr(), ws.numel(), st)
 
     def _check_inputs(self, node_inp, edge_time):
         if node_inp.device.type != "cuda":
@@ -399,7 +405,9 @@ class HGTConv(nn.Module):
               gelu_before_a, x_split=None, kv_runs=None, bf16=False, plan=None, impl=None, dst=False):
         """Everything up to and including the typed a_linear: plan, weight fold, typed projections, fused edge kernel
         (gelu fused iff gelu_before_a and not save), a_linears.  Returns a dict of the intermediates.  bf16: bf16 [K'|V'] and
-        RTE tables (Q and everything else fp32).  impl: the GEMMs' C impl (autograd.gemm_impl; 3 = one bf16 product, no lo
+        RTE tables (Q and everything else fp32).  Otherwise a forward that keeps nothing for a backward (not save) with
+        d % 8 == 0 builds 24-bit tables (uint8 tensors in the planar format of hgt_typed_linear_t24), as hgt_conv_forward
+        does; every other forward keeps fp32 tables.  impl: the GEMMs' C impl (autograd.gemm_impl; 3 = one bf16 product, no lo
         halves are made or read), linear_impl by default.  dst: tables over each type's destination extent
         (plan.layer_tables); `o` then holds only the rows inside the extents."""
         if impl is None:
@@ -441,55 +449,53 @@ class HGTConv(nn.Module):
                   plan.pair_rel_dev.data_ptr(), lt.cat_row0_dev.data_ptr(), lt.q_row0_dev.data_ptr(),
                   w_cat.data_ptr(), b_cat.data_ptr(), st)
 
-        # 2. typed projections: Q [N,d] and the folded [K'|V'] table (+ trailing all-zero row)
-        tab_dtype = torch.bfloat16 if bf16 else torch.float32
+        # 2. typed projections: Q [N,d] and the folded [K'|V'] table (+ trailing all-zero row).  bf16: Q by its own fp32
+        # call, the K'/V' blocks straight into the bf16 table.  24-bit: one call writes the Q blocks (before kv_off) as
+        # fp32 and the K'/V' blocks into the 24-bit table.
+        t24 = not save and not bf16 and d % 8 == 0
+        tab_dtype = torch.bfloat16 if bf16 else torch.uint8 if t24 else torch.float32
+        row_len = 2 * d * (3 if t24 else 1)                       # table row in tab_dtype elements
+        proj = None
         if bf16:
-            proj = None
             q_tab = torch.empty(N * d, **f32)
-            kv_tab = torch.empty((plan.kv_rows + 1) * 2 * d, dtype=tab_dtype, device=dev)
+            kv_tab = torch.empty((plan.kv_rows + 1) * row_len, dtype=tab_dtype, device=dev)
+            calls = ((lt.q_groups, q_tab, None), (lt.kv_groups, kv_tab, None))
+        elif t24:
+            q_buf = torch.empty(lt.kv_off, **f32)
+            q_tab = q_buf[lt.q_off:lt.q_off + N * d]
+            kv_tab = torch.empty((plan.kv_rows + 1) * row_len, dtype=tab_dtype, device=dev)
+            calls = ((lt.proj_groups, kv_tab, q_buf),)
         else:
             proj = torch.empty(lt.proj_elems, **f32)
             q_tab = proj[lt.q_off:lt.q_off + N * d]
             kv_tab = proj[lt.kv_off:]
-        kv_tab[plan.kv_rows * 2 * d:].zero_()
+            calls = ((lt.proj_groups, proj, None),)
+        kv_tab[plan.kv_rows * row_len:].zero_()                    # zero encodes to zero bytes in every format
         with self._stage("proj_linear"):
-            if bf16:
-                # Q by its own fp32 call, the K'/V' blocks straight into the bf16 table; the tensor-core GEMM splits
-                # fp32 x as it loads it, unless the previous layer left x split
-                xs = x_split if plan.sorted_types else None
-                for tab, dst in ((lt.q_groups, q_tab), (lt.kv_groups, kv_tab)):
-                    if xs is None:
-                        self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, dst, impl, st)
-                        continue
-                    g_dev, g_host, n_g, c_dev = tab
-                    wsb = ctypes.c_size_t()
-                    _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, d_in, d,
-                              ctypes.byref(wsb))
-                    ws1 = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                    _lib.call("hgt_typed_linear_presplit_bf16" if dst.dtype == torch.bfloat16 else "hgt_typed_linear_presplit",
-                              xs[0].data_ptr(), None if one else _lib.ptr(xs[1]), w_cat.data_ptr(), b_cat.data_ptr(), d_in, d,
-                              g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(), dst.data_ptr(), ws1.data_ptr(),
-                              ws1.numel(), st)
-            elif x_split is not None and plan.sorted_types:
-                # A operand already split by its producer (the fused halo pull): tensor-core GEMM without the split pass
-                g_dev, g_host, n_g, c_dev = lt.proj_groups
+            # the tensor-core GEMM splits fp32 x as it loads it, unless x arrives split (left by the previous layer, or
+            # by the fused halo pull)
+            xs = x_split if plan.sorted_types else None
+            for tab, out, out32 in calls:
+                if xs is None:
+                    self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, out, impl, st, out32, lt.kv_off)
+                    continue
+                g_dev, g_host, n_g, c_dev = tab
                 wsb = ctypes.c_size_t()
-                _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, d_in, d, ctypes.byref(wsb))
+                _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, d_in, d,
+                          ctypes.byref(wsb))
                 ws1 = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                _lib.call("hgt_typed_linear_presplit", x_split[0].data_ptr(), None if one else _lib.ptr(x_split[1]),
-                          w_cat.data_ptr(),
-                          b_cat.data_ptr(), d_in, d, g_dev.data_ptr(), g_host.ctypes.data, n_g, c_dev.data_ptr(),
-                          proj.data_ptr(), ws1.data_ptr(), ws1.numel(), st)
-            else:
-                self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, lt.proj_groups, proj, impl, st)
+                outs = (out32.data_ptr(), lt.kv_off, out.data_ptr()) if t24 else (out.data_ptr(),)
+                _lib.call("hgt_typed_linear_presplit" + _TABLE_SUFFIX[out.dtype], xs[0].data_ptr(),
+                          None if one else _lib.ptr(xs[1]), w_cat.data_ptr(), b_cat.data_ptr(), d_in, d, g_dev.data_ptr(),
+                          g_host.ctypes.data, n_g, c_dev.data_ptr(), *outs, ws1.data_ptr(), ws1.numel(), st)
         kvr = None
         if self.use_RTE:
             # RT = lin(emb.weight) [240,d] (conv.py:299), then projected with every pair's K'/V' weights (no bias)
             rt = torch.empty((_plan.RTE_MAX_LEN, d_in), **f32)
             self._typed_linear(self.emb.emb.weight, d_in, self.emb.lin.weight, self.emb.lin.bias, d_in, d_in,
                                lt.rt_group, rt, 1, st)
-            kvr = torch.empty((P * _plan.RTE_MAX_LEN + 1) * 2 * d, dtype=tab_dtype, device=dev)
-            kvr[P * _plan.RTE_MAX_LEN * 2 * d:].zero_()
+            kvr = torch.empty((P * _plan.RTE_MAX_LEN + 1) * row_len, dtype=tab_dtype, device=dev)
+            kvr[P * _plan.RTE_MAX_LEN * row_len:].zero_()
             self._typed_linear(rt, d_in, w_cat, None, d_in, d, lt.rte_groups, kvr, 1, st)
 
         # 3. fused edge kernel -> gelu(aggregate)
@@ -506,7 +512,7 @@ class HGTConv(nn.Module):
         att = torch.empty((E, H), **f32) if want_att else None
         stats = torch.empty((N, 2 * H), **f32) if save else None
         with self._stage("edge"):
-            _lib.call("hgt_edge_forward_bf16" if bf16 else "hgt_edge_forward", q_tab.data_ptr(), kv_tab.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
+            _lib.call("hgt_edge_forward" + _TABLE_SUFFIX[tab_dtype], q_tab.data_ptr(), kv_tab.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
                       plan.kv_row.data_ptr(), _lib.ptr(plan.rte_row) if self.use_RTE else None,
                       plan.csr_eid.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, plan.n_split,
                       plan.hubs.data_ptr(), plan.n_hubs, N, E, d, H, 1 if (gelu_before_a and not save) else 0,

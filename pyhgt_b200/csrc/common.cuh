@@ -44,6 +44,30 @@ __device__ __forceinline__ float hgt_gelu_erf(float x) {
   return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
 }
 
+// ---- 24-bit gather tables (format: include/hgt_b200.h, "24-bit gather tables") -------------------------------------
+// Element type tag of the planar 24-bit table: kernels templated on a table element type take it like float or bf16,
+// but a row of n elements is 3n bytes in two planes, so it is addressed through hgt_t24_at, never by pointer arithmetic.
+struct hgt_t24 {};
+
+// fp32 word -> the rounded word whose bits 31..8 are stored (bits 7..0 are zero).
+__host__ __device__ __forceinline__ uint32_t hgt_t24_round(uint32_t b) {
+  const uint32_t r = (b + 0x7fu + ((b >> 8) & 1u)) & 0xffffff00u;   // past FLT_MAX the carry lands on Inf; Inf stays
+  // NaN: quiet, sign kept (the add could carry a NaN into Inf or into the sign bit)
+  return (b & 0x7fffffffu) > 0x7f800000u ? ((b | 0x00400000u) & 0xffffff00u) : r;
+}
+
+// Element (row, col) of a table whose rows hold ld logical elements, given its logical offset off = row * ld + col:
+// the byte of its hi (u16) and of its lo (u8); element col + j has them 2 j and j bytes further.
+struct hgt_t24_at {
+  unsigned char* hi;
+  unsigned char* lo;
+  __host__ __device__ __forceinline__ hgt_t24_at(void* base, int64_t off, int64_t ld) {
+    const int64_t row = off / ld, col = off - row * ld;
+    hi = static_cast<unsigned char*>(base) + row * 3 * ld + 2 * col;
+    lo = static_cast<unsigned char*>(base) + row * 3 * ld + 2 * ld + col;
+  }
+};
+
 // ---- in-kernel dropout (mask contract: include/hgt_b200.h, "Fused dropout") ------------------------------------------
 // Host side of the contract: keep threshold and scale of a drop probability p > 0.
 struct HgtDrop {

@@ -10,15 +10,17 @@
 // slice of Q / K' / V' / acc in registers, so the per-head dot product is a log2(LPH)-step shuffle
 // reduction of a single value and the softmax state (m, l) is per lane.
 //
-// Two data paths for the per-edge [K'|V'] row (2*d floats, contiguous):
+// Two data paths for the per-edge [K'|V'] row (2*d elements, contiguous):
 //   variant 1 (LDG)  : vector loads straight into registers, EDGE_UNROLL rows in flight per warp.
 //   variant 2 (TMA)  : cp.async.bulk (1-D bulk tensor copy, SASS UBLKCP) into a per-warp shared-memory
 //                      ring with mbarrier transaction counting; the warp issues STAGES rows ahead.
 // Roofline: HBM-bound; algorithmic bytes per edge = 2*d*s_kv (row) + 4 (kv_row) [+4 rte_row, +2*d*s_kv from L2]
-// and per destination d*4 (Q) + d*4 (agg) + 4 (row_ptr), with s_kv = 4 (fp32 tables) or 2 (bf16 tables,
-// hgt_edge_forward_bf16: every kernel is templated on the table element type KV and widens rows to fp32 in registers;
-// the lane map, the softmax and every output are the same).
+// and per destination d*4 (Q) + d*4 (agg) + 4 (row_ptr), with s_kv = 4 (fp32 tables), 2 (bf16 tables,
+// hgt_edge_forward_bf16) or 3 (24-bit tables, hgt_edge_forward_t24).  Every kernel is templated on the table element
+// type KV and decodes rows to fp32 in registers; the lane map, the softmax and every output are the same.
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -121,6 +123,62 @@ __device__ __forceinline__ void load_vec_nc(float (&dst)[VEC], const __nv_bfloat
     unsigned short a;
     asm volatile("ld.global.nc.L1::no_allocate.b16 %0, [%1];" : "=h"(a) : "l"(p));
     dst[0] = __uint_as_float((uint32_t)a << 16);
+  }
+}
+
+// 24-bit table rows (hgt_t24): VEC elements' hi halves (u16 each) and lo bytes, decoded to the fp32 words
+// (hi << 16) | (lo << 8), one byte permute per element.  l << 8 and l >> 8 put a zero byte next to each lo byte.
+template <int VEC>
+__device__ __forceinline__ void t24_decode(float (&dst)[VEC], uint32_t h0, uint32_t h1, uint32_t l) {
+  const uint32_t z0 = l << 8;
+  dst[0] = __uint_as_float(__byte_perm(h0, z0, 0x1054));
+  if constexpr (VEC >= 2) dst[1] = __uint_as_float(__byte_perm(h0, z0, 0x3264));
+  if constexpr (VEC == 4) {
+    const uint32_t z1 = l >> 8;
+    dst[2] = __uint_as_float(__byte_perm(h1, z1, 0x1057));
+    dst[3] = __uint_as_float(__byte_perm(h1, z1, 0x3267));
+  }
+}
+
+template <class KV> constexpr int64_t kv_elem_bytes() { return std::is_same<KV, hgt_t24>::value ? 3 : sizeof(KV); }
+
+// Elements e .. e + VEC - 1 of a table row of n elements that starts at `row`.  NC: a streaming gather from global
+// memory (read-only path, no L1 allocation); otherwise a plain load (shared-memory ring, L2-resident RTE rows).
+template <class KV, int VEC, bool NC>
+__device__ __forceinline__ void load_kv(float (&dst)[VEC], const unsigned char* row, int e, int n) {
+  if constexpr (std::is_same<KV, hgt_t24>::value) {
+    const unsigned char* hp = row + 2 * e;
+    const unsigned char* lp = row + 2 * n + e;
+    uint32_t h0 = 0, h1 = 0, l = 0;
+    if constexpr (NC) {
+      if constexpr (VEC == 4) {
+        asm volatile("ld.global.nc.L1::no_allocate.v2.b32 {%0,%1}, [%2];" : "=r"(h0), "=r"(h1) : "l"(hp));
+        asm volatile("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(l) : "l"(lp));
+      } else if constexpr (VEC == 2) {
+        asm volatile("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(h0) : "l"(hp));
+        asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=r"(l) : "l"(lp));
+      } else {
+        asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=r"(h0) : "l"(hp));
+        asm volatile("ld.global.nc.L1::no_allocate.u8 %0, [%1];" : "=r"(l) : "l"(lp));
+      }
+    } else {
+      if constexpr (VEC == 4) {
+        const uint2 h = *reinterpret_cast<const uint2*>(hp);
+        h0 = h.x; h1 = h.y;
+        l = *reinterpret_cast<const uint32_t*>(lp);
+      } else if constexpr (VEC == 2) {
+        h0 = *reinterpret_cast<const uint32_t*>(hp);
+        l = *reinterpret_cast<const uint16_t*>(lp);
+      } else {
+        h0 = *reinterpret_cast<const uint16_t*>(hp);
+        l = *lp;
+      }
+    }
+    t24_decode<VEC>(dst, h0, h1, l);
+  } else {
+    const KV* p = reinterpret_cast<const KV*>(row) + e;
+    if constexpr (NC) load_vec_nc<VEC>(dst, p);
+    else load_vec<VEC>(dst, p);
   }
 }
 
@@ -246,13 +304,16 @@ template <class KV, int VEC, int NCH>
 __global__ void __launch_bounds__(kCtaThreads, 1)
 k_edge_fwd_ldg(EdgeParams p) {
   // rows in flight per warp: bounded by the register budget (2 * U * NCH * VEC floats of staging)
-  constexpr int EDGE_UNROLL = (NCH * VEC >= 32) ? 1 : (NCH * VEC >= 16 ? 2 : 4);
+  // (24-bit rows: half as many, their two planes' addresses and raw words take the registers of the rest)
+  constexpr int W = std::is_same<KV, hgt_t24>::value ? 2 * NCH * VEC : NCH * VEC;
+  constexpr int EDGE_UNROLL = (W >= 32) ? 1 : (W >= 16 ? 2 : 4);
   const int lane = threadIdx.x & 31;
   const LaneMap lm(p, lane);
-  const KV* const kvt = static_cast<const KV*>(p.kv);
-  const KV* const kvrt = static_cast<const KV*>(p.kvr);
+  const unsigned char* const kvt = static_cast<const unsigned char*>(p.kv);
+  const unsigned char* const kvrt = static_cast<const unsigned char*>(p.kvr);
   const bool rte = kvrt != nullptr;
-  const int64_t row_stride = 2 * (int64_t)p.d;
+  const int n = 2 * p.d;                                      // elements per table row
+  const int64_t row_bytes = n * kv_elem_bytes<KV>();
   int offs[NCH];
 #pragma unroll
   for (int t = 0; t < NCH; ++t) offs[t] = lm.off<VEC>(t);
@@ -289,12 +350,12 @@ k_edge_fwd_ldg(EdgeParams p) {
 #pragma unroll
           for (int u = 0; u < EDGE_UNROLL; ++u) {
             if (u < nb) {
-              const KV* row = kvt + (int64_t)p.kv_row[c0 + u] * row_stride;
+              const unsigned char* row = kvt + (int64_t)p.kv_row[c0 + u] * row_bytes;
 #pragma unroll
               for (int t = 0; t < NCH; ++t) {
                 if (offs[t] >= 0) {
-                  load_vec_nc<VEC>(kk[u][t], row + offs[t]);
-                  load_vec_nc<VEC>(vv[u][t], row + p.d + offs[t]);
+                  load_kv<KV, VEC, true>(kk[u][t], row, offs[t], n);
+                  load_kv<KV, VEC, true>(vv[u][t], row, p.d + offs[t], n);
                 } else {
 #pragma unroll
                   for (int v = 0; v < VEC; ++v) { kk[u][t][v] = 0.f; vv[u][t][v] = 0.f; }
@@ -306,13 +367,13 @@ k_edge_fwd_ldg(EdgeParams p) {
 #pragma unroll
             for (int u = 0; u < EDGE_UNROLL; ++u) {
               if (u < nb) {
-                const KV* row = kvrt + (int64_t)p.rte_row[c0 + u] * row_stride;
+                const unsigned char* row = kvrt + (int64_t)p.rte_row[c0 + u] * row_bytes;
 #pragma unroll
                 for (int t = 0; t < NCH; ++t) {
                   if (offs[t] >= 0) {
                     float a[VEC], b[VEC];
-                    load_vec<VEC>(a, row + offs[t]);
-                    load_vec<VEC>(b, row + p.d + offs[t]);
+                    load_kv<KV, VEC, false>(a, row, offs[t], n);
+                    load_kv<KV, VEC, false>(b, row, p.d + offs[t], n);
 #pragma unroll
                     for (int v = 0; v < VEC; ++v) { kk[u][t][v] += a[v]; vv[u][t][v] += b[v]; }
                   }
@@ -407,13 +468,13 @@ k_edge_fwd_tma(EdgeParams p) {
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const LaneMap lm(p, lane);
-  const KV* const kvt = static_cast<const KV*>(p.kv);
-  const KV* const kvrt = static_cast<const KV*>(p.kvr);
+  const unsigned char* const kvt = static_cast<const unsigned char*>(p.kv);
+  const unsigned char* const kvrt = static_cast<const unsigned char*>(p.kvr);
   const bool rte = kvrt != nullptr;
   const int S = p.stages;
-  const uint32_t row_bytes = 2u * (uint32_t)p.d * (uint32_t)sizeof(KV);
+  const int n = 2 * p.d;                                      // elements per table row
+  const uint32_t row_bytes = (uint32_t)(n * kv_elem_bytes<KV>());
   const uint32_t slot_bytes = rte ? 2u * row_bytes : row_bytes;
-  const int64_t row_stride = 2 * (int64_t)p.d;
   // layout: [warps][S][slot_bytes] rows, then [warps][S] mbarriers
   unsigned char* ring = smem_raw + (size_t)warp * S * slot_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + (size_t)kWarpsPerCta * S * slot_bytes) + warp * S;
@@ -467,8 +528,8 @@ k_edge_fwd_tma(EdgeParams p) {
         const uint32_t bar = smem_u32(&bars[slot]);
         const uint32_t dst = smem_u32(ring + (size_t)slot * slot_bytes);
         mbar_expect_tx(bar, slot_bytes);
-        bulk_g2s(dst, kvt + (int64_t)row * row_stride, row_bytes, bar);
-        if (rte) bulk_g2s(dst + row_bytes, kvrt + (int64_t)rrow * row_stride, row_bytes, bar);
+        bulk_g2s(dst, kvt + (int64_t)row * row_bytes, row_bytes, bar);
+        if (rte) bulk_g2s(dst + row_bytes, kvrt + (int64_t)rrow * row_bytes, row_bytes, bar);
       }
       ++issue_it;
     };
@@ -495,18 +556,18 @@ k_edge_fwd_tma(EdgeParams p) {
         for (int c = seg_begin; c < seg_end; ++c) {
           const uint32_t slot = it % S;
           mbar_wait(smem_u32(&bars[slot]), (it / S) & 1u);
-          const KV* srow = reinterpret_cast<const KV*>(ring + (size_t)slot * slot_bytes);
+          const unsigned char* srow = ring + (size_t)slot * slot_bytes;
           float kk[NCH][VEC], vv[NCH][VEC];
           float part = 0.f;
 #pragma unroll
           for (int t = 0; t < NCH; ++t) {
             if (offs[t] >= 0) {
-              load_vec<VEC>(kk[t], srow + offs[t]);
-              load_vec<VEC>(vv[t], srow + p.d + offs[t]);
+              load_kv<KV, VEC, false>(kk[t], srow, offs[t], n);
+              load_kv<KV, VEC, false>(vv[t], srow, p.d + offs[t], n);
               if (rte) {
                 float a[VEC], b[VEC];
-                load_vec<VEC>(a, srow + row_stride + offs[t]);
-                load_vec<VEC>(b, srow + row_stride + p.d + offs[t]);
+                load_kv<KV, VEC, false>(a, srow + row_bytes, offs[t], n);
+                load_kv<KV, VEC, false>(b, srow + row_bytes, p.d + offs[t], n);
 #pragma unroll
                 for (int v = 0; v < VEC; ++v) { kk[t][v] += a[v]; vv[t][v] += b[v]; }
               }
@@ -693,6 +754,21 @@ extern "C" int hgt_edge_forward_bf16(const float* q, const void* kv, const void*
                                      type_active, (cudaStream_t)stream_);
 }
 
+extern "C" int hgt_edge_forward_t24(const float* q, const void* kv, const void* kvr, const int32_t* row_ptr,
+                                    const int32_t* kv_row, const int32_t* rte_row, const int32_t* csr_eid,
+                                    const int32_t* tiles, int32_t n_tiles, int32_t n_split_tiles, const int32_t* hubs,
+                                    int32_t n_hubs, int64_t n_nodes, int64_t n_edges, int32_t d, int32_t n_heads,
+                                    int32_t apply_gelu, float* agg_out, float* att_out, float* stats_out, void* g_hi,
+                                    void* g_lo, void* workspace, size_t workspace_bytes, int32_t variant,
+                                    const int32_t* d_tile_counts, const int32_t* type_row0, int32_t num_types,
+                                    const int32_t* type_active, void* stream_) {
+  (void)n_edges;
+  return edge_forward<hgt_t24>(q, static_cast<const hgt_t24*>(kv), static_cast<const hgt_t24*>(kvr), row_ptr, kv_row,
+                               rte_row, csr_eid, tiles, n_tiles, n_split_tiles, hubs, n_hubs, n_nodes, d, n_heads,
+                               apply_gelu, agg_out, att_out, stats_out, g_hi, g_lo, workspace, workspace_bytes, variant,
+                               d_tile_counts, type_row0, num_types, type_active, (cudaStream_t)stream_);
+}
+
 namespace {
 
 template <class KV>
@@ -742,7 +818,8 @@ int edge_forward(const float* q, const KV* kv, const KV* kvr, const int32_t* row
   const int sms = hgt_sm_count();
   int grid = sms;
   size_t smem = 0;
-  const size_t row_bytes = 2 * (size_t)d * sizeof(KV);
+  HGT_REQUIRE((!std::is_same<KV, hgt_t24>::value || d % 8 == 0), "hgt_edge_forward_t24: needs d %% 8 == 0 (d=%d)", d);
+  const size_t row_bytes = 2 * (size_t)d * kv_elem_bytes<KV>();
   const size_t slot_bytes = kvr ? 2 * row_bytes : row_bytes;
   if (variant == 0) variant = 2;
   // narrow rows (one float4 per lane): the kernel is bound by per-destination latency, not by bytes in flight, so two

@@ -6,6 +6,9 @@
 // one ctypes call instead of a dozen (the reference's sampled-subgraph batches are launch/host-bound).
 // linear_impl 3 runs the tensor-core GEMMs with one bf16 product: the edge kernel then writes gelu(agg) as bf16 hi only,
 // and a pre-split x needs no lo half.
+// With d_out % 8 == 0 the [K'|V'] and RTE tables are 24-bit (hgt_typed_linear_t24, hgt_edge_forward_t24): the projection
+// writes Q as fp32 and the K'/V' blocks straight into the 24-bit table.  A forward that keeps nothing for a backward needs
+// no more than that precision (DESIGN.md §4.2), and the edge pass reads 6d instead of 8d bytes per edge.
 #include "common.cuh"
 
 int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
@@ -31,10 +34,11 @@ struct Carver {
 };
 
 struct Layout {
-  float *x_sorted, *w_cat, *b_cat, *proj, *rt, *kvr, *g_act, *wa_cat, *ba_cat, *o;
+  float *x_sorted, *w_cat, *b_cat, *proj, *rt, *g_act, *wa_cat, *ba_cat, *o;
+  void *kv, *kvr;                                          // fp32 (inside proj) or 24-bit tables
   void *g_hi, *g_lo, *ws_proj, *ws_edge, *ws_upd;
   size_t ws_proj_bytes, ws_edge_bytes, ws_upd_bytes, total;
-  bool fuse_split, presplit_x;
+  bool fuse_split, presplit_x, t24;
 };
 
 int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
@@ -50,7 +54,14 @@ int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
   L->x_sorted = a->perm ? c.take<float>((size_t)N * din) : nullptr;
   L->w_cat = c.take<float>((size_t)(a->cat_rows > 0 ? a->cat_rows : 1) * din);
   L->b_cat = c.take<float>((size_t)(a->cat_rows > 0 ? a->cat_rows : 1));
-  L->proj = c.take<float>((size_t)a->proj_elems);
+  L->t24 = d % 8 == 0;
+  if (L->t24) {
+    L->proj = c.take<float>((size_t)a->kv_off);           // Q only
+    L->kv = c.take_bytes((size_t)(a->kv_rows + 1) * 6 * d);
+  } else {
+    L->proj = c.take<float>((size_t)a->proj_elems);
+    L->kv = base ? L->proj + a->kv_off : nullptr;
+  }
   int rc;
   if (L->presplit_x)
     rc = hgt_typed_linear_presplit_workspace_bytes(a->h_proj_groups, a->n_proj_groups, din, d, &L->ws_proj_bytes);
@@ -58,10 +69,11 @@ int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
     rc = hgt_typed_linear_workspace_bytes(a->h_proj_groups, a->n_proj_groups, din, d, a->linear_impl, &L->ws_proj_bytes);
   if (rc) return rc;
   L->ws_proj = c.take_bytes(L->ws_proj_bytes + 256);
-  L->rt = L->kvr = nullptr;
+  L->rt = nullptr;
+  L->kvr = nullptr;
   if (a->use_rte) {
     L->rt = c.take<float>((size_t)HGT_RTE_MAX_LEN * din);
-    L->kvr = c.take<float>(((size_t)a->n_pairs * HGT_RTE_MAX_LEN + 1) * 2 * d);
+    L->kvr = c.take_bytes(((size_t)a->n_pairs * HGT_RTE_MAX_LEN + 1) * 2 * d * (L->t24 ? 3 : 4));
   }
   if ((rc = hgt_edge_workspace_bytes(a->n_split, d, a->n_heads, &L->ws_edge_bytes))) return rc;
   L->ws_edge = c.take_bytes(L->ws_edge_bytes);
@@ -123,32 +135,54 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
                              a->relation_pri, T, a->num_relations, a->n_heads, din, d, P, a->pair_type, a->pair_rel,
                              a->cat_row0, a->q_row0, L.w_cat, L.b_cat, stream)))
     return rc;
-  // trailing all-zero [K'|V'] row (edges that match no <s,t,r> triple)
-  HGT_CHECK_CUDA(cudaMemsetAsync(L.proj + a->kv_off + a->kv_rows * 2 * (int64_t)d, 0, sizeof(float) * 2 * d, st));
-  if (L.presplit_x)
-    rc = hgt_typed_linear_presplit(a->x_hi, a->linear_impl == 3 ? nullptr : a->x_lo, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
+  // trailing all-zero [K'|V'] row (edges that match no <s,t,r> triple); zero encodes to zero bytes
+  const size_t row_bytes = (size_t)2 * d * (L.t24 ? 3 : 4);
+  HGT_CHECK_CUDA(cudaMemsetAsync(static_cast<char*>(L.kv) + a->kv_rows * row_bytes, 0, row_bytes, st));
+  const void* x_lo = a->linear_impl == 3 ? nullptr : a->x_lo;
+  if (L.t24) {
+    // Q blocks (out_off < kv_off) as fp32, the K'/V' blocks straight into the 24-bit table
+    if (L.presplit_x)
+      rc = hgt_typed_linear_presplit_t24(a->x_hi, x_lo, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
+                                         a->n_proj_groups, a->proj_cblocks, L.proj, a->kv_off, L.kv, L.ws_proj,
+                                         L.ws_proj_bytes + 256, stream);
+    else
+      rc = hgt_typed_linear_t24(x_sorted, din, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
+                                a->n_proj_groups, a->proj_cblocks, L.proj, a->kv_off, L.kv, a->linear_impl, L.ws_proj,
+                                L.ws_proj_bytes + 256, stream);
+  } else if (L.presplit_x) {
+    rc = hgt_typed_linear_presplit(a->x_hi, x_lo, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
                                    a->n_proj_groups, a->proj_cblocks, L.proj, L.ws_proj, L.ws_proj_bytes + 256, stream);
-  else
+  } else {
     rc = hgt_typed_linear(x_sorted, din, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups, a->n_proj_groups,
                           a->proj_cblocks, L.proj, a->linear_impl, L.ws_proj, L.ws_proj_bytes + 256, stream);
+  }
   if (rc) return rc;
   if (a->use_rte) {
     if ((rc = hgt_typed_linear(a->emb_weight, din, a->emb_lin_w, a->emb_lin_b, din, din, a->rt_groups, a->h_rt_groups, 1,
                                a->rt_cblocks, L.rt, 1, nullptr, 0, stream)))
       return rc;
-    HGT_CHECK_CUDA(cudaMemsetAsync(L.kvr + (int64_t)P * HGT_RTE_MAX_LEN * 2 * d, 0, sizeof(float) * 2 * d, st));
-    if ((rc = hgt_typed_linear(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups, a->n_rte_groups,
-                               a->rte_cblocks, L.kvr, 1, nullptr, 0, stream)))
-      return rc;
+    HGT_CHECK_CUDA(cudaMemsetAsync(static_cast<char*>(L.kvr) + (int64_t)P * HGT_RTE_MAX_LEN * row_bytes, 0, row_bytes, st));
+    rc = L.t24 ? hgt_typed_linear_t24(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups,
+                                      a->n_rte_groups, a->rte_cblocks, nullptr, 0, L.kvr, 1, nullptr, 0, stream)
+               : hgt_typed_linear(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups, a->n_rte_groups,
+                                  a->rte_cblocks, static_cast<float*>(L.kvr), 1, nullptr, 0, stream);
+    if (rc) return rc;
   }
   // rows past type_dst[t] have no in-edges: as type_active, the edge kernel skips them (their Q rows were not computed)
   const int32_t* dst_rows = a->type_active ? a->type_active : a->type_dst;
-  if ((rc = hgt_edge_forward(L.proj + a->q_off, L.proj + a->kv_off, L.kvr, a->row_ptr, a->kv_row,
-                             a->use_rte ? a->rte_row : nullptr, a->csr_eid, a->tiles, a->n_tiles, a->n_split, a->hubs,
-                             a->n_hubs, N, a->n_edges, d, a->n_heads, 1, L.g_act, a->att, nullptr, L.g_hi, L.g_lo,
-                             L.ws_edge, L.ws_edge_bytes, a->edge_variant, a->d_tile_counts, a->type_row0, T,
-                             dst_rows, stream)))
-    return rc;
+  const int32_t* rte_row = a->use_rte ? a->rte_row : nullptr;
+  if (L.t24)
+    rc = hgt_edge_forward_t24(L.proj + a->q_off, L.kv, L.kvr, a->row_ptr, a->kv_row, rte_row, a->csr_eid, a->tiles,
+                              a->n_tiles, a->n_split, a->hubs, a->n_hubs, N, a->n_edges, d, a->n_heads, 1, L.g_act,
+                              a->att, nullptr, L.g_hi, L.g_lo, L.ws_edge, L.ws_edge_bytes, a->edge_variant,
+                              a->d_tile_counts, a->type_row0, T, dst_rows, stream);
+  else
+    rc = hgt_edge_forward(L.proj + a->q_off, static_cast<const float*>(L.kv), static_cast<const float*>(L.kvr),
+                          a->row_ptr, a->kv_row, rte_row, a->csr_eid, a->tiles, a->n_tiles, a->n_split, a->hubs,
+                          a->n_hubs, N, a->n_edges, d, a->n_heads, 1, L.g_act, a->att, nullptr, L.g_hi, L.g_lo,
+                          L.ws_edge, L.ws_edge_bytes, a->edge_variant, a->d_tile_counts, a->type_row0, T, dst_rows,
+                          stream);
+  if (rc) return rc;
   if ((rc = hgt_concat_linears(a->wa, a->ba, T, d, d, L.wa_cat, L.ba_cat, stream))) return rc;
   if (L.fuse_split)
     rc = hgt_typed_linear_presplit(L.g_hi, L.g_lo, L.wa_cat, L.ba_cat, d, d, a->upd_groups, a->h_upd_groups,

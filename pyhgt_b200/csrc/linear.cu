@@ -2,8 +2,11 @@
 // relation_pri into the K/V projections, SURVEY.md §8 a4) and the grouped GEMM front end.
 // This file holds the fp32 SIMT kernel (impl 1); the wgmma tensor-core kernel (impl 2, split-bf16 x3; impl 3, auto with
 // one bf16 product on the tensor cores) lives in linear_tc.cu and is dispatched from hgt_typed_linear below.  hgt_typed_linear_bf16 runs the same kernels with a bf16
-// output, each fp32 result rounded to nearest-even once when it is stored.
+// output, each fp32 result rounded to nearest-even once when it is stored; hgt_typed_linear_t24 with the planar 24-bit
+// table output (include/hgt_b200.h), each result rounded by hgt_t24_round once when it is stored.
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -15,6 +18,10 @@ int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float
                         int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                         int32_t n_groups, const hgt_lin_cblock* cblocks, __nv_bfloat16* out, int32_t products,
                         void* workspace, size_t workspace_bytes, cudaStream_t st);
+int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                        int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                        int32_t n_groups, const hgt_lin_cblock* cblocks, float* out32, int64_t t24_off, hgt_t24* out,
+                        int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st);
 bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width);
 size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width,
                                      int32_t products);
@@ -91,7 +98,8 @@ __global__ void __launch_bounds__(GEMM_THREADS)
 k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __restrict__ W,
                     const float* __restrict__ bias, int K, int cb_width,
                     const hgt_lin_group* __restrict__ groups, int n_groups,
-                    const hgt_lin_cblock* __restrict__ cblocks, OutT* __restrict__ out, TilePrefix tp) {
+                    const hgt_lin_cblock* __restrict__ cblocks, OutT* __restrict__ out, TilePrefix tp,
+                    float* __restrict__ out32, int64_t t24_off) {
   __shared__ __align__(16) float As[BK][LDA_S];
   __shared__ __align__(16) float Ws[BK][LDW_S];
   int tile = blockIdx.x;
@@ -162,15 +170,46 @@ k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __res
     for (int j = 0; j < 4; ++j)
       if (tn * 4 + j < cols_here) bj[j] = bias[w_row0 + tn * 4 + j];
   }
-  OutT* Og = out + cblk.out_off + m0 * cblk.ld + n0;
+  if (std::is_same<OutT, hgt_t24>::value && cblk.out_off < t24_off) {   // an fp32 block of a 24-bit call
+    float* Og = out32 + cblk.out_off + m0 * cblk.ld + n0;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    int r = tm * 8 + i;
-    if (r >= rows_here) continue;
+    for (int i = 0; i < 8; ++i) {
+      int r = tm * 8 + i;
+      if (r >= rows_here) continue;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      int c = tn * 4 + j;
-      if (c < cols_here) store_out(Og + (int64_t)r * cblk.ld + c, acc[i][j] + bj[j]);
+      for (int j = 0; j < 4; ++j) {
+        int c = tn * 4 + j;
+        if (c < cols_here) Og[(int64_t)r * cblk.ld + c] = acc[i][j] + bj[j];
+      }
+    }
+  } else if constexpr (std::is_same<OutT, hgt_t24>::value) {
+    const hgt_t24_at e(out, cblk.out_off - t24_off + m0 * cblk.ld + n0, cblk.ld);
+    const int64_t rb = 3 * cblk.ld;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      int r = tm * 8 + i;
+      if (r >= rows_here) continue;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        int c = tn * 4 + j;
+        if (c < cols_here) {
+          const uint32_t w = hgt_t24_round(__float_as_uint(acc[i][j] + bj[j]));
+          *reinterpret_cast<uint16_t*>(e.hi + r * rb + 2 * c) = (uint16_t)(w >> 16);
+          e.lo[r * rb + c] = (unsigned char)(w >> 8);
+        }
+      }
+    }
+  } else {
+    OutT* Og = out + cblk.out_off + m0 * cblk.ld + n0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      int r = tm * 8 + i;
+      if (r >= rows_here) continue;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        int c = tn * 4 + j;
+        if (c < cols_here) store_out(Og + (int64_t)r * cblk.ld + c, acc[i][j] + bj[j]);
+      }
     }
   }
 }
@@ -234,7 +273,7 @@ template <class OutT>
 int typed_linear(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
                  const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
                  const hgt_lin_cblock* cblocks, OutT* out, int32_t impl, void* workspace, size_t workspace_bytes,
-                 cudaStream_t st) {
+                 cudaStream_t st, float* out32 = nullptr, int64_t t24_off = 0) {
   HGT_REQUIRE(n_groups >= 0, "hgt_typed_linear: n_groups=%d", n_groups);
   HGT_REQUIRE(K > 0 && cb_width > 0, "hgt_typed_linear: K=%d cb_width=%d", K, cb_width);
   if (n_groups == 0) return 0;
@@ -244,7 +283,7 @@ int typed_linear(const float* A, int64_t lda, const float* W, const float* bias,
     for (int g0 = 0; g0 < n_groups; g0 += kMaxGroups) {
       const int n = n_groups - g0 < kMaxGroups ? n_groups - g0 : kMaxGroups;
       int rc = typed_linear(A, lda, W, bias, K, cb_width, groups + g0, h_groups + g0, n, cblocks, out, impl, workspace,
-                            workspace_bytes, st);
+                            workspace_bytes, st, out32, t24_off);
       if (rc) return rc;
     }
     return 0;
@@ -255,8 +294,12 @@ int typed_linear(const float* A, int64_t lda, const float* W, const float* bias,
   if (impl == 2 || impl == 3) {
     HGT_REQUIRE(tc, "hgt_typed_linear: tensor-core kernel does not support lda=%lld K=%d cb_width=%d",
                 (long long)lda, K, cb_width);
-    return hgt_typed_linear_tc(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out,
-                               impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
+    if constexpr (std::is_same<OutT, hgt_t24>::value)
+      return hgt_typed_linear_tc(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out32, t24_off, out,
+                                 impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
+    else
+      return hgt_typed_linear_tc(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out,
+                                 impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
   }
   HGT_REQUIRE(impl == 1, "hgt_typed_linear: unknown impl %d", impl);
   TilePrefix tp;
@@ -271,7 +314,7 @@ int typed_linear(const float* A, int64_t lda, const float* W, const float* bias,
   tp.first_tile[n_groups] = (int32_t)total;
   if (total == 0) return 0;
   k_typed_linear_simt<OutT><<<(unsigned)total, GEMM_THREADS, 0, st>>>(A, lda, W, bias, K, cb_width, groups, n_groups,
-                                                                      cblocks, out, tp);
+                                                                      cblocks, out, tp, out32, t24_off);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -292,4 +335,12 @@ extern "C" int hgt_typed_linear_bf16(const float* A, int64_t lda, const float* W
                                      void* workspace, size_t workspace_bytes, void* stream_) {
   return typed_linear(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks,
                       static_cast<__nv_bfloat16*>(out), impl, workspace, workspace_bytes, (cudaStream_t)stream_);
+}
+
+extern "C" int hgt_typed_linear_t24(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                                    int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                    int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off,
+                                    void* out24, int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
+  return typed_linear(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, static_cast<hgt_t24*>(out24),
+                      impl, workspace, workspace_bytes, (cudaStream_t)stream_, out, t24_off);
 }

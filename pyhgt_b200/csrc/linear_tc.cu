@@ -12,8 +12,8 @@
 // leaves a ring of 3 x 48 KB stages at BN = 256 and 5 x 32 KB at BN = 128.  BN = 64 keeps 64-wide k-blocks (SWIZZLE_128B,
 // 4 stages) and the staged st.global epilogue: its k-blocks are short enough that halving them costs more in barrier
 // waits than the deeper ring gains (measured on the d = 400 OAG shape).  Output tiles follow the same group / column-block tables
-// as the SIMT kernel in linear.cu.  The output is fp32, or bf16 (hgt_typed_linear[_presplit]_bf16): the same tile, rounded
-// to nearest-even once as the epilogue stores it.
+// as the SIMT kernel in linear.cu.  The output is fp32, bf16 (hgt_typed_linear[_presplit]_bf16) or the planar 24-bit
+// table format (hgt_typed_linear[_presplit]_t24, include/hgt_b200.h): the same tile, rounded once as the epilogue stores it.
 //
 // One-product mode (P = 1: impl 3, or a presplit call with a_lo == NULL): the operands are rounded to bf16 (the hi half
 // of the split, bitwise) and one bf16 product per k-step is accumulated, torch's "medium" float32 matmul precision.  Its
@@ -89,6 +89,24 @@ __device__ __forceinline__ void store4(__nv_bfloat16* p, float4 v, bool aligned)
     p[0] = a.x; p[1] = a.y; p[2] = b.x; p[3] = b.y;
   }
 }
+// 24-bit tables: hi halves at `hi`, lo bytes at `lo`.  aligned: hi 8-byte and lo 4-byte aligned.
+__device__ __forceinline__ void store4_t24(unsigned char* hi, unsigned char* lo, float4 v, bool aligned) {
+  uint32_t h01, l01, h23, l23;
+  t24_pair(make_float2(v.x, v.y), h01, l01);
+  t24_pair(make_float2(v.z, v.w), h23, l23);
+  if (aligned) {
+    *reinterpret_cast<uint2*>(hi) = make_uint2(h01, h23);
+    *reinterpret_cast<uint32_t*>(lo) = __byte_perm(l01, l23, 0x5410);
+  } else {
+    const uint32_t h[4] = {h01 & 0xffffu, h01 >> 16, h23 & 0xffffu, h23 >> 16}, l[4] = {l01 & 0xffu, l01 >> 8, l23 & 0xffu, l23 >> 8};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      hi[2 * i] = (unsigned char)h[i];
+      hi[2 * i + 1] = (unsigned char)(h[i] >> 8);
+      lo[i] = (unsigned char)l[i];
+    }
+  }
+}
 
 // ---- the GEMM: out_cb[m, n] = A[a_row0 + m, :] . W[w_row0 + cb * cb_width + n, :] (+ bias) ------------------------------
 // Rows of a tile past the group and columns past the column block are computed on neighbouring (or zero-filled) operand
@@ -101,7 +119,9 @@ struct FwdJob {
   const hgt_lin_group* groups;
   const hgt_lin_cblock* cblocks;
   OutT* out;
-  const CUtensorMap* out_maps;             // BN = 128 / 256: output map of (group g, column block cb) at map_first[g] + cb
+  float* out32;                            // 24-bit jobs: column blocks with out_off < t24_off are fp32 at out32 + out_off
+  int64_t t24_off;                         // ... and the others 24-bit at `out`, logical offset out_off - t24_off
+  const CUtensorMap* out_maps;             // BN = 128 / 256: output map(s) of (group g, column block cb) at map_first[g] + cb
   int n_groups, cb_width, k_blocks, tile_n, n_tiles_n;
   int32_t first_tile[kMaxGroups + 1];
   int32_t map_first[kMaxGroups];
@@ -110,6 +130,8 @@ struct FwdJob {
     int a_row, w_row, cols, m0, n0;
     int64_t rows, ld;
     OutT* out;
+    float* out32;                          // 24-bit jobs: the tile's fp32 output, or NULL
+    unsigned char *hi, *lo;                // 24-bit tables: the planes' bytes of the tile's element (0, 0)
     const float* bias;
     const CUtensorMap* map;
   };
@@ -131,11 +153,19 @@ struct FwdJob {
     t.cols = cb_width - n0;
     t.rows = grp.m - m0;
     t.ld = cblk.ld;
-    t.out = out + cblk.out_off + m0 * cblk.ld + n0;
+    if constexpr (is_t24<OutT>()) {
+      const int64_t off = cblk.out_off + m0 * cblk.ld + n0;
+      t.out32 = cblk.out_off < t24_off ? out32 + off : nullptr;
+      const hgt_t24_at e(out, off - t24_off, cblk.ld);
+      t.hi = e.hi;
+      t.lo = e.lo;
+    } else {
+      t.out = out + cblk.out_off + m0 * cblk.ld + n0;
+    }
     t.bias = (grp.has_bias && bias) ? bias + t.w_row : nullptr;
     t.m0 = (int)m0;
     t.n0 = n0;
-    t.map = out_maps + map_first[g] + cb;
+    t.map = out_maps + out_maps_per_block<OutT>() * (map_first[g] + cb);
     return k_blocks;
   }
   __device__ void prefetch(const Tile&) const {
@@ -155,34 +185,64 @@ struct FwdJob {
     tma_load_2d(sa + B, &w_hi, k, t.w_row, bar);
     if constexpr (P == 3) tma_load_2d(sa + B + BN * KB * 2, &w_lo, k, t.w_row, bar);
   }
+  // OutT (or fp32 T, the fp32 blocks of a 24-bit job) at o, the tile's element (0, 0)
+  template <int BN, class T, class Pair>
+  __device__ void store_plain(const Tile& t, T* o, const float* acc, float* stage, int c, int wq, int lane,
+                              Pair pair) const {
+    o += (int64_t)(64 * c) * t.ld;
+    const int64_t rows = t.rows - 64 * c, ld = t.ld;
+    const int cols = t.cols;
+    const uintptr_t align = reinterpret_cast<uintptr_t>(o) | (uintptr_t)(ld * sizeof(T));
+    if constexpr (fwd_tma_store<BN>()) {
+      if ((align & 15) == 0) {
+        store_tma<BN, T>(acc, reinterpret_cast<unsigned char*>(stage), c, wq, lane, pair, t.map, t.n0, t.m0 + 64 * c,
+                         cols);
+        return;
+      }
+      if (wq == 0 && lane == 0) bulk_wait_read<0>();          // store_staged reuses the tensor stores' buffers
+    }
+    const bool vec4 = (align & (4 * sizeof(T) - 1)) == 0;
+    store_staged<BN>(acc, stage, c, wq, lane, pair, [&](int r, int col, float4 v) {
+      if (r < rows && col < cols) store4(o + r * ld + col, v, vec4);
+    });
+  }
   // BN = 128 / 256: asynchronous TMA tensor stores (tcp::store_tma) where the destination rows are 16-byte aligned, so
   // the stores overlap the next tile's products.  Otherwise, and at BN = 64, through shared memory with whole row segments
   // per warp (tcp::store_staged).  cols is a multiple of 16, so a 4-column group is either inside the column block or
   // past it.  Both paths add the bias in fp32 and round once, so they write the same bits.
   template <int BN>
   __device__ void store(const Tile& t, const float* acc, float* stage, int c, int wq, int lane) const {
-    OutT* o = t.out + (int64_t)(64 * c) * t.ld;
-    const int64_t rows = t.rows - 64 * c;
     const float* b = t.bias;
     const int cols = t.cols;
-    const int64_t ld = t.ld;
     auto pair = [&](int, int col, float v0, float v1) {
       if (b && col < cols) v0 += __ldg(b + col), v1 += __ldg(b + col + 1);
       return make_float2(v0, v1);
     };
-    const uintptr_t align = reinterpret_cast<uintptr_t>(o) | (uintptr_t)(ld * sizeof(OutT));
-    if constexpr (fwd_tma_store<BN>()) {
-      if ((align & 15) == 0) {
-        store_tma<BN, OutT>(acc, reinterpret_cast<unsigned char*>(stage), c, wq, lane, pair, t.map, t.n0, t.m0 + 64 * c,
-                            cols);
+    if constexpr (is_t24<OutT>()) {
+      if (t.out32) {
+        store_plain<BN>(t, t.out32, acc, stage, c, wq, lane, pair);
         return;
       }
-      if (wq == 0 && lane == 0) bulk_wait_read<0>();          // store_staged reuses the tensor stores' buffers
+      const int64_t rows = t.rows - 64 * c;
+      const int64_t rb = 3 * t.ld;                            // row stride in bytes
+      unsigned char* hi = t.hi + 64 * c * rb;
+      unsigned char* lo = t.lo + 64 * c * rb;
+      if constexpr (fwd_tma_store<BN>()) {
+        if (((reinterpret_cast<uintptr_t>(hi) | reinterpret_cast<uintptr_t>(lo) | (uintptr_t)rb) & 15) == 0) {
+          store_tma<BN, OutT>(acc, reinterpret_cast<unsigned char*>(stage), c, wq, lane, pair, t.map, t.n0,
+                              t.m0 + 64 * c, cols);
+          return;
+        }
+        if (wq == 0 && lane == 0) bulk_wait_read<0>();
+      }
+      const bool vec4 = ((reinterpret_cast<uintptr_t>(hi) | (uintptr_t)rb) & 7) == 0 &&
+                        ((reinterpret_cast<uintptr_t>(lo) | (uintptr_t)rb) & 3) == 0;
+      store_staged<BN>(acc, stage, c, wq, lane, pair, [&](int r, int col, float4 v) {
+        if (r < rows && col < cols) store4_t24(hi + r * rb + 2 * col, lo + r * rb + col, v, vec4);
+      });
+    } else {
+      store_plain<BN>(t, t.out, acc, stage, c, wq, lane, pair);
     }
-    const bool vec4 = (align & (4 * sizeof(OutT) - 1)) == 0;
-    store_staged<BN>(acc, stage, c, wq, lane, pair, [&](int r, int col, float4 v) {
-      if (r < rows && col < cols) store4(o + r * ld + col, v, vec4);
-    });
   }
 };
 
@@ -196,28 +256,51 @@ __global__ void __launch_bounds__(TILE_THREADS, 1)
 // One map per (group, column block) of a launch: base out + out_off, rows = the group's m, columns = cb_width, row stride
 // ld.  The column-block table lives on the device, so the maps are built there: a copy of a host-encoded template (element
 // type, box, swizzle, columns) with the address, the row count and the row stride replaced.  Maps of blocks whose rows
-// are not 16-byte aligned are left unwritten; their tiles take the staged epilogue.
+// are not 16-byte aligned are left unwritten; their tiles take the staged epilogue.  24-bit tables have two maps per block,
+// the hi plane's (from `tmpl`) and the lo plane's (from `tmpl_lo`), at the planes' bytes with row stride 3 ld bytes; the
+// fp32 blocks of a 24-bit job one (from `tmpl_f32`).
 struct MapFirst {
   int32_t v[kMaxGroups];
 };
 
+__device__ __forceinline__ void put_map(CUtensorMap* m, const CUtensorMap& tmpl, const void* base, int64_t rows,
+                                        uint64_t stride) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) reinterpret_cast<uint4*>(m)[i] = reinterpret_cast<const uint4*>(&tmpl)[i];
+  const uint64_t gm = (uint64_t)__cvta_generic_to_global(m);
+  asm volatile("tensormap.replace.tile.global_address.global.b1024.b64 [%0], %1;" ::"l"(gm), "l"(base) : "memory");
+  asm volatile("tensormap.replace.tile.global_dim.global.b1024.b32 [%0], 1, %1;" ::"l"(gm), "r"((uint32_t)rows)
+               : "memory");
+  asm volatile("tensormap.replace.tile.global_stride.global.b1024.b64 [%0], 0, %1;" ::"l"(gm), "l"(stride) : "memory");
+}
+
 template <class OutT>
-__global__ void k_out_maps(const __grid_constant__ CUtensorMap tmpl, const hgt_lin_group* __restrict__ groups,
-                           const hgt_lin_cblock* __restrict__ cblocks, OutT* out, const MapFirst first, CUtensorMap* maps) {
+__global__ void k_out_maps(const __grid_constant__ CUtensorMap tmpl, const __grid_constant__ CUtensorMap tmpl_lo,
+                           const __grid_constant__ CUtensorMap tmpl_f32, const hgt_lin_group* __restrict__ groups,
+                           const hgt_lin_cblock* __restrict__ cblocks, OutT* out, float* out32, int64_t t24_off,
+                           const MapFirst first, CUtensorMap* maps) {
   const hgt_lin_group grp = groups[blockIdx.x];
   for (int cb = threadIdx.x; cb < grp.n_cblocks; cb += blockDim.x) {
     const hgt_lin_cblock cblk = cblocks[grp.cb_first + cb];
-    OutT* base = out + cblk.out_off;
-    const uint64_t stride = (uint64_t)cblk.ld * sizeof(OutT);
-    if (grp.m <= 0 || ((reinterpret_cast<uintptr_t>(base) | stride) & 15) != 0) continue;
-    CUtensorMap* m = maps + first.v[blockIdx.x] + cb;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) reinterpret_cast<uint4*>(m)[i] = reinterpret_cast<const uint4*>(&tmpl)[i];
-    const uint64_t gm = (uint64_t)__cvta_generic_to_global(m);
-    asm volatile("tensormap.replace.tile.global_address.global.b1024.b64 [%0], %1;" ::"l"(gm), "l"(base) : "memory");
-    asm volatile("tensormap.replace.tile.global_dim.global.b1024.b32 [%0], 1, %1;" ::"l"(gm), "r"((uint32_t)grp.m)
-                 : "memory");
-    asm volatile("tensormap.replace.tile.global_stride.global.b1024.b64 [%0], 0, %1;" ::"l"(gm), "l"(stride) : "memory");
+    CUtensorMap* m = maps + out_maps_per_block<OutT>() * (first.v[blockIdx.x] + cb);
+    if (grp.m <= 0) continue;
+    if (is_t24<OutT>() && cblk.out_off < t24_off) {
+      const float* base = out32 + cblk.out_off;
+      const uint64_t stride = (uint64_t)cblk.ld * 4;
+      if (((reinterpret_cast<uintptr_t>(base) | stride) & 15) != 0) continue;
+      put_map(m, tmpl_f32, base, grp.m, stride);
+    } else if constexpr (is_t24<OutT>()) {
+      const hgt_t24_at e(out, cblk.out_off - t24_off, cblk.ld);
+      const uint64_t stride = 3 * (uint64_t)cblk.ld;
+      if (((reinterpret_cast<uintptr_t>(e.hi) | reinterpret_cast<uintptr_t>(e.lo) | stride) & 15) != 0) continue;
+      put_map(m, tmpl, e.hi, grp.m, stride);
+      put_map(m + 1, tmpl_lo, e.lo, grp.m, stride);
+    } else {
+      OutT* base = out + cblk.out_off;
+      const uint64_t stride = (uint64_t)cblk.ld * sizeof(OutT);
+      if (((reinterpret_cast<uintptr_t>(base) | stride) & 15) != 0) continue;
+      put_map(m, tmpl, base, grp.m, stride);
+    }
   }
   asm volatile("fence.proxy.tensormap::generic.release.gpu;" ::: "memory");
 }
@@ -277,19 +360,21 @@ bool a_fp32_loadable(const float* A, int64_t lda) {
   return A && (reinterpret_cast<uintptr_t>(A) & 15) == 0 && lda % 4 == 0;
 }
 
-// Template of the output maps: `cb_width` columns of OutT, boxes of 128 bytes x 64 rows with SWIZZLE_128B (the layout
-// tcp::store_tma stages).  `dummy` (16-byte aligned) and the row count / stride are placeholders that k_out_maps replaces.
-template <class OutT>
-int make_out_template(CUtensorMap* m, void* dummy, int cb_width) {
+// Template of the output maps: `cb_width` columns of `elem`-byte elements, boxes of 128 bytes x 64 rows with SWIZZLE_128B
+// (the layout tcp::store_tma stages), or of 64 bytes with SWIZZLE_64B (elem = 1: the lo plane of a 24-bit table).
+// `dummy` (16-byte aligned) and the row count / stride are placeholders that k_out_maps replaces.
+int make_out_template(CUtensorMap* m, void* dummy, int cb_width, int elem) {
   EncodeTiledFn fn = get_encode_fn();
   HGT_REQUIRE(fn != nullptr, "hgt_typed_linear: cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t dims[2] = {(cuuint64_t)cb_width, 64};
-  cuuint64_t strides[1] = {(cuuint64_t)hgt_align_up((size_t)cb_width * sizeof(OutT), 16)};
-  cuuint32_t box[2] = {128 / (cuuint32_t)sizeof(OutT), 64};
+  cuuint64_t strides[1] = {(cuuint64_t)hgt_align_up((size_t)cb_width * elem, 16)};
+  cuuint32_t box[2] = {elem == 1 ? 64u : 128 / (cuuint32_t)elem, 64};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, sizeof(OutT) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dummy, dims,
-                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUtensorMapDataType type = elem == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : elem == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8;
+  CUresult r = fn(m, type, 2, dummy, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  elem == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   HGT_REQUIRE(r == CUDA_SUCCESS, "hgt_typed_linear: cuTensorMapEncodeTiled (output) failed (%d) cb_width=%d", (int)r,
               cb_width);
   return 0;
@@ -320,6 +405,8 @@ struct FwdOps {
   const __nv_bfloat16 *a_hi, *a_lo, *w_hi, *w_lo;
   int64_t a_rows, w_rows;
   int K, Kp;
+  float* out32;                           // 24-bit jobs: see FwdJob
+  int64_t t24_off;
 };
 
 // The tensor maps and the k-block count follow the kernel's k-block KB.  At P = 1 (and for A under AF) the lo maps repeat
@@ -338,12 +425,18 @@ int launch_fwd(FwdJob<OutT, AF>& job, const FwdOps& ops, int tiles, cudaStream_t
   if ((rc = make_map(&job.w_lo, P == 3 ? ops.w_lo : ops.w_hi, ops.w_rows, ops.Kp, BN, KB))) return rc;
   job.k_blocks = (ops.Kp + KB - 1) / KB;
   if constexpr (fwd_tma_store<BN>()) {
-    CUtensorMap tmpl;
+    CUtensorMap tmpl, tmpl_lo, tmpl_f32;
     MapFirst first;
-    if ((rc = make_out_template<OutT>(&tmpl, const_cast<CUtensorMap*>(job.out_maps), job.cb_width))) return rc;
+    void* dummy = const_cast<CUtensorMap*>(job.out_maps);
+    // 24-bit tables: the hi plane's u16 elements as bf16 (the maps only move bytes), the lo plane's u8, fp32 blocks
+    if ((rc = make_out_template(&tmpl, dummy, job.cb_width, is_t24<OutT>() ? 2 : (int)sizeof(OutT)))) return rc;
+    tmpl_lo = tmpl_f32 = tmpl;
+    if (is_t24<OutT>() && ((rc = make_out_template(&tmpl_lo, dummy, job.cb_width, 1)) ||
+                           (rc = make_out_template(&tmpl_f32, dummy, job.cb_width, 4))))
+      return rc;
     for (int g = 0; g < job.n_groups; ++g) first.v[g] = job.map_first[g];
-    k_out_maps<OutT><<<job.n_groups, 64, 0, st>>>(tmpl, job.groups, job.cblocks, job.out, first,
-                                                  const_cast<CUtensorMap*>(job.out_maps));
+    k_out_maps<OutT><<<job.n_groups, 64, 0, st>>>(tmpl, tmpl_lo, tmpl_f32, job.groups, job.cblocks, job.out, job.out32,
+                                                  job.t24_off, first, const_cast<CUtensorMap*>(job.out_maps));
     HGT_LAUNCH_CHECK();
   }
   const size_t smem = tile_smem_bytes<BN, KB, fwd_out_stage<BN>(), P, AF>();
@@ -376,6 +469,8 @@ int run_fwd(const FwdOps& ops, const float* bias, int32_t cb_width, const hgt_li
   job.groups = groups;
   job.cblocks = cblocks;
   job.out = out;
+  job.out32 = ops.out32;
+  job.t24_off = ops.t24_off;
   job.out_maps = out_maps;
   job.n_groups = n_groups;
   job.cb_width = cb_width;
@@ -434,14 +529,15 @@ size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_gr
   const size_t halves = products == 1 ? 1 : 2;
   const size_t a = splits_a_first(cb_width) ? halves * hgt_align_up((size_t)a_rows * Kp * 2, 256) : 0;
   return 4 * 256 + a + halves * hgt_align_up((size_t)w_rows * Kp * 2, 256) +
-         hgt_align_up((size_t)n_out_maps(h_groups, n_groups) * sizeof(CUtensorMap), 256);
+         hgt_align_up((size_t)n_out_maps(h_groups, n_groups) * 2 * sizeof(CUtensorMap), 256);   // two for 24-bit tables
 }
 
 template <class OutT>
 static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, const __nv_bfloat16* a_lo_in,
                   const float* W, const float* bias, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
                   const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
-                  int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st);
+                  int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st, float* out32 = nullptr,
+                  int64_t t24_off = 0);
 
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
                         const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
@@ -459,6 +555,14 @@ int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float
                 workspace, workspace_bytes, st);
 }
 
+int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
+                        const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
+                        const hgt_lin_cblock* cblocks, float* out32, int64_t t24_off, hgt_t24* out,
+                        int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, products,
+                workspace, workspace_bytes, st, out32, t24_off);
+}
+
 extern "C" int hgt_typed_linear_presplit_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K,
                                                          int32_t cb_width, size_t* out_bytes) {
   HGT_REQUIRE(out_bytes && (h_groups || n_groups == 0), "hgt_typed_linear_presplit_workspace_bytes: NULL argument");
@@ -470,7 +574,8 @@ template <class OutT>
 static int typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W, const float* bias, int32_t K,
                                  int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                                  int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out, void* workspace,
-                                 size_t workspace_bytes, cudaStream_t st) {
+                                 size_t workspace_bytes, cudaStream_t st, float* out32 = nullptr,
+                                 int64_t t24_off = 0) {
   HGT_REQUIRE(a_hi, "hgt_typed_linear_presplit: NULL operand");          // a_lo == NULL: one bf16 product
   HGT_REQUIRE(K % 8 == 0 && hgt_typed_linear_tc_supported(K, K, cb_width),
               "hgt_typed_linear_presplit: unsupported shape K=%d cb_width=%d", K, cb_width);
@@ -479,14 +584,14 @@ static int typed_linear_presplit(const void* a_hi, const void* a_lo, const float
     for (int g0 = 0; g0 < n_groups; g0 += kMaxGroups) {
       const int n = n_groups - g0 < kMaxGroups ? n_groups - g0 : kMaxGroups;
       int rc = typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups + g0, h_groups + g0, n, cblocks, out,
-                                     workspace, workspace_bytes, st);
+                                     workspace, workspace_bytes, st, out32, t24_off);
       if (rc) return rc;
     }
     return 0;
   }
   return tc_run(nullptr, 0, reinterpret_cast<const __nv_bfloat16*>(a_hi), reinterpret_cast<const __nv_bfloat16*>(a_lo),
                 W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, a_lo ? 3 : 1, workspace, workspace_bytes,
-                st);
+                st, out32, t24_off);
 }
 
 extern "C" int hgt_typed_linear_presplit(const void* a_hi, const void* a_lo, const float* W, const float* bias,
@@ -507,16 +612,29 @@ extern "C" int hgt_typed_linear_presplit_bf16(const void* a_hi, const void* a_lo
                                static_cast<__nv_bfloat16*>(out), workspace, workspace_bytes, (cudaStream_t)stream_);
 }
 
+extern "C" int hgt_typed_linear_presplit_t24(const void* a_hi, const void* a_lo, const float* W, const float* bias,
+                                             int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                                             const hgt_lin_group* h_groups, int32_t n_groups,
+                                             const hgt_lin_cblock* cblocks, float* out, int64_t t24_off, void* out24,
+                                             void* workspace, size_t workspace_bytes, void* stream_) {
+  return typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks,
+                               static_cast<hgt_t24*>(out24), workspace, workspace_bytes, (cudaStream_t)stream_, out,
+                               t24_off);
+}
+
 template <class OutT>
 static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, const __nv_bfloat16* a_lo_in,
                   const float* W, const float* bias, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
                   const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
-                  int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+                  int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st, float* out32,
+                  int64_t t24_off) {
   HGT_REQUIRE(hgt_typed_linear_tc_supported(lda, K, cb_width), "hgt_typed_linear(tc): unsupported K=%d cb_width=%d", K,
               cb_width);
   HGT_REQUIRE(products == 3 || products == 1, "hgt_typed_linear(tc): products=%d", products);
   const bool one = products == 1;
   FwdOps ops;
+  ops.out32 = out32;
+  ops.t24_off = t24_off;
   ops.K = K;
   ops.Kp = (K + 7) / 8 * 8;
   extents(h_groups, n_groups, cb_width, &ops.a_rows, &ops.w_rows);

@@ -26,6 +26,8 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace tcp {
@@ -360,10 +362,24 @@ __device__ __forceinline__ void put2(__nv_bfloat16* p, float2 v) {
   *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(v.x, v.y);
 }
 
+// Two neighbouring 24-bit elements (hgt_t24_round of v.x, v.y): their hi halves as one u32 and their lo bytes as the low
+// 16 bits of `lo` (the upper 16 are not defined).
+__device__ __forceinline__ void t24_pair(float2 v, uint32_t& hi, uint32_t& lo) {
+  const uint32_t a = hgt_t24_round(__float_as_uint(v.x)), b = hgt_t24_round(__float_as_uint(v.y));
+  hi = __byte_perm(a, b, 0x7632);
+  lo = __byte_perm(a, b, 0x0051);
+}
+
+template <class OutT> constexpr bool is_t24() { return std::is_same<OutT, hgt_t24>::value; }
+// Output tensor maps per (group, column block): one, or a hi-plane and a lo-plane map for 24-bit tables.
+template <class OutT> constexpr int out_maps_per_block() { return is_t24<OutT>() ? 2 : 1; }
+
 // Asynchronous epilogue of one consumer warpgroup (c): its 64 x BN accumulator goes out in 64-column blocks.  Each block
 // is written to shared memory as OutT in the SWIZZLE_128B layout of `map`'s boxes (128-byte rows, 64 rows; 16-byte chunk q
 // of row r at q ^ (r & 7); fp32: two boxes of 32 columns, bf16: one box of 64) and sent to global memory by TMA tensor
-// stores that one thread (the warpgroup's first) issues.  The map's extents clip the rows past the group and the columns
+// stores that one thread (the warpgroup's first) issues.  24-bit tables (hgt_t24): the hi halves as a bf16-like box of
+// 64 u16 at the buffer and the lo bytes as a box of 64 u8 (64-byte rows, SWIZZLE_64B: chunk q of row r at
+// q ^ ((r >> 1) & 3)) 8 KB further, stored through map[0] and map[1].  The map's extents clip the rows past the group and the columns
 // past the column block.  The stores drain while the consumer goes on to the next block or the next tile's products.
 // Block b uses buffer b & 1 of `stage` (two TMA_BUF_BYTES buffers, 1024-byte aligned); BN / 64 is even, so the buffers
 // alternate across tiles too.  Before a buffer is rewritten the issuing thread waits until the bulk group that read it two
@@ -374,10 +390,14 @@ template <int BN, class OutT, class Pair>
 __device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage, int c, int wq, int lane, Pair pair,
                                           const CUtensorMap* map, int col0, int row0, int cols) {
   static_assert(BN % 128 == 0, "the two buffers alternate across tiles only for an even number of 64-column blocks");
-  constexpr int BOX_COLS = 128 / (int)sizeof(OutT);
+  constexpr bool T24 = is_t24<OutT>();
+  constexpr int BOX_COLS = T24 ? 64 : 128 / (int)sizeof(OutT);
   const bool issuer = wq == 0 && lane == 0;
   const int r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
-  if (issuer) tensormap_acquire(map);
+  if (issuer) {
+    tensormap_acquire(map);
+    if constexpr (T24) tensormap_acquire(map + 1);
+  }
 #pragma unroll
   for (int blk = 0; blk < BN / 64; ++blk) {
     unsigned char* buf = stage + (blk & 1) * TMA_BUF_BYTES;
@@ -388,9 +408,19 @@ __device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = r0 + 8 * h, lc = 8 * j + c0 - 64 * blk;
-        const uint32_t x = (uint32_t)(lc % BOX_COLS) * sizeof(OutT);       // byte in the box row
-        put2(reinterpret_cast<OutT*>(buf + (lc / BOX_COLS) * 8192 + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))),
-             pair(r, 8 * j + c0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+        const float2 v = pair(r, 8 * j + c0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        if constexpr (T24) {
+          uint32_t hi, lo;
+          t24_pair(v, hi, lo);
+          const uint32_t x = (uint32_t)lc * 2;
+          *reinterpret_cast<uint32_t*>(buf + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))) = hi;
+          *reinterpret_cast<uint16_t*>(buf + 8192 + r * 64 + ((((lc >> 4) ^ ((r >> 1) & 3)) << 4) | (lc & 15))) =
+              (uint16_t)lo;
+        } else {
+          const uint32_t x = (uint32_t)(lc % BOX_COLS) * sizeof(OutT);     // byte in the box row
+          put2(reinterpret_cast<OutT*>(buf + (lc / BOX_COLS) * 8192 + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))),
+               v);
+        }
       }
     }
     fence_proxy_async_smem();                                   // the writes are visible to the tensor stores
@@ -399,6 +429,8 @@ __device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage
 #pragma unroll
       for (int bx = 0; bx < 64 / BOX_COLS; ++bx)
         if (64 * blk + BOX_COLS * bx < cols) tma_store_2d(map, s_u32(buf + bx * 8192), col0 + 64 * blk + BOX_COLS * bx, row0);
+      if constexpr (T24)
+        if (64 * blk < cols) tma_store_2d(map + 1, s_u32(buf + 8192), col0 + 64 * blk, row0);
       bulk_commit();
     }
   }
