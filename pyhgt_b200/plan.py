@@ -175,6 +175,18 @@ def get_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relatio
     return plan
 
 
+def tile_bounds(n_rows, n_edges, n_ranges=0):
+    """(max_tiles, max_split, max_hubs): what hgt_plan_tiles can emit over `n_rows` rows holding `n_edges` edges (or over
+    `n_ranges` row ranges of them, hgt_plan_range_tiles).  Sync-free plans size their tile and hub arrays with these and
+    keep them as the host-side bounds; max_split is 0 when no row can exceed TILE_SPLIT_EDGES.  A tile starts at the
+    first row (of each range), where the cost prefix 2 * row_ptr[k] + k enters a new bucket of 2 * TILE_TARGET_EDGES, and
+    after each hub; a hub (deg > split) takes ceil(deg / split) <= 2 * (deg // split) pieces."""
+    split = TILE_SPLIT_EDGES
+    max_tiles = (2 * n_edges + n_rows) // (2 * TILE_TARGET_EDGES) + 3 * (n_edges // split) + 16 + n_ranges
+    max_split = 2 * (n_edges // split) + 1 if n_edges > split else 0
+    return max_tiles, max_split, n_edges // split + 1
+
+
 def build_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relations, host_meta=None):
     dev = node_type.device
     if dev.type != "cuda":
@@ -278,19 +290,17 @@ def build_plan(node_type, edge_index, edge_type, edge_time, num_types, num_relat
               csr_eid.data_ptr(), N, E, T, R, pair_of_d.data_ptr(), pair_row0_d.data_ptr(), type_row0_d.data_ptr(),
               rows, P * RTE_MAX_LEN, kv_row.data_ptr(), _lib.ptr(rte_row), flags_d.data_ptr(), st)
 
-    max_tiles = (2 * E + N) // (2 * TILE_TARGET_EDGES) + 3 * (E // TILE_SPLIT_EDGES) + 16
+    max_tiles, max_split, max_hubs = tile_bounds(N, E)
     tiles = torch.empty((max_tiles, 4), **i32)
-    max_hubs = E // TILE_SPLIT_EDGES + 1
     hubs = torch.empty((max_hubs, 4), **i32)
     n_tiles_d = torch.zeros(4, **i32)
     if sync_free:
         # counts stay on the device; the host-side fields become the bounds the arrays were sized with
         _lib.call("hgt_plan_tiles", row_ptr.data_ptr(), N, E, TILE_TARGET_EDGES, TILE_SPLIT_EDGES, tiles.data_ptr(),
                   max_tiles, hubs.data_ptr(), max_hubs, n_tiles_d.data_ptr(), None, ws.data_ptr(), ws.numel(), st)
-        has_hub = E > TILE_SPLIT_EDGES
         n_tiles = max_tiles if N > 0 else 0
-        n_split = 2 * (E // TILE_SPLIT_EDGES) + 1 if has_hub else 0
-        n_hubs = max_hubs if has_hub else 0
+        n_split = max_split
+        n_hubs = max_hubs if max_split > 0 else 0
     else:
         n_tiles_h = (ctypes.c_int32 * 4)()
         _lib.call("hgt_plan_tiles", row_ptr.data_ptr(), N, E, TILE_TARGET_EDGES, TILE_SPLIT_EDGES, tiles.data_ptr(),
@@ -369,17 +379,14 @@ def source_index(plan, which, with_pos=False):
         pos = None
         _lib.call("hgt_plan_source_index", key.data_ptr(), _lib.ptr(other), plan.row_ptr.data_ptr(), plan.n_nodes, E,
                   n_rows, ptr.data_ptr(), dst.data_ptr(), _lib.ptr(oth), ws.data_ptr(), ws.numel(), st)
-    max_tiles = (2 * E + n_rows) // (2 * TILE_TARGET_EDGES) + 3 * (E // TILE_SPLIT_EDGES) + 16
+    max_tiles, max_split, max_hubs = tile_bounds(n_rows, E)
     tiles = torch.empty((max_tiles, 4), **i32)
-    max_hubs = E // TILE_SPLIT_EDGES + 1
     hubs = torch.empty((max_hubs, 4), **i32)
     counts = torch.zeros(4, **i32)
     _lib.call("hgt_plan_tiles", ptr.data_ptr(), n_rows, E, TILE_TARGET_EDGES, TILE_SPLIT_EDGES, tiles.data_ptr(),
               max_tiles, hubs.data_ptr(), max_hubs, counts.data_ptr(), None, ws.data_ptr(), ws.numel(), st)
-    has_hub = E > TILE_SPLIT_EDGES
     idx = SourceIndex(n_rows=n_rows, ptr=ptr, dst=dst, oth=oth, tiles=tiles, n_tiles=max_tiles if n_rows > 0 else 0,
-                      n_split=2 * (E // TILE_SPLIT_EDGES) + 1 if has_hub else 0, hubs=hubs,
-                      n_hubs=max_hubs if has_hub else 0, counts_dev=counts, pos=pos)
+                      n_split=max_split, hubs=hubs, n_hubs=max_hubs if max_split > 0 else 0, counts_dev=counts, pos=pos)
     plan._source_index[which] = idx
     return idx
 

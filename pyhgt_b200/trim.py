@@ -303,9 +303,7 @@ def _range_view(plan, ranges):
     N, E = plan.n_nodes, plan.n_edges
     n_rows = sum(b - a for a, b in ranges)
     rng = _plan._to_dev_async(np.asarray(ranges if ranges else [(0, 0)], dtype=np.int32).reshape(-1), dev)
-    split = _plan.TILE_SPLIT_EDGES
-    max_tiles = (2 * E + N) // (2 * _plan.TILE_TARGET_EDGES) + 3 * (E // split) + 16 + len(ranges)
-    max_hubs = E // split + 1
+    max_tiles, max_split, max_hubs = _plan.tile_bounds(N, E, len(ranges))
     tiles = torch.empty((max_tiles, 4), **i32)
     hubs = torch.empty((max_hubs, 4), **i32)
     counts = torch.zeros(4, **i32)
@@ -313,10 +311,8 @@ def _range_view(plan, ranges):
     _lib.call("hgt_plan_workspace_bytes", N, E, ctypes.byref(ws_bytes))
     ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
     _lib.call("hgt_plan_range_tiles", plan.row_ptr.data_ptr(), N, E, rng.data_ptr(), len(ranges), n_rows,
-              _plan.TILE_TARGET_EDGES, split, tiles.data_ptr(), max_tiles, hubs.data_ptr(), max_hubs,
-              counts.data_ptr(), ws.data_ptr(), ws.numel(), _plan._stream())
-    has_hub = E > split
-    return dataclasses.replace(plan, tiles=tiles, n_tiles=max_tiles if n_rows > 0 else 0,
-                               n_split=2 * (E // split) + 1 if has_hub else 0, hubs=hubs,
-                               n_hubs=max_hubs if has_hub else 0, tile_counts_dev=counts, dst_ranges=rng,
+              _plan.TILE_TARGET_EDGES, _plan.TILE_SPLIT_EDGES, tiles.data_ptr(), max_tiles, hubs.data_ptr(),
+              max_hubs, counts.data_ptr(), ws.data_ptr(), ws.numel(), _plan._stream())
+    return dataclasses.replace(plan, tiles=tiles, n_tiles=max_tiles if n_rows > 0 else 0, n_split=max_split, hubs=hubs,
+                               n_hubs=max_hubs if max_split > 0 else 0, tile_counts_dev=counts, dst_ranges=rng,
                                n_dst_ranges=len(ranges), _layer_tables={}, _source_index={})

@@ -18,7 +18,8 @@ import torch
 
 from pyhgt_b200 import _lib, plan as P, synth
 from tests.test_gpu_bf16_tables import _conv, _dev, _gemm_table, _inputs, _rel, _st
-from tests.test_gpu_edge_instances import SHAPES, _edge_ref, _plan, _q_scale, _tables, lane_map, ring_fallback
+from tests.test_gpu_edge_instances import (HOT_SHAPES, SHAPES, _check_hot, _edge_ref, _plan, _q_scale, _tables, lane_map,
+                                           ring_fallback)
 from tests.test_t24_format_cpu import encode
 
 pytestmark = pytest.mark.gpu
@@ -163,6 +164,9 @@ def test_c2_projection_table_equals_encoded_fp32():
 # 2. the edge forward on 24-bit tables
 
 T24_SHAPES = [(d, H) for d, H in SHAPES if d % 8 == 0]
+# d % 8 == 0 shapes for the two lane maps the shared lists reach only with d % 8 != 0: <1,4> (d_k 9) and <2,2> (d_k 36)
+T24_EXTRA_SHAPES = [(72, 8), (72, 2)]
+T24_HOT_SHAPES = [(d, H) for d, H in HOT_SHAPES if d % 8 == 0] + T24_EXTRA_SHAPES
 
 
 def _edge(fn, plan, T, q, kv, kvr, d, H, variant, gelu):
@@ -189,9 +193,36 @@ def _edge(fn, plan, T, q, kv, kvr, d, H, variant, gelu):
 @pytest.mark.parametrize("rte", [False, True])
 @pytest.mark.parametrize("d,H", T24_SHAPES)
 def test_edge_forward_t24(d, H, rte, variant):
+    _check_edge_forward_t24(d, H, rte, variant, False)
+
+
+@pytest.mark.parametrize("variant", [1, 2])
+@pytest.mark.parametrize("rte", [False, True])
+@pytest.mark.parametrize("d,H", T24_EXTRA_SHAPES)
+def test_edge_forward_t24_extra_lane_maps(d, H, rte, variant):
+    _check_edge_forward_t24(d, H, rte, variant, False)
+
+
+def test_t24_shape_lists_reach_every_lane_map():
+    """The 24-bit forward runs (and its (m, l) is checked against float64) at all 12 <VEC, NCH> lane maps, with
+    ordinary and with hot scores."""
+    every = {(v, n) for v in (1, 2, 4) for n in (1, 2, 4, 8)}
+    assert {lane_map(d, H) for d, H in T24_SHAPES + T24_EXTRA_SHAPES} == every
+    assert {lane_map(d, H) for d, H in T24_HOT_SHAPES} == every
+    assert all(d % 8 == 0 for d, _ in T24_HOT_SHAPES + T24_EXTRA_SHAPES)
+
+
+@pytest.mark.parametrize("variant", [1, 2])
+@pytest.mark.parametrize("d,H", T24_HOT_SHAPES)
+def test_edge_forward_t24_hot(d, H, variant):
+    """Hot scores (most exp terms underflow in fp32): the online rescale and the hub pieces' merge on 24-bit rows."""
+    _check_edge_forward_t24(d, H, True, variant, True)
+
+
+def _check_edge_forward_t24(d, H, rte, variant, hot):
     plan, T = _plan(d, H, rte, seed=d + H)
     assert plan.n_split > 0
-    q, kv, kvr = _tables(plan, d, rte, d, torch.float32, _q_scale(d, H, False))
+    q, kv, kvr = _tables(plan, d, rte, d, torch.float32, _q_scale(d, H, hot))
     kv24 = encode_t(kv)
     kvr24 = None if kvr is None else encode_t(kvr)
     kv_dec = decode(kv24, 2 * d)
@@ -216,12 +247,19 @@ def test_edge_forward_t24(d, H, rte, variant):
                 if name == "stats":
                     a, b = a[has_in], b[has_in]
                 assert torch.equal(a, b), (name, gelu)
-    ref, att_ref, _, _ = _edge_ref(plan, q.cpu().double(), kv_dec.cpu().double(),
-                                   None if kvr_dec is None else kvr_dec.cpu().double(), H)
-    agg, att = got[0], got[1]
-    torch.testing.assert_close(agg.cpu().double(), torch.nn.functional.gelu(ref), rtol=1e-4, atol=1e-5)
+    ref, att_ref, m_ref, l_ref = _edge_ref(plan, q.cpu().double(), kv_dec.cpu().double(),
+                                           None if kvr_dec is None else kvr_dec.cpu().double(), H)
+    if hot:
+        _check_hot(att_ref)
+    agg, att, stats = got[0], got[1], got[2].cpu().double()
+    # the tolerances of tests/test_gpu_edge_instances.py (hot: the rounding error of a score grows with its size)
+    atol = 1e-4 if hot else 1e-5
+    torch.testing.assert_close(agg.cpu().double(), torch.nn.functional.gelu(ref), rtol=1e-4, atol=atol)
     eid = plan.csr_eid[:plan.n_edges].cpu().long()
     torch.testing.assert_close(att.cpu().double()[eid], att_ref, rtol=1e-4, atol=1e-6)
+    has_in = ((plan.row_ptr[1:] - plan.row_ptr[:-1]) > 0).cpu()
+    torch.testing.assert_close(stats[:, :H][has_in], m_ref[has_in], rtol=1e-5, atol=atol)
+    torch.testing.assert_close(stats[:, H:][has_in], l_ref[has_in], rtol=1e-4, atol=1e-5)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
