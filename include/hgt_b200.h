@@ -750,7 +750,8 @@ int64_t hgt_sampler_add_budget(const int64_t* h_target_ids, const int64_t* h_tar
  * ---------------------------------------------------------------------------------------------- */
 
 /* One <target type, source type, relation> adjacency in CSR form, rows in the reference dict's insertion order.  The
- * struct itself lives in DEVICE memory (an array of them per call), as do the arrays it points to. */
+ * struct itself lives in DEVICE memory (an array of them per call); the arrays it points to are device memory or
+ * device-mapped page-locked host memory (hgt_host_register). */
 typedef struct {
   const int64_t* row_of; int64_t n_row_of;   /* target id -> CSR row, -1 = no adjacency */
   const int64_t* ptr;                         /* [rows+1] positions into nbr / time */
@@ -911,6 +912,32 @@ int hgt_gsample_batch_rebuild_write_masked(const hgt_gsample_batch_state* h_stat
                                            int32_t feat_dim, int64_t* node_type, int64_t* node_time,
                                            float* node_feature, int64_t* edge_index, int64_t* edge_type,
                                            int64_t* edge_time, void* stream);
+
+/* Graphs in page-locked host memory (sampler.py: DeviceGraph(..., placement="host")).  hgt_host_register page-locks
+ * [host, host + bytes) (cudaHostRegister, mapped) and returns in *dev_ptr the address device code reads it at;
+ * hgt_host_unregister undoes it once no kernel reads the range any more.  Blocks whose row_of / ptr / nbr / time are
+ * such addresses work with every sampler entry point (the kernels read them in place); the two rebuild passes below are
+ * the ones meant for them: the count pass reads each sampled target's neighbour list once and leaves one 16-byte hit
+ * record per kept edge in `hits` (device, room for hit_cap < 2^31 records), with their number in *n_hits (device; it
+ * counts past hit_cap).  The write pass lays the edges out from the n_hits records alone, or, with hits NULL (the records
+ * did not fit), re-reads the lists like hgt_gsample_batch_rebuild_write; it gathers feature rows (feat may point to host
+ * tables) with 16-byte loads when they are 16-byte aligned.  min_ser may be NULL (no mask) or a table as for the _masked
+ * entry points.  Otherwise as hgt_gsample_batch_rebuild_count / _write: the outputs are identical. */
+int hgt_host_register(void* host, size_t bytes, void** dev_ptr);
+int hgt_host_unregister(void* host);
+int hgt_gsample_batch_rebuild_count_host(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
+                                         int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                         int64_t n_count, int64_t max_rows, const int64_t* feat_rows, void* hits,
+                                         int64_t hit_cap, int64_t* n_hits, int64_t* ex, int64_t* totals, int32_t* flags,
+                                         void* workspace, size_t workspace_bytes, void* stream);
+int hgt_gsample_batch_rebuild_write_host(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
+                                         int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                         const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
+                                         const int64_t* type_out, const int64_t* self_off, int64_t self_rel,
+                                         const int64_t* mem_out, int64_t max_rows, const void* hits, int64_t n_hits,
+                                         const float* const* feat, int32_t feat_dim, int64_t* node_type,
+                                         int64_t* node_time, float* node_feature, int64_t* edge_index,
+                                         int64_t* edge_type, int64_t* edge_time, void* stream);
 
 /* Disjoint union of B batches in the to_torch layout (sampler.py: merge_batches).  The member structs live in DEVICE
  * memory.  loc_off [B*(T+1)]: member b's first local row of each type (loc_off[b*(T+1)+T] = its node count); uoff [B*T]:

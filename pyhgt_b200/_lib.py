@@ -126,6 +126,13 @@ SIGNATURES = {
     "hgt_gsample_batch_rebuild_count_masked": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_gsample_batch_rebuild_write_masked": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p,
                                                _p, _p, _p, _p, _p, _p],
+    # graphs in page-locked host memory (sampler.DeviceGraph(..., placement="host"))
+    "hgt_host_register": [_p, _sz, _c.POINTER(_p)],
+    "hgt_host_unregister": [_p],
+    "hgt_gsample_batch_rebuild_count_host": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _sz,
+                                             _p],
+    "hgt_gsample_batch_rebuild_write_host": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p,
+                                             _i32, _p, _p, _p, _p, _p, _p, _p],
     "hgt_merge_batches": [_p, _i32, _i32, _p, _p, _i64, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p],
     # trimmed forward (GNN.forward(out_nodes=), trim.py)
     "hgt_trim_layout": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],

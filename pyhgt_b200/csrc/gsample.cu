@@ -469,6 +469,168 @@ __global__ void k_rb_nodes(hgt_gsample_batch_state st, const int64_t* node_off, 
   }
 }
 
+// ---- graphs in page-locked host memory (sampler.py: DeviceGraph(..., placement="host")) ------------------------------
+// The kernels above read row_of / ptr / nbr / time and the feature tables in place wherever they live, so add_budget's
+// random neighbour draws run unchanged on a host-resident graph.  The rebuild gets its own instances: over PCIe, reading
+// every sampled target's neighbour list twice (count pass, then write pass) doubles the dominant traffic, and 4-byte
+// feature copies leave the link idle.  The count pass below reads each list once and leaves one hit record per kept edge
+// in device scratch; the write pass lays the edges out from those records alone.
+
+constexpr int kListUnroll = 8;   // neighbour ids in flight per lane in the single-read count pass
+constexpr int kRowUnroll = 4;    // 16-byte feature loads in flight per lane in the host gather
+
+// A kept edge: {m * n_blocks + b, target ser r, rank among r's kept edges in list order, source ser}.  Its output position
+// is blk_out + (ex[r] - ex[0]) + rank, so the records may sit in the scratch in any order.
+using Hit = int4;
+
+// k_rb_count's counts, flags and mask, plus the hit records: slots claimed with one atomic per warp and kListUnroll * 32
+// neighbours; records past hit_cap are dropped (n_hits still counts them, so the caller sees the overflow).
+__global__ void k_rb_count_host(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
+                                const int64_t* min_ser, const int64_t* cnt_off, int64_t* cnt, Hit* hits,
+                                int64_t hit_cap, unsigned long long* n_hits, int32_t* flags) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int b = blockIdx.y;
+  const int64_t mbk = (int64_t)blockIdx.z * n_blocks + b;
+  const hgt_gsample_block blk = blocks[b];
+  const int T = blk.tgt_type, S = blk.src_type;
+  if (r >= cnt_off[mbk + 1] - cnt_off[mbk]) return;
+  const Member mb = member(st, blockIdx.z);
+  int64_t c = 0;                                                        // kept edges so far (warp-uniform)
+  if (r < mb.n_layer[T]) {
+    const int64_t tid = st.lid[mb.lid_off[T] + r];
+    const int64_t row = tid < blk.n_row_of ? blk.row_of[tid] : -1;
+    if (row >= 0) {
+      const int64_t a = blk.ptr[row], e = blk.ptr[row + 1];
+      const int64_t tt = st.ltime[mb.type_off[T] + tid];
+      const int64_t sb = mb.type_off[S], sn = mb.type_off[S + 1] - sb;
+      const unsigned below = (1u << lane) - 1u;
+      for (int64_t p0 = a; p0 < e; p0 += 32 * kListUnroll) {
+        int64_t sid[kListUnroll];
+#pragma unroll
+        for (int u = 0; u < kListUnroll; ++u) {
+          const int64_t p = p0 + 32 * u + lane;
+          sid[u] = p < e ? blk.nbr[p] : -1;
+        }
+        int32_t sser[kListUnroll];
+        unsigned keep[kListUnroll];
+        int n_kept = 0;
+#pragma unroll
+        for (int u = 0; u < kListUnroll; ++u) {
+          const int64_t p = p0 + 32 * u + lane;
+          sser[u] = -1;
+          if (p < e) {
+            if (sid[u] < 0 || sid[u] >= sn) flags[0] = 1;
+            else sser[u] = st.ser[sb + sid[u]];
+          }
+          const bool kept = sser[u] >= 0 && !masked_out(min_ser, b, r, sser[u]);
+          if (kept) {
+            const int64_t dt = tt - st.ltime[sb + sid[u]] + 120;
+            if (dt < 0 || dt >= HGT_RTE_MAX_LEN) flags[1] = 1;
+          }
+          keep[u] = __ballot_sync(kFull, kept);
+          n_kept += __popc(keep[u]);
+        }
+        if (n_kept == 0) continue;
+        unsigned long long base = 0;
+        if (lane == 0) base = atomicAdd(n_hits, (unsigned long long)n_kept);
+        base = __shfl_sync(kFull, base, 0);
+#pragma unroll
+        for (int u = 0; u < kListUnroll; ++u) {
+          const int k = __popc(keep[u] & below);
+          if ((keep[u] >> lane) & 1u && (int64_t)base + k < hit_cap)
+            hits[base + k] = make_int4((int)mbk, (int)r, (int)(c + k), sser[u]);
+          base += __popc(keep[u]);
+          c += __popc(keep[u]);
+        }
+      }
+    }
+  }
+  if (lane == 0) cnt[cnt_off[mbk] + r] = c;
+}
+
+// One thread per hit record: k_rb_write's outputs without touching the graph (the source id and both times come from
+// the member's device state).
+__global__ void k_rb_write_hits(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
+                                const Hit* hits, int64_t n_hits, const int64_t* cnt_off, const int64_t* ex,
+                                const int64_t* blk_out, const int64_t* node_off, MemOut mo, int64_t* edge_index,
+                                int64_t* edge_type, int64_t* edge_time) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n_hits) return;
+  const Hit h = hits[i];
+  const int64_t mbk = h.x;
+  const int m = (int)(mbk / n_blocks), b = (int)(mbk % n_blocks);
+  if (blk_out[mbk] < 0) return;
+  const int T = blocks[b].tgt_type, S = blocks[b].src_type;
+  const Member mb = member(st, m);
+  const int64_t r = h.y, sser = h.w;
+  const int64_t* noff = node_off + (int64_t)m * st.num_types;
+  const int64_t eb = mo.edge_base(m), n_edges = mo.edges(m);
+  const int64_t o = blk_out[mbk] + ex[cnt_off[mbk] + r] - ex[cnt_off[mbk]] + h.z;
+  const int64_t tid = st.lid[mb.lid_off[T] + r], sid = st.lid[mb.lid_off[S] + sser];
+  edge_index[2 * eb + o] = noff[S] + sser;                               // row 0 = source (data.py:245,254)
+  edge_index[2 * eb + n_edges + o] = noff[T] + r;
+  edge_type[eb + o] = blocks[b].rel;
+  edge_time[eb + o] = st.ltime[mb.type_off[T] + tid] - st.ltime[mb.type_off[S] + sid] + 120;   // data.py:250
+}
+
+// k_rb_nodes with the feature rows read from host memory: 16-byte loads when the row and the output row are 16-byte
+// aligned (feat_dim % 4 == 0 and aligned tables), kRowUnroll of them per lane issued before the first store.
+__global__ void k_rb_nodes_host(hgt_gsample_batch_state st, const int64_t* node_off, const int64_t* type_out,
+                                const int64_t* self_off, int64_t self_rel, MemOut mo, const float* const* feat,
+                                int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature,
+                                int64_t* edge_index, int64_t* edge_type, int64_t* edge_time) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int t = blockIdx.y;
+  const int m = blockIdx.z;
+  const Member mb = member(st, m);
+  const int64_t noff = node_off[(int64_t)m * st.num_types + t];
+  if (noff < 0 || r >= mb.n_layer[t]) return;
+  const int64_t lrow = noff + r;
+  const int64_t row = mo.node_base(m) + lrow;
+  const int64_t tid = st.lid[mb.lid_off[t] + r];
+  if (lane == 0) {
+    node_type[row] = type_out[t];
+    node_time[row] = st.ltime[mb.type_off[t] + tid];
+    const int64_t so = self_off[(int64_t)m * st.num_types + t];
+    if (so >= 0) {
+      const int64_t e = so + r, eb = mo.edge_base(m);
+      edge_index[2 * eb + e] = lrow;
+      edge_index[2 * eb + mo.edges(m) + e] = lrow;
+      edge_type[eb + e] = self_rel;
+      edge_time[eb + e] = 120;
+    }
+  }
+  if (!node_feature) return;
+  const float* src = feat[t] + tid * (int64_t)feat_dim;
+  float* dst = node_feature + row * (int64_t)feat_dim;
+  if ((feat_dim & 3) == 0 && (((uintptr_t)src | (uintptr_t)dst) & 15) == 0) {
+    const float4* s4 = reinterpret_cast<const float4*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    const int n4 = feat_dim >> 2;
+    for (int c0 = 0; c0 < n4; c0 += 32 * kRowUnroll) {
+      float4 v[kRowUnroll];
+#pragma unroll
+      for (int u = 0; u < kRowUnroll; ++u)
+        if (c0 + 32 * u + lane < n4) v[u] = s4[c0 + 32 * u + lane];
+#pragma unroll
+      for (int u = 0; u < kRowUnroll; ++u)
+        if (c0 + 32 * u + lane < n4) d4[c0 + 32 * u + lane] = v[u];
+    }
+  } else {
+    for (int c0 = 0; c0 < feat_dim; c0 += 32 * kRowUnroll) {
+      float v[kRowUnroll];
+#pragma unroll
+      for (int u = 0; u < kRowUnroll; ++u)
+        if (c0 + 32 * u + lane < feat_dim) v[u] = src[c0 + 32 * u + lane];
+#pragma unroll
+      for (int u = 0; u < kRowUnroll; ++u)
+        if (c0 + 32 * u + lane < feat_dim) dst[c0 + 32 * u + lane] = v[u];
+    }
+  }
+}
+
 struct BudgetScratch {
   int64_t *seg_cnt, *seg_off, *cand_pos, *cand_slot, *cand_time;
   void* cub_tmp;
@@ -637,10 +799,12 @@ int select(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMembe
   return 0;
 }
 
+// n_hits != NULL: the single-read count pass of a host-resident graph, leaving up to hit_cap hit records in `hits`.
 int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
                   const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count, int64_t max_rows,
-                  const int64_t* feat_rows, int64_t* ex, int64_t* totals, int32_t* flags, void* workspace,
-                  size_t workspace_bytes, void* stream, const char* what) {
+                  const int64_t* feat_rows, Hit* hits, int64_t hit_cap, unsigned long long* n_hits, int64_t* ex,
+                  int64_t* totals, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream,
+                  const char* what) {
   HGT_REQUIRE(n_blocks >= 0 && n_blocks < 65536 && hs.num_types < 65536 && hs.n_members >= 1 &&
                   hs.n_members < 65536 && max_rows >= 0,
               "%s: bad arguments", what);
@@ -652,7 +816,14 @@ int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* bl
   void* cub_tmp = (char*)workspace + hgt_align_up(sizeof(int64_t) * (n_count + 1), 256);
   size_t tmp = workspace_bytes - hgt_align_up(sizeof(int64_t) * (n_count + 1), 256);
   HGT_CHECK_CUDA(cudaMemsetAsync(cnt + n_count, 0, sizeof(int64_t), st));
-  if (n_blocks > 0 && max_rows > 0) {
+  if (n_hits) {
+    HGT_CHECK_CUDA(cudaMemsetAsync(n_hits, 0, sizeof(unsigned long long), st));
+    if (n_blocks > 0 && max_rows > 0) {
+      k_rb_count_host<<<dim3((unsigned)blocks_for(max_rows, kWarps), n_blocks, hs.n_members), kThreads, 0, st>>>(
+          hs, blocks, n_blocks, min_ser, cnt_off, cnt, hits, hit_cap, n_hits, flags);
+      HGT_LAUNCH_CHECK();
+    }
+  } else if (n_blocks > 0 && max_rows > 0) {
     k_rb_count<<<dim3((unsigned)blocks_for(max_rows, kWarps), n_blocks, hs.n_members), kThreads, 0, st>>>(
         hs, blocks, n_blocks, min_ser, cnt_off, cnt, flags);
     HGT_LAUNCH_CHECK();
@@ -671,10 +842,13 @@ int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* bl
   return 0;
 }
 
+// host_graph: the instances for a host-resident graph (k_rb_write_hits over the n_hits records in `hits`, or k_rb_write
+// when hits is NULL; k_rb_nodes_host).
 int rebuild_write(const hgt_gsample_batch_state& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
                   const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out,
                   const int64_t* node_off,
                   const int64_t* type_out, const int64_t* self_off, int64_t self_rel, MemOut mo, int64_t max_rows,
+                  bool host_graph, const Hit* hits, int64_t n_hits,
                   const float* const* feat, int32_t feat_dim, int64_t* node_type, int64_t* node_time,
                   float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream,
                   const char* what) {
@@ -683,15 +857,26 @@ int rebuild_write(const hgt_gsample_batch_state& hs, const hgt_gsample_block* bl
               "%s: bad arguments", what);
   cudaStream_t st = (cudaStream_t)stream;
   if (max_rows == 0) return 0;
-  if (n_blocks > 0) {
+  if (hits) {
+    if (n_hits > 0) {
+      k_rb_write_hits<<<(unsigned)blocks_for(n_hits), kThreads, 0, st>>>(hs, blocks, n_blocks, hits, n_hits, cnt_off, ex,
+                                                                        blk_out, node_off, mo, edge_index, edge_type,
+                                                                        edge_time);
+      HGT_LAUNCH_CHECK();
+    }
+  } else if (n_blocks > 0) {
     k_rb_write<<<dim3((unsigned)blocks_for(max_rows, kWarps), n_blocks, hs.n_members), kThreads, 0, st>>>(
         hs, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, mo, edge_index, edge_type, edge_time);
     HGT_LAUNCH_CHECK();
   }
   if (hs.num_types > 0) {
-    k_rb_nodes<<<dim3((unsigned)blocks_for(max_rows, kWarps), hs.num_types, hs.n_members), kThreads, 0, st>>>(
-        hs, node_off, type_out, self_off, self_rel, mo, feat, feat_dim, node_type, node_time, node_feature, edge_index,
-        edge_type, edge_time);
+    const dim3 grid((unsigned)blocks_for(max_rows, kWarps), hs.num_types, hs.n_members);
+    if (host_graph)
+      k_rb_nodes_host<<<grid, kThreads, 0, st>>>(hs, node_off, type_out, self_off, self_rel, mo, feat, feat_dim,
+                                                 node_type, node_time, node_feature, edge_index, edge_type, edge_time);
+    else
+      k_rb_nodes<<<grid, kThreads, 0, st>>>(hs, node_off, type_out, self_off, self_rel, mo, feat, feat_dim, node_type,
+                                            node_time, node_feature, edge_index, edge_type, edge_time);
     HGT_LAUNCH_CHECK();
   }
   return 0;
@@ -747,8 +932,8 @@ extern "C" int hgt_gsample_rebuild_count(const hgt_gsample_state* h_state, const
                                          const int64_t* feat_rows, int64_t* ex, int64_t* totals, int32_t* flags,
                                          void* workspace, size_t workspace_bytes, void* stream) {
   HGT_REQUIRE(h_state, "hgt_gsample_rebuild_count: bad arguments");
-  return rebuild_count(as_batch(*h_state), blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, ex, totals,
-                       flags, workspace, workspace_bytes, stream, "hgt_gsample_rebuild_count");
+  return rebuild_count(as_batch(*h_state), blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, nullptr, 0,
+                       nullptr, ex, totals, flags, workspace, workspace_bytes, stream, "hgt_gsample_rebuild_count");
 }
 
 extern "C" int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks,
@@ -760,8 +945,8 @@ extern "C" int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const
                                          int64_t* edge_type, int64_t* edge_time, void* stream) {
   HGT_REQUIRE(h_state && n_edges >= 0, "hgt_gsample_rebuild_write: bad arguments");
   return rebuild_write(as_batch(*h_state), blocks, n_blocks, nullptr, cnt_off, ex, blk_out, node_off, type_out,
-                       self_off, self_rel, {nullptr, n_edges}, max_rows, feat, feat_dim, node_type, node_time, node_feature,
-                       edge_index, edge_type, edge_time, stream, "hgt_gsample_rebuild_write");
+                       self_off, self_rel, {nullptr, n_edges}, max_rows, false, nullptr, 0, feat, feat_dim, node_type,
+                       node_time, node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_rebuild_write");
 }
 
 // ---- B subgraphs at once ----------------------------------------------------------------------------------------------
@@ -806,8 +991,8 @@ extern "C" int hgt_gsample_batch_rebuild_count(const hgt_gsample_batch_state* h_
                                                int64_t max_rows, const int64_t* feat_rows, int64_t* ex, int64_t* totals,
                                                int32_t* flags, void* workspace, size_t workspace_bytes, void* stream) {
   HGT_REQUIRE(h_state, "hgt_gsample_batch_rebuild_count: bad arguments");
-  return rebuild_count(*h_state, blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, ex, totals, flags,
-                       workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count");
+  return rebuild_count(*h_state, blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, nullptr, 0, nullptr,
+                       ex, totals, flags, workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count");
 }
 
 extern "C" int hgt_gsample_batch_rebuild_count_masked(const hgt_gsample_batch_state* h_state,
@@ -817,8 +1002,8 @@ extern "C" int hgt_gsample_batch_rebuild_count_masked(const hgt_gsample_batch_st
                                                       int64_t* totals, int32_t* flags, void* workspace,
                                                       size_t workspace_bytes, void* stream) {
   HGT_REQUIRE(h_state && min_ser, "hgt_gsample_batch_rebuild_count_masked: bad arguments");
-  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, ex, totals, flags,
-                       workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count_masked");
+  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, nullptr, 0, nullptr,
+                       ex, totals, flags, workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count_masked");
 }
 
 extern "C" int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
@@ -831,8 +1016,8 @@ extern "C" int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_
                                                void* stream) {
   HGT_REQUIRE(h_state && mem_out, "hgt_gsample_batch_rebuild_write: bad arguments");
   return rebuild_write(*h_state, blocks, n_blocks, nullptr, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {mem_out, 0}, max_rows, feat, feat_dim, node_type, node_time, node_feature,
-                       edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write");
+                       self_rel, {mem_out, 0}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
+                       node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write");
 }
 
 extern "C" int hgt_gsample_batch_rebuild_write_masked(
@@ -843,6 +1028,54 @@ extern "C" int hgt_gsample_batch_rebuild_write_masked(
     int64_t* edge_type, int64_t* edge_time, void* stream) {
   HGT_REQUIRE(h_state && min_ser && mem_out, "hgt_gsample_batch_rebuild_write_masked: bad arguments");
   return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {mem_out, 0}, max_rows, feat, feat_dim, node_type, node_time, node_feature,
-                       edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write_masked");
+                       self_rel, {mem_out, 0}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
+                       node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write_masked");
+}
+
+// ---- graphs in page-locked host memory ------------------------------------------------------------------------------
+
+extern "C" int hgt_host_register(void* host, size_t bytes, void** dev_ptr) {
+  HGT_REQUIRE(host && bytes > 0 && dev_ptr, "hgt_host_register: bad arguments");
+  HGT_CHECK_CUDA(cudaHostRegister(host, bytes, cudaHostRegisterMapped));
+  const cudaError_t e = cudaHostGetDevicePointer(dev_ptr, host, 0);
+  if (e != cudaSuccess) {
+    cudaHostUnregister(host);
+    hgt_set_error("hgt_host_register: cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  return 0;
+}
+
+extern "C" int hgt_host_unregister(void* host) {
+  HGT_REQUIRE(host, "hgt_host_unregister: bad arguments");
+  HGT_CHECK_CUDA(cudaHostUnregister(host));
+  return 0;
+}
+
+extern "C" int hgt_gsample_batch_rebuild_count_host(const hgt_gsample_batch_state* h_state,
+                                                    const hgt_gsample_block* blocks, int32_t n_blocks,
+                                                    const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count,
+                                                    int64_t max_rows, const int64_t* feat_rows, void* hits,
+                                                    int64_t hit_cap, int64_t* n_hits, int64_t* ex, int64_t* totals,
+                                                    int32_t* flags, void* workspace, size_t workspace_bytes,
+                                                    void* stream) {
+  HGT_REQUIRE(h_state && n_hits && hit_cap >= 0 && hit_cap < (int64_t(1) << 31) && (hits || hit_cap == 0) &&
+                  (int64_t)n_blocks * h_state->n_members < (int64_t(1) << 31),
+              "hgt_gsample_batch_rebuild_count_host: bad arguments");
+  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, (Hit*)hits, hit_cap,
+                       (unsigned long long*)n_hits, ex, totals, flags, workspace, workspace_bytes, stream,
+                       "hgt_gsample_batch_rebuild_count_host");
+}
+
+extern "C" int hgt_gsample_batch_rebuild_write_host(
+    const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks, const int64_t* min_ser,
+    const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
+    const int64_t* self_off, int64_t self_rel, const int64_t* mem_out, int64_t max_rows, const void* hits,
+    int64_t n_hits, const float* const* feat, int32_t feat_dim, int64_t* node_type, int64_t* node_time,
+    float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream) {
+  HGT_REQUIRE(h_state && mem_out && n_hits >= 0, "hgt_gsample_batch_rebuild_write_host: bad arguments");
+  return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
+                       self_rel, {mem_out, 0}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
+                       node_time, node_feature, edge_index, edge_type, edge_time, stream,
+                       "hgt_gsample_batch_rebuild_write_host");
 }

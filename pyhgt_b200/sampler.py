@@ -21,7 +21,9 @@ The sampled ``edge_list`` values are ``[E_block, 2]`` int64 arrays of ``[target_
 builds Python lists of pairs with the same content and order); ``pyhgt_b200.data.to_torch`` and the reference's
 ``to_torch`` accept both.
 """
+import contextlib
 import ctypes as _c
+import weakref
 from collections import defaultdict
 from itertools import chain as _chain
 
@@ -477,17 +479,91 @@ MERGE_MEMBER_DTYPE = np.dtype([("node_feature", "<u8"), ("edge_index", "<u8"), (
 
 
 _I64_MAX = np.iinfo(np.int64).max
+_PAGE = 4096
+_HIT_ROOM = 8.0          # hit records a host-placed graph's first rebuild reserves per count slot
+
+
+def _pin(a, dtype):
+    """One page-locked copy of array ``a`` (as ``dtype``), mapped for the device: (host view, device address, page-aligned
+    buffer to unregister).  The buffer is whole pages of its own, so no two registrations share a page."""
+    from . import _lib
+    a = np.asarray(a, dtype=dtype)
+    nbytes = max(a.nbytes, 1)
+    size = -(-nbytes // _PAGE) * _PAGE
+    raw = np.empty(size + _PAGE, dtype=np.uint8)
+    off = (-raw.ctypes.data) % _PAGE
+    buf = raw[off:off + size]
+    view = buf[:a.nbytes].view(dtype).reshape(a.shape)
+    view[...] = a
+    dptr = _c.c_void_p()
+    _lib.call("hgt_host_register", buf.ctypes.data, size, _c.byref(dptr))
+    return view, dptr.value, buf
+
+
+_UNPIN_LATER = []        # pinned buffers of collected graphs, unregistered when no stream capture is in progress
+_UNPIN_FAILED = []       # buffers CUDA would not unregister: kept alive so their pages are never reused while registered
+
+
+def _unpin(device, bufs):
+    """Unregister the pinned buffers of a collected DeviceGraph once the device has finished every kernel that may read
+    them (a batch's write pass can still be running when its graph is dropped).  Runs from a finalizer, so at any point:
+    during a stream capture (where a synchronise would invalidate the capture) the buffers wait for the next call.  Each
+    buffer is unregistered on its own; one CUDA refuses stays referenced rather than be freed while registered."""
+    import torch
+    from . import _lib
+    _UNPIN_LATER.append((device, bufs))
+    try:
+        if torch.cuda.is_current_stream_capturing():
+            return
+    except Exception:                                       # noqa: BLE001 (interpreter shutdown: CUDA may be gone)
+        pass
+    pending = list(_UNPIN_LATER)
+    _UNPIN_LATER.clear()
+    for dev, group in pending:
+        try:
+            torch.cuda.synchronize(dev)
+        except Exception:                                   # noqa: BLE001
+            pass
+        for buf in group:
+            try:
+                _lib.call("hgt_host_unregister", buf.ctypes.data)
+            except Exception:                               # noqa: BLE001
+                _UNPIN_FAILED.append(buf)
+
+
+def _hit_capacity(dg, n_count):
+    """Hit records the single-read rebuild of a host-placed graph reserves for n_count count slots."""
+    return min(int(dg.hit_room * n_count), 2 ** 31 - 1)
+
+
+def _grow_hit_room(dg, n_hits, n_count):
+    """After a rebuild that found n_hits kept edges in n_count slots: reserve a quarter more than that per slot from now
+    on, so that a batch like it fits next time (one that did not fit re-read the lists in its write pass)."""
+    if n_count and n_hits > _hit_capacity(dg, n_count):
+        dg.hit_room = max(dg.hit_room, 1.25 * n_hits / n_count)
 
 
 class DeviceGraph:
-    """A ``FrozenGraph`` uploaded once to a CUDA device for ``sample_subgraph_cuda``: the CSR blocks (neighbour ids and
+    """A ``FrozenGraph`` made readable by a CUDA device for ``sample_subgraph_cuda``: the CSR blocks (neighbour ids and
     edge times in dict order, id -> row maps) and, optionally, per-type feature tables ``{type: Tensor[n_ids, F]}``
     (row = node id) that the sampled batch's ``node_feature`` is gathered from.
+
+    ``placement="device"`` uploads the blocks and the tables to the device.  ``placement="host"`` keeps them, the arrays
+    that grow with the graph, in page-locked host memory mapped for the device, which the kernels read in place over
+    PCIe, so the graph may be far larger than device memory; only the per-block descriptors and per-type tables go to the
+    device.  There is one host copy of each array: the FrozenGraph's blocks are rebound to the pinned copies of their
+    ``row_of`` / ``ptr`` / ``nbr`` / ``time`` (the host sampler keeps working on them), and the feature tables passed in
+    are copied, not kept.  Sampling gives bitwise the same batches either way; the sampler state still lives on the device
+    (``sample_subgraphs_cuda``: about B x 52 bytes x the sum of the id ranges).
 
     Node types are laid out in ``graph.get_types()`` order (as ``to_torch`` does), so every type of the graph's
     ``edge_list`` must be one of them; relation names come from ``graph.get_meta_graph()`` plus ``'self'``."""
 
-    def __init__(self, frozen_graph, device, features=None):
+    PLACEMENTS = ("device", "host")
+
+    def __init__(self, frozen_graph, device, features=None, placement="device"):
+        if placement not in self.PLACEMENTS:
+            raise ValueError("placement must be one of %s, got %r" % (self.PLACEMENTS, placement))
         import torch
         fg = frozen_graph if isinstance(frozen_graph, FrozenGraph) else FrozenGraph(frozen_graph)
         self.fg, self.device = fg, torch.device(device)
@@ -502,24 +578,50 @@ class DeviceGraph:
         self.edge_dict = {e[2]: i for i, e in enumerate(graph.get_meta_graph())}     # data.py:237-238
         self.edge_dict['self'] = len(self.edge_dict)
         self.n_ids = [fg.n_ids.get(t, 0) for t in self.types]
+        self.placement = placement
+        self.hit_room = _HIT_ROOM
         dev = self.device
+        host = placement == "host"
 
         def up(a):
             return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(dev)
 
         self._keep = []
+        pinned = []                                       # page-aligned buffers registered with CUDA
+
+        def place(a, dtype=np.int64):
+            """Address the kernels read array ``a`` at; the array (device tensor or pinned host view) is kept."""
+            if not host:
+                self._keep.append(up(a))
+                return self._keep[-1].data_ptr()
+            view, dptr, buf = _pin(a, dtype)
+            pinned.append(buf)
+            self._keep.append(view)
+            return dptr
+
+        if host:
+            weakref.finalize(self, _unpin, dev, pinned)
+        with torch.cuda.device(dev) if host else contextlib.nullcontext():     # register on this graph's device
+            self._build(fg, features, place, up)
+
+    def _build(self, fg, features, place, up):
+        import torch
+        dev = self.device
         self.blocks = []                                  # (target slot, source slot, relation, skip) in dict order
         cblocks = []
+        if self.placement == "host":
+            fg._cblocks = {}        # the host sampler's cached block tables hold the addresses of arrays rebound below
         for t_t, tes in fg.blocks.items():
             for s_t, rels in tes.items():
                 for r, blk in rels.items():
                     if r not in self.edge_dict:
                         raise KeyError("relation %r of edge_list is not in graph.get_meta_graph()" % (r,))
-                    arrs = [up(blk.row_of), up(blk.ptr), up(blk.nbr), up(blk.time)]
-                    self._keep += arrs
-                    cb = _GBlock(arrs[0].data_ptr(), blk.row_of.shape[0], arrs[1].data_ptr(), arrs[2].data_ptr(),
-                                 arrs[3].data_ptr(), self.slot[t_t], self.slot[s_t], 1 if r == 'self' else 0,
-                                 self.edge_dict[r])
+                    ptrs = [place(blk.row_of), place(blk.ptr), place(blk.nbr), place(blk.time)]
+                    if self.placement == "host":           # the FrozenGraph reads the pinned copies: one copy each
+                        blk.row_of, blk.ptr, blk.nbr, blk.time = self._keep[-4:]
+                        blk.nbr_addr, blk.time_addr = blk.nbr.ctypes.data, blk.time.ctypes.data
+                    cb = _GBlock(ptrs[0], blk.row_of.shape[0], ptrs[1], ptrs[2], ptrs[3], self.slot[t_t],
+                                 self.slot[s_t], 1 if r == 'self' else 0, self.edge_dict[r])
                     self.blocks.append((self.slot[t_t], self.slot[s_t], r))
                     cblocks.append(cb)
         self.n_blocks = len(cblocks)
@@ -542,10 +644,16 @@ class DeviceGraph:
             tabs, ptrs, rows = {}, [], []
             for t in self.types:
                 v = features.get(t)
-                if v is not None:
+                p = 0
+                if v is not None and self.placement == "host":
+                    p = place(v.detach().to(device="cpu", dtype=torch.float32).contiguous().numpy(), np.float32)
+                    v = torch.from_numpy(self._keep[-1])
+                    tabs[t] = v
+                elif v is not None:
                     v = v.to(device=dev, dtype=torch.float32).contiguous()
                     tabs[t] = v
-                ptrs.append(0 if v is None else v.data_ptr())
+                    p = v.data_ptr()
+                ptrs.append(p)
                 rows.append(0 if v is None else v.shape[0])
             self.features = tabs
             self.feat_ptrs = torch.tensor(np.asarray(ptrs, dtype=np.uint64).view(np.int64), device=dev)
@@ -706,11 +814,12 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     bstamp = torch.full((max(n_slots, 1),), -1, **i64)
     last_seq = torch.full((max(n_slots, 1),), -1, **i64)
     first_seq = torch.full((max(n_slots, 1),), _I64_MAX, **i64)
-    # one small buffer the host reads: [n_layer B*T | type_seq B*2T | block totals B*NB | flags]
-    meta = torch.zeros(3 * B * T + B * NB + 2, **i64)
+    # one small buffer the host reads: [n_layer B*T | type_seq B*2T | block totals B*NB | flags | hit count (host graph)]
+    host = dg.placement == "host"
+    meta = torch.zeros(3 * B * T + B * NB + 2 + int(host), **i64)
     n_layer, type_seq = meta[:B * T], meta[B * T:3 * B * T]
     totals = meta[3 * B * T:3 * B * T + B * NB]
-    flags = meta[3 * B * T + B * NB:].view(torch.int32)   # 4 int32 flags
+    flags = meta[3 * B * T + B * NB:3 * B * T + B * NB + 2].view(torch.int32)   # 4 int32 flags
     type_min = torch.full((max(2 * B * T, 1),), _I64_MAX, **i64)
     counters = torch.zeros(2 * B, **i64)
 
@@ -839,14 +948,24 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     cnt_off_d = _plan._to_dev_async(cnt_off if min_ser is None else np.concatenate([cnt_off, min_ser]), dev)
     masked = () if min_ser is None else (cnt_off_d.data_ptr() + 8 * cnt_off.shape[0],)
     suffix = "" if min_ser is None else "_masked"
-    _lib.call("hgt_gsample_batch_rebuild_count" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
-              cnt_off_d.data_ptr(), n_count, max_rows, _lib.ptr(dg.feat_rows) if dg.features is not None else None,
-              ex.data_ptr(), totals.data_ptr(), flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
+    feat_rows_p = _lib.ptr(dg.feat_rows) if dg.features is not None else None
+    if host:
+        # single-read count pass: the kept edges' hit records (16 bytes each) stay in device scratch for the write pass
+        hit_cap = _hit_capacity(dg, n_count)
+        hits = torch.empty(16 * max(hit_cap, 1), dtype=torch.uint8, device=dev)
+        _lib.call("hgt_gsample_batch_rebuild_count_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
+                  masked[0] if masked else None, cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, hits.data_ptr(),
+                  hit_cap, meta[-1:].data_ptr(), ex.data_ptr(), totals.data_ptr(), flags.data_ptr(), rb.data_ptr(),
+                  rb.numel(), st)
+    else:
+        _lib.call("hgt_gsample_batch_rebuild_count" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
+                  cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, ex.data_ptr(), totals.data_ptr(),
+                  flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
     h = meta.cpu().numpy()
     nl = h[:B * T].reshape(B, T)
     ts = h[B * T:3 * B * T].reshape(B, 2 * T)
     tot = h[3 * B * T:3 * B * T + B * NB].reshape(B, NB)
-    fl = h[3 * B * T + B * NB:].view(np.int32)
+    fl = h[3 * B * T + B * NB:3 * B * T + B * NB + 2].view(np.int32)
     if fl[0]:
         raise IndexError("a neighbour id lies outside its node type's id range in the device graph")
     if fl[1]:
@@ -879,12 +998,24 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     edge_index = torch.empty(2 * E, **i64)                # member b's [2, E_b] block at 2 * edge_base[b]
     edge_type = torch.empty(E, **i64)
     edge_time = torch.empty(E, **i64)
-    _lib.call("hgt_gsample_batch_rebuild_write" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
-              cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
-              d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
-              _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
-              node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
-              edge_time.data_ptr(), st)
+    if host:
+        n_hits = int(h[-1])
+        _grow_hit_room(dg, n_hits, n_count)
+        fits = n_hits <= hit_cap                          # else the write pass re-reads the neighbour lists
+        _lib.call("hgt_gsample_batch_rebuild_write_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
+                  masked[0] if masked else None, cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"),
+                  d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
+                  hits.data_ptr() if fits else None, n_hits if fits else 0,
+                  _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
+                  node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
+                  edge_time.data_ptr(), st)
+    else:
+        _lib.call("hgt_gsample_batch_rebuild_write" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
+                  cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
+                  d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
+                  _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
+                  node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
+                  edge_time.data_ptr(), st)
 
     out = []
     for b in range(B):
