@@ -829,7 +829,9 @@ int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const hgt_gsampl
  * B subgraphs ("members") in one pass (pyhgt_b200/sampler.py: sample_subgraphs_cuda).  The members share the graph,
  * the time filter, the depth and the width; each has its own seeds, Philox seed, step numbers and rows of the state, and
  * member b's result is bitwise the single-subgraph run with its seed and steps (the entry points above are B = 1).
- * Memory: about 52 bytes per state slot, i.e. B x 52 B x (sum of the id ranges) for the dense arrays.
+ * Memory: about 52 bytes per state slot, i.e. B x 52 B x (sum of the id ranges) for the dense arrays; selection sorts
+ * every id of the selected type (int32 sort values: the ranges of one step must sum to less than 2^31 - 1).  The hashed
+ * state below (hgt_gsample_hash_state) holds the same fields in hash tables sized by the sample instead.
  * ---------------------------------------------------------------------------------------------- */
 
 /* Like hgt_gsample_state with a member dimension: type_off / lid_off hold [B*(T+1)] ABSOLUTE positions (member b's type
@@ -912,6 +914,88 @@ int hgt_gsample_batch_rebuild_write_masked(const hgt_gsample_batch_state* h_stat
                                            int32_t feat_dim, int64_t* node_type, int64_t* node_time,
                                            float* node_feature, int64_t* edge_index, int64_t* edge_type,
                                            int64_t* edge_time, void* stream);
+
+/* The hashed sampler state (sampler.py: sample_subgraphs_cuda picks it when the dense state is too large or slower):
+ * per (member, type) an open-addressing table of `room` entries keyed by node id, sized by the sample rather than by the
+ * id range.  Results are bitwise those of the dense state for the same inputs.
+ *   ent_off [B*(T+1)]: ABSOLUTE first entry of each (member, type) region (member b's type t: entries ent_off[b*(T+1)+t]
+ *     .. [b*(T+1)+t+1]); lid_off as for hgt_gsample_batch_state; n_ids [B*T]: the id range of each (member, type)
+ *     (neighbour ids outside it set flags[0], as in the dense state; ids must stay below 2^40).
+ *   key [entries]: node id of the entry, -1 = empty (every entry starts empty); ser / score / btime / bstamp /
+ *     last_seq / first_seq [entries]: the dense per-slot fields with the dense initial values.
+ *   ltime [lid entries]: the time of every sampled node, indexed like lid (per ser, not per id).
+ *   fill [B*T]: entries claimed per region, initially 0.  n_layer, type_min, type_seq, counters, seed: as dense.
+ * An entry is claimed with one compare-and-swap on its key; probing is linear and visits a region at most once.  A claim
+ * that takes a region past half full, or finds no free entry, sets flags[3] (overflow): the results of that run are
+ * incomplete and it must be repeated with larger regions.  Nothing is written outside the regions. */
+typedef struct {
+  int32_t num_types; int32_t n_members;
+  const int64_t* ent_off;
+  const int64_t* lid_off;
+  const int64_t* n_ids;
+  int64_t* key;
+  int32_t* ser;
+  int64_t* ltime;
+  int64_t* lid;
+  int64_t* n_layer;
+  unsigned long long* score;
+  int64_t* btime;
+  int64_t* bstamp;
+  int64_t* last_seq;
+  int64_t* first_seq;
+  unsigned long long* fill;
+  int64_t* type_min;
+  int64_t* type_seq;
+  int64_t* counters;
+  const uint64_t* seed;
+} hgt_gsample_hash_state;
+
+/* The seeds (data.py:135-137): seed i of region[i] = b*T + t (device arrays [n]) gets an entry for id[i] with ser[i],
+ * and lid / ltime at position ser[i] of that (member, type). */
+int hgt_gsample_hash_insert_seeds(const hgt_gsample_hash_state* h_state, int64_t n, const int64_t* region,
+                                  const int64_t* id, const int64_t* ser, const int64_t* time, int32_t* flags,
+                                  void* stream);
+/* As hgt_gsample_batch_add_budget (same arguments, same workspace: hgt_gsample_batch_add_budget_workspace_bytes). */
+int hgt_gsample_hash_add_budget(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
+                                const int32_t* type_blocks, int32_t max_blocks, const int32_t* type, const int64_t* step,
+                                const int64_t* tgt_id, const int64_t* tgt_time, int64_t max_targets,
+                                const int64_t* n_targets, int64_t sampled_number, int32_t time_filter, int64_t max_time,
+                                int64_t no_time, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
+/* As hgt_gsample_batch_select, over the selected type's REGION instead of its id range: sel_off [B+1] (device) are
+ * prefix sums of the region sizes (n_total = sel_off[B] < 2^31 - 1, max_room >= every region size).  The budget entries
+ * are ordered by id first, so keys and ties are exactly those of the dense selection. */
+int hgt_gsample_hash_select_workspace_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes);
+int hgt_gsample_hash_select(const hgt_gsample_hash_state* h_state, const int32_t* type, const int64_t* step,
+                            const int64_t* sel_off, int64_t n_total, int64_t max_room, int64_t sampled_number,
+                            int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets, int32_t* flags, void* workspace,
+                            size_t workspace_bytes, void* stream);
+/* The rebuild passes, as hgt_gsample_batch_rebuild_count / _write with min_ser NULL (no mask) or a mask table as for the
+ * _masked entry points, and the host-graph passes as hgt_gsample_batch_rebuild_count_host / _write_host.  Workspace:
+ * hgt_gsample_rebuild_workspace_bytes.  The outputs are those of the dense state. */
+int hgt_gsample_hash_rebuild_count(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
+                                   int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count,
+                                   int64_t max_rows, const int64_t* feat_rows, int64_t* ex, int64_t* totals,
+                                   int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
+int hgt_gsample_hash_rebuild_write(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
+                                   int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex,
+                                   const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
+                                   const int64_t* self_off, int64_t self_rel, const int64_t* mem_out, int64_t max_rows,
+                                   const float* const* feat, int32_t feat_dim, int64_t* node_type, int64_t* node_time,
+                                   float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time,
+                                   void* stream);
+int hgt_gsample_hash_rebuild_count_host(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
+                                        int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                        int64_t n_count, int64_t max_rows, const int64_t* feat_rows, void* hits,
+                                        int64_t hit_cap, int64_t* n_hits, int64_t* ex, int64_t* totals, int32_t* flags,
+                                        void* workspace, size_t workspace_bytes, void* stream);
+int hgt_gsample_hash_rebuild_write_host(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
+                                        int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                        const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
+                                        const int64_t* type_out, const int64_t* self_off, int64_t self_rel,
+                                        const int64_t* mem_out, int64_t max_rows, const void* hits, int64_t n_hits,
+                                        const float* const* feat, int32_t feat_dim, int64_t* node_type,
+                                        int64_t* node_time, float* node_feature, int64_t* edge_index,
+                                        int64_t* edge_type, int64_t* edge_time, void* stream);
 
 /* Graphs in page-locked host memory (sampler.py: DeviceGraph(..., placement="host")).  hgt_host_register page-locks
  * [host, host + bytes) (cudaHostRegister, mapped) and returns in *dev_ptr the address device code reads it at;

@@ -133,6 +133,19 @@ SIGNATURES = {
                                              _p],
     "hgt_gsample_batch_rebuild_write_host": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p,
                                              _i32, _p, _p, _p, _p, _p, _p, _p],
+    # the hashed sampler state, sized by the sample (sample_subgraphs_cuda on graphs with large id ranges)
+    "hgt_gsample_hash_insert_seeds": [_p, _i64, _p, _p, _p, _p, _p, _p],
+    "hgt_gsample_hash_add_budget": [_p, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _i64, _i32, _i64, _i64, _p, _p, _sz,
+                                    _p],
+    "hgt_gsample_hash_select_workspace_bytes": [_i32, _i64, _c.POINTER(_sz)],
+    "hgt_gsample_hash_select": [_p, _p, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_hash_rebuild_count": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_hash_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p,
+                                       _p, _p, _p, _p],
+    "hgt_gsample_hash_rebuild_count_host": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _sz,
+                                            _p],
+    "hgt_gsample_hash_rebuild_write_host": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p,
+                                            _i32, _p, _p, _p, _p, _p, _p, _p],
     "hgt_merge_batches": [_p, _i32, _i32, _p, _p, _i64, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p],
     # trimmed forward (GNN.forward(out_nodes=), trim.py)
     "hgt_trim_layout": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],

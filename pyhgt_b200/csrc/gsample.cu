@@ -47,6 +47,126 @@ __device__ __forceinline__ Member member(const hgt_gsample_batch_state& st, int 
           st.type_min + (int64_t)m * 2 * T, st.type_seq + (int64_t)m * 2 * T, st.counters + 2 * m};
 }
 
+// ---- where a node's state lives ---------------------------------------------------------------------------------------
+// The kernels shared by the two layouts are templates over the state struct; these overloads are the only place where
+// the layouts differ.  Dense: node id of type t sits at slot type_off[t] + id of an id-range-sized array.  Hashed: it
+// sits at the entry of its member's type-t region whose key is id, and its time is stored per ser (like lid).
+
+struct HMember {
+  const int64_t *type_off, *lid_off, *n_ids;                            // type_off: the region starts (ent_off)
+  int64_t *n_layer, *type_min, *type_seq, *counters;
+  unsigned long long* fill;
+};
+
+__device__ __forceinline__ HMember member(const hgt_gsample_hash_state& st, int m) {
+  const int T = st.num_types;
+  return {st.ent_off + (int64_t)m * (T + 1), st.lid_off + (int64_t)m * (T + 1), st.n_ids + (int64_t)m * T,
+          st.n_layer + (int64_t)m * T, st.type_min + (int64_t)m * 2 * T, st.type_seq + (int64_t)m * 2 * T,
+          st.counters + 2 * m, st.fill + (int64_t)m * T};
+}
+
+// A type of one member: its slots (base, n = the id range) or its region (base, room entries), id range n, lid start lt.
+struct DenseIx {
+  int64_t base, n;
+};
+struct HashIx {
+  int64_t base, room, n, lt;
+  unsigned long long* fill;
+};
+
+__device__ __forceinline__ DenseIx type_ix(const hgt_gsample_batch_state&, const Member& mb, int t) {
+  const int64_t base = mb.type_off[t];
+  return {base, mb.type_off[t + 1] - base};
+}
+__device__ __forceinline__ HashIx type_ix(const hgt_gsample_hash_state&, const HMember& mb, int t) {
+  const int64_t base = mb.type_off[t];
+  return {base, mb.type_off[t + 1] - base, mb.n_ids[t], mb.lid_off[t], mb.fill + t};
+}
+
+constexpr long long kEmptyKey = -1;
+
+// First probe position of id in a region of `room` entries (splitmix64 finaliser, then a multiply-high).
+__device__ __forceinline__ int64_t hash_home(int64_t id, int64_t room) {
+  uint64_t x = (uint64_t)id + 0x9e3779b97f4a7c15ULL;
+  x = (x ^ (x >> 30)) * 0xbf58476d1ce4e5b9ULL;
+  x = (x ^ (x >> 27)) * 0x94d049bb133111ebULL;
+  x ^= x >> 31;
+  return (int64_t)__umul64hi(x, (uint64_t)room);
+}
+
+// The entry of id, or -1 (not in the region).  Linear probing, each entry at most once.
+__device__ __forceinline__ int64_t hash_find(const int64_t* key, const HashIx& ix, int64_t id) {
+  int64_t j = hash_home(id, ix.room);
+  for (int64_t q = 0; q < ix.room; ++q) {
+    const int64_t k = key[ix.base + j];
+    if (k == id) return ix.base + j;
+    if (k == kEmptyKey) return -1;
+    if (++j == ix.room) j = 0;
+  }
+  return -1;
+}
+
+// The entry of id, claimed with one compare-and-swap if it has none.  A claim past half the room, or a region with no
+// free entry, raises the overflow flag (flags[3]); the latter also returns -1 (skip the candidate).
+__device__ __forceinline__ int64_t hash_claim(int64_t* key, const HashIx& ix, int64_t id, int32_t* flags) {
+  int64_t j = hash_home(id, ix.room);
+  for (int64_t q = 0; q < ix.room; ++q) {
+    unsigned long long* p = (unsigned long long*)(key + ix.base + j);
+    long long k = *(volatile long long*)p;
+    if (k == kEmptyKey) {
+      k = (long long)atomicCAS(p, (unsigned long long)kEmptyKey, (unsigned long long)id);
+      if (k == kEmptyKey) {
+        if (2 * (atomicAdd(ix.fill, 1ULL) + 1) > (unsigned long long)ix.room) flags[3] = 1;
+        return ix.base + j;
+      }
+    }
+    if (k == id) return ix.base + j;
+    if (++j == ix.room) j = 0;
+  }
+  flags[3] = 1;
+  return -1;
+}
+
+// add_budget's slot of a candidate (false: skip it).
+__device__ __forceinline__ bool budget_slot(const hgt_gsample_batch_state&, const DenseIx& ix, int64_t sid,
+                                            int32_t*, int64_t* slot) {
+  *slot = ix.base + sid;
+  return true;
+}
+__device__ __forceinline__ bool budget_slot(const hgt_gsample_hash_state& st, const HashIx& ix, int64_t sid,
+                                            int32_t* flags, int64_t* slot) {
+  *slot = hash_claim(st.key, ix, sid, flags);
+  return *slot >= 0;
+}
+
+// ser of id (in range) in the member's sample, -1 = not sampled.
+__device__ __forceinline__ int32_t ser_of(const hgt_gsample_batch_state& st, const DenseIx& ix, int64_t sid) {
+  return st.ser[ix.base + sid];
+}
+__device__ __forceinline__ int32_t ser_of(const hgt_gsample_hash_state& st, const HashIx& ix, int64_t sid) {
+  const int64_t e = hash_find(st.key, ix, sid);
+  return e >= 0 ? st.ser[e] : -1;
+}
+
+// Time of a sampled node of type t: id `id`, ser r.
+__device__ __forceinline__ int64_t node_ltime(const hgt_gsample_batch_state& st, const Member& mb, int t, int64_t id,
+                                             int64_t) {
+  return st.ltime[mb.type_off[t] + id];
+}
+__device__ __forceinline__ int64_t node_ltime(const hgt_gsample_hash_state& st, const HMember& mb, int t, int64_t,
+                                             int64_t r) {
+  return st.ltime[mb.lid_off[t] + r];
+}
+// The same for a source looked up through its type's index.
+__device__ __forceinline__ int64_t src_ltime(const hgt_gsample_batch_state& st, const DenseIx& ix, int64_t sid,
+                                            int32_t) {
+  return st.ltime[ix.base + sid];
+}
+__device__ __forceinline__ int64_t src_ltime(const hgt_gsample_hash_state& st, const HashIx& ix, int64_t,
+                                            int32_t sser) {
+  return st.ltime[ix.lt + sser];
+}
+
 // The blocks member m's add_budget walks: blocks[0, n_blocks) for every member (single type), or the blocks of the
 // member's current type (type_blocks [2T]: begin / end per target type; type[m] < 0 = the member sits this step out).
 struct BlockRange {
@@ -123,7 +243,8 @@ __global__ void k_seg_count(const hgt_gsample_block* blocks, BlockRange br, int3
 
 // One warp per <member, target k, block b>.  seq = seg_off + j orders the member's candidates like the reference's
 // processing order (target, block, neighbour in subset order), the key of every order-dependent rule.
-__global__ void k_candidates(hgt_gsample_batch_state st, PerMember<uint64_t> seed, PerMember<int64_t> step,
+template <class St>
+__global__ void k_candidates(St st, PerMember<uint64_t> seed, PerMember<int64_t> step,
                              const hgt_gsample_block* blocks, BlockRange br, int64_t S, const int64_t* tgt_id,
                              const int64_t* tgt_time, int64_t max_targets, const int64_t* seg_cnt,
                              const int64_t* seg_off, int64_t width, int32_t time_filter, int64_t max_time,
@@ -138,7 +259,7 @@ __global__ void k_candidates(hgt_gsample_batch_state st, PerMember<uint64_t> see
   const int64_t loc = seg % S;
   int32_t b0, nb;
   br.get(m, &b0, &nb);
-  const Member mb = member(st, m);
+  const auto mb = member(st, m);
   const int64_t k = loc / nb;
   const hgt_gsample_block blk = blocks[b0 + loc % nb];
   int64_t a, deg;
@@ -169,7 +290,7 @@ __global__ void k_candidates(hgt_gsample_batch_state st, PerMember<uint64_t> see
   }
   const int64_t target_time = tgt_time[m * max_targets + k];
   const int src = blk.src_type;
-  const int64_t base = mb.type_off[src], n_ids = mb.type_off[src + 1] - base;
+  const auto ix = type_ix(st, mb, src);
   const unsigned long long w = (unsigned long long)llrint(kScoreScale / (double)n_s);   // 1. / len(sampled_ids)
   for (int64_t j = lane; j < n_s; j += 32) {
     const int64_t seq = off + j;
@@ -180,8 +301,9 @@ __global__ void k_candidates(hgt_gsample_batch_state st, PerMember<uint64_t> see
     cand_slot[seq] = -1;
     if (time_filter && tm > max_time) continue;                         // data.py:127, first operand of the `or`
     atomicMin((long long*)&mb.type_min[2 * src], (long long)seq);      // layer_data[source_type] springs into being
-    if (sid < 0 || sid >= n_ids) { flags[0] = 1; continue; }
-    const int64_t slot = base + sid;
+    if (sid < 0 || sid >= ix.n) { flags[0] = 1; continue; }
+    int64_t slot;
+    if (!budget_slot(st, ix, sid, flags, &slot)) continue;
     if (st.ser[slot] >= 0) continue;                                    // already sampled
     atomicMin((long long*)&mb.type_min[2 * src + 1], (long long)seq);  // budget[source_type] springs into being
     atomicAdd(&st.score[slot], w);
@@ -195,7 +317,8 @@ __global__ void k_candidates(hgt_gsample_batch_state st, PerMember<uint64_t> see
 // The candidate that wrote last sets the budget time (data.py:130); the first one of a new entry sets its stamp (step
 // << 40 + its position among the member's candidates).  The matching candidate also resets the scratch word: no other
 // candidate of the slot can match either value.  grid.y = member; grid-stride over the member's candidates.
-__global__ void k_resolve(hgt_gsample_batch_state st, PerMember<int64_t> step, const int64_t* seg_off, int64_t S,
+template <class St>
+__global__ void k_resolve(St st, PerMember<int64_t> step, const int64_t* seg_off, int64_t S,
                           const int64_t* cand_slot, const int64_t* cand_time) {
   const int m = blockIdx.y;
   const int64_t lo = seg_off[m * S], hi = seg_off[(m + 1) * S];
@@ -217,10 +340,11 @@ __global__ void k_resolve(hgt_gsample_batch_state st, PerMember<int64_t> step, c
 
 // First-touch numbers of layer_data[t] / budget[t] (the key orders of the reference's defaultdicts): types touched for
 // the first time in this step are numbered in the order of their first qualifying candidate.  One thread per member.
-__global__ void k_touch(hgt_gsample_batch_state st) {
+template <class St>
+__global__ void k_touch(St st) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= st.n_members) return;
-  const Member mb = member(st, m);
+  const auto mb = member(st, m);
   for (int kind = 0; kind < 2; ++kind) {
     for (;;) {
       int best = -1;
@@ -320,7 +444,8 @@ __global__ void k_sel_take(hgt_gsample_batch_state st, PerMember<int32_t> type, 
   st.score[slot] = 0;
 }
 
-__global__ void k_sel_finish(hgt_gsample_batch_state st, PerMember<int32_t> type, int64_t width,
+template <class St>
+__global__ void k_sel_finish(St st, PerMember<int32_t> type, int64_t width,
                              const unsigned long long* count, int64_t* n_targets) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= st.n_members) return;
@@ -329,6 +454,103 @@ __global__ void k_sel_finish(hgt_gsample_batch_state st, PerMember<int32_t> type
   const int64_t c = (int64_t)count[m] < width ? (int64_t)count[m] : width;
   member(st, m).n_layer[t] += c;
   n_targets[m] = c;
+}
+
+// ---- the hashed state's own kernels: seeds and selection ------------------------------------------------------------
+
+// Seed i: an entry for id[i] in region[i] = m * T + t with its ser, and lid / ltime at that ser.
+__global__ void k_hash_seed(hgt_gsample_hash_state st, int64_t n, const int64_t* region, const int64_t* id,
+                            const int64_t* ser, const int64_t* time, int32_t* flags) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int m = (int)(region[i] / st.num_types), t = (int)(region[i] % st.num_types);
+  const HMember mb = member(st, m);
+  const HashIx ix = type_ix(st, mb, t);
+  const int64_t e = hash_claim(st.key, ix, id[i], flags);
+  if (e < 0) return;
+  st.ser[e] = (int32_t)ser[i];
+  st.lid[mb.lid_off[t] + ser[i]] = id[i];
+  st.ltime[mb.lid_off[t] + ser[i]] = time[i];
+}
+
+constexpr int kIdBits = 41;                                             // ids < 2^40, plus "not in the budget"
+constexpr uint64_t kNotBudget = (uint64_t(1) << kIdBits) - 1;
+
+// Selection pass 1: every entry of member m's region of type[m], at sel_off[m] + its index, gets the sort key
+// (m, id) when it is in the budget and (m, kNotBudget) otherwise, so that sorting puts each member's budget entries
+// first and in id order: the order of the dense selection's positions.  Counts the budget entries.
+__global__ void k_hsel_order(hgt_gsample_hash_state st, const int32_t* type, const int64_t* sel_off,
+                             uint64_t* okey, int64_t* oent, unsigned long long* count) {
+  const int m = blockIdx.y;
+  const int t = type[m];
+  if (t < 0) return;
+  const HMember mb = member(st, m);
+  const int64_t base = mb.type_off[t], n = mb.type_off[t + 1] - base, o = sel_off[m];
+  unsigned long long c = 0;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const bool in = st.bstamp[base + i] >= 0;
+    okey[o + i] = ((uint64_t)m << kIdBits) | (in ? (uint64_t)st.key[base + i] : kNotBudget);
+    oent[o + i] = base + i;
+    c += in;
+  }
+  for (int s = 16; s; s >>= 1) c += __shfl_xor_sync(kFull, c, s);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(&count[m], c);
+}
+
+// k_sel_keys over the id-ordered entries: the first count[m] positions of member m are its budget, the node id is the
+// Philox counter's local id, so every key is bitwise the dense one.
+__global__ void k_hsel_keys(hgt_gsample_hash_state st, const int32_t* type, const int64_t* sel_off, int64_t width,
+                            const unsigned long long* count, const int64_t* step, const uint64_t* okey,
+                            const int64_t* oent, double* keys, int32_t* vals) {
+  const int m = blockIdx.y;
+  const int t = type[m];
+  if (t < 0) return;
+  const HMember mb = member(st, m);
+  const int64_t n = mb.type_off[t + 1] - mb.type_off[t];
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t o = sel_off[m] + i;
+  double key = -INFINITY;
+  if (i < (int64_t)count[m]) {
+    const int64_t e = oent[o];
+    if (width > (int64_t)count[m]) {
+      key = -(double)st.bstamp[e];
+    } else {
+      const uint64_t id = okey[o] & kNotBudget;
+      curandStatePhilox4_32_10_t rs;
+      curand_init(st.seed[m] ^ kSelectStream, ((uint64_t)step[m] << 40) | id, 0, &rs);
+      const double u = (double)((rnd64(&rs) >> 11) + 1) * 0x1.0p-53;   // (0, 1]
+      const double s = (double)st.score[e] / kScoreScale;
+      key = log(u) / (s * s);
+    }
+  }
+  keys[o] = key;
+  vals[o] = (int32_t)o;
+}
+
+// k_sel_take with the chosen entry found through the id order.
+__global__ void k_hsel_take(hgt_gsample_hash_state st, const int32_t* type, const int64_t* sel_off, int64_t width,
+                            const unsigned long long* count, const int32_t* vals, const int64_t* oent, int64_t* tgt_id,
+                            int64_t* tgt_time, int32_t* flags) {
+  const int m = blockIdx.y;
+  const int t = type[m];
+  if (t < 0) return;
+  const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t c = (int64_t)count[m] < width ? (int64_t)count[m] : width;
+  if (r >= c) return;
+  const HMember mb = member(st, m);
+  const int64_t e = oent[vals[sel_off[m] + r]];
+  const int64_t id = st.key[e];
+  const int64_t ser = mb.n_layer[t] + r;
+  const int64_t l = mb.lid_off[t] + ser;
+  if (l >= mb.lid_off[t + 1]) { flags[0] = 1; return; }
+  st.ser[e] = (int32_t)ser;
+  st.ltime[l] = st.btime[e];
+  st.lid[l] = id;
+  tgt_id[m * width + r] = id;
+  tgt_time[m * width + r] = st.btime[e];
+  st.bstamp[e] = -1;
+  st.score[e] = 0;
 }
 
 // The caller's edge mask (sampler.py: edge_mask; the OAG scripts drop the edges that would leak a seed's label between
@@ -342,7 +564,8 @@ __device__ __forceinline__ bool masked_out(const int64_t* min_ser, int b, int64_
 // One warp per <member (grid.z), block (grid.y), target ser r>: neighbours of the target that are in the member's sample
 // (data.py:190-209) and not masked out, counted, with the edge_time range check of to_torch on those kept edges
 // (data.py:250; RelTemporalEncoding has 240 rows).
-__global__ void k_rb_count(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
+template <class St>
+__global__ void k_rb_count(St st, const hgt_gsample_block* blocks, int32_t n_blocks,
                            const int64_t* min_ser, const int64_t* cnt_off, int64_t* cnt, int32_t* flags) {
   const int lane = threadIdx.x & 31;
   const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
@@ -351,22 +574,22 @@ __global__ void k_rb_count(hgt_gsample_batch_state st, const hgt_gsample_block* 
   const hgt_gsample_block blk = blocks[b];
   const int T = blk.tgt_type, S = blk.src_type;
   if (r >= cnt_off[mbk + 1] - cnt_off[mbk]) return;
-  const Member mb = member(st, blockIdx.z);
+  const auto mb = member(st, blockIdx.z);
   int64_t c = 0;
   if (r < mb.n_layer[T]) {
     const int64_t tid = st.lid[mb.lid_off[T] + r];
     const int64_t row = tid < blk.n_row_of ? blk.row_of[tid] : -1;
     if (row >= 0) {
       const int64_t a = blk.ptr[row], e = blk.ptr[row + 1];
-      const int64_t tt = st.ltime[mb.type_off[T] + tid];
-      const int64_t sb = mb.type_off[S], sn = mb.type_off[S + 1] - sb;
+      const int64_t tt = node_ltime(st, mb, T, tid, r);
+      const auto ix = type_ix(st, mb, S);
       for (int64_t p = a + lane; p < e; p += 32) {
         const int64_t sid = blk.nbr[p];
-        if (sid < 0 || sid >= sn) { flags[0] = 1; continue; }
-        const int32_t sser = st.ser[sb + sid];
+        if (sid < 0 || sid >= ix.n) { flags[0] = 1; continue; }
+        const int32_t sser = ser_of(st, ix, sid);
         if (sser < 0 || masked_out(min_ser, b, r, sser)) continue;
         ++c;
-        const int64_t dt = tt - st.ltime[sb + sid] + 120;
+        const int64_t dt = tt - src_ltime(st, ix, sid, sser) + 120;
         if (dt < 0 || dt >= HGT_RTE_MAX_LEN) flags[1] = 1;
       }
     }
@@ -380,16 +603,18 @@ __global__ void k_rb_totals(const int64_t* ex, const int64_t* cnt_off, int64_t n
   if (b < n) totals[b] = ex[cnt_off[b + 1]] - ex[cnt_off[b]];
 }
 
-__global__ void k_rb_check_features(hgt_gsample_batch_state st, const int64_t* feat_rows, int32_t* flags) {
+template <class St>
+__global__ void k_rb_check_features(St st, const int64_t* feat_rows, int32_t* flags) {
   const int t = blockIdx.y;
-  const Member mb = member(st, blockIdx.z);
+  const auto mb = member(st, blockIdx.z);
   const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (r < mb.n_layer[t] && st.lid[mb.lid_off[t] + r] >= feat_rows[t]) flags[2] = 1;
 }
 
 // blk_out / node_off / self_off are member-local (member m's rows [m * n_blocks ...] / [m * T ...]); edge_index holds
 // each member's [2, E_m] block at 2 * edge_base, node ids member-local.  The ballot keeps the kept edges in block order.
-__global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
+template <class St>
+__global__ void k_rb_write(St st, const hgt_gsample_block* blocks, int32_t n_blocks,
                            const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out,
                            const int64_t* node_off, MemOut mo, int64_t* edge_index, int64_t* edge_type,
                            int64_t* edge_time) {
@@ -400,7 +625,7 @@ __global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* 
   const int64_t mbk = (int64_t)m * n_blocks + b;
   const hgt_gsample_block blk = blocks[b];
   const int T = blk.tgt_type, S = blk.src_type;
-  const Member mb = member(st, m);
+  const auto mb = member(st, m);
   if (blk_out[mbk] < 0 || r >= mb.n_layer[T]) return;
   const int64_t tid = st.lid[mb.lid_off[T] + r];
   const int64_t row = tid < blk.n_row_of ? blk.row_of[tid] : -1;
@@ -410,8 +635,8 @@ __global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* 
   int64_t* ei = edge_index + 2 * eb;
   int64_t e = blk_out[mbk] + ex[cnt_off[mbk] + r] - ex[cnt_off[mbk]];
   const int64_t a = blk.ptr[row], end = blk.ptr[row + 1];
-  const int64_t tt = st.ltime[mb.type_off[T] + tid];
-  const int64_t sb = mb.type_off[S], sn = mb.type_off[S + 1] - sb;
+  const int64_t tt = node_ltime(st, mb, T, tid, r);
+  const auto ix = type_ix(st, mb, S);
   const int64_t dst = noff[T] + r;
   for (int64_t p0 = a; p0 < end; p0 += 32) {
     const int64_t p = p0 + lane;
@@ -419,7 +644,7 @@ __global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* 
     int64_t sid = -1;
     if (p < end) {
       sid = blk.nbr[p];
-      if (sid >= 0 && sid < sn) sser = st.ser[sb + sid];
+      if (sid >= 0 && sid < ix.n) sser = ser_of(st, ix, sid);
     }
     const bool kept = sser >= 0 && !masked_out(min_ser, b, r, sser);
     const unsigned keep = __ballot_sync(kFull, kept);
@@ -428,7 +653,7 @@ __global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* 
       ei[o] = noff[S] + sser;                                           // row 0 = source (data.py:245,254)
       ei[n_edges + o] = dst;
       edge_type[eb + o] = blk.rel;
-      edge_time[eb + o] = tt - st.ltime[sb + sid] + 120;                // data.py:250
+      edge_time[eb + o] = tt - src_ltime(st, ix, sid, sser) + 120;        // data.py:250
     }
     e += __popc(keep);
   }
@@ -436,7 +661,8 @@ __global__ void k_rb_write(hgt_gsample_batch_state st, const hgt_gsample_block* 
 
 // Nodes type by type (graph.get_types() order, ser order within a type: data.py:228-235), their self loops
 // (data.py:181-184), and the feature rows gathered from the caller's per-type tables.  grid.z = member.
-__global__ void k_rb_nodes(hgt_gsample_batch_state st, const int64_t* node_off, const int64_t* type_out,
+template <class St>
+__global__ void k_rb_nodes(St st, const int64_t* node_off, const int64_t* type_out,
                            const int64_t* self_off, int64_t self_rel, MemOut mo, const float* const* feat,
                            int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature,
                            int64_t* edge_index, int64_t* edge_type, int64_t* edge_time) {
@@ -444,7 +670,7 @@ __global__ void k_rb_nodes(hgt_gsample_batch_state st, const int64_t* node_off, 
   const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int t = blockIdx.y;
   const int m = blockIdx.z;
-  const Member mb = member(st, m);
+  const auto mb = member(st, m);
   const int64_t noff = node_off[(int64_t)m * st.num_types + t];
   if (noff < 0 || r >= mb.n_layer[t]) return;
   const int64_t lrow = noff + r;
@@ -452,7 +678,7 @@ __global__ void k_rb_nodes(hgt_gsample_batch_state st, const int64_t* node_off, 
   const int64_t tid = st.lid[mb.lid_off[t] + r];
   if (lane == 0) {
     node_type[row] = type_out[t];
-    node_time[row] = st.ltime[mb.type_off[t] + tid];
+    node_time[row] = node_ltime(st, mb, t, tid, r);
     const int64_t so = self_off[(int64_t)m * st.num_types + t];
     if (so >= 0) {
       const int64_t e = so + r, eb = mo.edge_base(m);
@@ -485,7 +711,8 @@ using Hit = int4;
 
 // k_rb_count's counts, flags and mask, plus the hit records: slots claimed with one atomic per warp and kListUnroll * 32
 // neighbours; records past hit_cap are dropped (n_hits still counts them, so the caller sees the overflow).
-__global__ void k_rb_count_host(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
+template <class St>
+__global__ void k_rb_count_host(St st, const hgt_gsample_block* blocks, int32_t n_blocks,
                                 const int64_t* min_ser, const int64_t* cnt_off, int64_t* cnt, Hit* hits,
                                 int64_t hit_cap, unsigned long long* n_hits, int32_t* flags) {
   const int lane = threadIdx.x & 31;
@@ -495,15 +722,15 @@ __global__ void k_rb_count_host(hgt_gsample_batch_state st, const hgt_gsample_bl
   const hgt_gsample_block blk = blocks[b];
   const int T = blk.tgt_type, S = blk.src_type;
   if (r >= cnt_off[mbk + 1] - cnt_off[mbk]) return;
-  const Member mb = member(st, blockIdx.z);
+  const auto mb = member(st, blockIdx.z);
   int64_t c = 0;                                                        // kept edges so far (warp-uniform)
   if (r < mb.n_layer[T]) {
     const int64_t tid = st.lid[mb.lid_off[T] + r];
     const int64_t row = tid < blk.n_row_of ? blk.row_of[tid] : -1;
     if (row >= 0) {
       const int64_t a = blk.ptr[row], e = blk.ptr[row + 1];
-      const int64_t tt = st.ltime[mb.type_off[T] + tid];
-      const int64_t sb = mb.type_off[S], sn = mb.type_off[S + 1] - sb;
+      const int64_t tt = node_ltime(st, mb, T, tid, r);
+      const auto ix = type_ix(st, mb, S);
       const unsigned below = (1u << lane) - 1u;
       for (int64_t p0 = a; p0 < e; p0 += 32 * kListUnroll) {
         int64_t sid[kListUnroll];
@@ -520,12 +747,12 @@ __global__ void k_rb_count_host(hgt_gsample_batch_state st, const hgt_gsample_bl
           const int64_t p = p0 + 32 * u + lane;
           sser[u] = -1;
           if (p < e) {
-            if (sid[u] < 0 || sid[u] >= sn) flags[0] = 1;
-            else sser[u] = st.ser[sb + sid[u]];
+            if (sid[u] < 0 || sid[u] >= ix.n) flags[0] = 1;
+            else sser[u] = ser_of(st, ix, sid[u]);
           }
           const bool kept = sser[u] >= 0 && !masked_out(min_ser, b, r, sser[u]);
           if (kept) {
-            const int64_t dt = tt - st.ltime[sb + sid[u]] + 120;
+            const int64_t dt = tt - src_ltime(st, ix, sid[u], sser[u]) + 120;
             if (dt < 0 || dt >= HGT_RTE_MAX_LEN) flags[1] = 1;
           }
           keep[u] = __ballot_sync(kFull, kept);
@@ -551,7 +778,8 @@ __global__ void k_rb_count_host(hgt_gsample_batch_state st, const hgt_gsample_bl
 
 // One thread per hit record: k_rb_write's outputs without touching the graph (the source id and both times come from
 // the member's device state).
-__global__ void k_rb_write_hits(hgt_gsample_batch_state st, const hgt_gsample_block* blocks, int32_t n_blocks,
+template <class St>
+__global__ void k_rb_write_hits(St st, const hgt_gsample_block* blocks, int32_t n_blocks,
                                 const Hit* hits, int64_t n_hits, const int64_t* cnt_off, const int64_t* ex,
                                 const int64_t* blk_out, const int64_t* node_off, MemOut mo, int64_t* edge_index,
                                 int64_t* edge_type, int64_t* edge_time) {
@@ -562,7 +790,7 @@ __global__ void k_rb_write_hits(hgt_gsample_batch_state st, const hgt_gsample_bl
   const int m = (int)(mbk / n_blocks), b = (int)(mbk % n_blocks);
   if (blk_out[mbk] < 0) return;
   const int T = blocks[b].tgt_type, S = blocks[b].src_type;
-  const Member mb = member(st, m);
+  const auto mb = member(st, m);
   const int64_t r = h.y, sser = h.w;
   const int64_t* noff = node_off + (int64_t)m * st.num_types;
   const int64_t eb = mo.edge_base(m), n_edges = mo.edges(m);
@@ -571,12 +799,13 @@ __global__ void k_rb_write_hits(hgt_gsample_batch_state st, const hgt_gsample_bl
   edge_index[2 * eb + o] = noff[S] + sser;                               // row 0 = source (data.py:245,254)
   edge_index[2 * eb + n_edges + o] = noff[T] + r;
   edge_type[eb + o] = blocks[b].rel;
-  edge_time[eb + o] = st.ltime[mb.type_off[T] + tid] - st.ltime[mb.type_off[S] + sid] + 120;   // data.py:250
+  edge_time[eb + o] = node_ltime(st, mb, T, tid, r) - node_ltime(st, mb, S, sid, sser) + 120;   // data.py:250
 }
 
 // k_rb_nodes with the feature rows read from host memory: 16-byte loads when the row and the output row are 16-byte
 // aligned (feat_dim % 4 == 0 and aligned tables), kRowUnroll of them per lane issued before the first store.
-__global__ void k_rb_nodes_host(hgt_gsample_batch_state st, const int64_t* node_off, const int64_t* type_out,
+template <class St>
+__global__ void k_rb_nodes_host(St st, const int64_t* node_off, const int64_t* type_out,
                                 const int64_t* self_off, int64_t self_rel, MemOut mo, const float* const* feat,
                                 int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature,
                                 int64_t* edge_index, int64_t* edge_type, int64_t* edge_time) {
@@ -584,7 +813,7 @@ __global__ void k_rb_nodes_host(hgt_gsample_batch_state st, const int64_t* node_
   const int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int t = blockIdx.y;
   const int m = blockIdx.z;
-  const Member mb = member(st, m);
+  const auto mb = member(st, m);
   const int64_t noff = node_off[(int64_t)m * st.num_types + t];
   if (noff < 0 || r >= mb.n_layer[t]) return;
   const int64_t lrow = noff + r;
@@ -592,7 +821,7 @@ __global__ void k_rb_nodes_host(hgt_gsample_batch_state st, const int64_t* node_
   const int64_t tid = st.lid[mb.lid_off[t] + r];
   if (lane == 0) {
     node_type[row] = type_out[t];
-    node_time[row] = st.ltime[mb.type_off[t] + tid];
+    node_time[row] = node_ltime(st, mb, t, tid, r);
     const int64_t so = self_off[(int64_t)m * st.num_types + t];
     if (so >= 0) {
       const int64_t e = so + r, eb = mo.edge_base(m);
@@ -659,12 +888,15 @@ struct SelectScratch {
   double *keys_in, *keys_out;
   int32_t *vals_in, *vals_out, *mkey_in, *mkey_out;
   unsigned long long* count;
+  uint64_t *okey_in, *okey_out;                                         // hashed: (member, id) order of the entries
+  int64_t *oent_in, *oent_out;
   void* cub_tmp;
   size_t cub_bytes;
 };
 
-// One member sorts its n ids with one radix sort; B > 1 members add a stable sort by member (mkey) after it.
-size_t carve_select(SelectScratch& s, void* base, int64_t n, int32_t n_members) {
+// One member sorts its n ids with one radix sort; B > 1 members add a stable sort by member (mkey) after it.  The hashed
+// selection sorts its n region entries by (member, id) first.
+size_t carve_select(SelectScratch& s, void* base, int64_t n, int32_t n_members, bool hashed = false) {
   size_t off = 0;
   auto take = [&](size_t bytes) {
     size_t o = off;
@@ -681,6 +913,14 @@ size_t carve_select(SelectScratch& s, void* base, int64_t n, int32_t n_members) 
     s.mkey_out = (int32_t*)take(sizeof(int32_t) * (n + 1));
   }
   s.count = (unsigned long long*)take(sizeof(unsigned long long) * n_members);
+  s.okey_in = s.okey_out = nullptr;
+  s.oent_in = s.oent_out = nullptr;
+  if (hashed) {
+    s.okey_in = (uint64_t*)take(sizeof(uint64_t) * (n + 1));
+    s.okey_out = (uint64_t*)take(sizeof(uint64_t) * (n + 1));
+    s.oent_in = (int64_t*)take(sizeof(int64_t) * (n + 1));
+    s.oent_out = (int64_t*)take(sizeof(int64_t) * (n + 1));
+  }
   s.cub_bytes = 0;
   cub::DeviceRadixSort::SortPairsDescending(nullptr, s.cub_bytes, (const double*)nullptr, (double*)nullptr,
                                             (const int32_t*)nullptr, (int32_t*)nullptr, (int)(n + 1));
@@ -689,6 +929,12 @@ size_t carve_select(SelectScratch& s, void* base, int64_t n, int32_t n_members) 
     cub::DeviceRadixSort::SortPairs(nullptr, b2, (const int32_t*)nullptr, (int32_t*)nullptr, (const int32_t*)nullptr,
                                     (int32_t*)nullptr, (int)(n + 1));
     s.cub_bytes = s.cub_bytes > b2 ? s.cub_bytes : b2;
+  }
+  if (hashed) {
+    size_t b3 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, b3, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int64_t*)nullptr,
+                                    (int64_t*)nullptr, (int)(n + 1));
+    s.cub_bytes = s.cub_bytes > b3 ? s.cub_bytes : b3;
   }
   s.cub_tmp = take(s.cub_bytes);
   return off;
@@ -715,7 +961,8 @@ int budget_bytes(int32_t n_members, int64_t max_targets, int32_t n_blocks, int64
   return 0;
 }
 
-int add_budget(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMember<int64_t> step,
+template <class St>
+int add_budget(const St& hs, PerMember<uint64_t> seed, PerMember<int64_t> step,
                const hgt_gsample_block* blocks, BlockRange br, int32_t max_blocks, const int64_t* tgt_id,
                const int64_t* tgt_time, int64_t max_targets, const int64_t* n_targets, int64_t sampled_number,
                int32_t time_filter, int64_t max_time, int64_t no_time, int32_t* flags, void* workspace,
@@ -757,6 +1004,31 @@ int select_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes, const ch
   return 0;
 }
 
+inline int bits_for(int n) {
+  int bits = 0;
+  while ((1 << bits) < n) ++bits;
+  return bits;
+}
+
+// The keys_in / vals_in pairs of a selection sorted by key, descending and stable, then (B > 1) stably by member: each
+// member's positions end up together in key order, at the member's sel_off.
+int sort_keys(SelectScratch& s, int64_t n_total, int B, const int64_t* d_sel_off, cudaStream_t st,
+              const int32_t** vals) {
+  size_t tmp = s.cub_bytes;
+  HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairsDescending(s.cub_tmp, tmp, s.keys_in, s.keys_out, s.vals_in,
+                                                           s.vals_out, (int)n_total, 0, 64, st));
+  *vals = s.vals_out;
+  if (B > 1) {
+    k_sel_member<<<blocks_for(n_total), kThreads, 0, st>>>(d_sel_off, B, s.vals_out, n_total, s.mkey_in);
+    HGT_LAUNCH_CHECK();
+    tmp = s.cub_bytes;
+    HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, s.mkey_in, s.mkey_out, s.vals_out, s.vals_in,
+                                                   (int)n_total, 0, bits_for(B), st));
+    *vals = s.vals_in;
+  }
+  return 0;
+}
+
 int select(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMember<int64_t> step,
            PerMember<int32_t> type, PerMember<int64_t> sel_off, const int64_t* d_sel_off, int64_t n_total,
            int64_t max_ids, int64_t sampled_number, int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets,
@@ -776,20 +1048,8 @@ int select(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMembe
     k_sel_keys<<<dim3((unsigned)g, B), kThreads, 0, st>>>(hs, type, sel_off, sampled_number, s.count, seed, step,
                                                           s.keys_in, s.vals_in);
     HGT_LAUNCH_CHECK();
-    size_t tmp = s.cub_bytes;
-    HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairsDescending(s.cub_tmp, tmp, s.keys_in, s.keys_out, s.vals_in,
-                                                             s.vals_out, (int)n_total, 0, 64, st));
-    const int32_t* vals = s.vals_out;
-    if (B > 1) {
-      int bits = 0;
-      while ((1 << bits) < B) ++bits;
-      k_sel_member<<<blocks_for(n_total), kThreads, 0, st>>>(d_sel_off, B, s.vals_out, n_total, s.mkey_in);
-      HGT_LAUNCH_CHECK();
-      tmp = s.cub_bytes;
-      HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, s.mkey_in, s.mkey_out, s.vals_out, s.vals_in,
-                                                     (int)n_total, 0, bits, st));
-      vals = s.vals_in;
-    }
+    const int32_t* vals = nullptr;
+    if (int rc = sort_keys(s, n_total, B, d_sel_off, st, &vals)) return rc;
     k_sel_take<<<dim3((unsigned)blocks_for(sampled_number), B), kThreads, 0, st>>>(
         hs, type, sel_off, sampled_number, s.count, vals, tgt_id, tgt_time, flags);
     HGT_LAUNCH_CHECK();
@@ -799,8 +1059,52 @@ int select(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMembe
   return 0;
 }
 
+int hash_select_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes, const char* what) {
+  HGT_REQUIRE(out_bytes && n_members >= 1 && n_members < 65536 && n_total >= 0 && n_total < (int64_t(1) << 31) - 1,
+              "%s: %lld entries of %d members do not fit int32 sort values", what, (long long)n_total, n_members);
+  SelectScratch s;
+  *out_bytes = carve_select(s, nullptr, n_total, n_members, true);
+  return 0;
+}
+
+int hash_select(const hgt_gsample_hash_state& hs, const int32_t* type, const int64_t* step, const int64_t* sel_off,
+                int64_t n_total, int64_t max_room, int64_t sampled_number, int64_t* tgt_id, int64_t* tgt_time,
+                int64_t* n_targets, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream,
+                const char* what) {
+  size_t need = 0;
+  if (int rc = hash_select_bytes(hs.n_members, n_total, &need, what)) return rc;
+  HGT_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", what, workspace_bytes, need);
+  const int B = hs.n_members;
+  cudaStream_t st = (cudaStream_t)stream;
+  SelectScratch s;
+  carve_select(s, workspace, n_total, B, true);
+  HGT_CHECK_CUDA(cudaMemsetAsync(s.count, 0, sizeof(unsigned long long) * B, st));
+  if (n_total > 0 && max_room > 0) {
+    const int64_t g = blocks_for(max_room);
+    k_hsel_order<<<dim3((unsigned)(g < 1024 ? g : 1024), B), kThreads, 0, st>>>(hs, type, sel_off, s.okey_in,
+                                                                                 s.oent_in, s.count);
+    HGT_LAUNCH_CHECK();
+    size_t tmp = s.cub_bytes;
+    HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, s.okey_in, s.okey_out, s.oent_in, s.oent_out,
+                                                   (int)n_total, 0, kIdBits + bits_for(B), st));
+    k_hsel_keys<<<dim3((unsigned)g, B), kThreads, 0, st>>>(hs, type, sel_off, sampled_number, s.count, step,
+                                                           s.okey_out, s.oent_out, s.keys_in, s.vals_in);
+    HGT_LAUNCH_CHECK();
+    const int32_t* vals = nullptr;
+    if (int rc = sort_keys(s, n_total, B, sel_off, st, &vals)) return rc;
+    k_hsel_take<<<dim3((unsigned)blocks_for(sampled_number), B), kThreads, 0, st>>>(
+        hs, type, sel_off, sampled_number, s.count, vals, s.oent_out, tgt_id, tgt_time, flags);
+    HGT_LAUNCH_CHECK();
+  }
+  k_sel_finish<<<(unsigned)blocks_for(B, 32), 32, 0, st>>>(hs, PerMember<int32_t>{type, 0}, sampled_number, s.count,
+                                                           n_targets);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
 // n_hits != NULL: the single-read count pass of a host-resident graph, leaving up to hit_cap hit records in `hits`.
-int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
+template <class St>
+int rebuild_count(const St& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
                   const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count, int64_t max_rows,
                   const int64_t* feat_rows, Hit* hits, int64_t hit_cap, unsigned long long* n_hits, int64_t* ex,
                   int64_t* totals, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream,
@@ -844,7 +1148,8 @@ int rebuild_count(const hgt_gsample_batch_state& hs, const hgt_gsample_block* bl
 
 // host_graph: the instances for a host-resident graph (k_rb_write_hits over the n_hits records in `hits`, or k_rb_write
 // when hits is NULL; k_rb_nodes_host).
-int rebuild_write(const hgt_gsample_batch_state& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
+template <class St>
+int rebuild_write(const St& hs, const hgt_gsample_block* blocks, int32_t n_blocks,
                   const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out,
                   const int64_t* node_off,
                   const int64_t* type_out, const int64_t* self_off, int64_t self_rel, MemOut mo, int64_t max_rows,
@@ -1078,4 +1383,95 @@ extern "C" int hgt_gsample_batch_rebuild_write_host(
                        self_rel, {mem_out, 0}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
                        node_time, node_feature, edge_index, edge_type, edge_time, stream,
                        "hgt_gsample_batch_rebuild_write_host");
+}
+
+// ---- the hashed state -------------------------------------------------------------------------------------------------
+
+extern "C" int hgt_gsample_hash_insert_seeds(const hgt_gsample_hash_state* h_state, int64_t n, const int64_t* region,
+                                             const int64_t* id, const int64_t* ser, const int64_t* time, int32_t* flags,
+                                             void* stream) {
+  HGT_REQUIRE(h_state && h_state->num_types > 0 && n >= 0 && (n == 0 || (region && id && ser && time && flags)),
+              "hgt_gsample_hash_insert_seeds: bad arguments");
+  if (n == 0) return 0;
+  k_hash_seed<<<(unsigned)blocks_for(n), kThreads, 0, (cudaStream_t)stream>>>(*h_state, n, region, id, ser, time, flags);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int hgt_gsample_hash_add_budget(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
+                                           const int32_t* type_blocks, int32_t max_blocks, const int32_t* type,
+                                           const int64_t* step, const int64_t* tgt_id, const int64_t* tgt_time,
+                                           int64_t max_targets, const int64_t* n_targets, int64_t sampled_number,
+                                           int32_t time_filter, int64_t max_time, int64_t no_time, int32_t* flags,
+                                           void* workspace, size_t workspace_bytes, void* stream) {
+  HGT_REQUIRE(h_state && h_state->seed && type_blocks && type && step && n_targets && sampled_number > 0 &&
+                  max_targets >= 0 && max_blocks >= 0,
+              "hgt_gsample_hash_add_budget: bad arguments");
+  return add_budget(*h_state, {h_state->seed, 0}, {step, 0}, blocks, {type_blocks, type, max_blocks}, max_blocks,
+                    tgt_id, tgt_time, max_targets, n_targets, sampled_number, time_filter, max_time, no_time, flags,
+                    workspace, workspace_bytes, stream, "hgt_gsample_hash_add_budget");
+}
+
+extern "C" int hgt_gsample_hash_select_workspace_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes) {
+  return hash_select_bytes(n_members, n_total, out_bytes, "hgt_gsample_hash_select_workspace_bytes");
+}
+
+extern "C" int hgt_gsample_hash_select(const hgt_gsample_hash_state* h_state, const int32_t* type, const int64_t* step,
+                                       const int64_t* sel_off, int64_t n_total, int64_t max_room,
+                                       int64_t sampled_number, int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets,
+                                       int32_t* flags, void* workspace, size_t workspace_bytes, void* stream) {
+  HGT_REQUIRE(h_state && h_state->seed && type && step && sel_off && sampled_number > 0 && max_room >= 0,
+              "hgt_gsample_hash_select: bad arguments");
+  return hash_select(*h_state, type, step, sel_off, n_total, max_room, sampled_number, tgt_id, tgt_time, n_targets,
+                     flags, workspace, workspace_bytes, stream, "hgt_gsample_hash_select");
+}
+
+extern "C" int hgt_gsample_hash_rebuild_count(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
+                                              int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                              int64_t n_count, int64_t max_rows, const int64_t* feat_rows, int64_t* ex,
+                                              int64_t* totals, int32_t* flags, void* workspace,
+                                              size_t workspace_bytes, void* stream) {
+  HGT_REQUIRE(h_state, "hgt_gsample_hash_rebuild_count: bad arguments");
+  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, nullptr, 0, nullptr,
+                       ex, totals, flags, workspace, workspace_bytes, stream, "hgt_gsample_hash_rebuild_count");
+}
+
+extern "C" int hgt_gsample_hash_rebuild_write(
+    const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks, const int64_t* min_ser,
+    const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
+    const int64_t* self_off, int64_t self_rel, const int64_t* mem_out, int64_t max_rows, const float* const* feat,
+    int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature, int64_t* edge_index,
+    int64_t* edge_type, int64_t* edge_time, void* stream) {
+  HGT_REQUIRE(h_state && mem_out, "hgt_gsample_hash_rebuild_write: bad arguments");
+  return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
+                       self_rel, {mem_out, 0}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
+                       node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_hash_rebuild_write");
+}
+
+extern "C" int hgt_gsample_hash_rebuild_count_host(const hgt_gsample_hash_state* h_state,
+                                                   const hgt_gsample_block* blocks, int32_t n_blocks,
+                                                   const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count,
+                                                   int64_t max_rows, const int64_t* feat_rows, void* hits,
+                                                   int64_t hit_cap, int64_t* n_hits, int64_t* ex, int64_t* totals,
+                                                   int32_t* flags, void* workspace, size_t workspace_bytes,
+                                                   void* stream) {
+  HGT_REQUIRE(h_state && n_hits && hit_cap >= 0 && hit_cap < (int64_t(1) << 31) && (hits || hit_cap == 0) &&
+                  (int64_t)n_blocks * h_state->n_members < (int64_t(1) << 31),
+              "hgt_gsample_hash_rebuild_count_host: bad arguments");
+  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, (Hit*)hits, hit_cap,
+                       (unsigned long long*)n_hits, ex, totals, flags, workspace, workspace_bytes, stream,
+                       "hgt_gsample_hash_rebuild_count_host");
+}
+
+extern "C" int hgt_gsample_hash_rebuild_write_host(
+    const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks, const int64_t* min_ser,
+    const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
+    const int64_t* self_off, int64_t self_rel, const int64_t* mem_out, int64_t max_rows, const void* hits,
+    int64_t n_hits, const float* const* feat, int32_t feat_dim, int64_t* node_type, int64_t* node_time,
+    float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream) {
+  HGT_REQUIRE(h_state && mem_out && n_hits >= 0, "hgt_gsample_hash_rebuild_write_host: bad arguments");
+  return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
+                       self_rel, {mem_out, 0}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
+                       node_time, node_feature, edge_index, edge_type, edge_time, stream,
+                       "hgt_gsample_hash_rebuild_write_host");
 }

@@ -472,6 +472,13 @@ class _GBatchState(_c.Structure):            # hgt_gsample_batch_state
                 [(n, _c.c_void_p) for n in _GState._PTRS + ("seed",)])
 
 
+class _GHashState(_c.Structure):             # hgt_gsample_hash_state
+    _fields_ = ([("num_types", _c.c_int32), ("n_members", _c.c_int32)] +
+                [(n, _c.c_void_p) for n in ("ent_off", "lid_off", "n_ids", "key", "ser", "ltime", "lid", "n_layer",
+                                            "score", "btime", "bstamp", "last_seq", "first_seq", "fill", "type_min",
+                                            "type_seq", "counters", "seed")])
+
+
 # hgt_merge_member (include/hgt_b200.h)
 MERGE_MEMBER_DTYPE = np.dtype([("node_feature", "<u8"), ("edge_index", "<u8"), ("edge_type", "<u8"),
                                ("edge_time", "<u8"), ("n_nodes", "<i8"), ("n_edges", "<i8"), ("node_base", "<i8"),
@@ -481,6 +488,53 @@ MERGE_MEMBER_DTYPE = np.dtype([("node_feature", "<u8"), ("edge_index", "<u8"), (
 _I64_MAX = np.iinfo(np.int64).max
 _PAGE = 4096
 _HIT_ROOM = 8.0          # hit records a host-placed graph's first rebuild reserves per count slot
+_STATE_ROOM = 64.0       # hashed-state entries a graph's first call reserves per (layer capacity + width) of a region
+_ID_LIMIT = 2 ** 40      # node ids fill the low 40 bits of the selection's Philox counter
+_FORCE_LAYOUT = None     # tests only: "dense" or "hashed" instead of _state_layout's choice
+_SLOT_BYTES = 52         # dense state per id, hashed state per entry (key 8, ser 4, score / times / stamps 5 x 8)
+_DENSE_SHARE = 0.5       # the dense state may take at most this share of the device's free memory
+_MEMORY_CHECK_FROM = 1 << 28   # dense states smaller than this never ask the device for its free memory
+# hashed when the dense state has this many times more slots than the hashed one has entries, and at least
+# _HASHED_FROM_SLOTS slots.  scripts/hashed_state_sampler_bench.py (H100 80GB HBM3, 700 W): at 0.5-2.6 slots per entry
+# the dense state is faster at B = 1 (hashed 1.11-1.29x its time), at 7 still at B = 1 (1.19x) while B = 8 / 32 favour
+# the hashed one (0.60-0.90x), and from 21 on the hashed state is faster at every B (0.15-0.68x)
+_HASHED_FROM = 16.0
+_HASHED_FROM_SLOTS = 1 << 22   # below it (a 218 MB dense state) the dense state is cheap whatever the ratio
+
+
+def _hash_rooms(n_ids, cap, width, state_room):
+    """Entries of each (member, type) region of the hashed state: state_room per unit of layer capacity plus width, at
+    most twice the id range (a region that large holds every id at a load of 1/2 and cannot overflow)."""
+    want = np.ceil(state_room * (np.asarray(cap, dtype=np.float64) + width)).astype(np.int64)
+    return np.minimum(2 * np.asarray(n_ids, dtype=np.int64), want)
+
+
+def _state_layout(n_ids, rooms, free_bytes=None):
+    """The sampler state of a call whose members have id ranges n_ids [B, T] and hashed regions of rooms [B, T]
+    entries: "hashed" where the dense state cannot run (a selection step's ids past int32 sort values, or more than
+    _DENSE_SHARE of free_bytes, the device's free memory, None = not asked) or has at least _HASHED_FROM_SLOTS slots
+    and _HASHED_FROM times more slots than the hashed state has entries; "dense" otherwise."""
+    n_ids, rooms = np.asarray(n_ids, dtype=np.int64), np.asarray(rooms, dtype=np.int64)
+    if int(n_ids.max(axis=1).sum()) >= 2 ** 31 - 1:
+        return "hashed"
+    if free_bytes is not None and _SLOT_BYTES * int(n_ids.sum()) > _DENSE_SHARE * free_bytes:
+        return "hashed"
+    slots = int(n_ids.sum())
+    return "hashed" if slots >= _HASHED_FROM_SLOTS and slots > _HASHED_FROM * int(rooms.sum()) else "dense"
+
+
+def _free_bytes_if_dense_is_large(dev, n_ids):
+    """The device's free memory when the dense state of id ranges n_ids would be large enough for it to matter."""
+    import torch
+    if _SLOT_BYTES * int(np.asarray(n_ids).sum()) < _MEMORY_CHECK_FROM:
+        return None
+    return torch.cuda.mem_get_info(dev)[0]
+
+
+def _grow_state_room(dg, restarts):
+    """A hashed region overflowed: four times the room per unit from now on (the call restarts with it)."""
+    dg.state_room *= 4.0
+    return restarts + 1
 
 
 def _pin(a, dtype):
@@ -553,8 +607,10 @@ class DeviceGraph:
     PCIe, so the graph may be far larger than device memory; only the per-block descriptors and per-type tables go to the
     device.  There is one host copy of each array: the FrozenGraph's blocks are rebound to the pinned copies of their
     ``row_of`` / ``ptr`` / ``nbr`` / ``time`` (the host sampler keeps working on them), and the feature tables passed in
-    are copied, not kept.  Sampling gives bitwise the same batches either way; the sampler state still lives on the device
-    (``sample_subgraphs_cuda``: about B x 52 bytes x the sum of the id ranges).
+    are copied, not kept.  Sampling gives bitwise the same batches either way; the sampler state lives on the device
+    (``sample_subgraphs_cuda``: dense over the id ranges, or hash tables sized by the sample).  ``state_room`` is the
+    hashed state's current region size estimate (grown by calls that overflowed it), ``sampler_state`` describes the
+    last call's state.
 
     Node types are laid out in ``graph.get_types()`` order (as ``to_torch`` does), so every type of the graph's
     ``edge_list`` must be one of them; relation names come from ``graph.get_meta_graph()`` plus ``'self'``."""
@@ -580,6 +636,8 @@ class DeviceGraph:
         self.n_ids = [fg.n_ids.get(t, 0) for t in self.types]
         self.placement = placement
         self.hit_room = _HIT_ROOM
+        self.state_room = _STATE_ROOM
+        self.sampler_state = None     # the last sample_subgraphs_cuda call's {layout, entries, load, restarts}
         dev = self.device
         host = placement == "host"
 
@@ -771,8 +829,15 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     ``sample_subgraph_cuda`` returns from a generator advanced by b draws.  Every kernel launch and read-back is shared by
     the members: one read-back per sampling layer (every member's type order) and one at the end, whatever B is.
 
-    Device memory: about B x 52 bytes x (sum of the graph's id ranges) of sampler state (~100 MB per member at ogbn-mag
-    scale), plus add_budget scratch of B x 24 bytes x width x (max targets x blocks per type)."""
+    Device memory: the sampler state is dense or hashed, chosen per call from B, the id ranges, depth, width and the
+    graph's room estimate (``_state_layout``); both give bitwise the same batches.  The dense state takes about B x 52
+    bytes x (sum of the id ranges) (~100 MB per member at ogbn-mag scale) and sorts a selected type's whole id range
+    per step.  The hashed state keeps one hash table per (member, type) of at most twice the type's id range, sized by
+    the sample: about 52 bytes per entry plus 8 per layer slot, and a step sorts the type's table, not its ids.  It is
+    used where the dense state cannot run (a step's id ranges past 2^31 - 1 ids, or more than half the free device
+    memory) and where the id ranges outnumber the table entries 16 to 1 (at least 2^22 ids).  A table that overflows
+    restarts the call from the same draws with 4x larger tables (one more read-back; later calls start from that size).
+    Node ids must be below 2^40.  Plus add_budget scratch of B x 24 bytes x width x (max targets x blocks per type)."""
     import torch
     from . import _lib
     from . import plan as _plan
@@ -796,32 +861,25 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
         for s, ids, _ in seeds:
             n_ids[b, s] = max(n_ids[b, s], int(ids.max()) + 1)
             n_seed[b, s] = ids.shape[0]
+    if n_ids.size and int(n_ids.max()) > _ID_LIMIT:
+        raise ValueError("node ids must be below 2^40 (the Philox counter's id field), got %d" % (int(n_ids.max()) - 1))
     cap = np.minimum(n_ids, n_seed + depth * W)
 
     def offsets(per):                                      # [B, T] sizes -> [B, T+1] absolute starts
         flat = np.concatenate([[0], np.cumsum(per.reshape(-1))]).astype(np.int64)
         return np.stack([flat[b * T:b * T + T + 1] for b in range(B)]), int(flat[-1])
 
-    type_off, n_slots = offsets(n_ids)
     lid_off, n_lid = offsets(cap)
-
+    layout = _FORCE_LAYOUT or _state_layout(n_ids, _hash_rooms(n_ids, cap, W, dg.state_room),
+                                            _free_bytes_if_dense_is_large(dev, n_ids))
+    hashed = layout == "hashed"
     i64 = dict(dtype=torch.int64, device=dev)
-    ser = torch.full((max(n_slots, 1),), -1, dtype=torch.int32, device=dev)
-    ltime = torch.zeros(max(n_slots, 1), **i64)
-    lid = torch.zeros(max(n_lid, 1), **i64)
-    score = torch.zeros(max(n_slots, 1), **i64)
-    btime = torch.zeros(max(n_slots, 1), **i64)
-    bstamp = torch.full((max(n_slots, 1),), -1, **i64)
-    last_seq = torch.full((max(n_slots, 1),), -1, **i64)
-    first_seq = torch.full((max(n_slots, 1),), _I64_MAX, **i64)
-    # one small buffer the host reads: [n_layer B*T | type_seq B*2T | block totals B*NB | flags | hit count (host graph)]
     host = dg.placement == "host"
-    meta = torch.zeros(3 * B * T + B * NB + 2 + int(host), **i64)
-    n_layer, type_seq = meta[:B * T], meta[B * T:3 * B * T]
-    totals = meta[3 * B * T:3 * B * T + B * NB]
-    flags = meta[3 * B * T + B * NB:3 * B * T + B * NB + 2].view(torch.int32)   # 4 int32 flags
-    type_min = torch.full((max(2 * B * T, 1),), _I64_MAX, **i64)
-    counters = torch.zeros(2 * B, **i64)
+    # one small buffer the host reads: [n_layer B*T | type_seq B*2T | block totals B*NB | flags | hit count (host graph)
+    # | entries claimed per (member, type) region (hashed state)]
+    o_ts, o_tot, o_fl = B * T, 3 * B * T, 3 * B * T + B * NB
+    o_hit = o_fl + 2
+    o_fill = o_hit + int(host)
 
     if generator is None:
         draws = [int(torch.randint(0, 2 ** 63 - 1, (1,))) for _ in range(B)]
@@ -829,143 +887,199 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
         draws = [int(torch.randint(0, 2 ** 63 - 1, (1,), generator=generator, device=generator.device))
                  for _ in range(B)]
 
-    # seeds enter layer_data first, in inp order (data.py:135-137); their add_budget runs seed type after seed type,
-    # step j being every member's j-th seed type
-    up = _Upload()
-    up.add("type_off", type_off)
-    up.add("lid_off", lid_off)
-    up.add("seed", np.asarray(draws, dtype=np.uint64).view(np.int64))
-    seq0 = np.full((B, 2 * T), -1, dtype=np.int64)
-    nl0 = np.zeros((B, T), dtype=np.int64)
-    cnt0 = np.zeros((B, 2), dtype=np.int64)
-    slots, sers, tms, lpos, lids = [], [], [], [], []
-    for b, seeds in enumerate(members):
-        cnt0[b, 0] = len(seeds)
-        for k, (s, ids, tm) in enumerate(seeds):
-            seq0[b, 2 * s] = k
-            nl0[b, s] = ids.shape[0]
-            slots.append(type_off[b, s] + ids)
-            sers.append(np.arange(ids.shape[0]))
-            tms.append(tm)
-            lpos.append(lid_off[b, s] + np.arange(ids.shape[0]))
-            lids.append(ids)
-    n_in = sum(a.shape[0] for a in slots)
-    for name, parts in (("slots", slots), ("sers", sers), ("tms", tms), ("lpos", lpos), ("lids", lids)):
-        up.add(name, np.concatenate(parts) if parts else np.zeros(0, np.int64))
-    up.add("nl0", nl0)
-    up.add("seq0", seq0)
-    up.add("cnt0", cnt0)
-    J = max(len(s) for s in members)
-    seed_steps = []                                       # (max targets, names) of seed step j
-    for j in range(J):
-        M = max((s[j][1].shape[0] for s in members if j < len(s)), default=0)
-        ids_j, tms_j = np.zeros((B, M), np.int64), np.zeros((B, M), np.int64)
-        n_j, type_j = np.zeros(B, np.int64), np.full(B, -1, np.int32)
-        for b, seeds in enumerate(members):
-            if j < len(seeds):
-                s, ids, tm = seeds[j]
-                ids_j[b, :ids.shape[0]], tms_j[b, :ids.shape[0]] = ids, tm
-                n_j[b], type_j[b] = ids.shape[0], s
-        for name, arr, dt in (("ids", ids_j, np.int64), ("tms", tms_j, np.int64), ("n", n_j, np.int64),
-                              ("type", type_j, np.int32), ("step", np.full(B, j), np.int64)):
-            up.add("seed%d_%s" % (j, name), arr, dt)
-        seed_steps.append(M)
-    d = up.to(dev)
-    if n_in:
-        sl_d = d.view("slots")
-        ser.index_put_((sl_d,), d.view("sers").to(torch.int32))
-        ltime.index_put_((sl_d,), d.view("tms"))
-        lid.index_put_((d.view("lpos"),), d.view("lids"))
-    n_layer.copy_(d.view("nl0"))
-    type_seq.copy_(d.view("seq0"))
-    counters.copy_(d.view("cnt0"))
+    restarts = 0
+    while True:                 # hashed state: once more from the same draws with larger regions after an overflow
+        meta = torch.zeros(o_fill + B * T * int(hashed), **i64)
+        n_layer, type_seq = meta[:B * T], meta[o_ts:o_tot]
+        totals = meta[o_tot:o_fl]
+        flags = meta[o_fl:o_hit].view(torch.int32)          # 4 int32 flags; [3]: a hashed region overflowed
+        type_min = torch.full((max(2 * B * T, 1),), _I64_MAX, **i64)
+        counters = torch.zeros(2 * B, **i64)
+        lid = torch.zeros(max(n_lid, 1), **i64)
+        if hashed:
+            rooms = _hash_rooms(n_ids, cap, W, dg.state_room)
+            type_off, n_slots = offsets(rooms)             # the (member, type) regions
+            ltime = torch.zeros(max(n_lid, 1), **i64)
+            key = torch.full((max(n_slots, 1),), -1, **i64)
+        else:
+            rooms = n_ids
+            type_off, n_slots = offsets(n_ids)
+            ltime = torch.zeros(max(n_slots, 1), **i64)
+        ser = torch.full((max(n_slots, 1),), -1, dtype=torch.int32, device=dev)
+        score = torch.zeros(max(n_slots, 1), **i64)
+        btime = torch.zeros(max(n_slots, 1), **i64)
+        bstamp = torch.full((max(n_slots, 1),), -1, **i64)
+        last_seq = torch.full((max(n_slots, 1),), -1, **i64)
+        first_seq = torch.full((max(n_slots, 1),), _I64_MAX, **i64)
 
-    cst = _GBatchState(T, B, d.ptr("type_off"), d.ptr("lid_off"), ser.data_ptr(), ltime.data_ptr(), lid.data_ptr(),
-                       n_layer.data_ptr(), score.data_ptr(), btime.data_ptr(), bstamp.data_ptr(), last_seq.data_ptr(),
-                       first_seq.data_ptr(), type_min.data_ptr(), type_seq.data_ptr(), counters.data_ptr(),
-                       d.ptr("seed"))
-    st = torch.cuda.current_stream(dev).cuda_stream
-    time_filter = time_range is not None
-    max_time = int(np.max(list(time_range.keys()))) if time_filter else 0
-
-    max_nb = dg.max_type_blocks
-    max_tg = max([W] + seed_steps)
-    bud_ws, sel_ws = _c.c_size_t(), _c.c_size_t()
-    _lib.call("hgt_gsample_batch_add_budget_workspace_bytes", B, max_tg, max_nb, W, _c.byref(bud_ws))
-    _lib.call("hgt_gsample_batch_select_workspace_bytes", B, int(n_ids.max(axis=1).sum()), _c.byref(sel_ws))
-    ws = torch.empty(max(bud_ws.value, sel_ws.value, 1), dtype=torch.uint8, device=dev)
-    tgt = torch.zeros(2 * B * W + B, **i64)               # [ids B*W | times B*W | counts B]
-    tgt_id, tgt_time, n_tgt = tgt[:B * W], tgt[B * W:2 * B * W], tgt[2 * B * W:]
-
-    blocks_p, range_p, flags_p, ws_p, ws_n = (dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr(),
-                                              flags.data_ptr(), ws.data_ptr(), ws.numel())
-    tgt_id_p, tgt_time_p, n_tgt_p = tgt_id.data_ptr(), tgt_time.data_ptr(), n_tgt.data_ptr()
-
-    def add_budget(type_p, step_p, ids_p, tms_p, max_targets, count_p):
-        _lib.call("hgt_gsample_batch_add_budget", _c.byref(cst), blocks_p, range_p, max_nb, type_p, step_p, ids_p,
-                  tms_p, max_targets, count_p, W, int(time_filter), max_time, _NO_TIME, flags_p, ws_p, ws_n, st)
-
-    for j, M in enumerate(seed_steps):                    # the seeds' budgets (data.py:139-141)
-        add_budget(d.ptr("seed%d_type" % j), d.ptr("seed%d_step" % j), d.ptr("seed%d_ids" % j),
-                   d.ptr("seed%d_tms" % j), M, d.ptr("seed%d_n" % j))
-    step = np.asarray([len(s) for s in members], dtype=np.int64)   # a member's next step number
-    for _layer in range(depth):                           # data.py:146-170
-        ts = type_seq.cpu().numpy().reshape(B, 2 * T)     # the per-layer read-back: every member's list(budget.keys())
-        orders = [sorted((t for t in range(T) if ts[b, 2 * t + 1] >= 0), key=lambda t: ts[b, 2 * t + 1])
-                  for b in range(B)]
-        K = max(len(o) for o in orders)
-        if K == 0:
-            continue
-        # step k of the layer: member b selects its k-th budget type (or sits out), then adds its budget
-        typ = np.full((K, B), -1, dtype=np.int32)
-        for b, o in enumerate(orders):
-            typ[:len(o), b] = o
-        rng = np.where(typ >= 0, n_ids[np.arange(B)[None, :], np.maximum(typ, 0)], 0)      # ids each member sorts
-        off = np.zeros((K, B + 1), dtype=np.int64)
-        np.cumsum(rng, axis=1, out=off[:, 1:])
+        # seeds enter layer_data first, in inp order (data.py:135-137); their add_budget runs seed type after seed type,
+        # step j being every member's j-th seed type
         up = _Upload()
-        up.add("type", typ, np.int32)
-        up.add("step", step[None, :] + np.arange(K)[:, None])
-        up.add("off", off)
-        d = up.to(dev)
-        type0, step0, off0 = d.ptr("type"), d.ptr("step"), d.ptr("off")
-        for k in range(K):
-            type_p, step_p = type0 + 4 * k * B, step0 + 8 * k * B
-            _lib.call("hgt_gsample_batch_select", _c.byref(cst), type_p, step_p, off0 + 8 * k * (B + 1),
-                      int(off[k, B]), int(rng[k].max()), W, tgt_id_p, tgt_time_p, n_tgt_p, flags_p, ws_p, ws_n, st)
-            add_budget(type_p, step_p, tgt_id_p, tgt_time_p, W, n_tgt_p)
-        step += np.asarray([len(o) for o in orders], dtype=np.int64)
+        up.add("type_off", type_off)
+        up.add("lid_off", lid_off)
+        up.add("n_ids", n_ids)
+        up.add("seed", np.asarray(draws, dtype=np.uint64).view(np.int64))
+        seq0 = np.full((B, 2 * T), -1, dtype=np.int64)
+        nl0 = np.zeros((B, T), dtype=np.int64)
+        cnt0 = np.zeros((B, 2), dtype=np.int64)
+        slots, sers, tms, lpos, lids = [], [], [], [], []
+        for b, seeds in enumerate(members):
+            cnt0[b, 0] = len(seeds)
+            for k, (s, ids, tm) in enumerate(seeds):
+                seq0[b, 2 * s] = k
+                nl0[b, s] = ids.shape[0]
+                # the dense state's slots; the hashed state's (member, type) regions
+                slots.append(np.full(ids.shape[0], b * T + s) if hashed else type_off[b, s] + ids)
+                sers.append(np.arange(ids.shape[0]))
+                tms.append(tm)
+                lpos.append(lid_off[b, s] + np.arange(ids.shape[0]))
+                lids.append(ids)
+        n_in = sum(a.shape[0] for a in slots)
+        for name, parts in (("slots", slots), ("sers", sers), ("tms", tms), ("lpos", lpos), ("lids", lids)):
+            up.add(name, np.concatenate(parts) if parts else np.zeros(0, np.int64))
+        up.add("nl0", nl0)
+        up.add("seq0", seq0)
+        up.add("cnt0", cnt0)
+        J = max(len(s) for s in members)
+        seed_steps = []                                   # (max targets, names) of seed step j
+        for j in range(J):
+            M = max((s[j][1].shape[0] for s in members if j < len(s)), default=0)
+            ids_j, tms_j = np.zeros((B, M), np.int64), np.zeros((B, M), np.int64)
+            n_j, type_j = np.zeros(B, np.int64), np.full(B, -1, np.int32)
+            for b, seeds in enumerate(members):
+                if j < len(seeds):
+                    s, ids, tm = seeds[j]
+                    ids_j[b, :ids.shape[0]], tms_j[b, :ids.shape[0]] = ids, tm
+                    n_j[b], type_j[b] = ids.shape[0], s
+            for name, arr, dt in (("ids", ids_j, np.int64), ("tms", tms_j, np.int64), ("n", n_j, np.int64),
+                                  ("type", type_j, np.int32), ("step", np.full(B, j), np.int64)):
+                up.add("seed%d_%s" % (j, name), arr, dt)
+            seed_steps.append(M)
+        # the state's tables: cst points into this upload, so it is held until the call returns
+        tabs = d = up.to(dev)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        if hashed:
+            cst = _GHashState(T, B, tabs.ptr("type_off"), tabs.ptr("lid_off"), tabs.ptr("n_ids"), key.data_ptr(),
+                              ser.data_ptr(), ltime.data_ptr(), lid.data_ptr(), n_layer.data_ptr(), score.data_ptr(),
+                              btime.data_ptr(), bstamp.data_ptr(), last_seq.data_ptr(), first_seq.data_ptr(),
+                              meta[o_fill:].data_ptr(), type_min.data_ptr(), type_seq.data_ptr(), counters.data_ptr(),
+                              tabs.ptr("seed"))
+            _lib.call("hgt_gsample_hash_insert_seeds", _c.byref(cst), n_in, d.ptr("slots"), d.ptr("lids"),
+                      d.ptr("sers"), d.ptr("tms"), flags.data_ptr(), st)
+        else:
+            if n_in:
+                sl_d = d.view("slots")
+                ser.index_put_((sl_d,), d.view("sers").to(torch.int32))
+                ltime.index_put_((sl_d,), d.view("tms"))
+                lid.index_put_((d.view("lpos"),), d.view("lids"))
+            cst = _GBatchState(T, B, tabs.ptr("type_off"), tabs.ptr("lid_off"), ser.data_ptr(), ltime.data_ptr(),
+                               lid.data_ptr(), n_layer.data_ptr(), score.data_ptr(), btime.data_ptr(),
+                               bstamp.data_ptr(), last_seq.data_ptr(), first_seq.data_ptr(), type_min.data_ptr(),
+                               type_seq.data_ptr(), counters.data_ptr(), tabs.ptr("seed"))
+        n_layer.copy_(d.view("nl0"))
+        type_seq.copy_(d.view("seq0"))
+        counters.copy_(d.view("cnt0"))
+        api = "hgt_gsample_hash_" if hashed else "hgt_gsample_batch_"
+        time_filter = time_range is not None
+        max_time = int(np.max(list(time_range.keys()))) if time_filter else 0
 
-    # rebuild (data.py:181-209): count pass, then the one read-back of the batch
-    cnt_off = np.concatenate([[0], np.cumsum([cap[b, tt] for b in range(B) for tt, _, _ in dg.blocks])]).astype(np.int64)
-    n_count = int(cnt_off[-1])
-    max_rows = int(cap.max()) if cap.size else 0
-    rb_ws = _c.c_size_t()
-    _lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
-    rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
-    ex = torch.empty(n_count + 1, **i64)
-    # the mask table rides behind cnt_off in the same copy; the masked entry points take it right after n_blocks
-    cnt_off_d = _plan._to_dev_async(cnt_off if min_ser is None else np.concatenate([cnt_off, min_ser]), dev)
-    masked = () if min_ser is None else (cnt_off_d.data_ptr() + 8 * cnt_off.shape[0],)
-    suffix = "" if min_ser is None else "_masked"
-    feat_rows_p = _lib.ptr(dg.feat_rows) if dg.features is not None else None
-    if host:
-        # single-read count pass: the kept edges' hit records (16 bytes each) stay in device scratch for the write pass
-        hit_cap = _hit_capacity(dg, n_count)
-        hits = torch.empty(16 * max(hit_cap, 1), dtype=torch.uint8, device=dev)
-        _lib.call("hgt_gsample_batch_rebuild_count_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
-                  masked[0] if masked else None, cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, hits.data_ptr(),
-                  hit_cap, meta[-1:].data_ptr(), ex.data_ptr(), totals.data_ptr(), flags.data_ptr(), rb.data_ptr(),
-                  rb.numel(), st)
-    else:
-        _lib.call("hgt_gsample_batch_rebuild_count" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
-                  cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, ex.data_ptr(), totals.data_ptr(),
-                  flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
-    h = meta.cpu().numpy()
+        max_nb = dg.max_type_blocks
+        max_tg = max([W] + seed_steps)
+        bud_ws, sel_ws = _c.c_size_t(), _c.c_size_t()
+        _lib.call("hgt_gsample_batch_add_budget_workspace_bytes", B, max_tg, max_nb, W, _c.byref(bud_ws))
+        _lib.call(api + "select_workspace_bytes", B, int(rooms.max(axis=1).sum()), _c.byref(sel_ws))
+        ws = torch.empty(max(bud_ws.value, sel_ws.value, 1), dtype=torch.uint8, device=dev)
+        tgt = torch.zeros(2 * B * W + B, **i64)           # [ids B*W | times B*W | counts B]
+        tgt_id, tgt_time, n_tgt = tgt[:B * W], tgt[B * W:2 * B * W], tgt[2 * B * W:]
+
+        blocks_p, range_p, flags_p, ws_p, ws_n = (dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr(),
+                                                  flags.data_ptr(), ws.data_ptr(), ws.numel())
+        tgt_id_p, tgt_time_p, n_tgt_p = tgt_id.data_ptr(), tgt_time.data_ptr(), n_tgt.data_ptr()
+
+        def add_budget(type_p, step_p, ids_p, tms_p, max_targets, count_p):
+            _lib.call(api + "add_budget", _c.byref(cst), blocks_p, range_p, max_nb, type_p, step_p, ids_p, tms_p,
+                      max_targets, count_p, W, int(time_filter), max_time, _NO_TIME, flags_p, ws_p, ws_n, st)
+
+        for j, M in enumerate(seed_steps):                # the seeds' budgets (data.py:139-141)
+            add_budget(d.ptr("seed%d_type" % j), d.ptr("seed%d_step" % j), d.ptr("seed%d_ids" % j),
+                       d.ptr("seed%d_tms" % j), M, d.ptr("seed%d_n" % j))
+        step = np.asarray([len(s) for s in members], dtype=np.int64)   # a member's next step number
+        overflow = False
+        for _layer in range(depth):                       # data.py:146-170
+            # the per-layer read-back: every member's list(budget.keys()), and the flags
+            h = meta[o_ts:o_hit].cpu().numpy()
+            if h[o_fl - o_ts:].view(np.int32)[3]:
+                overflow = True
+                break
+            ts = h[:2 * B * T].reshape(B, 2 * T)
+            orders = [sorted((t for t in range(T) if ts[b, 2 * t + 1] >= 0), key=lambda t: ts[b, 2 * t + 1])
+                      for b in range(B)]
+            K = max(len(o) for o in orders)
+            if K == 0:
+                continue
+            # step k of the layer: member b selects its k-th budget type (or sits out), then adds its budget
+            typ = np.full((K, B), -1, dtype=np.int32)
+            for b, o in enumerate(orders):
+                typ[:len(o), b] = o
+            rng = np.where(typ >= 0, rooms[np.arange(B)[None, :], np.maximum(typ, 0)], 0)   # what each member sorts
+            off = np.zeros((K, B + 1), dtype=np.int64)
+            np.cumsum(rng, axis=1, out=off[:, 1:])
+            up = _Upload()
+            up.add("type", typ, np.int32)
+            up.add("step", step[None, :] + np.arange(K)[:, None])
+            up.add("off", off)
+            d = up.to(dev)
+            type0, step0, off0 = d.ptr("type"), d.ptr("step"), d.ptr("off")
+            for k in range(K):
+                type_p, step_p = type0 + 4 * k * B, step0 + 8 * k * B
+                _lib.call(api + "select", _c.byref(cst), type_p, step_p, off0 + 8 * k * (B + 1), int(off[k, B]),
+                          int(rng[k].max()), W, tgt_id_p, tgt_time_p, n_tgt_p, flags_p, ws_p, ws_n, st)
+                add_budget(type_p, step_p, tgt_id_p, tgt_time_p, W, n_tgt_p)
+            step += np.asarray([len(o) for o in orders], dtype=np.int64)
+        if overflow:
+            restarts = _grow_state_room(dg, restarts)
+            continue
+
+        # rebuild (data.py:181-209): count pass, then the one read-back of the batch
+        cnt_off = np.concatenate([[0], np.cumsum([cap[b, tt] for b in range(B) for tt, _, _ in dg.blocks])])
+        cnt_off = cnt_off.astype(np.int64)
+        n_count = int(cnt_off[-1])
+        max_rows = int(cap.max()) if cap.size else 0
+        rb_ws = _c.c_size_t()
+        _lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
+        rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
+        ex = torch.empty(n_count + 1, **i64)
+        # the mask table rides behind cnt_off in the same copy; the dense masked entry points take it right after
+        # n_blocks, the hashed ones always (NULL: no mask)
+        cnt_off_d = _plan._to_dev_async(cnt_off if min_ser is None else np.concatenate([cnt_off, min_ser]), dev)
+        masked = () if min_ser is None else (cnt_off_d.data_ptr() + 8 * cnt_off.shape[0],)
+        suffix = "" if min_ser is None else "_masked"
+        feat_rows_p = _lib.ptr(dg.feat_rows) if dg.features is not None else None
+        if host:
+            # single-read count pass: the kept edges' hit records (16 bytes each) stay in device scratch for the write
+            # pass
+            hit_cap = _hit_capacity(dg, n_count)
+            hits = torch.empty(16 * max(hit_cap, 1), dtype=torch.uint8, device=dev)
+            _lib.call(api + "rebuild_count_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
+                      masked[0] if masked else None, cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p,
+                      hits.data_ptr(), hit_cap, meta[o_hit:o_hit + 1].data_ptr(), ex.data_ptr(), totals.data_ptr(),
+                      flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
+        else:
+            mask_arg = (masked[0] if masked else None,) if hashed else masked
+            _lib.call(api + "rebuild_count" + ("" if hashed else suffix), _c.byref(cst), dg.blocks_dev.data_ptr(),
+                      NB, *mask_arg, cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, ex.data_ptr(),
+                      totals.data_ptr(), flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
+        h = meta.cpu().numpy()
+        fl = h[o_fl:o_hit].view(np.int32)
+        if fl[3]:
+            restarts = _grow_state_room(dg, restarts)
+            continue
+        break
+    dg.sampler_state = {"layout": layout, "entries": int(rooms.sum()), "restarts": restarts,
+                        "load": float((h[o_fill:].reshape(B, T) / np.maximum(rooms, 1)).max()) if hashed else None}
     nl = h[:B * T].reshape(B, T)
-    ts = h[B * T:3 * B * T].reshape(B, 2 * T)
-    tot = h[3 * B * T:3 * B * T + B * NB].reshape(B, NB)
-    fl = h[3 * B * T + B * NB:3 * B * T + B * NB + 2].view(np.int32)
+    ts = h[o_ts:o_tot].reshape(B, 2 * T)
+    tot = h[o_tot:o_fl].reshape(B, NB)
     if fl[0]:
         raise IndexError("a neighbour id lies outside its node type's id range in the device graph")
     if fl[1]:
@@ -999,10 +1113,10 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     edge_type = torch.empty(E, **i64)
     edge_time = torch.empty(E, **i64)
     if host:
-        n_hits = int(h[-1])
+        n_hits = int(h[o_hit])
         _grow_hit_room(dg, n_hits, n_count)
         fits = n_hits <= hit_cap                          # else the write pass re-reads the neighbour lists
-        _lib.call("hgt_gsample_batch_rebuild_write_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
+        _lib.call(api + "rebuild_write_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
                   masked[0] if masked else None, cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"),
                   d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
                   hits.data_ptr() if fits else None, n_hits if fits else 0,
@@ -1010,8 +1124,8 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
                   node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
                   edge_time.data_ptr(), st)
     else:
-        _lib.call("hgt_gsample_batch_rebuild_write" + suffix, _c.byref(cst), dg.blocks_dev.data_ptr(), NB, *masked,
-                  cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
+        _lib.call(api + "rebuild_write" + ("" if hashed else suffix), _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
+                  *mask_arg, cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
                   d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
                   _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
                   node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
