@@ -720,13 +720,21 @@ int64_t hgt_sampler_budget_update(const int64_t* h_ids, const int64_t* h_times, 
                                   uint8_t* h_in_budget, double* h_score, int64_t* h_budget_time, int64_t* h_stamp,
                                   int64_t* h_stamp_counter, int32_t* h_touched_layer);
 
+/* Bits of the `skip` word of hgt_sampler_block and hgt_gsample_block.  HGT_BLOCK_SKIP marks the 'self' relation
+ * (data.py:116), as the value 1 always has.  HGT_BLOCK_NARROW marks a block whose row_of / ptr / nbr / time arrays are
+ * int32 instead of int64 (the pointers keep their int64_t* type and are read as int32_t*); in its time array INT32_MIN
+ * stands for no_time (the reference's `None`).  A word of 0 or 1, which is all earlier callers pass, is the int64 layout.
+ * The flag rides in `skip` so that the structs keep their size: callers allocate arrays of them. */
+#define HGT_BLOCK_SKIP 1
+#define HGT_BLOCK_NARROW 2
+
 /* One <target type, source type, relation> adjacency of the frozen graph in CSR form (host arrays; rows in the
  * reference dict's insertion order) and the layer_data / budget of one node type as flat arrays over node ids. */
 typedef struct {
   const int64_t* row_of; int64_t n_row_of;   /* target id -> CSR row, -1 = no adjacency */
   const int64_t* ptr; const int64_t* nbr; const int64_t* time;
   int32_t src_state;                         /* index of the source type's hgt_sampler_state */
-  int32_t skip;                              /* 1 for the 'self' relation (data.py:116) */
+  int32_t skip;                              /* HGT_BLOCK_SKIP for the 'self' relation, | HGT_BLOCK_NARROW (see above) */
 } hgt_sampler_block;
 typedef struct {
   int64_t n;
@@ -757,7 +765,8 @@ typedef struct {
   const int64_t* ptr;                         /* [rows+1] positions into nbr / time */
   const int64_t* nbr; const int64_t* time;    /* neighbour ids and edge times in dict order (no_time = None) */
   int32_t tgt_type, src_type;                 /* type slots */
-  int32_t skip;                               /* 1 for the 'self' relation: never sampled from (data.py:116) */
+  int32_t skip;                               /* HGT_BLOCK_SKIP for the 'self' relation: never sampled from
+                                                 (data.py:116); | HGT_BLOCK_NARROW: the four arrays are int32 */
   int32_t rel;                                /* edge_type value in the to_torch layout (data.py:237-238) */
 } hgt_gsample_block;
 
@@ -1022,6 +1031,15 @@ int hgt_gsample_batch_rebuild_write_host(const hgt_gsample_batch_state* h_state,
                                          const float* const* feat, int32_t feat_dim, int64_t* node_type,
                                          int64_t* node_time, float* node_feature, int64_t* edge_index,
                                          int64_t* edge_type, int64_t* edge_time, void* stream);
+
+/* Feature rows from bf16 tables (sampler.py: DeviceGraph(..., feature_dtype=torch.bfloat16)), run after a rebuild write
+ * pass that was given feat = NULL: node_feature[i, :] = the widening to float of feat[row_type[i]][row_id[i], :] for the
+ * n_rows output rows.  feat is a DEVICE array of per-type pointers to [ids, feat_dim] bf16 tables (device memory or
+ * device-mapped host memory), row_type / row_id [n_rows] DEVICE arrays (a row's type slot and sampled id: the batch's
+ * node_type and the sampled ids in output order).  Reads 16 bytes at a time where a row is 16-byte aligned, element by
+ * element elsewhere.  Ids are not range-checked here: the rebuild count pass checks them against feat_rows. */
+int hgt_gsample_gather_features_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
+                                     const int64_t* row_id, int64_t n_rows, float* node_feature, void* stream);
 
 /* Disjoint union of B batches in the to_torch layout (sampler.py: merge_batches).  The member structs live in DEVICE
  * memory.  loc_off [B*(T+1)]: member b's first local row of each type (loc_off[b*(T+1)+T] = its node count); uoff [B*T]:

@@ -129,6 +129,8 @@ SIGNATURES = {
     # graphs in page-locked host memory (sampler.DeviceGraph(..., placement="host"))
     "hgt_host_register": [_p, _sz, _c.POINTER(_p)],
     "hgt_host_unregister": [_p],
+    # bf16 feature tables of the device sampler (DeviceGraph(..., feature_dtype=torch.bfloat16))
+    "hgt_gsample_gather_features_bf16": [_p, _i32, _p, _p, _i64, _p, _p],
     "hgt_gsample_batch_rebuild_count_host": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _sz,
                                              _p],
     "hgt_gsample_batch_rebuild_write_host": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p,

@@ -206,15 +206,38 @@ __device__ __forceinline__ int64_t rnd_below(curandStatePhilox4_32_10_t* s, int6
   return (int64_t)__umul64hi(rnd64(s), (uint64_t)m);
 }
 
+// ---- a block's arrays at either width ---------------------------------------------------------------------------------
+// Every kernel reads row_of / ptr / nbr / time through these.  A narrow block (skip & HGT_BLOCK_NARROW) holds them as
+// int32, with INT32_MIN for no_time.  A warp's segment or target row lies in one block, so the branch is warp-uniform.
+__device__ __forceinline__ bool blk_narrow(const hgt_gsample_block& b) { return b.skip & HGT_BLOCK_NARROW; }
+__device__ __forceinline__ int64_t blk_row(const hgt_gsample_block& b, int64_t tid) {
+  return blk_narrow(b) ? (int64_t)reinterpret_cast<const int32_t*>(b.row_of)[tid] : b.row_of[tid];
+}
+__device__ __forceinline__ int64_t blk_ptr(const hgt_gsample_block& b, int64_t row) {
+  return blk_narrow(b) ? (int64_t)reinterpret_cast<const int32_t*>(b.ptr)[row] : b.ptr[row];
+}
+__device__ __forceinline__ int64_t blk_nbr(const hgt_gsample_block& b, int64_t p) {
+  return blk_narrow(b) ? (int64_t)reinterpret_cast<const int32_t*>(b.nbr)[p] : b.nbr[p];
+}
+__device__ __forceinline__ int64_t blk_time(const hgt_gsample_block& b, int64_t p, int64_t no_time) {
+  if (!blk_narrow(b)) return b.time[p];
+  const int32_t t = reinterpret_cast<const int32_t*>(b.time)[p];
+  return t == INT32_MIN ? no_time : (int64_t)t;
+}
+// CSR row of target tid (-1: none); the neighbours of row are [blk_ptr(row), blk_ptr(row + 1)).
+__device__ __forceinline__ int64_t blk_row_of(const hgt_gsample_block& b, int64_t tid) {
+  return tid >= 0 && tid < b.n_row_of ? blk_row(b, tid) : -1;
+}
+
 __device__ __forceinline__ int64_t seg_size(const hgt_gsample_block& blk, int64_t tid, int64_t width, int64_t* a,
                                             int64_t* deg) {
   *a = 0;
   *deg = 0;
-  if (blk.skip || tid < 0 || tid >= blk.n_row_of) return 0;             // 'self' (data.py:116), or no adjacency
-  const int64_t row = blk.row_of[tid];
-  if (row < 0) return 0;
-  *a = blk.ptr[row];
-  *deg = blk.ptr[row + 1] - *a;
+  if (blk.skip & HGT_BLOCK_SKIP) return 0;                              // 'self' (data.py:116)
+  const int64_t row = blk_row_of(blk, tid);
+  if (row < 0) return 0;                                                // no adjacency
+  *a = blk_ptr(blk, row);
+  *deg = blk_ptr(blk, row + 1) - *a;
   return *deg < width ? *deg : width;                                   // data.py:119-122
 }
 
@@ -295,8 +318,8 @@ __global__ void k_candidates(St st, PerMember<uint64_t> seed, PerMember<int64_t>
   for (int64_t j = lane; j < n_s; j += 32) {
     const int64_t seq = off + j;
     const int64_t pos = a + (all ? j : S_[j]);
-    const int64_t sid = blk.nbr[pos];
-    int64_t tm = blk.time[pos];
+    const int64_t sid = blk_nbr(blk, pos);
+    int64_t tm = blk_time(blk, pos, no_time);
     if (tm == no_time) tm = target_time;                                // data.py:125-126
     cand_slot[seq] = -1;
     if (time_filter && tm > max_time) continue;                         // data.py:127, first operand of the `or`
@@ -578,13 +601,13 @@ __global__ void k_rb_count(St st, const hgt_gsample_block* blocks, int32_t n_blo
   int64_t c = 0;
   if (r < mb.n_layer[T]) {
     const int64_t tid = st.lid[mb.lid_off[T] + r];
-    const int64_t row = tid < blk.n_row_of ? blk.row_of[tid] : -1;
+    const int64_t row = blk_row_of(blk, tid);
     if (row >= 0) {
-      const int64_t a = blk.ptr[row], e = blk.ptr[row + 1];
+      const int64_t a = blk_ptr(blk, row), e = blk_ptr(blk, row + 1);
       const int64_t tt = node_ltime(st, mb, T, tid, r);
       const auto ix = type_ix(st, mb, S);
       for (int64_t p = a + lane; p < e; p += 32) {
-        const int64_t sid = blk.nbr[p];
+        const int64_t sid = blk_nbr(blk, p);
         if (sid < 0 || sid >= ix.n) { flags[0] = 1; continue; }
         const int32_t sser = ser_of(st, ix, sid);
         if (sser < 0 || masked_out(min_ser, b, r, sser)) continue;
@@ -628,13 +651,13 @@ __global__ void k_rb_write(St st, const hgt_gsample_block* blocks, int32_t n_blo
   const auto mb = member(st, m);
   if (blk_out[mbk] < 0 || r >= mb.n_layer[T]) return;
   const int64_t tid = st.lid[mb.lid_off[T] + r];
-  const int64_t row = tid < blk.n_row_of ? blk.row_of[tid] : -1;
+  const int64_t row = blk_row_of(blk, tid);
   if (row < 0) return;
   const int64_t* noff = node_off + (int64_t)m * st.num_types;
   const int64_t eb = mo.edge_base(m), n_edges = mo.edges(m);
   int64_t* ei = edge_index + 2 * eb;
   int64_t e = blk_out[mbk] + ex[cnt_off[mbk] + r] - ex[cnt_off[mbk]];
-  const int64_t a = blk.ptr[row], end = blk.ptr[row + 1];
+  const int64_t a = blk_ptr(blk, row), end = blk_ptr(blk, row + 1);
   const int64_t tt = node_ltime(st, mb, T, tid, r);
   const auto ix = type_ix(st, mb, S);
   const int64_t dst = noff[T] + r;
@@ -643,7 +666,7 @@ __global__ void k_rb_write(St st, const hgt_gsample_block* blocks, int32_t n_blo
     int32_t sser = -1;
     int64_t sid = -1;
     if (p < end) {
-      sid = blk.nbr[p];
+      sid = blk_nbr(blk, p);
       if (sid >= 0 && sid < ix.n) sser = ser_of(st, ix, sid);
     }
     const bool kept = sser >= 0 && !masked_out(min_ser, b, r, sser);
@@ -702,14 +725,67 @@ __global__ void k_rb_nodes(St st, const int64_t* node_off, const int64_t* type_o
 // feature copies leave the link idle.  The count pass below reads each list once and leaves one hit record per kept edge
 // in device scratch; the write pass lays the edges out from those records alone.
 
-constexpr int kListUnroll = 8;   // neighbour ids in flight per lane in the single-read count pass
+constexpr int kListUnroll = 8;   // neighbour ids in flight per lane in the single-read count pass (16 for int32 lists:
+                                 // the same 64 bytes per lane)
 constexpr int kRowUnroll = 4;    // 16-byte feature loads in flight per lane in the host gather
 
 // A kept edge: {m * n_blocks + b, target ser r, rank among r's kept edges in list order, source ser}.  Its output position
 // is blk_out + (ex[r] - ex[0]) + rank, so the records may sit in the scratch in any order.
 using Hit = int4;
 
-// k_rb_count's counts, flags and mask, plus the hit records: slots claimed with one atomic per warp and kListUnroll * 32
+// The list [a, e) of nbr (Id = the block's element type) in chunks of 32 * U ids, U loads in flight per lane: counts,
+// flags and hit records of k_rb_count_host.  Returns the number of kept edges.
+template <int U, typename Id, class St, class Ix>
+__device__ __forceinline__ int64_t count_list_host(const St& st, const Ix& ix, const Id* nbr, int64_t a, int64_t e,
+                                                   int64_t tt, const int64_t* min_ser, int b, int64_t r, int64_t mbk,
+                                                   Hit* hits, int64_t hit_cap, unsigned long long* n_hits,
+                                                   int32_t* flags) {
+  const int lane = threadIdx.x & 31;
+  const unsigned below = (1u << lane) - 1u;
+  int64_t c = 0;                                                        // kept edges so far (warp-uniform)
+  for (int64_t p0 = a; p0 < e; p0 += 32 * U) {
+    int64_t sid[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int64_t p = p0 + 32 * u + lane;
+      sid[u] = p < e ? (int64_t)nbr[p] : -1;
+    }
+    int32_t sser[U];
+    unsigned keep[U];
+    int n_kept = 0;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int64_t p = p0 + 32 * u + lane;
+      sser[u] = -1;
+      if (p < e) {
+        if (sid[u] < 0 || sid[u] >= ix.n) flags[0] = 1;
+        else sser[u] = ser_of(st, ix, sid[u]);
+      }
+      const bool kept = sser[u] >= 0 && !masked_out(min_ser, b, r, sser[u]);
+      if (kept) {
+        const int64_t dt = tt - src_ltime(st, ix, sid[u], sser[u]) + 120;
+        if (dt < 0 || dt >= HGT_RTE_MAX_LEN) flags[1] = 1;
+      }
+      keep[u] = __ballot_sync(kFull, kept);
+      n_kept += __popc(keep[u]);
+    }
+    if (n_kept == 0) continue;
+    unsigned long long base = 0;
+    if (lane == 0) base = atomicAdd(n_hits, (unsigned long long)n_kept);
+    base = __shfl_sync(kFull, base, 0);
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int k = __popc(keep[u] & below);
+      if ((keep[u] >> lane) & 1u && (int64_t)base + k < hit_cap)
+        hits[base + k] = make_int4((int)mbk, (int)r, (int)(c + k), sser[u]);
+      base += __popc(keep[u]);
+      c += __popc(keep[u]);
+    }
+  }
+  return c;
+}
+
+// k_rb_count's counts, flags and mask, plus the hit records: slots claimed with one atomic per warp and one chunk of
 // neighbours; records past hit_cap are dropped (n_hits still counts them, so the caller sees the overflow).
 template <class St>
 __global__ void k_rb_count_host(St st, const hgt_gsample_block* blocks, int32_t n_blocks,
@@ -723,54 +799,19 @@ __global__ void k_rb_count_host(St st, const hgt_gsample_block* blocks, int32_t 
   const int T = blk.tgt_type, S = blk.src_type;
   if (r >= cnt_off[mbk + 1] - cnt_off[mbk]) return;
   const auto mb = member(st, blockIdx.z);
-  int64_t c = 0;                                                        // kept edges so far (warp-uniform)
+  int64_t c = 0;
   if (r < mb.n_layer[T]) {
     const int64_t tid = st.lid[mb.lid_off[T] + r];
-    const int64_t row = tid < blk.n_row_of ? blk.row_of[tid] : -1;
+    const int64_t row = blk_row_of(blk, tid);
     if (row >= 0) {
-      const int64_t a = blk.ptr[row], e = blk.ptr[row + 1];
+      const int64_t a = blk_ptr(blk, row), e = blk_ptr(blk, row + 1);
       const int64_t tt = node_ltime(st, mb, T, tid, r);
       const auto ix = type_ix(st, mb, S);
-      const unsigned below = (1u << lane) - 1u;
-      for (int64_t p0 = a; p0 < e; p0 += 32 * kListUnroll) {
-        int64_t sid[kListUnroll];
-#pragma unroll
-        for (int u = 0; u < kListUnroll; ++u) {
-          const int64_t p = p0 + 32 * u + lane;
-          sid[u] = p < e ? blk.nbr[p] : -1;
-        }
-        int32_t sser[kListUnroll];
-        unsigned keep[kListUnroll];
-        int n_kept = 0;
-#pragma unroll
-        for (int u = 0; u < kListUnroll; ++u) {
-          const int64_t p = p0 + 32 * u + lane;
-          sser[u] = -1;
-          if (p < e) {
-            if (sid[u] < 0 || sid[u] >= ix.n) flags[0] = 1;
-            else sser[u] = ser_of(st, ix, sid[u]);
-          }
-          const bool kept = sser[u] >= 0 && !masked_out(min_ser, b, r, sser[u]);
-          if (kept) {
-            const int64_t dt = tt - src_ltime(st, ix, sid[u], sser[u]) + 120;
-            if (dt < 0 || dt >= HGT_RTE_MAX_LEN) flags[1] = 1;
-          }
-          keep[u] = __ballot_sync(kFull, kept);
-          n_kept += __popc(keep[u]);
-        }
-        if (n_kept == 0) continue;
-        unsigned long long base = 0;
-        if (lane == 0) base = atomicAdd(n_hits, (unsigned long long)n_kept);
-        base = __shfl_sync(kFull, base, 0);
-#pragma unroll
-        for (int u = 0; u < kListUnroll; ++u) {
-          const int k = __popc(keep[u] & below);
-          if ((keep[u] >> lane) & 1u && (int64_t)base + k < hit_cap)
-            hits[base + k] = make_int4((int)mbk, (int)r, (int)(c + k), sser[u]);
-          base += __popc(keep[u]);
-          c += __popc(keep[u]);
-        }
-      }
+      if (blk_narrow(blk))
+        c = count_list_host<2 * kListUnroll>(st, ix, reinterpret_cast<const int32_t*>(blk.nbr), a, e, tt, min_ser, b,
+                                             r, mbk, hits, hit_cap, n_hits, flags);
+      else
+        c = count_list_host<kListUnroll>(st, ix, blk.nbr, a, e, tt, min_ser, b, r, mbk, hits, hit_cap, n_hits, flags);
     }
   }
   if (lane == 0) cnt[cnt_off[mbk] + r] = c;
@@ -858,6 +899,52 @@ __global__ void k_rb_nodes_host(St st, const int64_t* node_off, const int64_t* t
         if (c0 + 32 * u + lane < feat_dim) dst[c0 + 32 * u + lane] = v[u];
     }
   }
+}
+
+// ---- bf16 feature tables (sampler.py: DeviceGraph(..., feature_dtype=torch.bfloat16)) --------------------------------
+// The widening is exact: a bf16 value is the high half of the float's bits.
+__device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+
+// One warp per output row i: node_feature[i] = widen(feat[row_type[i]][row_id[i]]).  Elements before the row's first
+// 16-byte boundary and after its last are copied one by one; between them each lane keeps kRowUnroll 16-byte loads (8
+// values each) in flight, so a table in host memory is read in whole 16-byte requests at any width.
+__global__ void k_gather_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
+                              const int64_t* row_id, int64_t n_rows, float* node_feature) {
+  const int lane = threadIdx.x & 31;
+  const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  if (i >= n_rows) return;
+  const uint16_t* src = feat[row_type[i]] + row_id[i] * (int64_t)feat_dim;
+  float* dst = node_feature + i * (int64_t)feat_dim;
+  int head = (int)((((uintptr_t)0 - (uintptr_t)src) & 15) >> 1);
+  if (head > feat_dim) head = feat_dim;
+  const int n8 = (feat_dim - head) >> 3;
+  for (int c = lane; c < head; c += 32) dst[c] = bf16_lo(src[c]);
+  const uint4* s8 = reinterpret_cast<const uint4*>(src + head);
+  float* d8 = dst + head;
+  const bool vec_store = ((uintptr_t)d8 & 15) == 0;
+  for (int c0 = 0; c0 < n8; c0 += 32 * kRowUnroll) {
+    uint4 v[kRowUnroll];
+#pragma unroll
+    for (int u = 0; u < kRowUnroll; ++u)
+      if (c0 + 32 * u + lane < n8) v[u] = s8[c0 + 32 * u + lane];
+#pragma unroll
+    for (int u = 0; u < kRowUnroll; ++u) {
+      const int c = c0 + 32 * u + lane;
+      if (c >= n8) continue;
+      const float4 a = make_float4(bf16_lo(v[u].x), bf16_hi(v[u].x), bf16_lo(v[u].y), bf16_hi(v[u].y));
+      const float4 b = make_float4(bf16_lo(v[u].z), bf16_hi(v[u].z), bf16_lo(v[u].w), bf16_hi(v[u].w));
+      float* d = d8 + 8 * (int64_t)c;
+      if (vec_store) {
+        reinterpret_cast<float4*>(d)[0] = a;
+        reinterpret_cast<float4*>(d)[1] = b;
+      } else {
+        d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w;
+        d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
+      }
+    }
+  }
+  for (int c = head + 8 * n8 + lane; c < feat_dim; c += 32) dst[c] = bf16_lo(src[c]);
 }
 
 struct BudgetScratch {
@@ -1474,4 +1561,19 @@ extern "C" int hgt_gsample_hash_rebuild_write_host(
                        self_rel, {mem_out, 0}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
                        node_time, node_feature, edge_index, edge_type, edge_time, stream,
                        "hgt_gsample_hash_rebuild_write_host");
+}
+
+// ---- bf16 feature tables ------------------------------------------------------------------------------------------------
+
+extern "C" int hgt_gsample_gather_features_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
+                                                const int64_t* row_id, int64_t n_rows, float* node_feature,
+                                                void* stream) {
+  HGT_REQUIRE(feat_dim >= 0 && n_rows >= 0 &&
+                  (n_rows == 0 || feat_dim == 0 || (feat && row_type && row_id && node_feature)),
+              "hgt_gsample_gather_features_bf16: bad arguments");
+  if (n_rows == 0 || feat_dim == 0) return 0;
+  k_gather_bf16<<<(unsigned)blocks_for(n_rows, kWarps), kThreads, 0, (cudaStream_t)stream>>>(feat, feat_dim, row_type,
+                                                                                           row_id, n_rows, node_feature);
+  HGT_LAUNCH_CHECK();
+  return 0;
 }

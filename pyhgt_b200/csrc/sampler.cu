@@ -36,6 +36,23 @@ extern "C" int64_t hgt_sampler_budget_update(const int64_t* ids, const int64_t* 
   return kept;
 }
 
+namespace {
+// A block's arrays at either width: int64, or int32 with INT32_MIN for no_time (skip & HGT_BLOCK_NARROW).
+struct Arrays {
+  const hgt_sampler_block& b;
+  bool narrow() const { return b.skip & HGT_BLOCK_NARROW; }
+  int64_t get(const int64_t* a, int64_t i) const { return narrow() ? (int64_t)((const int32_t*)a)[i] : a[i]; }
+  int64_t row_of(int64_t tid) const { return get(b.row_of, tid); }
+  int64_t ptr(int64_t row) const { return get(b.ptr, row); }
+  int64_t nbr(int64_t j) const { return get(b.nbr, j); }
+  int64_t time(int64_t j, int64_t no_time) const {
+    if (!narrow()) return b.time[j];
+    const int32_t t = ((const int32_t*)b.time)[j];
+    return t == INT32_MIN ? no_time : (int64_t)t;
+  }
+};
+}  // namespace
+
 // The whole `add_budget` (data.py:108-130) for a BATCH of target nodes of one type: every <source type, relation> block of
 // the target type, in the reference's dict order, target after target — one call per sampling layer and type instead of
 // one Python iteration per target and block.  The uniform draws (`np.random.choice(..., replace=False)`, data.py:122) do
@@ -53,10 +70,11 @@ extern "C" int64_t hgt_sampler_add_budget(const int64_t* target_ids, const int64
     const int64_t tid = target_ids[t], target_time = target_times[t];
     for (int32_t b = 0; b < n_blocks; ++b) {
       const hgt_sampler_block& blk = blocks[b];
-      if (blk.skip || tid < 0 || tid >= blk.n_row_of) continue;             // 'self', or target_id not in the block
-      const int64_t row = blk.row_of[tid];
+      if ((blk.skip & HGT_BLOCK_SKIP) || tid < 0 || tid >= blk.n_row_of) continue;   // 'self', or target_id not in it
+      const Arrays ar{blk};
+      const int64_t row = ar.row_of(tid);
       if (row < 0) continue;
-      const int64_t a = blk.ptr[row], n_adl = blk.ptr[row + 1] - a;
+      const int64_t a = ar.ptr(row), n_adl = ar.ptr(row + 1) - a;
       if (n_adl == 0) continue;
       if (blk.src_state < 0 || blk.src_state >= n_states) return -2;
       hgt_sampler_state& st = states[blk.src_state];
@@ -67,10 +85,11 @@ extern "C" int64_t hgt_sampler_add_budget(const int64_t* target_ids, const int64
       const double w = 1.0 / (double)n_s;                                   // 1. / len(sampled_ids), data.py:129
       for (int64_t i = 0; i < n_s; ++i) {
         const int64_t j = a + (all ? i : draw_pos[off + i]);
-        const int64_t tm = blk.time[j] == no_time ? target_time : blk.time[j];
+        const int64_t tj = ar.time(j, no_time);
+        const int64_t tm = tj == no_time ? target_time : tj;
         if (tm > max_time) continue;                                        // data.py:127, first operand of the `or`
         if (st.layer_seq < 0) st.layer_seq = counters[1]++;                 // layer_data[source_type] springs into being
-        const int64_t sid = blk.nbr[j];
+        const int64_t sid = ar.nbr(j);
         if (sid < 0 || sid >= st.n) return -2;
         if (st.in_layer[sid]) continue;                                     // second operand
         if (st.budget_seq < 0) st.budget_seq = counters[2]++;

@@ -30,6 +30,11 @@ from itertools import chain as _chain
 import numpy as np
 
 _NO_TIME = np.iinfo(np.int64).min          # stands for `None` in the neighbour-time arrays (data.py:125-126)
+_NO_TIME32 = np.iinfo(np.int32).min        # the same in a narrow block's int32 time array
+# A block is narrow (int32 arrays, half the bytes) when its entry and row counts, its neighbour and target ids fit
+# [-_NARROW_MAX - 1, _NARROW_MAX] and its non-None times [-_NARROW_MAX, _NARROW_MAX]; otherwise it keeps int64 arrays.
+_NARROW_MAX = 2 ** 31 - 1
+_BLOCK_SKIP, _BLOCK_NARROW = 1, 2          # bits of the blocks' `skip` word (HGT_BLOCK_SKIP / HGT_BLOCK_NARROW)
 
 
 class _CBlock(_c.Structure):                 # hgt_sampler_block (include/hgt_b200.h)
@@ -44,8 +49,10 @@ class _CState(_c.Structure):                 # hgt_sampler_state
 
 
 class _Block:
-    """One <target type, source type, relation> adjacency in CSR form, dict insertion order preserved."""
-    __slots__ = ("row_of", "ptr", "nbr", "time", "has_none", "nbr_addr", "time_addr", "ptr_list", "row_list")
+    """One <target type, source type, relation> adjacency in CSR form, dict insertion order preserved.  ``row_of`` /
+    ``ptr`` / ``nbr`` / ``time`` are int32 when the block is ``narrow`` (see _NARROW_MAX; a None time is then _NO_TIME32)
+    and int64 otherwise (None = _NO_TIME); ``span`` reads a neighbour list at either width."""
+    __slots__ = ("row_of", "ptr", "nbr", "time", "has_none", "narrow", "nbr_addr", "time_addr", "ptr_list", "row_list")
 
     def __init__(self, tesr, n_target_ids):
         adls = list(tesr.values())
@@ -66,10 +73,36 @@ class _Block:
             self.time = np.fromiter((_NO_TIME if v is None else v for adl in adls for v in adl.values()),
                                     dtype=np.int64, count=total)
         self.has_none = has_none
+        self.narrow = self._fits_narrow(n_keys, total, tesr)
+        if self.narrow:
+            self.row_of, self.ptr, self.nbr = (a.astype(np.int32) for a in (self.row_of, self.ptr, self.nbr))
+            t32 = self.time.astype(np.int32)
+            if has_none:
+                t32[self.time == _NO_TIME] = _NO_TIME32
+            self.time = t32
         self.nbr_addr = self.nbr.ctypes.data               # base addresses for the native budget update
         self.time_addr = self.time.ctypes.data
         self.ptr_list = self.ptr.tolist()                  # plain ints: the per-node lookups stay out of numpy
         self.row_list = self.row_of.tolist()
+
+    def _fits_narrow(self, n_keys, total, tesr):
+        lo, hi = -_NARROW_MAX - 1, _NARROW_MAX
+        if total > hi or n_keys > hi:
+            return False
+        if total and (int(self.nbr.min()) < lo or int(self.nbr.max()) > hi):
+            return False
+        if n_keys and (min(tesr) < lo or max(tesr) > hi):
+            return False
+        tm = self.time[self.time != _NO_TIME] if self.has_none else self.time
+        return not tm.size or (int(tm.min()) >= -hi and int(tm.max()) <= hi)
+
+    def span(self, a, b):
+        """nbr[a:b] and time[a:b] as int64, None times as _NO_TIME, at either width."""
+        nbr, tm = self.nbr[a:b], self.time[a:b]
+        if self.narrow:
+            nbr = nbr.astype(np.int64)
+            tm = np.where(tm == _NO_TIME32, _NO_TIME, tm.astype(np.int64))
+        return nbr, tm
 
     def row(self, target_id):
         if target_id < 0 or target_id >= len(self.row_list):
@@ -122,7 +155,7 @@ class FrozenGraph:
             for i, (si, blk, skip) in enumerate(lst):
                 arr[i].row_of, arr[i].n_row_of = blk.row_of.ctypes.data, blk.row_of.shape[0]
                 arr[i].ptr, arr[i].nbr, arr[i].time = blk.ptr.ctypes.data, blk.nbr_addr, blk.time_addr
-                arr[i].src_state, arr[i].skip = si, skip
+                arr[i].src_state, arr[i].skip = si, skip | (_BLOCK_NARROW if blk.narrow else 0)
             ent = self._cblocks[target_type] = (arr, lst)
         return ent
 
@@ -375,13 +408,18 @@ def _sample_slices(fg, time_range, sampled_depth, sampled_number, inp, feature_e
                 ids = tms = None
                 if n_adl < sampled_number:                # data.py:119-122: take the whole adjacency
                     n_s = n_adl
-                    ids_addr, tms_addr = blk.nbr_addr + 8 * a, blk.time_addr + 8 * a
+                    if blk.narrow:                        # the native update reads int64 lists
+                        ids, tms = blk.span(a, b)
+                        ids_addr, tms_addr = ids.ctypes.data, tms.ctypes.data
+                    else:
+                        ids_addr, tms_addr = blk.nbr_addr + 8 * a, blk.time_addr + 8 * a
                 else:
                     # == np.random.choice(list(adl.keys()), sampled_number, replace=False): RandomState.choice draws
                     # permutation(len(a))[:size] whether `a` is the population or its size, so the stream is the same
                     pos = np.random.choice(n_adl, sampled_number, replace=False)
-                    ids = np.ascontiguousarray(blk.nbr[a:b][pos])
-                    tms = np.ascontiguousarray(blk.time[a:b][pos])
+                    nbr, tm = blk.span(a, b)
+                    ids = np.ascontiguousarray(nbr[pos])
+                    tms = np.ascontiguousarray(tm[pos])
                     n_s = ids.shape[0]
                     ids_addr, tms_addr = ids.ctypes.data, tms.ctypes.data
                 if upd is not None:
@@ -399,7 +437,7 @@ def _sample_slices(fg, time_range, sampled_depth, sampled_number, inp, feature_e
                         continue
                 # numpy path: library not built, or an id past the arrays (grow them and redo this slice)
                 if ids is None:
-                    ids, tms = blk.nbr[a:b], blk.time[a:b]
+                    ids, tms = blk.span(a, b)
                 if blk.has_none:
                     tms = np.where(tms == _NO_TIME, target_time, tms)
                 late = tms > max_time                     # data.py:127 (short-circuit `or`: layer_data[source_type] is
@@ -612,15 +650,24 @@ class DeviceGraph:
     hashed state's current region size estimate (grown by calls that overflowed it), ``sampler_state`` describes the
     last call's state.
 
+    The blocks are read in the FrozenGraph's own format: int32 arrays for a narrow block (``_Block``), int64 otherwise.
+    ``feature_dtype=torch.bfloat16`` stores the tables as bf16, rounded once from float32 (nearest even) on the way in:
+    half the bytes, and the batch's ``node_feature`` is still float32, each value the exact widening of the stored one.
+    ``graph_bytes`` reports the bytes the graph's arrays hold.
+
     Node types are laid out in ``graph.get_types()`` order (as ``to_torch`` does), so every type of the graph's
     ``edge_list`` must be one of them; relation names come from ``graph.get_meta_graph()`` plus ``'self'``."""
 
     PLACEMENTS = ("device", "host")
 
-    def __init__(self, frozen_graph, device, features=None, placement="device"):
+    def __init__(self, frozen_graph, device, features=None, placement="device", feature_dtype=None):
         if placement not in self.PLACEMENTS:
             raise ValueError("placement must be one of %s, got %r" % (self.PLACEMENTS, placement))
         import torch
+        feature_dtype = torch.float32 if feature_dtype is None else feature_dtype
+        if feature_dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError("feature_dtype must be torch.float32 or torch.bfloat16, got %r" % (feature_dtype,))
+        self.feature_dtype = feature_dtype
         fg = frozen_graph if isinstance(frozen_graph, FrozenGraph) else FrozenGraph(frozen_graph)
         self.fg, self.device = fg, torch.device(device)
         if self.device.type != "cuda":
@@ -647,10 +694,12 @@ class DeviceGraph:
         self._keep = []
         pinned = []                                       # page-aligned buffers registered with CUDA
 
-        def place(a, dtype=np.int64):
-            """Address the kernels read array ``a`` at; the array (device tensor or pinned host view) is kept."""
+        def place(a, dtype=None):
+            """Address the kernels read array ``a`` (as ``dtype``, default its own) at; the array (device tensor or pinned
+            host view) is kept."""
+            dtype = a.dtype if dtype is None else dtype
             if not host:
-                self._keep.append(up(a))
+                self._keep.append(torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(dev))
                 return self._keep[-1].data_ptr()
             view, dptr, buf = _pin(a, dtype)
             pinned.append(buf)
@@ -666,6 +715,7 @@ class DeviceGraph:
         import torch
         dev = self.device
         self.blocks = []                                  # (target slot, source slot, relation, skip) in dict order
+        self._adjacency = []                              # the block arrays the kernels read (for graph_bytes)
         cblocks = []
         if self.placement == "host":
             fg._cblocks = {}        # the host sampler's cached block tables hold the addresses of arrays rebound below
@@ -675,11 +725,13 @@ class DeviceGraph:
                     if r not in self.edge_dict:
                         raise KeyError("relation %r of edge_list is not in graph.get_meta_graph()" % (r,))
                     ptrs = [place(blk.row_of), place(blk.ptr), place(blk.nbr), place(blk.time)]
+                    self._adjacency.extend(self._keep[-4:])
                     if self.placement == "host":           # the FrozenGraph reads the pinned copies: one copy each
                         blk.row_of, blk.ptr, blk.nbr, blk.time = self._keep[-4:]
                         blk.nbr_addr, blk.time_addr = blk.nbr.ctypes.data, blk.time.ctypes.data
+                    flags = (_BLOCK_SKIP if r == 'self' else 0) | (_BLOCK_NARROW if blk.narrow else 0)
                     cb = _GBlock(ptrs[0], blk.row_of.shape[0], ptrs[1], ptrs[2], ptrs[3], self.slot[t_t],
-                                 self.slot[s_t], 1 if r == 'self' else 0, self.edge_dict[r])
+                                 self.slot[s_t], flags, self.edge_dict[r])
                     self.blocks.append((self.slot[t_t], self.slot[s_t], r))
                     cblocks.append(cb)
         self.n_blocks = len(cblocks)
@@ -699,16 +751,23 @@ class DeviceGraph:
             if len(dims) != 1:
                 raise ValueError("feature tables must all have the same width, got %s" % sorted(dims))
             self.feat_dim = dims.pop()
+            bf16 = self.feature_dtype == torch.bfloat16
             tabs, ptrs, rows = {}, [], []
             for t in self.types:
                 v = features.get(t)
                 p = 0
                 if v is not None and self.placement == "host":
-                    p = place(v.detach().to(device="cpu", dtype=torch.float32).contiguous().numpy(), np.float32)
-                    v = torch.from_numpy(self._keep[-1])
+                    v = v.detach().to(device="cpu", dtype=torch.float32)
+                    if bf16:                               # numpy has no bf16: pinned as its 16-bit patterns
+                        p = place(v.to(torch.bfloat16).contiguous().view(torch.int16).numpy())
+                        v = torch.from_numpy(self._keep[-1]).view(torch.bfloat16)
+                    else:
+                        p = place(v.contiguous().numpy(), np.float32)
+                        v = torch.from_numpy(self._keep[-1])
                     tabs[t] = v
                 elif v is not None:
-                    v = v.to(device=dev, dtype=torch.float32).contiguous()
+                    v = v.to(device=dev, dtype=torch.float32)
+                    v = (v.to(torch.bfloat16) if bf16 else v).contiguous()
                     tabs[t] = v
                     p = v.data_ptr()
                 ptrs.append(p)
@@ -721,6 +780,16 @@ class DeviceGraph:
         import torch
         raw = b"".join(bytes(s) for s in structs) or b"\0"
         return torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.device)
+
+    @property
+    def graph_bytes(self):
+        """Bytes held by the arrays that grow with the graph, where ``placement`` says: ``adjacency`` (every block's
+        row_of, ptr, nbr and time: 4 bytes per element in a narrow block, 8 otherwise) and ``features`` (the tables, at
+        ``feature_dtype``)."""
+        def nbytes(a):
+            return a.nbytes if isinstance(a, np.ndarray) else a.numel() * a.element_size()
+        feats = sum(nbytes(v) for v in self.features.values()) if self.features is not None else 0
+        return {"adjacency": sum(nbytes(a) for a in self._adjacency), "features": feats, "placement": self.placement}
 
 
 def _device_seeds(dg, inp):
@@ -1109,6 +1178,9 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     node_type = torch.empty(N, **i64)
     node_time = torch.empty(N, **i64)
     node_feature = torch.empty((N, dg.feat_dim), dtype=torch.float32, device=dev) if dg.features is not None else None
+    # bf16 tables: the write pass leaves the features out, and hgt_gsample_gather_features_bf16 widens the rows after it
+    bf16 = node_feature is not None and dg.feature_dtype == torch.bfloat16
+    fp32_feature = None if bf16 else node_feature
     edge_index = torch.empty(2 * E, **i64)                # member b's [2, E_b] block at 2 * edge_base[b]
     edge_type = torch.empty(E, **i64)
     edge_time = torch.empty(E, **i64)
@@ -1120,16 +1192,22 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
                   masked[0] if masked else None, cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"),
                   d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
                   hits.data_ptr() if fits else None, n_hits if fits else 0,
-                  _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
-                  node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
+                  _lib.ptr(dg.feat_ptrs) if fp32_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
+                  node_time.data_ptr(), _lib.ptr(fp32_feature), edge_index.data_ptr(), edge_type.data_ptr(),
                   edge_time.data_ptr(), st)
     else:
         _lib.call(api + "rebuild_write" + ("" if hashed else suffix), _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
                   *mask_arg, cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
                   d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
-                  _lib.ptr(dg.feat_ptrs) if node_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
-                  node_time.data_ptr(), _lib.ptr(node_feature), edge_index.data_ptr(), edge_type.data_ptr(),
+                  _lib.ptr(dg.feat_ptrs) if fp32_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
+                  node_time.data_ptr(), _lib.ptr(fp32_feature), edge_index.data_ptr(), edge_type.data_ptr(),
                   edge_time.data_ptr(), st)
+    if bf16 and N:
+        # output rows are member after member, type slot after type slot, ser order: the sampled ids in that order
+        row_id = torch.cat([lid[int(lid_off[b, t]):int(lid_off[b, t] + nl[b, t])]
+                            for b in range(B) for t in range(T) if nl[b, t]])
+        _lib.call("hgt_gsample_gather_features_bf16", _lib.ptr(dg.feat_ptrs), dg.feat_dim, node_type.data_ptr(),
+                  row_id.data_ptr(), N, node_feature.data_ptr(), st)
 
     out = []
     for b in range(B):

@@ -49,11 +49,13 @@ def spread(fg, stride):
         for s_t, rels in tes.items():
             out.blocks[t_t][s_t] = {}
             for r, blk in rels.items():
-                nb = copy.copy(blk)
+                nb = copy.copy(blk)                  # int64 arrays whatever blk's width: spread ids may not fit int32
+                nbr, tm = blk.span(0, blk.nbr.shape[0])
+                nb.narrow, nb.ptr, nb.time = False, blk.ptr.astype(np.int64), tm
                 nb.row_of = np.full(out.n_ids[t_t], -1, dtype=np.int64)
                 nb.row_of[np.arange(blk.row_of.shape[0]) * stride] = blk.row_of
-                nb.nbr = np.ascontiguousarray(blk.nbr * stride)
-                nb.nbr_addr = nb.nbr.ctypes.data
+                nb.nbr = np.ascontiguousarray(nbr * stride)
+                nb.nbr_addr, nb.time_addr = nb.nbr.ctypes.data, nb.time.ctypes.data
                 out.blocks[t_t][s_t][r] = nb
     return out
 

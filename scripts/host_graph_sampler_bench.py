@@ -50,9 +50,10 @@ def read_bytes(dg, out, width, feat_dim):
                 rows = blk.row_of[inside]
                 rows = rows[rows >= 0]
                 deg = blk.ptr[rows + 1] - blk.ptr[rows]
-                rebuild += 8 * inside.size + 16 * rows.size + 8 * int(deg.sum())
+                w = blk.nbr.itemsize                  # 8, or 4 for a narrow block
+                rebuild += w * inside.size + 2 * w * rows.size + w * int(deg.sum())
                 if r != "self":
-                    budget += 2 * (8 * inside.size + 16 * rows.size) + 16 * int(np.minimum(deg, width).sum())
+                    budget += 2 * (w * inside.size + 2 * w * rows.size) + 2 * w * int(np.minimum(deg, width).sum())
     feats = 4 * feat_dim * int(out[1].numel())
     return {"add_budget": budget, "rebuild": rebuild, "features": feats, "total": budget + rebuild + feats}
 
