@@ -506,7 +506,8 @@ int hgt_edge_backward_rows_att_bf16(const float* q, const float* dagg, const flo
  * fp32 (split here; the dout split pass also yields db) or already split by their producers (dout_hi/lo in dout's
  * layout; a_hi/a_lo [rows, K] as left by hgt_act_split in the forward) — with a pre-split dout, db is NOT computed.
  * impl 1 = fp32 SIMT kernels (any shape; also chosen automatically for cb_width % 8, K % 16, K < 64, overlapping groups
- * such as the RTE tables, or tiny problems).  h_cblocks: HOST copy of the column-block table.  The call enqueues only
+ * such as the RTE tables, or tiny problems).  h_cblocks: HOST copy of the column-block table.  Any number of groups is
+ * accepted: the choice of path is made once over the whole table.  The call enqueues only
  * device work (the host-built tables travel in kernel parameters), so it can be captured in a CUDA graph. */
 int hgt_typed_linear_bwd_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
                                          int32_t K, int32_t cb_width, int64_t lda, int64_t dout_elems,

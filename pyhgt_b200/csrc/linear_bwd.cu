@@ -37,8 +37,6 @@ namespace {
 
 using namespace tcp;
 
-constexpr int kMaxGroups = 64;
-
 // Tensor maps are read from global memory (written by k_upload earlier on the stream): acquire them for the TMA proxy.
 __device__ __forceinline__ void map_acquire(const CUtensorMap* m) {
   asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(m) : "memory");
@@ -216,12 +214,12 @@ struct DxJob {
   int map_wt;
   const GcTask* tasks;
   const int32_t* group_task0;
+  const int64_t* first_tile;   // [n_groups + 1] first dA tile of every group (in the workspace: any number of groups)
   const hgt_lin_group* groups;
   int n_groups, K_in, width, n_tiles_n, tile_n;
   float* dA;
   int accumulate;
   const float* gelu_aux;
-  int32_t first_tile[kMaxGroups + 1];
 
   struct Tile {
     int m0, n0, task0, kb_per_c, n_cblocks;
@@ -232,7 +230,7 @@ struct DxJob {
     int g = 0;
     while (g + 1 < n_groups && tile >= first_tile[g + 1]) ++g;
     const hgt_lin_group grp = groups[g];
-    const int local = tile - first_tile[g];
+    const int local = (int)(tile - first_tile[g]);
     const int mt = local / n_tiles_n, nt = local - mt * n_tiles_n;
     t.m0 = mt * BM;
     t.n0 = nt * tile_n;
@@ -466,7 +464,8 @@ __global__ void k_lin_dx_simt_det(const float* __restrict__ dout, const float* _
 }
 
 // dW[w_row + n, k] += sum_m dOut_c[m, n] * A[a_row0 + m, k];  db[w_row + n] += sum_m dOut_c[m, n].
-// One CTA = one task x (32 n) x (32 k) x a chunk of rows; 256 threads, 4 outputs each.
+// One CTA = one task x (32 n) x (32 k) x a chunk of rows; 256 threads, 4 outputs each.  dW == NULL (db only): one k tile,
+// A (which may then be NULL) is not read.
 constexpr int DW_SIMT_ROWS = 2048;
 // DET: partial tiles / bias sums go to the unit's slot (unit / (n_tiles * k_tiles)) of dW = part [slot][width][K_in] and
 // db = db_part [slot][width]; chunks of chunk_rows rows.
@@ -496,7 +495,7 @@ __device__ __forceinline__ void lin_dw_simt(const float* __restrict__ dout, cons
       float dv = 0.f, av = 0.f;
       if (r < r1) {
         if (n0 + tx < width) dv = dout[tk.out_off + r * tk.ld + n0 + tx];
-        if (k0 + tx < K_in) av = A[(tk.a_row0 + r) * lda + k0 + tx];
+        if (dW && k0 + tx < K_in) av = A[(tk.a_row0 + r) * lda + k0 + tx];
       }
       sd[rr][tx] = dv;
       sa[rr][tx] = av;
@@ -516,7 +515,7 @@ __device__ __forceinline__ void lin_dw_simt(const float* __restrict__ dout, cons
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int n = n0 + ty + 8 * j;
-    if (n < width && k0 + tx < K_in) {
+    if (dW && n < width && k0 + tx < K_in) {
       if constexpr (DET) dW[((int64_t)(unit / (n_tiles * k_tiles)) * width + n) * K_in + k0 + tx] = acc[j];
       else atomicAdd(dW + ((int64_t)tk.w_row + n) * K_in + k0 + tx, acc[j]);
     }
@@ -747,7 +746,7 @@ int bwd_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, const h
                         int32_t cb_width, int64_t lda, int64_t dout_elems, int32_t have_dout_split, int32_t have_a_split,
                         int32_t impl, size_t* out_bytes, bool det) {
   HGT_REQUIRE(out_bytes && (n_groups == 0 || (h_groups && h_cblocks)), "hgt_typed_linear_bwd_workspace_bytes: NULL argument");
-  HGT_REQUIRE(n_groups >= 0 && n_groups <= kMaxGroups, "hgt_typed_linear_bwd: n_groups=%d exceeds %d", n_groups, kMaxGroups);
+  HGT_REQUIRE(n_groups >= 0, "hgt_typed_linear_bwd_workspace_bytes: n_groups=%d", n_groups);
   HGT_REQUIRE(impl >= 0 && impl <= 3, "hgt_typed_linear_bwd_workspace_bytes: unknown impl %d", impl);
   *out_bytes = bwd_layout(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dout_split != 0,
                           have_a_split != 0, impl, det).total;
@@ -761,7 +760,7 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
                      float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
                      int32_t impl, void* workspace, size_t workspace_bytes, void* stream_, bool det) {
   cudaStream_t st = (cudaStream_t)stream_;
-  HGT_REQUIRE(n_groups >= 0 && n_groups <= kMaxGroups, "hgt_typed_linear_bwd: n_groups=%d exceeds %d", n_groups, kMaxGroups);
+  HGT_REQUIRE(n_groups >= 0, "hgt_typed_linear_bwd: n_groups=%d", n_groups);
   HGT_REQUIRE(K > 0 && cb_width > 0 && W, "hgt_typed_linear_bwd: K=%d cb_width=%d", K, cb_width);
   if (n_groups == 0) return 0;
   HGT_REQUIRE(groups && h_groups && h_cblocks, "hgt_typed_linear_bwd: NULL group tables");
@@ -786,7 +785,7 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
   // ---- task table (one entry per group x column block) ----
   std::vector<GcTask> tasks(std::max(L.n_tasks, 1));
   std::vector<int32_t> gt0(n_groups + 1);
-  std::vector<int64_t> gfirst(n_groups + 1);
+  std::vector<int64_t> gfirst(n_groups + 1);   // per group: first dA element (SIMT) or first dA tile (tensor cores)
   int nt = 0;
   int64_t elems = 0;
   for (int g = 0; g < n_groups; ++g) {
@@ -862,8 +861,9 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
         HGT_LAUNCH_CHECK();
       }
     }
-    if (dW) {
-      const int n_tiles = (cb_width + 31) / 32, k_tiles = (K + 31) / 32;
+    // db comes out of the dW kernel here, so it runs for db alone too
+    if (dW || db) {
+      const int n_tiles = (cb_width + 31) / 32, k_tiles = dW ? (K + 31) / 32 : 1;
       const int64_t chunk_rows = det ? L.dw_chunk : DW_SIMT_ROWS;
       int64_t units = 0;
       for (int t = 0; t < nt; ++t) {
@@ -875,9 +875,9 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
       if ((rc = upload_tasks())) return rc;
       if (units > 0 && det) {
         k_lin_dw_simt_det<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles,
-                                                           chunk_rows, part, db ? db_part : nullptr);
+                                                           chunk_rows, dW ? part : nullptr, db ? db_part : nullptr);
         HGT_LAUNCH_CHECK();
-        if ((rc = reduce_rows(part, K, n_tiles * k_tiles, 0, dW))) return rc;
+        if (dW && (rc = reduce_rows(part, K, n_tiles * k_tiles, 0, dW))) return rc;
         if (db && (rc = reduce_rows(db_part, 1, n_tiles * k_tiles, 1, db))) return rc;
       } else if (units > 0) {
         k_lin_dw_simt<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles, dW, db);
@@ -930,6 +930,13 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
       HGT_REQUIRE(split_units < 2147483647ll, "hgt_typed_linear_bwd: too many units");
     }
   }
+  // the dX tiles of group g are [gfirst[g], gfirst[g + 1]); the prefix lives in the workspace, so a table may have any
+  // number of groups
+  const int dx_tile_n = pick_tile_n(K), dx_tiles_n = (K + dx_tile_n - 1) / dx_tile_n;
+  for (int g = 0; g < n_groups; ++g) {
+    gfirst[g + 1] = gfirst[g] + (h_groups[g].m + BM - 1) / BM * dx_tiles_n;
+    HGT_REQUIRE(gfirst[g + 1] < 2147483647ll, "hgt_typed_linear_bwd: too many tiles");
+  }
   if ((rc = upload_head(&maps))) return rc;
 
   // 2. dOut split (+ db) unless the producer already split it
@@ -970,21 +977,16 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
         pos = std::max(pos, p.second);
       }
     }
-    DxJob job;
-    job.tile_n = pick_tile_n(K);
-    job.n_tiles_n = (K + job.tile_n - 1) / job.tile_n;
-    int64_t total = 0;
-    for (int g = 0; g < n_groups; ++g) {
-      job.first_tile[g] = (int32_t)total;
-      total += (h_groups[g].m + BM - 1) / BM * job.n_tiles_n;
-      HGT_REQUIRE(total < 2147483647ll, "hgt_typed_linear_bwd: too many tiles");
-    }
-    job.first_tile[n_groups] = (int32_t)total;
+    const int64_t total = gfirst[n_groups];
     if (total > 0) {
+      DxJob job;
+      job.tile_n = dx_tile_n;
+      job.n_tiles_n = dx_tiles_n;
       job.maps = d_maps;
       job.map_wt = map_wt;
       job.tasks = d_tasks;
       job.group_task0 = d_gt0;
+      job.first_tile = d_gfirst;
       job.groups = groups;
       job.n_groups = n_groups;
       job.K_in = K;
