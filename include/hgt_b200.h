@@ -287,6 +287,16 @@ int hgt_typed_linear_presplit_bf16(const void* a_hi, const void* a_lo, const flo
                                    int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                                    int32_t n_groups, const hgt_lin_cblock* cblocks, void* out,
                                    void* workspace, size_t workspace_bytes, void* stream);
+/* hgt_typed_linear with a bf16 A (`A` bf16 [rows, K] at row stride lda elements; fp32 output): the same product as the
+ * fp32 call on A widened to float, bitwise, with the same impl values.  A bf16 value is exactly the hi half of the split
+ * and its lo half is zero, so the tensor cores run A*W_hi + A*W_lo (impl 0 / 2; A*W_hi at impl 3) with A read as the
+ * wgmma operand as it is: by TMA in place where K % 8 == 0, lda % 8 == 0 and A is 16-byte aligned, otherwise after a
+ * copy into zero-padded rows (stream-ordered memory of its own).  impl 1 (and shapes the tensor cores do not take) runs
+ * the SIMT kernel, which widens A as it loads it.  Workspace: hgt_typed_linear_workspace_bytes for the same arguments. */
+int hgt_typed_linear_bf16a(const void* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
+                           const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
+                           const hgt_lin_cblock* cblocks, float* out, int32_t impl, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* 24-bit gather tables (inference [K'|V'] and RTE tables).
  * Element: the fp32 bit pattern b rounded to nearest-even at bit 8 (b + 0x7F + ((b >> 8) & 1), low 8 bits cleared):
@@ -534,6 +544,20 @@ int hgt_typed_linear_bwd_det(const float* dout, const void* dout_hi, const void*
                              const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
                              float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
                              int32_t impl, void* workspace, size_t workspace_bytes, void* stream);
+
+/* dW and db of hgt_typed_linear_bf16a (no dA: a bf16 A takes no gradient), and the deterministic twin.  A is bf16
+ * [rows, K] at row stride lda; the other arguments are hgt_typed_linear_bwd's.  The tensor-core path (impl 2, 3, or 0
+ * where it would take the tensor cores; it needs lda == K) reads A as the dW product's operand as it is and runs
+ * dOut_hi*A + dOut_lo*A (dOut_hi*A at impl 3); the SIMT path widens A as it loads it.  dW and db are bitwise those of
+ * the fp32 call (same flag) on the widened A.  Workspace: the fp32 queries with have_a_split = 1. */
+int hgt_typed_linear_bwd_bf16a(const float* dout, int64_t dout_elems, const void* A, int64_t lda, int32_t K,
+                               int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                               int32_t n_groups, const hgt_lin_cblock* h_cblocks, float* dW, float* db, int32_t impl,
+                               void* workspace, size_t workspace_bytes, void* stream);
+int hgt_typed_linear_bwd_bf16a_det(const float* dout, int64_t dout_elems, const void* A, int64_t lda, int32_t K,
+                                   int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                   int32_t n_groups, const hgt_lin_cblock* h_cblocks, float* dW, float* db,
+                                   int32_t impl, void* workspace, size_t workspace_bytes, void* stream);
 
 /* act(in) as fp32 (out_f32 [rows, K], or NULL) and/or as the bf16 hi/lo operand split (hi/lo [rows, K], or NULL; needs
  * K % 8 == 0; hi without lo writes only the hi half, bitwise the same, the operand of a one-product GEMM).  act: 0 = identity, 1 = exact-erf gelu (conv.py:119).  The training forward keeps the split for the
@@ -1041,6 +1065,11 @@ int hgt_gsample_batch_rebuild_write_host(const hgt_gsample_batch_state* h_state,
  * element elsewhere.  Ids are not range-checked here: the rebuild count pass checks them against feat_rows. */
 int hgt_gsample_gather_features_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
                                      const int64_t* row_id, int64_t n_rows, float* node_feature, void* stream);
+/* The same rows kept in bf16 (sample_subgraph(s)_cuda(..., feature_dtype=torch.bfloat16)): node_feature is bf16
+ * [n_rows, feat_dim] and each row is copied as stored.  Loads as above; stores take 16 bytes where the output row is
+ * 16-byte aligned at that point, 4 or 2 bytes where it is not. */
+int hgt_gsample_gather_rows_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
+                                 const int64_t* row_id, int64_t n_rows, void* node_feature, void* stream);
 
 /* Disjoint union of B batches in the to_torch layout (sampler.py: merge_batches).  The member structs live in DEVICE
  * memory.  loc_off [B*(T+1)]: member b's first local row of each type (loc_off[b*(T+1)+T] = its node count); uoff [B*T]:
@@ -1059,6 +1088,11 @@ int hgt_merge_batches(const hgt_merge_member* members, int32_t n_members, int32_
                       const int64_t* uoff, int64_t max_rows, int64_t max_edges, int64_t n_edges, int32_t feat_dim,
                       int64_t* node_type, float* node_feature, int64_t* member_rows, int64_t* edge_index,
                       int64_t* edge_type, int64_t* edge_time, void* stream);
+/* The same union of bf16 feature rows: the members' node_feature pointers and node_feature are bf16 [*, feat_dim]. */
+int hgt_merge_batches_bf16(const hgt_merge_member* members, int32_t n_members, int32_t num_types, const int64_t* loc_off,
+                           const int64_t* uoff, int64_t max_rows, int64_t max_edges, int64_t n_edges, int32_t feat_dim,
+                           int64_t* node_type, void* node_feature, int64_t* member_rows, int64_t* edge_index,
+                           int64_t* edge_type, int64_t* edge_time, void* stream);
 
 #ifdef __cplusplus
 }

@@ -149,6 +149,12 @@ SIGNATURES = {
     "hgt_gsample_hash_rebuild_write_host": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i64, _p,
                                             _i32, _p, _p, _p, _p, _p, _p, _p],
     "hgt_merge_batches": [_p, _i32, _i32, _p, _p, _i64, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p],
+    # bf16 node features end to end (sample_subgraph(s)_cuda(..., feature_dtype=torch.bfloat16), GNN's adapter)
+    "hgt_gsample_gather_rows_bf16": [_p, _i32, _p, _p, _i64, _p, _p],
+    "hgt_merge_batches_bf16": [_p, _i32, _i32, _p, _p, _i64, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p],
+    "hgt_typed_linear_bf16a": [_p, _i64, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i32, _p, _sz, _p],
+    "hgt_typed_linear_bwd_bf16a": [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _i32, _p, _p, _p, _i32, _p, _sz, _p],
+    "hgt_typed_linear_bwd_bf16a_det": [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _i32, _p, _p, _p, _i32, _p, _sz, _p],
     # trimmed forward (GNN.forward(out_nodes=), trim.py)
     "hgt_trim_layout": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_trim_layout_bounded": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _i64, _p, _p, _p, _p, _p,

@@ -119,7 +119,11 @@ class _TypedLinear(torch.autograd.Function):
     into an fp32 Q buffer [q_elems] (q_table) and a bf16 table [out_elems - kv_off] (kv_table, offsets relative to kv_off,
     zero ranges relative to it too).  The forward then returns (stand-in, q, table): the stand-in is a zero-stride fp32
     tensor of out_elems that only carries the gradient, which arrives in the flat layout of the fp32 output, so the
-    backward is the same.  impl 3: one bf16 product on the tensor cores, only the hi half of act(A) is made and saved."""
+    backward is the same.  impl 3: one bf16 product on the tensor cores, only the hi half of act(A) is made and saved.
+
+    A bf16 `a` (the input adapter fed bf16 features; act 0, fp32 output, no gradient for a): the GEMM reads it as its
+    bf16 operand (hgt_typed_linear_bf16a) and it is saved as it is for dW (hgt_typed_linear_bwd_bf16a): no split, no lo
+    half, no fp32 copy.  Output, dW and db are bitwise those of the fp32 `a.float()`."""
 
     @staticmethod
     def forward(ctx, a, w_cat, b_cat, table, width, out_elems, impl, act, zero_ranges, tables16=None):
@@ -128,6 +132,18 @@ class _TypedLinear(torch.autograd.Function):
         K = a.shape[1]
         use_tc = impl in (0, 2, 3) and _tc_shape_ok(K, width)
         one = use_tc and impl == 3
+        ctx.bf16a = a.dtype == torch.bfloat16
+        if ctx.bf16a:
+            if act or tables16 is not None or a.requires_grad:
+                raise ValueError("a bf16 typed-linear input takes no activation, no bf16 tables and no gradient")
+            out = _linear_outputs(out_elems, zero_ranges, None, a.device)[0]
+            _linear_gemm_bf16a(a, w_cat, b_cat, table, width, (3 if one else 2) if use_tc else 1, out)
+            ctx.table, ctx.width, ctx.has_bias, ctx.act, ctx.use_tc = table, width, b_cat is not None, 0, use_tc
+            ctx.one = one
+            ctx.out_elems = out_elems
+            ctx.det = torch.are_deterministic_algorithms_enabled()
+            ctx.save_for_backward(a, w_cat)
+            return out
         out, q, kv = _linear_outputs(out_elems, zero_ranges, tables16, a.device)
         hi, lo, a_act = _split_operand(a, act, use_tc, one)
         _linear_gemms(hi, lo, a_act, w_cat, b_cat, table, width, use_tc, tables16, out, q, kv)
@@ -144,9 +160,45 @@ class _TypedLinear(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout, *_unused):
+        if ctx.bf16a:
+            a, w_cat = ctx.saved_tensors
+            dw, db = _linear_backward_bf16a(ctx, dout, a, w_cat)
+            return None, dw, db, None, None, None, None, None, None, None
         a, a_act, hi, lo, w_cat = ctx.saved_tensors
         da, dw, db = _linear_backward(ctx, dout, a, a_act, hi, lo, w_cat, ctx.needs_input_grad[0])
         return da, dw, db, None, None, None, None, None, None, None
+
+
+def _linear_gemm_bf16a(a, w_cat, b_cat, table, width, impl, out):
+    """out = a @ w_cat^T + b_cat over the table's groups for a bf16 `a` (hgt_typed_linear_bf16a, C impl `impl`)."""
+    K = a.shape[1]
+    g_dev, g_host, n_g, c_dev = table
+    wsb = ctypes.c_size_t()
+    _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, K, width, impl, ctypes.byref(wsb))
+    ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=a.device)
+    _lib.call("hgt_typed_linear_bf16a", a.data_ptr(), K, w_cat.data_ptr(), _lib.ptr(b_cat), K, width, g_dev.data_ptr(),
+              g_host.ctypes.data, n_g, c_dev.data_ptr(), out.data_ptr(), impl, ws.data_ptr(), ws.numel(), _stream())
+
+
+def _linear_backward_bf16a(ctx, dout, a, w_cat):
+    """dW, db of _TypedLinear with a bf16 `a`: hgt_typed_linear_bwd_bf16a[_det] with `a` as the dW operand."""
+    width = ctx.width
+    K = w_cat.shape[1]
+    dout = dout.contiguous()
+    dw = torch.zeros_like(w_cat)
+    db = torch.zeros(w_cat.shape[0], dtype=torch.float32, device=w_cat.device) if ctx.has_bias else None
+    impl = (3 if ctx.one else 2) if ctx.use_tc else 1
+    sfx = "_det" if ctx.det else ""
+    g_dev, g_host, n_g, _ = ctx.table
+    c_host = ctx.table.c_host
+    wsb = ctypes.c_size_t()
+    _lib.call("hgt_typed_linear_bwd" + sfx + "_workspace_bytes", g_host.ctypes.data, n_g, c_host.ctypes.data, K, width,
+              K, ctx.out_elems, 0, 1, impl, ctypes.byref(wsb))
+    ws = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=w_cat.device)
+    _lib.call("hgt_typed_linear_bwd_bf16a" + sfx, dout.data_ptr(), ctx.out_elems, a.data_ptr(), K, K, width,
+              g_dev.data_ptr(), g_host.ctypes.data, n_g, c_host.ctypes.data, dw.data_ptr(), _lib.ptr(db), impl,
+              ws.data_ptr(), ws.numel(), _stream())
+    return dw, db
 
 
 def _split_operand(a, act, use_tc, one):

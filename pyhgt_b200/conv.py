@@ -199,13 +199,14 @@ class HGTConv(nn.Module):
     def _typed_linear(self, a, lda, w, bias, k, width, table, out, impl, st, out32=None, t24_off=0):
         """hgt_typed_linear with its (impl-dependent) workspace; table = (groups_dev, groups_host, n, cblocks_dev).
         A bf16 `out` takes hgt_typed_linear_bf16, a uint8 one (a 24-bit table) hgt_typed_linear_t24, which writes the
-        column blocks before t24_off as fp32 to out32."""
+        column blocks before t24_off as fp32 to out32.  A bf16 `a` (fp32 `out`) takes hgt_typed_linear_bf16a."""
         g_dev, g_host, n_g, c_dev = table
         ws_bytes = ctypes.c_size_t()
         _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, k, width, impl, ctypes.byref(ws_bytes))
         ws = torch.empty(max(ws_bytes.value, 1), dtype=torch.uint8, device=out.device)
         outs = (_lib.ptr(out32), t24_off, out.data_ptr()) if out.dtype == torch.uint8 else (out.data_ptr(),)
-        _lib.call("hgt_typed_linear" + _TABLE_SUFFIX[out.dtype], a.data_ptr(), lda, w.data_ptr(), _lib.ptr(bias), k, width, g_dev.data_ptr(),
+        fn = "hgt_typed_linear_bf16a" if a.dtype == torch.bfloat16 else "hgt_typed_linear" + _TABLE_SUFFIX[out.dtype]
+        _lib.call(fn, a.data_ptr(), lda, w.data_ptr(), _lib.ptr(bias), k, width, g_dev.data_ptr(),
                   g_host.ctypes.data, n_g, c_dev.data_ptr(), *outs, impl, ws.data_ptr(), ws.numel(), st)
 
     def _check_inputs(self, node_inp, edge_time):

@@ -947,6 +947,50 @@ __global__ void k_gather_bf16(const uint16_t* const* feat, int32_t feat_dim, con
   for (int c = head + 8 * n8 + lane; c < feat_dim; c += 32) dst[c] = bf16_lo(src[c]);
 }
 
+// One warp per output row i: node_feature[i] = feat[row_type[i]][row_id[i]] as stored, bf16 (sampler.py:
+// sample_subgraph(s)_cuda(..., feature_dtype=torch.bfloat16)).  Loads as k_gather_bf16's: 16 bytes at a time from the
+// row's first 16-byte boundary on.  A store takes 16 bytes where the destination is 16-byte aligned at that point, 4
+// where it is 4-byte aligned, 2 otherwise (source and destination rows may sit at different phases when the width is
+// not a multiple of 8).
+__global__ void k_gather_rows_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
+                                   const int64_t* row_id, int64_t n_rows, uint16_t* node_feature) {
+  const int lane = threadIdx.x & 31;
+  const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  if (i >= n_rows) return;
+  const uint16_t* src = feat[row_type[i]] + row_id[i] * (int64_t)feat_dim;
+  uint16_t* dst = node_feature + i * (int64_t)feat_dim;
+  int head = (int)((((uintptr_t)0 - (uintptr_t)src) & 15) >> 1);
+  if (head > feat_dim) head = feat_dim;
+  const int n8 = (feat_dim - head) >> 3;
+  for (int c = lane; c < head; c += 32) dst[c] = src[c];
+  const uint4* s8 = reinterpret_cast<const uint4*>(src + head);
+  uint16_t* d8 = dst + head;
+  const int phase = (uintptr_t)d8 & 15;
+  for (int c0 = 0; c0 < n8; c0 += 32 * kRowUnroll) {
+    uint4 v[kRowUnroll];
+#pragma unroll
+    for (int u = 0; u < kRowUnroll; ++u)
+      if (c0 + 32 * u + lane < n8) v[u] = s8[c0 + 32 * u + lane];
+#pragma unroll
+    for (int u = 0; u < kRowUnroll; ++u) {
+      const int c = c0 + 32 * u + lane;
+      if (c >= n8) continue;
+      uint16_t* d = d8 + 8 * (int64_t)c;
+      if (phase == 0) {
+        *reinterpret_cast<uint4*>(d) = v[u];
+      } else if ((phase & 3) == 0) {
+        uint32_t* d4 = reinterpret_cast<uint32_t*>(d);
+        d4[0] = v[u].x; d4[1] = v[u].y; d4[2] = v[u].z; d4[3] = v[u].w;
+      } else {
+        const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) d[2 * j] = (uint16_t)w[j], d[2 * j + 1] = (uint16_t)(w[j] >> 16);
+      }
+    }
+  }
+  for (int c = head + 8 * n8 + lane; c < feat_dim; c += 32) dst[c] = src[c];
+}
+
 struct BudgetScratch {
   int64_t *seg_cnt, *seg_off, *cand_pos, *cand_slot, *cand_time;
   void* cub_tmp;
@@ -1574,6 +1618,18 @@ extern "C" int hgt_gsample_gather_features_bf16(const uint16_t* const* feat, int
   if (n_rows == 0 || feat_dim == 0) return 0;
   k_gather_bf16<<<(unsigned)blocks_for(n_rows, kWarps), kThreads, 0, (cudaStream_t)stream>>>(feat, feat_dim, row_type,
                                                                                            row_id, n_rows, node_feature);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int hgt_gsample_gather_rows_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
+                                            const int64_t* row_id, int64_t n_rows, void* node_feature, void* stream) {
+  HGT_REQUIRE(feat_dim >= 0 && n_rows >= 0 &&
+                  (n_rows == 0 || feat_dim == 0 || (feat && row_type && row_id && node_feature)),
+              "hgt_gsample_gather_rows_bf16: bad arguments");
+  if (n_rows == 0 || feat_dim == 0) return 0;
+  k_gather_rows_bf16<<<(unsigned)blocks_for(n_rows, kWarps), kThreads, 0, (cudaStream_t)stream>>>(
+      feat, feat_dim, row_type, row_id, n_rows, static_cast<uint16_t*>(node_feature));
   HGT_LAUNCH_CHECK();
   return 0;
 }

@@ -3,7 +3,9 @@
 // This file holds the fp32 SIMT kernel (impl 1); the wgmma tensor-core kernel (impl 2, split-bf16 x3; impl 3, auto with
 // one bf16 product on the tensor cores) lives in linear_tc.cu and is dispatched from hgt_typed_linear below.  hgt_typed_linear_bf16 runs the same kernels with a bf16
 // output, each fp32 result rounded to nearest-even once when it is stored; hgt_typed_linear_t24 with the planar 24-bit
-// table output (include/hgt_b200.h), each result rounded by hgt_t24_round once when it is stored.
+// table output (include/hgt_b200.h), each result rounded by hgt_t24_round once when it is stored.  hgt_typed_linear_bf16a
+// reads a bf16 A (fp32 output): the SIMT kernel widens each element as it loads it, the tensor cores skip the products
+// with A's zero lo half (linear_tc.cu); both write bitwise what the fp32 call on the widened A writes.
 #include <cuda_bf16.h>
 
 #include <type_traits>
@@ -22,6 +24,10 @@ int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float
                         int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                         int32_t n_groups, const hgt_lin_cblock* cblocks, float* out32, int64_t t24_off, hgt_t24* out,
                         int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st);
+int hgt_typed_linear_tc_bf16a(const __nv_bfloat16* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                              int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                              int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int32_t products,
+                              void* workspace, size_t workspace_bytes, cudaStream_t st);
 bool hgt_typed_linear_tc_supported(int64_t lda, int32_t K, int32_t cb_width);
 size_t hgt_typed_linear_tc_workspace(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K, int32_t cb_width,
                                      int32_t products);
@@ -92,10 +98,12 @@ struct TilePrefix {
 
 __device__ __forceinline__ void store_out(float* p, float v) { *p = v; }
 __device__ __forceinline__ void store_out(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+__device__ __forceinline__ float load_a(const float* p) { return *p; }
+__device__ __forceinline__ float load_a(const __nv_bfloat16* p) { return __bfloat162float(*p); }   // exact
 
-template <class OutT>
+template <class AT, class OutT>
 __global__ void __launch_bounds__(GEMM_THREADS)
-k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __restrict__ W,
+k_typed_linear_simt(const AT* __restrict__ A, int64_t lda, const float* __restrict__ W,
                     const float* __restrict__ bias, int K, int cb_width,
                     const hgt_lin_group* __restrict__ groups, int n_groups,
                     const hgt_lin_cblock* __restrict__ cblocks, OutT* __restrict__ out, TilePrefix tp,
@@ -128,7 +136,7 @@ k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __res
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 
-  const float* Ag = A + (grp.a_row0 + m0) * lda;
+  const AT* Ag = A + (grp.a_row0 + m0) * lda;
   const float* Wg = W + w_row0 * (int64_t)K;
 
   for (int k0 = 0; k0 < K; k0 += BK) {
@@ -138,7 +146,7 @@ k_typed_linear_simt(const float* __restrict__ A, int64_t lda, const float* __res
       int idx = tid + it * GEMM_THREADS;       // 0..2047
       int r = idx / BK, kk = idx % BK;
       float v = 0.f;
-      if (r < rows_here && k0 + kk < K) v = Ag[(int64_t)r * lda + k0 + kk];
+      if (r < rows_here && k0 + kk < K) v = load_a(Ag + (int64_t)r * lda + k0 + kk);
       As[kk][r] = v;
     }
 #pragma unroll
@@ -269,8 +277,8 @@ extern "C" int hgt_typed_linear_workspace_bytes(const hgt_lin_group* h_groups, i
 
 namespace {
 
-template <class OutT>
-int typed_linear(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
+template <class AT, class OutT>
+int typed_linear(const AT* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
                  const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
                  const hgt_lin_cblock* cblocks, OutT* out, int32_t impl, void* workspace, size_t workspace_bytes,
                  cudaStream_t st, float* out32 = nullptr, int64_t t24_off = 0) {
@@ -294,7 +302,10 @@ int typed_linear(const float* A, int64_t lda, const float* W, const float* bias,
   if (impl == 2 || impl == 3) {
     HGT_REQUIRE(tc, "hgt_typed_linear: tensor-core kernel does not support lda=%lld K=%d cb_width=%d",
                 (long long)lda, K, cb_width);
-    if constexpr (std::is_same<OutT, hgt_t24>::value)
+    if constexpr (std::is_same<AT, __nv_bfloat16>::value)
+      return hgt_typed_linear_tc_bf16a(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out,
+                                       impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
+    else if constexpr (std::is_same<OutT, hgt_t24>::value)
       return hgt_typed_linear_tc(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out32, t24_off, out,
                                  impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
     else
@@ -313,7 +324,7 @@ int typed_linear(const float* A, int64_t lda, const float* W, const float* bias,
   }
   tp.first_tile[n_groups] = (int32_t)total;
   if (total == 0) return 0;
-  k_typed_linear_simt<OutT><<<(unsigned)total, GEMM_THREADS, 0, st>>>(A, lda, W, bias, K, cb_width, groups, n_groups,
+  k_typed_linear_simt<AT, OutT><<<(unsigned)total, GEMM_THREADS, 0, st>>>(A, lda, W, bias, K, cb_width, groups, n_groups,
                                                                       cblocks, out, tp, out32, t24_off);
   HGT_LAUNCH_CHECK();
   return 0;
@@ -343,4 +354,12 @@ extern "C" int hgt_typed_linear_t24(const float* A, int64_t lda, const float* W,
                                     void* out24, int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
   return typed_linear(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, static_cast<hgt_t24*>(out24),
                       impl, workspace, workspace_bytes, (cudaStream_t)stream_, out, t24_off);
+}
+
+extern "C" int hgt_typed_linear_bf16a(const void* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                                      int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                      int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int32_t impl,
+                                      void* workspace, size_t workspace_bytes, void* stream_) {
+  return typed_linear(static_cast<const __nv_bfloat16*>(A), lda, W, bias, K, cb_width, groups, h_groups, n_groups,
+                      cblocks, out, impl, workspace, workspace_bytes, (cudaStream_t)stream_);
 }

@@ -21,6 +21,9 @@
 // SIMT fp32 path for shapes the tensor cores cannot take (width % 8, K % 16, overlapping groups such as the RTE tables).
 // impl 3: the tensor-core kernels with one bf16 product (tcp P = 1, torch's "medium" float32 matmul precision): only the
 // hi halves of dOut, A and W^T are written and read; db is still summed from the fp32 dOut.
+// bf16 A (hgt_typed_linear_bwd_bf16a, dW and db only): A is the dW product's B operand as it is, exact in bf16 with a zero
+// lo half, so the tensor cores run dOut_hi*A + dOut_lo*A (tcp P = 4; dOut_hi*A at impl 3) and the SIMT kernel widens A as
+// it loads it.  Either way dW and db are bitwise those of the fp32 call on the widened A.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -340,12 +343,12 @@ struct DwJob {
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       tma_load_2d(sa + j * ATOM_BYTES, d_hi, t.mt * BM + j * 64, row, bar);
-      if constexpr (P == 3) tma_load_2d(sa + A_BYTES + j * ATOM_BYTES, d_hi + 1, t.mt * BM + j * 64, row, bar);
+      if constexpr (has_a_lo<P>()) tma_load_2d(sa + A_BYTES + j * ATOM_BYTES, d_hi + 1, t.mt * BM + j * 64, row, bar);
     }
 #pragma unroll
     for (int j = 0; j < BN / 64; ++j) {
       tma_load_2d(sa + B + j * ATOM_BYTES, x_hi, t.n0 + j * 64, row, bar);
-      if constexpr (P == 3) tma_load_2d(sa + B + BN * BK * 2 + j * ATOM_BYTES, x_hi + 1, t.n0 + j * 64, row, bar);
+      if constexpr (has_b_lo<P>()) tma_load_2d(sa + B + BN * BK * 2 + j * ATOM_BYTES, x_hi + 1, t.n0 + j * 64, row, bar);
     }
   }
   template <int BN>
@@ -469,8 +472,11 @@ __global__ void k_lin_dx_simt_det(const float* __restrict__ dout, const float* _
 constexpr int DW_SIMT_ROWS = 2048;
 // DET: partial tiles / bias sums go to the unit's slot (unit / (n_tiles * k_tiles)) of dW = part [slot][width][K_in] and
 // db = db_part [slot][width]; chunks of chunk_rows rows.
-template <bool DET>
-__device__ __forceinline__ void lin_dw_simt(const float* __restrict__ dout, const float* __restrict__ A, int64_t lda,
+__device__ __forceinline__ float load_a(const float* p) { return *p; }
+__device__ __forceinline__ float load_a(const __nv_bfloat16* p) { return __bfloat162float(*p); }   // exact
+
+template <bool DET, class AT>
+__device__ __forceinline__ void lin_dw_simt(const float* __restrict__ dout, const AT* __restrict__ A, int64_t lda,
                                             const GcTask* __restrict__ tasks, int n_tasks, int K_in, int width,
                                             int n_tiles, int k_tiles, int64_t chunk_rows, float* __restrict__ dW,
                                             float* __restrict__ db) {
@@ -495,7 +501,7 @@ __device__ __forceinline__ void lin_dw_simt(const float* __restrict__ dout, cons
       float dv = 0.f, av = 0.f;
       if (r < r1) {
         if (n0 + tx < width) dv = dout[tk.out_off + r * tk.ld + n0 + tx];
-        if (dW && k0 + tx < K_in) av = A[(tk.a_row0 + r) * lda + k0 + tx];
+        if (dW && k0 + tx < K_in) av = load_a(A + (tk.a_row0 + r) * lda + k0 + tx);
       }
       sd[rr][tx] = dv;
       sa[rr][tx] = av;
@@ -525,13 +531,15 @@ __device__ __forceinline__ void lin_dw_simt(const float* __restrict__ dout, cons
     else atomicAdd(db + tk.w_row + n0 + tx, bsum);
   }
 }
+template <class AT>
 __global__ void __launch_bounds__(256)
-k_lin_dw_simt(const float* __restrict__ dout, const float* __restrict__ A, int64_t lda, const GcTask* __restrict__ tasks,
+k_lin_dw_simt(const float* __restrict__ dout, const AT* __restrict__ A, int64_t lda, const GcTask* __restrict__ tasks,
               int n_tasks, int K_in, int width, int n_tiles, int k_tiles, float* __restrict__ dW, float* __restrict__ db) {
   lin_dw_simt<false>(dout, A, lda, tasks, n_tasks, K_in, width, n_tiles, k_tiles, DW_SIMT_ROWS, dW, db);
 }
+template <class AT>
 __global__ void __launch_bounds__(256)
-k_lin_dw_simt_det(const float* __restrict__ dout, const float* __restrict__ A, int64_t lda,
+k_lin_dw_simt_det(const float* __restrict__ dout, const AT* __restrict__ A, int64_t lda,
                   const GcTask* __restrict__ tasks, int n_tasks, int K_in, int width, int n_tiles, int k_tiles,
                   int64_t chunk_rows, float* __restrict__ dw_part, float* __restrict__ db_part) {
   lin_dw_simt<true>(dout, A, lda, tasks, n_tasks, K_in, width, n_tiles, k_tiles, chunk_rows, dw_part, db_part);
@@ -712,9 +720,18 @@ int launch_bwd(const DwJobDet& job, int tiles, cudaStream_t st) {
   return 0;
 }
 
-// Tile width (64 / 128 / 256) x products (3 / 1) of one of the three tensor-core jobs.
+// Tile width (64 / 128 / 256) x products (3 / 1) of one of the three tensor-core jobs; b_exact (dW jobs): P = 4.
 template <class Job>
-int launch_bwd_any(const Job& job, int tile_n, bool one, int tiles, cudaStream_t st) {
+int launch_bwd_any(const Job& job, int tile_n, bool one, int tiles, cudaStream_t st, bool b_exact = false) {
+  if constexpr (!std::is_same<Job, DxJob>::value) {
+    if (b_exact && !one) {
+      switch (tile_n) {
+        case 64: return launch_bwd<64, 4>(job, tiles, st);
+        case 128: return launch_bwd<128, 4>(job, tiles, st);
+        default: return launch_bwd<256, 4>(job, tiles, st);
+      }
+    }
+  }
   switch (tile_n) {
     case 64: return one ? launch_bwd<64, 1>(job, tiles, st) : launch_bwd<64, 3>(job, tiles, st);
     case 128: return one ? launch_bwd<128, 1>(job, tiles, st) : launch_bwd<128, 3>(job, tiles, st);
@@ -753,20 +770,24 @@ int bwd_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, const h
   return 0;
 }
 
+// a16: A in bf16 (hgt_typed_linear_bwd_bf16a; A, a_hi_in and a_lo_in are then NULL, dA too).
 int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo, int64_t dout_elems,
                      const float* A, int64_t lda, const void* a_hi_in, const void* a_lo_in,
                      const float* W, int32_t K, int32_t cb_width, const hgt_lin_group* groups,
                      const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* h_cblocks,
                      float* dA, int32_t accumulate_dA, const float* gelu_aux, float* dW, float* db,
-                     int32_t impl, void* workspace, size_t workspace_bytes, void* stream_, bool det) {
+                     int32_t impl, void* workspace, size_t workspace_bytes, void* stream_, bool det,
+                     const __nv_bfloat16* a16 = nullptr) {
   cudaStream_t st = (cudaStream_t)stream_;
   HGT_REQUIRE(n_groups >= 0, "hgt_typed_linear_bwd: n_groups=%d", n_groups);
-  HGT_REQUIRE(K > 0 && cb_width > 0 && W, "hgt_typed_linear_bwd: K=%d cb_width=%d", K, cb_width);
+  HGT_REQUIRE(K > 0 && cb_width > 0 && (W || (a16 && !dA)), "hgt_typed_linear_bwd: K=%d cb_width=%d", K, cb_width);
   if (n_groups == 0) return 0;
   HGT_REQUIRE(groups && h_groups && h_cblocks, "hgt_typed_linear_bwd: NULL group tables");
   HGT_REQUIRE(impl >= 0 && impl <= 3, "hgt_typed_linear_bwd: unknown impl %d", impl);
-  // impl 3 reads only the hi halves, so a producer's split may come without its lo half
-  const bool have_dsplit = dout_hi && (dout_lo || impl == 3), have_asplit = a_hi_in && (a_lo_in || impl == 3);
+  if (a16) a_hi_in = a16, a_lo_in = nullptr;
+  // impl 3 reads only the hi halves, so a producer's split may come without its lo half; a bf16 A has no lo half
+  const bool have_dsplit = dout_hi && (dout_lo || impl == 3),
+             have_asplit = a_hi_in && (a_lo_in || impl == 3 || a16);
   HGT_REQUIRE(dout || have_dsplit, "hgt_typed_linear_bwd: neither dout nor its bf16 split given");
   const BwdLayout L = bwd_layout(h_groups, n_groups, h_cblocks, K, cb_width, lda, dout_elems, have_dsplit, have_asplit, impl,
                                  det);
@@ -777,7 +798,7 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
                 "hgt_typed_linear_bwd: tensor-core path does not support K=%d cb_width=%d lda=%lld (or overlapping groups)",
                 K, cb_width, (long long)lda);
   else
-    HGT_REQUIRE(dout && (A || !dW), "hgt_typed_linear_bwd: the SIMT path needs fp32 dout and A");
+    HGT_REQUIRE(dout && (A || a16 || !dW), "hgt_typed_linear_bwd: the SIMT path needs fp32 dout and A");
   char* base = reinterpret_cast<char*>(hgt_align_up(reinterpret_cast<size_t>(workspace), 256));
   float* part = det ? reinterpret_cast<float*>(base + L.off_part) : nullptr;
   float* db_part = det ? reinterpret_cast<float*>(base + L.off_dbp) : nullptr;
@@ -874,13 +895,20 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
       }
       if ((rc = upload_tasks())) return rc;
       if (units > 0 && det) {
-        k_lin_dw_simt_det<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles,
-                                                           chunk_rows, dW ? part : nullptr, db ? db_part : nullptr);
+        if (a16)
+          k_lin_dw_simt_det<<<(unsigned)units, 256, 0, st>>>(dout, a16, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles,
+                                                             chunk_rows, dW ? part : nullptr, db ? db_part : nullptr);
+        else
+          k_lin_dw_simt_det<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles,
+                                                             chunk_rows, dW ? part : nullptr, db ? db_part : nullptr);
         HGT_LAUNCH_CHECK();
         if (dW && (rc = reduce_rows(part, K, n_tiles * k_tiles, 0, dW))) return rc;
         if (db && (rc = reduce_rows(db_part, 1, n_tiles * k_tiles, 1, db))) return rc;
       } else if (units > 0) {
-        k_lin_dw_simt<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles, dW, db);
+        if (a16)
+          k_lin_dw_simt<<<(unsigned)units, 256, 0, st>>>(dout, a16, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles, dW, db);
+        else
+          k_lin_dw_simt<<<(unsigned)units, 256, 0, st>>>(dout, A, lda, d_tasks, nt, K, cb_width, n_tiles, k_tiles, dW, db);
         HGT_LAUNCH_CHECK();
       }
     }
@@ -899,10 +927,12 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
   __nv_bfloat16* wt_hi = reinterpret_cast<__nv_bfloat16*>(base + L.off_wthi);
   __nv_bfloat16* wt_lo = reinterpret_cast<__nv_bfloat16*>(base + L.off_wtlo);
   // One product: the producers write no lo halves; the lo maps repeat the hi ones (never loaded, valid to prefetch).
+  // The same for the lo half a bf16 A does not have.
   __nv_bfloat16* const d_lo_w = L.one ? nullptr : d_lo;
   __nv_bfloat16* const a_lo_w = L.one ? nullptr : a_lo;
   __nv_bfloat16* const wt_lo_w = L.one ? nullptr : wt_lo;
   if (L.one) d_lo = d_hi, a_lo = a_hi, wt_lo = wt_hi;
+  if (a16) a_lo = a_hi;
 
   // 1. tensor maps: per task dOut hi/lo {cols = width, rows = m}; per group A hi/lo {cols = K, rows = m}; W^T hi/lo.
   //    They encode addresses only, so they go up with the task table before any kernel runs.
@@ -1031,10 +1061,10 @@ int typed_linear_bwd(const float* dout, const void* dout_hi, const void* dout_lo
         DwJobDet dj;
         static_cast<DwJob&>(dj) = job;
         dj.part = part;
-        if ((rc = launch_bwd_any(dj, tile_n, L.one, (int)units, st))) return rc;
+        if ((rc = launch_bwd_any(dj, tile_n, L.one, (int)units, st, a16 != nullptr))) return rc;
         if ((rc = reduce_rows(part, K, m_tiles * n_tiles, 0, dW))) return rc;
       } else {
-        if ((rc = launch_bwd_any(job, tile_n, L.one, (int)units, st))) return rc;
+        if ((rc = launch_bwd_any(job, tile_n, L.one, (int)units, st, a16 != nullptr))) return rc;
       }
     }
   }
@@ -1079,4 +1109,25 @@ extern "C" int hgt_typed_linear_bwd_det(const float* dout, const void* dout_hi, 
   return typed_linear_bwd(dout, dout_hi, dout_lo, dout_elems, A, lda, a_hi_in, a_lo_in, W, K, cb_width, groups, h_groups,
                           n_groups, h_cblocks, dA, accumulate_dA, gelu_aux, dW, db, impl, workspace, workspace_bytes,
                           stream_, true);
+}
+
+extern "C" int hgt_typed_linear_bwd_bf16a(const float* dout, int64_t dout_elems, const void* A, int64_t lda, int32_t K,
+                                          int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                          int32_t n_groups, const hgt_lin_cblock* h_cblocks, float* dW, float* db,
+                                          int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
+  HGT_REQUIRE(dout && (A || !dW), "hgt_typed_linear_bwd_bf16a: NULL argument");
+  return typed_linear_bwd(dout, nullptr, nullptr, dout_elems, nullptr, lda, nullptr, nullptr, nullptr, K, cb_width, groups,
+                          h_groups, n_groups, h_cblocks, nullptr, 0, nullptr, dW, db, impl, workspace, workspace_bytes,
+                          stream_, false, static_cast<const __nv_bfloat16*>(A));
+}
+
+extern "C" int hgt_typed_linear_bwd_bf16a_det(const float* dout, int64_t dout_elems, const void* A, int64_t lda,
+                                              int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                                              const hgt_lin_group* h_groups, int32_t n_groups,
+                                              const hgt_lin_cblock* h_cblocks, float* dW, float* db, int32_t impl,
+                                              void* workspace, size_t workspace_bytes, void* stream_) {
+  HGT_REQUIRE(dout && (A || !dW), "hgt_typed_linear_bwd_bf16a_det: NULL argument");
+  return typed_linear_bwd(dout, nullptr, nullptr, dout_elems, nullptr, lda, nullptr, nullptr, nullptr, K, cb_width, groups,
+                          h_groups, n_groups, h_cblocks, nullptr, 0, nullptr, dW, db, impl, workspace, workspace_bytes,
+                          stream_, true, static_cast<const __nv_bfloat16*>(A));
 }

@@ -26,6 +26,13 @@
 // and there is no separate pass over A and no A halves in the workspace.  k_split_bf16 still splits A first for 64-column
 // tiles (splits_a_first) and for an A that TMA cannot load as fp32 (base not 16-byte aligned, or lda % 4 != 0).  W is
 // split once per call by k_split_bf16.
+//
+// bf16 A (hgt_typed_linear_bf16a): A is exactly its own hi half and its lo half is zero, so the x3 product loses its
+// A_lo*W_hi term (tcp P = 2: A*W_hi + A*W_lo, two products per k-step) and P = 1 stays A*W_hi.  The products that remain
+// run in P = 3's order and the dropped one adds exact zeros, so the output is bitwise that of the fp32 call on the
+// widened A.  TMA loads A in place where its rows are 16-byte multiples (K % 8 == 0, lda % 8 == 0, base 16-byte aligned);
+// otherwise (K = 129, 1169: the reference's input widths) k_pad_bf16 copies it first into zero-padded rows of Kp, the
+// same place the fp32 path splits such an A into, in stream-ordered memory of its own.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -68,6 +75,21 @@ __global__ void k_split_bf16(const float* __restrict__ in, int64_t ld_in, int64_
   }
   *reinterpret_cast<uint2*>(hi + r * Kp + c) = *reinterpret_cast<uint2*>(h);
   if (lo) *reinterpret_cast<uint2*>(lo + r * Kp + c) = *reinterpret_cast<uint2*>(l);
+}
+
+// ---- bf16 [rows, K] (row stride ld_in) -> [rows, Kp], columns K .. Kp - 1 zero --------------------------------------
+__global__ void k_pad_bf16(const __nv_bfloat16* __restrict__ in, int64_t ld_in, int64_t rows, int K, int Kp,
+                           __nv_bfloat16* __restrict__ out) {
+  const int vec_per_row = Kp / 4;
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= rows * vec_per_row) return;
+  int64_t r = i / vec_per_row;
+  int c = (int)(i - r * vec_per_row) * 4;
+  const __nv_bfloat16* src = in + r * ld_in + c;
+  __nv_bfloat16 v[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) v[j] = (c + j < K) ? src[j] : __float2bfloat16_rn(0.f);
+  *reinterpret_cast<uint2*>(out + r * Kp + c) = *reinterpret_cast<uint2*>(v);
 }
 
 // Columns col .. col + 3 of an output row: fp32, or bf16 rounded to nearest-even.  aligned: p is 4-element aligned.
@@ -180,10 +202,10 @@ struct FwdJob {
       for (int j = 0; j < KB / 32; ++j) tma_load_2d(sa + j * A32_BOX, &a_hi, k + 32 * j, t.a_row, bar);
     } else {
       tma_load_2d(sa, &a_hi, k, t.a_row, bar);
-      if constexpr (P == 3) tma_load_2d(sa + A, &a_lo, k, t.a_row, bar);
+      if constexpr (has_a_lo<P>()) tma_load_2d(sa + A, &a_lo, k, t.a_row, bar);
     }
     tma_load_2d(sa + B, &w_hi, k, t.w_row, bar);
-    if constexpr (P == 3) tma_load_2d(sa + B + BN * KB * 2, &w_lo, k, t.w_row, bar);
+    if constexpr (has_b_lo<P>()) tma_load_2d(sa + B + BN * KB * 2, &w_lo, k, t.w_row, bar);
   }
   // OutT (or fp32 T, the fp32 blocks of a 24-bit job) at o, the tile's element (0, 0)
   template <int BN, class T, class Pair>
@@ -322,11 +344,12 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int make_map(CUtensorMap* m, const void* base, int64_t rows, int Kp, int box_rows, int kb) {
+// bf16 [rows, Kp] at row stride ld elements (default Kp), boxes of kb columns x box_rows rows.
+int make_map(CUtensorMap* m, const void* base, int64_t rows, int Kp, int box_rows, int kb, int64_t ld = 0) {
   EncodeTiledFn fn = get_encode_fn();
   HGT_REQUIRE(fn != nullptr, "hgt_typed_linear: cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)Kp * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)(ld ? ld : Kp) * 2};
   cuuint32_t box[2] = {(cuuint32_t)kb, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
@@ -398,10 +421,10 @@ void extents(const hgt_lin_group* h_groups, int n_groups, int cb_width, int64_t*
 }
 
 // Operands of one launch: A as fp32 (a32, lda; AF) or as bf16 halves (a_hi, a_lo), W as bf16 halves.  Halves are K-major
-// at row stride Kp; a lo pointer is NULL at P = 1.
+// at row stride Kp (A's at a_ld where that is set: a bf16 A read in place); a lo pointer is NULL where P has no lo half.
 struct FwdOps {
   const float* a32;
-  int64_t lda;
+  int64_t lda, a_ld = 0;
   const __nv_bfloat16 *a_hi, *a_lo, *w_hi, *w_lo;
   int64_t a_rows, w_rows;
   int K, Kp;
@@ -418,11 +441,11 @@ int launch_fwd(FwdJob<OutT, AF>& job, const FwdOps& ops, int tiles, cudaStream_t
     if ((rc = make_map_f32(&job.a_hi, ops.a32, ops.a_rows, ops.K, ops.lda))) return rc;
     job.a_lo = job.a_hi;
   } else {
-    if ((rc = make_map(&job.a_hi, ops.a_hi, ops.a_rows, ops.Kp, BM, KB))) return rc;
-    if ((rc = make_map(&job.a_lo, P == 3 ? ops.a_lo : ops.a_hi, ops.a_rows, ops.Kp, BM, KB))) return rc;
+    if ((rc = make_map(&job.a_hi, ops.a_hi, ops.a_rows, ops.Kp, BM, KB, ops.a_ld))) return rc;
+    if ((rc = make_map(&job.a_lo, has_a_lo<P>() ? ops.a_lo : ops.a_hi, ops.a_rows, ops.Kp, BM, KB, ops.a_ld))) return rc;
   }
   if ((rc = make_map(&job.w_hi, ops.w_hi, ops.w_rows, ops.Kp, BN, KB))) return rc;
-  if ((rc = make_map(&job.w_lo, P == 3 ? ops.w_lo : ops.w_hi, ops.w_rows, ops.Kp, BN, KB))) return rc;
+  if ((rc = make_map(&job.w_lo, has_b_lo<P>() ? ops.w_lo : ops.w_hi, ops.w_rows, ops.Kp, BN, KB))) return rc;
   job.k_blocks = (ops.Kp + KB - 1) / KB;
   if constexpr (fwd_tma_store<BN>()) {
     CUtensorMap tmpl, tmpl_lo, tmpl_f32;
@@ -447,11 +470,12 @@ int launch_fwd(FwdJob<OutT, AF>& job, const FwdOps& ops, int tiles, cudaStream_t
   return 0;
 }
 
-// Fills the job's tile tables and launches the instance for its tile width, product count and A operand.
+// Fills the job's tile tables and launches the instance for its tile width, product count and A operand.  a_exact: A is
+// bf16 (no lo half), and one == false runs P = 2.
 template <class OutT, bool AF>
 int run_fwd(const FwdOps& ops, const float* bias, int32_t cb_width, const hgt_lin_group* groups,
             const hgt_lin_group* h_groups, int32_t n_groups, const hgt_lin_cblock* cblocks, OutT* out,
-            CUtensorMap* out_maps, bool one, cudaStream_t st) {
+            CUtensorMap* out_maps, bool one, cudaStream_t st, bool a_exact = false) {
   FwdJob<OutT, AF> job;
   job.tile_n = pick_tile_n(cb_width);
   job.n_tiles_n = (cb_width + job.tile_n - 1) / job.tile_n;
@@ -477,6 +501,16 @@ int run_fwd(const FwdOps& ops, const float* bias, int32_t cb_width, const hgt_li
   const int tiles = (int)total;
   // 64-column tiles read A split by k_split_bf16 (tc_run): only the presplit instances exist for them
   if constexpr (AF) HGT_REQUIRE(job.tile_n != 64, "hgt_typed_linear(tc): no fp32-A kernel for 64-column tiles");
+  if constexpr (!AF && std::is_same<OutT, float>::value) {
+    if (a_exact && !one) {
+      switch (job.tile_n) {
+        case 64: return launch_fwd<64, OutT, 2, fwd_bk<64>()>(job, ops, tiles, st);
+        case 128: return launch_fwd<128, OutT, 2, fwd_bk<128>()>(job, ops, tiles, st);
+        default: return launch_fwd<256, OutT, 2, fwd_bk<256>()>(job, ops, tiles, st);
+      }
+    }
+  }
+  HGT_REQUIRE(!a_exact || one, "hgt_typed_linear_bf16a(tc): fp32 output only");
   if (one) {
     // k-block of the one-product kernel at BN = 128 / 256 (DESIGN.md §5.2): 32 (SWIZZLE_64B, as at P = 3) for fp32 A,
     // whose 64-wide stages would leave a ring of two at BN = 256; 64 (SWIZZLE_128B) for presplit A.  HGT_TC_P1_KB=32 or
@@ -687,6 +721,63 @@ static int tc_run(const float* A, int64_t lda, const __nv_bfloat16* a_hi_in, con
     return run_fwd<OutT, false>(ops, bias, cb_width, groups, h_groups, n_groups, cblocks, out, out_maps, one, st);
   }();
   const cudaError_t freed = cudaFreeAsync(halves, st);
+  if (rc) return rc;
+  HGT_CHECK_CUDA(freed);
+  return 0;
+}
+
+// bf16 A (see the top of the file): W split as for fp32 A, A read in place or copied into zero-padded rows first.  The
+// workspace is hgt_typed_linear_tc_workspace's for the same shape (the A halves it reserves for 64-column tiles stay
+// unused).
+int hgt_typed_linear_tc_bf16a(const __nv_bfloat16* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                              int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                              int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int32_t products,
+                              void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  HGT_REQUIRE(hgt_typed_linear_tc_supported(lda, K, cb_width), "hgt_typed_linear_bf16a(tc): unsupported K=%d cb_width=%d",
+              K, cb_width);
+  HGT_REQUIRE(products == 3 || products == 1, "hgt_typed_linear_bf16a(tc): products=%d", products);
+  const bool one = products == 1;
+  FwdOps ops;
+  ops.a32 = nullptr;
+  ops.lda = 0;
+  ops.out32 = nullptr;
+  ops.t24_off = 0;
+  ops.K = K;
+  ops.Kp = (K + 7) / 8 * 8;
+  extents(h_groups, n_groups, cb_width, &ops.a_rows, &ops.w_rows);
+  const size_t need = hgt_typed_linear_tc_workspace(h_groups, n_groups, K, cb_width, products);
+  HGT_REQUIRE(workspace && workspace_bytes >= need, "hgt_typed_linear_bf16a(tc): workspace too small (%zu < %zu)",
+              workspace_bytes, need);
+  const size_t w_half = hgt_align_up((size_t)ops.w_rows * ops.Kp * 2, 256);
+  const size_t a_pad = hgt_align_up((size_t)ops.a_rows * ops.Kp * 2, 256);
+  char* p = reinterpret_cast<char*>(hgt_align_up(reinterpret_cast<size_t>(workspace), 256));
+  if (splits_a_first(cb_width)) p += (one ? 1 : 2) * a_pad;
+  __nv_bfloat16* w_hi = reinterpret_cast<__nv_bfloat16*>(p); p += w_half;
+  __nv_bfloat16* w_lo = one ? nullptr : reinterpret_cast<__nv_bfloat16*>(p); p += one ? 0 : w_half;
+  CUtensorMap* out_maps = reinterpret_cast<CUtensorMap*>(p);
+  ops.w_hi = w_hi;
+  ops.w_lo = w_lo;
+  int64_t n = ops.w_rows * (ops.Kp / 4);
+  if (n > 0) k_split_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(W, K, ops.w_rows, K, ops.Kp, w_hi, w_lo);
+  HGT_LAUNCH_CHECK();
+  ops.a_lo = nullptr;
+  if (A && (reinterpret_cast<uintptr_t>(A) & 15) == 0 && lda % 8 == 0 && K % 8 == 0) {
+    ops.a_hi = A;
+    ops.a_ld = lda;
+    return run_fwd<float, false>(ops, bias, cb_width, groups, h_groups, n_groups, cblocks, out, out_maps, one, st, true);
+  }
+  n = ops.a_rows * (ops.Kp / 4);
+  if (n == 0) return 0;
+  void* padded = nullptr;
+  HGT_CHECK_CUDA(cudaMallocAsync(&padded, a_pad, st));
+  const int rc = [&]() -> int {
+    k_pad_bf16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(A, lda, ops.a_rows, K, ops.Kp,
+                                                            static_cast<__nv_bfloat16*>(padded));
+    HGT_LAUNCH_CHECK();
+    ops.a_hi = static_cast<const __nv_bfloat16*>(padded);
+    return run_fwd<float, false>(ops, bias, cb_width, groups, h_groups, n_groups, cblocks, out, out_maps, one, st, true);
+  }();
+  const cudaError_t freed = cudaFreeAsync(padded, st);
   if (rc) return rc;
   HGT_CHECK_CUDA(freed);
   return 0;

@@ -19,9 +19,11 @@ __device__ __forceinline__ int64_t union_row(const int64_t* loc_off, const int64
   return uoff[t] + v - loc_off[t];
 }
 
-// One warp per <member (grid.y), local row i>: node_type, the member's row map and the feature row.
+// One warp per <member (grid.y), local row i>: node_type, the member's row map and the feature row (FeatT: float, or
+// uint16_t for bf16 rows, copied as they are).
+template <class FeatT>
 __global__ void k_merge_nodes(const hgt_merge_member* members, int32_t T, const int64_t* loc_off, const int64_t* uoff,
-                              int32_t feat_dim, int64_t* node_type, float* node_feature, int64_t* member_rows) {
+                              int32_t feat_dim, int64_t* node_type, FeatT* node_feature, int64_t* member_rows) {
   const int lane = threadIdx.x & 31;
   const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int b = blockIdx.y;
@@ -36,8 +38,8 @@ __global__ void k_merge_nodes(const hgt_merge_member* members, int32_t T, const 
     member_rows[mb.node_base + i] = u;
   }
   if (node_feature) {
-    const float* src = mb.node_feature + i * (int64_t)feat_dim;
-    float* dst = node_feature + u * (int64_t)feat_dim;
+    const FeatT* src = reinterpret_cast<const FeatT*>(mb.node_feature) + i * (int64_t)feat_dim;
+    FeatT* dst = node_feature + u * (int64_t)feat_dim;
     for (int c = lane; c < feat_dim; c += 32) dst[c] = src[c];
   }
 }
@@ -58,13 +60,11 @@ __global__ void k_merge_edges(const hgt_merge_member* members, int32_t T, const 
   edge_time[o] = mb.edge_time[e];
 }
 
-}  // namespace
-
-extern "C" int hgt_merge_batches(const hgt_merge_member* members, int32_t n_members, int32_t num_types,
-                                 const int64_t* loc_off, const int64_t* uoff, int64_t max_rows, int64_t max_edges,
-                                 int64_t n_edges, int32_t feat_dim, int64_t* node_type, float* node_feature,
-                                 int64_t* member_rows, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time,
-                                 void* stream) {
+template <class FeatT>
+int merge_batches(const hgt_merge_member* members, int32_t n_members, int32_t num_types, const int64_t* loc_off,
+                  const int64_t* uoff, int64_t max_rows, int64_t max_edges, int64_t n_edges, int32_t feat_dim,
+                  int64_t* node_type, FeatT* node_feature, int64_t* member_rows, int64_t* edge_index,
+                  int64_t* edge_type, int64_t* edge_time, void* stream) {
   HGT_REQUIRE(members && n_members >= 0 && n_members < 65536 && num_types > 0 && max_rows >= 0 && max_edges >= 0 &&
                   n_edges >= 0 && feat_dim >= 0,
               "hgt_merge_batches: bad arguments");
@@ -81,4 +81,24 @@ extern "C" int hgt_merge_batches(const hgt_merge_member* members, int32_t n_memb
     HGT_LAUNCH_CHECK();
   }
   return 0;
+}
+
+}  // namespace
+
+extern "C" int hgt_merge_batches(const hgt_merge_member* members, int32_t n_members, int32_t num_types,
+                                 const int64_t* loc_off, const int64_t* uoff, int64_t max_rows, int64_t max_edges,
+                                 int64_t n_edges, int32_t feat_dim, int64_t* node_type, float* node_feature,
+                                 int64_t* member_rows, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time,
+                                 void* stream) {
+  return merge_batches(members, n_members, num_types, loc_off, uoff, max_rows, max_edges, n_edges, feat_dim, node_type,
+                       node_feature, member_rows, edge_index, edge_type, edge_time, stream);
+}
+
+extern "C" int hgt_merge_batches_bf16(const hgt_merge_member* members, int32_t n_members, int32_t num_types,
+                                      const int64_t* loc_off, const int64_t* uoff, int64_t max_rows, int64_t max_edges,
+                                      int64_t n_edges, int32_t feat_dim, int64_t* node_type, void* node_feature,
+                                      int64_t* member_rows, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time,
+                                      void* stream) {
+  return merge_batches(members, n_members, num_types, loc_off, uoff, max_rows, max_edges, n_edges, feat_dim, node_type,
+                       static_cast<uint16_t*>(node_feature), member_rows, edge_index, edge_type, edge_time, stream);
 }

@@ -6,7 +6,10 @@
 //     A*B  ~=  A_hi*B_hi + A_hi*B_lo + A_lo*B_hi            (dropped term ~2^-18 relative)
 // is accumulated in one fp32 register accumulator, three bf16 wgmma products per k-step.  P = 1 is the single bf16
 // product A_hi*B_hi (torch.set_float32_matmul_precision("medium")): a stage holds {A_hi, B_hi} only, so it is half the
-// size and the ring twice as deep.
+// size and the ring twice as deep.  P = 2 and P = 4 are the x3 product with one operand exact in bf16 (its lo half is
+// zero, so the product with it adds exact zeros and is skipped): P = 2, A exact, runs A_hi*B_hi + A_hi*B_lo from
+// {A_hi, B_hi, B_lo}; P = 4, B exact, runs A_hi*B_hi + A_lo*B_hi from {A_hi, A_lo, B_hi}.  The products that remain run
+// in the order P = 3 runs them, so the accumulator takes the same values.
 //
 // split3_tile<BN, MN, KB, OUT, P, Job>: the body of a persistent kernel (384 threads, at most one CTA per SM) whose CTAs walk the
 // 128 x BN output tiles blockIdx.x, blockIdx.x + gridDim.x, ...
@@ -149,12 +152,15 @@ constexpr uint32_t TMA_STAGE_BYTES = 2 * 2 * TMA_BUF_BYTES;
 constexpr uint32_t A32_BOX = BM * 32 * 4;         // one fp32 A box: 128 rows x 128 bytes, 16 KB
 template <int KB> constexpr uint32_t a_bytes() { return BM * KB * 2; }
 template <int KB> constexpr uint32_t atom_bytes() { return 64 * KB * 2; }
+// Which lo halves a product count P loads and multiplies.
+template <int P> constexpr bool has_a_lo() { return P == 3 || P == 4; }
+template <int P> constexpr bool has_b_lo() { return P == 3 || P == 2; }
 template <int KB, int P, bool AF = false> constexpr uint32_t b_offset() {                 // B_hi in a stage
-  return AF ? 2u * a_bytes<KB>() : (P == 3 ? 2u : 1u) * a_bytes<KB>();
+  return AF ? 2u * a_bytes<KB>() : (has_a_lo<P>() ? 2u : 1u) * a_bytes<KB>();
 }
 template <int BN, int KB = BK, int P = 3, bool AF = false> constexpr uint32_t stage_bytes() {
-  static_assert(P == 3 || P == 1, "three bf16 products (split) or one");
-  return b_offset<KB, P, AF>() + (P == 3 ? 2u : 1u) * (uint32_t)BN * KB * 2;
+  static_assert(P == 3 || P == 1 || ((P == 2 || P == 4) && !AF), "split (3), hi only (1), one exact operand (2, 4)");
+  return b_offset<KB, P, AF>() + (has_b_lo<P>() ? 2u : 1u) * (uint32_t)BN * KB * 2;
 }
 template <int BN, int KB = BK, uint32_t OUT = OUT_STAGE_BYTES, int P = 3, bool AF = false> constexpr int n_stages() {
   constexpr uint32_t left = SMEM_LIMIT - 1024 - OUT - 256;
@@ -201,7 +207,7 @@ inline unsigned persistent_grid(int tiles) {
 }
 
 // The P products of one k-block.  a_hi / a_lo: this warpgroup's 64-row A slab, 8-row groups A_SBO bytes apart; b_hi /
-// b_lo: the BN-column B tile (the lo halves are not read at P = 1).
+// b_lo: the BN-column B tile (a lo half is not read where P has none: has_a_lo / has_b_lo).
 template <int BN, bool MN, int KB, int P = 3, uint32_t A_SBO = 16 * KB>
 __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
   static_assert(!MN || KB == 64, "MN-major operands use 64-row k-blocks");
@@ -216,23 +222,17 @@ __device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_hi, uint32_t a
     const uint64_t bh = make_desc<KB>(b_hi + o, lbo), bl = make_desc<KB>(b_lo + o, lbo);
     if constexpr (BN == 64) {
       wgmma_n64<T, T>(acc, ah, bh);
-      if constexpr (P == 3) {
-        wgmma_n64<T, T>(acc, ah, bl);
-        wgmma_n64<T, T>(acc, al, bh);
-      }
+      if constexpr (has_b_lo<P>()) wgmma_n64<T, T>(acc, ah, bl);
+      if constexpr (has_a_lo<P>()) wgmma_n64<T, T>(acc, al, bh);
     } else {
       wgmma_n128<T, T>(acc, ah, bh);
-      if constexpr (P == 3) {
-        wgmma_n128<T, T>(acc, ah, bl);
-        wgmma_n128<T, T>(acc, al, bh);
-      }
+      if constexpr (has_b_lo<P>()) wgmma_n128<T, T>(acc, ah, bl);
+      if constexpr (has_a_lo<P>()) wgmma_n128<T, T>(acc, al, bh);
       if constexpr (BN == 256) {
         const uint64_t bh2 = make_desc<KB>(b_hi + o + b_half, lbo), bl2 = make_desc<KB>(b_lo + o + b_half, lbo);
         wgmma_n128<T, T>(acc + 64, ah, bh2);
-        if constexpr (P == 3) {
-          wgmma_n128<T, T>(acc + 64, ah, bl2);
-          wgmma_n128<T, T>(acc + 64, al, bh2);
-        }
+        if constexpr (has_b_lo<P>()) wgmma_n128<T, T>(acc + 64, ah, bl2);
+        if constexpr (has_a_lo<P>()) wgmma_n128<T, T>(acc + 64, al, bh2);
       }
     }
   }

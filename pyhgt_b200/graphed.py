@@ -21,6 +21,10 @@ GraphedForward replays an inference forward; GraphedTrainStep replays a whole tr
 backward, gradient clipping, optimizer step).  The backward's typed GEMMs carry their host-built tables in kernel
 parameters (csrc/linear_bwd.cu: k_upload), which is what lets a graph record them.
 
+A signature's `feat_dtype` (float32, or bfloat16 for the batches of sample_subgraph(s)_cuda(..., feature_dtype=
+torch.bfloat16)) is the dtype of the static feature buffer; batches of another dtype raise ValueError.  A bf16 buffer is
+filled through hgt_merge_batches_bf16 (device batches) or as 16-bit patterns (host batches: numpy has no bf16).
+
 Both classes also record at capture whether the typed GEMMs ran with one bf16 product
 (torch.set_float32_matmul_precision("medium"), autograd.bf16_matmuls): the graph holds those kernels, so a later call
 under a setting that picks the other ones raises ValueError.
@@ -33,9 +37,13 @@ from . import plan as _plan
 
 
 class GraphSignature:
-    """Static shape of a family of batches."""
+    """Static shape of a family of batches.  feat_dtype: the dtype of their node features, torch.float32 or
+    torch.bfloat16."""
 
-    def __init__(self, type_counts, n_edges, pairs, num_relations, feat_dim, use_time=True):
+    def __init__(self, type_counts, n_edges, pairs, num_relations, feat_dim, use_time=True, feat_dtype=torch.float32):
+        if feat_dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError("feat_dtype must be torch.float32 or torch.bfloat16, got %r" % (feat_dtype,))
+        self.feat_dtype = feat_dtype
         self.type_counts = [int(c) for c in type_counts]
         self.n_edges = int(n_edges)
         self.pairs = sorted({(int(s), int(r)) for s, r in pairs})
@@ -62,7 +70,11 @@ class GraphSignature:
 def pad_batch(sig, node_feature, node_type, edge_time, edge_index, edge_type, out=None):
     """Host tensors of one batch (type-contiguous node order) -> padded numpy arrays of the signature's shape and the
     new index of every real node.  `out` = (x, edge_time, edge_index, edge_type) numpy views to fill in place (pinned
-    staging).  Raises if the batch does not fit."""
+    staging).  Raises if the batch does not fit, or if node_feature's dtype is not sig.feat_dtype.  For a bf16
+    signature x holds the features' 16-bit patterns as int16 (numpy has no bf16; torch.from_numpy(x).view(torch.bfloat16)
+    reads them back)."""
+    if node_feature.dtype != sig.feat_dtype:
+        raise ValueError("node_feature is %s, the signature's feat_dtype is %s" % (node_feature.dtype, sig.feat_dtype))
     nt = node_type.numpy()
     if nt.size and np.any(nt[1:] < nt[:-1]):
         raise ValueError("pad_batch needs type-contiguous nodes (what to_torch emits)")
@@ -87,11 +99,12 @@ def pad_batch(sig, node_feature, node_type, edge_time, edge_index, edge_type, ou
     shift = sig.row0[:T] - old0[:T]
     new_id = np.arange(nt.size, dtype=np.int64) + shift[nt] if nt.size else np.zeros(0, dtype=np.int64)
     if out is None:
-        out = (np.empty((sig.n_nodes, sig.feat_dim), dtype=np.float32), np.empty(sig.n_edges, dtype=np.int64),
+        xdt = np.int16 if sig.feat_dtype == torch.bfloat16 else np.float32
+        out = (np.empty((sig.n_nodes, sig.feat_dim), dtype=xdt), np.empty(sig.n_edges, dtype=np.int64),
                np.empty((2, sig.n_edges), dtype=np.int64), np.empty(sig.n_edges, dtype=np.int64))
     x, etm, ei, ety = out
-    x.fill(0.0)
-    x[new_id] = node_feature.numpy()
+    x.fill(0)
+    x[new_id] = (node_feature.view(torch.int16) if sig.feat_dtype == torch.bfloat16 else node_feature).numpy()
     pad_node = sig.n_nodes - 1
     ei[0, :E] = new_id[src]
     ei[1, :E] = new_id[dst]
@@ -121,9 +134,9 @@ def device_batch_sizes(sig, node_feature, node_type, edge_time, edge_index, edge
     counts = plan.type_count[:T]
     if not sig.fits(counts, plan.n_edges, plan.pairs):
         raise _misfit(sig, counts, plan.n_edges)
-    if (node_feature is None or node_feature.dtype != torch.float32 or node_feature.dim() != 2 or node_feature.shape[0] != plan.n_nodes
+    if (node_feature is None or node_feature.dtype != sig.feat_dtype or node_feature.dim() != 2 or node_feature.shape[0] != plan.n_nodes
             or node_feature.shape[1] != sig.feat_dim):
-        raise ValueError("node_feature must be float32 [%d, %d], got %s %s" % (plan.n_nodes, sig.feat_dim,
+        raise ValueError("node_feature must be %s [%d, %d], got %s %s" % (sig.feat_dtype, plan.n_nodes, sig.feat_dim,
                                                                             getattr(node_feature, "dtype", None),
                                                                             tuple(getattr(node_feature, "shape", ()))))
     return counts, plan.n_edges
@@ -157,7 +170,7 @@ class _Graphed:
             dev = torch.device("cuda", torch.cuda.current_device())    # "cuda" -> "cuda:<n>": compared with tensors' devices
         self.sig, self.dev = sig, dev
         i64 = dict(dtype=torch.int64, device=dev)
-        self.x = torch.zeros((sig.n_nodes, sig.feat_dim), dtype=torch.float32, device=dev)
+        self.x = torch.zeros((sig.n_nodes, sig.feat_dim), dtype=sig.feat_dtype, device=dev)
         self.nt = torch.from_numpy(sig.node_type).to(dev)                 # static
         self.ei = torch.zeros((2, sig.n_edges), **i64)
         self.et = torch.zeros(sig.n_edges, **i64)
@@ -196,7 +209,8 @@ class _Graphed:
         if self.h is None:
             self.h = [torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in (self.x, self.tm, self.ei, self.et)]
         hx, htm, hei, het = self.h
-        new_id = pad_batch(self.sig, *batch, out=(hx.numpy(), htm.numpy(), hei.numpy(), het.numpy()))[5]
+        hx_np = (hx.view(torch.int16) if hx.dtype == torch.bfloat16 else hx).numpy()
+        new_id = pad_batch(self.sig, *batch, out=(hx_np, htm.numpy(), hei.numpy(), het.numpy()))[5]
         for h, dst in ((hx, self.x), (htm, self.tm), (hei, self.ei), (het, self.et)):
             dst.copy_(h, non_blocking=True)
         self._staged = torch.cuda.Event()
@@ -224,7 +238,8 @@ class _Graphed:
         d = up.to(self.dev)
         rows = torch.empty(n, dtype=torch.int64, device=self.dev)
         self.x.zero_()
-        _lib.call("hgt_merge_batches", d.ptr("mem"), 1, T, d.ptr("loc_off"), d.ptr("uoff"), n, E, sig.n_edges,
+        merge = "hgt_merge_batches_bf16" if sig.feat_dtype == torch.bfloat16 else "hgt_merge_batches"
+        _lib.call(merge, d.ptr("mem"), 1, T, d.ptr("loc_off"), d.ptr("uoff"), n, E, sig.n_edges,
                   sig.feat_dim, self.nt.data_ptr(), self.x.data_ptr(), rows.data_ptr(), self.ei.data_ptr(),
                   self.et.data_ptr(), self.tm.data_ptr(), self.stream.cuda_stream)
         self.ei[:, E:].fill_(sig.n_nodes - 1)

@@ -6,6 +6,12 @@ The adapter is the same "per-type linear dispatch" as inside HGTConv and runs th
 (``hgt_typed_linear``: tensor cores when in_dim >= 64 and n_hid % 16 == 0, fp32 SIMT otherwise); every layer shares
 the one cached graph plan.  Under autograd the adapter uses the same GEMM with its native backward
 (``autograd._TypedLinear``).
+
+``node_feature`` may be float32 or bfloat16 (e.g. the batches of ``sample_subgraph(s)_cuda(..., feature_dtype=
+torch.bfloat16)``).  bf16 features are the adapter GEMM's bf16 operand as they are (hgt_typed_linear_bf16a, and
+hgt_typed_linear_bwd_bf16a for dW in training): no fp32 copy, no split.  A bf16 value is exactly the hi half of the
+split-bf16 scheme with a zero lo half, so every output, loss and gradient equals that of ``node_feature.float()``
+bitwise.  bf16 features take no gradient.
 """
 import torch
 import torch.nn as nn
@@ -61,7 +67,9 @@ class GNN(nn.Module):
         dev, N = node_feature.device, plan.n_nodes
         st = torch.cuda.current_stream().cuda_stream
         x = node_feature.contiguous()
-        if not plan.sorted_types:
+        if not plan.sorted_types and x.dtype == torch.bfloat16:
+            x = x.index_select(0, plan.perm.long())
+        elif not plan.sorted_types:
             xs = torch.empty_like(x)
             _lib.call("hgt_gather_rows", x.data_ptr(), plan.perm.data_ptr(), N, self.in_dim, xs.data_ptr(), st)
             x = xs
@@ -123,11 +131,18 @@ class GNN(nn.Module):
         without reading anything back (its pairs come from the batch's cached plan, which sample_subgraph(s)_cuda,
         merge_batches and the graphed classes leave), so the call can be captured in a CUDA graph.  Rows are padded to
         the bounds; padding changes no real row.  If a (type, hop) class of the batch exceeds its bound or an out_nodes id
-        is out of range, every returned row is NaN and the layout's check() raises (trim.get_layout(...).check())."""
+        is out of range, every returned row is NaN and the layout's check() raises (trim.get_layout(...).check()).
+
+        `node_feature` is float32 or bfloat16 (ValueError otherwise); bf16 features must not require grad."""
         grad = torch.is_grad_enabled() and (node_feature.requires_grad or any(p.requires_grad for p in self.parameters()))
         if not node_feature.is_cuda:
             raise _lib.HgtError("pyhgt_b200.GNN runs on CUDA tensors only (got %s): there is no CPU fallback"
                                 % node_feature.device)
+        if node_feature.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError("node_feature must be float32 or bfloat16, got %s" % (node_feature.dtype,))
+        if node_feature.dtype == torch.bfloat16 and node_feature.requires_grad:
+            raise ValueError("bf16 node_feature cannot require grad: features are data, and the adapter offers no bf16 "
+                             "input gradient")
         if out_nodes is not None:
             return self._forward_trimmed(node_feature, node_type, edge_time, edge_index, edge_type, out_nodes, grad,
                                          trim_signature)
@@ -153,7 +168,7 @@ class GNN(nn.Module):
             raise ValueError("node_feature must be [N, in_dim] with N = len(node_type), got %s"
                              % (tuple(node_feature.shape),))
         if out_nodes.numel() == 0:
-            return node_feature.new_zeros((0, self.n_hid))
+            return node_feature.new_zeros((0, self.n_hid), dtype=torch.float32)
         conv0 = self.gcs[0].base_conv
         tm = edge_time if conv0.use_RTE else None
         pairs = None

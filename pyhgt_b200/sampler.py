@@ -861,7 +861,8 @@ class _Upload:
         return (self.d[o:].view(torch.int32) if dtype == np.int32 else self.d[o:])[:n]
 
 
-def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None, edge_mask=None):
+def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None, edge_mask=None,
+                         feature_dtype=None):
     """HGSampling (pyHGT/data.py:87-210) and ``to_torch`` (data.py:212-256) on the GPU.
 
     Same distribution over sampled node sets, their times and their order as ``sample_subgraph`` (the host sampler,
@@ -882,15 +883,22 @@ def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp,
     from the DeviceGraph's feature tables, None without them), and per sampled type (in ``layer_data`` key order) the
     sampled ids (``indxs``) and times in ``ser`` order, as device tensors.  The sync-free plan of the graph is built.
     Host synchronisation: one small read-back per sampling layer (the type order) and one at the end.  This is
-    ``sample_subgraphs_cuda`` with one seed dict."""
-    return sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, [inp], generator, edge_mask)[0]
+    ``sample_subgraphs_cuda`` with one seed dict.
+
+    ``feature_dtype`` (None = torch.float32): the dtype of ``node_feature``.  torch.bfloat16 needs a graph built with
+    ``feature_dtype=torch.bfloat16`` (ValueError otherwise: rounding is the DeviceGraph's decision) and copies each stored
+    row as it is, half the bytes of the float32 batch, whose values are the exact widenings of these.  Everything else the
+    call returns, and the cached plan, is what the float32 call returns."""
+    return sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, [inp], generator, edge_mask,
+                                 feature_dtype)[0]
 
 
-def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inps, generator=None, edge_mask=None):
+def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inps, generator=None, edge_mask=None,
+                          feature_dtype=None):
     """B = len(inps) subgraphs in one device pass: the device equivalent of the reference's pool of ``sample_subgraph``
     calls (ogbn-mag/train_ogbn_mag.py:82-102, the variance-reduced evaluation's ``vr_num`` samples around the same seeds).
     ``edge_mask`` (see ``sample_subgraph_cuda``) applies to every member; it acts in the rebuild's count and write passes
-    and adds no launch and no read-back.
+    and adds no launch and no read-back.  ``feature_dtype`` is as for ``sample_subgraph_cuda``.
 
     Returns a list of B tuples, each with the shape and meaning of ``sample_subgraph_cuda``'s; the tensors are views into
     buffers shared by the batch, and each member's sync-free plan is built.  Member b's Philox seed is the b-th of B
@@ -912,6 +920,7 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     from . import plan as _plan
     dg = dgraph
     dev = dg.device
+    bf16_out = _batch_feature_dtype(dg, feature_dtype) == torch.bfloat16
     W = int(sampled_number)
     depth = int(sampled_depth)
     if W <= 0 or depth < 0:
@@ -1177,8 +1186,10 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     self_rel = dg.edge_dict['self']
     node_type = torch.empty(N, **i64)
     node_time = torch.empty(N, **i64)
-    node_feature = torch.empty((N, dg.feat_dim), dtype=torch.float32, device=dev) if dg.features is not None else None
+    node_feature = (torch.empty((N, dg.feat_dim), dtype=torch.bfloat16 if bf16_out else torch.float32, device=dev)
+                    if dg.features is not None else None)
     # bf16 tables: the write pass leaves the features out, and hgt_gsample_gather_features_bf16 widens the rows after it
+    # (hgt_gsample_gather_rows_bf16 copies them as they are for a bf16 batch)
     bf16 = node_feature is not None and dg.feature_dtype == torch.bfloat16
     fp32_feature = None if bf16 else node_feature
     edge_index = torch.empty(2 * E, **i64)                # member b's [2, E_b] block at 2 * edge_base[b]
@@ -1206,8 +1217,9 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
         # output rows are member after member, type slot after type slot, ser order: the sampled ids in that order
         row_id = torch.cat([lid[int(lid_off[b, t]):int(lid_off[b, t] + nl[b, t])]
                             for b in range(B) for t in range(T) if nl[b, t]])
-        _lib.call("hgt_gsample_gather_features_bf16", _lib.ptr(dg.feat_ptrs), dg.feat_dim, node_type.data_ptr(),
-                  row_id.data_ptr(), N, node_feature.data_ptr(), st)
+        _lib.call("hgt_gsample_gather_rows_bf16" if bf16_out else "hgt_gsample_gather_features_bf16",
+                  _lib.ptr(dg.feat_ptrs), dg.feat_dim, node_type.data_ptr(), row_id.data_ptr(), N,
+                  node_feature.data_ptr(), st)
 
     out = []
     for b in range(B):
@@ -1227,6 +1239,20 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
         out.append((node_feature[n0:n1] if node_feature is not None else None, nt, etime, ei, et, node_dict,
                     dict(dg.edge_dict), indxs, times))
     return out
+
+
+def _batch_feature_dtype(dg, feature_dtype):
+    """The node_feature dtype of a batch sampled from `dg` with `feature_dtype` (None: float32); ValueError when the graph
+    cannot give it."""
+    import torch
+    if feature_dtype is None or feature_dtype == torch.float32:
+        return torch.float32
+    if feature_dtype != torch.bfloat16:
+        raise ValueError("feature_dtype must be None, torch.float32 or torch.bfloat16, got %r" % (feature_dtype,))
+    if dg.feature_dtype != torch.bfloat16:
+        raise ValueError("bf16 batches need a DeviceGraph built with feature_dtype=torch.bfloat16 (its tables are %s): "
+                         "the graph decides how features are rounded" % (dg.feature_dtype,))
+    return torch.bfloat16
 
 
 def _member_layout(dg, nl, ts, tot):
@@ -1288,7 +1314,8 @@ def merge_batches(batches, num_types, num_relations):
     The union is type-major, so its ``node_type`` is sorted and the layers take their sorted, sync-free paths; edges
     keep their order, member after member.  Returns ``(node_feature, node_type, edge_time, edge_index, edge_type,
     member_rows)`` with ``member_rows[b]`` the union rows of member b's nodes in member order (``out[member_rows[b]]`` is
-    member b's output).  node_feature is None when the members have none.
+    member b's output).  node_feature is None when the members have none; it is float32 or bfloat16, the dtype of the
+    members' features, which must all have the same one (ValueError otherwise).
 
     Per-type counts and <source type, relation> pairs come from each member's cached plan (the samplers and
     ``to_torch(prebuild_plan=True)`` build one), so there is no device read-back; a member whose plan has left the plan
@@ -1305,14 +1332,20 @@ def merge_batches(batches, num_types, num_relations):
         raise ValueError("either every batch has node features or none has")
     with_feat = feats[0] is not None
     F = int(feats[0].shape[1]) if with_feat else 0
+    fdt = feats[0].dtype if with_feat else torch.float32
+    if fdt not in (torch.float32, torch.bfloat16):
+        raise ValueError("node features must be float32 or bfloat16, got %s" % (fdt,))
+    if with_feat and any(f.dtype != fdt for f in feats):
+        raise ValueError("node features of all batches must have the same dtype, got %s"
+                         % sorted({str(f.dtype) for f in feats}))
     plans, keep = [], []
     for bt in batches:
         nf, nt, etime, ei, et = bt[:5]
         p = _plan.get_plan(nt, ei, et, etime, T, R)
         if not p.sorted_types or p.type_count[T] != 0:
             raise ValueError("merge_batches needs batches whose node_type is sorted (the to_torch layout)")
-        if with_feat and (nf.dtype != torch.float32 or nf.dim() != 2 or nf.shape[1] != F or nf.shape[0] != p.n_nodes):
-            raise ValueError("node features must be float32 [N, %d] in every batch" % F)
+        if with_feat and (nf.dim() != 2 or nf.shape[1] != F or nf.shape[0] != p.n_nodes):
+            raise ValueError("node features must be [N, %d] in every batch" % F)
         plans.append(p)
         keep.append((nf.contiguous() if with_feat else None, ei.contiguous(), et.contiguous(), etime.contiguous()))
     loc_off, uoff, node_base, edge_base, union_count = union_layout([p.type_count[:T] for p in plans],
@@ -1330,12 +1363,12 @@ def merge_batches(batches, num_types, num_relations):
     N, E = int(node_base[-1]), int(edge_base[-1])
     i64 = dict(dtype=torch.int64, device=dev)
     node_type = torch.empty(N, **i64)
-    node_feature = torch.empty((N, F), dtype=torch.float32, device=dev) if with_feat else None
+    node_feature = torch.empty((N, F), dtype=fdt, device=dev) if with_feat else None
     rows = torch.empty(N, **i64)
     edge_index = torch.empty((2, E), **i64)
     edge_type = torch.empty(E, **i64)
     edge_time = torch.empty(E, **i64)
-    _lib.call("hgt_merge_batches", d.ptr("mem"), B, T, d.ptr("loc_off"), d.ptr("uoff"),
+    _lib.call("hgt_merge_batches_bf16" if fdt == torch.bfloat16 else "hgt_merge_batches", d.ptr("mem"), B, T, d.ptr("loc_off"), d.ptr("uoff"),
               int(loc_off[:, T].max()), int(max(p.n_edges for p in plans)), E, F, node_type.data_ptr(),
               _lib.ptr(node_feature), rows.data_ptr(), edge_index.data_ptr(), edge_type.data_ptr(),
               edge_time.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
