@@ -1094,6 +1094,25 @@ int hgt_merge_batches_bf16(const hgt_merge_member* members, int32_t n_members, i
                            int64_t* node_type, void* node_feature, int64_t* member_rows, int64_t* edge_index,
                            int64_t* edge_type, int64_t* edge_time, void* stream);
 
+/* Device-side build of one adjacency block from an edge array (sampler.py: DeviceGraph.from_edges).  Edge i, in array
+ * order, sets d[tgt[i]][src[i]] = time[i] in a dict of dicts; the block is that dict in the CSR form of
+ * hgt_gsample_block: rows in order of each target's first appearance, a row's neighbours in order of the pair's first
+ * appearance, a repeated pair keeping its first place and its last time.  tgt / src / time [n_edges] are DEVICE int64
+ * arrays (ids in [0, tgt_max] / [0, src_max]); time may be NULL (every time is None).  n_edges < 2^31.
+ * hgt_ingest_block_sort sorts the edges in the workspace and writes stats [4] (DEVICE int64): the number of rows, the
+ * number of entries (distinct pairs), and the least and greatest kept time (INT64_MAX / INT64_MIN when there is none or
+ * time is NULL).  The caller reads them back, chooses the block's width and allocates its arrays; then
+ * hgt_ingest_block_write, given the same tgt / src / time, the stats' counts and the same workspace (once per sort),
+ * writes row_of [n_row_of] (>= tgt_max + 1 entries, -1 = no row), ptr [n_rows + 1], nbr and time_out [n_entries]: int32
+ * arrays with INT32_MIN for a NULL time when narrow != 0 (HGT_BLOCK_NARROW), int64 with no_time otherwise.  Values are
+ * not range-checked against the width.  workspace: hgt_ingest_workspace_bytes(n_edges), 48 bytes per edge + CUB scratch. */
+int hgt_ingest_workspace_bytes(int64_t n_edges, size_t* out_bytes);
+int hgt_ingest_block_sort(const int64_t* tgt, const int64_t* src, const int64_t* time, int64_t n_edges, int64_t tgt_max,
+                          int64_t src_max, int64_t* stats, void* workspace, size_t workspace_bytes, void* stream);
+int hgt_ingest_block_write(const int64_t* tgt, const int64_t* src, const int64_t* time, int64_t n_edges, int64_t n_rows,
+                           int64_t n_entries, int32_t narrow, int64_t no_time, void* row_of, int64_t n_row_of, void* ptr,
+                           void* nbr, void* time_out, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

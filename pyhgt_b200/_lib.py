@@ -155,6 +155,10 @@ SIGNATURES = {
     "hgt_typed_linear_bf16a": [_p, _i64, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i32, _p, _sz, _p],
     "hgt_typed_linear_bwd_bf16a": [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _i32, _p, _p, _p, _i32, _p, _sz, _p],
     "hgt_typed_linear_bwd_bf16a_det": [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _i32, _p, _p, _p, _i32, _p, _sz, _p],
+    # the sampler's graph built on the device from typed edge arrays (sampler.DeviceGraph.from_edges)
+    "hgt_ingest_workspace_bytes": [_i64, _c.POINTER(_sz)],
+    "hgt_ingest_block_sort": [_p, _p, _p, _i64, _i64, _i64, _p, _p, _sz, _p],
+    "hgt_ingest_block_write": [_p, _p, _p, _i64, _i64, _i64, _i32, _i64, _p, _i64, _p, _p, _p, _p, _sz, _p],
     # trimmed forward (GNN.forward(out_nodes=), trim.py)
     "hgt_trim_layout": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_trim_layout_bounded": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _i64, _p, _p, _p, _p, _p,

@@ -48,6 +48,19 @@ class _CState(_c.Structure):                 # hgt_sampler_state
                 ("layer_seq", _c.c_int64), ("budget_seq", _c.c_int64)]
 
 
+def _fits_narrow(n_keys, total, nbr_range, tgt_range, time_range):
+    """Whether a block of n_keys rows and total entries is narrow (see _NARROW_MAX), given the (min, max) of its
+    neighbour ids, target ids and non-None times (None where there are none)."""
+    lo, hi = -_NARROW_MAX - 1, _NARROW_MAX
+    if total > hi or n_keys > hi:
+        return False
+    if nbr_range is not None and (nbr_range[0] < lo or nbr_range[1] > hi):
+        return False
+    if tgt_range is not None and (tgt_range[0] < lo or tgt_range[1] > hi):
+        return False
+    return time_range is None or (time_range[0] >= -hi and time_range[1] <= hi)
+
+
 class _Block:
     """One <target type, source type, relation> adjacency in CSR form, dict insertion order preserved.  ``row_of`` /
     ``ptr`` / ``nbr`` / ``time`` are int32 when the block is ``narrow`` (see _NARROW_MAX; a None time is then _NO_TIME32)
@@ -73,7 +86,10 @@ class _Block:
             self.time = np.fromiter((_NO_TIME if v is None else v for adl in adls for v in adl.values()),
                                     dtype=np.int64, count=total)
         self.has_none = has_none
-        self.narrow = self._fits_narrow(n_keys, total, tesr)
+        tm = self.time[self.time != _NO_TIME] if has_none else self.time
+        self.narrow = _fits_narrow(n_keys, total, (int(self.nbr.min()), int(self.nbr.max())) if total else None,
+                                   (min(tesr), max(tesr)) if n_keys else None,
+                                   (int(tm.min()), int(tm.max())) if tm.size else None)
         if self.narrow:
             self.row_of, self.ptr, self.nbr = (a.astype(np.int32) for a in (self.row_of, self.ptr, self.nbr))
             t32 = self.time.astype(np.int32)
@@ -84,17 +100,6 @@ class _Block:
         self.time_addr = self.time.ctypes.data
         self.ptr_list = self.ptr.tolist()                  # plain ints: the per-node lookups stay out of numpy
         self.row_list = self.row_of.tolist()
-
-    def _fits_narrow(self, n_keys, total, tesr):
-        lo, hi = -_NARROW_MAX - 1, _NARROW_MAX
-        if total > hi or n_keys > hi:
-            return False
-        if total and (int(self.nbr.min()) < lo or int(self.nbr.max()) > hi):
-            return False
-        if n_keys and (min(tesr) < lo or max(tesr) > hi):
-            return False
-        tm = self.time[self.time != _NO_TIME] if self.has_none else self.time
-        return not tm.size or (int(tm.min()) >= -hi and int(tm.max()) <= hi)
 
     def span(self, a, b):
         """nbr[a:b] and time[a:b] as int64, None times as _NO_TIME, at either width."""
@@ -576,17 +581,25 @@ def _grow_state_room(dg, restarts):
 
 
 def _pin(a, dtype):
-    """One page-locked copy of array ``a`` (as ``dtype``), mapped for the device: (host view, device address, page-aligned
-    buffer to unregister).  The buffer is whole pages of its own, so no two registrations share a page."""
+    """One page-locked copy of array ``a`` (as ``dtype``; a torch tensor, on any device, must have that dtype already),
+    mapped for the device: (host view, device address, page-aligned buffer to unregister).  The buffer is whole pages of
+    its own, so no two registrations share a page."""
+    import torch
     from . import _lib
-    a = np.asarray(a, dtype=dtype)
-    nbytes = max(a.nbytes, 1)
+    tensor = a if isinstance(a, torch.Tensor) else None
+    if tensor is None:
+        a = np.asarray(a, dtype=dtype)
+    shape, nb = tuple(a.shape), int(np.prod(a.shape, dtype=np.int64)) * np.dtype(dtype).itemsize
+    nbytes = max(nb, 1)
     size = -(-nbytes // _PAGE) * _PAGE
     raw = np.empty(size + _PAGE, dtype=np.uint8)
     off = (-raw.ctypes.data) % _PAGE
     buf = raw[off:off + size]
-    view = buf[:a.nbytes].view(dtype).reshape(a.shape)
-    view[...] = a
+    view = buf[:nb].view(dtype).reshape(shape)
+    if tensor is None:
+        view[...] = a
+    else:
+        torch.from_numpy(view).copy_(tensor)
     dptr = _c.c_void_p()
     _lib.call("hgt_host_register", buf.ctypes.data, size, _c.byref(dptr))
     return view, dptr.value, buf
@@ -635,6 +648,82 @@ def _grow_hit_room(dg, n_hits, n_count):
         dg.hit_room = max(dg.hit_room, 1.25 * n_hits / n_count)
 
 
+def _edge_dict(meta):
+    """Relation ids of a meta graph [(target type, source type, relation)] (pyHGT/data.py:237-238), plus 'self'."""
+    edge_dict = {e[2]: i for i, e in enumerate(meta)}
+    edge_dict['self'] = len(edge_dict)
+    return edge_dict
+
+
+def _ingest_plan(edges, slot, reverse):
+    """The validated keys of ``DeviceGraph.from_edges`` and the order of their blocks.  Each key is a dict: edge_index,
+    time, E, range ((min, max) of the source ids, of the target ids; (0, -1) when empty) and blocks [((target type,
+    source type, relation), row of edge_index holding its target ids)].  The order lists every (target type, source
+    type, relation) as the dict graph's edge_list walk meets it: the preprocessing loop touches edge_list[t][s][r] and
+    then edge_list[s][t]['rev_' + r], key by key, and nested dicts keep first-touch order."""
+    import torch
+    keys, nested = [], {}
+    for item in edges:
+        try:
+            key, ei, tm = item
+            s_t, r, t_t = key
+        except (TypeError, ValueError):
+            raise ValueError("edges holds ((source_type, relation, target_type), edge_index, time) items, got %r"
+                             % (item,)) from None
+        for ty in (s_t, t_t):
+            if ty not in slot:
+                raise KeyError("node type %r of key %r is not in types" % (ty, key))
+        if not isinstance(ei, torch.Tensor) or ei.dtype != torch.int64 or ei.dim() != 2 or ei.shape[0] != 2:
+            raise ValueError("edge_index of %r must be an int64 [2, E] tensor, got %s" % (
+                key, "%s %s" % (ei.dtype, list(ei.shape)) if isinstance(ei, torch.Tensor) else type(ei).__name__))
+        n = int(ei.shape[1])
+        if tm is not None and (not isinstance(tm, torch.Tensor) or tm.dtype != torch.int64 or tm.dim() != 1 or
+                               tm.shape[0] != n):
+            raise ValueError("time of %r must be None or an int64 [%d] tensor, got %s" % (
+                key, n, "%s %s" % (tm.dtype, list(tm.shape)) if isinstance(tm, torch.Tensor) else type(tm).__name__))
+        if n > 2 ** 31 - 1:
+            raise ValueError("key %r has %d edges; a block is built from at most 2^31 - 1" % (key, n))
+        if reverse and not isinstance(r, str):
+            raise ValueError("reverse=True names the twin of relation %r 'rev_' + relation: it must be a str" % (r,))
+        blocks = [((t_t, s_t, r), 1)] + ([((s_t, t_t, 'rev_' + r), 0)] if reverse else [])
+        for blk, _ in blocks:
+            rels = nested.setdefault(blk[0], {}).setdefault(blk[1], {})
+            if blk[2] in rels:
+                raise ValueError("block %r (target type, source type, relation) is made by two keys" % (blk,))
+            rels[blk[2]] = True
+        keys.append({"edge_index": ei, "time": tm, "E": n, "blocks": blocks})
+    for k in keys:                                         # every id is checked before any block is built
+        k["range"] = ((0, -1), (0, -1))
+        if k["E"]:
+            lo, hi = (v.tolist() for v in torch.aminmax(k["edge_index"], dim=1))
+            if min(lo) < 0:
+                raise ValueError("negative node id %d in edges" % min(lo))
+            if max(hi) >= _ID_LIMIT:
+                raise ValueError("node ids must be below 2^40, got %d" % max(hi))
+            k["range"] = ((lo[0], hi[0]), (lo[1], hi[1]))
+    order = [(t, s, r) for t, d1 in nested.items() for s, d2 in d1.items() for r in d2]
+    return keys, order
+
+
+def _ingest_n_ids(keys, order):
+    """FrozenGraph's id ranges for the blocks of ``_ingest_plan``: ({block: length of its row_of}, {type: n_ids}).  A
+    block's row_of spans its target type's largest target id, plus the neighbour ids of that type's blocks met before
+    it in the walk (FrozenGraph.__init__)."""
+    info = {blk: (k["E"], k["range"][tr][1], k["range"][1 - tr][1]) for k in keys for blk, tr in k["blocks"]}
+    n_ids = {}
+    for blk in order:
+        n, tgt_max, _ = info[blk]
+        if n:
+            n_ids[blk[0]] = max(n_ids.get(blk[0], 0), tgt_max + 1)
+    row_len = {}
+    for blk in order:
+        n, _, nbr_max = info[blk]
+        row_len[blk] = n_ids.get(blk[0], 0)
+        if n:
+            n_ids[blk[1]] = max(n_ids.get(blk[1], 0), nbr_max + 1)
+    return row_len, n_ids
+
+
 class DeviceGraph:
     """A ``FrozenGraph`` made readable by a CUDA device for ``sample_subgraph_cuda``: the CSR blocks (neighbour ids and
     edge times in dict order, id -> row maps) and, optionally, per-type feature tables ``{type: Tensor[n_ids, F]}``
@@ -656,11 +745,114 @@ class DeviceGraph:
     ``graph_bytes`` reports the bytes the graph's arrays hold.
 
     Node types are laid out in ``graph.get_types()`` order (as ``to_torch`` does), so every type of the graph's
-    ``edge_list`` must be one of them; relation names come from ``graph.get_meta_graph()`` plus ``'self'``."""
+    ``edge_list`` must be one of them; relation names come from ``graph.get_meta_graph()`` plus ``'self'``.
+
+    ``DeviceGraph.from_edges`` builds the same graph on the device from typed edge arrays, with no reference ``Graph``
+    (``fg`` is then None)."""
 
     PLACEMENTS = ("device", "host")
 
     def __init__(self, frozen_graph, device, features=None, placement="device", feature_dtype=None):
+        fg = frozen_graph if isinstance(frozen_graph, FrozenGraph) else FrozenGraph(frozen_graph)
+        graph = fg.graph
+        self._setup(graph.get_types(), device, placement, feature_dtype)
+        self.fg = fg
+        missing = [t for t in fg.types if t not in self.slot]
+        if missing:
+            raise KeyError("node types %r occur in edge_list but not in graph.get_types()" % (missing,))
+        self.edge_dict = _edge_dict(graph.get_meta_graph())
+        self.n_ids = [fg.n_ids.get(t, 0) for t in self.types]
+        host = self.placement == "host"
+        with self._placing():
+            if host:
+                fg._cblocks = {}    # the host sampler's cached block tables hold the addresses of arrays rebound below
+            for t_t, tes in fg.blocks.items():
+                for s_t, rels in tes.items():
+                    for r, blk in rels.items():
+                        if r not in self.edge_dict:
+                            raise KeyError("relation %r of edge_list is not in graph.get_meta_graph()" % (r,))
+                        placed = [self._place(a) for a in (blk.row_of, blk.ptr, blk.nbr, blk.time)]
+                        if host:                           # the FrozenGraph reads the pinned copies: one copy each
+                            blk.row_of, blk.ptr, blk.nbr, blk.time = (kept for kept, _ in placed)
+                            blk.nbr_addr, blk.time_addr = blk.nbr.ctypes.data, blk.time.ctypes.data
+                        self._add_block(t_t, s_t, r, placed, blk.narrow)
+            self._finish(features)
+
+    @classmethod
+    def from_edges(cls, edges, types, device, *, reverse=True, features=None, placement="device", feature_dtype=None):
+        """The DeviceGraph of typed edge arrays, built on the device (csrc/ingest.cu) with no per-edge host work.
+
+        ``edges``: an ordered sequence of ``((source_type, relation, target_type), edge_index, time)`` (OGB's
+        ``edge_index_dict`` convention): ``edge_index`` an int64 [2, E] CPU or CUDA tensor, row 0 the source ids and row 1
+        the target ids; ``time`` an int64 [E] tensor, or None for a relation without times (every time None).  ``types``
+        is the node-type list in ``graph.get_types()`` order: it fixes the batch layout.  ``reverse=True`` adds the
+        ``'rev_' + relation`` twin of every key, as ``Graph.add_edge`` does (pyHGT/data.py:59-61).  ``features``,
+        ``placement`` and ``feature_dtype`` are as for ``DeviceGraph(...)``.
+
+        The result equals ``DeviceGraph(FrozenGraph(g), ...)`` bitwise, where ``g`` is the dict graph the ogbn-mag
+        preprocessing loop (preprocess_ogbn_mag.py:29-42) makes from the same arrays: key by key, per edge in array order,
+        ``edge_list[t][s][r][target][source] = time`` and, with ``reverse``, ``edge_list[s][t]['rev_' + r][source][target]
+        = time``.  So: blocks in the order that loop first touches them (empty ones included), relation ids from that
+        meta graph plus ``'self'``, rows by a target's first appearance, neighbours by a pair's first appearance with the
+        last time written, ``row_of`` lengths and ``n_ids`` by FrozenGraph's rule, and each block's width by the same
+        narrow rule.
+
+        Device memory: the edges of one key (24 bytes per edge with times, copied in when they are CPU tensors), a
+        workspace of 48 bytes per edge of the largest key plus sort scratch, and the blocks themselves on device
+        placement; on host placement each finished block is copied into pinned memory and its device arrays are dropped.
+        One 32-byte read-back per block (its row and entry counts decide its width); the build is not meant for capture.
+
+        There is no reference ``Graph`` behind the result: ``fg`` is None, and the host sampler ``sample_subgraph``, which
+        replays the reference's numpy stream over a FrozenGraph, does not apply to it.  Raises KeyError for a key type
+        not in ``types`` and ValueError for repeated blocks, malformed arrays, negative ids or ids of 2^40 or more,
+        before any kernel builds a block."""
+        import torch
+        from . import _lib
+        self = cls.__new__(cls)
+        self._setup(types, device, placement, feature_dtype)
+        self.fg = None
+        if len(set(self.types)) != len(self.types):
+            raise ValueError("types must be distinct, got %r" % (self.types,))
+        keys, order = _ingest_plan(edges, self.slot, reverse)
+        self.edge_dict = _edge_dict(order)
+        row_len, n_ids = _ingest_n_ids(keys, order)
+        self.n_ids = [n_ids.get(t, 0) for t in self.types]
+        dev = self.device
+        built = {}
+        with self._placing():
+            ws_edges = max([k["E"] for k in keys] + [0])
+            ws_n = _c.c_size_t()
+            _lib.call("hgt_ingest_workspace_bytes", ws_edges, _c.byref(ws_n))
+            ws = torch.empty(max(ws_n.value, 1), dtype=torch.uint8, device=dev)
+            stats = torch.empty(4, dtype=torch.int64, device=dev)
+            st = torch.cuda.current_stream(dev).cuda_stream
+            for k in keys:
+                ei = k["edge_index"].to(device=dev).contiguous()
+                tm = k["time"].to(device=dev).contiguous() if k["time"] is not None else None
+                for blk, tr in k["blocks"]:
+                    tgt, src = ei[tr], ei[1 - tr]
+                    tgt_rng, nbr_rng = k["range"][tr], k["range"][1 - tr]
+                    _lib.call("hgt_ingest_block_sort", tgt.data_ptr(), src.data_ptr(), _lib.ptr(tm), k["E"],
+                              max(tgt_rng[1], 0), max(nbr_rng[1], 0), stats.data_ptr(), ws.data_ptr(), ws.numel(), st)
+                    rows, total, t_lo, t_hi = stats.tolist()
+                    narrow = _fits_narrow(rows, total, nbr_rng if total else None, tgt_rng if rows else None,
+                                          (t_lo, t_hi) if tm is not None and total else None)
+                    dt = torch.int32 if narrow else torch.int64
+                    arrays = [torch.empty(n, dtype=dt, device=dev) for n in (row_len[blk], rows + 1, total, total)]
+                    _lib.call("hgt_ingest_block_write", tgt.data_ptr(), src.data_ptr(), _lib.ptr(tm), k["E"], rows,
+                              total, int(narrow), _NO_TIME, *(a.data_ptr() for a in arrays[:1]), row_len[blk],
+                              *(a.data_ptr() for a in arrays[1:]), ws.data_ptr(), ws.numel(), st)
+                    built[blk] = ([self._place(a) for a in arrays], narrow)
+                del ei, tm
+            del ws
+            for blk in order:
+                self._add_block(*blk, *built.pop(blk))
+            self._finish(features)
+        return self
+
+    def _setup(self, types, device, placement, feature_dtype):
+        """What both constructors set before the blocks: the node-type layout, placement and feature dtype (validated),
+        and the empty lists _place / _add_block fill."""
         if placement not in self.PLACEMENTS:
             raise ValueError("placement must be one of %s, got %r" % (self.PLACEMENTS, placement))
         import torch
@@ -668,74 +860,63 @@ class DeviceGraph:
         if feature_dtype not in (torch.float32, torch.bfloat16):
             raise ValueError("feature_dtype must be torch.float32 or torch.bfloat16, got %r" % (feature_dtype,))
         self.feature_dtype = feature_dtype
-        fg = frozen_graph if isinstance(frozen_graph, FrozenGraph) else FrozenGraph(frozen_graph)
-        self.fg, self.device = fg, torch.device(device)
+        self.device = torch.device(device)
         if self.device.type != "cuda":
             raise ValueError("DeviceGraph needs a CUDA device, got %s" % self.device)
-        graph = fg.graph
-        self.types = list(graph.get_types())
+        self.types = list(types)
         self.slot = {t: i for i, t in enumerate(self.types)}
-        missing = [t for t in fg.types if t not in self.slot]
-        if missing:
-            raise KeyError("node types %r occur in edge_list but not in graph.get_types()" % (missing,))
-        self.edge_dict = {e[2]: i for i, e in enumerate(graph.get_meta_graph())}     # data.py:237-238
-        self.edge_dict['self'] = len(self.edge_dict)
-        self.n_ids = [fg.n_ids.get(t, 0) for t in self.types]
         self.placement = placement
         self.hit_room = _HIT_ROOM
         self.state_room = _STATE_ROOM
         self.sampler_state = None     # the last sample_subgraphs_cuda call's {layout, entries, load, restarts}
-        dev = self.device
-        host = placement == "host"
+        self._keep = []               # every array the kernels read (device tensors or pinned host views)
+        self._pinned = []             # page-aligned buffers registered with CUDA
+        self.blocks = []              # (target slot, source slot, relation) in dict order
+        self._adjacency = []          # the block arrays the kernels read (for graph_bytes)
+        self._cblocks = []
+        if placement == "host":
+            weakref.finalize(self, _unpin, self.device, self._pinned)
 
-        def up(a):
-            return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(dev)
+    def _placing(self):
+        """Context of the placement: host registrations are made on this graph's device."""
+        import torch
+        return torch.cuda.device(self.device) if self.placement == "host" else contextlib.nullcontext()
 
-        self._keep = []
-        pinned = []                                       # page-aligned buffers registered with CUDA
-
-        def place(a, dtype=None):
-            """Address the kernels read array ``a`` (as ``dtype``, default its own) at; the array (device tensor or pinned
-            host view) is kept."""
-            dtype = a.dtype if dtype is None else dtype
+    def _place(self, a, dtype=None):
+        """(kept array, address the kernels read it at) for array ``a``: a numpy array (as ``dtype``, default its own) is
+        uploaded to the device or pinned on the host, a device tensor is kept as it is or copied into pinned host memory,
+        as ``placement`` says.  The array is kept."""
+        import torch
+        host = self.placement == "host"
+        if isinstance(a, torch.Tensor):
             if not host:
-                self._keep.append(torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(dev))
-                return self._keep[-1].data_ptr()
-            view, dptr, buf = _pin(a, dtype)
-            pinned.append(buf)
-            self._keep.append(view)
-            return dptr
+                self._keep.append(a)
+                return a, a.data_ptr()
+            dtype = {torch.int32: np.int32, torch.int64: np.int64}[a.dtype]
+        dtype = a.dtype if dtype is None else dtype
+        if not host:
+            self._keep.append(torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(self.device))
+            return self._keep[-1], self._keep[-1].data_ptr()
+        view, dptr, buf = _pin(a, dtype)
+        self._pinned.append(buf)
+        self._keep.append(view)
+        return view, dptr
 
-        if host:
-            weakref.finalize(self, _unpin, dev, pinned)
-        with torch.cuda.device(dev) if host else contextlib.nullcontext():     # register on this graph's device
-            self._build(fg, features, place, up)
+    def _add_block(self, t_t, s_t, r, placed, narrow):
+        """Append the descriptor of block <t_t, s_t, r> whose row_of / ptr / nbr / time were placed (``_place``)."""
+        (row_of, p_row), (_, p_ptr), (_, p_nbr), (_, p_time) = placed
+        self._adjacency.extend(kept for kept, _ in placed)
+        flags = (_BLOCK_SKIP if r == 'self' else 0) | (_BLOCK_NARROW if narrow else 0)
+        self._cblocks.append(_GBlock(p_row, row_of.shape[0], p_ptr, p_nbr, p_time, self.slot[t_t], self.slot[s_t], flags,
+                                     self.edge_dict[r]))
+        self.blocks.append((self.slot[t_t], self.slot[s_t], r))
 
-    def _build(self, fg, features, place, up):
+    def _finish(self, features):
+        """Upload the block descriptors (added in dict order) and per-type block ranges, and place the feature tables."""
         import torch
         dev = self.device
-        self.blocks = []                                  # (target slot, source slot, relation, skip) in dict order
-        self._adjacency = []                              # the block arrays the kernels read (for graph_bytes)
-        cblocks = []
-        if self.placement == "host":
-            fg._cblocks = {}        # the host sampler's cached block tables hold the addresses of arrays rebound below
-        for t_t, tes in fg.blocks.items():
-            for s_t, rels in tes.items():
-                for r, blk in rels.items():
-                    if r not in self.edge_dict:
-                        raise KeyError("relation %r of edge_list is not in graph.get_meta_graph()" % (r,))
-                    ptrs = [place(blk.row_of), place(blk.ptr), place(blk.nbr), place(blk.time)]
-                    self._adjacency.extend(self._keep[-4:])
-                    if self.placement == "host":           # the FrozenGraph reads the pinned copies: one copy each
-                        blk.row_of, blk.ptr, blk.nbr, blk.time = self._keep[-4:]
-                        blk.nbr_addr, blk.time_addr = blk.nbr.ctypes.data, blk.time.ctypes.data
-                    flags = (_BLOCK_SKIP if r == 'self' else 0) | (_BLOCK_NARROW if blk.narrow else 0)
-                    cb = _GBlock(ptrs[0], blk.row_of.shape[0], ptrs[1], ptrs[2], ptrs[3], self.slot[t_t],
-                                 self.slot[s_t], flags, self.edge_dict[r])
-                    self.blocks.append((self.slot[t_t], self.slot[s_t], r))
-                    cblocks.append(cb)
-        self.n_blocks = len(cblocks)
-        self.blocks_dev = self._struct_array(cblocks)
+        self.n_blocks = len(self._cblocks)
+        self.blocks_dev = self._struct_array(self._cblocks)
         # the blocks of a target type are contiguous (edge_list is walked target type first), in dict order: the
         # add_budget of that type walks blocks_dev[begin:end)
         rng = np.zeros(2 * max(len(self.types), 1), dtype=np.int32)
@@ -759,11 +940,11 @@ class DeviceGraph:
                 if v is not None and self.placement == "host":
                     v = v.detach().to(device="cpu", dtype=torch.float32)
                     if bf16:                               # numpy has no bf16: pinned as its 16-bit patterns
-                        p = place(v.to(torch.bfloat16).contiguous().view(torch.int16).numpy())
-                        v = torch.from_numpy(self._keep[-1]).view(torch.bfloat16)
+                        view, p = self._place(v.to(torch.bfloat16).contiguous().view(torch.int16).numpy())
+                        v = torch.from_numpy(view).view(torch.bfloat16)
                     else:
-                        p = place(v.contiguous().numpy(), np.float32)
-                        v = torch.from_numpy(self._keep[-1])
+                        view, p = self._place(v.contiguous().numpy(), np.float32)
+                        v = torch.from_numpy(view)
                     tabs[t] = v
                 elif v is not None:
                     v = v.to(device=dev, dtype=torch.float32)
@@ -774,7 +955,7 @@ class DeviceGraph:
                 rows.append(0 if v is None else v.shape[0])
             self.features = tabs
             self.feat_ptrs = torch.tensor(np.asarray(ptrs, dtype=np.uint64).view(np.int64), device=dev)
-            self.feat_rows = up(rows)
+            self.feat_rows = torch.from_numpy(np.asarray(rows, dtype=np.int64)).to(dev)
 
     def _struct_array(self, structs):
         import torch
