@@ -795,106 +795,45 @@ typedef struct {
   int32_t rel;                                /* edge_type value in the to_torch layout (data.py:237-238) */
 } hgt_gsample_block;
 
-/* Sampler state of one batch: the struct is passed by HOST pointer, its fields are DEVICE arrays.
- * Initial values: ser -1, n_layer 0, score 0, bstamp -1, last_seq -1, first_seq / type_min INT64_MAX, type_seq -1
- * (except the seed types' layer numbers), counters {number of seed types, 0}. */
+/* ------------------------------------------------------------------------------------------------
+ * B subgraphs ("members") in one pass (pyhgt_b200/sampler.py: sample_subgraphs_cuda; sample_subgraph_cuda is B = 1).
+ * The members share the graph, the time filter, the depth and the width; each has its own seeds, Philox seed, step
+ * numbers and rows of the state, and member b's result is bitwise that of a batch of b alone with the same seed and
+ * steps.  Memory: about 52 bytes per state slot, i.e. B x 52 B x (sum of the id ranges) for the dense arrays; selection
+ * sorts every id of the selected type (int32 sort values: the ranges of one step must sum to less than 2^31 - 1).  The
+ * hashed state below (hgt_gsample_hash_state) holds the same fields in hash tables sized by the sample instead.
+ * ---------------------------------------------------------------------------------------------- */
+
+/* Dense sampler state of B members: the struct is passed by HOST pointer, its fields are DEVICE arrays.  type_off /
+ * lid_off hold ABSOLUTE positions (member b's type t: slots type_off[b*(T+1)+t] .. [b*(T+1)+t+1], lid entries likewise);
+ * the per-slot arrays hold every member's slots.  Initial values, per member: ser -1, n_layer 0, score 0, bstamp -1,
+ * last_seq -1, first_seq / type_min INT64_MAX, type_seq -1 (except the seed types' layer numbers), counters {number of
+ * seed types, 0}. */
 typedef struct {
-  int32_t num_types; int32_t pad;
-  const int64_t* type_off;   /* [T+1] first state slot of each type (id range of type t: type_off[t+1]-type_off[t]) */
-  const int64_t* lid_off;    /* [T+1] first entry of each type in lid (capacity of type t: lid_off[t+1]-lid_off[t]) */
+  int32_t num_types; int32_t n_members;
+  const int64_t* type_off;   /* [B*(T+1)] first state slot of each (member, type) (id range: the difference to the next) */
+  const int64_t* lid_off;    /* [B*(T+1)] first entry of each (member, type) in lid (capacity: likewise) */
   int32_t* ser;              /* [slots] position of the node in layer_data[type] (data.py:133-141,166), -1 = not sampled */
   int64_t* ltime;            /* [slots] its time in layer_data */
-  int64_t* lid;              /* sampled ids of every type in ser order */
-  int64_t* n_layer;          /* [T] nodes sampled per type */
+  int64_t* lid;              /* sampled ids of every (member, type) in ser order */
+  int64_t* n_layer;          /* [B*T] nodes sampled per type */
   unsigned long long* score; /* [slots] budget score, fixed point with 40 fraction bits */
   int64_t* btime;            /* [slots] budget time (last writer, data.py:130) */
   int64_t* bstamp;           /* [slots] budget insertion stamp, -1 = not in the budget */
   int64_t* last_seq;         /* [slots] scratch */
   int64_t* first_seq;        /* [slots] scratch */
-  int64_t* type_min;         /* [2T] scratch */
-  int64_t* type_seq;         /* [2T] first-touch number of layer_data[t] (2t) and budget[t] (2t+1), -1 = untouched */
-  int64_t* counters;         /* [2] next first-touch numbers */
-} hgt_gsample_state;
-
-/* add_budget (data.py:108-130) for the targets tgt_id / tgt_time [max_targets] of one type, whose blocks (non-'self'
- * ones are sampled) are blocks[0..n_blocks) in dict order.  n_targets: device count (<= max_targets), or NULL =
- * max_targets.  time_filter = 0 disables the max_time test (ogbn-mag variant: time_range=None).  `step`: a number unique
- * to this call within the batch (< 2^22), selects the random stream and orders the insertion stamps.
- * flags[0] is set when a neighbour id lies outside its type's id range. */
-int hgt_gsample_add_budget_workspace_bytes(int64_t max_targets, int32_t n_blocks, int64_t sampled_number,
-                                           size_t* out_bytes);
-int hgt_gsample_add_budget(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks,
-                           const int64_t* tgt_id, const int64_t* tgt_time, int64_t max_targets, const int64_t* n_targets,
-                           int64_t sampled_number, int32_t time_filter, int64_t max_time, int64_t no_time, uint64_t seed,
-                           int64_t step, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
-
-/* Selection of one (layer, type) (data.py:150-170): every budget entry in insertion order when the budget holds fewer
- * than sampled_number entries, else sampled_number entries without replacement with p ~ score^2 (ordered); they join
- * the layer, leave the budget, and are written to tgt_id / tgt_time [sampled_number] with their count in *n_targets
- * (device), ready for hgt_gsample_add_budget.  n_ids: the type's id range.  flags[0]: layer capacity exceeded. */
-int hgt_gsample_select_workspace_bytes(int64_t n_ids, size_t* out_bytes);
-int hgt_gsample_select(const hgt_gsample_state* h_state, int32_t type, int64_t n_ids, int64_t sampled_number,
-                       uint64_t seed, int64_t step, int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets,
-                       int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
-
-/* Rebuild of the sampled adjacency (data.py:190-209), pass 1: for every block b (all relations, 'self' included) and
- * every sampled target r of its type, the number of neighbours in the sample, at cnt_off[b] + r (cnt_off [n_blocks+1]:
- * room for lid capacity of the target type; n_count = cnt_off[n_blocks]).  ex [n_count+1]: exclusive prefix of those
- * counts; totals [n_blocks]: edges per block.  max_rows >= every type's lid capacity.  flags[1]: an edge_time outside
- * [0, 240) (data.py:250, RelTemporalEncoding size); flags[2]: a sampled id >= feat_rows[type] (feat_rows [T] or NULL). */
-int hgt_gsample_rebuild_workspace_bytes(int64_t n_count, size_t* out_bytes);
-int hgt_gsample_rebuild_count(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks,
-                              const int64_t* cnt_off, int64_t n_count, int64_t max_rows, const int64_t* feat_rows,
-                              int64_t* ex, int64_t* totals, int32_t* flags, void* workspace, size_t workspace_bytes,
-                              void* stream);
-/* Pass 2: the to_torch layout (data.py:226-256).  node_off [T]: first output row of each type (-1 = not laid out),
- * type_out [T]: its node_type value; self_off [T]: first edge of its self loops (-1 = none), blk_out [n_blocks]: first
- * edge of each block's edges (-1 = none).  edge_index [2, n_edges] (row 0 = source), edge_type / edge_time [n_edges],
- * node_type / node_time [rows]; node_feature [rows, feat_dim] gathered from feat[t] (a DEVICE array of T device
- * pointers to [ids, feat_dim] float tables) or NULL. */
-int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks,
-                              const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
-                              const int64_t* type_out, const int64_t* self_off, int64_t self_rel, int64_t max_rows,
-                              int64_t n_edges, const float* const* feat, int32_t feat_dim, int64_t* node_type,
-                              int64_t* node_time, float* node_feature, int64_t* edge_index, int64_t* edge_type,
-                              int64_t* edge_time, void* stream);
-
-/* ------------------------------------------------------------------------------------------------
- * B subgraphs ("members") in one pass (pyhgt_b200/sampler.py: sample_subgraphs_cuda).  The members share the graph,
- * the time filter, the depth and the width; each has its own seeds, Philox seed, step numbers and rows of the state, and
- * member b's result is bitwise the single-subgraph run with its seed and steps (the entry points above are B = 1).
- * Memory: about 52 bytes per state slot, i.e. B x 52 B x (sum of the id ranges) for the dense arrays; selection sorts
- * every id of the selected type (int32 sort values: the ranges of one step must sum to less than 2^31 - 1).  The hashed
- * state below (hgt_gsample_hash_state) holds the same fields in hash tables sized by the sample instead.
- * ---------------------------------------------------------------------------------------------- */
-
-/* Like hgt_gsample_state with a member dimension: type_off / lid_off hold [B*(T+1)] ABSOLUTE positions (member b's type
- * t: slots type_off[b*(T+1)+t] .. [b*(T+1)+t+1], lid entries likewise); the dense arrays hold every member's slots;
- * n_layer [B*T], type_min / type_seq [B*2T], counters [B*2]; seed [B] is each member's Philox seed.  Initial values as
- * for hgt_gsample_state, per member. */
-typedef struct {
-  int32_t num_types; int32_t n_members;
-  const int64_t* type_off;
-  const int64_t* lid_off;
-  int32_t* ser;
-  int64_t* ltime;
-  int64_t* lid;
-  int64_t* n_layer;
-  unsigned long long* score;
-  int64_t* btime;
-  int64_t* bstamp;
-  int64_t* last_seq;
-  int64_t* first_seq;
-  int64_t* type_min;
-  int64_t* type_seq;
-  int64_t* counters;
-  const uint64_t* seed;
+  int64_t* type_min;         /* [B*2T] scratch */
+  int64_t* type_seq;         /* [B*2T] first-touch number of layer_data[t] (2t) and budget[t] (2t+1), -1 = untouched */
+  int64_t* counters;         /* [B*2] next first-touch numbers */
+  const uint64_t* seed;      /* [B] each member's Philox seed */
 } hgt_gsample_batch_state;
 
-/* add_budget for every member at once: member b's targets are tgt_id / tgt_time [b*max_targets ...] (n_targets[b] of
- * them, device) of node type type[b] (device [B]; -1 = the member sits this step out), whose blocks are
- * blocks[type_blocks[2t] .. type_blocks[2t+1]) (device [2T]; max_blocks >= every such count); step [B] (device) is the
- * member's step number.  Otherwise as hgt_gsample_add_budget. */
+/* add_budget (data.py:108-130) for every member at once: member b's targets are tgt_id / tgt_time [b*max_targets ...]
+ * (n_targets[b] of them, device) of node type type[b] (device [B]; -1 = the member sits this step out), whose blocks are
+ * blocks[type_blocks[2t] .. type_blocks[2t+1]) (device [2T], dict order; max_blocks >= every such count; non-'self'
+ * blocks are sampled).  time_filter = 0 disables the max_time test (ogbn-mag variant: time_range=None).  step [B]
+ * (device): the member's step number, unique to this call within the member's run (< 2^22); it selects the random
+ * stream and orders the insertion stamps.  flags[0] is set when a neighbour id lies outside its type's id range. */
 int hgt_gsample_batch_add_budget_workspace_bytes(int32_t n_members, int64_t max_targets, int32_t max_blocks,
                                                  int64_t sampled_number, size_t* out_bytes);
 int hgt_gsample_batch_add_budget(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
@@ -903,51 +842,49 @@ int hgt_gsample_batch_add_budget(const hgt_gsample_batch_state* h_state, const h
                                  const int64_t* n_targets, int64_t sampled_number, int32_t time_filter, int64_t max_time,
                                  int64_t no_time, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Selection for every member at once: member b selects from type[b] (-1 = none: n_targets[b] = 0) with step[b]; its ids
- * are sorted at positions sel_off[b] .. sel_off[b+1] (device [B+1], = the type's id range; n_total = sel_off[B],
- * max_ids >= every range).  Member b's targets go to tgt_id / tgt_time [b*sampled_number ...], their count to
- * n_targets[b].  Otherwise as hgt_gsample_select. */
+/* Selection of one (layer, type) per member (data.py:150-170): member b selects from type[b] (-1 = none: n_targets[b] =
+ * 0) with step[b].  Every budget entry in insertion order when the budget holds fewer than sampled_number entries, else
+ * sampled_number entries without replacement with p ~ score^2 (ordered); they join the layer, leave the budget, and go
+ * to tgt_id / tgt_time [b*sampled_number ...] with their count in n_targets[b] (device), ready for add_budget.  Member
+ * b's ids are sorted at positions sel_off[b] .. sel_off[b+1] (device [B+1], = the type's id range; n_total =
+ * sel_off[B], max_ids >= every range).  flags[0]: layer capacity exceeded. */
 int hgt_gsample_batch_select_workspace_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes);
 int hgt_gsample_batch_select(const hgt_gsample_batch_state* h_state, const int32_t* type, const int64_t* step,
                              const int64_t* sel_off, int64_t n_total, int64_t max_ids, int64_t sampled_number,
                              int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets, int32_t* flags, void* workspace,
                              size_t workspace_bytes, void* stream);
 
-/* Rebuild of every member at once (workspace: hgt_gsample_rebuild_workspace_bytes(n_count)).  cnt_off [B*n_blocks+1]:
- * member b, block k counts at cnt_off[b*n_blocks+k]; totals [B*n_blocks]. */
+/* Rebuild of the sampled adjacency (data.py:190-209), pass 1: for every member b, block k (all relations, 'self'
+ * included) and sampled target r of its type, the number of neighbours in the sample, at cnt_off[b*n_blocks+k] + r
+ * (cnt_off [B*n_blocks+1]: room for the lid capacity of the target type; n_count = cnt_off[B*n_blocks]).  ex
+ * [n_count+1]: exclusive prefix of those counts; totals [B*n_blocks]: edges per (member, block).  max_rows >= every
+ * lid capacity.  flags[1]: an edge_time outside [0, 240) (data.py:250, RelTemporalEncoding size); flags[2]: a sampled
+ * id >= feat_rows[type] (feat_rows [T] or NULL).  Workspace: hgt_gsample_rebuild_workspace_bytes(n_count), the same for
+ * every rebuild count pass (dense, hashed and host-graph).
+ * min_ser: NULL (no mask) or an edge mask [2*n_blocks] (device, sampler.py: sample_subgraphs_cuda(..., edge_mask=...))
+ * shared by every member: an edge of block k is kept iff its target ser >= min_ser[2k] and its source ser >=
+ * min_ser[2k+1]; {0, 0} keeps the whole block.  Pass the same table to both passes: totals and the edge layout then
+ * count kept edges only, in block order, and the edge_time check (flags[1]) looks at kept edges only.  The neighbour id
+ * check (flags[0]) covers every edge. */
+int hgt_gsample_rebuild_workspace_bytes(int64_t n_count, size_t* out_bytes);
 int hgt_gsample_batch_rebuild_count(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
-                                    int32_t n_blocks, const int64_t* cnt_off, int64_t n_count, int64_t max_rows,
-                                    const int64_t* feat_rows, int64_t* ex, int64_t* totals, int32_t* flags,
-                                    void* workspace, size_t workspace_bytes, void* stream);
-/* blk_out [B*n_blocks], node_off / self_off [B*T]: member-local as in hgt_gsample_rebuild_write; mem_out [B*3] (device):
- * member b's {first node row, first edge, edge count} in the shared outputs.  Member b's edge_index is the [2, E_b]
- * block at edge_index + 2 * first edge, with member-local node ids: each member is exactly a to_torch layout. */
+                                    int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count,
+                                    int64_t max_rows, const int64_t* feat_rows, int64_t* ex, int64_t* totals,
+                                    int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
+/* Pass 2: the to_torch layout (data.py:226-256) of every member.  Member-local tables: node_off [B*T]: first output row
+ * of each type (-1 = not laid out), type_out [T]: its node_type value; self_off [B*T]: first edge of its self loops (-1
+ * = none), blk_out [B*n_blocks]: first edge of each block's edges (-1 = none).  mem_out [B*3] (device): member b's
+ * {first node row, first edge, edge count} in the shared outputs.  edge_type / edge_time [edges], node_type / node_time
+ * [rows]; member b's edge_index is the [2, E_b] block (row 0 = source) at edge_index + 2 * first edge, with
+ * member-local node ids: each member is exactly a to_torch layout.  node_feature [rows, feat_dim] gathered from feat[t]
+ * (a DEVICE array of T device pointers to [ids, feat_dim] float tables) or NULL. */
 int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
-                                    int32_t n_blocks, const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out,
-                                    const int64_t* node_off, const int64_t* type_out, const int64_t* self_off,
-                                    int64_t self_rel, const int64_t* mem_out, int64_t max_rows, const float* const* feat,
-                                    int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature,
-                                    int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream);
-
-/* The two rebuild passes with an edge mask (sampler.py: sample_subgraphs_cuda(..., edge_mask=...)).  min_ser
- * [2*n_blocks] (device, not NULL), shared by every member: an edge of block k is kept iff its target ser >=
- * min_ser[2k] and its source ser >= min_ser[2k+1]; {0, 0} keeps the whole block.  Pass the same table to both passes:
- * totals and the edge layout then count kept edges only, in block order, and the edge_time check (flags[1]) looks at
- * kept edges only.  The neighbour id check (flags[0]) still covers every edge.  Otherwise as the unmasked entry points,
- * which are these with no mask. */
-int hgt_gsample_batch_rebuild_count_masked(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
-                                           int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
-                                           int64_t n_count, int64_t max_rows, const int64_t* feat_rows, int64_t* ex,
-                                           int64_t* totals, int32_t* flags, void* workspace, size_t workspace_bytes,
-                                           void* stream);
-int hgt_gsample_batch_rebuild_write_masked(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
-                                           int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
-                                           const int64_t* ex, const int64_t* blk_out, const int64_t* node_off,
-                                           const int64_t* type_out, const int64_t* self_off, int64_t self_rel,
-                                           const int64_t* mem_out, int64_t max_rows, const float* const* feat,
-                                           int32_t feat_dim, int64_t* node_type, int64_t* node_time,
-                                           float* node_feature, int64_t* edge_index, int64_t* edge_type,
-                                           int64_t* edge_time, void* stream);
+                                    int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex,
+                                    const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
+                                    const int64_t* self_off, int64_t self_rel, const int64_t* mem_out, int64_t max_rows,
+                                    const float* const* feat, int32_t feat_dim, int64_t* node_type, int64_t* node_time,
+                                    float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time,
+                                    void* stream);
 
 /* The hashed sampler state (sampler.py: sample_subgraphs_cuda picks it when the dense state is too large or slower):
  * per (member, type) an open-addressing table of `room` entries keyed by node id, sized by the sample rather than by the
@@ -1003,9 +940,9 @@ int hgt_gsample_hash_select(const hgt_gsample_hash_state* h_state, const int32_t
                             const int64_t* sel_off, int64_t n_total, int64_t max_room, int64_t sampled_number,
                             int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets, int32_t* flags, void* workspace,
                             size_t workspace_bytes, void* stream);
-/* The rebuild passes, as hgt_gsample_batch_rebuild_count / _write with min_ser NULL (no mask) or a mask table as for the
- * _masked entry points, and the host-graph passes as hgt_gsample_batch_rebuild_count_host / _write_host.  Workspace:
- * hgt_gsample_rebuild_workspace_bytes.  The outputs are those of the dense state. */
+/* The rebuild passes, as hgt_gsample_batch_rebuild_count / _write (min_ser included), and the host-graph passes as
+ * hgt_gsample_batch_rebuild_count_host / _write_host.  Workspace: hgt_gsample_rebuild_workspace_bytes.  The outputs
+ * are those of the dense state. */
 int hgt_gsample_hash_rebuild_count(const hgt_gsample_hash_state* h_state, const hgt_gsample_block* blocks,
                                    int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count,
                                    int64_t max_rows, const int64_t* feat_rows, int64_t* ex, int64_t* totals,
@@ -1039,8 +976,8 @@ int hgt_gsample_hash_rebuild_write_host(const hgt_gsample_hash_state* h_state, c
  * record per kept edge in `hits` (device, room for hit_cap < 2^31 records), with their number in *n_hits (device; it
  * counts past hit_cap).  The write pass lays the edges out from the n_hits records alone, or, with hits NULL (the records
  * did not fit), re-reads the lists like hgt_gsample_batch_rebuild_write; it gathers feature rows (feat may point to host
- * tables) with 16-byte loads when they are 16-byte aligned.  min_ser may be NULL (no mask) or a table as for the _masked
- * entry points.  Otherwise as hgt_gsample_batch_rebuild_count / _write: the outputs are identical. */
+ * tables) with 16-byte loads when they are 16-byte aligned.  Otherwise, min_ser included, as
+ * hgt_gsample_batch_rebuild_count / _write: the outputs are identical. */
 int hgt_host_register(void* host, size_t bytes, void** dev_ptr);
 int hgt_host_unregister(void* host);
 int hgt_gsample_batch_rebuild_count_host(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,

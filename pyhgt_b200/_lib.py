@@ -103,29 +103,16 @@ SIGNATURES = {
                                        _i32, _p, _p, _p, _sz, _p, _p],
     "hgt_edge_backward_rows_att_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _p, _i32, _i32, _p, _i32,
                                         _i32, _i32, _p, _p, _sz, _p, _p],
-    # HGSampling on the GPU (sampler.sample_subgraph_cuda)
-    "hgt_gsample_add_budget_workspace_bytes": [_i64, _i32, _i64, _c.POINTER(_sz)],
-    "hgt_gsample_add_budget": [_p, _p, _i32, _p, _p, _i64, _p, _i64, _i32, _i64, _i64, _c.c_uint64, _i64, _p, _p, _sz,
-                               _p],
-    "hgt_gsample_select_workspace_bytes": [_i64, _c.POINTER(_sz)],
-    "hgt_gsample_select": [_p, _i32, _i64, _i64, _c.c_uint64, _i64, _p, _p, _p, _p, _p, _sz, _p],
-    "hgt_gsample_rebuild_workspace_bytes": [_i64, _c.POINTER(_sz)],
-    "hgt_gsample_rebuild_count": [_p, _p, _i32, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
-    "hgt_gsample_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _p, _i32, _p, _p, _p, _p, _p,
-                                  _p, _p],
-    # B subgraphs per pass (sampler.sample_subgraphs_cuda) and their disjoint union (sampler.merge_batches)
+    # HGSampling on the GPU, B subgraphs per pass (sampler.sample_subgraphs_cuda), and their union (merge_batches)
     "hgt_gsample_batch_add_budget_workspace_bytes": [_i32, _i64, _i32, _i64, _c.POINTER(_sz)],
     "hgt_gsample_batch_add_budget": [_p, _p, _p, _i32, _p, _p, _p, _p, _i64, _p, _i64, _i32, _i64, _i64, _p, _p, _sz,
                                      _p],
     "hgt_gsample_batch_select_workspace_bytes": [_i32, _i64, _c.POINTER(_sz)],
     "hgt_gsample_batch_select": [_p, _p, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
-    "hgt_gsample_batch_rebuild_count": [_p, _p, _i32, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
-    "hgt_gsample_batch_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p, _p,
-                                        _p, _p, _p],
-    # the same rebuild with a per-block edge mask (sample_subgraphs_cuda(..., edge_mask=...))
-    "hgt_gsample_batch_rebuild_count_masked": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
-    "hgt_gsample_batch_rebuild_write_masked": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p,
-                                               _p, _p, _p, _p, _p, _p],
+    "hgt_gsample_rebuild_workspace_bytes": [_i64, _c.POINTER(_sz)],
+    "hgt_gsample_batch_rebuild_count": [_p, _p, _i32, _p, _p, _i64, _i64, _p, _p, _p, _p, _p, _sz, _p],
+    "hgt_gsample_batch_rebuild_write": [_p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p,
+                                        _p, _p, _p, _p],
     # graphs in page-locked host memory (sampler.DeviceGraph(..., placement="host"))
     "hgt_host_register": [_p, _sz, _c.POINTER(_p)],
     "hgt_host_unregister": [_p],

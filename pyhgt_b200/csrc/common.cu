@@ -27,4 +27,4 @@ unsigned long long g_hgt_launches = 0;
 
 extern "C" uint64_t hgt_kernel_launches(void) { return g_hgt_launches; }
 extern "C" const char* hgt_last_error(void) { return g_err; }
-extern "C" int hgt_abi_version(void) { return 4; }
+extern "C" int hgt_abi_version(void) { return 5; }

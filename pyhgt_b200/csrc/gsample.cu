@@ -11,7 +11,7 @@
 //     dropping edges by per-block minimum target / source sers (the OAG scripts' label-leak mask).
 // Every stage runs B independent subgraphs ("members") at once: each member has its own rows of the state, its own seed
 // and its own step numbers, and everything a member computes depends on its own rows alone, so member b of a batch is
-// bitwise the single-subgraph run with b's seed.  The single-subgraph entry points are the B = 1 case.
+// bitwise a batch of b alone with b's seed (sample_subgraph_cuda is such a batch of one).
 #include "common.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
@@ -26,14 +26,6 @@ constexpr double kScoreScale = 1099511627776.0;          // 2^40: budget scores 
 constexpr long long kNoSeq = 0x7fffffffffffffffLL;
 constexpr unsigned kFull = 0xffffffffu;
 constexpr uint64_t kSelectStream = 0x5e1ec7ULL << 40;     // keeps selection draws apart from neighbour draws
-
-// A per-member value: a device array of B values, or one value (the single-subgraph entry points pass scalars).
-template <typename V>
-struct PerMember {
-  const V* p;
-  V v;
-  __device__ __forceinline__ V operator[](int m) const { return p ? p[m] : v; }
-};
 
 // Member m's rows of the batch state (the dense per-slot arrays are shared: type_off / lid_off hold absolute positions).
 struct Member {
@@ -167,34 +159,29 @@ __device__ __forceinline__ int64_t src_ltime(const hgt_gsample_hash_state& st, c
   return st.ltime[ix.lt + sser];
 }
 
-// The blocks member m's add_budget walks: blocks[0, n_blocks) for every member (single type), or the blocks of the
-// member's current type (type_blocks [2T]: begin / end per target type; type[m] < 0 = the member sits this step out).
+// The blocks member m's add_budget walks: those of the member's current type (type_blocks [2T]: begin / end per target
+// type; type[m] < 0 = the member sits this step out).
 struct BlockRange {
   const int32_t* type_blocks;
   const int32_t* type;
-  int32_t n_blocks;
   __device__ __forceinline__ void get(int m, int32_t* b0, int32_t* nb) const {
+    const int t = type[m];
     *b0 = 0;
-    *nb = n_blocks;
-    if (type_blocks) {
-      const int t = type[m];
-      *nb = 0;
-      if (t >= 0) {
-        *b0 = type_blocks[2 * t];
-        *nb = type_blocks[2 * t + 1] - *b0;
-      }
+    *nb = 0;
+    if (t >= 0) {
+      *b0 = type_blocks[2 * t];
+      *nb = type_blocks[2 * t + 1] - *b0;
     }
   }
 };
 
-// Where member m's nodes and edges go in the output buffers: {node_base, edge_base, n_edges} per member, or one member
-// at 0 with n_edges edges.
+// Where member m's nodes and edges go in the output buffers: {node_base, edge_base, n_edges} per member.  Read-only
+// loads: with plain ones the hashed k_rb_write takes 52 registers instead of 48 (sm_90a, CUDA 12.9).
 struct MemOut {
   const int64_t* p;
-  int64_t n_edges;
-  __device__ __forceinline__ int64_t node_base(int m) const { return p ? p[3 * m] : 0; }
-  __device__ __forceinline__ int64_t edge_base(int m) const { return p ? p[3 * m + 1] : 0; }
-  __device__ __forceinline__ int64_t edges(int m) const { return p ? p[3 * m + 2] : n_edges; }
+  __device__ __forceinline__ int64_t node_base(int m) const { return __ldg(p + 3 * m); }
+  __device__ __forceinline__ int64_t edge_base(int m) const { return __ldg(p + 3 * m + 1); }
+  __device__ __forceinline__ int64_t edges(int m) const { return __ldg(p + 3 * m + 2); }
 };
 
 __device__ __forceinline__ uint64_t rnd64(curandStatePhilox4_32_10_t* s) {
@@ -242,7 +229,7 @@ __device__ __forceinline__ int64_t seg_size(const hgt_gsample_block& blk, int64_
 }
 
 // Segments are member-major with stride S = max_targets * max_blocks; inside a member, segment k * nb + b is target k,
-// block b (nb = the member's block count), the numbering of the single-subgraph run.
+// block b (nb = the member's block count), the numbering of a batch of that member alone.
 __global__ void k_seg_count(const hgt_gsample_block* blocks, BlockRange br, int32_t n_members, int64_t S,
                             const int64_t* tgt_id, int64_t max_targets, const int64_t* n_targets, int64_t width,
                             int64_t* seg_cnt) {
@@ -257,9 +244,8 @@ __global__ void k_seg_count(const hgt_gsample_block* blocks, BlockRange br, int3
   int64_t c = 0;
   if (loc < max_targets * nb) {
     const int64_t k = loc / nb;
-    const int64_t n = n_targets ? n_targets[m] : max_targets;
     int64_t a, deg;
-    if (k < n) c = seg_size(blocks[b0 + loc % nb], tgt_id[m * max_targets + k], width, &a, &deg);
+    if (k < n_targets[m]) c = seg_size(blocks[b0 + loc % nb], tgt_id[m * max_targets + k], width, &a, &deg);
   }
   seg_cnt[i] = c;
 }
@@ -267,12 +253,11 @@ __global__ void k_seg_count(const hgt_gsample_block* blocks, BlockRange br, int3
 // One warp per <member, target k, block b>.  seq = seg_off + j orders the member's candidates like the reference's
 // processing order (target, block, neighbour in subset order), the key of every order-dependent rule.
 template <class St>
-__global__ void k_candidates(St st, PerMember<uint64_t> seed, PerMember<int64_t> step,
-                             const hgt_gsample_block* blocks, BlockRange br, int64_t S, const int64_t* tgt_id,
-                             const int64_t* tgt_time, int64_t max_targets, const int64_t* seg_cnt,
-                             const int64_t* seg_off, int64_t width, int32_t time_filter, int64_t max_time,
-                             int64_t no_time, int64_t* cand_pos, int64_t* cand_slot, int64_t* cand_time,
-                             int32_t* flags) {
+__global__ void k_candidates(St st, const int64_t* step, const hgt_gsample_block* blocks, BlockRange br, int64_t S,
+                             const int64_t* tgt_id, const int64_t* tgt_time, int64_t max_targets,
+                             const int64_t* seg_cnt, const int64_t* seg_off, int64_t width, int32_t time_filter,
+                             int64_t max_time, int64_t no_time, int64_t* cand_pos, int64_t* cand_slot,
+                             int64_t* cand_time, int32_t* flags) {
   const int lane = threadIdx.x & 31;
   const int64_t seg = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   if (seg >= S * st.n_members) return;
@@ -293,7 +278,7 @@ __global__ void k_candidates(St st, PerMember<uint64_t> seed, PerMember<int64_t>
   if (!all) {
     // Floyd: a uniform n_s-subset of [0, deg); then a uniform order (Fisher-Yates).  Every lane runs the same stream.
     curandStatePhilox4_32_10_t rs;
-    curand_init(seed[m], ((uint64_t)step[m] << 32) | (uint64_t)loc, 0, &rs);
+    curand_init(st.seed[m], ((uint64_t)step[m] << 32) | (uint64_t)loc, 0, &rs);
     for (int64_t c = 0, jj = deg - n_s; jj < deg; ++jj, ++c) {
       const int64_t t = rnd_below(&rs, jj + 1);
       bool found = false;
@@ -341,7 +326,7 @@ __global__ void k_candidates(St st, PerMember<uint64_t> seed, PerMember<int64_t>
 // << 40 + its position among the member's candidates).  The matching candidate also resets the scratch word: no other
 // candidate of the slot can match either value.  grid.y = member; grid-stride over the member's candidates.
 template <class St>
-__global__ void k_resolve(St st, PerMember<int64_t> step, const int64_t* seg_off, int64_t S,
+__global__ void k_resolve(St st, const int64_t* step, const int64_t* seg_off, int64_t S,
                           const int64_t* cand_slot, const int64_t* cand_time) {
   const int m = blockIdx.y;
   const int64_t lo = seg_off[m * S], hi = seg_off[(m + 1) * S];
@@ -382,7 +367,7 @@ __global__ void k_touch(St st) {
 }
 
 // grid.y = member, which selects from its own type[m] (< 0: none this step).
-__global__ void k_sel_count(hgt_gsample_batch_state st, PerMember<int32_t> type, unsigned long long* count) {
+__global__ void k_sel_count(hgt_gsample_batch_state st, const int32_t* type, unsigned long long* count) {
   const int m = blockIdx.y;
   const int t = type[m];
   if (t < 0) return;
@@ -398,9 +383,8 @@ __global__ void k_sel_count(hgt_gsample_batch_state st, PerMember<int32_t> type,
 // Sort keys (descending): budget smaller than the width -> every entry in insertion order (key -stamp); otherwise
 // Efraimidis-Spirakis log(u) / score^2 (data.py:158-160).  Entries outside the budget sort last.  Member m's ids sit at
 // sel_off[m] + i; the sort value is that position.
-__global__ void k_sel_keys(hgt_gsample_batch_state st, PerMember<int32_t> type, PerMember<int64_t> sel_off,
-                           int64_t width, const unsigned long long* count, PerMember<uint64_t> seed,
-                           PerMember<int64_t> step, double* keys, int32_t* vals) {
+__global__ void k_sel_keys(hgt_gsample_batch_state st, const int32_t* type, const int64_t* sel_off, int64_t width,
+                           const unsigned long long* count, const int64_t* step, double* keys, int32_t* vals) {
   const int m = blockIdx.y;
   const int t = type[m];
   if (t < 0) return;
@@ -416,7 +400,7 @@ __global__ void k_sel_keys(hgt_gsample_batch_state st, PerMember<int32_t> type, 
       key = -(double)stamp;
     } else {
       curandStatePhilox4_32_10_t rs;
-      curand_init(seed[m] ^ kSelectStream, ((uint64_t)step[m] << 40) | (uint64_t)i, 0, &rs);
+      curand_init(st.seed[m] ^ kSelectStream, ((uint64_t)step[m] << 40) | (uint64_t)i, 0, &rs);
       const double u = (double)((rnd64(&rs) >> 11) + 1) * 0x1.0p-53;   // (0, 1]
       const double s = (double)st.score[slot] / kScoreScale;
       key = log(u) / (s * s);
@@ -443,9 +427,9 @@ __global__ void k_sel_member(const int64_t* sel_off, int32_t n_members, const in
 
 // data.py:166-170: the chosen ids join layer_data in key order (ser), become the next add_budget's targets (member m's
 // at tgt_id[m * width ...]), and leave the budget.
-__global__ void k_sel_take(hgt_gsample_batch_state st, PerMember<int32_t> type, PerMember<int64_t> sel_off,
-                           int64_t width, const unsigned long long* count, const int32_t* vals, int64_t* tgt_id,
-                           int64_t* tgt_time, int32_t* flags) {
+__global__ void k_sel_take(hgt_gsample_batch_state st, const int32_t* type, const int64_t* sel_off, int64_t width,
+                           const unsigned long long* count, const int32_t* vals, int64_t* tgt_id, int64_t* tgt_time,
+                           int32_t* flags) {
   const int m = blockIdx.y;
   const int t = type[m];
   if (t < 0) return;
@@ -468,8 +452,8 @@ __global__ void k_sel_take(hgt_gsample_batch_state st, PerMember<int32_t> type, 
 }
 
 template <class St>
-__global__ void k_sel_finish(St st, PerMember<int32_t> type, int64_t width,
-                             const unsigned long long* count, int64_t* n_targets) {
+__global__ void k_sel_finish(St st, const int32_t* type, int64_t width, const unsigned long long* count,
+                             int64_t* n_targets) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= st.n_members) return;
   const int t = type[m];
@@ -1073,11 +1057,6 @@ size_t carve_select(SelectScratch& s, void* base, int64_t n, int32_t n_members, 
 
 inline int64_t blocks_for(int64_t n, int per = kThreads) { return (n + per - 1) / per; }
 
-hgt_gsample_batch_state as_batch(const hgt_gsample_state& s) {
-  return {s.num_types, 1,         s.type_off, s.lid_off,  s.ser,      s.ltime,    s.lid,      s.n_layer,
-          s.score,     s.btime,   s.bstamp,   s.last_seq, s.first_seq, s.type_min, s.type_seq, s.counters, nullptr};
-}
-
 int budget_bytes(int32_t n_members, int64_t max_targets, int32_t n_blocks, int64_t sampled_number, size_t* out_bytes,
                  const char* what) {
   HGT_REQUIRE(out_bytes && n_members >= 1 && n_members < 65536 && max_targets >= 0 && n_blocks >= 0 &&
@@ -1093,11 +1072,10 @@ int budget_bytes(int32_t n_members, int64_t max_targets, int32_t n_blocks, int64
 }
 
 template <class St>
-int add_budget(const St& hs, PerMember<uint64_t> seed, PerMember<int64_t> step,
-               const hgt_gsample_block* blocks, BlockRange br, int32_t max_blocks, const int64_t* tgt_id,
-               const int64_t* tgt_time, int64_t max_targets, const int64_t* n_targets, int64_t sampled_number,
-               int32_t time_filter, int64_t max_time, int64_t no_time, int32_t* flags, void* workspace,
-               size_t workspace_bytes, void* stream, const char* what) {
+int add_budget(const St& hs, const int64_t* step, const hgt_gsample_block* blocks, BlockRange br, int32_t max_blocks,
+               const int64_t* tgt_id, const int64_t* tgt_time, int64_t max_targets, const int64_t* n_targets,
+               int64_t sampled_number, int32_t time_filter, int64_t max_time, int64_t no_time, int32_t* flags,
+               void* workspace, size_t workspace_bytes, void* stream, const char* what) {
   const int64_t S = max_targets * max_blocks;
   if (S == 0) return 0;
   size_t need = 0;
@@ -1114,7 +1092,7 @@ int add_budget(const St& hs, PerMember<uint64_t> seed, PerMember<int64_t> step,
   size_t tmp = s.cub_bytes;
   HGT_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(s.cub_tmp, tmp, s.seg_cnt, s.seg_off, (int)(n_seg + 1), st));
   k_candidates<<<blocks_for(n_seg, kWarps), kThreads, 0, st>>>(
-      hs, seed, step, blocks, br, S, tgt_id, tgt_time, max_targets, s.seg_cnt, s.seg_off, sampled_number, time_filter,
+      hs, step, blocks, br, S, tgt_id, tgt_time, max_targets, s.seg_cnt, s.seg_off, sampled_number, time_filter,
       max_time, no_time, s.cand_pos, s.cand_slot, s.cand_time, flags);
   HGT_LAUNCH_CHECK();
   const int64_t gx = blocks_for(cap / hs.n_members);
@@ -1143,14 +1121,14 @@ inline int bits_for(int n) {
 
 // The keys_in / vals_in pairs of a selection sorted by key, descending and stable, then (B > 1) stably by member: each
 // member's positions end up together in key order, at the member's sel_off.
-int sort_keys(SelectScratch& s, int64_t n_total, int B, const int64_t* d_sel_off, cudaStream_t st,
+int sort_keys(SelectScratch& s, int64_t n_total, int B, const int64_t* sel_off, cudaStream_t st,
               const int32_t** vals) {
   size_t tmp = s.cub_bytes;
   HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairsDescending(s.cub_tmp, tmp, s.keys_in, s.keys_out, s.vals_in,
                                                            s.vals_out, (int)n_total, 0, 64, st));
   *vals = s.vals_out;
   if (B > 1) {
-    k_sel_member<<<blocks_for(n_total), kThreads, 0, st>>>(d_sel_off, B, s.vals_out, n_total, s.mkey_in);
+    k_sel_member<<<blocks_for(n_total), kThreads, 0, st>>>(sel_off, B, s.vals_out, n_total, s.mkey_in);
     HGT_LAUNCH_CHECK();
     tmp = s.cub_bytes;
     HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, s.mkey_in, s.mkey_out, s.vals_out, s.vals_in,
@@ -1160,10 +1138,10 @@ int sort_keys(SelectScratch& s, int64_t n_total, int B, const int64_t* d_sel_off
   return 0;
 }
 
-int select(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMember<int64_t> step,
-           PerMember<int32_t> type, PerMember<int64_t> sel_off, const int64_t* d_sel_off, int64_t n_total,
-           int64_t max_ids, int64_t sampled_number, int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets,
-           int32_t* flags, void* workspace, size_t workspace_bytes, void* stream, const char* what) {
+int select(const hgt_gsample_batch_state& hs, const int32_t* type, const int64_t* step, const int64_t* sel_off,
+           int64_t n_total, int64_t max_ids, int64_t sampled_number, int64_t* tgt_id, int64_t* tgt_time,
+           int64_t* n_targets, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream,
+           const char* what) {
   size_t need = 0;
   if (int rc = select_bytes(hs.n_members, n_total, &need, what)) return rc;
   HGT_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", what, workspace_bytes, need);
@@ -1176,11 +1154,11 @@ int select(const hgt_gsample_batch_state& hs, PerMember<uint64_t> seed, PerMembe
     const int64_t g = blocks_for(max_ids);
     k_sel_count<<<dim3((unsigned)(g < 1024 ? g : 1024), B), kThreads, 0, st>>>(hs, type, s.count);
     HGT_LAUNCH_CHECK();
-    k_sel_keys<<<dim3((unsigned)g, B), kThreads, 0, st>>>(hs, type, sel_off, sampled_number, s.count, seed, step,
-                                                          s.keys_in, s.vals_in);
+    k_sel_keys<<<dim3((unsigned)g, B), kThreads, 0, st>>>(hs, type, sel_off, sampled_number, s.count, step, s.keys_in,
+                                                          s.vals_in);
     HGT_LAUNCH_CHECK();
     const int32_t* vals = nullptr;
-    if (int rc = sort_keys(s, n_total, B, d_sel_off, st, &vals)) return rc;
+    if (int rc = sort_keys(s, n_total, B, sel_off, st, &vals)) return rc;
     k_sel_take<<<dim3((unsigned)blocks_for(sampled_number), B), kThreads, 0, st>>>(
         hs, type, sel_off, sampled_number, s.count, vals, tgt_id, tgt_time, flags);
     HGT_LAUNCH_CHECK();
@@ -1227,8 +1205,7 @@ int hash_select(const hgt_gsample_hash_state& hs, const int32_t* type, const int
         hs, type, sel_off, sampled_number, s.count, vals, s.oent_out, tgt_id, tgt_time, flags);
     HGT_LAUNCH_CHECK();
   }
-  k_sel_finish<<<(unsigned)blocks_for(B, 32), 32, 0, st>>>(hs, PerMember<int32_t>{type, 0}, sampled_number, s.count,
-                                                           n_targets);
+  k_sel_finish<<<(unsigned)blocks_for(B, 32), 32, 0, st>>>(hs, type, sampled_number, s.count, n_targets);
   HGT_LAUNCH_CHECK();
   return 0;
 }
@@ -1320,72 +1297,7 @@ int rebuild_write(const St& hs, const hgt_gsample_block* blocks, int32_t n_block
 
 }  // namespace
 
-// ---- one subgraph (B = 1) -------------------------------------------------------------------------------------------
-
-extern "C" int hgt_gsample_add_budget_workspace_bytes(int64_t max_targets, int32_t n_blocks, int64_t sampled_number,
-                                                      size_t* out_bytes) {
-  return budget_bytes(1, max_targets, n_blocks, sampled_number, out_bytes, "hgt_gsample_add_budget_workspace_bytes");
-}
-
-extern "C" int hgt_gsample_add_budget(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks,
-                                      int32_t n_blocks, const int64_t* tgt_id, const int64_t* tgt_time,
-                                      int64_t max_targets, const int64_t* n_targets, int64_t sampled_number,
-                                      int32_t time_filter, int64_t max_time, int64_t no_time, uint64_t seed,
-                                      int64_t step, int32_t* flags, void* workspace, size_t workspace_bytes,
-                                      void* stream) {
-  HGT_REQUIRE(h_state && sampled_number > 0 && max_targets >= 0 && n_blocks >= 0 && step >= 0 && step < (1 << 22),
-              "hgt_gsample_add_budget: bad arguments");
-  return add_budget(as_batch(*h_state), {nullptr, seed}, {nullptr, step}, blocks, {nullptr, nullptr, n_blocks},
-                    n_blocks, tgt_id, tgt_time, max_targets, n_targets, sampled_number, time_filter, max_time, no_time,
-                    flags, workspace, workspace_bytes, stream, "hgt_gsample_add_budget");
-}
-
-extern "C" int hgt_gsample_select_workspace_bytes(int64_t n_ids, size_t* out_bytes) {
-  return select_bytes(1, n_ids, out_bytes, "hgt_gsample_select_workspace_bytes");
-}
-
-extern "C" int hgt_gsample_select(const hgt_gsample_state* h_state, int32_t type, int64_t n_ids, int64_t sampled_number,
-                                  uint64_t seed, int64_t step, int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets,
-                                  int32_t* flags, void* workspace, size_t workspace_bytes, void* stream) {
-  HGT_REQUIRE(h_state && type >= 0 && type < h_state->num_types && sampled_number > 0 && step >= 0 && step < (1 << 22),
-              "hgt_gsample_select: bad arguments");
-  return select(as_batch(*h_state), {nullptr, seed}, {nullptr, step}, {nullptr, type}, {nullptr, 0}, nullptr, n_ids,
-                n_ids, sampled_number, tgt_id, tgt_time, n_targets, flags, workspace, workspace_bytes, stream,
-                "hgt_gsample_select");
-}
-
-extern "C" int hgt_gsample_rebuild_workspace_bytes(int64_t n_count, size_t* out_bytes) {
-  HGT_REQUIRE(out_bytes && n_count >= 0 && n_count < (int64_t(1) << 31) - 1,
-              "hgt_gsample_rebuild_workspace_bytes: bad count %lld", (long long)n_count);
-  size_t b = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, b, (const int64_t*)nullptr, (int64_t*)nullptr, (int)(n_count + 1));
-  *out_bytes = hgt_align_up(sizeof(int64_t) * (n_count + 1), 256) + b;
-  return 0;
-}
-
-extern "C" int hgt_gsample_rebuild_count(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks,
-                                         int32_t n_blocks, const int64_t* cnt_off, int64_t n_count, int64_t max_rows,
-                                         const int64_t* feat_rows, int64_t* ex, int64_t* totals, int32_t* flags,
-                                         void* workspace, size_t workspace_bytes, void* stream) {
-  HGT_REQUIRE(h_state, "hgt_gsample_rebuild_count: bad arguments");
-  return rebuild_count(as_batch(*h_state), blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, nullptr, 0,
-                       nullptr, ex, totals, flags, workspace, workspace_bytes, stream, "hgt_gsample_rebuild_count");
-}
-
-extern "C" int hgt_gsample_rebuild_write(const hgt_gsample_state* h_state, const hgt_gsample_block* blocks,
-                                         int32_t n_blocks, const int64_t* cnt_off, const int64_t* ex,
-                                         const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
-                                         const int64_t* self_off, int64_t self_rel, int64_t max_rows, int64_t n_edges,
-                                         const float* const* feat, int32_t feat_dim, int64_t* node_type,
-                                         int64_t* node_time, float* node_feature, int64_t* edge_index,
-                                         int64_t* edge_type, int64_t* edge_time, void* stream) {
-  HGT_REQUIRE(h_state && n_edges >= 0, "hgt_gsample_rebuild_write: bad arguments");
-  return rebuild_write(as_batch(*h_state), blocks, n_blocks, nullptr, cnt_off, ex, blk_out, node_off, type_out,
-                       self_off, self_rel, {nullptr, n_edges}, max_rows, false, nullptr, 0, feat, feat_dim, node_type,
-                       node_time, node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_rebuild_write");
-}
-
-// ---- B subgraphs at once ----------------------------------------------------------------------------------------------
+// ---- the dense state ------------------------------------------------------------------------------------------------
 
 extern "C" int hgt_gsample_batch_add_budget_workspace_bytes(int32_t n_members, int64_t max_targets, int32_t max_blocks,
                                                             int64_t sampled_number, size_t* out_bytes) {
@@ -1402,9 +1314,9 @@ extern "C" int hgt_gsample_batch_add_budget(const hgt_gsample_batch_state* h_sta
   HGT_REQUIRE(h_state && h_state->seed && type_blocks && type && step && n_targets && sampled_number > 0 &&
                   max_targets >= 0 && max_blocks >= 0,
               "hgt_gsample_batch_add_budget: bad arguments");
-  return add_budget(*h_state, {h_state->seed, 0}, {step, 0}, blocks, {type_blocks, type, max_blocks}, max_blocks,
-                    tgt_id, tgt_time, max_targets, n_targets, sampled_number, time_filter, max_time, no_time, flags,
-                    workspace, workspace_bytes, stream, "hgt_gsample_batch_add_budget");
+  return add_budget(*h_state, step, blocks, {type_blocks, type}, max_blocks, tgt_id, tgt_time, max_targets, n_targets,
+                    sampled_number, time_filter, max_time, no_time, flags, workspace, workspace_bytes, stream,
+                    "hgt_gsample_batch_add_budget");
 }
 
 extern "C" int hgt_gsample_batch_select_workspace_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes) {
@@ -1417,55 +1329,39 @@ extern "C" int hgt_gsample_batch_select(const hgt_gsample_batch_state* h_state, 
                                         int32_t* flags, void* workspace, size_t workspace_bytes, void* stream) {
   HGT_REQUIRE(h_state && h_state->seed && type && step && sel_off && sampled_number > 0 && max_ids >= 0,
               "hgt_gsample_batch_select: bad arguments");
-  return select(*h_state, {h_state->seed, 0}, {step, 0}, {type, 0}, {sel_off, 0}, sel_off, n_total, max_ids,
-                sampled_number, tgt_id, tgt_time, n_targets, flags, workspace, workspace_bytes, stream,
-                "hgt_gsample_batch_select");
+  return select(*h_state, type, step, sel_off, n_total, max_ids, sampled_number, tgt_id, tgt_time, n_targets, flags,
+                workspace, workspace_bytes, stream, "hgt_gsample_batch_select");
+}
+
+extern "C" int hgt_gsample_rebuild_workspace_bytes(int64_t n_count, size_t* out_bytes) {
+  HGT_REQUIRE(out_bytes && n_count >= 0 && n_count < (int64_t(1) << 31) - 1,
+              "hgt_gsample_rebuild_workspace_bytes: bad count %lld", (long long)n_count);
+  size_t b = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, b, (const int64_t*)nullptr, (int64_t*)nullptr, (int)(n_count + 1));
+  *out_bytes = hgt_align_up(sizeof(int64_t) * (n_count + 1), 256) + b;
+  return 0;
 }
 
 extern "C" int hgt_gsample_batch_rebuild_count(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
-                                               int32_t n_blocks, const int64_t* cnt_off, int64_t n_count,
-                                               int64_t max_rows, const int64_t* feat_rows, int64_t* ex, int64_t* totals,
-                                               int32_t* flags, void* workspace, size_t workspace_bytes, void* stream) {
+                                               int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off,
+                                               int64_t n_count, int64_t max_rows, const int64_t* feat_rows,
+                                               int64_t* ex, int64_t* totals, int32_t* flags, void* workspace,
+                                               size_t workspace_bytes, void* stream) {
   HGT_REQUIRE(h_state, "hgt_gsample_batch_rebuild_count: bad arguments");
-  return rebuild_count(*h_state, blocks, n_blocks, nullptr, cnt_off, n_count, max_rows, feat_rows, nullptr, 0, nullptr,
+  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, nullptr, 0, nullptr,
                        ex, totals, flags, workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count");
 }
 
-extern "C" int hgt_gsample_batch_rebuild_count_masked(const hgt_gsample_batch_state* h_state,
-                                                      const hgt_gsample_block* blocks, int32_t n_blocks,
-                                                      const int64_t* min_ser, const int64_t* cnt_off, int64_t n_count,
-                                                      int64_t max_rows, const int64_t* feat_rows, int64_t* ex,
-                                                      int64_t* totals, int32_t* flags, void* workspace,
-                                                      size_t workspace_bytes, void* stream) {
-  HGT_REQUIRE(h_state && min_ser, "hgt_gsample_batch_rebuild_count_masked: bad arguments");
-  return rebuild_count(*h_state, blocks, n_blocks, min_ser, cnt_off, n_count, max_rows, feat_rows, nullptr, 0, nullptr,
-                       ex, totals, flags, workspace, workspace_bytes, stream, "hgt_gsample_batch_rebuild_count_masked");
-}
-
-extern "C" int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
-                                               int32_t n_blocks, const int64_t* cnt_off, const int64_t* ex,
-                                               const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
-                                               const int64_t* self_off, int64_t self_rel, const int64_t* mem_out,
-                                               int64_t max_rows, const float* const* feat, int32_t feat_dim,
-                                               int64_t* node_type, int64_t* node_time, float* node_feature,
-                                               int64_t* edge_index, int64_t* edge_type, int64_t* edge_time,
-                                               void* stream) {
-  HGT_REQUIRE(h_state && mem_out, "hgt_gsample_batch_rebuild_write: bad arguments");
-  return rebuild_write(*h_state, blocks, n_blocks, nullptr, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {mem_out, 0}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
-                       node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write");
-}
-
-extern "C" int hgt_gsample_batch_rebuild_write_masked(
+extern "C" int hgt_gsample_batch_rebuild_write(
     const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks, int32_t n_blocks, const int64_t* min_ser,
     const int64_t* cnt_off, const int64_t* ex, const int64_t* blk_out, const int64_t* node_off, const int64_t* type_out,
     const int64_t* self_off, int64_t self_rel, const int64_t* mem_out, int64_t max_rows, const float* const* feat,
     int32_t feat_dim, int64_t* node_type, int64_t* node_time, float* node_feature, int64_t* edge_index,
     int64_t* edge_type, int64_t* edge_time, void* stream) {
-  HGT_REQUIRE(h_state && min_ser && mem_out, "hgt_gsample_batch_rebuild_write_masked: bad arguments");
+  HGT_REQUIRE(h_state && mem_out, "hgt_gsample_batch_rebuild_write: bad arguments");
   return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {mem_out, 0}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
-                       node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write_masked");
+                       self_rel, {mem_out}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
+                       node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_batch_rebuild_write");
 }
 
 // ---- graphs in page-locked host memory ------------------------------------------------------------------------------
@@ -1511,7 +1407,7 @@ extern "C" int hgt_gsample_batch_rebuild_write_host(
     float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream) {
   HGT_REQUIRE(h_state && mem_out && n_hits >= 0, "hgt_gsample_batch_rebuild_write_host: bad arguments");
   return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {mem_out, 0}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
+                       self_rel, {mem_out}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
                        node_time, node_feature, edge_index, edge_type, edge_time, stream,
                        "hgt_gsample_batch_rebuild_write_host");
 }
@@ -1538,9 +1434,9 @@ extern "C" int hgt_gsample_hash_add_budget(const hgt_gsample_hash_state* h_state
   HGT_REQUIRE(h_state && h_state->seed && type_blocks && type && step && n_targets && sampled_number > 0 &&
                   max_targets >= 0 && max_blocks >= 0,
               "hgt_gsample_hash_add_budget: bad arguments");
-  return add_budget(*h_state, {h_state->seed, 0}, {step, 0}, blocks, {type_blocks, type, max_blocks}, max_blocks,
-                    tgt_id, tgt_time, max_targets, n_targets, sampled_number, time_filter, max_time, no_time, flags,
-                    workspace, workspace_bytes, stream, "hgt_gsample_hash_add_budget");
+  return add_budget(*h_state, step, blocks, {type_blocks, type}, max_blocks, tgt_id, tgt_time, max_targets, n_targets,
+                    sampled_number, time_filter, max_time, no_time, flags, workspace, workspace_bytes, stream,
+                    "hgt_gsample_hash_add_budget");
 }
 
 extern "C" int hgt_gsample_hash_select_workspace_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes) {
@@ -1575,7 +1471,7 @@ extern "C" int hgt_gsample_hash_rebuild_write(
     int64_t* edge_type, int64_t* edge_time, void* stream) {
   HGT_REQUIRE(h_state && mem_out, "hgt_gsample_hash_rebuild_write: bad arguments");
   return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {mem_out, 0}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
+                       self_rel, {mem_out}, max_rows, false, nullptr, 0, feat, feat_dim, node_type, node_time,
                        node_feature, edge_index, edge_type, edge_time, stream, "hgt_gsample_hash_rebuild_write");
 }
 
@@ -1602,7 +1498,7 @@ extern "C" int hgt_gsample_hash_rebuild_write_host(
     float* node_feature, int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* stream) {
   HGT_REQUIRE(h_state && mem_out && n_hits >= 0, "hgt_gsample_hash_rebuild_write_host: bad arguments");
   return rebuild_write(*h_state, blocks, n_blocks, min_ser, cnt_off, ex, blk_out, node_off, type_out, self_off,
-                       self_rel, {mem_out, 0}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
+                       self_rel, {mem_out}, max_rows, true, (const Hit*)hits, n_hits, feat, feat_dim, node_type,
                        node_time, node_feature, edge_index, edge_type, edge_time, stream,
                        "hgt_gsample_hash_rebuild_write_host");
 }

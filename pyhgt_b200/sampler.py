@@ -504,15 +504,11 @@ class _GBlock(_c.Structure):                 # hgt_gsample_block (include/hgt_b2
                 ("rel", _c.c_int32)]
 
 
-class _GState(_c.Structure):                 # hgt_gsample_state
-    _PTRS = ("type_off", "lid_off", "ser", "ltime", "lid", "n_layer", "score", "btime", "bstamp", "last_seq",
-             "first_seq", "type_min", "type_seq", "counters")
-    _fields_ = [("num_types", _c.c_int32), ("pad", _c.c_int32)] + [(n, _c.c_void_p) for n in _PTRS]
-
-
 class _GBatchState(_c.Structure):            # hgt_gsample_batch_state
     _fields_ = ([("num_types", _c.c_int32), ("n_members", _c.c_int32)] +
-                [(n, _c.c_void_p) for n in _GState._PTRS + ("seed",)])
+                [(n, _c.c_void_p) for n in ("type_off", "lid_off", "ser", "ltime", "lid", "n_layer", "score", "btime",
+                                            "bstamp", "last_seq", "first_seq", "type_min", "type_seq", "counters",
+                                            "seed")])
 
 
 class _GHashState(_c.Structure):             # hgt_gsample_hash_state
@@ -1308,26 +1304,23 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
         _lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
         rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
         ex = torch.empty(n_count + 1, **i64)
-        # the mask table rides behind cnt_off in the same copy; the dense masked entry points take it right after
-        # n_blocks, the hashed ones always (NULL: no mask)
+        # the mask table rides behind cnt_off in the same copy (NULL: no mask)
         cnt_off_d = _plan._to_dev_async(cnt_off if min_ser is None else np.concatenate([cnt_off, min_ser]), dev)
-        masked = () if min_ser is None else (cnt_off_d.data_ptr() + 8 * cnt_off.shape[0],)
-        suffix = "" if min_ser is None else "_masked"
+        mask_p = None if min_ser is None else cnt_off_d.data_ptr() + 8 * cnt_off.shape[0]
         feat_rows_p = _lib.ptr(dg.feat_rows) if dg.features is not None else None
         if host:
             # single-read count pass: the kept edges' hit records (16 bytes each) stay in device scratch for the write
             # pass
             hit_cap = _hit_capacity(dg, n_count)
             hits = torch.empty(16 * max(hit_cap, 1), dtype=torch.uint8, device=dev)
-            _lib.call(api + "rebuild_count_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
-                      masked[0] if masked else None, cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p,
-                      hits.data_ptr(), hit_cap, meta[o_hit:o_hit + 1].data_ptr(), ex.data_ptr(), totals.data_ptr(),
-                      flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
+            _lib.call(api + "rebuild_count_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p,
+                      cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, hits.data_ptr(), hit_cap,
+                      meta[o_hit:o_hit + 1].data_ptr(), ex.data_ptr(), totals.data_ptr(), flags.data_ptr(),
+                      rb.data_ptr(), rb.numel(), st)
         else:
-            mask_arg = (masked[0] if masked else None,) if hashed else masked
-            _lib.call(api + "rebuild_count" + ("" if hashed else suffix), _c.byref(cst), dg.blocks_dev.data_ptr(),
-                      NB, *mask_arg, cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, ex.data_ptr(),
-                      totals.data_ptr(), flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
+            _lib.call(api + "rebuild_count", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p,
+                      cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, ex.data_ptr(), totals.data_ptr(),
+                      flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
         h = meta.cpu().numpy()
         fl = h[o_fl:o_hit].view(np.int32)
         if fl[3]:
@@ -1380,17 +1373,17 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
         n_hits = int(h[o_hit])
         _grow_hit_room(dg, n_hits, n_count)
         fits = n_hits <= hit_cap                          # else the write pass re-reads the neighbour lists
-        _lib.call(api + "rebuild_write_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
-                  masked[0] if masked else None, cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"),
-                  d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
+        _lib.call(api + "rebuild_write_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p,
+                  cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
+                  d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
                   hits.data_ptr() if fits else None, n_hits if fits else 0,
                   _lib.ptr(dg.feat_ptrs) if fp32_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
                   node_time.data_ptr(), _lib.ptr(fp32_feature), edge_index.data_ptr(), edge_type.data_ptr(),
                   edge_time.data_ptr(), st)
     else:
-        _lib.call(api + "rebuild_write" + ("" if hashed else suffix), _c.byref(cst), dg.blocks_dev.data_ptr(), NB,
-                  *mask_arg, cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
-                  d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
+        _lib.call(api + "rebuild_write", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p, cnt_off_d.data_ptr(),
+                  ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel,
+                  d.ptr("mem_out"), max_rows,
                   _lib.ptr(dg.feat_ptrs) if fp32_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
                   node_time.data_ptr(), _lib.ptr(fp32_feature), edge_index.data_ptr(), edge_type.data_ptr(),
                   edge_time.data_ptr(), st)

@@ -1,45 +1,39 @@
-"""CPU-side checks of the edge-masked rebuild: the masked entry points exist and check their arguments, the unmasked
-ones keep their ABI, and sample_subgraphs_cuda's edge_mask is validated before anything reaches a device."""
+"""CPU-side checks of the edge-masked rebuild: the dense rebuild entry points take the mask table where the hashed ones
+do and check their arguments, and sample_subgraphs_cuda's edge_mask is validated before anything reaches a device."""
 import ctypes
 
 import pytest
 
 
-def test_masked_rebuild_entry_points_and_argument_checks():
+def test_rebuild_entry_points_take_the_mask_and_check_their_arguments():
     import __graft_entry__ as ge
     ge.build()
     from pyhgt_b200 import _lib
     lib = _lib.load()
-    assert lib.hgt_abi_version() == 4
-    for name in ("hgt_gsample_batch_rebuild_count_masked", "hgt_gsample_batch_rebuild_write_masked",
-                 "hgt_gsample_batch_rebuild_count", "hgt_gsample_batch_rebuild_write"):
+    assert lib.hgt_abi_version() == 5
+    for name in ("hgt_gsample_batch_rebuild_count", "hgt_gsample_batch_rebuild_write"):
         assert hasattr(lib, name) and name in _lib.SIGNATURES
-    # the masked twins take min_ser right after n_blocks; the rest is the unmasked signature
+    # dense and hashed rebuild passes take the same arguments, min_ser (NULL: no mask) right after n_blocks
     for name in ("count", "write"):
-        plain = _lib.SIGNATURES["hgt_gsample_batch_rebuild_%s" % name]
-        twin = _lib.SIGNATURES["hgt_gsample_batch_rebuild_%s_masked" % name]
-        assert twin[:3] + twin[4:] == plain and twin[3] is ctypes.c_void_p
+        dense = _lib.SIGNATURES["hgt_gsample_batch_rebuild_%s" % name]
+        assert dense == _lib.SIGNATURES["hgt_gsample_hash_rebuild_%s" % name] and dense[3] is ctypes.c_void_p
     from pyhgt_b200 import sampler
     st = sampler._GBatchState()
     st.num_types, st.n_members = 2, 1
-    with pytest.raises(_lib.HgtError, match="count_masked"):           # NULL state
-        _lib.call("hgt_gsample_batch_rebuild_count_masked", None, None, 0, None, None, 0, 0, None, None, None, None,
-                  None, 0, None)
-    with pytest.raises(_lib.HgtError, match="count_masked"):           # NULL mask table
-        _lib.call("hgt_gsample_batch_rebuild_count_masked", ctypes.byref(st), None, 0, None, None, 0, 0, None, None,
-                  None, None, None, 0, None)
-    with pytest.raises(_lib.HgtError, match="write_masked"):           # NULL mask table
-        _lib.call("hgt_gsample_batch_rebuild_write_masked", ctypes.byref(st), None, 0, None, None, None, None, None,
-                  None, None, 0, 8, 0, None, 0, None, None, None, None, None, None, None)
-    with pytest.raises(_lib.HgtError, match="write_masked"):           # NULL member table
-        _lib.call("hgt_gsample_batch_rebuild_write_masked", ctypes.byref(st), None, 0, 8, None, None, None, None,
-                  None, None, 0, None, 0, None, 0, None, None, None, None, None, None, None)
+    with pytest.raises(_lib.HgtError, match="batch_rebuild_count"):    # NULL state
+        _lib.call("hgt_gsample_batch_rebuild_count", None, None, 0, None, None, 0, 0, None, None, None, None, None, 0,
+                  None)
+    with pytest.raises(_lib.HgtError, match="batch_rebuild_write"):    # NULL state
+        _lib.call("hgt_gsample_batch_rebuild_write", None, None, 0, None, None, None, None, None, None, None, 0, 8, 0,
+                  None, 0, None, None, None, None, None, None, None)
+    with pytest.raises(_lib.HgtError, match="batch_rebuild_write"):    # NULL member table
+        _lib.call("hgt_gsample_batch_rebuild_write", ctypes.byref(st), None, 0, 8, None, None, None, None, None,
+                  None, 0, None, 0, None, 0, None, None, None, None, None, None, None)
 
 
 def test_struct_layouts_are_unchanged():
     from pyhgt_b200 import sampler
     assert ctypes.sizeof(sampler._GBlock) == 5 * 8 + 4 * 4
-    assert ctypes.sizeof(sampler._GState) == 8 + 14 * 8
     assert ctypes.sizeof(sampler._GBatchState) == 8 + 15 * 8
 
 

@@ -182,40 +182,44 @@ def test_a_rule_on_a_never_sampled_target_type_has_no_effect():
         _assert_bitwise(sampler.sample_subgraph_cuda(dg, fx["time_range"], 1, 8, inp, _gen(s), edge_mask=mask), plain)
 
 
-def _spy(monkeypatch):
+def _spy(monkeypatch, rebuild_masks=None):
+    """Records the name of every C-ABI call, and into rebuild_masks the min_ser argument of every rebuild pass."""
     from pyhgt_b200 import _lib
     calls, real = [], _lib.call
 
     def spy(name, *args):
         calls.append(name)
+        if rebuild_masks is not None and name.endswith(("_rebuild_count", "_rebuild_write")):
+            rebuild_masks.append(args[3])
         return real(name, *args)
 
     monkeypatch.setattr(_lib, "call", spy)
     return calls
 
 
-def test_no_mask_runs_the_unmasked_kernels_and_a_mask_swaps_only_the_rebuild(monkeypatch):
-    """edge_mask=None and {} call the same entry points (none of them masked), launch as many kernels and give the same
-    batch; a mask replaces the two rebuild passes by their masked twins and changes no other sampler call."""
+def test_no_mask_passes_no_table_and_a_mask_changes_only_the_rebuild_argument(monkeypatch):
+    """edge_mask=None and {} make the same calls with no mask table (min_ser NULL), launch as many kernels and give the
+    same batch; a mask makes the same sampler calls and hands both rebuild passes one table."""
     from pyhgt_b200 import _lib, sampler
     fx, fg, dg, big = _graph("sampler_large")
     inps = _inps(fx, fg, big, 5)
-    calls = _spy(monkeypatch)
+    masks = []
+    calls = _spy(monkeypatch, masks)
     runs = {}
     for label, mask in (("none", None), ("empty", {}), ("mask", _rules(16)["paper_venue"])):
-        del calls[:]
+        del calls[:], masks[:]
         k0 = _lib.kernel_launches()
         out = sampler.sample_subgraphs_cuda(dg, fx["time_range"], 4, 32, inps, _gen(3), edge_mask=mask)
-        runs[label] = (list(calls), _lib.kernel_launches() - k0, out)
+        runs[label] = (list(calls), _lib.kernel_launches() - k0, out, list(masks))
     assert runs["none"][0] == runs["empty"][0] and runs["none"][1] == runs["empty"][1]
-    assert not any(n.endswith("_masked") for n in runs["none"][0])
     for a, b in zip(runs["none"][2], runs["empty"][2]):
         _assert_bitwise(a, b)
-    rename = {"hgt_gsample_batch_rebuild_count": "hgt_gsample_batch_rebuild_count_masked",
-              "hgt_gsample_batch_rebuild_write": "hgt_gsample_batch_rebuild_write_masked"}
+    assert runs["none"][3] == runs["empty"][3] == [None, None]
     # the plan builds that follow see other edges, so only the sampler's own calls are compared
     sampler_calls = lambda names: [n for n in names if n.startswith("hgt_gsample")]
-    assert sampler_calls(runs["mask"][0]) == [rename.get(n, n) for n in sampler_calls(runs["none"][0])]
+    assert sampler_calls(runs["mask"][0]) == sampler_calls(runs["none"][0])
+    count_mask, write_mask = runs["mask"][3]
+    assert count_mask is not None and count_mask == write_mask
 
 
 @pytest.mark.parametrize("mask,err", [

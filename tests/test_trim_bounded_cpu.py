@@ -46,7 +46,7 @@ def test_views_from_hand_made_bounds():
 
 def test_bounded_entry_point_argument_checks():
     lib = _lib()
-    assert lib.load().hgt_abi_version() == 4
+    assert lib.load().hgt_abi_version() == 5
     assert "hgt_trim_layout_bounded" in lib.SIGNATURES and hasattr(lib.load(), "hgt_trim_layout_bounded")
     assert len(lib.SIGNATURES["hgt_trim_layout_bounded"]) == len(lib.SIGNATURES["hgt_trim_layout"]) + 2
     T, R, L, N, E = 2, 3, 2, 10, 0
