@@ -1050,6 +1050,23 @@ int hgt_ingest_block_write(const int64_t* tgt, const int64_t* src, const int64_t
                            int64_t n_entries, int32_t narrow, int64_t no_time, void* row_of, int64_t n_row_of, void* ptr,
                            void* nbr, void* time_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Node features derived from the sampler's blocks (sampler.py: mag_features, the ogbn-mag preprocessing rules).
+ * `blocks` is a DEVICE array of n_blocks descriptors (the DeviceGraph's own, device- or host-placed, narrow or wide),
+ * all with one target type of n_nodes ids; a block's row_of may be shorter than n_nodes (ids past it have no row).
+ * hgt_feat_degree: deg[id] (DEVICE int64 [n_nodes]) = the sum over the blocks of id's row length, an integer sum, and
+ * out[id * ld_out] = (float)log10((double)deg[id]), -inf for 0.
+ * hgt_feat_neighbour_mean: for each id, the mean of the source rows src[s * src_ld + 0 .. feat_dim) over every entry s of
+ * id's rows in the given blocks, in block order (a pair in two blocks counts twice), summed in fp64 in a fixed order
+ * and divided by the entry count; zero for an id with no entries.  src is a DEVICE fp32 table, or fp64 when src_fp64,
+ * and every neighbour id must be a row of it (not checked).  The mean is written as fp64 to out64 (row stride ld64)
+ * and/or, rounded once, as fp32 to out32 (row stride ld32); either may be NULL, not both.  Both passes are bitwise
+ * repeatable; nothing is allocated or synchronised. */
+int hgt_feat_degree(const hgt_gsample_block* blocks, int32_t n_blocks, int64_t n_nodes, int64_t* deg, float* out,
+                    int64_t ld_out, void* stream);
+int hgt_feat_neighbour_mean(const hgt_gsample_block* blocks, int32_t n_blocks, int64_t n_nodes, const void* src,
+                            int32_t src_fp64, int64_t src_ld, int32_t feat_dim, double* out64, int64_t ld64,
+                            float* out32, int64_t ld32, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

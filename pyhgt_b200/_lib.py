@@ -146,6 +146,9 @@ SIGNATURES = {
     "hgt_ingest_workspace_bytes": [_i64, _c.POINTER(_sz)],
     "hgt_ingest_block_sort": [_p, _p, _p, _i64, _i64, _i64, _p, _p, _sz, _p],
     "hgt_ingest_block_write": [_p, _p, _p, _i64, _i64, _i64, _i32, _i64, _p, _i64, _p, _p, _p, _p, _sz, _p],
+    # ogbn-mag node features from the sampler's blocks (sampler.mag_features)
+    "hgt_feat_degree": [_p, _i32, _i64, _p, _p, _i64, _p],
+    "hgt_feat_neighbour_mean": [_p, _i32, _i64, _p, _i32, _i64, _i32, _p, _i64, _p, _i64, _p],
     # trimmed forward (GNN.forward(out_nodes=), trim.py)
     "hgt_trim_layout": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_trim_layout_bounded": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _i64, _p, _p, _p, _p, _p,

@@ -10,7 +10,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB_PATH = os.path.join(HERE, "libhgt_b200.so")
-SOURCES = ["common.cu", "plan.cu", "linear.cu", "linear_tc.cu", "edge.cu", "edge_bwd.cu", "update.cu", "layer.cu", "linear_bwd.cu", "update_bwd.cu", "sampler.cu", "gsample.cu", "merge.cu", "ingest.cu"]
+SOURCES = ["common.cu", "plan.cu", "linear.cu", "linear_tc.cu", "edge.cu", "edge_bwd.cu", "update.cu", "layer.cu", "linear_bwd.cu", "update_bwd.cu", "sampler.cu", "gsample.cu", "merge.cu", "ingest.cu", "features.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 

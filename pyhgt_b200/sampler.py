@@ -924,9 +924,21 @@ class DeviceGraph:
         self.type_block_range = torch.from_numpy(rng).to(dev)
         self.features, self.feat_dim = None, 0
         if features is not None:
-            dims = {int(v.shape[1]) for v in features.values()}
-            if len(dims) != 1:
-                raise ValueError("feature tables must all have the same width, got %s" % sorted(dims))
+            self.set_features(features)
+
+    def set_features(self, features):
+        """Place the per-type feature tables ``{type: Tensor[rows, F]}`` (row = node id; every table of one width F) that
+        the sampled batches' ``node_feature`` is gathered from, as the constructors' ``features=`` does: stored at
+        ``feature_dtype`` (bf16 rounded once from float32), on the device or in pinned host memory as ``placement``
+        says.  A type without a table gathers no features.  Replaces the tables of an earlier call (on host placement
+        their pinned copies stay registered until the graph is collected).  Typical use builds the graph with
+        ``from_edges`` and then sets ``mag_features(dg, x, num_nodes)``.  Raises ValueError for tables of unequal width."""
+        import torch
+        dev = self.device
+        dims = {int(v.shape[1]) for v in features.values()}
+        if len(dims) != 1:
+            raise ValueError("feature tables must all have the same width, got %s" % sorted(dims))
+        with self._placing():
             self.feat_dim = dims.pop()
             bf16 = self.feature_dtype == torch.bfloat16
             tabs, ptrs, rows = {}, [], []
@@ -967,6 +979,99 @@ class DeviceGraph:
             return a.nbytes if isinstance(a, np.ndarray) else a.numel() * a.element_size()
         feats = sum(nbytes(v) for v in self.features.values()) if self.features is not None else 0
         return {"adjacency": sum(nbytes(a) for a in self._adjacency), "features": feats, "placement": self.placement}
+
+
+def _block_run(dg, t, s=None):
+    """(address of the first descriptor in dg.blocks_dev, count, entries) of dg's blocks into type t (from type s when
+    given).  They are contiguous: blocks are in edge_list order, target type, then source type, then relation."""
+    ti, si = dg.slot.get(t), dg.slot.get(s)
+    run = [b for b, (tt, st, _) in enumerate(dg.blocks) if tt == ti and (s is None or st == si)]
+    if ti is None or (s is not None and si is None) or not run:
+        return 0, 0, 0
+    assert run == list(range(run[0], run[-1] + 1)), (t, s, run)
+    entries = sum(int(dg._adjacency[4 * b + 2].shape[0]) for b in run)
+    return dg.blocks_dev.data_ptr() + run[0] * _c.sizeof(_GBlock), len(run), entries
+
+
+def mag_features(dg, x_paper, num_nodes):
+    """The node-feature tables of the ogbn-mag preprocessing (preprocess_ogbn_mag.py:45-99), computed on the device from
+    the blocks of ``dg`` (a ``DeviceGraph``, typically ``DeviceGraph.from_edges`` of OGB's ``edge_index_dict``):
+    ``{type: float32 Tensor[num_nodes[type], F + 1]}`` on ``dg.device``, F = ``x_paper.shape[1]``, for
+    ``dg.set_features``.  The rules are the script's over its dict graph, whose blocks ``dg`` holds:
+
+      * paper: ``x_paper`` || log10(deg);
+      * every other type of ``num_nodes`` but institution, in ``num_nodes`` order: the mean of the ``x_paper`` rows of
+        its paper neighbours || log10(deg); a type with no paper neighbour gets no table;
+      * institution: the mean of its authors' means (their float64 values, without the degree column) || log10(deg);
+        no table when it has no author neighbour or author has no table.
+
+    A neighbour list is the union of the node's rows in every block from the source type, in block order: a pair
+    repeated inside one relation counts once (the block holds it once), a pair under two relations counts twice (the
+    script's COO matrix sums duplicates), and the mean divides by that pair count; a node without pairs gets a zero
+    row.  deg counts the node's row length in every block into its type, ``rev_`` blocks included; a node without edges
+    has log10(0) = -inf.  The means are summed in float64 in a fixed order and rounded once to float32, the degrees are
+    integer sums (csrc/features.cu), so the result is bitwise repeatable.  Host-placed blocks are read in place.
+
+    ``x_paper``: a float32 or float64 [num_nodes['paper'], F] tensor on any device (copied to ``dg.device`` when it is
+    elsewhere).  ``num_nodes``: ``{type: node count}`` (OGB's ``num_nodes_dict``), at least the graph's id range of each
+    of its types.  Device memory at the peak: the tables (4 (F + 1) bytes per node of each type with a table), the paper
+    source (x_paper's bytes when it is copied), the float64 author means while institution reads them (8 F bytes per
+    author) and one int64 degree per node of the largest type; at ogbn-mag's sizes with F = 128 about 1.0 + 0.38 + 1.16
+    GB, 2.5 GB (by shape arithmetic).  Nothing is read back: the calls are queued on the current stream.
+
+    Raises ValueError when ``num_nodes`` has no 'paper', when a type's count is below the graph's id range of it (a type
+    the graph has ids for must be in ``num_nodes``), or when ``x_paper`` is not a 2-D float32 / float64 tensor of
+    ``num_nodes['paper']`` rows."""
+    import torch
+    from . import _lib
+    if "paper" not in num_nodes:
+        raise ValueError("num_nodes must count the 'paper' nodes, got types %r" % (list(num_nodes),))
+    if (not isinstance(x_paper, torch.Tensor) or x_paper.dim() != 2 or
+            x_paper.dtype not in (torch.float32, torch.float64) or x_paper.shape[0] != int(num_nodes["paper"])):
+        raise ValueError("x_paper must be a 2-D float32 or float64 tensor of num_nodes['paper'] = %d rows, got %s" % (
+            int(num_nodes["paper"]), "%s %s" % (x_paper.dtype, list(x_paper.shape)) if isinstance(x_paper, torch.Tensor)
+            else type(x_paper).__name__))
+    for t, n in zip(dg.types, dg.n_ids):
+        if n > int(num_nodes.get(t, 0)):
+            raise ValueError("num_nodes[%r] = %s is below the graph's id range of %r (%d ids)" % (
+                t, num_nodes.get(t), t, n))
+    dev, F = dg.device, int(x_paper.shape[1])
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream(dev).cuda_stream
+        src = x_paper.to(dev).contiguous()
+        fp64 = int(src.dtype == torch.float64)
+
+        def table(t):
+            n = int(num_nodes[t])
+            out = torch.empty(n, F + 1, dtype=torch.float32, device=dev)
+            deg = torch.empty(n, dtype=torch.int64, device=dev)
+            blocks, n_blocks, _ = _block_run(dg, t)
+            _lib.call("hgt_feat_degree", blocks, n_blocks, n, deg.data_ptr(), out.data_ptr() + 4 * F, F + 1, st)
+            return out
+
+        def mean(out, t, s, source, source_fp64, keep64=False):
+            blocks, n_blocks, _ = _block_run(dg, t, s)
+            out64 = torch.empty(out.shape[0], F, dtype=torch.float64, device=dev) if keep64 else None
+            _lib.call("hgt_feat_neighbour_mean", blocks, n_blocks, out.shape[0], source.data_ptr(), source_fp64, F, F,
+                      _lib.ptr(out64), F, out.data_ptr(), F + 1, st)
+            return out64
+
+        tables = {"paper": table("paper")}
+        tables["paper"][:, :F] = src
+        inst = "institution" in num_nodes and _block_run(dg, "institution", "author")[2] > 0
+        author64 = None
+        for t in num_nodes:
+            if t in ("paper", "institution") or _block_run(dg, t, "paper")[2] == 0:
+                continue
+            tables[t] = table(t)
+            m64 = mean(tables[t], t, "paper", src, fp64, keep64=inst and t == "author")
+            if t == "author":
+                author64 = m64
+        del src
+        if inst and author64 is not None:
+            tables["institution"] = table("institution")
+            mean(tables["institution"], "institution", "author", author64, 1)
+    return tables
 
 
 def _device_seeds(dg, inp):
