@@ -873,10 +873,13 @@ int hgt_gsample_batch_rebuild_count(const hgt_gsample_batch_state* h_state, cons
                                     int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
 /* Pass 2: the to_torch layout (data.py:226-256) of every member.  Member-local tables: node_off [B*T]: first output row
  * of each type (-1 = not laid out), type_out [T]: its node_type value; self_off [B*T]: first edge of its self loops (-1
- * = none), blk_out [B*n_blocks]: first edge of each block's edges (-1 = none).  mem_out [B*3] (device): member b's
- * {first node row, first edge, edge count} in the shared outputs.  edge_type / edge_time [edges], node_type / node_time
- * [rows]; member b's edge_index is the [2, E_b] block (row 0 = source) at edge_index + 2 * first edge, with
- * member-local node ids: each member is exactly a to_torch layout.  node_feature [rows, feat_dim] gathered from feat[t]
+ * = none), blk_out [B*n_blocks]: first edge of each block's edges (-1 = none).  mem_out [B*4] (device): member b's
+ * {first node row, first edge, position of its first source, position of its first destination} in the shared outputs
+ * (four columns since the fixed-shape sampler below: before it, three, {first node row, first edge, edge count}):
+ * its edge e has edge_type / edge_time at first edge + e and edge_index[src + e] / [dst + e].  edge_type / edge_time
+ * [edges], node_type / node_time [rows].  Node ids in edge_index are node_off + ser (without the first node row):
+ * sample_subgraphs_cuda passes {node_base, edge_base, 2 * edge_base, 2 * edge_base + E_b}, so that member b's
+ * edge_index is the [2, E_b] block at edge_index + 2 * edge_base with member-local ids, exactly a to_torch layout.  node_feature [rows, feat_dim] gathered from feat[t]
  * (a DEVICE array of T device pointers to [ids, feat_dim] float tables) or NULL. */
 int hgt_gsample_batch_rebuild_write(const hgt_gsample_batch_state* h_state, const hgt_gsample_block* blocks,
                                     int32_t n_blocks, const int64_t* min_ser, const int64_t* cnt_off, const int64_t* ex,
@@ -922,7 +925,7 @@ typedef struct {
 } hgt_gsample_hash_state;
 
 /* The seeds (data.py:135-137): seed i of region[i] = b*T + t (device arrays [n]) gets an entry for id[i] with ser[i],
- * and lid / ltime at position ser[i] of that (member, type). */
+ * and lid / ltime at position ser[i] of that (member, type).  region[i] < 0: no seed (padding of a fixed-size table). */
 int hgt_gsample_hash_insert_seeds(const hgt_gsample_hash_state* h_state, int64_t n, const int64_t* region,
                                   const int64_t* id, const int64_t* ser, const int64_t* time, int32_t* flags,
                                   void* stream);
@@ -933,8 +936,10 @@ int hgt_gsample_hash_add_budget(const hgt_gsample_hash_state* h_state, const hgt
                                 const int64_t* n_targets, int64_t sampled_number, int32_t time_filter, int64_t max_time,
                                 int64_t no_time, int32_t* flags, void* workspace, size_t workspace_bytes, void* stream);
 /* As hgt_gsample_batch_select, over the selected type's REGION instead of its id range: sel_off [B+1] (device) are
- * prefix sums of the region sizes (n_total = sel_off[B] < 2^31 - 1, max_room >= every region size).  The budget entries
- * are ordered by id first, so keys and ties are exactly those of the dense selection. */
+ * prefix sums of the region sizes (max_room >= every region size).  The budget entries are ordered by id first, so keys
+ * and ties are exactly those of the dense selection.  n_total (< 2^31 - 1) is the number of sorted positions: sel_off[B],
+ * or, when the regions are chosen on the device, an upper bound of it up to B * max_room; the positions past sel_off[B]
+ * are padding that sorts behind every entry, and the selection is the one n_total = sel_off[B] makes. */
 int hgt_gsample_hash_select_workspace_bytes(int32_t n_members, int64_t n_total, size_t* out_bytes);
 int hgt_gsample_hash_select(const hgt_gsample_hash_state* h_state, const int32_t* type, const int64_t* step,
                             const int64_t* sel_off, int64_t n_total, int64_t max_room, int64_t sampled_number,
@@ -996,7 +1001,7 @@ int hgt_gsample_batch_rebuild_write_host(const hgt_gsample_batch_state* h_state,
 
 /* Feature rows from bf16 tables (sampler.py: DeviceGraph(..., feature_dtype=torch.bfloat16)), run after a rebuild write
  * pass that was given feat = NULL: node_feature[i, :] = the widening to float of feat[row_type[i]][row_id[i], :] for the
- * n_rows output rows.  feat is a DEVICE array of per-type pointers to [ids, feat_dim] bf16 tables (device memory or
+ * n_rows output rows (a row with row_id[i] < 0 is left as it is).  feat is a DEVICE array of per-type pointers to [ids, feat_dim] bf16 tables (device memory or
  * device-mapped host memory), row_type / row_id [n_rows] DEVICE arrays (a row's type slot and sampled id: the batch's
  * node_type and the sampled ids in output order).  Reads 16 bytes at a time where a row is 16-byte aligned, element by
  * element elsewhere.  Ids are not range-checked here: the rebuild count pass checks them against feat_rows. */
@@ -1007,6 +1012,44 @@ int hgt_gsample_gather_features_bf16(const uint16_t* const* feat, int32_t feat_d
  * 16-byte aligned at that point, 4 or 2 bytes where it is not. */
 int hgt_gsample_gather_rows_bf16(const uint16_t* const* feat, int32_t feat_dim, const int64_t* row_type,
                                  const int64_t* row_id, int64_t n_rows, void* node_feature, void* stream);
+
+/* Sampling with fixed shapes and no read-back (sampler.py: GraphedSampler): the host decisions of
+ * sample_subgraphs_cuda made on the device, so that a whole call can be captured in a CUDA graph.
+ *
+ * hgt_gsample_layer_order, after each layer's last add_budget: from type_seq [B*2T] (device, the state's first-touch
+ * numbers) member b's budget types in first-touch order go to type [T*B] (step k of the layer: type[k*B + b], -1 past
+ * the member's last type) with step numbers step [T*B] = next_step[b] + k; next_step [B] advances by the member's type
+ * count, and sel_off [T*(B+1)] holds, per step, the prefix sums over members of rooms [B*T] (region sizes) of the
+ * selected types.  Run T select + add_budget steps with these; a member with type -1 does nothing in a step.
+ *
+ * hgt_gsample_graphed_layout, after the rebuild count pass: the write pass's node_off [B*T], blk_out [B*n_blocks],
+ * self_off [B*T] and mem_out [B*4] that place every member in a padded signature layout, members joined type-major (as
+ * merge_batches): member b's type-t rows start at row0[t] + (type-t nodes of members before b), its edges follow those of
+ * the members before it, and edge_index is one [2, n_edges] array.  n_layer [B*T], type_seq [B*2T], totals [B*n_blocks]
+ * from the state and the count pass.  grp_off [T+1] / grp_blk [n_blocks]: target type t's blocks in the order its edges
+ * are laid out after its self loops.  blk_pair [n_blocks] / self_pair [T]: 0 when the block's (self loops') <source
+ * type, relation> pair is in the signature, else a nonzero code; has_feat [T]: 1 when type t has a feature table;
+ * type_cap [T]: the signature's rows of each type.  flags [8] (int32, device): [0..3] the sampler's, and the bounds this
+ * call sets: [4] = 1 + the first type over type_cap, [5] = 1 when the edges exceed n_edges, [6] = the first pair code
+ * met outside the signature, [7] = 1 + the first sampled type without a table.  With any flag set every table is -1 (the
+ * write pass then writes nothing) and *n_real_edges (device) is 0; otherwise it is the edge count.
+ *
+ * hgt_gsample_graphed_rows: node_id[node_off + r] = the sampled id of ser r of every laid-out (member, type); the other
+ * rows keep their value.  hgt_gsample_graphed_pad: edges n_real_edges.. n_edges - 1 become self loops on pad_node with
+ * type 0 and time 120; with any of flags [8] set, all n_values of feature (float32, or bf16 when bf16 != 0) become NaN. */
+int hgt_gsample_layer_order(const int64_t* type_seq, int32_t n_members, int32_t num_types, const int64_t* rooms,
+                            int64_t* next_step, int32_t* type, int64_t* step, int64_t* sel_off, void* stream);
+int hgt_gsample_graphed_layout(int32_t n_members, int32_t num_types, int32_t n_blocks, const int64_t* n_layer,
+                               const int64_t* type_seq, const int64_t* totals, const int32_t* grp_off,
+                               const int32_t* grp_blk, const int32_t* blk_pair, const int32_t* self_pair,
+                               const int32_t* has_feat, const int64_t* row0, const int64_t* type_cap, int64_t n_edges,
+                               int32_t* flags, int64_t* node_off, int64_t* blk_out, int64_t* self_off, int64_t* mem_out,
+                               int64_t* n_real_edges, void* stream);
+int hgt_gsample_graphed_rows(const hgt_gsample_hash_state* h_state, const int64_t* node_off, int64_t max_rows,
+                             int64_t* node_id, void* stream);
+int hgt_gsample_graphed_pad(const int64_t* n_real_edges, int64_t n_edges, int64_t pad_node, const int32_t* flags,
+                            int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* feature,
+                            int64_t n_values, int32_t bf16, void* stream);
 
 /* Disjoint union of B batches in the to_torch layout (sampler.py: merge_batches).  The member structs live in DEVICE
  * memory.  loc_off [B*(T+1)]: member b's first local row of each type (loc_off[b*(T+1)+T] = its node count); uoff [B*T]:

@@ -149,6 +149,12 @@ SIGNATURES = {
     # ogbn-mag node features from the sampler's blocks (sampler.mag_features)
     "hgt_feat_degree": [_p, _i32, _i64, _p, _p, _i64, _p],
     "hgt_feat_neighbour_mean": [_p, _i32, _i64, _p, _i32, _i64, _i32, _p, _i64, _p, _i64, _p],
+    # sampling with fixed shapes and no read-back (sampler.GraphedSampler)
+    "hgt_gsample_layer_order": [_p, _i32, _i32, _p, _p, _p, _p, _p, _p],
+    "hgt_gsample_graphed_layout": [_i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p,
+                                   _p, _p],
+    "hgt_gsample_graphed_rows": [_p, _p, _i64, _p, _p],
+    "hgt_gsample_graphed_pad": [_p, _i64, _i64, _p, _p, _p, _p, _p, _i64, _i32, _p],
     # trimmed forward (GNN.forward(out_nodes=), trim.py)
     "hgt_trim_layout": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "hgt_trim_layout_bounded": [_p, _p, _p, _p, _i64, _i64, _i32, _i32, _p, _i64, _i32, _p, _i64, _p, _p, _p, _p, _p,

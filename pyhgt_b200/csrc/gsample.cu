@@ -175,13 +175,15 @@ struct BlockRange {
   }
 };
 
-// Where member m's nodes and edges go in the output buffers: {node_base, edge_base, n_edges} per member.  Read-only
+// Where member m's nodes and edges go in the output buffers: {node_base, edge_base, src_pos, dst_pos} per member: its
+// edge e has edge_type / edge_time at edge_base + e and its endpoints at edge_index[src_pos + e] / [dst_pos + e].  Read-only
 // loads: with plain ones the hashed k_rb_write takes 52 registers instead of 48 (sm_90a, CUDA 12.9).
 struct MemOut {
   const int64_t* p;
-  __device__ __forceinline__ int64_t node_base(int m) const { return __ldg(p + 3 * m); }
-  __device__ __forceinline__ int64_t edge_base(int m) const { return __ldg(p + 3 * m + 1); }
-  __device__ __forceinline__ int64_t edges(int m) const { return __ldg(p + 3 * m + 2); }
+  __device__ __forceinline__ int64_t node_base(int m) const { return __ldg(p + 4 * m); }
+  __device__ __forceinline__ int64_t edge_base(int m) const { return __ldg(p + 4 * m + 1); }
+  __device__ __forceinline__ int64_t src_pos(int m) const { return __ldg(p + 4 * m + 2); }
+  __device__ __forceinline__ int64_t dst_pos(int m) const { return __ldg(p + 4 * m + 3); }
 };
 
 __device__ __forceinline__ uint64_t rnd64(curandStatePhilox4_32_10_t* s) {
@@ -465,11 +467,11 @@ __global__ void k_sel_finish(St st, const int32_t* type, int64_t width, const un
 
 // ---- the hashed state's own kernels: seeds and selection ------------------------------------------------------------
 
-// Seed i: an entry for id[i] in region[i] = m * T + t with its ser, and lid / ltime at that ser.
+// Seed i: an entry for id[i] in region[i] = m * T + t with its ser, and lid / ltime at that ser (region[i] < 0: none).
 __global__ void k_hash_seed(hgt_gsample_hash_state st, int64_t n, const int64_t* region, const int64_t* id,
                             const int64_t* ser, const int64_t* time, int32_t* flags) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= n || region[i] < 0) return;
   const int m = (int)(region[i] / st.num_types), t = (int)(region[i] % st.num_types);
   const HMember mb = member(st, m);
   const HashIx ix = type_ix(st, mb, t);
@@ -483,18 +485,35 @@ __global__ void k_hash_seed(hgt_gsample_hash_state st, int64_t n, const int64_t*
 constexpr int kIdBits = 41;                                             // ids < 2^40, plus "not in the budget"
 constexpr uint64_t kNotBudget = (uint64_t(1) << kIdBits) - 1;
 
+// A sort of n_total >= sel_off[B] positions (the caller's upper bound when the regions are chosen on the device): the
+// positions past sel_off[B] are padding, max_room - (member m's region size) of them per member, member after member.
+// Position of member m's padding j, or -1 when it lies past n_total (always so when n_total = sel_off[B]).
+__device__ __forceinline__ int64_t sel_pad_pos(const int64_t* sel_off, int B, int m, int64_t max_room, int64_t n_total,
+                                               int64_t j) {
+  const int64_t p = sel_off[B] + m * max_room - sel_off[m] + j;
+  return p < n_total ? p : -1;
+}
+
 // Selection pass 1: every entry of member m's region of type[m], at sel_off[m] + its index, gets the sort key
 // (m, id) when it is in the budget and (m, kNotBudget) otherwise, so that sorting puts each member's budget entries
-// first and in id order: the order of the dense selection's positions.  Counts the budget entries.
-__global__ void k_hsel_order(hgt_gsample_hash_state st, const int32_t* type, const int64_t* sel_off,
-                             uint64_t* okey, int64_t* oent, unsigned long long* count) {
+// first and in id order: the order of the dense selection's positions.  Counts the budget entries.  Padding positions
+// take the largest key, so they sort behind every member's entries.
+__global__ void k_hsel_order(hgt_gsample_hash_state st, const int32_t* type, const int64_t* sel_off, int64_t max_room,
+                             int64_t n_total, uint64_t* okey, int64_t* oent, unsigned long long* count) {
   const int m = blockIdx.y;
   const int t = type[m];
-  if (t < 0) return;
   const HMember mb = member(st, m);
-  const int64_t base = mb.type_off[t], n = mb.type_off[t + 1] - base, o = sel_off[m];
+  const int64_t base = t >= 0 ? mb.type_off[t] : 0, n = t >= 0 ? mb.type_off[t + 1] - base : 0, o = sel_off[m];
   unsigned long long c = 0;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < max_room; i += (int64_t)gridDim.x * blockDim.x) {
+    if (i >= n) {
+      const int64_t p = sel_pad_pos(sel_off, st.n_members, m, max_room, n_total, i - n);
+      if (p >= 0) {
+        okey[p] = ~0ULL;
+        oent[p] = -1;
+      }
+      continue;
+    }
     const bool in = st.bstamp[base + i] >= 0;
     okey[o + i] = ((uint64_t)m << kIdBits) | (in ? (uint64_t)st.key[base + i] : kNotBudget);
     oent[o + i] = base + i;
@@ -506,16 +525,23 @@ __global__ void k_hsel_order(hgt_gsample_hash_state st, const int32_t* type, con
 
 // k_sel_keys over the id-ordered entries: the first count[m] positions of member m are its budget, the node id is the
 // Philox counter's local id, so every key is bitwise the dense one.
-__global__ void k_hsel_keys(hgt_gsample_hash_state st, const int32_t* type, const int64_t* sel_off, int64_t width,
-                            const unsigned long long* count, const int64_t* step, const uint64_t* okey,
-                            const int64_t* oent, double* keys, int32_t* vals) {
+// Padding positions get key -inf, behind every budget key.
+__global__ void k_hsel_keys(hgt_gsample_hash_state st, const int32_t* type, const int64_t* sel_off, int64_t max_room,
+                            int64_t n_total, int64_t width, const unsigned long long* count, const int64_t* step,
+                            const uint64_t* okey, const int64_t* oent, double* keys, int32_t* vals) {
   const int m = blockIdx.y;
   const int t = type[m];
-  if (t < 0) return;
   const HMember mb = member(st, m);
-  const int64_t n = mb.type_off[t + 1] - mb.type_off[t];
+  const int64_t n = t >= 0 ? mb.type_off[t + 1] - mb.type_off[t] : 0;
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= n) {
+    const int64_t p = i < max_room ? sel_pad_pos(sel_off, st.n_members, m, max_room, n_total, i - n) : -1;
+    if (p >= 0) {
+      keys[p] = -INFINITY;
+      vals[p] = (int32_t)p;
+    }
+    return;
+  }
   const int64_t o = sel_off[m] + i;
   double key = -INFINITY;
   if (i < (int64_t)count[m]) {
@@ -638,8 +664,9 @@ __global__ void k_rb_write(St st, const hgt_gsample_block* blocks, int32_t n_blo
   const int64_t row = blk_row_of(blk, tid);
   if (row < 0) return;
   const int64_t* noff = node_off + (int64_t)m * st.num_types;
-  const int64_t eb = mo.edge_base(m), n_edges = mo.edges(m);
-  int64_t* ei = edge_index + 2 * eb;
+  const int64_t eb = mo.edge_base(m);
+  int64_t* ei_src = edge_index + mo.src_pos(m);
+  int64_t* ei_dst = edge_index + mo.dst_pos(m);
   int64_t e = blk_out[mbk] + ex[cnt_off[mbk] + r] - ex[cnt_off[mbk]];
   const int64_t a = blk_ptr(blk, row), end = blk_ptr(blk, row + 1);
   const int64_t tt = node_ltime(st, mb, T, tid, r);
@@ -657,8 +684,8 @@ __global__ void k_rb_write(St st, const hgt_gsample_block* blocks, int32_t n_blo
     const unsigned keep = __ballot_sync(kFull, kept);
     if (kept) {
       const int64_t o = e + __popc(keep & ((1u << lane) - 1u));
-      ei[o] = noff[S] + sser;                                           // row 0 = source (data.py:245,254)
-      ei[n_edges + o] = dst;
+      ei_src[o] = noff[S] + sser;                                       // row 0 = source (data.py:245,254)
+      ei_dst[o] = dst;
       edge_type[eb + o] = blk.rel;
       edge_time[eb + o] = tt - src_ltime(st, ix, sid, sser) + 120;        // data.py:250
     }
@@ -689,8 +716,8 @@ __global__ void k_rb_nodes(St st, const int64_t* node_off, const int64_t* type_o
     const int64_t so = self_off[(int64_t)m * st.num_types + t];
     if (so >= 0) {
       const int64_t e = so + r, eb = mo.edge_base(m);
-      edge_index[2 * eb + e] = lrow;
-      edge_index[2 * eb + mo.edges(m) + e] = lrow;
+      edge_index[mo.src_pos(m) + e] = lrow;
+      edge_index[mo.dst_pos(m) + e] = lrow;
       edge_type[eb + e] = self_rel;
       edge_time[eb + e] = 120;
     }
@@ -818,11 +845,11 @@ __global__ void k_rb_write_hits(St st, const hgt_gsample_block* blocks, int32_t 
   const auto mb = member(st, m);
   const int64_t r = h.y, sser = h.w;
   const int64_t* noff = node_off + (int64_t)m * st.num_types;
-  const int64_t eb = mo.edge_base(m), n_edges = mo.edges(m);
+  const int64_t eb = mo.edge_base(m);
   const int64_t o = blk_out[mbk] + ex[cnt_off[mbk] + r] - ex[cnt_off[mbk]] + h.z;
   const int64_t tid = st.lid[mb.lid_off[T] + r], sid = st.lid[mb.lid_off[S] + sser];
-  edge_index[2 * eb + o] = noff[S] + sser;                               // row 0 = source (data.py:245,254)
-  edge_index[2 * eb + n_edges + o] = noff[T] + r;
+  edge_index[mo.src_pos(m) + o] = noff[S] + sser;                        // row 0 = source (data.py:245,254)
+  edge_index[mo.dst_pos(m) + o] = noff[T] + r;
   edge_type[eb + o] = blocks[b].rel;
   edge_time[eb + o] = node_ltime(st, mb, T, tid, r) - node_ltime(st, mb, S, sid, sser) + 120;   // data.py:250
 }
@@ -850,8 +877,8 @@ __global__ void k_rb_nodes_host(St st, const int64_t* node_off, const int64_t* t
     const int64_t so = self_off[(int64_t)m * st.num_types + t];
     if (so >= 0) {
       const int64_t e = so + r, eb = mo.edge_base(m);
-      edge_index[2 * eb + e] = lrow;
-      edge_index[2 * eb + mo.edges(m) + e] = lrow;
+      edge_index[mo.src_pos(m) + e] = lrow;
+      edge_index[mo.dst_pos(m) + e] = lrow;
       edge_type[eb + e] = self_rel;
       edge_time[eb + e] = 120;
     }
@@ -897,7 +924,7 @@ __global__ void k_gather_bf16(const uint16_t* const* feat, int32_t feat_dim, con
                               const int64_t* row_id, int64_t n_rows, float* node_feature) {
   const int lane = threadIdx.x & 31;
   const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
-  if (i >= n_rows) return;
+  if (i >= n_rows || row_id[i] < 0) return;
   const uint16_t* src = feat[row_type[i]] + row_id[i] * (int64_t)feat_dim;
   float* dst = node_feature + i * (int64_t)feat_dim;
   int head = (int)((((uintptr_t)0 - (uintptr_t)src) & 15) >> 1);
@@ -940,7 +967,7 @@ __global__ void k_gather_rows_bf16(const uint16_t* const* feat, int32_t feat_dim
                                    const int64_t* row_id, int64_t n_rows, uint16_t* node_feature) {
   const int lane = threadIdx.x & 31;
   const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
-  if (i >= n_rows) return;
+  if (i >= n_rows || row_id[i] < 0) return;
   const uint16_t* src = feat[row_type[i]] + row_id[i] * (int64_t)feat_dim;
   uint16_t* dst = node_feature + i * (int64_t)feat_dim;
   int head = (int)((((uintptr_t)0 - (uintptr_t)src) & 15) >> 1);
@@ -1190,14 +1217,14 @@ int hash_select(const hgt_gsample_hash_state& hs, const int32_t* type, const int
   HGT_CHECK_CUDA(cudaMemsetAsync(s.count, 0, sizeof(unsigned long long) * B, st));
   if (n_total > 0 && max_room > 0) {
     const int64_t g = blocks_for(max_room);
-    k_hsel_order<<<dim3((unsigned)(g < 1024 ? g : 1024), B), kThreads, 0, st>>>(hs, type, sel_off, s.okey_in,
-                                                                                 s.oent_in, s.count);
+    k_hsel_order<<<dim3((unsigned)(g < 1024 ? g : 1024), B), kThreads, 0, st>>>(hs, type, sel_off, max_room, n_total,
+                                                                                 s.okey_in, s.oent_in, s.count);
     HGT_LAUNCH_CHECK();
     size_t tmp = s.cub_bytes;
     HGT_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(s.cub_tmp, tmp, s.okey_in, s.okey_out, s.oent_in, s.oent_out,
                                                    (int)n_total, 0, kIdBits + bits_for(B), st));
-    k_hsel_keys<<<dim3((unsigned)g, B), kThreads, 0, st>>>(hs, type, sel_off, sampled_number, s.count, step,
-                                                           s.okey_out, s.oent_out, s.keys_in, s.vals_in);
+    k_hsel_keys<<<dim3((unsigned)g, B), kThreads, 0, st>>>(hs, type, sel_off, max_room, n_total, sampled_number,
+                                                           s.count, step, s.okey_out, s.oent_out, s.keys_in, s.vals_in);
     HGT_LAUNCH_CHECK();
     const int32_t* vals = nullptr;
     if (int rc = sort_keys(s, n_total, B, sel_off, st, &vals)) return rc;
@@ -1447,7 +1474,8 @@ extern "C" int hgt_gsample_hash_select(const hgt_gsample_hash_state* h_state, co
                                        const int64_t* sel_off, int64_t n_total, int64_t max_room,
                                        int64_t sampled_number, int64_t* tgt_id, int64_t* tgt_time, int64_t* n_targets,
                                        int32_t* flags, void* workspace, size_t workspace_bytes, void* stream) {
-  HGT_REQUIRE(h_state && h_state->seed && type && step && sel_off && sampled_number > 0 && max_room >= 0,
+  HGT_REQUIRE(h_state && h_state->seed && type && step && sel_off && sampled_number > 0 && max_room >= 0 &&
+                  n_total <= (int64_t)h_state->n_members * max_room,
               "hgt_gsample_hash_select: bad arguments");
   return hash_select(*h_state, type, step, sel_off, n_total, max_room, sampled_number, tgt_id, tgt_time, n_targets,
                      flags, workspace, workspace_bytes, stream, "hgt_gsample_hash_select");
@@ -1526,6 +1554,216 @@ extern "C" int hgt_gsample_gather_rows_bf16(const uint16_t* const* feat, int32_t
   if (n_rows == 0 || feat_dim == 0) return 0;
   k_gather_rows_bf16<<<(unsigned)blocks_for(n_rows, kWarps), kThreads, 0, (cudaStream_t)stream>>>(
       feat, feat_dim, row_type, row_id, n_rows, static_cast<uint16_t*>(node_feature));
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- sampling with fixed shapes (sampler.py: GraphedSampler) --------------------------------------------------------
+// The host decisions of sample_subgraphs_cuda made on the device, so that a whole call can be captured in a CUDA graph.
+
+namespace {
+
+// One thread per member: its budget types in first-touch order (the reference's list(budget.keys()), data.py:150) as
+// steps k = 0.. of this layer, -1 past its last one; step numbers continue the member's counter, which advances by the
+// member's number of budget types.
+__global__ void k_layer_order(const int64_t* type_seq, int32_t n_members, int32_t num_types, int64_t* next_step,
+                              int32_t* type, int64_t* step) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n_members) return;
+  const int T = num_types, B = n_members;
+  const int64_t* ts = type_seq + (int64_t)m * 2 * T;
+  int k = 0;
+  for (long long last = -1;; ++k) {                                   // the next budget type after first-touch `last`
+    int best = -1;
+    long long bv = kNoSeq;
+    for (int t = 0; t < T; ++t)
+      if (ts[2 * t + 1] > last && ts[2 * t + 1] < bv) { bv = ts[2 * t + 1]; best = t; }
+    if (best < 0) break;
+    type[(int64_t)k * B + m] = best;
+    step[(int64_t)k * B + m] = next_step[m] + k;
+    last = bv;
+  }
+  for (int j = k; j < T; ++j) {
+    type[(int64_t)j * B + m] = -1;
+    step[(int64_t)j * B + m] = next_step[m] + j;
+  }
+  next_step[m] += k;
+}
+
+// After k_layer_order: sel_off [T, B+1] from the chosen regions (one thread per step).
+__global__ void k_layer_offsets(int32_t n_members, int32_t num_types, const int64_t* rooms, const int32_t* type,
+                                int64_t* sel_off) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= num_types) return;
+  const int B = n_members;
+  int64_t o = 0;
+  for (int m = 0; m < B; ++m) {
+    sel_off[(int64_t)k * (B + 1) + m] = o;
+    const int t = type[(int64_t)k * B + m];
+    if (t >= 0) o += rooms[(int64_t)m * num_types + t];
+  }
+  sel_off[(int64_t)k * (B + 1) + B] = o;
+}
+
+// The to_torch layout of every member (sampler.py: _member_layout) written into a signature's padded layout, members
+// joined type-major as merge_batches joins them: member m's type-t rows start at row0[t] + (type-t nodes of the members
+// before it), its edges follow the edges of the members before it, and edge_index is one [2, n_edges] array.  One
+// thread: B x (T + n_blocks) steps.  A count past a bound, a pair outside the signature, a sampled type without a
+// feature table, or any flag the sampler raised empties every table (-1), so the write pass writes nothing.
+__global__ void k_graphed_layout(int32_t n_members, int32_t num_types, int32_t n_blocks, const int64_t* n_layer,
+                                 const int64_t* type_seq, const int64_t* totals, const int32_t* grp_off,
+                                 const int32_t* grp_blk, const int32_t* blk_pair, const int32_t* self_pair,
+                                 const int32_t* has_feat, const int64_t* row0, const int64_t* type_cap,
+                                 int64_t n_edges, int32_t* flags, int64_t* node_off, int64_t* blk_out,
+                                 int64_t* self_off, int64_t* mem_out, int64_t* n_real_edges) {
+  if (blockIdx.x || threadIdx.x) return;
+  const int B = n_members, T = num_types, NB = n_blocks;
+  int64_t eb = 0;
+  for (int m = 0; m < B; ++m) {
+    const int64_t* nl = n_layer + (int64_t)m * T;
+    const int64_t* ts = type_seq + (int64_t)m * 2 * T;
+    for (int t = 0; t < T; ++t) {
+      int64_t before = 0;
+      for (int q = 0; q < m; ++q) before += n_layer[(int64_t)q * T + t];
+      node_off[(int64_t)m * T + t] = row0[t] + before;
+      self_off[(int64_t)m * T + t] = -1;
+      if (before + nl[t] > type_cap[t] && !flags[4]) flags[4] = t + 1;
+      if (nl[t] && !has_feat[t] && !flags[7]) flags[7] = t + 1;
+    }
+    for (int b = 0; b < NB; ++b) blk_out[(int64_t)m * NB + b] = -1;
+    int64_t E = 0;
+    for (long long last = -1;;) {                                     // layer_data key order (data.py:181-184)
+      int tt = -1;
+      long long bv = kNoSeq;
+      for (int t = 0; t < T; ++t)
+        if (ts[2 * t] > last && ts[2 * t] < bv) { bv = ts[2 * t]; tt = t; }
+      if (tt < 0) break;
+      last = bv;
+      if (nl[tt] == 0) continue;
+      self_off[(int64_t)m * T + tt] = E;
+      E += nl[tt];
+      if (self_pair[tt] > 0 && !flags[6]) flags[6] = self_pair[tt];
+      for (int g = grp_off[tt]; g < grp_off[tt + 1]; ++g) {
+        const int b = grp_blk[g];
+        const int64_t n = totals[(int64_t)m * NB + b];
+        if (!n) continue;
+        blk_out[(int64_t)m * NB + b] = E;
+        E += n;
+        if (blk_pair[b] > 0 && !flags[6]) flags[6] = blk_pair[b];
+      }
+    }
+    mem_out[4 * m] = 0;
+    mem_out[4 * m + 1] = eb;
+    mem_out[4 * m + 2] = eb;
+    mem_out[4 * m + 3] = n_edges + eb;
+    eb += E;
+  }
+  if (eb > n_edges) flags[5] = 1;
+  bool bad = false;
+  for (int f = 0; f < 8; ++f) bad |= flags[f] != 0;
+  *n_real_edges = bad ? 0 : eb;
+  if (!bad) return;
+  for (int64_t i = 0; i < (int64_t)B * T; ++i) node_off[i] = self_off[i] = -1;
+  for (int64_t i = 0; i < (int64_t)B * NB; ++i) blk_out[i] = -1;
+}
+
+// The sampled id of every laid-out row (node_id, -1 stays on the rest).  One thread per <member (z), type (y), ser>.
+template <class St>
+__global__ void k_graphed_rows(St st, const int64_t* node_off, int64_t* node_id) {
+  const int t = blockIdx.y, m = blockIdx.z;
+  const auto mb = member(st, m);
+  const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t noff = node_off[(int64_t)m * st.num_types + t];
+  if (noff < 0 || r >= mb.n_layer[t]) return;
+  node_id[noff + r] = st.lid[mb.lid_off[t] + r];
+}
+
+// Edges from n_real on become self loops on pad_node with type 0 and time 120 (graphed.py: _Graphed._scatter); when a
+// flag is set every feature value becomes NaN.
+__global__ void k_graphed_pad(const int64_t* n_real, int64_t n_edges, int64_t pad_node, const int32_t* flags,
+                              int64_t* edge_index, int64_t* edge_type, int64_t* edge_time, void* feature,
+                              int64_t n_values, int32_t bf16) {
+  const int64_t e0 = *n_real;
+  bool bad = false;
+  for (int f = 0; f < 8; ++f) bad |= flags[f] != 0;
+  const int64_t n = n_values > n_edges ? n_values : n_edges;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    if (i >= e0 && i < n_edges) {
+      edge_index[i] = pad_node;
+      edge_index[n_edges + i] = pad_node;
+      edge_type[i] = 0;
+      edge_time[i] = 120;
+    }
+    if (bad && i < n_values) {
+      if (bf16)
+        reinterpret_cast<uint16_t*>(feature)[i] = 0x7fc0;
+      else
+        reinterpret_cast<float*>(feature)[i] = __int_as_float(0x7fc00000);
+    }
+  }
+}
+
+}  // namespace
+
+extern "C" int hgt_gsample_layer_order(const int64_t* type_seq, int32_t n_members, int32_t num_types,
+                                       const int64_t* rooms, int64_t* next_step, int32_t* type, int64_t* step,
+                                       int64_t* sel_off, void* stream) {
+  HGT_REQUIRE(type_seq && rooms && next_step && type && step && sel_off && n_members >= 1 && n_members < 65536 &&
+                  num_types >= 1 && num_types < 65536,
+              "hgt_gsample_layer_order: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  k_layer_order<<<(unsigned)blocks_for(n_members, 32), 32, 0, st>>>(type_seq, n_members, num_types, next_step, type,
+                                                                     step);
+  HGT_LAUNCH_CHECK();
+  k_layer_offsets<<<(unsigned)blocks_for(num_types, 32), 32, 0, st>>>(n_members, num_types, rooms, type, sel_off);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int hgt_gsample_graphed_layout(int32_t n_members, int32_t num_types, int32_t n_blocks,
+                                          const int64_t* n_layer, const int64_t* type_seq, const int64_t* totals,
+                                          const int32_t* grp_off, const int32_t* grp_blk, const int32_t* blk_pair,
+                                          const int32_t* self_pair, const int32_t* has_feat, const int64_t* row0,
+                                          const int64_t* type_cap, int64_t n_edges, int32_t* flags, int64_t* node_off,
+                                          int64_t* blk_out, int64_t* self_off, int64_t* mem_out,
+                                          int64_t* n_real_edges, void* stream) {
+  HGT_REQUIRE(n_members >= 1 && num_types >= 1 && n_blocks >= 0 && n_edges >= 0 && n_layer && type_seq && totals &&
+                  grp_off && (grp_blk || n_blocks == 0) && (blk_pair || n_blocks == 0) && self_pair && has_feat &&
+                  row0 && type_cap && flags && node_off && (blk_out || n_blocks == 0) && self_off && mem_out &&
+                  n_real_edges,
+              "hgt_gsample_graphed_layout: bad arguments");
+  k_graphed_layout<<<1, 32, 0, (cudaStream_t)stream>>>(n_members, num_types, n_blocks, n_layer, type_seq, totals,
+                                                       grp_off, grp_blk, blk_pair, self_pair, has_feat, row0, type_cap,
+                                                       n_edges, flags, node_off, blk_out, self_off, mem_out,
+                                                       n_real_edges);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int hgt_gsample_graphed_rows(const hgt_gsample_hash_state* h_state, const int64_t* node_off,
+                                        int64_t max_rows, int64_t* node_id, void* stream) {
+  HGT_REQUIRE(h_state && node_off && node_id && max_rows >= 0 && h_state->num_types < 65536 &&
+                  h_state->n_members >= 1 && h_state->n_members < 65536,
+              "hgt_gsample_graphed_rows: bad arguments");
+  if (max_rows == 0 || h_state->num_types == 0) return 0;
+  k_graphed_rows<<<dim3((unsigned)blocks_for(max_rows), h_state->num_types, h_state->n_members), kThreads, 0,
+                   (cudaStream_t)stream>>>(*h_state, node_off, node_id);
+  HGT_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int hgt_gsample_graphed_pad(const int64_t* n_real_edges, int64_t n_edges, int64_t pad_node,
+                                       const int32_t* flags, int64_t* edge_index, int64_t* edge_type,
+                                       int64_t* edge_time, void* feature, int64_t n_values, int32_t bf16,
+                                       void* stream) {
+  HGT_REQUIRE(n_real_edges && flags && n_edges >= 0 && n_values >= 0 &&
+                  (n_edges == 0 || (edge_index && edge_type && edge_time)) && (n_values == 0 || feature),
+              "hgt_gsample_graphed_pad: bad arguments");
+  const int64_t n = n_values > n_edges ? n_values : n_edges;
+  if (n == 0) return 0;
+  const int64_t g = blocks_for(n);
+  k_graphed_pad<<<(unsigned)(g < 2048 ? g : 2048), kThreads, 0, (cudaStream_t)stream>>>(
+      n_real_edges, n_edges, pad_node, flags, edge_index, edge_type, edge_time, feature, n_values, bf16);
   HGT_LAUNCH_CHECK();
   return 0;
 }

@@ -160,9 +160,10 @@ def _check_targets(spec, targets, counts, device):
 
 
 class _Graphed:
-    """Static padded input buffers of one signature and the per-batch copy-in (host or device batches)."""
+    """Static padded input buffers of one signature and the per-batch copy-in (host or device batches).  With a
+    `sampler.GraphedSampler` the static buffers are the sampler's, and the captured graph starts with its sampling."""
 
-    def __init__(self, sig, device):
+    def __init__(self, sig, device, sampler=None):
         dev = torch.device(device)
         if dev.type != "cuda":
             raise _lib.HgtError("%s needs a CUDA device" % type(self).__name__)
@@ -182,6 +183,26 @@ class _Graphed:
         self._staged = None
         self._pins = []
         self.stream = torch.cuda.Stream(device=dev)
+        self.sampler = sampler
+        if sampler is not None:
+            if sampler.sig is not sig:
+                raise ValueError("sampler= must be a GraphedSampler built for this signature")
+            if sampler.x.device != dev:
+                raise ValueError("the sampler runs on %s, the graph on %s" % (sampler.x.device, dev))
+            self.x, self.nt, self.ei, self.et, self.tm = sampler.x, sampler.nt, sampler.ei, sampler.et, sampler.tm
+
+    def _sample(self):
+        if self.sampler is not None:
+            self.sampler.run()
+
+    def _refuse_batches(self):
+        if self.sampler is not None:
+            raise ValueError("%s(sampler=...) samples its own batches: call step(seeds, philox=None, ...)"
+                             % type(self).__name__)
+
+    def _need_sampler(self):
+        if self.sampler is None:
+            raise ValueError("step() needs a %s built with sampler=" % type(self).__name__)
 
     def _rebuild_plan(self):
         s = self.sig
@@ -302,18 +323,42 @@ class GraphedForward(_Graphed):
     buffers and check it: trim.get_layout(g.nt, g.ei, g.et, g.tm, rows, T, R, n_layers, tsig, g.plan.pairs).check().
     """
 
-    def __init__(self, fn, sig, device, per_node=True):
-        super().__init__(sig, device)
+    def __init__(self, fn, sig, device, per_node=True, sampler=None):
+        super().__init__(sig, device, sampler)
         self.fn = fn
         self.per_node = bool(per_node)
         self.out = None
 
     def _run(self):
+        self._sample()
         self._rebuild_plan()
         with torch.no_grad():
             return self.fn(self.x, self.nt, self.tm, self.ei, self.et)
 
+    def step(self, seeds, philox=None):
+        """With sampler=: sample `seeds` (as `GraphedSampler.fill`) and run the forward, as one graph replay with no host
+        synchronisation.  Returns (a copy of) fn's output over the signature's rows (per_node) or fn's own rows; the
+        sampler's `node_id` names the node of every row.  With `members=vr_num` this is the variance-reduced
+        evaluation (ogbn-mag/eval_ogbn_mag.py:128-152) in one replay."""
+        self._need_sampler()
+        self._check_precision()
+        cur = torch.cuda.current_stream(self.dev)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            self.sampler.stage(seeds)
+            self.sampler.copy_in(philox)
+            if self.graph is None:
+                for _ in range(2):                          # eager warm-up: pointer tables, pinned-block cache
+                    self._run()
+                self.out = self._capture(self._run)
+            self.graph.replay()
+            res = self.out.clone()
+        cur.wait_stream(self.stream)
+        res.record_stream(cur)
+        return res
+
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type):
+        self._refuse_batches()
         self._check_precision()
         batch = (node_feature, node_type, edge_time, edge_index, edge_type)
         cur = torch.cuda.current_stream(self.dev)
@@ -360,7 +405,7 @@ class GraphedTrainStep(_Graphed):
     first call: a later call with one of them changed raises RuntimeError.  A batch that does not fit
     the signature raises ValueError before anything is copied."""
 
-    def __init__(self, loss_fn, sig, device, optimizer=None, clip_norm=None, targets=None, params=None):
+    def __init__(self, loss_fn, sig, device, optimizer=None, clip_norm=None, targets=None, params=None, sampler=None):
         if optimizer is not None:
             for g in optimizer.param_groups:
                 if not g.get("capturable", False):
@@ -379,7 +424,7 @@ class GraphedTrainStep(_Graphed):
             if not isinstance(dtype, torch.dtype):
                 raise ValueError("targets[%d]: dtype must be a torch.dtype, got %r" % (t, dtype))
             spec[t] = (tuple(int(v) for v in shape), dtype, fill)
-        super().__init__(sig, device)
+        super().__init__(sig, device, sampler)
         self.loss_fn, self.optimizer, self.clip_norm = loss_fn, optimizer, clip_norm
         self.params = [p for p in params if p.requires_grad]
         self.spec = spec
@@ -409,6 +454,7 @@ class GraphedTrainStep(_Graphed):
                 buf[:r].copy_(y if y.is_cuda else y.pin_memory(), non_blocking=True)
 
     def _forward_backward(self):
+        self._sample()
         self._rebuild_plan()
         res = self.loss_fn(self.x, self.nt, self.tm, self.ei, self.et, self.y)
         res = tuple(res) if isinstance(res, (tuple, list)) else (res,)
@@ -453,6 +499,50 @@ class GraphedTrainStep(_Graphed):
                 p.grad.copy_(g)
 
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type, targets=None):
+        self._refuse_batches()
+        self._check_call()
+        batch = (node_feature, node_type, edge_time, edge_index, edge_type)
+        cur = torch.cuda.current_stream(self.dev)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            sizes = self._sizes(batch)
+            targets = _check_targets(self.spec, targets, sizes[0], self.dev)
+            self._feed(batch, sizes)
+            self._copy_targets(targets)
+            self._update()
+        cur.wait_stream(self.stream)
+        return self.out
+
+    def step(self, seeds, philox=None, targets=None):
+        """With sampler=: sample `seeds` (as `GraphedSampler.fill`, `philox` as there) and make one update on the
+        batch, as one copy-in and one graph replay with no host synchronisation.  loss_fn reads the labels of the
+        sampled rows through the sampler's static `node_id` (e.g. y[node_id.clamp(min=0)], -100 where node_id < 0);
+        `targets` work as for a call, with at most sig.type_counts[t] rows."""
+        self._need_sampler()
+        self._check_call()
+        cur = torch.cuda.current_stream(self.dev)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            targets = _check_targets(self.spec, targets, self.sig.type_counts, self.dev)
+            self.sampler.stage(seeds)
+            self.sampler.copy_in(philox)
+            self._copy_targets(targets)
+            self._update()
+        cur.wait_stream(self.stream)
+        return self.out
+
+    def _update(self):
+        """First call: warm up, update eagerly and capture; later calls: replay."""
+        if self.graph is None:
+            self._first_call()
+            from .autograd import fused_dropout_switches, recompute_switches
+            self.recompute = recompute_switches(self.params)
+            self.fused_drop = fused_dropout_switches(self.params)
+            self.hyper = self._hyperparameters()
+        else:
+            self.graph.replay()
+
+    def _check_call(self):
         if self.capture_failed:
             raise RuntimeError("the first call of this GraphedTrainStep made its update but failed to capture the step; "
                                "build a new one")
@@ -474,22 +564,5 @@ class GraphedTrainStep(_Graphed):
                                    "their captured values (keep them fixed, or make them tensors updated in place)"
                                    % changed)
         self._check_precision()
-        batch = (node_feature, node_type, edge_time, edge_index, edge_type)
-        cur = torch.cuda.current_stream(self.dev)
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            sizes = self._sizes(batch)
-            targets = _check_targets(self.spec, targets, sizes[0], self.dev)
-            self._feed(batch, sizes)
-            self._copy_targets(targets)
-            if self.graph is None:
-                self.det = det
-                self._first_call()
-                from .autograd import fused_dropout_switches, recompute_switches
-                self.recompute = recompute_switches(self.params)
-                self.fused_drop = fused_dropout_switches(self.params)
-                self.hyper = self._hyperparameters()
-            else:
-                self.graph.replay()
-        cur.wait_stream(self.stream)
-        return self.out
+        if self.graph is None:
+            self.det = det

@@ -1459,7 +1459,7 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     up.add("node_off", np.concatenate([l[0][:T] for l in lay]))
     up.add("type_out", np.arange(T))
     up.add("self_off", np.concatenate([l[2] for l in lay]))
-    up.add("mem_out", np.stack([node_base[:B], edge_base[:B], E_b], 1))
+    up.add("mem_out", np.stack([node_base[:B], edge_base[:B], 2 * edge_base[:B], 2 * edge_base[:B] + E_b], 1))
     d = up.to(dev)
     N, E = int(node_base[-1]), int(edge_base[-1])
     self_rel = dg.edge_dict['self']
@@ -1656,6 +1656,445 @@ def merge_batches(batches, num_types, num_relations):
                    host_meta={"type_count": [int(v) for v in union_count] + [0], "sorted": True, "pairs": pairs})
     member_rows = [rows[int(node_base[b]):int(node_base[b + 1])] for b in range(B)]
     return node_feature, node_type, edge_time, edge_index, edge_type, member_rows
+
+
+def _mag_pairs(dg):
+    """Every <source type, relation> pair a batch of dg can hold: each block's, and 'self' on every type."""
+    self_rel = dg.edge_dict['self']
+    return sorted({(s, dg.edge_dict[r]) for _, s, r in dg.blocks} | {(t, self_rel) for t in range(len(dg.types))})
+
+
+def graph_signature_for(dg, sampled_depth, sampled_number, probe_inps, slack, members=1, time_range=None,
+                        edge_mask=None, feature_dtype=None):
+    """A ``graphed.GraphSignature`` for ``GraphedSampler`` sized from eager probe samples: ``sample_subgraphs_cuda`` of
+    every seed dict in ``probe_inps``; each type's node bound and the edge bound are the probes' maximum per subgraph
+    times ``members`` times ``1 + slack`` (rounded up).  The pair set is every <source type, relation> of dg's blocks
+    plus 'self' on every type, a superset of what any batch can hold.
+
+    Probes bound what is typical, not what is possible: a batch past them overflows (``GraphedSampler.check`` raises and
+    its features are NaN).  A node bound that can never overflow is ``members * min(id range, seeds + depth * width)``
+    per type (a subgraph holds at most its seeds plus ``width`` nodes per layer and type), usually far more rows."""
+    from . import graphed as _graphed
+    import torch
+    if not probe_inps:
+        raise ValueError("graph_signature_for needs at least one probe seed dict")
+    if slack < 0:
+        raise ValueError("slack must be non-negative, got %r" % (slack,))
+    T, R = len(dg.types), len(dg.edge_dict)
+    fdt = _batch_feature_dtype(dg, feature_dtype)
+    counts, edges = np.zeros(T, dtype=np.int64), 0
+    for b in sample_subgraphs_cuda(dg, time_range, sampled_depth, sampled_number, probe_inps, edge_mask=edge_mask,
+                                   feature_dtype=feature_dtype):
+        counts = np.maximum(counts, np.bincount(b[1].cpu().numpy(), minlength=T)[:T])
+        edges = max(edges, int(b[4].numel()))
+    grow = lambda v: int(np.ceil(int(members) * int(v) * (1.0 + slack)))
+    return _graphed.GraphSignature([grow(c) for c in counts], grow(edges), _mag_pairs(dg), R, dg.feat_dim,
+                                   feat_dtype=fdt if fdt is not None else torch.float32)
+
+
+def _graphed_bounds(dg, decl, depth, width, members, state_room=None):
+    """The sizes a GraphedSampler fixes at construction, for seeds decl [(type slot, largest count)]: layer_capacity [T]
+    (rows of each type per member: its seeds plus `width` per layer, at most its id range plus its seeds, since seeds
+    past the range add ids of their own), region_entries [T] (hashed entries per (member, type) region, from
+    state_room, default dg.state_room), max_room, sort_positions (members x max_room: what each selection sorts), cnt_off / count_slots (the
+    rebuild count pass's slots)."""
+    T = len(dg.types)
+    seed_max = np.zeros(T, dtype=np.int64)
+    for s, n in decl:
+        seed_max[s] = n
+    n_ids0 = np.asarray(dg.n_ids, dtype=np.int64)
+    cap = np.minimum(n_ids0 + seed_max, seed_max + depth * width)
+    rooms = _hash_rooms(n_ids0 + seed_max, cap, width, dg.state_room if state_room is None else state_room)
+    max_room = int(rooms.max())
+    n_sort = members * max_room
+    if n_sort >= 2 ** 31 - 1:
+        raise ValueError("%d members x %d hashed entries per region do not fit int32 sort values" % (members, max_room))
+    cnt_off = np.concatenate([[0], np.cumsum([cap[t] for _ in range(members) for t, _, _ in dg.blocks])])
+    cnt_off = cnt_off.astype(np.int64)
+    return {"layer_capacity": cap, "region_entries": rooms, "max_room": max_room, "sort_positions": n_sort,
+            "cnt_off": cnt_off, "count_slots": int(cnt_off[-1])}
+
+
+class GraphedSampler:
+    """``sample_subgraphs_cuda`` with shapes fixed at construction and no host read-back, so that a call can be captured
+    in a CUDA graph (with the training step: ``graphed.GraphedTrainStep``).
+
+        sig = sampler.graph_signature_for(dg, 6, 520, probe_inps, 0.25)
+        gs = sampler.GraphedSampler(dg, sig, 6, 520, seeds={"paper": 128})
+        gs.fill({"paper": seed_array})     # [n, 2] (id, time) per seed type, n <= the declared count
+        gs.check()                          # optional: reads the flags back (one synchronisation)
+
+    ``fill`` samples ``members`` subgraphs (one seed dict for all, or a list of ``members`` dicts) and writes them into
+    static tensors in the signature's padded layout (``graphed.GraphedForward`` / ``GraphedTrainStep``): ``x``
+    [sig.n_nodes, F] (sig.feat_dtype), ``nt`` (static), ``ei`` [2, sig.n_edges], ``et``, ``tm``, and ``node_id`` /
+    ``node_time`` [sig.n_nodes]: the original id (-1 on padding rows) and time (0 on padding rows) of every row.  With
+    ``members > 1`` the subgraphs are joined type-major, as ``merge_batches`` joins them.  Given the same seeds and Philox
+    keys, the tensors are bitwise what ``sample_subgraphs_cuda`` (then ``merge_batches`` for ``members > 1``) scattered
+    into the signature by ``GraphedTrainStep`` holds: padding rows zero, padding edges self loops on the last node with
+    type 0 and time 120.
+
+    ``philox``: None draws each member's Philox key on the device (a replay of a captured fill samples afresh); a device
+    int64 [members] tensor is used as given (member b's key is what ``sample_subgraphs_cuda`` draws from its generator
+    for member b).  ``time_range``, ``edge_mask`` and ``feature_dtype`` mean what they mean for ``sample_subgraphs_cuda``;
+    ``feature_dtype`` must give ``sig.feat_dtype``.
+
+    Bounds.  Node counts per type, the edge count and the pair set come from ``sig``; the sampler keeps the hashed state,
+    one region per (member, type) sized at construction from ``state_room`` (default ``dg.state_room``) entries per unit
+    of layer capacity (declared seeds + depth x width) plus width, at most twice the type's id range (a region that large
+    cannot overflow); nothing grows.  The budget of a hub-heavy graph can outgrow the default: a larger ``state_room``
+    trades sort work (every selection sorts ``members`` x the largest region) for headroom.  A count past the signature, a pair outside it, a region past half full, a neighbour id
+    or edge_time out of range, a sampled id past its feature table or a sampled type without one sets a device flag: the
+    fill then writes no node or edge, its features are all NaN (a NaN loss shows the batch), and ``check()`` raises
+    ValueError naming the bound, or the IndexError / KeyError ``sample_subgraphs_cuda`` raises.  Nothing is written
+    outside a buffer.  Graphs placed in host memory are not supported (ValueError).
+
+    Capture.  ``fill`` is ``stage(seeds)`` (host: validates the seeds and writes them to a pinned buffer),
+    ``copy_in(philox)`` (one copy from that buffer to the device, which ``copied`` follows) and ``run()`` (kernels
+    only).  Capture ``run()``; per batch call ``stage`` and ``copy_in``, then replay.  ``stage`` waits for the previous
+    copy only (not for the replay that reads it), so the host can run a batch ahead of the device.
+    ``graphed.GraphedTrainStep`` / ``GraphedForward`` take ``sampler=`` and do this in their ``step``."""
+
+    def __init__(self, dg, sig, sampled_depth, sampled_number, seeds, members=1, time_range=None, edge_mask=None,
+                 feature_dtype=None, state_room=None):
+        import torch
+        from . import _lib
+        if dg.placement == "host":
+            raise ValueError("GraphedSampler samples graphs placed on the device; this one has placement='host'")
+        if dg.features is None:
+            raise ValueError("GraphedSampler needs a DeviceGraph with feature tables")
+        fdt = _batch_feature_dtype(dg, feature_dtype)
+        if fdt != sig.feat_dtype:
+            raise ValueError("feature_dtype gives %s batches, the signature's feat_dtype is %s" % (fdt, sig.feat_dtype))
+        T, NB, R = len(dg.types), dg.n_blocks, len(dg.edge_dict)
+        if sig.num_types != T or sig.num_relations != R or sig.feat_dim != dg.feat_dim:
+            raise ValueError("the signature has %d types, %d relations and %d features; the graph %d, %d and %d"
+                             % (sig.num_types, sig.num_relations, sig.feat_dim, T, R, dg.feat_dim))
+        W, depth, B = int(sampled_number), int(sampled_depth), int(members)
+        if W <= 0 or depth < 0 or B < 1:
+            raise ValueError("sampled_number and members must be positive and sampled_depth non-negative")
+        self.decl = []                                     # [(type slot, largest seed count)] in declaration order
+        for name, n in seeds.items():
+            if name not in dg.slot:
+                raise KeyError("seed type %r is not in graph.get_types()" % (name,))
+            if int(n) <= 0:
+                raise ValueError("seeds[%r]: the largest seed count must be positive, got %r" % (name, n))
+            self.decl.append((dg.slot[name], int(n)))
+        if not self.decl:
+            raise ValueError("GraphedSampler needs at least one seed type")
+        self.min_ser = _edge_mask_table(dg, edge_mask)
+        self.dg, self.sig, self.depth, self.W, self.B, self.T, self.NB = dg, sig, depth, W, B, T, NB
+        self.time_filter = time_range is not None
+        self.max_time = int(np.max(list(time_range.keys()))) if self.time_filter else 0
+        dev = dg.device
+        self.dev = dev
+
+        bd = _graphed_bounds(dg, self.decl, depth, W, B, state_room)
+        self.cap, self.rooms, self.max_room, self.n_sort = (bd["layer_capacity"], bd["region_entries"],
+                                                            bd["max_room"], bd["sort_positions"])
+        caps, rooms = np.tile(self.cap, (B, 1)), np.tile(self.rooms, (B, 1))
+        ent_off = np.concatenate([[0], np.cumsum(rooms.reshape(-1))]).astype(np.int64)
+        lid_off = np.concatenate([[0], np.cumsum(caps.reshape(-1))]).astype(np.int64)
+        per = lambda flat: np.stack([flat[b * T:b * T + T + 1] for b in range(B)])
+        n_slots, n_lid = int(ent_off[-1]), int(lid_off[-1])
+        self.M = max(n for _, n in self.decl)
+        max_tg = max(W, self.M)
+        self.cnt_off = bd["cnt_off"]
+        self.n_count = bd["count_slots"]
+        self.max_rows = int(self.cap.max())
+        bud_ws, sel_ws, rb_ws = _c.c_size_t(), _c.c_size_t(), _c.c_size_t()
+        _lib.call("hgt_gsample_batch_add_budget_workspace_bytes", B, max_tg, dg.max_type_blocks, W, _c.byref(bud_ws))
+        _lib.call("hgt_gsample_hash_select_workspace_bytes", B, self.n_sort, _c.byref(sel_ws))
+        _lib.call("hgt_gsample_rebuild_workspace_bytes", self.n_count, _c.byref(rb_ws))
+        self.workspace_bytes = max(bud_ws.value, sel_ws.value, 1)
+
+        i64 = dict(dtype=torch.int64, device=dev)
+        # the static tables: region / lid starts, rooms, the layout's block order and pair codes, the signature's rows
+        self_rel = dg.edge_dict['self']
+        grp_off, grp_blk = [0], []
+        for tt in range(T):
+            own = [b for b, (t_, _, _) in enumerate(dg.blocks) if t_ == tt]
+            same = [b for b in own if dg.blocks[b][1] == tt]
+            grp_blk += ([b for b in same if dg.blocks[b][2] == 'self'] + [b for b in same if dg.blocks[b][2] != 'self']
+                        + [b for b in own if dg.blocks[b][1] != tt])
+            grp_off.append(len(grp_blk))
+        pairs = set(sig.pairs)
+        code = lambda s, r: 0 if (s, r) in pairs else 1 + s * R + r
+        blk_pair = [code(s, dg.edge_dict[r]) for _, s, r in dg.blocks]
+        self_pair = [code(t, self_rel) for t in range(T)]
+        has_feat = [int(dg.types[t] in dg.features) for t in range(T)]
+        st = _Upload()
+        st.add("ent_off", per(ent_off))
+        st.add("lid_off", per(lid_off))
+        st.add("rooms", rooms)
+        st.add("cnt_off", self.cnt_off if self.min_ser is None else np.concatenate([self.cnt_off, self.min_ser]))
+        st.add("row0", sig.row0[:T])
+        st.add("type_cap", np.asarray(sig.type_counts, dtype=np.int64))
+        st.add("type_out", np.arange(T))
+        st.add("grp_off", grp_off, np.int32)
+        st.add("grp_blk", grp_blk, np.int32)
+        st.add("blk_pair", blk_pair, np.int32)
+        st.add("self_pair", self_pair, np.int32)
+        st.add("has_feat", has_feat, np.int32)
+        self.tabs = st.to(dev)
+        self.mask_p = self.tabs.ptr("cnt_off") + 8 * self.cnt_off.shape[0] if self.min_ser is not None else None
+
+        # the state (hgt_gsample_hash_state), reset by every fill
+        self.key = torch.empty(max(n_slots, 1), **i64)
+        self.ser = torch.empty(max(n_slots, 1), dtype=torch.int32, device=dev)
+        self.score = torch.empty(max(n_slots, 1), **i64)
+        self.btime = torch.empty(max(n_slots, 1), **i64)
+        self.bstamp = torch.empty(max(n_slots, 1), **i64)
+        self.last_seq = torch.empty(max(n_slots, 1), **i64)
+        self.first_seq = torch.empty(max(n_slots, 1), **i64)
+        self.lid = torch.empty(max(n_lid, 1), **i64)
+        self.ltime = torch.empty(max(n_lid, 1), **i64)
+        self.fill_count = torch.empty(B * T, **i64)
+        self.type_min = torch.empty(2 * B * T, **i64)
+        self.seed = torch.empty(B, **i64)
+        self.flags = torch.empty(8, dtype=torch.int32, device=dev)
+        # what each fill copies in: [n_ids B*T | n_layer B*T | type_seq 2BT | counters 2B | next step B | seed table
+        # 4 x NS | seed step j: ids B*M, times B*M, counts B, steps B]; the seed steps' types go in the int32 copy
+        J, M, NS = len(self.decl), self.M, B * sum(n for _, n in self.decl)
+        self.J, self.NS = J, NS
+        o = {}
+        at = 0
+        for name, n in (("n_ids", B * T), ("nl0", B * T), ("seq0", 2 * B * T), ("cnt0", 2 * B), ("next", B),
+                        ("region", NS), ("id", NS), ("ser", NS), ("time", NS)):
+            o[name] = (at, n)
+            at += n
+        for j in range(J):
+            for name, n in (("ids", B * M), ("tms", B * M), ("n", B), ("step", B)):
+                o["s%d_%s" % (j, name)] = (at, n)
+                at += n
+        self.layout = o
+        self.h64 = torch.empty(at, dtype=torch.int64).pin_memory()
+        self.h32 = torch.empty(J * B, dtype=torch.int32).pin_memory()
+        self.d64 = torch.empty(at, **i64)
+        self.d32 = torch.empty(J * B, dtype=torch.int32, device=dev)
+        self.state_in = {k: self.d64[a:a + n] for k, (a, n) in o.items()}
+        si = self.state_in
+        # the state's counts and first-touch numbers: run() starts them from the copied-in values every time, so a run
+        # repeated without a new copy_in (warm-ups, replays) samples the same batch
+        self.n_layer, self.type_seq, self.counters = (torch.empty_like(si["nl0"]), torch.empty_like(si["seq0"]),
+                                                      torch.empty_like(si["cnt0"]))
+        self.next_step = torch.empty(B, **i64)
+        self.cst = _GHashState(T, B, self.tabs.ptr("ent_off"), self.tabs.ptr("lid_off"), si["n_ids"].data_ptr(),
+                               self.key.data_ptr(), self.ser.data_ptr(), self.ltime.data_ptr(), self.lid.data_ptr(),
+                               self.n_layer.data_ptr(), self.score.data_ptr(), self.btime.data_ptr(),
+                               self.bstamp.data_ptr(), self.last_seq.data_ptr(), self.first_seq.data_ptr(),
+                               self.fill_count.data_ptr(), self.type_min.data_ptr(), self.type_seq.data_ptr(),
+                               self.counters.data_ptr(), self.seed.data_ptr())
+        self.ws = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=dev)
+        self.rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
+        self.tgt = torch.empty(2 * B * W + B, **i64)
+        self.typ = torch.empty(T * B, dtype=torch.int32, device=dev)
+        self.stepk = torch.empty(T * B, **i64)
+        self.off = torch.empty(T * (B + 1), **i64)
+        self.ex = torch.empty(self.n_count + 1, **i64)
+        self.totals = torch.empty(max(B * NB, 1), **i64)
+        self.node_off = torch.empty(B * T, **i64)
+        self.blk_out = torch.empty(max(B * NB, 1), **i64)
+        self.self_off = torch.empty(B * T, **i64)
+        self.mem_out = torch.empty(4 * B, **i64)
+        self.n_real = torch.empty(1, **i64)
+        # the outputs, in the signature's layout
+        self.x = torch.zeros((sig.n_nodes, sig.feat_dim), dtype=sig.feat_dtype, device=dev)
+        self.nt = torch.from_numpy(sig.node_type).to(dev)
+        self.ei = torch.zeros((2, sig.n_edges), **i64)
+        self.et = torch.zeros(sig.n_edges, **i64)
+        self.tm = torch.zeros(sig.n_edges, **i64)
+        self.node_id = torch.full((sig.n_nodes,), -1, **i64)
+        self.node_time = torch.zeros(sig.n_nodes, **i64)
+        self.copied = torch.cuda.Event()
+        self.philox_in = torch.zeros(B, **i64)
+        self.given = torch.zeros(1, **i64)
+
+
+    def stage(self, seeds):
+        """Validate ``seeds`` (one dict for every member, or a list of ``members`` dicts) on the host and write them to
+        the pinned buffer the next ``copy_in`` copies from.  No device work and no synchronisation with the device
+        beyond waiting for the copy of the previous fill (``copied``)."""
+        dg, B, T = self.dg, self.B, self.T
+        inps = [seeds] * B if isinstance(seeds, dict) else list(seeds)
+        if len(inps) != B:
+            raise ValueError("%d seed dicts for %d members" % (len(inps), B))
+        declared = dict(self.decl)
+        members = [_device_seeds(dg, inp) for inp in inps]
+        for sd in members:
+            for s, ids, _ in sd:
+                if s not in declared:
+                    raise ValueError("seed type %r was not declared in seeds=" % (dg.types[s],))
+                if ids.shape[0] > declared[s]:
+                    raise ValueError("%d seeds of type %r, more than the declared %d" % (ids.shape[0], dg.types[s],
+                                                                                       declared[s]))
+        self.copied.synchronize()
+        h = self.h64.numpy()
+        v = {k: h[a:a + n] for k, (a, n) in self.layout.items()}
+        n_ids = np.tile(np.asarray(dg.n_ids, dtype=np.int64), (B, 1))
+        nl0, seq0, cnt0 = np.zeros((B, T), np.int64), np.full((B, 2 * T), -1, np.int64), np.zeros((B, 2), np.int64)
+        for k in ("region", "id", "ser", "time"):
+            v[k][:] = -1 if k == "region" else 0
+        at = 0
+        h32 = self.h32.numpy().reshape(self.J, B)
+        h32[:] = -1
+        for j in range(self.J):
+            v["s%d_n" % j][:] = 0
+            v["s%d_step" % j][:] = j
+        for b, sd in enumerate(members):
+            cnt0[b, 0] = len(sd)
+            for k, (s, ids, tm) in enumerate(sd):
+                n = ids.shape[0]
+                n_ids[b, s] = max(n_ids[b, s], int(ids.max()) + 1)
+                seq0[b, 2 * s] = k
+                nl0[b, s] = n
+                v["region"][at:at + n] = b * T + s
+                v["id"][at:at + n] = ids
+                v["ser"][at:at + n] = np.arange(n)
+                v["time"][at:at + n] = tm
+                at += n
+                M = self.M
+                v["s%d_ids" % k][b * M:b * M + n] = ids
+                v["s%d_tms" % k][b * M:b * M + n] = tm
+                v["s%d_n" % k][b] = n
+                h32[k, b] = s
+        if int(n_ids.max()) > _ID_LIMIT:
+            raise ValueError("node ids must be below 2^40 (the Philox counter's id field), got %d" % (int(n_ids.max()) - 1))
+        v["n_ids"][:] = n_ids.reshape(-1)
+        v["nl0"][:] = nl0.reshape(-1)
+        v["seq0"][:] = seq0.reshape(-1)
+        v["cnt0"][:] = cnt0.reshape(-1)
+        v["next"][:] = cnt0[:, 0]
+
+    def copy_in(self, philox=None):
+        """Enqueue the copy of the staged seeds, and of ``philox`` (a device int64 [members] tensor, or None: ``run``
+        draws the keys on the device), into the device buffers ``run`` reads; ``copied`` follows the copy.  Not captured:
+        a replayed ``run`` reads whatever the last ``copy_in`` left."""
+        import torch
+        B = self.B
+        self.d64.copy_(self.h64, non_blocking=True)
+        self.d32.copy_(self.h32, non_blocking=True)
+        self.copied.record()
+        if philox is None:
+            self.given.zero_()
+        else:
+            if (not isinstance(philox, torch.Tensor) or philox.dtype != torch.int64 or tuple(philox.shape) != (B,)
+                    or philox.device != self.x.device):
+                raise ValueError("philox must be an int64 tensor of shape [%d] on %s" % (B, self.x.device))
+            self.philox_in.copy_(philox)
+            self.given.fill_(1)
+
+    def run(self):
+        """The device part of ``fill``: sample from the copied-in seeds and lay the batch out.  Kernel launches and
+        stream-ordered fills only: no host synchronisation, capturable."""
+        import torch
+        from . import _lib
+        dg, B, T, W, NB, sig = self.dg, self.B, self.T, self.W, self.NB, self.sig
+        st = torch.cuda.current_stream(self.dev).cuda_stream
+        drawn = torch.randint(0, 2 ** 63 - 1, (B,), dtype=torch.int64, device=self.x.device)
+        self.seed.copy_(torch.where(self.given > 0, self.philox_in, drawn))
+        self.key.fill_(-1)
+        self.ser.fill_(-1)
+        self.score.zero_()
+        self.btime.zero_()
+        self.bstamp.fill_(-1)
+        self.last_seq.fill_(-1)
+        self.first_seq.fill_(_I64_MAX)
+        self.lid.zero_()
+        self.ltime.zero_()
+        self.fill_count.zero_()
+        self.type_min.fill_(_I64_MAX)
+        self.flags.zero_()
+        self.next_step.copy_(self.state_in["next"])
+        self.n_layer.copy_(self.state_in["nl0"])
+        self.type_seq.copy_(self.state_in["seq0"])
+        self.counters.copy_(self.state_in["cnt0"])
+        si, cst, flags_p = self.state_in, _c.byref(self.cst), self.flags.data_ptr()
+        _lib.call("hgt_gsample_hash_insert_seeds", cst, self.NS, si["region"].data_ptr(), si["id"].data_ptr(),
+                  si["ser"].data_ptr(), si["time"].data_ptr(), flags_p, st)
+        blocks_p, range_p, max_nb = dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr(), dg.max_type_blocks
+        ws_p, ws_n = self.ws.data_ptr(), self.ws.numel()
+
+        def add_budget(type_p, step_p, ids_p, tms_p, max_targets, count_p):
+            _lib.call("hgt_gsample_hash_add_budget", cst, blocks_p, range_p, max_nb, type_p, step_p, ids_p, tms_p,
+                      max_targets, count_p, W, int(self.time_filter), self.max_time, _NO_TIME, flags_p, ws_p, ws_n, st)
+
+        for j in range(self.J):                           # the seeds' budgets (data.py:139-141)
+            add_budget(self.d32.data_ptr() + 4 * j * B, si["s%d_step" % j].data_ptr(), si["s%d_ids" % j].data_ptr(),
+                       si["s%d_tms" % j].data_ptr(), self.M, si["s%d_n" % j].data_ptr())
+        tgt_id_p, tgt_time_p = self.tgt.data_ptr(), self.tgt.data_ptr() + 8 * B * W
+        n_tgt_p = self.tgt.data_ptr() + 16 * B * W
+        typ0, step0, off0 = self.typ.data_ptr(), self.stepk.data_ptr(), self.off.data_ptr()
+        for _layer in range(self.depth):                  # data.py:146-170, every member's budget types on the device
+            _lib.call("hgt_gsample_layer_order", self.type_seq.data_ptr(), B, T, self.tabs.ptr("rooms"),
+                      self.next_step.data_ptr(), typ0, step0, off0, st)
+            for k in range(T):
+                type_p, step_p = typ0 + 4 * k * B, step0 + 8 * k * B
+                _lib.call("hgt_gsample_hash_select", cst, type_p, step_p, off0 + 8 * k * (B + 1), self.n_sort,
+                          self.max_room, W, tgt_id_p, tgt_time_p, n_tgt_p, flags_p, ws_p, ws_n, st)
+                add_budget(type_p, step_p, tgt_id_p, tgt_time_p, W, n_tgt_p)
+        cnt_off_p = self.tabs.ptr("cnt_off")
+        _lib.call("hgt_gsample_hash_rebuild_count", cst, blocks_p, NB, self.mask_p, cnt_off_p, self.n_count,
+                  self.max_rows, _lib.ptr(dg.feat_rows), self.ex.data_ptr(), self.totals.data_ptr(), flags_p,
+                  self.rb.data_ptr(), self.rb.numel(), st)
+        tb = self.tabs
+        _lib.call("hgt_gsample_graphed_layout", B, T, NB, self.n_layer.data_ptr(), self.type_seq.data_ptr(),
+                  self.totals.data_ptr(), tb.ptr("grp_off"), tb.ptr("grp_blk"), tb.ptr("blk_pair"), tb.ptr("self_pair"),
+                  tb.ptr("has_feat"), tb.ptr("row0"), tb.ptr("type_cap"), sig.n_edges, flags_p,
+                  self.node_off.data_ptr(), self.blk_out.data_ptr(), self.self_off.data_ptr(), self.mem_out.data_ptr(),
+                  self.n_real.data_ptr(), st)
+        self.x.zero_()
+        self.node_time.zero_()
+        self.node_id.fill_(-1)
+        bf16 = dg.feature_dtype == torch.bfloat16
+        _lib.call("hgt_gsample_hash_rebuild_write", cst, blocks_p, NB, self.mask_p, cnt_off_p, self.ex.data_ptr(),
+                  self.blk_out.data_ptr(), self.node_off.data_ptr(), tb.ptr("type_out"), self.self_off.data_ptr(),
+                  dg.edge_dict['self'], self.mem_out.data_ptr(), self.max_rows,
+                  None if bf16 else _lib.ptr(dg.feat_ptrs), dg.feat_dim, self.nt.data_ptr(),
+                  self.node_time.data_ptr(), None if bf16 else self.x.data_ptr(), self.ei.data_ptr(),
+                  self.et.data_ptr(), self.tm.data_ptr(), st)
+        _lib.call("hgt_gsample_graphed_rows", cst, self.node_off.data_ptr(), self.max_rows, self.node_id.data_ptr(), st)
+        if bf16:
+            _lib.call("hgt_gsample_gather_rows_bf16" if sig.feat_dtype == torch.bfloat16 else
+                      "hgt_gsample_gather_features_bf16", _lib.ptr(dg.feat_ptrs), dg.feat_dim, self.nt.data_ptr(),
+                      self.node_id.data_ptr(), sig.n_nodes, self.x.data_ptr(), st)
+        _lib.call("hgt_gsample_graphed_pad", self.n_real.data_ptr(), sig.n_edges, sig.n_nodes - 1, flags_p,
+                  self.ei.data_ptr(), self.et.data_ptr(), self.tm.data_ptr(), self.x.data_ptr(), self.x.numel(),
+                  int(sig.feat_dtype == torch.bfloat16), st)
+
+    def fill(self, seeds, philox=None):
+        """Sample ``members`` subgraphs from ``seeds`` into the static tensors: ``stage(seeds)``, ``copy_in(philox)``,
+        ``run()``.  No host synchronisation."""
+        self.stage(seeds)
+        self.copy_in(philox)
+        self.run()
+
+    def check(self):
+        """Read the last fill's flags back (one synchronisation) and raise what went wrong: ValueError for a bound
+        (signature node or edge count, a pair outside the signature, a hashed region), else the IndexError / KeyError
+        of ``sample_subgraphs_cuda``."""
+        fl = self.flags.cpu().numpy()
+        dg, sig, R = self.dg, self.sig, self.sig.num_relations
+        if fl[3]:
+            raise ValueError("a hashed state region overflowed (%s entries per region, from dg.state_room = %g): build "
+                             "the GraphedSampler after raising dg.state_room" % (self.rooms.tolist(), dg.state_room))
+        if fl[4]:
+            t = int(fl[4]) - 1
+            raise ValueError("node type %r: the batch has more nodes than the signature's %d rows"
+                             % (dg.types[t], sig.type_counts[t]))
+        if fl[5]:
+            raise ValueError("the batch has more edges than the signature's %d" % sig.n_edges)
+        if fl[6]:
+            s, r = divmod(int(fl[6]) - 1, R)
+            raise ValueError("the batch has the <source type, relation> pair (%d, %d), which is not in the signature's "
+                             "pairs" % (s, r))
+        if fl[0]:
+            raise IndexError("a neighbour id lies outside its node type's id range in the device graph")
+        if fl[1]:
+            raise IndexError("edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
+        if fl[7]:
+            raise KeyError("no feature table for sampled node types %r" % ([dg.types[int(fl[7]) - 1]],))
+        if fl[2]:
+            raise IndexError("a sampled node id lies outside its type's feature table")
 
 
 def _finish(fg, states, layer_order, feature_extractor):
