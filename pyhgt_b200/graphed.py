@@ -178,6 +178,9 @@ class _Graphed:
         self.tm = torch.zeros(sig.n_edges, **i64)
         self.h = None                                                      # pinned staging, made by the first host batch
         self.graph = None
+        self.graph_run = None                                              # run()'s capture: no sampling at its head
+        self._sampling = True                                              # _sample() runs the sampler (off for run())
+        self.published = torch.cuda.Event()                                # run(): set 1 copied into the static tensors
         self.one_product = None                                            # bf16_matmuls() at capture
         self.plan = None
         self._staged = None
@@ -192,17 +195,41 @@ class _Graphed:
             self.x, self.nt, self.ei, self.et, self.tm = sampler.x, sampler.nt, sampler.ei, sampler.et, sampler.tm
 
     def _sample(self):
-        if self.sampler is not None:
+        if self.sampler is not None and self._sampling:
             self.sampler.run()
+
+    def _captured(self):
+        return self.graph is not None or self.graph_run is not None
 
     def _refuse_batches(self):
         if self.sampler is not None:
             raise ValueError("%s(sampler=...) samples its own batches: call step(seeds, philox=None, ...)"
                              % type(self).__name__)
 
-    def _need_sampler(self):
+    def _need_sampler(self, call="step()"):
         if self.sampler is None:
-            raise ValueError("step() needs a %s built with sampler=" % type(self).__name__)
+            raise ValueError("%s needs a %s built with sampler=" % (call, type(self).__name__))
+
+    def _pipelined(self, seed_batches, philox, each):
+        """run(): stage every batch, then for batch k on self.stream wait for its sample, publish it into the static
+        tensors and call each(k); batch k + 1 is sampled on the sampler's prefetch stream as soon as batch k is published,
+        so it runs beside each(k).  Only events order the two streams: no host synchronisation."""
+        gs = self.sampler
+        staged = gs.stage_batches(seed_batches, philox)    # host checks, then the prefetch stream waits for cur
+        cur = torch.cuda.current_stream(self.dev)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            gs.sample_staged(staged, 0)
+            for k in range(staged.n):
+                self.stream.wait_event(gs.sampled)
+                gs.publish()
+                self.published.record(self.stream)
+                if k + 1 < staged.n:
+                    gs.prefetch_stream.wait_event(self.published)
+                    gs.sample_staged(staged, k + 1)
+                each(k)
+        cur.wait_stream(self.stream)
+        cur.wait_stream(gs.prefetch_stream)
 
     def _rebuild_plan(self):
         s = self.sig
@@ -275,7 +302,7 @@ class _Graphed:
         """Record bf16_matmuls() before the first capture; raise ValueError if a later call's setting differs."""
         from .autograd import bf16_matmuls
         one = bf16_matmuls()
-        if self.graph is None:
+        if not self._captured():
             self.one_product = one
         elif one != self.one_product:
             raise ValueError("%s was captured with %s typed GEMMs, but torch.get_float32_matmul_precision() is now %r: "
@@ -284,18 +311,19 @@ class _Graphed:
                                                                     torch.get_float32_matmul_precision()))
 
     def _capture(self, fn):
-        """Capture fn() on self.stream; the table uploads captured in it re-read their pinned sources at every replay, so
-        those are kept (self._pins)."""
+        """Capture fn() on self.stream and return (graph, its output); the table uploads captured in it re-read their
+        pinned sources at every replay, so those are kept (self._pins).  step()'s and run()'s graphs share one memory
+        pool: they never run at the same time."""
         self.stream.synchronize()
+        pool = next((g.pool() for g in (self.graph, self.graph_run) if g is not None), None)
         _plan._PIN_KEEP = self._pins
         try:
             graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph, stream=self.stream):
+            with torch.cuda.graph(graph, pool=pool, stream=self.stream):
                 out = fn()
         finally:
             _plan._PIN_KEEP = None
-        self.graph = graph
-        return out
+        return graph, out
 
 
 class GraphedForward(_Graphed):
@@ -328,6 +356,7 @@ class GraphedForward(_Graphed):
         self.fn = fn
         self.per_node = bool(per_node)
         self.out = None
+        self.out_run = None
 
     def _run(self):
         self._sample()
@@ -350,12 +379,42 @@ class GraphedForward(_Graphed):
             if self.graph is None:
                 for _ in range(2):                          # eager warm-up: pointer tables, pinned-block cache
                     self._run()
-                self.out = self._capture(self._run)
+                self.graph, self.out = self._capture(self._run)
             self.graph.replay()
             res = self.out.clone()
         cur.wait_stream(self.stream)
         res.record_stream(cur)
         return res
+
+    def run(self, seed_batches, consume, philox=None):
+        """With sampler=: the forward of every batch of `seed_batches` (a non-empty list, each as `step` takes its
+        seeds), in order, sampling batch k + 1 on the sampler's prefetch stream while the forward of batch k runs.
+        After the forward of batch k, `consume(rows, node_id)` is called on the forward's stream with the static output
+        (what `step` returns a copy of) and the sampler's static `node_id`; work it enqueues on the current stream runs
+        before the next batch overwrites them.  `philox`: None, or a device int64 [len(seed_batches), members] tensor
+        (row k as `step` takes it).  Everything is checked on the host before any device work, and nothing
+        synchronises with the host after the first call (which captures).  `sampler.check()` names the first batch
+        that broke a bound; only that batch's rows are NaN."""
+        self._need_sampler("run()")
+        if not callable(consume):
+            raise ValueError("consume must be a callable consume(rows, node_id)")
+        self._check_precision()
+        gs = self.sampler
+
+        def each(k):
+            if self.graph_run is None:
+                self._sampling = False
+                try:
+                    if self.graph is None:
+                        for _ in range(2):                  # eager warm-up: pointer tables, pinned-block cache
+                            self._run()
+                    self.graph_run, self.out_run = self._capture(self._run)
+                finally:
+                    self._sampling = True
+            self.graph_run.replay()
+            consume(self.out_run, gs.node_id)
+
+        self._pipelined(seed_batches, philox, each)
 
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type):
         self._refuse_batches()
@@ -368,7 +427,7 @@ class GraphedForward(_Graphed):
             if self.graph is None:
                 for _ in range(2):                          # eager warm-up: pointer tables, pinned-block cache
                     self._run()
-                self.out = self._capture(self._run)
+                self.graph, self.out = self._capture(self._run)
             self.graph.replay()
             res = self.out.index_select(0, idx) if self.per_node else self.out.clone()
         cur.wait_stream(self.stream)
@@ -435,7 +494,10 @@ class GraphedTrainStep(_Graphed):
         self.fused_drop = None
         self.hyper = None
         self.out = None
+        self.out_run = None
         self.capture_failed = False
+        self._grads = {}                                   # graph (step or run) -> the static .grad tensors it writes
+        self._grads_of = None                              # whose .grad tensors `params` show
 
     def _hyperparameters(self):
         """The optimizer's per-group hyperparameters that a captured step holds by value (tensors are read at replay)."""
@@ -469,7 +531,7 @@ class GraphedTrainStep(_Graphed):
             self.optimizer.step()
         return res
 
-    def _first_call(self):
+    def _first_call(self, prefetched):
         for p in self.params:
             p.grad = None
         for _ in range(2):                                  # warm-up: pointer tables, pinned-block cache; no update
@@ -487,16 +549,41 @@ class GraphedTrainStep(_Graphed):
         from .autograd import release_att_graphs
         release_att_graphs(self.params)
         try:
-            self.out = self._capture(self._step)
+            graph, out = self._capture(self._step)
         except Exception:
             self.capture_failed = True          # the update is done: a retry must not make a second one
             raise
         release_att_graphs(self.params)
-        for o, e in zip(self.out, eager):
+        self._keep(prefetched, graph, out)
+        for o, e in zip(out, eager):
             o.copy_(e)
         for p, g in zip(self.params, grads):
             if p.grad is not None and g is not None:
                 p.grad.copy_(g)
+
+    def _keep(self, prefetched, graph, out):
+        if prefetched:
+            self.graph_run, self.out_run = graph, out
+        else:
+            self.graph, self.out = graph, out
+        self._grads[prefetched] = [p.grad for p in self.params]
+        self._grads_of = prefetched
+
+    def _capture_other(self, prefetched):
+        """The first call of the second entry point: capture its graph in the first one's memory pool, with .grad
+        tensors of its own (the first graph's stay in self._grads), and let the caller replay it."""
+        from .autograd import release_att_graphs
+        for p in self.params:
+            p.grad = None
+        release_att_graphs(self.params)
+        try:
+            graph, out = self._capture(self._step)
+        except Exception:
+            for p, g in zip(self.params, self._grads[not prefetched]):
+                p.grad = g
+            raise
+        release_att_graphs(self.params)
+        self._keep(prefetched, graph, out)
 
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type, targets=None):
         self._refuse_batches()
@@ -531,32 +618,76 @@ class GraphedTrainStep(_Graphed):
         cur.wait_stream(self.stream)
         return self.out
 
-    def _update(self):
-        """First call: warm up, update eagerly and capture; later calls: replay."""
-        if self.graph is None:
-            self._first_call()
-            from .autograd import fused_dropout_switches, recompute_switches
-            self.recompute = recompute_switches(self.params)
-            self.fused_drop = fused_dropout_switches(self.params)
-            self.hyper = self._hyperparameters()
-        else:
-            self.graph.replay()
+    def run(self, seed_batches, philox=None, targets=None):
+        """With sampler=: one update per batch of `seed_batches` (a non-empty list, each as `step` takes its seeds), in
+        order, sampling batch k + 1 on the sampler's prefetch stream while step k runs.  `philox`: None, or a device
+        int64 [len(seed_batches), members] tensor (row k as `step` takes it); `targets`: None, or one `step` targets
+        argument per batch.  Returns the n losses as one device tensor.  Everything is checked on the host before any
+        device work, and nothing synchronises with the host after the first call (which captures).  The updates are
+        those of `step` on the same batches and keys, and calls of `step` and `run` may be mixed in any order.
+        `sampler.check()` names the first batch that broke a bound; its loss is NaN, and so is every later one, as after
+        `step` calls (the NaN update reaches the parameters)."""
+        from . import sampler as _sampler
+        self._need_sampler("run()")
+        n = _sampler._seed_batch_count(seed_batches)
+        if targets is None:
+            targets = [None] * n
+        elif not isinstance(targets, (list, tuple)) or len(targets) != n:
+            raise ValueError("targets must be None or a list of one targets dict per seed batch (%d)" % n)
+        targets = [_check_targets(self.spec, t, self.sig.type_counts, self.dev) for t in targets]
+        self._check_call()
+        losses = []
+
+        def each(k):
+            self._copy_targets(targets[k])
+            self._update(prefetched=True)
+            if not losses:
+                losses.append(torch.empty((n,) + tuple(self.out_run[0].shape), dtype=self.out_run[0].dtype,
+                                          device=self.dev))
+            losses[0][k].copy_(self.out_run[0])
+
+        self._pipelined(seed_batches, philox, each)
+        losses[0].record_stream(torch.cuda.current_stream(self.dev))
+        return losses[0]
+
+    def _update(self, prefetched=False):
+        """First call: warm up, update eagerly and capture; later calls: replay.  `prefetched` (run()): the batch is
+        already in the static tensors, so the graph has no sampling at its head; the first run() after step() calls
+        (or the reverse) captures that graph next to the other and replays it."""
+        self._sampling = not prefetched
+        try:
+            if not self._captured():
+                self._first_call(prefetched)
+                from .autograd import fused_dropout_switches, recompute_switches
+                self.recompute = recompute_switches(self.params)
+                self.fused_drop = fused_dropout_switches(self.params)
+                self.hyper = self._hyperparameters()
+                return
+            if (self.graph_run if prefetched else self.graph) is None:
+                self._capture_other(prefetched)
+        finally:
+            self._sampling = True
+        (self.graph_run if prefetched else self.graph).replay()
+        if self._grads_of != prefetched:
+            for p, g in zip(self.params, self._grads[prefetched]):
+                p.grad = g
+            self._grads_of = prefetched
 
     def _check_call(self):
         if self.capture_failed:
             raise RuntimeError("the first call of this GraphedTrainStep made its update but failed to capture the step; "
                                "build a new one")
         det = torch.are_deterministic_algorithms_enabled()
-        if self.graph is not None and det != self.det:
+        if self._captured() and det != self.det:
             raise RuntimeError("GraphedTrainStep was captured with torch deterministic algorithms %s: the flag cannot "
                                "change afterwards" % ("on" if self.det else "off"))
-        if self.graph is not None and any(bool(m.recompute_tables) != v for m, v in self.recompute.items()):
+        if self._captured() and any(bool(m.recompute_tables) != v for m, v in self.recompute.items()):
             raise RuntimeError("a layer's recompute_tables changed after the GraphedTrainStep was captured: the graph "
                                "holds the backward of the switch as it was at the first call")
-        if self.graph is not None and any(bool(m.fused_dropout) != v for m, v in self.fused_drop.items()):
+        if self._captured() and any(bool(m.fused_dropout) != v for m, v in self.fused_drop.items()):
             raise RuntimeError("a module's fused_dropout changed after the GraphedTrainStep was captured: the graph "
                                "holds the dropout kernels of the switch as it was at the first call")
-        if self.graph is not None:
+        if self._captured():
             hyper = self._hyperparameters()
             if hyper != self.hyper:
                 changed = sorted({k for a, b in zip(hyper, self.hyper) for k in set(a) | set(b) if a.get(k) != b.get(k)})
@@ -564,5 +695,5 @@ class GraphedTrainStep(_Graphed):
                                    "their captured values (keep them fixed, or make them tensors updated in place)"
                                    % changed)
         self._check_precision()
-        if self.graph is None:
+        if not self._captured():
             self.det = det

@@ -1692,6 +1692,16 @@ def graph_signature_for(dg, sampled_depth, sampled_number, probe_inps, slack, me
                                    feat_dtype=fdt if fdt is not None else torch.float32)
 
 
+PREFETCH_PRIORITY = -1       # GraphedSampler.prefetch_stream: above the default 0 of the training stream
+_OUTPUTS = ("x", "nt", "ei", "et", "tm", "node_id", "node_time", "flags")   # one output set of GraphedSampler.run
+
+
+def _seed_batch_count(seed_batches):
+    if not isinstance(seed_batches, (list, tuple)) or not seed_batches:
+        raise ValueError("seed_batches must be a non-empty list of seed dicts")
+    return len(seed_batches)
+
+
 def _graphed_bounds(dg, decl, depth, width, members, state_room=None):
     """The sizes a GraphedSampler fixes at construction, for seeds decl [(type slot, largest count)]: layer_capacity [T]
     (rows of each type per member: its seeds plus `width` per layer, at most its id range plus its seeds, since seeds
@@ -1752,7 +1762,16 @@ class GraphedSampler:
     ``copy_in(philox)`` (one copy from that buffer to the device, which ``copied`` follows) and ``run()`` (kernels
     only).  Capture ``run()``; per batch call ``stage`` and ``copy_in``, then replay.  ``stage`` waits for the previous
     copy only (not for the replay that reads it), so the host can run a batch ahead of the device.
-    ``graphed.GraphedTrainStep`` / ``GraphedForward`` take ``sampler=`` and do this in their ``step``."""
+    ``graphed.GraphedTrainStep`` / ``GraphedForward`` take ``sampler=`` and do this in their ``step``.
+
+    Pipelined runs.  ``run(1)`` writes a second output set (``x``, ``ei``, ``et``, ``tm``, ``node_id``, ``node_time``,
+    the flags; made at the first use) while the static tensors above keep the batch a step reads.  The state stays
+    single, so sampler runs stay serialised.  ``stage_batches(seed_batches, philox)`` validates a whole list of seed
+    batches on the host and copies their seed tables to the device at once; ``sample_staged(run, k)`` samples batch k
+    into set 1 on ``prefetch_stream`` (a replay of a capture of ``run(1)``; ``sampled`` follows it), and ``publish()``
+    copies set 1 into the static tensors on the current stream.  ``GraphedTrainStep.run`` / ``GraphedForward.run``
+    drive them so that batch k + 1 is sampled while step k runs.  ``prefetch_stream`` is made with priority
+    ``PREFETCH_PRIORITY``; assigning another stream to it changes where the next runs sample."""
 
     def __init__(self, dg, sig, sampled_depth, sampled_number, seeds, members=1, time_range=None, edge_mask=None,
                  feature_dtype=None, state_room=None):
@@ -1908,13 +1927,26 @@ class GraphedSampler:
         self.copied = torch.cuda.Event()
         self.philox_in = torch.zeros(B, **i64)
         self.given = torch.zeros(1, **i64)
-
+        # pipelined runs (stage_batches / sample_staged / publish): output set 1, made at the first such run, and the
+        # captured run(1) replayed on prefetch_stream
+        self.prefetch_stream = torch.cuda.Stream(device=dev, priority=PREFETCH_PRIORITY)
+        self.sampled = torch.cuda.Event()
+        self.batch_flags = None
+        self._set1 = None
+        self._graph1 = None
 
     def stage(self, seeds):
         """Validate ``seeds`` (one dict for every member, or a list of ``members`` dicts) on the host and write them to
         the pinned buffer the next ``copy_in`` copies from.  No device work and no synchronisation with the device
         beyond waiting for the copy of the previous fill (``copied``)."""
-        dg, B, T = self.dg, self.B, self.T
+        members = self._members(seeds)
+        self.copied.synchronize()
+        self.batch_flags = None
+        self._pack(members, self.h64.numpy(), self.h32.numpy())
+
+    def _members(self, seeds):
+        """The host checks of ``stage``: each member's [(type slot, ids, times)]."""
+        dg, B = self.dg, self.B
         inps = [seeds] * B if isinstance(seeds, dict) else list(seeds)
         if len(inps) != B:
             raise ValueError("%d seed dicts for %d members" % (len(inps), B))
@@ -1927,15 +1959,18 @@ class GraphedSampler:
                 if ids.shape[0] > declared[s]:
                     raise ValueError("%d seeds of type %r, more than the declared %d" % (ids.shape[0], dg.types[s],
                                                                                        declared[s]))
-        self.copied.synchronize()
-        h = self.h64.numpy()
+        return members
+
+    def _pack(self, members, h, h32):
+        """Write checked members into one seed table: h (int64, the layout of ``h64``) and h32 (``h32``'s)."""
+        dg, B, T = self.dg, self.B, self.T
         v = {k: h[a:a + n] for k, (a, n) in self.layout.items()}
         n_ids = np.tile(np.asarray(dg.n_ids, dtype=np.int64), (B, 1))
         nl0, seq0, cnt0 = np.zeros((B, T), np.int64), np.full((B, 2 * T), -1, np.int64), np.zeros((B, 2), np.int64)
         for k in ("region", "id", "ser", "time"):
             v[k][:] = -1 if k == "region" else 0
         at = 0
-        h32 = self.h32.numpy().reshape(self.J, B)
+        h32 = h32.reshape(self.J, B)
         h32[:] = -1
         for j in range(self.J):
             v["s%d_n" % j][:] = 0
@@ -1983,12 +2018,14 @@ class GraphedSampler:
             self.philox_in.copy_(philox)
             self.given.fill_(1)
 
-    def run(self):
-        """The device part of ``fill``: sample from the copied-in seeds and lay the batch out.  Kernel launches and
-        stream-ordered fills only: no host synchronisation, capturable."""
+    def run(self, out=0):
+        """The device part of ``fill``: sample from the copied-in seeds and lay the batch out in output set ``out`` (0:
+        the static tensors, 1: the pipelined runs' set).  Kernel launches and stream-ordered fills only: no host
+        synchronisation, capturable."""
         import torch
         from . import _lib
         dg, B, T, W, NB, sig = self.dg, self.B, self.T, self.W, self.NB, self.sig
+        o = self._output_set(out)
         st = torch.cuda.current_stream(self.dev).cuda_stream
         drawn = torch.randint(0, 2 ** 63 - 1, (B,), dtype=torch.int64, device=self.x.device)
         self.seed.copy_(torch.where(self.given > 0, self.philox_in, drawn))
@@ -2003,12 +2040,12 @@ class GraphedSampler:
         self.ltime.zero_()
         self.fill_count.zero_()
         self.type_min.fill_(_I64_MAX)
-        self.flags.zero_()
+        o.flags.zero_()
         self.next_step.copy_(self.state_in["next"])
         self.n_layer.copy_(self.state_in["nl0"])
         self.type_seq.copy_(self.state_in["seq0"])
         self.counters.copy_(self.state_in["cnt0"])
-        si, cst, flags_p = self.state_in, _c.byref(self.cst), self.flags.data_ptr()
+        si, cst, flags_p = self.state_in, _c.byref(self.cst), o.flags.data_ptr()
         _lib.call("hgt_gsample_hash_insert_seeds", cst, self.NS, si["region"].data_ptr(), si["id"].data_ptr(),
                   si["ser"].data_ptr(), si["time"].data_ptr(), flags_p, st)
         blocks_p, range_p, max_nb = dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr(), dg.max_type_blocks
@@ -2042,23 +2079,23 @@ class GraphedSampler:
                   tb.ptr("has_feat"), tb.ptr("row0"), tb.ptr("type_cap"), sig.n_edges, flags_p,
                   self.node_off.data_ptr(), self.blk_out.data_ptr(), self.self_off.data_ptr(), self.mem_out.data_ptr(),
                   self.n_real.data_ptr(), st)
-        self.x.zero_()
-        self.node_time.zero_()
-        self.node_id.fill_(-1)
+        o.x.zero_()
+        o.node_time.zero_()
+        o.node_id.fill_(-1)
         bf16 = dg.feature_dtype == torch.bfloat16
         _lib.call("hgt_gsample_hash_rebuild_write", cst, blocks_p, NB, self.mask_p, cnt_off_p, self.ex.data_ptr(),
                   self.blk_out.data_ptr(), self.node_off.data_ptr(), tb.ptr("type_out"), self.self_off.data_ptr(),
                   dg.edge_dict['self'], self.mem_out.data_ptr(), self.max_rows,
-                  None if bf16 else _lib.ptr(dg.feat_ptrs), dg.feat_dim, self.nt.data_ptr(),
-                  self.node_time.data_ptr(), None if bf16 else self.x.data_ptr(), self.ei.data_ptr(),
-                  self.et.data_ptr(), self.tm.data_ptr(), st)
-        _lib.call("hgt_gsample_graphed_rows", cst, self.node_off.data_ptr(), self.max_rows, self.node_id.data_ptr(), st)
+                  None if bf16 else _lib.ptr(dg.feat_ptrs), dg.feat_dim, o.nt.data_ptr(),
+                  o.node_time.data_ptr(), None if bf16 else o.x.data_ptr(), o.ei.data_ptr(),
+                  o.et.data_ptr(), o.tm.data_ptr(), st)
+        _lib.call("hgt_gsample_graphed_rows", cst, self.node_off.data_ptr(), self.max_rows, o.node_id.data_ptr(), st)
         if bf16:
             _lib.call("hgt_gsample_gather_rows_bf16" if sig.feat_dtype == torch.bfloat16 else
-                      "hgt_gsample_gather_features_bf16", _lib.ptr(dg.feat_ptrs), dg.feat_dim, self.nt.data_ptr(),
-                      self.node_id.data_ptr(), sig.n_nodes, self.x.data_ptr(), st)
+                      "hgt_gsample_gather_features_bf16", _lib.ptr(dg.feat_ptrs), dg.feat_dim, o.nt.data_ptr(),
+                      o.node_id.data_ptr(), sig.n_nodes, o.x.data_ptr(), st)
         _lib.call("hgt_gsample_graphed_pad", self.n_real.data_ptr(), sig.n_edges, sig.n_nodes - 1, flags_p,
-                  self.ei.data_ptr(), self.et.data_ptr(), self.tm.data_ptr(), self.x.data_ptr(), self.x.numel(),
+                  o.ei.data_ptr(), o.et.data_ptr(), o.tm.data_ptr(), o.x.data_ptr(), o.x.numel(),
                   int(sig.feat_dtype == torch.bfloat16), st)
 
     def fill(self, seeds, philox=None):
@@ -2068,33 +2105,125 @@ class GraphedSampler:
         self.copy_in(philox)
         self.run()
 
+    def _output_set(self, out):
+        if out == 0:
+            return self
+        if out != 1:
+            raise ValueError("out must be 0 (the static tensors) or 1 (the pipelined runs' set), got %r" % (out,))
+        if self._set1 is None:
+            import types
+            import torch
+            self._set1 = types.SimpleNamespace(**{k: self.nt.clone() if k == "nt" else torch.zeros_like(getattr(self, k))
+                                                  for k in _OUTPUTS})
+        return self._set1
+
+    def stage_batches(self, seed_batches, philox=None):
+        """Check a pipelined run on the host and copy its seed tables to the device.  ``seed_batches``: a non-empty
+        list of seed batches, each as ``stage`` takes it; ``philox``: None, or a device int64 [len(seed_batches),
+        members] tensor (row k as ``copy_in`` takes it for batch k).  Every check runs before any device work, and
+        ValueErrors name the batch.  Then one copy of all the tables, from a pinned buffer of the run's own (so nothing
+        waits for an earlier copy), is enqueued on ``prefetch_stream`` after the current stream's work.  Returns the
+        staged run for ``sample_staged``; its per-batch flags become what ``check()`` reads."""
+        import types
+        import torch
+        n, B = _seed_batch_count(seed_batches), self.B
+        if philox is not None and (not isinstance(philox, torch.Tensor) or philox.dtype != torch.int64
+                                   or tuple(philox.shape) != (n, B) or philox.device != self.x.device):
+            raise ValueError("philox must be an int64 tensor of shape [%d, %d] on %s" % (n, B, self.dev))
+        members = []
+        for k, seeds in enumerate(seed_batches):
+            try:
+                members.append(self._members(seeds))
+            except ValueError as e:
+                raise ValueError("seed batch %d: %s" % (k, e)) from None
+        h64 = np.empty((n, self.h64.numel()), dtype=np.int64)
+        h32 = np.empty((n, self.h32.numel()), dtype=np.int32)
+        for k, mb in enumerate(members):
+            try:
+                self._pack(mb, h64[k], h32[k])
+            except ValueError as e:
+                raise ValueError("seed batch %d: %s" % (k, e)) from None
+        ss = self.prefetch_stream
+        ss.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(ss):
+            run = types.SimpleNamespace(
+                n=n, d64=torch.from_numpy(h64).pin_memory().to(self.dev, non_blocking=True),
+                d32=torch.from_numpy(h32).pin_memory().to(self.dev, non_blocking=True), philox=philox,
+                flags=torch.zeros((n, self.flags.numel()), dtype=self.flags.dtype, device=self.dev))
+        if philox is not None:
+            philox.record_stream(ss)
+        self.batch_flags = run.flags
+        return run
+
+    def sample_staged(self, run, k):
+        """Sample batch k of a staged run into output set 1 on ``prefetch_stream``: copy its seed table (and Philox
+        keys) into the buffers ``run()`` reads, replay the capture of ``run(1)`` (made at the first call, after one
+        eager run), keep the batch's flags in ``run.flags[k]`` and record ``sampled``.  The caller orders it after
+        the previous ``publish`` (set 1's last reader).  No host synchronisation after the first call."""
+        import torch
+        ss = self.prefetch_stream
+        with torch.cuda.stream(ss):
+            self.d64.copy_(run.d64[k])
+            self.d32.copy_(run.d32[k])
+            if run.philox is None:
+                self.given.zero_()
+            else:
+                self.philox_in.copy_(run.philox[k])
+                self.given.fill_(1)
+            if self._graph1 is None:
+                self.run(1)                                 # eager warm-up: module loads, pointer tables
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph, stream=ss):
+                    self.run(1)
+                self._graph1 = graph
+            self._graph1.replay()
+            run.flags[k].copy_(self._set1.flags)
+            self.sampled.record(ss)
+
+    def publish(self):
+        """Copy output set 1 (the batch of the last ``sample_staged``) into the static tensors, on the current stream,
+        device to device; the caller orders it after ``sampled``.  ``nt`` is not copied: both sets hold the
+        signature's static node types."""
+        for name in _OUTPUTS:
+            if name not in ("nt", "flags"):
+                getattr(self, name).copy_(getattr(self._set1, name))
+
     def check(self):
         """Read the last fill's flags back (one synchronisation) and raise what went wrong: ValueError for a bound
         (signature node or edge count, a pair outside the signature, a hashed region), else the IndexError / KeyError
-        of ``sample_subgraphs_cuda``."""
-        fl = self.flags.cpu().numpy()
+        of ``sample_subgraphs_cuda``.  After a pipelined run (``stage_batches``) the error is that of the first batch
+        with a flag set, and its message starts with the batch's index in the run."""
+        if self.batch_flags is None:
+            self._raise_flags(self.flags.cpu().numpy(), "")
+            return
+        fl = self.batch_flags.cpu().numpy()
+        bad = np.flatnonzero(fl.any(axis=1))
+        if bad.size:
+            self._raise_flags(fl[bad[0]], "seed batch %d: " % bad[0])
+
+    def _raise_flags(self, fl, where):
         dg, sig, R = self.dg, self.sig, self.sig.num_relations
         if fl[3]:
-            raise ValueError("a hashed state region overflowed (%s entries per region, from dg.state_room = %g): build "
-                             "the GraphedSampler after raising dg.state_room" % (self.rooms.tolist(), dg.state_room))
+            raise ValueError(where + "a hashed state region overflowed (%s entries per region, from dg.state_room = %g): "
+                             "build the GraphedSampler after raising dg.state_room" % (self.rooms.tolist(), dg.state_room))
         if fl[4]:
             t = int(fl[4]) - 1
-            raise ValueError("node type %r: the batch has more nodes than the signature's %d rows"
+            raise ValueError(where + "node type %r: the batch has more nodes than the signature's %d rows"
                              % (dg.types[t], sig.type_counts[t]))
         if fl[5]:
-            raise ValueError("the batch has more edges than the signature's %d" % sig.n_edges)
+            raise ValueError(where + "the batch has more edges than the signature's %d" % sig.n_edges)
         if fl[6]:
             s, r = divmod(int(fl[6]) - 1, R)
-            raise ValueError("the batch has the <source type, relation> pair (%d, %d), which is not in the signature's "
-                             "pairs" % (s, r))
+            raise ValueError(where + "the batch has the <source type, relation> pair (%d, %d), which is not in the "
+                             "signature's pairs" % (s, r))
         if fl[0]:
-            raise IndexError("a neighbour id lies outside its node type's id range in the device graph")
+            raise IndexError(where + "a neighbour id lies outside its node type's id range in the device graph")
         if fl[1]:
-            raise IndexError("edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
+            raise IndexError(where + "edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
         if fl[7]:
-            raise KeyError("no feature table for sampled node types %r" % ([dg.types[int(fl[7]) - 1]],))
+            raise KeyError(where + "no feature table for sampled node types %r" % ([dg.types[int(fl[7]) - 1]],))
         if fl[2]:
-            raise IndexError("a sampled node id lies outside its type's feature table")
+            raise IndexError(where + "a sampled node id lies outside its type's feature table")
 
 
 def _finish(fg, states, layer_order, feature_extractor):
