@@ -1143,6 +1143,280 @@ class _Upload:
         return (self.d[o:].view(torch.int32) if dtype == np.int32 else self.d[o:])[:n]
 
 
+def _region_offsets(per):
+    """Member-major [B, T] region sizes -> ([B, T+1] absolute starts of each member's regions, total size)."""
+    B, T = per.shape
+    flat = np.concatenate([[0], np.cumsum(per.reshape(-1))]).astype(np.int64)
+    return np.stack([flat[b * T:b * T + T + 1] for b in range(B)]), int(flat[-1])
+
+
+def _count_offsets(cap, blocks):
+    """The rebuild count pass's slot starts: member after member (cap [B, T] layer capacities), per block its target
+    type's capacity."""
+    return np.concatenate([[0], np.cumsum([cap[b, t] for b in range(cap.shape[0]) for t, _, _ in blocks])]).astype(
+        np.int64)
+
+
+def _seed_ranges(dg, members):
+    """(n_ids [B, T], n_seed [B, T]): each member's id ranges, extended by seeds past the graph's range (they become
+    isolated nodes), and seed counts.  ValueError for ids past the Philox counter's id field."""
+    n_ids = np.tile(np.asarray(dg.n_ids, dtype=np.int64).reshape(1, -1), (len(members), 1))
+    n_seed = np.zeros_like(n_ids)
+    for b, seeds in enumerate(members):
+        for s, ids, _ in seeds:
+            n_ids[b, s] = max(n_ids[b, s], int(ids.max()) + 1)
+            n_seed[b, s] = ids.shape[0]
+    if n_ids.size and int(n_ids.max()) > _ID_LIMIT:
+        raise ValueError("node ids must be below 2^40 (the Philox counter's id field), got %d" % (int(n_ids.max()) - 1))
+    return n_ids, n_seed
+
+
+class _SeedTable:
+    """The seeds of a sampling pass over B members of T types in one int64 and one int32 table.  int64, member-major:
+    n_ids [B, T], the seeds' layer counts ``nl0`` [B, T], first-touch numbers ``seq0`` [B, 2T], counters ``cnt0`` [B, 2]
+    and next step numbers ``next`` [B]; per seed row (NS, member after member, inp order) its ``region`` (hashed:
+    member * T + type, -1 on padding rows) or dense slot, ``id``, ``ser``, ``time`` and, dense only, ``lpos`` (its
+    place in ``lid``); per seed step j (every member's j-th seed type, data.py:139-141) ids and times [B, Ms[j]],
+    counts and step numbers [B].  int32: the seed steps' types [J, B], -1 where a member has fewer seed types."""
+
+    def __init__(self, B, T, Ms, NS, dense):
+        self.B, self.T, self.Ms, self.NS = B, T, list(Ms), NS
+        sizes = [("n_ids", B * T), ("nl0", B * T), ("seq0", 2 * B * T), ("cnt0", 2 * B), ("next", B), ("region", NS),
+                 ("id", NS), ("ser", NS), ("time", NS)] + ([("lpos", NS)] if dense else [])
+        for j, M in enumerate(self.Ms):
+            sizes += [("s%d_ids" % j, B * M), ("s%d_tms" % j, B * M), ("s%d_n" % j, B), ("s%d_step" % j, B)]
+        self.at, self.n64 = {}, 0
+        for name, n in sizes:
+            self.at[name] = (self.n64, n)
+            self.n64 += n
+        self.n32 = len(self.Ms) * B
+
+    def ptr(self, base, name):
+        """Device address of a field of the int64 table at ``base``."""
+        return base + 8 * self.at[name][0]
+
+    def view(self, d64, name):
+        a, n = self.at[name]
+        return d64[a:a + n]
+
+    def pack(self, members, n_ids, h, h32, dense_off=None):
+        """Write members' checked seeds [(type slot, ids, times)] and id ranges n_ids [B, T] into h (int64 [n64]) and
+        h32 (int32 [n32]).  The dense layout takes dense_off: the [B, T+1] starts of each member's types in its slots
+        and in ``lid``."""
+        B, T = self.B, self.T
+        h[:] = 0
+        h32 = h32.reshape(len(self.Ms), B)
+        h32[:] = -1
+        v = {k: h[a:a + n] for k, (a, n) in self.at.items()}
+        v["region"][:] = -1
+        nl0, seq0, cnt0 = v["nl0"].reshape(B, T), v["seq0"].reshape(B, 2 * T), v["cnt0"].reshape(B, 2)
+        seq0[:] = -1
+        v["n_ids"][:] = n_ids.reshape(-1)
+        for j in range(len(self.Ms)):
+            v["s%d_step" % j][:] = j
+        at = 0
+        for b, seeds in enumerate(members):
+            cnt0[b, 0] = v["next"][b] = len(seeds)
+            for k, (s, ids, tm) in enumerate(seeds):
+                n, M = ids.shape[0], self.Ms[k]
+                seq0[b, 2 * s] = k
+                nl0[b, s] = n
+                v["region"][at:at + n] = b * T + s if dense_off is None else dense_off[0][b, s] + ids
+                v["id"][at:at + n] = ids
+                v["ser"][at:at + n] = np.arange(n)
+                v["time"][at:at + n] = tm
+                if dense_off is not None:
+                    v["lpos"][at:at + n] = dense_off[1][b, s] + np.arange(n)
+                at += n
+                v["s%d_ids" % k][b * M:b * M + n] = ids
+                v["s%d_tms" % k][b * M:b * M + n] = tm
+                v["s%d_n" % k][b] = n
+                h32[k, b] = s
+
+
+class _SamplingPass:
+    """The device HGSampling pass (data.py:131-209) of B members, shared by ``sample_subgraphs_cuda`` and
+    ``GraphedSampler`` so that the two stay bitwise equal: the sampler state, dense (hgt_gsample_batch_*: a slot per id
+    of each (member, type), ``ltime`` per slot) or ``hashed`` (hgt_gsample_hash_*: a region of entries per (member,
+    type), a ``key`` per entry, ``ltime`` per layer position), its ctypes block, and a launcher per step, run in the
+    order reset, seed_state, workspace, seed_budgets, step (per layer and budget type), rebuild_tables, rebuild_count,
+    rebuild_write, gather_bf16.  The callers choose a layer's steps and lay out the batch.  ``meta`` holds what the
+    host reads back: [n_layer B*T | type_seq B*2T | block totals B*NB | 4 int32 flags | hit count (host-placed graph) |
+    entries claimed per region B*T (hashed)], at offsets o_ts, o_tot, o_fl, o_hit and o_fill.
+
+    ``seeds``: the ``_SeedTable``, d64 / d32_p: its tables on the device; off_p, lid_off_p, seed_p: device addresses
+    of the [B, T+1] region (or slot) and layer position starts and of the B Philox keys, which must outlive the pass."""
+
+    def __init__(self, dg, hashed, n_slots, n_lid, W, time_range, seeds, d64, d32_p, off_p, lid_off_p, seed_p):
+        import torch
+        from . import _lib
+        self._lib = _lib             # imported once: the steps run per layer and budget type
+        B, T = seeds.B, seeds.T
+        self.dg, self.hashed, self.host, self.W, self.seeds, self.d64, self.d32_p = (
+            dg, hashed, dg.placement == "host", W, seeds, d64, d32_p)
+        self.api = "hgt_gsample_hash_" if hashed else "hgt_gsample_batch_"
+        self.time_filter = int(time_range is not None)
+        self.max_time = int(np.max(list(time_range.keys()))) if time_range is not None else 0
+        self.blocks_p, self.range_p = dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr()
+        dev = self.dev = dg.device
+        i64 = dict(dtype=torch.int64, device=dev)
+        self.o_ts, self.o_tot, self.o_fl = B * T, 3 * B * T, 3 * B * T + B * dg.n_blocks
+        self.o_hit = self.o_fl + 2
+        self.o_fill = self.o_hit + int(self.host)
+        self.meta = torch.empty(self.o_fill + B * T * int(hashed), **i64)
+        self.n_layer, self.type_seq = self.meta[:B * T], self.meta[self.o_ts:self.o_tot]
+        self.totals = self.meta[self.o_tot:self.o_fl]
+        self.flags = self.meta[self.o_fl:self.o_hit].view(torch.int32)
+        n = max(n_slots, 1)
+        self.key = torch.empty(n, **i64) if hashed else None
+        self.ser = torch.empty(n, dtype=torch.int32, device=dev)
+        self.score, self.btime, self.bstamp, self.last_seq, self.first_seq = (torch.empty(n, **i64) for _ in range(5))
+        self.lid = torch.empty(max(n_lid, 1), **i64)
+        self.ltime = torch.empty(max(n_lid if hashed else n_slots, 1), **i64)
+        self.type_min = torch.empty(max(2 * B * T, 1), **i64)
+        self.counters = torch.empty(2 * B, **i64)
+        self.initial = [(self.ser, -1), (self.score, 0), (self.btime, 0), (self.bstamp, -1), (self.last_seq, -1),
+                        (self.first_seq, _I64_MAX), (self.lid, 0), (self.ltime, 0), (self.type_min, _I64_MAX)] + (
+                            [(self.key, -1)] if hashed else [])
+        p = lambda ts: [t.data_ptr() for t in ts]
+        mid = p([self.ser, self.ltime, self.lid, self.n_layer, self.score, self.btime, self.bstamp, self.last_seq,
+                 self.first_seq])
+        tail = p([self.type_min, self.type_seq, self.counters]) + [seed_p]
+        if hashed:
+            self.cst = _GHashState(T, B, off_p, lid_off_p, seeds.ptr(d64.data_ptr(), "n_ids"), self.key.data_ptr(),
+                                   *mid, self.meta.data_ptr() + 8 * self.o_fill, *tail)
+        else:
+            self.cst = _GBatchState(T, B, off_p, lid_off_p, *mid, *tail)
+
+    def reset(self, flags=None):
+        """The state's ``initial`` values, ``meta`` and the flags zero: ``flags``, the int32 vector the launches set, or
+        None for the four in ``meta``.  The launches run on the current stream."""
+        import torch
+        self.st = torch.cuda.current_stream(self.dev).cuda_stream
+        self.flags_p = (self.flags if flags is None else flags).data_ptr()
+        self.meta.zero_()
+        if flags is not None:
+            flags.zero_()
+        for t, v in self.initial:
+            t.fill_(v)
+
+    def seed_state(self):
+        """Seeds enter layer_data first, in inp order (data.py:135-137): hgt_gsample_hash_insert_seeds, or index_put_
+        at their dense slots; then the seeds' layer counts, first-touch numbers and counters."""
+        import torch
+        sd, d = self.seeds, self.d64
+        if self.hashed:
+            self._lib.call("hgt_gsample_hash_insert_seeds", _c.byref(self.cst), sd.NS,
+                           *(sd.ptr(d.data_ptr(), k) for k in ("region", "id", "ser", "time")), self.flags_p, self.st)
+        elif sd.NS:
+            slot = sd.view(d, "region")
+            self.ser.index_put_((slot,), sd.view(d, "ser").to(torch.int32))
+            self.ltime.index_put_((slot,), sd.view(d, "time"))
+            self.lid.index_put_((sd.view(d, "lpos"),), sd.view(d, "id"))
+        self.n_layer.copy_(sd.view(d, "nl0"))
+        self.type_seq.copy_(sd.view(d, "seq0"))
+        self.counters.copy_(sd.view(d, "cnt0"))
+
+    def workspace(self, sort_positions):
+        """Scratch for add_budget (seed steps and selections) and for selections that sort sort_positions positions."""
+        import torch
+        B, W = self.seeds.B, self.W
+        bud_ws, sel_ws = _c.c_size_t(), _c.c_size_t()
+        self._lib.call("hgt_gsample_batch_add_budget_workspace_bytes", B, max([W] + self.seeds.Ms),
+                       self.dg.max_type_blocks, W, _c.byref(bud_ws))
+        self._lib.call(self.api + "select_workspace_bytes", B, sort_positions, _c.byref(sel_ws))
+        self.ws = torch.empty(max(bud_ws.value, sel_ws.value, 1), dtype=torch.uint8, device=self.dev)
+        self.ws_p = (self.ws.data_ptr(), self.ws.numel())
+        self.tgt = torch.zeros(2 * B * W + B, dtype=torch.int64, device=self.dev)   # [ids B*W | times B*W | counts B]
+        t = self.tgt.data_ptr()
+        self.tgt_p = (t, t + 8 * B * W, t + 16 * B * W)
+
+    def _add_budget(self, type_p, step_p, ids_p, tms_p, max_targets, count_p):
+        self._lib.call(self.api + "add_budget", _c.byref(self.cst), self.blocks_p, self.range_p,
+                       self.dg.max_type_blocks, type_p, step_p, ids_p, tms_p, max_targets, count_p, self.W,
+                       self.time_filter, self.max_time, _NO_TIME, self.flags_p, *self.ws_p, self.st)
+
+    def seed_budgets(self):
+        """add_budget of the seeds (data.py:139-141), seed step after seed step."""
+        sd, base = self.seeds, self.d64.data_ptr()
+        for j, M in enumerate(sd.Ms):
+            self._add_budget(self.d32_p + 4 * j * sd.B, sd.ptr(base, "s%d_step" % j), sd.ptr(base, "s%d_ids" % j),
+                             sd.ptr(base, "s%d_tms" % j), M, sd.ptr(base, "s%d_n" % j))
+
+    def step(self, type_p, step_p, off_p, n_total, max_range):
+        """One step of a layer (data.py:146-170): member b selects from its budget of type type_p[b] (-1: it sits out)
+        and adds the selected nodes' budget.  off_p: the [B+1] sort offsets, n_total the positions sorted, max_range
+        the largest id range (dense) or region (hashed) one member sorts."""
+        self._lib.call(self.api + "select", _c.byref(self.cst), type_p, step_p, off_p, n_total, max_range, self.W,
+                       *self.tgt_p, self.flags_p, *self.ws_p, self.st)
+        self._add_budget(type_p, step_p, self.tgt_p[0], self.tgt_p[1], self.W, self.tgt_p[2])
+
+    def rebuild_tables(self, cnt_off, max_rows, min_ser):
+        """The rebuild's count slot starts cnt_off (data.py:181-209) on the device, with the edge mask's min_ser table
+        (None: no mask) behind them in the same copy; max_rows is the largest layer capacity.  Sizes the rebuild's
+        scratch, and on a host-placed graph the hit records of its single-read count pass."""
+        import torch
+        from . import plan as _plan
+        n_count = int(cnt_off[-1])
+        self.cnt_off_d = _plan._to_dev_async(cnt_off if min_ser is None else np.concatenate([cnt_off, min_ser]),
+                                             self.dev)
+        rb_ws = _c.c_size_t()
+        self._lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
+        self.rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=self.dev)
+        self.ex = torch.empty(n_count + 1, dtype=torch.int64, device=self.dev)
+        if self.host:        # the kept edges' hit records (16 bytes each) stay in device scratch for the write pass
+            self.hit_cap = _hit_capacity(self.dg, n_count)
+            self.hits = torch.empty(16 * max(self.hit_cap, 1), dtype=torch.uint8, device=self.dev)
+        self.cnt_off_p, self.n_count, self.max_rows = self.cnt_off_d.data_ptr(), n_count, max_rows
+        self.mask_p = None if min_ser is None else self.cnt_off_p + 8 * cnt_off.shape[0]
+
+    def rebuild_count(self):
+        """The rebuild's count pass: kept edges per count slot, and per-block totals into ``meta``."""
+        dg = self.dg
+        hits = (self.hits.data_ptr(), self.hit_cap, self.meta.data_ptr() + 8 * self.o_hit) if self.host else ()
+        self._lib.call(self.api + ("rebuild_count_host" if self.host else "rebuild_count"), _c.byref(self.cst),
+                       self.blocks_p, dg.n_blocks, self.mask_p, self.cnt_off_p, self.n_count, self.max_rows,
+                       self._lib.ptr(dg.feat_rows) if dg.features is not None else None, *hits, self.ex.data_ptr(),
+                       self.totals.data_ptr(), self.flags_p, self.rb.data_ptr(), self.rb.numel(), self.st)
+
+    def rebuild_write(self, blk_out_p, node_off_p, type_out_p, self_off_p, mem_out_p, x, nt, node_time, ei, et, tm,
+                      n_hits=0):
+        """The rebuild's write pass into the layout the caller built (blk_out_p ... mem_out_p): node types and times,
+        fp32 features into ``x`` (None: none gathered here), edges.  n_hits: the hit records the count pass found
+        (host-placed graph; past the reserve, the write pass re-reads the neighbour lists)."""
+        dg = self.dg
+        hits = ()
+        if self.host:
+            fits = n_hits <= self.hit_cap
+            hits = (self.hits.data_ptr() if fits else None, n_hits if fits else 0)
+        self._lib.call(self.api + ("rebuild_write_host" if self.host else "rebuild_write"), _c.byref(self.cst),
+                       self.blocks_p, dg.n_blocks, self.mask_p, self.cnt_off_p, self.ex.data_ptr(), blk_out_p,
+                       node_off_p, type_out_p, self_off_p, dg.edge_dict['self'], mem_out_p, self.max_rows, *hits,
+                       self._lib.ptr(dg.feat_ptrs) if x is not None else None, dg.feat_dim, nt.data_ptr(),
+                       node_time.data_ptr(), self._lib.ptr(x), ei.data_ptr(), et.data_ptr(), tm.data_ptr(), self.st)
+
+    def gather_bf16(self, bf16_out, nt, row_id, n, out):
+        """The n output rows of a bf16 graph's features (node types nt, node ids row_id): copied as stored into a bf16
+        batch (``bf16_out``), widened into a float32 one."""
+        self._lib.call("hgt_gsample_gather_rows_bf16" if bf16_out else "hgt_gsample_gather_features_bf16",
+                       self._lib.ptr(self.dg.feat_ptrs), self.dg.feat_dim, nt.data_ptr(), row_id.data_ptr(), n,
+                       out.data_ptr(), self.st)
+
+
+def _raise_pass_flags(fl, lacking, where=""):
+    """Raise the error a sampling pass's flags fl report (fl[0]: a neighbour id out of range, fl[1]: an edge time out
+    of range, fl[2]: a sampled id past its feature table), with ``lacking`` (the sampled node types without a feature
+    table) checked before fl[2]; ``where`` prefixes the message."""
+    if fl[0]:
+        raise IndexError(where + "a neighbour id lies outside its node type's id range in the device graph")
+    if fl[1]:
+        raise IndexError(where + "edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
+    if lacking:
+        raise KeyError(where + "no feature table for sampled node types %r" % (lacking,))
+    if fl[2]:
+        raise IndexError(where + "a sampled node id lies outside its type's feature table")
+
+
 def sample_subgraph_cuda(dgraph, time_range, sampled_depth, sampled_number, inp, generator=None, edge_mask=None,
                          feature_dtype=None):
     """HGSampling (pyHGT/data.py:87-210) and ``to_torch`` (data.py:212-256) on the GPU.
@@ -1196,9 +1470,12 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     used where the dense state cannot run (a step's id ranges past 2^31 - 1 ids, or more than half the free device
     memory) and where the id ranges outnumber the table entries 16 to 1 (at least 2^22 ids).  A table that overflows
     restarts the call from the same draws with 4x larger tables (one more read-back; later calls start from that size).
-    Node ids must be below 2^40.  Plus add_budget scratch of B x 24 bytes x width x (max targets x blocks per type)."""
+    Node ids must be below 2^40.  Plus add_budget scratch of B x 24 bytes x width x (max targets x blocks per type).
+
+    The pass itself (state, seeding, selection and budget steps, rebuild, flags) is ``_SamplingPass``, shared with
+    ``GraphedSampler``; this function adds the exact-size parts: each layer's steps from a read-back of the budget
+    types, the per-member layout and the restarts."""
     import torch
-    from . import _lib
     from . import plan as _plan
     dg = dgraph
     dev = dg.device
@@ -1215,31 +1492,17 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     T, NB = len(dg.types), dg.n_blocks
 
     # per member: id ranges (seeds beyond the graph become isolated nodes) and layer capacities, laid out member-major
-    n_ids = np.tile(np.asarray(dg.n_ids, dtype=np.int64).reshape(1, T), (B, 1))
-    n_seed = np.zeros((B, T), dtype=np.int64)
-    for b, seeds in enumerate(members):
-        for s, ids, _ in seeds:
-            n_ids[b, s] = max(n_ids[b, s], int(ids.max()) + 1)
-            n_seed[b, s] = ids.shape[0]
-    if n_ids.size and int(n_ids.max()) > _ID_LIMIT:
-        raise ValueError("node ids must be below 2^40 (the Philox counter's id field), got %d" % (int(n_ids.max()) - 1))
+    n_ids, n_seed = _seed_ranges(dg, members)
     cap = np.minimum(n_ids, n_seed + depth * W)
-
-    def offsets(per):                                      # [B, T] sizes -> [B, T+1] absolute starts
-        flat = np.concatenate([[0], np.cumsum(per.reshape(-1))]).astype(np.int64)
-        return np.stack([flat[b * T:b * T + T + 1] for b in range(B)]), int(flat[-1])
-
-    lid_off, n_lid = offsets(cap)
+    lid_off, n_lid = _region_offsets(cap)
     layout = _FORCE_LAYOUT or _state_layout(n_ids, _hash_rooms(n_ids, cap, W, dg.state_room),
                                             _free_bytes_if_dense_is_large(dev, n_ids))
     hashed = layout == "hashed"
-    i64 = dict(dtype=torch.int64, device=dev)
     host = dg.placement == "host"
-    # one small buffer the host reads: [n_layer B*T | type_seq B*2T | block totals B*NB | flags | hit count (host graph)
-    # | entries claimed per (member, type) region (hashed state)]
-    o_ts, o_tot, o_fl = B * T, 3 * B * T, 3 * B * T + B * NB
-    o_hit = o_fl + 2
-    o_fill = o_hit + int(host)
+    # the seed table at this call's exact sizes: seed step j is every member's j-th seed type
+    J = max(len(s) for s in members)
+    seed_tab = _SeedTable(B, T, [max(s[j][1].shape[0] for s in members if j < len(s)) for j in range(J)],
+                          int(n_seed.sum()), not hashed)
 
     if generator is None:
         draws = [int(torch.randint(0, 2 ** 63 - 1, (1,))) for _ in range(B)]
@@ -1249,126 +1512,30 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
 
     restarts = 0
     while True:                 # hashed state: once more from the same draws with larger regions after an overflow
-        meta = torch.zeros(o_fill + B * T * int(hashed), **i64)
-        n_layer, type_seq = meta[:B * T], meta[o_ts:o_tot]
-        totals = meta[o_tot:o_fl]
-        flags = meta[o_fl:o_hit].view(torch.int32)          # 4 int32 flags; [3]: a hashed region overflowed
-        type_min = torch.full((max(2 * B * T, 1),), _I64_MAX, **i64)
-        counters = torch.zeros(2 * B, **i64)
-        lid = torch.zeros(max(n_lid, 1), **i64)
-        if hashed:
-            rooms = _hash_rooms(n_ids, cap, W, dg.state_room)
-            type_off, n_slots = offsets(rooms)             # the (member, type) regions
-            ltime = torch.zeros(max(n_lid, 1), **i64)
-            key = torch.full((max(n_slots, 1),), -1, **i64)
-        else:
-            rooms = n_ids
-            type_off, n_slots = offsets(n_ids)
-            ltime = torch.zeros(max(n_slots, 1), **i64)
-        ser = torch.full((max(n_slots, 1),), -1, dtype=torch.int32, device=dev)
-        score = torch.zeros(max(n_slots, 1), **i64)
-        btime = torch.zeros(max(n_slots, 1), **i64)
-        bstamp = torch.full((max(n_slots, 1),), -1, **i64)
-        last_seq = torch.full((max(n_slots, 1),), -1, **i64)
-        first_seq = torch.full((max(n_slots, 1),), _I64_MAX, **i64)
-
-        # seeds enter layer_data first, in inp order (data.py:135-137); their add_budget runs seed type after seed type,
-        # step j being every member's j-th seed type
+        rooms = _hash_rooms(n_ids, cap, W, dg.state_room) if hashed else n_ids
+        type_off, n_slots = _region_offsets(rooms)         # the (member, type) regions, or the dense slots
+        h64, h32 = np.empty(seed_tab.n64, dtype=np.int64), np.empty(seed_tab.n32, dtype=np.int32)
+        seed_tab.pack(members, n_ids, h64, h32, None if hashed else (type_off, lid_off))
         up = _Upload()
         up.add("type_off", type_off)
         up.add("lid_off", lid_off)
-        up.add("n_ids", n_ids)
         up.add("seed", np.asarray(draws, dtype=np.uint64).view(np.int64))
-        seq0 = np.full((B, 2 * T), -1, dtype=np.int64)
-        nl0 = np.zeros((B, T), dtype=np.int64)
-        cnt0 = np.zeros((B, 2), dtype=np.int64)
-        slots, sers, tms, lpos, lids = [], [], [], [], []
-        for b, seeds in enumerate(members):
-            cnt0[b, 0] = len(seeds)
-            for k, (s, ids, tm) in enumerate(seeds):
-                seq0[b, 2 * s] = k
-                nl0[b, s] = ids.shape[0]
-                # the dense state's slots; the hashed state's (member, type) regions
-                slots.append(np.full(ids.shape[0], b * T + s) if hashed else type_off[b, s] + ids)
-                sers.append(np.arange(ids.shape[0]))
-                tms.append(tm)
-                lpos.append(lid_off[b, s] + np.arange(ids.shape[0]))
-                lids.append(ids)
-        n_in = sum(a.shape[0] for a in slots)
-        for name, parts in (("slots", slots), ("sers", sers), ("tms", tms), ("lpos", lpos), ("lids", lids)):
-            up.add(name, np.concatenate(parts) if parts else np.zeros(0, np.int64))
-        up.add("nl0", nl0)
-        up.add("seq0", seq0)
-        up.add("cnt0", cnt0)
-        J = max(len(s) for s in members)
-        seed_steps = []                                   # (max targets, names) of seed step j
-        for j in range(J):
-            M = max((s[j][1].shape[0] for s in members if j < len(s)), default=0)
-            ids_j, tms_j = np.zeros((B, M), np.int64), np.zeros((B, M), np.int64)
-            n_j, type_j = np.zeros(B, np.int64), np.full(B, -1, np.int32)
-            for b, seeds in enumerate(members):
-                if j < len(seeds):
-                    s, ids, tm = seeds[j]
-                    ids_j[b, :ids.shape[0]], tms_j[b, :ids.shape[0]] = ids, tm
-                    n_j[b], type_j[b] = ids.shape[0], s
-            for name, arr, dt in (("ids", ids_j, np.int64), ("tms", tms_j, np.int64), ("n", n_j, np.int64),
-                                  ("type", type_j, np.int32), ("step", np.full(B, j), np.int64)):
-                up.add("seed%d_%s" % (j, name), arr, dt)
-            seed_steps.append(M)
-        # the state's tables: cst points into this upload, so it is held until the call returns
-        tabs = d = up.to(dev)
-        st = torch.cuda.current_stream(dev).cuda_stream
-        if hashed:
-            cst = _GHashState(T, B, tabs.ptr("type_off"), tabs.ptr("lid_off"), tabs.ptr("n_ids"), key.data_ptr(),
-                              ser.data_ptr(), ltime.data_ptr(), lid.data_ptr(), n_layer.data_ptr(), score.data_ptr(),
-                              btime.data_ptr(), bstamp.data_ptr(), last_seq.data_ptr(), first_seq.data_ptr(),
-                              meta[o_fill:].data_ptr(), type_min.data_ptr(), type_seq.data_ptr(), counters.data_ptr(),
-                              tabs.ptr("seed"))
-            _lib.call("hgt_gsample_hash_insert_seeds", _c.byref(cst), n_in, d.ptr("slots"), d.ptr("lids"),
-                      d.ptr("sers"), d.ptr("tms"), flags.data_ptr(), st)
-        else:
-            if n_in:
-                sl_d = d.view("slots")
-                ser.index_put_((sl_d,), d.view("sers").to(torch.int32))
-                ltime.index_put_((sl_d,), d.view("tms"))
-                lid.index_put_((d.view("lpos"),), d.view("lids"))
-            cst = _GBatchState(T, B, tabs.ptr("type_off"), tabs.ptr("lid_off"), ser.data_ptr(), ltime.data_ptr(),
-                               lid.data_ptr(), n_layer.data_ptr(), score.data_ptr(), btime.data_ptr(),
-                               bstamp.data_ptr(), last_seq.data_ptr(), first_seq.data_ptr(), type_min.data_ptr(),
-                               type_seq.data_ptr(), counters.data_ptr(), tabs.ptr("seed"))
-        n_layer.copy_(d.view("nl0"))
-        type_seq.copy_(d.view("seq0"))
-        counters.copy_(d.view("cnt0"))
-        api = "hgt_gsample_hash_" if hashed else "hgt_gsample_batch_"
-        time_filter = time_range is not None
-        max_time = int(np.max(list(time_range.keys()))) if time_filter else 0
-
-        max_nb = dg.max_type_blocks
-        max_tg = max([W] + seed_steps)
-        bud_ws, sel_ws = _c.c_size_t(), _c.c_size_t()
-        _lib.call("hgt_gsample_batch_add_budget_workspace_bytes", B, max_tg, max_nb, W, _c.byref(bud_ws))
-        _lib.call(api + "select_workspace_bytes", B, int(rooms.max(axis=1).sum()), _c.byref(sel_ws))
-        ws = torch.empty(max(bud_ws.value, sel_ws.value, 1), dtype=torch.uint8, device=dev)
-        tgt = torch.zeros(2 * B * W + B, **i64)           # [ids B*W | times B*W | counts B]
-        tgt_id, tgt_time, n_tgt = tgt[:B * W], tgt[B * W:2 * B * W], tgt[2 * B * W:]
-
-        blocks_p, range_p, flags_p, ws_p, ws_n = (dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr(),
-                                                  flags.data_ptr(), ws.data_ptr(), ws.numel())
-        tgt_id_p, tgt_time_p, n_tgt_p = tgt_id.data_ptr(), tgt_time.data_ptr(), n_tgt.data_ptr()
-
-        def add_budget(type_p, step_p, ids_p, tms_p, max_targets, count_p):
-            _lib.call(api + "add_budget", _c.byref(cst), blocks_p, range_p, max_nb, type_p, step_p, ids_p, tms_p,
-                      max_targets, count_p, W, int(time_filter), max_time, _NO_TIME, flags_p, ws_p, ws_n, st)
-
-        for j, M in enumerate(seed_steps):                # the seeds' budgets (data.py:139-141)
-            add_budget(d.ptr("seed%d_type" % j), d.ptr("seed%d_step" % j), d.ptr("seed%d_ids" % j),
-                       d.ptr("seed%d_tms" % j), M, d.ptr("seed%d_n" % j))
+        up.add("seeds", h64)
+        up.add("seed_types", h32, np.int32)
+        # the state's tables: the pass's state block points into this upload, so it is held until the call returns
+        tabs = up.to(dev)
+        pss = _SamplingPass(dg, hashed, n_slots, n_lid, W, time_range, seed_tab, tabs.view("seeds"),
+                            tabs.ptr("seed_types"), tabs.ptr("type_off"), tabs.ptr("lid_off"), tabs.ptr("seed"))
+        pss.reset()
+        pss.seed_state()
+        pss.workspace(int(rooms.max(axis=1).sum()))
+        pss.seed_budgets()
         step = np.asarray([len(s) for s in members], dtype=np.int64)   # a member's next step number
         overflow = False
         for _layer in range(depth):                       # data.py:146-170
             # the per-layer read-back: every member's list(budget.keys()), and the flags
-            h = meta[o_ts:o_hit].cpu().numpy()
-            if h[o_fl - o_ts:].view(np.int32)[3]:
+            h = pss.meta[pss.o_ts:pss.o_hit].cpu().numpy()
+            if h[pss.o_fl - pss.o_ts:].view(np.int32)[3]:
                 overflow = True
                 break
             ts = h[:2 * B * T].reshape(B, 2 * T)
@@ -1391,62 +1558,30 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
             d = up.to(dev)
             type0, step0, off0 = d.ptr("type"), d.ptr("step"), d.ptr("off")
             for k in range(K):
-                type_p, step_p = type0 + 4 * k * B, step0 + 8 * k * B
-                _lib.call(api + "select", _c.byref(cst), type_p, step_p, off0 + 8 * k * (B + 1), int(off[k, B]),
-                          int(rng[k].max()), W, tgt_id_p, tgt_time_p, n_tgt_p, flags_p, ws_p, ws_n, st)
-                add_budget(type_p, step_p, tgt_id_p, tgt_time_p, W, n_tgt_p)
+                pss.step(type0 + 4 * k * B, step0 + 8 * k * B, off0 + 8 * k * (B + 1), int(off[k, B]),
+                         int(rng[k].max()))
             step += np.asarray([len(o) for o in orders], dtype=np.int64)
         if overflow:
             restarts = _grow_state_room(dg, restarts)
             continue
 
         # rebuild (data.py:181-209): count pass, then the one read-back of the batch
-        cnt_off = np.concatenate([[0], np.cumsum([cap[b, tt] for b in range(B) for tt, _, _ in dg.blocks])])
-        cnt_off = cnt_off.astype(np.int64)
-        n_count = int(cnt_off[-1])
-        max_rows = int(cap.max()) if cap.size else 0
-        rb_ws = _c.c_size_t()
-        _lib.call("hgt_gsample_rebuild_workspace_bytes", n_count, _c.byref(rb_ws))
-        rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
-        ex = torch.empty(n_count + 1, **i64)
-        # the mask table rides behind cnt_off in the same copy (NULL: no mask)
-        cnt_off_d = _plan._to_dev_async(cnt_off if min_ser is None else np.concatenate([cnt_off, min_ser]), dev)
-        mask_p = None if min_ser is None else cnt_off_d.data_ptr() + 8 * cnt_off.shape[0]
-        feat_rows_p = _lib.ptr(dg.feat_rows) if dg.features is not None else None
-        if host:
-            # single-read count pass: the kept edges' hit records (16 bytes each) stay in device scratch for the write
-            # pass
-            hit_cap = _hit_capacity(dg, n_count)
-            hits = torch.empty(16 * max(hit_cap, 1), dtype=torch.uint8, device=dev)
-            _lib.call(api + "rebuild_count_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p,
-                      cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, hits.data_ptr(), hit_cap,
-                      meta[o_hit:o_hit + 1].data_ptr(), ex.data_ptr(), totals.data_ptr(), flags.data_ptr(),
-                      rb.data_ptr(), rb.numel(), st)
-        else:
-            _lib.call(api + "rebuild_count", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p,
-                      cnt_off_d.data_ptr(), n_count, max_rows, feat_rows_p, ex.data_ptr(), totals.data_ptr(),
-                      flags.data_ptr(), rb.data_ptr(), rb.numel(), st)
-        h = meta.cpu().numpy()
-        fl = h[o_fl:o_hit].view(np.int32)
+        pss.rebuild_tables(_count_offsets(cap, dg.blocks), int(cap.max()) if cap.size else 0, min_ser)
+        pss.rebuild_count()
+        h = pss.meta.cpu().numpy()
+        fl = h[pss.o_fl:pss.o_hit].view(np.int32)
         if fl[3]:
             restarts = _grow_state_room(dg, restarts)
             continue
         break
     dg.sampler_state = {"layout": layout, "entries": int(rooms.sum()), "restarts": restarts,
-                        "load": float((h[o_fill:].reshape(B, T) / np.maximum(rooms, 1)).max()) if hashed else None}
+                        "load": float((h[pss.o_fill:].reshape(B, T) / np.maximum(rooms, 1)).max()) if hashed else None}
     nl = h[:B * T].reshape(B, T)
-    ts = h[o_ts:o_tot].reshape(B, 2 * T)
-    tot = h[o_tot:o_fl].reshape(B, NB)
-    if fl[0]:
-        raise IndexError("a neighbour id lies outside its node type's id range in the device graph")
-    if fl[1]:
-        raise IndexError("edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
-    if dg.features is not None:
-        lacking = sorted({dg.types[t] for b in range(B) for t in range(T) if nl[b, t] and dg.types[t] not in dg.features})
-        if lacking:
-            raise KeyError("no feature table for sampled node types %r" % (lacking,))
-    if fl[2]:
-        raise IndexError("a sampled node id lies outside its type's feature table")
+    ts = h[pss.o_ts:pss.o_tot].reshape(B, 2 * T)
+    tot = h[pss.o_tot:pss.o_fl].reshape(B, NB)
+    lacking = (sorted({dg.types[t] for b in range(B) for t in range(T) if nl[b, t] and dg.types[t] not in dg.features})
+               if dg.features is not None else None)
+    _raise_pass_flags(fl, lacking)
 
     # the to_torch layout of every member (data.py:226-256), member after member in the shared outputs
     lay = [_member_layout(dg, nl[b], ts[b], tot[b]) for b in range(B)]
@@ -1462,43 +1597,28 @@ def sample_subgraphs_cuda(dgraph, time_range, sampled_depth, sampled_number, inp
     up.add("mem_out", np.stack([node_base[:B], edge_base[:B], 2 * edge_base[:B], 2 * edge_base[:B] + E_b], 1))
     d = up.to(dev)
     N, E = int(node_base[-1]), int(edge_base[-1])
-    self_rel = dg.edge_dict['self']
+    i64 = dict(dtype=torch.int64, device=dev)
     node_type = torch.empty(N, **i64)
     node_time = torch.empty(N, **i64)
     node_feature = (torch.empty((N, dg.feat_dim), dtype=torch.bfloat16 if bf16_out else torch.float32, device=dev)
                     if dg.features is not None else None)
-    # bf16 tables: the write pass leaves the features out, and hgt_gsample_gather_features_bf16 widens the rows after it
-    # (hgt_gsample_gather_rows_bf16 copies them as they are for a bf16 batch)
+    # bf16 tables: the write pass leaves the features out, and gather_bf16 widens or copies the rows after it
     bf16 = node_feature is not None and dg.feature_dtype == torch.bfloat16
-    fp32_feature = None if bf16 else node_feature
     edge_index = torch.empty(2 * E, **i64)                # member b's [2, E_b] block at 2 * edge_base[b]
     edge_type = torch.empty(E, **i64)
     edge_time = torch.empty(E, **i64)
+    n_hits = 0
     if host:
-        n_hits = int(h[o_hit])
-        _grow_hit_room(dg, n_hits, n_count)
-        fits = n_hits <= hit_cap                          # else the write pass re-reads the neighbour lists
-        _lib.call(api + "rebuild_write_host", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p,
-                  cnt_off_d.data_ptr(), ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"),
-                  d.ptr("self_off"), self_rel, d.ptr("mem_out"), max_rows,
-                  hits.data_ptr() if fits else None, n_hits if fits else 0,
-                  _lib.ptr(dg.feat_ptrs) if fp32_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
-                  node_time.data_ptr(), _lib.ptr(fp32_feature), edge_index.data_ptr(), edge_type.data_ptr(),
-                  edge_time.data_ptr(), st)
-    else:
-        _lib.call(api + "rebuild_write", _c.byref(cst), dg.blocks_dev.data_ptr(), NB, mask_p, cnt_off_d.data_ptr(),
-                  ex.data_ptr(), d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), self_rel,
-                  d.ptr("mem_out"), max_rows,
-                  _lib.ptr(dg.feat_ptrs) if fp32_feature is not None else None, dg.feat_dim, node_type.data_ptr(),
-                  node_time.data_ptr(), _lib.ptr(fp32_feature), edge_index.data_ptr(), edge_type.data_ptr(),
-                  edge_time.data_ptr(), st)
+        n_hits = int(h[pss.o_hit])
+        _grow_hit_room(dg, n_hits, pss.n_count)
+    pss.rebuild_write(d.ptr("blk_out"), d.ptr("node_off"), d.ptr("type_out"), d.ptr("self_off"), d.ptr("mem_out"),
+                      None if bf16 else node_feature, node_type, node_time, edge_index, edge_type, edge_time, n_hits)
+    lid = pss.lid
     if bf16 and N:
         # output rows are member after member, type slot after type slot, ser order: the sampled ids in that order
         row_id = torch.cat([lid[int(lid_off[b, t]):int(lid_off[b, t] + nl[b, t])]
                             for b in range(B) for t in range(T) if nl[b, t]])
-        _lib.call("hgt_gsample_gather_rows_bf16" if bf16_out else "hgt_gsample_gather_features_bf16",
-                  _lib.ptr(dg.feat_ptrs), dg.feat_dim, node_type.data_ptr(), row_id.data_ptr(), N,
-                  node_feature.data_ptr(), st)
+        pss.gather_bf16(bf16_out, node_type, row_id, N, node_feature)
 
     out = []
     for b in range(B):
@@ -1719,8 +1839,7 @@ def _graphed_bounds(dg, decl, depth, width, members, state_room=None):
     n_sort = members * max_room
     if n_sort >= 2 ** 31 - 1:
         raise ValueError("%d members x %d hashed entries per region do not fit int32 sort values" % (members, max_room))
-    cnt_off = np.concatenate([[0], np.cumsum([cap[t] for _ in range(members) for t, _, _ in dg.blocks])])
-    cnt_off = cnt_off.astype(np.int64)
+    cnt_off = _count_offsets(np.tile(cap, (members, 1)), dg.blocks)
     return {"layer_capacity": cap, "region_entries": rooms, "max_room": max_room, "sort_positions": n_sort,
             "cnt_off": cnt_off, "count_slots": int(cnt_off[-1])}
 
@@ -1741,7 +1860,8 @@ class GraphedSampler:
     ``members > 1`` the subgraphs are joined type-major, as ``merge_batches`` joins them.  Given the same seeds and Philox
     keys, the tensors are bitwise what ``sample_subgraphs_cuda`` (then ``merge_batches`` for ``members > 1``) scattered
     into the signature by ``GraphedTrainStep`` holds: padding rows zero, padding edges self loops on the last node with
-    type 0 and time 120.
+    type 0 and time 120.  Both run the same ``_SamplingPass``; this class adds the bounds, the layer order on the device
+    and the signature's layout.
 
     ``philox``: None draws each member's Philox key on the device (a replay of a captured fill samples afresh); a device
     int64 [members] tensor is used as given (member b's key is what ``sample_subgraphs_cuda`` draws from its generator
@@ -1776,7 +1896,6 @@ class GraphedSampler:
     def __init__(self, dg, sig, sampled_depth, sampled_number, seeds, members=1, time_range=None, edge_mask=None,
                  feature_dtype=None, state_room=None):
         import torch
-        from . import _lib
         if dg.placement == "host":
             raise ValueError("GraphedSampler samples graphs placed on the device; this one has placement='host'")
         if dg.features is None:
@@ -1800,31 +1919,18 @@ class GraphedSampler:
             self.decl.append((dg.slot[name], int(n)))
         if not self.decl:
             raise ValueError("GraphedSampler needs at least one seed type")
-        self.min_ser = _edge_mask_table(dg, edge_mask)
+        min_ser = _edge_mask_table(dg, edge_mask)
         self.dg, self.sig, self.depth, self.W, self.B, self.T, self.NB = dg, sig, depth, W, B, T, NB
-        self.time_filter = time_range is not None
-        self.max_time = int(np.max(list(time_range.keys()))) if self.time_filter else 0
         dev = dg.device
         self.dev = dev
 
         bd = _graphed_bounds(dg, self.decl, depth, W, B, state_room)
         self.cap, self.rooms, self.max_room, self.n_sort = (bd["layer_capacity"], bd["region_entries"],
                                                             bd["max_room"], bd["sort_positions"])
-        caps, rooms = np.tile(self.cap, (B, 1)), np.tile(self.rooms, (B, 1))
-        ent_off = np.concatenate([[0], np.cumsum(rooms.reshape(-1))]).astype(np.int64)
-        lid_off = np.concatenate([[0], np.cumsum(caps.reshape(-1))]).astype(np.int64)
-        per = lambda flat: np.stack([flat[b * T:b * T + T + 1] for b in range(B)])
-        n_slots, n_lid = int(ent_off[-1]), int(lid_off[-1])
+        rooms = np.tile(self.rooms, (B, 1))
+        ent_off, n_slots = _region_offsets(rooms)
+        lid_off, n_lid = _region_offsets(np.tile(self.cap, (B, 1)))
         self.M = max(n for _, n in self.decl)
-        max_tg = max(W, self.M)
-        self.cnt_off = bd["cnt_off"]
-        self.n_count = bd["count_slots"]
-        self.max_rows = int(self.cap.max())
-        bud_ws, sel_ws, rb_ws = _c.c_size_t(), _c.c_size_t(), _c.c_size_t()
-        _lib.call("hgt_gsample_batch_add_budget_workspace_bytes", B, max_tg, dg.max_type_blocks, W, _c.byref(bud_ws))
-        _lib.call("hgt_gsample_hash_select_workspace_bytes", B, self.n_sort, _c.byref(sel_ws))
-        _lib.call("hgt_gsample_rebuild_workspace_bytes", self.n_count, _c.byref(rb_ws))
-        self.workspace_bytes = max(bud_ws.value, sel_ws.value, 1)
 
         i64 = dict(dtype=torch.int64, device=dev)
         # the static tables: region / lid starts, rooms, the layout's block order and pair codes, the signature's rows
@@ -1842,10 +1948,9 @@ class GraphedSampler:
         self_pair = [code(t, self_rel) for t in range(T)]
         has_feat = [int(dg.types[t] in dg.features) for t in range(T)]
         st = _Upload()
-        st.add("ent_off", per(ent_off))
-        st.add("lid_off", per(lid_off))
+        st.add("ent_off", ent_off)
+        st.add("lid_off", lid_off)
         st.add("rooms", rooms)
-        st.add("cnt_off", self.cnt_off if self.min_ser is None else np.concatenate([self.cnt_off, self.min_ser]))
         st.add("row0", sig.row0[:T])
         st.add("type_cap", np.asarray(sig.type_counts, dtype=np.int64))
         st.add("type_out", np.arange(T))
@@ -1855,62 +1960,25 @@ class GraphedSampler:
         st.add("self_pair", self_pair, np.int32)
         st.add("has_feat", has_feat, np.int32)
         self.tabs = st.to(dev)
-        self.mask_p = self.tabs.ptr("cnt_off") + 8 * self.cnt_off.shape[0] if self.min_ser is not None else None
 
-        # the state (hgt_gsample_hash_state), reset by every fill
-        self.key = torch.empty(max(n_slots, 1), **i64)
-        self.ser = torch.empty(max(n_slots, 1), dtype=torch.int32, device=dev)
-        self.score = torch.empty(max(n_slots, 1), **i64)
-        self.btime = torch.empty(max(n_slots, 1), **i64)
-        self.bstamp = torch.empty(max(n_slots, 1), **i64)
-        self.last_seq = torch.empty(max(n_slots, 1), **i64)
-        self.first_seq = torch.empty(max(n_slots, 1), **i64)
-        self.lid = torch.empty(max(n_lid, 1), **i64)
-        self.ltime = torch.empty(max(n_lid, 1), **i64)
-        self.fill_count = torch.empty(B * T, **i64)
-        self.type_min = torch.empty(2 * B * T, **i64)
+        # what each fill copies in: the pass's seed table at the declared maxima (seed entries padded with region -1)
+        self.seeds = _SeedTable(B, T, [self.M] * len(self.decl), B * sum(n for _, n in self.decl), dense=False)
+        self.h64 = torch.empty(self.seeds.n64, dtype=torch.int64).pin_memory()
+        self.h32 = torch.empty(self.seeds.n32, dtype=torch.int32).pin_memory()
+        self.d64 = torch.empty(self.seeds.n64, **i64)
+        self.d32 = torch.empty(self.seeds.n32, dtype=torch.int32, device=dev)
         self.seed = torch.empty(B, **i64)
+        # the hashed state, reset by every run(), which starts the counts from the copied-in values every time, so a
+        # run repeated without a new copy_in (warm-ups, replays) samples the same batch
+        self.pss = _SamplingPass(dg, True, n_slots, n_lid, W, time_range, self.seeds, self.d64, self.d32.data_ptr(),
+                                 self.tabs.ptr("ent_off"), self.tabs.ptr("lid_off"), self.seed.data_ptr())
+        self.pss.workspace(self.n_sort)
+        self.pss.rebuild_tables(bd["cnt_off"], int(self.cap.max()), min_ser)
         self.flags = torch.empty(8, dtype=torch.int32, device=dev)
-        # what each fill copies in: [n_ids B*T | n_layer B*T | type_seq 2BT | counters 2B | next step B | seed table
-        # 4 x NS | seed step j: ids B*M, times B*M, counts B, steps B]; the seed steps' types go in the int32 copy
-        J, M, NS = len(self.decl), self.M, B * sum(n for _, n in self.decl)
-        self.J, self.NS = J, NS
-        o = {}
-        at = 0
-        for name, n in (("n_ids", B * T), ("nl0", B * T), ("seq0", 2 * B * T), ("cnt0", 2 * B), ("next", B),
-                        ("region", NS), ("id", NS), ("ser", NS), ("time", NS)):
-            o[name] = (at, n)
-            at += n
-        for j in range(J):
-            for name, n in (("ids", B * M), ("tms", B * M), ("n", B), ("step", B)):
-                o["s%d_%s" % (j, name)] = (at, n)
-                at += n
-        self.layout = o
-        self.h64 = torch.empty(at, dtype=torch.int64).pin_memory()
-        self.h32 = torch.empty(J * B, dtype=torch.int32).pin_memory()
-        self.d64 = torch.empty(at, **i64)
-        self.d32 = torch.empty(J * B, dtype=torch.int32, device=dev)
-        self.state_in = {k: self.d64[a:a + n] for k, (a, n) in o.items()}
-        si = self.state_in
-        # the state's counts and first-touch numbers: run() starts them from the copied-in values every time, so a run
-        # repeated without a new copy_in (warm-ups, replays) samples the same batch
-        self.n_layer, self.type_seq, self.counters = (torch.empty_like(si["nl0"]), torch.empty_like(si["seq0"]),
-                                                      torch.empty_like(si["cnt0"]))
         self.next_step = torch.empty(B, **i64)
-        self.cst = _GHashState(T, B, self.tabs.ptr("ent_off"), self.tabs.ptr("lid_off"), si["n_ids"].data_ptr(),
-                               self.key.data_ptr(), self.ser.data_ptr(), self.ltime.data_ptr(), self.lid.data_ptr(),
-                               self.n_layer.data_ptr(), self.score.data_ptr(), self.btime.data_ptr(),
-                               self.bstamp.data_ptr(), self.last_seq.data_ptr(), self.first_seq.data_ptr(),
-                               self.fill_count.data_ptr(), self.type_min.data_ptr(), self.type_seq.data_ptr(),
-                               self.counters.data_ptr(), self.seed.data_ptr())
-        self.ws = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=dev)
-        self.rb = torch.empty(max(rb_ws.value, 1), dtype=torch.uint8, device=dev)
-        self.tgt = torch.empty(2 * B * W + B, **i64)
         self.typ = torch.empty(T * B, dtype=torch.int32, device=dev)
         self.stepk = torch.empty(T * B, **i64)
         self.off = torch.empty(T * (B + 1), **i64)
-        self.ex = torch.empty(self.n_count + 1, **i64)
-        self.totals = torch.empty(max(B * NB, 1), **i64)
         self.node_off = torch.empty(B * T, **i64)
         self.blk_out = torch.empty(max(B * NB, 1), **i64)
         self.self_off = torch.empty(B * T, **i64)
@@ -1942,7 +2010,7 @@ class GraphedSampler:
         members = self._members(seeds)
         self.copied.synchronize()
         self.batch_flags = None
-        self._pack(members, self.h64.numpy(), self.h32.numpy())
+        self.seeds.pack(members, _seed_ranges(self.dg, members)[0], self.h64.numpy(), self.h32.numpy())
 
     def _members(self, seeds):
         """The host checks of ``stage``: each member's [(type slot, ids, times)]."""
@@ -1960,45 +2028,6 @@ class GraphedSampler:
                     raise ValueError("%d seeds of type %r, more than the declared %d" % (ids.shape[0], dg.types[s],
                                                                                        declared[s]))
         return members
-
-    def _pack(self, members, h, h32):
-        """Write checked members into one seed table: h (int64, the layout of ``h64``) and h32 (``h32``'s)."""
-        dg, B, T = self.dg, self.B, self.T
-        v = {k: h[a:a + n] for k, (a, n) in self.layout.items()}
-        n_ids = np.tile(np.asarray(dg.n_ids, dtype=np.int64), (B, 1))
-        nl0, seq0, cnt0 = np.zeros((B, T), np.int64), np.full((B, 2 * T), -1, np.int64), np.zeros((B, 2), np.int64)
-        for k in ("region", "id", "ser", "time"):
-            v[k][:] = -1 if k == "region" else 0
-        at = 0
-        h32 = h32.reshape(self.J, B)
-        h32[:] = -1
-        for j in range(self.J):
-            v["s%d_n" % j][:] = 0
-            v["s%d_step" % j][:] = j
-        for b, sd in enumerate(members):
-            cnt0[b, 0] = len(sd)
-            for k, (s, ids, tm) in enumerate(sd):
-                n = ids.shape[0]
-                n_ids[b, s] = max(n_ids[b, s], int(ids.max()) + 1)
-                seq0[b, 2 * s] = k
-                nl0[b, s] = n
-                v["region"][at:at + n] = b * T + s
-                v["id"][at:at + n] = ids
-                v["ser"][at:at + n] = np.arange(n)
-                v["time"][at:at + n] = tm
-                at += n
-                M = self.M
-                v["s%d_ids" % k][b * M:b * M + n] = ids
-                v["s%d_tms" % k][b * M:b * M + n] = tm
-                v["s%d_n" % k][b] = n
-                h32[k, b] = s
-        if int(n_ids.max()) > _ID_LIMIT:
-            raise ValueError("node ids must be below 2^40 (the Philox counter's id field), got %d" % (int(n_ids.max()) - 1))
-        v["n_ids"][:] = n_ids.reshape(-1)
-        v["nl0"][:] = nl0.reshape(-1)
-        v["seq0"][:] = seq0.reshape(-1)
-        v["cnt0"][:] = cnt0.reshape(-1)
-        v["next"][:] = cnt0[:, 0]
 
     def copy_in(self, philox=None):
         """Enqueue the copy of the staged seeds, and of ``philox`` (a device int64 [members] tensor, or None: ``run``
@@ -2024,77 +2053,40 @@ class GraphedSampler:
         synchronisation, capturable."""
         import torch
         from . import _lib
-        dg, B, T, W, NB, sig = self.dg, self.B, self.T, self.W, self.NB, self.sig
+        dg, B, T, NB, sig, pss = self.dg, self.B, self.T, self.NB, self.sig, self.pss
         o = self._output_set(out)
         st = torch.cuda.current_stream(self.dev).cuda_stream
         drawn = torch.randint(0, 2 ** 63 - 1, (B,), dtype=torch.int64, device=self.x.device)
         self.seed.copy_(torch.where(self.given > 0, self.philox_in, drawn))
-        self.key.fill_(-1)
-        self.ser.fill_(-1)
-        self.score.zero_()
-        self.btime.zero_()
-        self.bstamp.fill_(-1)
-        self.last_seq.fill_(-1)
-        self.first_seq.fill_(_I64_MAX)
-        self.lid.zero_()
-        self.ltime.zero_()
-        self.fill_count.zero_()
-        self.type_min.fill_(_I64_MAX)
-        o.flags.zero_()
-        self.next_step.copy_(self.state_in["next"])
-        self.n_layer.copy_(self.state_in["nl0"])
-        self.type_seq.copy_(self.state_in["seq0"])
-        self.counters.copy_(self.state_in["cnt0"])
-        si, cst, flags_p = self.state_in, _c.byref(self.cst), o.flags.data_ptr()
-        _lib.call("hgt_gsample_hash_insert_seeds", cst, self.NS, si["region"].data_ptr(), si["id"].data_ptr(),
-                  si["ser"].data_ptr(), si["time"].data_ptr(), flags_p, st)
-        blocks_p, range_p, max_nb = dg.blocks_dev.data_ptr(), dg.type_block_range.data_ptr(), dg.max_type_blocks
-        ws_p, ws_n = self.ws.data_ptr(), self.ws.numel()
-
-        def add_budget(type_p, step_p, ids_p, tms_p, max_targets, count_p):
-            _lib.call("hgt_gsample_hash_add_budget", cst, blocks_p, range_p, max_nb, type_p, step_p, ids_p, tms_p,
-                      max_targets, count_p, W, int(self.time_filter), self.max_time, _NO_TIME, flags_p, ws_p, ws_n, st)
-
-        for j in range(self.J):                           # the seeds' budgets (data.py:139-141)
-            add_budget(self.d32.data_ptr() + 4 * j * B, si["s%d_step" % j].data_ptr(), si["s%d_ids" % j].data_ptr(),
-                       si["s%d_tms" % j].data_ptr(), self.M, si["s%d_n" % j].data_ptr())
-        tgt_id_p, tgt_time_p = self.tgt.data_ptr(), self.tgt.data_ptr() + 8 * B * W
-        n_tgt_p = self.tgt.data_ptr() + 16 * B * W
+        pss.reset(o.flags)
+        self.next_step.copy_(self.seeds.view(self.d64, "next"))
+        pss.seed_state()
+        pss.seed_budgets()
         typ0, step0, off0 = self.typ.data_ptr(), self.stepk.data_ptr(), self.off.data_ptr()
         for _layer in range(self.depth):                  # data.py:146-170, every member's budget types on the device
-            _lib.call("hgt_gsample_layer_order", self.type_seq.data_ptr(), B, T, self.tabs.ptr("rooms"),
+            _lib.call("hgt_gsample_layer_order", pss.type_seq.data_ptr(), B, T, self.tabs.ptr("rooms"),
                       self.next_step.data_ptr(), typ0, step0, off0, st)
             for k in range(T):
-                type_p, step_p = typ0 + 4 * k * B, step0 + 8 * k * B
-                _lib.call("hgt_gsample_hash_select", cst, type_p, step_p, off0 + 8 * k * (B + 1), self.n_sort,
-                          self.max_room, W, tgt_id_p, tgt_time_p, n_tgt_p, flags_p, ws_p, ws_n, st)
-                add_budget(type_p, step_p, tgt_id_p, tgt_time_p, W, n_tgt_p)
-        cnt_off_p = self.tabs.ptr("cnt_off")
-        _lib.call("hgt_gsample_hash_rebuild_count", cst, blocks_p, NB, self.mask_p, cnt_off_p, self.n_count,
-                  self.max_rows, _lib.ptr(dg.feat_rows), self.ex.data_ptr(), self.totals.data_ptr(), flags_p,
-                  self.rb.data_ptr(), self.rb.numel(), st)
+                pss.step(typ0 + 4 * k * B, step0 + 8 * k * B, off0 + 8 * k * (B + 1), self.n_sort, self.max_room)
+        pss.rebuild_count()
         tb = self.tabs
-        _lib.call("hgt_gsample_graphed_layout", B, T, NB, self.n_layer.data_ptr(), self.type_seq.data_ptr(),
-                  self.totals.data_ptr(), tb.ptr("grp_off"), tb.ptr("grp_blk"), tb.ptr("blk_pair"), tb.ptr("self_pair"),
-                  tb.ptr("has_feat"), tb.ptr("row0"), tb.ptr("type_cap"), sig.n_edges, flags_p,
+        _lib.call("hgt_gsample_graphed_layout", B, T, NB, pss.n_layer.data_ptr(), pss.type_seq.data_ptr(),
+                  pss.totals.data_ptr(), tb.ptr("grp_off"), tb.ptr("grp_blk"), tb.ptr("blk_pair"), tb.ptr("self_pair"),
+                  tb.ptr("has_feat"), tb.ptr("row0"), tb.ptr("type_cap"), sig.n_edges, o.flags.data_ptr(),
                   self.node_off.data_ptr(), self.blk_out.data_ptr(), self.self_off.data_ptr(), self.mem_out.data_ptr(),
                   self.n_real.data_ptr(), st)
         o.x.zero_()
         o.node_time.zero_()
         o.node_id.fill_(-1)
         bf16 = dg.feature_dtype == torch.bfloat16
-        _lib.call("hgt_gsample_hash_rebuild_write", cst, blocks_p, NB, self.mask_p, cnt_off_p, self.ex.data_ptr(),
-                  self.blk_out.data_ptr(), self.node_off.data_ptr(), tb.ptr("type_out"), self.self_off.data_ptr(),
-                  dg.edge_dict['self'], self.mem_out.data_ptr(), self.max_rows,
-                  None if bf16 else _lib.ptr(dg.feat_ptrs), dg.feat_dim, o.nt.data_ptr(),
-                  o.node_time.data_ptr(), None if bf16 else o.x.data_ptr(), o.ei.data_ptr(),
-                  o.et.data_ptr(), o.tm.data_ptr(), st)
-        _lib.call("hgt_gsample_graphed_rows", cst, self.node_off.data_ptr(), self.max_rows, o.node_id.data_ptr(), st)
+        pss.rebuild_write(self.blk_out.data_ptr(), self.node_off.data_ptr(), tb.ptr("type_out"),
+                          self.self_off.data_ptr(), self.mem_out.data_ptr(), None if bf16 else o.x, o.nt, o.node_time,
+                          o.ei, o.et, o.tm)
+        _lib.call("hgt_gsample_graphed_rows", _c.byref(pss.cst), self.node_off.data_ptr(), pss.max_rows,
+                  o.node_id.data_ptr(), st)
         if bf16:
-            _lib.call("hgt_gsample_gather_rows_bf16" if sig.feat_dtype == torch.bfloat16 else
-                      "hgt_gsample_gather_features_bf16", _lib.ptr(dg.feat_ptrs), dg.feat_dim, o.nt.data_ptr(),
-                      o.node_id.data_ptr(), sig.n_nodes, o.x.data_ptr(), st)
-        _lib.call("hgt_gsample_graphed_pad", self.n_real.data_ptr(), sig.n_edges, sig.n_nodes - 1, flags_p,
+            pss.gather_bf16(sig.feat_dtype == torch.bfloat16, o.nt, o.node_id, sig.n_nodes, o.x)
+        _lib.call("hgt_gsample_graphed_pad", self.n_real.data_ptr(), sig.n_edges, sig.n_nodes - 1, o.flags.data_ptr(),
                   o.ei.data_ptr(), o.et.data_ptr(), o.tm.data_ptr(), o.x.data_ptr(), o.x.numel(),
                   int(sig.feat_dtype == torch.bfloat16), st)
 
@@ -2140,7 +2132,7 @@ class GraphedSampler:
         h32 = np.empty((n, self.h32.numel()), dtype=np.int32)
         for k, mb in enumerate(members):
             try:
-                self._pack(mb, h64[k], h32[k])
+                self.seeds.pack(mb, _seed_ranges(self.dg, mb)[0], h64[k], h32[k])
             except ValueError as e:
                 raise ValueError("seed batch %d: %s" % (k, e)) from None
         ss = self.prefetch_stream
@@ -2216,14 +2208,7 @@ class GraphedSampler:
             s, r = divmod(int(fl[6]) - 1, R)
             raise ValueError(where + "the batch has the <source type, relation> pair (%d, %d), which is not in the "
                              "signature's pairs" % (s, r))
-        if fl[0]:
-            raise IndexError(where + "a neighbour id lies outside its node type's id range in the device graph")
-        if fl[1]:
-            raise IndexError(where + "edge_time contains values outside [0, 240) (RelTemporalEncoding table size)")
-        if fl[7]:
-            raise KeyError(where + "no feature table for sampled node types %r" % ([dg.types[int(fl[7]) - 1]],))
-        if fl[2]:
-            raise IndexError(where + "a sampled node id lies outside its type's feature table")
+        _raise_pass_flags(fl, [dg.types[int(fl[7]) - 1]] if fl[7] else None, where)
 
 
 def _finish(fg, states, layer_order, feature_extractor):
