@@ -161,7 +161,8 @@ def _check_targets(spec, targets, counts, device):
 
 class _Graphed:
     """Static padded input buffers of one signature and the per-batch copy-in (host or device batches).  With a
-    `sampler.GraphedSampler` the static buffers are the sampler's, and the captured graph starts with its sampling."""
+    `sampler.GraphedSampler` the static buffers are the sampler's: `step` replays the sampler's capture into them, then
+    the graph, which starts at the plan rebuild."""
 
     def __init__(self, sig, device, sampler=None):
         dev = torch.device(device)
@@ -178,8 +179,6 @@ class _Graphed:
         self.tm = torch.zeros(sig.n_edges, **i64)
         self.h = None                                                      # pinned staging, made by the first host batch
         self.graph = None
-        self.graph_run = None                                              # run()'s capture: no sampling at its head
-        self._sampling = True                                              # _sample() runs the sampler (off for run())
         self.published = torch.cuda.Event()                                # run(): set 1 copied into the static tensors
         self.one_product = None                                            # bf16_matmuls() at capture
         self.plan = None
@@ -193,13 +192,6 @@ class _Graphed:
             if sampler.x.device != dev:
                 raise ValueError("the sampler runs on %s, the graph on %s" % (sampler.x.device, dev))
             self.x, self.nt, self.ei, self.et, self.tm = sampler.x, sampler.nt, sampler.ei, sampler.et, sampler.tm
-
-    def _sample(self):
-        if self.sampler is not None and self._sampling:
-            self.sampler.run()
-
-    def _captured(self):
-        return self.graph is not None or self.graph_run is not None
 
     def _refuse_batches(self):
         if self.sampler is not None:
@@ -302,7 +294,7 @@ class _Graphed:
         """Record bf16_matmuls() before the first capture; raise ValueError if a later call's setting differs."""
         from .autograd import bf16_matmuls
         one = bf16_matmuls()
-        if not self._captured():
+        if self.graph is None:
             self.one_product = one
         elif one != self.one_product:
             raise ValueError("%s was captured with %s typed GEMMs, but torch.get_float32_matmul_precision() is now %r: "
@@ -312,14 +304,12 @@ class _Graphed:
 
     def _capture(self, fn):
         """Capture fn() on self.stream and return (graph, its output); the table uploads captured in it re-read their
-        pinned sources at every replay, so those are kept (self._pins).  step()'s and run()'s graphs share one memory
-        pool: they never run at the same time."""
+        pinned sources at every replay, so those are kept (self._pins)."""
         self.stream.synchronize()
-        pool = next((g.pool() for g in (self.graph, self.graph_run) if g is not None), None)
         _plan._PIN_KEEP = self._pins
         try:
             graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph, pool=pool, stream=self.stream):
+            with torch.cuda.graph(graph, stream=self.stream):
                 out = fn()
         finally:
             _plan._PIN_KEEP = None
@@ -356,19 +346,27 @@ class GraphedForward(_Graphed):
         self.fn = fn
         self.per_node = bool(per_node)
         self.out = None
-        self.out_run = None
 
     def _run(self):
-        self._sample()
         self._rebuild_plan()
         with torch.no_grad():
             return self.fn(self.x, self.nt, self.tm, self.ei, self.et)
 
+    def _replay(self):
+        """Replay the forward on the static tensors and return its static output; the first call warms up and
+        captures."""
+        if self.graph is None:
+            for _ in range(2):                              # eager warm-up: pointer tables, pinned-block cache
+                self._run()
+            self.graph, self.out = self._capture(self._run)
+        self.graph.replay()
+        return self.out
+
     def step(self, seeds, philox=None):
-        """With sampler=: sample `seeds` (as `GraphedSampler.fill`) and run the forward, as one graph replay with no host
-        synchronisation.  Returns (a copy of) fn's output over the signature's rows (per_node) or fn's own rows; the
-        sampler's `node_id` names the node of every row.  With `members=vr_num` this is the variance-reduced
-        evaluation (ogbn-mag/eval_ogbn_mag.py:128-152) in one replay."""
+        """With sampler=: sample `seeds` (as `GraphedSampler.fill`) and run the forward, as one copy-in, a replay of
+        the sampler's capture and a replay of the forward's, with no host synchronisation.  Returns (a copy of) fn's
+        output over the signature's rows (per_node) or fn's own rows; the sampler's `node_id` names the node of every
+        row.  With `members=vr_num` this is the variance-reduced evaluation (ogbn-mag/eval_ogbn_mag.py:128-152)."""
         self._need_sampler()
         self._check_precision()
         cur = torch.cuda.current_stream(self.dev)
@@ -376,12 +374,8 @@ class GraphedForward(_Graphed):
         with torch.cuda.stream(self.stream):
             self.sampler.stage(seeds)
             self.sampler.copy_in(philox)
-            if self.graph is None:
-                for _ in range(2):                          # eager warm-up: pointer tables, pinned-block cache
-                    self._run()
-                self.graph, self.out = self._capture(self._run)
-            self.graph.replay()
-            res = self.out.clone()
+            self.sampler._replay(0)
+            res = self._replay().clone()
         cur.wait_stream(self.stream)
         res.record_stream(cur)
         return res
@@ -399,22 +393,7 @@ class GraphedForward(_Graphed):
         if not callable(consume):
             raise ValueError("consume must be a callable consume(rows, node_id)")
         self._check_precision()
-        gs = self.sampler
-
-        def each(k):
-            if self.graph_run is None:
-                self._sampling = False
-                try:
-                    if self.graph is None:
-                        for _ in range(2):                  # eager warm-up: pointer tables, pinned-block cache
-                            self._run()
-                    self.graph_run, self.out_run = self._capture(self._run)
-                finally:
-                    self._sampling = True
-            self.graph_run.replay()
-            consume(self.out_run, gs.node_id)
-
-        self._pipelined(seed_batches, philox, each)
+        self._pipelined(seed_batches, philox, lambda k: consume(self._replay(), self.sampler.node_id))
 
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type):
         self._refuse_batches()
@@ -424,12 +403,8 @@ class GraphedForward(_Graphed):
         self.stream.wait_stream(cur)
         with torch.cuda.stream(self.stream):
             idx = self._feed(batch, self._sizes(batch))
-            if self.graph is None:
-                for _ in range(2):                          # eager warm-up: pointer tables, pinned-block cache
-                    self._run()
-                self.graph, self.out = self._capture(self._run)
-            self.graph.replay()
-            res = self.out.index_select(0, idx) if self.per_node else self.out.clone()
+            out = self._replay()
+            res = out.index_select(0, idx) if self.per_node else out.clone()
         cur.wait_stream(self.stream)
         res.record_stream(cur)
         return res
@@ -494,10 +469,7 @@ class GraphedTrainStep(_Graphed):
         self.fused_drop = None
         self.hyper = None
         self.out = None
-        self.out_run = None
         self.capture_failed = False
-        self._grads = {}                                   # graph (step or run) -> the static .grad tensors it writes
-        self._grads_of = None                              # whose .grad tensors `params` show
 
     def _hyperparameters(self):
         """The optimizer's per-group hyperparameters that a captured step holds by value (tensors are read at replay)."""
@@ -516,7 +488,6 @@ class GraphedTrainStep(_Graphed):
                 buf[:r].copy_(y if y.is_cuda else y.pin_memory(), non_blocking=True)
 
     def _forward_backward(self):
-        self._sample()
         self._rebuild_plan()
         res = self.loss_fn(self.x, self.nt, self.tm, self.ei, self.et, self.y)
         res = tuple(res) if isinstance(res, (tuple, list)) else (res,)
@@ -531,7 +502,7 @@ class GraphedTrainStep(_Graphed):
             self.optimizer.step()
         return res
 
-    def _first_call(self, prefetched):
+    def _first_call(self):
         for p in self.params:
             p.grad = None
         for _ in range(2):                                  # warm-up: pointer tables, pinned-block cache; no update
@@ -549,41 +520,16 @@ class GraphedTrainStep(_Graphed):
         from .autograd import release_att_graphs
         release_att_graphs(self.params)
         try:
-            graph, out = self._capture(self._step)
+            self.graph, self.out = self._capture(self._step)
         except Exception:
             self.capture_failed = True          # the update is done: a retry must not make a second one
             raise
         release_att_graphs(self.params)
-        self._keep(prefetched, graph, out)
-        for o, e in zip(out, eager):
+        for o, e in zip(self.out, eager):
             o.copy_(e)
         for p, g in zip(self.params, grads):
             if p.grad is not None and g is not None:
                 p.grad.copy_(g)
-
-    def _keep(self, prefetched, graph, out):
-        if prefetched:
-            self.graph_run, self.out_run = graph, out
-        else:
-            self.graph, self.out = graph, out
-        self._grads[prefetched] = [p.grad for p in self.params]
-        self._grads_of = prefetched
-
-    def _capture_other(self, prefetched):
-        """The first call of the second entry point: capture its graph in the first one's memory pool, with .grad
-        tensors of its own (the first graph's stay in self._grads), and let the caller replay it."""
-        from .autograd import release_att_graphs
-        for p in self.params:
-            p.grad = None
-        release_att_graphs(self.params)
-        try:
-            graph, out = self._capture(self._step)
-        except Exception:
-            for p, g in zip(self.params, self._grads[not prefetched]):
-                p.grad = g
-            raise
-        release_att_graphs(self.params)
-        self._keep(prefetched, graph, out)
 
     def __call__(self, node_feature, node_type, edge_time, edge_index, edge_type, targets=None):
         self._refuse_batches()
@@ -602,9 +548,10 @@ class GraphedTrainStep(_Graphed):
 
     def step(self, seeds, philox=None, targets=None):
         """With sampler=: sample `seeds` (as `GraphedSampler.fill`, `philox` as there) and make one update on the
-        batch, as one copy-in and one graph replay with no host synchronisation.  loss_fn reads the labels of the
-        sampled rows through the sampler's static `node_id` (e.g. y[node_id.clamp(min=0)], -100 where node_id < 0);
-        `targets` work as for a call, with at most sig.type_counts[t] rows."""
+        batch, as one copy-in, a replay of the sampler's capture and a replay of the step's, with no host
+        synchronisation.  loss_fn reads the labels of the sampled rows through the sampler's static `node_id` (e.g.
+        y[node_id.clamp(min=0)], -100 where node_id < 0); `targets` work as for a call, with at most sig.type_counts[t]
+        rows."""
         self._need_sampler()
         self._check_call()
         cur = torch.cuda.current_stream(self.dev)
@@ -613,6 +560,7 @@ class GraphedTrainStep(_Graphed):
             targets = _check_targets(self.spec, targets, self.sig.type_counts, self.dev)
             self.sampler.stage(seeds)
             self.sampler.copy_in(philox)
+            self.sampler._replay(0)
             self._copy_targets(targets)
             self._update()
         cur.wait_stream(self.stream)
@@ -640,54 +588,41 @@ class GraphedTrainStep(_Graphed):
 
         def each(k):
             self._copy_targets(targets[k])
-            self._update(prefetched=True)
+            self._update()
             if not losses:
-                losses.append(torch.empty((n,) + tuple(self.out_run[0].shape), dtype=self.out_run[0].dtype,
-                                          device=self.dev))
-            losses[0][k].copy_(self.out_run[0])
+                losses.append(torch.empty((n,) + tuple(self.out[0].shape), dtype=self.out[0].dtype, device=self.dev))
+            losses[0][k].copy_(self.out[0])
 
         self._pipelined(seed_batches, philox, each)
         losses[0].record_stream(torch.cuda.current_stream(self.dev))
         return losses[0]
 
-    def _update(self, prefetched=False):
-        """First call: warm up, update eagerly and capture; later calls: replay.  `prefetched` (run()): the batch is
-        already in the static tensors, so the graph has no sampling at its head; the first run() after step() calls
-        (or the reverse) captures that graph next to the other and replays it."""
-        self._sampling = not prefetched
-        try:
-            if not self._captured():
-                self._first_call(prefetched)
-                from .autograd import fused_dropout_switches, recompute_switches
-                self.recompute = recompute_switches(self.params)
-                self.fused_drop = fused_dropout_switches(self.params)
-                self.hyper = self._hyperparameters()
-                return
-            if (self.graph_run if prefetched else self.graph) is None:
-                self._capture_other(prefetched)
-        finally:
-            self._sampling = True
-        (self.graph_run if prefetched else self.graph).replay()
-        if self._grads_of != prefetched:
-            for p, g in zip(self.params, self._grads[prefetched]):
-                p.grad = g
-            self._grads_of = prefetched
+    def _update(self):
+        """First call: warm up, update eagerly and capture; later calls: replay."""
+        if self.graph is None:
+            self._first_call()
+            from .autograd import fused_dropout_switches, recompute_switches
+            self.recompute = recompute_switches(self.params)
+            self.fused_drop = fused_dropout_switches(self.params)
+            self.hyper = self._hyperparameters()
+        else:
+            self.graph.replay()
 
     def _check_call(self):
         if self.capture_failed:
             raise RuntimeError("the first call of this GraphedTrainStep made its update but failed to capture the step; "
                                "build a new one")
         det = torch.are_deterministic_algorithms_enabled()
-        if self._captured() and det != self.det:
+        if self.graph is not None and det != self.det:
             raise RuntimeError("GraphedTrainStep was captured with torch deterministic algorithms %s: the flag cannot "
                                "change afterwards" % ("on" if self.det else "off"))
-        if self._captured() and any(bool(m.recompute_tables) != v for m, v in self.recompute.items()):
+        if self.graph is not None and any(bool(m.recompute_tables) != v for m, v in self.recompute.items()):
             raise RuntimeError("a layer's recompute_tables changed after the GraphedTrainStep was captured: the graph "
                                "holds the backward of the switch as it was at the first call")
-        if self._captured() and any(bool(m.fused_dropout) != v for m, v in self.fused_drop.items()):
+        if self.graph is not None and any(bool(m.fused_dropout) != v for m, v in self.fused_drop.items()):
             raise RuntimeError("a module's fused_dropout changed after the GraphedTrainStep was captured: the graph "
                                "holds the dropout kernels of the switch as it was at the first call")
-        if self._captured():
+        if self.graph is not None:
             hyper = self._hyperparameters()
             if hyper != self.hyper:
                 changed = sorted({k for a, b in zip(hyper, self.hyper) for k in set(a) | set(b) if a.get(k) != b.get(k)})
@@ -695,5 +630,5 @@ class GraphedTrainStep(_Graphed):
                                    "their captured values (keep them fixed, or make them tensors updated in place)"
                                    % changed)
         self._check_precision()
-        if not self._captured():
+        if self.graph is None:
             self.det = det

@@ -1882,7 +1882,8 @@ class GraphedSampler:
     ``copy_in(philox)`` (one copy from that buffer to the device, which ``copied`` follows) and ``run()`` (kernels
     only).  Capture ``run()``; per batch call ``stage`` and ``copy_in``, then replay.  ``stage`` waits for the previous
     copy only (not for the replay that reads it), so the host can run a batch ahead of the device.
-    ``graphed.GraphedTrainStep`` / ``GraphedForward`` take ``sampler=`` and do this in their ``step``.
+    ``graphed.GraphedTrainStep`` / ``GraphedForward`` take ``sampler=`` and do this in their ``step``: they replay the
+    sampler's own capture of ``run()``, then their step's or forward's.
 
     Pipelined runs.  ``run(1)`` writes a second output set (``x``, ``ei``, ``et``, ``tm``, ``node_id``, ``node_time``,
     the flags; made at the first use) while the static tensors above keep the batch a step reads.  The state stays
@@ -1995,13 +1996,13 @@ class GraphedSampler:
         self.copied = torch.cuda.Event()
         self.philox_in = torch.zeros(B, **i64)
         self.given = torch.zeros(1, **i64)
-        # pipelined runs (stage_batches / sample_staged / publish): output set 1, made at the first such run, and the
-        # captured run(1) replayed on prefetch_stream
+        # pipelined runs (stage_batches / sample_staged / publish): output set 1, made at the first such run; and the
+        # captures of run(0) (a graphed step()) and run(1) (sample_staged), each made at its set's first replay
         self.prefetch_stream = torch.cuda.Stream(device=dev, priority=PREFETCH_PRIORITY)
         self.sampled = torch.cuda.Event()
         self.batch_flags = None
         self._set1 = None
-        self._graph1 = None
+        self._graphs = [None, None]
 
     def stage(self, seeds):
         """Validate ``seeds`` (one dict for every member, or a list of ``members`` dicts) on the host and write them to
@@ -2097,6 +2098,19 @@ class GraphedSampler:
         self.copy_in(philox)
         self.run()
 
+    def _replay(self, out):
+        """Replay a capture of ``run(out)`` on the current stream.  The first call for a set runs it once eagerly
+        (module loads, pointer tables) and captures it; a graph replays on any stream.  No host synchronisation after
+        that first call."""
+        import torch
+        if self._graphs[out] is None:
+            self.run(out)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, stream=torch.cuda.current_stream(self.dev)):
+                self.run(out)
+            self._graphs[out] = graph
+        self._graphs[out].replay()
+
     def _output_set(self, out):
         if out == 0:
             return self
@@ -2149,9 +2163,9 @@ class GraphedSampler:
 
     def sample_staged(self, run, k):
         """Sample batch k of a staged run into output set 1 on ``prefetch_stream``: copy its seed table (and Philox
-        keys) into the buffers ``run()`` reads, replay the capture of ``run(1)`` (made at the first call, after one
-        eager run), keep the batch's flags in ``run.flags[k]`` and record ``sampled``.  The caller orders it after
-        the previous ``publish`` (set 1's last reader).  No host synchronisation after the first call."""
+        keys) into the buffers ``run()`` reads, replay the capture of ``run(1)`` (``_replay``), keep the batch's flags
+        in ``run.flags[k]`` and record ``sampled``.  The caller orders it after the previous ``publish`` (set 1's last
+        reader).  No host synchronisation after the first call."""
         import torch
         ss = self.prefetch_stream
         with torch.cuda.stream(ss):
@@ -2162,13 +2176,7 @@ class GraphedSampler:
             else:
                 self.philox_in.copy_(run.philox[k])
                 self.given.fill_(1)
-            if self._graph1 is None:
-                self.run(1)                                 # eager warm-up: module loads, pointer tables
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph, stream=ss):
-                    self.run(1)
-                self._graph1 = graph
-            self._graph1.replay()
+            self._replay(1)
             run.flags[k].copy_(self._set1.flags)
             self.sampled.record(ss)
 

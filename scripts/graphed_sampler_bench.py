@@ -1,13 +1,13 @@
-"""Sampling inside the captured training step (sampler.GraphedSampler) against the sampler outside it.
+"""The captured sampler (sampler.GraphedSampler) feeding the captured training step against the eager sampler.
 
 Workload: the MAG-schema graph of gpu_sampler_bench.make_graph, the ogbn-mag recipe model of graphed_train_bench.py
 (GNN 128 -> 512, 4 HGT layers, 8 heads, RTE, dropout 0.2, linear head, AdamW capturable), 128 seed papers per subgraph,
 at each --settings depth x width.  Variants, alternated round after round in one run:
   a  sample_subgraph_cuda per step, then a GraphedTrainStep replay fed that device batch;
   b  one sample_subgraphs_cuda(B=32) per 32 steps, then 32 GraphedTrainStep replays;
-  c  32 replays of GraphedTrainStep(sampler=GraphedSampler(...)): sampling, plan, step in one graph;
+  c  32 GraphedTrainStep(sampler=GraphedSampler(...)).step calls: a sampler replay, then the step's (plan, step);
   d  eager sample_subgraphs_cuda(B=8) + merge_batches + forward (variance-reduced evaluation);
-  e  GraphedForward(sampler=GraphedSampler(..., members=8)): the same as one replay.
+  e  GraphedForward(sampler=GraphedSampler(..., members=8)): the same as a sampler replay and a forward replay.
 Per variant: ms per step from CUDA events and from a host clock ending in a synchronise, host CPU time per step, host
 synchronisations per step (counted in an untimed pass with torch.cuda.set_sync_debug_mode("warn")), the padding of the
 signature, the first call's time (warm-up + capture), and the card's name and power limit read in the same run.  One

@@ -3,11 +3,11 @@
 Workload: the MAG-schema graph of gpu_sampler_bench.make_graph, 128 seed papers per subgraph, at each --settings
 depth x width, and the ogbn-mag recipe model of graphed_train_bench.py (GNN 128 -> 512, 4 HGT layers, 8 heads, RTE,
 dropout 0.2, linear head, AdamW capturable, clip 1.0).  Training variants, alternated round after round in one process:
-  step      32 GraphedTrainStep(sampler=).step(seeds) calls: sampling at the head of each step's graph;
+  step      32 GraphedTrainStep(sampler=).step(seeds) calls: each replays the sampler's graph, then the step's;
   run       GraphedTrainStep.run(32 seed dicts): batch k + 1 sampled on the prefetch stream (priority
             sampler.PREFETCH_PRIORITY) while step k runs;
   run_p0    the same with the prefetch stream at the default priority 0;
-  floor     the step alone on 32 pre-sampled batches (publish copies + run()'s training graph, no sampling);
+  floor     the step alone on 32 pre-sampled batches (publish copies + the training graph, no sampling);
   sample    the 32 samples alone (the sampler's captured run on the prefetch stream, no training).
 Variance-reduced forward (members=8), per forward of 8 subgraphs:
   vr_step   GraphedForward(sampler=).step(seeds) calls;
@@ -178,13 +178,13 @@ def main():
             "step": lambda inps, _: [steps["step"].step(i) for i in inps],
             "run": run_with(hi),
             "run_p0": run_with(lo),
-            "floor": lambda _, pre: floor(steps["run"], pre, steps["run"].graph_run.replay),
+            "floor": lambda _, pre: floor(steps["run"], pre, steps["run"].graph.replay),
             "sample": sample_only,
         }
         vr = {
             "vr_step": lambda inps, _: [fwd.step(i) for i in inps],
             "vr_run": lambda inps, _: fwd.run(inps, lambda rows, ids: None),
-            "vr_floor": lambda _, pre: floor(fwd, pre, fwd.graph_run.replay),
+            "vr_floor": lambda _, pre: floor(fwd, pre, fwd.graph.replay),
         }
         steps["step"].step(inputs(1, 1)[0])                # first calls: warm-up + capture
         steps["run"].run(inputs(1, 2))

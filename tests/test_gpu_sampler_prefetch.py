@@ -129,7 +129,7 @@ def test_run_trains_bitwise_like_step_calls(B, dtype, masked):
 @pytest.mark.parametrize("order", ["step-run-step", "run-step-run"])
 def test_step_and_run_mix_in_any_order(order):
     """step(), run(), step() (or run(), step(), run()) on one object: the parameters and losses of the same batches
-    through step() alone."""
+    through step() alone, with one set of .grad tensors for both entry points."""
     (s1, p1), (s2, p2), n, year = _two_trainers("fp32", 1, None)
     seeds = list(range(70, 77))
     batches = [_seeds(n, year, s) for s in seeds]
@@ -138,12 +138,13 @@ def test_step_and_run_mix_in_any_order(order):
     torch.use_deterministic_algorithms(True)
     try:
         l1 = torch.stack([s1.step(b, keys[k])[0].clone() for k, b in enumerate(batches)])
-        l2 = []
+        l2, grad_ptrs = [], []
         for i, (a, b) in enumerate(parts):
             if (i % 2 == 0) == order.startswith("step"):
                 l2 += [s2.step(batches[k], keys[k])[0].clone() for k in range(a, b)]
             else:
                 l2 += list(s2.run(batches[a:b], keys[a:b]))
+            grad_ptrs.append([p.grad.data_ptr() for p in p2])
         l2 = torch.stack(l2)
         torch.cuda.synchronize()
     finally:
@@ -152,6 +153,7 @@ def test_step_and_run_mix_in_any_order(order):
     for a, b in zip(p1, p2):
         assert _same(a, b)
         assert _same(a.grad, b.grad)                       # .grad shows the last call's gradients
+    assert all(ptrs == grad_ptrs[0] for ptrs in grad_ptrs)  # the same .grad tensors after step() and run() calls
 
 
 def _forwards(B):

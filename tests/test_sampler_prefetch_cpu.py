@@ -32,7 +32,7 @@ def _sampler(members=2):
 def _graphed(cls, gs):
     obj = cls.__new__(cls)
     obj.sampler, obj.sig, obj.dev, obj.spec = gs, _sig(), torch.device("cuda", 0), {}
-    obj.graph = obj.graph_run = None
+    obj.graph = None
     obj.capture_failed = False
     return obj
 
