@@ -323,6 +323,48 @@ int hgt_typed_linear_presplit_t24(const void* a_hi, const void* a_lo, const floa
                                   int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off,
                                   void* out24, void* workspace, size_t workspace_bytes, void* stream);
 
+/* bs16 gather tables (inference [K'|V'] and RTE tables that do not fit in L2; see hgt_gather_table_format).
+ * Blocks: a row of n logical elements (n % 16 == 0) is cut into blocks of 16 consecutive elements.  For a block with
+ * largest |x| = a (fp32):
+ *   s = fp32(a * fp32(1/32767)) rounded up to bf16;  r = 1 / s in IEEE fp32, times fp32(1 - 2^-15) when s >= 2^112;
+ *   m = rint_even(fp32(x * r)) as int16, |m| <= 32767.
+ * The element decodes to m * s, which is exact in fp32 (a 15-bit integer times an 8-bit significand, never past
+ * FLT_MAX: that is what the 1 - 2^-15 near the top of the range is for), so a decoded table holds ordinary fp32 values.
+ * Special blocks: one whose s would be below FLT_MIN (a < ~3.9e-34, all-zero blocks included) stores s = 0 and m = 0:
+ * zero encodes to zero bytes.  One holding a NaN or an Inf stores s = NaN (bf16 0x7FC0) and m = 0, so all its elements
+ * decode to NaN: a row that is non-finite in fp32 stays non-finite, a finite row stays finite.
+ * Rows (planar): [m x n (int16) | s x n/16 (bf16)], zero-padded to a multiple of 16 bytes: element c has its mantissa
+ * at byte 2c and its block's scale at byte 2n + 2 (c / 16).  A [K'|V'] row (n = 2d) takes (4.25 d rounded up to 16) bytes:
+ * 1088 at d = 256, 1712 at d = 400, 544 at d = 128.
+ * hgt_typed_linear_bs16 / hgt_typed_linear_presplit_bs16: as the _t24 calls (fp32 column blocks before t24_off at out,
+ * the others in the table at out16, 16-byte aligned, each block encoded once as it is stored, so the output equals the
+ * fp32 call's output encoded, bitwise); a block's rows of ld elements lie hgt_gather_table_row_bytes(HGT_TABLE_BS16, ld)
+ * bytes apart.
+ * Needs cb_width % 16 == 0, so that no 16-element block straddles two column blocks. */
+int hgt_typed_linear_bs16(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                          int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                          int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off, void* out16,
+                          int32_t impl, void* workspace, size_t workspace_bytes, void* stream);
+int hgt_typed_linear_presplit_bs16(const void* a_hi, const void* a_lo, const float* W, const float* bias, int32_t K,
+                                   int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                   int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off,
+                                   void* out16, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Storage format of an inference forward's [K'|V'] and RTE gather tables (one forward that keeps nothing for a
+ * backward, outside bf16 autocast), decided here for both hgt_conv_forward and the per-stage Python path so that they
+ * compute the same bits.  table_rows: rows of the [K'|V'] table (trailing zero row included); l2_bytes: the device's
+ * L2 size.  *out_format = HGT_TABLE_BS16 where d % 128 == 0 and the 24-bit table would be larger than L2 (the edge pass
+ * then reads its rows from HBM, and fewer bytes per row are time saved; at d % 128 == 0 the projection's tensor-store
+ * epilogue writes each tile's scales as one TMA box, elsewhere its scattered scale stores cost more than the edge pass
+ * gains), HGT_TABLE_T24 where d % 8 == 0 otherwise (an L2-resident table gains nothing from fewer bytes and keeps the
+ * smaller error), else HGT_TABLE_F32. */
+#define HGT_TABLE_F32 0
+#define HGT_TABLE_T24 1
+#define HGT_TABLE_BS16 2
+int hgt_gather_table_format(int32_t d, int64_t table_rows, int64_t l2_bytes, int32_t* out_format);
+/* *out_bytes = the bytes of a table row of n elements in a format: 4n, 3n or the bs16 row */
+int hgt_gather_table_row_bytes(int32_t format, int64_t n, int64_t* out_bytes);
+
 /* ------------------------------------------------------------------------------------------------
  * Fused edge kernel: gather -> relation-specific score -> softmax by destination -> weighted sum
  * (conv.py:99,108-111 + PyG scatter-add), one pass over the destination-sorted CSR.
@@ -426,6 +468,17 @@ int hgt_edge_forward_t24(const float* q, const void* kv, const void* kvr,
                          float* agg_out, float* att_out, float* stats_out, void* g_hi, void* g_lo,
                          void* workspace, size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
                          const int32_t* type_row0, int32_t num_types, const int32_t* type_active, void* stream);
+/* The edge forward on bs16 gather tables (see hgt_typed_linear_bs16): kv [rows+1] and kvr [P*240+1] rows of the bs16
+ * row bytes of 2d, decoded to fp32 in registers (each element's m * s, exact), so the result equals hgt_edge_forward's
+ * on the decoded tables, bitwise.  Everything else as hgt_edge_forward_bf16.  Needs d % 16 == 0.  No backward. */
+int hgt_edge_forward_bs16(const float* q, const void* kv, const void* kvr,
+                          const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
+                          const int32_t* csr_eid, const int32_t* tiles, int32_t n_tiles, int32_t n_split_tiles,
+                          const int32_t* hubs, int32_t n_hubs,
+                          int64_t n_nodes, int64_t n_edges, int32_t d, int32_t n_heads, int32_t apply_gelu,
+                          float* agg_out, float* att_out, float* stats_out, void* g_hi, void* g_lo,
+                          void* workspace, size_t workspace_bytes, int32_t variant, const int32_t* d_tile_counts,
+                          const int32_t* type_row0, int32_t num_types, const int32_t* type_active, void* stream);
 int hgt_edge_backward_bf16(const float* q, const void* kv, const void* kvr, const float* agg, const float* dagg,
                            const float* stats, const int32_t* row_ptr, const int32_t* kv_row, const int32_t* rte_row,
                            const int32_t* tiles, int32_t n_tiles, int64_t n_nodes, int32_t d, int32_t n_heads,
@@ -679,7 +732,8 @@ int hgt_tanh_dropout_bwd(const float* dout, const float* out, int64_t n_rows, in
  * per nn.Linear / nn.LayerNorm of the module (conv.py:34-40).  The plan arrays come from hgt_plan_*; the typed-linear
  * tables are the ones hgt_typed_linear takes (projection: Q + [K'|V'] blocks; rte: K'R/V'R tables; rt: the single
  * 240 x d group of RelTemporalEncoding.lin; upd: a_linears).  Nothing is allocated or synchronised.
- * With d_out % 8 == 0 the [K'|V'] and RTE tables are 24-bit (hgt_typed_linear_t24, hgt_edge_forward_t24).
+ * The [K'|V'] and RTE tables take the format hgt_gather_table_format picks for the device's L2: bs16
+ * (hgt_typed_linear_bs16, hgt_edge_forward_bs16), 24-bit (hgt_typed_linear_t24, hgt_edge_forward_t24) or fp32.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
   /* sizes and switches */

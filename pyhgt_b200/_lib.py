@@ -77,11 +77,18 @@ SIGNATURES = {
     # 24-bit gather tables: the fp32 twins' arguments with (out, t24_off, out24) for out
     "hgt_typed_linear_t24": [_p, _i64, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i64, _p, _i32, _p, _sz, _p],
     "hgt_typed_linear_presplit_t24": [_p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _sz, _p],
+    # bs16 gather tables: the 24-bit calls' arguments
+    "hgt_gather_table_format": [_i32, _i64, _i64, _c.POINTER(_i32)],
+    "hgt_gather_table_row_bytes": [_i32, _i64, _c.POINTER(_i64)],
+    "hgt_typed_linear_bs16": [_p, _i64, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i64, _p, _i32, _p, _sz, _p],
+    "hgt_typed_linear_presplit_bs16": [_p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _i64, _p, _p, _sz, _p],
     "hgt_edge_forward_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i64, _i32, _i32, _i32, _p, _p,
                               _p, _p, _p, _p, _sz, _i32, _p, _p, _i32, _p, _p],
     # 24-bit gather tables (inference forwards that keep nothing for a backward): same arguments as the bf16 twins
     "hgt_edge_forward_t24": [_p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i64, _i32, _i32, _i32, _p, _p,
                              _p, _p, _p, _p, _sz, _i32, _p, _p, _i32, _p, _p],
+    "hgt_edge_forward_bs16": [_p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i64, _i32, _i32, _i32, _p, _p,
+                              _p, _p, _p, _p, _sz, _i32, _p, _p, _i32, _p, _p],
     "hgt_edge_backward_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, _i64, _i64, _p, _p, _p, _p,
                                _sz, _p, _p],
     "hgt_edge_backward_dst_bf16": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _i32, _i64, _i32, _i32, _p, _p,
@@ -235,6 +242,25 @@ def check(rc, what):
 def call(name, *args):
     lib = load()
     check(getattr(lib, name)(*args), name)
+
+
+TABLE_F32, TABLE_T24, TABLE_BS16 = 0, 1, 2                     # HGT_TABLE_* (include/hgt_b200.h)
+TABLE_SUFFIX = {TABLE_F32: "", TABLE_T24: "_t24", TABLE_BS16: "_bs16"}   # entry-point suffix of a format
+
+
+def gather_table_format(d, table_rows, device):
+    """hgt_gather_table_format for an inference forward's [K'|V'] table of table_rows rows on `device`."""
+    import torch
+    out = _c.c_int32()
+    call("hgt_gather_table_format", d, table_rows, torch.cuda.get_device_properties(device).L2_cache_size,
+         _c.byref(out))
+    return out.value
+
+
+def gather_table_row_bytes(fmt, n):
+    out = _c.c_int64()
+    call("hgt_gather_table_row_bytes", fmt, n, _c.byref(out))
+    return out.value
 
 
 def kernel_launches():

@@ -60,8 +60,9 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-# entry-point suffix of a gather table's storage dtype: fp32, bf16 (autocast) or 24-bit (uint8 bytes, planar)
-_TABLE_SUFFIX = {torch.float32: "", torch.bfloat16: "_bf16", torch.uint8: "_t24"}
+# entry-point suffix of a gather table's format: fp32, bf16 (autocast), or the uint8 byte formats 24-bit and bs16
+_TABLE_SUFFIX = {"f32": "", "bf16": "_bf16", _lib.TABLE_T24: "_t24", _lib.TABLE_BS16: "_bs16", _lib.TABLE_F32: ""}
+_BYTE_TABLES = ("_t24", "_bs16")                             # their producers write fp32 blocks to out32
 
 
 def _output_rows(rows, d, dev, lt, out_map):
@@ -196,16 +197,18 @@ class HGTConv(nn.Module):
                     HGTConv.event_sink.append((name, self_.a, self_.b))
         return _T()
 
-    def _typed_linear(self, a, lda, w, bias, k, width, table, out, impl, st, out32=None, t24_off=0):
+    def _typed_linear(self, a, lda, w, bias, k, width, table, out, impl, st, out32=None, t24_off=0, fmt=None):
         """hgt_typed_linear with its (impl-dependent) workspace; table = (groups_dev, groups_host, n, cblocks_dev).
-        A bf16 `out` takes hgt_typed_linear_bf16, a uint8 one (a 24-bit table) hgt_typed_linear_t24, which writes the
-        column blocks before t24_off as fp32 to out32.  A bf16 `a` (fp32 `out`) takes hgt_typed_linear_bf16a."""
+        A bf16 `out` takes hgt_typed_linear_bf16; a uint8 one is a table in the byte format `fmt` (_lib.TABLE_T24 or
+        TABLE_BS16) and takes hgt_typed_linear_t24 / _bs16, which write the column blocks before t24_off as fp32 to
+        out32.  A bf16 `a` (fp32 `out`) takes hgt_typed_linear_bf16a."""
         g_dev, g_host, n_g, c_dev = table
         ws_bytes = ctypes.c_size_t()
         _lib.call("hgt_typed_linear_workspace_bytes", g_host.ctypes.data, n_g, k, width, impl, ctypes.byref(ws_bytes))
         ws = torch.empty(max(ws_bytes.value, 1), dtype=torch.uint8, device=out.device)
-        outs = (_lib.ptr(out32), t24_off, out.data_ptr()) if out.dtype == torch.uint8 else (out.data_ptr(),)
-        fn = "hgt_typed_linear_bf16a" if a.dtype == torch.bfloat16 else "hgt_typed_linear" + _TABLE_SUFFIX[out.dtype]
+        sfx = "_bf16" if out.dtype == torch.bfloat16 else _TABLE_SUFFIX[fmt] if out.dtype == torch.uint8 else ""
+        outs = (_lib.ptr(out32), t24_off, out.data_ptr()) if sfx in _BYTE_TABLES else (out.data_ptr(),)
+        fn = "hgt_typed_linear_bf16a" if a.dtype == torch.bfloat16 else "hgt_typed_linear" + sfx
         _lib.call(fn, a.data_ptr(), lda, w.data_ptr(), _lib.ptr(bias), k, width, g_dev.data_ptr(),
                   g_host.ctypes.data, n_g, c_dev.data_ptr(), *outs, impl, ws.data_ptr(), ws.numel(), st)
 
@@ -406,9 +409,9 @@ class HGTConv(nn.Module):
               gelu_before_a, x_split=None, kv_runs=None, bf16=False, plan=None, impl=None, dst=False):
         """Everything up to and including the typed a_linear: plan, weight fold, typed projections, fused edge kernel
         (gelu fused iff gelu_before_a and not save), a_linears.  Returns a dict of the intermediates.  bf16: bf16 [K'|V'] and
-        RTE tables (Q and everything else fp32).  Otherwise a forward that keeps nothing for a backward (not save) with
-        d % 8 == 0 builds 24-bit tables (uint8 tensors in the planar format of hgt_typed_linear_t24), as hgt_conv_forward
-        does; every other forward keeps fp32 tables.  impl: the GEMMs' C impl (autograd.gemm_impl; 3 = one bf16 product, no lo
+        RTE tables (Q and everything else fp32).  Otherwise a forward that keeps nothing for a backward (not save) builds
+        its tables in the format hgt_gather_table_format picks, as hgt_conv_forward does: bs16 or 24-bit (uint8 tensors
+        in the planar formats of hgt_typed_linear_bs16 / _t24) or fp32; every other forward keeps fp32 tables.  impl: the GEMMs' C impl (autograd.gemm_impl; 3 = one bf16 product, no lo
         halves are made or read), linear_impl by default.  dst: tables over each type's destination extent
         (plan.layer_tables); `o` then holds only the rows inside the extents."""
         if impl is None:
@@ -453,15 +456,16 @@ class HGTConv(nn.Module):
         # 2. typed projections: Q [N,d] and the folded [K'|V'] table (+ trailing all-zero row).  bf16: Q by its own fp32
         # call, the K'/V' blocks straight into the bf16 table.  24-bit: one call writes the Q blocks (before kv_off) as
         # fp32 and the K'/V' blocks into the 24-bit table.
-        t24 = not save and not bf16 and d % 8 == 0
-        tab_dtype = torch.bfloat16 if bf16 else torch.uint8 if t24 else torch.float32
-        row_len = 2 * d * (3 if t24 else 1)                       # table row in tab_dtype elements
+        fmt = "bf16" if bf16 else _lib.TABLE_F32 if save else _lib.gather_table_format(d, plan.kv_rows + 1, dev)
+        byte_tab = fmt in (_lib.TABLE_T24, _lib.TABLE_BS16)        # uint8 tables; Q goes to its own fp32 buffer
+        tab_dtype = torch.bfloat16 if bf16 else torch.uint8 if byte_tab else torch.float32
+        row_len = _lib.gather_table_row_bytes(fmt, 2 * d) if byte_tab else 2 * d   # table row in tab_dtype elements
         proj = None
         if bf16:
             q_tab = torch.empty(N * d, **f32)
             kv_tab = torch.empty((plan.kv_rows + 1) * row_len, dtype=tab_dtype, device=dev)
             calls = ((lt.q_groups, q_tab, None), (lt.kv_groups, kv_tab, None))
-        elif t24:
+        elif byte_tab:
             q_buf = torch.empty(lt.kv_off, **f32)
             q_tab = q_buf[lt.q_off:lt.q_off + N * d]
             kv_tab = torch.empty((plan.kv_rows + 1) * row_len, dtype=tab_dtype, device=dev)
@@ -478,15 +482,17 @@ class HGTConv(nn.Module):
             xs = x_split if plan.sorted_types else None
             for tab, out, out32 in calls:
                 if xs is None:
-                    self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, out, impl, st, out32, lt.kv_off)
+                    self._typed_linear(x_sorted, d_in, w_cat, b_cat, d_in, d, tab, out, impl, st, out32, lt.kv_off,
+                                       fmt)
                     continue
                 g_dev, g_host, n_g, c_dev = tab
                 wsb = ctypes.c_size_t()
                 _lib.call("hgt_typed_linear_presplit_workspace_bytes", g_host.ctypes.data, n_g, d_in, d,
                           ctypes.byref(wsb))
                 ws1 = torch.empty(max(wsb.value, 1), dtype=torch.uint8, device=dev)
-                outs = (out32.data_ptr(), lt.kv_off, out.data_ptr()) if t24 else (out.data_ptr(),)
-                _lib.call("hgt_typed_linear_presplit" + _TABLE_SUFFIX[out.dtype], xs[0].data_ptr(),
+                outs = (out32.data_ptr(), lt.kv_off, out.data_ptr()) if byte_tab else (out.data_ptr(),)
+                sfx = _TABLE_SUFFIX[fmt] if out is kv_tab else ""
+                _lib.call("hgt_typed_linear_presplit" + sfx, xs[0].data_ptr(),
                           None if one else _lib.ptr(xs[1]), w_cat.data_ptr(), b_cat.data_ptr(), d_in, d, g_dev.data_ptr(),
                           g_host.ctypes.data, n_g, c_dev.data_ptr(), *outs, ws1.data_ptr(), ws1.numel(), st)
         kvr = None
@@ -497,7 +503,7 @@ class HGTConv(nn.Module):
                                lt.rt_group, rt, 1, st)
             kvr = torch.empty((P * _plan.RTE_MAX_LEN + 1) * row_len, dtype=tab_dtype, device=dev)
             kvr[P * _plan.RTE_MAX_LEN * row_len:].zero_()
-            self._typed_linear(rt, d_in, w_cat, None, d_in, d, lt.rte_groups, kvr, 1, st)
+            self._typed_linear(rt, d_in, w_cat, None, d_in, d, lt.rte_groups, kvr, 1, st, fmt=fmt)
 
         # 3. fused edge kernel -> gelu(aggregate)
         ws_bytes = ctypes.c_size_t()
@@ -513,7 +519,7 @@ class HGTConv(nn.Module):
         att = torch.empty((E, H), **f32) if want_att else None
         stats = torch.empty((N, 2 * H), **f32) if save else None
         with self._stage("edge"):
-            _lib.call("hgt_edge_forward" + _TABLE_SUFFIX[tab_dtype], q_tab.data_ptr(), kv_tab.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
+            _lib.call("hgt_edge_forward" + _TABLE_SUFFIX[fmt], q_tab.data_ptr(), kv_tab.data_ptr(), _lib.ptr(kvr), plan.row_ptr.data_ptr(),
                       plan.kv_row.data_ptr(), _lib.ptr(plan.rte_row) if self.use_RTE else None,
                       plan.csr_eid.data_ptr(), plan.tiles.data_ptr(), plan.n_tiles, plan.n_split,
                       plan.hubs.data_ptr(), plan.n_hubs, N, E, d, H, 1 if (gelu_before_a and not save) else 0,

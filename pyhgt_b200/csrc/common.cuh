@@ -68,6 +68,70 @@ struct hgt_t24_at {
   }
 };
 
+// ---- bs16 gather tables (format: include/hgt_b200.h, "bs16 gather tables") -----------------------------------------
+// Element type tag of the block-scaled 16-bit table: a row of n elements is hgt_bs16_row_bytes(n) bytes in two planes
+// (n int16 mantissas, then n / 16 bf16 scales), addressed through hgt_bs16_at.
+struct hgt_bs16 {};
+
+__host__ __device__ __forceinline__ int64_t hgt_bs16_row_bytes(int64_t n) { return (2 * n + n / 8 + 15) / 16 * 16; }
+
+// fp32(1 / (1 + i / 128)), i < 128: the correctly rounded reciprocal of a bf16 significand (a constant expression,
+// rounded by the compiler)
+struct HgtBs16RcpTab {
+  float v[128];
+};
+constexpr HgtBs16RcpTab hgt_bs16_rcp_tab() {
+  HgtBs16RcpTab t{};
+  for (int i = 0; i < 128; ++i) t.v[i] = 1.0f / (1.0f + (float)i / 128.0f);
+  return t;
+}
+static __device__ const HgtBs16RcpTab kHgtBs16Rcp = hgt_bs16_rcp_tab();
+
+// Scale of a 16-element block from the largest |x| as fp32 bits (amax = max of bits & 0x7fffffff): the bf16 bits of s,
+// and r, the factor the elements are multiplied by before rounding (0 where the block stores no mantissas).  Branch-free
+// so that the epilogues overlap the blocks' shuffles and loads: r = 1 / s is the significand's reciprocal from the
+// table with s's exponent negated, exact scaling by a power of two while 1 / s stays normal (s in [2^-126, 2^114]).
+__device__ __forceinline__ uint32_t hgt_bs16_scale(uint32_t amax, float& r) {
+  const float t = __fmul_rn(__uint_as_float(amax), 3.0518509447574615e-05f);  // fp32(1 / 32767)
+  const uint32_t sb = (__float_as_uint(t) + 0xffffu) >> 16;                 // rounded up to bf16
+  const int e = (int)((sb >> 7) & 0xffu);
+  float rr = __uint_as_float(__float_as_uint(__ldg(&kHgtBs16Rcp.v[sb & 0x7fu])) + ((uint32_t)(127 - e) << 23));
+  rr = sb >= 0x7780u ? __fmul_rn(rr, 0.999969482421875f) : rr;             // s >= 2^112: keep m * s below 2^128
+  const bool nonfinite = amax >= 0x7f800000u;                               // NaN or Inf in the block: NaN scale,
+                                                                            // zero mantissas (hgt_bs16_pack)
+  const bool tiny = sb < 0x80u;                                             // s below FLT_MIN: the block stores zero
+  r = nonfinite || tiny ? 0.f : rr;
+  return nonfinite ? 0x7fc0u : tiny ? 0u : sb;
+}
+
+// Mantissas of two elements of a block with scale bits sb as (m0 & 0xffff) | (m1 << 16), m = rint_even(fl(x * r)):
+// adding 1.5 * 2^23 rounds the product to an integer and leaves it, two's complement, in the low bits of the sum
+// (|x * r| <= 32767.5).  A NaN-scale block stores zero mantissas.
+__device__ __forceinline__ uint32_t hgt_bs16_pack(float x0, float x1, float r, uint32_t sb) {
+  const float y0 = __fadd_rn(__fmul_rn(x0, r), 12582912.f), y1 = __fadd_rn(__fmul_rn(x1, r), 12582912.f);
+  return sb == 0x7fc0u ? 0u : __byte_perm(__float_as_uint(y0), __float_as_uint(y1), 0x5410);
+}
+
+// Largest |x| bits over the 16-element block that the four lanes of an aligned quad hold (`a`: this lane's part).
+__device__ __forceinline__ uint32_t hgt_bs16_quad_amax(uint32_t a) {
+  a = max(a, __shfl_xor_sync(0xffffffffu, a, 1));
+  return max(a, __shfl_xor_sync(0xffffffffu, a, 2));
+}
+__device__ __forceinline__ uint32_t hgt_abs_bits(float x) { return __float_as_uint(x) & 0x7fffffffu; }
+
+// Element (row, col) of a table whose rows hold ld logical elements, given its logical offset off = row * ld + col:
+// the byte of its mantissa and of its block's scale (col % 16 == 0 for the scale to be the block's first).
+struct hgt_bs16_at {
+  unsigned char* m;
+  unsigned char* s;
+  __host__ __device__ __forceinline__ hgt_bs16_at(void* base, int64_t off, int64_t ld) {
+    const int64_t row = off / ld, col = off - row * ld;
+    unsigned char* r = static_cast<unsigned char*>(base) + row * hgt_bs16_row_bytes(ld);
+    m = r + 2 * col;
+    s = r + 2 * ld + 2 * (col / 16);
+  }
+};
+
 // ---- in-kernel dropout (mask contract: include/hgt_b200.h, "Fused dropout") ------------------------------------------
 // Host side of the contract: keep threshold and scale of a drop probability p > 0.
 struct HgtDrop {

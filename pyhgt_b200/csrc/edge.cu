@@ -16,7 +16,8 @@
 //                      ring with mbarrier transaction counting; the warp issues STAGES rows ahead.
 // Roofline: HBM-bound; algorithmic bytes per edge = 2*d*s_kv (row) + 4 (kv_row) [+4 rte_row, +2*d*s_kv from L2]
 // and per destination d*4 (Q) + d*4 (agg) + 4 (row_ptr), with s_kv = 4 (fp32 tables), 2 (bf16 tables,
-// hgt_edge_forward_bf16) or 3 (24-bit tables, hgt_edge_forward_t24).  Every kernel is templated on the table element
+// hgt_edge_forward_bf16), 3 (24-bit tables, hgt_edge_forward_t24) or 2.125 (bs16 tables, hgt_edge_forward_bs16: 16-bit
+// mantissas and a bf16 scale per 16 elements, rows padded to 16 bytes).  Every kernel is templated on the table element
 // type KV and decodes rows to fp32 in registers; the lane map, the softmax and every output are the same.
 #include <cuda_bf16.h>
 
@@ -140,7 +141,25 @@ __device__ __forceinline__ void t24_decode(float (&dst)[VEC], uint32_t h0, uint3
   }
 }
 
-template <class KV> constexpr int64_t kv_elem_bytes() { return std::is_same<KV, hgt_t24>::value ? 3 : sizeof(KV); }
+// bs16 table rows (hgt_bs16): VEC int16 mantissas (a VEC-aligned run never leaves its 16-element block) times the
+// block's bf16 scale.  m * s is exact in fp32, so the row decodes to the same fp32 values whatever the lane map.
+template <int VEC>
+__device__ __forceinline__ void bs16_decode(float (&dst)[VEC], uint32_t m0, uint32_t m1, uint32_t sb) {
+  const float s = __uint_as_float(sb << 16);
+  dst[0] = __fmul_rn(__int2float_rn((int)(int16_t)(m0 & 0xffffu)), s);
+  if constexpr (VEC >= 2) dst[1] = __fmul_rn(__int2float_rn((int)m0 >> 16), s);
+  if constexpr (VEC == 4) {
+    dst[2] = __fmul_rn(__int2float_rn((int)(int16_t)(m1 & 0xffffu)), s);
+    dst[3] = __fmul_rn(__int2float_rn((int)m1 >> 16), s);
+  }
+}
+
+template <class KV> constexpr bool is_bs16() { return std::is_same<KV, hgt_bs16>::value; }
+// bytes of a table row of n elements
+template <class KV> __host__ __device__ __forceinline__ int64_t kv_row_bytes(int64_t n) {
+  if constexpr (is_bs16<KV>()) return hgt_bs16_row_bytes(n);
+  return n * (std::is_same<KV, hgt_t24>::value ? 3 : (int64_t)sizeof(KV));
+}
 
 // Elements e .. e + VEC - 1 of a table row of n elements that starts at `row`.  NC: a streaming gather from global
 // memory (read-only path, no L1 allocation); otherwise a plain load (shared-memory ring, L2-resident RTE rows).
@@ -175,6 +194,27 @@ __device__ __forceinline__ void load_kv(float (&dst)[VEC], const unsigned char* 
       }
     }
     t24_decode<VEC>(dst, h0, h1, l);
+  } else if constexpr (is_bs16<KV>()) {
+    const unsigned char* mp = row + 2 * e;
+    const unsigned char* sp = row + 2 * n + 2 * (e >> 4);
+    uint32_t m0 = 0, m1 = 0, sb = 0;
+    if constexpr (NC) {
+      if constexpr (VEC == 4) asm volatile("ld.global.nc.L1::no_allocate.v2.b32 {%0,%1}, [%2];" : "=r"(m0), "=r"(m1) : "l"(mp));
+      else if constexpr (VEC == 2) asm volatile("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(m0) : "l"(mp));
+      else asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=r"(m0) : "l"(mp));
+      asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=r"(sb) : "l"(sp));
+    } else {
+      if constexpr (VEC == 4) {
+        const uint2 m = *reinterpret_cast<const uint2*>(mp);
+        m0 = m.x; m1 = m.y;
+      } else if constexpr (VEC == 2) {
+        m0 = *reinterpret_cast<const uint32_t*>(mp);
+      } else {
+        m0 = *reinterpret_cast<const uint16_t*>(mp);
+      }
+      sb = *reinterpret_cast<const uint16_t*>(sp);
+    }
+    bs16_decode<VEC>(dst, m0, m1, sb);
   } else {
     const KV* p = reinterpret_cast<const KV*>(row) + e;
     if constexpr (NC) load_vec_nc<VEC>(dst, p);
@@ -304,8 +344,8 @@ template <class KV, int VEC, int NCH>
 __global__ void __launch_bounds__(kCtaThreads, 1)
 k_edge_fwd_ldg(EdgeParams p) {
   // rows in flight per warp: bounded by the register budget (2 * U * NCH * VEC floats of staging)
-  // (24-bit rows: half as many, their two planes' addresses and raw words take the registers of the rest)
-  constexpr int W = std::is_same<KV, hgt_t24>::value ? 2 * NCH * VEC : NCH * VEC;
+  // (24-bit and bs16 rows: half as many, their two planes' addresses and raw words take the registers of the rest)
+  constexpr int W = std::is_same<KV, hgt_t24>::value || is_bs16<KV>() ? 2 * NCH * VEC : NCH * VEC;
   constexpr int EDGE_UNROLL = (W >= 32) ? 1 : (W >= 16 ? 2 : 4);
   const int lane = threadIdx.x & 31;
   const LaneMap lm(p, lane);
@@ -313,7 +353,7 @@ k_edge_fwd_ldg(EdgeParams p) {
   const unsigned char* const kvrt = static_cast<const unsigned char*>(p.kvr);
   const bool rte = kvrt != nullptr;
   const int n = 2 * p.d;                                      // elements per table row
-  const int64_t row_bytes = n * kv_elem_bytes<KV>();
+  const int64_t row_bytes = kv_row_bytes<KV>(n);
   int offs[NCH];
 #pragma unroll
   for (int t = 0; t < NCH; ++t) offs[t] = lm.off<VEC>(t);
@@ -473,7 +513,7 @@ k_edge_fwd_tma(EdgeParams p) {
   const bool rte = kvrt != nullptr;
   const int S = p.stages;
   const int n = 2 * p.d;                                      // elements per table row
-  const uint32_t row_bytes = (uint32_t)(n * kv_elem_bytes<KV>());
+  const uint32_t row_bytes = (uint32_t)kv_row_bytes<KV>(n);
   const uint32_t slot_bytes = rte ? 2u * row_bytes : row_bytes;
   // layout: [warps][S][slot_bytes] rows, then [warps][S] mbarriers
   unsigned char* ring = smem_raw + (size_t)warp * S * slot_bytes;
@@ -769,6 +809,21 @@ extern "C" int hgt_edge_forward_t24(const float* q, const void* kv, const void* 
                                d_tile_counts, type_row0, num_types, type_active, (cudaStream_t)stream_);
 }
 
+extern "C" int hgt_edge_forward_bs16(const float* q, const void* kv, const void* kvr, const int32_t* row_ptr,
+                                     const int32_t* kv_row, const int32_t* rte_row, const int32_t* csr_eid,
+                                     const int32_t* tiles, int32_t n_tiles, int32_t n_split_tiles, const int32_t* hubs,
+                                     int32_t n_hubs, int64_t n_nodes, int64_t n_edges, int32_t d, int32_t n_heads,
+                                     int32_t apply_gelu, float* agg_out, float* att_out, float* stats_out, void* g_hi,
+                                     void* g_lo, void* workspace, size_t workspace_bytes, int32_t variant,
+                                     const int32_t* d_tile_counts, const int32_t* type_row0, int32_t num_types,
+                                     const int32_t* type_active, void* stream_) {
+  (void)n_edges;
+  return edge_forward<hgt_bs16>(q, static_cast<const hgt_bs16*>(kv), static_cast<const hgt_bs16*>(kvr), row_ptr, kv_row,
+                                rte_row, csr_eid, tiles, n_tiles, n_split_tiles, hubs, n_hubs, n_nodes, d, n_heads,
+                                apply_gelu, agg_out, att_out, stats_out, g_hi, g_lo, workspace, workspace_bytes, variant,
+                                d_tile_counts, type_row0, num_types, type_active, (cudaStream_t)stream_);
+}
+
 namespace {
 
 template <class KV>
@@ -819,7 +874,8 @@ int edge_forward(const float* q, const KV* kv, const KV* kvr, const int32_t* row
   int grid = sms;
   size_t smem = 0;
   HGT_REQUIRE((!std::is_same<KV, hgt_t24>::value || d % 8 == 0), "hgt_edge_forward_t24: needs d %% 8 == 0 (d=%d)", d);
-  const size_t row_bytes = 2 * (size_t)d * kv_elem_bytes<KV>();
+  HGT_REQUIRE((!is_bs16<KV>() || d % 16 == 0), "hgt_edge_forward_bs16: needs d %% 16 == 0 (d=%d)", d);
+  const size_t row_bytes = (size_t)kv_row_bytes<KV>(2 * (int64_t)d);
   const size_t slot_bytes = kvr ? 2 * row_bytes : row_bytes;
   if (variant == 0) variant = 2;
   // narrow rows (one float4 per lane): the kernel is bound by per-destination latency, not by bytes in flight, so two
@@ -828,7 +884,9 @@ int edge_forward(const float* q, const KV* kv, const KV* kvr, const int32_t* row
   if (variant == 2) {
     const size_t budget = two_ctas ? 100 * 1024 : 200 * 1024;
     int stages = (int)(budget / (kWarpsPerCta * slot_bytes));
-    if (stages > 8) stages = 8;
+    // bs16 rows (17 d bytes): up to 12 stages, about the bytes in flight of 8 24-bit rows
+    const int max_stages = is_bs16<KV>() ? 12 : 8;
+    if (stages > max_stages) stages = max_stages;
     if (stages < 2 || row_bytes % 16 != 0) variant = 1;     // rows too wide / misaligned for the ring
     else {
       p.stages = stages;

@@ -6,9 +6,11 @@
 // one ctypes call instead of a dozen (the reference's sampled-subgraph batches are launch/host-bound).
 // linear_impl 3 runs the tensor-core GEMMs with one bf16 product: the edge kernel then writes gelu(agg) as bf16 hi only,
 // and a pre-split x needs no lo half.
-// With d_out % 8 == 0 the [K'|V'] and RTE tables are 24-bit (hgt_typed_linear_t24, hgt_edge_forward_t24): the projection
-// writes Q as fp32 and the K'/V' blocks straight into the 24-bit table.  A forward that keeps nothing for a backward needs
-// no more than that precision (DESIGN.md §4.2), and the edge pass reads 6d instead of 8d bytes per edge.
+// The [K'|V'] and RTE tables take the format hgt_gather_table_format picks: bs16 when the 24-bit table would not fit in
+// L2 and d_out % 128 == 0 (hgt_typed_linear_bs16, hgt_edge_forward_bs16; 4.25d bytes per row), else 24-bit when d_out % 8
+// == 0 (hgt_typed_linear_t24, hgt_edge_forward_t24; 6d bytes), else fp32.  The projection writes Q as fp32 and the
+// K'/V' blocks straight into the table.  A forward that keeps nothing for a backward needs no more than that precision
+// (DESIGN.md §4.2, §4.3), and the edge pass reads fewer bytes per edge.
 #include "common.cuh"
 
 int hgt_update_epilogue_impl(const float* o, const float* x, const int32_t* type_row0, int32_t num_types,
@@ -35,10 +37,12 @@ struct Carver {
 
 struct Layout {
   float *x_sorted, *w_cat, *b_cat, *proj, *rt, *g_act, *wa_cat, *ba_cat, *o;
-  void *kv, *kvr;                                          // fp32 (inside proj) or 24-bit tables
+  void *kv, *kvr;                                          // fp32 (inside proj), 24-bit or bs16 tables
   void *g_hi, *g_lo, *ws_proj, *ws_edge, *ws_upd;
   size_t ws_proj_bytes, ws_edge_bytes, ws_upd_bytes, total;
-  bool fuse_split, presplit_x, t24;
+  size_t row_bytes;                                        // of a [K'|V'] or RTE table row
+  int32_t fmt;                                             // HGT_TABLE_*
+  bool fuse_split, presplit_x;
 };
 
 int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
@@ -54,15 +58,20 @@ int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
   L->x_sorted = a->perm ? c.take<float>((size_t)N * din) : nullptr;
   L->w_cat = c.take<float>((size_t)(a->cat_rows > 0 ? a->cat_rows : 1) * din);
   L->b_cat = c.take<float>((size_t)(a->cat_rows > 0 ? a->cat_rows : 1));
-  L->t24 = d % 8 == 0;
-  if (L->t24) {
+  int dev = 0, l2 = 0;
+  HGT_CHECK_CUDA(cudaGetDevice(&dev));
+  HGT_CHECK_CUDA(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
+  int rc = hgt_gather_table_format(d, a->kv_rows + 1, l2, &L->fmt);
+  int64_t rbytes = 0;
+  if (rc || (rc = hgt_gather_table_row_bytes(L->fmt, 2 * (int64_t)d, &rbytes))) return rc;
+  const size_t row_bytes = L->row_bytes = (size_t)rbytes;
+  if (L->fmt != HGT_TABLE_F32) {
     L->proj = c.take<float>((size_t)a->kv_off);           // Q only
-    L->kv = c.take_bytes((size_t)(a->kv_rows + 1) * 6 * d);
+    L->kv = c.take_bytes((size_t)(a->kv_rows + 1) * row_bytes);
   } else {
     L->proj = c.take<float>((size_t)a->proj_elems);
     L->kv = base ? L->proj + a->kv_off : nullptr;
   }
-  int rc;
   if (L->presplit_x)
     rc = hgt_typed_linear_presplit_workspace_bytes(a->h_proj_groups, a->n_proj_groups, din, d, &L->ws_proj_bytes);
   else
@@ -73,7 +82,7 @@ int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
   L->kvr = nullptr;
   if (a->use_rte) {
     L->rt = c.take<float>((size_t)HGT_RTE_MAX_LEN * din);
-    L->kvr = c.take_bytes(((size_t)a->n_pairs * HGT_RTE_MAX_LEN + 1) * 2 * d * (L->t24 ? 3 : 4));
+    L->kvr = c.take_bytes(((size_t)a->n_pairs * HGT_RTE_MAX_LEN + 1) * row_bytes);
   }
   if ((rc = hgt_edge_workspace_bytes(a->n_split, d, a->n_heads, &L->ws_edge_bytes))) return rc;
   L->ws_edge = c.take_bytes(L->ws_edge_bytes);
@@ -99,6 +108,24 @@ int plan_layout(const hgt_conv_args* a, void* base, Layout* L) {
 }
 
 }  // namespace
+
+extern "C" int hgt_gather_table_format(int32_t d, int64_t table_rows, int64_t l2_bytes, int32_t* out_format) {
+  HGT_REQUIRE(out_format, "hgt_gather_table_format: out_format is NULL");
+  // d % 128 == 0: the projection's tiles are 128 or 256 columns wide and every one stores its scales as a whole
+  // TMA box; the staged epilogue's scattered 8-byte scale stores (d = 400) cost the projection more than the edge
+  // pass gains
+  if (d % 128 == 0 && table_rows * 6 * (int64_t)d > l2_bytes) *out_format = HGT_TABLE_BS16;
+  else *out_format = d % 8 == 0 ? HGT_TABLE_T24 : HGT_TABLE_F32;
+  return 0;
+}
+
+extern "C" int hgt_gather_table_row_bytes(int32_t format, int64_t n, int64_t* out_bytes) {
+  HGT_REQUIRE(out_bytes, "hgt_gather_table_row_bytes: out_bytes is NULL");
+  HGT_REQUIRE(format == HGT_TABLE_F32 || format == HGT_TABLE_T24 || format == HGT_TABLE_BS16,
+              "hgt_gather_table_row_bytes: unknown format %d", format);
+  *out_bytes = format == HGT_TABLE_BS16 ? hgt_bs16_row_bytes(n) : n * (format == HGT_TABLE_T24 ? 3 : 4);
+  return 0;
+}
 
 extern "C" uint64_t hgt_conv_args_size(void) { return sizeof(hgt_conv_args); }
 
@@ -136,10 +163,20 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
                              a->cat_row0, a->q_row0, L.w_cat, L.b_cat, stream)))
     return rc;
   // trailing all-zero [K'|V'] row (edges that match no <s,t,r> triple); zero encodes to zero bytes
-  const size_t row_bytes = (size_t)2 * d * (L.t24 ? 3 : 4);
+  const size_t row_bytes = L.row_bytes;
   HGT_CHECK_CUDA(cudaMemsetAsync(static_cast<char*>(L.kv) + a->kv_rows * row_bytes, 0, row_bytes, st));
   const void* x_lo = a->linear_impl == 3 ? nullptr : a->x_lo;
-  if (L.t24) {
+  if (L.fmt == HGT_TABLE_BS16) {
+    // Q blocks (out_off < kv_off) as fp32, the K'/V' blocks straight into the bs16 table
+    if (L.presplit_x)
+      rc = hgt_typed_linear_presplit_bs16(a->x_hi, x_lo, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
+                                          a->n_proj_groups, a->proj_cblocks, L.proj, a->kv_off, L.kv, L.ws_proj,
+                                          L.ws_proj_bytes + 256, stream);
+    else
+      rc = hgt_typed_linear_bs16(x_sorted, din, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
+                                 a->n_proj_groups, a->proj_cblocks, L.proj, a->kv_off, L.kv, a->linear_impl, L.ws_proj,
+                                 L.ws_proj_bytes + 256, stream);
+  } else if (L.fmt == HGT_TABLE_T24) {
     // Q blocks (out_off < kv_off) as fp32, the K'/V' blocks straight into the 24-bit table
     if (L.presplit_x)
       rc = hgt_typed_linear_presplit_t24(a->x_hi, x_lo, L.w_cat, L.b_cat, din, d, a->proj_groups, a->h_proj_groups,
@@ -162,16 +199,26 @@ extern "C" int hgt_conv_forward(const hgt_conv_args* a, void* workspace, size_t 
                                a->rt_cblocks, L.rt, 1, nullptr, 0, stream)))
       return rc;
     HGT_CHECK_CUDA(cudaMemsetAsync(static_cast<char*>(L.kvr) + (int64_t)P * HGT_RTE_MAX_LEN * row_bytes, 0, row_bytes, st));
-    rc = L.t24 ? hgt_typed_linear_t24(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups,
-                                      a->n_rte_groups, a->rte_cblocks, nullptr, 0, L.kvr, 1, nullptr, 0, stream)
-               : hgt_typed_linear(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups, a->n_rte_groups,
-                                  a->rte_cblocks, static_cast<float*>(L.kvr), 1, nullptr, 0, stream);
+    if (L.fmt == HGT_TABLE_BS16)
+      rc = hgt_typed_linear_bs16(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups, a->n_rte_groups,
+                                 a->rte_cblocks, nullptr, 0, L.kvr, 1, nullptr, 0, stream);
+    else if (L.fmt == HGT_TABLE_T24)
+      rc = hgt_typed_linear_t24(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups, a->n_rte_groups,
+                                a->rte_cblocks, nullptr, 0, L.kvr, 1, nullptr, 0, stream);
+    else
+      rc = hgt_typed_linear(L.rt, din, L.w_cat, nullptr, din, d, a->rte_groups, a->h_rte_groups, a->n_rte_groups,
+                            a->rte_cblocks, static_cast<float*>(L.kvr), 1, nullptr, 0, stream);
     if (rc) return rc;
   }
   // rows past type_dst[t] have no in-edges: as type_active, the edge kernel skips them (their Q rows were not computed)
   const int32_t* dst_rows = a->type_active ? a->type_active : a->type_dst;
   const int32_t* rte_row = a->use_rte ? a->rte_row : nullptr;
-  if (L.t24)
+  if (L.fmt == HGT_TABLE_BS16)
+    rc = hgt_edge_forward_bs16(L.proj + a->q_off, L.kv, L.kvr, a->row_ptr, a->kv_row, rte_row, a->csr_eid, a->tiles,
+                               a->n_tiles, a->n_split, a->hubs, a->n_hubs, N, a->n_edges, d, a->n_heads, 1, L.g_act,
+                               a->att, nullptr, L.g_hi, L.g_lo, L.ws_edge, L.ws_edge_bytes, a->edge_variant,
+                               a->d_tile_counts, a->type_row0, T, dst_rows, stream);
+  else if (L.fmt == HGT_TABLE_T24)
     rc = hgt_edge_forward_t24(L.proj + a->q_off, L.kv, L.kvr, a->row_ptr, a->kv_row, rte_row, a->csr_eid, a->tiles,
                               a->n_tiles, a->n_split, a->hubs, a->n_hubs, N, a->n_edges, d, a->n_heads, 1, L.g_act,
                               a->att, nullptr, L.g_hi, L.g_lo, L.ws_edge, L.ws_edge_bytes, a->edge_variant,

@@ -3,7 +3,8 @@
 // This file holds the fp32 SIMT kernel (impl 1); the wgmma tensor-core kernel (impl 2, split-bf16 x3; impl 3, auto with
 // one bf16 product on the tensor cores) lives in linear_tc.cu and is dispatched from hgt_typed_linear below.  hgt_typed_linear_bf16 runs the same kernels with a bf16
 // output, each fp32 result rounded to nearest-even once when it is stored; hgt_typed_linear_t24 with the planar 24-bit
-// table output (include/hgt_b200.h), each result rounded by hgt_t24_round once when it is stored.  hgt_typed_linear_bf16a
+// table output (include/hgt_b200.h), each result rounded by hgt_t24_round once when it is stored; hgt_typed_linear_bs16
+// with the block-scaled bs16 table output, each 16-column block encoded once when it is stored.  hgt_typed_linear_bf16a
 // reads a bf16 A (fp32 output): the SIMT kernel widens each element as it loads it, the tensor cores skip the products
 // with A's zero lo half (linear_tc.cu); both write bitwise what the fp32 call on the widened A writes.
 #include <cuda_bf16.h>
@@ -23,6 +24,10 @@ int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float
 int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
                         int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
                         int32_t n_groups, const hgt_lin_cblock* cblocks, float* out32, int64_t t24_off, hgt_t24* out,
+                        int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st);
+int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                        int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                        int32_t n_groups, const hgt_lin_cblock* cblocks, float* out32, int64_t t24_off, hgt_bs16* out,
                         int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st);
 int hgt_typed_linear_tc_bf16a(const __nv_bfloat16* A, int64_t lda, const float* W, const float* bias, int32_t K,
                               int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
@@ -178,7 +183,8 @@ k_typed_linear_simt(const AT* __restrict__ A, int64_t lda, const float* __restri
     for (int j = 0; j < 4; ++j)
       if (tn * 4 + j < cols_here) bj[j] = bias[w_row0 + tn * 4 + j];
   }
-  if (std::is_same<OutT, hgt_t24>::value && cblk.out_off < t24_off) {   // an fp32 block of a 24-bit call
+  constexpr bool table = std::is_same<OutT, hgt_t24>::value || std::is_same<OutT, hgt_bs16>::value;
+  if (table && cblk.out_off < t24_off) {                 // an fp32 block of a 24-bit or bs16 call
     float* Og = out32 + cblk.out_off + m0 * cblk.ld + n0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -205,6 +211,28 @@ k_typed_linear_simt(const AT* __restrict__ A, int64_t lda, const float* __restri
           *reinterpret_cast<uint16_t*>(e.hi + r * rb + 2 * c) = (uint16_t)(w >> 16);
           e.lo[r * rb + c] = (unsigned char)(w >> 8);
         }
+      }
+    }
+  } else if constexpr (std::is_same<OutT, hgt_bs16>::value) {
+    // the four threads tn = 4 k .. 4 k + 3 (an aligned quad of lanes) hold a row's 16-column block k
+    const hgt_bs16_at e(out, cblk.out_off - t24_off + m0 * cblk.ld + n0, cblk.ld);
+    const int64_t rb = hgt_bs16_row_bytes(cblk.ld);
+    const int lane = tid & 31;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int r = tm * 8 + i, c = tn * 4;
+      float v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] = acc[i][j] + bj[j];
+      const uint32_t a = hgt_bs16_quad_amax(max(max(hgt_abs_bits(v[0]), hgt_abs_bits(v[1])),
+                                                max(hgt_abs_bits(v[2]), hgt_abs_bits(v[3]))));
+      float rc;
+      const uint32_t sb = hgt_bs16_scale(a, rc);
+      if (r < rows_here && c < cols_here) {
+        // 8-byte aligned: the column is a multiple of 4 (d % 16 == 0) and rows are 16-byte multiples
+        *reinterpret_cast<uint2*>(e.m + r * rb + 2 * c) =
+            make_uint2(hgt_bs16_pack(v[0], v[1], rc, sb), hgt_bs16_pack(v[2], v[3], rc, sb));
+        if ((lane & 3) == 0) *reinterpret_cast<uint16_t*>(e.s + r * rb + 2 * (c / 16)) = (uint16_t)sb;
       }
     }
   } else {
@@ -305,7 +333,7 @@ int typed_linear(const AT* A, int64_t lda, const float* W, const float* bias, in
     if constexpr (std::is_same<AT, __nv_bfloat16>::value)
       return hgt_typed_linear_tc_bf16a(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out,
                                        impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
-    else if constexpr (std::is_same<OutT, hgt_t24>::value)
+    else if constexpr (std::is_same<OutT, hgt_t24>::value || std::is_same<OutT, hgt_bs16>::value)
       return hgt_typed_linear_tc(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out32, t24_off, out,
                                  impl == 3 ? 1 : 3, workspace, workspace_bytes, st);
     else
@@ -353,6 +381,15 @@ extern "C" int hgt_typed_linear_t24(const float* A, int64_t lda, const float* W,
                                     int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off,
                                     void* out24, int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
   return typed_linear(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, static_cast<hgt_t24*>(out24),
+                      impl, workspace, workspace_bytes, (cudaStream_t)stream_, out, t24_off);
+}
+
+extern "C" int hgt_typed_linear_bs16(const float* A, int64_t lda, const float* W, const float* bias, int32_t K,
+                                     int32_t cb_width, const hgt_lin_group* groups, const hgt_lin_group* h_groups,
+                                     int32_t n_groups, const hgt_lin_cblock* cblocks, float* out, int64_t t24_off,
+                                     void* out16, int32_t impl, void* workspace, size_t workspace_bytes, void* stream_) {
+  HGT_REQUIRE(cb_width % 16 == 0, "hgt_typed_linear_bs16: needs cb_width %% 16 == 0 (cb_width=%d)", cb_width);
+  return typed_linear(A, lda, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, static_cast<hgt_bs16*>(out16),
                       impl, workspace, workspace_bytes, (cudaStream_t)stream_, out, t24_off);
 }
 

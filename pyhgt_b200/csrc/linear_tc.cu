@@ -12,8 +12,9 @@
 // leaves a ring of 3 x 48 KB stages at BN = 256 and 5 x 32 KB at BN = 128.  BN = 64 keeps 64-wide k-blocks (SWIZZLE_128B,
 // 4 stages) and the staged st.global epilogue: its k-blocks are short enough that halving them costs more in barrier
 // waits than the deeper ring gains (measured on the d = 400 OAG shape).  Output tiles follow the same group / column-block tables
-// as the SIMT kernel in linear.cu.  The output is fp32, bf16 (hgt_typed_linear[_presplit]_bf16) or the planar 24-bit
-// table format (hgt_typed_linear[_presplit]_t24, include/hgt_b200.h): the same tile, rounded once as the epilogue stores it.
+// as the SIMT kernel in linear.cu.  The output is fp32, bf16 (hgt_typed_linear[_presplit]_bf16), the planar 24-bit
+// table format (hgt_typed_linear[_presplit]_t24) or the block-scaled bs16 format (hgt_typed_linear[_presplit]_bs16,
+// include/hgt_b200.h): the same tile, rounded or encoded once as the epilogue stores it.
 //
 // One-product mode (P = 1: impl 3, or a presplit call with a_lo == NULL): the operands are rounded to bf16 (the hi half
 // of the split, bitwise) and one bf16 product per k-step is accumulated, torch's "medium" float32 matmul precision.  Its
@@ -130,6 +131,19 @@ __device__ __forceinline__ void store4_t24(unsigned char* hi, unsigned char* lo,
   }
 }
 
+// bs16 tables: columns col .. col + 3 of a row (a quarter of a 16-column block, whose other quarters the neighbouring
+// lanes of an aligned quad hold; every lane of the warp calls this) as mantissas at `m` and, from the quad's first lane,
+// the block's scale at `s`.  store: the row and the columns lie inside the output.
+__device__ __forceinline__ void store4_bs16(unsigned char* m, unsigned char* s, float4 v, bool store, int lane) {
+  const uint32_t a = hgt_bs16_quad_amax(max(max(hgt_abs_bits(v.x), hgt_abs_bits(v.y)),
+                                            max(hgt_abs_bits(v.z), hgt_abs_bits(v.w))));
+  float r;
+  const uint32_t sb = hgt_bs16_scale(a, r);
+  if (!store) return;
+  *reinterpret_cast<uint2*>(m) = make_uint2(hgt_bs16_pack(v.x, v.y, r, sb), hgt_bs16_pack(v.z, v.w, r, sb));
+  if ((lane & 3) == 0) *reinterpret_cast<uint16_t*>(s) = (uint16_t)sb;
+}
+
 // ---- the GEMM: out_cb[m, n] = A[a_row0 + m, :] . W[w_row0 + cb * cb_width + n, :] (+ bias) ------------------------------
 // Rows of a tile past the group and columns past the column block are computed on neighbouring (or zero-filled) operand
 // rows and not stored.
@@ -141,8 +155,8 @@ struct FwdJob {
   const hgt_lin_group* groups;
   const hgt_lin_cblock* cblocks;
   OutT* out;
-  float* out32;                            // 24-bit jobs: column blocks with out_off < t24_off are fp32 at out32 + out_off
-  int64_t t24_off;                         // ... and the others 24-bit at `out`, logical offset out_off - t24_off
+  float* out32;                            // table jobs (24-bit, bs16): column blocks with out_off < t24_off are fp32 at
+  int64_t t24_off;                         // out32 + out_off, the others in the table at `out`, logical offset out_off - t24_off
   const CUtensorMap* out_maps;             // BN = 128 / 256: output map(s) of (group g, column block cb) at map_first[g] + cb
   int n_groups, cb_width, k_blocks, tile_n, n_tiles_n;
   int32_t first_tile[kMaxGroups + 1];
@@ -152,8 +166,9 @@ struct FwdJob {
     int a_row, w_row, cols, m0, n0;
     int64_t rows, ld;
     OutT* out;
-    float* out32;                          // 24-bit jobs: the tile's fp32 output, or NULL
-    unsigned char *hi, *lo;                // 24-bit tables: the planes' bytes of the tile's element (0, 0)
+    float* out32;                          // table jobs: the tile's fp32 output, or NULL
+    unsigned char *hi, *lo;                // 24-bit tables: the planes' bytes of the tile's element (0, 0); bs16: its
+                                           // mantissa and its block's scale
     const float* bias;
     const CUtensorMap* map;
   };
@@ -181,6 +196,12 @@ struct FwdJob {
       const hgt_t24_at e(out, off - t24_off, cblk.ld);
       t.hi = e.hi;
       t.lo = e.lo;
+    } else if constexpr (is_bs16<OutT>()) {
+      const int64_t off = cblk.out_off + m0 * cblk.ld + n0;
+      t.out32 = cblk.out_off < t24_off ? out32 + off : nullptr;
+      const hgt_bs16_at e(out, off - t24_off, cblk.ld);
+      t.hi = e.m;
+      t.lo = e.s;
     } else {
       t.out = out + cblk.out_off + m0 * cblk.ld + n0;
     }
@@ -262,6 +283,30 @@ struct FwdJob {
       store_staged<BN>(acc, stage, c, wq, lane, pair, [&](int r, int col, float4 v) {
         if (r < rows && col < cols) store4_t24(hi + r * rb + 2 * col, lo + r * rb + col, v, vec4);
       });
+    } else if constexpr (is_bs16<OutT>()) {
+      if (t.out32) {
+        // the fp32 boxes fill whole buffers: the scale box of a previous bs16 tile must have been read out
+        if (fwd_tma_store<BN>() && wq == 0 && lane == 0) bulk_wait_read<0>();
+        store_plain<BN>(t, t.out32, acc, stage, c, wq, lane, pair);
+        return;
+      }
+      const int64_t rows = t.rows - 64 * c;
+      const int64_t rb = hgt_bs16_row_bytes(t.ld);             // row stride in bytes, a multiple of 16
+      unsigned char* m = t.hi + 64 * c * rb;
+      unsigned char* sc = t.lo + 64 * c * rb;
+      if constexpr (fwd_tma_store<BN>()) {
+        // k_out_maps' alignment rule, and a tile whose scale box lies inside the column block (a box that TMA clips at
+        // a column that is not a 16-byte multiple wrote wrong scales)
+        if (((reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(sc)) & 15) == 0 && cols >= BN) {
+          store_tma<BN, OutT>(acc, reinterpret_cast<unsigned char*>(stage), c, wq, lane, pair, t.map, t.n0,
+                              t.m0 + 64 * c, cols);
+          return;
+        }
+        if (wq == 0 && lane == 0) bulk_wait_read<0>();
+      }
+      store_staged<BN>(acc, stage, c, wq, lane, pair, [&](int r, int col, float4 v) {
+        store4_bs16(m + r * rb + 2 * col, sc + r * rb + 2 * (col / 16), v, r < rows && col < cols, lane);
+      });
     } else {
       store_plain<BN>(t, t.out, acc, stage, c, wq, lane, pair);
     }
@@ -306,7 +351,7 @@ __global__ void k_out_maps(const __grid_constant__ CUtensorMap tmpl, const __gri
     const hgt_lin_cblock cblk = cblocks[grp.cb_first + cb];
     CUtensorMap* m = maps + out_maps_per_block<OutT>() * (first.v[blockIdx.x] + cb);
     if (grp.m <= 0) continue;
-    if (is_t24<OutT>() && cblk.out_off < t24_off) {
+    if (is_table<OutT>() && cblk.out_off < t24_off) {
       const float* base = out32 + cblk.out_off;
       const uint64_t stride = (uint64_t)cblk.ld * 4;
       if (((reinterpret_cast<uintptr_t>(base) | stride) & 15) != 0) continue;
@@ -317,6 +362,12 @@ __global__ void k_out_maps(const __grid_constant__ CUtensorMap tmpl, const __gri
       if (((reinterpret_cast<uintptr_t>(e.hi) | reinterpret_cast<uintptr_t>(e.lo) | stride) & 15) != 0) continue;
       put_map(m, tmpl, e.hi, grp.m, stride);
       put_map(m + 1, tmpl_lo, e.lo, grp.m, stride);
+    } else if constexpr (is_bs16<OutT>()) {
+      const hgt_bs16_at e(out, cblk.out_off - t24_off, cblk.ld);
+      const uint64_t stride = (uint64_t)hgt_bs16_row_bytes(cblk.ld);
+      if (((reinterpret_cast<uintptr_t>(e.m) | reinterpret_cast<uintptr_t>(e.s)) & 15) != 0) continue;
+      put_map(m, tmpl, e.m, grp.m, stride);
+      put_map(m + 1, tmpl_lo, e.s, grp.m, stride);
     } else {
       OutT* base = out + cblk.out_off;
       const uint64_t stride = (uint64_t)cblk.ld * sizeof(OutT);
@@ -385,19 +436,22 @@ bool a_fp32_loadable(const float* A, int64_t lda) {
 
 // Template of the output maps: `cb_width` columns of `elem`-byte elements, boxes of 128 bytes x 64 rows with SWIZZLE_128B
 // (the layout tcp::store_tma stages), or of 64 bytes with SWIZZLE_64B (elem = 1: the lo plane of a 24-bit table).
+// scale_box > 0: the scale plane of a bs16 table, cb_width / 16 bf16 per row, unswizzled boxes of scale_box x 64.
 // `dummy` (16-byte aligned) and the row count / stride are placeholders that k_out_maps replaces.
-int make_out_template(CUtensorMap* m, void* dummy, int cb_width, int elem) {
+int make_out_template(CUtensorMap* m, void* dummy, int cb_width, int elem, int scale_box = 0) {
   EncodeTiledFn fn = get_encode_fn();
   HGT_REQUIRE(fn != nullptr, "hgt_typed_linear: cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[2] = {(cuuint64_t)cb_width, 64};
-  cuuint64_t strides[1] = {(cuuint64_t)hgt_align_up((size_t)cb_width * elem, 16)};
-  cuuint32_t box[2] = {elem == 1 ? 64u : 128 / (cuuint32_t)elem, 64};
+  const int cols = scale_box ? cb_width / 16 : cb_width;
+  cuuint64_t dims[2] = {(cuuint64_t)cols, 64};
+  cuuint64_t strides[1] = {(cuuint64_t)hgt_align_up((size_t)cols * elem, 16)};
+  cuuint32_t box[2] = {scale_box ? (cuuint32_t)scale_box : elem == 1 ? 64u : 128 / (cuuint32_t)elem, 64};
   cuuint32_t estr[2] = {1, 1};
   const CUtensorMapDataType type = elem == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
                                    : elem == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8;
   CUresult r = fn(m, type, 2, dummy, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  elem == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  scale_box ? CU_TENSOR_MAP_SWIZZLE_NONE
+                            : elem == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   HGT_REQUIRE(r == CUDA_SUCCESS, "hgt_typed_linear: cuTensorMapEncodeTiled (output) failed (%d) cb_width=%d", (int)r,
               cb_width);
   return 0;
@@ -451,12 +505,13 @@ int launch_fwd(FwdJob<OutT, AF>& job, const FwdOps& ops, int tiles, cudaStream_t
     CUtensorMap tmpl, tmpl_lo, tmpl_f32;
     MapFirst first;
     void* dummy = const_cast<CUtensorMap*>(job.out_maps);
-    // 24-bit tables: the hi plane's u16 elements as bf16 (the maps only move bytes), the lo plane's u8, fp32 blocks
-    if ((rc = make_out_template(&tmpl, dummy, job.cb_width, is_t24<OutT>() ? 2 : (int)sizeof(OutT)))) return rc;
+    // 24-bit tables: the hi plane's u16 elements as bf16 (the maps only move bytes), the lo plane's u8, fp32 blocks;
+    // bs16 tables: the int16 mantissas as bf16, fp32 blocks
+    if ((rc = make_out_template(&tmpl, dummy, job.cb_width, is_table<OutT>() ? 2 : (int)sizeof(OutT)))) return rc;
     tmpl_lo = tmpl_f32 = tmpl;
-    if (is_t24<OutT>() && ((rc = make_out_template(&tmpl_lo, dummy, job.cb_width, 1)) ||
-                           (rc = make_out_template(&tmpl_f32, dummy, job.cb_width, 4))))
-      return rc;
+    if (is_t24<OutT>() && (rc = make_out_template(&tmpl_lo, dummy, job.cb_width, 1))) return rc;
+    if (is_bs16<OutT>() && (rc = make_out_template(&tmpl_lo, dummy, job.cb_width, 2, BN / 16))) return rc;
+    if (is_table<OutT>() && (rc = make_out_template(&tmpl_f32, dummy, job.cb_width, 4))) return rc;
     for (int g = 0; g < job.n_groups; ++g) first.v[g] = job.map_first[g];
     k_out_maps<OutT><<<job.n_groups, 64, 0, st>>>(tmpl, tmpl_lo, tmpl_f32, job.groups, job.cblocks, job.out, job.out32,
                                                   job.t24_off, first, const_cast<CUtensorMap*>(job.out_maps));
@@ -597,6 +652,14 @@ int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float
                 workspace, workspace_bytes, st, out32, t24_off);
 }
 
+int hgt_typed_linear_tc(const float* A, int64_t lda, const float* W, const float* bias, int32_t K, int32_t cb_width,
+                        const hgt_lin_group* groups, const hgt_lin_group* h_groups, int32_t n_groups,
+                        const hgt_lin_cblock* cblocks, float* out32, int64_t t24_off, hgt_bs16* out,
+                        int32_t products, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  return tc_run(A, lda, nullptr, nullptr, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks, out, products,
+                workspace, workspace_bytes, st, out32, t24_off);
+}
+
 extern "C" int hgt_typed_linear_presplit_workspace_bytes(const hgt_lin_group* h_groups, int32_t n_groups, int32_t K,
                                                          int32_t cb_width, size_t* out_bytes) {
   HGT_REQUIRE(out_bytes && (h_groups || n_groups == 0), "hgt_typed_linear_presplit_workspace_bytes: NULL argument");
@@ -653,6 +716,17 @@ extern "C" int hgt_typed_linear_presplit_t24(const void* a_hi, const void* a_lo,
                                              void* workspace, size_t workspace_bytes, void* stream_) {
   return typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks,
                                static_cast<hgt_t24*>(out24), workspace, workspace_bytes, (cudaStream_t)stream_, out,
+                               t24_off);
+}
+
+extern "C" int hgt_typed_linear_presplit_bs16(const void* a_hi, const void* a_lo, const float* W, const float* bias,
+                                              int32_t K, int32_t cb_width, const hgt_lin_group* groups,
+                                              const hgt_lin_group* h_groups, int32_t n_groups,
+                                              const hgt_lin_cblock* cblocks, float* out, int64_t t24_off, void* out16,
+                                              void* workspace, size_t workspace_bytes, void* stream_) {
+  HGT_REQUIRE(cb_width % 16 == 0, "hgt_typed_linear_presplit_bs16: needs cb_width %% 16 == 0 (cb_width=%d)", cb_width);
+  return typed_linear_presplit(a_hi, a_lo, W, bias, K, cb_width, groups, h_groups, n_groups, cblocks,
+                               static_cast<hgt_bs16*>(out16), workspace, workspace_bytes, (cudaStream_t)stream_, out,
                                t24_off);
 }
 

@@ -371,16 +371,27 @@ __device__ __forceinline__ void t24_pair(float2 v, uint32_t& hi, uint32_t& lo) {
 }
 
 template <class OutT> constexpr bool is_t24() { return std::is_same<OutT, hgt_t24>::value; }
-// Output tensor maps per (group, column block): one, or a hi-plane and a lo-plane map for 24-bit tables.
-template <class OutT> constexpr int out_maps_per_block() { return is_t24<OutT>() ? 2 : 1; }
+template <class OutT> constexpr bool is_bs16() { return std::is_same<OutT, hgt_bs16>::value; }
+// Gather-table outputs (24-bit or bs16): planar byte formats whose jobs write their fp32 column blocks elsewhere.
+template <class OutT> constexpr bool is_table() { return is_t24<OutT>() || is_bs16<OutT>(); }
+// Output tensor maps per (group, column block): one, or a hi-plane and a lo-plane map for 24-bit tables, a mantissa and
+// a scale map for bs16 tables.
+template <class OutT> constexpr int out_maps_per_block() { return is_table<OutT>() ? 2 : 1; }
 
 // Asynchronous epilogue of one consumer warpgroup (c): its 64 x BN accumulator goes out in 64-column blocks.  Each block
 // is written to shared memory as OutT in the SWIZZLE_128B layout of `map`'s boxes (128-byte rows, 64 rows; 16-byte chunk q
 // of row r at q ^ (r & 7); fp32: two boxes of 32 columns, bf16: one box of 64) and sent to global memory by TMA tensor
 // stores that one thread (the warpgroup's first) issues.  24-bit tables (hgt_t24): the hi halves as a bf16-like box of
 // 64 u16 at the buffer and the lo bytes as a box of 64 u8 (64-byte rows, SWIZZLE_64B: chunk q of row r at
-// q ^ ((r >> 1) & 3)) 8 KB further, stored through map[0] and map[1].  The map's extents clip the rows past the group and the columns
-// past the column block.  The stores drain while the consumer goes on to the next block or the next tile's products.
+// q ^ ((r >> 1) & 3)) 8 KB further, stored through map[0] and map[1].  bs16 tables (hgt_bs16): the int16 mantissas as
+// a bf16-like box of 64 through map[0]; the quad that holds a row's 16-column block finds its largest |x| with two
+// shuffles, and lane h of the quad (rows r0 and r0 + 8 are h = 0 and 1) writes the row's four scales of the block into
+// the tile's scale box (64 rows x BN / 16 bf16, unswizzled, in the unused upper half of buffer 0), which goes out
+// through map[1] with the last block.  A block's own four scales per row are 8 bytes, below TMA's 16-byte inner box;
+// scattered 8-byte st.global of them cost as much as the rest of the epilogue.  Before block 0 writes scales the
+// previous tile's scale box has been read out (wait for all groups rather than all but the last).  The map's extents
+// clip the rows past the group and the columns past the column block.  The stores drain while the consumer goes on to
+// the next block or the next tile's products.
 // Block b uses buffer b & 1 of `stage` (two TMA_BUF_BYTES buffers, 1024-byte aligned); BN / 64 is even, so the buffers
 // alternate across tiles too.  Before a buffer is rewritten the issuing thread waits until the bulk group that read it two
 // blocks earlier is done (it commits one group per block).
@@ -390,36 +401,68 @@ template <int BN, class OutT, class Pair>
 __device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage, int c, int wq, int lane, Pair pair,
                                           const CUtensorMap* map, int col0, int row0, int cols) {
   static_assert(BN % 128 == 0, "the two buffers alternate across tiles only for an even number of 64-column blocks");
-  constexpr bool T24 = is_t24<OutT>();
-  constexpr int BOX_COLS = T24 ? 64 : 128 / (int)sizeof(OutT);
+  constexpr bool T24 = is_t24<OutT>(), BS16 = is_bs16<OutT>();
+  constexpr int BOX_COLS = T24 || BS16 ? 64 : 128 / (int)sizeof(OutT);
   const bool issuer = wq == 0 && lane == 0;
   const int r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
   if (issuer) {
     tensormap_acquire(map);
-    if constexpr (T24) tensormap_acquire(map + 1);
+    if constexpr (T24 || BS16) tensormap_acquire(map + 1);
   }
+  unsigned char* const scale_box = stage + 8192;                 // bs16: 64 rows x BN / 8 bytes
 #pragma unroll
   for (int blk = 0; blk < BN / 64; ++blk) {
     unsigned char* buf = stage + (blk & 1) * TMA_BUF_BYTES;
-    if (issuer) bulk_wait_read<1>();
+    if (issuer) {
+      if (BS16 && blk == 0) bulk_wait_read<0>();                // ... and the previous tile's scale box
+      else bulk_wait_read<1>();
+    }
     bar_sync_named(1 + c, 128);                                 // the buffer has been read out
-#pragma unroll
-    for (int j = 8 * blk; j < 8 * blk + 8; ++j) {
+    if constexpr (BS16) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int r = r0 + 8 * h, lc = 8 * j + c0 - 64 * blk;
-        const float2 v = pair(r, 8 * j + c0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-        if constexpr (T24) {
-          uint32_t hi, lo;
-          t24_pair(v, hi, lo);
-          const uint32_t x = (uint32_t)lc * 2;
-          *reinterpret_cast<uint32_t*>(buf + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))) = hi;
-          *reinterpret_cast<uint16_t*>(buf + 8192 + r * 64 + ((((lc >> 4) ^ ((r >> 1) & 3)) << 4) | (lc & 15))) =
-              (uint16_t)lo;
-        } else {
-          const uint32_t x = (uint32_t)(lc % BOX_COLS) * sizeof(OutT);     // byte in the box row
-          put2(reinterpret_cast<OutT*>(buf + (lc / BOX_COLS) * 8192 + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))),
-               v);
+        const int r = r0 + 8 * h;
+        uint32_t sc[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {                           // 16-column block k: fragment columns j = 2k, 2k + 1
+          const int j = 8 * blk + 2 * k;
+          const float2 v0 = pair(r, 8 * j + c0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          const float2 v1 = pair(r, 8 * j + 8 + c0, acc[4 * j + 4 + 2 * h], acc[4 * j + 4 + 2 * h + 1]);
+          const uint32_t a = hgt_bs16_quad_amax(max(max(hgt_abs_bits(v0.x), hgt_abs_bits(v0.y)),
+                                                    max(hgt_abs_bits(v1.x), hgt_abs_bits(v1.y))));
+          float rc;
+          sc[k] = hgt_bs16_scale(a, rc);
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const float2 v = u ? v1 : v0;
+            const uint32_t x = (uint32_t)(16 * k + 8 * u + c0) * 2;
+            *reinterpret_cast<uint32_t*>(buf + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))) =
+                hgt_bs16_pack(v.x, v.y, rc, sc[k]);
+          }
+        }
+        if ((lane & 3) == h)
+          *reinterpret_cast<uint2*>(scale_box + r * (BN / 8) + 8 * blk) =
+              make_uint2(sc[0] | (sc[1] << 16), sc[2] | (sc[3] << 16));
+      }
+    } else {
+#pragma unroll
+      for (int j = 8 * blk; j < 8 * blk + 8; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + 8 * h, lc = 8 * j + c0 - 64 * blk;
+          const float2 v = pair(r, 8 * j + c0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          if constexpr (T24) {
+            uint32_t hi, lo;
+            t24_pair(v, hi, lo);
+            const uint32_t x = (uint32_t)lc * 2;
+            *reinterpret_cast<uint32_t*>(buf + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))) = hi;
+            *reinterpret_cast<uint16_t*>(buf + 8192 + r * 64 + ((((lc >> 4) ^ ((r >> 1) & 3)) << 4) | (lc & 15))) =
+                (uint16_t)lo;
+          } else {
+            const uint32_t x = (uint32_t)(lc % BOX_COLS) * sizeof(OutT);     // byte in the box row
+            put2(reinterpret_cast<OutT*>(buf + (lc / BOX_COLS) * 8192 + r * 128 + ((((x >> 4) ^ (r & 7)) << 4) | (x & 15))),
+                 v);
+          }
         }
       }
     }
@@ -431,6 +474,8 @@ __device__ __forceinline__ void store_tma(const float* acc, unsigned char* stage
         if (64 * blk + BOX_COLS * bx < cols) tma_store_2d(map, s_u32(buf + bx * 8192), col0 + 64 * blk + BOX_COLS * bx, row0);
       if constexpr (T24)
         if (64 * blk < cols) tma_store_2d(map + 1, s_u32(buf + 8192), col0 + 64 * blk, row0);
+      if constexpr (BS16)
+        if (blk == BN / 64 - 1) tma_store_2d(map + 1, s_u32(scale_box), col0 / 16, row0);
       bulk_commit();
     }
   }
